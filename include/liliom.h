@@ -1,4 +1,4 @@
-/* liliom.h — C ABI of libliliom_b200.so: a B200-native (sm_100a) drop-in for the per-scan hot
+/* liliom.h — C ABI of libliliom_b200.so: an H100-native (sm_90a) drop-in for the per-scan hot
  * path of KIT-ISAS/lili-om.  The reference has no FFI/plugin interface for this path (it is
  * private member functions of two ROS node classes), so each entry point cites the reference
  * code it replaces; INTEGRATION.md shows the call a maintainer adds inside the node.
@@ -305,8 +305,8 @@ int liliom_get_counters(liliom_ctx* c, liliom_counters* out, int reset);
  * (pruning; knn_candidates above counts those).  Not on the hot path. */
 int liliom_knn_block_stats(liliom_ctx* c, const double pose7[7], unsigned long long out2[2]);
 /* on = 1: bracket every kNN+Jacobian launch with a CUDA-event pair on the context stream and count its queries /
- * candidates on the device; on = N > 1: do so on every N-th scan-to-map call only (an event pair costs the step ~4 us each
- * of dependent stream latency, measured: profiles/r02_ab_host_results.txt); 0 (default): off. */
+ * candidates on the device; on = N > 1: do so on every N-th scan-to-map call only (each event of the pair adds dependent
+ * stream latency to the step); 0 (default): off. */
 int liliom_set_kernel_timing(liliom_ctx* c, int on);
 /* Run all library work on a caller-owned CUDA stream (cudaStream_t passed as void*; NULL restores the
  * context's own stream).  Calls stay synchronous; this only lets the caller bracket them with events. */

@@ -1,4 +1,4 @@
-"""liliom_b200 — B200-native (sm_100a) implementation of the per-scan hot path of KIT-ISAS/lili-om.
+"""liliom_b200 — H100-native (sm_90a) implementation of the per-scan hot path of KIT-ISAS/lili-om.
 
 Layout (SURVEY.md §8): `csrc/` hand-written CUDA kernels + the C ABI (include/liliom.h),
 `_lib.py` ctypes binding, `synth.py` seeded synthetic worlds and sweeps.

@@ -98,7 +98,7 @@ def lib() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  liliom_b200 has no CPU fallback.")
+            "(nvcc, sm_90a).  liliom_b200 has no CPU fallback.")
     L = C.CDLL(LIB_PATH, mode=C.RTLD_GLOBAL)
     vp, ip, dp, fp = C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_double), C.POINTER(C.c_float)
     L.liliom_default_params.argtypes = [C.POINTER(Params), C.c_int]

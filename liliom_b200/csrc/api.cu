@@ -76,8 +76,8 @@ __global__ void k_transform_cloud(const unsigned char* __restrict__ in, int n, i
 }
 
 // Concatenation of the FIFO frames (L/src/LidarOdometry.cpp:301-302) in ONE launch: blockIdx.y = frame, the blocks of a row
-// stream that frame's 16-byte words to its offset in the concatenated cloud.  (20 cudaMemcpyAsync calls cost ~210 us whatever
-// the size — measured on B200 for both a 10 M-point map and its 5.4 M-point shard, profiles/r02_map_rebuild_phases_before.txt.)
+// stream that frame's 16-byte words to its offset in the concatenated cloud.  (20 cudaMemcpyAsync calls cost a fixed
+// latency per copy whatever the size, which a single launch does not.)
 constexpr int kConcatMax = 64;
 struct ConcatTab { const float4* src[kConcatMax]; long long off[kConcatMax + 1]; };      // offsets in 16-byte words
 __global__ void k_concat_frames(const __grid_constant__ ConcatTab tab, float4* __restrict__ out) {
@@ -654,7 +654,7 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
     if (total > 0) {
         int* hp = reinterpret_cast<int*>(c->h_pin);
         // (The single-launch cooperative filter of the scan VoxelGrid was tried here for maps of <= 32k points: within the noise
-        // of the real-size streamed lifecycle, profiles/r02_stream_real_lifecycle_mapcoop_ab.txt — not kept.)
+        // of the real-size streamed lifecycle — not kept.)
         {
             LILI_TRY(voxelgrid_dev(c, c->map_raw.p, (int)total, stride, c->prm.leaf_map, c->map_ds.p, c->vg_count.as<int>(),   // :316-317
                                    c->nranks == 1 ? c->map_xyzw.as<float4>() : nullptr, box));

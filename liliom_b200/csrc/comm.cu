@@ -99,7 +99,7 @@ extern "C" int liliom_comm_set_shard_block(liliom_ctx* c, int metres) {
 }
 
 // ---- fused exchange over NVLink / NVSwitch peer memory (SURVEY.md §8 e, "one kernel that does both") -------------------------
-// The NCCL path costs, per GN iteration, a kernel, an all-reduce of 232 bytes (~20 us of latency on 2 B200s, more than the
+// The NCCL path costs, per GN iteration, a kernel, an all-reduce of 232 bytes (tens of microseconds of latency on 2 GPUs, more than the
 // sharded search saves at 1.4k queries) and an update kernel.  Here every rank runs its persistent GN kernel; after the local
 // grid reduction block 0 stores the rank's 29 sums straight into EVERY peer's exchange buffer (flag-in-data words, system scope)
 // and all blocks read the ranks' sums from their own buffer: all iterations of a scan in one launch per rank, no collective call.

@@ -11,8 +11,8 @@
 
 namespace lili {
 
-// One growable device allocation.  Buffers only grow; 180 GB of HBM3e per GPU makes
-// reallocation-on-demand a cold path (first scan), never a steady-state cost.
+// One growable device allocation.  Buffers only grow; 80 GB of HBM3 per GPU (a 10 M-point map needs well under 1 GB)
+// makes reallocation-on-demand a cold path (first scan), never a steady-state cost.
 struct DevBuf {
     void*  p = nullptr;
     size_t cap = 0;
@@ -107,7 +107,7 @@ struct liliom_ctx {
     int    early_cut_cap = 0;
     bool   early_cut_issued = false;
     std::string last_error;
-    int sm_count = 148;
+    int sm_count = 132;                  // H100 SXM; replaced by the device's multiProcessorCount at create
 
     // ---- staging (pinned host) ----
     void*  h_pin = nullptr;      // small pinned block: counts, pose, stats

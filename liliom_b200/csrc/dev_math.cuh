@@ -1,4 +1,4 @@
-// Device scalar routines of the LiLi-OM hot path (sm_100a).
+// Device scalar routines of the LiLi-OM hot path (sm_90a).
 // The *_x ("exact") helpers spell every operation with round-to-nearest intrinsics so that
 // nvcc never contracts them into FMAs: they reproduce bit-for-bit what the reference's
 // generic x86-64 build computes (no FMA; SURVEY.md Appendix C.2), which is what makes the

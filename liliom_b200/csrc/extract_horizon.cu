@@ -1,4 +1,4 @@
-// Livox-Horizon feature extraction on sm_100a — replaces the loops of
+// Livox-Horizon feature extraction on sm_90a — replaces the loops of
 // Preprocessing::cloudHandler, L/src/Preprocessing.cpp:225-383:
 //   k_hz_flags     removeNaN (:225) + removeClosedPointCloud 0.1 m (:72-97,226) + scan_id>=0 (:253)
 //   (scan)         stable compaction index = position in lidar_cloud_cutted

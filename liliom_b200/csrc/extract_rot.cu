@@ -1,4 +1,4 @@
-// Spinning-LiDAR (LOAM-style) feature extraction on sm_100a — replaces the loops of
+// Spinning-LiDAR (LOAM-style) feature extraction on sm_90a — replaces the loops of
 // Preprocessing::cloudHandler, R/src/Preprocessing.cpp:280-509.
 //
 //   k_rot_pre      removeNaN + removeClosedPointCloud 3.0 m (:280-281), elevation -> scanID
@@ -225,9 +225,8 @@ __global__ void __launch_bounds__(512) k_rot_ring(const Pt32* __restrict__ cloud
             // whether a candidate qualifies (curvature class, range) and which neighbours a pick marks (the break test between
             // consecutive points) are static, so all of that is computed in parallel first, the sorted order becomes a rank per
             // point (counting sort: one barrier instead of the 45 of a bitonic network), and "the next unpicked candidate" is the
-            // highest / lowest set bit of a 32-word availability mask that every pick clears bits in.  Measured before, per
-            // segment of ~316 points: sort 11k cycles, walk 40k cycles of dependent single-warp instructions, kernel 90 us
-            // (profiles/r02_rot_ring_stage_cycles.txt).
+            // highest / lowest set bit of a 32-word availability mask that every pick clears bits in (the sorted walk it
+            // replaces was a chain of dependent single-warp instructions per candidate; LILIOM_DEBUG_TIMING shows the stages).
             for (int t = threadIdx.x; t < L; t += blockDim.x) {
                 const unsigned long long mine = S.keys[t];
                 int r = 0;
@@ -338,8 +337,8 @@ __global__ void __launch_bounds__(512) k_rot_ring(const Pt32* __restrict__ cloud
             // The picks are sequential by definition (a pick marks its +-5 neighbours, which later candidates must see), but the
             // candidates BETWEEN picks are not: warp 0 examines 32 sorted candidates at a time, a ballot finds the first one that
             // is still unpicked (or the first that ends the walk), and only that one is acted on before the scan resumes behind it
-            // with the fresh marks.  Sequential steps = picks (<= 14 per segment), not candidates; one thread walking the list took
-            // ~23k of the ~30k cycles per segment (k_rot_ring 90 us, profiles/r02_stream_1gpu_launches.csv).
+            // with the fresh marks.  Sequential steps = picks (<= 14 per segment), not candidates; one thread walking the list
+            // spends most of the segment's cycles in that walk.
             if (threadIdx.x < 32) {
                 const unsigned full = 0xffffffffu;
                 const int lane = threadIdx.x;

@@ -1,4 +1,4 @@
-// Scan-to-map on sm_100a: dense 1 m cell grid over the down-sampled map (stand-in for the
+// Scan-to-map on sm_90a: dense 1 m cell grid over the down-sampled map (stand-in for the
 // per-scan FLANN kd-tree, L/src/LidarOdometry.cpp:490) and the fused
 //   transform -> exact 5-NN -> 5x3 QR plane -> gates -> residual + SE(3) Jacobian row ->
 //   Huber -> 21+6 reduction -> 6x6 solve -> pose update
@@ -101,8 +101,8 @@ __global__ void k_gather_sorted(const float4* __restrict__ p, const int* __restr
 
 // cell_start[c] = first sorted position whose key >= c = number of points with key < c = upper bound of cell c-1.
 // Run ENDS are scattered (cell_start[key+1] = position after the run) into a zeroed table and a running maximum fills the
-// empty cells: two streaming passes over the table.  (The first version filled every gap with one warp per sorted
-// position: 724 us for a 10 M-point map, profiles/r02_stream_1gpu_launches.txt; this is ~60 us.)
+// empty cells: two streaming passes over the table.  (Filling every gap with one warp per sorted position is an order of
+// magnitude slower on a 10 M-point map.)
 __global__ void k_cell_run_ends(const uint32_t* __restrict__ keys, int n, int* __restrict__ cell_start) {
     const int w = blockIdx.x * blockDim.x + threadIdx.x;
     if (w >= n) return;
@@ -536,8 +536,8 @@ __device__ __forceinline__ void peer_exchange(const PeerArgs& pa, unsigned int e
 }
 
 // Inside one GPU only block 0 talks to the peers: it republishes the sums over all ranks (and the loss flag) for the other
-// blocks, which wait on one epoch word instead of polling nranks x 29 system-scope words each (148 blocks doing that cost
-// ~20 us per pass on 2 GPUs, profiles/r02_bench_2gpu_first.json).
+// blocks, which wait on one epoch word instead of polling nranks x 29 system-scope words each (one block per SM doing that
+// adds tens of microseconds per pass on 2 GPUs).
 __device__ __forceinline__ void peer_local_publish(const PeerArgs& pa, unsigned int epoch, KnnSmem& S) {
     double* dst = pa.lsum + (size_t)(epoch & 1u) * 32;
     if (threadIdx.x < kNormEq) dst[threadIdx.x] = S.red[0][threadIdx.x];
@@ -593,12 +593,11 @@ __device__ __forceinline__ void write_neq_stats(const KnnArgs& a, const KnnSmem&
 }
 
 
-// (Search and fit as two kernels — the search alone runs at 64 registers and twice the resident warps — was measured twice,
-// with the exhaustive search of round 1 and with the pruned one: 62.3 vs 57.6 us per pass at 128k queries.  The search
-// alone takes 32 us at 47 % lane utilisation; what limits the one-thread-per-query shape is divergence between the lanes'
-// candidate lists, not latency hiding.  profiles/r02_knn_dense_split_ab.txt, r02_knn_search_only_ncu.txt.)
-// Blocks per SM of the one-thread-per-query instance: that shape is bound by latency per issued instruction (8.8 cycles at
-// ~4 warps per scheduler, profiles/r02_knn_dense_v1_ncu.txt), so it trades registers (spills in the fp64 fit) for resident warps.
+// (Search and fit as two kernels — the search alone runs at 64 registers and twice the resident warps — was slower than the
+// fused kernel at 128k queries, with the exhaustive and with the pruned search: what limits the one-thread-per-query shape is
+// divergence between the lanes' candidate lists, not latency hiding.)
+// Blocks per SM of the one-thread-per-query instance: that shape is bound by latency per issued instruction at ~4 warps per
+// scheduler, so it trades registers (spills in the fp64 fit) for resident warps.
 #ifndef LILI_KNN1_MINBLOCKS
 #define LILI_KNN1_MINBLOCKS 2
 #endif
@@ -655,8 +654,7 @@ __global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) 
 // The persistent kernel never runs more than one block per SM (grid <= sm_count), so it takes a 176-register cap instead
 // of the 128 of __launch_bounds__(256, 2): the spills (200-600 B per thread in the fp64 fit) disappear, while a
 // 64-register block of the Preprocessing node's cooperative kernel still fits beside it (176*256 + 64*256 <= 65536
-// registers), which the two-node e2e leg relies on.  Measured on B200 (1.5k-query scans, A/B in one process,
-// tools/ab_variants.py): 12.70 -> 12.32 us per pass; with the release-only barrier below 11.04 us.
+// registers), which the two-node e2e leg relies on (A/B of the caps in one process: tools/ab_variants.py).
 // (__maxnreg__ and __launch_bounds__ cannot be combined; the block size is fixed by the host code.)
 #ifndef LILI_GN_MAXNREG
 #define LILI_GN_MAXNREG 176
@@ -711,7 +709,7 @@ __global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned in
         // RED, no L1 invalidate) and NO acquire fence after the relaxed poll.  An acquire would only add an L1 invalidation:
         // everything this kernel reads through L1 (map, cell table, features) is immutable for the launch, and the partials are
         // read with L2-scope loads (__ldcg) issued after the poll's control dependency and a bar.sync.  The PTX model formally
-        // asks for the acquire: mode 1 polls with ld.acquire (+5 % per pass, profiles/r02_ab_gn_switches.txt), mode 0 fences both
+        // asks for the acquire: mode 1 polls with ld.acquire (slower per pass: tools/ab_variants.py), mode 0 fences both
         // sides; tests pin all three to the same bits (test_gpu_variants.py, test_persistent_barrier_stress_all_sync_modes).
         // Multi-GPU (fused exchange): the other blocks of this GPU arrive but do not wait here — they wait for block 0's
         // republished sums over all ranks.
@@ -1062,8 +1060,8 @@ static void pick_shape(int n, int sm_count, int& lanes, int& rounds) {
     const long long w8 = (long long)sm_count * 8;      // warps for ~8 per SM
     rounds = 1;
     if ((long long)n >= w8 * 32) { lanes = 1; return; }
-    // 9.5k..38k queries: two lanes per query (measured at 16k queries, profiles/r02_knn_lanes_sweep.txt: 20.8 us per pass with
-    // 2 lanes, 22.1 with 1, 27.2 with 4, 33.5 with 8)
+    // 8..32 warps' worth of queries per SM: two lanes per query (a sweep of the lane count at 16k queries, tools/knn_sweep.py,
+    // put 2 lanes ahead of 1, 4 and 8)
     if ((long long)n >= w8 * 8) { lanes = 2; return; }
     lanes = ((long long)n * 16 / 32 <= w8 * 2) ? 16 : 8;   // tiny scans: one run per lane (9 of 16 lanes)
 }
@@ -1088,9 +1086,8 @@ int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int
     int ntasks = cdiv(c->d_nfeats ? max(n_est + n_est / 4, 1) : n, per_task);
     int grid = min(max(cdiv(ntasks, kWarps), 1), c->sm_count * 2);
     // A 16-lane scan that needs more than one block per SM (1.9k-3.8k queries, e.g. a down-sampled HDL-64E sweep) would
-    // leave the single-launch path.  Eight lanes per query (four queries per warp, one round) keep it there; measured on the
-    // configs[2] workload, 3.1k queries: 13.7 us per pass, against 16.1 for two rounds of 16 lanes and 21 for per-iteration
-    // launches (profiles/r02_ab_lanes_3k.txt).
+    // leave the single-launch path.  Eight lanes per query (four queries per warp, one round) keep it there, which on the
+    // configs[2] workload (3.1k queries) is faster than two rounds of 16 lanes or per-iteration launches.
     if (lanes == 16 && rounds == 1 && !c->force_lanes && grid > c->sm_count && mode == LILIOM_MODE_GN && !want_corr) {
         const int ntasks8 = cdiv(c->d_nfeats ? max(n_est + n_est / 4, 1) : n, 4);
         const int grid8 = max(cdiv(ntasks8, kWarps), 1);

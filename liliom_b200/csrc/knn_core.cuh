@@ -6,8 +6,8 @@
 // so a single unsigned compare implements FLANN's distance order plus our index tie-break with
 // no branches and no extra loads.
 //
-// Pruning (round 2; profiles/r01_knn_dense_lanes1_ncu.txt had 57 % of the issued instructions in the 64-bit ranking
-// chain and every query ranking all ~63 points of its 27 cells).  A correspondence needs its FIFTH neighbour inside the
+// Pruning (without it, every query ranks all ~63 points of its 27 cells and the 64-bit ranking chain dominates the issued
+// instructions).  A correspondence needs its FIFTH neighbour inside the
 // gate (d5 < knn_max_sqdist, L/src/LidarOdometry.cpp:365), so a candidate at or beyond the gate can never be part of an
 // accepted set, and once five candidates are held nothing beyond the current fifth distance can enter the set either:
 //   * every candidate is tested against the running threshold `tau` with ONE fp32 compare before its key is built;
@@ -17,9 +17,8 @@
 //     multiplication and addition are monotonic, hence its computed distance is >= the bound.  The accepted sets and
 //     their order are bit-identical to the exhaustive search (and to the oracle's kd-tree); a query that ends with
 //     fewer than five candidates inside the gate is rejected by both.
-// Loops are deliberately NOT unrolled: the first version of this kernel was 11.7k SASS
-// instructions and spent 47 % of its issue slots in stall_no_inst (instruction-cache misses,
-// profiles/r01_knn_v1_ncu.txt).
+// Loops are deliberately NOT unrolled: unrolled, this kernel grows to ~12k SASS instructions and
+// stalls on instruction-cache misses.
 #pragma once
 #include "ctx.cuh"
 #include "dev_math.cuh"
@@ -140,7 +139,7 @@ __device__ __forceinline__ bool row_cells(const QCell& q, const GridDesc& g, int
     return true;
 }
 
-// ---- bulk-asynchronous staging of a lane's run in shared memory (sm_90+/sm_100a: cp.async.bulk + mbarrier; SASS UBLKCP / SYNCS) ----
+// ---- bulk-asynchronous staging of a lane's run in shared memory (sm_90a: cp.async.bulk + mbarrier; SASS UBLKCP / SYNCS) ----
 // The 16-lane search gives every (y,z) row of the 27-cell block to one lane.  Instead of pulling its run through registers in
 // batches of eight 16-byte loads (a dependent L2 round trip per batch), a lane hands the whole run to the copy engine — one
 // cp.async.bulk of 16 x length bytes into its slot of the warp's staging tile — and the 16 lanes of the query meet at one
@@ -242,9 +241,9 @@ __device__ __forceinline__ void group_knn5(float sx, float sy, float sz, const f
     }
     if (dbg) dbg[10] = clock64() + (long long)(top.k0 & 0);
     // merge: 5 rounds of "group-wide minimum of the list heads, winner pops".  The minimum is an xor
-    // butterfly of 64-bit keys (REDUX.MIN on a partial lane mask measured ~350 cycles per call on
-    // B200, the shuffle butterfly ~35 cycles per step).  Keys are unique — a map point lives in
-    // exactly one lane's list — so exactly one lane pops per round.
+    // butterfly of 64-bit keys (a hardware redux on a partial lane mask is not cheaper: it only takes
+    // 32-bit operands).  Keys are unique — a map point lives in exactly one lane's list — so exactly
+    // one lane pops per round.
     Top5 res;
 #define LILI_MERGE_ROUND(KJ)                                                              \
     {                                                                                     \
@@ -270,8 +269,7 @@ __device__ __forceinline__ void group_knn5(float sx, float sy, float sz, const f
 //   2. the eight other rows are bounded against that tau; the survivors' trimmed runs go to a per-thread list in shared
 //      memory, all their cell-table loads in flight together;
 //   3. ONE loop over the concatenated list.  A warp's trip count is then the maximum over its lanes of the total number of
-//      batches — not the sum over rows of the per-row maxima, which is what cost the first version of this kernel twice
-//      the mean (profiles/r01_knn_dense_lanes1_ncu.txt).
+//      batches — not the sum over rows of the per-row maxima, which costs up to twice the mean.
 // `runs`: this thread's slots of a [kRunCap][run_stride] int4 array in shared memory {begin, end, bound bits, -}.
 constexpr int kRunCap = 8;
 template <int BATCH1 = 8, int BATCH3 = 4>

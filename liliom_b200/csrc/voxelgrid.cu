@@ -408,8 +408,8 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
             }
         }
         // rank by counting over ALL listed keys: from shared memory when the list fits (a down-sampled 24k sweep lists 1-2k
-        // voxels) — measured on B200 (LILIOM_DEBUG_TIMING, 1.7k voxels): 19-20k cycles of this phase were ~50 dependent L2 round
-        // trips per voxel when every compare re-read the list through L2
+        // voxels): when every compare re-read the list through L2 this phase was ~50 dependent L2 round trips per voxel
+        // (LILIOM_DEBUG_TIMING shows the phase's cycles)
         const bool in_smem = U <= VGC_UKEYS;
         if (in_smem) {
             for (int v = tid; v < U; v += VGC_THREADS) S.ukeys[v] = __ldcg(&B.ukey[v]);

@@ -2,7 +2,7 @@
  *
  * C interface of the CPU restatement of LiLi-OM's per-scan hot path.  Loaded through
  * ctypes by tests/, __graft_entry__.smoke() and bench.py's CPU-baseline legs — never by
- * the product package (liliom_b200/).  Citations are relative to /root/reference/.
+ * the product package (liliom_b200/).  Citations are relative to the reference repository's root.
  */
 #ifndef LILIOM_ORACLE_API_H
 #define LILIOM_ORACLE_API_H

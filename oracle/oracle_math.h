@@ -7,7 +7,7 @@
 // none present, no network).  This file restates, from knowledge, the third-party
 // numerical routines the reference calls on the hot path (marked "from-knowledge"),
 // so that the rest of the oracle can follow the reference source expression by
-// expression.  Citations are relative to /root/reference/.
+// expression.  Citations are relative to the reference repository's root.
 //
 // Compile with -O3 -ffp-contract=off (the reference builds with -O3 for generic x86-64:
 // no FMA contraction, LiLi-OM/CMakeLists.txt:5).

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Per-kernel totals and shares of an `ncu --metrics gpu__time_duration.sum --csv` launch list (profiles/*_launches*.csv).
+"""Per-kernel totals and shares of an `ncu --metrics gpu__time_duration.sum --csv` launch list.
 usage: launch_summary.py list.csv [first_kernel_of_a_step]   — with a step marker the last complete step is summarised as well."""
 import csv
 import sys

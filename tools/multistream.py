@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Throughput of S independent scan streams sharing ONE B200 (one liliom context + CUDA stream + host
+"""Throughput of S independent scan streams sharing ONE H100 (one liliom context + CUDA stream + host
 thread per scan stream, as S robots' LidarOdometry/Preprocessing node pairs would).  The single-stream
 step is latency-bound (~20 % SM activity), so concurrent streams fill the machine.
 usage: multistream.py [streams ...]"""

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-kernel SASS summary of libliliom_b200.so (cuobjdump -sass; no GPU needed): instruction count and the mnemonics that
-matter for this library — global/shared/local memory ops, barriers, atomics, fp64, and the Blackwell/Hopper asynchronous-copy
-instructions (UBLKCP = cp.async.bulk, SYNCS = mbarrier).  usage: sass_summary.py [lib.so] > profiles/rNN_sass_summary.txt"""
+matter for this library — global/shared/local memory ops, barriers, atomics, fp64, and the Hopper asynchronous-copy
+instructions (UBLKCP = cp.async.bulk, SYNCS = mbarrier).  usage: sass_summary.py [lib.so]"""
 import collections, os, re, subprocess, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "liliom_b200", "libliliom_b200.so")
