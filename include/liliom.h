@@ -220,6 +220,66 @@ int liliom_backend_edge_block(liliom_ctx* c, const double pose7_body[7], double 
 int liliom_backend_surf_block(liliom_ctx* c, const double pose7_body[7], const double q_lb_wxyz[4], const double t_lb[3],
                               double cauchy_b, double out29[29]);
 
+/* ---- SURVEY §8 (f5): the backend's keyframe clouds and local map on the device, a whole window's LiDAR rows per call ----
+ * Single-GPU (LILIOM_E_ARG on a sharded context), point_stride bytes per point.  None of these calls touches the odometry map
+ * (liliom_map_*, scan-to-map, ICP target); a dedicated backend context is still the recommended set-up (INTEGRATION.md §3). */
+typedef struct {
+    int    variant;             /* 0 = L/ (Horizon): reflectivity-weighted planes, edge s = (float)lidar_const;
+                                   1 = R/ (ROT): dist < 0.1 edge gate (R:1443), 200/N_edge and 1000/N_surf weights (R:843, :861) */
+    float  edge_leaf, surf_leaf;            /* /backend_fusion/edge_ds, surf_ds (L:229-230, :339-348, :563-566) */
+    double kd_max_radius;                   /* squared-distance gate of the surf search (L:1615, R:1476) */
+    double surf_dist_thres;                 /* plane gate (L:1651) */
+    double w_gate;                          /* weight gate (L:1665 0.2, R:1504 0.3) */
+    double lidar_const;                     /* L:1581 / :1676, R:843 */
+    double reflect_thres;                   /* L:1628 (variant 0 only) */
+    double cauchy_b;                        /* ceres::CauchyLoss(1.0), L:845 */
+    double q_lb[4], t_lb[3];                /* lidar -> body extrinsics of LidarPlaneNormFactor (wxyz, metres) */
+} liliom_backend_params;
+/* The values of L/config/config_fr_iosb.yaml (variant 0) and R/config/config_fr_iosb.yaml (variant 1). */
+void liliom_backend_default_params(liliom_backend_params* p, int variant);
+
+/* Keyframe store: BackendFusion::downSampleCloud, scan half (L:1502-1514) + saveKeyFramesAndFactors' clouds (:1688-1695).
+ * VoxelGrid(edge_leaf) / VoxelGrid(surf_leaf) of the received body-frame clouds on the device, appended to a device arena.
+ * *kf_id = 0, 1, 2, ... in call order.  Host outputs are optional (NULL: no download; LILIOM_E_CAPACITY when too small).
+ * The arena grows geometrically (copying); steady state allocates nothing. */
+int liliom_kf_add(liliom_ctx* c, const liliom_backend_params* bp, const void* edge_last, int n_edge, const void* surf_last, int n_surf,
+                  int* kf_id, void* edge_ds_out, int edge_cap, int* n_edge_ds, void* surf_ds_out, int surf_cap, int* n_surf_ds);
+int liliom_kf_count(const liliom_ctx* c);
+int liliom_kf_clear(liliom_ctx* c);      /* drops every keyframe, the local map and the window correspondences */
+
+/* Backend local map: buildLocalMapWithLandMark (L:1387-1484) + downSampleCloud, map half (:1486-1492).  For each listed keyframe,
+ * in list order, its stored clouds transformed by poses7[i] (transformCloud, :730-767; the caller composes q_po*q_bl,
+ * q_po*t_bl + t_po as at :1425-1426), edge and surf concatenated separately (:1479-1483), VoxelGrid(edge_leaf) /
+ * VoxelGrid(surf_leaf), a cell grid per layer (edge: the 1.0 gate of :1543; surf: kd_max_radius).  Stateless: the reference's
+ * deque policy (:1407-1477) stays with the caller, who passes each deque entry's cached pose.  An unknown id: LILIOM_E_ARG,
+ * the previous layers stay.  k = 0 builds empty layers. */
+int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7, int k,
+                      int* n_edge_map, int* n_surf_map);
+/* edge_local_map_ds (layer 0) / surf_local_map_ds (layer 1) with all fields (published on every run, :1516-1526).
+ * out = NULL: *m = size only. */
+int liliom_bmap_download(liliom_ctx* c, int layer, void* out, int cap, int* m);
+
+/* optimizeSlidingWindowWithLandMark, LiDAR rows (L:919-979, again at :1087-1148).  The caller passes the lidar poses
+ * Q2 = Q * q_lb^-1, T2 = T - Q2 * t_lb (:929-930) and the keyframe ids (the reference's idx-1, :935-936), k <= 16.  Runs the
+ * edge search (L:1531-1599 / R:1394-1462) and the surf search (L:1601-1681 / R:1464-1520) of every window keyframe against the
+ * two layers (one launch per kind); the correspondences stay on the device.  n_*_corr[i] = found correspondences of keyframe i.
+ * The gate of :933 (surf layer > 50 && edge layer > 0) failing: LILIOM_E_FEWMAP, counts 0, nothing resident. */
+int liliom_backend_window_correspond(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7_lidar,
+                                     int k, int* n_edge_corr, int* n_surf_corr);
+/* Every LidarEdgeFactor / LidarPlaneNormFactor row of every window keyframe at its body pose poses7_body[i] under
+ * CauchyLoss(cauchy_b), reduced per keyframe and kind as liliom_backend_edge_block / _surf_block do (same partition, same
+ * fixed-order sums): out29[i][0] = edge block, out29[i][1] = surf block of keyframe i (k * 2 * 29 doubles).  The variant's weights
+ * are applied on the device: variant 1 s = fl(fl(fl(lidar_const)*200)/N_edge) (R:843), score*1000/N_surf in double (R:861);
+ * variant 0 s = (double)(float)lidar_const (L:1581).  k must be the k of the resident window; may be called repeatedly. */
+int liliom_backend_window_blocks(liliom_ctx* c, const double* poses7_body, int k, double* out29);
+/* Test hook: one window keyframe's resident correspondences.  kind 0: valid, a (3 floats), b (3 floats) per edge query;
+ * kind 1: valid, plane (4 floats), score (1 double) per surf query.  *n = that keyframe's query count. */
+int liliom_backend_window_corr(liliom_ctx* c, int slot, int kind, unsigned char* valid, void* a, void* b, int cap, int* n);
+
+/* Loop-closure clouds from the store, detectLoopClosure (L:2473-2547): per keyframe, edge THEN surf (:2492-2493, :2519-2520)
+ * transformed by poses7[i], concatenated, VoxelGrid(leaf), downloaded (out = NULL: *n only).  The result feeds liliom_icp_align. */
+int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, float leaf, void* out, int cap, int* n);
+
 /* ---- SURVEY §8 (f3): wire format on the sensor side — FormatConvert's livoxLidarHandler on the device ----
  * L/src/FormatConvert.cpp:11-24: livox_ros_driver::CustomPoint {uint32 offset_time; float x,y,z; uint8 reflectivity,
  * tag, line} -> pcl::PointXYZINormal with intensity = line + 0.1*float(offset_time/(float)time_end) (:19-20),

@@ -44,6 +44,13 @@ class IterStats(C.Structure):
                 ("jtj_jtr", C.c_double * 27), ("pose7", C.c_double * 7)]
 
 
+class BackendParams(C.Structure):
+    """liliom_backend_params (include/liliom.h): the BackendFusion settings the keyframe store, local map and window use."""
+    _fields_ = [("variant", C.c_int), ("edge_leaf", C.c_float), ("surf_leaf", C.c_float),
+                ("kd_max_radius", C.c_double), ("surf_dist_thres", C.c_double), ("w_gate", C.c_double), ("lidar_const", C.c_double),
+                ("reflect_thres", C.c_double), ("cauchy_b", C.c_double), ("q_lb", C.c_double * 4), ("t_lb", C.c_double * 3)]
+
+
 class Counters(C.Structure):
     _fields_ = [("launches", C.c_ulonglong), ("lib_launches", C.c_ulonglong), ("knn_ms", C.c_double),
                 ("knn_launches", C.c_ulonglong), ("knn_queries", C.c_ulonglong), ("knn_candidates", C.c_ulonglong)]
@@ -63,6 +70,9 @@ EXPORTS = [
     "liliom_map_push_frame_device", "liliom_knn_block_stats", "liliom_comm_set_shard_block", "liliom_undistort",
     "liliom_map_update", "liliom_map_update_device", "liliom_map_download_cloud", "liliom_icp_align",
     "liliom_comm_peer_epoch", "liliom_comm_peer_set_epoch",
+    "liliom_backend_default_params", "liliom_kf_add", "liliom_kf_count", "liliom_kf_clear", "liliom_bmap_build",
+    "liliom_bmap_download", "liliom_backend_window_correspond", "liliom_backend_window_blocks", "liliom_backend_window_corr",
+    "liliom_kf_cloud",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -155,6 +165,17 @@ def lib() -> C.CDLL:
     L.liliom_map_download_cloud.argtypes = [vp, vp, C.c_int, ip]
     L.liliom_icp_align.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_double, C.c_double, dp, dp, ip, ip]
     L.liliom_knn_block_stats.argtypes = [vp, dp, C.POINTER(C.c_ulonglong)]
+    bpp = C.POINTER(BackendParams)
+    L.liliom_backend_default_params.argtypes = [bpp, C.c_int]; L.liliom_backend_default_params.restype = None
+    L.liliom_kf_add.argtypes = [vp, bpp, vp, C.c_int, vp, C.c_int, ip, vp, C.c_int, ip, vp, C.c_int, ip]
+    L.liliom_kf_count.argtypes = [vp]
+    L.liliom_kf_clear.argtypes = [vp]
+    L.liliom_bmap_build.argtypes = [vp, bpp, ip, dp, C.c_int, ip, ip]
+    L.liliom_bmap_download.argtypes = [vp, C.c_int, vp, C.c_int, ip]
+    L.liliom_backend_window_correspond.argtypes = [vp, bpp, ip, dp, C.c_int, ip, ip]
+    L.liliom_backend_window_blocks.argtypes = [vp, dp, C.c_int, dp]
+    L.liliom_backend_window_corr.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, ip]
+    L.liliom_kf_cloud.argtypes = [vp, ip, dp, C.c_int, C.c_float, vp, C.c_int, ip]
     L.liliom_pre_create.argtypes = [vp, C.c_int, dp]; L.liliom_pre_create.restype = vp
     L.liliom_pre_destroy.argtypes = [vp]; L.liliom_pre_destroy.restype = None
     L.liliom_pre_imu.argtypes = [vp, C.c_double, dp]; L.liliom_pre_imu.restype = None
@@ -181,6 +202,22 @@ def _ptr(a: np.ndarray | None):
 
 def _dptr(a: np.ndarray):
     return a.ctypes.data_as(C.POINTER(C.c_double))
+
+
+def backend_default_params(variant: int = 0) -> BackendParams:
+    p = BackendParams()
+    lib().liliom_backend_default_params(C.byref(p), variant)
+    return p
+
+
+def _ids(ids):
+    return np.ascontiguousarray(ids, dtype=np.int32).reshape(-1)
+
+
+def _poses(poses7, k):
+    p = np.ascontiguousarray(poses7, dtype=np.float64).reshape(-1, 7) if k else np.zeros((1, 7))
+    assert len(p) >= k
+    return p
 
 
 def default_params(variant: int = 0) -> Params:
@@ -443,6 +480,80 @@ class Context:
         self._check(lib().liliom_backend_surf_block(self._h, _dptr(np.asarray(pose7_body, np.float64)), _dptr(np.asarray(q_lb, np.float64)),
                                                     _dptr(np.asarray(t_lb, np.float64)), float(cauchy_b), _dptr(out)))
         return out
+
+    # ---- backend keyframe store, local map and window (f5) ----
+    def kf_add(self, bp: BackendParams, edge_last: np.ndarray, surf_last: np.ndarray, download: bool = True):
+        """downSampleCloud (scan half) + store: returns (kf_id, edge_ds, surf_ds); the clouds are None when download=False."""
+        e = np.ascontiguousarray(edge_last, dtype=self.dtype); s = np.ascontiguousarray(surf_last, dtype=self.dtype)
+        kid, ne, ns = C.c_int(), C.c_int(), C.c_int()
+        eo = np.zeros(max(len(e), 1), self.dtype) if download else None
+        so = np.zeros(max(len(s), 1), self.dtype) if download else None
+        self._check(lib().liliom_kf_add(self._h, C.byref(bp), _ptr(e), len(e), _ptr(s), len(s), C.byref(kid),
+                                        _ptr(eo), len(eo) if download else 0, C.byref(ne), _ptr(so), len(so) if download else 0, C.byref(ns)))
+        if not download:
+            return kid.value, None, None
+        return kid.value, eo[:ne.value], so[:ns.value]
+
+    def kf_count(self) -> int:
+        return lib().liliom_kf_count(self._h)
+
+    def kf_clear(self):
+        self._check(lib().liliom_kf_clear(self._h))
+
+    def bmap_build(self, bp: BackendParams, kf_ids, poses7):
+        """buildLocalMapWithLandMark + downSampleCloud (map half) on the device: returns (edge layer size, surf layer size)."""
+        ids = _ids(kf_ids); p = _poses(poses7, len(ids))
+        ne, ns = C.c_int(), C.c_int()
+        self._check(lib().liliom_bmap_build(self._h, C.byref(bp), ids.ctypes.data_as(C.POINTER(C.c_int)), _dptr(p), len(ids),
+                                            C.byref(ne), C.byref(ns)))
+        return ne.value, ns.value
+
+    def bmap_download(self, layer: int) -> np.ndarray:
+        """edge_local_map_ds (layer 0) or surf_local_map_ds (layer 1), all fields."""
+        m = C.c_int()
+        self._check(lib().liliom_bmap_download(self._h, layer, None, 0, C.byref(m)))
+        out = np.zeros(max(m.value, 1), self.dtype)
+        self._check(lib().liliom_bmap_download(self._h, layer, _ptr(out), len(out), C.byref(m)))
+        return out[:m.value]
+
+    def backend_window_correspond(self, bp: BackendParams, kf_ids, poses7_lidar):
+        """Edge and surf searches of the window keyframes against the local map: returns (n_edge_corr, n_surf_corr) per keyframe."""
+        ids = _ids(kf_ids); k = len(ids); p = _poses(poses7_lidar, k)
+        ne = np.zeros(max(k, 1), np.int32); ns = np.zeros(max(k, 1), np.int32)
+        ipp = C.POINTER(C.c_int)
+        self._check(lib().liliom_backend_window_correspond(self._h, C.byref(bp), ids.ctypes.data_as(ipp), _dptr(p), k,
+                                                           ne.ctypes.data_as(ipp), ns.ctypes.data_as(ipp)))
+        return ne[:k], ns[:k]
+
+    def backend_window_blocks(self, poses7_body) -> np.ndarray:
+        """(k, 2, 29): the edge and surf normal-equation blocks of every window keyframe at its body pose."""
+        p = np.ascontiguousarray(poses7_body, dtype=np.float64).reshape(-1, 7)
+        out = np.zeros((len(p), 2, 29))
+        self._check(lib().liliom_backend_window_blocks(self._h, _dptr(p), len(p), _dptr(out)))
+        return out
+
+    def backend_window_corr(self, slot: int, kind: int):
+        """Test hook: (valid, pa, pb) of window keyframe `slot` for kind 0, (valid, plane, score) for kind 1."""
+        n = C.c_int()
+        self._check(lib().liliom_backend_window_corr(self._h, slot, kind, None, None, None, 0, C.byref(n)))
+        m = max(n.value, 1)
+        valid = np.zeros(m, np.uint8)
+        if kind == 0:
+            a = np.zeros((m, 3), np.float32); b = np.zeros((m, 3), np.float32)
+        else:
+            a = np.zeros((m, 4), np.float32); b = np.zeros(m, np.float64)
+        self._check(lib().liliom_backend_window_corr(self._h, slot, kind, _ptr(valid), _ptr(a), _ptr(b), m, C.byref(n)))
+        return valid[:n.value], a[:n.value], b[:n.value]
+
+    def kf_cloud(self, kf_ids, poses7, leaf: float) -> np.ndarray:
+        """detectLoopClosure's clouds: edge then surf of every listed keyframe, transformed, VoxelGrid(leaf)."""
+        ids = _ids(kf_ids); p = _poses(poses7, len(ids))
+        ipp = C.POINTER(C.c_int)
+        n = C.c_int()
+        self._check(lib().liliom_kf_cloud(self._h, ids.ctypes.data_as(ipp), _dptr(p), len(ids), leaf, None, 0, C.byref(n)))
+        out = np.zeros(max(n.value, 1), self.dtype)
+        self._check(lib().liliom_kf_cloud(self._h, ids.ctypes.data_as(ipp), _dptr(p), len(ids), leaf, _ptr(out), len(out), C.byref(n)))
+        return out[:n.value]
 
     # ---- wire formats (f3) ----
     @staticmethod

@@ -59,20 +59,7 @@ __global__ void k_compact_f4(const float4* __restrict__ in, const int* __restric
 __global__ void k_transform_cloud(const unsigned char* __restrict__ in, int n, int stride, Q4 q, D3 t, unsigned char* __restrict__ out) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float4 a = *reinterpret_cast<const float4*>(in + (size_t)i * stride);
-    D3 r = qrot_x(q, D3{(double)a.x, (double)a.y, (double)a.z});
-    float4 o = make_float4((float)addx(r.x, t.x), (float)addx(r.y, t.y), (float)addx(r.z, t.z), 1.0f);
-    *reinterpret_cast<float4*>(out + (size_t)i * stride) = o;
-    if (stride == 48) {
-        const float4 b = *reinterpret_cast<const float4*>(in + (size_t)i * stride + 16);
-        const float4 cc = *reinterpret_cast<const float4*>(in + (size_t)i * stride + 32);
-        D3 nr = qrot_x(q, D3{(double)b.x, (double)b.y, (double)b.z});
-        *reinterpret_cast<float4*>(out + (size_t)i * stride + 16) = make_float4((float)nr.x, (float)nr.y, (float)nr.z, 0.f);
-        *reinterpret_cast<float4*>(out + (size_t)i * stride + 32) = make_float4(cc.x, cc.y, 0.f, 0.f);
-    } else {
-        const float4 b = *reinterpret_cast<const float4*>(in + (size_t)i * stride + 16);
-        *reinterpret_cast<float4*>(out + (size_t)i * stride + 16) = make_float4(b.x, 0.f, 0.f, 0.f);
-    }
+    pcl_transform_point(in + (size_t)i * stride, stride, q, t, out + (size_t)i * stride);
 }
 
 // Concatenation of the FIFO frames (L/src/LidarOdometry.cpp:301-302) in ONE launch: blockIdx.y = frame, the blocks of a row
@@ -122,7 +109,7 @@ __global__ void k_gather_refl48(const unsigned char* __restrict__ pts, int n, fl
 }
 
 static int install_map_from_xyzw(liliom_ctx* c, int m) {
-    // c->map_xyzw holds m float4 (w = global index).  Shard when a communicator is attached.
+    // c->map.xyzw holds m float4 (w = global index).  Shard when a communicator is attached.
     c->map_n_global = m;
     if (c->nranks > 1 && m > 0) {
         LILI_CUDA(c, c->flags.ensure(((size_t)m + 2) * 4));
@@ -130,15 +117,15 @@ static int install_map_from_xyzw(liliom_ctx* c, int m) {
         LILI_CUDA(c, c->map_ds.ensure((size_t)m * sizeof(float4)));
         float cell = 1.0f;
         while ((double)cell * (double)cell < c->prm.knn_max_sqdist) cell *= 2.0f;
-        k_shard_flags<<<cdiv(m + 1, 256), 256, 0, c->stream>>>(c->map_xyzw.as<float4>(), m, cell, c->shard_inv_block, c->nranks, c->rank, c->flags.as<int>());
+        k_shard_flags<<<cdiv(m + 1, 256), 256, 0, c->stream>>>(c->map.xyzw.as<float4>(), m, cell, c->shard_inv_block, c->nranks, c->rank, c->flags.as<int>());
         LILI_TRY(launch_check(c, "k_shard_flags"));
         LILI_TRY(exclusive_scan_i32(c, c->flags.as<int>(), c->idx_a.as<int>(), m));
-        k_compact_f4<<<cdiv(m, 256), 256, 0, c->stream>>>(c->map_xyzw.as<float4>(), c->flags.as<int>(), c->idx_a.as<int>(), m, c->map_ds.as<float4>());
+        k_compact_f4<<<cdiv(m, 256), 256, 0, c->stream>>>(c->map.xyzw.as<float4>(), c->flags.as<int>(), c->idx_a.as<int>(), m, c->map_ds.as<float4>());
         LILI_TRY(launch_check(c, "k_compact_f4"));
         int local = 0;
         LILI_CUDA(c, cudaMemcpyAsync(&local, c->idx_a.as<int>() + m, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
         LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-        LILI_CUDA(c, cudaMemcpyAsync(c->map_xyzw.p, c->map_ds.p, (size_t)local * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
+        LILI_CUDA(c, cudaMemcpyAsync(c->map.xyzw.p, c->map_ds.p, (size_t)local * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
         m = local;
     }
     return grid_build(c, m);
@@ -256,11 +243,12 @@ extern "C" void liliom_destroy(liliom_ctx* c) {
                       &c->hz_stage_edge, &c->hz_counts, &c->rot_keys, &c->rot_keys2, &c->rot_vals, &c->rot_vals2, &c->rot_cloud, &c->rot_curv,
                       &c->rot_label, &c->rot_picked, &c->rot_sort, &c->rot_ring, &c->rot_meta, &c->rot_lessflat, &c->rot_seg_edge, &c->vg_keys,
                       &c->vg_keys2, &c->vg_vals, &c->vg_vals2, &c->vg_flags, &c->vg_rank, &c->vg_params, &c->vg_out, &c->vg_minmax, &c->vg_count,
-                      &c->cub_tmp, &c->vg_coop, &c->hz_ctl, &c->map_raw, &c->map_ds, &c->map_xyzw, &c->map_sorted, &c->cell_start, &c->grid_keys, &c->grid_keys2,
+                      &c->cub_tmp, &c->vg_coop, &c->hz_ctl, &c->map_raw, &c->map_ds, &c->map.xyzw, &c->map.sorted, &c->map.cell_start, &c->grid_keys, &c->grid_keys2,
                       &c->grid_vals, &c->grid_vals2, &c->feats, &c->corr_valid, &c->corr_plane, &c->nn_idx, &c->nn_sqd, &c->pose_dev,
-                      &c->partials, &c->neq, &c->stats_dev, &c->counter, &c->lm_state, &c->raw_scan, &c->map_refl, &c->livox_in, &c->qstate, &c->inc_key[0], &c->inc_key[1], &c->inc_ref[0], &c->inc_ref[1], &c->inc_newkey[0], &c->inc_newkey[1],
+                      &c->partials, &c->neq, &c->stats_dev, &c->counter, &c->lm_state, &c->raw_scan, &c->map.refl, &c->livox_in, &c->qstate, &c->inc_key[0], &c->inc_key[1], &c->inc_ref[0], &c->inc_ref[1], &c->inc_newkey[0], &c->inc_newkey[1],
                       &c->inc_newref[0], &c->inc_newref[1], &c->inc_removed, &c->inc_rpos, &c->inc_flags, &c->inc_rank, &c->inc_mm};
     for (DevBuf* b : bufs) b->release();
+    backend_release(c);
     for (auto& f : c->frames) f.buf.release();
     for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
     if (c->h_pin) cudaFreeHost(c->h_pin);
@@ -445,7 +433,7 @@ extern "C" int liliom_map_clear(liliom_ctx* c) {
     for (auto& f : c->frames) f.buf.release();
     c->frames.clear();
     c->inc_valid = false;
-    c->map_ready = false; c->map_n = 0; c->map_n_global = 0;
+    c->map.ready = false; c->map.n = 0; c->map_n_global = 0;
     return LILIOM_OK;
 }
 
@@ -540,9 +528,9 @@ void frames_box(const liliom_ctx* c, int mm[7]) {
 
 int map_finish_from_ds(liliom_ctx* c, int m) {
     const int stride = c->prm.point_stride;
-    LILI_CUDA(c, c->map_xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
+    LILI_CUDA(c, c->map.xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
     c->map_n_global = m;
-    LILI_TRY(repack_to_f4(c, c->map_ds.p, m, stride, c->map_xyzw.as<float4>()));
+    LILI_TRY(repack_to_f4(c, c->map_ds.p, m, stride, c->map.xyzw.as<float4>()));
     int mm[7];
     frames_box(c, mm);
     LILI_TRY(grid_build(c, m, mm[6] > 0 ? mm : nullptr));
@@ -561,7 +549,7 @@ static int map_update_from_device(liliom_ctx* c, const void* d_src, int n, const
     if ((int)c->frames.size() >= c->prm.max_map_frames && !c->frames.empty()) { popped_slot = c->frames.front().slot; popped_nfin = c->frames.front().nfin; }
     LILI_TRY(push_frame_from_device(c, d_src, n, pose7, incremental));
     if (incremental) {
-        c->map_ready = false; c->map_n = 0; c->map_n_global = 0;
+        c->map.ready = false; c->map.n = 0; c->map_n_global = 0;
         int m = 0;
         const int rc = map_inc_update(c, popped_slot, popped_nfin, &m);
         if (rc == LILIOM_OK) {
@@ -619,9 +607,9 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
     mark();
     size_t total = 0;
     for (auto& f : c->frames) total += (size_t)f.n;
-    c->map_ready = false; c->map_n = 0; c->map_n_global = 0;
+    c->map.ready = false; c->map.n = 0; c->map_n_global = 0;
     if (n_map_out) *n_map_out = 0;
-    if (total == 0 && c->nranks == 1) { c->map_ready = true; return LILIOM_OK; }
+    if (total == 0 && c->nranks == 1) { c->map.ready = true; return LILIOM_OK; }
     LILI_CUDA(c, c->map_raw.ensure((total > 0 ? total : 1) * stride));
     LILI_CUDA(c, c->map_ds.ensure((total > 0 ? total : 1) * stride));
     LILI_CUDA(c, c->vg_count.ensure(16));
@@ -629,7 +617,7 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
     int box[7];
     frames_box(c, box);
     // single GPU: the centroid kernel writes the float4 map itself (no repack pass); at most `total` voxels
-    if (c->nranks == 1) LILI_CUDA(c, c->map_xyzw.ensure((total > 0 ? total : 1) * sizeof(float4)));
+    if (c->nranks == 1) LILI_CUDA(c, c->map.xyzw.ensure((total > 0 ? total : 1) * sizeof(float4)));
     size_t off = 0;
     if (c->frames.size() <= (size_t)kConcatMax && total > 0) {
         ConcatTab tab{};
@@ -654,13 +642,13 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
         // (The single-launch cooperative filter of the scan VoxelGrid was tried here for maps of <= 32k points: within the noise
         // of the real-size streamed lifecycle — not kept.)
         LILI_TRY(voxelgrid_dev(c, c->map_raw.p, (int)total, stride, c->prm.leaf_map, c->map_ds.p, c->vg_count.as<int>(),   // :316-317
-                               c->nranks == 1 ? c->map_xyzw.as<float4>() : nullptr, box));
+                               c->nranks == 1 ? c->map.xyzw.as<float4>() : nullptr, box));
         LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->vg_count, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
         LILI_CUDA(c, cudaStreamSynchronize(c->stream));
         m = c->h_pin->vg_count;
     }
     mark();      // [2] VoxelGrid
-    LILI_CUDA(c, c->map_xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
+    LILI_CUDA(c, c->map.xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
     c->map_n_global = m;
     if (c->nranks > 1) {
         // Every rank ENTERS the all-reduce whatever happened locally (a rank that returned early would leave its peers waiting
@@ -678,7 +666,7 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
                 LILI_TRY(launch_check(c, "k_shard_flags_strided"));
                 LILI_TRY(exclusive_scan_i32(c, c->flags.as<int>(), c->idx_a.as<int>(), m));
                 k_compact_repack<<<cdiv(m, 256), 256, 0, c->stream>>>((const unsigned char*)c->map_ds.p, c->flags.as<int>(), c->idx_a.as<int>(), m, stride,
-                                                                     c->map_xyzw.as<float4>());
+                                                                     c->map.xyzw.as<float4>());
                 LILI_TRY(launch_check(c, "k_compact_repack"));
                 LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->kept, c->idx_a.as<int>() + m, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
                 LILI_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -691,14 +679,14 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
         // the "< 10 map points" guard (L/src/LidarOdometry.cpp:485-488) is about the whole map: sum the owned-voxel counts
         LILI_CUDA(c, c->neq.ensure(32 * sizeof(double)));
         double* pin = c->h_pin->map_status;
-        pin[0] = rc_local == LILIOM_OK ? (double)c->map_n : 0.0;
+        pin[0] = rc_local == LILIOM_OK ? (double)c->map.n : 0.0;
         pin[1] = rc_local == LILIOM_OK ? 0.0 : 1.0;
         LILI_CUDA(c, cudaMemcpyAsync(c->neq.p, pin, 2 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
         LILI_TRY(nccl_allreduce_sum_f64(c, c->neq.as<double>(), 2));
         LILI_CUDA(c, cudaMemcpyAsync(pin + 2, c->neq.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
         LILI_CUDA(c, cudaStreamSynchronize(c->stream));
         if (rc_local != LILIOM_OK) return rc_local;
-        if (pin[3] != 0.0) { c->map_ready = false; c->last_error = "liliom_map_rebuild failed on another rank"; return LILIOM_E_NCCL; }
+        if (pin[3] != 0.0) { c->map.ready = false; c->last_error = "liliom_map_rebuild failed on another rank"; return LILIOM_E_NCCL; }
         c->map_n_global = (int)pin[2];                  // halo voxels are counted on several ranks: an upper bound >= the true size
     } else {
         LILI_TRY(grid_build(c, m, box[6] > 0 ? box : nullptr));     // map_xyzw was written by the VoxelGrid's centroid kernel
@@ -718,13 +706,13 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
 extern "C" int liliom_map_set_points(liliom_ctx* c, const liliom_f4* xyzw, int m) {
     if (!c || m < 0 || (m > 0 && !xyzw)) return LILIOM_E_ARG;
     LILI_CUDA(c, cudaSetDevice(c->device));
-    c->map_refl.release();
-    c->map_ready = false;
-    LILI_CUDA(c, c->map_xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
+    c->map.refl.release();
+    c->map.ready = false;
+    LILI_CUDA(c, c->map.xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
     LILI_CUDA(c, c->raw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
     if (m > 0) {
         LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, xyzw, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice, c->stream));
-        LILI_TRY(repack_to_f4(c, c->raw.p, m, 16, c->map_xyzw.as<float4>()));
+        LILI_TRY(repack_to_f4(c, c->raw.p, m, 16, c->map.xyzw.as<float4>()));
     }
     LILI_TRY(install_map_from_xyzw(c, m));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -736,33 +724,33 @@ extern "C" int liliom_map_set_cloud(liliom_ctx* c, const void* pts, int m, int s
     if (!c || m < 0 || (m > 0 && !pts) || (stride != 48 && stride != 32)) return LILIOM_E_ARG;
     LILI_CUDA(c, cudaSetDevice(c->device));
     if (c->nranks > 1) { c->last_error = "liliom_map_set_cloud is single-GPU"; return LILIOM_E_ARG; }
-    c->map_ready = false;
-    LILI_CUDA(c, c->map_xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
-    LILI_CUDA(c, c->map_refl.ensure((size_t)(m > 0 ? m : 1) * sizeof(float)));
+    c->map.ready = false;
+    LILI_CUDA(c, c->map.xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
+    LILI_CUDA(c, c->map.refl.ensure((size_t)(m > 0 ? m : 1) * sizeof(float)));
     LILI_CUDA(c, c->raw.ensure((size_t)(m > 0 ? m : 1) * stride));
     if (m > 0) {
         LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, pts, (size_t)m * stride, cudaMemcpyHostToDevice, c->stream));
-        LILI_TRY(repack_to_f4(c, c->raw.p, m, stride, c->map_xyzw.as<float4>()));
+        LILI_TRY(repack_to_f4(c, c->raw.p, m, stride, c->map.xyzw.as<float4>()));
         if (stride == 48) {
-            k_gather_refl48<<<cdiv(m, 256), 256, 0, c->stream>>>((const unsigned char*)c->raw.p, m, c->map_refl.as<float>());
+            k_gather_refl48<<<cdiv(m, 256), 256, 0, c->stream>>>((const unsigned char*)c->raw.p, m, c->map.refl.as<float>());
             LILI_TRY(launch_check(c, "k_gather_refl48"));
-        } else LILI_CUDA(c, cudaMemsetAsync(c->map_refl.p, 0, (size_t)m * sizeof(float), c->stream));
+        } else LILI_CUDA(c, cudaMemsetAsync(c->map.refl.p, 0, (size_t)m * sizeof(float), c->stream));
     }
     LILI_TRY(install_map_from_xyzw(c, m));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     return LILIOM_OK;
 }
 
-extern "C" int liliom_map_size(const liliom_ctx* c) { return c ? c->map_n : 0; }
+extern "C" int liliom_map_size(const liliom_ctx* c) { return c ? c->map.n : 0; }
 
 extern "C" int liliom_map_download(liliom_ctx* c, liliom_f4* out, int cap, int* m_out) {
     if (!c || !m_out) return LILIOM_E_ARG;
     LILI_CUDA(c, cudaSetDevice(c->device));
-    const int m = c->map_n;
+    const int m = c->map.n;
     *m_out = m;
     if (!out) return LILIOM_OK;
     if (m > cap) return LILIOM_E_CAPACITY;
-    if (m) LILI_CUDA(c, cudaMemcpyAsync(out, c->map_xyzw.p, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
+    if (m) LILI_CUDA(c, cudaMemcpyAsync(out, c->map.xyzw.p, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     return LILIOM_OK;
 }
@@ -786,7 +774,7 @@ extern "C" int liliom_scan_to_map(liliom_ctx* c, const void* feats, int n, int s
                                   int mode, liliom_iter_stats* stats) {
     if (!c || !pose7 || (mode != LILIOM_MODE_CERES && mode != LILIOM_MODE_GN) || match_cnt < 0) return LILIOM_E_ARG;
     LILI_CUDA(c, cudaSetDevice(c->device));
-    if (!c->map_ready) return LILIOM_E_NOMAP;
+    if (!c->map.ready) return LILIOM_E_NOMAP;
     if (c->map_n_global < 10) return LILIOM_E_FEWMAP;
     LILI_TRY(upload_feats(c, feats, n, stride));
     return s2m_run(c, pose7, match_cnt, max_num_iter, mode, stats, false, nullptr);
@@ -875,7 +863,7 @@ static int odometry_on_resident_surf(liliom_ctx* c, double pose7[7], int match_c
     }
     c->n_feats = n_max;
     int rc = LILIOM_OK;
-    if (!c->map_ready) rc = LILIOM_E_NOMAP;
+    if (!c->map.ready) rc = LILIOM_E_NOMAP;
     else if (c->map_n_global < 10) rc = LILIOM_E_FEWMAP;
     double pose_in[7];
     memcpy(pose_in, pose7, sizeof(pose_in));
@@ -918,7 +906,7 @@ extern "C" int liliom_find_surf_corr(liliom_ctx* c, const void* feats, int n, in
                                      float* plane, int* nn_idx, float* sqd, double out29[29]) {
     if (!c || !pose7) return LILIOM_E_ARG;
     LILI_CUDA(c, cudaSetDevice(c->device));
-    if (!c->map_ready) return LILIOM_E_NOMAP;
+    if (!c->map.ready) return LILIOM_E_NOMAP;
     if (c->map_n_global < 10) return LILIOM_E_FEWMAP;
     LILI_TRY(upload_feats(c, feats, n, stride));
     double p[7];
@@ -942,14 +930,14 @@ extern "C" int liliom_icp_align(liliom_ctx* c, const void* src, int n_src, const
     LILI_CUDA(c, cudaSetDevice(c->device));
     if (c->nranks > 1) { c->last_error = "liliom_icp_align is single-GPU"; return LILIOM_E_ARG; }
     // target -> the context's map (cell grid), source -> the resident query array
-    c->map_refl.release();
-    c->map_ready = false;
+    c->map.refl.release();
+    c->map.ready = false;
     c->inc_valid = false;
-    LILI_CUDA(c, c->map_xyzw.ensure((size_t)(n_tgt > 0 ? n_tgt : 1) * sizeof(float4)));
+    LILI_CUDA(c, c->map.xyzw.ensure((size_t)(n_tgt > 0 ? n_tgt : 1) * sizeof(float4)));
     LILI_CUDA(c, c->raw.ensure((size_t)(n_tgt > 0 ? n_tgt : 1) * stride));
     if (n_tgt > 0) {
         LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, tgt, (size_t)n_tgt * stride, cudaMemcpyHostToDevice, c->stream));
-        LILI_TRY(repack_to_f4(c, c->raw.p, n_tgt, stride, c->map_xyzw.as<float4>()));
+        LILI_TRY(repack_to_f4(c, c->raw.p, n_tgt, stride, c->map.xyzw.as<float4>()));
     }
     LILI_TRY(install_map_from_xyzw(c, n_tgt));
     LILI_TRY(upload_feats(c, src, n_src, stride));

@@ -48,6 +48,29 @@ struct GridDesc {
     int   ncells;
 };
 
+// One searchable point set: the float4 points, their cell grid and (optionally) a reflectivity channel.  grid_build writes it.
+// The odometry map (liliom_ctx::map) and the two layers of the backend local map (liliom_ctx::bmap) are each one.
+struct MapIndex {
+    DevBuf xyzw;                         // float4 in download order (w = index)
+    DevBuf refl;                         // optional per-point reflectivity channel (liliom_map_set_cloud, backend surf layer)
+    DevBuf sorted;                       // float4 sorted by cell, w = original index bits
+    DevBuf cell_start;                   // ncells + 1
+    GridDesc grid{};
+    int  n = 0;                          // points resident on this rank (sorted grid)
+    bool ready = false;
+    void release() { xyzw.release(); refl.release(); sorted.release(); cell_start.release(); n = 0; ready = false; }
+};
+
+// Cell edge for a squared-distance gate: the smallest power of two whose square reaches it (1.0 for the reference's gates).
+inline float gate_cell(double sqgate) {
+    float cell = 1.0f;
+    while ((double)cell * (double)cell < sqgate) cell *= 2.0f;
+    return cell;
+}
+
+// Keyframe store (keyframes.cu): body-frame clouds of every keyframe in one device arena, edge then surf per keyframe.
+struct KfEntry { long long edge_off, surf_off; int n_edge, n_surf; };   // offsets in points
+
 // Fused multi-GPU exchange (single node): pointers to every rank's exchange buffer (own entry = own buffer), see
 // peer_exchange() in grid_knn.cu.  Passed to the persistent GN kernel by value.
 constexpr int kMaxPeers = 16;
@@ -81,6 +104,7 @@ struct PinBlock {
     int    escaped;            // grid_build: a point lies outside the handed-in box
     double map_status[4];      // multi-rank map rebuild: {owned voxels, failed} out, their sums over the ranks back
     unsigned long long block27[2];   // block27_stats: queries, points in their cell blocks
+    int    bk_cnt[2 * 16];     // backend: VoxelGrid output counts (keyframe store, local map), window correspondence counts [kind][16]
     double stats[];            // kStatsDoubles per GN iteration, up to the end of the block (h_pin_bytes)
 };
 
@@ -169,15 +193,24 @@ struct liliom_ctx {
     bool inc_valid = false;
     lili::DevBuf map_raw;                // concatenated frames (stride bytes)
     lili::DevBuf map_ds;                 // VoxelGrid output (stride bytes) or installed float4
-    lili::DevBuf map_xyzw;               // float4 in map_download order (w = index)
-    lili::DevBuf map_refl;               // optional per-point reflectivity channel (liliom_map_set_cloud)
-    lili::DevBuf map_sorted;             // float4 sorted by cell, w = original index bits
-    lili::DevBuf cell_start;             // ncells + 1
-    lili::DevBuf grid_keys, grid_keys2, grid_vals, grid_vals2;
-    lili::GridDesc grid{};
-    int map_n = 0;                       // points resident on this rank (sorted grid)
+    lili::MapIndex map;                  // the odometry map's search index (scan-to-map, backend single-keyframe calls, ICP target)
+    lili::DevBuf grid_keys, grid_keys2, grid_vals, grid_vals2;   // grid_build scratch, shared by every index
     int map_n_global = 0;
-    bool map_ready = false;
+
+    // ---- backend (keyframes.cu, backend_corr.cu): keyframe store, local map layers, window correspondences ----
+    lili::DevBuf kf_arena;               // body-frame clouds of every keyframe (point_stride bytes per point)
+    long long kf_used = 0;               // points in use
+    std::vector<lili::KfEntry> kfs;      // per keyframe: offsets and counts (host)
+    lili::DevBuf kf_tab;                 // per-call gather table (k_kf_gather)
+    lili::MapIndex bmap[2];              // backend local map: [0] edge layer, [1] surf layer
+    lili::DevBuf bmap_raw, bmap_ds[2];   // concatenation of the transformed keyframes; the filtered layers (all fields)
+    int bmap_n[2] = {0, 0};
+    bool bmap_built = false;
+    int win_k = 0;                       // window correspondences resident (liliom_backend_window_correspond)
+    liliom_backend_params win_bp{};      // ... and the parameters they were found with (weights, extrinsics, loss of the blocks)
+    std::vector<int> win_ids;
+    std::vector<long long> win_qoff[2];  // per kind: query prefix offsets (k + 1)
+    lili::DevBuf win_valid[2], win_line, win_plane, win_score, win_cnt, win_tab;
 
     // ---- scan-to-map ----
     lili::DevBuf feats;                  // float4 body-frame queries
@@ -267,9 +300,13 @@ int voxelgrid_coop(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, i
 int voxelgrid_dev2(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride, float leaf, void* d_out, int* d_count, float4* d_feats,
                    int key_bits = 32, const int* host_mm = nullptr);
 
-// grid build from float4 points already on the device (map_xyzw[0..m)).  host_box (optional): 6 ordered ints, a box known to
-// contain the points up to rounding of a mean (the union of the frames' boxes): no min/max pass and no host round trip.
-int grid_build(liliom_ctx* c, int m, const int* host_box = nullptr);
+// grid build of index `mi` from float4 points already on the device (mi.xyzw[0..m)), cells of `cell` metres (gate_cell).
+// host_box (optional): 6 ordered ints, a box known to contain the points up to rounding of a mean (the union of the frames'
+// boxes): no min/max pass and no host round trip.
+int grid_build(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_box = nullptr);
+inline int grid_build(liliom_ctx* c, int m, const int* host_box = nullptr) {      // the odometry map
+    return grid_build(c, c->map, gate_cell(c->prm.knn_max_sqdist), m, host_box);
+}
 
 const long long* vg_coop_stamps(liliom_ctx* c);   // voxelgrid.cu
 
@@ -288,5 +325,7 @@ void frames_box(const liliom_ctx* c, int mm[7]);                                
 int block27_stats(liliom_ctx* c, const double pose7[7], unsigned long long out[2]);   // grid_knn.cu
 
 int repack_to_f4(liliom_ctx* c, const void* d_in, int n, int stride, float4* d_out, const int* d_n = nullptr);
+
+void backend_release(liliom_ctx* c);                                                  // keyframes.cu: the backend's device buffers
 
 }  // namespace lili

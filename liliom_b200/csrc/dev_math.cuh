@@ -520,4 +520,23 @@ __device__ inline void pose_plus(const double x[7], const double d[6], double ou
     out[4] = x[4] + d[3]; out[5] = x[5] + d[4]; out[6] = x[6] + d[5];
 }
 
+// transformCloud of one PCL point (L/src/LidarOdometry.cpp:246-278, L/src/BackendFusion.cpp:730-767; R/src/LidarOdometry.cpp:239-264):
+// fp64 rotation of xyz (and, for 48-byte points, of the normal); intensity/curvature copied, padding cleared.
+__device__ __forceinline__ void pcl_transform_point(const unsigned char* in, int stride, Q4 q, D3 t, unsigned char* out) {
+    const float4 a = *reinterpret_cast<const float4*>(in);
+    D3 r = qrot_x(q, D3{(double)a.x, (double)a.y, (double)a.z});
+    float4 o = make_float4((float)addx(r.x, t.x), (float)addx(r.y, t.y), (float)addx(r.z, t.z), 1.0f);
+    *reinterpret_cast<float4*>(out) = o;
+    if (stride == 48) {
+        const float4 b = *reinterpret_cast<const float4*>(in + 16);
+        const float4 cc = *reinterpret_cast<const float4*>(in + 32);
+        D3 nr = qrot_x(q, D3{(double)b.x, (double)b.y, (double)b.z});
+        *reinterpret_cast<float4*>(out + 16) = make_float4((float)nr.x, (float)nr.y, (float)nr.z, 0.f);
+        *reinterpret_cast<float4*>(out + 32) = make_float4(cc.x, cc.y, 0.f, 0.f);
+    } else {
+        const float4 b = *reinterpret_cast<const float4*>(in + 16);
+        *reinterpret_cast<float4*>(out + 16) = make_float4(b.x, 0.f, 0.f, 0.f);
+    }
+}
+
 }  // namespace lili

@@ -109,22 +109,22 @@ __global__ void k_cell_run_ends(const uint32_t* __restrict__ keys, int n, int* _
     if (w == n - 1 || keys[w + 1] != k) cell_start[(size_t)k + 1] = w + 1;
 }
 
-int grid_build(liliom_ctx* c, int m, const int* host_box) {
-    c->map_ready = false;
-    c->map_n = m;
+int grid_build(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_box) {
+    mi.ready = false;
+    mi.n = m;
     if (m <= 0) {   // empty (shard of the) map: a 1-cell grid with no points, so that collective callers still run every launch
         GridDesc g{};
         g.inv_cell = 1.0f; g.dim[0] = g.dim[1] = g.dim[2] = 1; g.ncells = 1;
-        c->grid = g;
-        LILI_CUDA(c, c->cell_start.ensure(4 * sizeof(int)));
-        LILI_CUDA(c, cudaMemsetAsync(c->cell_start.p, 0, 4 * sizeof(int), c->stream));
-        LILI_CUDA(c, c->map_sorted.ensure(sizeof(float4)));
-        LILI_CUDA(c, c->map_xyzw.ensure(sizeof(float4)));
-        c->map_n = 0;
-        c->map_ready = true;
+        mi.grid = g;
+        LILI_CUDA(c, mi.cell_start.ensure(4 * sizeof(int)));
+        LILI_CUDA(c, cudaMemsetAsync(mi.cell_start.p, 0, 4 * sizeof(int), c->stream));
+        LILI_CUDA(c, mi.sorted.ensure(sizeof(float4)));
+        LILI_CUDA(c, mi.xyzw.ensure(sizeof(float4)));
+        mi.n = 0;
+        mi.ready = true;
         return LILIOM_OK;
     }
-    float4* pts = c->map_xyzw.as<float4>();
+    float4* pts = mi.xyzw.as<float4>();
     int h[6];
     // A box handed in by the caller contains the raw points.  A voxel centroid (a sequential fp32 mean of such points) can leave
     // it by rounding, in which case its cell may not exist: k_cell_keys reports that, and the grid is rebuilt from the exact
@@ -148,9 +148,6 @@ int grid_build(liliom_ctx* c, int m, const int* host_box) {
         LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     }
     auto dec = [](int i) { int j = i >= 0 ? i : i ^ 0x7fffffff; float f; memcpy(&f, &j, 4); return f; };
-    // cell size: smallest power of two >= sqrt(knn_max_sqdist) (1.0 for the reference's gate)
-    float cell = 1.0f;
-    while ((double)cell * (double)cell < c->prm.knn_max_sqdist) cell *= 2.0f;
     GridDesc g;
     g.inv_cell = 1.0f / cell;
     long long nc = 1;
@@ -164,31 +161,31 @@ int grid_build(liliom_ctx* c, int m, const int* host_box) {
     }
     if (nc > (1LL << 29)) { c->last_error = "map extent needs more than 2^29 cells"; return LILIOM_E_GRID; }
     g.ncells = (int)nc;
-    c->grid = g;
+    mi.grid = g;
     LILI_CUDA(c, c->grid_keys.ensure((size_t)m * 4));
     LILI_CUDA(c, c->grid_keys2.ensure((size_t)m * 4));
     LILI_CUDA(c, c->grid_vals.ensure((size_t)m * 4));
     LILI_CUDA(c, c->grid_vals2.ensure((size_t)m * 4));
-    LILI_CUDA(c, c->map_sorted.ensure((size_t)m * sizeof(float4)));
-    LILI_CUDA(c, c->cell_start.ensure(((size_t)g.ncells + 2) * 4));
+    LILI_CUDA(c, mi.sorted.ensure((size_t)m * sizeof(float4)));
+    LILI_CUDA(c, mi.cell_start.ensure(((size_t)g.ncells + 2) * 4));
     k_cell_keys<<<cdiv(m, 256), 256, 0, c->stream>>>(pts, m, g, c->grid_keys.as<uint32_t>(), c->grid_vals.as<int>(), escaped);
     LILI_TRY(launch_check(c, "k_cell_keys"));
     int bits = 1;
     while ((1LL << bits) < nc) ++bits;
     LILI_TRY(sort_pairs_u32(c, c->grid_keys.as<uint32_t>(), c->grid_keys2.as<uint32_t>(), c->grid_vals.as<int>(),
                             c->grid_vals2.as<int>(), m, bits));
-    k_gather_sorted<<<cdiv(m, 256), 256, 0, c->stream>>>(pts, c->grid_vals2.as<int>(), m, c->map_sorted.as<float4>());
+    k_gather_sorted<<<cdiv(m, 256), 256, 0, c->stream>>>(pts, c->grid_vals2.as<int>(), m, mi.sorted.as<float4>());
     LILI_TRY(launch_check(c, "k_gather_sorted"));
-    LILI_CUDA(c, cudaMemsetAsync(c->cell_start.p, 0, ((size_t)g.ncells + 2) * 4, c->stream));
-    k_cell_run_ends<<<cdiv(m, 256), 256, 0, c->stream>>>(c->grid_keys2.as<uint32_t>(), m, c->cell_start.as<int>());
+    LILI_CUDA(c, cudaMemsetAsync(mi.cell_start.p, 0, ((size_t)g.ncells + 2) * 4, c->stream));
+    k_cell_run_ends<<<cdiv(m, 256), 256, 0, c->stream>>>(c->grid_keys2.as<uint32_t>(), m, mi.cell_start.as<int>());
     LILI_TRY(launch_check(c, "k_cell_run_ends"));
-    LILI_TRY(inclusive_max_scan_i32(c, c->cell_start.as<int>(), g.ncells + 1));
+    LILI_TRY(inclusive_max_scan_i32(c, mi.cell_start.as<int>(), g.ncells + 1));
     if (escaped) {
         LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->escaped, escaped, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
         LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-        if (c->h_pin->escaped) return grid_build(c, m, nullptr);
+        if (c->h_pin->escaped) return grid_build(c, mi, cell, m, nullptr);
     }
-    c->map_ready = true;
+    mi.ready = true;
     return LILIOM_OK;
 }
 
@@ -1028,7 +1025,7 @@ __global__ void k_block27_count(const float4* __restrict__ feats, int n, Q4 q, D
 
 int block27_stats(liliom_ctx* c, const double pose7[7], unsigned long long out[2]) {
     out[0] = out[1] = 0;
-    if (!c->map_ready) return LILIOM_E_NOMAP;
+    if (!c->map.ready) return LILIOM_E_NOMAP;
     const int n = c->n_feats_actual;
     if (n <= 0) return LILIOM_OK;
     LILI_CUDA(c, c->lm_state.ensure(64 * sizeof(long long)));
@@ -1036,7 +1033,7 @@ int block27_stats(liliom_ctx* c, const double pose7[7], unsigned long long out[2
     LILI_CUDA(c, cudaMemsetAsync(d, 0, 16, c->stream));
     const Q4 q{pose7[0], pose7[1], pose7[2], pose7[3]};
     const D3 t{pose7[4], pose7[5], pose7[6]};
-    k_block27_count<<<min(cdiv(n, 256), c->sm_count * 4), 256, 0, c->stream>>>(c->feats.as<float4>(), n, q, t, c->cell_start.as<int>(), c->grid,
+    k_block27_count<<<min(cdiv(n, 256), c->sm_count * 4), 256, 0, c->stream>>>(c->feats.as<float4>(), n, q, t, c->map.cell_start.as<int>(), c->map.grid,
                                                                               c->nranks, c->rank, c->shard_inv_block, d);
     LILI_TRY(launch_check(c, "k_block27_count"));
     unsigned long long* hp = c->h_pin->block27;
@@ -1105,7 +1102,7 @@ static int s2m_prepare(liliom_ctx* c, const S2mPlan& p, int iters, int mode, boo
     LILI_CUDA(c, c->qstate.ensure((size_t)(n > 0 ? n : 1) * sizeof(float4)));
     a = KnnArgs{};
     a.feats = c->feats.as<float4>(); a.n = n; a.n_dev = c->d_nfeats;
-    a.map = c->map_sorted.as<float4>(); a.map_orig = c->map_xyzw.as<float4>(); a.cell_start = c->cell_start.as<int>(); a.g = c->grid;
+    a.map = c->map.sorted.as<float4>(); a.map_orig = c->map.xyzw.as<float4>(); a.cell_start = c->map.cell_start.as<int>(); a.g = c->map.grid;
     a.pose = c->pose_dev.as<double>(); a.pose_out = c->pose_dev.as<double>();
     a.max_sqd = c->prm.knn_max_sqdist; a.plane_thres = c->prm.plane_thres; a.w_gate = c->prm.weight_gate; a.huber_a = c->prm.huber_a;
     a.valid = need_corr ? c->corr_valid.as<unsigned char>() : nullptr; a.plane = need_corr ? c->corr_plane.as<float4>() : nullptr;
@@ -1166,7 +1163,7 @@ static void print_debug_timing(liliom_ctx* c, const long long* dbg, bool persist
 
 int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int mode, liliom_iter_stats* stats,
             bool want_corr, double out29[29]) {
-    if (!c->map_ready) return LILIOM_E_NOMAP;
+    if (!c->map.ready) return LILIOM_E_NOMAP;
     if (c->map_n_global < 10) return LILIOM_E_FEWMAP;          // L/src/LidarOdometry.cpp:485-488
     const int n = c->n_feats, iters = match_cnt;
     if (iters < 0) return LILIOM_E_ARG;

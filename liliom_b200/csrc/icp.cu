@@ -166,13 +166,13 @@ int icp_align(liliom_ctx* c, const float4* d_src, int n, double max_corr_dist, i
               double T16[16], double* fitness, int* converged, int* iters) {
     for (int k = 0; k < 16; ++k) T16[k] = (k % 5 == 0) ? 1.0 : 0.0;
     *fitness = 0.0; *converged = 0; *iters = 0;
-    if (n <= 0 || c->map_n <= 0) return LILIOM_OK;
+    if (n <= 0 || c->map.n <= 0) return LILIOM_OK;
     const int grid = cdiv(n, 256);
     LILI_CUDA(c, c->partials.ensure((size_t)kIcpSums * grid * sizeof(double)));
     IcpArgs a{};
-    a.src = d_src; a.n = n; a.map = c->map_sorted.as<float4>(); a.map_orig = c->map_xyzw.as<float4>(); a.cell_start = c->cell_start.as<int>(); a.g = c->grid;
+    a.src = d_src; a.n = n; a.map = c->map.sorted.as<float4>(); a.map_orig = c->map.xyzw.as<float4>(); a.cell_start = c->map.cell_start.as<int>(); a.g = c->map.grid;
     a.partials = c->partials.as<double>();
-    const float cell = 1.0f / c->grid.inv_cell;
+    const float cell = 1.0f / c->map.grid.inv_cell;
     a.max_d2 = (float)(max_corr_dist * max_corr_dist);
     a.rmax = (int)std::ceil(max_corr_dist / cell) + 1;
     double F[4][4] = {{1, 0, 0, 0}, {0, 1, 0, 0}, {0, 0, 1, 0}, {0, 0, 0, 1}};
@@ -223,7 +223,7 @@ int icp_align(liliom_ctx* c, const float4* d_src, int n, double max_corr_dist, i
     // getFitnessScore(): mean squared NN distance of the aligned source, no cut-off
     for (int r = 0; r < 3; ++r) for (int k = 0; k < 4; ++k) a.T[4 * r + k] = F[r][k];
     a.max_d2 = -1.0f;
-    a.rmax = std::max(c->grid.dim[0], std::max(c->grid.dim[1], c->grid.dim[2])) + 1;
+    a.rmax = std::max(c->map.grid.dim[0], std::max(c->map.grid.dim[1], c->map.grid.dim[2])) + 1;
     {   // sources far outside the grid would walk many empty shells: bound the walk by the distance to the grid plus its extent
         double s[kIcpSums];
         LILI_TRY(icp_pass(c, a, grid, s));

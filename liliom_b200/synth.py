@@ -235,3 +235,42 @@ def default_true_pose():
     """Sensor 1.8 m above ground inside a block, yawed 8 deg, slightly pitched."""
     q = qmul(q_from_axis_angle([0, 0, 1], np.deg2rad(8.0)), q_from_axis_angle([0, 1, 0], np.deg2rad(-1.5)))
     return np.concatenate([q, [2.0, 3.0, 1.8]])
+
+
+def make_keyframe_sequence(n: int, stride: int = 48, seed: int = 7, step=1.5, yaw_deg=2.0, surf_every: int = 8):
+    """A seeded keyframe stream for the backend (SURVEY.md §8 f5): n Horizon sweeps (no rotation inside a sweep, i.e. the
+    clouds the backend receives after de-skew) taken every `step` metres along a gently turning path through the world.
+    Each keyframe is split the way the extractors split a sweep: edge = returns from poles and wall tops (line-like
+    neighbourhoods), surf = every `surf_every`-th other return.  Reflectivity (the `curvature` field, FormatConvert.cpp:21)
+    is per surface kind plus a little noise, so the reflectivity-weighted plane fit of the Horizon backend sees real planes.
+    Returns a list of (edge, surf, pose7) with clouds in the body frame, PT48 (stride 48) or PT32 (stride 32)."""
+    rng = np.random.default_rng(seed)
+    T0 = default_true_pose()
+    out = []
+    for i in range(n):
+        yaw = np.deg2rad(yaw_deg * i)
+        q = qmul(q_from_axis_angle([0, 0, 1], yaw), T0[:4])
+        t = T0[4:] + np.array([step * i, 0.35 * np.sin(0.4 * i), 0.0])
+        pose = np.concatenate([q, t])
+        pts, _ = make_horizon_sweep(pose, seed=seed * 1000 + i, omega=(0.0, 0.0, 0.0))
+        p = np.stack([pts["x"], pts["y"], pts["z"]], 1).astype(np.float64)
+        w = _rotate_many(np.broadcast_to(q, (len(p), 4)), p) + t
+        px = (w[:, 0] - 10.0) - 20.0 * np.round((w[:, 0] - 10.0) / 20.0)
+        py = (w[:, 1] - 6.0) - 20.0 * np.round((w[:, 1] - 6.0) / 20.0)
+        pole = np.hypot(px, py) < 0.4
+        top = w[:, 2] > WALL_H - 0.6
+        ground = w[:, 2] < 0.2
+        edge_m = pole | top
+        base = np.where(pole, 12.0, np.where(top, 8.0, np.where(ground, 2.0, 6.0)))
+        pts["curvature"] = (base + rng.normal(0.0, 0.05, len(pts))).astype(np.float32)
+        surf_idx = np.flatnonzero(~edge_m)[::surf_every]
+        edge, surf = pts[edge_m], pts[surf_idx]
+        if stride == 32:
+            def to32(a):
+                b = np.zeros(len(a), PT32)
+                for f in ("x", "y", "z", "w", "intensity"):
+                    b[f] = a[f]
+                return b
+            edge, surf = to32(edge), to32(surf)
+        out.append((edge, surf, pose))
+    return out

@@ -1,0 +1,214 @@
+#!/usr/bin/env python
+"""The backend's LiDAR step (SURVEY.md §8 f5) on one GPU: device-resident keyframe store + local map + window calls, against the
+same step through the single-keyframe ABI and the 1-thread oracle composition.  Prints one JSON line.
+usage: backend_bench.py [--steps K] [--warmup W] [--dump-outputs DIR]
+--dump-outputs DIR writes the last timed step's layers and blocks of the device-resident leg as DIR/<name>.npy."""
+from __future__ import annotations
+
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def dump_outputs(d, arrays):
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(d, name + ".npy"), a)
+
+
+BK_MAP_WIDTH = 40      # local_map_width (L/config/config_fr_iosb.yaml)
+BK_WINDOW = 3          # slide_window_width
+BK_EVALS = 16          # max_num_iter (15) LM evaluations + 1 for the marginalisation
+
+
+def bench_backend(args):
+    """One step of BackendFusion's LiDAR side (SURVEY.md §8 f5) per new keyframe, Horizon variant, on the
+    seeded keyframe stream of synth.make_keyframe_sequence.  A step: store the new keyframe's received clouds (VoxelGrid on the
+    device), build the local map over the latest 40 keyframes, download both layers (published every run), search the window's
+    3 keyframes, evaluate the window's blocks 16 times (15 LM iterations + the marginalisation).
+    Legs: (a) this path; (b) the same step through the single-keyframe ABI (host transform + concatenation in NumPy,
+    liliom_voxelgrid x2, liliom_map_set_cloud on an edge and a surf context, then for each of the 16 evaluations and each window
+    keyframe liliom_correspond_edge / _surf_refl + the block: one context holds one keyframe's correspondences at a time);
+    (c) the 1-thread oracle composition of (b), on a bounded sample."""
+    import torch
+    import liliom_b200 as L
+    from liliom_b200 import synth
+    if not torch.cuda.is_available():
+        raise SystemExit("backend_bench.py needs a CUDA device (no CPU fallback)")
+    name = torch.cuda.get_device_name(0)
+    try:
+        plim = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
+                              text=True, timeout=20).stdout.strip()
+    except Exception as e:      # noqa: BLE001
+        plim = "unknown (" + type(e).__name__ + ")"
+    bp = L.backend_default_params(0)
+    pool = synth.make_keyframe_sequence(BK_MAP_WIDTH + 8, stride=48)
+    steps, warmup = args.steps, args.warmup
+    q_lb, t_lb = np.array(bp.q_lb[:]), np.array(bp.t_lb[:])
+
+    def body_of(p):         # inverse of :929-930, quaternion kept unit as Ceres' QuaternionParameterization keeps it
+        q = synth.qmul(p[:4], q_lb)
+        return np.concatenate([q / np.linalg.norm(q), p[4:] + synth.qrot(p[:4], t_lb)])
+
+    def trial(p, it):       # LM trial poses: small deterministic steps
+        dq = synth.q_from_axis_angle([1, -1, 2], np.deg2rad(0.01 * it))
+        return np.concatenate([synth.qmul(p[:4], dq), p[4:] + 1e-3 * it])
+
+    psz = 48
+    # ---- (a) device-resident store and local map
+    c = L.Context(variant=0)
+    kf_pose = []
+    for e, s, p in pool[:BK_MAP_WIDTH]:                        # a stream already BK_MAP_WIDTH keyframes long
+        c.kf_add(bp, e, s, download=False); kf_pose.append(p)
+    kf_sizes = []                                               # stored (edge, surf) points per keyframe, for leg (b)'s byte count
+
+    def step_a(j):
+        e, s, p = pool[j % len(pool)]
+        kid, _, _ = c.kf_add(bp, e, s, download=False); kf_pose.append(p)
+        ids = list(range(kid + 1 - BK_MAP_WIDTH, kid + 1))
+        c.bmap_build(bp, ids, [kf_pose[i] for i in ids])
+        em, sm = c.bmap_download(0), c.bmap_download(1)
+        win = list(range(kid - BK_WINDOW, kid))                 # idx - 1
+        pl = [kf_pose[i] for i in win]
+        ne, ns = c.backend_window_correspond(bp, win, pl)
+        blocks = [c.backend_window_blocks([trial(body_of(p), it) for p in pl]) for it in range(BK_EVALS)]
+        h2d = (len(e) + len(s)) * psz
+        d2h = (len(em) + len(sm)) * psz + BK_EVALS * BK_WINDOW * 2 * 29 * 8
+        return (em, sm, blocks[-1]), h2d, d2h
+
+    def timed(fn, n, w):
+        for j in range(w):
+            fn(j)
+        ms, out = [], None
+        for j in range(w, w + n):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            out = fn(j)
+            ms.append((time.perf_counter() - t0) * 1e3)
+        return ms, out
+
+    def stats(ms, out):
+        return {"median_ms": float(np.median(ms)), "min_ms": float(np.min(ms)), "max_ms": float(np.max(ms)), "steps": len(ms),
+                "h2d_bytes_per_step": int(out[1]), "d2h_bytes_per_step": int(out[2])}
+
+    ms_a, out_a = timed(step_a, steps, warmup)
+    # ---- (b) the single-keyframe ABI: the adapter keeps every keyframe cloud and builds the local map on the host
+    cb, ce, cs = L.Context(variant=0), L.Context(variant=0), L.Context(variant=0)
+    store = []                                                  # host copies of edge_frames / surf_frames (:1688-1695)
+    pose_b = []
+    for e, s, p in pool[:BK_MAP_WIDTH]:
+        store.append((cb.voxelgrid(e, bp.edge_leaf), cb.voxelgrid(s, bp.surf_leaf))); pose_b.append(p)
+
+    def host_transform(cloud, p):
+        out = cloud.copy()
+        xyz = np.stack([cloud["x"], cloud["y"], cloud["z"]], 1).astype(np.float64)
+        w = synth._rotate_many(np.broadcast_to(p[:4], (len(xyz), 4)), xyz) + p[4:]
+        n = synth._rotate_many(np.broadcast_to(p[:4], (len(xyz), 4)), np.stack([cloud["nx"], cloud["ny"], cloud["nz"]], 1).astype(np.float64))
+        out["x"], out["y"], out["z"] = w[:, 0], w[:, 1], w[:, 2]
+        out["nx"], out["ny"], out["nz"] = n[:, 0], n[:, 1], n[:, 2]
+        return out
+
+    def step_b(j):
+        e, s, p = pool[j % len(pool)]
+        eds, sds = cb.voxelgrid(e, bp.edge_leaf), cb.voxelgrid(s, bp.surf_leaf)
+        store.append((eds, sds)); pose_b.append(p)
+        kid = len(store) - 1
+        h2d = (len(e) + len(s)) * psz; d2h = (len(eds) + len(sds)) * psz
+        ids = range(kid + 1 - BK_MAP_WIDTH, kid + 1)
+        E = np.concatenate([host_transform(store[i][0], pose_b[i]) for i in ids])
+        S = np.concatenate([host_transform(store[i][1], pose_b[i]) for i in ids])
+        em, sm = cb.voxelgrid(E, bp.edge_leaf), cb.voxelgrid(S, bp.surf_leaf)
+        h2d += (len(E) + len(S)) * psz; d2h += (len(em) + len(sm)) * psz
+        ce.map_set_cloud(em); cs.map_set_cloud(sm)
+        h2d += (len(em) + len(sm)) * psz
+        win = list(range(kid - BK_WINDOW, kid))
+        pl = [pose_b[i] for i in win]
+        blocks = np.zeros((BK_WINDOW, 2, 29))
+        for it in range(BK_EVALS):
+            for k, i in enumerate(win):
+                fe, fs = store[i]
+                v, _, _ = ce.correspond_edge(fe, pl[k], 0)
+                blocks[k, 0] = ce.backend_edge_block(trial(body_of(pl[k]), it), float(np.float32(bp.lidar_const)), bp.cauchy_b)
+                ve, _, _ = cs.correspond_surf_refl(fs, pl[k], bp.kd_max_radius, bp.surf_dist_thres, bp.w_gate, bp.lidar_const, bp.reflect_thres)
+                blocks[k, 1] = cs.backend_surf_block(trial(body_of(pl[k]), it), q_lb, t_lb, bp.cauchy_b)
+                h2d += (len(fe) + len(fs)) * psz
+                d2h += len(fe) * 25 + len(fs) * 25 + 2 * 29 * 8
+        return (em, sm, blocks), h2d, d2h
+
+    ms_b, out_b = timed(step_b, steps, warmup)
+    # ---- (c) 1-thread oracle composition of (b), bounded sample
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import oracle_lib as O
+    store_o = [(O.voxelgrid(e, bp.edge_leaf), O.voxelgrid(s, bp.surf_leaf)) for e, s, _ in pool[:BK_MAP_WIDTH]]
+    pose_o = [p for _, _, p in pool[:BK_MAP_WIDTH]]
+
+    def f4(a):
+        return np.stack([a["x"], a["y"], a["z"], np.ones(len(a), np.float32)], 1)
+
+    def step_c(j):
+        e, s, p = pool[j % len(pool)]
+        store_o.append((O.voxelgrid(e, bp.edge_leaf), O.voxelgrid(s, bp.surf_leaf))); pose_o.append(p)
+        kid = len(store_o) - 1
+        ids = range(kid + 1 - BK_MAP_WIDTH, kid + 1)
+        em = O.voxelgrid(np.concatenate([O.transform_cloud(store_o[i][0], pose_o[i]) for i in ids]), bp.edge_leaf)
+        sm = O.voxelgrid(np.concatenate([O.transform_cloud(store_o[i][1], pose_o[i]) for i in ids]), bp.surf_leaf)
+        te, ts = O.KdTree(f4(em)), O.KdTree(f4(sm))
+        win = list(range(kid - BK_WINDOW, kid))
+        blocks = np.zeros((BK_WINDOW, 2, 29))
+        corr = []
+        for i in win:
+            fe, fs = store_o[i]
+            corr.append((O.correspond_edge(te, fe, pose_o[i], 0),
+                         O.correspond_surf_backend(ts, fs, pose_o[i], bp.kd_max_radius, bp.surf_dist_thres, bp.w_gate, bp.lidar_const,
+                                                   sm["curvature"], fs["curvature"], bp.reflect_thres)))
+        for it in range(BK_EVALS):
+            for k, i in enumerate(win):
+                (v, pa, pb), (vs, pls, sc) = corr[k]
+                b = trial(body_of(pose_o[i]), it)
+                blocks[k, 0] = O.backend_edge_block(store_o[i][0], v, pa, pb, float(np.float32(bp.lidar_const)), b, bp.cauchy_b)
+                blocks[k, 1] = O.backend_surf_block(store_o[i][1], vs, pls, sc, b, q_lb, t_lb, bp.cauchy_b)
+        return (em, sm, blocks), 0, 0
+
+    n_c = min(steps, 5)
+    ms_c, out_c = timed(step_c, n_c, 0)
+    n_edge, n_surf = len(out_a[0][0]), len(out_a[0][1])
+    line = {
+        "metric": "ms per BackendFusion LiDAR step (keyframe store + 40-keyframe local map + 3-keyframe window, 16 block evaluations)",
+        "workload": "backend", "unit": "ms/step", "higher_is_better": False, "n_gpus": 1, "steps": steps, "warmup": warmup,
+        "value": float(np.median(ms_a)), "gpu": name, "power_limit": plim, "data": "synthetic (synth.make_keyframe_sequence)",
+        "config": {"variant": 0, "local_map_width": BK_MAP_WIDTH, "slide_window_width": BK_WINDOW, "block_evaluations": BK_EVALS,
+                   "edge_layer_points": n_edge, "surf_layer_points": n_surf,
+                   "keyframe_points_received": int(np.mean([len(e) + len(s) for e, s, _ in pool]))},
+        "device_resident": stats(ms_a, out_a),
+        "single_keyframe_abi": stats(ms_b, out_b),
+        "oracle_1_thread": {**stats(ms_c, out_c), "h2d_bytes_per_step": None, "d2h_bytes_per_step": None,
+                            "sample": f"{n_c} steps, 1 thread, correspondences searched once per window keyframe"},
+        "timing": "host wall clock around each step (every library call ends in a stream synchronise)",
+    }
+    if args.dump_outputs:
+        (em, sm, blk) = out_a[0]
+        dump_outputs(args.dump_outputs, {"backend_edge_layer": em.view(np.float32).reshape(-1), "backend_surf_layer": sm.view(np.float32).reshape(-1),
+                                         "backend_blocks": np.asarray(blk, np.float64)})
+    print(json.dumps(line), flush=True)
+    for x in (c, cb, ce, cs):
+        x.close()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=30)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--dump-outputs", default="", metavar="DIR")
+    bench_backend(ap.parse_args())
+
+
+if __name__ == "__main__":
+    main()
