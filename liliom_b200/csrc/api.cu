@@ -115,8 +115,7 @@ static int install_map_from_xyzw(liliom_ctx* c, int m) {
         LILI_CUDA(c, c->flags.ensure(((size_t)m + 2) * 4));
         LILI_CUDA(c, c->idx_a.ensure(((size_t)m + 2) * 4));
         LILI_CUDA(c, c->map_ds.ensure((size_t)m * sizeof(float4)));
-        float cell = 1.0f;
-        while ((double)cell * (double)cell < c->prm.knn_max_sqdist) cell *= 2.0f;
+        const float cell = gate_cell(c->prm.knn_max_sqdist);
         k_shard_flags<<<cdiv(m + 1, 256), 256, 0, c->stream>>>(c->map.xyzw.as<float4>(), m, cell, c->shard_inv_block, c->nranks, c->rank, c->flags.as<int>());
         LILI_TRY(launch_check(c, "k_shard_flags"));
         LILI_TRY(exclusive_scan_i32(c, c->flags.as<int>(), c->idx_a.as<int>(), m));
@@ -246,7 +245,7 @@ extern "C" void liliom_destroy(liliom_ctx* c) {
                       &c->cub_tmp, &c->vg_coop, &c->hz_ctl, &c->map_raw, &c->map_ds, &c->map.xyzw, &c->map.sorted, &c->map.cell_start, &c->grid_keys, &c->grid_keys2,
                       &c->grid_vals, &c->grid_vals2, &c->feats, &c->corr_valid, &c->corr_plane, &c->nn_idx, &c->nn_sqd, &c->pose_dev,
                       &c->partials, &c->neq, &c->stats_dev, &c->counter, &c->lm_state, &c->raw_scan, &c->map.refl, &c->livox_in, &c->qstate, &c->inc_key[0], &c->inc_key[1], &c->inc_ref[0], &c->inc_ref[1], &c->inc_newkey[0], &c->inc_newkey[1],
-                      &c->inc_newref[0], &c->inc_newref[1], &c->inc_removed, &c->inc_rpos, &c->inc_flags, &c->inc_rank, &c->inc_mm};
+                      &c->inc_newref[0], &c->inc_newref[1], &c->inc_removed, &c->inc_rpos, &c->inc_flags, &c->inc_rank, &c->inc_bad};
     for (DevBuf* b : bufs) b->release();
     backend_release(c);
     for (auto& f : c->frames) f.buf.release();
@@ -472,9 +471,7 @@ static int push_frame_from_device(liliom_ctx* c, const void* d_src, int n, const
             LILI_CUDA(c, c->idx_a.ensure(((size_t)n + 2) * 4));
             k_transform_cloud<<<cdiv(n, 256), 256, 0, c->stream>>>((const unsigned char*)d_src, n, stride, q, t, (unsigned char*)c->map_ds.p);
             LILI_TRY(launch_check(c, "k_transform_cloud"));
-            float cell = 1.0f;
-            while ((double)cell * (double)cell < c->prm.knn_max_sqdist) cell *= 2.0f;
-            const float halo = cell + 1.7320508f * c->prm.leaf_map + 0.05f;
+            const float halo = gate_cell(c->prm.knn_max_sqdist) + 1.7320508f * c->prm.leaf_map + 0.05f;
             k_shard_flags_strided<<<cdiv(n + 1, 256), 256, 0, c->stream>>>((const unsigned char*)c->map_ds.p, n, stride, halo, c->shard_inv_block, c->nranks, c->rank, c->flags.as<int>());
             LILI_TRY(launch_check(c, "k_shard_flags_strided"));
             LILI_TRY(exclusive_scan_i32(c, c->flags.as<int>(), c->idx_a.as<int>(), n));
@@ -515,15 +512,9 @@ extern "C" int liliom_map_push_frame_device(liliom_ctx* c, const void* d_surf_ds
 
 namespace lili {
 // tail shared by the rebuild and the incremental update (single GPU): c->map_ds holds m filtered points
-void frames_box(const liliom_ctx* c, int mm[7]) {
-    for (int k = 0; k < 3; ++k) { mm[k] = INT_MAX; mm[3 + k] = INT_MIN; }
-    long long nfin = 0;
-    for (const auto& f : c->frames) {
-        if (f.mm[6] <= 0) continue;
-        for (int k = 0; k < 3; ++k) { mm[k] = std::min(mm[k], f.mm[k]); mm[3 + k] = std::max(mm[3 + k], f.mm[3 + k]); }
-        nfin += f.mm[6];
-    }
-    mm[6] = (int)nfin;
+void frames_box(const liliom_ctx* c, int mm[kBoxInts]) {
+    for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_empty(k);
+    for (const auto& f : c->frames) vg_box_merge(mm, f.mm);
 }
 
 int map_finish_from_ds(liliom_ctx* c, int m) {
@@ -546,7 +537,7 @@ static int map_update_from_device(liliom_ctx* c, const void* d_src, int n, const
     if (n_map_out) *n_map_out = 0;
     const bool incremental = c->nranks == 1 && c->prm.max_map_frames <= 64 && n < (1 << 24);
     int popped_slot = -1, popped_nfin = 0;
-    if ((int)c->frames.size() >= c->prm.max_map_frames && !c->frames.empty()) { popped_slot = c->frames.front().slot; popped_nfin = c->frames.front().nfin; }
+    if ((int)c->frames.size() >= c->prm.max_map_frames && !c->frames.empty()) { popped_slot = c->frames.front().slot; popped_nfin = c->frames.front().mm[6]; }
     LILI_TRY(push_frame_from_device(c, d_src, n, pose7, incremental));
     if (incremental) {
         c->map.ready = false; c->map.n = 0; c->map_n_global = 0;
@@ -659,10 +650,8 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
             if (m > 0) {
                 LILI_CUDA(c, c->flags.ensure(((size_t)m + 2) * 4));
                 LILI_CUDA(c, c->idx_a.ensure(((size_t)m + 2) * 4));
-                float cell = 1.0f;
-                while ((double)cell * (double)cell < c->prm.knn_max_sqdist) cell *= 2.0f;
-                k_shard_flags_strided<<<cdiv(m + 1, 256), 256, 0, c->stream>>>((const unsigned char*)c->map_ds.p, m, stride, cell, c->shard_inv_block, c->nranks,
-                                                                             c->rank, c->flags.as<int>());
+                k_shard_flags_strided<<<cdiv(m + 1, 256), 256, 0, c->stream>>>((const unsigned char*)c->map_ds.p, m, stride, gate_cell(c->prm.knn_max_sqdist),
+                                                                             c->shard_inv_block, c->nranks, c->rank, c->flags.as<int>());
                 LILI_TRY(launch_check(c, "k_shard_flags_strided"));
                 LILI_TRY(exclusive_scan_i32(c, c->flags.as<int>(), c->idx_a.as<int>(), m));
                 k_compact_repack<<<cdiv(m, 256), 256, 0, c->stream>>>((const unsigned char*)c->map_ds.p, c->flags.as<int>(), c->idx_a.as<int>(), m, stride,

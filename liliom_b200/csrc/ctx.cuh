@@ -8,6 +8,7 @@
 #include <string>
 #include <vector>
 #include "../../include/liliom.h"
+#include "vg_box.h"
 
 namespace lili {
 
@@ -27,17 +28,6 @@ struct DevBuf {
     }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
     template <class T> T* as() const { return reinterpret_cast<T*>(p); }
-};
-
-// Parameters of one VoxelGrid pass, produced on the device (no host round trip).
-struct VgParams {
-    float inv_leaf;
-    int   min_b[3];
-    int   div_b[3];
-    int   mul[3];
-    int   overflow;    // PCL: "Leaf size is too small" -> output = input
-    int   n_finite;
-    int   bail;        // cooperative single-launch filter declined this input (see k_vg_coop): redo with the sort chain
 };
 
 // Dense cell grid over the down-sampled map (the kd-tree's stand-in).
@@ -100,7 +90,7 @@ struct PinBlock {
     int    vg_count;           // output count of a VoxelGrid or of the map's incremental filter
     VgParams vgp;              // liliom_voxelgrid: the cooperative filter's verdict
     int    kept;               // points a shard filter kept (pushed frame, map rebuild)
-    int    box[8];             // a pushed frame's box + finite count (k_vg_minmax), or box, count, key flag (k_inc_keys)
+    int    box[8];             // a pushed frame's box (k_vg_minmax), a map's box (grid_build), or the incremental map's key flag (k_inc_keys)
     int    escaped;            // grid_build: a point lies outside the handed-in box
     double map_status[4];      // multi-rank map rebuild: {owned voxels, failed} out, their sums over the ranks back
     unsigned long long block27[2];   // block27_stats: queries, points in their cell blocks
@@ -129,12 +119,12 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 struct Frame {        // one entry of recent_surf_frames (world frame, point_stride bytes per point)
     DevBuf buf;
     int n = 0;
-    // incremental map (map_inc.cu): slot id carried by the frame's entries, finite points, box (ordered ints), unrepresentable key seen
-    int slot = 0, nfin = 0, box[6] = {0, 0, 0, 0, 0, 0};
+    // incremental map (map_inc.cu): slot id carried by the frame's entries, unrepresentable key seen
+    int slot = 0;
     bool bad = false;
-    // box and finite count of the stored points (k_vg_minmax's encoding), taken when the frame was pushed: the rebuild's
-    // VoxelGrid and cell grid get their bounding boxes from the union over the frames instead of two passes over the map
-    int mm[7] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
+    // box of the stored points (vg_box.h; mm[6] = finite points), taken when the frame was pushed: the rebuild's VoxelGrid, the
+    // cell grid and the incremental map get their bounding boxes from the union over the frames instead of passes over the map
+    int mm[kBoxInts] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
 };
 
 }  // namespace lili
@@ -188,7 +178,7 @@ struct liliom_ctx {
     // ---- map ----
     std::vector<lili::Frame> frames;     // FIFO, oldest first
     // incremental map (liliom_map_update, map_inc.cu): entries {voxel key, slot<<24|index} sorted by (key, frame age, index), double-buffered
-    lili::DevBuf inc_key[2], inc_ref[2], inc_newkey[2], inc_newref[2], inc_removed, inc_rpos, inc_flags, inc_rank, inc_mm;
+    lili::DevBuf inc_key[2], inc_ref[2], inc_newkey[2], inc_newref[2], inc_removed, inc_rpos, inc_flags, inc_rank, inc_bad;
     int inc_cur = 0, inc_E = 0;
     bool inc_valid = false;
     lili::DevBuf map_raw;                // concatenated frames (stride bytes)

@@ -442,23 +442,19 @@ __global__ void __launch_bounds__(512) k_rot_ring(const Pt32* __restrict__ cloud
 }
 
 // ---- per-ring VoxelGrid(0.6) of the less-flat points, batched over rings
-// ringmm: [ring][8] ordered-int min xyz, max xyz, count
+// ringmm: [ring][8] a box (vg_box.h) per ring, word 7 unused
 __global__ void k_rot_lf_init(int* ringmm) {
     int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= ROT_MAX_RINGS * 8) return;
-    int f = t & 7;
-    ringmm[t] = f < 3 ? INT_MAX : (f < 6 ? INT_MIN : 0);
+    ringmm[t] = vg_box_empty(t & 7);
 }
-
-__device__ __forceinline__ int rf2ord(float f) { int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }
-__device__ __forceinline__ float rord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
 
 __global__ void k_rot_lf_gather(const Pt32* __restrict__ cloud, const uint32_t* __restrict__ skeys, const int* __restrict__ lessflat,
                                 const int* __restrict__ lfpos, int n, int* __restrict__ lf_src, int* __restrict__ ringmm, int* __restrict__ meta) {
     // per-ring boxes: block-local in shared memory first (the cloud is ring-major, so a block meets one to three rings), then one
     // set of global atomics per ring the block saw — per-point global atomics on 64 x 7 words cost this kernel 38 us
     __shared__ int s_mm[ROT_MAX_RINGS * 8];
-    for (int t = threadIdx.x; t < ROT_MAX_RINGS * 8; t += blockDim.x) { const int f = t & 7; s_mm[t] = f < 3 ? INT_MAX : (f < 6 ? INT_MIN : 0); }
+    for (int t = threadIdx.x; t < ROT_MAX_RINGS * 8; t += blockDim.x) s_mm[t] = vg_box_empty(t & 7);
     __syncthreads();
     int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k == 0) meta[M_NLF] = lfpos[n];
@@ -467,42 +463,22 @@ __global__ void k_rot_lf_gather(const Pt32* __restrict__ cloud, const uint32_t* 
         const int ring = (int)skeys[k];
         float4 a = cloud[k].a;
         int* mm = s_mm + ring * 8;
-        atomicMin(&mm[0], rf2ord(a.x)); atomicMin(&mm[1], rf2ord(a.y)); atomicMin(&mm[2], rf2ord(a.z));
-        atomicMax(&mm[3], rf2ord(a.x)); atomicMax(&mm[4], rf2ord(a.y)); atomicMax(&mm[5], rf2ord(a.z));
+        atomicMin(&mm[0], vg_f2ord(a.x)); atomicMin(&mm[1], vg_f2ord(a.y)); atomicMin(&mm[2], vg_f2ord(a.z));
+        atomicMax(&mm[3], vg_f2ord(a.x)); atomicMax(&mm[4], vg_f2ord(a.y)); atomicMax(&mm[5], vg_f2ord(a.z));
         atomicAdd(&mm[6], 1);
     }
     __syncthreads();
     for (int t = threadIdx.x; t < ROT_MAX_RINGS * 8; t += blockDim.x) {
         const int f = t & 7;
         if (f == 7 || s_mm[(t & ~7) + 6] == 0) continue;          // ring not seen by this block
-        if (f < 3) atomicMin(&ringmm[t], s_mm[t]);
-        else if (f < 6) atomicMax(&ringmm[t], s_mm[t]);
-        else atomicAdd(&ringmm[t], s_mm[t]);
+        vg_box_atomic(&ringmm[t], f, s_mm[t]);
     }
 }
 
 __global__ void k_rot_lf_params(const int* __restrict__ ringmm, float leaf, VgParams* __restrict__ prm) {
     int ring = threadIdx.x;
     if (ring >= ROT_MAX_RINGS) return;
-    const int* mm = ringmm + ring * 8;
-    VgParams p;
-    p.inv_leaf = 1.0f / leaf;
-    p.n_finite = mm[6];
-    p.overflow = 0;
-    if (p.n_finite == 0) {
-        for (int k = 0; k < 3; ++k) { p.min_b[k] = 0; p.div_b[k] = 1; }
-    } else {
-        long long d[3];
-        for (int k = 0; k < 3; ++k) {
-            float lo = rord2f(mm[k]), hi = rord2f(mm[3 + k]);
-            d[k] = (long long)((hi - lo) * p.inv_leaf) + 1;
-            p.min_b[k] = (int)floorf(lo * p.inv_leaf);
-            p.div_b[k] = (int)floorf(hi * p.inv_leaf) - p.min_b[k] + 1;
-        }
-        if (d[0] * d[1] * d[2] > (long long)INT_MAX) p.overflow = 1;
-    }
-    p.mul[0] = 1; p.mul[1] = p.div_b[0]; p.mul[2] = p.div_b[0] * p.div_b[1];
-    prm[ring] = p;
+    prm[ring] = vg_params(ringmm + ring * 8, leaf);
 }
 
 __global__ void k_rot_lf_keys(const Pt32* __restrict__ cloud, const uint32_t* __restrict__ skeys, const int* __restrict__ lf_src,

@@ -40,38 +40,6 @@ int repack_to_f4(liliom_ctx* c, const void* d_in, int n, int stride, float4* d_o
     return launch_check(c, "k_repack_f4");
 }
 
-__device__ __forceinline__ int f2ord(float f) { int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }
-__device__ __forceinline__ float ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
-
-// mm[0..2] = min xyz (ordered-int encoding), mm[3..5] = max
-__global__ void k_minmax_f4(const float4* __restrict__ p, int n, int* __restrict__ mm) {
-    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        float4 v = p[i];
-        int a = f2ord(v.x), b = f2ord(v.y), cz = f2ord(v.z);
-        lo[0] = min(lo[0], a); hi[0] = max(hi[0], a);
-        lo[1] = min(lo[1], b); hi[1] = max(hi[1], b);
-        lo[2] = min(lo[2], cz); hi[2] = max(hi[2], cz);
-    }
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o));
-            hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o));
-        }
-    }
-    if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-        for (int k = 0; k < 3; ++k) { atomicMin(&mm[k], lo[k]); atomicMax(&mm[3 + k], hi[k]); }
-    }
-}
-
-__global__ void k_init_minmax(int* mm) {
-    if (threadIdx.x < 3) mm[threadIdx.x] = INT_MAX;
-    else if (threadIdx.x < 6) mm[threadIdx.x] = INT_MIN;
-}
-
 // `escaped` (optional): set when a point lies outside the grid's box — only possible when the box was handed in by the caller
 // (grid_build's host_box); the key is then clamped into range for memory safety and the caller rebuilds with the exact box.
 __global__ void k_cell_keys(const float4* __restrict__ p, int n, GridDesc g, uint32_t* __restrict__ keys, int* __restrict__ vals,
@@ -138,22 +106,18 @@ int grid_build(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_b
         escaped = c->vg_minmax.as<int>() + 7;
         LILI_CUDA(c, cudaMemsetAsync(escaped, 0, sizeof(int), c->stream));
     } else {
-        LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
-        int* mm = c->vg_minmax.as<int>();
-        k_init_minmax<<<1, 32, 0, c->stream>>>(mm);
-        LILI_TRY(launch_check(c, "k_init_minmax"));
-        k_minmax_f4<<<min(cdiv(m, 256), c->sm_count * 8), 256, 0, c->stream>>>(pts, m, mm);
-        LILI_TRY(launch_check(c, "k_minmax_f4"));
-        LILI_CUDA(c, cudaMemcpyAsync(h, mm, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
+        LILI_TRY(vg_minmax_dev(c, pts, m, nullptr, sizeof(float4)));
+        int* hb = c->h_pin->box;
+        LILI_CUDA(c, cudaMemcpyAsync(hb, c->vg_minmax.p, kBoxInts * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
         LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+        if (hb[6] < m) { c->last_error = "non-finite map point"; return LILIOM_E_ARG; }      // the box counts finite points only
+        for (int k = 0; k < 6; ++k) h[k] = hb[k];
     }
-    auto dec = [](int i) { int j = i >= 0 ? i : i ^ 0x7fffffff; float f; memcpy(&f, &j, 4); return f; };
     GridDesc g;
     g.inv_cell = 1.0f / cell;
     long long nc = 1;
     for (int k = 0; k < 3; ++k) {
-        float lo = dec(h[k]), hi = dec(h[3 + k]);
-        if (!(std::isfinite(lo) && std::isfinite(hi))) { c->last_error = "non-finite map point"; return LILIOM_E_ARG; }
+        float lo = vg_ord2f(h[k]), hi = vg_ord2f(h[3 + k]);
         int clo = (int)floorf(lo * g.inv_cell), chi = (int)floorf(hi * g.inv_cell);
         g.org[k] = clo;
         g.dim[k] = chi - clo + 1;

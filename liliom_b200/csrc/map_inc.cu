@@ -27,50 +27,20 @@ constexpr int kIncSlots = 64;                 // frame slots (refs carry the slo
 constexpr unsigned kIncIdxMask = (1u << 24) - 1u;
 struct FrameTab { const unsigned char* base[kIncSlots]; };
 
-__device__ __forceinline__ int inc_f2ord(float f) { int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }
-
-// keys of one frame's points (world frame, already transformed), refs = slot << 24 | index; per-frame box + finite count
-// mm[0..2] min, mm[3..5] max (ordered ints), mm[6] finite count, mm[7] |= 1 when a voxel coordinate does not fit 21 bits
+// keys of one frame's points (world frame, already transformed), refs = slot << 24 | index; *bad |= 1 when a voxel coordinate
+// does not fit 21 bits (the frame's box and finite count were measured at its push: Frame::mm)
 __global__ void k_inc_keys(const unsigned char* __restrict__ pts, int n, int stride, float inv_leaf, unsigned slot, u64* __restrict__ keys,
-                           unsigned* __restrict__ refs, int* __restrict__ mm) {
+                           unsigned* __restrict__ refs, int* __restrict__ bad) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN}, cnt = 0, bad = 0;
+    bool miss = false;
     if (i < n) {
         const float4 v = *reinterpret_cast<const float4*>(pts + (size_t)i * stride);
         u64 key = ~0ull;
-        if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) {
-            cnt = 1;
-            lo[0] = hi[0] = inc_f2ord(v.x); lo[1] = hi[1] = inc_f2ord(v.y); lo[2] = hi[2] = inc_f2ord(v.z);
-            const float fx = floorf(v.x * inv_leaf), fy = floorf(v.y * inv_leaf), fz = floorf(v.z * inv_leaf);
-            const float lim = 1048576.0f;
-            if (fabsf(fx) < lim && fabsf(fy) < lim && fabsf(fz) < lim)
-                key = ((u64)((int)fz + (1 << 20)) << 42) | ((u64)((int)fy + (1 << 20)) << 21) | (u64)((int)fx + (1 << 20));
-            else bad = 1;
-        }
+        if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) miss = !vg_abs_key(v.x, v.y, v.z, inv_leaf, &key);
         keys[i] = key;
         refs[i] = (slot << 24) | (unsigned)i;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o));
-            hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o));
-        }
-        cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-        bad |= __shfl_xor_sync(0xffffffffu, bad, o);
-    }
-    if ((threadIdx.x & 31) == 0 && cnt > 0) {
-#pragma unroll
-        for (int k = 0; k < 3; ++k) { atomicMin(&mm[k], lo[k]); atomicMax(&mm[3 + k], hi[k]); }
-        atomicAdd(&mm[6], cnt);
-        if (bad) atomicOr(&mm[7], 1);
-    }
-}
-__global__ void k_inc_mm_init(int* mm) {
-    if (threadIdx.x < 3) mm[threadIdx.x] = INT_MAX;
-    else if (threadIdx.x < 6) mm[threadIdx.x] = INT_MIN;
-    else if (threadIdx.x < 8) mm[threadIdx.x] = 0;
+    if (__any_sync(0xffffffffu, miss) && (threadIdx.x & 31) == 0) atomicOr(bad, 1);
 }
 
 __device__ __forceinline__ int lower_bound_u64(const u64* __restrict__ a, int n, u64 k) {      // first i with a[i] >= k
@@ -183,43 +153,30 @@ __global__ void k_inc_centroid(const __grid_constant__ FrameTab tab, const u64* 
     }
 }
 
-static float ord2f_host(int i) { int j = i >= 0 ? i : i ^ 0x7fffffff; float f; memcpy(&f, &j, 4); return f; }
-
-// keys + refs + per-frame statistics of frame `f` (points already in f.buf), written at keys/refs; one sync
+// keys + refs of frame `f` (points already in f.buf), written at keys/refs, and its key flag; one sync
 static int inc_frame_keys(liliom_ctx* c, Frame& f, u64* keys, unsigned* refs) {
     const int stride = c->prm.point_stride;
-    LILI_CUDA(c, c->inc_mm.ensure(8 * sizeof(int)));
-    int* mm = c->inc_mm.as<int>();
-    k_inc_mm_init<<<1, 32, 0, c->stream>>>(mm);
-    LILI_TRY(launch_check(c, "k_inc_mm_init"));
+    LILI_CUDA(c, c->inc_bad.ensure(sizeof(int)));
+    int* bad = c->inc_bad.as<int>();
+    LILI_CUDA(c, cudaMemsetAsync(bad, 0, sizeof(int), c->stream));
     if (f.n > 0) {
-        k_inc_keys<<<cdiv(f.n, 256), 256, 0, c->stream>>>((const unsigned char*)f.buf.p, f.n, stride, 1.0f / c->prm.leaf_map, (unsigned)f.slot, keys, refs, mm);
+        k_inc_keys<<<cdiv(f.n, 256), 256, 0, c->stream>>>((const unsigned char*)f.buf.p, f.n, stride, 1.0f / c->prm.leaf_map, (unsigned)f.slot, keys, refs, bad);
         LILI_TRY(launch_check(c, "k_inc_keys"));
     }
     int* hp = c->h_pin->box;
-    LILI_CUDA(c, cudaMemcpyAsync(hp, mm, 8 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaMemcpyAsync(hp, bad, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    for (int k = 0; k < 6; ++k) f.box[k] = hp[k];
-    f.nfin = hp[6];
-    f.bad = hp[7] != 0;
+    f.bad = hp[0] != 0;
     return LILIOM_OK;
 }
 
-// PCL's "leaf size too small" test on the union box of the live frames, and the representability of the absolute keys
+// the representability of the absolute keys, and PCL's "leaf size too small" test on the union box of the live frames
 static bool inc_representable(liliom_ctx* c) {
-    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
-    bool any = false;
-    for (auto& f : c->frames) {
+    for (auto& f : c->frames)
         if (f.bad) return false;
-        if (f.nfin <= 0) continue;
-        any = true;
-        for (int k = 0; k < 3; ++k) { lo[k] = std::min(lo[k], f.box[k]); hi[k] = std::max(hi[k], f.box[3 + k]); }
-    }
-    if (!any) return true;
-    const float inv_leaf = 1.0f / c->prm.leaf_map;
-    long long d[3];
-    for (int k = 0; k < 3; ++k) d[k] = (long long)((ord2f_host(hi[k]) - ord2f_host(lo[k])) * inv_leaf) + 1;      // voxel_grid.hpp: dx*dy*dz > INT_MAX -> input copied
-    return d[0] * d[1] * d[2] <= (long long)INT_MAX;
+    int box[kBoxInts];
+    frames_box(c, box);
+    return !vg_params(box, c->prm.leaf_map).overflow;
 }
 
 int map_finish_from_ds(liliom_ctx* c, int m);      // api.cu: repack + cell grid of the filtered cloud in c->map_ds
@@ -237,7 +194,7 @@ static int inc_build_all(liliom_ctx* c) {
     long long nfin = 0;
     for (auto& f : c->frames) {
         LILI_TRY(inc_frame_keys(c, f, c->inc_key[1].as<u64>() + off, c->inc_ref[1].as<unsigned>() + off));
-        off += (size_t)f.n; nfin += f.nfin;
+        off += (size_t)f.n; nfin += f.mm[6];
     }
     if (total > 0)      // stable: equal keys stay in concatenation order (frames oldest first, points in frame order); ~0 keys last
         LILI_TRY(sort_pairs_u64(c, c->inc_key[1].as<u64>(), c->inc_key[0].as<u64>(), c->inc_ref[1].as<int>(), c->inc_ref[0].as<int>(), (int)total, 64));
@@ -284,7 +241,7 @@ int map_inc_update(liliom_ctx* c, int popped_slot, int popped_nfin, int* m_out) 
         c->inc_valid = true;
         return inc_emit(c, m_out);
     }
-    {   // new frame: keys, refs, statistics; sorted on its own below
+    {   // new frame: keys, refs, key flag; sorted on its own below
         const size_t ncap = (size_t)(fn.n > 0 ? fn.n : 1);
         for (int b = 0; b < 2; ++b) {
             LILI_CUDA(c, c->inc_newkey[b].ensure(ncap * sizeof(u64) + 64));
@@ -293,7 +250,7 @@ int map_inc_update(liliom_ctx* c, int popped_slot, int popped_nfin, int* m_out) 
         LILI_TRY(inc_frame_keys(c, fn, c->inc_newkey[0].as<u64>(), c->inc_newref[0].as<unsigned>()));
     }
     if (!inc_representable(c)) { c->inc_valid = false; return LILIOM_E_GRID; }
-    const int E = c->inc_E, nnew = fn.nfin;
+    const int E = c->inc_E, nnew = fn.mm[6];
     if (fn.n > 0)
         LILI_TRY(sort_pairs_u64(c, c->inc_newkey[0].as<u64>(), c->inc_newkey[1].as<u64>(), c->inc_newref[0].as<int>(), c->inc_newref[1].as<int>(), fn.n, 64));
     const int E2 = E - (popped_slot >= 0 ? popped_nfin : 0) + nnew;

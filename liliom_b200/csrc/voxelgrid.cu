@@ -13,87 +13,51 @@
 
 namespace lili {
 
-__device__ __forceinline__ int vg_f2ord(float f) { int i = __float_as_int(f); return i >= 0 ? i : i ^ 0x7fffffff; }
-__device__ __forceinline__ float vg_ord2f(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
-
 __global__ void k_vg_init(int* mm) {
-    if (threadIdx.x < 3) mm[threadIdx.x] = INT_MAX;
-    else if (threadIdx.x < 6) mm[threadIdx.x] = INT_MIN;
-    else if (threadIdx.x == 6) mm[6] = 0;
+    if (threadIdx.x < kBoxInts) mm[threadIdx.x] = vg_box_empty(threadIdx.x);
 }
 
-// mm[0..2] min, mm[3..5] max (ordered ints), mm[6] = finite count
+// box of the finite points (vg_box.h)
 __global__ void k_vg_minmax(const unsigned char* __restrict__ pts, int n_max, const int* __restrict__ d_n, int stride, int* __restrict__ mm) {
     const int n = d_n ? min(*d_n, n_max) : n_max;
-    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
-    int cnt = 0;
+    int box[kBoxInts];
+#pragma unroll
+    for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_empty(k);
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         float4 v = *reinterpret_cast<const float4*>(pts + (size_t)i * stride);
         if (!(isfinite(v.x) && isfinite(v.y) && isfinite(v.z))) continue;
-        ++cnt;
-        int a = vg_f2ord(v.x), b = vg_f2ord(v.y), c = vg_f2ord(v.z);
-        lo[0] = min(lo[0], a); hi[0] = max(hi[0], a);
-        lo[1] = min(lo[1], b); hi[1] = max(hi[1], b);
-        lo[2] = min(lo[2], c); hi[2] = max(hi[2], c);
+        vg_box_add(box, v.x, v.y, v.z);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
 #pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o));
-            hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o));
-        }
-        cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+        for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_join(k, box[k], __shfl_xor_sync(0xffffffffu, box[k], o));
     }
     // one set of atomics per BLOCK: the seven words are single addresses, and one set per warp (9.5k warps) serialised into
     // ~55 us at the L2 whatever the input size (measured on a 500k-point frame: push 25 -> 83 us)
-    __shared__ int s_lo[3][8], s_hi[3][8], s_cnt[8];
+    __shared__ int s_box[kBoxInts][8];
     const int w = threadIdx.x >> 5;
     if ((threadIdx.x & 31) == 0) {
 #pragma unroll
-        for (int k = 0; k < 3; ++k) { s_lo[k][w] = lo[k]; s_hi[k][w] = hi[k]; }
-        s_cnt[w] = cnt;
+        for (int k = 0; k < kBoxInts; ++k) s_box[k][w] = box[k];
     }
     __syncthreads();
-    if (threadIdx.x < 7) {
+    if (threadIdx.x < kBoxInts) {
         const int k = threadIdx.x, nw = (blockDim.x + 31) >> 5;
-        if (k < 3) { int v = INT_MAX; for (int j = 0; j < nw; ++j) v = min(v, s_lo[k][j]); if (v != INT_MAX) atomicMin(&mm[k], v); }
-        else if (k < 6) { int v = INT_MIN; for (int j = 0; j < nw; ++j) v = max(v, s_hi[k - 3][j]); if (v != INT_MIN) atomicMax(&mm[k], v); }
-        else { int v = 0; for (int j = 0; j < nw; ++j) v += s_cnt[j]; if (v) atomicAdd(&mm[6], v); }
+        int v = vg_box_empty(k);
+        for (int j = 0; j < nw; ++j) v = vg_box_join(k, v, s_box[k][j]);
+        if (v != vg_box_empty(k)) vg_box_atomic(&mm[k], k, v);
     }
 }
 
-struct VgBox { int mm[7]; };      // min xyz, max xyz (ordered ints), finite count — k_vg_minmax's output, by value
-
-__device__ __forceinline__ void vg_params_from(const int* mm, float leaf, VgParams* __restrict__ out) {
-    VgParams p;
-    p.inv_leaf = 1.0f / leaf;                       // Eigen::Array4f::Ones() / leaf_size_
-    p.n_finite = mm[6];
-    p.overflow = 0;
-    p.bail = 0;
-    if (p.n_finite == 0) {
-        for (int k = 0; k < 3; ++k) { p.min_b[k] = 0; p.div_b[k] = 1; }
-    } else {
-        long long d[3];
-        for (int k = 0; k < 3; ++k) {
-            float lo = vg_ord2f(mm[k]), hi = vg_ord2f(mm[3 + k]);
-            d[k] = (long long)((hi - lo) * p.inv_leaf) + 1;
-            p.min_b[k] = (int)floorf(lo * p.inv_leaf);
-            int max_b = (int)floorf(hi * p.inv_leaf);
-            p.div_b[k] = max_b - p.min_b[k] + 1;
-        }
-        if (d[0] * d[1] * d[2] > (long long)INT_MAX) p.overflow = 1;
-    }
-    p.mul[0] = 1; p.mul[1] = p.div_b[0]; p.mul[2] = p.div_b[0] * p.div_b[1];
-    *out = p;
-}
+struct VgBox { int mm[kBoxInts]; };      // a box (vg_box.h) by value
 
 __global__ void k_vg_params(const int* __restrict__ mm, float leaf, VgParams* __restrict__ out) {
-    if (threadIdx.x == 0) vg_params_from(mm, leaf, out);
+    if (threadIdx.x == 0) *out = vg_params(mm, leaf);
 }
 // the bounding box is already known on the host (map rebuild: the union of the frames' boxes, kept since their push)
 __global__ void k_vg_params_box(const VgBox b, float leaf, VgParams* __restrict__ out) {
-    if (threadIdx.x == 0) vg_params_from(b.mm, leaf, out);
+    if (threadIdx.x == 0) *out = vg_params(b.mm, leaf);
 }
 
 __global__ void k_vg_keys(const unsigned char* __restrict__ pts, int n_max, const int* __restrict__ d_n, int stride, const VgParams* __restrict__ pp,
@@ -290,7 +254,9 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
     const float inv_leaf = 1.0f / leaf;
 
     // ---- phase 1: hash insert + bounding box partials
-    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN}, cnt = 0;
+    int box[kBoxInts];
+#pragma unroll
+    for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_empty(k);
     // (warp-uniform trip count: the first writers of a warp append to the voxel list with ONE atomic per warp — 1-2k atomics on a
     // single counter were a serial chain of their own)
     for (int i0 = gtid - lane; i0 < n; i0 += gthreads) {
@@ -302,18 +268,11 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
         bool won = false;
         unsigned long long wkey = 0;
         if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) {
-            ++cnt;
-            const int a = vg_f2ord(v.x), b = vg_f2ord(v.y), c = vg_f2ord(v.z);
-            lo[0] = min(lo[0], a); hi[0] = max(hi[0], a);
-            lo[1] = min(lo[1], b); hi[1] = max(hi[1], b);
-            lo[2] = min(lo[2], c); hi[2] = max(hi[2], c);
-            const float fx = floorf(v.x * inv_leaf), fy = floorf(v.y * inv_leaf), fz = floorf(v.z * inv_leaf);
-            const float lim = 1048576.0f;
-            if (!(fabsf(fx) < lim && fabsf(fy) < lim && fabsf(fz) < lim)) {
+            vg_box_add(box, v.x, v.y, v.z);
+            unsigned long long key;
+            if (!vg_abs_key(v.x, v.y, v.z, inv_leaf, &key)) {
                 atomicOr(&ctl[1], 1u);
             } else {
-                const unsigned long long key = ((unsigned long long)((int)fz + (1 << 20)) << 42) | ((unsigned long long)((int)fy + (1 << 20)) << 21) |
-                                               (unsigned long long)((int)fx + (1 << 20));
                 unsigned int s = (unsigned int)((key * 0x9E3779B97F4A7C15ull) >> 48) & (VGC_T - 1);
                 while (true) {
                     const unsigned long long prev = atomicCAS(&B.hkey[s], VGC_EMPTY, key);
@@ -338,21 +297,16 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
 #pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o));
-            hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o));
-        }
-        cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+        for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_join(k, box[k], __shfl_xor_sync(0xffffffffu, box[k], o));
     }
     if (lane == 0) {
 #pragma unroll
-        for (int k = 0; k < 3; ++k) { S.red[k][warp] = lo[k]; S.red[3 + k][warp] = hi[k]; }
-        S.red[6][warp] = cnt;
+        for (int k = 0; k < kBoxInts; ++k) S.red[k][warp] = box[k];
     }
     __syncthreads();
-    if (tid < 7) {
+    if (tid < kBoxInts) {
         int v = S.red[tid][0];
-        for (int w = 1; w < VGC_WARPS; ++w) v = tid < 3 ? min(v, S.red[tid][w]) : tid < 6 ? max(v, S.red[tid][w]) : v + S.red[tid][w];
+        for (int w = 1; w < VGC_WARPS; ++w) v = vg_box_join(tid, v, S.red[tid][w]);
         B.mmpart[tid * G + blockIdx.x] = v;
     }
     vgc_barrier(&ctl[0], G);
@@ -367,42 +321,21 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
     if (!bail) {
         // ---- phase 2: box parameters (block 0), output ranks and member segments
         if (blockIdx.x == 0 && warp == 0) {
-            int mm[7] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
+            int mm[kBoxInts];
+#pragma unroll
+            for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_empty(k);
             for (unsigned int b = lane; b < G; b += 32) {
 #pragma unroll
-                for (int k = 0; k < 7; ++k) {
-                    const int v = __ldcg(&B.mmpart[k * G + b]);
-                    mm[k] = k < 3 ? min(mm[k], v) : k < 6 ? max(mm[k], v) : mm[k] + v;
-                }
+                for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_join(k, mm[k], __ldcg(&B.mmpart[k * G + b]));
             }
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) {
 #pragma unroll
-                for (int k = 0; k < 7; ++k) {
-                    const int v = __shfl_xor_sync(0xffffffffu, mm[k], o);
-                    mm[k] = k < 3 ? min(mm[k], v) : k < 6 ? max(mm[k], v) : mm[k] + v;
-                }
+                for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_join(k, mm[k], __shfl_xor_sync(0xffffffffu, mm[k], o));
             }
             if (lane == 0) {
-                VgParams p;
-                p.inv_leaf = inv_leaf;
-                p.n_finite = mm[6];
-                p.overflow = 0;
-                p.bail = 0;
-                if (p.n_finite == 0) {
-                    for (int k = 0; k < 3; ++k) { p.min_b[k] = 0; p.div_b[k] = 1; }
-                } else {
-                    long long d[3];
-                    for (int k = 0; k < 3; ++k) {
-                        const float flo = vg_ord2f(mm[k]), fhi = vg_ord2f(mm[3 + k]);
-                        d[k] = (long long)((fhi - flo) * p.inv_leaf) + 1;
-                        p.min_b[k] = (int)floorf(flo * p.inv_leaf);
-                        const int max_b = (int)floorf(fhi * p.inv_leaf);
-                        p.div_b[k] = max_b - p.min_b[k] + 1;
-                    }
-                    if (d[0] * d[1] * d[2] > (long long)INT_MAX) { p.overflow = 1; p.bail = 1; atomicOr(&ctl[1], 4u); }   // PCL copies the input: sort chain
-                }
-                p.mul[0] = 1; p.mul[1] = p.div_b[0]; p.mul[2] = p.div_b[0] * p.div_b[1];
+                VgParams p = vg_params(mm, leaf);
+                if (p.overflow) { p.bail = 1; atomicOr(&ctl[1], 4u); }   // PCL copies the input: sort chain
                 *pp = p;
                 *count_out = p.bail ? 0 : U;
             }
@@ -585,7 +518,7 @@ int voxelgrid_coop(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, i
     return LILIOM_OK;
 }
 
-// box of the finite points of a device cloud, left in c->vg_minmax (7 ints, k_vg_minmax's encoding); no sync
+// box of the finite points of a device cloud, left in c->vg_minmax (7 ints, vg_box.h); no sync
 int vg_minmax_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride) {
     LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
     int* mm = c->vg_minmax.as<int>();
@@ -620,7 +553,7 @@ int voxelgrid_dev2(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, i
     VgParams* pp = c->vg_params.as<VgParams>();
     if (host_mm) {
         VgBox b;
-        for (int k = 0; k < 7; ++k) b.mm[k] = host_mm[k];
+        for (int k = 0; k < kBoxInts; ++k) b.mm[k] = host_mm[k];
         k_vg_params_box<<<1, 32, 0, c->stream>>>(b, leaf, pp);
         LILI_TRY(launch_check(c, "k_vg_params_box"));
     } else {
@@ -650,26 +583,10 @@ int voxelgrid_dev2(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, i
     return LILIOM_OK;
 }
 
-static float vg_ord2f_host(int i) { int j = i >= 0 ? i : i ^ 0x7fffffff; float f; memcpy(&f, &j, 4); return f; }
-
 // d_feats (optional): the centroids also as float4 {x, y, z, output index}; host_mm (optional): see voxelgrid_dev2 — the
-// key width of the sort then follows from the box (k_vg_params' arithmetic repeated on the host) instead of 32 bits.
+// key width of the sort then follows from the box (vg_key_bits) instead of 32 bits.
 int voxelgrid_dev(liliom_ctx* c, const void* d_in, int n, int stride, float leaf, void* d_out, int* d_count, float4* d_feats, const int* host_mm) {
-    int key_bits = 32;
-    if (host_mm && host_mm[6] > 0) {
-        const float inv_leaf = 1.0f / leaf;
-        long long cells = 1, dd = 1;
-        for (int k = 0; k < 3; ++k) {
-            const float lo = vg_ord2f_host(host_mm[k]), hi = vg_ord2f_host(host_mm[3 + k]);
-            dd *= (long long)((hi - lo) * inv_leaf) + 1;
-            cells *= (long long)((int)floorf(hi * inv_leaf) - (int)floorf(lo * inv_leaf) + 1);
-        }
-        if (dd <= (long long)INT_MAX && cells > 0 && cells < (1LL << 31)) {      // not PCL's overflow case; all-ones of the width stays free for the sentinel
-            key_bits = 1;
-            while ((1LL << key_bits) <= cells) ++key_bits;
-            if (key_bits < 8) key_bits = 8;
-        }
-    }
+    const int key_bits = host_mm ? vg_key_bits(host_mm, leaf) : 32;
     return voxelgrid_dev2(c, d_in, n, nullptr, stride, leaf, d_out, d_count, d_feats, key_bits, host_mm);
 }
 

@@ -528,6 +528,12 @@ def test_map_too_large_for_dense_grid():
     with pytest.raises(L.LiliomError) as e:
         c.map_set_points(m)
     assert e.value.code == -5           # LILIOM_E_GRID: extent needs more than 2^29 one-metre cells
+    for bad in (np.nan, np.inf):        # a non-finite map point is an argument error, not a point outside the box
+        m = np.ones((16, 4), np.float32)
+        m[7, 1] = bad
+        with pytest.raises(L.LiliomError) as e:
+            c.map_set_points(m)
+        assert e.value.code == -1       # LILIOM_E_ARG
     c.close()
 
 
