@@ -48,7 +48,6 @@ __global__ void k_compact_strided(const unsigned char* __restrict__ in, const in
     float4* dst = reinterpret_cast<float4*>(out + (size_t)pos[i] * stride);
     for (int k = 0; k < stride / 16; ++k) dst[k] = src[k];
 }
-__global__ void k_int_to_double(const int* __restrict__ in, double* __restrict__ out) { if (threadIdx.x == 0) out[0] = (double)in[0]; }
 
 __global__ void k_compact_f4(const float4* __restrict__ in, const int* __restrict__ flags, const int* __restrict__ pos, int n, float4* __restrict__ out) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -101,11 +100,6 @@ __global__ void k_undistort(unsigned char* __restrict__ pts, int n, int stride, 
     a.y = (float)addx(r.y, mulx(ratio_i, trans.y));
     a.z = (float)addx(r.z, mulx(ratio_i, trans.z));
     p0[0] = a;
-}
-
-__global__ void k_gather_refl48(const unsigned char* __restrict__ pts, int n, float* __restrict__ out) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = reinterpret_cast<const float*>(pts + (size_t)i * 48)[9];
 }
 
 static int install_map_from_xyzw(liliom_ctx* c, int m) {
@@ -396,7 +390,7 @@ extern "C" int liliom_voxelgrid(liliom_ctx* c, const void* pts, int n, int strid
         if (hp->vgp.bail) coop = false;
     }
     if (!coop) {
-        LILI_TRY(voxelgrid_dev(c, c->raw.p, n, stride, leaf, c->vg_out.p, c->vg_count.as<int>()));
+        LILI_TRY(voxelgrid_dev(c, c->raw.p, n, nullptr, stride, leaf, c->vg_out.p, c->vg_count.as<int>()));
         LILI_CUDA(c, cudaMemcpyAsync(&hp->vg_count, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
         LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     }
@@ -632,8 +626,8 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
     if (total > 0) {
         // (The single-launch cooperative filter of the scan VoxelGrid was tried here for maps of <= 32k points: within the noise
         // of the real-size streamed lifecycle — not kept.)
-        LILI_TRY(voxelgrid_dev(c, c->map_raw.p, (int)total, stride, c->prm.leaf_map, c->map_ds.p, c->vg_count.as<int>(),   // :316-317
-                               c->nranks == 1 ? c->map.xyzw.as<float4>() : nullptr, box));
+        LILI_TRY(voxelgrid_dev(c, c->map_raw.p, (int)total, nullptr, stride, c->prm.leaf_map, c->map_ds.p, c->vg_count.as<int>(),   // :316-317
+                               c->nranks == 1 ? c->map.xyzw.as<float4>() : nullptr, 32, box));
         LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->vg_count, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
         LILI_CUDA(c, cudaStreamSynchronize(c->stream));
         m = c->h_pin->vg_count;
@@ -721,8 +715,8 @@ extern "C" int liliom_map_set_cloud(liliom_ctx* c, const void* pts, int m, int s
         LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, pts, (size_t)m * stride, cudaMemcpyHostToDevice, c->stream));
         LILI_TRY(repack_to_f4(c, c->raw.p, m, stride, c->map.xyzw.as<float4>()));
         if (stride == 48) {
-            k_gather_refl48<<<cdiv(m, 256), 256, 0, c->stream>>>((const unsigned char*)c->raw.p, m, c->map.refl.as<float>());
-            LILI_TRY(launch_check(c, "k_gather_refl48"));
+            k_kf_refl<<<cdiv(m, 256), 256, 0, c->stream>>>((const unsigned char*)c->raw.p, m, c->map.refl.as<float>());
+            LILI_TRY(launch_check(c, "k_kf_refl"));
         } else LILI_CUDA(c, cudaMemsetAsync(c->map.refl.p, 0, (size_t)m * sizeof(float), c->stream));
     }
     LILI_TRY(install_map_from_xyzw(c, m));
@@ -840,7 +834,7 @@ static int odometry_on_resident_surf(liliom_ctx* c, double pose7[7], int match_c
         if (!spec_failed)
             LILI_TRY(voxelgrid_coop(c, c->surf.p, n_max, d_n, stride, c->prm.leaf_scan, c->vg_out.p, c->vg_count.as<int>(), c->feats.as<float4>(), &coop));
         if (!coop)
-            LILI_TRY(voxelgrid_dev2(c, c->surf.p, n_max, d_n, stride, c->prm.leaf_scan, c->vg_out.p, c->vg_count.as<int>(), c->feats.as<float4>(), key_bits));
+            LILI_TRY(voxelgrid_dev(c, c->surf.p, n_max, d_n, stride, c->prm.leaf_scan, c->vg_out.p, c->vg_count.as<int>(), c->feats.as<float4>(), key_bits));
         c->d_nfeats = c->vg_count.as<int>();
         c->vg_used24 = !coop && key_bits < 32;
         c->vg_check = coop || key_bits < 32;

@@ -280,15 +280,14 @@ int sort_pairs_u64(liliom_ctx* c, const unsigned long long* kin, unsigned long l
 int exclusive_scan_i32(liliom_ctx* c, const int* in, int* out, int n);   // out has n+1 entries (total at out[n])
 int inclusive_max_scan_i32(liliom_ctx* c, int* data, int n);            // in-place running maximum
 
-// VoxelGrid on device buffers; d_count receives the output count (int, device).
-int voxelgrid_dev(liliom_ctx* c, const void* d_in, int n, int stride, float leaf, void* d_out, int* d_count, float4* d_feats = nullptr,
-                  const int* host_mm = nullptr);
+// VoxelGrid on device buffers; d_count receives the output count (int, device).  n_max = host upper bound, d_n = optional
+// device-side count (<= n_max); d_feats (optional) also receives float4{x,y,z,index}.  key_bits, host_mm: see voxelgrid.cu.
+int voxelgrid_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride, float leaf, void* d_out, int* d_count,
+                  float4* d_feats = nullptr, int key_bits = 32, const int* host_mm = nullptr);
 int vg_minmax_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride);
-// n_max = host upper bound, d_n = optional device-side count (<= n_max); d_feats (optional) also receives float4{x,y,z,index}
 int voxelgrid_coop(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride, float leaf, void* d_out, int* d_count, float4* d_feats,
                    bool* used);
-int voxelgrid_dev2(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride, float leaf, void* d_out, int* d_count, float4* d_feats,
-                   int key_bits = 32, const int* host_mm = nullptr);
+__global__ void k_kf_refl(const unsigned char* __restrict__ pts, int n, float* __restrict__ out);      // keyframes.cu: reflectivity of 48-byte points
 
 // grid build of index `mi` from float4 points already on the device (mi.xyzw[0..m)), cells of `cell` metres (gate_cell).
 // host_box (optional): 6 ordered ints, a box known to contain the points up to rounding of a mean (the union of the frames'

@@ -494,24 +494,11 @@ __global__ void k_rot_lf_keys(const Pt32* __restrict__ cloud, const uint32_t* __
         float4 a = cloud[k].a;
         unsigned idx;
         if (p.overflow) idx = (unsigned)t;     // PCL returns the input unchanged: every point its own voxel, input order
-        else {
-            int i0 = (int)(floorf(a.x * p.inv_leaf) - (float)p.min_b[0]);
-            int i1 = (int)(floorf(a.y * p.inv_leaf) - (float)p.min_b[1]);
-            int i2 = (int)(floorf(a.z * p.inv_leaf) - (float)p.min_b[2]);
-            idx = (unsigned)(i0 * p.mul[0] + i1 * p.mul[1] + i2 * p.mul[2]);
-        }
+        else idx = vg_rel_index(p, a.x, a.y, a.z);
         key = ((unsigned long long)ring << 32) | idx;
     }
     keys[t] = key;
     vals[t] = t;
-}
-
-__global__ void k_rot_lf_heads(const unsigned long long* __restrict__ keys, const int* __restrict__ meta, int cap, int* __restrict__ flags) {
-    int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t > cap) return;
-    int f = 0;
-    if (t < cap && t < meta[M_NLF]) f = (t == 0 || keys[t] != keys[t - 1]);
-    flags[t] = f;
 }
 
 __global__ void k_rot_lf_centroid(const Pt32* __restrict__ cloud, const int* __restrict__ lf_src, const unsigned long long* __restrict__ keys,
@@ -519,21 +506,10 @@ __global__ void k_rot_lf_centroid(const Pt32* __restrict__ cloud, const int* __r
                                   const int* __restrict__ meta, int cap, Pt32* __restrict__ out, int* __restrict__ n_out) {
     int t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t == 0) *n_out = rank[cap];
-    const int nlf = meta[M_NLF];
-    if (t >= cap || t >= nlf || !flags[t]) return;
-    const unsigned long long key = keys[t];
-    float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f;
-    int cnt = 0;
-    for (int j = t; j < nlf && keys[j] == key; ++j) {
-        const Pt32 p = cloud[lf_src[vals[j]]];
-        sx += p.a.x; sy += p.a.y; sz += p.a.z; si += p.b.x;
-        ++cnt;
-    }
-    const float fc = (float)cnt;
-    Pt32 o;
-    o.a = make_float4(sx / fc, sy / fc, sz / fc, 1.0f);
-    o.b = make_float4(si / fc, 0.f, 0.f, 0.f);
-    out[rank[t]] = o;
+    if (t >= cap || !flags[t]) return;
+    const VgAcc<32> a = vg_walk<32>(keys, t, meta[M_NLF], [&](int j) { return lf_src[vals[j]]; },
+                                    [&](int m) { return reinterpret_cast<const unsigned char*>(cloud + m); });
+    vg_write<32>(a.s, a.n, reinterpret_cast<unsigned char*>(out + rank[t]));
 }
 
 // edge output: segment-major, pick order inside the segment (one block, 64*6 = 384 segments)
@@ -650,8 +626,8 @@ int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_
     k_rot_lf_keys<<<cdiv(n, 256), 256, 0, c->stream>>>(cloud, ring_of, lf_src, meta, rprm, k64, vals, n);
     LILI_TRY(launch_check(c, "k_rot_lf_keys"));
     LILI_TRY(sort_pairs_u64(c, k64, k64b, vals, vals2, n, 40));
-    k_rot_lf_heads<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(k64b, meta, n, c->vg_flags.as<int>());
-    LILI_TRY(launch_check(c, "k_rot_lf_heads"));
+    k_vg_heads<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(k64b, n, meta + M_NLF, c->vg_flags.as<int>());
+    LILI_TRY(launch_check(c, "k_vg_heads"));
     LILI_TRY(exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), n));
     k_rot_lf_centroid<<<cdiv(n, 128), 128, 0, c->stream>>>(cloud, lf_src, k64b, vals2, c->vg_flags.as<int>(), c->vg_rank.as<int>(), meta, n,
                                                            c->surf.as<Pt32>(), c->vg_count.as<int>());

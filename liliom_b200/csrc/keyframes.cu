@@ -132,8 +132,8 @@ extern "C" int liliom_kf_add(liliom_ctx* c, const liliom_backend_params* bp, con
     if (n_surf) LILI_CUDA(c, cudaMemcpyAsync(raw + (size_t)n_edge * stride, surf_last, (size_t)n_surf * stride, cudaMemcpyHostToDevice, c->stream));
     unsigned char* tail = (unsigned char*)c->kf_arena.p + (size_t)c->kf_used * stride;
     int* cnt = c->vg_count.as<int>();
-    LILI_TRY(voxelgrid_dev(c, raw, n_edge, stride, bp->edge_leaf, tail, cnt));                                           // :1502-1507
-    LILI_TRY(voxelgrid_dev(c, raw + (size_t)n_edge * stride, n_surf, stride, bp->surf_leaf, c->vg_out.p, cnt + 1));     // :1509-1514
+    LILI_TRY(voxelgrid_dev(c, raw, n_edge, nullptr, stride, bp->edge_leaf, tail, cnt));                                           // :1502-1507
+    LILI_TRY(voxelgrid_dev(c, raw + (size_t)n_edge * stride, n_surf, nullptr, stride, bp->surf_leaf, c->vg_out.p, cnt + 1));     // :1509-1514
     LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, cnt, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     const int me = c->h_pin->bk_cnt[0], ms = c->h_pin->bk_cnt[1];
@@ -191,7 +191,7 @@ extern "C" int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp,
     for (int l = 0; l < 2; ++l) {                                 // :1486-1492; the centroid kernel also writes the float4 points
         LILI_CUDA(c, c->bmap_ds[l].ensure((size_t)std::max(nl[l], 1LL) * stride));
         LILI_CUDA(c, c->bmap[l].xyzw.ensure((size_t)std::max(nl[l], 1LL) * sizeof(float4)));
-        LILI_TRY(voxelgrid_dev(c, src[l], (int)nl[l], stride, leaf[l], c->bmap_ds[l].p, cnt + l, c->bmap[l].xyzw.as<float4>()));
+        LILI_TRY(voxelgrid_dev(c, src[l], (int)nl[l], nullptr, stride, leaf[l], c->bmap_ds[l].p, cnt + l, c->bmap[l].xyzw.as<float4>()));
     }
     LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, cnt, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -248,7 +248,7 @@ extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* p
     LILI_CUDA(c, c->vg_out.ensure((size_t)off * stride));
     LILI_CUDA(c, c->vg_count.ensure(16));
     LILI_TRY(kf_gather(c, tab, largest, c->bmap_raw.p));
-    LILI_TRY(voxelgrid_dev(c, c->bmap_raw.p, (int)off, stride, leaf, c->vg_out.p, c->vg_count.as<int>()));
+    LILI_TRY(voxelgrid_dev(c, c->bmap_raw.p, (int)off, nullptr, stride, leaf, c->vg_out.p, c->vg_count.as<int>()));
     LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     const int m = c->h_pin->bk_cnt[0];

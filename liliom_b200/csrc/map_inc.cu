@@ -88,15 +88,7 @@ __global__ void k_inc_merge_new(const u64* __restrict__ newkeys, const unsigned*
     const int pos = j + (ub - rpos[ub]);
     keys2[pos] = k; refs2[pos] = newrefs[j];
 }
-// flags[i] = 1 at the first entry of every voxel; flags[E] = 0 (scan sentinel)
-__global__ void k_inc_heads(const u64* __restrict__ keys, int E, int* __restrict__ flags) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i > E) return;
-    flags[i] = (i < E && (i == 0 || keys[i] != keys[i - 1])) ? 1 : 0;
-}
-
-// centroid of every voxel, members in entry order: the arithmetic of k_vg_centroid (voxelgrid.cu), the points fetched through
-// the frame table
+// centroid of every voxel, members in entry order (vg_box.h), the points fetched through the frame table
 template <int STRIDE>
 __global__ void k_inc_centroid(const __grid_constant__ FrameTab tab, const u64* __restrict__ keys, const unsigned* __restrict__ refs,
                                const int* __restrict__ flags, const int* __restrict__ rank, int E, unsigned char* __restrict__ out,
@@ -104,53 +96,9 @@ __global__ void k_inc_centroid(const __grid_constant__ FrameTab tab, const u64* 
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i == 0) *count_out = rank[E];
     if (i >= E || !flags[i]) return;
-    const int o = rank[i];
-    const u64 key = keys[i];
-    float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f, sc = 0.f, snx = 0.f, sny = 0.f, snz = 0.f;
-    int cnt = 0;
-    bool more = true;
-#pragma unroll 1
-    for (int k0 = i; more; k0 += 8) {
-        const unsigned char* src[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-            src[u] = nullptr;
-            if (k0 + u < E && keys[k0 + u] == key) {
-                const unsigned r = refs[k0 + u];
-                src[u] = tab.base[r >> 24] + (size_t)(r & kIncIdxMask) * STRIDE;
-            }
-        }
-        float4 A[8], B[8], Cc[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-            if (src[u]) {
-                A[u] = *reinterpret_cast<const float4*>(src[u]);
-                B[u] = *reinterpret_cast<const float4*>(src[u] + 16);
-                if (STRIDE == 48) Cc[u] = *reinterpret_cast<const float4*>(src[u] + 32);
-            }
-        }
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-            if (src[u]) {
-                sx += A[u].x; sy += A[u].y; sz += A[u].z;
-                if (STRIDE == 48) { snx += B[u].x; sny += B[u].y; snz += B[u].z; si += Cc[u].x; sc += Cc[u].y; }
-                else si += B[u].x;
-                ++cnt;
-            }
-        }
-        more = src[7] != nullptr;
-    }
-    const float fc = (float)cnt;
-    unsigned char* dst = out + (size_t)o * STRIDE;
-    *reinterpret_cast<float4*>(dst) = make_float4(sx / fc, sy / fc, sz / fc, 1.0f);
-    if (STRIDE == 48) {
-        float n2 = snx * snx + sny * sny + snz * snz;
-        if (n2 > 0.0f) { float nn = sqrtf(n2); snx = snx / nn; sny = sny / nn; snz = snz / nn; }
-        *reinterpret_cast<float4*>(dst + 16) = make_float4(snx, sny, snz, 0.0f);
-        *reinterpret_cast<float4*>(dst + 32) = make_float4(si / fc, sc / fc, 0.0f, 0.0f);
-    } else {
-        *reinterpret_cast<float4*>(dst + 16) = make_float4(si / fc, 0.0f, 0.0f, 0.0f);
-    }
+    const VgAcc<STRIDE> a = vg_walk<STRIDE>(keys, i, E, [&](int j) { return (int)refs[j]; },       // (slot < 64: a ref is below 2^30)
+                                            [&](int r) { return tab.base[r >> 24] + (size_t)(r & kIncIdxMask) * STRIDE; });
+    vg_write<STRIDE>(a.s, a.n, out + (size_t)rank[i] * STRIDE);
 }
 
 // keys + refs of frame `f` (points already in f.buf), written at keys/refs, and its key flag; one sync
@@ -215,8 +163,8 @@ static int inc_emit(liliom_ctx* c, int* m_out) {
     LILI_CUDA(c, c->inc_rank.ensure(((size_t)E + 2) * 4));
     const u64* keys = c->inc_key[c->inc_cur].as<u64>();
     const unsigned* refs = c->inc_ref[c->inc_cur].as<unsigned>();
-    k_inc_heads<<<cdiv(E + 1, 256), 256, 0, c->stream>>>(keys, E, c->inc_flags.as<int>());
-    LILI_TRY(launch_check(c, "k_inc_heads"));
+    k_vg_heads<<<cdiv(E + 1, 256), 256, 0, c->stream>>>(keys, E, nullptr, c->inc_flags.as<int>());
+    LILI_TRY(launch_check(c, "k_vg_heads"));
     LILI_TRY(exclusive_scan_i32(c, c->inc_flags.as<int>(), c->inc_rank.as<int>(), E));
     FrameTab tab{};
     for (auto& f : c->frames) tab.base[f.slot] = (const unsigned char*)f.buf.p;

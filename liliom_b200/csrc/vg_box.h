@@ -1,13 +1,18 @@
-// The bounding box every VoxelGrid and cell grid starts from, and PCL's VoxelGrid parameters derived from it
-// (pcl::getMinMax3D + pcl::VoxelGrid::applyFilter, voxel_grid.hpp).  The box is 7 ints: min xyz and max xyz of the finite
-// points in the ordered-int encoding below, so that integer atomics order floats, then the finite count.  Every kernel that
-// measures a box or turns one into voxel indices (voxelgrid.cu, map_inc.cu, extract_rot.cu, grid_knn.cu) and the host code
-// that reads a box back use this file, so they agree on every voxel.  Plain C++ usable from device code and from the host
-// (tests/vg_box_host.cpp compiles this same file for the CPU test tier).
+// The VoxelGrid arithmetic shared by host and device (pcl::getMinMax3D + pcl::VoxelGrid::applyFilter, voxel_grid.hpp, and
+// pcl::CentroidPoint, centroid.hpp):
+//   * the bounding box every VoxelGrid and cell grid starts from: 7 ints, min xyz and max xyz of the finite points in the
+//     ordered-int encoding below, so that integer atomics order floats, then the finite count;
+//   * PCL's parameters derived from it and a point's voxel index;
+//   * a voxel's centroid: the fields summed, the walk over its members in a sorted entry array, and the output point.
+// The kernels that measure a box, index voxels or write centroids (the sort chain and k_vg_coop in voxelgrid.cu, the
+// incremental map in map_inc.cu, the per-ring filter in extract_rot.cu, the cell grid in grid_knn.cu) and the host code that
+// reads a box back use this file, so they agree on every voxel and every bit of a centroid.  Plain C++ usable from device
+// code and from the host (tests/vg_box_host.cpp compiles this same file for the CPU test tier).
 //
 // No expression here is a contractible a*b+c: the file is compiled both with --fmad=false (voxelgrid.cu) and without it
-// (grid_knn.cu) and must give the same bits either way.  Integer products that can leave int / long long are formed in
-// unsigned arithmetic and converted back: the device's wrapped bits, no undefined behaviour in the host build.
+// (grid_knn.cu) and must give the same bits either way; the one sum of products (a normal's squared norm) is spelled with
+// round-to-nearest intrinsics on the device.  Integer products that can leave int / long long are formed in unsigned
+// arithmetic and converted back: the device's wrapped bits, no undefined behaviour in the host build.
 #pragma once
 #include <climits>
 #include <cmath>
@@ -15,8 +20,10 @@
 
 #ifdef __CUDACC__
 #define VGB_HD __host__ __device__ __forceinline__
+#define VGB_PRAGMA(x) _Pragma(#x)      // loop pragmas of the device build
 #else
 #define VGB_HD inline
+#define VGB_PRAGMA(x)
 #endif
 
 namespace lili {
@@ -102,6 +109,14 @@ VGB_HD VgParams vg_params(const int* box, float leaf) {
     return p;
 }
 
+// PCL's voxel index of a finite point relative to the box: i0·mul0 + i1·mul1 + i2·mul2 with ik = floor(p_k / leaf) - min_b[k]
+VGB_HD unsigned vg_rel_index(const VgParams& p, float x, float y, float z) {
+    const int i0 = (int)(floorf(x * p.inv_leaf) - (float)p.min_b[0]);
+    const int i1 = (int)(floorf(y * p.inv_leaf) - (float)p.min_b[1]);
+    const int i2 = (int)(floorf(z * p.inv_leaf) - (float)p.min_b[2]);
+    return (unsigned)i0 * (unsigned)p.mul[0] + (unsigned)i1 * (unsigned)p.mul[1] + (unsigned)i2 * (unsigned)p.mul[2];
+}
+
 // Width of the VoxelGrid sort chain's keys for a cloud with this box: the fewest bits (at least 8) that hold every voxel
 // index with the all-ones key of that width left free for the non-finite points' sentinel; 32 when the box is empty, in
 // PCL's overflow case, or when the voxel count does not fit.
@@ -125,5 +140,111 @@ VGB_HD bool vg_abs_key(float x, float y, float z, float inv_leaf, unsigned long 
            (unsigned long long)((int)fx + (1 << 20));
     return true;
 }
+
+// ---- the centroid of a voxel (pcl::CentroidPoint over a 48-byte PointXYZINormal or a 32-byte PointXYZI)
+#ifdef __CUDACC__
+typedef float4 VgF4;
+VGB_HD VgF4 vg_ld4(const unsigned char* p) { return *reinterpret_cast<const float4*>(p); }
+VGB_HD void vg_st4(unsigned char* p, float a, float b, float c, float d) { *reinterpret_cast<float4*>(p) = make_float4(a, b, c, d); }
+#else
+struct VgF4 { float x, y, z, w; };
+inline VgF4 vg_ld4(const unsigned char* p) { VgF4 v; memcpy(&v, p, 16); return v; }
+inline void vg_st4(unsigned char* p, float a, float b, float c, float d) { const VgF4 v{a, b, c, d}; memcpy(p, &v, 16); }
+#endif
+
+// The fields of a point the centroid sums, in this order: x y z nx ny nz intensity curvature (48 bytes), x y z intensity (32).
+template <int STRIDE> constexpr int kVgFields = STRIDE == 48 ? 8 : 4;
+template <int STRIDE>
+VGB_HD void vg_load(const unsigned char* src, float* f) {
+    const VgF4 a = vg_ld4(src), b = vg_ld4(src + 16);
+    f[0] = a.x; f[1] = a.y; f[2] = a.z;
+    if constexpr (STRIDE == 48) {
+        const VgF4 c = vg_ld4(src + 32);
+        f[3] = b.x; f[4] = b.y; f[5] = b.z; f[6] = c.x; f[7] = c.y;
+    } else {
+        f[3] = b.x;
+    }
+}
+
+// Per-field fp32 sums and the member count; points are added in member order.
+template <int STRIDE>
+struct VgAcc {
+    float s[kVgFields<STRIDE>] = {};
+    int n = 0;
+    VGB_HD void add(const float* f) {
+        VGB_PRAGMA(unroll)
+        for (int k = 0; k < kVgFields<STRIDE>; ++k) s[k] += f[k];
+        ++n;
+    }
+};
+
+// Entry i of a sorted key array whose first n_valid entries are valid starts a voxel.
+template <typename K>
+VGB_HD bool vg_is_head(const K* keys, int i, int n_valid) { return i < n_valid && (i == 0 || keys[i] != keys[i - 1]); }
+
+// The sums of the voxel whose first sorted entry is `head`: entries j = head, head + 1, ... while j < n_valid and keys[j] is
+// keys[head], in entry order.  member(j) is the point of entry j (an int >= 0), point(m) that point's address.  Members are
+// fetched 8 at a time so that their loads overlap; the sums stay sequential.
+template <int STRIDE, typename K, typename Member, typename Point>
+VGB_HD VgAcc<STRIDE> vg_walk(const K* keys, int head, int n_valid, Member member, Point point) {
+    VgAcc<STRIDE> acc;
+    const K key = keys[head];
+    VGB_PRAGMA(unroll 1)
+    for (int k0 = head;; k0 += 8) {
+        int m[8];
+        VGB_PRAGMA(unroll)
+        for (int u = 0; u < 8; ++u) m[u] = (k0 + u < n_valid && keys[k0 + u] == key) ? member(k0 + u) : -1;
+        float f[8][kVgFields<STRIDE>];
+        VGB_PRAGMA(unroll)
+        for (int u = 0; u < 8; ++u)
+            if (m[u] >= 0) vg_load<STRIDE>(point(m[u]), f[u]);
+        VGB_PRAGMA(unroll)
+        for (int u = 0; u < 8; ++u)
+            if (m[u] >= 0) acc.add(f[u]);
+        if (m[7] < 0) return acc;
+    }
+}
+
+// ((x·x + y·y) + z·z), never contracted
+VGB_HD float vg_sqnorm(float x, float y, float z) {
+#ifdef __CUDA_ARCH__
+    return __fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z));
+#else
+    return (x * x + y * y) + z * z;
+#endif
+}
+
+struct VgXyz { float x, y, z; };
+
+// Writes the output point of a voxel from its sums s and member count n, as pcl::CentroidPoint::get does: xyz, intensity and
+// curvature divided by the count, the normal normalised (not divided) when its squared norm is > 0, w = 1, padding 0.
+// Returns the centroid's xyz.
+template <int STRIDE>
+VGB_HD VgXyz vg_write(const float* s, int n, unsigned char* dst) {
+    const float fc = (float)n;
+    const VgXyz c{s[0] / fc, s[1] / fc, s[2] / fc};
+    vg_st4(dst, c.x, c.y, c.z, 1.0f);
+    if constexpr (STRIDE == 48) {
+        float nx = s[3], ny = s[4], nz = s[5];
+        const float n2 = vg_sqnorm(nx, ny, nz);
+        if (n2 > 0.0f) { const float nn = sqrtf(n2); nx = nx / nn; ny = ny / nn; nz = nz / nn; }
+        vg_st4(dst + 16, nx, ny, nz, 0.0f);
+        vg_st4(dst + 32, s[6] / fc, s[7] / fc, 0.0f, 0.0f);
+    } else {
+        vg_st4(dst + 16, s[3] / fc, 0.0f, 0.0f, 0.0f);
+    }
+    return c;
+}
+
+#ifdef __CUDACC__
+// flags[i] = 1 at the first entry of every voxel of a sorted key array; 0 at entries past the valid count (*d_valid, or n
+// when d_valid is null) and at flags[n] (the sentinel of the exclusive scan that numbers the voxels)
+template <typename K>
+__global__ void k_vg_heads(const K* __restrict__ keys, int n, const int* __restrict__ d_valid, int* __restrict__ flags) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i > n) return;
+    flags[i] = i < n && vg_is_head(keys, i, d_valid ? *d_valid : n);
+}
+#endif
 
 }  // namespace lili

@@ -69,39 +69,22 @@ __global__ void k_vg_keys(const unsigned char* __restrict__ pts, int n_max, cons
     float4 v = make_float4(NAN, 0.f, 0.f, 0.f);
     if (i < n) v = *reinterpret_cast<const float4*>(pts + (size_t)i * stride);
     uint32_t key = 0xffffffffu;
-    if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) {
-        int i0 = (int)(floorf(v.x * p.inv_leaf) - (float)p.min_b[0]);
-        int i1 = (int)(floorf(v.y * p.inv_leaf) - (float)p.min_b[1]);
-        int i2 = (int)(floorf(v.z * p.inv_leaf) - (float)p.min_b[2]);
-        key = (uint32_t)(i0 * p.mul[0] + i1 * p.mul[1] + i2 * p.mul[2]);
-    }
+    if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) key = vg_rel_index(p, v.x, v.y, v.z);
     keys[i] = key;
     vals[i] = i;
-}
-
-// flags[i] = 1 at the first sorted entry of every occupied voxel; flags[n] = 0 (scan sentinel)
-__global__ void k_vg_heads(const uint32_t* __restrict__ keys, int n, const VgParams* __restrict__ pp, int* __restrict__ flags) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i > n) return;
-    int f = 0;
-    if (i < n) {
-        int nf = pp->n_finite;   // non-finite points carry key 0xffffffff and sort last; exclude by count
-        f = (i < nf) && (i == 0 || keys[i] != keys[i - 1]);
-    }
-    flags[i] = f;
 }
 
 template <int STRIDE>
 __global__ void k_vg_centroid(const unsigned char* __restrict__ pts, const uint32_t* __restrict__ keys, const int* __restrict__ vals,
                               const int* __restrict__ flags, const int* __restrict__ rank, int n_max, const int* __restrict__ d_n,
-                              const VgParams* __restrict__ pp, unsigned char* __restrict__ out, int cap, int* __restrict__ count_out,
+                              const VgParams* __restrict__ pp, unsigned char* __restrict__ out, int* __restrict__ count_out,
                               float4* __restrict__ feats_out) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     const VgParams p = *pp;
     const int n = d_n ? min(*d_n, n_max) : n_max;
     if (i == 0) *count_out = p.overflow ? n : rank[n_max];
-    if (p.overflow) {   // PCL: output = *input_
-        if (i < n && i < cap) {
+    if (p.overflow) {   // PCL: output = *input_ (not the centroids of one-point voxels: the normal and the padding would differ)
+        if (i < n) {
             const float4* src = reinterpret_cast<const float4*>(pts + (size_t)i * STRIDE);
             float4* dst = reinterpret_cast<float4*>(out + (size_t)i * STRIDE);
 #pragma unroll
@@ -112,51 +95,10 @@ __global__ void k_vg_centroid(const unsigned char* __restrict__ pts, const uint3
     }
     if (i >= n || !flags[i]) return;
     const int o = rank[i];
-    if (o >= cap) return;
-    const uint32_t key = keys[i];
-    float sx = 0.f, sy = 0.f, sz = 0.f, si = 0.f, sc = 0.f, snx = 0.f, sny = 0.f, snz = 0.f;
-    int cnt = 0;
-    // strictly sequential fp32 sums (index order), memory latency overlapped in batches of 8 members
-    bool more = true;
-#pragma unroll 1
-    for (int k0 = i; more; k0 += 8) {
-        int idx[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) idx[u] = (k0 + u < p.n_finite && keys[k0 + u] == key) ? vals[k0 + u] : -1;
-        float4 A[8], B[8], Cc[8];
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-            if (idx[u] >= 0) {
-                const unsigned char* src = pts + (size_t)idx[u] * STRIDE;
-                A[u] = *reinterpret_cast<const float4*>(src);
-                B[u] = *reinterpret_cast<const float4*>(src + 16);
-                if (STRIDE == 48) Cc[u] = *reinterpret_cast<const float4*>(src + 32);
-            }
-        }
-#pragma unroll
-        for (int u = 0; u < 8; ++u) {
-            if (idx[u] >= 0) {
-                sx += A[u].x; sy += A[u].y; sz += A[u].z;
-                if (STRIDE == 48) { snx += B[u].x; sny += B[u].y; snz += B[u].z; si += Cc[u].x; sc += Cc[u].y; }
-                else si += B[u].x;
-                ++cnt;
-            }
-        }
-        more = idx[7] >= 0;
-    }
-    const float fc = (float)cnt;
-    unsigned char* dst = out + (size_t)o * STRIDE;
-    *reinterpret_cast<float4*>(dst) = make_float4(sx / fc, sy / fc, sz / fc, 1.0f);
-    if (feats_out) feats_out[o] = make_float4(sx / fc, sy / fc, sz / fc, __int_as_float(o));
-    if (STRIDE == 48) {
-        // pcl::CentroidPoint: normal accumulated then normalised (not divided), curvature/intensity averaged
-        float n2 = snx * snx + sny * sny + snz * snz;
-        if (n2 > 0.0f) { float nn = sqrtf(n2); snx = snx / nn; sny = sny / nn; snz = snz / nn; }
-        *reinterpret_cast<float4*>(dst + 16) = make_float4(snx, sny, snz, 0.0f);
-        *reinterpret_cast<float4*>(dst + 32) = make_float4(si / fc, sc / fc, 0.0f, 0.0f);
-    } else {
-        *reinterpret_cast<float4*>(dst + 16) = make_float4(si / fc, 0.0f, 0.0f, 0.0f);
-    }
+    const VgAcc<STRIDE> a = vg_walk<STRIDE>(keys, i, p.n_finite, [&](int j) { return vals[j]; },
+                                            [&](int m) { return pts + (size_t)m * STRIDE; });
+    const VgXyz c = vg_write<STRIDE>(a.s, a.n, out + (size_t)o * STRIDE);
+    if (feats_out) feats_out[o] = make_float4(c.x, c.y, c.z, __int_as_float(o));
 }
 
 // ---------------------------------------------------------------------------------------
@@ -414,7 +356,7 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
     if (stamp) stamp[3] = clock64();
 
     // ---- phase 4: one warp per voxel — members in ascending original index, sequential fp32 sums
-    constexpr int NF = STRIDE == 48 ? 8 : 4;
+    constexpr int NF = kVgFields<STRIDE>;
     for (int u = gwarp; u < U; u += gwarps) {
         const int s = __ldcg(&B.uslot[u]);
         const int c = __ldcg(&B.hcnt[s]);
@@ -431,19 +373,7 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
         float acc = 0.f;       // lane f < NF owns field f
         for (int base = 0; base < c; base += 32) {
             const int j = base + lane;
-            if (j < c) {
-                const unsigned char* src = pts + (size_t)S.sidx[warp][j] * STRIDE;
-                const float4 A = *reinterpret_cast<const float4*>(src);
-                const float4 Bv = *reinterpret_cast<const float4*>(src + 16);
-                float* st = S.stage[warp][lane];
-                st[0] = A.x; st[1] = A.y; st[2] = A.z;
-                if (STRIDE == 48) {
-                    const float4 Cv = *reinterpret_cast<const float4*>(src + 32);
-                    st[3] = Bv.x; st[4] = Bv.y; st[5] = Bv.z; st[6] = Cv.x; st[7] = Cv.y;
-                } else {
-                    st[3] = Bv.x;
-                }
-            }
+            if (j < c) vg_load<STRIDE>(pts + (size_t)S.sidx[warp][j] * STRIDE, S.stage[warp][lane]);
             __syncwarp();
             if (lane < NF) {
                 const int m = min(32, c - base);
@@ -455,22 +385,8 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
 #pragma unroll
         for (int k = 0; k < 8; ++k) f[k] = __shfl_sync(0xffffffffu, acc, k);
         if (lane == 0) {
-            const float fc = (float)c;
-            const float sx = f[0], sy = f[1], sz = f[2];
-            unsigned char* dst = out + (size_t)o * STRIDE;
-            *reinterpret_cast<float4*>(dst) = make_float4(sx / fc, sy / fc, sz / fc, 1.0f);
-            if (feats_out) feats_out[o] = make_float4(sx / fc, sy / fc, sz / fc, __int_as_float(o));
-            if (STRIDE == 48) {
-                float snx = f[3], sny = f[4], snz = f[5];
-                const float si = f[6], sc = f[7];
-                float n2 = snx * snx + sny * sny + snz * snz;
-                if (n2 > 0.0f) { float nn = sqrtf(n2); snx = snx / nn; sny = sny / nn; snz = snz / nn; }
-                *reinterpret_cast<float4*>(dst + 16) = make_float4(snx, sny, snz, 0.0f);
-                *reinterpret_cast<float4*>(dst + 32) = make_float4(si / fc, sc / fc, 0.0f, 0.0f);
-            } else {
-                const float si = f[3];
-                *reinterpret_cast<float4*>(dst + 16) = make_float4(si / fc, 0.0f, 0.0f, 0.0f);
-            }
+            const VgXyz cxyz = vg_write<STRIDE>(f, c, out + (size_t)o * STRIDE);
+            if (feats_out) feats_out[o] = make_float4(cxyz.x, cxyz.y, cxyz.z, __int_as_float(o));
             B.hkey[s] = VGC_EMPTY;      // hand the slot back
             B.hcnt[s] = 0;
         }
@@ -488,7 +404,7 @@ const long long* vg_coop_stamps(liliom_ctx* c) {
 }
 
 // Returns LILIOM_OK after enqueueing the cooperative filter; the caller must look at VgParams::bail (vg_params)
-// after its next sync and fall back to voxelgrid_dev2 when it is set.  *used = false: not applicable, nothing enqueued.
+// after its next sync and fall back to voxelgrid_dev when it is set.  *used = false: not applicable, nothing enqueued.
 int voxelgrid_coop(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride, float leaf, void* d_out, int* d_count,
                    float4* d_feats, bool* used) {
     *used = false;
@@ -531,10 +447,13 @@ int vg_minmax_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, in
     return LILIOM_OK;
 }
 
-// host_mm (optional): the cloud's box and finite count already known on the host -> no pass over the input for it
-int voxelgrid_dev2(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride, float leaf, void* d_out, int* d_count,
-                   float4* d_feats, int key_bits, const int* host_mm) {
+// key_bits < 32: the caller speculates that the voxel index fits that width (one onesweep pass less per 8 bits) and must check
+// `ncells <= 2^key_bits - 1` afterwards (vg_params stays on the device).  host_mm (optional): the cloud's box and finite count
+// already known on the host -> no pass over the input for it, and the key width follows from the box (vg_key_bits).
+int voxelgrid_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride, float leaf, void* d_out, int* d_count,
+                  float4* d_feats, int key_bits, const int* host_mm) {
     if (stride != 48 && stride != 32) return LILIOM_E_ARG;
+    if (host_mm) key_bits = vg_key_bits(host_mm, leaf);
     if (n_max <= 0) {
         LILI_CUDA(c, cudaMemsetAsync(d_count, 0, sizeof(int), c->stream));
         return LILIOM_OK;
@@ -566,28 +485,19 @@ int voxelgrid_dev2(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, i
     }
     k_vg_keys<<<cdiv(n, 256), 256, 0, c->stream>>>(in, n, d_n, stride, pp, c->vg_keys.as<uint32_t>(), c->vg_vals.as<int>());
     LILI_TRY(launch_check(c, "k_vg_keys"));
-    // key_bits < 32: the caller speculates that the voxel index fits (one onesweep pass less per 8 bits);
-    // invalid (sentinel) keys are folded to the all-ones key of that width and VgParams::n_finite excludes them.
-    // The caller must check `ncells <= 2^key_bits - 1` afterwards (vg_params stays on the device).
+    // non-finite points carry the all-ones key (folded to the sort's width) and sort last; VgParams::n_finite excludes them
     LILI_TRY(sort_pairs_u32(c, c->vg_keys.as<uint32_t>(), c->vg_keys2.as<uint32_t>(), c->vg_vals.as<int>(), c->vg_vals2.as<int>(), n, key_bits));
-    k_vg_heads<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(c->vg_keys2.as<uint32_t>(), n, pp, c->vg_flags.as<int>());
+    k_vg_heads<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(c->vg_keys2.as<uint32_t>(), n, &pp->n_finite, c->vg_flags.as<int>());
     LILI_TRY(launch_check(c, "k_vg_heads"));
     LILI_TRY(exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), n));
     if (stride == 48)
         k_vg_centroid<48><<<cdiv(n, 128), 128, 0, c->stream>>>(in, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(), c->vg_flags.as<int>(),
-                                                               c->vg_rank.as<int>(), n, d_n, pp, (unsigned char*)d_out, INT_MAX, d_count, d_feats);
+                                                               c->vg_rank.as<int>(), n, d_n, pp, (unsigned char*)d_out, d_count, d_feats);
     else
         k_vg_centroid<32><<<cdiv(n, 128), 128, 0, c->stream>>>(in, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(), c->vg_flags.as<int>(),
-                                                               c->vg_rank.as<int>(), n, d_n, pp, (unsigned char*)d_out, INT_MAX, d_count, d_feats);
+                                                               c->vg_rank.as<int>(), n, d_n, pp, (unsigned char*)d_out, d_count, d_feats);
     LILI_TRY(launch_check(c, "k_vg_centroid"));
     return LILIOM_OK;
-}
-
-// d_feats (optional): the centroids also as float4 {x, y, z, output index}; host_mm (optional): see voxelgrid_dev2 — the
-// key width of the sort then follows from the box (vg_key_bits) instead of 32 bits.
-int voxelgrid_dev(liliom_ctx* c, const void* d_in, int n, int stride, float leaf, void* d_out, int* d_count, float4* d_feats, const int* host_mm) {
-    const int key_bits = host_mm ? vg_key_bits(host_mm, leaf) : 32;
-    return voxelgrid_dev2(c, d_in, n, nullptr, stride, leaf, d_out, d_count, d_feats, key_bits, host_mm);
 }
 
 }  // namespace lili

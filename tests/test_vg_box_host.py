@@ -1,7 +1,8 @@
-"""CPU tier for the VoxelGrid box arithmetic: liliom_b200/csrc/vg_box.h compiled for the host (tests/vg_box_host.cpp).  The
+"""CPU tier for the VoxelGrid arithmetic: liliom_b200/csrc/vg_box.h compiled for the host (tests/vg_box_host.cpp).  The
 ordered-int encoding, the box of a cloud, PCL's VoxelGrid parameters (pcl::getMinMax3D and the leaf division of
 voxel_grid.hpp), the sort chain's key width and the absolute 21-bit voxel key against NumPy float32 restatements, at the
-leaves the reference uses (0.2, 0.4, 0.6)."""
+leaves the reference uses (0.2, 0.4, 0.6); and the whole sort chain and the ROT extractor's per-ring filter composed from the
+header (voxel index, heads, member walk, pcl::CentroidPoint writer) against the oracle's VoxelGrid, byte for byte."""
 import ctypes as C
 import os
 import subprocess
@@ -34,6 +35,10 @@ def vb():
     L.vb_key_bits.restype = C.c_int
     L.vb_abs_key.argtypes = [C.c_float, C.c_float, C.c_float, C.c_float, C.POINTER(C.c_ulonglong)]
     L.vb_abs_key.restype = C.c_int
+    L.vb_voxelgrid.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p, fp]
+    L.vb_voxelgrid.restype = C.c_int
+    L.vb_voxelgrid_rings.argtypes = [C.c_void_p, ip, C.c_int, C.c_float, C.c_void_p, fp]
+    L.vb_voxelgrid_rings.restype = C.c_int
     return L
 
 
@@ -226,3 +231,132 @@ def test_absolute_key_and_its_limit(vb, leaf):
         else:
             assert key.value == 0xDEADBEEF                                # untouched
     assert 0 < n_ok < len(pts)
+
+
+# ---- the centroid: sort chain and per-ring filter composed from the header, against the oracle
+
+def host_voxelgrid(vb, pts, leaf, ring=None):
+    """(output cloud, the centroids' xyz returned by the writer); ring: per-point ring ids -> the per-ring batch of 32-byte points"""
+    pts = np.ascontiguousarray(pts)
+    out = np.zeros(max(len(pts), 1), pts.dtype)
+    xyz = np.zeros((max(len(pts), 1), 3), np.float32)
+    if ring is None:
+        m = vb.vb_voxelgrid(pts.ctypes.data, len(pts), pts.dtype.itemsize, leaf, out.ctypes.data, xyz)
+    else:
+        m = vb.vb_voxelgrid_rings(pts.ctypes.data, np.ascontiguousarray(ring, np.int32), len(pts), leaf, out.ctypes.data, xyz)
+    assert m >= 0
+    return out[:m], xyz[:m]
+
+
+def check_voxelgrid(vb, want, pts, leaf, ring=None):
+    got, xyz = host_voxelgrid(vb, pts, leaf, ring)
+    assert len(got) == len(want)
+    assert got.tobytes() == want.tobytes()
+    assert np.array_equal(xyz.view(np.uint32), np.stack([got["x"], got["y"], got["z"]], 1).view(np.uint32))
+    return got
+
+
+def as_layout(pts, dt):
+    """the cloud in the other PCL layout: the fields both have copied, the others zero"""
+    out = np.zeros(len(pts), dt)
+    for f in dt.names:
+        if f in pts.dtype.names:
+            out[f] = pts[f]
+    return out
+
+
+@pytest.mark.parametrize("leaf", LEAVES)
+@pytest.mark.parametrize("sweep", ["hz", "hdl"])
+def test_sort_chain_matches_oracle_on_sweeps(vb, oracle, world_small, sweep, leaf):
+    for dt in (oracle.PT48, oracle.PT32):
+        pts = as_layout(world_small[sweep], dt)
+        got = check_voxelgrid(vb, oracle.voxelgrid(pts, leaf), pts, leaf)
+        assert 0 < len(got) < len(pts)
+
+
+def test_sort_chain_matches_oracle_on_adversarial_inputs(vb, oracle):
+    """points exactly on voxel faces, duplicates, non-finite points, a single point, an empty cloud"""
+    rng = np.random.default_rng(8)
+    for dt, leaf in ((oracle.PT48, 0.4), (oracle.PT32, 0.6), (oracle.PT48, 0.25), (oracle.PT32, 0.2)):
+        n = 3000
+        c = np.zeros(n, dt)
+        xyz = rng.uniform(-7, 7, (n, 3)).astype(np.float32)
+        xyz[:300] = np.round(xyz[:300] / np.float32(leaf)) * np.float32(leaf)
+        xyz[300:400] = xyz[:100]
+        c["x"], c["y"], c["z"] = xyz.T
+        c["intensity"] = rng.uniform(0, 50, n).astype(np.float32)
+        if dt is oracle.PT48:
+            c["curvature"] = rng.uniform(0, 25, n).astype(np.float32)
+            for f in ("nx", "ny", "nz"):
+                c[f] = rng.uniform(-1, 1, n).astype(np.float32)
+        bad = rng.choice(n, 40, replace=False)
+        c["x"][bad[:15]] = np.nan; c["y"][bad[15:30]] = np.inf; c["z"][bad[30:]] = -np.inf
+        check_voxelgrid(vb, oracle.voxelgrid(c, leaf), c, leaf)
+        check_voxelgrid(vb, oracle.voxelgrid(c[bad], leaf), c[bad], leaf)                        # no finite point: nothing out
+    for dt in (oracle.PT48, oracle.PT32):
+        one = np.zeros(1, dt); one["x"] = 1.5; one["intensity"] = 3
+        assert len(check_voxelgrid(vb, oracle.voxelgrid(one, 0.4), one, 0.4)) == 1
+        assert len(check_voxelgrid(vb, oracle.voxelgrid(one[:0], 0.4), one[:0], 0.4)) == 0
+
+
+def cloud_of_voxels(dt, counts, leaf, rng):
+    """len(counts) voxels with counts[k] members each, in a shuffled input order; members well inside their voxel, voxel k is
+    output k"""
+    cells = np.array([[3 * k - 11, (k * 5) % 4, 2 * k - 3] for k in range(len(counts))], np.float64)
+    member = np.repeat(np.arange(len(counts)), counts)
+    pos = (cells[member] + rng.uniform(0.1, 0.9, (len(member), 3))) * leaf
+    c = np.zeros(len(member), dt)
+    c["x"], c["y"], c["z"] = pos.astype(np.float32).T
+    c["intensity"] = rng.uniform(0, 100, len(c)).astype(np.float32)
+    if "nx" in dt.names:
+        c["curvature"] = rng.uniform(0, 10, len(c)).astype(np.float32)
+        for f in ("nx", "ny", "nz"):
+            c[f] = rng.uniform(-1, 1, len(c)).astype(np.float32)
+    perm = rng.permutation(len(c))
+    return c[perm], member[perm]
+
+
+@pytest.mark.parametrize("leaf", LEAVES)
+def test_walk_across_batches_of_eight(vb, oracle, leaf):
+    """voxels of 1, 7, 8, 9, 16, 17 and 300 members: the walk fetches 8 entries at a time and stops inside or at a batch's end"""
+    counts = (1, 7, 8, 9, 16, 17, 300)
+    rng = np.random.default_rng(int(leaf * 10) + 3)
+    for dt in (oracle.PT48, oracle.PT32):
+        c, _ = cloud_of_voxels(dt, counts, leaf, rng)
+        assert len(check_voxelgrid(vb, oracle.voxelgrid(c, leaf), c, leaf)) == len(counts)
+
+
+def test_normals_summing_to_zero_stay_zero(vb, oracle):
+    """pcl::CentroidPoint normalises the normal sum only when its squared norm is > 0: a zero sum is written as it is"""
+    rng = np.random.default_rng(5)
+    counts = (2, 4, 10, 3, 16)
+    c, member = cloud_of_voxels(oracle.PT48, counts, 0.4, rng)
+    for k in (0, 1, 2, 4):                          # members in pairs n, -n (in input order): the fp32 sum is exactly zero
+        idx = np.flatnonzero(member == k)
+        for a, b in zip(idx[0::2], idx[1::2]):
+            for f in ("nx", "ny", "nz"):
+                c[f][b] = -c[f][a]
+    c["nx"][member == 4] = c["ny"][member == 4] = c["nz"][member == 4] = 0.0
+    got = check_voxelgrid(vb, oracle.voxelgrid(c, 0.4), c, 0.4)
+    n = np.stack([got["nx"], got["ny"], got["nz"]], 1)
+    assert (n[[0, 1, 2, 4]] == 0).all()
+    np.testing.assert_allclose(np.linalg.norm(n[3]), 1.0, rtol=1e-6)
+
+
+@pytest.mark.parametrize("leaf", LEAVES)
+def test_per_ring_batch_matches_oracle_ring_by_ring(vb, oracle, world_small, leaf):
+    """the ROT extractor's batch: ring << 32 | voxel index keys over all rings at once = the oracle's VoxelGrid of every ring's
+    points, rings in ascending order; one ring in PCL's overflow case keeps its points, one point per voxel"""
+    rng = np.random.default_rng(int(leaf * 10) + 7)
+    pts = world_small["hdl"]
+    pts = pts[np.isfinite(pts["x"]) & np.isfinite(pts["y"]) & np.isfinite(pts["z"])][::3]
+    ring = rng.integers(0, 64, len(pts)).astype(np.int32)
+    far = np.zeros(5, pts.dtype)
+    far["x"], far["y"], far["z"] = ([-5000.0, 5000.0, 0.0, 1.0, 2.5], [-5000.0, 5000.0, 3.0, 1.0, 0.5], [-5000.0, 5000.0, -1.0, 2.0, 0.0])
+    far["w"] = 1.0
+    far["intensity"] = [1.0, 2.0, 3.0, 4.0, 5.0]
+    pts = np.concatenate([pts, far])
+    ring = np.concatenate([ring, np.full(5, 64, np.int32)])
+    want = np.concatenate([oracle.voxelgrid(pts[ring == r], leaf) for r in range(65)])
+    got = check_voxelgrid(vb, want, pts, leaf, ring)
+    assert np.array_equal(got[-5:], far)
