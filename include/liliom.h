@@ -280,6 +280,24 @@ int liliom_backend_window_corr(liliom_ctx* c, int slot, int kind, unsigned char*
  * transformed by poses7[i], concatenated, VoxelGrid(leaf), downloaded (out = NULL: *n only).  The result feeds liliom_icp_align. */
 int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, float leaf, void* out, int cap, int* n);
 
+/* downSampleCloud, full-cloud half (L:1494-1500, R:1373-1376): attach the keyframe's /full_point_cloud (body frame,
+ * point_stride bytes per point) to keyframe kf_id.  variant 0 stores it as received (full_clouds); variant 1 stores
+ * VoxelGrid(surf_leaf) of it (full_clouds_ds).  Once per keyframe (a second call: LILIOM_E_ARG, nothing changes).
+ * *n_stored (optional) = points stored.  The full clouds have a device arena of their own (geometric growth, copying). */
+int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp, int kf_id, const void* full, int n, int* n_stored);
+
+enum { LILIOM_KF_FULL = 0, LILIOM_KF_SURF = 1 };
+/* publishCompleteMap (L:2644-2685, R:2409-2447) / the save_pcd map of mapVisualizationThread (L:2703-2718, R:2463-2477).
+ * For each listed keyframe, in list order: its stored cloud of `kind`, transformed by pre7 (optional, NULL = skip; the
+ * intermediate cloud rounded to fp32 as PCL stores it) and then by poses7[i]; all of them concatenated; VoxelGrid(leaf).
+ * The caller selects the keyframes (every mapping_interval-th, the > 10 gate of :2646) and composes the poses
+ * (q_po*q_bl, q_po*t_bl + t_po, :2659-2660); stateless, like liliom_bmap_build.  PCL's index overflow: the output is the
+ * transformed concatenation itself, as PCL publishes it.  out = NULL: *n only.  Listed points >= 2^31: LILIOM_E_CAPACITY.
+ * A listed keyframe without a full cloud (kind FULL) or an unknown id: LILIOM_E_ARG, nothing changes.
+ * The filter reads the stored clouds where they lie (no concatenation buffer outside PCL's declined case). */
+int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, const double* poses7, int k, const double pre7[7],
+                      float leaf, void* out, int cap, int* n);
+
 /* ---- SURVEY §8 (f3): wire format on the sensor side — FormatConvert's livoxLidarHandler on the device ----
  * L/src/FormatConvert.cpp:11-24: livox_ros_driver::CustomPoint {uint32 offset_time; float x,y,z; uint8 reflectivity,
  * tag, line} -> pcl::PointXYZINormal with intensity = line + 0.1*float(offset_time/(float)time_end) (:19-20),

@@ -27,6 +27,7 @@ assert PT48.itemsize == 48 and PT32.itemsize == 32 and LIVOX20.itemsize == 20
 
 OK, E_ARG, E_CUDA, E_FEWMAP, E_CAPACITY, E_GRID, E_LINES, E_NCCL, E_NOMAP = 0, -1, -2, -3, -4, -5, -6, -7, -8
 MODE_CERES, MODE_GN = 0, 1
+KF_FULL, KF_SURF = 0, 1      # liliom_global_map: which stored cloud of each keyframe
 
 
 class Params(C.Structure):
@@ -72,7 +73,7 @@ EXPORTS = [
     "liliom_comm_peer_epoch", "liliom_comm_peer_set_epoch",
     "liliom_backend_default_params", "liliom_kf_add", "liliom_kf_count", "liliom_kf_clear", "liliom_bmap_build",
     "liliom_bmap_download", "liliom_backend_window_correspond", "liliom_backend_window_blocks", "liliom_backend_window_corr",
-    "liliom_kf_cloud",
+    "liliom_kf_cloud", "liliom_kf_add_full", "liliom_global_map",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -176,6 +177,8 @@ def lib() -> C.CDLL:
     L.liliom_backend_window_blocks.argtypes = [vp, dp, C.c_int, dp]
     L.liliom_backend_window_corr.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, ip]
     L.liliom_kf_cloud.argtypes = [vp, ip, dp, C.c_int, C.c_float, vp, C.c_int, ip]
+    L.liliom_kf_add_full.argtypes = [vp, bpp, C.c_int, vp, C.c_int, ip]
+    L.liliom_global_map.argtypes = [vp, C.c_int, ip, dp, C.c_int, dp, C.c_float, vp, C.c_int, ip]
     L.liliom_pre_create.argtypes = [vp, C.c_int, dp]; L.liliom_pre_create.restype = vp
     L.liliom_pre_destroy.argtypes = [vp]; L.liliom_pre_destroy.restype = None
     L.liliom_pre_imu.argtypes = [vp, C.c_double, dp]; L.liliom_pre_imu.restype = None
@@ -553,6 +556,28 @@ class Context:
         self._check(lib().liliom_kf_cloud(self._h, ids.ctypes.data_as(ipp), _dptr(p), len(ids), leaf, None, 0, C.byref(n)))
         out = np.zeros(max(n.value, 1), self.dtype)
         self._check(lib().liliom_kf_cloud(self._h, ids.ctypes.data_as(ipp), _dptr(p), len(ids), leaf, _ptr(out), len(out), C.byref(n)))
+        return out[:n.value]
+
+    def kf_add_full(self, bp: BackendParams, kf_id: int, full: np.ndarray) -> int:
+        """downSampleCloud (full-cloud half): attach keyframe kf_id's full body-frame cloud, stored as received (variant 0) or
+        VoxelGrid(surf_leaf) of it (variant 1).  Returns the points stored."""
+        f = np.ascontiguousarray(full, dtype=self.dtype)
+        m = C.c_int()
+        self._check(lib().liliom_kf_add_full(self._h, C.byref(bp), int(kf_id), _ptr(f), len(f), C.byref(m)))
+        return m.value
+
+    def global_map(self, kind: int, kf_ids, poses7, leaf: float, pre7=None) -> np.ndarray:
+        """publishCompleteMap / save_pcd's map: the stored cloud of `kind` (KF_FULL or KF_SURF) of every listed keyframe,
+        transformed by pre7 (optional) and then by its pose, concatenated, VoxelGrid(leaf); the transformed concatenation itself
+        when PCL declines the filter (index overflow)."""
+        ids = _ids(kf_ids); p = _poses(poses7, len(ids))
+        pre = None if pre7 is None else np.ascontiguousarray(pre7, dtype=np.float64).reshape(7)
+        ipp = C.POINTER(C.c_int)
+        args = (self._h, int(kind), ids.ctypes.data_as(ipp), _dptr(p), len(ids), None if pre is None else _dptr(pre), leaf)
+        n = C.c_int()
+        self._check(lib().liliom_global_map(*args, None, 0, C.byref(n)))
+        out = np.zeros(max(n.value, 1), self.dtype)
+        self._check(lib().liliom_global_map(*args, _ptr(out), len(out), C.byref(n)))
         return out[:n.value]
 
     # ---- wire formats (f3) ----

@@ -58,8 +58,14 @@ inline float gate_cell(double sqgate) {
     return cell;
 }
 
-// Keyframe store (keyframes.cu): body-frame clouds of every keyframe in one device arena, edge then surf per keyframe.
-struct KfEntry { long long edge_off, surf_off; int n_edge, n_surf; };   // offsets in points
+// Keyframe store (keyframes.cu): body-frame clouds of every keyframe in one device arena, edge then surf per keyframe; the full
+// clouds (liliom_kf_add_full) in an arena of their own.  Offsets in points; n_full < 0: no full cloud attached.
+struct KfEntry {
+    long long edge_off, surf_off;
+    int n_edge, n_surf;
+    long long full_off = 0;
+    int n_full = -1;
+};
 
 // Fused multi-GPU exchange (single node): pointers to every rank's exchange buffer (own entry = own buffer), see
 // peer_exchange() in grid_knn.cu.  Passed to the persistent GN kernel by value.
@@ -190,8 +196,10 @@ struct liliom_ctx {
     // ---- backend (keyframes.cu, backend_corr.cu): keyframe store, local map layers, window correspondences ----
     lili::DevBuf kf_arena;               // body-frame clouds of every keyframe (point_stride bytes per point)
     long long kf_used = 0;               // points in use
+    lili::DevBuf kf_full;                // full clouds of the keyframes (liliom_kf_add_full), point_stride bytes per point
+    long long kf_full_used = 0;          // points in use
     std::vector<lili::KfEntry> kfs;      // per keyframe: offsets and counts (host)
-    lili::DevBuf kf_tab;                 // per-call gather table (k_kf_gather)
+    lili::DevBuf kf_tab;                 // per-call keyframe table (kf_table.h: k_kf_gather, the global map's kernels)
     lili::MapIndex bmap[2];              // backend local map: [0] edge layer, [1] surf layer
     lili::DevBuf bmap_raw, bmap_ds[2];   // concatenation of the transformed keyframes; the filtered layers (all fields)
     int bmap_n[2] = {0, 0};

@@ -4,22 +4,71 @@
 //   local map        buildLocalMapWithLandMark (:1387-1484) + downSampleCloud, map half (:1486-1492): transform + concatenate
 //                    the listed keyframes in ONE launch, VoxelGrid per layer, a cell grid per layer (MapIndex)
 //   loop closure     detectLoopClosure's clouds (:2473-2547): edge then surf per keyframe, transformed, VoxelGrid
+//   full clouds      downSampleCloud, full-cloud half (:1494-1500; R:1373-1376): the /full_point_cloud of a keyframe, stored
+//   global map       publishCompleteMap (:2644-2685) and save_pcd's map (:2703-2718): listed keyframes transformed, concatenated,
+//                    VoxelGrid, in a VoxelGrid that reads the store through the keyframe table (kf_table.h): no concatenation
 // The deque policy of the local map (:1407-1477) stays with the caller: every call lists the keyframes and the poses to use.
 // Compiled with --fmad=false (the VoxelGrid centroids and the transform are bit-exact with the reference's arithmetic).
 #include "ctx.cuh"
 #include "dev_math.cuh"
+#include "kf_table.h"
 
 namespace lili {
 
-// One row of the gather table: n points of the arena at src_off, transformed by (q, t), written at dst_off of the output.
-struct GatherEnt { long long src_off, dst_off; Q4 q; D3 t; int n, pad; };
+// The table kernels: blockIdx.y walks the rows (grid-strided past 65535 rows), the blocks of a row stream through its points.
+// The table lives in device memory, so one launch serves any number of keyframes (the odometry map's ConcatTab holds 64).
+static dim3 kf_row_grid(size_t rows, long long largest, int bx_max, int by_max = 65535) {
+    return dim3(std::max(1, std::min(cdiv(largest, 256), bx_max)), (unsigned)std::min<size_t>(rows, by_max));
+}
 
-// blockIdx.y = table row; the blocks of a row stream through that row's points.  The table lives in device memory, so one
-// launch serves any number of keyframes (the odometry map's ConcatTab parameter holds 64).
-__global__ void k_kf_gather(const unsigned char* __restrict__ arena, const GatherEnt* __restrict__ tab, int stride, unsigned char* __restrict__ out) {
-    const GatherEnt& e = tab[blockIdx.y];
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < e.n; i += gridDim.x * blockDim.x)
-        pcl_transform_point(arena + (size_t)(e.src_off + i) * stride, stride, e.q, e.t, out + (size_t)(e.dst_off + i) * stride);
+// the transformed concatenation of the rows
+__global__ void k_kf_gather(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride,
+                            unsigned char* __restrict__ out) {
+    for (int y = blockIdx.y; y < rows; y += gridDim.y) {
+        const KfRow& r = tab[y];
+        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < r.n; i += gridDim.x * blockDim.x)
+            kf_row_point(r, arena + (size_t)(r.src_off + i) * stride, stride, out + (size_t)(r.dst_off + i) * stride);
+    }
+}
+
+// box (vg_box.h) of the finite transformed points of the rows, joined into mm
+__global__ void k_kf_box(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride, int* __restrict__ mm) {
+    int box[kBoxInts];
+#pragma unroll
+    for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_empty(k);
+    for (int y = blockIdx.y; y < rows; y += gridDim.y) {
+        const KfRow& r = tab[y];
+        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < r.n; i += gridDim.x * blockDim.x) {
+            const VgXyz p = kf_row_xyz(r, arena + (size_t)(r.src_off + i) * stride);
+            if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) vg_box_add(box, p.x, p.y, p.z);
+        }
+    }
+    vg_box_commit(box, mm);
+}
+
+// PCL's relative voxel index of every transformed point (all-ones: not finite), value = its index in the concatenation
+__global__ void k_kf_keys(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride, const VgParams p,
+                          uint32_t* __restrict__ keys, int* __restrict__ vals) {
+    for (int y = blockIdx.y; y < rows; y += gridDim.y) {
+        const KfRow& r = tab[y];
+        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < r.n; i += gridDim.x * blockDim.x) {
+            const VgXyz x = kf_row_xyz(r, arena + (size_t)(r.src_off + i) * stride);
+            const long long d = r.dst_off + i;
+            keys[d] = (isfinite(x.x) && isfinite(x.y) && isfinite(x.z)) ? vg_rel_index(p, x.x, x.y, x.z) : 0xffffffffu;
+            vals[d] = (int)d;
+        }
+    }
+}
+
+// centroid of every voxel of the sorted keys (the first n_fin entries are the finite points), members transformed on load
+template <int STRIDE>
+__global__ void k_kf_centroid(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, const uint32_t* __restrict__ keys,
+                              const int* __restrict__ vals, const int* __restrict__ flags, const int* __restrict__ rank, int n_fin,
+                              unsigned char* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_fin || !flags[i]) return;
+    const VgAcc<STRIDE> a = vg_walk<STRIDE>(keys, i, n_fin, [&](int j) { return vals[j]; }, KfRowLoader<STRIDE>{arena, tab, rows});
+    vg_write<STRIDE>(a.s, a.n, out + (size_t)rank[i] * STRIDE);
 }
 
 // reflectivity (curvature = 0.1 * reflectivity, L/src/FormatConvert.cpp:21) of 48-byte points
@@ -29,28 +78,30 @@ __global__ void k_kf_refl(const unsigned char* __restrict__ pts, int n, float* _
 }
 
 void backend_release(liliom_ctx* c) {
-    DevBuf* bufs[] = {&c->kf_arena, &c->kf_tab, &c->bmap_raw, &c->bmap_ds[0], &c->bmap_ds[1], &c->win_valid[0], &c->win_valid[1],
+    DevBuf* bufs[] = {&c->kf_arena, &c->kf_full, &c->kf_tab, &c->bmap_raw, &c->bmap_ds[0], &c->bmap_ds[1], &c->win_valid[0], &c->win_valid[1],
                       &c->win_line, &c->win_plane, &c->win_score, &c->win_cnt, &c->win_tab};
     for (DevBuf* b : bufs) b->release();
     c->bmap[0].release(); c->bmap[1].release();
 }
 
-// Room for `pts` points in the arena.  Grows geometrically and COPIES the stored keyframes (DevBuf::ensure would discard them);
-// the cudaFree of the old block synchronises, which only happens on growth.
-static int kf_reserve(liliom_ctx* c, long long pts) {
+// Room for `pts` points in `arena`, of which the first `used` are stored.  Grows geometrically and COPIES the stored points
+// (DevBuf::ensure would discard them); the cudaFree of the old block synchronises, which only happens on growth.
+// The store has two arenas: kf_arena (the down-sampled edge/surf clouds, ~2k points per keyframe) and kf_full (the full clouds,
+// ~20k points per keyframe, GBs over a long run).  One arena would recopy every full cloud each time the small clouds grow it.
+static int kf_reserve(liliom_ctx* c, DevBuf& arena, long long used, long long pts) {
     const size_t stride = (size_t)c->prm.point_stride;
     const size_t need = (size_t)pts * stride;
-    if (need <= c->kf_arena.cap) return LILIOM_OK;
-    size_t want = std::max(need + need / 2, std::max(c->kf_arena.cap * 2, (size_t)1 << 20));
+    if (need <= arena.cap) return LILIOM_OK;
+    size_t want = std::max(need + need / 2, std::max(arena.cap * 2, (size_t)1 << 20));
     void* p = nullptr;
     LILI_CUDA(c, cudaMalloc(&p, want));
-    if (c->kf_used > 0) {
-        const cudaError_t e = cudaMemcpyAsync(p, c->kf_arena.p, (size_t)c->kf_used * stride, cudaMemcpyDeviceToDevice, c->stream);
+    if (used > 0) {
+        const cudaError_t e = cudaMemcpyAsync(p, arena.p, (size_t)used * stride, cudaMemcpyDeviceToDevice, c->stream);
         if (e != cudaSuccess) { cudaFree(p); return fail_cuda(c, e, "kf_reserve copy"); }
         LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     }
-    c->kf_arena.release();
-    c->kf_arena.p = p; c->kf_arena.cap = want;
+    arena.release();
+    arena.p = p; arena.cap = want;
     return LILIOM_OK;
 }
 
@@ -65,22 +116,32 @@ static bool kf_ids_ok(liliom_ctx* c, const int* ids, int k) {
     return true;
 }
 
-// Transform + concatenate rows of the store into `out` (one launch).  rows: {keyframe list index, layer 0 edge / 1 surf}.
-static int kf_gather(liliom_ctx* c, const std::vector<GatherEnt>& tab, long long largest, void* out) {
+static int kf_upload_table(liliom_ctx* c, const std::vector<KfRow>& tab) {
+    LILI_CUDA(c, c->kf_tab.ensure(tab.size() * sizeof(KfRow)));
+    LILI_CUDA(c, cudaMemcpyAsync(c->kf_tab.p, tab.data(), tab.size() * sizeof(KfRow), cudaMemcpyHostToDevice, c->stream));
+    return LILIOM_OK;
+}
+
+// Transform + concatenate rows of `arena` into `out` (one launch).
+static int kf_gather(liliom_ctx* c, const void* arena, const std::vector<KfRow>& tab, long long largest, void* out) {
     if (tab.empty() || largest <= 0) return LILIOM_OK;
-    LILI_CUDA(c, c->kf_tab.ensure(tab.size() * sizeof(GatherEnt)));
-    LILI_CUDA(c, cudaMemcpyAsync(c->kf_tab.p, tab.data(), tab.size() * sizeof(GatherEnt), cudaMemcpyHostToDevice, c->stream));
-    const int bx = std::max(1, std::min(cdiv(largest, 256), c->sm_count * 4));
-    k_kf_gather<<<dim3(bx, (unsigned)tab.size()), 256, 0, c->stream>>>((const unsigned char*)c->kf_arena.p, c->kf_tab.as<GatherEnt>(),
-                                                                      c->prm.point_stride, (unsigned char*)out);
+    LILI_TRY(kf_upload_table(c, tab));
+    k_kf_gather<<<kf_row_grid(tab.size(), largest, c->sm_count * 4), 256, 0, c->stream>>>(
+        (const unsigned char*)arena, c->kf_tab.as<KfRow>(), (int)tab.size(), c->prm.point_stride, (unsigned char*)out);
     return launch_check(c, "k_kf_gather");
 }
 
-static GatherEnt gather_row(long long src, long long dst, int n, const double* pose7) {
-    GatherEnt e{};
+// a table row: n points from src -> dst, transformed by pre7 (optional) and then by pose7
+static KfRow kf_row(long long src, long long dst, int n, const double* pose7, const double* pre7 = nullptr) {
+    KfRow e{};
     e.src_off = src; e.dst_off = dst; e.n = n;
     e.q = Q4{pose7[0], pose7[1], pose7[2], pose7[3]};
     e.t = D3{pose7[4], pose7[5], pose7[6]};
+    if (pre7) {
+        e.pre = 1;
+        e.pq = Q4{pre7[0], pre7[1], pre7[2], pre7[3]};
+        e.pt = D3{pre7[4], pre7[5], pre7[6]};
+    }
     return e;
 }
 
@@ -123,7 +184,7 @@ extern "C" int liliom_kf_add(liliom_ctx* c, const liliom_backend_params* bp, con
     LILI_CUDA(c, cudaSetDevice(c->device));
     const int stride = c->prm.point_stride;
     const long long n = (long long)n_edge + n_surf;
-    LILI_TRY(kf_reserve(c, c->kf_used + n));          // VoxelGrid never outputs more points than it reads
+    LILI_TRY(kf_reserve(c, c->kf_arena, c->kf_used, c->kf_used + n));          // VoxelGrid never outputs more points than it reads
     LILI_CUDA(c, c->raw.ensure((size_t)(n > 0 ? n : 1) * stride));
     LILI_CUDA(c, c->vg_out.ensure((size_t)(n_surf > 0 ? n_surf : 1) * stride));
     LILI_CUDA(c, c->vg_count.ensure(16));
@@ -155,7 +216,8 @@ extern "C" int liliom_kf_count(const liliom_ctx* c) { return c ? (int)c->kfs.siz
 extern "C" int liliom_kf_clear(liliom_ctx* c) {
     if (!c) return LILIOM_E_ARG;
     c->kfs.clear();
-    c->kf_used = 0;                      // the arena keeps its allocation
+    c->kf_used = 0;                      // the arenas keep their allocations
+    c->kf_full_used = 0;
     c->bmap_built = false; c->bmap_n[0] = c->bmap_n[1] = 0;
     c->bmap[0].ready = c->bmap[1].ready = false;
     c->win_k = 0;
@@ -172,17 +234,17 @@ extern "C" int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp,
     c->bmap_built = false;
     long long E = 0, S = 0, largest = 0;
     for (int i = 0; i < k; ++i) { const KfEntry& f = c->kfs[kf_ids[i]]; E += f.n_edge; S += f.n_surf; largest = std::max(largest, (long long)std::max(f.n_edge, f.n_surf)); }
-    std::vector<GatherEnt> tab;
+    std::vector<KfRow> tab;
     tab.reserve(2 * (size_t)k);
     long long de = 0, ds = E;
     for (int i = 0; i < k; ++i) {                                 // :1479-1483 edge and surf layers, list order
         const KfEntry& f = c->kfs[kf_ids[i]];
-        if (f.n_edge) tab.push_back(gather_row(f.edge_off, de, f.n_edge, poses7 + 7 * (size_t)i));
-        if (f.n_surf) tab.push_back(gather_row(f.surf_off, ds, f.n_surf, poses7 + 7 * (size_t)i));
+        if (f.n_edge) tab.push_back(kf_row(f.edge_off, de, f.n_edge, poses7 + 7 * (size_t)i));
+        if (f.n_surf) tab.push_back(kf_row(f.surf_off, ds, f.n_surf, poses7 + 7 * (size_t)i));
         de += f.n_edge; ds += f.n_surf;
     }
     LILI_CUDA(c, c->bmap_raw.ensure((size_t)std::max(E + S, 1LL) * stride));
-    LILI_TRY(kf_gather(c, tab, largest, c->bmap_raw.p));
+    LILI_TRY(kf_gather(c, c->kf_arena.p, tab, largest, c->bmap_raw.p));
     const long long nl[2] = {E, S};
     const float leaf[2] = {bp->edge_leaf, bp->surf_leaf};
     const unsigned char* src[2] = {(const unsigned char*)c->bmap_raw.p, (const unsigned char*)c->bmap_raw.p + (size_t)E * stride};
@@ -233,13 +295,13 @@ extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* p
     LILI_CUDA(c, cudaSetDevice(c->device));
     const int stride = c->prm.point_stride;
     *n_out = 0;
-    std::vector<GatherEnt> tab;
+    std::vector<KfRow> tab;
     long long off = 0, largest = 0;
     for (int i = 0; i < k; ++i) {                                 // :2492-2493 / :2519-2520: *edge_frames[i] then *surf_frames[i]
         const KfEntry& f = c->kfs[kf_ids[i]];
-        if (f.n_edge) tab.push_back(gather_row(f.edge_off, off, f.n_edge, poses7 + 7 * (size_t)i));
+        if (f.n_edge) tab.push_back(kf_row(f.edge_off, off, f.n_edge, poses7 + 7 * (size_t)i));
         off += f.n_edge;
-        if (f.n_surf) tab.push_back(gather_row(f.surf_off, off, f.n_surf, poses7 + 7 * (size_t)i));
+        if (f.n_surf) tab.push_back(kf_row(f.surf_off, off, f.n_surf, poses7 + 7 * (size_t)i));
         off += f.n_surf;
         largest = std::max(largest, (long long)std::max(f.n_edge, f.n_surf));
     }
@@ -247,7 +309,7 @@ extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* p
     LILI_CUDA(c, c->bmap_raw.ensure((size_t)off * stride));      // scratch: the local map's layers live in bmap_ds / bmap
     LILI_CUDA(c, c->vg_out.ensure((size_t)off * stride));
     LILI_CUDA(c, c->vg_count.ensure(16));
-    LILI_TRY(kf_gather(c, tab, largest, c->bmap_raw.p));
+    LILI_TRY(kf_gather(c, c->kf_arena.p, tab, largest, c->bmap_raw.p));
     LILI_TRY(voxelgrid_dev(c, c->bmap_raw.p, (int)off, nullptr, stride, leaf, c->vg_out.p, c->vg_count.as<int>()));
     LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
@@ -256,6 +318,132 @@ extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* p
     if (!out) return LILIOM_OK;
     if (m > cap) return LILIOM_E_CAPACITY;
     if (m) LILI_CUDA(c, cudaMemcpyAsync(out, c->vg_out.p, (size_t)m * stride, cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    return LILIOM_OK;
+}
+
+extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp, int kf_id, const void* full, int n, int* n_stored) {
+    if (!c || !bp || n < 0 || (n > 0 && !full)) return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, bp));
+    if (!kf_ids_ok(c, &kf_id, 1)) return LILIOM_E_ARG;
+    if (c->kfs[kf_id].n_full >= 0) {
+        c->last_error = "keyframe " + std::to_string(kf_id) + " already has its full cloud";
+        return LILIOM_E_ARG;
+    }
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    const int stride = c->prm.point_stride;
+    LILI_TRY(kf_reserve(c, c->kf_full, c->kf_full_used, c->kf_full_used + n));     // VoxelGrid never outputs more points than it reads
+    unsigned char* tail = (unsigned char*)c->kf_full.p + (size_t)c->kf_full_used * stride;
+    int m = n;
+    if (n > 0 && bp->variant == 0) {                              // L:1498-1500 full_clouds: the cloud as received
+        LILI_CUDA(c, cudaMemcpyAsync(tail, full, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
+        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    } else if (n > 0) {                                           // R:1373-1376 full_clouds_ds: VoxelGrid(surf_leaf) of it
+        LILI_CUDA(c, c->raw.ensure((size_t)n * stride));
+        LILI_CUDA(c, c->vg_count.ensure(16));
+        LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, full, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
+        LILI_TRY(voxelgrid_dev(c, c->raw.p, n, nullptr, stride, bp->surf_leaf, tail, c->vg_count.as<int>()));
+        LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+        m = c->h_pin->bk_cnt[0];
+    }
+    c->kfs[kf_id].full_off = c->kf_full_used;
+    c->kfs[kf_id].n_full = m;
+    c->kf_full_used += m;
+    if (n_stored) *n_stored = m;
+    return LILIOM_OK;
+}
+
+// The global map without a concatenation buffer: box, voxel keys and centroids read the stored clouds through the keyframe table
+// and transform every point on load (kf_table.h); the sort chain in between is voxelgrid_dev's (sort_pairs_u32 at the key width of
+// the box, k_vg_heads, the scan).  Device memory: the table, 16 bytes per listed point for keys and values (sort included), and
+// the output; only PCL's declined case writes the transformed concatenation, which is then the output.
+extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, const double* poses7, int k, const double pre7[7],
+                                 float leaf, void* out, int cap, int* n) {
+    if (!c || !n || k < 0 || (k > 0 && (!kf_ids || !poses7)) || (kind != LILIOM_KF_FULL && kind != LILIOM_KF_SURF) || !(leaf > 0))
+        return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, nullptr));
+    if (!kf_ids_ok(c, kf_ids, k)) return LILIOM_E_ARG;
+    for (int i = 0; i < k && kind == LILIOM_KF_FULL; ++i)
+        if (c->kfs[kf_ids[i]].n_full < 0) {
+            c->last_error = "keyframe " + std::to_string(kf_ids[i]) + " has no full cloud (liliom_kf_add_full)";
+            return LILIOM_E_ARG;
+        }
+    const int stride = c->prm.point_stride;
+    std::vector<KfRow> tab;
+    long long N = 0, largest = 0;
+    for (int i = 0; i < k; ++i) {                                 // :2652-2662 list order, one cloud per keyframe
+        const KfEntry& f = c->kfs[kf_ids[i]];
+        const long long off = kind == LILIOM_KF_FULL ? f.full_off : f.surf_off;
+        const int m = kind == LILIOM_KF_FULL ? f.n_full : f.n_surf;
+        if (m) tab.push_back(kf_row(off, N, m, poses7 + 7 * (size_t)i, pre7));
+        N += m;
+        largest = std::max(largest, (long long)m);
+    }
+    if (N >= (1LL << 31)) {                                       // the sort chain's values and PCL's indices are ints
+        c->last_error = "the listed keyframes hold " + std::to_string(N) + " points (at most 2^31 - 1)";
+        return LILIOM_E_CAPACITY;
+    }
+    if (N == 0) { *n = 0; return LILIOM_OK; }
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    const unsigned char* arena = (const unsigned char*)(kind == LILIOM_KF_FULL ? c->kf_full.p : c->kf_arena.p);
+    const int rows = (int)tab.size();
+    LILI_TRY(kf_upload_table(c, tab));
+    const KfRow* d_tab = c->kf_tab.as<KfRow>();
+    // box of the transformed concatenation (pcl::getMinMax3D), read back: the overflow test and the key width are decided here
+    LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
+    int* mm = c->vg_minmax.as<int>();
+    for (int w = 0; w < kBoxInts; ++w) c->h_pin->box[w] = vg_box_empty(w);
+    LILI_CUDA(c, cudaMemcpyAsync(mm, c->h_pin->box, kBoxInts * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    k_kf_box<<<kf_row_grid(tab.size(), largest, 8, 1024), 256, 0, c->stream>>>(arena, d_tab, rows, stride, mm);
+    LILI_TRY(launch_check(c, "k_kf_box"));
+    LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->box, mm, kBoxInts * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    int box[kBoxInts];
+    memcpy(box, c->h_pin->box, sizeof(box));
+    const VgParams p = vg_params(box, leaf);
+    if (p.overflow) {                                             // PCL declines the filter and publishes its input
+        if (!out) { *n = (int)N; return LILIOM_OK; }
+        if (N > cap) { *n = (int)N; return LILIOM_E_CAPACITY; }
+        LILI_CUDA(c, c->vg_out.ensure((size_t)N * stride));
+        LILI_TRY(kf_gather(c, arena, tab, largest, c->vg_out.p));
+        LILI_CUDA(c, cudaMemcpyAsync(out, c->vg_out.p, (size_t)N * stride, cudaMemcpyDeviceToHost, c->stream));
+        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+        *n = (int)N;
+        return LILIOM_OK;
+    }
+    const int n_fin = p.n_finite;
+    if (n_fin == 0) { *n = 0; return LILIOM_OK; }
+    LILI_CUDA(c, c->vg_keys.ensure((size_t)N * 4));
+    LILI_CUDA(c, c->vg_vals.ensure((size_t)N * 4));
+    LILI_CUDA(c, c->vg_keys2.ensure((size_t)N * 4));
+    LILI_CUDA(c, c->vg_vals2.ensure((size_t)N * 4));
+    LILI_CUDA(c, c->vg_flags.ensure(((size_t)n_fin + 2) * 4));
+    LILI_CUDA(c, c->vg_rank.ensure(((size_t)n_fin + 2) * 4));
+    k_kf_keys<<<kf_row_grid(tab.size(), largest, 8), 256, 0, c->stream>>>(arena, d_tab, rows, stride, p, c->vg_keys.as<uint32_t>(),
+                                                                             c->vg_vals.as<int>());
+    LILI_TRY(launch_check(c, "k_kf_keys"));
+    // non-finite points carry the all-ones key and sort last: the first n_fin sorted entries are the finite points
+    LILI_TRY(sort_pairs_u32(c, c->vg_keys.as<uint32_t>(), c->vg_keys2.as<uint32_t>(), c->vg_vals.as<int>(), c->vg_vals2.as<int>(), (int)N,
+                            vg_key_bits(box, leaf)));
+    k_vg_heads<<<cdiv(n_fin + 1LL, 256), 256, 0, c->stream>>>(c->vg_keys2.as<uint32_t>(), n_fin, nullptr, c->vg_flags.as<int>());
+    LILI_TRY(launch_check(c, "k_vg_heads"));
+    LILI_TRY(exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin));
+    LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, c->vg_rank.as<int>() + n_fin, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    const int m = c->h_pin->bk_cnt[0];
+    *n = m;
+    if (!out) return LILIOM_OK;
+    if (m > cap) return LILIOM_E_CAPACITY;
+    LILI_CUDA(c, c->vg_out.ensure((size_t)m * stride));
+    if (stride == 48)
+        k_kf_centroid<48><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(),
+                                                                   c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
+    else
+        k_kf_centroid<32><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(),
+                                                                   c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
+    LILI_TRY(launch_check(c, "k_kf_centroid"));
+    LILI_CUDA(c, cudaMemcpyAsync(out, c->vg_out.p, (size_t)m * stride, cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     return LILIOM_OK;
 }

@@ -5,7 +5,8 @@
 //   * PCL's parameters derived from it and a point's voxel index;
 //   * a voxel's centroid: the fields summed, the walk over its members in a sorted entry array, and the output point.
 // The kernels that measure a box, index voxels or write centroids (the sort chain and k_vg_coop in voxelgrid.cu, the
-// incremental map in map_inc.cu, the per-ring filter in extract_rot.cu, the cell grid in grid_knn.cu) and the host code that
+// incremental map in map_inc.cu, the per-ring filter in extract_rot.cu, the cell grid in grid_knn.cu, the global map's table
+// filter in keyframes.cu) and the host code that
 // reads a box back use this file, so they agree on every voxel and every bit of a centroid.  Plain C++ usable from device
 // code and from the host (tests/vg_box_host.cpp compiles this same file for the CPU test tier).
 //
@@ -17,6 +18,7 @@
 #include <climits>
 #include <cmath>
 #include <cstring>
+#include <type_traits>
 
 #ifdef __CUDACC__
 #define VGB_HD __host__ __device__ __forceinline__
@@ -78,6 +80,29 @@ __device__ __forceinline__ void vg_box_atomic(int* dst, int k, int v) {      // 
     if (k < 3) atomicMin(dst, v);
     else if (k < 6) atomicMax(dst, v);
     else atomicAdd(dst, v);
+}
+// Every thread of a block (blockDim.x <= 256) joins its box into the box at mm: a warp reduction, then one set of atomics per
+// BLOCK.  (The seven words are single addresses, and one set per warp (9.5k warps) serialised into ~55 us at the L2 whatever
+// the input size: measured on a 500k-point frame, push 25 -> 83 us.)
+__device__ __forceinline__ void vg_box_commit(int* box, int* mm) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+        for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_join(k, box[k], __shfl_xor_sync(0xffffffffu, box[k], o));
+    }
+    __shared__ int s_box[kBoxInts][8];
+    const int w = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int k = 0; k < kBoxInts; ++k) s_box[k][w] = box[k];
+    }
+    __syncthreads();
+    if (threadIdx.x < kBoxInts) {
+        const int k = threadIdx.x, nw = (blockDim.x + 31) >> 5;
+        int v = vg_box_empty(k);
+        for (int j = 0; j < nw; ++j) v = vg_box_join(k, v, s_box[k][j]);
+        if (v != vg_box_empty(k)) vg_box_atomic(&mm[k], k, v);
+    }
 }
 #endif
 
@@ -182,11 +207,19 @@ struct VgAcc {
 template <typename K>
 VGB_HD bool vg_is_head(const K* keys, int i, int n_valid) { return i < n_valid && (i == 0 || keys[i] != keys[i - 1]); }
 
+// The fields of point m through a loader: either the plain loader load(m), the address of a stored point (read with vg_load),
+// or load(m, f), which writes the fields itself (a point transformed on load, kf_table.h).
+template <int STRIDE, typename Load>
+VGB_HD void vg_fetch(const Load& load, int m, float* f) {
+    if constexpr (std::is_invocable_v<const Load&, int, float*>) load(m, f);
+    else vg_load<STRIDE>(load(m), f);
+}
+
 // The sums of the voxel whose first sorted entry is `head`: entries j = head, head + 1, ... while j < n_valid and keys[j] is
-// keys[head], in entry order.  member(j) is the point of entry j (an int >= 0), point(m) that point's address.  Members are
-// fetched 8 at a time so that their loads overlap; the sums stay sequential.
-template <int STRIDE, typename K, typename Member, typename Point>
-VGB_HD VgAcc<STRIDE> vg_walk(const K* keys, int head, int n_valid, Member member, Point point) {
+// keys[head], in entry order.  member(j) is the point of entry j (an int >= 0), load the loader of its fields (vg_fetch).
+// Members are fetched 8 at a time so that their loads overlap; the sums stay sequential.
+template <int STRIDE, typename K, typename Member, typename Load>
+VGB_HD VgAcc<STRIDE> vg_walk(const K* keys, int head, int n_valid, Member member, Load load) {
     VgAcc<STRIDE> acc;
     const K key = keys[head];
     VGB_PRAGMA(unroll 1)
@@ -197,7 +230,7 @@ VGB_HD VgAcc<STRIDE> vg_walk(const K* keys, int head, int n_valid, Member member
         float f[8][kVgFields<STRIDE>];
         VGB_PRAGMA(unroll)
         for (int u = 0; u < 8; ++u)
-            if (m[u] >= 0) vg_load<STRIDE>(point(m[u]), f[u]);
+            if (m[u] >= 0) vg_fetch<STRIDE>(load, m[u], f[u]);
         VGB_PRAGMA(unroll)
         for (int u = 0; u < 8; ++u)
             if (m[u] >= 0) acc.add(f[u]);

@@ -28,26 +28,7 @@ __global__ void k_vg_minmax(const unsigned char* __restrict__ pts, int n_max, co
         if (!(isfinite(v.x) && isfinite(v.y) && isfinite(v.z))) continue;
         vg_box_add(box, v.x, v.y, v.z);
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-        for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_join(k, box[k], __shfl_xor_sync(0xffffffffu, box[k], o));
-    }
-    // one set of atomics per BLOCK: the seven words are single addresses, and one set per warp (9.5k warps) serialised into
-    // ~55 us at the L2 whatever the input size (measured on a 500k-point frame: push 25 -> 83 us)
-    __shared__ int s_box[kBoxInts][8];
-    const int w = threadIdx.x >> 5;
-    if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-        for (int k = 0; k < kBoxInts; ++k) s_box[k][w] = box[k];
-    }
-    __syncthreads();
-    if (threadIdx.x < kBoxInts) {
-        const int k = threadIdx.x, nw = (blockDim.x + 31) >> 5;
-        int v = vg_box_empty(k);
-        for (int j = 0; j < nw; ++j) v = vg_box_join(k, v, s_box[k][j]);
-        if (v != vg_box_empty(k)) vg_box_atomic(&mm[k], k, v);
-    }
+    vg_box_commit(box, mm);
 }
 
 struct VgBox { int mm[kBoxInts]; };      // a box (vg_box.h) by value

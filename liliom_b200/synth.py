@@ -237,13 +237,14 @@ def default_true_pose():
     return np.concatenate([q, [2.0, 3.0, 1.8]])
 
 
-def make_keyframe_sequence(n: int, stride: int = 48, seed: int = 7, step=1.5, yaw_deg=2.0, surf_every: int = 8):
+def make_keyframe_sequence(n: int, stride: int = 48, seed: int = 7, step=1.5, yaw_deg=2.0, surf_every: int = 8, full: bool = False):
     """A seeded keyframe stream for the backend (SURVEY.md §8 f5): n Horizon sweeps (no rotation inside a sweep, i.e. the
     clouds the backend receives after de-skew) taken every `step` metres along a gently turning path through the world.
     Each keyframe is split the way the extractors split a sweep: edge = returns from poles and wall tops (line-like
     neighbourhoods), surf = every `surf_every`-th other return.  Reflectivity (the `curvature` field, FormatConvert.cpp:21)
     is per surface kind plus a little noise, so the reflectivity-weighted plane fit of the Horizon backend sees real planes.
-    Returns a list of (edge, surf, pose7) with clouds in the body frame, PT48 (stride 48) or PT32 (stride 32)."""
+    Returns a list of (edge, surf, pose7) with clouds in the body frame, PT48 (stride 48) or PT32 (stride 32); full=True appends
+    each keyframe's whole sweep (the /full_point_cloud the edge and surf clouds were split from): (edge, surf, pose7, full)."""
     rng = np.random.default_rng(seed)
     T0 = default_true_pose()
     out = []
@@ -271,6 +272,6 @@ def make_keyframe_sequence(n: int, stride: int = 48, seed: int = 7, step=1.5, ya
                 for f in ("x", "y", "z", "w", "intensity"):
                     b[f] = a[f]
                 return b
-            edge, surf = to32(edge), to32(surf)
-        out.append((edge, surf, pose))
+            edge, surf, pts = to32(edge), to32(surf), to32(pts)
+        out.append((edge, surf, pose, pts) if full else (edge, surf, pose))
     return out

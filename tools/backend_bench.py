@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """The backend's LiDAR step (SURVEY.md §8 f5) on one GPU: device-resident keyframe store + local map + window calls, against the
 same step through the single-keyframe ABI and the 1-thread oracle composition.  Prints one JSON line.
-usage: backend_bench.py [--steps K] [--warmup W] [--dump-outputs DIR]
---dump-outputs DIR writes the last timed step's layers and blocks of the device-resident leg as DIR/<name>.npy."""
+usage: backend_bench.py [--steps K] [--warmup W] [--dump-outputs DIR] [--global-map [--gm-keyframes 300,2000]]
+--dump-outputs DIR writes the last timed step's layers and blocks of the device-resident leg as DIR/<name>.npy.
+--global-map runs the global-map leg instead (publishCompleteMap over the stored full clouds, one JSON line)."""
 from __future__ import annotations
 
 import argparse
@@ -43,12 +44,7 @@ def bench_backend(args):
     from liliom_b200 import synth
     if not torch.cuda.is_available():
         raise SystemExit("backend_bench.py needs a CUDA device (no CPU fallback)")
-    name = torch.cuda.get_device_name(0)
-    try:
-        plim = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
-                              text=True, timeout=20).stdout.strip()
-    except Exception as e:      # noqa: BLE001
-        plim = "unknown (" + type(e).__name__ + ")"
+    name, plim = gpu_card()
     bp = L.backend_default_params(0)
     pool = synth.make_keyframe_sequence(BK_MAP_WIDTH + 8, stride=48)
     steps, warmup = args.steps, args.warmup
@@ -202,12 +198,115 @@ def bench_backend(args):
         x.close()
 
 
+def gpu_card():
+    import torch
+    name = torch.cuda.get_device_name(0)
+    try:
+        plim = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit", "--format=csv,noheader"], capture_output=True,
+                              text=True, timeout=20).stdout.strip()
+    except Exception as e:      # noqa: BLE001
+        plim = "unknown (" + type(e).__name__ + ")"
+    return name, plim
+
+
+GM_LEAF = 0.3          # mapping_ds (L/src/BackendFusion.cpp:568)
+GM_SWEEPS = 24         # distinct full sweeps, reused cyclically along the path
+
+
+def bench_global_map(args):
+    """publishCompleteMap (L/src/BackendFusion.cpp:2644-2685) over a whole trajectory: every keyframe's full cloud (~20k points,
+    Horizon variant, stored as received) transformed by its pose, concatenated, VoxelGrid(mapping_ds = 0.3).  Per trajectory length:
+    (a) liliom_global_map on the full clouds kept in the device store (one call, output downloaded);
+    (b) what a host-side adapter does without it: host copies of the full clouds, transformed on one CPU thread (PCL's
+        transformPointCloud: the oracle's transform_cloud), concatenated in NumPy, then liliom_voxelgrid (upload, filter, download);
+    (c) the 1-thread oracle composition voxelgrid(concat(transform_cloud(...))).
+    The path is synth.make_keyframe_sequence's (1.5 m and 2 deg of yaw per keyframe); GM_SWEEPS generated sweeps are reused."""
+    import torch
+    import ctypes as C
+    import liliom_b200 as L
+    from liliom_b200 import synth
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import oracle_lib as O
+    if not torch.cuda.is_available():
+        raise SystemExit("backend_bench.py needs a CUDA device (no CPU fallback)")
+    name, plim = gpu_card()
+    sweeps = [kf[3] for kf in synth.make_keyframe_sequence(GM_SWEEPS, stride=48, full=True)]
+    T0 = synth.default_true_pose()
+    bp = L.backend_default_params(0)
+    lengths = [int(x) for x in args.gm_keyframes.split(",")]
+    steps = max(1, args.steps)
+    legs = []
+    for n_kf in lengths:
+        poses = []
+        for i in range(n_kf):
+            q = synth.qmul(synth.q_from_axis_angle([0, 0, 1], np.deg2rad(2.0 * i)), T0[:4])
+            poses.append(np.concatenate([q, T0[4:] + np.array([1.5 * i, 0.35 * np.sin(0.4 * i), 0.0])]))
+        clouds = [sweeps[i % GM_SWEEPS] for i in range(n_kf)]
+        n_in = int(sum(len(x) for x in clouds))
+        c = L.Context(variant=0)
+        empty = sweeps[0][:0]
+        for x in clouds:
+            kid, _, _ = c.kf_add(bp, empty, empty, download=False)
+            c.kf_add_full(bp, kid, x)
+        ids = np.arange(n_kf, dtype=np.int32)
+        p7 = np.ascontiguousarray(np.stack(poses))
+        out = np.zeros(n_in, L.PT48)
+        m = C.c_int()
+
+        def arm_a():
+            c._check(L._binding.lib().liliom_global_map(c._h, L.KF_FULL, ids.ctypes.data_as(C.POINTER(C.c_int)),
+                                                        p7.ctypes.data_as(C.POINTER(C.c_double)), n_kf, None, GM_LEAF,
+                                                        out.ctypes.data_as(C.c_void_p), len(out), C.byref(m)))
+            return out[:m.value]
+
+        def arm_b():
+            cat = np.concatenate([O.transform_cloud(x, p) for x, p in zip(clouds, poses)])
+            return c.voxelgrid(cat, GM_LEAF)
+
+        def arm_c():
+            return O.voxelgrid(np.concatenate([O.transform_cloud(x, p) for x, p in zip(clouds, poses)]), GM_LEAF)
+
+        def timed(fn, n):
+            fn()                                                  # warm-up (allocations)
+            ms, res = [], None
+            for _ in range(n):
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                res = fn()
+                ms.append((time.perf_counter() - t0) * 1e3)
+            return float(np.median(ms)), res
+
+        ms_a, got_a = timed(arm_a, steps)
+        ms_b, got_b = timed(arm_b, steps)
+        t0 = time.perf_counter()
+        got_c = arm_c()
+        ms_c = (time.perf_counter() - t0) * 1e3
+        same = got_a.tobytes() == got_b.tobytes() == got_c.tobytes()
+        legs.append({"keyframes": n_kf, "points_in": n_in, "bytes_in": n_in * 48, "points_out": int(len(got_a)),
+                     "pcl_declined": bool(len(got_a) == n_in), "outputs_bit_identical": bool(same),
+                     "a_global_map_median_ms": ms_a, "b_host_transform_concat_voxelgrid_median_ms": ms_b,
+                     "c_oracle_1_thread_ms": ms_c, "timed_runs_a_b": steps, "timed_runs_c": 1})
+        del out
+        c.close()
+    line = {"metric": "ms per publishCompleteMap over the whole trajectory (full clouds, VoxelGrid 0.3 m)", "workload": "backend_global_map",
+            "unit": "ms", "higher_is_better": False, "n_gpus": 1, "gpu": name, "power_limit": plim,
+            "data": f"synthetic: {GM_SWEEPS} synth.make_keyframe_sequence full sweeps reused along the path", "legs": legs,
+            "timing": "host wall clock around each call, output on the host; (b) includes the host transform and concatenation"}
+    print(json.dumps(line), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--dump-outputs", default="", metavar="DIR")
-    bench_backend(ap.parse_args())
+    ap.add_argument("--global-map", action="store_true", help="run the global-map leg instead of the LiDAR step")
+    ap.add_argument("--gm-keyframes", default="300,2000", help="trajectory lengths of the global-map leg")
+    args = ap.parse_args()
+    if args.global_map:
+        bench_global_map(args)
+    else:
+        bench_backend(args)
 
 
 if __name__ == "__main__":
