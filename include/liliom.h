@@ -277,8 +277,21 @@ int liliom_backend_window_blocks(liliom_ctx* c, const double* poses7_body, int k
 int liliom_backend_window_corr(liliom_ctx* c, int slot, int kind, unsigned char* valid, void* a, void* b, int cap, int* n);
 
 /* Loop-closure clouds from the store, detectLoopClosure (L:2473-2547): per keyframe, edge THEN surf (:2492-2493, :2519-2520)
- * transformed by poses7[i], concatenated, VoxelGrid(leaf), downloaded (out = NULL: *n only).  The result feeds liliom_icp_align. */
+ * transformed by poses7[i], concatenated, VoxelGrid(leaf), downloaded (out = NULL: *n only).  The result feeds liliom_icp_align
+ * (callers that bring their own clouds); liliom_loop_align composes both loop-closure clouds and aligns them on the device. */
 int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, float leaf, void* out, int cap, int* n);
+
+/* Loop closure from the store in one call, detectLoopClosure's clouds + performLoopClosure's alignment (L:2473-2582):
+ * source = liliom_kf_cloud(src_ids, src_poses7, k_src, leaf) (latest_key_frames_ds), target = liliom_kf_cloud(tgt_ids,
+ * tgt_poses7, k_tgt, leaf) (his_key_frames_ds), both kept on the device, then liliom_icp_align's ICP on them.  The result is
+ * bit-identical to those three calls (the ICP on a second context of the same point layout); *n_src / *n_tgt (optional) = the
+ * two cloud sizes.  The target gets a search index of its own: the odometry map, the local map, the resident correspondences
+ * (single keyframe and window) and the keyframe store are left as they were.  An empty source or target: LILIOM_OK, identity,
+ * *converged = 0, *iters = 0.  LILIOM_E_ARG (nothing changes): an unknown id, leaf <= 0, max_corr_dist <= 0, max_iter < 1, a
+ * sharded context. */
+int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids,
+                      const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps,
+                      double fit_eps, double T16[16], double* fitness, int* converged, int* iters, int* n_src, int* n_tgt);
 
 /* downSampleCloud, full-cloud half (L:1494-1500, R:1373-1376): attach the keyframe's /full_point_cloud (body frame,
  * point_stride bytes per point) to keyframe kf_id.  variant 0 stores it as received (full_clouds); variant 1 stores
@@ -318,8 +331,10 @@ int liliom_extract_horizon_livox(liliom_ctx* c, const void* custom_pts, int n, i
  * (host clouds, stride 48|32|16): per iteration the nearest target point of every transformed source point (kept within
  * max_corr_dist), the rigid transform by the SVD closed form, PCL's default convergence criteria.  T16 = getFinalTransformation()
  * (row-major 4x4, target <- source), *fitness = getFitnessScore(), *converged = hasConverged(), *iters = iterations run.
- * The target is installed as the context's map (use a context of its own for the backend).  fp64 where PCL is fp32; PCL's
- * setRANSACIterations is a no-op for this class (no rejector installed), so the alignment is deterministic. */
+ * The target is installed as the context's map (the backend aligns its own keyframes with liliom_loop_align instead, which
+ * leaves the map alone).  The whole loop, the fitness pass included, is one cooperative launch with one stream synchronise.
+ * fp64 where PCL is fp32; PCL's setRANSACIterations is a no-op for this class (no rejector installed), so the alignment is
+ * deterministic. */
 int liliom_icp_align(liliom_ctx* c, const void* src, int n_src, const void* tgt, int n_tgt, int stride, double max_corr_dist,
                      int max_iter, double trans_eps, double fit_eps, double T16[16], double* fitness, int* converged, int* iters);
 

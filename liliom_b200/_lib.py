@@ -73,7 +73,7 @@ EXPORTS = [
     "liliom_comm_peer_epoch", "liliom_comm_peer_set_epoch",
     "liliom_backend_default_params", "liliom_kf_add", "liliom_kf_count", "liliom_kf_clear", "liliom_bmap_build",
     "liliom_bmap_download", "liliom_backend_window_correspond", "liliom_backend_window_blocks", "liliom_backend_window_corr",
-    "liliom_kf_cloud", "liliom_kf_add_full", "liliom_global_map",
+    "liliom_kf_cloud", "liliom_kf_add_full", "liliom_global_map", "liliom_loop_align",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -179,6 +179,8 @@ def lib() -> C.CDLL:
     L.liliom_kf_cloud.argtypes = [vp, ip, dp, C.c_int, C.c_float, vp, C.c_int, ip]
     L.liliom_kf_add_full.argtypes = [vp, bpp, C.c_int, vp, C.c_int, ip]
     L.liliom_global_map.argtypes = [vp, C.c_int, ip, dp, C.c_int, dp, C.c_float, vp, C.c_int, ip]
+    L.liliom_loop_align.argtypes = [vp, ip, dp, C.c_int, ip, dp, C.c_int, C.c_float, C.c_double, C.c_int, C.c_double, C.c_double,
+                                    dp, dp, ip, ip, ip, ip]
     L.liliom_pre_create.argtypes = [vp, C.c_int, dp]; L.liliom_pre_create.restype = vp
     L.liliom_pre_destroy.argtypes = [vp]; L.liliom_pre_destroy.restype = None
     L.liliom_pre_imu.argtypes = [vp, C.c_double, dp]; L.liliom_pre_imu.restype = None
@@ -557,6 +559,19 @@ class Context:
         out = np.zeros(max(n.value, 1), self.dtype)
         self._check(lib().liliom_kf_cloud(self._h, ids.ctypes.data_as(ipp), _dptr(p), len(ids), leaf, _ptr(out), len(out), C.byref(n)))
         return out[:n.value]
+
+    def loop_align(self, src_ids, src_poses, tgt_ids, tgt_poses, leaf: float, max_corr_dist=30.0, max_iter=100, trans_eps=1e-6,
+                   fit_eps=1e-6):
+        """Loop closure from the store: kf_cloud of both lists and icp_align of the first onto the second, on the device.
+        Returns (T 4x4, fitness, converged, iterations, n_src, n_tgt)."""
+        si = _ids(src_ids); sp = _poses(src_poses, len(si))
+        ti = _ids(tgt_ids); tp = _poses(tgt_poses, len(ti))
+        ipp = C.POINTER(C.c_int)
+        T = np.zeros(16, np.float64); fit = C.c_double(); conv = C.c_int(); it = C.c_int(); ns = C.c_int(); nt = C.c_int()
+        self._check(lib().liliom_loop_align(self._h, si.ctypes.data_as(ipp), _dptr(sp), len(si), ti.ctypes.data_as(ipp), _dptr(tp), len(ti),
+                                            leaf, max_corr_dist, max_iter, trans_eps, fit_eps, _dptr(T), C.byref(fit), C.byref(conv),
+                                            C.byref(it), C.byref(ns), C.byref(nt)))
+        return T.reshape(4, 4), fit.value, bool(conv.value), it.value, ns.value, nt.value
 
     def kf_add_full(self, bp: BackendParams, kf_id: int, full: np.ndarray) -> int:
         """downSampleCloud (full-cloud half): attach keyframe kf_id's full body-frame cloud, stored as received (variant 0) or

@@ -239,7 +239,7 @@ extern "C" void liliom_destroy(liliom_ctx* c) {
                       &c->cub_tmp, &c->vg_coop, &c->hz_ctl, &c->map_raw, &c->map_ds, &c->map.xyzw, &c->map.sorted, &c->map.cell_start, &c->grid_keys, &c->grid_keys2,
                       &c->grid_vals, &c->grid_vals2, &c->feats, &c->corr_valid, &c->corr_plane, &c->nn_idx, &c->nn_sqd, &c->pose_dev,
                       &c->partials, &c->neq, &c->stats_dev, &c->counter, &c->lm_state, &c->raw_scan, &c->map.refl, &c->livox_in, &c->qstate, &c->inc_key[0], &c->inc_key[1], &c->inc_ref[0], &c->inc_ref[1], &c->inc_newkey[0], &c->inc_newkey[1],
-                      &c->inc_newref[0], &c->inc_newref[1], &c->inc_removed, &c->inc_rpos, &c->inc_flags, &c->inc_rank, &c->inc_bad};
+                      &c->inc_newref[0], &c->inc_newref[1], &c->inc_removed, &c->inc_rpos, &c->inc_flags, &c->inc_rank, &c->inc_bad, &c->icp_ctl};
     for (DevBuf* b : bufs) b->release();
     backend_release(c);
     for (auto& f : c->frames) f.buf.release();
@@ -924,7 +924,7 @@ extern "C" int liliom_icp_align(liliom_ctx* c, const void* src, int n_src, const
     }
     LILI_TRY(install_map_from_xyzw(c, n_tgt));
     LILI_TRY(upload_feats(c, src, n_src, stride));
-    return icp_align(c, c->feats.as<float4>(), n_src, max_corr_dist, max_iter, trans_eps, fit_eps, T16, fitness, converged, iters);
+    return icp_align(c, c->map, c->feats.as<float4>(), n_src, max_corr_dist, max_iter, trans_eps, fit_eps, T16, fitness, converged, iters);
 }
 
 // ===================== wire format, publishing side =====================

@@ -82,6 +82,12 @@ struct PeerArgs {
 constexpr int kStatsDoubles = 40;   // per outer iteration on the device: n_corr, lm_iters, cost, 27, pose7, pad
 constexpr int kNormEq = 29;         // 21 + 6 + cost + count
 
+struct PinIcp {                // ICP results (icp.cu), stored by the last block of the ICP kernel
+    double T[16];              // row-major 4x4 source -> target
+    double fitness;
+    int    converged, iters;
+};
+
 // The context's small pinned host block (liliom_ctx::h_pin): disjoint members, each read after its user's stream synchronise.
 struct PinResult {             // scan-to-map results: stored by the persistent GN kernel through GnIo::host_out, or copied
     double pose[8];            // pose (wxyz, t) + peer-loss flag
@@ -101,7 +107,8 @@ struct PinBlock {
     double map_status[4];      // multi-rank map rebuild: {owned voxels, failed} out, their sums over the ranks back
     unsigned long long block27[2];   // block27_stats: queries, points in their cell blocks
     int    bk_cnt[2 * 16];     // backend: VoxelGrid output counts (keyframe store, local map), window correspondence counts [kind][16]
-    double stats[];            // kStatsDoubles per GN iteration, up to the end of the block (h_pin_bytes)
+    PinIcp icp;                // ICP: the results of k_icp_persistent
+    double stats[];         // kStatsDoubles per GN iteration, up to the end of the block (h_pin_bytes)
 };
 
 // Scan-to-map results written straight into the context's pinned host block by the persistent GN kernel (zero-copy: the
@@ -119,6 +126,23 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
     return t;
+}
+
+// Grid barrier of the persistent kernels (k_gn_persistent, k_icp_persistent), run by thread 0 of each block after the block's
+// __syncthreads: one arrival on `bar`, then, when `wait`, a poll until the arrivals reach `target`.  sync_mode (LILIOM_GN_SYNC,
+// see liliom_ctx::gn_sync): 3 = release-only arrival and a relaxed poll, 1 = acquire poll, 0 = full fences on both sides.
+__device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int target, int sync_mode, bool wait) {
+    unsigned int v;
+    if (sync_mode == 0) {
+        atomicAdd(bar, 1u);
+        if (wait) { while ((int)(*reinterpret_cast<volatile unsigned int*>(bar) - target) < 0) { } __threadfence(); }
+    } else {
+        asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(bar), "r"(1u) : "memory");
+        if (wait) {
+            if (sync_mode == 1) { do { asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory"); } while ((int)(v - target) < 0); }
+            else { do { asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory"); } while ((int)(v - target) < 0); }
+        }
+    }
 }
 #endif
 
@@ -209,6 +233,8 @@ struct liliom_ctx {
     std::vector<int> win_ids;
     std::vector<long long> win_qoff[2];  // per kind: query prefix offsets (k + 1)
     lili::DevBuf win_valid[2], win_line, win_plane, win_score, win_cnt, win_tab;
+    lili::MapIndex loop;                 // loop-closure target (liliom_loop_align): its own index, so the odometry map stays
+    lili::DevBuf loop_src;               // ... and its float4 source
 
     // ---- scan-to-map ----
     lili::DevBuf feats;                  // float4 body-frame queries
@@ -221,6 +247,7 @@ struct liliom_ctx {
     lili::DevBuf stats_dev;              // iterations x kStatsDoubles
     lili::DevBuf counter;                // last-block ticket + scratch ints
     lili::DevBuf lm_state;
+    lili::DevBuf icp_ctl;                // ICP kernel: barrier word, and its results when the pinned block is not mappable
     int bk_kind = 0, bk_n = 0;           // backend correspondences resident from the last liliom_correspond_* call (1 edge, 2 surf)
     unsigned int bar_arrivals = 0;       // total grid-barrier arrivals issued so far (persistent GN kernel)
 
@@ -241,7 +268,7 @@ struct liliom_ctx {
     unsigned time_calls = 0;
     // run-time switches: read by liliom_create and nowhere else (DESIGN.md §6)
     int force_lanes = 0, force_rounds = 0;   // tuning override (LILIOM_KNN_LANES / LILIOM_KNN_ROUNDS)
-    int gn_sync = 3;                     // persistent GN kernel grid barrier (LILIOM_GN_SYNC): 3 = release-only arrival, no acquire fence (default),
+    int gn_sync = 3;                     // persistent kernels' grid barrier (LILIOM_GN_SYNC): 3 = release-only arrival, no acquire fence (default),
                                          // 1 = acquire poll, 0 = full fences on both sides
     bool dbg_timing = false;             // LILIOM_DEBUG_TIMING: stage clocks of the cooperative kernels, printed by s2m_run
     bool rot_slow_walk = false;          // LILIOM_ROT_SLOW_WALK (test hook): the general walk of k_rot_ring for every segment
@@ -313,8 +340,8 @@ int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int
 int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf, int* n_edge, int* n_cut, bool sync_counts = true);
 int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut);
 
-int icp_align(liliom_ctx* c, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps, double fit_eps,
-              double T16[16], double* fitness, int* converged, int* iters);           // icp.cu
+int icp_align(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,
+              double fit_eps, double T16[16], double* fitness, int* converged, int* iters);     // icp.cu
 int map_inc_update(liliom_ctx* c, int popped_slot, int popped_nfin, int* m_out);     // map_inc.cu
 int map_finish_from_ds(liliom_ctx* c, int m);                                        // api.cu
 void frames_box(const liliom_ctx* c, int mm[7]);                                     // api.cu: union of the frames' boxes

@@ -689,20 +689,7 @@ __global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned in
         if (sync_mode == 0) __threadfence();
         __syncthreads();
         if (stamp) a.dbg[18] = clock64();
-        if (threadIdx.x == 0) {
-            const unsigned int target = bar_base + (unsigned int)(it + 1) * G;
-            unsigned int v;
-            if (sync_mode == 0) {
-                atomicAdd(bar, 1u);
-                if (!follower) { while ((int)(*reinterpret_cast<volatile unsigned int*>(bar) - target) < 0) { } __threadfence(); }
-            } else {
-                asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(bar), "r"(1u) : "memory");
-                if (!follower) {
-                    if (sync_mode == 1) { do { asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory"); } while ((int)(v - target) < 0); }
-                    else { do { asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory"); } while ((int)(v - target) < 0); }
-                }
-            }
-        }
+        if (threadIdx.x == 0) grid_barrier(bar, bar_base + (unsigned int)(it + 1) * G, sync_mode, !follower);
         if (!follower) {
             __syncthreads();
             if (stamp) a.dbg[19] = clock64();

@@ -14,26 +14,32 @@
 // PCL runs this in single precision (Matrix4f, float clouds); here the transform and the sums are fp64 — parity with PCL is at
 // tolerance level either way.
 //
-// One thread per source point: expanding-shell exact 1-NN over the target's 1 m cells (the 27-cell block first, then shells of
-// Chebyshev radius r; the search stops once the best distance is below r-1 cells or the shell lies beyond the cut-off), the 16
-// sums of the closed form + the count reduced per block in a fixed order, the 3x3 SVD on the host (one-sided Jacobi).
+// The whole loop is ONE cooperative launch (k_icp_persistent).  The source is dealt in virtual blocks of 256 points; per
+// iteration each virtual block runs one thread per point — expanding-shell exact 1-NN over the target's cells (the 27-cell
+// block first, then shells of Chebyshev radius r; the search stops once the best distance is below r-1 cells or the shell lies
+// beyond the cut-off) — and reduces the 16 sums of the closed form + the count in a fixed order into its partials slot; after
+// a grid barrier every block folds the partials in virtual-block order and takes the step of icp_math.h (SVD, Umeyama,
+// composition, convergence) redundantly, with the same bits, so no broadcast is needed.  The final fitness pass runs in the
+// same launch, and the results go straight to the context's pinned block: one stream synchronise per alignment.
 #include "ctx.cuh"
 #include "dev_math.cuh"
 #include "knn_core.cuh"
+#include "icp_math.h"
 #include <cmath>
-#include <vector>
 
 namespace lili {
 
-constexpr int kIcpSums = 17;      // sum p (3), sum q (3), sum p q^T (9, row = p, col = q), sum d2, count
+constexpr int kIcpBlock = 256;    // points per virtual block = threads per block
 
 struct IcpArgs {
-    const float4* src; int n;                       // source points (float4 xyz*)
+    const float4* src; int n, nvb;                   // source points (float4 xyz*), virtual blocks cdiv(n, 256)
     const float4* map; const float4* map_orig; const int* cell_start; GridDesc g;
-    double T[12];                                    // current source -> target transform, row-major 3x4
-    float max_d2;                                    // squared correspondence cut-off (<0: none, fitness pass)
-    int rmax;                                        // shells to visit at most
-    double* partials;                                // [kIcpSums][gridDim.x]
+    float max_d2;                                    // squared correspondence cut-off
+    int rmax, rmax_fit;                              // shells to visit at most: correspondence passes, the fitness pass
+    int max_iter; double trans_eps, fit_eps;
+    double* partials;                                // [2 parities][kIcpSums][nvb]
+    unsigned int* bar; int sync_mode;                // grid barrier word (zeroed before the launch), LILIOM_GN_SYNC
+    PinIcp* out;                                     // results (the pinned block, or device memory)
 };
 
 __device__ __forceinline__ void icp_run(const float4* __restrict__ map, int b, int e, float sx, float sy, float sz, u64& best) {
@@ -44,29 +50,31 @@ __device__ __forceinline__ void icp_run(const float4* __restrict__ map, int b, i
     }
 }
 
-__global__ void __launch_bounds__(256) k_icp_pass(IcpArgs a) {
-    __shared__ double red[8][kIcpSums];
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+// One virtual block of one pass: the 17 sums of source points vb*256 .. vb*256+255 under T (row-major 3x4), written to
+// part[k * nvb + vb].  max_d2 < 0: no cut-off (fitness pass).
+__device__ __forceinline__ void icp_vblock(const IcpArgs& a, int vb, const double* T, float max_d2, int rmax, double* part,
+                                           double (*red)[kIcpSums]) {
+    const int i = vb * kIcpBlock + threadIdx.x;
     double v[kIcpSums];
 #pragma unroll
     for (int k = 0; k < kIcpSums; ++k) v[k] = 0.0;
     if (i < a.n) {
         const float4 s = a.src[i];
-        const double px = a.T[0] * s.x + a.T[1] * s.y + a.T[2] * s.z + a.T[3];
-        const double py = a.T[4] * s.x + a.T[5] * s.y + a.T[6] * s.z + a.T[7];
-        const double pz = a.T[8] * s.x + a.T[9] * s.y + a.T[10] * s.z + a.T[11];
+        const double px = T[0] * s.x + T[1] * s.y + T[2] * s.z + T[3];
+        const double py = T[4] * s.x + T[5] * s.y + T[6] * s.z + T[7];
+        const double pz = T[8] * s.x + T[9] * s.y + T[10] * s.z + T[11];
         const float sx = (float)px, sy = (float)py, sz = (float)pz;
         const GridDesc& g = a.g;
         const float cell = 1.0f / g.inv_cell;
         const int cx = cell_coord(sx, g.inv_cell) - g.org[0], cy = cell_coord(sy, g.inv_cell) - g.org[1], cz = cell_coord(sz, g.inv_cell) - g.org[2];
-        const bool cut = a.max_d2 >= 0.f;
+        const bool cut = max_d2 >= 0.f;
         u64 best = ~0ull;
 #pragma unroll 1
-        for (int r = 1; r <= a.rmax; ++r) {
+        for (int r = 1; r <= rmax; ++r) {
             if (r >= 2) {
                 // every unvisited point is at least (r-1) cells away: stop when the best is strictly closer, or the shell is out of range
                 const float gap = (float)(r - 1) * cell, gap2 = gap * gap;
-                if (cut && gap2 > a.max_d2) break;
+                if (cut && gap2 > max_d2) break;
                 if (best != ~0ull && top5_dist(best) < gap2) break;
             }
             const int z0 = max(cz - r, 0), z1 = min(cz + r, g.dim[2] - 1), y0 = max(cy - r, 0), y1 = min(cy + r, g.dim[1] - 1);
@@ -84,7 +92,7 @@ __global__ void __launch_bounds__(256) k_icp_pass(IcpArgs a) {
                 }
             }
         }
-        if (best != ~0ull && (!cut || top5_dist(best) <= a.max_d2)) {
+        if (best != ~0ull && (!cut || top5_dist(best) <= max_d2)) {
             const float4 q = __ldg(a.map_orig + top5_index(best));
             v[0] = px; v[1] = py; v[2] = pz;
             v[3] = q.x; v[4] = q.y; v[5] = q.z;
@@ -106,132 +114,105 @@ __global__ void __launch_bounds__(256) k_icp_pass(IcpArgs a) {
     if (threadIdx.x < kIcpSums) {
         double s = 0.0;
         for (int w = 0; w < 8; ++w) s += red[w][threadIdx.x];
-        a.partials[(size_t)threadIdx.x * gridDim.x + blockIdx.x] = s;
+        part[(size_t)threadIdx.x * a.nvb + vb] = s;
+    }
+    __syncthreads();      // red is reused by the block's next virtual block
+}
+
+// One pass over every virtual block under T, the grid barrier `phase`, and the fold of the partials in virtual-block order
+// 0..nvb-1 into sums[] (every block).
+__device__ __forceinline__ void icp_pass(const IcpArgs& a, const double* T, float max_d2, int rmax, int phase, double (*red)[kIcpSums],
+                                         double* sums) {
+    double* part = a.partials + (size_t)(phase & 1) * kIcpSums * a.nvb;
+    for (int vb = blockIdx.x; vb < a.nvb; vb += gridDim.x) icp_vblock(a, vb, T, max_d2, rmax, part, red);
+    if (a.sync_mode == 0) __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) grid_barrier(a.bar, (unsigned int)(phase + 1) * gridDim.x, a.sync_mode, true);
+    __syncthreads();
+    if (threadIdx.x < kIcpSums) {
+        const double* p = part + (size_t)threadIdx.x * a.nvb;
+        double s = 0.0;
+#pragma unroll 8
+        for (int b = 0; b < a.nvb; ++b) s = addx(s, __ldcg(p + b));
+        sums[threadIdx.x] = s;
+    }
+    __syncthreads();
+}
+
+// The step of thread 0 out of line: its fp64 SVD and local arrays stay off the register budget of the search
+__device__ __noinline__ int icp_step_dev(IcpState& st, const double* sums, int max_iter, double trans_eps, double fit_eps) {
+    return icp_step(st, sums, max_iter, trans_eps, fit_eps);
+}
+
+// The whole alignment in one cooperative launch (grid <= co-resident blocks; any grid gives the same bits).  The partials
+// alternate between two buffers by barrier parity: a block can only write phase p + 2's partials after every block has
+// arrived at barrier p + 1, i.e. after every block has folded phase p's.
+__global__ void __launch_bounds__(kIcpBlock) k_icp_persistent(const __grid_constant__ IcpArgs a) {
+    __shared__ double red[8][kIcpSums];
+    __shared__ double sums[kIcpSums];
+    __shared__ double T[12];                // rows 0..2 of F, the transform of the next pass
+    __shared__ int verdict;
+    IcpState st;                            // thread 0's copy (the step is redundant across blocks)
+    icp_init(st);
+    if (threadIdx.x < 12) T[threadIdx.x] = st.F[threadIdx.x / 4][threadIdx.x % 4];
+    __syncthreads();
+    int phase = 0;
+#pragma unroll 1
+    while (true) {
+        icp_pass(a, T, a.max_d2, a.rmax, phase++, red, sums);
+        if (threadIdx.x == 0) {
+            verdict = icp_step_dev(st, sums, a.max_iter, a.trans_eps, a.fit_eps);
+            for (int k = 0; k < 12; ++k) T[k] = st.F[k / 4][k % 4];
+        }
+        __syncthreads();
+        if (verdict != kIcpGo) break;
+    }
+    // getFitnessScore(): mean squared NN distance of the aligned source, no cut-off; the walk is bounded by the grid's extent
+    icp_pass(a, T, -1.0f, a.rmax_fit, phase, red, sums);
+    if (blockIdx.x == 0 && threadIdx.x == 0) {
+        for (int k = 0; k < 16; ++k) a.out->T[k] = st.F[k / 4][k % 4];
+        a.out->fitness = icp_fitness(sums);
+        a.out->converged = verdict == kIcpConverged ? 1 : 0;
+        a.out->iters = st.it;
+        __threadfence_system();
     }
 }
 
-// ---- host side: 3x3 SVD by one-sided Jacobi (Hestenes), A = U diag(s) V^T
-static void svd3(const double A[3][3], double U[3][3], double s[3], double V[3][3]) {
-    double B[3][3];
-    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) { B[i][j] = A[i][j]; V[i][j] = i == j ? 1.0 : 0.0; }
-    for (int sweep = 0; sweep < 60; ++sweep) {
-        double off = 0.0;
-        for (int p = 0; p < 2; ++p)
-            for (int q = p + 1; q < 3; ++q) {
-                double alpha = 0, beta = 0, gamma = 0;
-                for (int i = 0; i < 3; ++i) { alpha += B[i][p] * B[i][p]; beta += B[i][q] * B[i][q]; gamma += B[i][p] * B[i][q]; }
-                off = std::fmax(off, std::fabs(gamma) / std::sqrt(alpha * beta + 1e-300));
-                if (std::fabs(gamma) < 1e-300) continue;
-                const double zeta = (beta - alpha) / (2.0 * gamma);
-                const double t = (zeta >= 0 ? 1.0 : -1.0) / (std::fabs(zeta) + std::sqrt(1.0 + zeta * zeta));
-                const double c = 1.0 / std::sqrt(1.0 + t * t), sn = c * t;
-                for (int i = 0; i < 3; ++i) {
-                    const double bp = B[i][p], bq = B[i][q];
-                    B[i][p] = c * bp - sn * bq; B[i][q] = sn * bp + c * bq;
-                    const double vp = V[i][p], vq = V[i][q];
-                    V[i][p] = c * vp - sn * vq; V[i][q] = sn * vp + c * vq;
-                }
-            }
-        if (off < 1e-15) break;
-    }
-    for (int j = 0; j < 3; ++j) {
-        s[j] = std::sqrt(B[0][j] * B[0][j] + B[1][j] * B[1][j] + B[2][j] * B[2][j]);
-        for (int i = 0; i < 3; ++i) U[i][j] = s[j] > 1e-300 ? B[i][j] / s[j] : 0.0;
-    }
-    // a zero singular value leaves a zero column in U: complete it to an orthonormal basis (cross product of the other two)
-    for (int j = 0; j < 3; ++j) {
-        if (s[j] > 1e-300) continue;
-        const int a = (j + 1) % 3, b = (j + 2) % 3;
-        U[0][j] = U[1][a] * U[2][b] - U[2][a] * U[1][b];
-        U[1][j] = U[2][a] * U[0][b] - U[0][a] * U[2][b];
-        U[2][j] = U[0][a] * U[1][b] - U[1][a] * U[0][b];
-    }
-}
-static double det3(const double M[3][3]) {
-    return M[0][0] * (M[1][1] * M[2][2] - M[1][2] * M[2][1]) - M[0][1] * (M[1][0] * M[2][2] - M[1][2] * M[2][0]) + M[0][2] * (M[1][0] * M[2][1] - M[1][1] * M[2][0]);
-}
-
-static int icp_pass(liliom_ctx* c, IcpArgs& a, int grid, double sums[kIcpSums]) {
-    k_icp_pass<<<grid, 256, 0, c->stream>>>(a);
-    LILI_TRY(launch_check(c, "k_icp_pass"));
-    std::vector<double> h((size_t)kIcpSums * grid);
-    LILI_CUDA(c, cudaMemcpyAsync(h.data(), a.partials, h.size() * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    for (int k = 0; k < kIcpSums; ++k) { double s = 0.0; for (int b = 0; b < grid; ++b) s += h[(size_t)k * grid + b]; sums[k] = s; }      // fixed order
-    return LILIOM_OK;
-}
-
-// src (device float4, n points) against the map installed in c; T16 row-major 4x4 out
-int icp_align(liliom_ctx* c, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps, double fit_eps,
-              double T16[16], double* fitness, int* converged, int* iters) {
+// src (device float4, n points) against the index `tgt`; T16 row-major 4x4 out
+int icp_align(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,
+              double fit_eps, double T16[16], double* fitness, int* converged, int* iters) {
     for (int k = 0; k < 16; ++k) T16[k] = (k % 5 == 0) ? 1.0 : 0.0;
     *fitness = 0.0; *converged = 0; *iters = 0;
-    if (n <= 0 || c->map.n <= 0) return LILIOM_OK;
-    const int grid = cdiv(n, 256);
-    LILI_CUDA(c, c->partials.ensure((size_t)kIcpSums * grid * sizeof(double)));
+    if (n <= 0 || tgt.n <= 0) return LILIOM_OK;
     IcpArgs a{};
-    a.src = d_src; a.n = n; a.map = c->map.sorted.as<float4>(); a.map_orig = c->map.xyzw.as<float4>(); a.cell_start = c->map.cell_start.as<int>(); a.g = c->map.grid;
-    a.partials = c->partials.as<double>();
-    const float cell = 1.0f / c->map.grid.inv_cell;
+    a.src = d_src; a.n = n; a.nvb = cdiv(n, kIcpBlock);
+    a.map = tgt.sorted.as<float4>(); a.map_orig = tgt.xyzw.as<float4>(); a.cell_start = tgt.cell_start.as<int>(); a.g = tgt.grid;
+    const float cell = 1.0f / tgt.grid.inv_cell;
     a.max_d2 = (float)(max_corr_dist * max_corr_dist);
     a.rmax = (int)std::ceil(max_corr_dist / cell) + 1;
-    double F[4][4] = {{1, 0, 0, 0}, {0, 1, 0, 0}, {0, 0, 1, 0}, {0, 0, 0, 1}};
-    double prev_mse = std::numeric_limits<double>::max();
-    int it = 0;
-    bool conv = false;
-    while (true) {
-        for (int r = 0; r < 3; ++r) for (int k = 0; k < 4; ++k) a.T[4 * r + k] = F[r][k];
-        double s[kIcpSums];
-        LILI_TRY(icp_pass(c, a, grid, s));
-        const double cnt = s[16];
-        if (cnt < 3.0) { conv = false; break; }                       // icp.hpp: "Not enough correspondences found"
-        // Umeyama without scale on the matched pairs (p = transformed source, q = target)
-        const double mp[3] = {s[0] / cnt, s[1] / cnt, s[2] / cnt}, mq[3] = {s[3] / cnt, s[4] / cnt, s[5] / cnt};
-        double Sg[3][3];                                              // sigma = 1/n sum (q - mq)(p - mp)^T  (dst x src^T)
-        for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Sg[i][j] = s[6 + 3 * j + i] / cnt - mq[i] * mp[j];
-        double U[3][3], sv[3], V[3][3];
-        svd3(Sg, U, sv, V);
-        const double sgn = det3(U) * det3(V) < 0 ? -1.0 : 1.0;
-        // the reflection fix belongs to the SMALLEST singular value (Eigen sorts them descending and flips the last)
-        int jmin = 0;
-        for (int j = 1; j < 3; ++j) if (sv[j] < sv[jmin]) jmin = j;
-        double R[3][3];
-        for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) {
-            double acc = 0.0;
-            for (int k = 0; k < 3; ++k) acc += U[i][k] * (k == jmin ? sgn : 1.0) * V[j][k];
-            R[i][j] = acc;
-        }
-        double t[3];
-        for (int i = 0; i < 3; ++i) t[i] = mq[i] - (R[i][0] * mp[0] + R[i][1] * mp[1] + R[i][2] * mp[2]);
-        double N[4][4] = {{0}};                                       // final = incremental * final
-        for (int i = 0; i < 3; ++i) {
-            for (int j = 0; j < 4; ++j) N[i][j] = R[i][0] * F[0][j] + R[i][1] * F[1][j] + R[i][2] * F[2][j] + (j == 3 ? t[i] : 0.0);
-        }
-        N[3][3] = 1.0;
-        memcpy(F, N, sizeof(F));
-        ++it;
-        // DefaultConvergenceCriteria::hasConverged (max_iterations_similar_transforms_ = 0)
-        const double mse = s[15] / cnt;
-        if (it >= max_iter) { conv = true; break; }
-        const double cos_angle = 0.5 * (R[0][0] + R[1][1] + R[2][2] - 1.0);
-        const double tr2 = t[0] * t[0] + t[1] * t[1] + t[2] * t[2];
-        if (cos_angle >= 1.0 - trans_eps && tr2 <= trans_eps) { conv = true; break; }
-        if (std::fabs(mse - prev_mse) / prev_mse < fit_eps) { conv = true; break; }
-        if (std::fabs(mse - prev_mse) < 1e-12) { conv = true; break; }
-        prev_mse = mse;
-    }
-    // getFitnessScore(): mean squared NN distance of the aligned source, no cut-off
-    for (int r = 0; r < 3; ++r) for (int k = 0; k < 4; ++k) a.T[4 * r + k] = F[r][k];
-    a.max_d2 = -1.0f;
-    a.rmax = std::max(c->map.grid.dim[0], std::max(c->map.grid.dim[1], c->map.grid.dim[2])) + 1;
-    {   // sources far outside the grid would walk many empty shells: bound the walk by the distance to the grid plus its extent
-        double s[kIcpSums];
-        LILI_TRY(icp_pass(c, a, grid, s));
-        *fitness = s[16] > 0 ? s[15] / s[16] : std::numeric_limits<double>::max();
-    }
-    for (int i = 0; i < 4; ++i) for (int j = 0; j < 4; ++j) T16[4 * i + j] = F[i][j];
-    *converged = conv ? 1 : 0;
-    *iters = it;
+    a.rmax_fit = std::max(tgt.grid.dim[0], std::max(tgt.grid.dim[1], tgt.grid.dim[2])) + 1;
+    a.max_iter = max_iter; a.trans_eps = trans_eps; a.fit_eps = fit_eps;
+    a.sync_mode = c->gn_sync;
+    int per_sm = 0;
+    LILI_CUDA(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_icp_persistent, kIcpBlock, 0));
+    const int grid = std::max(1, std::min(a.nvb, per_sm * c->sm_count));
+    LILI_CUDA(c, c->partials.ensure((size_t)2 * kIcpSums * a.nvb * sizeof(double)));
+    LILI_CUDA(c, c->icp_ctl.ensure(64 + sizeof(PinIcp)));
+    LILI_CUDA(c, cudaMemsetAsync(c->icp_ctl.p, 0, sizeof(unsigned int), c->stream));
+    a.partials = c->partials.as<double>();
+    a.bar = c->icp_ctl.as<unsigned int>();
+    PinIcp* dev_out = reinterpret_cast<PinIcp*>(c->icp_ctl.as<unsigned char>() + 64);
+    a.out = c->h_pin_dev ? &c->h_pin_dev->icp : dev_out;
+    void* kargs[] = {&a};
+    LILI_CUDA(c, cudaLaunchCooperativeKernel((const void*)k_icp_persistent, dim3(grid), dim3(kIcpBlock), kargs, 0, c->stream));
+    LILI_TRY(launch_check(c, "k_icp_persistent"));
+    if (!c->h_pin_dev) LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->icp, dev_out, sizeof(PinIcp), cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    const PinIcp& r = c->h_pin->icp;
+    for (int k = 0; k < 16; ++k) T16[k] = r.T[k];
+    *fitness = r.fitness;
+    *converged = r.converged;
+    *iters = r.iters;
     return LILIOM_OK;
 }
 

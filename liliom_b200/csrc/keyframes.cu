@@ -3,7 +3,8 @@
 //                    saveKeyFramesAndFactors (:1688-1695): VoxelGrid of the received body-frame clouds, appended to one arena
 //   local map        buildLocalMapWithLandMark (:1387-1484) + downSampleCloud, map half (:1486-1492): transform + concatenate
 //                    the listed keyframes in ONE launch, VoxelGrid per layer, a cell grid per layer (MapIndex)
-//   loop closure     detectLoopClosure's clouds (:2473-2547): edge then surf per keyframe, transformed, VoxelGrid
+//   loop closure     detectLoopClosure's clouds (:2473-2547): edge then surf per keyframe, transformed, VoxelGrid; with
+//                    performLoopClosure's ICP (:2552-2582) on them in the same call (liliom_loop_align)
 //   full clouds      downSampleCloud, full-cloud half (:1494-1500; R:1373-1376): the /full_point_cloud of a keyframe, stored
 //   global map       publishCompleteMap (:2644-2685) and save_pcd's map (:2703-2718): listed keyframes transformed, concatenated,
 //                    VoxelGrid, in a VoxelGrid that reads the store through the keyframe table (kf_table.h): no concatenation
@@ -79,9 +80,10 @@ __global__ void k_kf_refl(const unsigned char* __restrict__ pts, int n, float* _
 
 void backend_release(liliom_ctx* c) {
     DevBuf* bufs[] = {&c->kf_arena, &c->kf_full, &c->kf_tab, &c->bmap_raw, &c->bmap_ds[0], &c->bmap_ds[1], &c->win_valid[0], &c->win_valid[1],
-                      &c->win_line, &c->win_plane, &c->win_score, &c->win_cnt, &c->win_tab};
+                      &c->win_line, &c->win_plane, &c->win_score, &c->win_cnt, &c->win_tab, &c->loop_src};
     for (DevBuf* b : bufs) b->release();
     c->bmap[0].release(); c->bmap[1].release();
+    c->loop.release();
 }
 
 // Room for `pts` points in `arena`, of which the first `used` are stored.  Grows geometrically and COPIES the stored points
@@ -143,6 +145,29 @@ static KfRow kf_row(long long src, long long dst, int n, const double* pose7, co
         e.pt = D3{pre7[4], pre7[5], pre7[6]};
     }
     return e;
+}
+
+// detectLoopClosure's cloud of the listed keyframes (:2476-2497, :2502-2547): edge then surf of each, transformed by its pose,
+// concatenated into bmap_raw (one launch), VoxelGrid(leaf) into vg_out with its count at d_count (device).  *n_in: the points
+// read (0: nothing was launched and d_count is not written).
+static int kf_cloud_dev(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, float leaf, int* d_count, long long* n_in) {
+    const int stride = c->prm.point_stride;
+    std::vector<KfRow> tab;
+    long long off = 0, largest = 0;
+    for (int i = 0; i < k; ++i) {                                 // :2492-2493 / :2519-2520: *edge_frames[i] then *surf_frames[i]
+        const KfEntry& f = c->kfs[kf_ids[i]];
+        if (f.n_edge) tab.push_back(kf_row(f.edge_off, off, f.n_edge, poses7 + 7 * (size_t)i));
+        off += f.n_edge;
+        if (f.n_surf) tab.push_back(kf_row(f.surf_off, off, f.n_surf, poses7 + 7 * (size_t)i));
+        off += f.n_surf;
+        largest = std::max(largest, (long long)std::max(f.n_edge, f.n_surf));
+    }
+    *n_in = off;
+    if (off == 0) return LILIOM_OK;
+    LILI_CUDA(c, c->bmap_raw.ensure((size_t)off * stride));      // scratch: the local map's layers live in bmap_ds / bmap
+    LILI_CUDA(c, c->vg_out.ensure((size_t)off * stride));
+    LILI_TRY(kf_gather(c, c->kf_arena.p, tab, largest, c->bmap_raw.p));
+    return voxelgrid_dev(c, c->bmap_raw.p, (int)off, nullptr, stride, leaf, c->vg_out.p, d_count);
 }
 
 static int backend_check(liliom_ctx* c, const liliom_backend_params* bp) {
@@ -295,22 +320,10 @@ extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* p
     LILI_CUDA(c, cudaSetDevice(c->device));
     const int stride = c->prm.point_stride;
     *n_out = 0;
-    std::vector<KfRow> tab;
-    long long off = 0, largest = 0;
-    for (int i = 0; i < k; ++i) {                                 // :2492-2493 / :2519-2520: *edge_frames[i] then *surf_frames[i]
-        const KfEntry& f = c->kfs[kf_ids[i]];
-        if (f.n_edge) tab.push_back(kf_row(f.edge_off, off, f.n_edge, poses7 + 7 * (size_t)i));
-        off += f.n_edge;
-        if (f.n_surf) tab.push_back(kf_row(f.surf_off, off, f.n_surf, poses7 + 7 * (size_t)i));
-        off += f.n_surf;
-        largest = std::max(largest, (long long)std::max(f.n_edge, f.n_surf));
-    }
-    if (off == 0) return LILIOM_OK;
-    LILI_CUDA(c, c->bmap_raw.ensure((size_t)off * stride));      // scratch: the local map's layers live in bmap_ds / bmap
-    LILI_CUDA(c, c->vg_out.ensure((size_t)off * stride));
     LILI_CUDA(c, c->vg_count.ensure(16));
-    LILI_TRY(kf_gather(c, c->kf_arena.p, tab, largest, c->bmap_raw.p));
-    LILI_TRY(voxelgrid_dev(c, c->bmap_raw.p, (int)off, nullptr, stride, leaf, c->vg_out.p, c->vg_count.as<int>()));
+    long long off = 0;
+    LILI_TRY(kf_cloud_dev(c, kf_ids, poses7, k, leaf, c->vg_count.as<int>(), &off));
+    if (off == 0) return LILIOM_OK;
     LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     const int m = c->h_pin->bk_cnt[0];
@@ -320,6 +333,40 @@ extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* p
     if (m) LILI_CUDA(c, cudaMemcpyAsync(out, c->vg_out.p, (size_t)m * stride, cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     return LILIOM_OK;
+}
+
+// detectLoopClosure + performLoopClosure's alignment (:2473-2582) without leaving the device: the history cloud goes into the
+// loop index (its own cell grid: the odometry map, the local map and every resident correspondence stay), the latest cloud into
+// loop_src, and the ICP runs on them (icp.cu).  Scratch shared with the other calls: bmap_raw, vg_out, the sort chain, grid_keys*,
+// partials.  Two stream synchronises: the cloud sizes (the grid build needs the target's on the host), and the grid's box.
+extern "C" int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids,
+                                 const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps,
+                                 double fit_eps, double T16[16], double* fitness, int* converged, int* iters, int* n_src, int* n_tgt) {
+    if (!c || k_src < 0 || k_tgt < 0 || (k_src > 0 && (!src_ids || !src_poses7)) || (k_tgt > 0 && (!tgt_ids || !tgt_poses7)) ||
+        !(leaf > 0) || !(max_corr_dist > 0) || max_iter < 1 || !T16 || !fitness || !converged || !iters)
+        return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, nullptr));
+    if (!kf_ids_ok(c, src_ids, k_src) || !kf_ids_ok(c, tgt_ids, k_tgt)) return LILIOM_E_ARG;     // before anything changes
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    const int stride = c->prm.point_stride;
+    LILI_CUDA(c, c->vg_count.ensure(16));
+    int* cnt = c->vg_count.as<int>();
+    long long off_t = 0, off_s = 0;
+    // :2502-2547 his_key_frames_ds -> the loop index's points (float4, w = index), as liliom_icp_align installs a target
+    LILI_TRY(kf_cloud_dev(c, tgt_ids, tgt_poses7, k_tgt, leaf, cnt, &off_t));
+    LILI_CUDA(c, c->loop.xyzw.ensure((size_t)std::max(off_t, 1LL) * sizeof(float4)));
+    LILI_TRY(repack_to_f4(c, c->vg_out.p, (int)off_t, stride, c->loop.xyzw.as<float4>(), cnt));
+    // :2476-2497 latest_key_frames_ds -> the source
+    LILI_TRY(kf_cloud_dev(c, src_ids, src_poses7, k_src, leaf, cnt + 1, &off_s));
+    LILI_CUDA(c, c->loop_src.ensure((size_t)std::max(off_s, 1LL) * sizeof(float4)));
+    LILI_TRY(repack_to_f4(c, c->vg_out.p, (int)off_s, stride, c->loop_src.as<float4>(), cnt + 1));
+    LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, cnt, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    const int m_t = off_t ? c->h_pin->bk_cnt[0] : 0, m_s = off_s ? c->h_pin->bk_cnt[1] : 0;
+    if (n_src) *n_src = m_s;
+    if (n_tgt) *n_tgt = m_t;
+    LILI_TRY(grid_build(c, c->loop, gate_cell(c->prm.knn_max_sqdist), m_t));      // the cell of liliom_icp_align's target
+    return icp_align(c, c->loop, c->loop_src.as<float4>(), m_s, max_corr_dist, max_iter, trans_eps, fit_eps, T16, fitness, converged, iters);
 }
 
 extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp, int kf_id, const void* full, int n, int* n_stored) {

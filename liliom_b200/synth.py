@@ -237,21 +237,24 @@ def default_true_pose():
     return np.concatenate([q, [2.0, 3.0, 1.8]])
 
 
-def make_keyframe_sequence(n: int, stride: int = 48, seed: int = 7, step=1.5, yaw_deg=2.0, surf_every: int = 8, full: bool = False):
+def make_keyframe_sequence(n: int, stride: int = 48, seed: int = 7, step=1.5, yaw_deg=2.0, surf_every: int = 8, full: bool = False,
+                           revisit: int = 0):
     """A seeded keyframe stream for the backend (SURVEY.md §8 f5): n Horizon sweeps (no rotation inside a sweep, i.e. the
     clouds the backend receives after de-skew) taken every `step` metres along a gently turning path through the world.
     Each keyframe is split the way the extractors split a sweep: edge = returns from poles and wall tops (line-like
     neighbourhoods), surf = every `surf_every`-th other return.  Reflectivity (the `curvature` field, FormatConvert.cpp:21)
     is per surface kind plus a little noise, so the reflectivity-weighted plane fit of the Horizon backend sees real planes.
     Returns a list of (edge, surf, pose7) with clouds in the body frame, PT48 (stride 48) or PT32 (stride 32); full=True appends
-    each keyframe's whole sweep (the /full_point_cloud the edge and surf clouds were split from): (edge, surf, pose7, full)."""
+    each keyframe's whole sweep (the /full_point_cloud the edge and surf clouds were split from): (edge, surf, pose7, full).
+    revisit > 0 appends that many keyframes that come back to the poses of keyframes 0, 1, ... with new sweeps (a loop closure)."""
     rng = np.random.default_rng(seed)
     T0 = default_true_pose()
     out = []
-    for i in range(n):
-        yaw = np.deg2rad(yaw_deg * i)
+    for i in range(n + revisit):
+        j = i if i < n else i - n
+        yaw = np.deg2rad(yaw_deg * j)
         q = qmul(q_from_axis_angle([0, 0, 1], yaw), T0[:4])
-        t = T0[4:] + np.array([step * i, 0.35 * np.sin(0.4 * i), 0.0])
+        t = T0[4:] + np.array([step * j, 0.35 * np.sin(0.4 * j), 0.0])
         pose = np.concatenate([q, t])
         pts, _ = make_horizon_sweep(pose, seed=seed * 1000 + i, omega=(0.0, 0.0, 0.0))
         p = np.stack([pts["x"], pts["y"], pts["z"]], 1).astype(np.float64)

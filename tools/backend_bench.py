@@ -1,9 +1,10 @@
 #!/usr/bin/env python
 """The backend's LiDAR step (SURVEY.md §8 f5) on one GPU: device-resident keyframe store + local map + window calls, against the
 same step through the single-keyframe ABI and the 1-thread oracle composition.  Prints one JSON line.
-usage: backend_bench.py [--steps K] [--warmup W] [--dump-outputs DIR] [--global-map [--gm-keyframes 300,2000]]
+usage: backend_bench.py [--steps K] [--warmup W] [--dump-outputs DIR] [--global-map [--gm-keyframes 300,2000]] [--loop]
 --dump-outputs DIR writes the last timed step's layers and blocks of the device-resident leg as DIR/<name>.npy.
---global-map runs the global-map leg instead (publishCompleteMap over the stored full clouds, one JSON line)."""
+--global-map runs the global-map leg instead (publishCompleteMap over the stored full clouds, one JSON line).
+--loop runs the loop-closure leg instead (liliom_loop_align against kf_cloud x2 + icp_align and the oracle, one JSON line)."""
 from __future__ import annotations
 
 import argparse
@@ -295,6 +296,102 @@ def bench_global_map(args):
     print(json.dumps(line), flush=True)
 
 
+LC_HIST = 41           # his_key_frames_ds: 2 * lc_map_width (20) + 1 keyframes (L/src/BackendFusion.cpp:2502-2547)
+LC_LEAF = 0.4          # the loop-closure clouds' VoxelGrid (:2494, :2545)
+
+
+def bench_loop(args):
+    """detectLoopClosure's clouds + performLoopClosure's ICP (L/src/BackendFusion.cpp:2473-2582) on a keyframe sequence whose end
+    revisits its start (synth.make_keyframe_sequence(41, revisit=1)): source = the revisit keyframe, listed with a pose off by
+    2 deg / 0.5 m (the drift a loop closure corrects), target = the 41 history keyframes; leaf 0.4, the reference's ICP settings
+    (:2566-2570).  Three legs:
+    (a) liliom_loop_align on the backend context (one call, both clouds stay on the device);
+    (b) liliom_kf_cloud x2 to the host, then liliom_icp_align on a second context (the composition (a) replaces);
+    (c) the 1-thread oracle composition voxelgrid(concat(transform_cloud(...))) x2 + the NumPy / kd-tree restatement of PCL's
+        loop (tests/test_gpu_widen.py::_icp_numpy), a few calls."""
+    import torch
+    import liliom_b200 as L
+    from liliom_b200 import synth
+    sys.path.insert(0, os.path.join(ROOT, "tests"))
+    import oracle_lib as O
+    from test_gpu_widen import _icp_numpy
+    if not torch.cuda.is_available():
+        raise SystemExit("backend_bench.py needs a CUDA device (no CPU fallback)")
+    name, plim = gpu_card()
+    seq = synth.make_keyframe_sequence(LC_HIST, stride=48, revisit=1)
+    bp = L.backend_default_params(0)
+    c = L.Context(variant=0)
+    for e, s, _ in seq:
+        c.kf_add(bp, e, s, download=False)
+    c2 = L.Context(variant=0)
+    poses = [p for _, _, p in seq]
+    qd = synth.q_from_axis_angle([0.1, -0.1, 1.0], np.deg2rad(2.0))
+    w, x, y, z = qd
+    Rd = np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - w * z), 2 * (x * z + w * y)],
+                   [2 * (x * y + w * z), 1 - 2 * (x * x + z * z), 2 * (y * z - w * x)],
+                   [2 * (x * z - w * y), 2 * (y * z + w * x), 1 - 2 * (x * x + y * y)]])
+    p_src = poses[LC_HIST]
+    src_pose = np.concatenate([synth.qmul(qd, p_src[:4]), Rd @ p_src[4:] + np.array([0.4, -0.25, 0.15])])
+    si, sp = [LC_HIST], [src_pose]
+    ti, tp = list(range(LC_HIST)), poses[:LC_HIST]
+    stride = 48
+
+    def arm_a():
+        return c.loop_align(si, sp, ti, tp, LC_LEAF)
+
+    def arm_b():
+        src = c.kf_cloud(si, sp, LC_LEAF)
+        tgt = c.kf_cloud(ti, tp, LC_LEAF)
+        T, fit, conv, it = c2.icp_align(src, tgt)
+        return T, fit, conv, it, len(src), len(tgt)
+
+    def oracle_cloud(ids, ps):
+        return O.voxelgrid(np.concatenate([O.transform_cloud(np.concatenate([seq[i][0], seq[i][1]]), p) for i, p in zip(ids, ps)]), LC_LEAF)
+
+    def arm_c():
+        src, tgt = oracle_cloud(si, sp), oracle_cloud(ti, tp)
+        f4 = lambda a: np.ascontiguousarray(np.stack([a["x"], a["y"], a["z"], np.ones(len(a), np.float32)], 1))
+        T, fit, conv, it = _icp_numpy(O, f4(src), f4(tgt))
+        return T, fit, conv, it, len(src), len(tgt)
+
+    def timed(fn, n, warm):
+        for _ in range(warm):
+            fn()
+        ms, res = [], None
+        for _ in range(n):
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            res = fn()
+            ms.append((time.perf_counter() - t0) * 1e3)
+        return {"median_ms": float(np.median(ms)), "min_ms": float(np.min(ms)), "max_ms": float(np.max(ms)), "timed_runs": n}, res
+
+    steps = max(1, args.steps)
+    ta, ra = timed(arm_a, steps, max(1, args.warmup))
+    tb, rb = timed(arm_b, steps, max(1, args.warmup))
+    tc, rc = timed(arm_c, 3, 0)
+    n_src, n_tgt = ra[4], ra[5]
+    pts_src = sum(len(seq[i][0]) + len(seq[i][1]) for i in si)
+    pts_tgt = sum(len(seq[i][0]) + len(seq[i][1]) for i in ti)
+    legs = {
+        "a_loop_align": dict(ta, iters=ra[3], converged=bool(ra[2]), fitness=ra[1], cloud_h2d_bytes=0, cloud_d2h_bytes=0),
+        "b_kf_cloud_x2_icp_align_second_context": dict(tb, iters=rb[3], converged=bool(rb[2]), fitness=rb[1],
+                                                        cloud_h2d_bytes=(n_src + n_tgt) * stride, cloud_d2h_bytes=(n_src + n_tgt) * stride),
+        "c_oracle_composition_numpy_icp": dict(tc, iters=rc[3], converged=bool(rc[2]), fitness=rc[1]),
+    }
+    T_err = float(np.abs(rc[0] - ra[0]).max())
+    line = {"metric": "ms per loop closure (both clouds from the keyframe store + ICP)", "workload": "backend_loop_closure", "unit": "ms",
+            "higher_is_better": False, "n_gpus": 1, "gpu": name, "power_limit": plim,
+            "data": f"synthetic: synth.make_keyframe_sequence({LC_HIST}, revisit=1), source 1 keyframe ({pts_src} points in, {n_src} after "
+                    f"VoxelGrid {LC_LEAF}), target {len(ti)} keyframes ({pts_tgt} points in, {n_tgt} after)",
+            "a_b_T16_bit_identical": bool(ra[0].tobytes() == rb[0].tobytes() and ra[1:] == rb[1:]),
+            "a_vs_c_max_abs_T_diff": T_err, "legs": legs,
+            "bytes": "cloud bytes crossing the host link per call (b: both filtered clouds down and up again); not counted: the "
+                     "keyframe tables, the counts and the results, a few kB per call in both legs",
+            "timing": "host wall clock around each call, results on the host"}
+    print(json.dumps(line), flush=True)
+    c.close(); c2.close()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=30)
@@ -302,8 +399,11 @@ def main():
     ap.add_argument("--dump-outputs", default="", metavar="DIR")
     ap.add_argument("--global-map", action="store_true", help="run the global-map leg instead of the LiDAR step")
     ap.add_argument("--gm-keyframes", default="300,2000", help="trajectory lengths of the global-map leg")
+    ap.add_argument("--loop", action="store_true", help="run the loop-closure leg instead of the LiDAR step")
     args = ap.parse_args()
-    if args.global_map:
+    if args.loop:
+        bench_loop(args)
+    elif args.global_map:
         bench_global_map(args)
     else:
         bench_backend(args)
