@@ -116,8 +116,7 @@ static int install_map_from_xyzw(liliom_ctx* c, int m) {
         k_compact_f4<<<cdiv(m, 256), 256, 0, c->stream>>>(c->map.xyzw.as<float4>(), c->flags.as<int>(), c->idx_a.as<int>(), m, c->map_ds.as<float4>());
         LILI_TRY(launch_check(c, "k_compact_f4"));
         int local = 0;
-        LILI_CUDA(c, cudaMemcpyAsync(&local, c->idx_a.as<int>() + m, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+        LILI_TRY(read_back(c, {{&local, c->idx_a.as<int>() + m, sizeof(int)}}));
         LILI_CUDA(c, cudaMemcpyAsync(c->map.xyzw.p, c->map_ds.p, (size_t)local * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
         m = local;
     }
@@ -196,20 +195,17 @@ extern "C" int liliom_create(liliom_ctx** out, const liliom_params* p, int devic
     if (!c) return LILIOM_E_ARG;
     c->prm = *p;
     c->device = device;
-    LILI_CUDA(c, cudaSetDevice(device));
+    cudaError_t e = cudaSetDevice(device);
     cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) c->sm_count = prop.multiProcessorCount;
-    cudaError_t e = cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking);
-    if (e != cudaSuccess) { delete c; return LILIOM_E_CUDA; }
+    if (e == cudaSuccess && cudaGetDeviceProperties(&prop, device) == cudaSuccess) c->sm_count = prop.multiProcessorCount;
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking);
     c->stream = c->own_stream;
-    if (cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&c->ev_ready, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&c->ev_copied, cudaEventDisableTiming) != cudaSuccess) {
-        cudaStreamDestroy(c->own_stream); delete c; return LILIOM_E_CUDA;
-    }
+    if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_ready, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_copied, cudaEventDisableTiming);
     c->h_pin_bytes = sizeof(PinBlock) + (1 << 20);      // the header + 1 MiB of per-iteration stats (3276 iterations)
-    e = cudaHostAlloc((void**)&c->h_pin, c->h_pin_bytes, cudaHostAllocDefault);
-    if (e != cudaSuccess) { cudaStreamDestroy(c->own_stream); delete c; return LILIOM_E_CUDA; }
+    if (e == cudaSuccess) e = cudaHostAlloc((void**)&c->h_pin, c->h_pin_bytes, cudaHostAllocDefault);
+    if (e != cudaSuccess) { liliom_destroy(c); return LILIOM_E_CUDA; }      // tears down whatever was created
     // the GN kernel writes its results straight into this block when the device can address it (UVA: always, in practice)
     if (cudaHostGetDevicePointer((void**)&c->h_pin_dev, c->h_pin, 0) != cudaSuccess) { c->h_pin_dev = nullptr; (void)cudaGetLastError(); }
     if (const char* e1 = getenv("LILIOM_KNN_LANES")) { int v = atoi(e1); if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) c->force_lanes = v; }
@@ -230,26 +226,15 @@ extern "C" int liliom_create(liliom_ctx** out, const liliom_params* p, int devic
 extern "C" void liliom_destroy(liliom_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
-    cudaStreamSynchronize(c->stream);
+    if (c->stream) cudaStreamSynchronize(c->stream);
     nccl_destroy(c);
-    DevBuf* bufs[] = {&c->raw, &c->cut, &c->surf, &c->edge, &c->flags, &c->scan_tmp, &c->idx_a, &c->idx_b, &c->hz_mat, &c->hz_stage_surf,
-                      &c->hz_stage_edge, &c->hz_counts, &c->rot_keys, &c->rot_keys2, &c->rot_vals, &c->rot_vals2, &c->rot_cloud, &c->rot_curv,
-                      &c->rot_label, &c->rot_picked, &c->rot_sort, &c->rot_ring, &c->rot_meta, &c->rot_lessflat, &c->rot_seg_edge, &c->vg_keys,
-                      &c->vg_keys2, &c->vg_vals, &c->vg_vals2, &c->vg_flags, &c->vg_rank, &c->vg_params, &c->vg_out, &c->vg_minmax, &c->vg_count,
-                      &c->cub_tmp, &c->vg_coop, &c->hz_ctl, &c->map_raw, &c->map_ds, &c->map.xyzw, &c->map.sorted, &c->map.cell_start, &c->grid_keys, &c->grid_keys2,
-                      &c->grid_vals, &c->grid_vals2, &c->feats, &c->corr_valid, &c->corr_plane, &c->nn_idx, &c->nn_sqd, &c->pose_dev,
-                      &c->partials, &c->neq, &c->stats_dev, &c->counter, &c->lm_state, &c->raw_scan, &c->map.refl, &c->livox_in, &c->qstate, &c->inc_key[0], &c->inc_key[1], &c->inc_ref[0], &c->inc_ref[1], &c->inc_newkey[0], &c->inc_newkey[1],
-                      &c->inc_newref[0], &c->inc_newref[1], &c->inc_removed, &c->inc_rpos, &c->inc_flags, &c->inc_rank, &c->inc_bad, &c->icp_ctl};
-    for (DevBuf* b : bufs) b->release();
-    backend_release(c);
-    for (auto& f : c->frames) f.buf.release();
     for (cudaEvent_t e : c->ev_pool) cudaEventDestroy(e);
     if (c->h_pin) cudaFreeHost(c->h_pin);
     if (c->ev_ready) cudaEventDestroy(c->ev_ready);
     if (c->ev_copied) cudaEventDestroy(c->ev_copied);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
-    delete c;
+    delete c;      // the device buffers (DevBuf members, frames, indices) free themselves here, with the device still current
 }
 
 // ===================== L1 =====================
@@ -382,19 +367,16 @@ extern "C" int liliom_voxelgrid(liliom_ctx* c, const void* pts, int n, int strid
     LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, pts, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
     bool coop = false;
     LILI_TRY(voxelgrid_coop(c, c->raw.p, n, nullptr, stride, leaf, c->vg_out.p, c->vg_count.as<int>(), nullptr, &coop));
-    PinBlock* hp = c->h_pin;
+    int m = 0;
     if (coop) {      // the cooperative filter may decline the input: its verdict comes back with the count
-        LILI_CUDA(c, cudaMemcpyAsync(&hp->vg_count, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaMemcpyAsync(&hp->vgp, c->vg_params.p, sizeof(VgParams), cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-        if (hp->vgp.bail) coop = false;
+        VgParams vp;
+        LILI_TRY(read_back(c, {{&m, c->vg_count.p, sizeof(int)}, {&vp, c->vg_params.p, sizeof(VgParams)}}));
+        if (vp.bail) coop = false;
     }
     if (!coop) {
         LILI_TRY(voxelgrid_dev(c, c->raw.p, n, nullptr, stride, leaf, c->vg_out.p, c->vg_count.as<int>()));
-        LILI_CUDA(c, cudaMemcpyAsync(&hp->vg_count, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+        LILI_TRY(read_back(c, {{&m, c->vg_count.p, sizeof(int)}}));
     }
-    const int m = hp->vg_count;
     if (out && m > cap) return LILIOM_E_CAPACITY;
     if (out && m) {
         LILI_CUDA(c, cudaMemcpyAsync(out, c->vg_out.p, (size_t)m * stride, cudaMemcpyDeviceToHost, c->stream));
@@ -423,7 +405,6 @@ extern "C" int liliom_undistort(liliom_ctx* c, void* pts_inout, int n, const dou
 // ===================== L2: map =====================
 extern "C" int liliom_map_clear(liliom_ctx* c) {
     if (!c) return LILIOM_E_ARG;
-    for (auto& f : c->frames) f.buf.release();
     c->frames.clear();
     c->inc_valid = false;
     c->map.ready = false; c->map.n = 0; c->map_n_global = 0;
@@ -437,7 +418,7 @@ static int push_frame_from_device(liliom_ctx* c, const void* d_src, int n, const
     Frame f;
     f.slot = (int)c->frames.size();
     if ((int)c->frames.size() >= c->prm.max_map_frames && !c->frames.empty()) {      // L/src/LidarOdometry.cpp:293-296 pop_front
-        f.buf = c->frames.front().buf;          // the popped frame's allocation is recycled: cudaFree + cudaMalloc per scan cost
+        f.buf = std::move(c->frames.front().buf);   // the popped frame's allocation is recycled: cudaFree + cudaMalloc per scan cost
         f.slot = c->frames.front().slot;        // more than the whole map maintenance of a 10 M-point map (cudaFree synchronises)
         c->frames.erase(c->frames.begin());
     }
@@ -452,10 +433,7 @@ static int push_frame_from_device(liliom_ctx* c, const void* d_src, int n, const
                 k_transform_cloud<<<cdiv(n, 256), 256, 0, c->stream>>>((const unsigned char*)d_src, n, stride, q, t, (unsigned char*)f.buf.p);
                 LILI_TRY(launch_check(c, "k_transform_cloud"));
                 LILI_TRY(vg_minmax_dev(c, f.buf.p, n, nullptr, stride));                 // the frame's box, for the rebuilds it takes part in
-                LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->box, c->vg_minmax.p, 7 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-                LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-                for (int k = 0; k < 7; ++k) f.mm[k] = c->h_pin->box[k];
-                return LILIOM_OK;
+                return read_back(c, {{f.mm, c->vg_minmax.p, 7 * sizeof(int)}});
             }
             // sharded map maintenance: every rank receives the frame, keeps the points within (search radius + one voxel
             // diagonal) of a block it owns — every voxel that can reach an owned query's 1 m ball is then complete locally —
@@ -473,17 +451,12 @@ static int push_frame_from_device(liliom_ctx* c, const void* d_src, int n, const
                                                                   (unsigned char*)f.buf.p);
             LILI_TRY(launch_check(c, "k_compact_strided"));
             LILI_TRY(vg_minmax_dev(c, f.buf.p, n, c->idx_a.as<int>() + n, stride));     // box of the points this rank keeps
-            LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->kept, c->idx_a.as<int>() + n, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-            LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->box, c->vg_minmax.p, 7 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-            LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-            f.n = c->h_pin->kept;
-            for (int k = 0; k < 7; ++k) f.mm[k] = c->h_pin->box[k];
-            return LILIOM_OK;
+            return read_back(c, {{&f.n, c->idx_a.as<int>() + n, sizeof(int)}, {f.mm, c->vg_minmax.p, 7 * sizeof(int)}});
         };
         rc = body();
     }
-    if (rc != LILIOM_OK) { f.buf.release(); return rc; }      // no leak on the error paths (DevBuf has no destructor)
-    c->frames.push_back(f);
+    if (rc != LILIOM_OK) return rc;
+    c->frames.push_back(std::move(f));
     return LILIOM_OK;
 }
 
@@ -570,13 +543,7 @@ extern "C" int liliom_map_download_cloud(liliom_ctx* c, void* out, int cap, int*
     if (!c || !m_out) return LILIOM_E_ARG;
     LILI_CUDA(c, cudaSetDevice(c->device));
     if (c->nranks > 1) { c->last_error = "liliom_map_download_cloud is single-GPU"; return LILIOM_E_ARG; }
-    const int m = c->map_n_global;
-    *m_out = m;
-    if (!out) return LILIOM_OK;
-    if (m > cap) return LILIOM_E_CAPACITY;
-    if (m) LILI_CUDA(c, cudaMemcpyAsync(out, c->map_ds.p, (size_t)m * c->prm.point_stride, cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    return LILIOM_OK;
+    return download_sized(c, c->map_ds, c->map_n_global, c->prm.point_stride, out, cap, m_out);
 }
 
 extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
@@ -628,9 +595,7 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
         // of the real-size streamed lifecycle — not kept.)
         LILI_TRY(voxelgrid_dev(c, c->map_raw.p, (int)total, nullptr, stride, c->prm.leaf_map, c->map_ds.p, c->vg_count.as<int>(),   // :316-317
                                c->nranks == 1 ? c->map.xyzw.as<float4>() : nullptr, 32, box));
-        LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->vg_count, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-        m = c->h_pin->vg_count;
+        LILI_TRY(read_back(c, {{&m, c->vg_count.p, sizeof(int)}}));
     }
     mark();      // [2] VoxelGrid
     LILI_CUDA(c, c->map.xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
@@ -651,9 +616,7 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
                 k_compact_repack<<<cdiv(m, 256), 256, 0, c->stream>>>((const unsigned char*)c->map_ds.p, c->flags.as<int>(), c->idx_a.as<int>(), m, stride,
                                                                      c->map.xyzw.as<float4>());
                 LILI_TRY(launch_check(c, "k_compact_repack"));
-                LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->kept, c->idx_a.as<int>() + m, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-                LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-                local = c->h_pin->kept;
+                LILI_TRY(read_back(c, {{&local, c->idx_a.as<int>() + m, sizeof(int)}}));
             }
             return grid_build(c, local, box[6] > 0 ? box : nullptr);
         };
@@ -729,13 +692,7 @@ extern "C" int liliom_map_size(const liliom_ctx* c) { return c ? c->map.n : 0; }
 extern "C" int liliom_map_download(liliom_ctx* c, liliom_f4* out, int cap, int* m_out) {
     if (!c || !m_out) return LILIOM_E_ARG;
     LILI_CUDA(c, cudaSetDevice(c->device));
-    const int m = c->map.n;
-    *m_out = m;
-    if (!out) return LILIOM_OK;
-    if (m > cap) return LILIOM_E_CAPACITY;
-    if (m) LILI_CUDA(c, cudaMemcpyAsync(out, c->map.xyzw.p, (size_t)m * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    return LILIOM_OK;
+    return download_sized(c, c->map.xyzw, c->map.n, sizeof(float4), out, cap, m_out);
 }
 
 // ===================== L2: scan-to-map =====================
@@ -862,9 +819,9 @@ static int odometry_on_resident_surf(liliom_ctx* c, double pose7[7], int match_c
         c->vg_check = false;
     } else {   // still report surf_last_ds: read the count back
         if (c->d_nfeats) {
-            LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->vg_count, c->d_nfeats, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-            LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-            c->n_feats_actual = min(c->h_pin->vg_count, n_max);
+            int nq = 0;
+            LILI_TRY(read_back(c, {{&nq, c->d_nfeats, sizeof(int)}}));
+            c->n_feats_actual = min(nq, n_max);
         } else c->n_feats_actual = n_max;
     }
     c->d_nfeats = nullptr;

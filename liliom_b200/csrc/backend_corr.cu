@@ -345,15 +345,9 @@ static int backend_block_run(liliom_ctx* c, const std::vector<BlkSeg>& segs, Blk
     LILI_TRY(launch_check(c, "k_backend_block"));
     k_backend_block_sum<<<nseg, 32, 0, c->stream>>>(c->win_tab.as<BlkSeg>(), a.partials, c->neq.as<double>());
     LILI_TRY(launch_check(c, "k_backend_block_sum"));
-    if (nseg == 1) {    // the pinned block's 29 sums
-        double* hp = c->h_pin->s2m.neq;
-        LILI_CUDA(c, cudaMemcpyAsync(hp, c->neq.p, kNormEq * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-        for (int k = 0; k < kNormEq; ++k) out[k] = hp[k];
-    } else {
-        LILI_CUDA(c, cudaMemcpyAsync(out, c->neq.p, (size_t)nseg * kNormEq * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    }
+    if (nseg == 1) return read_back(c, {{out, c->neq.p, kNormEq * sizeof(double)}});     // the 29 sums through pinned memory
+    LILI_CUDA(c, cudaMemcpyAsync(out, c->neq.p, (size_t)nseg * kNormEq * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     return LILIOM_OK;
 }
 
@@ -544,9 +538,9 @@ extern "C" int liliom_backend_window_correspond(liliom_ctx* c, const liliom_back
     for (int i = 0; i <= k; ++i) { ca.start[0][i] = ae.start[i]; ca.start[1][i] = as.start[i]; }
     k_win_count<<<dim3(k, 2), 256, 0, c->stream>>>(ca);
     LILI_TRY(launch_check(c, "k_win_count"));
-    LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, c->win_cnt.p, 2 * kWinMax * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    for (int i = 0; i < k; ++i) { n_edge_corr[i] = c->h_pin->bk_cnt[i]; n_surf_corr[i] = c->h_pin->bk_cnt[kWinMax + i]; }
+    int cnt[2 * kWinMax];
+    LILI_TRY(read_back(c, {{cnt, c->win_cnt.p, sizeof(cnt)}}));
+    for (int i = 0; i < k; ++i) { n_edge_corr[i] = cnt[i]; n_surf_corr[i] = cnt[kWinMax + i]; }
     c->win_ids.assign(kf_ids, kf_ids + k);
     c->win_qoff[0].assign(ae.start, ae.start + k + 1);
     c->win_qoff[1].assign(as.start, as.start + k + 1);

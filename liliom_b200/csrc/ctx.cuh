@@ -5,6 +5,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <initializer_list>
 #include <string>
 #include <vector>
 #include "../../include/liliom.h"
@@ -12,11 +13,21 @@
 
 namespace lili {
 
-// One growable device allocation.  Buffers only grow; 80 GB of HBM3 per GPU (a 10 M-point map needs well under 1 GB)
-// makes reallocation-on-demand a cold path (first scan), never a steady-state cost.
+// One growable device allocation, owned: freed by the destructor, moved (never copied) between owners.  Buffers only grow;
+// 80 GB of HBM3 per GPU (a 10 M-point map needs well under 1 GB) makes reallocation-on-demand a cold path (first scan),
+// never a steady-state cost.
 struct DevBuf {
     void*  p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    DevBuf(DevBuf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+    DevBuf& operator=(DevBuf&& o) noexcept {
+        if (this != &o) { release(); p = o.p; cap = o.cap; o.p = nullptr; o.cap = 0; }
+        return *this;
+    }
+    ~DevBuf() { release(); }
     cudaError_t ensure(size_t bytes) {
         if (bytes <= cap) return cudaSuccess;
         if (p) cudaFree(p);
@@ -48,7 +59,6 @@ struct MapIndex {
     GridDesc grid{};
     int  n = 0;                          // points resident on this rank (sorted grid)
     bool ready = false;
-    void release() { xyzw.release(); refl.release(); sorted.release(); cell_start.release(); n = 0; ready = false; }
 };
 
 // Cell edge for a squared-distance gate: the smallest power of two whose square reaches it (1.0 for the reference's gates).
@@ -91,22 +101,15 @@ struct PinIcp {                // ICP results (icp.cu), stored by the last block
 // The context's small pinned host block (liliom_ctx::h_pin): disjoint members, each read after its user's stream synchronise.
 struct PinResult {             // scan-to-map results: stored by the persistent GN kernel through GnIo::host_out, or copied
     double pose[8];            // pose (wxyz, t) + peer-loss flag
-    double neq[kNormEq];       // the 29 sums of the last pass (also the backend correspondence kernels' sums)
+    double neq[kNormEq];       // the 29 sums of the last pass
     int    n_feats;            // device-side query count
     VgParams vgp;              // parameters of the scan's VoxelGrid (speculation check)
 };
 struct PinBlock {
-    int    extract[9];         // extractor counts: Horizon {surf, edge, cut}; rotating {meta[8], surf}
     PinResult s2m;
     double pose_stage[8];      // scan-to-map start pose + cleared peer-loss flag, copied to the device for per-pass launches
-    int    vg_count;           // output count of a VoxelGrid or of the map's incremental filter
-    VgParams vgp;              // liliom_voxelgrid: the cooperative filter's verdict
-    int    kept;               // points a shard filter kept (pushed frame, map rebuild)
-    int    box[8];             // a pushed frame's box (k_vg_minmax), a map's box (grid_build), or the incremental map's key flag (k_inc_keys)
-    int    escaped;            // grid_build: a point lies outside the handed-in box
     double map_status[4];      // multi-rank map rebuild: {owned voxels, failed} out, their sums over the ranks back
-    unsigned long long block27[2];   // block27_stats: queries, points in their cell blocks
-    int    bk_cnt[2 * 16];     // backend: VoxelGrid output counts (keyframe store, local map), window correspondence counts [kind][16]
+    alignas(16) unsigned char scratch[kNormEq * sizeof(double)];   // read_back(); its largest user: the backend's 29 sums
     PinIcp icp;                // ICP: the results of k_icp_persistent
     double stats[];         // kStatsDoubles per GN iteration, up to the end of the block (h_pin_bytes)
 };
@@ -309,6 +312,38 @@ inline int launch_check(liliom_ctx* c, const char* name) {
 
 inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// One read-back of a few device words: every range is copied into the pinned block's scratch region, the stream is synchronised
+// once, and the bytes land in the range's host destination.  The scratch region is never read after the call returns.
+struct ReadBack { void* dst; const void* src; size_t bytes; };
+inline int read_back(liliom_ctx* c, std::initializer_list<ReadBack> parts) {
+    unsigned char* s = c->h_pin->scratch;
+    size_t off = 0;
+    for (const ReadBack& r : parts) {
+        if (off + r.bytes > sizeof(PinBlock::scratch)) { c->last_error = "read_back: larger than the pinned scratch region"; return LILIOM_E_ARG; }
+        LILI_CUDA(c, cudaMemcpyAsync(s + off, r.src, r.bytes, cudaMemcpyDeviceToHost, c->stream));
+        off += r.bytes;
+    }
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    off = 0;
+    for (const ReadBack& r : parts) { memcpy(r.dst, s + off, r.bytes); off += r.bytes; }
+    return LILIOM_OK;
+}
+
+// The caller-buffer contract of the download entry points: *n_out = m; out == NULL is a size query; m > cap gives
+// LILIOM_E_CAPACITY and leaves out untouched; otherwise fill() runs (the work that produces the m items, if any is left) and
+// m * elem bytes of src are copied and the stream synchronised.
+struct NoFill { int operator()() const { return LILIOM_OK; } };
+template <class Fill = NoFill>
+int download_sized(liliom_ctx* c, const DevBuf& src, int m, size_t elem, void* out, int cap, int* n_out, Fill fill = {}) {
+    *n_out = m;
+    if (!out) return LILIOM_OK;
+    if (m > cap) return LILIOM_E_CAPACITY;
+    LILI_TRY(fill());
+    if (m) LILI_CUDA(c, cudaMemcpyAsync(out, src.p, (size_t)m * elem, cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    return LILIOM_OK;
+}
+
 // ---- modules (implemented in the .cu files) ----
 int sort_pairs_u32(liliom_ctx* c, const uint32_t* kin, uint32_t* kout, const int* vin, int* vout, int n, int end_bit);
 int sort_pairs_u64(liliom_ctx* c, const unsigned long long* kin, unsigned long long* kout, const int* vin, int* vout, int n, int end_bit);
@@ -349,7 +384,5 @@ void frames_box(const liliom_ctx* c, int mm[7]);                                
 int block27_stats(liliom_ctx* c, const double pose7[7], unsigned long long out[2]);   // grid_knn.cu
 
 int repack_to_f4(liliom_ctx* c, const void* d_in, int n, int stride, float4* d_out, const int* d_n = nullptr);
-
-void backend_release(liliom_ctx* c);                                                  // keyframes.cu: the backend's device buffers
 
 }  // namespace lili

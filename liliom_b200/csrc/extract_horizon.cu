@@ -517,10 +517,8 @@ int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf
         *n_surf = *n_edge = *n_cut = -1;
         return LILIOM_OK;
     }
-    int* hp = c->h_pin->extract;
-    LILI_CUDA(c, cudaMemcpyAsync(hp, totals, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaMemcpyAsync(hp + 2, cidx + n, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    int hp[3];
+    LILI_TRY(read_back(c, {{hp, totals, 2 * sizeof(int)}, {hp + 2, cidx + n, sizeof(int)}}));
     *n_surf = hp[0]; *n_edge = hp[1]; *n_cut = hp[2];
     c->n_surf_dev = hp[0];
     return LILIOM_OK;

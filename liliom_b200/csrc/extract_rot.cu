@@ -632,10 +632,8 @@ int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_
     k_rot_lf_centroid<<<cdiv(n, 128), 128, 0, c->stream>>>(cloud, lf_src, k64b, vals2, c->vg_flags.as<int>(), c->vg_rank.as<int>(), meta, n,
                                                            c->surf.as<Pt32>(), c->vg_count.as<int>());
     LILI_TRY(launch_check(c, "k_rot_lf_centroid"));
-    int* hp = c->h_pin->extract;
-    LILI_CUDA(c, cudaMemcpyAsync(hp, meta, 8 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaMemcpyAsync(hp + 8, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    int hp[9];
+    LILI_TRY(read_back(c, {{hp, meta, 8 * sizeof(int)}, {hp + 8, c->vg_count.p, sizeof(int)}}));
     if (hp[M_ERR]) { c->last_error = "ring/segment larger than the shared-memory capacity (16384 / 4096 points)"; return LILIOM_E_CAPACITY; }
     *n_cut = hp[M_NVALID]; *n_edge = hp[M_NEDGE]; *n_surf = hp[8];
     c->n_surf_dev = hp[8];

@@ -107,9 +107,8 @@ int grid_build(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_b
         LILI_CUDA(c, cudaMemsetAsync(escaped, 0, sizeof(int), c->stream));
     } else {
         LILI_TRY(vg_minmax_dev(c, pts, m, nullptr, sizeof(float4)));
-        int* hb = c->h_pin->box;
-        LILI_CUDA(c, cudaMemcpyAsync(hb, c->vg_minmax.p, kBoxInts * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+        int hb[kBoxInts];
+        LILI_TRY(read_back(c, {{hb, c->vg_minmax.p, sizeof(hb)}}));
         if (hb[6] < m) { c->last_error = "non-finite map point"; return LILIOM_E_ARG; }      // the box counts finite points only
         for (int k = 0; k < 6; ++k) h[k] = hb[k];
     }
@@ -145,9 +144,9 @@ int grid_build(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_b
     LILI_TRY(launch_check(c, "k_cell_run_ends"));
     LILI_TRY(inclusive_max_scan_i32(c, mi.cell_start.as<int>(), g.ncells + 1));
     if (escaped) {
-        LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->escaped, escaped, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-        if (c->h_pin->escaped) return grid_build(c, mi, cell, m, nullptr);
+        int esc = 0;
+        LILI_TRY(read_back(c, {{&esc, escaped, sizeof(int)}}));
+        if (esc) return grid_build(c, mi, cell, m, nullptr);
     }
     mi.ready = true;
     return LILIOM_OK;
@@ -987,11 +986,7 @@ int block27_stats(liliom_ctx* c, const double pose7[7], unsigned long long out[2
     k_block27_count<<<min(cdiv(n, 256), c->sm_count * 4), 256, 0, c->stream>>>(c->feats.as<float4>(), n, q, t, c->map.cell_start.as<int>(), c->map.grid,
                                                                               c->nranks, c->rank, c->shard_inv_block, d);
     LILI_TRY(launch_check(c, "k_block27_count"));
-    unsigned long long* hp = c->h_pin->block27;
-    LILI_CUDA(c, cudaMemcpyAsync(hp, d, 16, cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    out[0] = hp[0]; out[1] = hp[1];
-    return LILIOM_OK;
+    return read_back(c, {{out, d, 16}});
 }
 
 // ------------------------------------------------------------------ host orchestration

@@ -78,14 +78,6 @@ __global__ void k_kf_refl(const unsigned char* __restrict__ pts, int n, float* _
     if (i < n) out[i] = reinterpret_cast<const float*>(pts + (size_t)i * 48)[9];
 }
 
-void backend_release(liliom_ctx* c) {
-    DevBuf* bufs[] = {&c->kf_arena, &c->kf_full, &c->kf_tab, &c->bmap_raw, &c->bmap_ds[0], &c->bmap_ds[1], &c->win_valid[0], &c->win_valid[1],
-                      &c->win_line, &c->win_plane, &c->win_score, &c->win_cnt, &c->win_tab, &c->loop_src};
-    for (DevBuf* b : bufs) b->release();
-    c->bmap[0].release(); c->bmap[1].release();
-    c->loop.release();
-}
-
 // Room for `pts` points in `arena`, of which the first `used` are stored.  Grows geometrically and COPIES the stored points
 // (DevBuf::ensure would discard them); the cudaFree of the old block synchronises, which only happens on growth.
 // The store has two arenas: kf_arena (the down-sampled edge/surf clouds, ~2k points per keyframe) and kf_full (the full clouds,
@@ -94,16 +86,15 @@ static int kf_reserve(liliom_ctx* c, DevBuf& arena, long long used, long long pt
     const size_t stride = (size_t)c->prm.point_stride;
     const size_t need = (size_t)pts * stride;
     if (need <= arena.cap) return LILIOM_OK;
-    size_t want = std::max(need + need / 2, std::max(arena.cap * 2, (size_t)1 << 20));
-    void* p = nullptr;
-    LILI_CUDA(c, cudaMalloc(&p, want));
+    const size_t want = std::max(need + need / 2, std::max(arena.cap * 2, (size_t)1 << 20));
+    DevBuf grown;
+    LILI_CUDA(c, cudaMalloc(&grown.p, want));
+    grown.cap = want;
     if (used > 0) {
-        const cudaError_t e = cudaMemcpyAsync(p, arena.p, (size_t)used * stride, cudaMemcpyDeviceToDevice, c->stream);
-        if (e != cudaSuccess) { cudaFree(p); return fail_cuda(c, e, "kf_reserve copy"); }
+        LILI_CUDA(c, cudaMemcpyAsync(grown.p, arena.p, (size_t)used * stride, cudaMemcpyDeviceToDevice, c->stream));
         LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     }
-    arena.release();
-    arena.p = p; arena.cap = want;
+    arena = std::move(grown);
     return LILIOM_OK;
 }
 
@@ -220,9 +211,9 @@ extern "C" int liliom_kf_add(liliom_ctx* c, const liliom_backend_params* bp, con
     int* cnt = c->vg_count.as<int>();
     LILI_TRY(voxelgrid_dev(c, raw, n_edge, nullptr, stride, bp->edge_leaf, tail, cnt));                                           // :1502-1507
     LILI_TRY(voxelgrid_dev(c, raw + (size_t)n_edge * stride, n_surf, nullptr, stride, bp->surf_leaf, c->vg_out.p, cnt + 1));     // :1509-1514
-    LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, cnt, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    const int me = c->h_pin->bk_cnt[0], ms = c->h_pin->bk_cnt[1];
+    int m[2];
+    LILI_TRY(read_back(c, {{m, cnt, sizeof(m)}}));
+    const int me = m[0], ms = m[1];
     if (n_edge_ds) *n_edge_ds = me;
     if (n_surf_ds) *n_surf_ds = ms;
     if ((edge_ds_out && me > edge_cap) || (surf_ds_out && ms > surf_cap)) return LILIOM_E_CAPACITY;   // nothing stored
@@ -280,9 +271,8 @@ extern "C" int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp,
         LILI_CUDA(c, c->bmap[l].xyzw.ensure((size_t)std::max(nl[l], 1LL) * sizeof(float4)));
         LILI_TRY(voxelgrid_dev(c, src[l], (int)nl[l], nullptr, stride, leaf[l], c->bmap_ds[l].p, cnt + l, c->bmap[l].xyzw.as<float4>()));
     }
-    LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, cnt, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    const int m[2] = {c->h_pin->bk_cnt[0], c->h_pin->bk_cnt[1]};
+    int m[2];
+    LILI_TRY(read_back(c, {{m, cnt, sizeof(m)}}));
     LILI_TRY(grid_build(c, c->bmap[0], gate_cell(1.0), m[0]));                 // :1543 sqdist[4] < 1.0
     LILI_TRY(grid_build(c, c->bmap[1], gate_cell(bp->kd_max_radius), m[1]));   // :1615 sqdist[4] < kd_max_radius
     if (stride == 48) {                                                         // reflectivity of the surf layer (:1617-1638)
@@ -304,13 +294,7 @@ extern "C" int liliom_bmap_download(liliom_ctx* c, int layer, void* out, int cap
     if (!c || !m_out || (layer != 0 && layer != 1)) return LILIOM_E_ARG;
     if (!c->bmap_built) return LILIOM_E_NOMAP;
     LILI_CUDA(c, cudaSetDevice(c->device));
-    const int m = c->bmap_n[layer];
-    *m_out = m;
-    if (!out) return LILIOM_OK;
-    if (m > cap) return LILIOM_E_CAPACITY;
-    if (m) LILI_CUDA(c, cudaMemcpyAsync(out, c->bmap_ds[layer].p, (size_t)m * c->prm.point_stride, cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    return LILIOM_OK;
+    return download_sized(c, c->bmap_ds[layer], c->bmap_n[layer], c->prm.point_stride, out, cap, m_out);
 }
 
 extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, float leaf, void* out, int cap, int* n_out) {
@@ -324,15 +308,9 @@ extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* p
     long long off = 0;
     LILI_TRY(kf_cloud_dev(c, kf_ids, poses7, k, leaf, c->vg_count.as<int>(), &off));
     if (off == 0) return LILIOM_OK;
-    LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    const int m = c->h_pin->bk_cnt[0];
-    *n_out = m;
-    if (!out) return LILIOM_OK;
-    if (m > cap) return LILIOM_E_CAPACITY;
-    if (m) LILI_CUDA(c, cudaMemcpyAsync(out, c->vg_out.p, (size_t)m * stride, cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    return LILIOM_OK;
+    int m = 0;
+    LILI_TRY(read_back(c, {{&m, c->vg_count.p, sizeof(int)}}));
+    return download_sized(c, c->vg_out, m, stride, out, cap, n_out);
 }
 
 // detectLoopClosure + performLoopClosure's alignment (:2473-2582) without leaving the device: the history cloud goes into the
@@ -360,9 +338,9 @@ extern "C" int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double
     LILI_TRY(kf_cloud_dev(c, src_ids, src_poses7, k_src, leaf, cnt + 1, &off_s));
     LILI_CUDA(c, c->loop_src.ensure((size_t)std::max(off_s, 1LL) * sizeof(float4)));
     LILI_TRY(repack_to_f4(c, c->vg_out.p, (int)off_s, stride, c->loop_src.as<float4>(), cnt + 1));
-    LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, cnt, 2 * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    const int m_t = off_t ? c->h_pin->bk_cnt[0] : 0, m_s = off_s ? c->h_pin->bk_cnt[1] : 0;
+    int m[2];
+    LILI_TRY(read_back(c, {{m, cnt, sizeof(m)}}));
+    const int m_t = off_t ? m[0] : 0, m_s = off_s ? m[1] : 0;
     if (n_src) *n_src = m_s;
     if (n_tgt) *n_tgt = m_t;
     LILI_TRY(grid_build(c, c->loop, gate_cell(c->prm.knn_max_sqdist), m_t));      // the cell of liliom_icp_align's target
@@ -390,9 +368,7 @@ extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp
         LILI_CUDA(c, c->vg_count.ensure(16));
         LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, full, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
         LILI_TRY(voxelgrid_dev(c, c->raw.p, n, nullptr, stride, bp->surf_leaf, tail, c->vg_count.as<int>()));
-        LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-        m = c->h_pin->bk_cnt[0];
+        LILI_TRY(read_back(c, {{&m, c->vg_count.p, sizeof(int)}}));
     }
     c->kfs[kf_id].full_off = c->kf_full_used;
     c->kfs[kf_id].n_full = m;
@@ -440,25 +416,19 @@ extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, con
     // box of the transformed concatenation (pcl::getMinMax3D), read back: the overflow test and the key width are decided here
     LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
     int* mm = c->vg_minmax.as<int>();
-    for (int w = 0; w < kBoxInts; ++w) c->h_pin->box[w] = vg_box_empty(w);
-    LILI_CUDA(c, cudaMemcpyAsync(mm, c->h_pin->box, kBoxInts * sizeof(int), cudaMemcpyHostToDevice, c->stream));
+    int* empty = reinterpret_cast<int*>(c->h_pin->scratch);       // pinned staging of the empty box; the stream orders the read-back after it
+    for (int w = 0; w < kBoxInts; ++w) empty[w] = vg_box_empty(w);
+    LILI_CUDA(c, cudaMemcpyAsync(mm, empty, kBoxInts * sizeof(int), cudaMemcpyHostToDevice, c->stream));
     k_kf_box<<<kf_row_grid(tab.size(), largest, 8, 1024), 256, 0, c->stream>>>(arena, d_tab, rows, stride, mm);
     LILI_TRY(launch_check(c, "k_kf_box"));
-    LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->box, mm, kBoxInts * sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     int box[kBoxInts];
-    memcpy(box, c->h_pin->box, sizeof(box));
+    LILI_TRY(read_back(c, {{box, mm, sizeof(box)}}));
     const VgParams p = vg_params(box, leaf);
-    if (p.overflow) {                                             // PCL declines the filter and publishes its input
-        if (!out) { *n = (int)N; return LILIOM_OK; }
-        if (N > cap) { *n = (int)N; return LILIOM_E_CAPACITY; }
-        LILI_CUDA(c, c->vg_out.ensure((size_t)N * stride));
-        LILI_TRY(kf_gather(c, arena, tab, largest, c->vg_out.p));
-        LILI_CUDA(c, cudaMemcpyAsync(out, c->vg_out.p, (size_t)N * stride, cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-        *n = (int)N;
-        return LILIOM_OK;
-    }
+    if (p.overflow)                                               // PCL declines the filter and publishes its input
+        return download_sized(c, c->vg_out, (int)N, stride, out, cap, n, [&]() -> int {
+            LILI_CUDA(c, c->vg_out.ensure((size_t)N * stride));
+            return kf_gather(c, arena, tab, largest, c->vg_out.p);
+        });
     const int n_fin = p.n_finite;
     if (n_fin == 0) { *n = 0; return LILIOM_OK; }
     LILI_CUDA(c, c->vg_keys.ensure((size_t)N * 4));
@@ -476,21 +446,16 @@ extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, con
     k_vg_heads<<<cdiv(n_fin + 1LL, 256), 256, 0, c->stream>>>(c->vg_keys2.as<uint32_t>(), n_fin, nullptr, c->vg_flags.as<int>());
     LILI_TRY(launch_check(c, "k_vg_heads"));
     LILI_TRY(exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin));
-    LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->bk_cnt, c->vg_rank.as<int>() + n_fin, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    const int m = c->h_pin->bk_cnt[0];
-    *n = m;
-    if (!out) return LILIOM_OK;
-    if (m > cap) return LILIOM_E_CAPACITY;
-    LILI_CUDA(c, c->vg_out.ensure((size_t)m * stride));
-    if (stride == 48)
-        k_kf_centroid<48><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(),
-                                                                   c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
-    else
-        k_kf_centroid<32><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(),
-                                                                   c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
-    LILI_TRY(launch_check(c, "k_kf_centroid"));
-    LILI_CUDA(c, cudaMemcpyAsync(out, c->vg_out.p, (size_t)m * stride, cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    return LILIOM_OK;
+    int m = 0;
+    LILI_TRY(read_back(c, {{&m, c->vg_rank.as<int>() + n_fin, sizeof(int)}}));
+    return download_sized(c, c->vg_out, m, stride, out, cap, n, [&]() -> int {
+        LILI_CUDA(c, c->vg_out.ensure((size_t)m * stride));
+        if (stride == 48)
+            k_kf_centroid<48><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(),
+                                                                       c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
+        else
+            k_kf_centroid<32><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(),
+                                                                       c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
+        return launch_check(c, "k_kf_centroid");
+    });
 }

@@ -111,10 +111,9 @@ static int inc_frame_keys(liliom_ctx* c, Frame& f, u64* keys, unsigned* refs) {
         k_inc_keys<<<cdiv(f.n, 256), 256, 0, c->stream>>>((const unsigned char*)f.buf.p, f.n, stride, 1.0f / c->prm.leaf_map, (unsigned)f.slot, keys, refs, bad);
         LILI_TRY(launch_check(c, "k_inc_keys"));
     }
-    int* hp = c->h_pin->box;
-    LILI_CUDA(c, cudaMemcpyAsync(hp, bad, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    f.bad = hp[0] != 0;
+    int flag = 0;
+    LILI_TRY(read_back(c, {{&flag, bad, sizeof(int)}}));
+    f.bad = flag != 0;
     return LILIOM_OK;
 }
 
@@ -173,10 +172,7 @@ static int inc_emit(liliom_ctx* c, int* m_out) {
     else
         k_inc_centroid<32><<<cdiv(E, 128), 128, 0, c->stream>>>(tab, keys, refs, c->inc_flags.as<int>(), c->inc_rank.as<int>(), E, (unsigned char*)c->map_ds.p, c->vg_count.as<int>());
     LILI_TRY(launch_check(c, "k_inc_centroid"));
-    LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->vg_count, c->vg_count.p, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    *m_out = c->h_pin->vg_count;
-    return LILIOM_OK;
+    return read_back(c, {{m_out, c->vg_count.p, sizeof(int)}});
 }
 
 // The frame at the back of c->frames has just been pushed (points in its buffer, slot assigned); `popped` is the slot of the
