@@ -354,6 +354,37 @@ int liliom_undistort(liliom_ctx* c, void* pts_inout, int n, const double trans[3
 typedef struct { char name[16]; unsigned int offset; unsigned char datatype; unsigned int count; } liliom_pc2_field;
 int liliom_pc2_layout(int point_stride, liliom_pc2_field* fields, int cap, int* point_step);
 
+/* ---- SURVEY §8 (f3), sensor side of the ROT package: the driver's sensor_msgs::PointCloud2 as received ----
+ * R/src/Preprocessing.cpp:248-281 receives the spinning LiDAR's PointCloud2 (Velodyne, Ouster, ...) and runs
+ * pcl::fromROSMsg(msg, pcl::PointXYZI) (:277) before removeNaNFromPointCloud / removeClosedPointCloud (:280-281).  These calls
+ * take the message's fields and payload as they are: only height * row_step bytes cross PCIe (22 B per point for a packed
+ * Velodyne XYZIRT layout instead of 32), and the decode runs on the device.
+ * Decode (pcl::fromROSMsg): each of x, y, z, intensity is read from the FIRST message field with that name, datatype FLOAT32 (7)
+ * and count 1 or 0 (a FLOAT64 "x" before a FLOAT32 "x" is skipped); a field without such a match keeps PCL's default value 0;
+ * w = 1 and the padding floats are 0.  Point (r, c) is read at r * row_step + c * point_step (organised clouds, padded rows):
+ * n = width * height points in row-major order, read byte by byte (any point_step and offset alignment).
+ * The decoded sweep then goes through liliom_extract_rot unchanged.  is_dense is not an input: non-finite x/y/z are always
+ * dropped, as liliom_extract_rot does.  (PCL's removeNaNFromPointCloud skips that check for is_dense = true; a driver that sets
+ * is_dense and still emits NaN leaves the reference undefined — its start / end azimuth at :285-288 can become NaN.)
+ * LILIOM_E_ARG, nothing changed: a null msg, a null data with a non-empty payload, null fields with n_fields > 0, n_fields < 0,
+ * point_step 0, row_step < width * point_step, width * height > INT_MAX, a mapped field with offset + 4 > point_step,
+ * is_bigendian != 0, or a context that is not 32-byte (ROT). */
+typedef struct {
+    const void* data;                          /* msg.data.data(): height * row_step bytes, little-endian */
+    unsigned int height, width, point_step, row_step;
+    const liliom_pc2_field* fields; int n_fields;   /* msg.fields; names NUL-terminated (longer names truncated to 15 chars) */
+    int is_bigendian;                          /* msg.is_bigendian; nonzero is rejected */
+} liliom_pc2_msg;
+
+/* pcl::fromROSMsg(msg, pcl::PointXYZI) on the device (R/src/Preprocessing.cpp:277).  The decoded sweep stays resident like
+ * liliom_upload_scan's (liliom_extract_resident can run on it).  *n = width * height; out = NULL: no download; out with
+ * cap < *n: LILIOM_E_CAPACITY (*n reported, nothing converted). */
+int liliom_convert_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, liliom_pt32* out, int cap, int* n);
+/* = liliom_convert_pc2 + liliom_extract_rot without the 32-byte host cloud in between (R/src/Preprocessing.cpp:277-509). */
+int liliom_extract_rot_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, const double q_imu_wxyz[4], const double q_lb_wxyz[4],
+                           liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
+                           liliom_pt32* cutted_out, int cut_cap, int* n_cut);
+
 /* ===================== multi-GPU (one context per rank) ===================== */
 /* 128-byte NCCL unique id: rank 0 calls get, the launcher broadcasts it, every rank calls init.
  * After init, liliom_map_set_points shards the map by 16 m block hash (+halo) and every

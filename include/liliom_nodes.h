@@ -2,7 +2,8 @@
  * (liliom_b200/csrc/host/nodes.{h,cpp}).  ROS is not available in this image, so the node classes take
  * plain buffers where the reference takes sensor_msgs; their control flow, state and method names
  * follow L/src/Preprocessing.cpp:5-409 (R/src/Preprocessing.cpp:7-536) and L/src/LidarOdometry.cpp:6-687.
- * A ROS adapter is ~30 lines per node: fromROSMsg -> *_cloud(), publish the returned buffers.
+ * A ROS adapter is ~30 lines per node: fromROSMsg -> *_cloud() (the ROT node: the PointCloud2 itself ->
+ * liliom_pre_cloud_pc2()), publish the returned buffers.
  * Every compute step goes through the C ABI of liliom.h on the context passed at creation. */
 #ifndef LILIOM_NODES_H
 #define LILIOM_NODES_H
@@ -26,6 +27,13 @@ void liliom_pre_imu(liliom_pre_node*, double stamp, const double gyro_xyz[3]);
 int liliom_pre_cloud(liliom_pre_node*, double stamp, const void* pts, int n,
                      void* surf, int surf_cap, int* n_surf, void* edge, int edge_cap, int* n_edge,
                      void* cutted, int cut_cap, int* n_cut, double* stamp_out, double q_imu_out[4]);
+/* cloudHandler of the ROT package (R/src/Preprocessing.cpp:248-535) on the driver's PointCloud2 as received: the queued message
+ * keeps its payload and field list (the reference copies the whole message, :251), and the processed one goes through
+ * liliom_extract_rot_pc2 (fromROSMsg on the device, :277).  Same outputs and return values as liliom_pre_cloud; ROT nodes
+ * only.  A message liliom_convert_pc2 would reject: LILIOM_E_ARG, nothing queued. */
+int liliom_pre_cloud_pc2(liliom_pre_node*, double stamp, const liliom_pc2_msg* msg,
+                         void* surf, int surf_cap, int* n_surf, void* edge, int edge_cap, int* n_edge,
+                         void* cutted, int cut_cap, int* n_cut, double* stamp_out, double q_imu_out[4]);
 
 /* mode = LILIOM_MODE_CERES (reference semantics) or LILIOM_MODE_GN. */
 liliom_lo_node* liliom_lo_create(liliom_ctx* gpu, int max_num_iter, int scan_match_cnt, int if_to_deskew, int mode);

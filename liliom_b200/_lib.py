@@ -74,8 +74,9 @@ EXPORTS = [
     "liliom_backend_default_params", "liliom_kf_add", "liliom_kf_count", "liliom_kf_clear", "liliom_bmap_build",
     "liliom_bmap_download", "liliom_backend_window_correspond", "liliom_backend_window_blocks", "liliom_backend_window_corr",
     "liliom_kf_cloud", "liliom_kf_add_full", "liliom_global_map", "liliom_loop_align",
+    "liliom_convert_pc2", "liliom_extract_rot_pc2",
 ]
-NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud",
+NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
 
 
@@ -91,6 +92,32 @@ def pc2_layout(point_stride: int):
     if n < 0:
         raise LiliomError(n)
     return [(f[i].name.decode(), f[i].offset, f[i].datatype, f[i].count) for i in range(n)], step.value
+
+
+class Pc2Msg(C.Structure):
+    """liliom_pc2_msg (include/liliom.h)."""
+    _fields_ = [("data", C.c_void_p), ("height", C.c_uint), ("width", C.c_uint), ("point_step", C.c_uint), ("row_step", C.c_uint),
+                ("fields", C.POINTER(Pc2Field)), ("n_fields", C.c_int), ("is_bigendian", C.c_int)]
+
+
+class PC2:
+    """A sensor_msgs/PointCloud2 as a driver publishes it: the payload bytes (height * row_step, little-endian), the header
+    fields the decode reads and the field list as (name, offset, datatype, count) tuples."""
+
+    def __init__(self, data, height: int, width: int, point_step: int, row_step: int, fields, is_bigendian: bool = False):
+        self.data = np.ascontiguousarray(np.frombuffer(data, np.uint8) if isinstance(data, (bytes, bytearray)) else data).view(np.uint8).reshape(-1)
+        self.height, self.width, self.point_step, self.row_step = int(height), int(width), int(point_step), int(row_step)
+        self.fields = [(str(n), int(o), int(d), int(c)) for n, o, d, c in fields]
+        self.is_bigendian = bool(is_bigendian)
+
+    def c_msg(self):
+        """(Pc2Msg, field array): the field array must stay alive as long as the Pc2Msg is used."""
+        f = (Pc2Field * max(len(self.fields), 1))()
+        for i, (n, o, d, c) in enumerate(self.fields):
+            f[i].name = n.encode()[:15]; f[i].offset = o; f[i].datatype = d; f[i].count = c
+        m = Pc2Msg(self.data.ctypes.data_as(C.c_void_p) if self.data.size else None, self.height, self.width, self.point_step,
+                   self.row_step, f, len(self.fields), 1 if self.is_bigendian else 0)
+        return m, f
 
 
 class LoOutput(C.Structure):
@@ -154,6 +181,8 @@ def lib() -> C.CDLL:
     L.liliom_convert_livox.argtypes = [vp, vp, C.c_int, C.c_int, vp, C.c_int]
     L.liliom_extract_horizon_livox.argtypes = [vp, vp, C.c_int, C.c_int, dp, vp, C.c_int, ip, vp, C.c_int, ip, vp, C.c_int, ip]
     L.liliom_pc2_layout.argtypes = [C.c_int, vp, C.c_int, ip]
+    L.liliom_convert_pc2.argtypes = [vp, C.POINTER(Pc2Msg), vp, C.c_int, ip]
+    L.liliom_extract_rot_pc2.argtypes = [vp, C.POINTER(Pc2Msg), dp, dp, vp, C.c_int, ip, vp, C.c_int, ip, vp, C.c_int, ip]
     L.liliom_comm_peer_export.argtypes = [vp, vp]
     L.liliom_comm_peer_attach.argtypes = [vp, vp, C.c_int, C.c_int]
     L.liliom_comm_peer_epoch.argtypes = [vp, C.POINTER(C.c_uint)]
@@ -185,6 +214,7 @@ def lib() -> C.CDLL:
     L.liliom_pre_destroy.argtypes = [vp]; L.liliom_pre_destroy.restype = None
     L.liliom_pre_imu.argtypes = [vp, C.c_double, dp]; L.liliom_pre_imu.restype = None
     L.liliom_pre_cloud.argtypes = [vp, C.c_double, vp, C.c_int, vp, C.c_int, ip, vp, C.c_int, ip, vp, C.c_int, ip, dp, dp]
+    L.liliom_pre_cloud_pc2.argtypes = [vp, C.c_double, C.POINTER(Pc2Msg), vp, C.c_int, ip, vp, C.c_int, ip, vp, C.c_int, ip, dp, dp]
     L.liliom_lo_create.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int]; L.liliom_lo_create.restype = vp
     L.liliom_lo_destroy.argtypes = [vp]; L.liliom_lo_destroy.restype = None
     for f in (L.liliom_lo_edge, L.liliom_lo_surf, L.liliom_lo_full):
@@ -622,6 +652,30 @@ class Context:
                                                        _ptr(edge), len(edge), C.byref(ne), _ptr(cut), len(cut), C.byref(nc)))
         return surf[:ns.value], edge[:ne.value], cut[:nc.value]
 
+    def convert_pc2(self, msg: PC2, download: bool = True):
+        """pcl::fromROSMsg(msg, PointXYZI) on the device; the sweep stays resident (extract_resident).  Returns the PT32 cloud,
+        or its size when download=False."""
+        m, _f = msg.c_msg()
+        n = msg.width * msg.height
+        out = np.zeros(max(n, 1), PT32) if download else None
+        got = C.c_int()
+        self._check(lib().liliom_convert_pc2(self._h, C.byref(m), _ptr(out), len(out) if download else 0, C.byref(got)))
+        return out[:got.value] if download else got.value
+
+    def extract_rot_pc2(self, msg: PC2, q_imu, q_lb=(1.0, 0.0, 0.0, 0.0), out=None):
+        """extract_rot on the decoded PointCloud2 without a host cloud in between; out = optional (surf, edge, cut) PT32 arrays."""
+        m, _f = msg.c_msg()
+        n = msg.width * msg.height
+        q = np.asarray(q_imu, dtype=np.float64); ql = np.asarray(q_lb, dtype=np.float64)
+        if out is None:
+            surf = np.empty(max(n, 1), PT32); edge = np.empty(max(n, 1), PT32); cut = np.empty(max(n, 1), PT32)
+        else:
+            surf, edge, cut = out
+        ns, ne, nc = C.c_int(), C.c_int(), C.c_int()
+        self._check(lib().liliom_extract_rot_pc2(self._h, C.byref(m), _dptr(q), _dptr(ql), _ptr(surf), len(surf), C.byref(ns),
+                                                 _ptr(edge), len(edge), C.byref(ne), _ptr(cut), len(cut), C.byref(nc)))
+        return surf[:ns.value], edge[:ne.value], cut[:nc.value]
+
     # ---- multi-GPU / instrumentation ----
     def comm_init(self, unique_id: bytes, nranks: int, rank: int):
         buf = C.create_string_buffer(unique_id, 128)
@@ -693,18 +747,34 @@ class PreprocessingNode:
     def imu(self, stamp: float, gyro):
         lib().liliom_pre_imu(self._h, float(stamp), _dptr(np.asarray(gyro, np.float64)))
 
+    def _out_bufs(self, n: int):
+        cap = max(self._cap, n)
+        if cap > self._cap or self._bufs is None:
+            self._cap = cap
+            self._bufs = [np.empty(max(cap, 1), self.ctx.dtype) for _ in range(3)]
+        return self._bufs, max(cap, 1)
+
     def cloud(self, stamp: float, pts: np.ndarray):
         """Returns None while queueing / waiting for IMU, else (stamp, surf, edge, cutted, q_imu)."""
         pts = np.ascontiguousarray(pts, dtype=self.ctx.dtype)
-        cap = max(self._cap, len(pts))
-        if cap > self._cap or self._bufs is None:
-            self._cap = cap
-            self._bufs = [np.empty(cap, self.ctx.dtype) for _ in range(3)]
-        surf, edge, cut = self._bufs
+        (surf, edge, cut), cap = self._out_bufs(len(pts))
         ns, ne, nc = C.c_int(), C.c_int(), C.c_int()
         st = C.c_double(); q = np.zeros(4)
         rc = lib().liliom_pre_cloud(self._h, float(stamp), _ptr(pts), len(pts), _ptr(surf), cap, C.byref(ns), _ptr(edge), cap, C.byref(ne),
                                     _ptr(cut), cap, C.byref(nc), C.byref(st), _dptr(q))
+        return self._result(rc, st, surf, edge, cut, ns, ne, nc, q)
+
+    def cloud_pc2(self, stamp: float, msg: PC2):
+        """The ROT node's cloudHandler on the driver's PointCloud2 (liliom_pre_cloud_pc2); same results as cloud()."""
+        m, _f = msg.c_msg()
+        (surf, edge, cut), cap = self._out_bufs(msg.width * msg.height)
+        ns, ne, nc = C.c_int(), C.c_int(), C.c_int()
+        st = C.c_double(); q = np.zeros(4)
+        rc = lib().liliom_pre_cloud_pc2(self._h, float(stamp), C.byref(m), _ptr(surf), cap, C.byref(ns), _ptr(edge), cap, C.byref(ne),
+                                        _ptr(cut), cap, C.byref(nc), C.byref(st), _dptr(q))
+        return self._result(rc, st, surf, edge, cut, ns, ne, nc, q)
+
+    def _result(self, rc, st, surf, edge, cut, ns, ne, nc, q):
         if rc < 0:
             raise LiliomError(rc, lib().liliom_last_error(self.ctx._h).decode())
         if rc == 0:

@@ -2,6 +2,7 @@
 #include "ctx.cuh"
 #include "dev_math.cuh"
 #include "knn_core.cuh"
+#include "pc2_fields.h"
 #include <new>
 #include <cstdlib>
 #include <ctime>
@@ -276,10 +277,13 @@ extern "C" int liliom_extract_horizon(liliom_ctx* c, const liliom_pt48* pts, int
 
 // ---- (f3) FormatConvert on the device: livox_ros_driver::CustomPoint[] -> pcl::PointXYZINormal[] (L/src/FormatConvert.cpp:11-24)
 namespace lili {
+// little-endian 32-bit word assembled from bytes: sensor payloads carry fields at any byte offset, never read them wider
+__device__ __forceinline__ unsigned rd32(const unsigned char* p) {
+    return (unsigned)p[0] | ((unsigned)p[1] << 8) | ((unsigned)p[2] << 16) | ((unsigned)p[3] << 24);
+}
 __global__ void k_livox_to_pt48(const unsigned char* __restrict__ in, int n, int stride, float4* __restrict__ out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    auto rd32 = [](const unsigned char* p) { return (unsigned)p[0] | ((unsigned)p[1] << 8) | ((unsigned)p[2] << 16) | ((unsigned)p[3] << 24); };
     const unsigned time_end = rd32(in + (size_t)(n - 1) * stride);                       // :13 points.back().offset_time
     const unsigned char* p = in + (size_t)i * stride;
     const unsigned off = rd32(p);
@@ -294,9 +298,9 @@ __global__ void k_livox_to_pt48(const unsigned char* __restrict__ in, int n, int
 }
 static int livox_to_dev(liliom_ctx* c, const void* custom_pts, int n, int stride, void* d_out48) {
     if (n <= 0) return LILIOM_OK;
-    LILI_CUDA(c, c->livox_in.ensure((size_t)n * stride));
-    LILI_CUDA(c, cudaMemcpyAsync(c->livox_in.p, custom_pts, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
-    k_livox_to_pt48<<<cdiv(n, 256), 256, 0, c->stream>>>((const unsigned char*)c->livox_in.p, n, stride, (float4*)d_out48);
+    LILI_CUDA(c, c->wire_in.ensure((size_t)n * stride));
+    LILI_CUDA(c, cudaMemcpyAsync(c->wire_in.p, custom_pts, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
+    k_livox_to_pt48<<<cdiv(n, 256), 256, 0, c->stream>>>((const unsigned char*)c->wire_in.p, n, stride, (float4*)d_out48);
     return launch_check(c, "k_livox_to_pt48");
 }
 }  // namespace lili
@@ -325,6 +329,10 @@ extern "C" int liliom_extract_horizon_livox(liliom_ctx* c, const void* custom_pt
     return extract_horizon_from_raw(c, n, q_imu, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut);
 }
 
+static int extract_rot_from_raw(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4],
+                                liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
+                                liliom_pt32* cut_out, int cut_cap, int* n_cut);
+
 extern "C" int liliom_extract_rot(liliom_ctx* c, const liliom_pt32* pts, int n, const double q_imu[4], const double q_lb[4],
                                   liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
                                   liliom_pt32* cut_out, int cut_cap, int* n_cut) {
@@ -333,6 +341,66 @@ extern "C" int liliom_extract_rot(liliom_ctx* c, const liliom_pt32* pts, int n, 
     LILI_CUDA(c, cudaSetDevice(c->device));
     LILI_CUDA(c, c->raw.ensure((size_t)(n > 0 ? n : 1) * 32));
     if (n > 0) LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, pts, (size_t)n * 32, cudaMemcpyHostToDevice, c->stream));
+    return extract_rot_from_raw(c, n, q_imu, q_lb, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut);
+}
+
+// ---- (f3) pcl::fromROSMsg(PointCloud2 -> pcl::PointXYZI) on the device (R/src/Preprocessing.cpp:277); field matching: pc2_fields.h
+namespace lili {
+// One thread per point, row-major over (row, column).  src = Pc2Map::src of x, y, z, intensity (-1: unmapped -> 0).
+// Kept a pass of its own rather than fused into k_rot_pre: k_rot_hp and k_rot_build read the decoded sweep again.
+__global__ void k_pc2_to_pt32(const unsigned char* __restrict__ in, int n, unsigned width, unsigned point_step, unsigned row_step, int4 src,
+                              float4* __restrict__ out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned r = (unsigned)i / width, col = (unsigned)i - r * width;
+    const unsigned char* p = in + (size_t)r * row_step + (size_t)col * point_step;
+    auto fld = [p](int off) { return off < 0 ? 0.0f : __uint_as_float(rd32(p + off)); };
+    out[2 * (size_t)i] = make_float4(fld(src.x), fld(src.y), fld(src.z), 1.0f);          // pcl::PointXYZI default ctor: data[3] = 1
+    out[2 * (size_t)i + 1] = make_float4(fld(src.w), 0.f, 0.f, 0.f);
+}
+// msg already accepted by pc2_match (m): stage the payload, decode into d_out32 (m.n points of 32 bytes)
+static int pc2_to_dev(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, void* d_out32) {
+    if (m.n <= 0) return LILIOM_OK;
+    const size_t bytes = (size_t)msg->height * msg->row_step;
+    LILI_CUDA(c, c->wire_in.ensure(bytes));
+    LILI_CUDA(c, cudaMemcpyAsync(c->wire_in.p, msg->data, bytes, cudaMemcpyHostToDevice, c->stream));
+    k_pc2_to_pt32<<<cdiv(m.n, 256), 256, 0, c->stream>>>((const unsigned char*)c->wire_in.p, m.n, msg->width, msg->point_step, msg->row_step,
+                                                          make_int4(m.src[0], m.src[1], m.src[2], m.src[3]), (float4*)d_out32);
+    return launch_check(c, "k_pc2_to_pt32");
+}
+}  // namespace lili
+
+extern "C" int liliom_convert_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, liliom_pt32* out, int cap, int* n) {
+    Pc2Map m;
+    if (!c || !n || pc2_match(msg, &m) != LILIOM_OK) return LILIOM_E_ARG;
+    if (c->prm.point_stride != 32) return LILIOM_E_ARG;
+    if (out && m.n > cap) { *n = m.n; return LILIOM_E_CAPACITY; }
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    LILI_CUDA(c, c->raw_scan.ensure((size_t)(m.n > 0 ? m.n : 1) * 32));
+    LILI_TRY(pc2_to_dev(c, msg, m, c->raw_scan.p));
+    c->n_raw_scan = m.n;
+    if (out && m.n) LILI_CUDA(c, cudaMemcpyAsync(out, c->raw_scan.p, (size_t)m.n * 32, cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    *n = m.n;
+    return LILIOM_OK;
+}
+
+extern "C" int liliom_extract_rot_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, const double q_imu[4], const double q_lb[4],
+                                      liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
+                                      liliom_pt32* cut_out, int cut_cap, int* n_cut) {
+    Pc2Map m;
+    if (!c || !q_imu || !q_lb || !n_surf || !n_edge || !n_cut || pc2_match(msg, &m) != LILIOM_OK) return LILIOM_E_ARG;
+    if (c->prm.point_stride != 32) return LILIOM_E_ARG;
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    LILI_CUDA(c, c->raw.ensure((size_t)(m.n > 0 ? m.n : 1) * 32));
+    LILI_TRY(pc2_to_dev(c, msg, m, c->raw.p));
+    return extract_rot_from_raw(c, m.n, q_imu, q_lb, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut);
+}
+
+// Shared tail of the ROT entry points: c->raw holds n 32-byte points (upload / decode already queued on the stream).
+static int extract_rot_from_raw(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4],
+                                liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
+                                liliom_pt32* cut_out, int cut_cap, int* n_cut) {
     int ns = 0, ne = 0, nc = 0;
     LILI_TRY(rot_extract_dev(c, n, q_imu, q_lb, &ns, &ne, &nc));
     if ((surf_out && ns > surf_cap) || (edge_out && ne > edge_cap) || (cut_out && nc > cut_cap)) return LILIOM_E_CAPACITY;
@@ -885,21 +953,18 @@ extern "C" int liliom_icp_align(liliom_ctx* c, const void* src, int n_src, const
 }
 
 // ===================== wire format, publishing side =====================
-// from-knowledge: POINT_CLOUD_REGISTER_POINT_STRUCT of pcl::PointXYZINormal / pcl::PointXYZI (PCL 1.8-1.10) as pcl::toROSMsg lists them
+// PCL's field tables (pc2_fields.h) as pcl::toROSMsg lists them
 extern "C" int liliom_pc2_layout(int point_stride, liliom_pc2_field* fields, int cap, int* point_step) {
-    struct F { const char* name; unsigned int off; };
-    static const F f48[] = {{"x", 0}, {"y", 4}, {"z", 8}, {"normal_x", 16}, {"normal_y", 20}, {"normal_z", 24}, {"intensity", 32}, {"curvature", 36}};
-    static const F f32[] = {{"x", 0}, {"y", 4}, {"z", 8}, {"intensity", 16}};
     if (point_stride != 48 && point_stride != 32) return LILIOM_E_ARG;
-    const F* src = point_stride == 48 ? f48 : f32;
-    const int n = point_stride == 48 ? 8 : 4;
+    const Pc2Name* src = point_stride == 48 ? kPc2Fields48 : kPc2Fields32;
+    const int n = point_stride == 48 ? (int)(sizeof(kPc2Fields48) / sizeof(kPc2Fields48[0])) : kPc2Fields32N;
     if (point_step) *point_step = point_stride;
     if (!fields) return n;
     if (cap < n) return LILIOM_E_CAPACITY;
     for (int i = 0; i < n; ++i) {
         memset(&fields[i], 0, sizeof(fields[i]));
         strncpy(fields[i].name, src[i].name, sizeof(fields[i].name) - 1);
-        fields[i].offset = src[i].off; fields[i].datatype = 7; fields[i].count = 1;
+        fields[i].offset = src[i].offset; fields[i].datatype = kPc2Float32; fields[i].count = 1;
     }
     return n;
 }

@@ -198,8 +198,8 @@ struct liliom_ctx {
     lili::DevBuf hz_ctl;         // barrier words + per-block counts of the cooperative Horizon extractor
     unsigned int hz_coop_calls = 0;
     long long vg_ncells = 0;     // voxel-box cell count of that VoxelGrid, valid after the sync
-    lili::DevBuf raw_scan;       // resident raw sweep (liliom_upload_scan / liliom_convert_livox)
-    lili::DevBuf livox_in;       // staged livox CustomPoint records (19/20 bytes each)
+    lili::DevBuf raw_scan;       // resident raw sweep (liliom_upload_scan / liliom_convert_livox / liliom_convert_pc2)
+    lili::DevBuf wire_in;        // staged sensor payload: livox CustomPoint records (19/20 bytes each) or PointCloud2 data
     int n_raw_scan = 0;
     const void* raw_src = nullptr; // when set, the extractors read the sweep from here instead of c->raw (resident pipeline: no copy)
     int n_rot_cloud = 0;

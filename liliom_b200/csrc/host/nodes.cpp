@@ -1,5 +1,6 @@
 // See nodes.h.  Line citations are to the reference tree (L/ = LiLi-OM/, R/ = LiLi-OM-ROT/).
 #include "nodes.h"
+#include "../pc2_fields.h"
 #include <cmath>
 #include <cstring>
 #include <cstdlib>
@@ -86,6 +87,24 @@ int Preprocessing::cloudHandler(double stamp, const void* pts, int n, void* surf
     CloudMsg m;
     m.stamp = stamp; m.n = n;
     m.data.assign((const unsigned char*)pts, (const unsigned char*)pts + (size_t)n * stride);
+    return handleCloud(std::move(m), surf, surf_cap, n_surf, edge, edge_cap, n_edge, cutted, cut_cap, n_cut, stamp_out, q_imu_out);
+}
+
+// R/src/Preprocessing.cpp:248-535 on the PointCloud2 itself: the queue keeps a copy of the whole message (:251)
+int Preprocessing::cloudHandlerPc2(double stamp, const liliom_pc2_msg* msg, void* surf, int surf_cap, int* n_surf, void* edge, int edge_cap,
+                                   int* n_edge, void* cutted, int cut_cap, int* n_cut, double* stamp_out, double q_imu_out[4]) {
+    lili::Pc2Map map;
+    if (variant != 1 || lili::pc2_match(msg, &map) != LILIOM_OK) return LILIOM_E_ARG;
+    CloudMsg m;
+    m.stamp = stamp; m.n = map.n; m.pc2 = true;
+    m.height = msg->height; m.width = msg->width; m.point_step = msg->point_step; m.row_step = msg->row_step;
+    if (map.n > 0) m.data.assign((const unsigned char*)msg->data, (const unsigned char*)msg->data + (size_t)msg->height * msg->row_step);
+    if (msg->n_fields > 0) m.fields.assign(msg->fields, msg->fields + msg->n_fields);
+    return handleCloud(std::move(m), surf, surf_cap, n_surf, edge, edge_cap, n_edge, cutted, cut_cap, n_cut, stamp_out, q_imu_out);
+}
+
+int Preprocessing::handleCloud(CloudMsg&& m, void* surf, int surf_cap, int* n_surf, void* edge, int edge_cap, int* n_edge, void* cutted,
+                               int cut_cap, int* n_cut, double* stamp_out, double q_imu_out[4]) {
     cloud_queue.push_back(std::move(m));                                   // :196
     if (cloud_queue.size() <= 2) return 0;                                 // :197-198
     CloudMsg cur = std::move(cloud_queue.front());                         // :201-202
@@ -100,7 +119,12 @@ int Preprocessing::cloudHandler(double stamp, const void* pts, int n, void* surf
     if (variant == 0)
         rc = liliom_extract_horizon(gpu, (const liliom_pt48*)cur.data.data(), cur.n, q, (liliom_pt48*)surf, surf_cap, n_surf,
                                     (liliom_pt48*)edge, edge_cap, n_edge, (liliom_pt48*)cutted, cut_cap, n_cut);           // :225-383
-    else {
+    else if (cur.pc2) {
+        const double ql[4] = {q_lb.w, q_lb.x, q_lb.y, q_lb.z};
+        const liliom_pc2_msg msg{cur.data.data(), cur.height, cur.width, cur.point_step, cur.row_step, cur.fields.data(), (int)cur.fields.size(), 0};
+        rc = liliom_extract_rot_pc2(gpu, &msg, q, ql, (liliom_pt32*)surf, surf_cap, n_surf, (liliom_pt32*)edge, edge_cap, n_edge,
+                                    (liliom_pt32*)cutted, cut_cap, n_cut);                                                   // R:277-509
+    } else {
         const double ql[4] = {q_lb.w, q_lb.x, q_lb.y, q_lb.z};
         rc = liliom_extract_rot(gpu, (const liliom_pt32*)cur.data.data(), cur.n, q, ql, (liliom_pt32*)surf, surf_cap, n_surf,
                                 (liliom_pt32*)edge, edge_cap, n_edge, (liliom_pt32*)cutted, cut_cap, n_cut);               // R:280-509
@@ -306,6 +330,11 @@ int liliom_pre_cloud(liliom_pre_node* n, double stamp, const void* pts, int np, 
                      int* n_edge, void* cutted, int cut_cap, int* n_cut, double* stamp_out, double q_imu_out[4]) {
     if (!n || np < 0 || (np > 0 && !pts)) return LILIOM_E_ARG;
     return n->impl.cloudHandler(stamp, pts, np, surf, surf_cap, n_surf, edge, edge_cap, n_edge, cutted, cut_cap, n_cut, stamp_out, q_imu_out);
+}
+int liliom_pre_cloud_pc2(liliom_pre_node* n, double stamp, const liliom_pc2_msg* msg, void* surf, int surf_cap, int* n_surf, void* edge,
+                         int edge_cap, int* n_edge, void* cutted, int cut_cap, int* n_cut, double* stamp_out, double q_imu_out[4]) {
+    if (!n) return LILIOM_E_ARG;
+    return n->impl.cloudHandlerPc2(stamp, msg, surf, surf_cap, n_surf, edge, edge_cap, n_edge, cutted, cut_cap, n_cut, stamp_out, q_imu_out);
 }
 liliom_lo_node* liliom_lo_create(liliom_ctx* gpu, int max_num_iter, int scan_match_cnt, int if_to_deskew, int mode) {
     return gpu ? new liliom_lo_node(gpu, max_num_iter, scan_match_cnt, if_to_deskew != 0, mode) : nullptr;

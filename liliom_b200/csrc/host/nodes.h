@@ -15,7 +15,13 @@ struct Quat { double w = 1, x = 0, y = 0, z = 0; };
 struct Vec3 { double x = 0, y = 0, z = 0; };
 
 struct ImuMsg { double stamp; Vec3 angular_velocity; bool valid; };
-struct CloudMsg { double stamp; std::vector<unsigned char> data; int n; };
+struct CloudMsg {
+    double stamp; std::vector<unsigned char> data; int n;
+    // a PointCloud2 as received (liliom_pre_cloud_pc2): data is its payload, these are the rest of the message it needs
+    bool pc2 = false;
+    unsigned int height = 0, width = 0, point_step = 0, row_step = 0;
+    std::vector<liliom_pc2_field> fields;
+};
 
 class Preprocessing {
 public:
@@ -23,8 +29,12 @@ public:
     void imuHandler(double stamp, const double gyro[3]);
     int cloudHandler(double stamp, const void* pts, int n, void* surf, int surf_cap, int* n_surf, void* edge, int edge_cap, int* n_edge,
                      void* cutted, int cut_cap, int* n_cut, double* stamp_out, double q_imu_out[4]);
+    int cloudHandlerPc2(double stamp, const liliom_pc2_msg* msg, void* surf, int surf_cap, int* n_surf, void* edge, int edge_cap, int* n_edge,
+                        void* cutted, int cut_cap, int* n_cut, double* stamp_out, double q_imu_out[4]);
 
 private:
+    int handleCloud(CloudMsg&& msg, void* surf, int surf_cap, int* n_surf, void* edge, int edge_cap, int* n_edge,
+                    void* cutted, int cut_cap, int* n_cut, double* stamp_out, double q_imu_out[4]);
     void solveRotation(double dt, const Vec3& angular_velocity);
     void processIMU(double t_cur);
 

@@ -16,7 +16,7 @@ from __future__ import annotations
 
 import numpy as np
 
-from ._lib import PT32, PT48
+from ._lib import PC2, PT32, PT48
 
 BLOCK = 40.0
 WALL_H = 8.0
@@ -205,8 +205,9 @@ def hdl64_elevations():
     return np.concatenate([up, lo])
 
 
-def make_hdl64_sweep(true_pose7, seed: int = 2, omega=(0.0, 0.0, 0.2), steps: int = 2031, noise=0.02, dropout=0.01):
-    """~130k-point HDL-64E-like sweep in firing order (azimuth-major, clockwise). Returns (PT32[n], q_imu)."""
+def make_hdl64_sweep(true_pose7, seed: int = 2, omega=(0.0, 0.0, 0.2), steps: int = 2031, noise=0.02, dropout=0.01, grid: bool = False):
+    """~130k-point HDL-64E-like sweep in firing order (azimuth-major, clockwise). Returns (PT32[n], q_imu); grid=True appends
+    each return's ring (0..63, the row of hdl64_elevations) and azimuth step (0..steps-1), which organised layouts need."""
     rng = np.random.default_rng(seed)
     elev = np.deg2rad(hdl64_elevations())
     k = np.arange(steps)
@@ -228,7 +229,69 @@ def make_hdl64_sweep(true_pose7, seed: int = 2, omega=(0.0, 0.0, 0.2), steps: in
     out = np.zeros(int(hit.sum()), PT32)
     out["x"] = p[hit, 0]; out["y"] = p[hit, 1]; out["z"] = p[hit, 2]; out["w"] = 1.0
     out["intensity"] = rng.integers(0, 256, size=len(out)).astype(np.float32)
+    if grid:
+        return out, q_imu, R[hit].astype(np.int32), K[hit].astype(np.int32)
     return out, q_imu
+
+
+# ------------------------------------------------------------------ PointCloud2 as spinning-LiDAR drivers publish it
+PC2_F32, PC2_U8, PC2_U16, PC2_U32 = 7, 2, 4, 6      # sensor_msgs::PointField datatypes
+_PC2_NP = {PC2_F32: "<f4", PC2_U8: "u1", PC2_U16: "<u2", PC2_U32: "<u4"}
+# Representative driver layouts, described from knowledge of the drivers' published point types (not from their sources):
+#   velodyne22    packed x, y, z, intensity (f32), ring (u16), time (f32): 22 B per point, one row in firing order
+#   pcl32         PCL-aligned 32 B: x, y, z at 0-11, intensity at 16, ring (u16) at 20, the rest padding; one row
+#   ouster48      organised rings x columns (64 x steps), 48 B: x, y, z, intensity (f32) at 16, t (u32), reflectivity (u16),
+#                 ring (u8), ambient (u16), range (u32); (0, 0, 0) for a missing return
+#   organised_nan organised 64 x steps, 16 B points listed intensity first, NaN for a missing return, rows padded by 40 bytes
+PC2_LAYOUTS = ("velodyne22", "pcl32", "ouster48", "organised_nan")
+
+
+def encode_pc2(pts, ring, step, layout: str, steps: int = 2031, lines: int = 64) -> PC2:
+    """The sweep pts (PT32, with make_hdl64_sweep(grid=True)'s ring and step per return) as the PointCloud2 a driver of the
+    given layout would publish.  Bytes that no field covers are filled with a non-zero pattern."""
+    F, U8, U16, U32 = PC2_F32, PC2_U8, PC2_U16, PC2_U32
+    xyz = [("x", 0, F, 1), ("y", 4, F, 1), ("z", 8, F, 1)]
+    organised, pad, missing = False, 0, 0.0
+    if layout == "velodyne22":
+        fields, point_step = xyz + [("intensity", 12, F, 1), ("ring", 16, U16, 1), ("time", 18, F, 1)], 22
+    elif layout == "pcl32":
+        fields, point_step = xyz + [("intensity", 16, F, 1), ("ring", 20, U16, 1)], 32
+    elif layout == "ouster48":
+        fields = xyz + [("intensity", 16, F, 1), ("t", 20, U32, 1), ("reflectivity", 24, U16, 1), ("ring", 26, U8, 1),
+                        ("ambient", 28, U16, 1), ("range", 32, U32, 1)]
+        point_step, organised = 48, True
+    elif layout == "organised_nan":
+        fields = [("intensity", 12, F, 1)] + xyz
+        point_step, organised, pad, missing = 16, True, 40, np.nan
+    else:
+        raise ValueError(f"unknown PointCloud2 layout {layout!r}")
+    dt = np.dtype({"names": [f[0] for f in fields], "formats": [_PC2_NP[f[2]] for f in fields],
+                   "offsets": [f[1] for f in fields], "itemsize": point_step})
+    height, width = (lines, steps) if organised else (1, len(pts))
+    rec = np.full(height * width * point_step, 0xA5, np.uint8).view(dt)
+    ring = np.asarray(ring, np.int64); step = np.asarray(step, np.int64)
+    if organised:
+        for f in fields:
+            rec[f[0]] = missing if f[0] in ("x", "y", "z") else 0
+        idx = ring * width + step
+    else:
+        idx = np.arange(len(pts))
+    for f in ("x", "y", "z", "intensity"):
+        rec[f][idx] = pts[f]
+    if "ring" in dt.names:
+        rec["ring"][idx] = ring
+    if layout == "velodyne22":
+        rec["time"][idx] = (step * (0.1 / steps)).astype(np.float32)
+    if layout == "ouster48":
+        r = np.sqrt(pts["x"].astype(np.float64) ** 2 + pts["y"].astype(np.float64) ** 2 + pts["z"].astype(np.float64) ** 2)
+        rec["t"][idx] = step * (100_000_000 // steps)
+        rec["reflectivity"][idx] = pts["intensity"].astype(np.uint16)
+        rec["ambient"][idx] = 100
+        rec["range"][idx] = np.round(r * 1000.0).astype(np.uint32)
+    row_step = width * point_step + pad
+    data = np.full((height, row_step), 0xA5, np.uint8)
+    data[:, :width * point_step] = rec.view(np.uint8).reshape(height, width * point_step)
+    return PC2(data.reshape(-1), height, width, point_step, row_step, fields)
 
 
 def default_true_pose():

@@ -1,0 +1,133 @@
+#!/usr/bin/env python
+"""ROT-package ingest of the spinning LiDAR's PointCloud2 (SURVEY §8 f3): host decode + the 32-byte path against the device decode.
+
+For each synthetic driver layout (synth.PC2_LAYOUTS, the seeded 130k-point HDL-64E sweep) one step is
+  (i)  a NumPy decode of the message into a pinned PointXYZI array (standing in for pcl::fromROSMsg on the node's host; PCL is
+       not used here, so this is not PCL's cost) + liliom_extract_rot on it, or
+  (ii) liliom_extract_rot_pc2 on the message payload, from the message's own (pageable) buffer and from a pinned copy of it.
+Every call is synchronous (the library drains its stream before it returns), so a host clock around each call is the step time.
+Reports the median step time of each path (and of the NumPy decode and of liliom_extract_rot on the decoded pinned cloud alone),
+the host-to-device bytes per sweep, and whether (i) and (ii) give the same bytes.
+The card's name and power limit are printed with the numbers.
+usage: pc2_ingest_bench.py [--steps K] [--warmup W] [--out FILE]"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+import liliom_b200 as L                      # noqa: E402
+from liliom_b200 import synth                # noqa: E402
+
+F32 = 7
+
+
+def pinned(nbytes):
+    import torch
+    return torch.empty(max(nbytes, 1), dtype=torch.uint8, pin_memory=True).numpy()
+
+
+def host_decode(msg, out):
+    """pcl::fromROSMsg(msg, PointXYZI) with NumPy: out (PT32, n points) gets x, y, z, intensity from the first FLOAT32 field of
+    each name with count 0 or 1 (0 when none), w = 1, padding 0.  One strided copy per field, no Python loop over points."""
+    n = msg.width * msg.height
+    o = out[:n]
+    o[...] = np.zeros(1, L.PT32)
+    o["w"] = 1.0
+    for name in ("x", "y", "z", "intensity"):
+        hit = [f for f in msg.fields if f[0] == name and f[2] == F32 and f[3] in (0, 1)]
+        if not hit or n == 0:
+            continue
+        src = np.ndarray((msg.height, msg.width), "<f4", buffer=msg.data, offset=hit[0][1], strides=(msg.row_step, msg.point_step))
+        dst = o[name].reshape(msg.height, msg.width)
+        dst[...] = src
+    return o
+
+
+def card():
+    import torch
+    name = torch.cuda.get_device_name(0)
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                           capture_output=True, text=True, timeout=30).stdout.strip()
+    except Exception as e:          # the numbers are still printed; the power limit is then reported as unknown
+        q = f"unknown ({e})"
+    return name, q
+
+
+def median_ms(fn, steps, warmup):
+    for _ in range(warmup):
+        fn()
+    ts = []
+    for _ in range(steps):
+        t0 = time.perf_counter()
+        fn()
+        ts.append((time.perf_counter() - t0) * 1e3)
+    return float(np.median(ts)), float(np.min(ts)), float(np.max(ts))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=200)
+    ap.add_argument("--warmup", type=int, default=20)
+    ap.add_argument("--out", default=None, help="also write the JSON lines here")
+    a = ap.parse_args()
+    name, power = card()
+    print(f"card: {name}; power limit, max SM clock: {power}", flush=True)
+    T = synth.default_true_pose()
+    pts, q_imu, ring, step = synth.make_hdl64_sweep(T, grid=True)
+    q_lb = np.array([1.0, 0.0, 0.0, 0.0])
+    ctx = L.Context(variant=1)
+    rows = []
+    for layout in synth.PC2_LAYOUTS:
+        msg = synth.encode_pc2(pts, ring, step, layout)
+        n = msg.width * msg.height
+        pin_msg = L.PC2(pinned(msg.data.size)[:msg.data.size], msg.height, msg.width, msg.point_step, msg.row_step, msg.fields)
+        pin_msg.data[:] = msg.data
+        cloud = pinned(n * 32)[:n * 32].view(L.PT32)
+        outs = [[pinned(n * 32)[:n * 32].view(L.PT32) for _ in range(3)] for _ in range(2)]
+
+        def path_host():
+            host_decode(msg, cloud)
+            return ctx.extract_rot(cloud, q_imu, q_lb, out=outs[0])
+
+        def path_pc2(m):
+            return ctx.extract_rot_pc2(m, q_imu, q_lb, out=outs[1])
+
+        ref = [x.tobytes() for x in path_host()]
+        same = [x.tobytes() for x in path_pc2(msg)] == ref and [x.tobytes() for x in path_pc2(pin_msg)] == ref
+        t_dec = median_ms(lambda: host_decode(msg, cloud), a.steps, a.warmup)
+        t_host = median_ms(path_host, a.steps, a.warmup)
+        t_ext = median_ms(lambda: ctx.extract_rot(cloud, q_imu, q_lb, out=outs[0]), a.steps, a.warmup)    # (i) without its decode
+        t_pg = median_ms(lambda: path_pc2(msg), a.steps, a.warmup)
+        t_pn = median_ms(lambda: path_pc2(pin_msg), a.steps, a.warmup)
+        row = dict(layout=layout, points=n, point_step=msg.point_step, h2d_bytes_host_path=n * 32, h2d_bytes_pc2=msg.height * msg.row_step,
+                   numpy_decode_ms=t_dec[0], extract_rot_pinned_pt32_ms=t_ext[0], host_decode_plus_extract_rot_ms=t_host[0],
+                   extract_rot_pc2_pageable_ms=t_pg[0], extract_rot_pc2_pinned_ms=t_pn[0], min_max_ms={"host": t_host[1:], "pc2_pageable": t_pg[1:], "pc2_pinned": t_pn[1:]},
+                   outputs_identical=bool(same), steps=a.steps, warmup=a.warmup, card=name, power_limit_max_sm_clock=power)
+        rows.append(row)
+        print(json.dumps(row), flush=True)
+    ctx.close()
+    if a.out:
+        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
+        with open(a.out, "w") as f:
+            for r in rows:
+                f.write(json.dumps(r) + "\n")
+    print(f"\n{'layout':<14} {'B/pt in':>8} {'H2D host':>10} {'H2D pc2':>10} {'decode':>8} {'32B ext':>8} {'(i) host':>9} "
+          f"{'(ii) pg':>8} {'(ii) pin':>9} same")
+    for r in rows:
+        print(f"{r['layout']:<14} {r['point_step']:>8} {r['h2d_bytes_host_path']:>10} {r['h2d_bytes_pc2']:>10} {r['numpy_decode_ms']:>8.3f} "
+              f"{r['extract_rot_pinned_pt32_ms']:>8.3f} {r['host_decode_plus_extract_rot_ms']:>9.3f} {r['extract_rot_pc2_pageable_ms']:>8.3f} {r['extract_rot_pc2_pinned_ms']:>9.3f} "
+              f"{r['outputs_identical']}")
+    print(f"(ms, median of {a.steps} steps after {a.warmup} warm-up steps; {name}, power limit / max SM clock {power})")
+    if not all(r["outputs_identical"] for r in rows):
+        sys.exit(1)
+
+
+if __name__ == "__main__":
+    main()
