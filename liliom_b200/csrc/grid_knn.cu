@@ -195,20 +195,6 @@ __device__ __forceinline__ double warp_sum(double v) {
     return v;
 }
 
-// Temporal coherence of the GN passes: a query whose five neighbours lay within r = sqrt(d5) at its previous position p'
-// still has those five map points within r + |p - p'| of its new position p, so its new fifth distance is at most
-// (r + |p - p'|)^2.  Starting the search with that bound instead of the gate skips most cells outright and leaves little to
-// rank — from the second pass of a scan on the poses move by centimetres.  The bound is evaluated with upward roundings and
-// a 1e-5 relative margin (the candidate distance expression carries ~3 fp32 roundings, ~2e-7), so every point of the true
-// 5-NN set passes the filter: the sets found, their order and the accept decisions are exactly those of the full search.
-__device__ __forceinline__ float coherence_tau(const float4& st, float sx, float sy, float sz, float tau0) {
-    if (!(st.w <= tau0)) return tau0;                    // no five neighbours inside the gate last time (or NaN): nothing to exploit
-    const float dx = fsubx(sx, st.x), dy = fsubx(sy, st.y), dz = fsubx(sz, st.z);
-    const float mv = __fsqrt_ru(__fadd_ru(__fadd_ru(__fmul_ru(dx, dx), __fmul_ru(dy, dy)), __fmul_ru(dz, dz)));
-    const float r = __fadd_ru(__fsqrt_ru(st.w), mv);
-    return fminf(tau0, __fmul_ru(__fmul_ru(r, r), 1.00001f));
-}
-
 // Per-query scratch a warp keeps in shared memory between the phases.
 struct Slot {
     int   idx[5];            // neighbour indices into map_orig; idx[0] < 0: no 5-NN inside the radius

@@ -41,7 +41,8 @@ def test_gn_variants_bit_identical(oracle, world_small):
     ds = oracle.voxelgrid(surf, 0.4)
     guess = world_small["guess"]
     # scans of different sizes back to back: the grid size changes between launches, the larger ones leave the 16-lane shape
-    scans = [ds, ds[: len(ds) // 3], ds[::2], ds[:40], surf[:6000], surf[:3000], ds]     # 3000: two search rounds per warp task
+    # 3000: eight lanes per query (sixteen would need more than one block per SM and leave the single launch)
+    scans = [ds, ds[: len(ds) // 3], ds[::2], ds[:40], surf[:6000], surf[:3000], ds]
     ref = None
     for ll in VARIANTS:
         c = _ctx(ll)
