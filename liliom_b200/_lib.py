@@ -28,6 +28,7 @@ assert PT48.itemsize == 48 and PT32.itemsize == 32 and LIVOX20.itemsize == 20
 OK, E_ARG, E_CUDA, E_FEWMAP, E_CAPACITY, E_GRID, E_LINES, E_NCCL, E_NOMAP = 0, -1, -2, -3, -4, -5, -6, -7, -8
 MODE_CERES, MODE_GN = 0, 1
 KF_FULL, KF_SURF = 0, 1      # liliom_global_map: which stored cloud of each keyframe
+RING_ELEVATION, RING_FIELD = 0, 1   # liliom_set_ring_source: ROT scanID from the elevation tables / the PointCloud2 `ring` field
 
 
 class Params(C.Structure):
@@ -74,7 +75,7 @@ EXPORTS = [
     "liliom_backend_default_params", "liliom_kf_add", "liliom_kf_count", "liliom_kf_clear", "liliom_bmap_build",
     "liliom_bmap_download", "liliom_backend_window_correspond", "liliom_backend_window_blocks", "liliom_backend_window_corr",
     "liliom_kf_cloud", "liliom_kf_add_full", "liliom_global_map", "liliom_loop_align",
-    "liliom_convert_pc2", "liliom_extract_rot_pc2",
+    "liliom_convert_pc2", "liliom_extract_rot_pc2", "liliom_set_ring_source",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -183,6 +184,7 @@ def lib() -> C.CDLL:
     L.liliom_pc2_layout.argtypes = [C.c_int, vp, C.c_int, ip]
     L.liliom_convert_pc2.argtypes = [vp, C.POINTER(Pc2Msg), vp, C.c_int, ip]
     L.liliom_extract_rot_pc2.argtypes = [vp, C.POINTER(Pc2Msg), dp, dp, vp, C.c_int, ip, vp, C.c_int, ip, vp, C.c_int, ip]
+    L.liliom_set_ring_source.argtypes = [vp, C.c_int]
     L.liliom_comm_peer_export.argtypes = [vp, vp]
     L.liliom_comm_peer_attach.argtypes = [vp, vp, C.c_int, C.c_int]
     L.liliom_comm_peer_epoch.argtypes = [vp, C.POINTER(C.c_uint)]
@@ -661,6 +663,11 @@ class Context:
         got = C.c_int()
         self._check(lib().liliom_convert_pc2(self._h, C.byref(m), _ptr(out), len(out) if download else 0, C.byref(got)))
         return out[:got.value] if download else got.value
+
+    def set_ring_source(self, source: int):
+        """RING_ELEVATION (default): the ROT extractor takes each return's ring from its elevation (line_num 16/32/64 tables);
+        RING_FIELD: from the PointCloud2's `ring` field (convert_pc2 / extract_rot_pc2 / extract_resident, line_num 1..128)."""
+        self._check(lib().liliom_set_ring_source(self._h, int(source)))
 
     def extract_rot_pc2(self, msg: PC2, q_imu, q_lb=(1.0, 0.0, 0.0, 0.0), out=None):
         """extract_rot on the decoded PointCloud2 without a host cloud in between; out = optional (surf, edge, cut) PT32 arrays."""

@@ -202,6 +202,10 @@ struct liliom_ctx {
     lili::DevBuf wire_in;        // staged sensor payload: livox CustomPoint records (19/20 bytes each) or PointCloud2 data
     int n_raw_scan = 0;
     const void* raw_src = nullptr; // when set, the extractors read the sweep from here instead of c->raw (resident pipeline: no copy)
+    int ring_source = LILIOM_RING_ELEVATION;   // liliom_set_ring_source
+    lili::DevBuf raw_ring;       // LILIOM_RING_FIELD: u16 ring id per point of c->raw (liliom_extract_rot_pc2)
+    lili::DevBuf raw_scan_ring;  // ... of the resident sweep (liliom_convert_pc2)
+    bool raw_scan_rings = false; // raw_scan_ring holds the ring ids of the resident sweep
     int n_rot_cloud = 0;
 
     // ---- voxel grid scratch ----
@@ -373,7 +377,10 @@ int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int
             bool want_corr, double out29[29]);
 
 int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf, int* n_edge, int* n_cut, bool sync_counts = true);
-int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut);
+// rings: nullptr = scanID from the elevation tables (line_num 16/32/64), else the u16 ring id of every input point (line_num 1..128)
+int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut,
+                    const uint16_t* rings = nullptr);
+bool rot_lines_ok(int line_num, bool field);
 
 int icp_align(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,
               double fit_eps, double T16[16], double* fitness, int* converged, int* iters);     // icp.cu

@@ -2,7 +2,8 @@
 // Preprocessing::cloudHandler, R/src/Preprocessing.cpp:280-509.
 //
 //   k_rot_pre      removeNaN + removeClosedPointCloud 3.0 m (:280-281), elevation -> scanID
-//                  (:315-347), raw azimuth -atan2f(y,x) (:349); first/last surviving index
+//                  (:315-347) or the driver's ring id (LILIOM_RING_FIELD), raw azimuth -atan2f(y,x)
+//                  (:349); first/last surviving index
 //   k_rot_hp       the sequential `halfPassed` latch (:350-358) as a prefix-min: the first valid
 //                  index whose (un-latched) azimuth passes startOri + pi
 //   (stable sort)  bucket by ring preserving arrival order == laserCloudScans[scanID] (:371,378-382)
@@ -32,21 +33,24 @@ namespace lili {
 
 struct Pt32 { float4 a, b; };   // {x,y,z,1} {intensity,0,0,0}
 
-constexpr int ROT_MAX_RINGS = 64;
+// One CTA of k_rot_ring per ring, ~122 KB of shared memory each (RingSmem): one CTA per SM, so 128 rings are one wave on a
+// 132-SM H100.  Ring keys stay below the 255 sentinel (8-bit ring sort, 40-bit (ring, voxel) keys).
+constexpr int ROT_MAX_RINGS = 128;
 constexpr int ROT_SEG_CAP = 4096;          // max points per segment (ring <= ~24k points)
 constexpr int ROT_RING_CAP = 16384;        // picked[] bytes per ring in shared memory
 constexpr double ROT_PI = 3.14159265358979323846;   // M_PI
 
 // meta layout (ints): [0] first idx, [1] last idx, [2] halfPassed idx, [3] n_valid (cloudSize),
-// [4] error flag, [5] n_lessflat, [6] n_edge, [8..8+64) ring_first, [72..72+64) ring_end
-constexpr int M_FIRST = 0, M_LAST = 1, M_HP = 2, M_NVALID = 3, M_ERR = 4, M_NLF = 5, M_NEDGE = 6, M_RF = 8, M_RE = 72, M_SIZE = 144;
+// [4] error flag, [5] n_lessflat, [6] n_edge, [M_RF..M_RF+ROT_MAX_RINGS) ring_first, [M_RE..M_RE+ROT_MAX_RINGS) ring_end
+constexpr int M_FIRST = 0, M_LAST = 1, M_HP = 2, M_NVALID = 3, M_ERR = 4, M_NLF = 5, M_NEDGE = 6, M_RF = 8, M_RE = M_RF + ROT_MAX_RINGS,
+              M_SIZE = M_RE + ROT_MAX_RINGS;
+
+bool rot_lines_ok(int line_num, bool field) {
+    return field ? (line_num >= 1 && line_num <= ROT_MAX_RINGS) : (line_num == 16 || line_num == 32 || line_num == 64);
+}
 
 __global__ void k_rot_meta_init(int* meta) {
-    int t = threadIdx.x;
-    if (t < M_SIZE) meta[t] = 0;
-    if (t == M_FIRST) meta[t] = INT_MAX;
-    if (t == M_LAST) meta[t] = -1;
-    if (t == M_HP) meta[t] = INT_MAX;
+    for (int t = threadIdx.x; t < M_SIZE; t += blockDim.x) meta[t] = t == M_LAST ? -1 : (t == M_FIRST || t == M_HP) ? INT_MAX : 0;
 }
 
 __device__ __forceinline__ bool rot_keep(float4 a) {
@@ -55,8 +59,29 @@ __device__ __forceinline__ bool rot_keep(float4 a) {
     return !(a.x * a.x + a.y * a.y + a.z * a.z < thres * thres);
 }
 
-__global__ void k_rot_pre(const Pt32* __restrict__ pts, int n, int n_scans, uint32_t* __restrict__ keys, int* __restrict__ vals,
-                          float* __restrict__ ori, int* __restrict__ meta) {
+// scanID of a point from its elevation through the reference's tables (:315-347), -1 for a table miss
+__device__ __forceinline__ int rot_table_scan_id(float4 a, int n_scans) {
+    float angle = (float)((double)(det_atanf(a.z / sqrtf(a.x * a.x + a.y * a.y)) * 180.0f) / ROT_PI);        // :315
+    int scanID = 0;
+    bool ok = true;
+    if (n_scans == 16) {
+        scanID = (int)((double)((angle + 15.0f) / 2.0f) + 0.5);
+        if (scanID > (n_scans - 1) || scanID < 0) ok = false;
+    } else if (n_scans == 32) {
+        scanID = (int)(((double)angle + 92.0 / 3.0) * 3.0 / 4.0);
+        if (scanID > (n_scans - 1) || scanID < 0) ok = false;
+    } else {
+        if ((double)angle >= -8.83) scanID = (int)((double)(2.0f - angle) * 3.0 + 0.5);
+        else scanID = n_scans / 2 + (int)((-8.83 - (double)angle) * 2.0 + 0.5);
+        if (angle > 2.0f || (double)angle < -24.33 || scanID > 50 || scanID < 0) ok = false;
+    }
+    return ok ? scanID : -1;
+}
+
+// rings: nullptr = the elevation tables; else the driver's ring id of each point, kept iff < n_scans (LILIOM_RING_FIELD: the
+// only difference between the two modes)
+__global__ void k_rot_pre(const Pt32* __restrict__ pts, const uint16_t* __restrict__ rings, int n, int n_scans, uint32_t* __restrict__ keys,
+                          int* __restrict__ vals, float* __restrict__ ori, int* __restrict__ meta) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     float4 a = pts[i].a;
@@ -65,22 +90,9 @@ __global__ void k_rot_pre(const Pt32* __restrict__ pts, int n, int n_scans, uint
     if (rot_keep(a)) {
         atomicMin(&meta[M_FIRST], i);
         atomicMax(&meta[M_LAST], i);
-        float angle = (float)((double)(det_atanf(a.z / sqrtf(a.x * a.x + a.y * a.y)) * 180.0f) / ROT_PI);    // :315
-        int scanID = 0;
-        bool ok = true;
-        if (n_scans == 16) {
-            scanID = (int)((double)((angle + 15.0f) / 2.0f) + 0.5);
-            if (scanID > (n_scans - 1) || scanID < 0) ok = false;
-        } else if (n_scans == 32) {
-            scanID = (int)(((double)angle + 92.0 / 3.0) * 3.0 / 4.0);
-            if (scanID > (n_scans - 1) || scanID < 0) ok = false;
-        } else {
-            if ((double)angle >= -8.83) scanID = (int)((double)(2.0f - angle) * 3.0 + 0.5);
-            else scanID = n_scans / 2 + (int)((-8.83 - (double)angle) * 2.0 + 0.5);
-            if (angle > 2.0f || (double)angle < -24.33 || scanID > 50 || scanID < 0) ok = false;
-        }
+        const int scanID = rings ? (rings[i] < (unsigned)n_scans ? (int)rings[i] : -1) : rot_table_scan_id(a, n_scans);
         o = -det_atan2f(a.y, a.x);                                                                          // :349
-        if (ok) key = (uint32_t)scanID;
+        if (scanID >= 0) key = (uint32_t)scanID;
     }
     keys[i] = key;
     vals[i] = i;
@@ -450,11 +462,12 @@ __global__ void k_rot_lf_init(int* ringmm) {
 }
 
 __global__ void k_rot_lf_gather(const Pt32* __restrict__ cloud, const uint32_t* __restrict__ skeys, const int* __restrict__ lessflat,
-                                const int* __restrict__ lfpos, int n, int* __restrict__ lf_src, int* __restrict__ ringmm, int* __restrict__ meta) {
+                                const int* __restrict__ lfpos, int n, int n_rings, int* __restrict__ lf_src, int* __restrict__ ringmm,
+                                int* __restrict__ meta) {
     // per-ring boxes: block-local in shared memory first (the cloud is ring-major, so a block meets one to three rings), then one
     // set of global atomics per ring the block saw — per-point global atomics on 64 x 7 words cost this kernel 38 us
     __shared__ int s_mm[ROT_MAX_RINGS * 8];
-    for (int t = threadIdx.x; t < ROT_MAX_RINGS * 8; t += blockDim.x) s_mm[t] = vg_box_empty(t & 7);
+    for (int t = threadIdx.x; t < n_rings * 8; t += blockDim.x) s_mm[t] = vg_box_empty(t & 7);
     __syncthreads();
     int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k == 0) meta[M_NLF] = lfpos[n];
@@ -468,7 +481,7 @@ __global__ void k_rot_lf_gather(const Pt32* __restrict__ cloud, const uint32_t* 
         atomicAdd(&mm[6], 1);
     }
     __syncthreads();
-    for (int t = threadIdx.x; t < ROT_MAX_RINGS * 8; t += blockDim.x) {
+    for (int t = threadIdx.x; t < n_rings * 8; t += blockDim.x) {
         const int f = t & 7;
         if (f == 7 || s_mm[(t & ~7) + 6] == 0) continue;          // ring not seen by this block
         vg_box_atomic(&ringmm[t], f, s_mm[t]);
@@ -512,10 +525,13 @@ __global__ void k_rot_lf_centroid(const Pt32* __restrict__ cloud, const int* __r
     vg_write<32>(a.s, a.n, reinterpret_cast<unsigned char*>(out + rank[t]));
 }
 
-// edge output: segment-major, pick order inside the segment (one block, 64*6 = 384 segments)
-__global__ void __launch_bounds__(384) k_rot_edge_emit(const Pt32* __restrict__ cloud, const int* __restrict__ seg_edge,
-                                                       const int* __restrict__ seg_cnt, int nseg, Pt32* __restrict__ edge, int* __restrict__ meta) {
-    __shared__ int wsum[12];
+// edge output: segment-major, pick order inside the segment (one block, one thread per possible segment: 128*6 = 768)
+constexpr int ROT_EMIT_THREADS = ROT_MAX_RINGS * 6;
+__global__ void __launch_bounds__(ROT_EMIT_THREADS) k_rot_edge_emit(const Pt32* __restrict__ cloud, const int* __restrict__ seg_edge,
+                                                                    const int* __restrict__ seg_cnt, int nseg, Pt32* __restrict__ edge,
+                                                                    int* __restrict__ meta) {
+    constexpr int nwarps = ROT_EMIT_THREADS / 32;
+    __shared__ int wsum[nwarps];
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
     int v = t < nseg ? seg_cnt[t] : 0;
     int inc = v;
@@ -523,15 +539,16 @@ __global__ void __launch_bounds__(384) k_rot_edge_emit(const Pt32* __restrict__ 
     for (int o = 1; o < 32; o <<= 1) { int u = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += u; }
     if (lane == 31) wsum[warp] = inc;
     __syncthreads();
-    if (t == 0) { int acc = 0; for (int w = 0; w < 12; ++w) { int x = wsum[w]; wsum[w] = acc; acc += x; } meta[M_NEDGE] = acc; }
+    if (t == 0) { int acc = 0; for (int w = 0; w < nwarps; ++w) { int x = wsum[w]; wsum[w] = acc; acc += x; } meta[M_NEDGE] = acc; }
     __syncthreads();
     const int off = inc - v + wsum[warp];
     for (int e = 0; e < v; ++e) edge[off + e] = cloud[seg_edge[t * 10 + e]];
 }
 
-int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut) {
+int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut,
+                    const uint16_t* rings) {
     const int n_scans = c->prm.line_num;
-    if (n_scans != 16 && n_scans != 32 && n_scans != 64) return LILIOM_E_LINES;
+    if (!rot_lines_ok(n_scans, rings != nullptr)) return LILIOM_E_LINES;
     if (c->prm.ds_rate < 1) return LILIOM_E_ARG;
     *n_surf = *n_edge = *n_cut = 0;
     c->n_surf_dev = 0; c->n_rot_cloud = 0;
@@ -568,7 +585,7 @@ int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_
 
     k_rot_meta_init<<<1, 256, 0, c->stream>>>(meta);
     LILI_TRY(launch_check(c, "k_rot_meta_init"));
-    k_rot_pre<<<cdiv(n, 256), 256, 0, c->stream>>>(raw, n, n_scans, keys, vals, ori, meta);
+    k_rot_pre<<<cdiv(n, 256), 256, 0, c->stream>>>(raw, rings, n, n_scans, keys, vals, ori, meta);
     LILI_TRY(launch_check(c, "k_rot_pre"));
     k_rot_hp<<<cdiv(n, 256), 256, 0, c->stream>>>(raw, n, keys, ori, meta);
     LILI_TRY(launch_check(c, "k_rot_hp"));
@@ -605,7 +622,7 @@ int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_
             }
         }
     }
-    k_rot_edge_emit<<<1, 384, 0, c->stream>>>(cloud, seg_edge, seg_cnt, n_scans * 6, c->edge.as<Pt32>(), meta);
+    k_rot_edge_emit<<<1, ROT_EMIT_THREADS, 0, c->stream>>>(cloud, seg_edge, seg_cnt, n_scans * 6, c->edge.as<Pt32>(), meta);
     LILI_TRY(launch_check(c, "k_rot_edge_emit"));
     // less-flat -> per-ring VoxelGrid
     int* lfpos = c->rot_sort.as<int>();
@@ -613,9 +630,9 @@ int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_
     LILI_TRY(exclusive_scan_i32(c, c->rot_lessflat.as<int>(), lfpos, n));
     k_rot_lf_init<<<cdiv(ROT_MAX_RINGS * 8, 256), 256, 0, c->stream>>>(ringmm);
     LILI_TRY(launch_check(c, "k_rot_lf_init"));
-    k_rot_lf_gather<<<cdiv(n, 256), 256, 0, c->stream>>>(cloud, keys2, c->rot_lessflat.as<int>(), lfpos, n, lf_src, ringmm, meta);
+    k_rot_lf_gather<<<cdiv(n, 256), 256, 0, c->stream>>>(cloud, keys2, c->rot_lessflat.as<int>(), lfpos, n, n_scans, lf_src, ringmm, meta);
     LILI_TRY(launch_check(c, "k_rot_lf_gather"));
-    k_rot_lf_params<<<1, 64, 0, c->stream>>>(ringmm, c->prm.rot_ds_leaf, rprm);
+    k_rot_lf_params<<<1, ROT_MAX_RINGS, 0, c->stream>>>(ringmm, c->prm.rot_ds_leaf, rprm);
     LILI_TRY(launch_check(c, "k_rot_lf_params"));
     unsigned long long* k64 = c->rot_keys.as<unsigned long long>();
     unsigned long long* k64b = c->rot_keys2.as<unsigned long long>();

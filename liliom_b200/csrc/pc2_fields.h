@@ -1,6 +1,8 @@
 // PCL's field tables of the library's two point types and the field matching of pcl::fromROSMsg, for the publishing side
-// (liliom_pc2_layout) and the PointCloud2 ingest (liliom_convert_pc2 / liliom_extract_rot_pc2, liliom_pre_cloud_pc2).
-// Host-only and free of CUDA types, so that the CPU tests compile it as it is (tests/pc2_host.cpp).
+// (liliom_pc2_layout) and the PointCloud2 ingest (liliom_convert_pc2 / liliom_extract_rot_pc2, liliom_pre_cloud_pc2), and the
+// match and read of the driver's per-point `ring` field (LILIOM_RING_FIELD).
+// Free of CUDA types, so that the CPU tests compile it as it is (tests/pc2_host.cpp, tests/pc2_ring_host.cpp); the one
+// function the decode kernel shares with the host (pc2_ring_value) is __host__ __device__ under nvcc.
 #pragma once
 #include <climits>
 #include <cstring>
@@ -8,7 +10,15 @@
 
 namespace lili {
 
+#if defined(__CUDACC__)
+#define PC2_HD __host__ __device__ __forceinline__
+#else
+#define PC2_HD inline
+#endif
+
 constexpr unsigned char kPc2Float32 = 7;       // sensor_msgs::PointField::FLOAT32
+constexpr unsigned char kPc2Uint8 = 2;         // sensor_msgs::PointField::UINT8
+constexpr unsigned char kPc2Uint16 = 4;        // sensor_msgs::PointField::UINT16
 
 // from-knowledge: POINT_CLOUD_REGISTER_POINT_STRUCT of pcl::PointXYZINormal / pcl::PointXYZI (PCL 1.8-1.10), in the order
 // pcl::toROSMsg lists the fields; every field is FLOAT32 with count 1
@@ -20,9 +30,13 @@ constexpr int kPc2Fields32N = 4;
 
 // Where each field of pcl::PointXYZI comes from in one message: src[k] = byte offset inside a point of the message field
 // mapped to kPc2Fields32[k] (x, y, z, intensity), or -1 when no field matches (the point keeps PCL's default value 0).
+// ring_src / ring_bytes: the `ring` field (offset, 1 for UINT8 or 2 for UINT16), matched only when the caller asks for it;
+// -1 / 0 otherwise.
 struct Pc2Map {
     int src[kPc2Fields32N];
     int n;                          // width * height
+    int ring_src = -1;
+    int ring_bytes = 0;
 };
 
 // name equality on the 16-byte, NUL-terminated liliom_pc2_field::name (a name without a NUL in 16 bytes matches nothing)
@@ -36,7 +50,10 @@ inline bool pc2_name_is(const char (&name)[16], const char* want) {
 // match is simply unmapped.  The message itself is input from outside the program: LILIOM_E_ARG for a null msg / data (a
 // non-empty payload) / fields (n_fields > 0), n_fields < 0, point_step 0, row_step < width * point_step, width * height > INT_MAX,
 // a mapped field that does not fit in point_step, or a big-endian payload.
-inline int pc2_match(const liliom_pc2_msg* msg, Pc2Map* out) {
+// want_ring (LILIOM_RING_FIELD): the ring source is the FIRST field named `ring` with datatype UINT8 or UINT16 and count 1 or 0
+// (what Velodyne, Ouster, Hesai and Robosense drivers publish; any other datatype is skipped).  LILIOM_E_ARG, too, when there
+// is no such field or it does not fit in point_step.  Without want_ring the `ring` field is not looked at.
+inline int pc2_match(const liliom_pc2_msg* msg, Pc2Map* out, bool want_ring = false) {
     if (!msg || !out || msg->n_fields < 0 || (msg->n_fields > 0 && !msg->fields)) return LILIOM_E_ARG;
     if (msg->point_step == 0 || msg->is_bigendian != 0) return LILIOM_E_ARG;
     if ((unsigned long long)msg->row_step < (unsigned long long)msg->width * msg->point_step) return LILIOM_E_ARG;
@@ -55,8 +72,27 @@ inline int pc2_match(const liliom_pc2_msg* msg, Pc2Map* out) {
             break;
         }
     }
+    if (want_ring) {
+        for (int f = 0; f < msg->n_fields; ++f) {
+            const liliom_pc2_field& F = msg->fields[f];
+            if (!pc2_name_is(F.name, "ring") || (F.datatype != kPc2Uint8 && F.datatype != kPc2Uint16) || (F.count != 1 && F.count != 0))
+                continue;
+            const int bytes = F.datatype == kPc2Uint16 ? 2 : 1;
+            if ((unsigned long long)F.offset + bytes > msg->point_step) return LILIOM_E_ARG;
+            m.ring_src = (int)F.offset;
+            m.ring_bytes = bytes;
+            break;
+        }
+        if (m.ring_src < 0) return LILIOM_E_ARG;
+    }
     *out = m;
     return LILIOM_OK;
+}
+
+// The ring of one point (its bytes at `point`): the little-endian UINT8 / UINT16 at ring_src, read byte by byte (any offset).
+PC2_HD unsigned pc2_ring_value(const unsigned char* point, int ring_src, int ring_bytes) {
+    const unsigned char* p = point + ring_src;
+    return ring_bytes == 2 ? (unsigned)p[0] | ((unsigned)p[1] << 8) : (unsigned)p[0];
 }
 
 }  // namespace lili

@@ -208,12 +208,31 @@ def hdl64_elevations():
 def make_hdl64_sweep(true_pose7, seed: int = 2, omega=(0.0, 0.0, 0.2), steps: int = 2031, noise=0.02, dropout=0.01, grid: bool = False):
     """~130k-point HDL-64E-like sweep in firing order (azimuth-major, clockwise). Returns (PT32[n], q_imu); grid=True appends
     each return's ring (0..63, the row of hdl64_elevations) and azimuth step (0..steps-1), which organised layouts need."""
+    pts, q_imu, ring, step = make_spinning_sweep(true_pose7, hdl64_elevations(), steps, seed=seed, omega=omega, noise=noise,
+                                                 dropout=dropout)
+    if grid:
+        return pts, q_imu, ring, step
+    return pts, q_imu
+
+
+def uniform_elevations(lines: int = 128, top_deg: float = 22.5, bottom_deg: float = -22.5):
+    """Ring elevations (deg) of a uniform spinning LiDAR numbered from the top, as Ouster numbers its beams: ring 0 at top_deg,
+    ring lines-1 at bottom_deg (an OS-1-128-like fan by default)."""
+    return np.linspace(top_deg, bottom_deg, lines)
+
+
+def make_spinning_sweep(true_pose7, elevations_deg, steps: int, seed: int = 2, omega=(0.0, 0.0, 0.2), noise=0.02, dropout=0.01,
+                        max_range=120.0):
+    """One sweep of a spinning LiDAR with any beam layout: ring r fires at elevations_deg[r], `steps` azimuth columns per turn,
+    in firing order (azimuth-major, clockwise), ray-cast from true_pose7 while the sensor turns at the gyro rate omega.
+    Returns (PT32[n], q_imu, ring[n], step[n]): each return's ring (the index into elevations_deg) and azimuth step, which the
+    driver publishes in its `ring` field and organised layouts need."""
     rng = np.random.default_rng(seed)
-    elev = np.deg2rad(hdl64_elevations())
+    elev = np.deg2rad(np.asarray(elevations_deg, float))
     k = np.arange(steps)
     frac = k / float(steps)
     az = -(2.0 * np.pi * frac) - 0.3        # clockwise: -atan2(y,x) increases with time
-    K, R = np.meshgrid(k, np.arange(64), indexing="ij")
+    K, R = np.meshgrid(k, np.arange(len(elev)), indexing="ij")
     K = K.ravel(); R = R.ravel()
     e = elev[R]; a = az[K]; f = frac[K]
     d_s = np.stack([np.cos(e) * np.cos(a), np.cos(e) * np.sin(a), np.sin(e)], 1)
@@ -222,16 +241,14 @@ def make_hdl64_sweep(true_pose7, seed: int = 2, omega=(0.0, 0.0, 0.2), steps: in
     d_start = _rotate_many(q_t, d_s)
     T = np.asarray(true_pose7, float)
     d_w = _rotate_many(np.broadcast_to(T[:4], (len(d_start), 4)), d_start)
-    rng_m = _raycast(T[4:], d_w, max_range=120.0)
+    rng_m = _raycast(T[4:], d_w, max_range=max_range)
     hit = np.isfinite(rng_m) & (rng.uniform(size=len(rng_m)) >= dropout)
     r = np.where(hit, rng_m, 0.0) + rng.normal(0.0, noise, len(rng_m))
     p = d_s * r[:, None]
     out = np.zeros(int(hit.sum()), PT32)
     out["x"] = p[hit, 0]; out["y"] = p[hit, 1]; out["z"] = p[hit, 2]; out["w"] = 1.0
     out["intensity"] = rng.integers(0, 256, size=len(out)).astype(np.float32)
-    if grid:
-        return out, q_imu, R[hit].astype(np.int32), K[hit].astype(np.int32)
-    return out, q_imu
+    return out, q_imu, R[hit].astype(np.int32), K[hit].astype(np.int32)
 
 
 # ------------------------------------------------------------------ PointCloud2 as spinning-LiDAR drivers publish it
@@ -247,8 +264,9 @@ PC2_LAYOUTS = ("velodyne22", "pcl32", "ouster48", "organised_nan")
 
 
 def encode_pc2(pts, ring, step, layout: str, steps: int = 2031, lines: int = 64) -> PC2:
-    """The sweep pts (PT32, with make_hdl64_sweep(grid=True)'s ring and step per return) as the PointCloud2 a driver of the
-    given layout would publish.  Bytes that no field covers are filled with a non-zero pattern."""
+    """The sweep pts (PT32, with make_hdl64_sweep(grid=True)'s or make_spinning_sweep's ring and step per return) as the
+    PointCloud2 a driver of the given layout would publish; organised layouts are lines x steps.  Bytes that no field covers
+    are filled with a non-zero pattern."""
     F, U8, U16, U32 = PC2_F32, PC2_U8, PC2_U16, PC2_U32
     xyz = [("x", 0, F, 1), ("y", 4, F, 1), ("z", 8, F, 1)]
     organised, pad, missing = False, 0, 0.0

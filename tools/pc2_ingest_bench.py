@@ -8,6 +8,9 @@ For each synthetic driver layout (synth.PC2_LAYOUTS, the seeded 130k-point HDL-6
 Every call is synchronous (the library drains its stream before it returns), so a host clock around each call is the step time.
 Reports the median step time of each path (and of the NumPy decode and of liliom_extract_rot on the decoded pinned cloud alone),
 the host-to-device bytes per sweep, and whether (i) and (ii) give the same bytes.
+Ring-field leg (LILIOM_RING_FIELD, the scanID read from the message's `ring` field): liliom_extract_rot_pc2 from a pinned payload
+on a 128-ring x 1024-column Ouster-like sweep (packed u16 ring and organised u8 ring, line_num 128) and on the 64-ring HDL sweep
+(line_num 64), each at ds_rate 4 (the ROT default) and 1.
 The card's name and power limit are printed with the numbers.
 usage: pc2_ingest_bench.py [--steps K] [--warmup W] [--out FILE]"""
 import argparse
@@ -113,10 +116,11 @@ def main():
         rows.append(row)
         print(json.dumps(row), flush=True)
     ctx.close()
+    ring_rows = ring_leg(a, name, power)
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         with open(a.out, "w") as f:
-            for r in rows:
+            for r in rows + ring_rows:
                 f.write(json.dumps(r) + "\n")
     print(f"\n{'layout':<14} {'B/pt in':>8} {'H2D host':>10} {'H2D pc2':>10} {'decode':>8} {'32B ext':>8} {'(i) host':>9} "
           f"{'(ii) pg':>8} {'(ii) pin':>9} same")
@@ -125,8 +129,44 @@ def main():
               f"{r['extract_rot_pinned_pt32_ms']:>8.3f} {r['host_decode_plus_extract_rot_ms']:>9.3f} {r['extract_rot_pc2_pageable_ms']:>8.3f} {r['extract_rot_pc2_pinned_ms']:>9.3f} "
               f"{r['outputs_identical']}")
     print(f"(ms, median of {a.steps} steps after {a.warmup} warm-up steps; {name}, power limit / max SM clock {power})")
+    print(f"\n{'ring-field leg':<24} {'rings':>5} {'ds':>3} {'points':>7} {'H2D B':>9} {'pinned ms':>9} {'min':>7} {'max':>7} {'edge':>5} {'surf':>6}")
+    for r in ring_rows:
+        print(f"{r['sweep'] + ' ' + r['layout']:<24} {r['line_num']:>5} {r['ds_rate']:>3} {r['points']:>7} {r['h2d_bytes_pc2']:>9} "
+              f"{r['extract_rot_pc2_pinned_ms']:>9.3f} {r['min_max_ms'][0]:>7.3f} {r['min_max_ms'][1]:>7.3f} {r['n_edge']:>5} {r['n_surf']:>6}")
+    print(f"(ms, median of {a.steps} steps after {a.warmup} warm-up steps; {name}, power limit / max SM clock {power})")
     if not all(r["outputs_identical"] for r in rows):
         sys.exit(1)
+
+
+def ring_leg(a, name, power):
+    """liliom_extract_rot_pc2 with the ring taken from the message (LILIOM_RING_FIELD), pinned payload: 128 x 1024 vs the HDL sweep."""
+    T = synth.default_true_pose()
+    p128, q128, r128, s128 = synth.make_spinning_sweep(T, synth.uniform_elevations(128), 1024)
+    p64, q64, r64, s64 = synth.make_hdl64_sweep(T, grid=True)
+    cases = [("128x1024", "velodyne22", synth.encode_pc2(p128, r128, s128, "velodyne22", steps=1024, lines=128), q128, 128),
+             ("128x1024", "ouster48", synth.encode_pc2(p128, r128, s128, "ouster48", steps=1024, lines=128), q128, 128),
+             ("hdl64", "velodyne22", synth.encode_pc2(p64, r64, s64, "velodyne22"), q64, 64)]
+    rows = []
+    q_lb = np.array([1.0, 0.0, 0.0, 0.0])
+    for sweep, layout, msg, q, lines in cases:
+        pin = L.PC2(pinned(msg.data.size)[:msg.data.size], msg.height, msg.width, msg.point_step, msg.row_step, msg.fields)
+        pin.data[:] = msg.data
+        n = msg.width * msg.height
+        outs = [pinned(n * 32)[:n * 32].view(L.PT32) for _ in range(3)]
+        for ds in (4, 1):
+            prm = L.default_params(1)
+            prm.line_num = lines; prm.ds_rate = ds
+            ctx = L.Context(prm)
+            ctx.set_ring_source(L.RING_FIELD)
+            surf, edge, _ = ctx.extract_rot_pc2(pin, q, q_lb, out=outs)
+            t = median_ms(lambda: ctx.extract_rot_pc2(pin, q, q_lb, out=outs), a.steps, a.warmup)
+            row = dict(leg="ring_field", sweep=sweep, layout=layout, line_num=lines, ds_rate=ds, points=n, point_step=msg.point_step,
+                       h2d_bytes_pc2=msg.height * msg.row_step, extract_rot_pc2_pinned_ms=t[0], min_max_ms=t[1:], n_edge=len(edge),
+                       n_surf=len(surf), steps=a.steps, warmup=a.warmup, card=name, power_limit_max_sm_clock=power)
+            rows.append(row)
+            print(json.dumps(row), flush=True)
+            ctx.close()
+    return rows
 
 
 if __name__ == "__main__":
