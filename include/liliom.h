@@ -405,6 +405,32 @@ int liliom_extract_rot_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, const doubl
 enum { LILIOM_RING_ELEVATION = 0, LILIOM_RING_FIELD = 1 };
 int liliom_set_ring_source(liliom_ctx* c, int source);
 
+/* Where the ROT extractor takes each return's relTime from; a second setting of the context beside the ring source (the two
+ * are independent: all four combinations are valid).
+ * LILIOM_TIME_AZIMUTH (the default): the reference's azimuth rule (R/src/Preprocessing.cpp:285-294, 349-367): start / end
+ *   azimuth from the first / last surviving point and the halfPassed latch, which assume the points arrive in firing order.
+ *   On ring-major organised clouds (Ouster, organised Velodyne) the latch fires inside the first ring and relTime is wrong.
+ * LILIOM_TIME_FIELD: from the driver's per-point time field of the PointCloud2, named by field_name (Velodyne "time",
+ *   Ouster "t", Hesai / Robosense "timestamp").  The extraction is the reference's with exactly one substitution:
+ *     relTime = (float)((t_i - t_min) / (t_max - t_min))   (in double; 0 for every point when t_max == t_min)
+ *   where t_min / t_max are the smallest / largest time over the points that survive the NaN / 3 m removal (the set the
+ *   reference takes startOri / endOri from, before the ring filter): the reference's own normalisation, first return 0 and
+ *   last 1, with the time in place of the azimuth, so any unit and any origin work (seconds, nanoseconds, absolute stamps).
+ *   A point whose FLOAT32 / FLOAT64 time is not finite is dropped with the NaN points and does not enter t_min / t_max.
+ *   Everything else (the NaN / 3 m removal, the ring source, intensity = ring + 0.1 * relTime, the de-skew
+ *   q_lb * slerp(I, qIMU, ratio) * q_lb^-1, ring concatenation, curvature, picks, VoxelGrid 0.6) is unchanged.
+ *   - the time field: the FIRST field named field_name (at most 15 characters, matched like the other names) with datatype
+ *     FLOAT32 (7), FLOAT64 (8) or UINT32 (6) and count 1 or 0, read byte by byte and converted exactly to double; a message
+ *     without one, or with one that does not fit in point_step, is refused with LILIOM_E_ARG and changes nothing;
+ *   - liliom_convert_pc2 and liliom_extract_rot_pc2 decode the time with the sweep; liliom_extract_resident uses the times
+ *     decoded with the resident sweep.  After liliom_upload_scan, liliom_convert_livox or any liliom_set_time_source call no
+ *     times are resident and liliom_extract_resident returns LILIOM_E_ARG;
+ *   - liliom_extract_rot (host 32-byte points carry no time) returns LILIOM_E_ARG.
+ * field_name is ignored for LILIOM_TIME_AZIMUTH.  Returns LILIOM_E_ARG for another source, for LILIOM_TIME_FIELD with a NULL
+ * or longer name, or for LILIOM_TIME_FIELD on a context that is not 32-byte (ROT). */
+enum { LILIOM_TIME_AZIMUTH = 0, LILIOM_TIME_FIELD = 1 };
+int liliom_set_time_source(liliom_ctx* c, int source, const char* field_name);
+
 /* ===================== multi-GPU (one context per rank) ===================== */
 /* 128-byte NCCL unique id: rank 0 calls get, the launcher broadcasts it, every rank calls init.
  * After init, liliom_map_set_points shards the map by 16 m block hash (+halo) and every

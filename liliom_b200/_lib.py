@@ -29,6 +29,7 @@ OK, E_ARG, E_CUDA, E_FEWMAP, E_CAPACITY, E_GRID, E_LINES, E_NCCL, E_NOMAP = 0, -
 MODE_CERES, MODE_GN = 0, 1
 KF_FULL, KF_SURF = 0, 1      # liliom_global_map: which stored cloud of each keyframe
 RING_ELEVATION, RING_FIELD = 0, 1   # liliom_set_ring_source: ROT scanID from the elevation tables / the PointCloud2 `ring` field
+TIME_AZIMUTH, TIME_FIELD = 0, 1     # liliom_set_time_source: ROT relTime from the azimuth rule / a PointCloud2 per-point time field
 
 
 class Params(C.Structure):
@@ -75,7 +76,7 @@ EXPORTS = [
     "liliom_backend_default_params", "liliom_kf_add", "liliom_kf_count", "liliom_kf_clear", "liliom_bmap_build",
     "liliom_bmap_download", "liliom_backend_window_correspond", "liliom_backend_window_blocks", "liliom_backend_window_corr",
     "liliom_kf_cloud", "liliom_kf_add_full", "liliom_global_map", "liliom_loop_align",
-    "liliom_convert_pc2", "liliom_extract_rot_pc2", "liliom_set_ring_source",
+    "liliom_convert_pc2", "liliom_extract_rot_pc2", "liliom_set_ring_source", "liliom_set_time_source",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -185,6 +186,7 @@ def lib() -> C.CDLL:
     L.liliom_convert_pc2.argtypes = [vp, C.POINTER(Pc2Msg), vp, C.c_int, ip]
     L.liliom_extract_rot_pc2.argtypes = [vp, C.POINTER(Pc2Msg), dp, dp, vp, C.c_int, ip, vp, C.c_int, ip, vp, C.c_int, ip]
     L.liliom_set_ring_source.argtypes = [vp, C.c_int]
+    L.liliom_set_time_source.argtypes = [vp, C.c_int, C.c_char_p]
     L.liliom_comm_peer_export.argtypes = [vp, vp]
     L.liliom_comm_peer_attach.argtypes = [vp, vp, C.c_int, C.c_int]
     L.liliom_comm_peer_epoch.argtypes = [vp, C.POINTER(C.c_uint)]
@@ -668,6 +670,13 @@ class Context:
         """RING_ELEVATION (default): the ROT extractor takes each return's ring from its elevation (line_num 16/32/64 tables);
         RING_FIELD: from the PointCloud2's `ring` field (convert_pc2 / extract_rot_pc2 / extract_resident, line_num 1..128)."""
         self._check(lib().liliom_set_ring_source(self._h, int(source)))
+
+    def set_time_source(self, source: int, name=None):
+        """TIME_AZIMUTH (default): the ROT extractor takes each return's relTime from the reference's azimuth rule;
+        TIME_FIELD: from the PointCloud2's per-point time field `name` (e.g. "time", "t", "timestamp"), normalised over the
+        surviving returns (convert_pc2 / extract_rot_pc2 / extract_resident)."""
+        nm = name.encode() if isinstance(name, str) else name
+        self._check(lib().liliom_set_time_source(self._h, int(source), nm))
 
     def extract_rot_pc2(self, msg: PC2, q_imu, q_lb=(1.0, 0.0, 0.0, 0.0), out=None):
         """extract_rot on the decoded PointCloud2 without a host cloud in between; out = optional (surf, edge, cut) PT32 arrays."""

@@ -314,6 +314,7 @@ extern "C" int liliom_convert_livox(liliom_ctx* c, const void* custom_pts, int n
     LILI_TRY(livox_to_dev(c, custom_pts, n, stride, c->raw_scan.p));
     c->n_raw_scan = n;
     c->raw_scan_rings = false;
+    c->raw_scan_times = false;
     if (out && n) LILI_CUDA(c, cudaMemcpyAsync(out, c->raw_scan.p, (size_t)n * 48, cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     return LILIOM_OK;
@@ -332,7 +333,8 @@ extern "C" int liliom_extract_horizon_livox(liliom_ctx* c, const void* custom_pt
 
 static int extract_rot_from_raw(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4],
                                 liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
-                                liliom_pt32* cut_out, int cut_cap, int* n_cut, const uint16_t* rings = nullptr);
+                                liliom_pt32* cut_out, int cut_cap, int* n_cut, const uint16_t* rings = nullptr,
+                                const double* times = nullptr);
 
 extern "C" int liliom_extract_rot(liliom_ctx* c, const liliom_pt32* pts, int n, const double q_imu[4], const double q_lb[4],
                                   liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
@@ -340,6 +342,7 @@ extern "C" int liliom_extract_rot(liliom_ctx* c, const liliom_pt32* pts, int n, 
     if (!c || n < 0 || (n > 0 && !pts) || !q_imu || !q_lb || !n_surf || !n_edge || !n_cut) return LILIOM_E_ARG;
     if (c->prm.point_stride != 32) return LILIOM_E_ARG;
     if (c->ring_source == LILIOM_RING_FIELD) return LILIOM_E_ARG;     // host 32-byte points carry no ring
+    if (c->time_source == LILIOM_TIME_FIELD) return LILIOM_E_ARG;     // ... and no time
     LILI_CUDA(c, cudaSetDevice(c->device));
     LILI_CUDA(c, c->raw.ensure((size_t)(n > 0 ? n : 1) * 32));
     if (n > 0) LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, pts, (size_t)n * 32, cudaMemcpyHostToDevice, c->stream));
@@ -351,8 +354,10 @@ namespace lili {
 // One thread per point, row-major over (row, column).  src = Pc2Map::src of x, y, z, intensity (-1: unmapped -> 0).
 // Kept a pass of its own rather than fused into k_rot_pre: k_rot_hp and k_rot_build read the decoded sweep again.
 // ring_out (LILIOM_RING_FIELD only; nullptr otherwise, a uniform branch): the point's `ring` field (Pc2Map::ring_src / ring_bytes).
+// time_out (LILIOM_TIME_FIELD only; nullptr otherwise, a uniform branch): the point's time field as double (Pc2Map::time_src /
+// time_type).
 __global__ void k_pc2_to_pt32(const unsigned char* __restrict__ in, int n, unsigned width, unsigned point_step, unsigned row_step, int4 src,
-                              float4* __restrict__ out, int2 ring, uint16_t* __restrict__ ring_out) {
+                              float4* __restrict__ out, int2 ring, uint16_t* __restrict__ ring_out, int2 tm, double* __restrict__ time_out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const unsigned r = (unsigned)i / width, col = (unsigned)i - r * width;
@@ -361,34 +366,47 @@ __global__ void k_pc2_to_pt32(const unsigned char* __restrict__ in, int n, unsig
     out[2 * (size_t)i] = make_float4(fld(src.x), fld(src.y), fld(src.z), 1.0f);          // pcl::PointXYZI default ctor: data[3] = 1
     out[2 * (size_t)i + 1] = make_float4(fld(src.w), 0.f, 0.f, 0.f);
     if (ring_out) ring_out[i] = (uint16_t)pc2_ring_value(p, ring.x, ring.y);
+    if (time_out) time_out[i] = pc2_time_value(p, tm.x, tm.y);
 }
 // msg already accepted by pc2_match (m): stage the payload, decode into d_out32 (m.n points of 32 bytes) and, when d_ring is
-// given (m matched with want_ring), the ring ids into d_ring (m.n u16)
-static int pc2_to_dev(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, void* d_out32, uint16_t* d_ring) {
+// given (m matched with want_ring), the ring ids into d_ring (m.n u16), when d_time is given (m matched with a time name), the
+// times into d_time (m.n double)
+static int pc2_to_dev(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, void* d_out32, uint16_t* d_ring, double* d_time) {
     if (m.n <= 0) return LILIOM_OK;
     const size_t bytes = (size_t)msg->height * msg->row_step;
     LILI_CUDA(c, c->wire_in.ensure(bytes));
     LILI_CUDA(c, cudaMemcpyAsync(c->wire_in.p, msg->data, bytes, cudaMemcpyHostToDevice, c->stream));
     k_pc2_to_pt32<<<cdiv(m.n, 256), 256, 0, c->stream>>>((const unsigned char*)c->wire_in.p, m.n, msg->width, msg->point_step, msg->row_step,
                                                           make_int4(m.src[0], m.src[1], m.src[2], m.src[3]), (float4*)d_out32,
-                                                          make_int2(m.ring_src, m.ring_bytes), d_ring);
+                                                          make_int2(m.ring_src, m.ring_bytes), d_ring, make_int2(m.time_src, m.time_type),
+                                                          d_time);
     return launch_check(c, "k_pc2_to_pt32");
 }
 }  // namespace lili
 
+// the name of the time field a context reads (LILIOM_TIME_FIELD), or nullptr (LILIOM_TIME_AZIMUTH: no time field is looked at)
+static const char* time_field_of(const liliom_ctx* c) {
+    return c && c->time_source == LILIOM_TIME_FIELD ? c->time_name : nullptr;
+}
+
 extern "C" int liliom_convert_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, liliom_pt32* out, int cap, int* n) {
     Pc2Map m;
     const bool field = c && c->ring_source == LILIOM_RING_FIELD;
-    if (!c || !n || pc2_match(msg, &m, field) != LILIOM_OK) return LILIOM_E_ARG;
+    const char* tname = time_field_of(c);
+    if (!c || !n || pc2_match(msg, &m, field, tname) != LILIOM_OK) return LILIOM_E_ARG;
     if (c->prm.point_stride != 32) return LILIOM_E_ARG;
     if (out && m.n > cap) { *n = m.n; return LILIOM_E_CAPACITY; }
     LILI_CUDA(c, cudaSetDevice(c->device));
     LILI_CUDA(c, c->raw_scan.ensure((size_t)(m.n > 0 ? m.n : 1) * 32));
     c->raw_scan_rings = false;
+    c->raw_scan_times = false;
     if (field) LILI_CUDA(c, c->raw_scan_ring.ensure((size_t)(m.n > 0 ? m.n : 1) * sizeof(uint16_t)));
-    LILI_TRY(pc2_to_dev(c, msg, m, c->raw_scan.p, field ? c->raw_scan_ring.as<uint16_t>() : nullptr));
+    if (tname) LILI_CUDA(c, c->raw_scan_time.ensure((size_t)(m.n > 0 ? m.n : 1) * sizeof(double)));
+    LILI_TRY(pc2_to_dev(c, msg, m, c->raw_scan.p, field ? c->raw_scan_ring.as<uint16_t>() : nullptr,
+                        tname ? c->raw_scan_time.as<double>() : nullptr));
     c->n_raw_scan = m.n;
     c->raw_scan_rings = field;
+    c->raw_scan_times = tname != nullptr;
     if (out && m.n) LILI_CUDA(c, cudaMemcpyAsync(out, c->raw_scan.p, (size_t)m.n * 32, cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     *n = m.n;
@@ -400,24 +418,28 @@ extern "C" int liliom_extract_rot_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, 
                                       liliom_pt32* cut_out, int cut_cap, int* n_cut) {
     Pc2Map m;
     const bool field = c && c->ring_source == LILIOM_RING_FIELD;
-    if (!c || !q_imu || !q_lb || !n_surf || !n_edge || !n_cut || pc2_match(msg, &m, field) != LILIOM_OK) return LILIOM_E_ARG;
+    const char* tname = time_field_of(c);
+    if (!c || !q_imu || !q_lb || !n_surf || !n_edge || !n_cut || pc2_match(msg, &m, field, tname) != LILIOM_OK) return LILIOM_E_ARG;
     if (c->prm.point_stride != 32) return LILIOM_E_ARG;
     if (field && !rot_lines_ok(c->prm.line_num, true)) return LILIOM_E_LINES;
     LILI_CUDA(c, cudaSetDevice(c->device));
     LILI_CUDA(c, c->raw.ensure((size_t)(m.n > 0 ? m.n : 1) * 32));
     if (field) LILI_CUDA(c, c->raw_ring.ensure((size_t)(m.n > 0 ? m.n : 1) * sizeof(uint16_t)));
+    if (tname) LILI_CUDA(c, c->raw_time.ensure((size_t)(m.n > 0 ? m.n : 1) * sizeof(double)));
     uint16_t* rings = field ? c->raw_ring.as<uint16_t>() : nullptr;
-    LILI_TRY(pc2_to_dev(c, msg, m, c->raw.p, rings));
-    return extract_rot_from_raw(c, m.n, q_imu, q_lb, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut, rings);
+    double* times = tname ? c->raw_time.as<double>() : nullptr;
+    LILI_TRY(pc2_to_dev(c, msg, m, c->raw.p, rings, times));
+    return extract_rot_from_raw(c, m.n, q_imu, q_lb, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut, rings,
+                                times);
 }
 
 // Shared tail of the ROT entry points: c->raw holds n 32-byte points (upload / decode already queued on the stream); rings: their
-// ring ids (LILIOM_RING_FIELD) or nullptr (elevation tables).
+// ring ids (LILIOM_RING_FIELD) or nullptr (elevation tables); times: their times (LILIOM_TIME_FIELD) or nullptr (azimuth rule).
 static int extract_rot_from_raw(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4],
                                 liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
-                                liliom_pt32* cut_out, int cut_cap, int* n_cut, const uint16_t* rings) {
+                                liliom_pt32* cut_out, int cut_cap, int* n_cut, const uint16_t* rings, const double* times) {
     int ns = 0, ne = 0, nc = 0;
-    LILI_TRY(rot_extract_dev(c, n, q_imu, q_lb, &ns, &ne, &nc, rings));
+    LILI_TRY(rot_extract_dev(c, n, q_imu, q_lb, &ns, &ne, &nc, rings, times));
     if ((surf_out && ns > surf_cap) || (edge_out && ne > edge_cap) || (cut_out && nc > cut_cap)) return LILIOM_E_CAPACITY;
     if (surf_out && ns) LILI_CUDA(c, cudaMemcpyAsync(surf_out, c->surf.p, (size_t)ns * 32, cudaMemcpyDeviceToHost, c->stream));
     if (edge_out && ne) LILI_CUDA(c, cudaMemcpyAsync(edge_out, c->edge.p, (size_t)ne * 32, cudaMemcpyDeviceToHost, c->stream));
@@ -834,6 +856,7 @@ extern "C" int liliom_upload_scan(liliom_ctx* c, const void* pts, int n) {
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     c->n_raw_scan = n;
     c->raw_scan_rings = false;
+    c->raw_scan_times = false;
     return LILIOM_OK;
 }
 
@@ -842,6 +865,20 @@ extern "C" int liliom_set_ring_source(liliom_ctx* c, int source) {
     if (source == LILIOM_RING_FIELD && c->prm.point_stride != 32) return LILIOM_E_ARG;
     if (source != c->ring_source) c->raw_scan_rings = false;       // the resident sweep was decoded under the other source
     c->ring_source = source;
+    return LILIOM_OK;
+}
+
+extern "C" int liliom_set_time_source(liliom_ctx* c, int source, const char* field_name) {
+    if (!c || (source != LILIOM_TIME_AZIMUTH && source != LILIOM_TIME_FIELD)) return LILIOM_E_ARG;
+    if (source == LILIOM_TIME_FIELD) {
+        if (c->prm.point_stride != 32 || !field_name) return LILIOM_E_ARG;
+        const size_t len = strnlen(field_name, sizeof(c->time_name));
+        if (len >= sizeof(c->time_name)) return LILIOM_E_ARG;
+        memset(c->time_name, 0, sizeof(c->time_name));
+        memcpy(c->time_name, field_name, len);
+    }
+    c->raw_scan_times = false;       // any call: the resident sweep's times (if any) may belong to another field
+    c->time_source = source;
     return LILIOM_OK;
 }
 
@@ -857,8 +894,11 @@ extern "C" int liliom_extract_resident(liliom_ctx* c, const double q_imu[4], con
     else {
         const double ident[4] = {1, 0, 0, 0};
         const bool field = c->ring_source == LILIOM_RING_FIELD;
+        const bool timed = c->time_source == LILIOM_TIME_FIELD;
         if (field && !c->raw_scan_rings) rc = LILIOM_E_ARG;       // no ring ids decoded with the resident sweep
-        else rc = rot_extract_dev(c, n, q_imu, q_lb ? q_lb : ident, n_surf, n_edge, n_cut, field ? c->raw_scan_ring.as<uint16_t>() : nullptr);
+        else if (timed && !c->raw_scan_times) rc = LILIOM_E_ARG;  // no times decoded with the resident sweep
+        else rc = rot_extract_dev(c, n, q_imu, q_lb ? q_lb : ident, n_surf, n_edge, n_cut, field ? c->raw_scan_ring.as<uint16_t>() : nullptr,
+                                  timed ? c->raw_scan_time.as<double>() : nullptr);
     }
     c->raw_src = nullptr;
     return rc;

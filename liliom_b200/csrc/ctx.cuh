@@ -206,6 +206,11 @@ struct liliom_ctx {
     lili::DevBuf raw_ring;       // LILIOM_RING_FIELD: u16 ring id per point of c->raw (liliom_extract_rot_pc2)
     lili::DevBuf raw_scan_ring;  // ... of the resident sweep (liliom_convert_pc2)
     bool raw_scan_rings = false; // raw_scan_ring holds the ring ids of the resident sweep
+    int time_source = LILIOM_TIME_AZIMUTH;     // liliom_set_time_source
+    char time_name[16] = {};     // LILIOM_TIME_FIELD: the name of the per-point time field
+    lili::DevBuf raw_time;       // LILIOM_TIME_FIELD: double time per point of c->raw (liliom_extract_rot_pc2)
+    lili::DevBuf raw_scan_time;  // ... of the resident sweep (liliom_convert_pc2)
+    bool raw_scan_times = false; // raw_scan_time holds the times of the resident sweep
     int n_rot_cloud = 0;
 
     // ---- voxel grid scratch ----
@@ -378,8 +383,9 @@ int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int
 
 int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf, int* n_edge, int* n_cut, bool sync_counts = true);
 // rings: nullptr = scanID from the elevation tables (line_num 16/32/64), else the u16 ring id of every input point (line_num 1..128)
+// times: nullptr = relTime from the azimuth rule, else the time of every input point (LILIOM_TIME_FIELD)
 int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut,
-                    const uint16_t* rings = nullptr);
+                    const uint16_t* rings = nullptr, const double* times = nullptr);
 bool rot_lines_ok(int line_num, bool field);
 
 int icp_align(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,

@@ -3,11 +3,12 @@
 //
 //   k_rot_pre      removeNaN + removeClosedPointCloud 3.0 m (:280-281), elevation -> scanID
 //                  (:315-347) or the driver's ring id (LILIOM_RING_FIELD), raw azimuth -atan2f(y,x)
-//                  (:349); first/last surviving index
+//                  (:349); first/last surviving index; with the driver's times (LILIOM_TIME_FIELD)
+//                  their min / max over the surviving points instead
 //   k_rot_hp       the sequential `halfPassed` latch (:350-358) as a prefix-min: the first valid
-//                  index whose (un-latched) azimuth passes startOri + pi
+//                  index whose (un-latched) azimuth passes startOri + pi (not launched with times)
 //   (stable sort)  bucket by ring preserving arrival order == laserCloudScans[scanID] (:371,378-382)
-//   k_rot_build    azimuth wrap (:350-365), relTime (:367), intensity (:368), de-skew with
+//   k_rot_build    azimuth wrap (:350-365), relTime (:367; from the time with LILIOM_TIME_FIELD), intensity (:368), de-skew with
 //                  q_lb*slerp*q_lb^-1 (:153-177) -> laserCloud; ring start/end
 //   k_rot_curv     11-point curvature in the literal left-to-right fp32 order (:385-394)
 //   k_rot_ring     one CTA per ring: its 6 segments in order (the picked[] marks of segment j
@@ -23,6 +24,7 @@
 #include "ctx.cuh"
 #include "dev_math.cuh"
 #include "detmath.h"
+#include "pc2_fields.h"
 #include <climits>
 #include <cstdlib>
 #include <cstdint>
@@ -41,16 +43,29 @@ constexpr int ROT_RING_CAP = 16384;        // picked[] bytes per ring in shared 
 constexpr double ROT_PI = 3.14159265358979323846;   // M_PI
 
 // meta layout (ints): [0] first idx, [1] last idx, [2] halfPassed idx, [3] n_valid (cloudSize),
-// [4] error flag, [5] n_lessflat, [6] n_edge, [M_RF..M_RF+ROT_MAX_RINGS) ring_first, [M_RE..M_RE+ROT_MAX_RINGS) ring_end
+// [4] error flag, [5] n_lessflat, [6] n_edge, [M_RF..M_RF+ROT_MAX_RINGS) ring_first, [M_RE..M_RE+ROT_MAX_RINGS) ring_end,
+// [M_TMIN, M_TMAX) / [M_TMAX, M_SIZE): t_min / t_max as 64-bit order keys (LILIOM_TIME_FIELD; 8-byte aligned)
 constexpr int M_FIRST = 0, M_LAST = 1, M_HP = 2, M_NVALID = 3, M_ERR = 4, M_NLF = 5, M_NEDGE = 6, M_RF = 8, M_RE = M_RF + ROT_MAX_RINGS,
-              M_SIZE = M_RE + ROT_MAX_RINGS;
+              M_TMIN = M_RE + ROT_MAX_RINGS, M_TMAX = M_TMIN + 2, M_SIZE = M_TMAX + 2;
+static_assert(M_TMIN % 2 == 0, "the time keys are 8-byte words");
+
+// A double as an unsigned key with the same order (finite values): sign bit flipped for >= 0, every bit for < 0.
+__device__ __forceinline__ unsigned long long rot_time_key(double t) {
+    const unsigned long long b = (unsigned long long)__double_as_longlong(t);
+    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double rot_key_time(unsigned long long k) {
+    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
 
 bool rot_lines_ok(int line_num, bool field) {
     return field ? (line_num >= 1 && line_num <= ROT_MAX_RINGS) : (line_num == 16 || line_num == 32 || line_num == 64);
 }
 
 __global__ void k_rot_meta_init(int* meta) {
-    for (int t = threadIdx.x; t < M_SIZE; t += blockDim.x) meta[t] = t == M_LAST ? -1 : (t == M_FIRST || t == M_HP) ? INT_MAX : 0;
+    // t_min key starts at ~0 (both words -1), t_max key at 0
+    for (int t = threadIdx.x; t < M_SIZE; t += blockDim.x)
+        meta[t] = (t == M_LAST || t == M_TMIN || t == M_TMIN + 1) ? -1 : (t == M_FIRST || t == M_HP) ? INT_MAX : 0;
 }
 
 __device__ __forceinline__ bool rot_keep(float4 a) {
@@ -80,23 +95,51 @@ __device__ __forceinline__ int rot_table_scan_id(float4 a, int n_scans) {
 
 // rings: nullptr = the elevation tables; else the driver's ring id of each point, kept iff < n_scans (LILIOM_RING_FIELD: the
 // only difference between the two modes)
-__global__ void k_rot_pre(const Pt32* __restrict__ pts, const uint16_t* __restrict__ rings, int n, int n_scans, uint32_t* __restrict__ keys,
-                          int* __restrict__ vals, float* __restrict__ ori, int* __restrict__ meta) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    float4 a = pts[i].a;
-    uint32_t key = 255u;
-    float o = 0.f;
-    if (rot_keep(a)) {
-        atomicMin(&meta[M_FIRST], i);
-        atomicMax(&meta[M_LAST], i);
-        const int scanID = rings ? (rings[i] < (unsigned)n_scans ? (int)rings[i] : -1) : rot_table_scan_id(a, n_scans);
-        o = -det_atan2f(a.y, a.x);                                                                          // :349
-        if (scanID >= 0) key = (uint32_t)scanID;
+// kTimed (LILIOM_TIME_FIELD): times[i] is the driver's time of each point; a non-finite time drops the point with the NaN
+// points, the raw azimuth is not needed, and t_min / t_max over the surviving points are reduced per block, then one atomic per
+// block on the order keys.  The azimuth instantiation is the kernel as it was without a time source.
+constexpr int ROT_PRE_THREADS = 256;
+template <bool kTimed>
+__global__ void __launch_bounds__(ROT_PRE_THREADS) k_rot_pre(const Pt32* __restrict__ pts, const uint16_t* __restrict__ rings,
+                                                             const double* __restrict__ times, int n, int n_scans, uint32_t* __restrict__ keys,
+                                                             int* __restrict__ vals, float* __restrict__ ori, int* __restrict__ meta) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (!kTimed && i >= n) return;
+    unsigned long long kmin = ~0ull, kmax = 0ull;
+    if (i < n) {
+        const float4 a = pts[i].a;
+        uint32_t key = 255u;
+        float o = 0.f;
+        const double t = kTimed ? times[i] : 0.0;
+        if (rot_keep(a) && (!kTimed || isfinite(t))) {
+            atomicMin(&meta[M_FIRST], i);
+            atomicMax(&meta[M_LAST], i);
+            const int scanID = rings ? (rings[i] < (unsigned)n_scans ? (int)rings[i] : -1) : rot_table_scan_id(a, n_scans);
+            if (!kTimed) o = -det_atan2f(a.y, a.x);                                                         // :349
+            if (scanID >= 0) key = (uint32_t)scanID;
+            if (kTimed) kmin = kmax = rot_time_key(t);
+        }
+        keys[i] = key;
+        vals[i] = i;
+        ori[i] = o;
     }
-    keys[i] = key;
-    vals[i] = i;
-    ori[i] = o;
+    if (!kTimed) return;
+    __shared__ unsigned long long s_min[ROT_PRE_THREADS / 32], s_max[ROT_PRE_THREADS / 32];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        kmin = min(kmin, __shfl_xor_sync(0xffffffffu, kmin, o));
+        kmax = max(kmax, __shfl_xor_sync(0xffffffffu, kmax, o));
+    }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0) { s_min[warp] = kmin; s_max[warp] = kmax; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < ROT_PRE_THREADS / 32; ++w) { kmin = min(kmin, s_min[w]); kmax = max(kmax, s_max[w]); }
+        if (kmin != ~0ull) {          // the block kept a point
+            atomicMin(reinterpret_cast<unsigned long long*>(meta + M_TMIN), kmin);
+            atomicMax(reinterpret_cast<unsigned long long*>(meta + M_TMAX), kmax);
+        }
+    }
 }
 
 __device__ __forceinline__ void rot_start_end(const Pt32* __restrict__ pts, const int* __restrict__ meta, float& startOri, float& endOri) {
@@ -121,8 +164,11 @@ __global__ void k_rot_hp(const Pt32* __restrict__ pts, int n, const uint32_t* __
     if ((double)(ori - startOri) > ROT_PI) atomicMin(&meta[M_HP], i);
 }
 
+// kTimed: relTime from the point's time over [t_min, t_max] (pc2_rel_time); else from the azimuth rule (:350-367)
+template <bool kTimed>
 __global__ void k_rot_build(const Pt32* __restrict__ pts, int n, const uint32_t* __restrict__ skeys, const int* __restrict__ svals,
-                            const float* __restrict__ ori_raw, Q4 qIMU, Q4 q_lb, Pt32* __restrict__ cloud, int* __restrict__ meta) {
+                            const float* __restrict__ ori_raw, const double* __restrict__ times, Q4 qIMU, Q4 q_lb, Pt32* __restrict__ cloud,
+                            int* __restrict__ meta) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n) return;
     const uint32_t key = skeys[s];
@@ -135,18 +181,25 @@ __global__ void k_rot_build(const Pt32* __restrict__ pts, int n, const uint32_t*
     if (s == n - 1 && key != 255u) { meta[M_RE + key] = n; meta[M_NVALID] = n; }
     if (key == 255u) return;
     const int i = svals[s];
-    float startOri, endOri;
-    rot_start_end(pts, meta, startOri, endOri);
-    float ori = ori_raw[i];
-    if (i <= meta[M_HP]) {                                                                                  // :350-358
-        if ((double)ori < (double)startOri - ROT_PI / 2) ori = (float)((double)ori + 2 * ROT_PI);
-        else if ((double)ori > (double)startOri + ROT_PI * 3 / 2) ori = (float)((double)ori - 2 * ROT_PI);
-    } else {                                                                                                // :359-365
-        ori = (float)((double)ori + 2 * ROT_PI);
-        if ((double)ori < (double)endOri - ROT_PI * 3 / 2) ori = (float)((double)ori + 2 * ROT_PI);
-        else if ((double)ori > (double)endOri + ROT_PI / 2) ori = (float)((double)ori - 2 * ROT_PI);
+    float relTime;
+    if constexpr (kTimed) {                                                                                 // LILIOM_TIME_FIELD
+        const double t_min = rot_key_time(*reinterpret_cast<const unsigned long long*>(meta + M_TMIN));
+        const double t_max = rot_key_time(*reinterpret_cast<const unsigned long long*>(meta + M_TMAX));
+        relTime = pc2_rel_time(times[i], t_min, t_max);
+    } else {
+        float startOri, endOri;
+        rot_start_end(pts, meta, startOri, endOri);
+        float ori = ori_raw[i];
+        if (i <= meta[M_HP]) {                                                                              // :350-358
+            if ((double)ori < (double)startOri - ROT_PI / 2) ori = (float)((double)ori + 2 * ROT_PI);
+            else if ((double)ori > (double)startOri + ROT_PI * 3 / 2) ori = (float)((double)ori - 2 * ROT_PI);
+        } else {                                                                                            // :359-365
+            ori = (float)((double)ori + 2 * ROT_PI);
+            if ((double)ori < (double)endOri - ROT_PI * 3 / 2) ori = (float)((double)ori + 2 * ROT_PI);
+            else if ((double)ori > (double)endOri + ROT_PI / 2) ori = (float)((double)ori - 2 * ROT_PI);
+        }
+        relTime = (ori - startOri) / (endOri - startOri);                                                   // :367
     }
-    const float relTime = (ori - startOri) / (endOri - startOri);                                           // :367
     const float intensity = (float)((double)(int)key + 0.1 * (double)relTime);                              // :368
     // undistortion, :153-177
     const int line = (int)intensity;
@@ -546,7 +599,7 @@ __global__ void __launch_bounds__(ROT_EMIT_THREADS) k_rot_edge_emit(const Pt32* 
 }
 
 int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut,
-                    const uint16_t* rings) {
+                    const uint16_t* rings, const double* times) {
     const int n_scans = c->prm.line_num;
     if (!rot_lines_ok(n_scans, rings != nullptr)) return LILIOM_E_LINES;
     if (c->prm.ds_rate < 1) return LILIOM_E_ARG;
@@ -585,12 +638,18 @@ int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_
 
     k_rot_meta_init<<<1, 256, 0, c->stream>>>(meta);
     LILI_TRY(launch_check(c, "k_rot_meta_init"));
-    k_rot_pre<<<cdiv(n, 256), 256, 0, c->stream>>>(raw, rings, n, n_scans, keys, vals, ori, meta);
-    LILI_TRY(launch_check(c, "k_rot_pre"));
-    k_rot_hp<<<cdiv(n, 256), 256, 0, c->stream>>>(raw, n, keys, ori, meta);
-    LILI_TRY(launch_check(c, "k_rot_hp"));
+    if (times) {
+        k_rot_pre<true><<<cdiv(n, ROT_PRE_THREADS), ROT_PRE_THREADS, 0, c->stream>>>(raw, rings, times, n, n_scans, keys, vals, ori, meta);
+        LILI_TRY(launch_check(c, "k_rot_pre"));
+    } else {
+        k_rot_pre<false><<<cdiv(n, ROT_PRE_THREADS), ROT_PRE_THREADS, 0, c->stream>>>(raw, rings, nullptr, n, n_scans, keys, vals, ori, meta);
+        LILI_TRY(launch_check(c, "k_rot_pre"));
+        k_rot_hp<<<cdiv(n, 256), 256, 0, c->stream>>>(raw, n, keys, ori, meta);     // the halfPassed latch: azimuth rule only
+        LILI_TRY(launch_check(c, "k_rot_hp"));
+    }
     LILI_TRY(sort_pairs_u32(c, keys, keys2, vals, vals2, n, 8));
-    k_rot_build<<<cdiv(n, 128), 128, 0, c->stream>>>(raw, n, keys2, vals2, ori, qI, qL, cloud, meta);
+    if (times) k_rot_build<true><<<cdiv(n, 128), 128, 0, c->stream>>>(raw, n, keys2, vals2, ori, times, qI, qL, cloud, meta);
+    else k_rot_build<false><<<cdiv(n, 128), 128, 0, c->stream>>>(raw, n, keys2, vals2, ori, nullptr, qI, qL, cloud, meta);
     LILI_TRY(launch_check(c, "k_rot_build"));
     k_rot_curv<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(cloud, meta, c->rot_curv.as<float>(), c->rot_label.as<int>(),
                                                         c->rot_lessflat.as<int>(), n);

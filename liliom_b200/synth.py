@@ -252,21 +252,27 @@ def make_spinning_sweep(true_pose7, elevations_deg, steps: int, seed: int = 2, o
 
 
 # ------------------------------------------------------------------ PointCloud2 as spinning-LiDAR drivers publish it
-PC2_F32, PC2_U8, PC2_U16, PC2_U32 = 7, 2, 4, 6      # sensor_msgs::PointField datatypes
-_PC2_NP = {PC2_F32: "<f4", PC2_U8: "u1", PC2_U16: "<u2", PC2_U32: "<u4"}
+PC2_F32, PC2_F64, PC2_U8, PC2_U16, PC2_U32 = 7, 8, 2, 4, 6      # sensor_msgs::PointField datatypes
+_PC2_NP = {PC2_F32: "<f4", PC2_F64: "<f8", PC2_U8: "u1", PC2_U16: "<u2", PC2_U32: "<u4"}
 # Representative driver layouts, described from knowledge of the drivers' published point types (not from their sources):
 #   velodyne22    packed x, y, z, intensity (f32), ring (u16), time (f32): 22 B per point, one row in firing order
 #   pcl32         PCL-aligned 32 B: x, y, z at 0-11, intensity at 16, ring (u16) at 20, the rest padding; one row
 #   ouster48      organised rings x columns (64 x steps), 48 B: x, y, z, intensity (f32) at 16, t (u32), reflectivity (u16),
 #                 ring (u8), ambient (u16), range (u32); (0, 0, 0) for a missing return
 #   organised_nan organised 64 x steps, 16 B points listed intensity first, NaN for a missing return, rows padded by 40 bytes
+#   hesai26       packed x, y, z, intensity (f32), timestamp (f64, absolute seconds) at 16, ring (u16) at 24: 26 B per point,
+#                 one row in firing order
 PC2_LAYOUTS = ("velodyne22", "pcl32", "ouster48", "organised_nan")
+# the per-point time field of the layouts that carry one (LILIOM_TIME_FIELD): a step-k return fires k * 0.1 / steps s into the sweep
+PC2_TIME_FIELDS = {"velodyne22": "time", "ouster48": "t", "hesai26": "timestamp"}
+HESAI_EPOCH = 1.7e9                   # hesai26: absolute stamp of the sweep start, s
 
 
-def encode_pc2(pts, ring, step, layout: str, steps: int = 2031, lines: int = 64) -> PC2:
+def encode_pc2(pts, ring, step, layout: str, steps: int = 2031, lines: int = 64, t0: float = 0.0) -> PC2:
     """The sweep pts (PT32, with make_hdl64_sweep(grid=True)'s or make_spinning_sweep's ring and step per return) as the
     PointCloud2 a driver of the given layout would publish; organised layouts are lines x steps.  Bytes that no field covers
-    are filled with a non-zero pattern."""
+    are filled with a non-zero pattern.  t0: seconds added to every return's time (velodyne22 `time`, ouster48 `t` in whole
+    ns, hesai26 `timestamp`), so that the first return need not be at 0; t0 = 0 leaves the existing layouts as they were."""
     F, U8, U16, U32 = PC2_F32, PC2_U8, PC2_U16, PC2_U32
     xyz = [("x", 0, F, 1), ("y", 4, F, 1), ("z", 8, F, 1)]
     organised, pad, missing = False, 0, 0.0
@@ -281,6 +287,8 @@ def encode_pc2(pts, ring, step, layout: str, steps: int = 2031, lines: int = 64)
     elif layout == "organised_nan":
         fields = [("intensity", 12, F, 1)] + xyz
         point_step, organised, pad, missing = 16, True, 40, np.nan
+    elif layout == "hesai26":
+        fields, point_step = xyz + [("intensity", 12, F, 1), ("timestamp", 16, PC2_F64, 1), ("ring", 24, U16, 1)], 26
     else:
         raise ValueError(f"unknown PointCloud2 layout {layout!r}")
     dt = np.dtype({"names": [f[0] for f in fields], "formats": [_PC2_NP[f[2]] for f in fields],
@@ -299,10 +307,12 @@ def encode_pc2(pts, ring, step, layout: str, steps: int = 2031, lines: int = 64)
     if "ring" in dt.names:
         rec["ring"][idx] = ring
     if layout == "velodyne22":
-        rec["time"][idx] = (step * (0.1 / steps)).astype(np.float32)
+        rec["time"][idx] = (step * (0.1 / steps) + t0).astype(np.float32)
+    if layout == "hesai26":
+        rec["timestamp"][idx] = HESAI_EPOCH + t0 + step * (0.1 / steps)
     if layout == "ouster48":
         r = np.sqrt(pts["x"].astype(np.float64) ** 2 + pts["y"].astype(np.float64) ** 2 + pts["z"].astype(np.float64) ** 2)
-        rec["t"][idx] = step * (100_000_000 // steps)
+        rec["t"][idx] = step * (100_000_000 // steps) + int(round(t0 * 1e9))
         rec["reflectivity"][idx] = pts["intensity"].astype(np.uint16)
         rec["ambient"][idx] = 100
         rec["range"][idx] = np.round(r * 1000.0).astype(np.uint32)

@@ -11,6 +11,9 @@ the host-to-device bytes per sweep, and whether (i) and (ii) give the same bytes
 Ring-field leg (LILIOM_RING_FIELD, the scanID read from the message's `ring` field): liliom_extract_rot_pc2 from a pinned payload
 on a 128-ring x 1024-column Ouster-like sweep (packed u16 ring and organised u8 ring, line_num 128) and on the 64-ring HDL sweep
 (line_num 64), each at ds_rate 4 (the ROT default) and 1.
+Time-field leg (LILIOM_TIME_FIELD, relTime from the message's per-point time field): liliom_extract_rot_pc2 from a pinned payload
+on the 128 x 1024 sweep as velodyne22 (`time`), ouster48 (`t`) and hesai26 (`timestamp`), ring field, line_num 128, ds_rate 4,
+with the azimuth rule and with the time field on the same message, alternated in rounds so that both see the same clock drift.
 The card's name and power limit are printed with the numbers.
 usage: pc2_ingest_bench.py [--steps K] [--warmup W] [--out FILE]"""
 import argparse
@@ -117,10 +120,11 @@ def main():
         print(json.dumps(row), flush=True)
     ctx.close()
     ring_rows = ring_leg(a, name, power)
+    time_rows = time_leg(a, name, power)
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
         with open(a.out, "w") as f:
-            for r in rows + ring_rows:
+            for r in rows + ring_rows + time_rows:
                 f.write(json.dumps(r) + "\n")
     print(f"\n{'layout':<14} {'B/pt in':>8} {'H2D host':>10} {'H2D pc2':>10} {'decode':>8} {'32B ext':>8} {'(i) host':>9} "
           f"{'(ii) pg':>8} {'(ii) pin':>9} same")
@@ -133,6 +137,11 @@ def main():
     for r in ring_rows:
         print(f"{r['sweep'] + ' ' + r['layout']:<24} {r['line_num']:>5} {r['ds_rate']:>3} {r['points']:>7} {r['h2d_bytes_pc2']:>9} "
               f"{r['extract_rot_pc2_pinned_ms']:>9.3f} {r['min_max_ms'][0]:>7.3f} {r['min_max_ms'][1]:>7.3f} {r['n_edge']:>5} {r['n_surf']:>6}")
+    print(f"(ms, median of {a.steps} steps after {a.warmup} warm-up steps; {name}, power limit / max SM clock {power})")
+    print(f"\n{'time-field leg':<24} {'field':>9} {'B/pt':>4} {'azimuth ms':>10} {'time ms':>8} {'delta us':>8} {'edge az/t':>10} {'surf az/t':>12}")
+    for r in time_rows:
+        print(f"{r['sweep'] + ' ' + r['layout']:<24} {r['time_field']:>9} {r['point_step']:>4} {r['azimuth_ms']:>10.3f} {r['time_field_ms']:>8.3f} "
+              f"{(r['time_field_ms'] - r['azimuth_ms']) * 1e3:>8.1f} {str(r['n_edge']):>10} {str(r['n_surf']):>12}")
     print(f"(ms, median of {a.steps} steps after {a.warmup} warm-up steps; {name}, power limit / max SM clock {power})")
     if not all(r["outputs_identical"] for r in rows):
         sys.exit(1)
@@ -165,6 +174,50 @@ def ring_leg(a, name, power):
                        n_surf=len(surf), steps=a.steps, warmup=a.warmup, card=name, power_limit_max_sm_clock=power)
             rows.append(row)
             print(json.dumps(row), flush=True)
+            ctx.close()
+    return rows
+
+
+def time_leg(a, name, power):
+    """liliom_extract_rot_pc2 with relTime from the azimuth rule vs from the message's time field (LILIOM_TIME_FIELD), pinned
+    payload, same message: the 128 x 1024 sweep as velodyne22, ouster48 and hesai26 (ring field, line_num 128, ds_rate 4)."""
+    T = synth.default_true_pose()
+    p128, q128, r128, s128 = synth.make_spinning_sweep(T, synth.uniform_elevations(128), 1024)
+    q_lb = np.array([1.0, 0.0, 0.0, 0.0])
+    rows = []
+    for layout in ("velodyne22", "ouster48", "hesai26"):
+        msg = synth.encode_pc2(p128, r128, s128, layout, steps=1024, lines=128)
+        pin = L.PC2(pinned(msg.data.size)[:msg.data.size], msg.height, msg.width, msg.point_step, msg.row_step, msg.fields)
+        pin.data[:] = msg.data
+        n = msg.width * msg.height
+        field = synth.PC2_TIME_FIELDS[layout]
+        ctxs, outs, counts = [], [], []
+        for timed in (False, True):
+            prm = L.default_params(1)
+            prm.line_num = 128; prm.ds_rate = 4
+            ctx = L.Context(prm)
+            ctx.set_ring_source(L.RING_FIELD)
+            if timed:
+                ctx.set_time_source(L.TIME_FIELD, field)
+            out = [pinned(n * 32)[:n * 32].view(L.PT32) for _ in range(3)]
+            surf, edge, _ = ctx.extract_rot_pc2(pin, q128, q_lb, out=out)
+            ctxs.append(ctx); outs.append(out); counts.append((len(edge), len(surf)))
+        # alternate the two modes in rounds of 10 calls so that clock drift lands on both
+        ts = [[], []]
+        for k in range(a.warmup + a.steps):
+            for j in (0, 1):
+                t0 = time.perf_counter()
+                ctxs[j].extract_rot_pc2(pin, q128, q_lb, out=outs[j])
+                if k >= a.warmup:
+                    ts[j].append((time.perf_counter() - t0) * 1e3)
+        row = dict(leg="time_field", sweep="128x1024", layout=layout, time_field=field, line_num=128, ds_rate=4, points=n,
+                   point_step=msg.point_step, h2d_bytes_pc2=msg.height * msg.row_step, azimuth_ms=float(np.median(ts[0])),
+                   time_field_ms=float(np.median(ts[1])), min_max_ms={"azimuth": [min(ts[0]), max(ts[0])], "time_field": [min(ts[1]), max(ts[1])]},
+                   n_edge=[counts[0][0], counts[1][0]], n_surf=[counts[0][1], counts[1][1]], steps=a.steps, warmup=a.warmup, card=name,
+                   power_limit_max_sm_clock=power)
+        rows.append(row)
+        print(json.dumps(row), flush=True)
+        for ctx in ctxs:
             ctx.close()
     return rows
 
