@@ -125,8 +125,9 @@ __device__ __forceinline__ void eig3_step(Eig3State& S, double& x, double& z, bo
     }
 }
 
-__device__ inline void eigen_sym3(double a00, double a10, double a20, double a11, double a21, double a22,
-                                  double eval[3], double evec[3][3]) {
+// Returns the eigenvalues (ascending) in d0..d2 and eigenvector c in column c of q: a value, so that a caller that picks a
+// column at run time does not force the result through local memory (eigen_sym3 below is the array form).
+__device__ __forceinline__ Eig3State eigen_sym3_s(double a00, double a10, double a20, double a11, double a21, double a22) {
     double scale = fmax(fmax(fmax(fabs(a00), fabs(a10)), fmax(fabs(a20), fabs(a11))), fmax(fabs(a21), fabs(a22)));
     if (scale == 0.0) scale = 1.0;
     a00 /= scale; a10 /= scale; a20 /= scale; a11 /= scale; a21 /= scale; a22 /= scale;
@@ -200,7 +201,14 @@ __device__ inline void eigen_sym3(double a00, double a10, double a20, double a11
         else if (k == 2) { double t = S.d0; S.d0 = S.d2; S.d2 = t; t = S.q00; S.q00 = S.q02; S.q02 = t; t = S.q10; S.q10 = S.q12; S.q12 = t; t = S.q20; S.q20 = S.q22; S.q22 = t; }
         if (S.d2 < S.d1) { double t = S.d1; S.d1 = S.d2; S.d2 = t; t = S.q01; S.q01 = S.q02; S.q02 = t; t = S.q11; S.q11 = S.q12; S.q12 = t; t = S.q21; S.q21 = S.q22; S.q22 = t; }
     }
-    eval[0] = S.d0 * scale; eval[1] = S.d1 * scale; eval[2] = S.d2 * scale;
+    S.d0 = S.d0 * scale; S.d1 = S.d1 * scale; S.d2 = S.d2 * scale;
+    return S;
+}
+
+__device__ inline void eigen_sym3(double a00, double a10, double a20, double a11, double a21, double a22,
+                                  double eval[3], double evec[3][3]) {
+    const Eig3State S = eigen_sym3_s(a00, a10, a20, a11, a21, a22);
+    eval[0] = S.d0; eval[1] = S.d1; eval[2] = S.d2;
     evec[0][0] = S.q00; evec[0][1] = S.q01; evec[0][2] = S.q02;
     evec[1][0] = S.q10; evec[1][1] = S.q11; evec[1][2] = S.q12;
     evec[2][0] = S.q20; evec[2][1] = S.q21; evec[2][2] = S.q22;

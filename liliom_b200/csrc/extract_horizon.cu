@@ -111,13 +111,32 @@ __device__ __forceinline__ void hz_patch_eval(HzPatchSmem& P, const Pt48* __rest
 #define HZ_ST(i) do { if (st) st[i] = clock64(); } while (0)
     const int i0 = 5 + 6 * patch;
     HzCell* W = P.win;
-    for (int e = lane; e < HZ_LINES * HZ_WIN; e += 32) {
-        int k = e / HZ_WIN, cc = e % HZ_WIN;
+    // the window in two round trips: a lane's (up to three) cell claims first, then the points they name
+    constexpr int WN = (HZ_LINES * HZ_WIN + 31) / 32;
+    int idx[WN];
+#pragma unroll
+    for (int r = 0; r < WN; ++r) {
+        const int e = lane + 32 * r;
+        const int k = e / HZ_WIN, cc = e % HZ_WIN;
         // COHERENT: mat / cut were produced earlier in the same (cooperative) launch by other SMs -> bypass L1
-        int idx = COHERENT ? __ldcg(&mat[k * HZ_COLS + (i0 - 4 + cc)]) : mat[k * HZ_COLS + (i0 - 4 + cc)];
+        idx[r] = HZ_EMPTY;
+        if (e < HZ_LINES * HZ_WIN) idx[r] = COHERENT ? __ldcg(&mat[k * HZ_COLS + (i0 - 4 + cc)]) : mat[k * HZ_COLS + (i0 - 4 + cc)];
+    }
+    float4 pa[WN], pc[WN];
+#pragma unroll
+    for (int r = 0; r < WN; ++r) {
+        if (idx[r] != HZ_EMPTY) {
+            pa[r] = COHERENT ? __ldcg(&cut[idx[r]].a) : cut[idx[r]].a;
+            pc[r] = COHERENT ? __ldcg(&cut[idx[r]].c) : cut[idx[r]].c;
+        }
+    }
+#pragma unroll
+    for (int r = 0; r < WN; ++r) {
+        const int e = lane + 32 * r;
+        if (e >= HZ_LINES * HZ_WIN) break;
         HzCell h{0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-        if (idx != HZ_EMPTY) {
-            float4 a = COHERENT ? __ldcg(&cut[idx].a) : cut[idx].a, c = COHERENT ? __ldcg(&cut[idx].c) : cut[idx].c;
+        if (idx[r] != HZ_EMPTY) {
+            const float4 a = pa[r], c = pc[r];
             h.x = a.x; h.y = a.y; h.z = a.z; h.inten = c.x; h.curv = c.y;
             h.depth = sqrtf(a.x * a.x + a.y * a.y + a.z * a.z);                                   // getDepth :99-102
         }
@@ -217,11 +236,12 @@ __device__ __forceinline__ void hz_patch_eval(HzPatchSmem& P, const Pt48* __rest
         // ---- (5) the two eigen-solves side by side (:298, :351)
         if (lane < 2 && (lane == 0 || nedge > 0)) {
             const double* M = P.cov + 6 * lane;
-            double ev[3], evec[3][3];
-            eigen_sym3(M[0], M[1], M[2], M[3], M[4], M[5], ev, evec);
-            P.ev[3 * lane] = ev[0]; P.ev[3 * lane + 1] = ev[1]; P.ev[3 * lane + 2] = ev[2];
-            const int col = lane == 0 ? 0 : 2;
-            P.nrm[3 * lane] = (float)evec[0][col]; P.nrm[3 * lane + 1] = (float)evec[1][col]; P.nrm[3 * lane + 2] = (float)evec[2][col];
+            const Eig3State E = eigen_sym3_s(M[0], M[1], M[2], M[3], M[4], M[5]);      // in registers (no stack frame)
+            P.ev[3 * lane] = E.d0; P.ev[3 * lane + 1] = E.d1; P.ev[3 * lane + 2] = E.d2;
+            // surf normal: eigenvector 0; edge direction: eigenvector 2 (selected by value, not by a run-time column index)
+            P.nrm[3 * lane] = (float)(lane == 0 ? E.q00 : E.q02);
+            P.nrm[3 * lane + 1] = (float)(lane == 0 ? E.q10 : E.q12);
+            P.nrm[3 * lane + 2] = (float)(lane == 0 ? E.q20 : E.q22);
         }
         __syncwarp();
         HZ_ST(3);  // eigen-solves

@@ -1074,7 +1074,7 @@ static void print_debug_timing(liliom_ctx* c, const long long* dbg, bool persist
     const long long* vs = vg_coop_stamps(c);
     if (vs && cudaMemcpy(t, vs, 7 * sizeof(long long), cudaMemcpyDeviceToHost) == cudaSuccess && t[4] > t[0]) {
         gt[2] = t[5]; gt[3] = t[6];
-        fprintf(stderr, "[k_vg_coop, cycles, block 0] 1 hash insert+barrier %lld, 2 ranks+barrier %lld, 3 group+barrier %lld, 4 centroids %lld\n",
+        fprintf(stderr, "[k_vg_coop, cycles, block 0] 1 hash insert+barrier %lld, 2 box+key staging %lld, 3 first rank %lld, 4 centroids %lld\n",
                 t[1] - t[0], t[2] - t[1], t[3] - t[2], t[4] - t[3]);
     }
     if (cudaMemcpy(t, dbg + 30, 2 * sizeof(long long), cudaMemcpyDeviceToHost) == cudaSuccess) { gt[4] = t[0]; gt[5] = t[1]; }

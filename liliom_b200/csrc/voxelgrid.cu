@@ -91,35 +91,40 @@ __global__ void k_vg_centroid(const unsigned char* __restrict__ pts, const uint3
 // i/j/k differ from the absolute cell coordinate floor(p*inv_leaf) only by the box minimum (exact in fp32
 // below 2^24), so neither (a) nor (b) needs the bounding box:
 //   phase 1  every point inserts its absolute (kz, jy, ix) key into a hash table (64-bit CAS), the first
-//            writer appends the key to a dense list; per-slot member count by atomicAdd; box partials
-//   phase 2  output rank of a voxel = number of listed keys below its key (all pairs, one warp per voxel,
-//            the list is a few KB and L1-resident); member segment start by atomicAdd (scratch order)
-//   phase 3  every point drops its index into its voxel's segment
-//   phase 4  one warp per voxel: members ordered by original index (rank by counting), fp32 sums in that
-//            order — the order of the sort chain and of the oracle — centroid written at the voxel's rank
-// Three grid barriers instead of twelve launch boundaries.  Inputs it declines (|cell coordinate| >= 2^20,
-// PCL's index overflow, a voxel with more than VGC_VCAP members) set VgParams::bail and an output count
-// of 0; the caller re-runs the sort chain.  Semantics otherwise identical to k_vg_* above.
+//            writer appends the key to a dense list; the point's arrival number in its voxel (atomicAdd on
+//            the slot's count) places its index in the slot's fixed-size member bucket; box partials
+//   -------- the one grid barrier
+//   phase 2  every block reduces the box partials itself (VgParams: PCL's overflow test) and stages the key
+//            list in shared memory
+//   phase 3  one warp per voxel: output rank = number of listed keys below its key (all pairs); members read
+//            from the slot's bucket and ordered by original index (rank by counting in shared memory), fp32
+//            sums in that order — the order of the sort chain and of the oracle — centroid written at the rank
+// Inputs it declines (|cell coordinate| >= 2^20, PCL's index overflow, a voxel with more than VGC_VCAP members)
+// set VgParams::bail and an output count of 0; the caller re-runs the sort chain.  Semantics otherwise
+// identical to k_vg_* above.
+// One barrier is enough because every bail condition is final when it is passed: bits 0 (unrepresentable
+// key) and 1 (arrival number VGC_VCAP, i.e. a voxel over VGC_VCAP members) are only set in phase 1, and the
+// overflow test reads the box partials, which phase 1 completes.  So every block takes the same decision, and
+// no block decides to bail on a bit that another block can still set (a block that bailed on a late bit would
+// never reach a later barrier, and the blocks waiting there would spin forever).  After the barrier a warp
+// touches only its own voxel's slot (count, bucket, and handing the slot back) plus data no block writes any
+// more (key list, slots, box partials), so no second barrier is needed either.
 // ---------------------------------------------------------------------------------------
-constexpr int VGC_NCAP = 32768;
+constexpr int VGC_NCAP = 32768;       // point indices fit the 16-bit bucket entries
 constexpr int VGC_T = 65536;          // hash slots (load factor <= 0.5)
-constexpr int VGC_THREADS = 256;
+constexpr int VGC_THREADS = 512;      // 132 x 16 warps: one voxel round covers a down-sampled 24k sweep (1-2k voxels)
 constexpr int VGC_WARPS = VGC_THREADS / 32;
-constexpr int VGC_VCAP = 256;         // members per voxel handled in shared memory
+constexpr int VGC_VCAP = 256;         // members per voxel handled in shared memory (= bucket size)
 constexpr unsigned long long VGC_EMPTY = ~0ull;
 
 struct VgCoopBufs {
     unsigned long long* hkey;   // [T]   voxel key per slot (VGC_EMPTY when free; restored by the kernel itself)
     int* hcnt;                  // [T]   members per slot (0 when free; restored by the kernel itself)
-    int* hoff;                  // [T]   start of the slot's member segment
+    unsigned short* bucket;     // [T][VCAP] point indices of the slot's members, in arrival order
     unsigned long long* ukey;   // [NCAP] dense list of occupied keys (arbitrary order)
     int* uslot;                 // [NCAP] their slots
-    int* urank;                 // [NCAP] their output ranks
-    int* pslot;                 // [NCAP] slot of point i (-1: not finite)
-    int* ppos;                  // [NCAP] arrival number of point i inside its voxel
-    int* members;               // [NCAP] point indices grouped by voxel
     int* mmpart;                // [7][grid] per-block box partials
-    unsigned int* ctl;          // [4][4] rotating {barrier arrivals, bail flag, #voxels, segment cursor}; slot = call & 3
+    unsigned int* ctl;          // [4][4] rotating {barrier arrivals, bail flags, #voxels, spare}; slot = call & 3
 };
 
 static size_t vgc_layout(VgCoopBufs& B, unsigned char* base, int grid) {
@@ -127,13 +132,9 @@ static size_t vgc_layout(VgCoopBufs& B, unsigned char* base, int grid) {
     auto take = [&](size_t bytes) { unsigned char* p = base ? base + off : nullptr; off += (bytes + 255) & ~(size_t)255; return p; };
     B.hkey = (unsigned long long*)take((size_t)VGC_T * 8);
     B.hcnt = (int*)take((size_t)VGC_T * 4);
-    B.hoff = (int*)take((size_t)VGC_T * 4);
+    B.bucket = (unsigned short*)take((size_t)VGC_T * VGC_VCAP * 2);
     B.ukey = (unsigned long long*)take((size_t)VGC_NCAP * 8);
     B.uslot = (int*)take((size_t)VGC_NCAP * 4);
-    B.urank = (int*)take((size_t)VGC_NCAP * 4);
-    B.pslot = (int*)take((size_t)VGC_NCAP * 4);
-    B.ppos = (int*)take((size_t)VGC_NCAP * 4);
-    B.members = (int*)take((size_t)VGC_NCAP * 4);
     B.mmpart = (int*)take((size_t)7 * grid * 4);
     B.ctl = (unsigned int*)take(16 * 4);
     return off;
@@ -150,19 +151,23 @@ __device__ __forceinline__ void vgc_barrier(unsigned int* bar, unsigned int targ
     __syncthreads();
 }
 
-constexpr int VGC_UKEYS = 4032;    // occupied-voxel keys a block can hold in shared memory for phase 2 (static smem limit: 48 KB)
+constexpr int VGC_UKEYS = 8192;    // occupied-voxel keys a block holds in shared memory for the ranks (more: read through L2)
 struct VgCoopSmem {
     int   red[7][VGC_WARPS];
-    int   sidx[VGC_WARPS][VGC_VCAP];
+    int   mm[kBoxInts];
+    unsigned int bail;
+    int   mem[VGC_WARPS][VGC_VCAP];     // a voxel's members in arrival order
+    int   sidx[VGC_WARPS][VGC_VCAP];    // ... in ascending original index
     float stage[VGC_WARPS][32][8];
     unsigned long long ukeys[VGC_UKEYS];
 };
 
 template <int STRIDE>
-__global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __restrict__ pts, int n_max, const int* __restrict__ d_n, float leaf,
+__global__ void __launch_bounds__(VGC_THREADS, 1) k_vg_coop(const unsigned char* __restrict__ pts, int n_max, const int* __restrict__ d_n, float leaf,
                                                          VgCoopBufs B, unsigned int call, VgParams* __restrict__ pp,
                                                          unsigned char* __restrict__ out, int* __restrict__ count_out, float4* __restrict__ feats_out) {
-    __shared__ VgCoopSmem S;
+    extern __shared__ __align__(16) unsigned char vgc_smem[];
+    VgCoopSmem& S = *reinterpret_cast<VgCoopSmem*>(vgc_smem);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const unsigned int G = gridDim.x;
     const int gtid = blockIdx.x * VGC_THREADS + tid, gthreads = G * VGC_THREADS;
@@ -171,23 +176,24 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
     long long* stamp = ((call >> 31) != 0u && blockIdx.x == 0 && tid == 0) ? reinterpret_cast<long long*>(B.ctl + 16) : nullptr;
     call &= 0x7fffffffu;
     if (stamp) { stamp[0] = clock64(); stamp[5] = (long long)globaltimer_ns(); }
-    unsigned int* ctl = B.ctl + 4 * (call & 3u);          // [0] barrier, [1] bail, [2] #voxels, [3] segment cursor
+    unsigned int* ctl = B.ctl + 4 * (call & 3u);          // [0] barrier, [1] bail, [2] #voxels
     if (blockIdx.x == 0 && tid < 4) B.ctl[4 * ((call + 1u) & 3u) + tid] = 0u;   // the next launch's slot (nobody uses it now)
     const int n = d_n ? min(*d_n, n_max) : n_max;
     const float inv_leaf = 1.0f / leaf;
 
-    // ---- phase 1: hash insert + bounding box partials
+    // ---- phase 1: hash insert, member buckets, bounding box partials
     int box[kBoxInts];
 #pragma unroll
     for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_empty(k);
     // (warp-uniform trip count: the first writers of a warp append to the voxel list with ONE atomic per warp — 1-2k atomics on a
-    // single counter were a serial chain of their own)
-    for (int i0 = gtid - lane; i0 < n; i0 += gthreads) {
+    // single counter were a serial chain of their own.  Warp w of block b takes the 32 points of global warp w*G + b: a ~10k-point
+    // scan spreads its loads and atomics over every SM instead of queueing 512 points on each of the first 20 blocks)
+    for (int i0 = (warp * (int)G + (int)blockIdx.x) * 32; i0 < n; i0 += gthreads) {
         const int i = i0 + lane;
         const bool active = i < n;
         float4 v = make_float4(NAN, 0.f, 0.f, 0.f);
         if (active) v = *reinterpret_cast<const float4*>(pts + (size_t)i * STRIDE);
-        int slot = -1, pos = 0;
+        int slot = -1;
         bool won = false;
         unsigned long long wkey = 0;
         if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) {
@@ -204,7 +210,9 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
                     s = (s + 1) & (VGC_T - 1);
                 }
                 slot = (int)s;
-                pos = atomicAdd(&B.hcnt[s], 1);
+                const int pos = atomicAdd(&B.hcnt[s], 1);
+                if (pos < VGC_VCAP) B.bucket[(size_t)s * VGC_VCAP + pos] = (unsigned short)i;
+                else if (pos == VGC_VCAP) atomicOr(&ctl[1], 2u);      // more members than a warp orders in shared memory
             }
         }
         const unsigned wm = __ballot_sync(0xffffffffu, won);
@@ -215,7 +223,6 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
             ubase = __shfl_sync(0xffffffffu, ubase, leader);
             if (won) { const unsigned int u = ubase + (unsigned int)__popc(wm & ((1u << lane) - 1u)); B.ukey[u] = wkey; B.uslot[u] = slot; }
         }
-        if (active) { B.pslot[i] = slot; B.ppos[i] = pos; }
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -235,85 +242,36 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
     vgc_barrier(&ctl[0], G);
     if (stamp) stamp[1] = clock64();
 
-    int U = (int)*reinterpret_cast<volatile unsigned int*>(&ctl[2]);
-    // Only bit 0 (set in phase 1) is final before barrier 1.  Bits 1 and 2 are set DURING phase 2, so a block that leaves the
-    // barrier late could already see them: were it to take the bail path here it would never arrive at barrier 2 and the
-    // blocks that read 0 would spin there forever.  Every block therefore decides on bit 0 alone; the full word is read
-    // again after barrier 2, when it is final for all blocks.
-    unsigned int bail = *reinterpret_cast<volatile unsigned int*>(&ctl[1]) & 1u;
-    if (!bail) {
-        // ---- phase 2: box parameters (block 0), output ranks and member segments
-        if (blockIdx.x == 0 && warp == 0) {
-            int mm[kBoxInts];
+    // ---- phase 2: box parameters (every block, warp 0) and the key list in shared memory (the other warps)
+    const int U = (int)*reinterpret_cast<volatile unsigned int*>(&ctl[2]);
+    unsigned int bail = *reinterpret_cast<volatile unsigned int*>(&ctl[1]);    // final (see above)
+    // rank by counting over ALL listed keys: from shared memory when the list fits (a down-sampled 24k sweep lists 1-2k voxels)
+    const bool in_smem = U <= VGC_UKEYS;
+    if (warp == 0) {
+        int mm[kBoxInts];
 #pragma unroll
-            for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_empty(k);
-            for (unsigned int b = lane; b < G; b += 32) {
+        for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_empty(k);
+        for (unsigned int b = lane; b < G; b += 32) {
 #pragma unroll
-                for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_join(k, mm[k], __ldcg(&B.mmpart[k * G + b]));
-            }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-                for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_join(k, mm[k], __shfl_xor_sync(0xffffffffu, mm[k], o));
-            }
-            if (lane == 0) {
-                VgParams p = vg_params(mm, leaf);
-                if (p.overflow) { p.bail = 1; atomicOr(&ctl[1], 4u); }   // PCL copies the input: sort chain
-                *pp = p;
-                *count_out = p.bail ? 0 : U;
-            }
+            for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_join(k, mm[k], __ldcg(&B.mmpart[k * G + b]));
         }
-        // rank by counting over ALL listed keys: from shared memory when the list fits (a down-sampled 24k sweep lists 1-2k
-        // voxels): when every compare re-read the list through L2 this phase was ~50 dependent L2 round trips per voxel
-        // (LILIOM_DEBUG_TIMING shows the phase's cycles)
-        const bool in_smem = U <= VGC_UKEYS;
-        if (in_smem) {
-            for (int v = tid; v < U; v += VGC_THREADS) S.ukeys[v] = __ldcg(&B.ukey[v]);
-            __syncthreads();
-        }
-        // (block-uniform trip count: the member segments of a block's voxels are carved out of the cursor with ONE atomic per block
-        // and iteration instead of one per voxel on the same word)
-        for (int ub = 0; ub < U; ub += gwarps) {
-            const int u = ub + gwarp;
-            const bool valid = u < U;
-            int below = 0, s = 0, c = 0;
-            if (valid) {
-                const unsigned long long my = in_smem ? S.ukeys[u] : __ldcg(&B.ukey[u]);
-                if (in_smem) {
-#pragma unroll 4
-                    for (int v = lane; v < U; v += 32) below += (S.ukeys[v] < my) ? 1 : 0;
-                } else {
-#pragma unroll 4
-                    for (int v = lane; v < U; v += 32) below += (__ldcg(&B.ukey[v]) < my) ? 1 : 0;
-                }
 #pragma unroll
-                for (int o = 16; o > 0; o >>= 1) below += __shfl_xor_sync(0xffffffffu, below, o);
-                if (lane == 0) {
-                    s = __ldcg(&B.uslot[u]);
-                    c = __ldcg(&B.hcnt[s]);
-                    if (c > VGC_VCAP) atomicOr(&ctl[1], 2u);
-                }
-            }
-            if (lane == 0) S.red[0][warp] = c;                 // (the box partials in S.red were consumed before barrier 1)
-            __syncthreads();
-            if (tid == 0) {
-                int tot = 0;
-                for (int w = 0; w < VGC_WARPS; ++w) tot += S.red[0][w];
-                S.red[1][0] = tot ? (int)atomicAdd(&ctl[3], (unsigned int)tot) : 0;
-            }
-            __syncthreads();
-            if (valid && lane == 0) {
-                int off = S.red[1][0];
-                for (int w = 0; w < warp; ++w) off += S.red[0][w];
-                B.hoff[s] = off;
-                B.urank[u] = below;
-            }
-            __syncthreads();
+        for (int o = 16; o > 0; o >>= 1) {
+#pragma unroll
+            for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_join(k, mm[k], __shfl_xor_sync(0xffffffffu, mm[k], o));
         }
-        vgc_barrier(&ctl[0], 2u * G);
-        if (stamp) stamp[2] = clock64();
-        bail = *reinterpret_cast<volatile unsigned int*>(&ctl[1]);
+        if (lane == 0) {
+            const VgParams p = vg_params(mm, leaf);
+            if (p.overflow) bail |= 4u;                                  // PCL copies the input: sort chain
+            if (blockIdx.x == 0 && !bail) { *pp = p; *count_out = U; }
+            S.bail = bail;
+        }
+    } else if (!bail && in_smem) {
+        for (int v = tid - 32; v < U; v += VGC_THREADS - 32) S.ukeys[v] = __ldcg(&B.ukey[v]);
     }
+    __syncthreads();
+    bail = S.bail;
+    if (stamp) stamp[2] = clock64();
     if (bail) {
         // declined: leave the table clean for the next launch and report an empty result with the bail mark
         for (int s = gtid; s < VGC_T; s += gthreads) { B.hkey[s] = VGC_EMPTY; B.hcnt[s] = 0; }
@@ -328,33 +286,39 @@ __global__ void __launch_bounds__(VGC_THREADS) k_vg_coop(const unsigned char* __
         return;
     }
 
-    // ---- phase 3: group the point indices by voxel
-    for (int i = gtid; i < n; i += gthreads) {
-        const int s = __ldcg(&B.pslot[i]);
-        if (s >= 0) B.members[__ldcg(&B.hoff[s]) + __ldcg(&B.ppos[i])] = i;
-    }
-    vgc_barrier(&ctl[0], 3u * G);
-    if (stamp) stamp[3] = clock64();
-
-    // ---- phase 4: one warp per voxel — members in ascending original index, sequential fp32 sums
+    // ---- phase 3: one warp per voxel — output rank, members in ascending original index, sequential fp32 sums
     constexpr int NF = kVgFields<STRIDE>;
+    int* mem = S.mem[warp];
+    int* sidx = S.sidx[warp];
     for (int u = gwarp; u < U; u += gwarps) {
         const int s = __ldcg(&B.uslot[u]);
-        const int c = __ldcg(&B.hcnt[s]);
-        const int off = __ldcg(&B.hoff[s]);
-        const int o = __ldcg(&B.urank[u]);
+        const int c = __ldcg(&B.hcnt[s]);                    // <= VGC_VCAP (bit 1 otherwise)
+        const unsigned long long my = in_smem ? S.ukeys[u] : __ldcg(&B.ukey[u]);
+        int o = 0;
+        if (in_smem) {
+#pragma unroll 4
+            for (int v = lane; v < U; v += 32) o += (S.ukeys[v] < my) ? 1 : 0;
+        } else {
+#pragma unroll 4
+            for (int v = lane; v < U; v += 32) o += (__ldcg(&B.ukey[v]) < my) ? 1 : 0;
+        }
+#pragma unroll
+        for (int k = 16; k > 0; k >>= 1) o += __shfl_xor_sync(0xffffffffu, o, k);
+        if (stamp && u == gwarp) stamp[3] = clock64();
+        for (int j = lane; j < c; j += 32) mem[j] = __ldcg(&B.bucket[(size_t)s * VGC_VCAP + j]);
+        __syncwarp();
         // order by counting (indices are distinct)
         for (int j = lane; j < c; j += 32) {
-            const int m = __ldcg(&B.members[off + j]);
+            const int m = mem[j];
             int below = 0;
-            for (int k = 0; k < c; ++k) below += (__ldcg(&B.members[off + k]) < m) ? 1 : 0;
-            S.sidx[warp][below] = m;
+            for (int k = 0; k < c; ++k) below += (mem[k] < m) ? 1 : 0;
+            sidx[below] = m;
         }
         __syncwarp();
         float acc = 0.f;       // lane f < NF owns field f
         for (int base = 0; base < c; base += 32) {
             const int j = base + lane;
-            if (j < c) vg_load<STRIDE>(pts + (size_t)S.sidx[warp][j] * STRIDE, S.stage[warp][lane]);
+            if (j < c) vg_load<STRIDE>(pts + (size_t)sidx[j] * STRIDE, S.stage[warp][lane]);
             __syncwarp();
             if (lane < NF) {
                 const int m = min(32, c - base);
@@ -399,6 +363,8 @@ int voxelgrid_coop(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, i
         LILI_CUDA(c, cudaMemsetAsync(c->vg_coop.p, 0, c->vg_coop.cap, c->stream));
         LILI_CUDA(c, cudaMemsetAsync(B.hkey, 0xff, (size_t)VGC_T * 8, c->stream));
         c->vg_coop_calls = 0;
+        LILI_CUDA(c, cudaFuncSetAttribute(k_vg_coop<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VgCoopSmem)));
+        LILI_CUDA(c, cudaFuncSetAttribute(k_vg_coop<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(VgCoopSmem)));
     }
     vgc_layout(B, (unsigned char*)c->vg_coop.p, grid);
     LILI_CUDA(c, c->vg_params.ensure(sizeof(VgParams)));
@@ -408,7 +374,7 @@ int voxelgrid_coop(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, i
     unsigned int call = (c->vg_coop_calls & 0x7fffffffu) | (c->dbg_timing ? 0x80000000u : 0u);
     void* kargs[] = {&in, &n_max, &d_n, &leaf, &B, &call, &pp, &outp, &d_count, &d_feats};
     const void* fn = stride == 48 ? (const void*)k_vg_coop<48> : (const void*)k_vg_coop<32>;
-    LILI_CUDA(c, cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(VGC_THREADS), kargs, 0, c->stream));
+    LILI_CUDA(c, cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(VGC_THREADS), kargs, sizeof(VgCoopSmem), c->stream));
     LILI_TRY(launch_check(c, "k_vg_coop"));
     c->vg_coop_calls++;
     *used = true;
