@@ -313,8 +313,7 @@ extern "C" int liliom_convert_livox(liliom_ctx* c, const void* custom_pts, int n
     LILI_CUDA(c, c->raw_scan.ensure((size_t)(n > 0 ? n : 1) * 48));
     LILI_TRY(livox_to_dev(c, custom_pts, n, stride, c->raw_scan.p));
     c->n_raw_scan = n;
-    c->raw_scan_rings = false;
-    c->raw_scan_times = false;
+    c->raw_scan_side.clear();
     if (out && n) LILI_CUDA(c, cudaMemcpyAsync(out, c->raw_scan.p, (size_t)n * 48, cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     return LILIOM_OK;
@@ -382,31 +381,36 @@ static int pc2_to_dev(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m,
                                                           d_time);
     return launch_check(c, "k_pc2_to_pt32");
 }
-}  // namespace lili
 
-// the name of the time field a context reads (LILIOM_TIME_FIELD), or nullptr (LILIOM_TIME_AZIMUTH: no time field is looked at)
-static const char* time_field_of(const liliom_ctx* c) {
-    return c && c->time_source == LILIOM_TIME_FIELD ? c->time_name : nullptr;
+// pc2_match under the context's sources: the `ring` field under LILIOM_RING_FIELD, the named time field under LILIOM_TIME_FIELD
+static int pc2_match_ctx(const liliom_ctx* c, const liliom_pc2_msg* msg, Pc2Map* m) {
+    return pc2_match(msg, m, c->ring_source == LILIOM_RING_FIELD, c->time_source == LILIOM_TIME_FIELD ? c->time_name : nullptr);
 }
+
+// msg accepted by pc2_match_ctx (m): size out32 and the side buffers of the channels m matched, decode into them and record in
+// side which channels it now holds (none when the decode fails)
+static int pc2_decode(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, DevBuf& out32, Pc2Side& side) {
+    const size_t n = (size_t)(m.n > 0 ? m.n : 1);
+    const bool ring = m.ring_src >= 0, time = m.time_src >= 0;
+    LILI_CUDA(c, out32.ensure(n * 32));
+    side.clear();
+    if (ring) LILI_CUDA(c, side.ring.ensure(n * sizeof(uint16_t)));
+    if (time) LILI_CUDA(c, side.time.ensure(n * sizeof(double)));
+    LILI_TRY(pc2_to_dev(c, msg, m, out32.p, ring ? side.ring.as<uint16_t>() : nullptr, time ? side.time.as<double>() : nullptr));
+    side.has_ring = ring;
+    side.has_time = time;
+    return LILIOM_OK;
+}
+}  // namespace lili
 
 extern "C" int liliom_convert_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, liliom_pt32* out, int cap, int* n) {
     Pc2Map m;
-    const bool field = c && c->ring_source == LILIOM_RING_FIELD;
-    const char* tname = time_field_of(c);
-    if (!c || !n || pc2_match(msg, &m, field, tname) != LILIOM_OK) return LILIOM_E_ARG;
+    if (!c || !n || pc2_match_ctx(c, msg, &m) != LILIOM_OK) return LILIOM_E_ARG;
     if (c->prm.point_stride != 32) return LILIOM_E_ARG;
     if (out && m.n > cap) { *n = m.n; return LILIOM_E_CAPACITY; }
     LILI_CUDA(c, cudaSetDevice(c->device));
-    LILI_CUDA(c, c->raw_scan.ensure((size_t)(m.n > 0 ? m.n : 1) * 32));
-    c->raw_scan_rings = false;
-    c->raw_scan_times = false;
-    if (field) LILI_CUDA(c, c->raw_scan_ring.ensure((size_t)(m.n > 0 ? m.n : 1) * sizeof(uint16_t)));
-    if (tname) LILI_CUDA(c, c->raw_scan_time.ensure((size_t)(m.n > 0 ? m.n : 1) * sizeof(double)));
-    LILI_TRY(pc2_to_dev(c, msg, m, c->raw_scan.p, field ? c->raw_scan_ring.as<uint16_t>() : nullptr,
-                        tname ? c->raw_scan_time.as<double>() : nullptr));
+    LILI_TRY(pc2_decode(c, msg, m, c->raw_scan, c->raw_scan_side));
     c->n_raw_scan = m.n;
-    c->raw_scan_rings = field;
-    c->raw_scan_times = tname != nullptr;
     if (out && m.n) LILI_CUDA(c, cudaMemcpyAsync(out, c->raw_scan.p, (size_t)m.n * 32, cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     *n = m.n;
@@ -417,20 +421,13 @@ extern "C" int liliom_extract_rot_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, 
                                       liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
                                       liliom_pt32* cut_out, int cut_cap, int* n_cut) {
     Pc2Map m;
-    const bool field = c && c->ring_source == LILIOM_RING_FIELD;
-    const char* tname = time_field_of(c);
-    if (!c || !q_imu || !q_lb || !n_surf || !n_edge || !n_cut || pc2_match(msg, &m, field, tname) != LILIOM_OK) return LILIOM_E_ARG;
+    if (!c || !q_imu || !q_lb || !n_surf || !n_edge || !n_cut || pc2_match_ctx(c, msg, &m) != LILIOM_OK) return LILIOM_E_ARG;
     if (c->prm.point_stride != 32) return LILIOM_E_ARG;
-    if (field && !rot_lines_ok(c->prm.line_num, true)) return LILIOM_E_LINES;
+    if (c->ring_source == LILIOM_RING_FIELD && !rot_lines_ok(c->prm.line_num, true)) return LILIOM_E_LINES;
     LILI_CUDA(c, cudaSetDevice(c->device));
-    LILI_CUDA(c, c->raw.ensure((size_t)(m.n > 0 ? m.n : 1) * 32));
-    if (field) LILI_CUDA(c, c->raw_ring.ensure((size_t)(m.n > 0 ? m.n : 1) * sizeof(uint16_t)));
-    if (tname) LILI_CUDA(c, c->raw_time.ensure((size_t)(m.n > 0 ? m.n : 1) * sizeof(double)));
-    uint16_t* rings = field ? c->raw_ring.as<uint16_t>() : nullptr;
-    double* times = tname ? c->raw_time.as<double>() : nullptr;
-    LILI_TRY(pc2_to_dev(c, msg, m, c->raw.p, rings, times));
-    return extract_rot_from_raw(c, m.n, q_imu, q_lb, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut, rings,
-                                times);
+    LILI_TRY(pc2_decode(c, msg, m, c->raw, c->raw_side));
+    return extract_rot_from_raw(c, m.n, q_imu, q_lb, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut,
+                                c->raw_side.rings(), c->raw_side.times());
 }
 
 // Shared tail of the ROT entry points: c->raw holds n 32-byte points (upload / decode already queued on the stream); rings: their
@@ -855,15 +852,14 @@ extern "C" int liliom_upload_scan(liliom_ctx* c, const void* pts, int n) {
     if (n > 0) LILI_CUDA(c, cudaMemcpyAsync(c->raw_scan.p, pts, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     c->n_raw_scan = n;
-    c->raw_scan_rings = false;
-    c->raw_scan_times = false;
+    c->raw_scan_side.clear();
     return LILIOM_OK;
 }
 
 extern "C" int liliom_set_ring_source(liliom_ctx* c, int source) {
     if (!c || (source != LILIOM_RING_ELEVATION && source != LILIOM_RING_FIELD)) return LILIOM_E_ARG;
     if (source == LILIOM_RING_FIELD && c->prm.point_stride != 32) return LILIOM_E_ARG;
-    if (source != c->ring_source) c->raw_scan_rings = false;       // the resident sweep was decoded under the other source
+    if (source != c->ring_source) c->raw_scan_side.has_ring = false;   // the resident sweep was decoded under the other source
     c->ring_source = source;
     return LILIOM_OK;
 }
@@ -877,7 +873,7 @@ extern "C" int liliom_set_time_source(liliom_ctx* c, int source, const char* fie
         memset(c->time_name, 0, sizeof(c->time_name));
         memcpy(c->time_name, field_name, len);
     }
-    c->raw_scan_times = false;       // any call: the resident sweep's times (if any) may belong to another field
+    c->raw_scan_side.has_time = false;   // any call: the resident sweep's times (if any) may belong to another field
     c->time_source = source;
     return LILIOM_OK;
 }
@@ -895,10 +891,11 @@ extern "C" int liliom_extract_resident(liliom_ctx* c, const double q_imu[4], con
         const double ident[4] = {1, 0, 0, 0};
         const bool field = c->ring_source == LILIOM_RING_FIELD;
         const bool timed = c->time_source == LILIOM_TIME_FIELD;
-        if (field && !c->raw_scan_rings) rc = LILIOM_E_ARG;       // no ring ids decoded with the resident sweep
-        else if (timed && !c->raw_scan_times) rc = LILIOM_E_ARG;  // no times decoded with the resident sweep
-        else rc = rot_extract_dev(c, n, q_imu, q_lb ? q_lb : ident, n_surf, n_edge, n_cut, field ? c->raw_scan_ring.as<uint16_t>() : nullptr,
-                                  timed ? c->raw_scan_time.as<double>() : nullptr);
+        const lili::Pc2Side& side = c->raw_scan_side;
+        if (field && !side.has_ring) rc = LILIOM_E_ARG;       // no ring ids decoded with the resident sweep
+        else if (timed && !side.has_time) rc = LILIOM_E_ARG;  // no times decoded with the resident sweep
+        else rc = rot_extract_dev(c, n, q_imu, q_lb ? q_lb : ident, n_surf, n_edge, n_cut, field ? side.rings() : nullptr,
+                                  timed ? side.times() : nullptr);
     }
     c->raw_src = nullptr;
     return rc;

@@ -160,6 +160,18 @@ struct Frame {        // one entry of recent_surf_frames (world frame, point_str
     int mm[kBoxInts] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
 };
 
+// The per-point side channels decoded with one PointCloud2 sweep: the `ring` field (LILIOM_RING_FIELD) and the time field
+// (LILIOM_TIME_FIELD), and whether each buffer holds them for that sweep.
+struct Pc2Side {
+    DevBuf ring;               // u16 ring id per point
+    DevBuf time;               // double time per point
+    bool has_ring = false;
+    bool has_time = false;
+    void clear() { has_ring = has_time = false; }
+    const uint16_t* rings() const { return has_ring ? ring.as<uint16_t>() : nullptr; }
+    const double* times() const { return has_time ? time.as<double>() : nullptr; }
+};
+
 }  // namespace lili
 
 struct liliom_ctx {
@@ -203,14 +215,10 @@ struct liliom_ctx {
     int n_raw_scan = 0;
     const void* raw_src = nullptr; // when set, the extractors read the sweep from here instead of c->raw (resident pipeline: no copy)
     int ring_source = LILIOM_RING_ELEVATION;   // liliom_set_ring_source
-    lili::DevBuf raw_ring;       // LILIOM_RING_FIELD: u16 ring id per point of c->raw (liliom_extract_rot_pc2)
-    lili::DevBuf raw_scan_ring;  // ... of the resident sweep (liliom_convert_pc2)
-    bool raw_scan_rings = false; // raw_scan_ring holds the ring ids of the resident sweep
     int time_source = LILIOM_TIME_AZIMUTH;     // liliom_set_time_source
     char time_name[16] = {};     // LILIOM_TIME_FIELD: the name of the per-point time field
-    lili::DevBuf raw_time;       // LILIOM_TIME_FIELD: double time per point of c->raw (liliom_extract_rot_pc2)
-    lili::DevBuf raw_scan_time;  // ... of the resident sweep (liliom_convert_pc2)
-    bool raw_scan_times = false; // raw_scan_time holds the times of the resident sweep
+    lili::Pc2Side raw_side;      // side channels of c->raw (liliom_extract_rot_pc2)
+    lili::Pc2Side raw_scan_side; // ... of the resident sweep (liliom_convert_pc2)
     int n_rot_cloud = 0;
 
     // ---- voxel grid scratch ----

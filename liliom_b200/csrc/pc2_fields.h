@@ -1,9 +1,8 @@
 // PCL's field tables of the library's two point types and the field matching of pcl::fromROSMsg, for the publishing side
 // (liliom_pc2_layout) and the PointCloud2 ingest (liliom_convert_pc2 / liliom_extract_rot_pc2, liliom_pre_cloud_pc2), the
 // match and read of the driver's per-point `ring` field (LILIOM_RING_FIELD) and of its per-point time field (LILIOM_TIME_FIELD).
-// Free of CUDA types, so that the CPU tests compile it as it is (tests/pc2_host.cpp, tests/pc2_ring_host.cpp,
-// tests/pc2_time_host.cpp); the functions the kernels share with the host (pc2_ring_value, pc2_time_value, pc2_rel_time) are
-// __host__ __device__ under nvcc.
+// Free of CUDA types, so that the CPU tests compile it as it is (tests/pc2_host.cpp); the functions the kernels share with the
+// host (pc2_ring_value, pc2_time_value, pc2_rel_time) are __host__ __device__ under nvcc.
 #pragma once
 #include <climits>
 #include <cstring>
@@ -52,6 +51,26 @@ inline bool pc2_name_is(const char (&name)[16], const char* want) {
     return len < sizeof(name) && memcmp(name, want, len) == 0 && name[len] == '\0';
 }
 
+constexpr unsigned pc2_type_bit(unsigned char datatype) { return datatype < 32 ? 1u << datatype : 0u; }
+
+// The one field rule of pc2_match: the FIRST field whose name is `name`, whose datatype is one of `types` (pc2_type_bit mask) and
+// whose count is 1 or 0.  *off / *type = its offset and datatype, or -1 / 0 when there is none.  LILIOM_E_ARG when that field
+// does not fit in point_step at its datatype's width; a field of another datatype is skipped, so it is never read.
+inline int pc2_find(const liliom_pc2_msg* msg, const char* name, unsigned types, int* off, int* type) {
+    *off = -1;
+    *type = 0;
+    for (int f = 0; f < msg->n_fields; ++f) {
+        const liliom_pc2_field& F = msg->fields[f];
+        if (!pc2_name_is(F.name, name) || !(types & pc2_type_bit(F.datatype)) || (F.count != 1 && F.count != 0)) continue;
+        const int bytes = F.datatype == kPc2Float64 ? 8 : F.datatype == kPc2Uint16 ? 2 : F.datatype == kPc2Uint8 ? 1 : 4;
+        if ((unsigned long long)F.offset + bytes > msg->point_step) return LILIOM_E_ARG;
+        *off = (int)F.offset;
+        *type = F.datatype;
+        break;
+    }
+    return LILIOM_OK;
+}
+
 // from-knowledge: pcl::createMapping / pcl::detail::FieldMatches (PCL 1.8-1.10) — a point field is mapped to the FIRST message
 // field whose name is equal, whose datatype is the point field's (FLOAT32) and whose count is 1 or 0.  A field that does not
 // match is simply unmapped.  The message itself is input from outside the program: LILIOM_E_ARG for a null msg / data (a
@@ -72,41 +91,17 @@ inline int pc2_match(const liliom_pc2_msg* msg, Pc2Map* out, bool want_ring = fa
     if (!msg->data && (unsigned long long)msg->height * msg->row_step > 0) return LILIOM_E_ARG;
     Pc2Map m;
     m.n = (int)n;
-    for (int k = 0; k < kPc2Fields32N; ++k) {
-        m.src[k] = -1;
-        for (int f = 0; f < msg->n_fields; ++f) {
-            const liliom_pc2_field& F = msg->fields[f];
-            if (!pc2_name_is(F.name, kPc2Fields32[k].name) || F.datatype != kPc2Float32 || (F.count != 1 && F.count != 0)) continue;
-            if ((unsigned long long)F.offset + 4 > msg->point_step) return LILIOM_E_ARG;
-            m.src[k] = (int)F.offset;
-            break;
-        }
-    }
+    int type;
+    for (int k = 0; k < kPc2Fields32N; ++k)
+        if (pc2_find(msg, kPc2Fields32[k].name, pc2_type_bit(kPc2Float32), &m.src[k], &type) != LILIOM_OK) return LILIOM_E_ARG;
     if (want_ring) {
-        for (int f = 0; f < msg->n_fields; ++f) {
-            const liliom_pc2_field& F = msg->fields[f];
-            if (!pc2_name_is(F.name, "ring") || (F.datatype != kPc2Uint8 && F.datatype != kPc2Uint16) || (F.count != 1 && F.count != 0))
-                continue;
-            const int bytes = F.datatype == kPc2Uint16 ? 2 : 1;
-            if ((unsigned long long)F.offset + bytes > msg->point_step) return LILIOM_E_ARG;
-            m.ring_src = (int)F.offset;
-            m.ring_bytes = bytes;
-            break;
-        }
-        if (m.ring_src < 0) return LILIOM_E_ARG;
+        if (pc2_find(msg, "ring", pc2_type_bit(kPc2Uint8) | pc2_type_bit(kPc2Uint16), &m.ring_src, &type) != LILIOM_OK || m.ring_src < 0)
+            return LILIOM_E_ARG;
+        m.ring_bytes = type == kPc2Uint16 ? 2 : 1;
     }
     if (time_name) {
-        for (int f = 0; f < msg->n_fields; ++f) {
-            const liliom_pc2_field& F = msg->fields[f];
-            if (!pc2_name_is(F.name, time_name) || (F.count != 1 && F.count != 0)) continue;
-            if (F.datatype != kPc2Float32 && F.datatype != kPc2Float64 && F.datatype != kPc2Uint32) continue;
-            const int bytes = F.datatype == kPc2Float64 ? 8 : 4;
-            if ((unsigned long long)F.offset + bytes > msg->point_step) return LILIOM_E_ARG;
-            m.time_src = (int)F.offset;
-            m.time_type = F.datatype;
-            break;
-        }
-        if (m.time_src < 0) return LILIOM_E_ARG;
+        const unsigned types = pc2_type_bit(kPc2Float32) | pc2_type_bit(kPc2Float64) | pc2_type_bit(kPc2Uint32);
+        if (pc2_find(msg, time_name, types, &m.time_src, &m.time_type) != LILIOM_OK || m.time_src < 0) return LILIOM_E_ARG;
     }
     *out = m;
     return LILIOM_OK;

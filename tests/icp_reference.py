@@ -7,17 +7,14 @@ by pass on it, with the kernel's own arithmetic from the host build of icp_math.
 contracted source transform), im_sums (the kernel's reduction order) and im_step (SVD, Umeyama, composition, convergence).  The
 CPU tier checks both against brute force and NumPy; the GPU tier checks the device against the trace bit for bit."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 from scipy.spatial import cKDTree
 
+import host_build
 from knn_reference import _point_at, fp32_sqdist
 
 F32 = np.float32
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "build", "libicp_math_host.so")
 GO, CONVERGED, STUCK = 0, 1, 2
 DBL_MAX = float(np.finfo(np.float64).max)
 MAX_CORRS = (0.3, 1.0, 1.7, 30.0)
@@ -32,15 +29,8 @@ def host_lib():
     global _lib
     if _lib is not None:
         return _lib
-    src = os.path.join(ROOT, "tests", "icp_math_host.cpp")
-    deps = [src] + [os.path.join(ROOT, "liliom_b200", "csrc", h) for h in ("icp_math.h", "pcl_xform.h", "vg_box.h")]
-    if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(p) for p in deps):
-        os.makedirs(os.path.dirname(SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        tmp = f"{SO}.{os.getpid()}"
-        subprocess.run([gxx, "-O2", "-std=c++17", "-fPIC", "-Wall", "-ffp-contract=off", "-shared", "-o", tmp, src], check=True)
-        os.replace(tmp, SO)
-    L = C.CDLL(SO)
+    L = host_build.load("icp_math_host", ["tests/icp_math_host.cpp"], ["-O2", "-std=c++17", "-fPIC", "-Wall", "-ffp-contract=off"],
+                        deps=[f"liliom_b200/csrc/{h}" for h in ("icp_math.h", "pcl_xform.h", "vg_box.h")])
     dp = np.ctypeslib.ndpointer(np.float64, flags="C")
     fp = np.ctypeslib.ndpointer(np.float32, flags="C")
     ip = np.ctypeslib.ndpointer(np.int32, flags="C")

@@ -3,14 +3,11 @@ INFRASTRUCTURE (the product never imports this).  Built on first use into build/
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "pc2_oracle.cpp")
-SO = os.path.join(ROOT, "build", "libpc2_oracle.so")
+import host_build
+
 PT32 = np.dtype([("x", "f4"), ("y", "f4"), ("z", "f4"), ("w", "f4"), ("intensity", "f4"), ("p0", "f4"), ("p1", "f4"), ("p2", "f4")])
 
 
@@ -24,13 +21,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        if not os.path.exists(SO) or os.path.getmtime(SO) < os.path.getmtime(SRC):
-            os.makedirs(os.path.dirname(SO), exist_ok=True)
-            gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-            tmp = f"{SO}.{os.getpid()}"
-            subprocess.run([gxx, "-O2", "-std=c++17", "-fPIC", "-Wall", "-Wextra", "-shared", "-o", tmp, SRC], check=True)
-            os.replace(tmp, SO)
-        L = C.CDLL(SO)
+        L = host_build.load("pc2_oracle", ["tests/pc2_oracle.cpp"], ["-O2", "-std=c++17", "-fPIC", "-Wall", "-Wextra"])
         L.orc_pc2_to_pt32.argtypes = [C.c_void_p, C.c_uint, C.c_uint, C.c_uint, C.c_uint, C.POINTER(Field), C.c_int, C.c_void_p]
         L.orc_pc2_to_pt32.restype = C.c_int
         _lib = L

@@ -2,25 +2,17 @@
 (tests/bk_window_host.cpp).  The query -> keyframe lookup (empty keyframes included) and the three weight formulas of the
 reference (L/src/BackendFusion.cpp:1581, R/src/BackendFusion.cpp:843, :861) against NumPy restatements at the reference's widths."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "build", "libbk_window_host.so")
+import host_build
 
 
 @pytest.fixture(scope="module")
 def bw():
-    src = os.path.join(ROOT, "tests", "bk_window_host.cpp")
-    deps = [src, os.path.join(ROOT, "liliom_b200", "csrc", "bk_window.h")]
-    if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(p) for p in deps):
-        os.makedirs(os.path.dirname(SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O2", "-std=c++17", "-fPIC", "-Wall", "-ffp-contract=off", "-shared", "-o", SO, src], check=True)
-    L = C.CDLL(SO)
+    L = host_build.load("bk_window_host", ["tests/bk_window_host.cpp"], ["-O2", "-std=c++17", "-fPIC", "-Wall", "-ffp-contract=off"],
+                        deps=["liliom_b200/csrc/bk_window.h"])
     L.bw_find.argtypes = [C.POINTER(C.c_longlong), C.c_int, C.c_longlong]
     L.bw_find.restype = C.c_int
     L.bw_edge_weight.argtypes = [C.c_int, C.c_double, C.c_int]

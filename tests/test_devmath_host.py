@@ -2,28 +2,21 @@
 checked against NumPy and against the oracle's independent copies — the same source the kernels compile, without a GPU."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "build", "libdevmath_host.so")
+import host_build
 
 
 @pytest.fixture(scope="module")
 def dm():
-    src = os.path.join(ROOT, "tests", "devmath_host.cpp")
-    hdr = os.path.join(ROOT, "liliom_b200", "csrc", "dev_math.cuh")
     cuda_inc = "/usr/local/cuda/include"
     if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
         pytest.skip("CUDA headers not found")
-    if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(src), os.path.getmtime(hdr)):
-        os.makedirs(os.path.dirname(SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-D_GNU_SOURCE", "-Wno-attributes", "-I", cuda_inc,
-                        "-shared", "-o", SO, src], check=True)
-    L = C.CDLL(SO)
+    L = host_build.load("devmath_host", ["tests/devmath_host.cpp"],
+                        ["-O2", "-std=c++17", "-fPIC", "-ffp-contract=off", "-D_GNU_SOURCE", "-Wno-attributes", "-I", cuda_inc],
+                        deps=[f"liliom_b200/csrc/{h}" for h in ("dev_math.cuh", "pcl_xform.h", "vg_box.h")])
     dp, fp = C.POINTER(C.c_double), C.POINTER(C.c_float)
     L.dm_plane_fit5.argtypes = [fp, dp]; L.dm_solve6.argtypes = [dp, dp, dp]; L.dm_gn_safe_step.argtypes = [dp, dp, dp]
     L.dm_pose_plus.argtypes = [dp, dp, dp]; L.dm_pose_plus.restype = None

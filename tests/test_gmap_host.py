@@ -4,27 +4,19 @@ stable sort, heads, vg_walk through the transforming loader, the centroid writer
 oracle's voxelgrid(concat(transform_cloud(...))) byte for byte: both point layouts, with and without the pre-transform of
 save_pcd, lists that repeat keyframes, empty clouds, non-finite points, and boxes on both sides of PCL's overflow test."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "build", "libgmap_host.so")
-CSRC = os.path.join(ROOT, "liliom_b200", "csrc")
+import host_build
+
 T_BL = np.array([0.7071, 0.0, 0.0, 0.7071, -0.18, 0.0, -0.095])      # R/config/config_fr_iosb.yaml ql2b_*, tl2b_* (not quite unit)
 
 
 @pytest.fixture(scope="module")
 def gm():
-    src = os.path.join(ROOT, "tests", "gmap_host.cpp")
-    deps = [src] + [os.path.join(CSRC, h) for h in ("kf_table.h", "pcl_xform.h", "vg_box.h")]
-    if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(p) for p in deps):
-        os.makedirs(os.path.dirname(SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O2", "-std=c++17", "-fPIC", "-Wall", "-ffp-contract=off", "-shared", "-o", SO, src], check=True)
-    L = C.CDLL(SO)
+    L = host_build.load("gmap_host", ["tests/gmap_host.cpp"], ["-O2", "-std=c++17", "-fPIC", "-Wall", "-ffp-contract=off"],
+                        deps=[f"liliom_b200/csrc/{h}" for h in ("kf_table.h", "pcl_xform.h", "vg_box.h")])
     vp, llp, ip, dp = C.c_void_p, np.ctypeslib.ndpointer(np.int64, flags="C"), np.ctypeslib.ndpointer(np.int32, flags="C"), C.c_void_p
     L.gm_global_map.argtypes = [vp, C.c_int, llp, ip, C.c_int, dp, dp, C.c_float, vp, C.POINTER(C.c_int)]
     L.gm_global_map.restype = C.c_longlong

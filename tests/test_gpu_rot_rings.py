@@ -89,12 +89,12 @@ def s128(world_small):
 @pytest.mark.parametrize("lines", [16, 32, 64])
 def test_table_identity_on_the_device(hdl, layout, lines):
     import pc2_oracle
-    import rot_rings_oracle as R
+    import rot_oracle as R
     from liliom_b200 import synth
     pts, q, ring, step = hdl
     k = SUBSAMPLE[lines]
     msg = synth.encode_pc2(pts[::k].copy(), ring[::k], step[::k], layout)
-    msg = _set_rings(msg, R.rot_scan_ids(pc2_oracle.pc2_to_pt32(msg), lines))
+    msg = _set_rings(msg, R.scan_ids(pc2_oracle.pc2_to_pt32(msg), lines))
     for ds_rate in (1, 2, 4):
         ce, cf = _ctx(lines, ds_rate, False), _ctx(lines, ds_rate, True)
         want = _extract(ce, msg, q)
@@ -109,7 +109,7 @@ def test_table_identity_on_the_device(hdl, layout, lines):
 @pytest.mark.parametrize("layout", ["velodyne22", "pcl32", "ouster48"])
 def test_128_rings_against_the_oracle(s128, layout, ds_rate):
     import pc2_oracle
-    import rot_rings_oracle as R
+    import rot_oracle as R
     pts, q, ring, step, msgs = s128
     msg = msgs[layout]
     cloud = pc2_oracle.pc2_to_pt32(msg)
@@ -117,7 +117,7 @@ def test_128_rings_against_the_oracle(s128, layout, ds_rate):
     for line_num in (128, 40):
         c = _ctx(line_num, ds_rate, True)
         surf, edge, cut, lab, cur = _extract(c, msg, q)
-        rc, surf_o, edge_o, cut_o, lab_o, cur_o = R.extract_rot_rings(cloud, rings, q, Q_LB, line_num, ds_rate)
+        rc, surf_o, edge_o, cut_o, lab_o, cur_o = R.extract_rot(cloud, q, Q_LB, line_num, ds_rate, rings=rings)
         assert rc == 0
         _fields_equal(cut, cut_o); _fields_equal(edge, edge_o); _fields_equal(surf, surf_o)
         assert np.array_equal(lab, lab_o) and np.array_equal(cur.view(np.uint32), cur_o.view(np.uint32))
@@ -258,7 +258,7 @@ def test_128_beam_sweep_scan_to_map_end_to_end(oracle):
     the tolerance the 64-beam sweep's end-to-end test uses."""
     import liliom_b200 as L
     import pc2_oracle
-    import rot_rings_oracle as R
+    import rot_oracle as R
     from liliom_b200 import synth
     m, _ = synth.make_map(2_000_000)
     T = synth.default_true_pose()
@@ -268,7 +268,7 @@ def test_128_beam_sweep_scan_to_map_end_to_end(oracle):
     c = _ctx(128, 4, True)
     c.map_set_points(m)
     surf, edge, cut = c.extract_rot_pc2(msg, q, (1.0, 0, 0, 0))
-    rc, surf_o, edge_o, cut_o, _, _ = R.extract_rot_rings(pc2_oracle.pc2_to_pt32(msg), ring, q, (1.0, 0, 0, 0), 128, 4)
+    rc, surf_o, edge_o, cut_o, _, _ = R.extract_rot(pc2_oracle.pc2_to_pt32(msg), q, (1.0, 0, 0, 0), 128, 4, rings=ring)
     _fields_equal(surf, surf_o); _fields_equal(edge, edge_o); _fields_equal(cut, cut_o)
     ds_o = oracle.voxelgrid(surf_o, 0.4)
     pose, _, ds = c.odometry(surf, guess, 10, mode=L.MODE_GN)

@@ -71,9 +71,9 @@ def _extract(c, msg, q):
 
 
 def _check_against_oracle(c, msg, q, rings, times, cloud, line_num, ds_rate):
-    import rot_time_oracle as RT
+    import rot_oracle as RT
     surf, edge, cut, lab, cur = _extract(c, msg, q)
-    rc, surf_o, edge_o, cut_o, lab_o, cur_o = RT.extract_rot_timed(cloud, rings, times, q, Q_LB, line_num, ds_rate)
+    rc, surf_o, edge_o, cut_o, lab_o, cur_o = RT.extract_rot(cloud, q, Q_LB, line_num, ds_rate, rings=rings, times=times)
     assert rc == 0
     _fields_equal(cut, cut_o); _fields_equal(edge, edge_o); _fields_equal(surf, surf_o)
     assert np.array_equal(lab, lab_o) and np.array_equal(cur.view(np.uint32), cur_o.view(np.uint32))
@@ -303,7 +303,7 @@ def test_fast_turn_ring_major_sweep_scan_to_map_end_to_end(oracle):
     """The fast-turn ouster48 sweep through the time-field extractor and liliom_odometry (GN, 10 iterations) against a 2 M-point
     map: the oracle's pose on the oracle's clouds within 1e-4 m / 1e-4 rad.  Each mode's distance from the true pose is printed."""
     import liliom_b200 as L
-    import rot_time_oracle as RT
+    import rot_oracle as RT
     from liliom_b200 import synth
     m, _ = synth.make_map(2_000_000)
     T = synth.default_true_pose()
@@ -317,7 +317,7 @@ def test_fast_turn_ring_major_sweep_scan_to_map_end_to_end(oracle):
         c = _ctx(128, 4, True, name)
         c.map_set_points(m)
         surf, edge, cut = c.extract_rot_pc2(msg, q, ident)
-        rc, surf_o, edge_o, cut_o, _, _ = RT.extract_rot_timed(cloud, rings, times if name else None, q, ident, 128, 4)
+        rc, surf_o, edge_o, cut_o, _, _ = RT.extract_rot(cloud, q, ident, 128, 4, rings=rings, times=times if name else None)
         assert rc == 0
         _fields_equal(surf, surf_o); _fields_equal(edge, edge_o); _fields_equal(cut, cut_o)
         ds_o = oracle.voxelgrid(surf_o, 0.4)

@@ -7,30 +7,26 @@ cell block are never inside the gate; every lane of a group ends with the merged
 the device with (tests/knn_reference.py) is itself checked here against the host build."""
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "build", "libknncore_host.so")
+import host_build
+
 F = np.float32
 EMPTY = np.uint64(0xFFFFFFFFFFFFFFFF)
 
 
 @pytest.fixture(scope="module")
 def kc():
-    src = os.path.join(ROOT, "tests", "knncore_host.cpp")
-    hdrs = [os.path.join(ROOT, "liliom_b200", "csrc", h) for h in ("knn_core.cuh", "dev_math.cuh", "ctx.cuh")]
     cuda_inc = "/usr/local/cuda/include"
     if not os.path.exists(os.path.join(cuda_inc, "cuda_runtime.h")):
         pytest.skip("CUDA headers not found")
-    if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(p) for p in [src] + hdrs):
-        os.makedirs(os.path.dirname(SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O2", "-std=c++20", "-pthread", "-fPIC", "-ffp-contract=off", "-frounding-math", "-D_GNU_SOURCE", "-Wno-attributes", "-Wno-unknown-pragmas",
-                        "-I", cuda_inc, "-shared", "-o", SO, src], check=True)
-    L = C.CDLL(SO)
+    L = host_build.load("knncore_host", ["tests/knncore_host.cpp"],
+                        ["-O2", "-std=c++20", "-pthread", "-fPIC", "-ffp-contract=off", "-frounding-math", "-D_GNU_SOURCE", "-Wno-attributes",
+                         "-Wno-unknown-pragmas", "-I", cuda_inc],
+                        deps=[f"liliom_b200/csrc/{h}" for h in ("knn_core.cuh", "dev_math.cuh", "ctx.cuh", "s2m_plan.h", "pcl_xform.h", "vg_box.h")]
+                        + ["include/liliom.h"])
     L.kc_gate_tau.argtypes = [C.c_double]; L.kc_gate_tau.restype = C.c_float
     L.kc_thread_knn5.argtypes = [C.c_float, C.c_float, C.c_float, C.POINTER(C.c_float), C.POINTER(C.c_int), C.c_float,
                                  C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_float, C.POINTER(C.c_uint64)]

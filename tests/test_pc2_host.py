@@ -3,31 +3,19 @@ liliom_b200/csrc/pc2_fields.h compiled for the host (tests/pc2_host.cpp), the CP
 (tests/pc2_oracle.cpp) against a NumPy structured-dtype decode on the synthetic driver layouts, and the publishing-side table
 that now comes from the same header."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "build", "libpc2_host.so")
+import pc2_host
+
 F32, F64, U8, U16 = 7, 8, 2, 4
 E_ARG = -1
 
 
 @pytest.fixture(scope="module")
 def ph():
-    src = os.path.join(ROOT, "tests", "pc2_host.cpp")
-    deps = [src, os.path.join(ROOT, "liliom_b200", "csrc", "pc2_fields.h"), os.path.join(ROOT, "include", "liliom.h")]
-    if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(p) for p in deps):
-        os.makedirs(os.path.dirname(SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O2", "-std=c++17", "-fPIC", "-Wall", "-Wextra", "-shared", "-o", SO, src], check=True)
-    from liliom_b200 import _lib
-    L = C.CDLL(SO)
-    L.ph_match.argtypes = [C.POINTER(_lib.Pc2Msg), C.POINTER(C.c_int)]
-    L.ph_match.restype = C.c_int
-    return L
+    return pc2_host.lib()
 
 
 def _match(ph, fields, point_step, width=10, height=1, row_step=None, is_bigendian=False, data=True, raw_fields=None):

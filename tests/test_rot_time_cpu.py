@@ -1,19 +1,18 @@
 """CPU tier for the ROT extractor's time source LILIOM_TIME_FIELD (relTime from the driver's per-point PointCloud2 time field):
-  - the time field rules of liliom_b200/csrc/pc2_fields.h compiled for the host (tests/pc2_time_host.cpp): matching, refusals,
+  - the time field rules of liliom_b200/csrc/pc2_fields.h compiled for the host (tests/pc2_host.cpp): matching, refusals,
     the per-point read against a NumPy structured-dtype decode on every layout, and the relTime expression;
-  - the timed oracle (tests/rot_time_oracle.cpp): without times it is the untimed oracle byte for byte, and its intensity
-    column is a NumPy restatement of the rule (span 0 and non-finite times included);
+  - the timed oracle (tests/rot_oracle.cpp): without times it is the untimed oracle (orc_extract_rot) byte for byte, and its
+    intensity column is a NumPy restatement of the rule (span 0 and non-finite times included);
   - on a fast-turning ring-major (ouster48) sweep the timed de-skew lands every cutted point where it was at the sweep start,
     which the azimuth rule does not."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "build", "libpc2_time_host.so")
+import pc2_host
+import rot_oracle as RT
+
 F32, F64, U8, U16, I32, U32 = 7, 8, 2, 4, 5, 6
 E_ARG = -1
 Q_LB = np.array([0.999, 0.01, -0.02, 0.03]) / np.linalg.norm([0.999, 0.01, -0.02, 0.03])
@@ -28,21 +27,7 @@ def _same(a, b):
 
 @pytest.fixture(scope="module")
 def pth():
-    src = os.path.join(ROOT, "tests", "pc2_time_host.cpp")
-    deps = [src, os.path.join(ROOT, "liliom_b200", "csrc", "pc2_fields.h"), os.path.join(ROOT, "include", "liliom.h")]
-    if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(p) for p in deps):
-        os.makedirs(os.path.dirname(SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        tmp = f"{SO}.{os.getpid()}"
-        subprocess.run([gxx, "-O2", "-std=c++17", "-fPIC", "-Wall", "-Wextra", "-shared", "-o", tmp, src], check=True)
-        os.replace(tmp, SO)
-    from liliom_b200 import _lib
-    L = C.CDLL(SO)
-    L.pth_match.argtypes = [C.POINTER(_lib.Pc2Msg), C.c_int, C.c_char_p, C.POINTER(C.c_int)]
-    L.pth_decode_times.argtypes = [C.POINTER(_lib.Pc2Msg), C.c_char_p, C.c_void_p]
-    L.pth_rel_times.argtypes = [C.c_void_p, C.c_int, C.c_double, C.c_double, C.c_void_p]
-    L.pth_rel_times.restype = None
-    return L
+    return pc2_host.lib()
 
 
 @pytest.fixture(scope="module")
@@ -55,12 +40,7 @@ XYZI = [("x", 0, F32, 1), ("y", 4, F32, 1), ("z", 8, F32, 1), ("intensity", 12, 
 
 
 def _match(pth, fields, point_step, name="time", want_ring=False, width=10):
-    from liliom_b200 import PC2
-    msg = PC2(np.zeros(max(width * point_step, 1), np.uint8), 1, width, point_step, width * point_step, fields)
-    m, _keep = msg.c_msg()
-    out = (C.c_int * 9)(*([-7] * 9))
-    rc = pth.pth_match(C.byref(m), int(want_ring), None if name is None else name.encode(), out)
-    return rc, tuple(out)
+    return pc2_host.match_sources(pth, fields, point_step, want_ring=want_ring, time_name=name, width=width)
 
 
 def test_each_time_datatype_matches(pth):
@@ -120,7 +100,7 @@ def test_host_time_decode_equals_numpy(pth, sweep128, layout, t0):
     m, _keep = msg.c_msg()
     n = msg.width * msg.height
     got = np.full(n, -1.0)
-    assert pth.pth_decode_times(C.byref(m), name.encode(), got.ctypes.data_as(C.c_void_p)) == n
+    assert pth.ph_decode_times(C.byref(m), name.encode(), got.ctypes.data_as(C.c_void_p)) == n
     want = _numpy_times(msg, name)
     assert np.array_equal(got.view(np.uint64), want.view(np.uint64))
     if layout == "hesai26":                          # 26-byte points: most FLOAT64 stamps are unaligned
@@ -151,7 +131,7 @@ def test_rel_time_expression(pth):
     for t in (rng.uniform(0, 0.1, 1000), 1.7e9 + rng.uniform(0, 0.1, 1000), rng.integers(0, 100_000_000, 1000).astype(np.float64),
               np.full(10, 3.25)):
         got = np.zeros(len(t), np.float32)
-        pth.pth_rel_times(t.ctypes.data_as(C.c_void_p), len(t), t.min(), t.max(), got.ctypes.data_as(C.c_void_p))
+        pth.ph_rel_times(t.ctypes.data_as(C.c_void_p), len(t), t.min(), t.max(), got.ctypes.data_as(C.c_void_p))
         want = _np_rel(t, t.min(), t.max())
         assert np.array_equal(got.view(np.uint32), want.view(np.uint32))
         assert got.min() == 0.0 and got.max() == (1.0 if t.max() > t.min() else 0.0)
@@ -164,24 +144,24 @@ def hdl():
     return synth.make_hdl64_sweep(synth.default_true_pose(), grid=True)
 
 
-def test_timed_oracle_without_times_is_the_untimed_oracle(hdl, sweep128):
-    import rot_rings_oracle as R
-    import rot_time_oracle as RT
+def test_timed_oracle_without_times_is_the_untimed_oracle(oracle, hdl, sweep128):
     pts, q, ring, _step = sweep128
+    hp, hq, _hr, _hs = hdl
+    ids = RT.scan_ids(hp, 64)
+    rings = np.where(ids < 0, 65535, ids)                   # the tables' verdicts as the ring field
     for ds_rate in (1, 4):
-        want = R.extract_rot_rings(pts, ring, q, Q_LB, 128, ds_rate)
-        got = RT.extract_rot_timed(pts, ring, None, q, Q_LB, 128, ds_rate)
+        want = oracle.extract_rot(hp, hq, Q_LB, 64, ds_rate)
+        got = RT.extract_rot(hp, hq, Q_LB, 64, ds_rate, rings=rings, times=None)
         assert got[0] == want[0] == 0
         for g, w in zip(got[1:], want[1:]):
             _same(g, w)
-    hp, hq, _hr, _hs = hdl
-    want = R.extract_rot_tables(hp, hq, Q_LB, 64, 2)
-    got = RT.extract_rot_timed(hp, None, None, hq, Q_LB, 64, 2)
+    want = oracle.extract_rot(hp, hq, Q_LB, 64, 2)
+    got = RT.extract_rot(hp, hq, Q_LB, 64, 2, rings=None, times=None)
     assert got[0] == want[0] == 0
     for g, w in zip(got[1:], want[1:]):
         _same(g, w)
-    assert RT.extract_rot_timed(hp[:100], None, None, hq, Q_LB, 40, 1)[0] == -2      # the tables know 16 / 32 / 64 only
-    assert RT.extract_rot_timed(pts[:100], ring[:100], None, q, Q_LB, 129, 1)[0] == -2
+    assert RT.extract_rot(hp[:100], hq, Q_LB, 40, 1)[0] == -2      # the tables know 16 / 32 / 64 only
+    assert RT.extract_rot(pts[:100], q, Q_LB, 129, 1, rings=ring[:100])[0] == -2
 
 
 def _np_intensity(pts, ring, times, line_num):
@@ -211,10 +191,9 @@ def _times_of(step, kind):
 @pytest.mark.parametrize("kind", ["plain", "equal", "nonfinite"])
 @pytest.mark.parametrize("line_num", [128, 40])
 def test_timed_oracle_intensity_is_the_rule(sweep128, kind, line_num):
-    import rot_time_oracle as RT
     pts, q, ring, step = sweep128
     times = _times_of(step, kind)
-    rc, surf, edge, cut, lab, cur = RT.extract_rot_timed(pts, ring, times, q, Q_LB, line_num, 1)
+    rc, surf, edge, cut, lab, cur = RT.extract_rot(pts, q, Q_LB, line_num, 1, rings=ring, times=times)
     assert rc == 0
     order, inten = _np_intensity(pts, ring, times, line_num)
     assert len(cut) == len(order)
@@ -244,14 +223,13 @@ def _ground_truth(cloud, step, q_imu):
 
 def deskew_errors(timed):
     """(|cutted - truth| / range per cutted point, bound factor angle(qIMU) / (STEPS - 1)) on the fast-turn ouster48 sweep."""
-    import rot_time_oracle as RT
     from liliom_b200 import synth
     pts, q, ring, step = synth.make_spinning_sweep(synth.default_true_pose(), synth.uniform_elevations(128), STEPS, omega=FAST_OMEGA)
     q = q / np.linalg.norm(q)        # a unit rotation: the de-skew rotates by it as given (a non-unit one also scales the point)
     msg = synth.encode_pc2(pts, ring, step, "ouster48", steps=STEPS, lines=128, t0=0.5)
     cloud, rings, times = _decode_organised(msg, "t")
     ident = (1.0, 0.0, 0.0, 0.0)
-    rc, _s, _e, cut, _l, _c = RT.extract_rot_timed(cloud, rings, times if timed else None, q, ident, 128, 1)
+    rc, _s, _e, cut, _l, _c = RT.extract_rot(cloud, q, ident, 128, 1, rings=rings, times=times if timed else None)
     assert rc == 0
     order, _ = _np_intensity(cloud, rings, times, 128)
     assert len(order) == len(cut) and len(cut) > 80_000

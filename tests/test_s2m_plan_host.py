@@ -3,13 +3,11 @@ Which kernel shape runs for a given query count, SM count, mode and rank set is 
 library makes today (measured shapes, DESIGN.md §3), the invariants what every plan must satisfy for its kernels to be valid."""
 import ctypes as C
 import itertools
-import os
-import subprocess
 
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "build", "libs2m_plan_host.so")
+import host_build
+
 GN, CERES = 1, 0
 
 # (n, n_last, dev_count, sm_count, mode, iters, want_corr, nranks, peer, force_lanes, force_rounds, knn_tma)
@@ -37,13 +35,8 @@ TABLE = [
 
 @pytest.fixture(scope="module")
 def sp():
-    src = os.path.join(ROOT, "tests", "s2m_plan_host.cpp")
-    deps = [src, os.path.join(ROOT, "liliom_b200", "csrc", "s2m_plan.h"), os.path.join(ROOT, "include", "liliom.h")]
-    if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(p) for p in deps):
-        os.makedirs(os.path.dirname(SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O2", "-std=c++17", "-fPIC", "-Wall", "-shared", "-o", SO, src], check=True)
-    L = C.CDLL(SO)
+    L = host_build.load("s2m_plan_host", ["tests/s2m_plan_host.cpp"], ["-O2", "-std=c++17", "-fPIC", "-Wall"],
+                        deps=["liliom_b200/csrc/s2m_plan.h", "include/liliom.h"])
     L.sp_plan.argtypes = [C.c_int] * 12 + [C.POINTER(C.c_longlong)]
     L.sp_plan.restype = None
     return L

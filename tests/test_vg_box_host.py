@@ -4,14 +4,12 @@ voxel_grid.hpp), the sort chain's key width and the absolute 21-bit voxel key ag
 leaves the reference uses (0.2, 0.4, 0.6); and the whole sort chain and the ROT extractor's per-ring filter composed from the
 header (voxel index, heads, member walk, pcl::CentroidPoint writer) against the oracle's VoxelGrid, byte for byte."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SO = os.path.join(ROOT, "build", "libvg_box_host.so")
+import host_build
+
 INT_MAX = 2**31 - 1
 LEAVES = (0.2, 0.4, 0.6)
 F = np.float32
@@ -19,13 +17,8 @@ F = np.float32
 
 @pytest.fixture(scope="module")
 def vb():
-    src = os.path.join(ROOT, "tests", "vg_box_host.cpp")
-    deps = [src, os.path.join(ROOT, "liliom_b200", "csrc", "vg_box.h")]
-    if not os.path.exists(SO) or os.path.getmtime(SO) < max(os.path.getmtime(p) for p in deps):
-        os.makedirs(os.path.dirname(SO), exist_ok=True)
-        gxx = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-        subprocess.run([gxx, "-O2", "-std=c++17", "-fPIC", "-Wall", "-ffp-contract=off", "-shared", "-o", SO, src], check=True)
-    L = C.CDLL(SO)
+    L = host_build.load("vg_box_host", ["tests/vg_box_host.cpp"], ["-O2", "-std=c++17", "-fPIC", "-Wall", "-ffp-contract=off"],
+                        deps=["liliom_b200/csrc/vg_box.h"])
     fp, ip = np.ctypeslib.ndpointer(np.float32, flags="C"), np.ctypeslib.ndpointer(np.int32, flags="C")
     L.vb_f2ord.argtypes = [fp, ip, C.c_int]
     L.vb_ord2f.argtypes = [ip, fp, C.c_int]
