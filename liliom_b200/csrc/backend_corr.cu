@@ -41,8 +41,8 @@ __global__ void __launch_bounds__(kBlock) k_backend_edge(const __grid_constant__
     if (qi >= a.start[a.k]) return;   // uniform per octet
     Q4 q; D3 t;
     const float4 f = *reinterpret_cast<const float4*>(bk_query(a, qi, q, t));
-    D3 pw = qrot_x(q, D3{(double)f.x, (double)f.y, (double)f.z});
-    const float sx = (float)addx(pw.x, t.x), sy = (float)addx(pw.y, t.y), sz = (float)addx(pw.z, t.z);
+    const VgXyz pw = pcl_transform_xyz(q, t, f.x, f.y, f.z);
+    const float sx = pw.x, sy = pw.y, sz = pw.z;
     Top5 top;
     top5_init(top);
     unsigned long long cand = 0;
@@ -50,8 +50,8 @@ __global__ void __launch_bounds__(kBlock) k_backend_edge(const __grid_constant__
     if (sub != 0) return;
     bool ok = false;
     float A3[3] = {0, 0, 0}, B3[3] = {0, 0, 0};
-    if (top.k4 != ~0ull && (double)top5_dist(top.k4) < 1.0) {                                        // L:1543
-        const int pos[5] = {top5_index(top.k0), top5_index(top.k1), top5_index(top.k2), top5_index(top.k3), top5_index(top.k4)};
+    if (top5_accepts(top, 1.0)) {                                                                    // L:1543
+        int pos[5]; top5_indices(top, pos);
         double px[5], py[5], pz[5], cx = 0, cy = 0, cz = 0;
         for (int j = 0; j < 5; ++j) {
             float4 m = a.map_orig[pos[j]];
@@ -99,8 +99,8 @@ __global__ void __launch_bounds__(kBlock) k_backend_surf(const __grid_constant__
     Q4 q; D3 t;
     const unsigned char* qp = bk_query(a, qi, q, t);
     const float4 f = *reinterpret_cast<const float4*>(qp);
-    D3 pw = qrot_x(q, D3{(double)f.x, (double)f.y, (double)f.z});
-    const float sx = (float)addx(pw.x, t.x), sy = (float)addx(pw.y, t.y), sz = (float)addx(pw.z, t.z);
+    const VgXyz pw = pcl_transform_xyz(q, t, f.x, f.y, f.z);
+    const float sx = pw.x, sy = pw.y, sz = pw.z;
     Top5 top;
     top5_init(top);
     unsigned long long cand = 0;
@@ -109,8 +109,8 @@ __global__ void __launch_bounds__(kBlock) k_backend_surf(const __grid_constant__
     bool ok = false;
     float4 pl = make_float4(0, 0, 0, 0);
     double sc = 0;
-    if (top.k4 != ~0ull && (double)top5_dist(top.k4) < a.max_sqd) {                                   // R:1476
-        const int pos[5] = {top5_index(top.k0), top5_index(top.k1), top5_index(top.k2), top5_index(top.k3), top5_index(top.k4)};
+    if (top5_accepts(top, a.max_sqd)) {                                                               // R:1476
+        int pos[5]; top5_indices(top, pos);
         double A[5][3], B[5];
         float4 m[5];
         for (int j = 0; j < 5; ++j) { m[j] = a.map_orig[pos[j]]; A[j][0] = m[j].x; A[j][1] = m[j].y; A[j][2] = m[j].z; B[j] = -1.0; }
@@ -133,25 +133,11 @@ __global__ void __launch_bounds__(kBlock) k_backend_surf(const __grid_constant__
         }
         double nv[3] = {0, 0, 0};
         if (!skip) colpiv_qr_solve_5x3(A, B, nv);                                      // R:1484 / L:1641
-        double n2 = nv[0] * nv[0] + nv[1] * nv[1] + nv[2] * nv[2];
-        double nn = sqrt(n2);
-        double normInverse = 1.0 / nn;
-        if (n2 > 0) { nv[0] /= nn; nv[1] /= nn; nv[2] /= nn; }
-        bool planeValid = true;
-        for (int j = 0; j < 5; ++j)                                                    // R:1489-1497
-            if (fabs(nv[0] * m[j].x + nv[1] * m[j].y + nv[2] * m[j].z + normInverse) > a.plane_thres) planeValid = false;
-        if (skip) planeValid = false;
-        if (planeValid) {
-            float pd = (float)addx(addx(addx(mulx(nv[0], (double)sx), mulx(nv[1], (double)sy)), mulx(nv[2], (double)sz)), normInverse);
-            float rng = __fsqrt_rn(__fsqrt_rn(faddx(faddx(fmulx(sx, sx), fmulx(sy, sy)), fmulx(sz, sz))));
-            float weight = (float)subx(1.0, mulx(0.9, (double)fabsf(pd)) / (double)rng);   // R:1502
-            if ((double)weight > a.w_gate) {                                           // R:1504
-                pl = make_float4((float)mulx((double)weight, nv[0]), (float)mulx((double)weight, nv[1]),
-                                 (float)mulx((double)weight, nv[2]), (float)mulx((double)weight, normInverse));
-                sc = a.map_refl ? a.lidar_const * ((double)weight + exp(-sum_w))          // L:1676
-                                : a.lidar_const * (double)weight;                             // R:1515
-                ok = true;
-            }
+        float weight;
+        if (plane_gate(nv, m, sx, sy, sz, a.plane_thres, a.w_gate, skip, pl, weight)) {
+            sc = a.map_refl ? a.lidar_const * ((double)weight + exp(-sum_w))              // L:1676
+                            : a.lidar_const * (double)weight;                                 // R:1515
+            ok = true;
         }
     }
     a.valid[qi] = ok ? 1 : 0;
@@ -281,43 +267,17 @@ __global__ void __launch_bounds__(kBlkThreads) k_backend_block(const BlkSeg* __r
             g = D3{sc * (double)pl.x, sc * (double)pl.y, sc * (double)pl.z};
         }
         const D3 rp = qrot_x(q, pr);
-        double J[6];
-        J[0] = g.x; J[1] = g.y; J[2] = g.z;
-        J[3] = 2.0 * (rp.y * g.z - rp.z * g.y);
-        J[4] = 2.0 * (rp.z * g.x - rp.x * g.z);
-        J[5] = 2.0 * (rp.x * g.y - rp.y * g.x);
-        // ceres::CauchyLoss(b) + Corrector (rho'' < 0 branch)
-        const double sum = 1.0 + r * r * c2;
-        const double rho0 = b2 * log(sum);
-        const double sr = sqrt(fmax(DBL_MIN, 1.0 / sum));
-#pragma unroll
-        for (int k = 0; k < 6; ++k) J[k] *= sr;
-        r *= sr;
-        int k = 0;
-#pragma unroll
-        for (int i2 = 0; i2 < 6; ++i2)
-#pragma unroll
-            for (int j = i2; j < 6; ++j) acc[k++] += J[i2] * J[j];
-#pragma unroll
-        for (int i2 = 0; i2 < 6; ++i2) acc[21 + i2] += J[i2] * r;
-        acc[27] += 0.5 * rho0;
-        acc[28] += 1.0;
+        Row R;
+        R.J[0] = g.x; R.J[1] = g.y; R.J[2] = g.z;
+        R.J[3] = 2.0 * (rp.y * g.z - rp.z * g.y);
+        R.J[4] = 2.0 * (rp.z * g.x - rp.x * g.z);
+        R.J[5] = 2.0 * (rp.x * g.y - rp.y * g.x);
+        R.r = r;
+        cauchy_correct(R, b2, c2);
+        add_row29(acc, R);
     }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < kNormEq; ++k) {
-        double v = acc[k];
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if (lane == 0) red[warp][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < kNormEq) {
-        double v = 0;
-#pragma unroll
-        for (int w = 0; w < kBlkThreads / 32; ++w) v += red[w][threadIdx.x];
-        a.partials[((size_t)blockIdx.y * kMaxBlk + blockIdx.x) * kNormEq + threadIdx.x] = v;
-    }
+    const double v = block_sum29(acc, red, kBlkThreads / 32);
+    if (threadIdx.x < kNormEq) a.partials[((size_t)blockIdx.y * kMaxBlk + blockIdx.x) * kNormEq + threadIdx.x] = v;
 }
 
 // fixed-order sum over each segment's block partials (run-to-run deterministic): blockIdx.x = segment

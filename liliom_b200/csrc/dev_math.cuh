@@ -508,4 +508,109 @@ __device__ inline void pose_plus(const double x[7], const double d[6], double ou
     out[4] = x[4] + d[3]; out[5] = x[5] + d[4]; out[6] = x[6] + d[5];
 }
 
+// ---- correspondence arithmetic of the GN pass, the LM solve (grid_knn.cu) and the backend kernels (backend_corr.cu) ----
+
+// The gates of a fitted plane  nv . p + 1 = 0  of the five neighbours m (L/src/LidarOdometry.cpp:376-405, R/src/BackendFusion.cpp:
+// 1486-1504) in the reference's mixed fp32/fp64 widths: normalise nv, every neighbour within plane_thres, then the fp32 weight of the
+// transformed query (sx, sy, sz) above w_gate.  `refuse` rejects the plane after the distance test (the backend's reflectivity gate).
+// On acceptance pl = weight * [n, 1/|nv|] and `weight` are set; otherwise neither is touched.
+__device__ __forceinline__ bool plane_gate(double nv[3], const float4 m[5], float sx, float sy, float sz, double plane_thres,
+                                           double w_gate, bool refuse, float4& pl, float& weight) {
+    const double n2 = nv[0] * nv[0] + nv[1] * nv[1] + nv[2] * nv[2];
+    const double nn = sqrt(n2);
+    const double normInverse = 1.0 / nn;                                                                      // :376
+    if (n2 > 0) { nv[0] /= nn; nv[1] /= nn; nv[2] /= nn; }                                                    // :377
+    bool planeValid = true;
+#pragma unroll
+    for (int j = 0; j < 5; ++j)                                                                                // :386-393
+        if (fabs(nv[0] * m[j].x + nv[1] * m[j].y + nv[2] * m[j].z + normInverse) > plane_thres) planeValid = false;
+    if (refuse) planeValid = false;
+    bool ok = false;
+    if (planeValid) {
+        // :397-398; exact ops keep the fp32 roundings stable
+        const float pd = (float)addx(addx(addx(mulx(nv[0], (double)sx), mulx(nv[1], (double)sy)), mulx(nv[2], (double)sz)), normInverse);
+        const float rng = __fsqrt_rn(__fsqrt_rn(faddx(faddx(fmulx(sx, sx), fmulx(sy, sy)), fmulx(sz, sz))));
+        const float w = (float)subx(1.0, mulx(0.9, (double)fabsf(pd)) / (double)rng);
+        if ((double)w > w_gate) {                                                                              // :400
+            pl = make_float4((float)mulx((double)w, nv[0]), (float)mulx((double)w, nv[1]),                     // :402-405
+                             (float)mulx((double)w, nv[2]), (float)mulx((double)w, normInverse));
+            weight = w;
+            ok = true;
+        }
+    }
+    return ok;
+}
+
+struct Row { double J[6]; double r; double half_rho; };     // Jacobian row, residual and (after a corrector) rho / 2
+
+// LidarPlaneNormIncreFactor (LidarKeyframeFactor.h:118-128) in closed form, before the loss:
+//   r = n~ . (R p + t) + d~ ;  J = [ 2 (R p x n~)^T , n~^T ]   (tangent order [rot, t]; SURVEY.md Appendix A)
+__device__ __forceinline__ Row plane_row(const Q4& q, const D3& t, float x, float y, float z, const float4& pl) {
+    const D3 rp = qrot_x(q, D3{(double)x, (double)y, (double)z});
+    const double nx = pl.x, ny = pl.y, nz = pl.z;
+    Row R;
+    R.r = nx * (rp.x + t.x) + ny * (rp.y + t.y) + nz * (rp.z + t.z) + (double)pl.w;
+    R.J[0] = 2.0 * (rp.y * nz - rp.z * ny);
+    R.J[1] = 2.0 * (rp.z * nx - rp.x * nz);
+    R.J[2] = 2.0 * (rp.x * ny - rp.y * nx);
+    R.J[3] = nx; R.J[4] = ny; R.J[5] = nz;
+    return R;
+}
+
+// ceres::HuberLoss(a) and ceres::CauchyLoss(b) with Ceres' Corrector on a raw row: J and r scaled by sqrt(rho'), rho / 2 kept.
+// Both have rho'' <= 0, the branch in which the Corrector is that scaling alone.  The Cauchy form takes the caller's loop
+// invariants b2 = b^2 and inv_b2 = 1 / b^2.
+__device__ __forceinline__ void huber_correct(Row& R, double a) {
+    const double s2 = R.r * R.r, b2 = a * a;
+    double rho0 = s2, rho1 = 1.0;
+    if (s2 > b2) { const double rt = sqrt(s2); rho0 = 2.0 * a * rt - b2; rho1 = fmax(DBL_MIN, a / rt); }
+    const double sr = sqrt(rho1);
+#pragma unroll
+    for (int k = 0; k < 6; ++k) R.J[k] *= sr;
+    R.r *= sr;
+    R.half_rho = 0.5 * rho0;
+}
+__device__ __forceinline__ void cauchy_correct(Row& R, double b2, double inv_b2) {
+    const double sum = 1.0 + R.r * R.r * inv_b2;
+    const double rho0 = b2 * log(sum);
+    const double sr = sqrt(fmax(DBL_MIN, 1.0 / sum));
+#pragma unroll
+    for (int k = 0; k < 6; ++k) R.J[k] *= sr;
+    R.r *= sr;
+    R.half_rho = 0.5 * rho0;
+}
+
+// Fold one corrected row into the 29 sums.  This order defines the layout every consumer of the sums reads.
+__device__ __forceinline__ void add_row29(double acc[29], const Row& R) {
+    int k = 0;
+#pragma unroll
+    for (int i = 0; i < 6; ++i)
+#pragma unroll
+        for (int j = i; j < 6; ++j) acc[k++] += R.J[i] * R.J[j];
+#pragma unroll
+    for (int i = 0; i < 6; ++i) acc[21 + i] += R.J[i] * R.r;
+    acc[27] += R.half_rho;
+    acc[28] += 1.0;
+}
+
+#ifdef __CUDACC__
+// Block sum of every thread's acc[29] in a fixed order: an xor tree inside each warp, then the nwarps warp sums in warp order
+// through red[nwarps][29] in shared memory.  Thread k < 29 gets the total of scalar k; every thread must call it.
+__device__ __forceinline__ double block_sum29(const double acc[29], double (*red)[29], int nwarps) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < 29; ++k) {
+        double v = acc[k];
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if (lane == 0) red[warp][k] = v;
+    }
+    __syncthreads();
+    double v = 0;
+    if (threadIdx.x < 29)
+        for (int w = 0; w < nwarps; ++w) v += red[w][threadIdx.x];
+    return v;
+}
+#endif
+
 }  // namespace lili

@@ -189,12 +189,6 @@ template <int LANES> __device__ __forceinline__ int first_task(int warp) {
 constexpr int kCandBits = 40;
 constexpr unsigned long long kCandMask = (1ull << kCandBits) - 1ull;
 
-__device__ __forceinline__ double warp_sum(double v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // Per-query scratch a warp keeps in shared memory between the phases.
 struct Slot {
     int   idx[5];            // neighbour indices into map_orig; idx[0] < 0: no 5-NN inside the radius
@@ -202,9 +196,9 @@ struct Slot {
     float fx, fy, fz;        // body-frame query (phase B re-derives R p from it)
     int   pad;               // 48 bytes
 };
-struct Row { double J[6]; double r; double half_rho; };   // robustified Jacobian row, residual, rho/2
 
-// scalar k of the 29-vector is  sum_i row.J[kA[k]] * row.X[kB[k]]  (X = J for k<21, r for 21..26)
+// scalar k of the 29-vector is  sum_i row.J[kA[k]] * row.X[kB[k]]  (X = J for k<21, r for 21..26): the order of add_row29
+// (dev_math.cuh), which defines it, accumulated lane-wise instead of row-wise
 __constant__ unsigned char kPairA[27] = {0,0,0,0,0,0, 1,1,1,1,1, 2,2,2,2, 3,3,3, 4,4, 5, 0,1,2,3,4,5};
 __constant__ unsigned char kPairB[27] = {0,1,2,3,4,5, 1,2,3,4,5, 2,3,4,5, 3,4,5, 4,5, 5, 6,6,6,6,6,6};
 
@@ -265,8 +259,8 @@ __device__ __forceinline__ void knn_phases(const KnnArgs& a, const Q4& q, const 
             bool live = qi < n_q;
             if (live) {
                 f = fpre ? *fpre : a.feats[qi];   // (persistent kernel: the query stays in registers across iterations)
-                const D3 pw = qrot_x(q, D3{(double)f.x, (double)f.y, (double)f.z});             // L/src/LidarOdometry.cpp:230-231
-                sx = (float)addx(pw.x, t.x); sy = (float)addx(pw.y, t.y); sz = (float)addx(pw.z, t.z);   // :236-238
+                const VgXyz pw = pcl_transform_xyz(q, t, f.x, f.y, f.z);                          // L/src/LidarOdometry.cpp:230-238
+                sx = pw.x; sy = pw.y; sz = pw.z;
                 if (a.nranks > 1 && owner_of(sx, sy, sz, a.nranks, a.inv_block) != a.rank) live = false;
             }
             // `live` is uniform inside a lane group and the shuffles are masked per group
@@ -282,19 +276,18 @@ __device__ __forceinline__ void knn_phases(const KnnArgs& a, const Q4& q, const 
             LILI_STAMP(11);
             if (sub == 0) {
                 Slot& s = S.slots[warp][slot];
-                const bool ok = live && top.k4 != ~0ull && ((double)top5_dist(top.k4) < a.max_sqd);  // :365
+                const bool ok = live && top5_accepts(top, a.max_sqd);
                 // this pass's position and fifth distance for the next pass (a query this rank does not own keeps no bound)
                 if (qi < n_q) a.qstate[qi] = make_float4(sx, sy, sz, ok ? top5_dist(top.k4) : __int_as_float(0x7f800000));
-                s.idx[0] = ok ? top5_index(top.k0) : -1; s.idx[1] = top5_index(top.k1); s.idx[2] = top5_index(top.k2);
-                s.idx[3] = top5_index(top.k3); s.idx[4] = top5_index(top.k4);
+                int nn[5]; top5_indices(top, nn);
+                s.idx[0] = ok ? nn[0] : -1; s.idx[1] = nn[1]; s.idx[2] = nn[2]; s.idx[3] = nn[3]; s.idx[4] = nn[4];
                 s.sx = sx; s.sy = sy; s.sz = sz;
                 s.fx = f.x; s.fy = f.y; s.fz = f.z;
                 s.pad = 0;
                 if (live && a.nn_idx) {
                     int* o = a.nn_idx + (size_t)qi * 5;
-                    const u64 kk[5] = {top.k0, top.k1, top.k2, top.k3, top.k4};
 #pragma unroll
-                    for (int j = 0; j < 5; ++j) { const int li = top5_index(kk[j]); o[j] = li >= 0 ? __float_as_int(a.map_orig[li].w) : -1; }
+                    for (int j = 0; j < 5; ++j) o[j] = nn[j] >= 0 ? __float_as_int(a.map_orig[nn[j]].w) : -1;
                 }
                 if (live && a.nn_sqd) {
                     float* o = a.nn_sqd + (size_t)qi * 5;
@@ -309,57 +302,24 @@ __device__ __forceinline__ void knn_phases(const KnnArgs& a, const Q4& q, const 
         if (lane < per_task) {
             const int qi = task * per_task + lane;
             const Slot s = S.slots[warp][lane];
-            float pl0 = 0.f, pl1 = 0.f, pl2 = 0.f, pl3 = 0.f;
+            float4 pl = make_float4(0.f, 0.f, 0.f, 0.f);
             if (qi < n_q && s.idx[0] >= 0) {
                 float4 m[5];
 #pragma unroll
                 for (int j = 0; j < 5; ++j) m[j] = __ldg(a.map_orig + s.idx[j]);                                     // :369-371
                 double nv[3];
                 if (!plane_fit5_fast(m, nv)) plane_fit5_qr(m, nv);                                                    // :375 (see dev_math.cuh)
-                const double n2 = nv[0] * nv[0] + nv[1] * nv[1] + nv[2] * nv[2];
-                const double nn = sqrt(n2);
-                const double normInverse = 1.0 / nn;                                                                  // :376
-                if (n2 > 0) { nv[0] /= nn; nv[1] /= nn; nv[2] /= nn; }                                                // :377
-                bool planeValid = true;
-#pragma unroll
-                for (int j = 0; j < 5; ++j)                                                                            // :386-393
-                    if (fabs(nv[0] * m[j].x + nv[1] * m[j].y + nv[2] * m[j].z + normInverse) > a.plane_thres) planeValid = false;
-                if (planeValid) {
-                    // :397-398 with the reference's mixed widths; exact ops keep the fp32 roundings stable
-                    const float pd = (float)addx(addx(addx(mulx(nv[0], (double)s.sx), mulx(nv[1], (double)s.sy)), mulx(nv[2], (double)s.sz)), normInverse);
-                    const float rng = __fsqrt_rn(__fsqrt_rn(faddx(faddx(fmulx(s.sx, s.sx), fmulx(s.sy, s.sy)), fmulx(s.sz, s.sz))));
-                    const float weight = (float)subx(1.0, mulx(0.9, (double)fabsf(pd)) / (double)rng);
-                    if ((double)weight > a.w_gate) {                                                                  // :400
-                        pl0 = (float)mulx((double)weight, nv[0]);                                                     // :402-405
-                        pl1 = (float)mulx((double)weight, nv[1]);
-                        pl2 = (float)mulx((double)weight, nv[2]);
-                        pl3 = (float)mulx((double)weight, normInverse);
-                        ok = true;
-                    }
-                }
+                float weight;
+                ok = plane_gate(nv, m, s.sx, s.sy, s.sz, a.plane_thres, a.w_gate, false, pl, weight);
             }
             if (qi < n_q) {
                 if (a.valid) a.valid[qi] = ok ? 1 : 0;
-                if (a.plane) a.plane[qi] = make_float4(pl0, pl1, pl2, pl3);
+                if (a.plane) a.plane[qi] = pl;
             }
             if (ok) {
-                // LidarPlaneNormIncreFactor (LidarKeyframeFactor.h:118-128) in closed form:
-                //   r = n~ . (q*p + t) + d~ ;  row = [ 2 (R p x n~)^T , n~^T ]  (SURVEY.md Appendix A)
-                const D3 rp = qrot_x(q, D3{(double)s.fx, (double)s.fy, (double)s.fz});
-                const double nx = pl0, ny = pl1, nz = pl2;
-                double r = nx * (rp.x + t.x) + ny * (rp.y + t.y) + nz * (rp.z + t.z) + (double)pl3;
-                // ceres::HuberLoss(a) + Corrector (rho'' <= 0 branch): scale row and residual by sqrt(rho')
-                const double s2 = r * r, b2 = a.huber_a * a.huber_a;
-                double rho0 = s2, rho1 = 1.0;
-                if (s2 > b2) { const double rt = sqrt(s2); rho0 = 2.0 * a.huber_a * rt - b2; rho1 = fmax(DBL_MIN, a.huber_a / rt); }
-                const double sr = sqrt(rho1);
-                Row& R = S.rows[warp][lane];
-                R.J[0] = sr * 2.0 * (rp.y * nz - rp.z * ny);
-                R.J[1] = sr * 2.0 * (rp.z * nx - rp.x * nz);
-                R.J[2] = sr * 2.0 * (rp.x * ny - rp.y * nx);
-                R.J[3] = sr * nx; R.J[4] = sr * ny; R.J[5] = sr * nz;
-                R.r = sr * r;
-                R.half_rho = 0.5 * rho0;
+                Row R = plane_row(q, t, s.fx, s.fy, s.fz, pl);
+                huber_correct(R, a.huber_a);
+                S.rows[warp][lane] = R;
             }
             S.rvalid[warp][lane] = ok ? 1 : 0;
         }
@@ -748,53 +708,20 @@ struct LmArgs {
 constexpr int kLmBlock = 512;
 
 __device__ void lm_eval(const LmArgs& a, const double x[7], double out[kNormEq], double (*red)[kNormEq]) {
-    Q4 q{x[0], x[1], x[2], x[3]};
+    const Q4 q{x[0], x[1], x[2], x[3]}; const D3 t{x[4], x[5], x[6]};
     double acc[kNormEq];
 #pragma unroll
     for (int k = 0; k < kNormEq; ++k) acc[k] = 0.0;
     const int n_c = a.n_dev ? min(*a.n_dev, a.n) : a.n;
     for (int i = threadIdx.x; i < n_c; i += blockDim.x) {
         if (!a.valid[i]) continue;
-        float4 f = a.feats[i];
-        float4 pl = a.plane[i];
-        D3 rp = qrot_x(q, D3{(double)f.x, (double)f.y, (double)f.z});
-        double nx = pl.x, ny = pl.y, nz = pl.z;
-        double r = nx * (rp.x + x[4]) + ny * (rp.y + x[5]) + nz * (rp.z + x[6]) + (double)pl.w;
-        double J[6];
-        J[0] = 2.0 * (rp.y * nz - rp.z * ny);
-        J[1] = 2.0 * (rp.z * nx - rp.x * nz);
-        J[2] = 2.0 * (rp.x * ny - rp.y * nx);
-        J[3] = nx; J[4] = ny; J[5] = nz;
-        double s2 = r * r, rho0, rho1;
-        const double b2 = a.huber_a * a.huber_a;
-        if (s2 > b2) { double rt = sqrt(s2); rho0 = 2.0 * a.huber_a * rt - b2; rho1 = fmax(DBL_MIN, a.huber_a / rt); }
-        else { rho0 = s2; rho1 = 1.0; }
-        double sr = sqrt(rho1);
-#pragma unroll
-        for (int k = 0; k < 6; ++k) J[k] *= sr;
-        r *= sr;
-        int k = 0;
-#pragma unroll
-        for (int i2 = 0; i2 < 6; ++i2)
-#pragma unroll
-            for (int j = i2; j < 6; ++j) acc[k++] += J[i2] * J[j];
-#pragma unroll
-        for (int i2 = 0; i2 < 6; ++i2) acc[21 + i2] += J[i2] * r;
-        acc[27] += 0.5 * rho0;
-        acc[28] += 1.0;
+        const float4 f = a.feats[i];
+        Row R = plane_row(q, t, f.x, f.y, f.z, a.plane[i]);
+        huber_correct(R, a.huber_a);
+        add_row29(acc, R);
     }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < kNormEq; ++k) {
-        double v = warp_sum(acc[k]);
-        if (lane == 0) red[warp][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < kNormEq) {
-        double v = 0;
-        for (int w = 0; w < (int)(blockDim.x >> 5); ++w) v += red[w][threadIdx.x];
-        red[0][threadIdx.x] = v;
-    }
+    const double v = block_sum29(acc, red, (int)(blockDim.x >> 5));
+    if (threadIdx.x < kNormEq) red[0][threadIdx.x] = v;
     __syncthreads();
     for (int k = 0; k < kNormEq; ++k) out[k] = red[0][k];
     __syncthreads();
@@ -940,8 +867,8 @@ __global__ void k_block27_count(const float4* __restrict__ feats, int n, Q4 q, D
     unsigned long long cnt = 0, nq = 0;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const float4 f = feats[i];
-        const D3 pw = qrot_x(q, D3{(double)f.x, (double)f.y, (double)f.z});
-        const float sx = (float)addx(pw.x, t.x), sy = (float)addx(pw.y, t.y), sz = (float)addx(pw.z, t.z);
+        const VgXyz pw = pcl_transform_xyz(q, t, f.x, f.y, f.z);
+        const float sx = pw.x, sy = pw.y, sz = pw.z;
         if (nranks > 1 && owner_of(sx, sy, sz, nranks, inv_block) != rank) continue;
         ++nq;
         const int cx = cell_coord(sx, g.inv_cell) - g.org[0], cy = cell_coord(sy, g.inv_cell) - g.org[1], cz = cell_coord(sz, g.inv_cell) - g.org[2];

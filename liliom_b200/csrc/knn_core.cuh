@@ -59,6 +59,11 @@ struct Top5 { u64 k0, k1, k2, k3, k4; };
 __device__ __forceinline__ void top5_init(Top5& t) { t.k0 = t.k1 = t.k2 = t.k3 = t.k4 = ~0ull; }
 __device__ __forceinline__ float top5_dist(u64 k) { return __uint_as_float((unsigned)(k >> 32)); }
 __device__ __forceinline__ int top5_index(u64 k) { return k == ~0ull ? -1 : (int)(unsigned)(k & 0xffffffffull); }
+// a correspondence needs five neighbours, the fifth inside the gate (L/src/LidarOdometry.cpp:365, L:1543, R:1476 of BackendFusion.cpp)
+__device__ __forceinline__ bool top5_accepts(const Top5& t, double max_sqd) { return t.k4 != ~0ull && (double)top5_dist(t.k4) < max_sqd; }
+__device__ __forceinline__ void top5_indices(const Top5& t, int idx[5]) {
+    idx[0] = top5_index(t.k0); idx[1] = top5_index(t.k1); idx[2] = top5_index(t.k2); idx[3] = top5_index(t.k3); idx[4] = top5_index(t.k4);
+}
 
 __device__ __forceinline__ void cswap(u64& a, u64& b) {   // afterwards a <= b
     const bool s = b < a;

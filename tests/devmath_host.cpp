@@ -1,7 +1,8 @@
 // TEST INFRASTRUCTURE: host build of the device scalar routines (liliom_b200/csrc/dev_math.cuh) so that the CPU test tier can
-// exercise the SAME SOURCE the kernels compile — plane fit (fast path + rank-revealing QR fallback), 6x6 LDL^T, Ceres' Plus,
-// the 3x3 symmetric eigensolver — against NumPy and against the oracle's independent copies.  The round-to-nearest intrinsics
-// become plain operators (this file is compiled with -ffp-contract=off, so nothing is fused either).
+// exercise the SAME SOURCE the kernels compile — plane fit (fast path + rank-revealing QR fallback), plane gates, residual rows,
+// Huber / Cauchy correctors and the 29-sum fold, 6x6 LDL^T, Ceres' Plus, the 3x3 symmetric eigensolver — against NumPy and
+// against the oracle's independent copies.  The round-to-nearest intrinsics become plain operators (this file is compiled with
+// -ffp-contract=off, so nothing is fused either).
 #include <cmath>
 #include <cfloat>
 #include <cstring>
@@ -11,6 +12,7 @@ static inline double __dsub_rn(double a, double b) { return a - b; }
 static inline float __fmul_rn(float a, float b) { return a * b; }
 static inline float __fadd_rn(float a, float b) { return a + b; }
 static inline float __fsub_rn(float a, float b) { return a - b; }
+static inline float __fsqrt_rn(float a) { return std::sqrt(a); }
 using std::isfinite;
 #include <cuda_runtime.h>
 #ifndef __noinline__
@@ -44,5 +46,42 @@ void dm_colpiv_qr(const double A15[15], const double b5[5], double x[3]) {
 void dm_qrot(const double q[4], const double v[3], double out[3]) {
     D3 r = qrot_x(Q4{q[0], q[1], q[2], q[3]}, D3{v[0], v[1], v[2]});
     out[0] = r.x; out[1] = r.y; out[2] = r.z;
+}
+// plane_gate on the fitted nv (normalised in place) of the neighbours m20 and the query s3; pl4 / weight are left as passed in
+// when the plane is refused
+int dm_plane_gate(double nv[3], const float* m20, const float s3[3], double plane_thres, double w_gate, int refuse, float pl4[4],
+                  float* weight) {
+    float4 m[5];
+    for (int j = 0; j < 5; ++j) m[j] = make_float4(m20[4 * j], m20[4 * j + 1], m20[4 * j + 2], m20[4 * j + 3]);
+    float4 pl = make_float4(pl4[0], pl4[1], pl4[2], pl4[3]);
+    const bool ok = plane_gate(nv, m, s3[0], s3[1], s3[2], plane_thres, w_gate, refuse != 0, pl, *weight);
+    pl4[0] = pl.x; pl4[1] = pl.y; pl4[2] = pl.z; pl4[3] = pl.w;
+    return ok ? 1 : 0;
+}
+// the 29 sums of the scan-to-map rows (plane_row + huber_correct + add_row29) of the valid correspondences at pose7
+void dm_plane_neq(const float* feats4, int n, const unsigned char* valid, const float* plane4, const double pose7[7], double huber_a,
+                  double out29[29]) {
+    const Q4 q{pose7[0], pose7[1], pose7[2], pose7[3]};
+    const D3 t{pose7[4], pose7[5], pose7[6]};
+    for (int k = 0; k < 29; ++k) out29[k] = 0.0;
+    for (int i = 0; i < n; ++i) {
+        if (!valid[i]) continue;
+        const float* f = feats4 + 4 * (size_t)i;
+        Row R = plane_row(q, t, f[0], f[1], f[2], make_float4(plane4[4 * i], plane4[4 * i + 1], plane4[4 * i + 2], plane4[4 * i + 3]));
+        huber_correct(R, huber_a);
+        add_row29(out29, R);
+    }
+}
+// the 29 sums of n raw rows (J6[6 * i ..], r[i]) through cauchy_correct + add_row29
+void dm_cauchy_fold(const double* J6, const double* r, int n, double cauchy_b, double out29[29]) {
+    const double b2 = cauchy_b * cauchy_b, c2 = 1.0 / b2;
+    for (int k = 0; k < 29; ++k) out29[k] = 0.0;
+    for (int i = 0; i < n; ++i) {
+        Row R;
+        for (int k = 0; k < 6; ++k) R.J[k] = J6[6 * (size_t)i + k];
+        R.r = r[i];
+        cauchy_correct(R, b2, c2);
+        add_row29(out29, R);
+    }
 }
 }

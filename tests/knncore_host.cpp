@@ -28,6 +28,7 @@ static inline double __dsub_rn(double a, double b) { return a - b; }
 static inline float __fmul_rn(float a, float b) { return a * b; }
 static inline float __fadd_rn(float a, float b) { return a + b; }
 static inline float __fsub_rn(float a, float b) { return a - b; }
+static inline float __fsqrt_rn(float a) { return std::sqrt(a); }
 // round toward +inf: the operation runs under FE_UPWARD, the previous mode is restored afterwards
 struct Upward {
     int old;

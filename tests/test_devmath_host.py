@@ -23,6 +23,10 @@ def dm():
     L.dm_eigen_sym3.argtypes = [dp, dp, dp]; L.dm_eigen_sym3.restype = None
     L.dm_colpiv_qr.argtypes = [dp, dp, dp]; L.dm_colpiv_qr.restype = None
     L.dm_qrot.argtypes = [dp, dp, dp]; L.dm_qrot.restype = None
+    vp = C.c_void_p
+    L.dm_plane_gate.argtypes = [dp, fp, fp, C.c_double, C.c_double, C.c_int, fp, fp]
+    L.dm_plane_neq.argtypes = [vp, C.c_int, vp, vp, dp, C.c_double, dp]; L.dm_plane_neq.restype = None
+    L.dm_cauchy_fold.argtypes = [dp, dp, C.c_int, C.c_double, dp]; L.dm_cauchy_fold.restype = None
     return L
 
 
@@ -153,3 +157,163 @@ def test_gn_safe_step_device_copy(dm):
     assert dm.dm_gn_safe_step(_d(np.zeros(21)), _d(np.ones(6)), _d(d)) == 0
     bad = _upper21(np.eye(6)); bad[0] = np.nan
     assert dm.dm_gn_safe_step(_d(bad), _d(np.ones(6)), _d(d)) == 0
+
+
+def _f(a):
+    return a.ctypes.data_as(C.POINTER(C.c_float))
+
+
+def _gate_numpy(nv, m, s, plane_thres, w_gate):
+    """L/src/LidarOdometry.cpp:376-405 restated in the reference's widths: fp64 normal and distances, the query's range in fp32,
+    pd and the weight narrowed to fp32.  Returns (ok, normalised nv, pl, weight)."""
+    f64, f32 = np.float64, np.float32
+    n0, n1, n2_ = f64(nv[0]), f64(nv[1]), f64(nv[2])
+    n2 = n0 * n0 + n1 * n1 + n2_ * n2_
+    nn = np.sqrt(n2)
+    inv = f64(1.0) / nn
+    if n2 > 0:
+        n0, n1, n2_ = n0 / nn, n1 / nn, n2_ / nn
+    valid = not any(abs(n0 * f64(p[0]) + n1 * f64(p[1]) + n2_ * f64(p[2]) + inv) > plane_thres for p in m)
+    sx, sy, sz = (f32(v) for v in s)
+    nvn = np.array([n0, n1, n2_])
+    if not valid:
+        return False, nvn, None, None
+    pd = f32(((n0 * f64(sx) + n1 * f64(sy)) + n2_ * f64(sz)) + inv)
+    rng = np.sqrt(np.sqrt((sx * sx + sy * sy) + sz * sz))
+    assert rng.dtype == np.float32
+    w = f32(f64(1.0) - (f64(0.9) * f64(abs(pd))) / f64(rng))
+    if not f64(w) > w_gate:
+        return False, nvn, None, None
+    pl = np.array([f32(f64(w) * n0), f32(f64(w) * n1), f32(f64(w) * n2_), f32(f64(w) * inv)], np.float32)
+    return True, nvn, pl, w
+
+
+def _gate_max_dist(nv, m):
+    """the largest neighbour distance of the plane gate, as _gate_numpy computes it"""
+    f64 = np.float64
+    n0, n1, n2_ = (f64(v) for v in nv)
+    nn = np.sqrt(n0 * n0 + n1 * n1 + n2_ * n2_)
+    inv = f64(1.0) / nn
+    n0, n1, n2_ = n0 / nn, n1 / nn, n2_ / nn
+    return max(abs(n0 * f64(p[0]) + n1 * f64(p[1]) + n2_ * f64(p[2]) + inv) for p in m)
+
+
+def test_plane_gate_bit_for_bit_against_numpy(dm):
+    """dev_math.cuh::plane_gate (the gates of the GN pass and of the backend's surf search) against a NumPy restatement of
+    L:376-405 in the reference's fp32/fp64 widths, bit for bit: flag, normalised normal, weighted plane and weight — on random
+    neighbourhoods and on ones exactly at plane_thres and at w_gate, where one ulp decides."""
+    rng = np.random.default_rng(5)
+    n_ok = n_edge = 0
+    for k in range(600):
+        c = rng.uniform(-150, 150, 3); c[2] = rng.uniform(-3, 3)
+        nrm = rng.normal(size=3); nrm /= np.linalg.norm(nrm)
+        P = c + rng.uniform(-0.5, 0.5, (5, 3))
+        P -= np.outer((P - c) @ nrm, nrm) * (1.0 - 10.0 ** rng.uniform(-4, -0.5))
+        m = np.ones((5, 4), np.float32); m[:, :3] = P
+        s = (c + nrm * rng.uniform(-0.4, 0.4) + rng.uniform(-0.3, 0.3, 3)).astype(np.float32)
+        nv0 = np.zeros(3)
+        dm.dm_plane_fit5(_f(m), _d(nv0))
+        dmax = _gate_max_dist(nv0, m[:, :3])
+        thr = [0.06, 0.2, float(dmax), float(np.nextafter(dmax, 0.0))]         # on the threshold: kept; one ulp below: refused
+        for plane_thres in thr:
+            ok_r, nvn_r, pl_r, w_r = _gate_numpy(nv0, m[:, :3], s, plane_thres, 0.1)
+            gates = [0.1, 0.5]
+            if ok_r:
+                gates += [float(w_r), float(np.nextafter(np.float64(w_r), -np.inf))]  # weight == w_gate: refused; one ulp below: kept
+            for w_gate in gates:
+                ok_r, nvn_r, pl_r, w_r = _gate_numpy(nv0, m[:, :3], s, plane_thres, w_gate)
+                for refuse in (0, 1):
+                    nv = nv0.copy(); pl = np.full(4, -7.0, np.float32); w = np.full(1, -7.0, np.float32)
+                    ok = dm.dm_plane_gate(_d(nv), _f(m), _f(s), plane_thres, w_gate, refuse, _f(pl), _f(w))
+                    assert nv.tobytes() == nvn_r.tobytes()
+                    assert ok == (ok_r and not refuse)
+                    if ok:
+                        assert pl.tobytes() == pl_r.tobytes() and w[0].tobytes() == np.float32(w_r).tobytes()
+                        n_ok += 1
+                        n_edge += plane_thres == dmax or w_gate != float(w_r) and w_gate not in (0.1, 0.5)
+                    else:
+                        assert (pl == -7.0).all() and w[0] == -7.0                  # a refused plane leaves the outputs alone
+    assert n_ok > 500 and n_edge > 100
+
+
+def _qrot_np(q, v):
+    """Eigen's quaternion * vector on rows of v (fp64)"""
+    qv = np.broadcast_to(np.asarray(q[1:], np.float64), v.shape)
+    uv = 2.0 * np.cross(qv, v)
+    return v + q[0] * uv + np.cross(qv, uv)
+
+
+def _unit_pose(rng):
+    p = np.concatenate([rng.normal(size=4), rng.uniform(-20, 20, 3)])
+    p[:4] /= np.linalg.norm(p[:4])
+    return p
+
+
+def test_plane_rows_huber_fold_match_oracle_normal_equations(dm, oracle):
+    """plane_row + huber_correct + add_row29 (the scan-to-map rows of the GN pass and of the LM solve) against the oracle's
+    normal equations on random correspondences, residuals on both sides of the Huber threshold, at the tolerance the device's
+    sums are held to."""
+    rng = np.random.default_rng(6)
+    for trial in range(6):
+        n = 3000
+        pose = _unit_pose(rng)
+        feats = np.ones((n, 4), np.float32); feats[:, :3] = rng.uniform(-60, 60, (n, 3))
+        pw = _qrot_np(pose[:4], feats[:, :3].astype(np.float64)) + pose[4:]
+        nrm = rng.normal(size=(n, 3)); nrm /= np.linalg.norm(nrm, axis=1, keepdims=True)
+        d = -(nrm * pw).sum(1) + rng.uniform(-0.3, 0.3, n)
+        w = rng.uniform(0.3, 1.0, n)
+        plane = np.concatenate([nrm * w[:, None], (d * w)[:, None]], 1).astype(np.float32)
+        valid = (rng.uniform(size=n) < 0.8).astype(np.uint8)
+        out = np.zeros(29)
+        dm.dm_plane_neq(feats.ctypes.data, n, valid.ctypes.data, plane.ctypes.data, _d(pose), 0.1, _d(out))
+        ref = oracle.normal_equations(feats, valid, plane, pose, 0.1)
+        assert out[28] == ref[28] == valid.sum()
+        np.testing.assert_allclose(out, ref, rtol=1e-9, atol=1e-9)
+
+
+def test_cauchy_fold_matches_oracle_backend_blocks(dm, oracle):
+    """cauchy_correct + add_row29 (k_backend_block's loss and fold) on LidarPlaneNormFactor and LidarEdgeFactor rows built here
+    from their closed forms, against the oracle's backend blocks at the tolerances of the device's backend blocks."""
+    rng = np.random.default_rng(7)
+    for trial in range(4):
+        n = 2000
+        pose = _unit_pose(rng)
+        q_lb = rng.normal(size=4); q_lb /= np.linalg.norm(q_lb); t_lb = rng.uniform(-0.2, 0.2, 3)
+        feats = np.ones((n, 4), np.float32); feats[:, :3] = rng.uniform(-60, 60, (n, 3))
+        valid = (rng.uniform(size=n) < 0.8).astype(np.uint8)
+        sel = valid.astype(bool)
+        cp = feats[:, :3].astype(np.float64)
+        # surf: r = score (n~ . p_w + d~), p_w = q (q_lb^-1 (p - t_lb)) + t, g = score n~
+        pbody = _qrot_np(np.array([q_lb[0], -q_lb[1], -q_lb[2], -q_lb[3]]), cp - t_lb)
+        rp = _qrot_np(pose[:4], pbody)
+        nrm = rng.normal(size=(n, 3)); nrm /= np.linalg.norm(nrm, axis=1, keepdims=True)
+        d = -(nrm * (rp + pose[4:])).sum(1) + rng.uniform(-3.0, 3.0, n)
+        w = rng.uniform(0.3, 1.0, n)
+        plane = np.concatenate([nrm * w[:, None], (d * w)[:, None]], 1).astype(np.float32)
+        score = rng.uniform(0.2, 1.5, n)
+        pl64 = plane.astype(np.float64)
+        r = score * ((pl64[:, :3] * (rp + pose[4:])).sum(1) + pl64[:, 3])
+        g = score[:, None] * pl64[:, :3]
+        J = np.concatenate([g, 2.0 * np.cross(rp, g)], 1)
+        out = np.zeros(29)
+        dm.dm_cauchy_fold(_d(np.ascontiguousarray(J[sel])), _d(np.ascontiguousarray(r[sel])), int(sel.sum()), 1.0, _d(out))
+        ref = oracle.backend_surf_block(feats, valid, plane, score, pose, q_lb, t_lb, 1.0)
+        assert out[28] == ref[28] == sel.sum()
+        np.testing.assert_allclose(out, ref, rtol=1e-9, atol=1e-9 * np.abs(ref[:21]).max())
+        # edge: r = s |u x v| / |a-b|, u = p_w - a, v = p_w - b, g = s ((a-b) x (u x v)^) / |a-b|
+        s_weight = 0.6
+        rp = _qrot_np(pose[:4], cp)
+        lp = rp + pose[4:]
+        u = rng.normal(size=(n, 3)); u /= np.linalg.norm(u, axis=1, keepdims=True)
+        c = lp + rng.uniform(-2.0, 2.0, (n, 3))
+        pa = (c + 0.1 * u).astype(np.float32); pb = (c - 0.1 * u).astype(np.float32)
+        A, B = pa.astype(np.float64), pb.astype(np.float64)
+        nu = np.cross(lp - A, lp - B); de = A - B
+        nn_, dn = np.linalg.norm(nu, axis=1), np.linalg.norm(de, axis=1)
+        r = nn_ / dn * s_weight
+        g = (s_weight / (dn * nn_))[:, None] * np.cross(de, nu)
+        J = np.concatenate([g, 2.0 * np.cross(rp, g)], 1)
+        dm.dm_cauchy_fold(_d(np.ascontiguousarray(J[sel])), _d(np.ascontiguousarray(r[sel])), int(sel.sum()), 1.0, _d(out))
+        ref = oracle.backend_edge_block(feats, valid, pa, pb, s_weight, pose, 1.0)
+        assert out[28] == ref[28] == sel.sum()
+        np.testing.assert_allclose(out, ref, rtol=1e-8, atol=1e-9 * np.abs(ref[:21]).max())
