@@ -127,12 +127,15 @@ int liliom_map_rebuild(liliom_ctx* c, int* n_map_out);
 /* SURVEY §8 (f2): the same two steps as ONE incremental call — liliom_map_update == liliom_map_push_frame followed by
  * liliom_map_rebuild, bit for bit (same FIFO, same filtered cloud in the same order, same cell grid), but the VoxelGrid state
  * lives on the device across scans: the new frame's voxel keys are sorted on their own and merged into the resident sorted entry
- * array while the dropped frame's entries leave it, instead of re-sorting the whole concatenation (liliom_b200/csrc/map_inc.cu).
+ * array while the dropped frame's entries leave it, instead of re-sorting the whole concatenation (liliom_b200/csrc/map.cu).
  * Mixing it with the two separate calls is allowed (the entry array is rebuilt once after them).  Sharded contexts and clouds
  * whose voxel coordinates do not fit 21 bits take the two-step path internally.  _device: d_surf_ds_body is a DEVICE pointer. */
 int liliom_map_update(liliom_ctx* c, const void* surf_ds_body, int n, const double pose7[7], int* n_map_out);
 int liliom_map_update_device(liliom_ctx* c, const void* d_surf_ds_body, int n, const double pose7[7], int* n_map_out);
-/* surf_from_map_ds with all its fields (point_stride bytes per point), in liliom_map_download order (single GPU). */
+/* surf_from_map_ds with all its fields (point_stride bytes per point), in liliom_map_download order (single GPU): the
+ * filtered cloud of the last liliom_map_rebuild or liliom_map_update (empty after liliom_map_clear).  A map installed with
+ * liliom_map_set_points, liliom_map_set_cloud or liliom_icp_align has no filtered cloud behind it: LILIOM_E_NOMAP (see
+ * liliom_last_error) until the next rebuild or update. */
 int liliom_map_download_cloud(liliom_ctx* c, void* out, int cap, int* m_out);
 
 /* push_frame for pipelines that keep surf_last_ds on the device (both nodes in one process): d_surf_ds_body is a DEVICE

@@ -371,6 +371,9 @@ class Context:
         return m.value
 
     def map_download_cloud(self) -> np.ndarray:
+        """The filtered cloud of the last map_rebuild / map_update, all fields (empty after map_clear).  An installed map
+        (map_set_points, map_set_cloud, icp_align's target) has none behind it: LiliomError E_NOMAP until the next rebuild or
+        update."""
         m = C.c_int()
         self._check(lib().liliom_map_download_cloud(self._h, None, 0, C.byref(m)))
         out = np.zeros(max(m.value, 1), self.dtype)

@@ -1,88 +1,12 @@
 // C ABI of libliliom_b200.so (see include/liliom.h for the contract and reference citations).
 #include "ctx.cuh"
 #include "dev_math.cuh"
-#include "knn_core.cuh"
 #include "pc2_fields.h"
 #include <new>
 #include <cstdlib>
-#include <ctime>
 
 namespace lili {
 void nccl_destroy(liliom_ctx* c);
-int nccl_allreduce_sum_f64(liliom_ctx* c, double* buf, int count);
-
-// ---- map sharding (multi-GPU): keep a point when any shard block (cube of 1/inv_block metres, default 16 m) touched by its
-// halo box is owned by `rank` (same hash as owner_of() in knn_core.cuh)
-__global__ void k_shard_flags(const float4* __restrict__ p, int n, float halo, float inv_block, int nranks, int rank, int* __restrict__ flags) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i > n) return;
-    int f = 0;
-    if (i < n) {
-        float4 v = p[i];
-        for (int c = 0; c < 8 && !f; ++c) {
-            float x = v.x + ((c & 1) ? halo : -halo), y = v.y + ((c & 2) ? halo : -halo), z = v.z + ((c & 4) ? halo : -halo);
-            if (owner_of(x, y, z, nranks, inv_block) == rank) f = 1;
-        }
-    }
-    flags[i] = f;
-}
-// same rule on PCL-layout points (stride bytes): used by the sharded liliom_map_push_frame
-__global__ void k_shard_flags_strided(const unsigned char* __restrict__ p, int n, int stride, float halo, float inv_block, int nranks, int rank,
-                                      int* __restrict__ flags) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i > n) return;
-    int f = 0;
-    if (i < n) {
-        const float4 v = *reinterpret_cast<const float4*>(p + (size_t)i * stride);
-        for (int c = 0; c < 8 && !f; ++c) {
-            float x = v.x + ((c & 1) ? halo : -halo), y = v.y + ((c & 2) ? halo : -halo), z = v.z + ((c & 4) ? halo : -halo);
-            if (owner_of(x, y, z, nranks, inv_block) == rank) f = 1;
-        }
-    }
-    flags[i] = f;
-}
-__global__ void k_compact_strided(const unsigned char* __restrict__ in, const int* __restrict__ flags, const int* __restrict__ pos, int n, int stride,
-                                  unsigned char* __restrict__ out) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n || !flags[i]) return;
-    const float4* src = reinterpret_cast<const float4*>(in + (size_t)i * stride);
-    float4* dst = reinterpret_cast<float4*>(out + (size_t)pos[i] * stride);
-    for (int k = 0; k < stride / 16; ++k) dst[k] = src[k];
-}
-
-__global__ void k_compact_f4(const float4* __restrict__ in, const int* __restrict__ flags, const int* __restrict__ pos, int n, float4* __restrict__ out) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n && flags[i]) out[pos[i]] = in[i];
-}
-
-// transformCloud (L/src/LidarOdometry.cpp:246-278; R/src/LidarOdometry.cpp:239-264)
-__global__ void k_transform_cloud(const unsigned char* __restrict__ in, int n, int stride, Q4 q, D3 t, unsigned char* __restrict__ out) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    pcl_transform_point(in + (size_t)i * stride, stride, q, t, out + (size_t)i * stride);
-}
-
-// Concatenation of the FIFO frames (L/src/LidarOdometry.cpp:301-302) in ONE launch: blockIdx.y = frame, the blocks of a row
-// stream that frame's 16-byte words to its offset in the concatenated cloud.  (20 cudaMemcpyAsync calls cost a fixed
-// latency per copy whatever the size, which a single launch does not.)
-constexpr int kConcatMax = 64;
-struct ConcatTab { const float4* src[kConcatMax]; long long off[kConcatMax + 1]; };      // offsets in 16-byte words
-__global__ void k_concat_frames(const __grid_constant__ ConcatTab tab, float4* __restrict__ out) {
-    const int f = blockIdx.y;
-    const long long n16 = tab.off[f + 1] - tab.off[f];
-    const float4* __restrict__ src = tab.src[f];
-    float4* __restrict__ dst = out + tab.off[f];
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n16; i += (long long)gridDim.x * blockDim.x) dst[i] = src[i];
-}
-// sharded rebuild: the shard filter and the repack to float4 {x,y,z,index} in one pass over the VoxelGrid output
-__global__ void k_compact_repack(const unsigned char* __restrict__ in, const int* __restrict__ flags, const int* __restrict__ pos, int n, int stride,
-                                 float4* __restrict__ out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n || !flags[i]) return;
-    float4 v = *reinterpret_cast<const float4*>(in + (size_t)i * stride);
-    v.w = __int_as_float(i);
-    out[pos[i]] = v;
-}
 
 // LidarOdometry::undistortion (L/src/LidarOdometry.cpp:178-199), in place on device points
 __global__ void k_undistort(unsigned char* __restrict__ pts, int n, int stride, D3 trans, Q4 quat) {
@@ -101,27 +25,6 @@ __global__ void k_undistort(unsigned char* __restrict__ pts, int n, int stride, 
     a.y = (float)addx(r.y, mulx(ratio_i, trans.y));
     a.z = (float)addx(r.z, mulx(ratio_i, trans.z));
     p0[0] = a;
-}
-
-static int install_map_from_xyzw(liliom_ctx* c, int m) {
-    // c->map.xyzw holds m float4 (w = global index).  Shard when a communicator is attached.
-    c->map_n_global = m;
-    if (c->nranks > 1 && m > 0) {
-        LILI_CUDA(c, c->flags.ensure(((size_t)m + 2) * 4));
-        LILI_CUDA(c, c->idx_a.ensure(((size_t)m + 2) * 4));
-        LILI_CUDA(c, c->map_ds.ensure((size_t)m * sizeof(float4)));
-        const float cell = gate_cell(c->prm.knn_max_sqdist);
-        k_shard_flags<<<cdiv(m + 1, 256), 256, 0, c->stream>>>(c->map.xyzw.as<float4>(), m, cell, c->shard_inv_block, c->nranks, c->rank, c->flags.as<int>());
-        LILI_TRY(launch_check(c, "k_shard_flags"));
-        LILI_TRY(exclusive_scan_i32(c, c->flags.as<int>(), c->idx_a.as<int>(), m));
-        k_compact_f4<<<cdiv(m, 256), 256, 0, c->stream>>>(c->map.xyzw.as<float4>(), c->flags.as<int>(), c->idx_a.as<int>(), m, c->map_ds.as<float4>());
-        LILI_TRY(launch_check(c, "k_compact_f4"));
-        int local = 0;
-        LILI_TRY(read_back(c, {{&local, c->idx_a.as<int>() + m, sizeof(int)}}));
-        LILI_CUDA(c, cudaMemcpyAsync(c->map.xyzw.p, c->map_ds.p, (size_t)local * sizeof(float4), cudaMemcpyDeviceToDevice, c->stream));
-        m = local;
-    }
-    return grid_build(c, m);
 }
 
 static int upload_feats(liliom_ctx* c, const void* feats, int n, int stride) {
@@ -504,299 +407,6 @@ extern "C" int liliom_undistort(liliom_ctx* c, void* pts_inout, int n, const dou
     return LILIOM_OK;
 }
 
-// ===================== L2: map =====================
-extern "C" int liliom_map_clear(liliom_ctx* c) {
-    if (!c) return LILIOM_E_ARG;
-    c->frames.clear();
-    c->inc_valid = false;
-    c->map.ready = false; c->map.n = 0; c->map_n_global = 0;
-    return LILIOM_OK;
-}
-
-// Shared body of the two push_frame entry points: d_src = n body-frame points of point_stride bytes ON THE DEVICE.
-static int push_frame_from_device(liliom_ctx* c, const void* d_src, int n, const double pose7[7], bool keep_inc = false) {
-    const int stride = c->prm.point_stride;
-    if (!keep_inc) c->inc_valid = false;        // the entry array of liliom_map_update no longer describes the FIFO
-    Frame f;
-    f.slot = (int)c->frames.size();
-    if ((int)c->frames.size() >= c->prm.max_map_frames && !c->frames.empty()) {      // L/src/LidarOdometry.cpp:293-296 pop_front
-        f.buf = std::move(c->frames.front().buf);   // the popped frame's allocation is recycled: cudaFree + cudaMalloc per scan cost
-        f.slot = c->frames.front().slot;        // more than the whole map maintenance of a 10 M-point map (cudaFree synchronises)
-        c->frames.erase(c->frames.begin());
-    }
-    f.n = n;
-    int rc = LILIOM_OK;
-    if (n > 0) {
-        Q4 q{pose7[0], pose7[1], pose7[2], pose7[3]};
-        D3 t{pose7[4], pose7[5], pose7[6]};
-        auto body = [&]() -> int {
-            LILI_CUDA(c, f.buf.ensure((size_t)n * stride));
-            if (c->nranks == 1) {
-                k_transform_cloud<<<cdiv(n, 256), 256, 0, c->stream>>>((const unsigned char*)d_src, n, stride, q, t, (unsigned char*)f.buf.p);
-                LILI_TRY(launch_check(c, "k_transform_cloud"));
-                LILI_TRY(vg_minmax_dev(c, f.buf.p, n, nullptr, stride));                 // the frame's box, for the rebuilds it takes part in
-                return read_back(c, {{f.mm, c->vg_minmax.p, 7 * sizeof(int)}});
-            }
-            // sharded map maintenance: every rank receives the frame, keeps the points within (search radius + one voxel
-            // diagonal) of a block it owns — every voxel that can reach an owned query's 1 m ball is then complete locally —
-            // and voxel-filters / indexes only its shard.  No inter-rank traffic.
-            LILI_CUDA(c, c->map_ds.ensure((size_t)n * stride));
-            LILI_CUDA(c, c->flags.ensure(((size_t)n + 2) * 4));
-            LILI_CUDA(c, c->idx_a.ensure(((size_t)n + 2) * 4));
-            k_transform_cloud<<<cdiv(n, 256), 256, 0, c->stream>>>((const unsigned char*)d_src, n, stride, q, t, (unsigned char*)c->map_ds.p);
-            LILI_TRY(launch_check(c, "k_transform_cloud"));
-            const float halo = gate_cell(c->prm.knn_max_sqdist) + 1.7320508f * c->prm.leaf_map + 0.05f;
-            k_shard_flags_strided<<<cdiv(n + 1, 256), 256, 0, c->stream>>>((const unsigned char*)c->map_ds.p, n, stride, halo, c->shard_inv_block, c->nranks, c->rank, c->flags.as<int>());
-            LILI_TRY(launch_check(c, "k_shard_flags_strided"));
-            LILI_TRY(exclusive_scan_i32(c, c->flags.as<int>(), c->idx_a.as<int>(), n));
-            k_compact_strided<<<cdiv(n, 256), 256, 0, c->stream>>>((const unsigned char*)c->map_ds.p, c->flags.as<int>(), c->idx_a.as<int>(), n, stride,
-                                                                  (unsigned char*)f.buf.p);
-            LILI_TRY(launch_check(c, "k_compact_strided"));
-            LILI_TRY(vg_minmax_dev(c, f.buf.p, n, c->idx_a.as<int>() + n, stride));     // box of the points this rank keeps
-            return read_back(c, {{&f.n, c->idx_a.as<int>() + n, sizeof(int)}, {f.mm, c->vg_minmax.p, 7 * sizeof(int)}});
-        };
-        rc = body();
-    }
-    if (rc != LILIOM_OK) return rc;
-    c->frames.push_back(std::move(f));
-    return LILIOM_OK;
-}
-
-extern "C" int liliom_map_push_frame(liliom_ctx* c, const void* surf_ds_body, int n, const double pose7[7]) {
-    if (!c || n < 0 || (n > 0 && !surf_ds_body) || !pose7) return LILIOM_E_ARG;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    const int stride = c->prm.point_stride;
-    if (n > 0) {
-        LILI_CUDA(c, c->raw.ensure((size_t)n * stride));
-        LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, surf_ds_body, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
-    }
-    return push_frame_from_device(c, c->raw.p, n, pose7);
-}
-
-extern "C" int liliom_map_push_frame_device(liliom_ctx* c, const void* d_surf_ds_body, int n, const double pose7[7]) {
-    if (!c || n < 0 || (n > 0 && !d_surf_ds_body) || !pose7) return LILIOM_E_ARG;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    return push_frame_from_device(c, d_surf_ds_body, n, pose7);
-}
-
-namespace lili {
-// tail shared by the rebuild and the incremental update (single GPU): c->map_ds holds m filtered points
-void frames_box(const liliom_ctx* c, int mm[kBoxInts]) {
-    for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_empty(k);
-    for (const auto& f : c->frames) vg_box_merge(mm, f.mm);
-}
-
-int map_finish_from_ds(liliom_ctx* c, int m) {
-    const int stride = c->prm.point_stride;
-    LILI_CUDA(c, c->map.xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
-    c->map_n_global = m;
-    LILI_TRY(repack_to_f4(c, c->map_ds.p, m, stride, c->map.xyzw.as<float4>()));
-    int mm[7];
-    frames_box(c, mm);
-    LILI_TRY(grid_build(c, m, mm[6] > 0 ? mm : nullptr));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    return LILIOM_OK;
-}
-}  // namespace lili
-
-extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out);
-
-// SURVEY §8 (f2): push + incremental refresh (map_inc.cu); same result as liliom_map_push_frame + liliom_map_rebuild
-static int map_update_from_device(liliom_ctx* c, const void* d_src, int n, const double pose7[7], int* n_map_out) {
-    if (n_map_out) *n_map_out = 0;
-    const bool incremental = c->nranks == 1 && c->prm.max_map_frames <= 64 && n < (1 << 24);
-    int popped_slot = -1, popped_nfin = 0;
-    if ((int)c->frames.size() >= c->prm.max_map_frames && !c->frames.empty()) { popped_slot = c->frames.front().slot; popped_nfin = c->frames.front().mm[6]; }
-    LILI_TRY(push_frame_from_device(c, d_src, n, pose7, incremental));
-    if (incremental) {
-        c->map.ready = false; c->map.n = 0; c->map_n_global = 0;
-        int m = 0;
-        const int rc = map_inc_update(c, popped_slot, popped_nfin, &m);
-        if (rc == LILIOM_OK) {
-            LILI_TRY(map_finish_from_ds(c, m));
-            if (n_map_out) *n_map_out = m;
-            return LILIOM_OK;
-        }
-        c->inc_valid = false;
-        if (rc != LILIOM_E_GRID) return rc;       // E_GRID: keys not representable / PCL's overflow case -> the sort chain decides
-    }
-    return liliom_map_rebuild(c, n_map_out);
-}
-
-extern "C" int liliom_map_update(liliom_ctx* c, const void* surf_ds_body, int n, const double pose7[7], int* n_map_out) {
-    if (!c || n < 0 || (n > 0 && !surf_ds_body) || !pose7) return LILIOM_E_ARG;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    const int stride = c->prm.point_stride;
-    if (n > 0) {
-        LILI_CUDA(c, c->raw.ensure((size_t)n * stride));
-        LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, surf_ds_body, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
-    }
-    return map_update_from_device(c, c->raw.p, n, pose7, n_map_out);
-}
-
-extern "C" int liliom_map_update_device(liliom_ctx* c, const void* d_surf_ds_body, int n, const double pose7[7], int* n_map_out) {
-    if (!c || n < 0 || (n > 0 && !d_surf_ds_body) || !pose7) return LILIOM_E_ARG;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    return map_update_from_device(c, d_surf_ds_body, n, pose7, n_map_out);
-}
-
-// surf_from_map_ds as a point cloud (all fields), in liliom_map_download order
-extern "C" int liliom_map_download_cloud(liliom_ctx* c, void* out, int cap, int* m_out) {
-    if (!c || !m_out) return LILIOM_E_ARG;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    if (c->nranks > 1) { c->last_error = "liliom_map_download_cloud is single-GPU"; return LILIOM_E_ARG; }
-    return download_sized(c, c->map_ds, c->map_n_global, c->prm.point_stride, out, cap, m_out);
-}
-
-extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
-    if (!c) return LILIOM_E_ARG;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    const int stride = c->prm.point_stride;
-    // LILIOM_DEBUG_TIMING: wall clock of the phases (each closed by a stream sync), printed by rank 0
-    double tph[8] = {0};
-    int nph = 0;
-    auto mark = [&]() {
-        if (c->dbg_timing && nph < 8) { cudaStreamSynchronize(c->stream); timespec ts; clock_gettime(CLOCK_MONOTONIC, &ts); tph[nph++] = ts.tv_sec * 1e6 + ts.tv_nsec * 1e-3; }
-    };
-    mark();
-    size_t total = 0;
-    for (auto& f : c->frames) total += (size_t)f.n;
-    c->map.ready = false; c->map.n = 0; c->map_n_global = 0;
-    if (n_map_out) *n_map_out = 0;
-    if (total == 0 && c->nranks == 1) { c->map.ready = true; return LILIOM_OK; }
-    LILI_CUDA(c, c->map_raw.ensure((total > 0 ? total : 1) * stride));
-    LILI_CUDA(c, c->map_ds.ensure((total > 0 ? total : 1) * stride));
-    LILI_CUDA(c, c->vg_count.ensure(16));
-    // bounding box and finite count of the concatenation = union over the frames (each measured once, at its push)
-    int box[7];
-    frames_box(c, box);
-    // single GPU: the centroid kernel writes the float4 map itself (no repack pass); at most `total` voxels
-    if (c->nranks == 1) LILI_CUDA(c, c->map.xyzw.ensure((total > 0 ? total : 1) * sizeof(float4)));
-    size_t off = 0;
-    if (c->frames.size() <= (size_t)kConcatMax && total > 0) {
-        ConcatTab tab{};
-        int k = 0;
-        size_t largest = 0;
-        for (auto& f : c->frames) {
-            tab.src[k] = (const float4*)f.buf.p; tab.off[k] = (long long)(off * (stride / 16));
-            off += (size_t)f.n; largest = f.n > (int)largest ? (size_t)f.n : largest; ++k;
-        }
-        for (; k <= kConcatMax; ++k) tab.off[k] = (long long)(off * (stride / 16));
-        const int bx = max(1, min(cdiv((long long)largest * (stride / 16), 256 * 4), c->sm_count * 4));
-        k_concat_frames<<<dim3(bx, (unsigned)c->frames.size()), 256, 0, c->stream>>>(tab, (float4*)c->map_raw.p);
-        LILI_TRY(launch_check(c, "k_concat_frames"));
-    } else
-    for (auto& f : c->frames) {                                                    // :301-302 concatenation, oldest first
-        if (f.n) LILI_CUDA(c, cudaMemcpyAsync((unsigned char*)c->map_raw.p + off * stride, f.buf.p, (size_t)f.n * stride, cudaMemcpyDeviceToDevice, c->stream));
-        off += (size_t)f.n;
-    }
-    mark();      // [1] concatenation
-    int m = 0;
-    if (total > 0) {
-        // (The single-launch cooperative filter of the scan VoxelGrid was tried here for maps of <= 32k points: within the noise
-        // of the real-size streamed lifecycle — not kept.)
-        LILI_TRY(voxelgrid_dev(c, c->map_raw.p, (int)total, nullptr, stride, c->prm.leaf_map, c->map_ds.p, c->vg_count.as<int>(),   // :316-317
-                               c->nranks == 1 ? c->map.xyzw.as<float4>() : nullptr, 32, box));
-        LILI_TRY(read_back(c, {{&m, c->vg_count.p, sizeof(int)}}));
-    }
-    mark();      // [2] VoxelGrid
-    LILI_CUDA(c, c->map.xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
-    c->map_n_global = m;
-    if (c->nranks > 1) {
-        // Every rank ENTERS the all-reduce whatever happened locally (a rank that returned early would leave its peers waiting
-        // in the collective): the local status travels as a second scalar and all ranks fail together.
-        // Shard filter: drops the (possibly incomplete) voxels beyond the 1-cell halo, fused with the repack to float4.
-        auto shard_and_index = [&]() -> int {
-            int local = 0;
-            if (m > 0) {
-                LILI_CUDA(c, c->flags.ensure(((size_t)m + 2) * 4));
-                LILI_CUDA(c, c->idx_a.ensure(((size_t)m + 2) * 4));
-                k_shard_flags_strided<<<cdiv(m + 1, 256), 256, 0, c->stream>>>((const unsigned char*)c->map_ds.p, m, stride, gate_cell(c->prm.knn_max_sqdist),
-                                                                             c->shard_inv_block, c->nranks, c->rank, c->flags.as<int>());
-                LILI_TRY(launch_check(c, "k_shard_flags_strided"));
-                LILI_TRY(exclusive_scan_i32(c, c->flags.as<int>(), c->idx_a.as<int>(), m));
-                k_compact_repack<<<cdiv(m, 256), 256, 0, c->stream>>>((const unsigned char*)c->map_ds.p, c->flags.as<int>(), c->idx_a.as<int>(), m, stride,
-                                                                     c->map.xyzw.as<float4>());
-                LILI_TRY(launch_check(c, "k_compact_repack"));
-                LILI_TRY(read_back(c, {{&local, c->idx_a.as<int>() + m, sizeof(int)}}));
-            }
-            return grid_build(c, local, box[6] > 0 ? box : nullptr);
-        };
-        const int rc_local = shard_and_index();
-        mark();  // [3] shard filter + cell grid
-        // the "< 10 map points" guard (L/src/LidarOdometry.cpp:485-488) is about the whole map: sum the owned-voxel counts
-        LILI_CUDA(c, c->neq.ensure(32 * sizeof(double)));
-        double* pin = c->h_pin->map_status;
-        pin[0] = rc_local == LILIOM_OK ? (double)c->map.n : 0.0;
-        pin[1] = rc_local == LILIOM_OK ? 0.0 : 1.0;
-        LILI_CUDA(c, cudaMemcpyAsync(c->neq.p, pin, 2 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-        LILI_TRY(nccl_allreduce_sum_f64(c, c->neq.as<double>(), 2));
-        LILI_CUDA(c, cudaMemcpyAsync(pin + 2, c->neq.p, 2 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-        if (rc_local != LILIOM_OK) return rc_local;
-        if (pin[3] != 0.0) { c->map.ready = false; c->last_error = "liliom_map_rebuild failed on another rank"; return LILIOM_E_NCCL; }
-        c->map_n_global = (int)pin[2];                  // halo voxels are counted on several ranks: an upper bound >= the true size
-    } else {
-        LILI_TRY(grid_build(c, m, box[6] > 0 ? box : nullptr));     // map_xyzw was written by the VoxelGrid's centroid kernel
-    }
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    mark();      // [3 or 4] cell grid (single GPU) / map-size all-reduce (sharded)
-    if (c->dbg_timing && c->rank == 0 && nph >= 4) {
-        fprintf(stderr, "[liliom_map_rebuild, us] %zu raw points, %d voxels: concat %.0f, VoxelGrid %.0f, %s %.0f", total, m, tph[1] - tph[0], tph[2] - tph[1],
-                c->nranks > 1 ? "shard filter + grid" : "grid", tph[3] - tph[2]);
-        if (nph >= 5) fprintf(stderr, ", all-reduce %.0f", tph[4] - tph[3]);
-        fprintf(stderr, "\n");
-    }
-    if (n_map_out) *n_map_out = m;
-    return LILIOM_OK;
-}
-
-extern "C" int liliom_map_set_points(liliom_ctx* c, const liliom_f4* xyzw, int m) {
-    if (!c || m < 0 || (m > 0 && !xyzw)) return LILIOM_E_ARG;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    c->map.refl.release();
-    c->map.ready = false;
-    LILI_CUDA(c, c->map.xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
-    LILI_CUDA(c, c->raw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
-    if (m > 0) {
-        LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, xyzw, (size_t)m * sizeof(float4), cudaMemcpyHostToDevice, c->stream));
-        LILI_TRY(repack_to_f4(c, c->raw.p, m, 16, c->map.xyzw.as<float4>()));
-    }
-    LILI_TRY(install_map_from_xyzw(c, m));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    return LILIOM_OK;
-}
-
-// Install a PCL-layout cloud as the map, keeping its reflectivity channel for the Horizon backend variant.
-extern "C" int liliom_map_set_cloud(liliom_ctx* c, const void* pts, int m, int stride) {
-    if (!c || m < 0 || (m > 0 && !pts) || (stride != 48 && stride != 32)) return LILIOM_E_ARG;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    if (c->nranks > 1) { c->last_error = "liliom_map_set_cloud is single-GPU"; return LILIOM_E_ARG; }
-    c->map.ready = false;
-    LILI_CUDA(c, c->map.xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
-    LILI_CUDA(c, c->map.refl.ensure((size_t)(m > 0 ? m : 1) * sizeof(float)));
-    LILI_CUDA(c, c->raw.ensure((size_t)(m > 0 ? m : 1) * stride));
-    if (m > 0) {
-        LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, pts, (size_t)m * stride, cudaMemcpyHostToDevice, c->stream));
-        LILI_TRY(repack_to_f4(c, c->raw.p, m, stride, c->map.xyzw.as<float4>()));
-        if (stride == 48) {
-            k_kf_refl<<<cdiv(m, 256), 256, 0, c->stream>>>((const unsigned char*)c->raw.p, m, c->map.refl.as<float>());
-            LILI_TRY(launch_check(c, "k_kf_refl"));
-        } else LILI_CUDA(c, cudaMemsetAsync(c->map.refl.p, 0, (size_t)m * sizeof(float), c->stream));
-    }
-    LILI_TRY(install_map_from_xyzw(c, m));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    return LILIOM_OK;
-}
-
-extern "C" int liliom_map_size(const liliom_ctx* c) { return c ? c->map.n : 0; }
-
-extern "C" int liliom_map_download(liliom_ctx* c, liliom_f4* out, int cap, int* m_out) {
-    if (!c || !m_out) return LILIOM_E_ARG;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    return download_sized(c, c->map.xyzw, c->map.n, sizeof(float4), out, cap, m_out);
-}
-
 // ===================== L2: scan-to-map =====================
 extern "C" int liliom_upload_feats(liliom_ctx* c, const void* feats, int n, int stride) {
     if (!c) return LILIOM_E_ARG;
@@ -1001,16 +611,8 @@ extern "C" int liliom_icp_align(liliom_ctx* c, const void* src, int n_src, const
     LILI_CUDA(c, cudaSetDevice(c->device));
     if (c->nranks > 1) { c->last_error = "liliom_icp_align is single-GPU"; return LILIOM_E_ARG; }
     // target -> the context's map (cell grid), source -> the resident query array
-    c->map.refl.release();
-    c->map.ready = false;
     c->inc_valid = false;
-    LILI_CUDA(c, c->map.xyzw.ensure((size_t)(n_tgt > 0 ? n_tgt : 1) * sizeof(float4)));
-    LILI_CUDA(c, c->raw.ensure((size_t)(n_tgt > 0 ? n_tgt : 1) * stride));
-    if (n_tgt > 0) {
-        LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, tgt, (size_t)n_tgt * stride, cudaMemcpyHostToDevice, c->stream));
-        LILI_TRY(repack_to_f4(c, c->raw.p, n_tgt, stride, c->map.xyzw.as<float4>()));
-    }
-    LILI_TRY(install_map_from_xyzw(c, n_tgt));
+    LILI_TRY(map_install_host(c, tgt, n_tgt, stride, false));
     LILI_TRY(upload_feats(c, src, n_src, stride));
     return icp_align(c, c->map, c->feats.as<float4>(), n_src, max_corr_dist, max_iter, trans_eps, fit_eps, T16, fitness, converged, iters);
 }

@@ -152,7 +152,7 @@ __device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int tar
 struct Frame {        // one entry of recent_surf_frames (world frame, point_stride bytes per point)
     DevBuf buf;
     int n = 0;
-    // incremental map (map_inc.cu): slot id carried by the frame's entries, unrepresentable key seen
+    // incremental map (map.cu): slot id carried by the frame's entries, unrepresentable key seen
     int slot = 0;
     bool bad = false;
     // box of the stored points (vg_box.h; mm[6] = finite points), taken when the frame was pushed: the rebuild's VoxelGrid, the
@@ -225,17 +225,18 @@ struct liliom_ctx {
     lili::DevBuf vg_keys, vg_keys2, vg_vals, vg_vals2, vg_flags, vg_rank, vg_params, vg_out, vg_minmax, vg_count;
     lili::DevBuf cub_tmp;
 
-    // ---- map ----
+    // ---- map (map.cu) ----
     std::vector<lili::Frame> frames;     // FIFO, oldest first
-    // incremental map (liliom_map_update, map_inc.cu): entries {voxel key, slot<<24|index} sorted by (key, frame age, index), double-buffered
+    // incremental map (liliom_map_update): entries {voxel key, slot<<24|index} sorted by (key, frame age, index), double-buffered
     lili::DevBuf inc_key[2], inc_ref[2], inc_newkey[2], inc_newref[2], inc_removed, inc_rpos, inc_flags, inc_rank, inc_bad;
     int inc_cur = 0, inc_E = 0;
     bool inc_valid = false;
     lili::DevBuf map_raw;                // concatenated frames (stride bytes)
-    lili::DevBuf map_ds;                 // VoxelGrid output (stride bytes) or installed float4
+    lili::DevBuf map_ds;                 // VoxelGrid output (stride bytes); scratch of the sharded install
+    int map_ds_n = 0;                    // records of the filtered cloud in map_ds; -1: an installed map has none behind it
     lili::MapIndex map;                  // the odometry map's search index (scan-to-map, backend single-keyframe calls, ICP target)
     lili::DevBuf grid_keys, grid_keys2, grid_vals, grid_vals2;   // grid_build scratch, shared by every index
-    int map_n_global = 0;
+    int map_n_global = 0;                // map size over all ranks: the "< 10 map points" guard
 
     // ---- backend (keyframes.cu, backend_corr.cu): keyframe store, local map layers, window correspondences ----
     lili::DevBuf kf_arena;               // body-frame clouds of every keyframe (point_stride bytes per point)
@@ -398,9 +399,7 @@ bool rot_lines_ok(int line_num, bool field);
 
 int icp_align(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,
               double fit_eps, double T16[16], double* fitness, int* converged, int* iters);     // icp.cu
-int map_inc_update(liliom_ctx* c, int popped_slot, int popped_nfin, int* m_out);     // map_inc.cu
-int map_finish_from_ds(liliom_ctx* c, int m);                                        // api.cu
-void frames_box(const liliom_ctx* c, int mm[7]);                                     // api.cu: union of the frames' boxes
+int map_install_host(liliom_ctx* c, const void* pts, int m, int stride, bool keep_refl);     // map.cu
 
 int block27_stats(liliom_ctx* c, const double pose7[7], unsigned long long out[2]);   // grid_knn.cu
 

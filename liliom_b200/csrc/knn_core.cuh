@@ -40,6 +40,14 @@ __device__ __forceinline__ int owner_of(float x, float y, float z, int nranks, f
     const int h = (bx + 3 * by + 5 * bz) % nranks;
     return h < 0 ? h + nranks : h;
 }
+// A rank's map shard: the points whose +-halo box touches a cube the rank owns.  The box's eight corners decide it while the
+// box is narrower than a cube (it then spans at most two per axis).  With a halo of at least the search radius every
+// neighbour of an owned query is local.
+__device__ __forceinline__ bool shard_keep(float x, float y, float z, float halo, int nranks, int rank, float inv_block) {
+    for (int c = 0; c < 8; ++c)
+        if (owner_of(x + ((c & 1) ? halo : -halo), y + ((c & 2) ? halo : -halo), z + ((c & 4) ? halo : -halo), nranks, inv_block) == rank) return true;
+    return false;
+}
 
 typedef unsigned long long u64;
 

@@ -5,7 +5,7 @@
 //   * PCL's parameters derived from it and a point's voxel index;
 //   * a voxel's centroid: the fields summed, the walk over its members in a sorted entry array, and the output point.
 // The kernels that measure a box, index voxels or write centroids (the sort chain and k_vg_coop in voxelgrid.cu, the
-// incremental map in map_inc.cu, the per-ring filter in extract_rot.cu, the cell grid in grid_knn.cu, the global map's table
+// incremental map in map.cu, the per-ring filter in extract_rot.cu, the cell grid in grid_knn.cu, the global map's table
 // filter in keyframes.cu) and the host code that
 // reads a box back use this file, so they agree on every voxel and every bit of a centroid.  Plain C++ usable from device
 // code and from the host (tests/vg_box_host.cpp compiles this same file for the CPU test tier).

@@ -1,5 +1,5 @@
 """Host-side statement of the multi-GPU partition rule implemented in csrc/ (knn_core.cuh
-`owner_of`, api.cu `k_shard_flags`): space is cut into 16 m blocks (shifted by half a block in z), a block belongs to rank
+`owner_of` and `shard_keep`): space is cut into 16 m blocks (shifted by half a block in z), a block belongs to rank
 (bx + 3 by + 5 bz) mod nranks, a query is processed by the owner of the block its transformed position
 falls in, and a rank's map shard holds every point whose +-halo box touches a block it owns (so the
 query's whole 1 m search ball is local).  Used by bench.py to report shard sizes and by the gloo tests."""

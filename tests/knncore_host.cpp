@@ -110,6 +110,10 @@ static void run_group(int nq, const float* q3, const float4* map, const int* cel
 extern "C" {
 float kc_gate_tau(double max_sqd) { return knn_gate_tau(max_sqd); }
 int kc_owner_of(float x, float y, float z, int nranks, float inv_block) { return owner_of(x, y, z, nranks, inv_block); }
+// shard_keep for n points xyz[3 * i ..]: keep[i] = 1 when rank keeps point i
+void kc_shard_keep(int n, const float* xyz, float halo, int nranks, int rank, float inv_block, unsigned char* keep) {
+    for (int i = 0; i < n; ++i) keep[i] = shard_keep(xyz[3 * i], xyz[3 * i + 1], xyz[3 * i + 2], halo, nranks, rank, inv_block) ? 1 : 0;
+}
 
 // map_sorted: m x {x, y, z, index bits} in cell order; returns the number of map points examined
 unsigned long long kc_thread_knn5(float sx, float sy, float sz, const float* map_sorted, const int* cell_start, float inv_cell,

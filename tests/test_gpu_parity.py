@@ -540,7 +540,7 @@ def test_map_too_large_for_dense_grid():
 # ---------------------------------------------------------------- (f2) incremental device map
 @pytest.mark.parametrize("variant", [0, 1])
 def test_incremental_map_update_equals_rebuild_over_a_stream(oracle, world_small, variant):
-    """liliom_map_update (push + incremental merge of the resident voxel entries, map_inc.cu) against the oracle's
+    """liliom_map_update (push + incremental merge of the resident voxel entries, map.cu) against the oracle's
     concat + VoxelGrid(0.4) of the last 20 frames, every scan of a 46-scan stream, every field bit for bit; and against a second
     context that takes the two-step path (push_frame + rebuild): same cloud, same correspondences.  The stream has overlapping
     frames (most voxels hold points of several frames), an empty frame, non-finite points, a frame of exact duplicates, and a
@@ -613,4 +613,76 @@ def test_incremental_map_falls_back_when_keys_do_not_fit(oracle, world_small):
         got = c.map_download_cloud()
         assert m == len(want) == len(got), k
         _fields_equal(got, want, ["x", "y", "z", "nx", "ny", "nz", "intensity", "curvature"])
+    c.close()
+
+
+def test_map_past_64_frames_equals_reference_pipeline(oracle, world_small):
+    """A FIFO longer than one concatenation launch holds (max_map_frames 70, 64 frames per launch): liliom_map_rebuild and
+    liliom_map_update (the two-step path at this FIFO length) against the oracle's VoxelGrid(0.4) of the concatenation, every
+    field bit for bit, at 64 frames, 65, 70 and after four pops.  One frame of the second launch is empty."""
+    import liliom_b200 as L
+    p = L.default_params(0); p.max_map_frames = 70
+    a, b = L.Context(p), L.Context(p)
+    surf, _, _ = oracle.extract_horizon(world_small["hz"], world_small["q_hz"])
+    ds = oracle.voxelgrid(surf, 0.4)
+    fields = ["x", "y", "z", "nx", "ny", "nz", "intensity", "curvature"]
+    rng = np.random.default_rng(41)
+    frames = []
+    for k in range(74):
+        pose = np.array(world_small["T"]); pose[4] += 0.07 * k; pose[5] += 0.02 * k
+        sub = ds[np.sort(rng.permutation(len(ds))[: int(len(ds) * rng.uniform(0.05, 0.3))])].copy()
+        if k == 66:
+            sub = sub[:0]
+        frames.append(oracle.transform_cloud(sub, pose))
+        a.map_push_frame(sub, pose)
+        mb = b.map_update(sub, pose)
+        if k in (63, 64, 69, 73):
+            ma = a.map_rebuild()
+            want = oracle.voxelgrid(np.concatenate(frames[-70:]), 0.4)
+            assert ma == mb == len(want), (k, ma, mb, len(want))
+            _fields_equal(a.map_download_cloud(), want, fields)
+            _fields_equal(b.map_download_cloud(), want, fields)
+            assert a.map_download().tobytes() == b.map_download().tobytes(), k
+    a.close(); b.close()
+
+
+def test_map_download_cloud_after_an_install_reports_no_map(oracle, world_small):
+    """An installed map (liliom_map_set_points) has no filtered cloud behind it: liliom_map_download_cloud returns LILIOM_E_NOMAP,
+    not the cloud of an earlier rebuild and not a copy from a buffer no rebuild has written.  The next rebuild brings the FIFO's
+    cloud back, and after liliom_map_clear the cloud is empty.  Only size queries are made while the answer may be stale."""
+    import ctypes as C
+    import liliom_b200 as L
+    lib = L._binding.lib()
+
+    def size_query(c):
+        n = C.c_int(-7)
+        return lib.liliom_map_download_cloud(c._h, None, 0, C.byref(n)), n.value
+
+    fresh = L.Context(variant=0)
+    fresh.map_set_points(world_small["map"][:5000])
+    assert size_query(fresh)[0] == L._binding.E_NOMAP
+    assert "installed" in lib.liliom_last_error(fresh._h).decode()
+    fresh.close()
+
+    surf, _, _ = oracle.extract_horizon(world_small["hz"], world_small["q_hz"])
+    ds = oracle.voxelgrid(surf, 0.4)
+    fields = ["x", "y", "z", "nx", "ny", "nz", "intensity", "curvature"]
+    c = L.Context(variant=0)
+    frames = []
+    for k in range(4):
+        pose = np.array(world_small["T"]); pose[4] += 0.3 * k
+        c.map_push_frame(ds, pose)
+        frames.append(oracle.transform_cloud(ds, pose))
+    m = c.map_rebuild()
+    want = oracle.voxelgrid(np.concatenate(frames), 0.4)
+    _fields_equal(c.map_download_cloud(), want, fields)
+    c.map_set_points(world_small["map"][: m // 2])
+    assert size_query(c)[0] == L._binding.E_NOMAP
+    with pytest.raises(L.LiliomError) as e:
+        c.map_download_cloud()
+    assert e.value.code == L._binding.E_NOMAP
+    assert c.map_rebuild() == m
+    _fields_equal(c.map_download_cloud(), want, fields)
+    c.map_clear()
+    assert size_query(c) == (L._binding.OK, 0)
     c.close()

@@ -37,6 +37,8 @@ def kc():
     L.kc_coherence_tau.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
     L.kc_coherence_tau.restype = None
     L.kc_owner_of.argtypes = [C.c_float, C.c_float, C.c_float, C.c_int, C.c_float]; L.kc_owner_of.restype = C.c_int
+    L.kc_shard_keep.argtypes = [C.c_int, C.c_void_p, C.c_float, C.c_int, C.c_int, C.c_float, C.c_void_p]
+    L.kc_shard_keep.restype = None
     return L
 
 
@@ -306,3 +308,30 @@ def test_partition_rule_mirror_equals_the_device_function(kc):
             if nranks > 1:
                 share = np.bincount(got[:3000], minlength=nranks) / 3000.0
                 assert share.max() < 2.2 / nranks                                   # the linear hash spreads a 1.4 km stretch evenly
+
+
+def test_shard_rule_mirror_equals_the_device_function(kc):
+    """liliom_b200/sharding.py::shard_mask (the gloo tests' restatement of the sharded map) against knn_core.cuh::shard_keep compiled
+    for the host, for every rank: the search-radius halo of the installed and rebuilt maps and the raw frames' halo (+ one voxel
+    diagonal, formed in fp32 as the push forms it), random points, points on cube faces (z faces half an edge up) and points whose
+    halo corners land on a face."""
+    from liliom_b200 import sharding
+    rng = np.random.default_rng(12)
+    halo_frame = F(F(1.0) + F(F(1.7320508) * F(0.4))) + F(0.05)
+    for block in (8, 16, 64):
+        faces = np.round(rng.uniform(-12, 12, (2400, 3))) * block - np.array([0.0, 0.0, block / 2])
+        for halo in (F(1.0), halo_frame):
+            kind = rng.integers(0, 4, (2400, 3))                                   # per coordinate: random, face, face +- halo, beside a face
+            near = np.where(kind == 0, rng.uniform(-300, 300, (2400, 3)),
+                   np.where(kind == 1, faces, np.where(kind == 2, faces + rng.choice([-1.0, 1.0], (2400, 3)) * float(halo),
+                                                        faces + rng.choice([-1e-3, 1e-3], (2400, 3)))))
+            pts = np.ascontiguousarray(near, F)
+            for nranks in (2, 4, 8):
+                owned = np.zeros(len(pts), bool)
+                for rank in range(nranks):
+                    got = np.zeros(len(pts), np.uint8)
+                    kc.kc_shard_keep(len(pts), pts.ctypes.data, halo, nranks, rank, F(1.0 / block), got.ctypes.data)
+                    want = sharding.shard_mask(pts, nranks, rank, halo=float(halo), block=block)
+                    assert np.array_equal(got.astype(bool), want), (block, float(halo), nranks, rank)
+                    owned |= want & (sharding.owner_of(pts, nranks, block) == rank)
+                assert owned.all()                                                  # every point is in its owner's shard

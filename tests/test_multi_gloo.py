@@ -82,7 +82,7 @@ def test_shard_rule_properties():
 
 
 def _maint_worker(rank, world, port, out):
-    """Sharded map maintenance (api.cu push_frame_from_device / liliom_map_rebuild with a communicator), restated on the host:
+    """Sharded map maintenance (map.cu push_frame_from_device / liliom_map_rebuild with a communicator), restated on the host:
     a rank keeps the frame points within (1 m + one voxel diagonal) of a block it owns, voxel-filters its shard alone, and
     keeps the voxels within 1 m of an owned block."""
     sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
