@@ -497,6 +497,27 @@ int liliom_upload_feats(liliom_ctx* c, const void* feats_body, int n, int stride
 int liliom_scan_to_map_resident(liliom_ctx* c, double pose7_inout[7], int match_cnt, int max_num_iter, int mode,
                                 liliom_iter_stats* stats);
 
+/* ===================== several sessions in one call ===================== */
+/* One GN-mode scan-to-map step of B independent sessions (contexts) in as few launches as fit on the device.
+ * Session i gets exactly what liliom_scan_to_map_resident(ctxs[i], poses7 + 7*i, match_cnt, 0, LILIOM_MODE_GN,
+ * stats ? stats + i*match_cnt : NULL) would give it, bit for bit, including the state it leaves in ctxs[i].
+ * status[i] = that call's return value; a session with LILIOM_E_NOMAP / LILIOM_E_FEWMAP keeps its pose, the others run.
+ * Sessions whose solo call runs all iterations in one cooperative launch share cooperative launches (each with its own grid
+ * barrier, so no session waits for another); the others take their solo path inside the same call.
+ * LILIOM_E_ARG for the whole call, nothing changed: B < 1, a NULL array (ctxs, poses7_inout, status), match_cnt < 0, a NULL
+ * or repeated context, contexts on different devices, a context with a communicator (liliom_comm_init; sharded or fused).
+ * Streams: the shared launches run on ctxs[0]'s stream; every other session's stream (liliom_set_stream) is ordered before
+ * and after them with events, and the call is synchronous like every other call.
+ * Counters: launches advances on every session that took part in a launch; knn_queries / knn_candidates are counted per
+ * session on the device; the event timing of the shared launches (knn_ms, knn_launches) goes to ctxs[0] only. */
+int liliom_scan_to_map_resident_batch(liliom_ctx* const* ctxs, int B, double* poses7_inout, int match_cnt,
+                                      liliom_iter_stats* stats, int* status);
+/* Same, with the semantics of liliom_odometry_resident per session: VoxelGrid(leaf_scan) of the surf features that the
+ * session's last liliom_extract_* / liliom_extract_resident left resident, then the step.  ds_out[i] / ds_cap[i] / n_ds[i]
+ * are optional per session (NULL arrays or NULL entries: no download). */
+int liliom_odometry_resident_batch(liliom_ctx* const* ctxs, int B, double* poses7_inout, int match_cnt,
+                                   liliom_iter_stats* stats, void* const* ds_out, const int* ds_cap, int* n_ds, int* status);
+
 #ifdef __cplusplus
 }
 #endif

@@ -77,6 +77,7 @@ EXPORTS = [
     "liliom_bmap_download", "liliom_backend_window_correspond", "liliom_backend_window_blocks", "liliom_backend_window_corr",
     "liliom_kf_cloud", "liliom_kf_add_full", "liliom_global_map", "liliom_loop_align",
     "liliom_convert_pc2", "liliom_extract_rot_pc2", "liliom_set_ring_source", "liliom_set_time_source",
+    "liliom_scan_to_map_resident_batch", "liliom_odometry_resident_batch",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -171,6 +172,8 @@ def lib() -> C.CDLL:
     L.liliom_set_kernel_timing.argtypes = [vp, C.c_int]
     L.liliom_upload_feats.argtypes = [vp, vp, C.c_int, C.c_int]
     L.liliom_scan_to_map_resident.argtypes = [vp, dp, C.c_int, C.c_int, C.c_int, C.POINTER(IterStats)]
+    L.liliom_scan_to_map_resident_batch.argtypes = [C.POINTER(vp), C.c_int, dp, C.c_int, C.POINTER(IterStats), ip]
+    L.liliom_odometry_resident_batch.argtypes = [C.POINTER(vp), C.c_int, dp, C.c_int, C.POINTER(IterStats), C.POINTER(vp), ip, ip, ip]
     L.liliom_odometry.argtypes = [vp, vp, C.c_int, dp, C.c_int, C.c_int, C.c_int, C.POINTER(IterStats), vp, C.c_int, ip]
     L.liliom_set_stream.argtypes = [vp, vp]
     L.liliom_upload_scan.argtypes = [vp, vp, C.c_int]
@@ -739,6 +742,49 @@ class Context:
     def set_kernel_timing(self, on):
         """True / 1: time every kNN+Jacobian launch; N > 1: every N-th scan-to-map call; False / 0: off."""
         self._check(lib().liliom_set_kernel_timing(self._h, int(on)))
+
+
+def _batch_args(ctxs, poses7, match_cnt, want_stats):
+    B = len(ctxs)
+    handles = (C.c_void_p * max(B, 1))(*[c._h if c is not None else None for c in ctxs])
+    poses = np.array(poses7, dtype=np.float64).reshape(B, 7) if B else np.zeros((1, 7))
+    st = (IterStats * max(B * match_cnt, 1))() if want_stats else None
+    status = np.zeros(max(B, 1), np.int32)
+    return B, handles, poses, st, status
+
+
+def _batch_stats(st, B, match_cnt):
+    return [[st[i * match_cnt + k] for k in range(match_cnt)] for i in range(B)] if st is not None else None
+
+
+def scan_to_map_resident_batch(ctxs, poses7, match_cnt: int, want_stats: bool = False):
+    """One GN step of every context in `ctxs` on its resident features (liliom_scan_to_map_resident_batch): session i gets what
+    ctxs[i].scan_to_map_resident(poses7[i], match_cnt, mode=MODE_GN) would give it.  Returns (poses (B, 7), status (B,),
+    per-session stats lists or None); a session's own error is its status, a whole-call error raises LiliomError."""
+    B, handles, poses, st, status = _batch_args(ctxs, poses7, match_cnt, want_stats)
+    rc = lib().liliom_scan_to_map_resident_batch(handles, B, _dptr(poses), match_cnt, st, status.ctypes.data_as(C.POINTER(C.c_int)))
+    if rc != OK:
+        raise LiliomError(rc)
+    return poses[:B], status[:B], _batch_stats(st, B, match_cnt)
+
+
+def odometry_resident_batch(ctxs, poses7, match_cnt: int, want_stats: bool = False, want_ds: bool = False, caps=None):
+    """liliom_odometry_resident_batch: VoxelGrid of each context's resident surf features, then one batched GN step.
+    caps: per-session DS capacity in points (default 65536 each).
+    Returns (poses (B, 7), status (B,), stats or None, per-session DS clouds (want_ds) or their sizes)."""
+    B, handles, poses, st, status = _batch_args(ctxs, poses7, match_cnt, want_stats)
+    caps = [int(x) for x in caps] if caps is not None else [65536] * B
+    bufs = [np.zeros(max(caps[i], 1), ctxs[i].dtype) for i in range(B)] if want_ds else None
+    outs = (C.c_void_p * max(B, 1))(*[b.ctypes.data for b in bufs]) if want_ds else None
+    cap_arr = np.array(caps + [0], np.int32)
+    nds = np.zeros(max(B, 1), np.int32)
+    ip = C.POINTER(C.c_int)
+    rc = lib().liliom_odometry_resident_batch(handles, B, _dptr(poses), match_cnt, st, outs, cap_arr.ctypes.data_as(ip), nds.ctypes.data_as(ip),
+                                             status.ctypes.data_as(ip))
+    if rc != OK:
+        raise LiliomError(rc)
+    ds = [bufs[i][:nds[i]] for i in range(B)] if want_ds else nds[:B].copy()
+    return poses[:B], status[:B], _batch_stats(st, B, match_cnt), ds
 
 
 def comm_get_unique_id() -> bytes:

@@ -107,6 +107,7 @@ extern "C" int liliom_create(liliom_ctx** out, const liliom_params* p, int devic
     if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_ready, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_copied, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->ev_batch, cudaEventDisableTiming);
     c->h_pin_bytes = sizeof(PinBlock) + (1 << 20);      // the header + 1 MiB of per-iteration stats (3276 iterations)
     if (e == cudaSuccess) e = cudaHostAlloc((void**)&c->h_pin, c->h_pin_bytes, cudaHostAllocDefault);
     if (e != cudaSuccess) { liliom_destroy(c); return LILIOM_E_CUDA; }      // tears down whatever was created
@@ -136,6 +137,7 @@ extern "C" void liliom_destroy(liliom_ctx* c) {
     if (c->h_pin) cudaFreeHost(c->h_pin);
     if (c->ev_ready) cudaEventDestroy(c->ev_ready);
     if (c->ev_copied) cudaEventDestroy(c->ev_copied);
+    if (c->ev_batch) cudaEventDestroy(c->ev_batch);
     if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
     if (c->own_stream) cudaStreamDestroy(c->own_stream);
     delete c;      // the device buffers (DevBuf members, frames, indices) free themselves here, with the device still current
@@ -511,10 +513,10 @@ extern "C" int liliom_extract_resident(liliom_ctx* c, const double q_imu[4], con
     return rc;
 }
 
-static int odometry_on_resident_surf(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int mode, liliom_iter_stats* stats,
-                                     void* ds_out, int ds_cap, int* n_ds, bool spec_failed) {
-    if (!c || !pose7 || (mode != LILIOM_MODE_CERES && mode != LILIOM_MODE_GN) || match_cnt < 0) return LILIOM_E_ARG;
-    LILI_CUDA(c, cudaSetDevice(c->device));
+// liliom_odometry_resident in three parts, shared by the solo and the batched call.
+// 1. The scan VoxelGrid of the resident surf features into the queries.  *step: LILIOM_OK when the step may run, or the map's
+//    refusal (LILIOM_E_NOMAP / LILIOM_E_FEWMAP).
+static int odo_filter(liliom_ctx* c, bool spec_failed, int* step) {
     const int stride = c->prm.point_stride;
     // surf count: exact on the host (n_surf_dev >= 0) or only on the device (resident pipeline, no round trip)
     const int n_max = c->n_surf_dev >= 0 ? c->n_surf_dev : c->n_surf_max;
@@ -543,27 +545,28 @@ static int odometry_on_resident_surf(liliom_ctx* c, double pose7[7], int match_c
         c->d_nfeats = d_n;
     }
     c->n_feats = n_max;
-    int rc = LILIOM_OK;
-    if (!c->map.ready) rc = LILIOM_E_NOMAP;
-    else if (c->map_n_global < 10) rc = LILIOM_E_FEWMAP;
-    double pose_in[7];
-    memcpy(pose_in, pose7, sizeof(pose_in));
-    if (rc == LILIOM_OK) {
-        rc = s2m_run(c, pose7, match_cnt, max_num_iter, mode, stats, false, nullptr);
-        if (rc == LILIOM_OK && c->vg_check && !spec_failed &&
-            (c->vg_bail || (c->vg_used24 && c->vg_ncells >= (1LL << 24) - 1))) {   // speculation missed: redo with the sort chain, 32-bit keys
-            c->vg_check = false;
-            c->d_nfeats = nullptr;
-            memcpy(pose7, pose_in, sizeof(pose_in));
-            return odometry_on_resident_surf(c, pose7, match_cnt, max_num_iter, mode, stats, ds_out, ds_cap, n_ds, true);
-        }
-        c->vg_check = false;
-    } else {   // still report surf_last_ds: read the count back
+    *step = !c->map.ready ? LILIOM_E_NOMAP : c->map_n_global < 10 ? LILIOM_E_FEWMAP : LILIOM_OK;
+    return LILIOM_OK;
+}
+
+// 2. After a step that ran and returned rc: true when the VoxelGrid's speculation missed, and the call must be redone from its
+//    start pose with the sort chain and 32-bit keys (spec_failed).  Clears the check either way.
+static bool odo_spec_missed(liliom_ctx* c, int rc, bool spec_failed) {
+    const bool miss = rc == LILIOM_OK && c->vg_check && !spec_failed &&
+                      (c->vg_bail || (c->vg_used24 && c->vg_ncells >= (1LL << 24) - 1));
+    c->vg_check = false;
+    if (miss) c->d_nfeats = nullptr;
+    return miss;
+}
+
+// 3. The query count of a step that did not run (ran = false), and surf_last_ds: *n_ds and the optional download.
+static int odo_finish(liliom_ctx* c, bool ran, int rc, void* ds_out, int ds_cap, int* n_ds) {
+    if (!ran) {   // still report surf_last_ds: read the count back
         if (c->d_nfeats) {
             int nq = 0;
             LILI_TRY(read_back(c, {{&nq, c->d_nfeats, sizeof(int)}}));
-            c->n_feats_actual = min(nq, n_max);
-        } else c->n_feats_actual = n_max;
+            c->n_feats_actual = min(nq, c->n_feats);
+        } else c->n_feats_actual = c->n_feats;
     }
     c->d_nfeats = nullptr;
     const int m = c->n_feats_actual;
@@ -571,16 +574,85 @@ static int odometry_on_resident_surf(liliom_ctx* c, double pose7[7], int match_c
     if (ds_out) {
         if (m > ds_cap) return LILIOM_E_CAPACITY;
         if (m) {
-            LILI_CUDA(c, cudaMemcpyAsync(ds_out, c->vg_out.p, (size_t)m * stride, cudaMemcpyDeviceToHost, c->stream));
+            LILI_CUDA(c, cudaMemcpyAsync(ds_out, c->vg_out.p, (size_t)m * c->prm.point_stride, cudaMemcpyDeviceToHost, c->stream));
             LILI_CUDA(c, cudaStreamSynchronize(c->stream));
         }
     }
     return rc;
 }
 
+static int odometry_on_resident_surf(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int mode, liliom_iter_stats* stats,
+                                     void* ds_out, int ds_cap, int* n_ds, bool spec_failed) {
+    if (!c || !pose7 || (mode != LILIOM_MODE_CERES && mode != LILIOM_MODE_GN) || match_cnt < 0) return LILIOM_E_ARG;
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    int rc = LILIOM_OK;
+    LILI_TRY(odo_filter(c, spec_failed, &rc));
+    const bool ran = rc == LILIOM_OK;
+    double pose_in[7];
+    memcpy(pose_in, pose7, sizeof(pose_in));
+    if (ran) {
+        rc = s2m_run(c, pose7, match_cnt, max_num_iter, mode, stats, false, nullptr);
+        if (odo_spec_missed(c, rc, spec_failed)) {
+            memcpy(pose7, pose_in, sizeof(pose_in));
+            return odometry_on_resident_surf(c, pose7, match_cnt, max_num_iter, mode, stats, ds_out, ds_cap, n_ds, true);
+        }
+    }
+    return odo_finish(c, ran, rc, ds_out, ds_cap, n_ds);
+}
+
 extern "C" int liliom_odometry_resident(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int mode, liliom_iter_stats* stats,
                                         void* ds_out, int ds_cap, int* n_ds) {
     return odometry_on_resident_surf(c, pose7, match_cnt, max_num_iter, mode, stats, ds_out, ds_cap, n_ds);
+}
+
+// The whole-call refusals of the batched steps: nothing is touched when one holds.
+static bool batch_args_ok(liliom_ctx* const* ctxs, int B, const double* poses7, int match_cnt, const int* status) {
+    if (B < 1 || !ctxs || !poses7 || !status || match_cnt < 0) return false;
+    for (int i = 0; i < B; ++i) {
+        const liliom_ctx* c = ctxs[i];
+        if (!c || c->device != ctxs[0]->device || c->nranks > 1 || c->nccl_comm || c->peer_ready) return false;
+        for (int j = 0; j < i; ++j) if (ctxs[j] == c) return false;
+    }
+    return true;
+}
+
+extern "C" int liliom_scan_to_map_resident_batch(liliom_ctx* const* ctxs, int B, double* poses7_inout, int match_cnt,
+                                                 liliom_iter_stats* stats, int* status) {
+    if (!batch_args_ok(ctxs, B, poses7_inout, match_cnt, status)) return LILIOM_E_ARG;
+    LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
+    for (int i = 0; i < B; ++i) status[i] = LILIOM_OK;
+    return s2m_batch(ctxs, B, poses7_inout, match_cnt, stats, status);
+}
+
+extern "C" int liliom_odometry_resident_batch(liliom_ctx* const* ctxs, int B, double* poses7_inout, int match_cnt,
+                                              liliom_iter_stats* stats, void* const* ds_out, const int* ds_cap, int* n_ds, int* status) {
+    if (!batch_args_ok(ctxs, B, poses7_inout, match_cnt, status)) return LILIOM_E_ARG;
+    LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
+    std::vector<int> step(B, LILIOM_OK);
+    std::vector<char> filtered(B, 0);
+    for (int i = 0; i < B; ++i) {
+        status[i] = odo_filter(ctxs[i], false, &step[i]);
+        filtered[i] = status[i] == LILIOM_OK;
+        if (!filtered[i]) step[i] = status[i];
+    }
+    const std::vector<double> pose_in(poses7_inout, poses7_inout + (size_t)7 * B);
+    std::vector<int> ran(step);
+    LILI_TRY(s2m_batch(ctxs, B, poses7_inout, match_cnt, stats, step.data()));
+    for (int i = 0; i < B; ++i) {
+        if (!filtered[i]) continue;
+        liliom_ctx* c = ctxs[i];
+        double* pose = poses7_inout + 7 * i;
+        liliom_iter_stats* st = stats ? stats + (size_t)i * match_cnt : nullptr;
+        void* out = ds_out ? ds_out[i] : nullptr;
+        const int cap = ds_cap ? ds_cap[i] : 0;
+        int* nd = n_ds ? n_ds + i : nullptr;
+        const bool did_run = ran[i] == LILIOM_OK;
+        if (did_run && odo_spec_missed(c, step[i], false)) {
+            memcpy(pose, pose_in.data() + 7 * i, 7 * sizeof(double));
+            status[i] = odometry_on_resident_surf(c, pose, match_cnt, 0, LILIOM_MODE_GN, st, out, cap, nd, true);
+        } else status[i] = odo_finish(c, did_run, step[i], out, cap, nd);
+    }
+    return LILIOM_OK;
 }
 
 extern "C" int liliom_find_surf_corr(liliom_ctx* c, const void* feats, int n, int stride, const double pose7[7], unsigned char* valid,

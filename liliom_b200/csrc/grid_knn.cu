@@ -171,6 +171,21 @@ struct KnnArgs {
     unsigned long long* queries_total;  // instrumentation: queries processed (device-side count), one add per pass
 };
 
+// One session of a batched persistent launch (k_gn_batch): what k_gn_persistent takes as parameters, per session.
+struct GnBatchEntry {
+    KnnArgs a;
+    unsigned int* bar;                  // the session's own grid-barrier word
+    double* stats_base;
+    unsigned int bar_base;              // arrivals of the session's earlier launches
+    GnIo io;
+};
+struct GnBatch {
+    int n, iters, sync_mode;            // sessions in this launch; GN iterations and LILIOM_GN_SYNC shared by all of them
+    int off[kBatchMax + 1];             // session s owns blocks [off[s], off[s + 1])
+    GnBatchEntry s[kBatchMax];
+};
+static_assert(sizeof(GnBatch) <= 32764, "k_gn_batch's session table must fit in the kernel parameter space");
+
 // What only the per-pass kernel (k_knn_plane) reads.
 struct PassArgs {
     unsigned int* ticket;               // last-block ticket
@@ -182,8 +197,21 @@ struct PassArgs {
 // Small scans (8 or 16 lanes per query) deal tasks to warps block-cyclically: queries arrive in voxel order (spatially sorted),
 // and dealing neighbouring tasks to different blocks evens out the per-block work (dense vs sparse regions) at the grid barrier;
 // large scans keep neighbours together for L1 reuse.
-template <int LANES> __device__ __forceinline__ int first_task(int warp) {
-    return LANES >= 8 ? warp * (int)gridDim.x + (int)blockIdx.x : (int)blockIdx.x * kWarps + warp; }
+// Where a block sits in its session: blk.bi() of blk.G() blocks.  A solo launch reads blockIdx.x / gridDim.x at each use
+// (the kernels keep the code and registers they had before the batched launch existed); a batched launch (k_gn_batch) passes
+// the block's place inside its session's range.
+struct SoloBlock {
+    __device__ __forceinline__ int bi() const { return (int)blockIdx.x; }
+    __device__ __forceinline__ unsigned int G() const { return gridDim.x; }
+};
+struct SessionBlock {
+    int b; unsigned int g;
+    __device__ __forceinline__ int bi() const { return b; }
+    __device__ __forceinline__ unsigned int G() const { return g; }
+};
+
+template <int LANES> __device__ __forceinline__ int first_task(int warp, int bi, int G) {
+    return LANES >= 8 ? warp * G + bi : bi * kWarps + warp; }
 
 // per-thread instrumentation word: examined candidates in the low 40 bits, searched queries above (summed per block)
 constexpr int kCandBits = 40;
@@ -218,15 +246,15 @@ struct KnnSmem {
     int peer_lost;               // fused exchange: a peer did not publish within the wait bound -> the pose is poisoned (NaN), the host reports it
 };
 
-#define LILI_STAMP(i) do { if (a.dbg && blockIdx.x == 0 && threadIdx.x == 0) a.dbg[i] = clock64(); } while (0)
+#define LILI_STAMP(i) do { if (a.dbg && blk.bi() == 0 && threadIdx.x == 0) a.dbg[i] = clock64(); } while (0)
 #define LILI_STAMP_LAST(i) do { if (a.dbg && threadIdx.x == 0) a.dbg[i] = clock64(); } while (0)
 
 // One pass over this block's share of the queries at pose (q,t): phases A (search), B (fit + row), C (lane k
 // accumulates scalar k).  On return lane k < 29 of every warp holds its partial of scalar k in `acc`.
-template <int LANES, bool TMA = false>
+template <int LANES, bool TMA = false, class Blk = SoloBlock>
 __device__ __forceinline__ void knn_phases(const KnnArgs& a, const Q4& q, const D3& t, const int n_q, KnnSmem& S,
-                                           double& acc, unsigned long long& cand, const bool use_state, const float4* fpre = nullptr,
-                                           unsigned* stage_phase = nullptr) {
+                                           double& acc, unsigned long long& cand, const bool use_state, const Blk blk,
+                                           const float4* fpre = nullptr, unsigned* stage_phase = nullptr) {
     constexpr int GROUPS = 32 / LANES;                 // queries a warp searches concurrently
     extern __shared__ __align__(16) unsigned char dyn_smem[];      // LANES == 1: [kRunCap][kBlock] int4 run lists (thread_knn5)
     int4* runs = reinterpret_cast<int4*>(dyn_smem) + threadIdx.x;
@@ -242,8 +270,8 @@ __device__ __forceinline__ void knn_phases(const KnnArgs& a, const Q4& q, const 
 
     const int per_task = GROUPS * a.rounds;            // <= 32
     const int ntasks = (n_q + per_task - 1) / per_task;
-    const int gw = first_task<LANES>(warp);
-    const int nw = gridDim.x * kWarps;
+    const int gw = first_task<LANES>(warp, blk.bi(), (int)blk.G());
+    const int nw = blk.G() * kWarps;
 
 #pragma unroll 1
     for (int task = gw; task < ntasks; task += nw) {
@@ -270,7 +298,7 @@ __device__ __forceinline__ void knn_phases(const KnnArgs& a, const Q4& q, const 
             if (live) {
                 if (sub == 0) cand += 1ull << kCandBits;
                 if constexpr (LANES == 1) thread_knn5(sx, sy, sz, a.map, a.cell_start, a.g, tau_q, runs, kBlock, top, cand);
-                else group_knn5<LANES>(sx, sy, sz, a.map, a.cell_start, a.g, sub, gmask, tau_q, top, cand, (a.dbg && blockIdx.x == 0 && threadIdx.x == 0) ? a.dbg : nullptr,
+                else group_knn5<LANES>(sx, sy, sz, a.map, a.cell_start, a.g, sub, gmask, tau_q, top, cand, (a.dbg && blk.bi() == 0 && threadIdx.x == 0) ? a.dbg : nullptr,
                                        stage, stage_phase);
             }
             LILI_STAMP(11);
@@ -348,7 +376,8 @@ __device__ __forceinline__ void knn_phases(const KnnArgs& a, const Q4& q, const 
 }
 
 // Block partial -> partials[29][G] (scalar-major) + candidate counter.
-__device__ __forceinline__ void write_block_partials(const KnnArgs& a, KnnSmem& S, double acc, unsigned long long cand) {
+template <class Blk>
+__device__ __forceinline__ void write_block_partials(const KnnArgs& a, KnnSmem& S, double acc, unsigned long long cand, const Blk blk) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (lane < kNormEq) S.red[warp][lane] = acc;
     {
@@ -358,12 +387,12 @@ __device__ __forceinline__ void write_block_partials(const KnnArgs& a, KnnSmem& 
         if (lane == 0) S.red_cand[warp] = v;
     }
     __syncthreads();
-    const int G = gridDim.x;
+    const int G = blk.G();
     if (threadIdx.x < kNormEq) {
         double v = 0;
 #pragma unroll
         for (int w = 0; w < kWarps; ++w) v += S.red[w][threadIdx.x];
-        a.partials[(size_t)threadIdx.x * G + blockIdx.x] = v;          // scalar-major: [29][G]
+        a.partials[(size_t)threadIdx.x * G + (unsigned int)blk.bi()] = v;          // scalar-major: [29][G]
     }
     if (threadIdx.x == 0 && a.cand_total) {     // instrumentation (liliom_set_kernel_timing): examined candidates | searched queries
         unsigned long long v = 0;
@@ -377,8 +406,9 @@ __device__ __forceinline__ void write_block_partials(const KnnArgs& a, KnnSmem& 
 // every load of a lane is issued before the first add: ONE L2 round trip for up to 8*kRedLoads = 160 blocks (the
 // persistent kernel never has more than one block per SM); larger grids take another trip per 160 blocks.
 constexpr int kRedLoads = 20;
-__device__ __forceinline__ void reduce_partials(const KnnArgs& a, KnnSmem& S) {
-    const int G = gridDim.x;
+template <class Blk>
+__device__ __forceinline__ void reduce_partials(const KnnArgs& a, KnnSmem& S, const Blk blk) {
+    const int G = blk.G();
     const int sc = threadIdx.x >> 3, l8 = threadIdx.x & 7;
     double v = 0.0;
     if (sc < kNormEq) {
@@ -523,6 +553,7 @@ __device__ __forceinline__ void write_neq_stats(const KnnArgs& a, const KnnSmem&
 template <int LANES>
 __global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) k_knn_plane(KnnArgs a, PassArgs p, const __grid_constant__ PeerArgs pa) {
     __shared__ __align__(16) KnnSmem S;
+    const SoloBlock blk;
     if (threadIdx.x == 0) S.peer_lost = 0;
     LILI_STAMP(0);
     const Q4 q{a.pose[0], a.pose[1], a.pose[2], a.pose[3]};
@@ -530,9 +561,9 @@ __global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) 
     const int n_q = a.n_dev ? min(*a.n_dev, a.n) : a.n;
     double acc = 0.0;
     unsigned long long cand = 0;
-    knn_phases<LANES>(a, q, t, n_q, S, acc, cand, p.use_state != 0);
+    knn_phases<LANES>(a, q, t, n_q, S, acc, cand, p.use_state != 0, blk);
     LILI_STAMP(3);
-    write_block_partials(a, S, acc, cand);
+    write_block_partials(a, S, acc, cand, blk);
     __threadfence();
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -545,7 +576,7 @@ __global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) 
     __threadfence();
     LILI_STAMP_LAST(5);
     // ---------------- last block: fixed-order sum over blocks, then the 6x6 step
-    reduce_partials(a, S);
+    reduce_partials(a, S, blk);
     if (pa.enabled) peer_exchange(pa, pa.epoch0, S, true);      // multi-GPU, one launch per iteration: the last block trades sums with the peers
     LILI_STAMP_LAST(6);
     if (threadIdx.x == 0) {
@@ -576,9 +607,11 @@ __global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) 
 #define LILI_GN_MAXNREG 176
 #endif
 #define LILI_GN_BOUNDS __maxnreg__(LILI_GN_MAXNREG)
-template <int LANES, bool TMA = false>
-__global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned int* bar, double* stats_base, unsigned int bar_base,
-                                                             int sync_mode, const __grid_constant__ PeerArgs pa, const __grid_constant__ GnIo io) {
+// The persistent kernel's body for one session.  Everything a session shares with other blocks goes through its own KnnArgs
+// buffers, `bar` and io, so sessions of one batched launch never wait for one another.
+template <int LANES, bool TMA, class Blk>
+__device__ __forceinline__ void gn_persistent_body(KnnArgs a, int iters, unsigned int* bar, double* stats_base, unsigned int bar_base,
+                                                   int sync_mode, const PeerArgs& pa, const GnIo& io, const Blk blk) {
     __shared__ __align__(16) KnnSmem S;
     unsigned stage_phase = 0;
     if constexpr (TMA) {       // one mbarrier per lane group, 16 arrivals (every lane of the group, with or without a run to stage)
@@ -590,9 +623,8 @@ __global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned in
     const int n_q = a.n_dev ? min(*a.n_dev, a.n) : a.n;
     if (threadIdx.x == 32) S.peer_lost = 0;
     if (threadIdx.x < 7) S.pose[threadIdx.x] = io.pose0[threadIdx.x];
-    if (a.dbg && blockIdx.x == 0 && threadIdx.x == 0) a.dbg[30] = (long long)globaltimer_ns();
+    if (a.dbg && blk.bi() == 0 && threadIdx.x == 0) a.dbg[30] = (long long)globaltimer_ns();
     __syncthreads();
-    const unsigned int G = gridDim.x;
     // bar_base = arrivals of all previous launches on this context (tracked by the host, advanced by iters*G per launch)
     // one task per warp and one round per task (the small-scan shape): each lane group serves the same
     // query in every iteration, so its body-frame point is loaded once and kept in registers
@@ -602,8 +634,8 @@ __global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned in
         constexpr int GROUPS = 32 / LANES;
         const int per_task = GROUPS * a.rounds;
         const int ntasks = (n_q + per_task - 1) / per_task;
-        const int gw = first_task<LANES>(threadIdx.x >> 5);
-        const int nw = gridDim.x * kWarps;
+        const int gw = first_task<LANES>(threadIdx.x >> 5, blk.bi(), (int)blk.G());
+        const int nw = blk.G() * kWarps;
         if (a.rounds == 1 && ntasks <= nw) {
             keep = true;
             const int qi = gw * per_task + ((threadIdx.x & 31) / LANES);
@@ -616,9 +648,9 @@ __global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned in
         const D3 t{S.pose[4], S.pose[5], S.pose[6]};
         double acc = 0.0;
         unsigned long long cand = 0;
-        const bool stamp = a.dbg && blockIdx.x == 0 && threadIdx.x == 0 && it == 2;
+        const bool stamp = a.dbg && blk.bi() == 0 && threadIdx.x == 0 && it == 2;
         if (stamp) a.dbg[16] = clock64();
-        knn_phases<LANES, TMA>(a, q, t, n_q, S, acc, cand, it > 0, keep ? &f_keep : nullptr, &stage_phase);
+        knn_phases<LANES, TMA>(a, q, t, n_q, S, acc, cand, it > 0, blk, keep ? &f_keep : nullptr, &stage_phase);
         if (stamp) a.dbg[17] = clock64();
         // ---- grid barrier + cross-block sum.  Mode 3 (default; measured 12.70 -> 11.99 us per pass against mode 0): one release by
         // thread 0 after the block barrier (cumulative over bar.sync, as in cooperative groups' grid.sync; SASS: MEMBAR.ALL.GPU +
@@ -629,16 +661,16 @@ __global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned in
         // sides; tests pin all three to the same bits (test_gpu_variants.py, test_persistent_barrier_stress_all_sync_modes).
         // Multi-GPU (fused exchange): the other blocks of this GPU arrive but do not wait here — they wait for block 0's
         // republished sums over all ranks.
-        const bool follower = pa.enabled && blockIdx.x != 0;
-        write_block_partials(a, S, acc, cand);
+        const bool follower = pa.enabled && blk.bi() != 0;
+        write_block_partials(a, S, acc, cand, blk);
         if (sync_mode == 0) __threadfence();
         __syncthreads();
         if (stamp) a.dbg[18] = clock64();
-        if (threadIdx.x == 0) grid_barrier(bar, bar_base + (unsigned int)(it + 1) * G, sync_mode, !follower);
+        if (threadIdx.x == 0) grid_barrier(bar, bar_base + (unsigned int)(it + 1) * blk.G(), sync_mode, !follower);
         if (!follower) {
             __syncthreads();
             if (stamp) a.dbg[19] = clock64();
-            reduce_partials(a, S);
+            reduce_partials(a, S, blk);
             if (pa.enabled) {       // block 0: this rank's sums -> sums over all ranks, then on to the other blocks
                 peer_exchange(pa, pa.epoch0 + (unsigned int)it, S, true);
                 peer_local_publish(pa, pa.epoch0 + (unsigned int)it, S);
@@ -652,15 +684,15 @@ __global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned in
             if (stamp) a.dbg[21] = clock64();
 #pragma unroll
             for (int k = 0; k < 7; ++k) S.pose[k] = xn[k];
-            if (blockIdx.x == 0) {
+            if (blk.bi() == 0) {
 #pragma unroll
                 for (int k = 0; k < 7; ++k) a.pose_out[k] = xn[k];
                 if (pa.enabled) a.pose_out[7] = S.peer_lost ? 1.0 : 0.0;      // explicit loss flag for the host (the pose is NaN as well)
                 if (stats) write_stats(stats, kNormEq, nullptr, 1.0, xn);
             }
         }
-        if (blockIdx.x == 0) write_neq_stats(a, S, stats);
-        if (blockIdx.x == 0 && it == iters - 1 && io.host_out) {      // results straight into the host's pinned block
+        if (blk.bi() == 0) write_neq_stats(a, S, stats);
+        if (blk.bi() == 0 && it == iters - 1 && io.host_out) {      // results straight into the host's pinned block
             if (threadIdx.x == 0) {
 #pragma unroll
                 for (int k = 0; k < 7; ++k) io.host_out->pose[k] = S.pose[k];
@@ -673,9 +705,29 @@ __global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned in
         __syncthreads();
         // the partials of this iteration may only be overwritten after every block has summed them: the next
         // barrier is behind the next write, so alternate between two partial buffers
-        a.partials = (it & 1) ? a.partials - (size_t)kNormEq * G : a.partials + (size_t)kNormEq * G;
+        a.partials = (it & 1) ? a.partials - (size_t)kNormEq * blk.G() : a.partials + (size_t)kNormEq * blk.G();
     }
-    if (a.dbg && blockIdx.x == 0 && threadIdx.x == 0) a.dbg[31] = (long long)globaltimer_ns();
+    if (a.dbg && blk.bi() == 0 && threadIdx.x == 0) a.dbg[31] = (long long)globaltimer_ns();
+}
+
+template <int LANES, bool TMA = false>
+__global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned int* bar, double* stats_base, unsigned int bar_base,
+                                                             int sync_mode, const __grid_constant__ PeerArgs pa, const __grid_constant__ GnIo io) {
+    gn_persistent_body<LANES, TMA>(a, iters, bar, stats_base, bar_base, sync_mode, pa, io, SoloBlock{});
+}
+
+// Several sessions' persistent GN steps in one cooperative launch (liliom_scan_to_map_resident_batch).  Session s owns blocks
+// [off[s], off[s+1]) and runs exactly the body its solo launch would, with its own barrier word, partials and pinned block;
+// the cooperative launch only guarantees that all blocks are resident.  Every session of a launch has the same instantiation
+// (lanes, staging) and the same iteration count; the fused exchange is never attached (communicator contexts are refused).
+template <int LANES, bool TMA = false>
+__global__ void LILI_GN_BOUNDS k_gn_batch(const __grid_constant__ GnBatch tab) {
+    int s = 0;
+    while (s + 1 < tab.n && (int)blockIdx.x >= tab.off[s + 1]) ++s;
+    const GnBatchEntry& e = tab.s[s];
+    const PeerArgs pa{};
+    gn_persistent_body<LANES, TMA>(e.a, tab.iters, e.bar, e.stats_base, e.bar_base, tab.sync_mode, pa, e.io,
+                                   SessionBlock{(int)blockIdx.x - tab.off[s], (unsigned int)(tab.off[s + 1] - tab.off[s])});
 }
 
 // GN step for the multi-GPU path: runs after the all-reduce of neq[29], identically on every rank.
@@ -1020,82 +1072,56 @@ static void print_debug_timing(liliom_ctx* c, const long long* dbg, bool persist
                 h[1] - h[0], h[2] - h[1], h[3] - h[2], 0LL, h[4] - h[3], h[6] - h[5], h[7] - h[6], h[7] - h[0]);
 }
 
-int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int mode, liliom_iter_stats* stats,
-            bool want_corr, double out29[29]) {
+// One scan-to-map call between its checks and its results: the plan, the kernel arguments and, for a persistent plan, the rest
+// of k_gn_persistent's parameters.  s2m_begin enqueues the call's set-up on the context's stream and s2m_finish its read-back;
+// s2m_run launches in between, s2m_batch packs several contexts' persistent launches into k_gn_batch.
+struct S2mCall {
+    S2mPlan p;
+    KnnArgs a;
+    int iters;
+    bool timed, peer, host_io;
+    unsigned int* bar; double* stats_base; unsigned int bar_base; PeerArgs pa; GnIo io;    // persistent plans
+};
+
+static int s2m_begin(liliom_ctx* c, const double pose7[7], int match_cnt, int mode, bool want_stats, bool want_corr, S2mCall& k) {
     if (!c->map.ready) return LILIOM_E_NOMAP;
     if (c->map_n_global < 10) return LILIOM_E_FEWMAP;          // L/src/LidarOdometry.cpp:485-488
     const int n = c->n_feats, iters = match_cnt;
     if (iters < 0) return LILIOM_E_ARG;
     // the per-iteration stats come back through the pinned block: check its capacity before anything is enqueued
-    if (stats && iters > 0 && offsetof(PinBlock, stats) + (size_t)iters * kStatsDoubles * sizeof(double) > c->h_pin_bytes) return LILIOM_E_CAPACITY;
+    if (want_stats && iters > 0 && offsetof(PinBlock, stats) + (size_t)iters * kStatsDoubles * sizeof(double) > c->h_pin_bytes) return LILIOM_E_CAPACITY;
+    k.iters = iters;
     // kernel timing (liliom_set_kernel_timing): an event pair + the device-side query/candidate counts on every time_every-th call
-    const bool timed = c->time_kernels && (c->time_calls++ % (unsigned)c->time_every) == 0;
-    const bool peer = c->peer_ready && c->peer_ptrs[c->rank] != nullptr;       // fused exchange instead of ncclAllReduce + k_gn_update
-    const S2mPlan p = s2m_plan({n, c->last_n_feats, c->d_nfeats != nullptr, c->sm_count, mode, iters, want_corr, c->nranks, peer,
-                                c->force_lanes, c->force_rounds, c->knn_tma});
-    KnnArgs a;
-    LILI_TRY(s2m_prepare(c, p, iters, mode, want_corr, timed, a));
+    k.timed = c->time_kernels && (c->time_calls++ % (unsigned)c->time_every) == 0;
+    k.peer = c->peer_ready && c->peer_ptrs[c->rank] != nullptr;       // fused exchange instead of ncclAllReduce + k_gn_update
+    k.p = s2m_plan({n, c->last_n_feats, c->d_nfeats != nullptr, c->sm_count, mode, iters, want_corr, c->nranks, k.peer,
+                    c->force_lanes, c->force_rounds, c->knn_tma});
+    LILI_TRY(s2m_prepare(c, k.p, iters, mode, want_corr, k.timed, k.a));
     // zero-copy results (GnIo): the persistent kernel leaves pose, query count and VoxelGrid parameters in the pinned block
     // itself when the device can address it; only per-iteration stats / the 29 sums still travel by copy
-    const bool host_io = p.persistent && c->h_pin_dev != nullptr;
-    if (p.persistent) {         // all iterations in one cooperative launch, the start pose as a kernel parameter
-        int iters_arg = iters, sync_mode = c->gn_sync;
-        unsigned int* bar = reinterpret_cast<unsigned int*>(c->counter.as<unsigned char>() + 32);
-        double* stats_base = c->stats_dev.as<double>();
-        unsigned int bar_base = c->bar_arrivals;
-        PeerArgs pa{};
-        if (peer) { pa = peer_args(c, c->peer_epoch + 1u); c->peer_epoch += (unsigned int)iters; }   // same calls on every rank: same epochs
-        GnIo io{};
-        memcpy(io.pose0, pose7, 7 * sizeof(double));
-        io.host_out = host_io ? &c->h_pin_dev->s2m : nullptr;
-        io.vgp = host_io && c->vg_check ? c->vg_params.as<int>() : nullptr;
-        void* kargs[] = {&a, &iters_arg, &bar, &stats_base, &bar_base, &sync_mode, &pa, &io};
-        LILI_TRY(timed_launch(c, timed, iters, [&] {
-            LILI_CUDA(c, cudaLaunchCooperativeKernel(gn_kernel(p.lanes, p.tma), dim3(p.grid), dim3(kBlock), kargs, p.dyn_smem, c->stream));
-            return launch_check(c, "k_gn_persistent");
-        }));
-        c->bar_arrivals += (unsigned int)iters * (unsigned int)p.grid;
-    } else {                    // one launch per iteration; the start pose goes through the pinned block to pose_dev
-        double* pin = c->h_pin->pose_stage;
-        memcpy(pin, pose7, 7 * sizeof(double)); pin[7] = 0.0;          // + cleared peer-loss flag
-        LILI_CUDA(c, cudaMemcpyAsync(c->pose_dev.p, pin, 8 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
-        const bool multi = c->nranks > 1;
-        // fused exchange, one launch per iteration (large scans: grid > one block per SM): the last block trades the sums with the
-        // peers and performs the GN step itself — no ncclAllReduce, no update kernel
-        const bool peer_iter = peer && multi && mode == LILIOM_MODE_GN && iters > 0;
-        const int update_pose = (mode == LILIOM_MODE_GN && (!multi || peer_iter) && iters > 0) ? 1 : 0;
-        const int launches = (iters == 0 && want_corr) ? 1 : iters;
-        for (int it = 0; it < launches; ++it) {
-            PassArgs pass{c->counter.as<unsigned int>(), c->stats_dev.as<double>() + (size_t)it * kStatsDoubles, update_pose, it > 0 ? 1 : 0};
-            PeerArgs pit = peer_iter ? peer_args(c, ++c->peer_epoch) : PeerArgs{};
-            void* kargs[] = {&a, &pass, &pit};
-            LILI_TRY(timed_launch(c, timed, 1, [&] {
-                LILI_CUDA(c, cudaLaunchKernel(knn_kernel(p.lanes), dim3(p.grid), dim3(kBlock), kargs, p.dyn_smem, c->stream));
-                return launch_check(c, "k_knn_plane");
-            }));
-            if (iters == 0) break;
-            if (multi && !peer_iter) LILI_TRY(nccl_allreduce_sum_f64(c, c->neq.as<double>(), kNormEq));
-            if (mode == LILIOM_MODE_GN && multi && !peer_iter) {
-                k_gn_update<<<1, 32, 0, c->stream>>>(c->neq.as<double>(), c->pose_dev.as<double>(), pass.stats);
-                LILI_TRY(launch_check(c, "k_gn_update"));
-            } else if (mode != LILIOM_MODE_GN) {
-                if (multi) { c->last_error = "CERES mode is single-GPU (the LM solve is one block); use GN mode with a communicator"; return LILIOM_E_ARG; }
-                LmArgs l{};
-                l.feats = a.feats; l.valid = a.valid; l.plane = a.plane; l.n = n; l.n_dev = c->d_nfeats;
-                l.pose = c->pose_dev.as<double>(); l.stats = pass.stats; l.huber_a = a.huber_a; l.max_num_iter = max_num_iter;
-                l.neq0 = c->neq.as<double>();
-                k_lm_solve<<<1, kLmBlock, 0, c->stream>>>(l);
-                LILI_TRY(launch_check(c, "k_lm_solve"));
-            }
-        }
+    k.host_io = k.p.persistent && c->h_pin_dev != nullptr;
+    if (k.p.persistent) {       // all iterations in one cooperative launch, the start pose as a kernel parameter
+        k.bar = reinterpret_cast<unsigned int*>(c->counter.as<unsigned char>() + 32);
+        k.stats_base = c->stats_dev.as<double>();
+        k.bar_base = c->bar_arrivals;
+        k.pa = PeerArgs{};
+        if (k.peer) { k.pa = peer_args(c, c->peer_epoch + 1u); c->peer_epoch += (unsigned int)iters; }   // same calls on every rank: same epochs
+        k.io = GnIo{};
+        memcpy(k.io.pose0, pose7, 7 * sizeof(double));
+        k.io.host_out = k.host_io ? &c->h_pin_dev->s2m : nullptr;
+        k.io.vgp = k.host_io && c->vg_check ? c->vg_params.as<int>() : nullptr;
     }
-    // ---- results: pose + stats in one pinned block
+    return LILIOM_OK;
+}
+
+static int s2m_finish(liliom_ctx* c, const S2mCall& k, double pose7[7], liliom_iter_stats* stats, double out29[29]) {
+    const int n = c->n_feats, iters = k.iters;
     PinResult& r = c->h_pin->s2m;
     const bool want_stats = stats && iters > 0;
-    if (!host_io) LILI_CUDA(c, cudaMemcpyAsync(r.pose, c->pose_dev.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));     // pose + peer-loss flag
+    if (!k.host_io) LILI_CUDA(c, cudaMemcpyAsync(r.pose, c->pose_dev.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, c->stream));     // pose + peer-loss flag
     if (out29) LILI_CUDA(c, cudaMemcpyAsync(r.neq, c->neq.p, kNormEq * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
-    if (c->d_nfeats && !host_io) LILI_CUDA(c, cudaMemcpyAsync(&r.n_feats, c->d_nfeats, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-    if (c->vg_check && !host_io) LILI_CUDA(c, cudaMemcpyAsync(&r.vgp, c->vg_params.p, sizeof(VgParams), cudaMemcpyDeviceToHost, c->stream));
+    if (c->d_nfeats && !k.host_io) LILI_CUDA(c, cudaMemcpyAsync(&r.n_feats, c->d_nfeats, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    if (c->vg_check && !k.host_io) LILI_CUDA(c, cudaMemcpyAsync(&r.vgp, c->vg_params.p, sizeof(VgParams), cudaMemcpyDeviceToHost, c->stream));
     if (want_stats) LILI_CUDA(c, cudaMemcpyAsync(c->h_pin->stats, c->stats_dev.p, (size_t)iters * kStatsDoubles * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     c->n_feats_actual = c->d_nfeats ? min(r.n_feats, n) : n;
@@ -1104,26 +1130,173 @@ int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int
         c->vg_ncells = r.vgp.overflow ? 0 : (long long)r.vgp.div_b[0] * r.vgp.div_b[1] * r.vgp.div_b[2];
         c->vg_bail = r.vgp.bail != 0;
     }
-    if (iters > 0 && peer && r.pose[7] != 0.0) {
+    if (iters > 0 && k.peer && r.pose[7] != 0.0) {
         c->last_error = "fused exchange: a peer rank did not publish its sums within the wait bound (collective call not entered on every rank?)";
         return LILIOM_E_NCCL;
     }
-    if (iters > 0) for (int k = 0; k < 7; ++k) pose7[k] = r.pose[k];
-    if (out29) for (int k = 0; k < kNormEq; ++k) out29[k] = r.neq[k];
+    if (iters > 0) for (int j = 0; j < 7; ++j) pose7[j] = r.pose[j];
+    if (out29) for (int j = 0; j < kNormEq; ++j) out29[j] = r.neq[j];
     for (int it = 0; want_stats && it < iters; ++it) {
         const double* s = c->h_pin->stats + (size_t)it * kStatsDoubles;
         stats[it].n_corr = (int)s[0]; stats[it].lm_iters = (int)s[1]; stats[it].cost = s[2];
         memcpy(stats[it].jtj_jtr, s + 3, 27 * sizeof(double)); memcpy(stats[it].pose7, s + 30, 7 * sizeof(double));
     }
-    if (c->dbg_timing) print_debug_timing(c, a.dbg, p.persistent);
-    for (size_t k = 0; timed && k < c->ev_passes.size(); ++k) {        // fold finished kernel timings into the counters
+    if (c->dbg_timing) print_debug_timing(c, k.a.dbg, k.p.persistent);
+    for (size_t e = 0; k.timed && e < c->ev_passes.size(); ++e) {        // fold finished kernel timings into the counters
         float ms = 0;
-        if (cudaEventElapsedTime(&ms, c->ev_pool[2 * k], c->ev_pool[2 * k + 1]) == cudaSuccess) {
+        if (cudaEventElapsedTime(&ms, c->ev_pool[2 * e], c->ev_pool[2 * e + 1]) == cudaSuccess) {
             // a persistent launch covers `iters` passes of the kernel body: count each pass as one "launch"
-            c->cnt.knn_ms += ms; c->cnt.knn_launches += (unsigned long long)c->ev_passes[k];
+            c->cnt.knn_ms += ms; c->cnt.knn_launches += (unsigned long long)c->ev_passes[e];
         }
     }
-    if (timed) c->ev_passes.clear();
+    if (k.timed) c->ev_passes.clear();
+    return LILIOM_OK;
+}
+
+// The launches of a call that s2m_begin planned, on the context's own stream.
+static int s2m_launch(liliom_ctx* c, S2mCall& k, const double pose7[7], int max_num_iter, int mode, bool want_corr) {
+    const S2mPlan& p = k.p;
+    KnnArgs& a = k.a;
+    const int n = c->n_feats, iters = k.iters;
+    if (p.persistent) {
+        int iters_arg = iters, sync_mode = c->gn_sync;
+        void* kargs[] = {&a, &iters_arg, &k.bar, &k.stats_base, &k.bar_base, &sync_mode, &k.pa, &k.io};
+        LILI_TRY(timed_launch(c, k.timed, iters, [&] {
+            LILI_CUDA(c, cudaLaunchCooperativeKernel(gn_kernel(p.lanes, p.tma), dim3(p.grid), dim3(kBlock), kargs, p.dyn_smem, c->stream));
+            return launch_check(c, "k_gn_persistent");
+        }));
+        c->bar_arrivals += (unsigned int)iters * (unsigned int)p.grid;
+        return LILIOM_OK;
+    }
+    // one launch per iteration; the start pose goes through the pinned block to pose_dev
+    double* pin = c->h_pin->pose_stage;
+    memcpy(pin, pose7, 7 * sizeof(double)); pin[7] = 0.0;          // + cleared peer-loss flag
+    LILI_CUDA(c, cudaMemcpyAsync(c->pose_dev.p, pin, 8 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    const bool multi = c->nranks > 1;
+    // fused exchange, one launch per iteration (large scans: grid > one block per SM): the last block trades the sums with the
+    // peers and performs the GN step itself — no ncclAllReduce, no update kernel
+    const bool peer_iter = k.peer && multi && mode == LILIOM_MODE_GN && iters > 0;
+    const int update_pose = (mode == LILIOM_MODE_GN && (!multi || peer_iter) && iters > 0) ? 1 : 0;
+    const int launches = (iters == 0 && want_corr) ? 1 : iters;
+    for (int it = 0; it < launches; ++it) {
+        PassArgs pass{c->counter.as<unsigned int>(), c->stats_dev.as<double>() + (size_t)it * kStatsDoubles, update_pose, it > 0 ? 1 : 0};
+        PeerArgs pit = peer_iter ? peer_args(c, ++c->peer_epoch) : PeerArgs{};
+        void* kargs[] = {&a, &pass, &pit};
+        LILI_TRY(timed_launch(c, k.timed, 1, [&] {
+            LILI_CUDA(c, cudaLaunchKernel(knn_kernel(p.lanes), dim3(p.grid), dim3(kBlock), kargs, p.dyn_smem, c->stream));
+            return launch_check(c, "k_knn_plane");
+        }));
+        if (iters == 0) break;
+        if (multi && !peer_iter) LILI_TRY(nccl_allreduce_sum_f64(c, c->neq.as<double>(), kNormEq));
+        if (mode == LILIOM_MODE_GN && multi && !peer_iter) {
+            k_gn_update<<<1, 32, 0, c->stream>>>(c->neq.as<double>(), c->pose_dev.as<double>(), pass.stats);
+            LILI_TRY(launch_check(c, "k_gn_update"));
+        } else if (mode != LILIOM_MODE_GN) {
+            if (multi) { c->last_error = "CERES mode is single-GPU (the LM solve is one block); use GN mode with a communicator"; return LILIOM_E_ARG; }
+            LmArgs l{};
+            l.feats = a.feats; l.valid = a.valid; l.plane = a.plane; l.n = n; l.n_dev = c->d_nfeats;
+            l.pose = c->pose_dev.as<double>(); l.stats = pass.stats; l.huber_a = a.huber_a; l.max_num_iter = max_num_iter;
+            l.neq0 = c->neq.as<double>();
+            k_lm_solve<<<1, kLmBlock, 0, c->stream>>>(l);
+            LILI_TRY(launch_check(c, "k_lm_solve"));
+        }
+    }
+    return LILIOM_OK;
+}
+
+int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int mode, liliom_iter_stats* stats,
+            bool want_corr, double out29[29]) {
+    S2mCall k;
+    LILI_TRY(s2m_begin(c, pose7, match_cnt, mode, stats != nullptr, want_corr, k));
+    LILI_TRY(s2m_launch(c, k, pose7, max_num_iter, mode, want_corr));
+    return s2m_finish(c, k, pose7, stats, out29);
+}
+
+static const void* gn_batch_kernel(int kind) {
+    switch (kind) {
+        case 0: return (const void*)k_gn_batch<1>;
+        case 1: return (const void*)k_gn_batch<2>;
+        case 2: return (const void*)k_gn_batch<4>;
+        case 3: return (const void*)k_gn_batch<8>;
+        case 4: return (const void*)k_gn_batch<16>;
+        default: return (const void*)k_gn_batch<16, true>;
+    }
+}
+
+int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, int match_cnt, liliom_iter_stats* stats, int* status) {
+    liliom_ctx* c0 = cs[0];
+    const cudaStream_t s0 = c0->stream;
+    std::vector<S2mCall> k(B);
+    std::vector<S2mPlan> plans(B);
+    std::vector<int> run;                   // sessions that passed s2m_begin, in call order
+    for (int i = 0; i < B; ++i) {
+        if (status[i] != LILIOM_OK) continue;
+        liliom_iter_stats* st = stats ? stats + (size_t)i * match_cnt : nullptr;
+        status[i] = s2m_begin(cs[i], poses7 + 7 * i, match_cnt, LILIOM_MODE_GN, st != nullptr, false, k[i]);
+        if (status[i] != LILIOM_OK) continue;
+        plans[run.size()] = k[i].p;
+        run.push_back(i);
+    }
+    plans.resize(run.size());
+    int occ[kGnKinds] = {};
+    for (int kind = 0; kind < kGnKinds; ++kind) {
+        bool used = false;
+        for (int j = 0; j < (int)run.size(); ++j) used |= plans[j].persistent && s2m_kind(plans[j]) == kind;
+        if (!used) continue;
+        size_t dyn = 0;
+        for (const S2mPlan& p : plans) if (p.persistent && s2m_kind(p) == kind) dyn = p.dyn_smem;
+        if (dyn) LILI_CUDA(c0, cudaFuncSetAttribute(gn_batch_kernel(kind), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
+        LILI_CUDA(c0, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[kind], gn_batch_kernel(kind), kBlock, dyn));
+    }
+    const S2mPack pack = s2m_batch_pack(plans, occ, c0->sm_count);
+    // every other session's stream (its set-up above) is ordered before the launches on ctxs[0]'s stream
+    for (const S2mLaunch& l : pack.launches)
+        for (int j : l.sessions) {
+            liliom_ctx* c = cs[run[j]];
+            if (c->stream == s0) continue;
+            LILI_CUDA(c, cudaEventRecord(c->ev_batch, c->stream));
+            LILI_CUDA(c0, cudaStreamWaitEvent(s0, c->ev_batch, 0));
+        }
+    const bool timed0 = !run.empty() && run[0] == 0 && k[0].timed && k[0].p.persistent;     // knn_ms / knn_launches: ctxs[0] only
+    for (const S2mLaunch& l : pack.launches) {
+        GnBatch tab{};
+        tab.n = (int)l.sessions.size(); tab.iters = match_cnt; tab.sync_mode = c0->gn_sync;
+        for (int m = 0; m < tab.n; ++m) {
+            const S2mCall& ki = k[run[l.sessions[m]]];
+            tab.off[m + 1] = tab.off[m] + ki.p.grid;
+            tab.s[m] = GnBatchEntry{ki.a, ki.bar, ki.stats_base, ki.bar_base, ki.io};
+        }
+        const S2mPlan& p = plans[l.sessions[0]];
+        void* kargs[] = {&tab};
+        LILI_TRY(timed_launch(c0, timed0, match_cnt, [&]() -> int {
+            LILI_CUDA(c0, cudaLaunchCooperativeKernel(gn_batch_kernel(l.kind), dim3(l.grid), dim3(kBlock), kargs, p.dyn_smem, s0));
+            LILI_CUDA(c0, cudaGetLastError());
+            return LILIOM_OK;
+        }));
+        for (int j : l.sessions) {
+            liliom_ctx* c = cs[run[j]];
+            c->cnt.launches++;
+            c->bar_arrivals += (unsigned int)match_cnt * (unsigned int)plans[j].grid;
+        }
+    }
+    // ... and after them
+    if (!pack.launches.empty()) LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, s0));
+    for (const S2mLaunch& l : pack.launches)
+        for (int j : l.sessions) {
+            liliom_ctx* c = cs[run[j]];
+            if (c->stream != s0) LILI_CUDA(c, cudaStreamWaitEvent(c->stream, c0->ev_batch, 0));
+        }
+    // sessions whose plan is not persistent: their solo launches, on their own streams, while the batch runs
+    for (int j : pack.solo) {
+        const int i = run[j];
+        status[i] = s2m_launch(cs[i], k[i], poses7 + 7 * i, 0, LILIOM_MODE_GN, false);
+        if (status[i] == LILIOM_OK) status[i] = s2m_finish(cs[i], k[i], poses7 + 7 * i, stats ? stats + (size_t)i * match_cnt : nullptr, nullptr);
+    }
+    for (const S2mLaunch& l : pack.launches)
+        for (int j : l.sessions) {
+            const int i = run[j];
+            status[i] = s2m_finish(cs[i], k[i], poses7 + 7 * i, stats ? stats + (size_t)i * match_cnt : nullptr, nullptr);
+        }
     return LILIOM_OK;
 }
 

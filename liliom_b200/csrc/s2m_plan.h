@@ -3,6 +3,7 @@
 #pragma once
 #include <algorithm>
 #include <cstddef>
+#include <vector>
 #include "../../include/liliom.h"
 
 namespace lili {
@@ -11,6 +12,7 @@ constexpr int kBlock = 256;
 constexpr int kWarps = kBlock / 32;
 constexpr int kRunCap = 8;                    // runs per thread of the one-thread-per-query search (thread_knn5, knn_core.cuh)
 constexpr size_t kStageTileBytes = 3616;      // sizeof(StageTile), knn_core.cuh (checked there)
+constexpr int kBatchMax = 32;                 // sessions per batched persistent launch (k_gn_batch's table, grid_knn.cu)
 
 struct S2mPlanIn {
     int n, n_last;                  // query upper bound (the exact count unless dev_count); count of the previous scan (0: none)
@@ -60,6 +62,41 @@ inline S2mPlan s2m_plan(const S2mPlanIn& in) {
     // one thread per query: per-thread run lists (int4) in dynamic shared memory (thread_knn5); static + dynamic exceed 48 KB
     p.dyn_smem = p.tma ? (size_t)kWarps * 2 * kStageTileBytes : p.lanes == 1 ? (size_t)kRunCap * kBlock * 16 : 0;
     return p;
+}
+
+// Instantiation of the persistent GN kernel a plan launches: 0..4 = 1, 2, 4, 8, 16 lanes; 5 = 16 lanes with bulk-copy staging.
+constexpr int kGnKinds = 6;
+inline int s2m_kind(const S2mPlan& p) {
+    return p.tma ? 5 : p.lanes == 1 ? 0 : p.lanes == 2 ? 1 : p.lanes == 4 ? 2 : p.lanes == 8 ? 3 : 4;
+}
+
+// The launches of a batched scan-to-map step (s2m_batch, grid_knn.cu).  Each session keeps the plan its solo call would make.
+// Persistent sessions are grouped by instantiation and packed first-fit, in call order, into cooperative launches whose summed
+// grid is co-resident (occ[kind] blocks per SM of k_gn_batch<kind> times sm_count) and that hold at most max_per_launch
+// sessions; a session whose plan is not persistent (or whose kernel cannot be resident at all) goes to `solo`.
+struct S2mLaunch {
+    int kind, grid;                 // instantiation (s2m_kind), summed grid
+    std::vector<int> sessions;      // indices into the plans, in call order; blocks follow in this order
+};
+struct S2mPack {
+    std::vector<S2mLaunch> launches;
+    std::vector<int> solo;          // sessions that take s2m_run's own path
+};
+inline S2mPack s2m_batch_pack(const std::vector<S2mPlan>& plans, const int occ[kGnKinds], int sm_count, int max_per_launch = kBatchMax) {
+    S2mPack out;
+    for (int i = 0; i < (int)plans.size(); ++i) {
+        const S2mPlan& p = plans[i];
+        const int kind = s2m_kind(p);
+        const long long cap = (long long)occ[kind] * sm_count;
+        if (!p.persistent || p.grid > cap) { out.solo.push_back(i); continue; }
+        S2mLaunch* fit = nullptr;
+        for (S2mLaunch& l : out.launches)
+            if (l.kind == kind && (int)l.sessions.size() < max_per_launch && l.grid + p.grid <= cap) { fit = &l; break; }
+        if (!fit) { out.launches.push_back(S2mLaunch{kind, 0, {}}); fit = &out.launches.back(); }
+        fit->grid += p.grid;
+        fit->sessions.push_back(i);
+    }
+    return out;
 }
 
 }  // namespace lili
