@@ -517,6 +517,27 @@ int liliom_scan_to_map_resident_batch(liliom_ctx* const* ctxs, int B, double* po
  * are optional per session (NULL arrays or NULL entries: no download). */
 int liliom_odometry_resident_batch(liliom_ctx* const* ctxs, int B, double* poses7_inout, int match_cnt,
                                    liliom_iter_stats* stats, void* const* ds_out, const int* ds_cap, int* n_ds, int* status);
+/* The batched step in either mode, with per-session counts.  Session i gets exactly what
+ * liliom_scan_to_map_resident(ctxs[i], poses7 + 7*i, match_cnt[i], max_num_iter[i], mode, stats ? stats[i] : NULL) would give
+ * it, bit for bit: pose, status, every liliom_iter_stats entry (lm_iters included), the device-side counts, launches and the
+ * state left in ctxs[i].  match_cnt: B entries >= 0 (0: the session runs no scan-to-map kernel, as its solo call).
+ * max_num_iter: B entries, passed on as the solo call takes them; may be NULL in LILIOM_MODE_GN, where it is ignored.
+ * stats: NULL, or B pointers, each NULL (no stats for that session) or match_cnt[i] records.
+ * LILIOM_MODE_CERES: per outer iteration, the sessions still iterating share one per-pass search launch per lane count
+ * (k_knn_plane_batch, up to 32 sessions each), then one LM launch with one 512-thread block per session (k_lm_solve_batch),
+ * so B LM solves run side by side on B SMs.  LILIOM_MODE_GN: as liliom_scan_to_map_resident_batch, sessions of equal
+ * match_cnt share cooperative launches.
+ * LILIOM_E_ARG for the whole call, nothing changed: every refusal of liliom_scan_to_map_resident_batch, a NULL match_cnt, a
+ * negative match_cnt[i], a mode other than LILIOM_MODE_CERES / LILIOM_MODE_GN, LILIOM_MODE_CERES with a NULL max_num_iter.
+ * Per-session errors, streams and counters as liliom_scan_to_map_resident_batch.  liliom_scan_to_map_resident_batch is
+ * this call with match_cnt[i] = match_cnt, LILIOM_MODE_GN and stats[i] = stats + i*match_cnt. */
+int liliom_scan_to_map_resident_batch_ex(liliom_ctx* const* ctxs, int B, double* poses7_inout, const int* match_cnt,
+                                         const int* max_num_iter, int mode, liliom_iter_stats* const* stats, int* status);
+/* Same, with the semantics of liliom_odometry_resident per session (as liliom_odometry_resident_batch).  A session whose
+ * VoxelGrid speculation misses is redone by its own solo path, in `mode` with its own max_num_iter[i]. */
+int liliom_odometry_resident_batch_ex(liliom_ctx* const* ctxs, int B, double* poses7_inout, const int* match_cnt,
+                                      const int* max_num_iter, int mode, liliom_iter_stats* const* stats, void* const* ds_out,
+                                      const int* ds_cap, int* n_ds, int* status);
 
 #ifdef __cplusplus
 }

@@ -78,6 +78,7 @@ EXPORTS = [
     "liliom_kf_cloud", "liliom_kf_add_full", "liliom_global_map", "liliom_loop_align",
     "liliom_convert_pc2", "liliom_extract_rot_pc2", "liliom_set_ring_source", "liliom_set_time_source",
     "liliom_scan_to_map_resident_batch", "liliom_odometry_resident_batch",
+    "liliom_scan_to_map_resident_batch_ex", "liliom_odometry_resident_batch_ex",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -174,6 +175,9 @@ def lib() -> C.CDLL:
     L.liliom_scan_to_map_resident.argtypes = [vp, dp, C.c_int, C.c_int, C.c_int, C.POINTER(IterStats)]
     L.liliom_scan_to_map_resident_batch.argtypes = [C.POINTER(vp), C.c_int, dp, C.c_int, C.POINTER(IterStats), ip]
     L.liliom_odometry_resident_batch.argtypes = [C.POINTER(vp), C.c_int, dp, C.c_int, C.POINTER(IterStats), C.POINTER(vp), ip, ip, ip]
+    sp = C.POINTER(C.POINTER(IterStats))
+    L.liliom_scan_to_map_resident_batch_ex.argtypes = [C.POINTER(vp), C.c_int, dp, ip, ip, C.c_int, sp, ip]
+    L.liliom_odometry_resident_batch_ex.argtypes = [C.POINTER(vp), C.c_int, dp, ip, ip, C.c_int, sp, C.POINTER(vp), ip, ip, ip]
     L.liliom_odometry.argtypes = [vp, vp, C.c_int, dp, C.c_int, C.c_int, C.c_int, C.POINTER(IterStats), vp, C.c_int, ip]
     L.liliom_set_stream.argtypes = [vp, vp]
     L.liliom_upload_scan.argtypes = [vp, vp, C.c_int]
@@ -785,6 +789,67 @@ def odometry_resident_batch(ctxs, poses7, match_cnt: int, want_stats: bool = Fal
         raise LiliomError(rc)
     ds = [bufs[i][:nds[i]] for i in range(B)] if want_ds else nds[:B].copy()
     return poses[:B], status[:B], _batch_stats(st, B, match_cnt), ds
+
+
+def _per_session(v, B):
+    """An int or a sequence of B ints -> (B,) int32 array; None stays None (a NULL array, which the call refuses or ignores)."""
+    if v is None:
+        return None
+    a = np.full(B, int(v), np.int32) if np.isscalar(v) else np.array(v, dtype=np.int32).reshape(-1)
+    if len(a) != B:
+        raise ValueError(f"expected {B} per-session values, got {len(a)}")
+    return np.concatenate([a, np.zeros(1, np.int32)])
+
+
+def _batch_ex_args(ctxs, poses7, match_cnt, max_num_iter, want_stats):
+    B = len(ctxs)
+    handles = (C.c_void_p * max(B, 1))(*[c._h if c is not None else None for c in ctxs])
+    poses = np.array(poses7, dtype=np.float64).reshape(B, 7) if B else np.zeros((1, 7))
+    cnt, mni = _per_session(match_cnt, B), _per_session(max_num_iter, B)
+    st = [(IterStats * max(int(cnt[i]), 1))() for i in range(B)] if want_stats and cnt is not None else None
+    st_arr = (C.POINTER(IterStats) * max(B, 1))(*[C.cast(s, C.POINTER(IterStats)) for s in st]) if st is not None else None
+    status = np.zeros(max(B, 1), np.int32)
+    return B, handles, poses, cnt, mni, st, st_arr, status
+
+
+def _ip(a):
+    return a.ctypes.data_as(C.POINTER(C.c_int)) if a is not None else None
+
+
+def _batch_ex_stats(st, cnt, B):
+    return [[st[i][k] for k in range(int(cnt[i]))] for i in range(B)] if st is not None else None
+
+
+def scan_to_map_resident_batch_ex(ctxs, poses7, match_cnt, max_num_iter=15, mode: int = MODE_CERES, want_stats: bool = False):
+    """One scan-to-map step of every context in `ctxs` on its resident features, in either mode, with per-session counts
+    (liliom_scan_to_map_resident_batch_ex): session i gets what ctxs[i].scan_to_map_resident(poses7[i], match_cnt[i],
+    max_num_iter[i], mode) would give it.  match_cnt and max_num_iter: an int for every session or one per session.
+    Returns (poses (B, 7), status (B,), per-session stats lists of length match_cnt[i], or None); a session's own error is
+    its status, a whole-call error raises LiliomError."""
+    B, handles, poses, cnt, mni, st, st_arr, status = _batch_ex_args(ctxs, poses7, match_cnt, max_num_iter, want_stats)
+    rc = lib().liliom_scan_to_map_resident_batch_ex(handles, B, _dptr(poses), _ip(cnt), _ip(mni), mode, st_arr, _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    return poses[:B], status[:B], _batch_ex_stats(st, cnt, B)
+
+
+def odometry_resident_batch_ex(ctxs, poses7, match_cnt, max_num_iter=15, mode: int = MODE_CERES, want_stats: bool = False,
+                               want_ds: bool = False, caps=None):
+    """liliom_odometry_resident_batch_ex: VoxelGrid of each context's resident surf features, then one batched step in `mode`
+    with per-session match_cnt / max_num_iter.  caps: per-session DS capacity in points (default 65536 each).
+    Returns (poses (B, 7), status (B,), stats or None, per-session DS clouds (want_ds) or their sizes)."""
+    B, handles, poses, cnt, mni, st, st_arr, status = _batch_ex_args(ctxs, poses7, match_cnt, max_num_iter, want_stats)
+    caps = [int(x) for x in caps] if caps is not None else [65536] * B
+    bufs = [np.zeros(max(caps[i], 1), ctxs[i].dtype) for i in range(B)] if want_ds else None
+    outs = (C.c_void_p * max(B, 1))(*[b.ctypes.data for b in bufs]) if want_ds else None
+    cap_arr = np.array(caps + [0], np.int32)
+    nds = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_odometry_resident_batch_ex(handles, B, _dptr(poses), _ip(cnt), _ip(mni), mode, st_arr, outs, _ip(cap_arr), _ip(nds),
+                                                _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    ds = [bufs[i][:nds[i]] for i in range(B)] if want_ds else nds[:B].copy()
+    return poses[:B], status[:B], _batch_ex_stats(st, cnt, B), ds
 
 
 def comm_get_unique_id() -> bytes:

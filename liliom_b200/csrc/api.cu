@@ -606,27 +606,32 @@ extern "C" int liliom_odometry_resident(liliom_ctx* c, double pose7[7], int matc
 }
 
 // The whole-call refusals of the batched steps: nothing is touched when one holds.
-static bool batch_args_ok(liliom_ctx* const* ctxs, int B, const double* poses7, int match_cnt, const int* status) {
-    if (B < 1 || !ctxs || !poses7 || !status || match_cnt < 0) return false;
+static bool batch_args_ok(liliom_ctx* const* ctxs, int B, const double* poses7, const int* match_cnt, const int* max_num_iter, int mode,
+                          const int* status) {
+    if (B < 1 || !ctxs || !poses7 || !status || !match_cnt) return false;
+    if (mode != LILIOM_MODE_CERES && mode != LILIOM_MODE_GN) return false;
+    if (mode == LILIOM_MODE_CERES && !max_num_iter) return false;
     for (int i = 0; i < B; ++i) {
         const liliom_ctx* c = ctxs[i];
+        if (match_cnt[i] < 0) return false;
         if (!c || c->device != ctxs[0]->device || c->nranks > 1 || c->nccl_comm || c->peer_ready) return false;
         for (int j = 0; j < i; ++j) if (ctxs[j] == c) return false;
     }
     return true;
 }
 
-extern "C" int liliom_scan_to_map_resident_batch(liliom_ctx* const* ctxs, int B, double* poses7_inout, int match_cnt,
-                                                 liliom_iter_stats* stats, int* status) {
-    if (!batch_args_ok(ctxs, B, poses7_inout, match_cnt, status)) return LILIOM_E_ARG;
+extern "C" int liliom_scan_to_map_resident_batch_ex(liliom_ctx* const* ctxs, int B, double* poses7_inout, const int* match_cnt,
+                                                    const int* max_num_iter, int mode, liliom_iter_stats* const* stats, int* status) {
+    if (!batch_args_ok(ctxs, B, poses7_inout, match_cnt, max_num_iter, mode, status)) return LILIOM_E_ARG;
     LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
     for (int i = 0; i < B; ++i) status[i] = LILIOM_OK;
-    return s2m_batch(ctxs, B, poses7_inout, match_cnt, stats, status);
+    return s2m_batch(ctxs, B, poses7_inout, match_cnt, max_num_iter, mode, stats, status);
 }
 
-extern "C" int liliom_odometry_resident_batch(liliom_ctx* const* ctxs, int B, double* poses7_inout, int match_cnt,
-                                              liliom_iter_stats* stats, void* const* ds_out, const int* ds_cap, int* n_ds, int* status) {
-    if (!batch_args_ok(ctxs, B, poses7_inout, match_cnt, status)) return LILIOM_E_ARG;
+extern "C" int liliom_odometry_resident_batch_ex(liliom_ctx* const* ctxs, int B, double* poses7_inout, const int* match_cnt,
+                                                 const int* max_num_iter, int mode, liliom_iter_stats* const* stats, void* const* ds_out,
+                                                 const int* ds_cap, int* n_ds, int* status) {
+    if (!batch_args_ok(ctxs, B, poses7_inout, match_cnt, max_num_iter, mode, status)) return LILIOM_E_ARG;
     LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
     std::vector<int> step(B, LILIOM_OK);
     std::vector<char> filtered(B, 0);
@@ -637,22 +642,47 @@ extern "C" int liliom_odometry_resident_batch(liliom_ctx* const* ctxs, int B, do
     }
     const std::vector<double> pose_in(poses7_inout, poses7_inout + (size_t)7 * B);
     std::vector<int> ran(step);
-    LILI_TRY(s2m_batch(ctxs, B, poses7_inout, match_cnt, stats, step.data()));
+    LILI_TRY(s2m_batch(ctxs, B, poses7_inout, match_cnt, max_num_iter, mode, stats, step.data()));
     for (int i = 0; i < B; ++i) {
         if (!filtered[i]) continue;
         liliom_ctx* c = ctxs[i];
         double* pose = poses7_inout + 7 * i;
-        liliom_iter_stats* st = stats ? stats + (size_t)i * match_cnt : nullptr;
+        liliom_iter_stats* st = stats ? stats[i] : nullptr;
         void* out = ds_out ? ds_out[i] : nullptr;
         const int cap = ds_cap ? ds_cap[i] : 0;
         int* nd = n_ds ? n_ds + i : nullptr;
         const bool did_run = ran[i] == LILIOM_OK;
-        if (did_run && odo_spec_missed(c, step[i], false)) {
+        if (did_run && odo_spec_missed(c, step[i], false)) {       // the session's solo call redone from its start pose
             memcpy(pose, pose_in.data() + 7 * i, 7 * sizeof(double));
-            status[i] = odometry_on_resident_surf(c, pose, match_cnt, 0, LILIOM_MODE_GN, st, out, cap, nd, true);
+            status[i] = odometry_on_resident_surf(c, pose, match_cnt[i], max_num_iter ? max_num_iter[i] : 0, mode, st, out, cap, nd, true);
         } else status[i] = odo_finish(c, did_run, step[i], out, cap, nd);
     }
     return LILIOM_OK;
+}
+
+// The uniform-count GN calls: liliom_*_batch_ex with match_cnt for every session and stats + i*match_cnt.
+struct UniformBatch {
+    std::vector<int> cnt;
+    std::vector<liliom_iter_stats*> st;
+    UniformBatch(int B, int match_cnt, liliom_iter_stats* stats) : cnt(B, match_cnt), st(B) {
+        for (int i = 0; i < B; ++i) st[i] = stats ? stats + (size_t)i * match_cnt : nullptr;
+    }
+};
+
+extern "C" int liliom_scan_to_map_resident_batch(liliom_ctx* const* ctxs, int B, double* poses7_inout, int match_cnt,
+                                                 liliom_iter_stats* stats, int* status) {
+    if (B < 1 || match_cnt < 0) return LILIOM_E_ARG;
+    const UniformBatch u(B, match_cnt, stats);
+    return liliom_scan_to_map_resident_batch_ex(ctxs, B, poses7_inout, u.cnt.data(), nullptr, LILIOM_MODE_GN, stats ? u.st.data() : nullptr,
+                                                status);
+}
+
+extern "C" int liliom_odometry_resident_batch(liliom_ctx* const* ctxs, int B, double* poses7_inout, int match_cnt,
+                                              liliom_iter_stats* stats, void* const* ds_out, const int* ds_cap, int* n_ds, int* status) {
+    if (B < 1 || match_cnt < 0) return LILIOM_E_ARG;
+    const UniformBatch u(B, match_cnt, stats);
+    return liliom_odometry_resident_batch_ex(ctxs, B, poses7_inout, u.cnt.data(), nullptr, LILIOM_MODE_GN, stats ? u.st.data() : nullptr,
+                                             ds_out, ds_cap, n_ds, status);
 }
 
 extern "C" int liliom_find_surf_corr(liliom_ctx* c, const void* feats, int n, int stride, const double pose7[7], unsigned char* valid,

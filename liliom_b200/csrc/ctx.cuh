@@ -390,9 +390,11 @@ const long long* vg_coop_stamps(liliom_ctx* c);   // voxelgrid.cu
 
 int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int mode, liliom_iter_stats* stats,
             bool want_corr, double out29[29]);
-// GN step of B distinct single-GPU contexts (grid_knn.cu): sessions with status[i] == LILIOM_OK run, status[i] = their result;
-// the others are skipped.  Poses at poses7 + 7 i, stats (optional) at stats + i match_cnt.  Returns a whole-call CUDA error.
-int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, int match_cnt, liliom_iter_stats* stats, int* status);
+// Scan-to-map step of B distinct single-GPU contexts (grid_knn.cu): sessions with status[i] == LILIOM_OK run, status[i] = their
+// result; the others are skipped.  Session i: pose at poses7 + 7 i, match_cnt[i] iterations, max_num_iter[i] (Ceres mode; may be
+// null in GN mode), stats (optional) at stats[i].  Returns a whole-call CUDA error.
+int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, const int* match_cnt, const int* max_num_iter, int mode,
+              liliom_iter_stats* const* stats, int* status);
 
 int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf, int* n_edge, int* n_cut, bool sync_counts = true);
 // rings: nullptr = scanID from the elevation tables (line_num 16/32/64), else the u16 ring id of every input point (line_num 1..128)

@@ -550,10 +550,11 @@ __device__ __forceinline__ void write_neq_stats(const KnnArgs& a, const KnnSmem&
 #ifndef LILI_KNN1_MINBLOCKS
 #define LILI_KNN1_MINBLOCKS 2
 #endif
-template <int LANES>
-__global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) k_knn_plane(KnnArgs a, PassArgs p, const __grid_constant__ PeerArgs pa) {
+// The per-pass kernel's body for one session: its own ticket, partials, neq and qstate, so that the last block of the session
+// (blk.G() arrivals) sums the session's partials in the solo launch's fixed order.
+template <int LANES, class Blk>
+__device__ __forceinline__ void knn_plane_body(const KnnArgs& a, const PassArgs& p, const PeerArgs& pa, const Blk blk) {
     __shared__ __align__(16) KnnSmem S;
-    const SoloBlock blk;
     if (threadIdx.x == 0) S.peer_lost = 0;
     LILI_STAMP(0);
     const Q4 q{a.pose[0], a.pose[1], a.pose[2], a.pose[3]};
@@ -568,7 +569,7 @@ __global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) 
     __syncthreads();
     if (threadIdx.x == 0) {
         const unsigned int tk = atomicAdd(p.ticket, 1u);
-        S.is_last = (tk == gridDim.x - 1);
+        S.is_last = (tk == blk.G() - 1);
     }
     __syncthreads();
     LILI_STAMP(4);
@@ -592,6 +593,35 @@ __global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) 
     }
     LILI_STAMP_LAST(7);
     write_neq_stats(a, S, p.update_pose ? p.stats : nullptr);
+}
+
+template <int LANES>
+__global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) k_knn_plane(KnnArgs a, PassArgs p, const __grid_constant__ PeerArgs pa) {
+    knn_plane_body<LANES>(a, p, pa, SoloBlock{});
+}
+
+// One pass of several sessions' per-pass searches in one launch (Ceres-mode liliom_scan_to_map_resident_batch_ex).  Session s
+// owns blocks [off[s], off[s+1]) and runs the body its solo k_knn_plane launch would; the launch is not cooperative, so
+// sessions of any size share it.  Every session of a launch has the same lane count; the fused exchange is never attached.
+struct KnnBatchEntry {
+    KnnArgs a;
+    PassArgs p;
+};
+struct KnnBatch {
+    int n;                              // sessions in this launch
+    int off[kBatchMax + 1];             // session s owns blocks [off[s], off[s + 1])
+    KnnBatchEntry s[kBatchMax];
+};
+static_assert(sizeof(KnnBatch) <= 32764, "k_knn_plane_batch's session table must fit in the kernel parameter space");
+
+template <int LANES>
+__global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) k_knn_plane_batch(const __grid_constant__ KnnBatch tab) {
+    int s = 0;
+    while (s + 1 < tab.n && (int)blockIdx.x >= tab.off[s + 1]) ++s;
+    const PeerArgs pa{};
+    const KnnArgs a = tab.s[s].a;       // register copies, as k_knn_plane's by-value parameters: the body compiles to the same arithmetic
+    const PassArgs p = tab.s[s].p;
+    knn_plane_body<LANES>(a, p, pa, SessionBlock{(int)blockIdx.x - tab.off[s], (unsigned int)(tab.off[s + 1] - tab.off[s])});
 }
 
 // All GN iterations in ONE cooperative launch (single GPU, GN mode): per iteration the blocks meet at one
@@ -779,7 +809,8 @@ __device__ void lm_eval(const LmArgs& a, const double x[7], double out[kNormEq],
     __syncthreads();
 }
 
-__global__ void __launch_bounds__(kLmBlock) k_lm_solve(LmArgs a) {
+// The LM solve of one session, by one block of kLmBlock threads.
+__device__ __forceinline__ void lm_solve_body(const LmArgs& a) {
     __shared__ double red[kLmBlock / 32][kNormEq];
     __shared__ double sh_x[7];
     __shared__ int sh_cmd;   // 0 = stop, 1 = evaluate candidate in sh_x
@@ -908,6 +939,20 @@ __global__ void __launch_bounds__(kLmBlock) k_lm_solve(LmArgs a) {
             for (int k = 0; k <= kNormEq; ++k) write_stats(a.stats, k, a.neq0, (double)iteration, x);
         }
     }
+}
+
+__global__ void __launch_bounds__(kLmBlock) k_lm_solve(LmArgs a) { lm_solve_body(a); }
+
+// Several sessions' LM solves of one pass, one block each (Ceres-mode liliom_scan_to_map_resident_batch_ex): block s runs
+// session s's solo k_lm_solve, with the same block size and so the same reduction order.
+struct LmBatch {
+    int n;
+    LmArgs s[kBatchMax];
+};
+static_assert(sizeof(LmBatch) <= 32764, "k_lm_solve_batch's session table must fit in the kernel parameter space");
+__global__ void __launch_bounds__(kLmBlock) k_lm_solve_batch(const __grid_constant__ LmBatch tab) {
+    const LmArgs a = tab.s[blockIdx.x];     // a register copy, as k_lm_solve's by-value parameter: the body compiles to the same arithmetic
+    lm_solve_body(a);
 }
 
 // ------------------------------------------------------------------ instrumentation: the C-bar of SURVEY.md §8(d)
@@ -1074,7 +1119,8 @@ static void print_debug_timing(liliom_ctx* c, const long long* dbg, bool persist
 
 // One scan-to-map call between its checks and its results: the plan, the kernel arguments and, for a persistent plan, the rest
 // of k_gn_persistent's parameters.  s2m_begin enqueues the call's set-up on the context's stream and s2m_finish its read-back;
-// s2m_run launches in between, s2m_batch packs several contexts' persistent launches into k_gn_batch.
+// s2m_run launches in between, s2m_batch packs several contexts' persistent launches into k_gn_batch (GN mode) or their passes
+// into k_knn_plane_batch and k_lm_solve_batch (Ceres mode).
 struct S2mCall {
     S2mPlan p;
     KnnArgs a;
@@ -1153,11 +1199,34 @@ static int s2m_finish(liliom_ctx* c, const S2mCall& k, double pose7[7], liliom_i
     return LILIOM_OK;
 }
 
+// The start pose of a per-pass call, through the pinned block to pose_dev, before its first launch.
+static int s2m_stage_pose(liliom_ctx* c, const double pose7[7]) {
+    double* pin = c->h_pin->pose_stage;
+    memcpy(pin, pose7, 7 * sizeof(double)); pin[7] = 0.0;          // + cleared peer-loss flag
+    LILI_CUDA(c, cudaMemcpyAsync(c->pose_dev.p, pin, 8 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    return LILIOM_OK;
+}
+
+// What the per-pass kernel of pass `it` reads besides KnnArgs.
+static PassArgs pass_args(liliom_ctx* c, int it, int update_pose) {
+    return PassArgs{c->counter.as<unsigned int>(), c->stats_dev.as<double>() + (size_t)it * kStatsDoubles, update_pose, it > 0 ? 1 : 0};
+}
+
+// The LM solve of pass `it` on the correspondences its per-pass search left (Ceres mode).
+static LmArgs lm_args(liliom_ctx* c, const KnnArgs& a, int it, int max_num_iter) {
+    LmArgs l{};
+    l.feats = a.feats; l.valid = a.valid; l.plane = a.plane; l.n = c->n_feats; l.n_dev = c->d_nfeats;
+    l.pose = c->pose_dev.as<double>(); l.stats = c->stats_dev.as<double>() + (size_t)it * kStatsDoubles; l.huber_a = a.huber_a;
+    l.max_num_iter = max_num_iter;
+    l.neq0 = c->neq.as<double>();
+    return l;
+}
+
 // The launches of a call that s2m_begin planned, on the context's own stream.
 static int s2m_launch(liliom_ctx* c, S2mCall& k, const double pose7[7], int max_num_iter, int mode, bool want_corr) {
     const S2mPlan& p = k.p;
     KnnArgs& a = k.a;
-    const int n = c->n_feats, iters = k.iters;
+    const int iters = k.iters;
     if (p.persistent) {
         int iters_arg = iters, sync_mode = c->gn_sync;
         void* kargs[] = {&a, &iters_arg, &k.bar, &k.stats_base, &k.bar_base, &sync_mode, &k.pa, &k.io};
@@ -1168,10 +1237,8 @@ static int s2m_launch(liliom_ctx* c, S2mCall& k, const double pose7[7], int max_
         c->bar_arrivals += (unsigned int)iters * (unsigned int)p.grid;
         return LILIOM_OK;
     }
-    // one launch per iteration; the start pose goes through the pinned block to pose_dev
-    double* pin = c->h_pin->pose_stage;
-    memcpy(pin, pose7, 7 * sizeof(double)); pin[7] = 0.0;          // + cleared peer-loss flag
-    LILI_CUDA(c, cudaMemcpyAsync(c->pose_dev.p, pin, 8 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    // one launch per iteration
+    LILI_TRY(s2m_stage_pose(c, pose7));
     const bool multi = c->nranks > 1;
     // fused exchange, one launch per iteration (large scans: grid > one block per SM): the last block trades the sums with the
     // peers and performs the GN step itself — no ncclAllReduce, no update kernel
@@ -1179,7 +1246,7 @@ static int s2m_launch(liliom_ctx* c, S2mCall& k, const double pose7[7], int max_
     const int update_pose = (mode == LILIOM_MODE_GN && (!multi || peer_iter) && iters > 0) ? 1 : 0;
     const int launches = (iters == 0 && want_corr) ? 1 : iters;
     for (int it = 0; it < launches; ++it) {
-        PassArgs pass{c->counter.as<unsigned int>(), c->stats_dev.as<double>() + (size_t)it * kStatsDoubles, update_pose, it > 0 ? 1 : 0};
+        PassArgs pass = pass_args(c, it, update_pose);
         PeerArgs pit = peer_iter ? peer_args(c, ++c->peer_epoch) : PeerArgs{};
         void* kargs[] = {&a, &pass, &pit};
         LILI_TRY(timed_launch(c, k.timed, 1, [&] {
@@ -1193,11 +1260,7 @@ static int s2m_launch(liliom_ctx* c, S2mCall& k, const double pose7[7], int max_
             LILI_TRY(launch_check(c, "k_gn_update"));
         } else if (mode != LILIOM_MODE_GN) {
             if (multi) { c->last_error = "CERES mode is single-GPU (the LM solve is one block); use GN mode with a communicator"; return LILIOM_E_ARG; }
-            LmArgs l{};
-            l.feats = a.feats; l.valid = a.valid; l.plane = a.plane; l.n = n; l.n_dev = c->d_nfeats;
-            l.pose = c->pose_dev.as<double>(); l.stats = pass.stats; l.huber_a = a.huber_a; l.max_num_iter = max_num_iter;
-            l.neq0 = c->neq.as<double>();
-            k_lm_solve<<<1, kLmBlock, 0, c->stream>>>(l);
+            k_lm_solve<<<1, kLmBlock, 0, c->stream>>>(lm_args(c, a, it, max_num_iter));
             LILI_TRY(launch_check(c, "k_lm_solve"));
         }
     }
@@ -1223,21 +1286,102 @@ static const void* gn_batch_kernel(int kind) {
     }
 }
 
-int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, int match_cnt, liliom_iter_stats* stats, int* status) {
+static const void* knn_batch_kernel(int lanes) {
+    return lanes == 16 ? (const void*)k_knn_plane_batch<16> : lanes == 1 ? (const void*)k_knn_plane_batch<1> : lanes == 2 ? (const void*)k_knn_plane_batch<2>
+         : lanes == 4 ? (const void*)k_knn_plane_batch<4> : (const void*)k_knn_plane_batch<8>;
+}
+
+// Every other session's stream (its set-up so far) is ordered before the shared launches on ctxs[0]'s stream ...
+static int batch_join_in(liliom_ctx* c0, liliom_ctx* c) {
+    if (c->stream == c0->stream) return LILIOM_OK;
+    LILI_CUDA(c, cudaEventRecord(c->ev_batch, c->stream));
+    LILI_CUDA(c0, cudaStreamWaitEvent(c0->stream, c->ev_batch, 0));
+    return LILIOM_OK;
+}
+// ... and after them (c0->ev_batch recorded behind the last shared launch)
+static int batch_join_out(liliom_ctx* c0, liliom_ctx* c) {
+    if (c->stream != c0->stream) LILI_CUDA(c, cudaStreamWaitEvent(c->stream, c0->ev_batch, 0));
+    return LILIOM_OK;
+}
+
+// Ceres mode: per pass, the sessions' searches in k_knn_plane_batch launches, then their LM solves in k_lm_solve_batch launches,
+// all on ctxs[0]'s stream.  The start poses are staged on each session's own stream before the join.
+static int s2m_batch_ceres(liliom_ctx* const* cs, std::vector<S2mCall>& k, const std::vector<int>& run, const std::vector<S2mPlan>& plans,
+                           const std::vector<int>& iters, double* poses7, const int* max_num_iter, bool timed0, int* status) {
+    liliom_ctx* c0 = cs[0];
+    const cudaStream_t s0 = c0->stream;
+    std::vector<int> live;                  // indices into run of the sessions that launch
+    for (int j = 0; j < (int)run.size(); ++j) {
+        const int i = run[j];
+        status[i] = s2m_stage_pose(cs[i], poses7 + 7 * i);
+        if (status[i] == LILIOM_OK && iters[j] > 0) live.push_back(j);
+    }
+    std::vector<S2mPlan> lp;
+    std::vector<int> li;
+    for (int j : live) { lp.push_back(plans[j]); li.push_back(iters[j]); }
+    const std::vector<S2mPass> passes = s2m_pass_pack(lp, li);
+    if (passes.empty()) return LILIOM_OK;
+    for (int j : live) LILI_TRY(batch_join_in(c0, cs[run[j]]));
+    for (int it = 0; it < (int)passes.size(); ++it) {
+        for (const S2mKnnLaunch& l : passes[it].knn) {
+            KnnBatch tab{};
+            tab.n = (int)l.sessions.size();
+            for (int m = 0; m < tab.n; ++m) {
+                const int j = live[l.sessions[m]];
+                liliom_ctx* c = cs[run[j]];
+                tab.off[m + 1] = tab.off[m] + plans[j].grid;
+                tab.s[m] = KnnBatchEntry{k[run[j]].a, pass_args(c, it, 0)};
+                c->cnt.launches++;
+            }
+            const size_t dyn = plans[live[l.sessions[0]]].dyn_smem;
+            if (l.lanes == 1) LILI_CUDA(c0, cudaFuncSetAttribute(knn_batch_kernel(1), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
+            void* kargs[] = {&tab};
+            LILI_TRY(timed_launch(c0, timed0, 1, [&]() -> int {
+                LILI_CUDA(c0, cudaLaunchKernel(knn_batch_kernel(l.lanes), dim3(tab.off[tab.n]), dim3(kBlock), kargs, dyn, s0));
+                LILI_CUDA(c0, cudaGetLastError());
+                return LILIOM_OK;
+            }));
+        }
+        for (const std::vector<int>& l : passes[it].lm) {
+            LmBatch tab{};
+            tab.n = (int)l.size();
+            for (int m = 0; m < tab.n; ++m) {
+                const int i = run[live[l[m]]];
+                tab.s[m] = lm_args(cs[i], k[i].a, it, max_num_iter[i]);
+                cs[i]->cnt.launches++;
+            }
+            k_lm_solve_batch<<<tab.n, kLmBlock, 0, s0>>>(tab);
+            LILI_CUDA(c0, cudaGetLastError());
+        }
+    }
+    LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, s0));
+    for (int j : live) LILI_TRY(batch_join_out(c0, cs[run[j]]));
+    return LILIOM_OK;
+}
+
+int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, const int* match_cnt, const int* max_num_iter, int mode,
+              liliom_iter_stats* const* stats, int* status) {
     liliom_ctx* c0 = cs[0];
     const cudaStream_t s0 = c0->stream;
     std::vector<S2mCall> k(B);
-    std::vector<S2mPlan> plans(B);
-    std::vector<int> run;                   // sessions that passed s2m_begin, in call order
+    std::vector<S2mPlan> plans;
+    std::vector<int> run, iters;            // sessions that passed s2m_begin, in call order, and their iteration counts
     for (int i = 0; i < B; ++i) {
         if (status[i] != LILIOM_OK) continue;
-        liliom_iter_stats* st = stats ? stats + (size_t)i * match_cnt : nullptr;
-        status[i] = s2m_begin(cs[i], poses7 + 7 * i, match_cnt, LILIOM_MODE_GN, st != nullptr, false, k[i]);
+        liliom_iter_stats* st = stats ? stats[i] : nullptr;
+        status[i] = s2m_begin(cs[i], poses7 + 7 * i, match_cnt[i], mode, st != nullptr, false, k[i]);
         if (status[i] != LILIOM_OK) continue;
-        plans[run.size()] = k[i].p;
+        plans.push_back(k[i].p);
+        iters.push_back(match_cnt[i]);
         run.push_back(i);
     }
-    plans.resize(run.size());
+    if (mode == LILIOM_MODE_CERES) {
+        const bool timed0 = !run.empty() && run[0] == 0 && k[0].timed;     // knn_ms / knn_launches: ctxs[0] only
+        LILI_TRY(s2m_batch_ceres(cs, k, run, plans, iters, poses7, max_num_iter, timed0, status));
+        for (int i : run)
+            if (status[i] == LILIOM_OK) status[i] = s2m_finish(cs[i], k[i], poses7 + 7 * i, stats ? stats[i] : nullptr, nullptr);
+        return LILIOM_OK;
+    }
     int occ[kGnKinds] = {};
     for (int kind = 0; kind < kGnKinds; ++kind) {
         bool used = false;
@@ -1248,55 +1392,51 @@ int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, int match_cnt, lilio
         if (dyn) LILI_CUDA(c0, cudaFuncSetAttribute(gn_batch_kernel(kind), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
         LILI_CUDA(c0, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[kind], gn_batch_kernel(kind), kBlock, dyn));
     }
-    const S2mPack pack = s2m_batch_pack(plans, occ, c0->sm_count);
-    // every other session's stream (its set-up above) is ordered before the launches on ctxs[0]'s stream
-    for (const S2mLaunch& l : pack.launches)
-        for (int j : l.sessions) {
-            liliom_ctx* c = cs[run[j]];
-            if (c->stream == s0) continue;
-            LILI_CUDA(c, cudaEventRecord(c->ev_batch, c->stream));
-            LILI_CUDA(c0, cudaStreamWaitEvent(s0, c->ev_batch, 0));
-        }
+    const std::vector<S2mGnGroup> groups = s2m_gn_groups(plans, iters, occ, c0->sm_count);
+    bool any = false;
+    for (const S2mGnGroup& g : groups)
+        for (const S2mLaunch& l : g.pack.launches)
+            for (int j : l.sessions) { LILI_TRY(batch_join_in(c0, cs[run[j]])); any = true; }
     const bool timed0 = !run.empty() && run[0] == 0 && k[0].timed && k[0].p.persistent;     // knn_ms / knn_launches: ctxs[0] only
-    for (const S2mLaunch& l : pack.launches) {
-        GnBatch tab{};
-        tab.n = (int)l.sessions.size(); tab.iters = match_cnt; tab.sync_mode = c0->gn_sync;
-        for (int m = 0; m < tab.n; ++m) {
-            const S2mCall& ki = k[run[l.sessions[m]]];
-            tab.off[m + 1] = tab.off[m] + ki.p.grid;
-            tab.s[m] = GnBatchEntry{ki.a, ki.bar, ki.stats_base, ki.bar_base, ki.io};
+    for (const S2mGnGroup& g : groups)
+        for (const S2mLaunch& l : g.pack.launches) {
+            GnBatch tab{};
+            tab.n = (int)l.sessions.size(); tab.iters = g.iters; tab.sync_mode = c0->gn_sync;
+            for (int m = 0; m < tab.n; ++m) {
+                const S2mCall& ki = k[run[l.sessions[m]]];
+                tab.off[m + 1] = tab.off[m] + ki.p.grid;
+                tab.s[m] = GnBatchEntry{ki.a, ki.bar, ki.stats_base, ki.bar_base, ki.io};
+            }
+            const S2mPlan& p = plans[l.sessions[0]];
+            void* kargs[] = {&tab};
+            LILI_TRY(timed_launch(c0, timed0, g.iters, [&]() -> int {
+                LILI_CUDA(c0, cudaLaunchCooperativeKernel(gn_batch_kernel(l.kind), dim3(l.grid), dim3(kBlock), kargs, p.dyn_smem, s0));
+                LILI_CUDA(c0, cudaGetLastError());
+                return LILIOM_OK;
+            }));
+            for (int j : l.sessions) {
+                liliom_ctx* c = cs[run[j]];
+                c->cnt.launches++;
+                c->bar_arrivals += (unsigned int)g.iters * (unsigned int)plans[j].grid;
+            }
         }
-        const S2mPlan& p = plans[l.sessions[0]];
-        void* kargs[] = {&tab};
-        LILI_TRY(timed_launch(c0, timed0, match_cnt, [&]() -> int {
-            LILI_CUDA(c0, cudaLaunchCooperativeKernel(gn_batch_kernel(l.kind), dim3(l.grid), dim3(kBlock), kargs, p.dyn_smem, s0));
-            LILI_CUDA(c0, cudaGetLastError());
-            return LILIOM_OK;
-        }));
-        for (int j : l.sessions) {
-            liliom_ctx* c = cs[run[j]];
-            c->cnt.launches++;
-            c->bar_arrivals += (unsigned int)match_cnt * (unsigned int)plans[j].grid;
-        }
-    }
-    // ... and after them
-    if (!pack.launches.empty()) LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, s0));
-    for (const S2mLaunch& l : pack.launches)
-        for (int j : l.sessions) {
-            liliom_ctx* c = cs[run[j]];
-            if (c->stream != s0) LILI_CUDA(c, cudaStreamWaitEvent(c->stream, c0->ev_batch, 0));
-        }
+    if (any) LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, s0));
+    for (const S2mGnGroup& g : groups)
+        for (const S2mLaunch& l : g.pack.launches)
+            for (int j : l.sessions) LILI_TRY(batch_join_out(c0, cs[run[j]]));
     // sessions whose plan is not persistent: their solo launches, on their own streams, while the batch runs
-    for (int j : pack.solo) {
-        const int i = run[j];
-        status[i] = s2m_launch(cs[i], k[i], poses7 + 7 * i, 0, LILIOM_MODE_GN, false);
-        if (status[i] == LILIOM_OK) status[i] = s2m_finish(cs[i], k[i], poses7 + 7 * i, stats ? stats + (size_t)i * match_cnt : nullptr, nullptr);
-    }
-    for (const S2mLaunch& l : pack.launches)
-        for (int j : l.sessions) {
+    for (const S2mGnGroup& g : groups)
+        for (int j : g.pack.solo) {
             const int i = run[j];
-            status[i] = s2m_finish(cs[i], k[i], poses7 + 7 * i, stats ? stats + (size_t)i * match_cnt : nullptr, nullptr);
+            status[i] = s2m_launch(cs[i], k[i], poses7 + 7 * i, max_num_iter ? max_num_iter[i] : 0, LILIOM_MODE_GN, false);
+            if (status[i] == LILIOM_OK) status[i] = s2m_finish(cs[i], k[i], poses7 + 7 * i, stats ? stats[i] : nullptr, nullptr);
         }
+    for (const S2mGnGroup& g : groups)
+        for (const S2mLaunch& l : g.pack.launches)
+            for (int j : l.sessions) {
+                const int i = run[j];
+                status[i] = s2m_finish(cs[i], k[i], poses7 + 7 * i, stats ? stats[i] : nullptr, nullptr);
+            }
     return LILIOM_OK;
 }
 

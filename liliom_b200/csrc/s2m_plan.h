@@ -12,7 +12,7 @@ constexpr int kBlock = 256;
 constexpr int kWarps = kBlock / 32;
 constexpr int kRunCap = 8;                    // runs per thread of the one-thread-per-query search (thread_knn5, knn_core.cuh)
 constexpr size_t kStageTileBytes = 3616;      // sizeof(StageTile), knn_core.cuh (checked there)
-constexpr int kBatchMax = 32;                 // sessions per batched persistent launch (k_gn_batch's table, grid_knn.cu)
+constexpr int kBatchMax = 32;                 // sessions per batched launch (the tables of k_gn_batch, k_knn_plane_batch, k_lm_solve_batch)
 
 struct S2mPlanIn {
     int n, n_last;                  // query upper bound (the exact count unless dev_count); count of the previous scan (0: none)
@@ -95,6 +95,69 @@ inline S2mPack s2m_batch_pack(const std::vector<S2mPlan>& plans, const int occ[k
         if (!fit) { out.launches.push_back(S2mLaunch{kind, 0, {}}); fit = &out.launches.back(); }
         fit->grid += p.grid;
         fit->sessions.push_back(i);
+    }
+    return out;
+}
+
+// A GN-mode batched step whose sessions run different iteration counts (liliom_scan_to_map_resident_batch_ex): k_gn_batch
+// shares one count per launch, so the sessions are grouped by count (groups in the order of their first session) and each
+// group is packed by s2m_batch_pack.  The pack's indices are into `plans`, as for one s2m_batch_pack call over all of them.
+struct S2mGnGroup {
+    int iters;
+    S2mPack pack;
+};
+inline std::vector<S2mGnGroup> s2m_gn_groups(const std::vector<S2mPlan>& plans, const std::vector<int>& iters, const int occ[kGnKinds],
+                                             int sm_count, int max_per_launch = kBatchMax) {
+    std::vector<S2mGnGroup> out;
+    std::vector<char> done(plans.size(), 0);
+    for (size_t i = 0; i < plans.size(); ++i) {
+        if (done[i]) continue;
+        std::vector<int> members;
+        std::vector<S2mPlan> sub;
+        for (size_t j = i; j < plans.size(); ++j)
+            if (!done[j] && iters[j] == iters[i]) { done[j] = 1; members.push_back((int)j); sub.push_back(plans[j]); }
+        S2mGnGroup g{iters[i], s2m_batch_pack(sub, occ, sm_count, max_per_launch)};
+        for (S2mLaunch& l : g.pack.launches)
+            for (int& s : l.sessions) s = members[s];
+        for (int& s : g.pack.solo) s = members[s];
+        out.push_back(std::move(g));
+    }
+    return out;
+}
+
+// The launches of a Ceres-mode batched step (s2m_batch, grid_knn.cu).  Outer iteration `it` (a pass) serves the sessions with
+// iters[j] > it: first the per-pass kNN launches (k_knn_plane_batch), each of one lane count and at most max_per_launch
+// sessions, lane counts in the order of their first session; then the LM launches (k_lm_solve_batch) of the same sessions, at
+// most max_per_launch each.  Sessions keep call order inside every launch.  Per-pass launches are not cooperative, so any grid
+// fits; each session keeps the plan (lanes, grid) of its solo call.
+struct S2mKnnLaunch {
+    int lanes;
+    std::vector<int> sessions;      // indices into the plans, in call order; blocks follow in this order
+};
+struct S2mPass {
+    std::vector<S2mKnnLaunch> knn;
+    std::vector<std::vector<int>> lm;
+};
+inline std::vector<S2mPass> s2m_pass_pack(const std::vector<S2mPlan>& plans, const std::vector<int>& iters, int max_per_launch = kBatchMax) {
+    int passes = 0;
+    for (int n : iters) passes = std::max(passes, n);
+    std::vector<S2mPass> out(passes);
+    for (int it = 0; it < passes; ++it) {
+        std::vector<int> live, lanes;
+        for (int j = 0; j < (int)plans.size(); ++j) {
+            if (iters[j] <= it) continue;
+            live.push_back(j);
+            if (std::find(lanes.begin(), lanes.end(), plans[j].lanes) == lanes.end()) lanes.push_back(plans[j].lanes);
+        }
+        for (int ln : lanes)
+            for (int j : live) {
+                if (plans[j].lanes != ln) continue;
+                std::vector<S2mKnnLaunch>& knn = out[it].knn;
+                if (knn.empty() || knn.back().lanes != ln || (int)knn.back().sessions.size() >= max_per_launch) knn.push_back(S2mKnnLaunch{ln, {}});
+                knn.back().sessions.push_back(j);
+            }
+        for (size_t k = 0; k < live.size(); k += (size_t)max_per_launch)
+            out[it].lm.emplace_back(live.begin() + k, live.begin() + std::min(live.size(), k + (size_t)max_per_launch));
     }
     return out;
 }

@@ -1,12 +1,16 @@
 #!/usr/bin/env python
 """Several odometry sessions on one GPU, three ways: (a) solo calls one after another, (b) one host thread + context stream
-per session (as tools/multistream.py), (c) one liliom_odometry_resident_batch call per step.  Headline workload per session:
-seeded 24k-point Horizon sweep (extracted on the device), 1 M-point map, 10 GN iterations; the sweeps and poses of
-tools/multistream.py.  Every timed scan is the whole resident step: upload of the raw sweep, extraction, VoxelGrid and GN.
-Prints the card, its power limit and maximum SM clock, then one JSON line per session count: aggregate scans/s and the median
-per-session step latency (the step call: odometry_resident in (a) and (b), the batch call in (c)), and the GN launches one
-batch call issues (k_gn_batch / k_gn_persistent / k_knn_plane kernels counted with torch.profiler in a separate call).
-usage: batch_bench.py [--sessions 1 2 4 8 16 32] [--steps 30] [--warmup 5]"""
+per session (as tools/multistream.py), (c) one liliom_odometry_resident_batch_ex call per step.  Headline workload per session:
+seeded 24k-point Horizon sweep (extracted on the device), 1 M-point map; the sweeps and poses of tools/multistream.py.
+--mode gn (default): 10 GN iterations; --mode ceres: the reference's configs, scan_match_cnt 2 outer iterations of at most
+max_num_iter 15 LM iterations (--match-cnt / --max-num-iter override either).  Every timed scan of (a)-(c) is the whole resident
+step: upload of the raw sweep, extraction, VoxelGrid and scan-to-map.  Two more legs time only the scan-to-map call on resident
+down-sampled features (the step legs are bound by the host's upload and extraction): (d) solo liliom_scan_to_map_resident calls
+one after another, (e) one liliom_scan_to_map_resident_batch_ex call; their *_call_ms_median is the time of all B sessions.
+Prints the card, its power limit and maximum SM clock, then one JSON line per session count: aggregate scans/s, the median
+per-session step latency (the step call: odometry_resident in (a) and (b), the batch call in (c)), and the scan-to-map kernels
+one batched scan-to-map call launches (counted with torch.profiler in a separate call).
+usage: batch_bench.py [--sessions 1 2 4 8 16 32] [--steps 30] [--warmup 5] [--mode {gn,ceres}] [--match-cnt N] [--max-num-iter N]"""
 import argparse
 import json
 import os
@@ -23,9 +27,6 @@ import torch  # noqa: E402
 import liliom_b200 as L  # noqa: E402
 from liliom_b200 import synth  # noqa: E402
 
-ITERS = 10
-
-
 def card():
     out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
                          capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
@@ -38,10 +39,16 @@ def main():
     ap.add_argument("--sessions", type=int, nargs="*", default=[1, 2, 4, 8, 16, 32])
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--mode", choices=("gn", "ceres"), default="gn")
+    ap.add_argument("--match-cnt", type=int, default=None, help="outer iterations (default: 10 in GN mode, 2 in Ceres mode)")
+    ap.add_argument("--max-num-iter", type=int, default=15, help="LM iterations per outer iteration (Ceres mode)")
     args = ap.parse_args()
+    mode = L.MODE_CERES if args.mode == "ceres" else L.MODE_GN
+    iters = args.match_cnt if args.match_cnt is not None else (2 if mode == L.MODE_CERES else 10)
+    mni = args.max_num_iter
     if not torch.cuda.is_available():
         raise SystemExit("batch_bench.py measures on a CUDA device; none is visible")
-    print(json.dumps(card()), flush=True)
+    print(json.dumps(dict(card(), mode=args.mode, match_cnt=iters, max_num_iter=mni)), flush=True)
     m, _ = synth.make_map(1_000_000)
     T0 = synth.default_true_pose()
     sweeps = []
@@ -66,13 +73,13 @@ def main():
         def solo_step(s, k, lat):
             sw = feed(s, k)
             t = time.perf_counter()
-            ctxs[s].odometry_resident(sw["guess"], ITERS, mode=L.MODE_GN, want_stats=False)
+            ctxs[s].odometry_resident(sw["guess"], iters, max_num_iter=mni, mode=mode, want_stats=False)
             lat.append(time.perf_counter() - t)
 
         def batch_step(k, lat):
             poses = np.array([feed(s, k)["guess"] for s in range(B)])
             t = time.perf_counter()
-            _, status, _, _ = L.odometry_resident_batch(ctxs, poses, ITERS)
+            _, status, _, _ = L.odometry_resident_batch_ex(ctxs, poses, iters, mni, mode)
             lat.append(time.perf_counter() - t)
             assert (status == 0).all(), status
 
@@ -106,12 +113,46 @@ def main():
             dt = time.perf_counter() - t0
             row[f"{name}_scans_per_s"] = round(B * args.steps / dt, 1)
             row[f"{name}_step_ms_median"] = round(float(np.median(lat)) * 1e3, 4)
+        # scan-to-map alone on resident down-sampled features: each session keeps its sweep's DS cloud
+        guesses = []
+        for s in range(B):
+            sw = feed(s, 0)
+            _, _, ds = ctxs[s].odometry_resident(sw["guess"], iters, max_num_iter=mni, mode=mode, want_ds=True, cap=len(sw["pts"]),
+                                                 want_stats=False)
+            ctxs[s].upload_feats(ds)
+            guesses.append(sw["guess"])
+        guesses = np.array(guesses)
+
+        def s2m_solo(n):
+            lat = []
+            for _ in range(n):
+                t = time.perf_counter()
+                for s in range(B):
+                    ctxs[s].scan_to_map_resident(guesses[s], iters, max_num_iter=mni, mode=mode)
+                lat.append(time.perf_counter() - t)
+            return lat
+
+        def s2m_batch(n):
+            lat = []
+            for _ in range(n):
+                t = time.perf_counter()
+                _, status, _ = L.scan_to_map_resident_batch_ex(ctxs, guesses, iters, mni, mode)
+                lat.append(time.perf_counter() - t)
+                assert (status == 0).all(), status
+            return lat
+
+        for name, fn in (("d_s2m_solo", s2m_solo), ("e_s2m_batch", s2m_batch)):
+            fn(args.warmup)
+            torch.cuda.synchronize()
+            lat = fn(args.steps)
+            row[f"{name}_call_ms_median"] = round(float(np.median(lat)) * 1e3, 4)
         with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            batched(1)
+            s2m_batch(1)
             torch.cuda.synchronize()
         names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-        row["batch_gn_launches"] = sum(1 for n in names if "k_gn_batch" in n)
-        row["batch_solo_gn_launches"] = sum(1 for n in names if "k_gn_persistent" in n or "k_knn_plane" in n)
+        for key, pat in (("k_gn_batch", "k_gn_batch"), ("k_knn_plane_batch", "k_knn_plane_batch"), ("k_lm_solve_batch", "k_lm_solve_batch"),
+                         ("k_gn_persistent", "k_gn_persistent"), ("k_knn_plane", "k_knn_plane<"), ("k_lm_solve", "k_lm_solve(")):
+            row[f"s2m_batch_launches_{key}"] = sum(1 for n in names if pat in n)
         print(json.dumps(row), flush=True)
         for c in ctxs:
             c.close()
