@@ -15,7 +15,7 @@ __global__ void k_undistort(unsigned char* __restrict__ pts, int n, int stride, 
     float4* p0 = reinterpret_cast<float4*>(pts + (size_t)i * stride);
     float4 a = p0[0];
     const float intensity = *reinterpret_cast<const float*>(pts + (size_t)i * stride + (stride == 48 ? 32 : 16));
-    const int line = (int)intensity;                                                    // :181
+    const int line = scan_id_of(intensity);                                             // :181 (x86's int(float))
     const double dt_i = (double)fsubx(intensity, (float)line);                         // :182 float - int -> float, then widened
     double ratio_i = dt_i / 0.1;                                                        // :183
     if (ratio_i > 1) ratio_i = 1;                                                       // :185-186
@@ -116,6 +116,7 @@ extern "C" int liliom_create(liliom_ctx** out, const liliom_params* p, int devic
     if (const char* e1 = getenv("LILIOM_KNN_LANES")) { int v = atoi(e1); if (v == 1 || v == 2 || v == 4 || v == 8 || v == 16) c->force_lanes = v; }
     c->dbg_timing = getenv("LILIOM_DEBUG_TIMING") != nullptr;
     c->rot_slow_walk = getenv("LILIOM_ROT_SLOW_WALK") != nullptr;
+    if (const char* e9 = getenv("LILIOM_HZ_CHAIN")) c->hz_chain = atoi(e9) != 0;
     c->test_shrink_box = getenv("LILIOM_TEST_SHRINK_BOX") != nullptr;
     if (const char* e8 = getenv("LILIOM_KNN_TMA")) c->knn_tma = atoi(e8) != 0;
     if (const char* e5 = getenv("LILIOM_GN_SYNC")) { int v = atoi(e5); if (v == 0 || v == 1 || v == 3) c->gn_sync = v; }

@@ -294,6 +294,7 @@ struct liliom_ctx {
                                          // 1 = acquire poll, 0 = full fences on both sides
     bool dbg_timing = false;             // LILIOM_DEBUG_TIMING: stage clocks of the cooperative kernels, printed by s2m_run
     bool rot_slow_walk = false;          // LILIOM_ROT_SLOW_WALK (test hook): the general walk of k_rot_ring for every segment
+    bool hz_chain = false;               // LILIOM_HZ_CHAIN=1 (test hook): the Horizon extractor's multi-launch chain, not k_hz_coop
     bool test_shrink_box = false;        // LILIOM_TEST_SHRINK_BOX (test hook): grid_build takes a box too small in x
     bool knn_tma = false, knn_tma_smem_set = false;   // LILIOM_KNN_TMA=1: bulk-copy (cp.async.bulk + mbarrier) staging of the runs in the 16-lane search
     bool knn1_smem_set = false;          // dynamic shared memory limit raised for the one-thread-per-query kernels on this device

@@ -30,7 +30,7 @@ __device__ __forceinline__ int hz_keep(const Pt48* __restrict__ pts, int i) {
     const float thres = 0.1f;
     bool fin = isfinite(a.x) && isfinite(a.y) && isfinite(a.z);
     bool close = (a.x * a.x + a.y * a.y + a.z * a.z) < thres * thres;
-    int scan_id = (int)inten;
+    int scan_id = scan_id_of(inten);     // x86's int(float): NaN, +-inf and |x| >= 2^31 give INT_MIN and drop the point
     return fin && !close && scan_id >= 0;
 }
 
@@ -50,9 +50,9 @@ __device__ __forceinline__ void hz_deskew_bin_point(const Pt48* __restrict__ pts
                                                     int* __restrict__ mat) {
     const float4 a = pts[i].a;
     const float intensity = pts[i].c.x, curvature = pts[i].c.y;
-    const int scan_id = (int)intensity;
+    const int scan_id = scan_id_of(intensity);
     // undistortion, :104-127
-    int line = (int)intensity;
+    int line = scan_id;
     double dt_i = (double)(intensity - (float)line);
     double ratio_i = dt_i / 0.1;
     if (ratio_i >= 1.0) ratio_i = 1.0;
@@ -484,7 +484,7 @@ int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf
     int* counts = c->hz_counts.as<int>();
     int* offs = counts + 2 * (HZ_PATCHES + 1);
     int* totals = counts + 4 * (HZ_PATCHES + 1);
-    const bool coop = c->sm_count * HZC_WARPS >= HZ_PATCHES && n > 0;
+    const bool coop = !c->hz_chain && c->sm_count * HZC_WARPS >= HZ_PATCHES && n > 0;
     if (coop) {
         // one cooperative launch; scratch: per-block counts behind the patch counts, barrier words in their own buffer
         if (!c->hz_ctl.p) {

@@ -21,6 +21,13 @@ VGB_HD double addx(double a, double b) { return a + b; }
 VGB_HD double subx(double a, double b) { return a - b; }
 #endif
 
+// int(intensity) as the reference's x86-64 build converts it (cvttss2si): truncation toward zero, and INT_MIN for NaN, +-inf and
+// every value outside [-2^31, 2^31).  The reference drops such a point by its negative scan id (L/src/Preprocessing.cpp:250-253);
+// a plain (int) on the device saturates instead (NaN -> 0, +inf -> INT_MAX) and would keep it.
+VGB_HD int scan_id_of(float x) {
+    return (x >= -2147483648.0f && x < 2147483648.0f) ? (int)x : INT_MIN;
+}
+
 VGB_HD D3 cross_x(D3 a, D3 b) {
     return {subx(mulx(a.y, b.z), mulx(a.z, b.y)), subx(mulx(a.z, b.x), mulx(a.x, b.z)), subx(mulx(a.x, b.y), mulx(a.y, b.x))};
 }

@@ -272,7 +272,7 @@ extern "C" void orc_undistort(void* pts, int n, int stride, const double trans[3
     for (int i = 0; i < n; ++i) {
         float* p = reinterpret_cast<float*>((unsigned char*)pts + (size_t)i * stride);
         const float intensity = stride == 48 ? p[8] : p[4];
-        const int line = int(intensity);
+        const int line = scan_id_of(intensity);
         const double dt_i = intensity - line;
         double ratio_i = dt_i / dt;
         if (ratio_i > 1) ratio_i = 1;

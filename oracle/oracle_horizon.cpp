@@ -51,10 +51,10 @@ extern "C" int orc_extract_horizon(const orc_pt48* pts, int n, const double q_im
         std::memset(&point, 0, sizeof(point));
         point.x = in.x; point.y = in.y; point.z = in.z;
         point.intensity = in.intensity; point.curvature = in.curvature;
-        int scan_id = (int)point.intensity;                          // :250-252
+        int scan_id = scan_id_of(point.intensity);                   // :250-252
         if (scan_id < 0) continue;                                   // :253
         // undistortion, :104-127
-        int line = int(point.intensity);
+        int line = scan_id_of(point.intensity);
         double dt_i = point.intensity - line;
         double ratio_i = dt_i / 0.1;
         if (ratio_i >= 1.0) ratio_i = 1.0;

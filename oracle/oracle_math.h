@@ -29,6 +29,13 @@ static inline V3 cross(V3 a, V3 b) {
 }
 static inline double norm(V3 a) { return std::sqrt(dot(a, a)); }
 
+// int(float) as the reference's x86-64 build converts it (cvttss2si): truncation toward zero, INT_MIN for NaN, +-inf and every
+// value outside [-2^31, 2^31).  Written out so that the oracle does not rest on an out-of-range conversion (undefined in C++).
+// Call sites: LiLi-OM/src/Preprocessing.cpp:106,250; LiLi-OM/src/LidarOdometry.cpp:181.
+static inline int scan_id_of(float x) {
+    return (x >= -2147483648.0f && x < 2147483648.0f) ? (int)x : INT32_MIN;
+}
+
 // Quaternion in Eigen's constructor order (w, x, y, z).
 struct Quat { double w, x, y, z; };
 

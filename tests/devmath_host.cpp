@@ -43,6 +43,11 @@ void dm_colpiv_qr(const double A15[15], const double b5[5], double x[3]) {
     for (int j = 0; j < 5; ++j) { for (int k = 0; k < 3; ++k) A[j][k] = A15[3 * j + k]; b[j] = b5[j]; }
     colpiv_qr_solve_5x3(A, b, x);
 }
+void dm_qslerp_identity(const double q[4], double t, double out[4]) {     // slerp(Identity -> q; t), not re-normalised
+    const Q4 r = qslerp_x(Q4{1.0, 0.0, 0.0, 0.0}, t, Q4{q[0], q[1], q[2], q[3]});
+    out[0] = r.w; out[1] = r.x; out[2] = r.y; out[3] = r.z;
+}
+int dm_scan_id_of(float x) { return scan_id_of(x); }
 void dm_qrot(const double q[4], const double v[3], double out[3]) {
     D3 r = qrot_x(Q4{q[0], q[1], q[2], q[3]}, D3{v[0], v[1], v[2]});
     out[0] = r.x; out[1] = r.y; out[2] = r.z;

@@ -23,6 +23,8 @@ def dm():
     L.dm_eigen_sym3.argtypes = [dp, dp, dp]; L.dm_eigen_sym3.restype = None
     L.dm_colpiv_qr.argtypes = [dp, dp, dp]; L.dm_colpiv_qr.restype = None
     L.dm_qrot.argtypes = [dp, dp, dp]; L.dm_qrot.restype = None
+    L.dm_qslerp_identity.argtypes = [dp, C.c_double, dp]; L.dm_qslerp_identity.restype = None
+    L.dm_scan_id_of.argtypes = [C.c_float]; L.dm_scan_id_of.restype = C.c_int
     vp = C.c_void_p
     L.dm_plane_gate.argtypes = [dp, fp, fp, C.c_double, C.c_double, C.c_int, fp, fp]
     L.dm_plane_neq.argtypes = [vp, C.c_int, vp, vp, dp, C.c_double, dp]; L.dm_plane_neq.restype = None
@@ -317,3 +319,42 @@ def test_cauchy_fold_matches_oracle_backend_blocks(dm, oracle):
         ref = oracle.backend_edge_block(feats, valid, pa, pb, s_weight, pose, 1.0)
         assert out[28] == ref[28] == sel.sum()
         np.testing.assert_allclose(out, ref, rtol=1e-8, atol=1e-9 * np.abs(ref[:21]).max())
+
+
+def test_qslerp_branches_match_oracle(dm, oracle):
+    """dev_math.cuh::qslerp_x (the de-skew's slerp from Identity, Eigen's Quaterniond::slerp) against the oracle's copy on every
+    branch: the linear one (|d| >= 1 - DBL_EPSILON, non-unit q included), d < 0 (s1 negated), t < 0 (a negative intensity's
+    extrapolation) and t > 1.  Compiled for the host, acos / sin are glibc's on both sides: bit for bit."""
+    eps = np.finfo(np.float64).eps
+    rng = np.random.default_rng(9)
+    qs = [np.array([1.0, 0, 0, 0]), np.array([1.0 - eps / 2, 1e-9, -2e-9, 3e-9]), np.array([1.0 - eps, 0, 1e-9, 0]),
+          np.array([1.0 - 2 * eps, 3e-8, 0, 0]), np.array([-1.0, 0, 0, 0]), np.array([-(1.0 - eps / 2), 1e-9, 0, 0])]
+    for _ in range(20):
+        q = rng.normal(size=4); q /= np.linalg.norm(q)
+        qs += [q, -q, q * 1.3, q * 0.7]
+    ts = [0.0, 1.0, 0.5, 1e-300, -0.5, -9.99, -1e-6, 1.5, 7.0, 0.999999]
+    hit = set()
+    out = np.zeros(4)
+    for q in qs:
+        d = q[0]
+        for t in ts:
+            dm.dm_qslerp_identity(_d(np.ascontiguousarray(q)), t, _d(out))
+            ref = oracle.slerp_identity(q, t)
+            assert out.tobytes() == ref.tobytes(), (q, t, out, ref)
+            hit.add(("linear" if abs(d) >= 1.0 - eps else "acos", d < 0, t < 0, t > 1))
+            if abs(d) >= 1.0 - eps:                      # the linear branch in closed form
+                s1 = -t if d < 0 else t
+                np.testing.assert_array_equal(out, [(1.0 - t) + s1 * q[0], s1 * q[1], s1 * q[2], s1 * q[3]])
+    for branch in ("linear", "acos"):
+        for neg in (False, True):
+            assert (branch, neg, True, False) in hit and (branch, neg, False, True) in hit, (branch, neg)
+
+
+def test_scan_id_of_is_x86_truncation(dm):
+    """pcl_xform.h::scan_id_of: int(float) as x86-64's cvttss2si gives it, INT_MIN for NaN, +-inf and |x| >= 2^31"""
+    f = np.float32
+    vals = [0.0, 0.999, 5.09, -0.5, -0.999, -1.0, -1.5, 2147483520.0, -2147483648.0]
+    for v in vals:
+        assert dm.dm_scan_id_of(float(f(v))) == int(f(v)), v
+    for v in (np.nan, np.inf, -np.inf, 3e9, -3e9, 2147483648.0, -2147483904.0, 1e38):
+        assert dm.dm_scan_id_of(float(f(v))) == -2147483648, v
