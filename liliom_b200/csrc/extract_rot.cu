@@ -385,7 +385,8 @@ __global__ void __launch_bounds__(512) k_rot_ring(const Pt32* __restrict__ cloud
                 }
             }
         } else {
-            // bitonic sort ascending on (curvature, index): curvature >= 0 so its bit pattern orders like the value
+            // bitonic sort ascending on (curvature, index): curvature >= 0 so its bit pattern orders like the value, and a NaN
+            // (0x7fffffff) sorts after +inf
             for (int size = 2; size <= P; size <<= 1) {
                 for (int stride = size >> 1; stride > 0; stride >>= 1) {
                     for (int t = threadIdx.x; t < P / 2; t += blockDim.x) {
@@ -435,8 +436,10 @@ __global__ void __launch_bounds__(512) k_rot_ring(const Pt32* __restrict__ cloud
                         const unsigned long long key = S.keys[kk];
                         ind = (int)(unsigned)(key & 0xffffffffu);
                         const float cv = __uint_as_float((unsigned)(key >> 32));
-                        stop = !((double)cv > 2.0);       // sorted: nothing further can be picked (no side effects skipped)
-                        avail = !stop && S.picked[ind - rf] == 0;
+                        // sorted: nothing further can be picked (no side effects skipped).  A NaN curvature (its bits sort above
+                        // +inf) neither stops the walk nor is picked, as in the mask walk.
+                        stop = (double)cv <= 2.0;
+                        avail = (double)cv > 2.0 && S.picked[ind - rf] == 0;
                     }
                     const unsigned ms = __ballot_sync(full, stop), ma = __ballot_sync(full, avail);
                     const int fs = ms ? __ffs(ms) - 1 : 32, fa = ma ? __ffs(ma) - 1 : 32;

@@ -38,7 +38,8 @@ struct VgParams {
     int   mul[3];
     int   overflow;    // PCL: "Leaf size is too small" -> output = input
     int   n_finite;
-    int   bail;        // cooperative single-launch filter declined this input (see k_vg_coop): redo with the sort chain
+    int   bail;        // cooperative single-launch filter declined this input (see k_vg_coop), or a box bound's cell lies outside
+                       // int range (vg_params: x86 then sends indices to INT_MIN, outside the box): redo with full-width sort keys
 };
 
 // float <-> ordered int: integer order = float order (-0 below +0; NaNs of either sign outside every finite value)
@@ -108,9 +109,16 @@ __device__ __forceinline__ void vg_box_commit(int* box, int* mm) {
 
 VGB_HD long long vgb_mul64(long long a, long long b) { return (long long)((unsigned long long)a * (unsigned long long)b); }
 
+// float -> int and float -> int64 as PCL's x86-64 build converts them (cvttss2si): truncation toward zero, and INT_MIN /
+// INT64_MIN for NaN, +-inf and every value outside the target's range.  The device's own conversion saturates instead, and in
+// C++ an out-of-range conversion is undefined, so the rule is written out: a far or huge box gives PCL's indices, not clamped ones.
+VGB_HD bool vg_int_ok(float v) { return v >= -2147483648.0f && v < 2147483648.0f; }
+VGB_HD int vg_f2i_x86(float v) { return vg_int_ok(v) ? (int)v : INT_MIN; }
+VGB_HD long long vg_f2ll_x86(float v) { return (v >= -9223372036854775808.0f && v < 9223372036854775808.0f) ? (long long)v : LLONG_MIN; }
+
 // PCL's parameters for a box: min_b = floor(min / leaf), div_b = max_b - min_b + 1, mul = {1, dx, dx*dy}, and the
 // "leaf size too small" test dx*dy*dz > INT_MAX with d = (long long)((max - min) / leaf) + 1.  An empty box gives
-// min_b = 0, div_b = 1.
+// min_b = 0, div_b = 1.  Conversions follow x86's rule (vg_f2i_x86); d + 1 and the products wrap as x86's do.
 VGB_HD VgParams vg_params(const int* box, float leaf) {
     VgParams p;
     p.inv_leaf = 1.0f / leaf;                       // Eigen::Array4f::Ones() / leaf_size_
@@ -123,9 +131,11 @@ VGB_HD VgParams vg_params(const int* box, float leaf) {
         long long d[3];
         for (int k = 0; k < 3; ++k) {
             const float lo = vg_ord2f(box[k]), hi = vg_ord2f(box[3 + k]);
-            d[k] = (long long)((unsigned long long)(long long)((hi - lo) * p.inv_leaf) + 1ull);
-            p.min_b[k] = (int)floorf(lo * p.inv_leaf);
-            const int max_b = (int)floorf(hi * p.inv_leaf);
+            d[k] = (long long)((unsigned long long)vg_f2ll_x86((hi - lo) * p.inv_leaf) + 1ull);
+            const float flo = floorf(lo * p.inv_leaf), fhi = floorf(hi * p.inv_leaf);
+            if (!vg_int_ok(flo) || !vg_int_ok(fhi)) p.bail = 1;
+            p.min_b[k] = vg_f2i_x86(flo);
+            const int max_b = vg_f2i_x86(fhi);
             p.div_b[k] = (int)((unsigned)max_b - (unsigned)p.min_b[k] + 1u);
         }
         if (vgb_mul64(vgb_mul64(d[0], d[1]), d[2]) > (long long)INT_MAX) p.overflow = 1;
@@ -135,19 +145,21 @@ VGB_HD VgParams vg_params(const int* box, float leaf) {
 }
 
 // PCL's voxel index of a finite point relative to the box: i0·mul0 + i1·mul1 + i2·mul2 with ik = floor(p_k / leaf) - min_b[k]
+// (x86's conversion: an ik out of int range is INT_MIN)
 VGB_HD unsigned vg_rel_index(const VgParams& p, float x, float y, float z) {
-    const int i0 = (int)(floorf(x * p.inv_leaf) - (float)p.min_b[0]);
-    const int i1 = (int)(floorf(y * p.inv_leaf) - (float)p.min_b[1]);
-    const int i2 = (int)(floorf(z * p.inv_leaf) - (float)p.min_b[2]);
+    const int i0 = vg_f2i_x86(floorf(x * p.inv_leaf) - (float)p.min_b[0]);
+    const int i1 = vg_f2i_x86(floorf(y * p.inv_leaf) - (float)p.min_b[1]);
+    const int i2 = vg_f2i_x86(floorf(z * p.inv_leaf) - (float)p.min_b[2]);
     return (unsigned)i0 * (unsigned)p.mul[0] + (unsigned)i1 * (unsigned)p.mul[1] + (unsigned)i2 * (unsigned)p.mul[2];
 }
 
 // Width of the VoxelGrid sort chain's keys for a cloud with this box: the fewest bits (at least 8) that hold every voxel
 // index with the all-ones key of that width left free for the non-finite points' sentinel; 32 when the box is empty, in
-// PCL's overflow case, or when the voxel count does not fit.
+// PCL's overflow case, when the voxel count does not fit, or when a box bound's cell leaves int range (x86 then sends the
+// indices to INT_MIN, outside the box).
 VGB_HD int vg_key_bits(const int* box, float leaf) {
     const VgParams p = vg_params(box, leaf);
-    if (p.n_finite <= 0 || p.overflow) return 32;
+    if (p.n_finite <= 0 || p.overflow || p.bail) return 32;
     const long long cells = vgb_mul64(vgb_mul64(p.div_b[0], p.div_b[1]), p.div_b[2]);
     if (!(cells > 0 && cells < (1LL << 31))) return 32;
     int bits = 8;

@@ -26,6 +26,18 @@ template <class P> struct Traits;
 template <> struct Traits<orc_pt48> { static constexpr bool has_normal = true; };
 template <> struct Traits<orc_pt32> { static constexpr bool has_normal = false; };
 
+// int(float) and int64_t(float) as PCL's x86-64 build converts them (cvttss2si): truncation, or INT_MIN / INT64_MIN for NaN,
+// +-inf and every value out of range (a far cluster: |x| / leaf >= 2^31 sends every x index to INT_MIN).  Written out: the
+// plain conversion is undefined in C++ out of range.
+static inline int x86_int(float v) { return scan_id_of(v); }
+static inline int64_t x86_int64(float v) {
+    return (v >= -9223372036854775808.0f && v < 9223372036854775808.0f) ? (int64_t)v : INT64_MIN;
+}
+static inline int64_t wrap_add(int64_t a, int64_t b) { return (int64_t)((uint64_t)a + (uint64_t)b); }
+static inline int64_t wrap_mul(int64_t a, int64_t b) { return (int64_t)((uint64_t)a * (uint64_t)b); }
+static inline int wrap_add32(int a, int b) { return (int)((unsigned)a + (unsigned)b); }
+static inline int wrap_mul32(int a, int b) { return (int)((unsigned)a * (unsigned)b); }
+
 template <class P>
 static int voxelgrid_t(const P* in, int n, float leaf, P* out, int cap) {
     if (n <= 0) return 0;
@@ -41,10 +53,10 @@ static int voxelgrid_t(const P* in, int n, float leaf, P* out, int cap) {
         mn[2] = std::min(mn[2], p.z); mx[2] = std::max(mx[2], p.z);
     }
     if (nfinite == 0) return 0;
-    int64_t dx = (int64_t)((mx[0] - mn[0]) * inv) + 1;
-    int64_t dy = (int64_t)((mx[1] - mn[1]) * inv) + 1;
-    int64_t dz = (int64_t)((mx[2] - mn[2]) * inv) + 1;
-    if (dx * dy * dz > (int64_t)INT_MAX) {
+    int64_t dx = wrap_add(x86_int64((mx[0] - mn[0]) * inv), 1);
+    int64_t dy = wrap_add(x86_int64((mx[1] - mn[1]) * inv), 1);
+    int64_t dz = wrap_add(x86_int64((mx[2] - mn[2]) * inv), 1);
+    if (wrap_mul(wrap_mul(dx, dy), dz) > (int64_t)INT_MAX) {
         // "Leaf size is too small for the input dataset. Integer indices would overflow." -> output = input
         int m = std::min(n, cap);
         std::memcpy(out, in, sizeof(P) * (size_t)m);
@@ -52,20 +64,20 @@ static int voxelgrid_t(const P* in, int n, float leaf, P* out, int cap) {
     }
     int min_b[3], max_b[3], div_b[3];
     for (int a = 0; a < 3; ++a) {
-        min_b[a] = (int)std::floor(mn[a] * inv);
-        max_b[a] = (int)std::floor(mx[a] * inv);
-        div_b[a] = max_b[a] - min_b[a] + 1;
+        min_b[a] = x86_int(std::floor(mn[a] * inv));
+        max_b[a] = x86_int(std::floor(mx[a] * inv));
+        div_b[a] = wrap_add32(wrap_add32(max_b[a], -min_b[a]), 1);
     }
-    const int mul[3] = {1, div_b[0], div_b[0] * div_b[1]};
+    const int mul[3] = {1, div_b[0], wrap_mul32(div_b[0], div_b[1])};
     std::vector<std::pair<unsigned, int>> iv;
     iv.reserve(n);
     for (int i = 0; i < n; ++i) {
         const P& p = in[i];
         if (!std::isfinite(p.x) || !std::isfinite(p.y) || !std::isfinite(p.z)) continue;
-        int i0 = (int)(std::floor(p.x * inv) - (float)min_b[0]);
-        int i1 = (int)(std::floor(p.y * inv) - (float)min_b[1]);
-        int i2 = (int)(std::floor(p.z * inv) - (float)min_b[2]);
-        int idx = i0 * mul[0] + i1 * mul[1] + i2 * mul[2];
+        int i0 = x86_int(std::floor(p.x * inv) - (float)min_b[0]);
+        int i1 = x86_int(std::floor(p.y * inv) - (float)min_b[1]);
+        int i2 = x86_int(std::floor(p.z * inv) - (float)min_b[2]);
+        int idx = wrap_add32(wrap_add32(wrap_mul32(i0, mul[0]), wrap_mul32(i1, mul[1])), wrap_mul32(i2, mul[2]));
         iv.emplace_back((unsigned)idx, i);
     }
     std::stable_sort(iv.begin(), iv.end(),

@@ -36,6 +36,14 @@ static inline int scan_id_of(float x) {
     return (x >= -2147483648.0f && x < 2147483648.0f) ? (int)x : INT32_MIN;
 }
 
+// The ROT extractor's curvature order (oracle_rot.cpp): a total order in which a NaN sorts after +inf and NaNs are equivalent,
+// so that std::stable_sort keeps them in index order (the reference's `curv[a] < curv[b]` is not a strict weak ordering with NaN).
+static inline bool rot_curv_less(float a, float b) {
+    const bool na = std::isnan(a), nb = std::isnan(b);
+    if (na || nb) return !na && nb;
+    return a < b;
+}
+
 // Quaternion in Eigen's constructor order (w, x, y, z).
 struct Quat { double w, x, y, z; };
 

@@ -5,7 +5,10 @@
 // gyro integration :179-223 stays host-side).  The class arrays cloudCurvature / SortInd /
 // NeighborPicked / Label (:9-12) persist across scans in the reference; every entry that is
 // read is first re-initialised at :390-393, so per-call arrays are equivalent.
-// std::sort at :410 is unstable; the order of equal curvatures is DEFINED as ascending index.
+// std::sort at :410 is unstable; the order of equal curvatures is DEFINED as ascending index.  Its comparator `curv[a] < curv[b]`
+// is no strict weak ordering once a curvature is NaN (returns of magnitude ~1e38 inside one 11-point window give inf - inf), and
+// the order is then undefined; DEFINED here: a NaN sorts after +inf (NaNs among themselves by index) and is never a candidate,
+// since both `> 2.0` and `< 0.1` are false for it.  rot_curv_less is that total order.
 #include "oracle_api.h"
 #include "oracle_math.h"
 #include <vector>
@@ -132,7 +135,7 @@ extern "C" int orc_extract_rot(const orc_pt32* pts, int n, const double q_imu_in
         for (int j = 0; j < 6; j++) {
             int sp = scanStartInd[i] + (scanEndInd[i] - scanStartInd[i]) * j / 6;
             int ep = scanStartInd[i] + (scanEndInd[i] - scanStartInd[i]) * (j + 1) / 6 - 1;
-            std::stable_sort(sortInd.begin() + sp, sortInd.begin() + ep + 1, [&](int a, int b) { return curv[a] < curv[b]; });  // :410
+            std::stable_sort(sortInd.begin() + sp, sortInd.begin() + ep + 1, [&](int a, int b) { return rot_curv_less(curv[a], curv[b]); });  // :410
 
             int largestPickedNum = 0;
             for (int k = ep; k >= sp; k--) {                                          // :413-453

@@ -163,7 +163,7 @@ int extract_rot(const orc_pt32* pts, const int* rings, const double* times, int 
         for (int j = 0; j < 6; j++) {
             int sp = scanStartInd[i] + (scanEndInd[i] - scanStartInd[i]) * j / 6;
             int ep = scanStartInd[i] + (scanEndInd[i] - scanStartInd[i]) * (j + 1) / 6 - 1;
-            std::stable_sort(sortInd.begin() + sp, sortInd.begin() + ep + 1, [&](int a, int b) { return curv[a] < curv[b]; });  // :410
+            std::stable_sort(sortInd.begin() + sp, sortInd.begin() + ep + 1, [&](int a, int b) { return rot_curv_less(curv[a], curv[b]); });  // :410
 
             int largestPickedNum = 0;
             for (int k = ep; k >= sp; k--) {                                          // :413-453

@@ -720,55 +720,12 @@ def test_horizon_deskew_second_restatement(oracle, world_small):
 
 def test_rot_ring_and_time_assignment_on_glibc(oracle, world_small):
     """R/src/Preprocessing.cpp:280-372 restated from the reference source with the float overloads resolved to glibc's own atanf /
-    atan2f through ctypes (what `using namespace std` makes the reference call): ring id, the halfPassed azimuth unwrapping and
+    atan2f through ctypes (what `using namespace std` makes the reference call, tests/rot_restate.py): ring id, the halfPassed azimuth unwrapping and
     intensity = ring + 0.1 * relTime, bucketed by ring in input order, must equal the oracle's laserCloud bit for bit."""
-    import ctypes as C
-    import math
-    libm = C.CDLL("libm.so.6")
-    libm.atanf.restype = C.c_float; libm.atanf.argtypes = [C.c_float]
-    libm.atan2f.restype = C.c_float; libm.atan2f.argtypes = [C.c_float, C.c_float]
-    f32 = np.float32
+    import rot_restate
     pts = world_small["hdl"]
     rc, _, _, cut, _, _ = oracle.extract_rot(pts, world_small["q_hdl"], (1, 0, 0, 0), 64, 1)
-    X, Y, Z = pts["x"], pts["y"], pts["z"]
-    keep = np.isfinite(X) & np.isfinite(Y) & np.isfinite(Z)
-    keep &= ~((X * X + Y * Y + Z * Z) < f32(3.0) * f32(3.0))                        # removeClosedPointCloud(3.0), float arithmetic
-    X, Y, Z = X[keep], Y[keep], Z[keep]
-    n = len(X)
-    startOri = f32(-libm.atan2f(Y[0], X[0]))
-    endOri = f32(float(f32(-libm.atan2f(Y[n - 1], X[n - 1]))) + 2 * math.pi)
-    if float(f32(endOri - startOri)) > 3 * math.pi:
-        endOri = f32(float(endOri) - 2 * math.pi)
-    elif float(f32(endOri - startOri)) < math.pi:
-        endOri = f32(float(endOri) + 2 * math.pi)
-    half = False
-    buckets = [[] for _ in range(64)]
-    rxy = np.sqrt(X * X + Y * Y)                                                    # sqrtf of float products (exactly rounded)
-    for i in range(n):
-        angle = f32(float(f32(f32(libm.atanf(f32(Z[i] / rxy[i]))) * f32(180))) / math.pi)
-        if angle >= -8.83:
-            scan = int(float(f32(f32(2) - angle)) * 3.0 + 0.5)
-        else:
-            scan = 32 + int((-8.83 - float(angle)) * 2.0 + 0.5)
-        if angle > 2 or angle < -24.33 or scan > 50 or scan < 0:
-            continue
-        ori = f32(-libm.atan2f(Y[i], X[i]))
-        if not half:
-            if float(ori) < float(startOri) - math.pi / 2:
-                ori = f32(float(ori) + 2 * math.pi)
-            elif float(ori) > float(startOri) + math.pi * 3 / 2:
-                ori = f32(float(ori) - 2 * math.pi)
-            if float(f32(ori - startOri)) > math.pi:
-                half = True
-        else:
-            ori = f32(float(ori) + 2 * math.pi)
-            if float(ori) < float(endOri) - math.pi * 3 / 2:
-                ori = f32(float(ori) + 2 * math.pi)
-            elif float(ori) > float(endOri) + math.pi / 2:
-                ori = f32(float(ori) - 2 * math.pi)
-        rel = f32(f32(ori - startOri) / f32(endOri - startOri))
-        buckets[scan].append(f32(scan + 0.1 * float(rel)))
-    got = np.array([v for b in buckets for v in b], np.float32)
+    got = rot_restate.assign(pts, 64)["intensity"]
     assert len(got) == len(cut)
     assert got.tobytes() == cut["intensity"].tobytes()
 

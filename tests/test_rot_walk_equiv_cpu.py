@@ -1,5 +1,5 @@
 """The availability-mask walk of k_rot_ring (liliom_b200/csrc/extract_rot.cu, segments up to 1024 points) against the sequential
-greedy walk it replaces (R/src/Preprocessing.cpp:401-500), both restated in Python for ONE ring:
+greedy walk it replaces (R/src/Preprocessing.cpp:401-500), both restated in Python for ONE ring (tests/rot_restate.py):
 
   * `walk_sequential` follows the reference loop line by line (it is also what oracle/oracle_rot.cpp does) and is pinned here
     against the oracle's labels on the synthetic HDL-64E sweep;
@@ -13,133 +13,7 @@ points within 0.5 m, gaps right at 0.05 m^2, picks next to segment boundaries.""
 import numpy as np
 import pytest
 
-F = np.float32
-
-
-def _gap_break(P, a, b):
-    d = P[a] - P[b]                                   # float32 arithmetic, ((dx*dx)+dy*dy)+dz*dz
-    g = F(F(d[0] * d[0]) + F(d[1] * d[1])) + F(d[2] * d[2])
-    return float(F(g)) > 0.05
-
-
-def _range2(P, k):
-    p = P[k]
-    return float(F(F(p[0] * p[0]) + F(p[1] * p[1])) + F(p[2] * p[2]))
-
-
-def _segments(rf, re):
-    scan_start, scan_end = rf + 5, re - 6            # :379-381
-    if scan_end - scan_start < 6:
-        return []
-    return [(scan_start + (scan_end - scan_start) * j // 6, scan_start + (scan_end - scan_start) * (j + 1) // 6 - 1) for j in range(6)]
-
-
-def walk_sequential(P, curv, rf, re):
-    """One ring, the reference loop.  Returns (label[], lessflat[], edge picks per segment)."""
-    n = len(P)
-    label = np.zeros(n, np.int32); picked = np.zeros(n, np.uint8); lessflat = np.zeros(n, np.uint8)
-    edges = []
-
-    def suppress(ind):
-        for l in range(1, 6):
-            if _gap_break(P, ind + l, ind + l - 1): break
-            picked[ind + l] = 1
-        for l in range(-1, -6, -1):
-            if _gap_break(P, ind + l, ind + l + 1): break
-            picked[ind + l] = 1
-
-    for sp, ep in _segments(rf, re):
-        order = sorted(range(sp, ep + 1), key=lambda i: (float(curv[i]), i))              # std::stable_sort on curvature: ties stay in index order
-        seg_edges = []
-        largest = 0
-        for ind in reversed(order):
-            if picked[ind] == 0 and float(curv[ind]) > 2.0:
-                largest += 1
-                if largest <= 2: label[ind] = 2; seg_edges.append(ind)
-                elif largest <= 10: label[ind] = 1; seg_edges.append(ind)
-                else: break
-                picked[ind] = 1
-                suppress(ind)
-        smallest = 0
-        for ind in order:
-            if _range2(P, ind) < 0.25: continue
-            if picked[ind] == 0 and float(curv[ind]) < 0.1:
-                label[ind] = -1
-                smallest += 1
-                if smallest >= 4: break
-                picked[ind] = 1
-                suppress(ind)
-        for k in range(sp, ep + 1):
-            if _range2(P, k) < 0.25: continue
-            if label[k] <= 0: lessflat[k] = 1
-        edges.append(seg_edges)
-    return label, lessflat, edges
-
-
-def walk_masks(P, curv, rf, re):
-    """One ring, the kernel's fast path (k_rot_ring, `L <= fast_cap` branch), same outputs."""
-    n = len(P)
-    label = np.zeros(n, np.int32); lessflat = np.zeros(n, np.uint8)
-    picked_ring = np.zeros(re - rf, np.uint8)          # S.picked, ring-local
-    edges = []
-    for sp, ep in _segments(rf, re):
-        L = ep - sp + 1
-        keys = [(int(np.float32(curv[sp + t]).view(np.uint32)) << 32) | (sp + t) for t in range(L)]
-        rank_of = [sum(1 for q in range(L) if keys[q] < keys[t]) for t in range(L)]          # counting sort
-        ind_of_rank = [0] * L
-        cls = [0] * L
-        for t in range(L):
-            r = rank_of[t]
-            ind_of_rank[r] = t
-            cv = float(curv[sp + t]); near = _range2(P, sp + t) < 0.25
-            cls[r] = (1 if cv > 2.0 else 0) | (2 if (cv < 0.1 and not near) else 0)
-        # window index i <-> global sp - 5 + i; brk[i]: pair (i, i-1)
-        brk = [0] * (L + 10)
-        for i in range(1, L + 10):
-            brk[i] = 1 if _gap_break(P, sp - 5 + i, sp - 5 + i - 1) else 0
-        ext = []
-        for t in range(L):
-            w = t + 5
-            nf = 0
-            while nf < 5 and not brk[w + nf + 1]: nf += 1
-            nb = 0
-            while nb < 5 and not brk[w - nb]: nb += 1
-            ext.append((nf, nb))
-        availS = 0; availF = 0                          # bit r: rank r still available
-        for r in range(L):
-            un = picked_ring[sp + ind_of_rank[r] - rf] == 0
-            if (cls[r] & 1) and un: availS |= 1 << r
-            if (cls[r] & 2) and un: availF |= 1 << r
-
-        def mark(t):
-            nonlocal availS, availF
-            nf, nb = ext[t]
-            for q in [t] + [t + l for l in range(1, nf + 1)] + [t - l for l in range(1, nb + 1)]:
-                picked_ring[sp + q - rf] = 1
-                if 0 <= q < L:
-                    availS &= ~(1 << rank_of[q]); availF &= ~(1 << rank_of[q])
-
-        seg_edges = []
-        largest = 0
-        while availS:
-            largest += 1
-            if largest > 10: break
-            t = ind_of_rank[availS.bit_length() - 1]    # highest set bit
-            label[sp + t] = 2 if largest <= 2 else 1
-            seg_edges.append(sp + t)
-            mark(t)
-        smallest = 0
-        while availF:
-            t = ind_of_rank[(availF & -availF).bit_length() - 1]      # lowest set bit
-            label[sp + t] = -1
-            smallest += 1
-            if smallest >= 4: break
-            mark(t)
-        for k in range(sp, ep + 1):
-            if _range2(P, k) < 0.25: continue
-            if label[k] <= 0: lessflat[k] = 1
-        edges.append(seg_edges)
-    return label, lessflat, edges
+from rot_restate import F, walk_masks, walk_sequential
 
 
 def _random_ring(rng, n):

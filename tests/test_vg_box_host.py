@@ -353,3 +353,38 @@ def test_per_ring_batch_matches_oracle_ring_by_ring(vb, oracle, world_small, lea
     want = np.concatenate([oracle.voxelgrid(pts[ring == r], leaf) for r in range(65)])
     got = check_voxelgrid(vb, want, pts, leaf, ring)
     assert np.array_equal(got[-5:], far)
+
+
+def _x86_int(v):
+    """int(float) as x86-64 converts it: truncation, INT_MIN out of range or not finite"""
+    v = float(np.float32(v))
+    return int(v) if -2.0 ** 31 <= v < 2.0 ** 31 else -(2 ** 31)
+
+
+@pytest.mark.parametrize("leaf", [0.6, 0.4])
+def test_params_and_sort_chain_on_out_of_range_boxes(vb, oracle, leaf):
+    """boxes whose cells leave int range: a tight far cluster (every x index INT_MIN, as PCL's x86 build computes it), a cluster
+    far on the negative side, and a box spanning ~1e38 (d out of int64 range).  min_b follows x86's conversion, the box is
+    flagged (bail) and the sort chain's key width is 32; the host sort chain equals the oracle's VoxelGrid on each."""
+    clouds = {}
+    k = np.arange(90)
+    clouds["far_x"] = np.stack([1.5e9 + 128.0 * (k // 30), 0.5 + (k % 30) * 0.125, np.zeros(90)], 1)
+    clouds["far_neg_y"] = np.stack([0.5 + (k % 30) * 0.125, -1.6e9 - 256.0 * (k // 30), np.ones(90)], 1)
+    clouds["huge"] = np.stack([np.where(k == 3, 1e38, k * 0.3), k * 0.1, np.zeros(90)], 1)
+    for name, xyz in clouds.items():
+        xyz = xyz.astype(np.float32)
+        box = np_box(xyz)
+        inv, min_b, div_b, mul, overflow, n_finite, bail = call_params(vb, box, leaf)
+        lo, hi = xyz.min(0), xyz.max(0)
+        assert min_b == [_x86_int(np.floor(F(lo[j]) * inv)) for j in range(3)], name
+        assert bail == 1 and vb.vb_key_bits(np.ascontiguousarray(box, np.int32), leaf) == 32, name
+        for dt in (oracle.PT48, oracle.PT32):
+            c = np.zeros(len(xyz), dt)
+            c["x"], c["y"], c["z"] = xyz.T
+            c["intensity"] = (k % 5).astype(np.float32)
+            got = check_voxelgrid(vb, oracle.voxelgrid(c, leaf), c, leaf)
+            if name == "far_x":
+                assert len(got) < 30 * 3                   # voxels that differ only in x merge
+    # in range: no flag
+    box = np_box(np.array([[1.0, 2.0, 3.0], [5.0, -4.0, 2.0]], np.float32))
+    assert call_params(vb, box, 0.4)[6] == 0
