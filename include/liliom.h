@@ -491,6 +491,13 @@ int liliom_set_stream(liliom_ctx* c, void* cuda_stream);
 int liliom_upload_scan(liliom_ctx* c, const void* pts, int n);
 int liliom_extract_resident(liliom_ctx* c, const double q_imu_wxyz[4], const double q_lb_wxyz[4],
                             int* n_surf, int* n_edge, int* n_cut);
+/* The three clouds the last extraction on this context left resident (liliom_extract_*, liliom_extract_resident or
+ * liliom_extract_resident_batch), as liliom_extract_horizon / liliom_extract_rot would have returned them: surf, edge and
+ * cutted (ROT: laserCloud), point_stride bytes per point.  The counts are always written; any cloud pointer may be NULL (count
+ * only).  A cloud larger than its capacity: LILIOM_E_CAPACITY, nothing written.  Nothing resident (no extraction yet, the last
+ * one failed, or liliom_odometry replaced the surf features): LILIOM_E_ARG. */
+int liliom_features_download(liliom_ctx* c, void* surf, int surf_cap, int* n_surf, void* edge, int edge_cap, int* n_edge,
+                             void* cut, int cut_cap, int* n_cut);
 /* keep `n` feature points resident (feats stride 16/32/48) */
 int liliom_upload_feats(liliom_ctx* c, const void* feats_body, int n, int stride);
 /* run scan-to-map on the resident features; pose in/out on host but no other traffic */
@@ -538,6 +545,26 @@ int liliom_scan_to_map_resident_batch_ex(liliom_ctx* const* ctxs, int B, double*
 int liliom_odometry_resident_batch_ex(liliom_ctx* const* ctxs, int B, double* poses7_inout, const int* match_cnt,
                                       const int* max_num_iter, int mode, liliom_iter_stats* const* stats, void* const* ds_out,
                                       const int* ds_cap, int* n_ds, int* status);
+/* liliom_extract_resident of B independent sessions in one call.  q_imu: 4*B doubles; q_lb: 4*B doubles or NULL (identity,
+ * as the solo call's NULL).  n_surf / n_edge / n_cut / status: B ints each.  Horizon (48-byte) and ROT (32-byte) contexts
+ * may be mixed.  Session i gets exactly what liliom_extract_resident(ctxs[i], q_imu + 4*i, q_lb ? q_lb + 4*i : NULL, ...)
+ * would give it, bit for bit: status and counts (-1 for Horizon sessions, whose counts stay on the device), the resident
+ * clouds, the labels and curvatures of liliom_extract_rot_labels, and the state left in ctxs[i].  Each session reads its
+ * own ring / time sources and side channels.  A session's own error (LILIOM_E_LINES, LILIOM_E_ARG for a missing side
+ * channel or ds_rate < 1, LILIOM_E_CAPACITY for a ring above 16384 or a segment above 4096 points) is its status; the
+ * others run.
+ * ROT sessions run every stage of the chain in shared launches of up to 32 sessions on ctxs[0]'s stream (the rings: one block
+ * per ring of every session); the library sorts and scans stay per session, in order on the same stream.  Horizon sessions whose solo call
+ * is one cooperative launch share cooperative launches (83 blocks and one barrier word per session, as many sessions per
+ * launch as are co-resident) on ctxs[0]'s stream; the others (LILIOM_HZ_CHAIN, empty sweeps) take their solo path.  Other
+ * sessions' streams are joined to ctxs[0]'s with events.  The call is synchronous, with one stream synchronise for all
+ * sessions (the solo ROT call has one per call).
+ * LILIOM_E_ARG for the whole call, nothing changed: B < 1, a NULL array (ctxs, q_imu, n_surf, n_edge, n_cut, status), a NULL
+ * or repeated context, contexts on different devices, a context with a communicator.
+ * Counters: every session's launches and lib_launches advance as in its solo call.  For a single session the solo call is
+ * faster (no event joins). */
+int liliom_extract_resident_batch(liliom_ctx* const* ctxs, int B, const double* q_imu, const double* q_lb,
+                                  int* n_surf, int* n_edge, int* n_cut, int* status);
 
 #ifdef __cplusplus
 }

@@ -79,6 +79,7 @@ EXPORTS = [
     "liliom_convert_pc2", "liliom_extract_rot_pc2", "liliom_set_ring_source", "liliom_set_time_source",
     "liliom_scan_to_map_resident_batch", "liliom_odometry_resident_batch",
     "liliom_scan_to_map_resident_batch_ex", "liliom_odometry_resident_batch_ex",
+    "liliom_extract_resident_batch", "liliom_features_download",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -182,6 +183,8 @@ def lib() -> C.CDLL:
     L.liliom_set_stream.argtypes = [vp, vp]
     L.liliom_upload_scan.argtypes = [vp, vp, C.c_int]
     L.liliom_extract_resident.argtypes = [vp, dp, dp, ip, ip, ip]
+    L.liliom_extract_resident_batch.argtypes = [C.POINTER(vp), C.c_int, dp, dp, ip, ip, ip, ip]
+    L.liliom_features_download.argtypes = [vp, vp, C.c_int, ip, vp, C.c_int, ip, vp, C.c_int, ip]
     L.liliom_point_stride.argtypes = [vp]
     L.liliom_map_set_cloud.argtypes = [vp, vp, C.c_int, C.c_int]
     L.liliom_correspond_surf_refl.argtypes = [vp, vp, C.c_int, dp, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, vp, vp, vp]
@@ -476,6 +479,17 @@ class Context:
         ns, ne, nc = C.c_int(), C.c_int(), C.c_int()
         self._check(lib().liliom_extract_resident(self._h, _dptr(q), _dptr(ql), C.byref(ns), C.byref(ne), C.byref(nc)))
         return ns.value, ne.value, nc.value
+
+    def features_download(self):
+        """The (surf, edge, cut) clouds the last extraction on this context left resident (liliom_features_download), as
+        extract_horizon / extract_rot would have returned them."""
+        ns, ne, nc = C.c_int(), C.c_int(), C.c_int()
+        self._check(lib().liliom_features_download(self._h, None, 0, C.byref(ns), None, 0, C.byref(ne), None, 0, C.byref(nc)))
+        surf = np.empty(max(ns.value, 1), self.dtype); edge = np.empty(max(ne.value, 1), self.dtype)
+        cut = np.empty(max(nc.value, 1), self.dtype)
+        self._check(lib().liliom_features_download(self._h, _ptr(surf), len(surf), C.byref(ns), _ptr(edge), len(edge), C.byref(ne),
+                                                   _ptr(cut), len(cut), C.byref(nc)))
+        return surf[:ns.value], edge[:ne.value], cut[:nc.value]
 
     def find_surf_corr(self, feats: np.ndarray, pose7):
         f, stride = self._feats(feats)
@@ -850,6 +864,28 @@ def odometry_resident_batch_ex(ctxs, poses7, match_cnt, max_num_iter=15, mode: i
         raise LiliomError(rc)
     ds = [bufs[i][:nds[i]] for i in range(B)] if want_ds else nds[:B].copy()
     return poses[:B], status[:B], _batch_ex_stats(st, cnt, B), ds
+
+
+def extract_resident_batch(ctxs, q_imu, q_lb=None):
+    """extract_resident of every context in `ctxs` on its resident sweep in one call (liliom_extract_resident_batch): session i
+    gets what ctxs[i].extract_resident(q_imu[i], q_lb[i]) would give it.  q_imu: (B, 4); q_lb: (B, 4) or None (identity).
+    Returns (counts (B, 3) as (n_surf, n_edge, n_cut), status (B,)); a session's own error is its status, a whole-call error
+    raises LiliomError."""
+    B = len(ctxs)
+    handles = (C.c_void_p * max(B, 1))(*[c._h if c is not None else None for c in ctxs])
+    qi = np.ascontiguousarray(q_imu, dtype=np.float64).reshape(-1) if q_imu is not None else None
+    ql = np.ascontiguousarray(q_lb, dtype=np.float64).reshape(-1) if q_lb is not None else None
+    for name, q in (("q_imu", qi), ("q_lb", ql)):
+        if q is not None and len(q) != 4 * B:
+            raise ValueError(f"{name}: expected {4 * B} doubles (B x 4), got {len(q)}")
+    counts = np.zeros((max(B, 1), 3), np.int32)
+    ns, ne, nc = (np.ascontiguousarray(counts[:, k]) for k in range(3))
+    status = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_extract_resident_batch(handles, B, _dptr(qi) if qi is not None else None, _dptr(ql) if ql is not None else None,
+                                            _ip(ns), _ip(ne), _ip(nc), _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    return np.stack([ns, ne, nc], axis=1)[:B], status[:B]
 
 
 def comm_get_unique_id() -> bytes:

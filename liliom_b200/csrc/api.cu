@@ -446,6 +446,7 @@ extern "C" int liliom_odometry(liliom_ctx* c, const void* surf_feats, int n, dou
     LILI_CUDA(c, c->surf.ensure((size_t)(n > 0 ? n : 1) * stride));
     if (n > 0) LILI_CUDA(c, cudaMemcpyAsync(c->surf.p, surf_feats, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
     c->n_surf_dev = n;
+    c->feat_ready = false;         // the caller's surf features replace the extracted ones
     return odometry_on_resident_surf(c, pose7, match_cnt, max_num_iter, mode, stats, ds_out, ds_cap, n_ds);
 }
 
@@ -491,6 +492,21 @@ extern "C" int liliom_set_time_source(liliom_ctx* c, int source, const char* fie
     return LILIOM_OK;
 }
 
+// The side channels a ROT extraction of the resident sweep reads under the context's sources: LILIOM_E_ARG when the sweep was
+// not decoded with one of them.
+static int resident_side(const liliom_ctx* c, const uint16_t** rings, const double** times) {
+    const bool field = c->ring_source == LILIOM_RING_FIELD;
+    const bool timed = c->time_source == LILIOM_TIME_FIELD;
+    const lili::Pc2Side& side = c->raw_scan_side;
+    if (field && !side.has_ring) return LILIOM_E_ARG;       // no ring ids decoded with the resident sweep
+    if (timed && !side.has_time) return LILIOM_E_ARG;       // no times decoded with the resident sweep
+    *rings = field ? side.rings() : nullptr;
+    *times = timed ? side.times() : nullptr;
+    return LILIOM_OK;
+}
+
+static const double kIdentityQ[4] = {1, 0, 0, 0};
+
 extern "C" int liliom_extract_resident(liliom_ctx* c, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut) {
     if (!c || !q_imu || !n_surf || !n_edge || !n_cut) return LILIOM_E_ARG;
     LILI_CUDA(c, cudaSetDevice(c->device));
@@ -501,17 +517,83 @@ extern "C" int liliom_extract_resident(liliom_ctx* c, const double q_imu[4], con
     int rc;
     if (stride == 48) rc = horizon_extract_dev(c, n, q_imu, n_surf, n_edge, n_cut, /*sync_counts=*/false);
     else {
-        const double ident[4] = {1, 0, 0, 0};
-        const bool field = c->ring_source == LILIOM_RING_FIELD;
-        const bool timed = c->time_source == LILIOM_TIME_FIELD;
-        const lili::Pc2Side& side = c->raw_scan_side;
-        if (field && !side.has_ring) rc = LILIOM_E_ARG;       // no ring ids decoded with the resident sweep
-        else if (timed && !side.has_time) rc = LILIOM_E_ARG;  // no times decoded with the resident sweep
-        else rc = rot_extract_dev(c, n, q_imu, q_lb ? q_lb : ident, n_surf, n_edge, n_cut, field ? side.rings() : nullptr,
-                                  timed ? side.times() : nullptr);
+        const uint16_t* rings = nullptr;
+        const double* times = nullptr;
+        rc = resident_side(c, &rings, &times);
+        if (rc == LILIOM_OK) rc = rot_extract_dev(c, n, q_imu, q_lb ? q_lb : kIdentityQ, n_surf, n_edge, n_cut, rings, times);
     }
     c->raw_src = nullptr;
     return rc;
+}
+
+// The contexts of a batched call: distinct, single-GPU, on one device.
+static bool batch_ctxs_ok(liliom_ctx* const* ctxs, int B) {
+    if (B < 1 || !ctxs) return false;
+    for (int i = 0; i < B; ++i) {
+        const liliom_ctx* c = ctxs[i];
+        if (!c || c->device != ctxs[0]->device || c->nranks > 1 || c->nccl_comm || c->peer_ready) return false;
+        for (int j = 0; j < i; ++j) if (ctxs[j] == c) return false;
+    }
+    return true;
+}
+
+extern "C" int liliom_extract_resident_batch(liliom_ctx* const* ctxs, int B, const double* q_imu, const double* q_lb, int* n_surf,
+                                             int* n_edge, int* n_cut, int* status) {
+    if (!batch_ctxs_ok(ctxs, B) || !q_imu || !n_surf || !n_edge || !n_cut || !status) return LILIOM_E_ARG;
+    liliom_ctx* c0 = ctxs[0];
+    LILI_CUDA(c0, cudaSetDevice(c0->device));
+    std::vector<HzBatchSession> hz;
+    std::vector<RotBatchSession> rot;
+    std::vector<int> hz_at, rot_at;         // index of each session in ctxs
+    for (int i = 0; i < B; ++i) {
+        liliom_ctx* c = ctxs[i];
+        const int n = c->n_raw_scan;
+        // the extractors only read their input: they take the resident sweep in place
+        if (c->prm.point_stride == 48) {
+            c->raw_src = n > 0 ? c->raw_scan.p : nullptr;
+            hz.push_back(HzBatchSession{c, n, q_imu + 4 * i, n_surf + i, n_edge + i, n_cut + i, LILIOM_OK});
+            hz_at.push_back(i);
+            continue;
+        }
+        RotBatchSession s{c, n, q_imu + 4 * i, q_lb ? q_lb + 4 * i : kIdentityQ, nullptr, nullptr, n_surf + i, n_edge + i, n_cut + i,
+                          LILIOM_OK, false};
+        status[i] = resident_side(c, &s.rings, &s.times);
+        if (status[i] != LILIOM_OK) continue;
+        c->raw_src = n > 0 ? c->raw_scan.p : nullptr;
+        rot.push_back(s);
+        rot_at.push_back(i);
+    }
+    int rc = horizon_batch_queue(c0, hz);
+    if (rc == LILIOM_OK) rc = rot_batch_queue(c0, rot);
+    for (const HzBatchSession& s : hz) s.c->raw_src = nullptr;
+    for (const RotBatchSession& s : rot) s.c->raw_src = nullptr;
+    LILI_TRY(rc);
+    for (size_t k = 0; k < hz.size(); ++k) status[hz_at[k]] = hz[k].status;
+    // one synchronise for the whole call: every session's stream joins ctxs[0]'s
+    for (int i = 0; i < B; ++i) LILI_TRY(batch_join_in(c0, ctxs[i]));
+    LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+    for (size_t k = 0; k < rot.size(); ++k) status[rot_at[k]] = rot[k].pending ? rot_batch_finish(rot[k]) : rot[k].status;
+    return LILIOM_OK;
+}
+
+extern "C" int liliom_features_download(liliom_ctx* c, void* surf, int surf_cap, int* n_surf, void* edge, int edge_cap, int* n_edge,
+                                        void* cut, int cut_cap, int* n_cut) {
+    if (!c || !n_surf || !n_edge || !n_cut) return LILIOM_E_ARG;
+    if (!c->feat_ready) return LILIOM_E_ARG;
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    const int stride = c->prm.point_stride;
+    int m[3] = {c->feat_counts[0], c->feat_counts[1], c->feat_counts[2]};
+    if (m[0] < 0)        // resident Horizon extraction: the counts are on the device
+        LILI_TRY(read_back(c, {{m, c->feat_dcounts, 2 * sizeof(int)}, {m + 2, c->feat_dcut, sizeof(int)}}));
+    *n_surf = m[0]; *n_edge = m[1]; *n_cut = m[2];
+    const DevBuf* src[3] = {&c->surf, &c->edge, stride == 48 ? &c->cut : &c->rot_cloud};
+    void* out[3] = {surf, edge, cut};
+    const int cap[3] = {surf_cap, edge_cap, cut_cap};
+    for (int k = 0; k < 3; ++k) if (out[k] && m[k] > cap[k]) return LILIOM_E_CAPACITY;
+    for (int k = 0; k < 3; ++k)
+        if (out[k] && m[k] > 0) LILI_CUDA(c, cudaMemcpyAsync(out[k], src[k]->p, (size_t)m[k] * stride, cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    return LILIOM_OK;
 }
 
 // liliom_odometry_resident in three parts, shared by the solo and the batched call.
@@ -609,15 +691,11 @@ extern "C" int liliom_odometry_resident(liliom_ctx* c, double pose7[7], int matc
 // The whole-call refusals of the batched steps: nothing is touched when one holds.
 static bool batch_args_ok(liliom_ctx* const* ctxs, int B, const double* poses7, const int* match_cnt, const int* max_num_iter, int mode,
                           const int* status) {
-    if (B < 1 || !ctxs || !poses7 || !status || !match_cnt) return false;
+    if (!batch_ctxs_ok(ctxs, B) || !poses7 || !status || !match_cnt) return false;
     if (mode != LILIOM_MODE_CERES && mode != LILIOM_MODE_GN) return false;
     if (mode == LILIOM_MODE_CERES && !max_num_iter) return false;
-    for (int i = 0; i < B; ++i) {
-        const liliom_ctx* c = ctxs[i];
+    for (int i = 0; i < B; ++i)
         if (match_cnt[i] < 0) return false;
-        if (!c || c->device != ctxs[0]->device || c->nranks > 1 || c->nccl_comm || c->peer_ready) return false;
-        for (int j = 0; j < i; ++j) if (ctxs[j] == c) return false;
-    }
     return true;
 }
 

@@ -125,6 +125,19 @@ struct GnIo {
 };
 
 #ifdef __CUDACC__
+// Where a block sits in its session: blk.bi() of blk.G() blocks.  A solo launch reads blockIdx.x / gridDim.x at each use
+// (the kernels keep the code and registers they had before the batched launch existed); a batched launch (k_gn_batch,
+// k_hz_batch) passes the block's place inside its session's range.
+struct SoloBlock {
+    __device__ __forceinline__ int bi() const { return (int)blockIdx.x; }
+    __device__ __forceinline__ unsigned int G() const { return gridDim.x; }
+};
+struct SessionBlock {
+    int b; unsigned int g;
+    __device__ __forceinline__ int bi() const { return b; }
+    __device__ __forceinline__ unsigned int G() const { return g; }
+};
+
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -221,6 +234,11 @@ struct liliom_ctx {
     lili::Pc2Side raw_side;      // side channels of c->raw (liliom_extract_rot_pc2)
     lili::Pc2Side raw_scan_side; // ... of the resident sweep (liliom_convert_pc2)
     int n_rot_cloud = 0;
+    // the clouds the last extraction left resident (surf, edge and cut / laserCloud; liliom_features_download)
+    bool feat_ready = false;
+    int feat_counts[3] = {0, 0, 0};      // their sizes; -1: only on the device (resident Horizon extraction)
+    int* feat_dcounts = nullptr;         // Horizon: the surf and edge counts on the device, a spare word behind them
+    const int* feat_dcut = nullptr;      // Horizon: the cut count on the device (idx_a[n], or feat_dcounts[2] once idx_a is reused)
 
     // ---- voxel grid scratch ----
     lili::DevBuf vg_keys, vg_keys2, vg_vals, vg_vals2, vg_flags, vg_rank, vg_params, vg_out, vg_minmax, vg_count;
@@ -364,6 +382,15 @@ int download_sized(liliom_ctx* c, const DevBuf& src, int m, size_t elem, void* o
     return LILIOM_OK;
 }
 
+// Before idx_a is reused as scratch: the cut count of a resident Horizon extraction, which sits in it, moves to the spare word
+// behind the surf / edge counts (liliom_features_download reads it there).
+inline int feat_keep_cut(liliom_ctx* c) {
+    if (!c->feat_ready || c->feat_counts[2] >= 0 || c->feat_dcut == c->feat_dcounts + 2) return LILIOM_OK;
+    LILI_CUDA(c, cudaMemcpyAsync(c->feat_dcounts + 2, c->feat_dcut, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
+    c->feat_dcut = c->feat_dcounts + 2;
+    return LILIOM_OK;
+}
+
 // ---- modules (implemented in the .cu files) ----
 int sort_pairs_u32(liliom_ctx* c, const uint32_t* kin, uint32_t* kout, const int* vin, int* vout, int n, int end_bit);
 int sort_pairs_u64(liliom_ctx* c, const unsigned long long* kin, unsigned long long* kout, const int* vin, int* vout, int n, int end_bit);
@@ -397,12 +424,52 @@ int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int
 int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, const int* match_cnt, const int* max_num_iter, int mode,
               liliom_iter_stats* const* stats, int* status);
 
+// A batched call's shared launches run on ctxs[0]'s stream (c0): every other session's stream (its work so far) is ordered
+// before them ...
+inline int batch_join_in(liliom_ctx* c0, liliom_ctx* c) {
+    if (c->stream == c0->stream) return LILIOM_OK;
+    LILI_CUDA(c, cudaEventRecord(c->ev_batch, c->stream));
+    LILI_CUDA(c0, cudaStreamWaitEvent(c0->stream, c->ev_batch, 0));
+    return LILIOM_OK;
+}
+// ... and after them (c0->ev_batch recorded behind the last shared launch)
+inline int batch_join_out(liliom_ctx* c0, liliom_ctx* c) {
+    if (c->stream != c0->stream) LILI_CUDA(c, cudaStreamWaitEvent(c->stream, c0->ev_batch, 0));
+    return LILIOM_OK;
+}
+
 int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf, int* n_edge, int* n_cut, bool sync_counts = true);
+// One Horizon session of liliom_extract_resident_batch (n points of the resident sweep): horizon_batch_queue queues every session
+// (status: its error, or LILIOM_OK; counts -1, as the solo resident call) and returns a whole-call CUDA error.
+struct HzBatchSession {
+    liliom_ctx* c;
+    int n;
+    const double* q_imu;
+    int* n_surf; int* n_edge; int* n_cut;
+    int status;
+};
+int horizon_batch_queue(liliom_ctx* c0, std::vector<HzBatchSession>& ss);
 // rings: nullptr = scanID from the elevation tables (line_num 16/32/64), else the u16 ring id of every input point (line_num 1..128)
 // times: nullptr = relTime from the azimuth rule, else the time of every input point (LILIOM_TIME_FIELD)
 int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut,
                     const uint16_t* rings = nullptr, const double* times = nullptr);
 bool rot_lines_ok(int line_num, bool field);
+// One ROT session of liliom_extract_resident_batch: what its solo rot_extract_dev call takes (n points of the resident sweep).
+// rot_batch_queue queues every session (status: its error, or LILIOM_OK; pending: read-back words queued on its stream); after
+// one synchronise of every session's stream, rot_batch_finish completes each pending session as its solo call would.
+struct RotBatchSession {
+    liliom_ctx* c;
+    int n;
+    const double* q_imu;
+    const double* q_lb;
+    const uint16_t* rings;
+    const double* times;
+    int* n_surf; int* n_edge; int* n_cut;
+    int status;
+    bool pending;
+};
+int rot_batch_queue(liliom_ctx* c0, std::vector<RotBatchSession>& ss);   // returns a whole-call CUDA error
+int rot_batch_finish(RotBatchSession& s);
 
 int icp_align(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,
               double fit_eps, double T16[16], double* fitness, int* converged, int* iters);     // icp.cu

@@ -13,6 +13,8 @@
 // non-FMA x86-64 build, so labels and feature indices are bit-exact against the oracle.
 #include "ctx.cuh"
 #include "dev_math.cuh"
+#include "s2m_plan.h"
+#include <algorithm>
 #include <climits>
 
 namespace lili {
@@ -387,16 +389,21 @@ __device__ __forceinline__ void hz_grid_barrier(unsigned int* bar, unsigned int 
     __syncthreads();
 }
 
-__global__ void __launch_bounds__(HZC_THREADS) k_hz_coop(const Pt48* __restrict__ pts, int n, Q4 q_imu, double surf_thres, double edge_thres,
-                                                         Pt48* __restrict__ cut, int* __restrict__ mat, int* __restrict__ blockcnt,
-                                                         int* __restrict__ counts, int* __restrict__ totals, int* __restrict__ ncut_out,
-                                                         Pt48* __restrict__ surf, Pt48* __restrict__ edge, unsigned int* __restrict__ ctl,
-                                                         unsigned int call) {
+// The body of k_hz_coop for the block at blk: blk.bi() of the blk.G() blocks of its session (SoloBlock: the whole grid).
+// A session's output does not depend on G: a kept point's place in the cutted cloud is the count of kept points before it
+// (the preceding blocks' counts plus the in-block prefix), and stage C gives each patch its own warp for any G with
+// G * HZC_WARPS >= HZ_PATCHES, so every G >= 83 writes the bytes of the solo launch.
+template <class Blk>
+__device__ __forceinline__ void hz_coop_body(const Pt48* __restrict__ pts, int n, Q4 q_imu, double surf_thres, double edge_thres,
+                                             Pt48* __restrict__ cut, int* __restrict__ mat, int* __restrict__ blockcnt,
+                                             int* __restrict__ counts, int* __restrict__ totals, int* __restrict__ ncut_out,
+                                             Pt48* __restrict__ surf, Pt48* __restrict__ edge, unsigned int* __restrict__ ctl,
+                                             unsigned int call, const Blk blk) {
     __shared__ HzPatchSmem sm[HZC_WARPS];
     __shared__ int wsum[HZC_WARPS];
     __shared__ int s_bpre;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int G = gridDim.x, b = blockIdx.x;
+    const int G = (int)blk.G(), b = blk.bi();
     // bit 31 of `call` (LILIOM_DEBUG_TIMING): block 0 leaves clock64 stamps of the stage boundaries in the spare control words
     long long* stamp = ((call >> 31) != 0u && b == 0 && tid == 0) ? reinterpret_cast<long long*>(ctl + 4) : nullptr;
     call &= 0x7fffffffu;
@@ -462,9 +469,50 @@ __global__ void __launch_bounds__(HZC_THREADS) k_hz_coop(const Pt48* __restrict_
     if (stamp) { stamp[4] = clock64(); stamp[11] = (long long)globaltimer_ns(); }
 }
 
-// raw points must already be in c->raw (n x 48 B).  Leaves cut/surf/edge on the device and the
-// three counts in pinned host memory (returned through the pointers after a stream sync).
-int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf, int* n_edge, int* n_cut, bool sync_counts) {
+__global__ void __launch_bounds__(HZC_THREADS) k_hz_coop(const Pt48* __restrict__ pts, int n, Q4 q_imu, double surf_thres, double edge_thres,
+                                                         Pt48* __restrict__ cut, int* __restrict__ mat, int* __restrict__ blockcnt,
+                                                         int* __restrict__ counts, int* __restrict__ totals, int* __restrict__ ncut_out,
+                                                         Pt48* __restrict__ surf, Pt48* __restrict__ edge, unsigned int* __restrict__ ctl,
+                                                         unsigned int call) {
+    hz_coop_body(pts, n, q_imu, surf_thres, edge_thres, cut, mat, blockcnt, counts, totals, ncut_out, surf, edge, ctl, call, SoloBlock{});
+}
+
+// Several sessions' extractions in one cooperative launch (liliom_extract_resident_batch): session s owns blocks
+// [off[s], off[s + 1]) and meets only at its own barrier word.  The entries are k_hz_coop's parameters; `call` never carries
+// the LILIOM_DEBUG_TIMING bit here.
+struct HzBatchEntry {
+    const Pt48* pts; int n; Q4 q_imu; double surf_thres, edge_thres;
+    Pt48* cut; int* mat; int* blockcnt; int* counts; int* totals; int* ncut_out; Pt48* surf; Pt48* edge; unsigned int* ctl;
+    unsigned int call;
+};
+struct HzBatch {
+    int n;                              // sessions in this launch
+    int off[kBatchMax + 1];
+    HzBatchEntry s[kBatchMax];
+};
+static_assert(sizeof(HzBatch) <= 32764, "k_hz_batch's session table must fit in the kernel parameter space");
+
+__global__ void __launch_bounds__(HZC_THREADS, 3) k_hz_batch(const __grid_constant__ HzBatch tab) {
+    int s = 0;
+    while (s + 1 < tab.n && (int)blockIdx.x >= tab.off[s + 1]) ++s;
+    const HzBatchEntry e = tab.s[s];    // a by-value copy, as k_hz_coop's parameters
+    hz_coop_body(e.pts, e.n, e.q_imu, e.surf_thres, e.edge_thres, e.cut, e.mat, e.blockcnt, e.counts, e.totals, e.ncut_out, e.surf,
+                 e.edge, e.ctl, e.call, SessionBlock{(int)blockIdx.x - tab.off[s], (unsigned int)(tab.off[s + 1] - tab.off[s])});
+}
+
+// horizon_extract_dev in parts, shared with the batch (horizon_batch_queue): hz_begin sizes the buffers and decides whether the
+// sweep takes the cooperative launch, hz_coop_entry gives that launch's parameters, hz_chain queues the multi-launch chain, and
+// hz_end records what the extraction left resident.
+struct HzJob {
+    liliom_ctx* c = nullptr;
+    int n = 0;
+    Q4 q{};
+    const Pt48* raw = nullptr;
+    bool coop = false;
+};
+
+static int hz_begin(liliom_ctx* c, int n, const double q_imu[4], HzJob& j) {
+    c->feat_ready = false;
     const size_t npts = (size_t)(n > 0 ? n : 1);
     LILI_CUDA(c, c->cut.ensure(npts * sizeof(Pt48)));
     LILI_CUDA(c, c->surf.ensure((size_t)HZ_PATCHES * 36 * sizeof(Pt48)));
@@ -475,72 +523,173 @@ int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf
     LILI_CUDA(c, c->hz_stage_surf.ensure((size_t)HZ_PATCHES * 36 * sizeof(Pt48)));
     LILI_CUDA(c, c->hz_stage_edge.ensure((size_t)HZ_PATCHES * 6 * sizeof(Pt48)));
     LILI_CUDA(c, c->hz_counts.ensure((size_t)(4 * (HZ_PATCHES + 1) + 8) * sizeof(int)));
-    Q4 q{q_imu[0], q_imu[1], q_imu[2], q_imu[3]};
-    if (std::isnan(q.w) || std::isnan(q.x) || std::isnan(q.y) || std::isnan(q.z)) q = Q4{1, 0, 0, 0};   // :232-234
-    const Pt48* raw = c->raw_src ? reinterpret_cast<const Pt48*>(c->raw_src) : c->raw.as<Pt48>();   // read-only input
+    j = HzJob{};
+    j.c = c;
+    j.n = n;
+    j.q = Q4{q_imu[0], q_imu[1], q_imu[2], q_imu[3]};
+    if (std::isnan(j.q.w) || std::isnan(j.q.x) || std::isnan(j.q.y) || std::isnan(j.q.z)) j.q = Q4{1, 0, 0, 0};   // :232-234
+    j.raw = c->raw_src ? reinterpret_cast<const Pt48*>(c->raw_src) : c->raw.as<Pt48>();   // read-only input
+    j.coop = !c->hz_chain && c->sm_count * HZC_WARPS >= HZ_PATCHES && n > 0;
+    if (j.coop && !c->hz_ctl.p) {
+        // scratch of the cooperative launch: per-block counts behind the patch counts, barrier words in their own buffer
+        LILI_CUDA(c, c->hz_ctl.ensure(128 + (size_t)c->sm_count * sizeof(int)));
+        LILI_CUDA(c, cudaMemsetAsync(c->hz_ctl.p, 0, c->hz_ctl.cap, c->stream));
+        c->hz_coop_calls = 0;
+    }
+    return LILIOM_OK;
+}
+
+// The parameters of the session's cooperative launch; the caller advances hz_coop_calls once it is launched
+static HzBatchEntry hz_coop_entry(const HzJob& j, bool stamps) {
+    liliom_ctx* c = j.c;
+    int* counts = c->hz_counts.as<int>();
+    return HzBatchEntry{j.raw, j.n, j.q, c->prm.surf_thres, c->prm.edge_thres, c->cut.as<Pt48>(), c->hz_mat.as<int>(),
+                        reinterpret_cast<int*>(c->hz_ctl.as<unsigned char>() + 128), counts, counts + 4 * (HZ_PATCHES + 1),
+                        c->idx_a.as<int>() + j.n, c->surf.as<Pt48>(), c->edge.as<Pt48>(), c->hz_ctl.as<unsigned int>(),
+                        (c->hz_coop_calls & 0x7fffffffu) | (stamps ? 0x80000000u : 0u)};
+}
+
+static int hz_coop_solo(const HzJob& j) {
+    liliom_ctx* c = j.c;
+    HzBatchEntry e = hz_coop_entry(j, c->dbg_timing);
+    void* kargs[] = {&e.pts, &e.n, &e.q_imu, &e.surf_thres, &e.edge_thres, &e.cut, &e.mat, &e.blockcnt, &e.counts, &e.totals, &e.ncut_out,
+                     &e.surf, &e.edge, &e.ctl, &e.call};
+    LILI_CUDA(c, cudaLaunchCooperativeKernel((const void*)k_hz_coop, dim3(c->sm_count), dim3(HZC_THREADS), kargs, 0, c->stream));
+    LILI_TRY(launch_check(c, "k_hz_coop"));
+    c->hz_coop_calls++;
+    return LILIOM_OK;
+}
+
+static int hz_chain(const HzJob& j) {
+    liliom_ctx* c = j.c;
+    const int n = j.n;
+    const Pt48* raw = j.raw;
     int* flags = c->flags.as<int>();
     int* cidx = c->idx_a.as<int>();
     int* mat = c->hz_mat.as<int>();
     int* counts = c->hz_counts.as<int>();
     int* offs = counts + 2 * (HZ_PATCHES + 1);
     int* totals = counts + 4 * (HZ_PATCHES + 1);
-    const bool coop = !c->hz_chain && c->sm_count * HZC_WARPS >= HZ_PATCHES && n > 0;
-    if (coop) {
-        // one cooperative launch; scratch: per-block counts behind the patch counts, barrier words in their own buffer
-        if (!c->hz_ctl.p) {
-            LILI_CUDA(c, c->hz_ctl.ensure(128 + (size_t)c->sm_count * sizeof(int)));
-            LILI_CUDA(c, cudaMemsetAsync(c->hz_ctl.p, 0, c->hz_ctl.cap, c->stream));
-            c->hz_coop_calls = 0;
+    k_hz_flags<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(raw, n, flags);
+    LILI_TRY(launch_check(c, "k_hz_flags"));
+    LILI_TRY(exclusive_scan_i32(c, flags, cidx, n));
+    k_hz_fill<<<cdiv(HZ_LINES * HZ_COLS, 256), 256, 0, c->stream>>>(mat, HZ_LINES * HZ_COLS, HZ_EMPTY);
+    LILI_TRY(launch_check(c, "k_hz_fill"));
+    if (n > 0) {
+        k_hz_deskew_bin<<<cdiv(n, 128), 128, 0, c->stream>>>(raw, n, flags, cidx, j.q, c->cut.as<Pt48>(), mat);
+        LILI_TRY(launch_check(c, "k_hz_deskew_bin"));
+        if (c->early_cut_dst && c->early_cut_cap >= n) {      // only when no count can overflow the caller's buffer: an error return leaves it untouched
+            const size_t cnt = (size_t)min(n, c->early_cut_cap);
+            LILI_CUDA(c, cudaEventRecord(c->ev_ready, c->stream));
+            LILI_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->ev_ready, 0));
+            LILI_CUDA(c, cudaMemcpyAsync(c->early_cut_dst, c->cut.p, cnt * sizeof(Pt48), cudaMemcpyDeviceToHost, c->copy_stream));
+            LILI_CUDA(c, cudaEventRecord(c->ev_copied, c->copy_stream));
+            c->early_cut_issued = true;
         }
-        unsigned int* ctl = c->hz_ctl.as<unsigned int>();
-        int* blockcnt = reinterpret_cast<int*>(c->hz_ctl.as<unsigned char>() + 128);
-        int* ncut_out = cidx + n;
-        const Pt48* raw_c = raw;
-        Pt48* cutp = c->cut.as<Pt48>(); Pt48* surfp = c->surf.as<Pt48>(); Pt48* edgep = c->edge.as<Pt48>();
-        double st = c->prm.surf_thres, et = c->prm.edge_thres;
-        unsigned int call = (c->hz_coop_calls & 0x7fffffffu) | (c->dbg_timing ? 0x80000000u : 0u);
-        void* kargs[] = {&raw_c, &n, &q, &st, &et, &cutp, &mat, &blockcnt, &counts, &totals, &ncut_out, &surfp, &edgep, &ctl, &call};
-        LILI_CUDA(c, cudaLaunchCooperativeKernel((const void*)k_hz_coop, dim3(c->sm_count), dim3(HZC_THREADS), kargs, 0, c->stream));
-        LILI_TRY(launch_check(c, "k_hz_coop"));
-        c->hz_coop_calls++;
-    } else {
-        k_hz_flags<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(raw, n, flags);
-        LILI_TRY(launch_check(c, "k_hz_flags"));
-        LILI_TRY(exclusive_scan_i32(c, flags, cidx, n));
-        k_hz_fill<<<cdiv(HZ_LINES * HZ_COLS, 256), 256, 0, c->stream>>>(mat, HZ_LINES * HZ_COLS, HZ_EMPTY);
-        LILI_TRY(launch_check(c, "k_hz_fill"));
-        if (n > 0) {
-            k_hz_deskew_bin<<<cdiv(n, 128), 128, 0, c->stream>>>(raw, n, flags, cidx, q, c->cut.as<Pt48>(), mat);
-            LILI_TRY(launch_check(c, "k_hz_deskew_bin"));
-            if (c->early_cut_dst && c->early_cut_cap >= n) {      // only when no count can overflow the caller's buffer: an error return leaves it untouched
-                const size_t cnt = (size_t)min(n, c->early_cut_cap);
-                LILI_CUDA(c, cudaEventRecord(c->ev_ready, c->stream));
-                LILI_CUDA(c, cudaStreamWaitEvent(c->copy_stream, c->ev_ready, 0));
-                LILI_CUDA(c, cudaMemcpyAsync(c->early_cut_dst, c->cut.p, cnt * sizeof(Pt48), cudaMemcpyDeviceToHost, c->copy_stream));
-                LILI_CUDA(c, cudaEventRecord(c->ev_copied, c->copy_stream));
-                c->early_cut_issued = true;
-            }
-        }
-        k_hz_patch<<<cdiv(HZ_PATCHES, HZ_WARPS), HZ_WARPS * 32, 0, c->stream>>>(c->cut.as<Pt48>(), mat, c->prm.surf_thres, c->prm.edge_thres,
-                                                                                c->hz_stage_surf.as<Pt48>(), c->hz_stage_edge.as<Pt48>(), counts);
-        LILI_TRY(launch_check(c, "k_hz_patch"));
-        k_hz_offsets<<<1, 1024, 0, c->stream>>>(counts, offs, totals);
-        LILI_TRY(launch_check(c, "k_hz_offsets"));
-        k_hz_emit<<<HZ_PATCHES, 64, 0, c->stream>>>(c->hz_stage_surf.as<Pt48>(), c->hz_stage_edge.as<Pt48>(), counts, offs,
-                                                    c->surf.as<Pt48>(), c->edge.as<Pt48>());
-        LILI_TRY(launch_check(c, "k_hz_emit"));
     }
+    k_hz_patch<<<cdiv(HZ_PATCHES, HZ_WARPS), HZ_WARPS * 32, 0, c->stream>>>(c->cut.as<Pt48>(), mat, c->prm.surf_thres, c->prm.edge_thres,
+                                                                            c->hz_stage_surf.as<Pt48>(), c->hz_stage_edge.as<Pt48>(), counts);
+    LILI_TRY(launch_check(c, "k_hz_patch"));
+    k_hz_offsets<<<1, 1024, 0, c->stream>>>(counts, offs, totals);
+    LILI_TRY(launch_check(c, "k_hz_offsets"));
+    k_hz_emit<<<HZ_PATCHES, 64, 0, c->stream>>>(c->hz_stage_surf.as<Pt48>(), c->hz_stage_edge.as<Pt48>(), counts, offs,
+                                                c->surf.as<Pt48>(), c->edge.as<Pt48>());
+    LILI_TRY(launch_check(c, "k_hz_emit"));
+    return LILIOM_OK;
+}
+
+static int hz_end(const HzJob& j, bool sync_counts, int* n_surf, int* n_edge, int* n_cut) {
+    liliom_ctx* c = j.c;
+    const int n = j.n;
+    int* totals = c->hz_counts.as<int>() + 4 * (HZ_PATCHES + 1);
     c->d_nsurf = totals;
     c->n_surf_max = min(n, HZ_PATCHES * 36);
+    c->feat_dcounts = totals;
+    c->feat_dcut = c->idx_a.as<int>() + n;
     if (!sync_counts) {          // resident pipeline: the counts stay on the device, no host round trip
         c->n_surf_dev = -1;
         *n_surf = *n_edge = *n_cut = -1;
+        c->feat_counts[0] = c->feat_counts[1] = c->feat_counts[2] = -1;
+        c->feat_ready = true;
         return LILIOM_OK;
     }
     int hp[3];
-    LILI_TRY(read_back(c, {{hp, totals, 2 * sizeof(int)}, {hp + 2, cidx + n, sizeof(int)}}));
+    LILI_TRY(read_back(c, {{hp, totals, 2 * sizeof(int)}, {hp + 2, c->idx_a.as<int>() + n, sizeof(int)}}));
     *n_surf = hp[0]; *n_edge = hp[1]; *n_cut = hp[2];
     c->n_surf_dev = hp[0];
+    for (int k = 0; k < 3; ++k) c->feat_counts[k] = hp[k];
+    c->feat_ready = true;
+    return LILIOM_OK;
+}
+
+// raw points must already be in c->raw (n x 48 B).  Leaves cut/surf/edge on the device and the
+// three counts in pinned host memory (returned through the pointers after a stream sync).
+int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf, int* n_edge, int* n_cut, bool sync_counts) {
+    HzJob j;
+    LILI_TRY(hz_begin(c, n, q_imu, j));
+    LILI_TRY(j.coop ? hz_coop_solo(j) : hz_chain(j));
+    return hz_end(j, sync_counts, n_surf, n_edge, n_cut);
+}
+
+// The Horizon sessions of liliom_extract_resident_batch.  Sessions whose solo call takes k_hz_coop share cooperative k_hz_batch
+// launches on c0's stream, kHzBatchGrid blocks each, packed by s2m_batch_pack (first-fit, in call order) into launches whose
+// summed grid is co-resident; each keeps its own barrier word and call sequence.  The others (LILIOM_HZ_CHAIN, empty sweeps),
+// and every session when no shared launch fits, take their solo path on their own stream.  The counts stay on the device, as in
+// the solo resident call.
+constexpr int kHzBatchGrid = (HZ_PATCHES + HZC_WARPS - 1) / HZC_WARPS;     // stage C: one warp per patch
+
+int horizon_batch_queue(liliom_ctx* c0, std::vector<HzBatchSession>& ss) {
+    std::vector<HzJob> jobs(ss.size());
+    std::vector<int> coop;                  // sessions that take k_hz_coop alone
+    std::vector<S2mPlan> plans;
+    for (size_t k = 0; k < ss.size(); ++k) {
+        HzBatchSession& s = ss[k];
+        s.status = hz_begin(s.c, s.n, s.q_imu, jobs[k]);
+        if (s.status != LILIOM_OK) continue;
+        if (jobs[k].coop) {
+            S2mPlan p{};
+            p.persistent = true; p.lanes = 1; p.grid = kHzBatchGrid;
+            plans.push_back(p);
+            coop.push_back((int)k);
+            continue;
+        }
+        s.status = hz_chain(jobs[k]);
+        if (s.status == LILIOM_OK) s.status = hz_end(jobs[k], false, s.n_surf, s.n_edge, s.n_cut);
+    }
+    if (coop.empty()) return LILIOM_OK;
+    int occ = 0;
+    LILI_CUDA(c0, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_hz_batch, HZC_THREADS, 0));
+    int occs[kGnKinds];
+    std::fill(occs, occs + kGnKinds, occ);
+    const S2mPack pack = s2m_batch_pack(plans, occs, c0->sm_count);
+    for (int j : pack.solo) {
+        HzBatchSession& s = ss[coop[j]];
+        s.status = hz_coop_solo(jobs[coop[j]]);
+        if (s.status == LILIOM_OK) s.status = hz_end(jobs[coop[j]], false, s.n_surf, s.n_edge, s.n_cut);
+    }
+    if (pack.launches.empty()) return LILIOM_OK;
+    for (const S2mLaunch& l : pack.launches)
+        for (int j : l.sessions) LILI_TRY(batch_join_in(c0, ss[coop[j]].c));
+    for (const S2mLaunch& l : pack.launches) {
+        HzBatch tab{};
+        tab.n = (int)l.sessions.size();
+        for (int m = 0; m < tab.n; ++m) {
+            tab.off[m + 1] = tab.off[m] + kHzBatchGrid;
+            tab.s[m] = hz_coop_entry(jobs[coop[l.sessions[m]]], false);
+        }
+        void* kargs[] = {&tab};
+        LILI_CUDA(c0, cudaLaunchCooperativeKernel((const void*)k_hz_batch, dim3(l.grid), dim3(HZC_THREADS), kargs, 0, c0->stream));
+        LILI_CUDA(c0, cudaGetLastError());
+        for (int j : l.sessions) {
+            HzBatchSession& s = ss[coop[j]];
+            s.c->cnt.launches++;
+            s.c->hz_coop_calls++;
+            s.status = hz_end(jobs[coop[j]], false, s.n_surf, s.n_edge, s.n_cut);
+        }
+    }
+    LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, c0->stream));
+    for (const S2mLaunch& l : pack.launches)
+        for (int j : l.sessions) LILI_TRY(batch_join_out(c0, ss[coop[j]].c));
     return LILIOM_OK;
 }
 

@@ -25,6 +25,7 @@
 #include "dev_math.cuh"
 #include "detmath.h"
 #include "pc2_fields.h"
+#include "s2m_plan.h"
 #include <climits>
 #include <cstdlib>
 #include <cstdint>
@@ -62,10 +63,13 @@ bool rot_lines_ok(int line_num, bool field) {
     return field ? (line_num >= 1 && line_num <= ROT_MAX_RINGS) : (line_num == 16 || line_num == 32 || line_num == 64);
 }
 
-__global__ void k_rot_meta_init(int* meta) {
+__device__ __forceinline__ void rot_meta_init_body(int* meta, const int bx) {
     // t_min key starts at ~0 (both words -1), t_max key at 0
     for (int t = threadIdx.x; t < M_SIZE; t += blockDim.x)
         meta[t] = (t == M_LAST || t == M_TMIN || t == M_TMIN + 1) ? -1 : (t == M_FIRST || t == M_HP) ? INT_MAX : 0;
+}
+__global__ void k_rot_meta_init(int* meta) {
+    rot_meta_init_body(meta, (int)blockIdx.x);
 }
 
 __device__ __forceinline__ bool rot_keep(float4 a) {
@@ -100,10 +104,10 @@ __device__ __forceinline__ int rot_table_scan_id(float4 a, int n_scans) {
 // block on the order keys.  The azimuth instantiation is the kernel as it was without a time source.
 constexpr int ROT_PRE_THREADS = 256;
 template <bool kTimed>
-__global__ void __launch_bounds__(ROT_PRE_THREADS) k_rot_pre(const Pt32* __restrict__ pts, const uint16_t* __restrict__ rings,
+__device__ __forceinline__ void rot_pre_body(const Pt32* __restrict__ pts, const uint16_t* __restrict__ rings,
                                                              const double* __restrict__ times, int n, int n_scans, uint32_t* __restrict__ keys,
-                                                             int* __restrict__ vals, float* __restrict__ ori, int* __restrict__ meta) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+                                                             int* __restrict__ vals, float* __restrict__ ori, int* __restrict__ meta, const int bx) {
+    const int i = bx * blockDim.x + threadIdx.x;
     if (!kTimed && i >= n) return;
     unsigned long long kmin = ~0ull, kmax = 0ull;
     if (i < n) {
@@ -141,6 +145,12 @@ __global__ void __launch_bounds__(ROT_PRE_THREADS) k_rot_pre(const Pt32* __restr
         }
     }
 }
+template <bool kTimed>
+__global__ void __launch_bounds__(ROT_PRE_THREADS) k_rot_pre(const Pt32* __restrict__ pts, const uint16_t* __restrict__ rings,
+                                                             const double* __restrict__ times, int n, int n_scans, uint32_t* __restrict__ keys,
+                                                             int* __restrict__ vals, float* __restrict__ ori, int* __restrict__ meta) {
+    rot_pre_body<kTimed>(pts, rings, times, n, n_scans, keys, vals, ori, meta, (int)blockIdx.x);
+}
 
 __device__ __forceinline__ void rot_start_end(const Pt32* __restrict__ pts, const int* __restrict__ meta, float& startOri, float& endOri) {
     float4 f = pts[meta[M_FIRST]].a, l = pts[meta[M_LAST]].a;
@@ -151,9 +161,9 @@ __device__ __forceinline__ void rot_start_end(const Pt32* __restrict__ pts, cons
 }
 
 // un-latched branch of :350-358 for every valid point; the latch fires at the smallest such index
-__global__ void k_rot_hp(const Pt32* __restrict__ pts, int n, const uint32_t* __restrict__ keys, const float* __restrict__ ori_raw,
-                         int* __restrict__ meta) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void rot_hp_body(const Pt32* __restrict__ pts, int n, const uint32_t* __restrict__ keys, const float* __restrict__ ori_raw,
+                         int* __restrict__ meta, const int bx) {
+    int i = bx * blockDim.x + threadIdx.x;
     if (i >= n || keys[i] == 255u) return;
     if (meta[M_FIRST] == INT_MAX) return;
     float startOri, endOri;
@@ -163,13 +173,17 @@ __global__ void k_rot_hp(const Pt32* __restrict__ pts, int n, const uint32_t* __
     else if ((double)ori > (double)startOri + ROT_PI * 3 / 2) ori = (float)((double)ori - 2 * ROT_PI);
     if ((double)(ori - startOri) > ROT_PI) atomicMin(&meta[M_HP], i);
 }
+__global__ void k_rot_hp(const Pt32* __restrict__ pts, int n, const uint32_t* __restrict__ keys, const float* __restrict__ ori_raw,
+                         int* __restrict__ meta) {
+    rot_hp_body(pts, n, keys, ori_raw, meta, (int)blockIdx.x);
+}
 
 // kTimed: relTime from the point's time over [t_min, t_max] (pc2_rel_time); else from the azimuth rule (:350-367)
 template <bool kTimed>
-__global__ void k_rot_build(const Pt32* __restrict__ pts, int n, const uint32_t* __restrict__ skeys, const int* __restrict__ svals,
+__device__ __forceinline__ void rot_build_body(const Pt32* __restrict__ pts, int n, const uint32_t* __restrict__ skeys, const int* __restrict__ svals,
                             const float* __restrict__ ori_raw, const double* __restrict__ times, Q4 qIMU, Q4 q_lb, Pt32* __restrict__ cloud,
-                            int* __restrict__ meta) {
-    int s = blockIdx.x * blockDim.x + threadIdx.x;
+                            int* __restrict__ meta, const int bx) {
+    int s = bx * blockDim.x + threadIdx.x;
     if (s >= n) return;
     const uint32_t key = skeys[s];
     const uint32_t prev = s > 0 ? skeys[s - 1] : 0xffffffffu;
@@ -215,10 +229,16 @@ __global__ void k_rot_build(const Pt32* __restrict__ pts, int n, const uint32_t*
     o.b = make_float4(intensity, 0.f, 0.f, 0.f);
     cloud[s] = o;
 }
+template <bool kTimed>
+__global__ void k_rot_build(const Pt32* __restrict__ pts, int n, const uint32_t* __restrict__ skeys, const int* __restrict__ svals,
+                            const float* __restrict__ ori_raw, const double* __restrict__ times, Q4 qIMU, Q4 q_lb, Pt32* __restrict__ cloud,
+                            int* __restrict__ meta) {
+    rot_build_body<kTimed>(pts, n, skeys, svals, ori_raw, times, qIMU, q_lb, cloud, meta, (int)blockIdx.x);
+}
 
-__global__ void k_rot_curv(const Pt32* __restrict__ cloud, const int* __restrict__ meta, float* __restrict__ curv, int* __restrict__ label,
-                           int* __restrict__ lessflat, int n_alloc) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void rot_curv_body(const Pt32* __restrict__ cloud, const int* __restrict__ meta, float* __restrict__ curv, int* __restrict__ label,
+                           int* __restrict__ lessflat, int n_alloc, const int bx) {
+    int i = bx * blockDim.x + threadIdx.x;
     if (i > n_alloc) return;
     const int cloudSize = meta[M_NVALID];
     float c = 0.f;
@@ -232,6 +252,10 @@ __global__ void k_rot_curv(const Pt32* __restrict__ cloud, const int* __restrict
     }
     if (i < n_alloc) { curv[i] = c; label[i] = 0; }
     lessflat[i] = 0;   // includes the scan sentinel at n_alloc
+}
+__global__ void k_rot_curv(const Pt32* __restrict__ cloud, const int* __restrict__ meta, float* __restrict__ curv, int* __restrict__ label,
+                           int* __restrict__ lessflat, int n_alloc) {
+    rot_curv_body(cloud, meta, curv, label, lessflat, n_alloc, (int)blockIdx.x);
 }
 
 // dynamic shared memory of k_rot_ring
@@ -249,14 +273,15 @@ struct RingSmem {
     unsigned int availS[32], availF[32];       // by rank: still-unpicked sharp / flat candidates
 };
 
-__global__ void __launch_bounds__(512) k_rot_ring(const Pt32* __restrict__ cloud, const float* __restrict__ curv, int* __restrict__ meta,
-                                                  int ds_rate, int* __restrict__ label, int* __restrict__ lessflat,
-                                                  int* __restrict__ seg_edge /* [rings*6][10] */, int* __restrict__ seg_cnt /* [rings*6] */,
-                                                  long long* __restrict__ dbg /* LILIOM_DEBUG_TIMING: [rings][8] cycles */,
-                                                  int fast_cap /* ROT_FAST_CAP; 0 (LILIOM_ROT_SLOW_WALK, tests): every segment takes the general path */) {
+// One ring of one sweep: the body of k_rot_ring (ring = blockIdx.x) and of k_rot_ring_batch (ring = the block's place in its session).
+__device__ __forceinline__ void rot_ring_body(const Pt32* __restrict__ cloud, const float* __restrict__ curv, int* __restrict__ meta,
+                                              int ds_rate, int* __restrict__ label, int* __restrict__ lessflat,
+                                              int* __restrict__ seg_edge /* [rings*6][10] */, int* __restrict__ seg_cnt /* [rings*6] */,
+                                              long long* __restrict__ dbg /* LILIOM_DEBUG_TIMING: [rings][8] cycles */,
+                                              int fast_cap /* ROT_FAST_CAP; 0 (LILIOM_ROT_SLOW_WALK, tests): every segment takes the general path */,
+                                              const int ring) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     RingSmem& S = *reinterpret_cast<RingSmem*>(smem_raw);
-    const int ring = blockIdx.x;
     long long t_all = 0, t_load = 0, t_sort = 0, t_walk = 0, t_flag = 0, t0 = 0;
     const bool tm = dbg != nullptr && threadIdx.x == 0;
     if (tm) { t_all = clock64(); for (int k = 0; k < 7; ++k) dbg[ring * 8 + k] = 0; dbg[ring * 8 + 7] = (long long)globaltimer_ns(); }
@@ -509,23 +534,52 @@ __global__ void __launch_bounds__(512) k_rot_ring(const Pt32* __restrict__ cloud
     }
 }
 
+__global__ void __launch_bounds__(512) k_rot_ring(const Pt32* __restrict__ cloud, const float* __restrict__ curv, int* __restrict__ meta,
+                                                  int ds_rate, int* __restrict__ label, int* __restrict__ lessflat,
+                                                  int* __restrict__ seg_edge, int* __restrict__ seg_cnt, long long* __restrict__ dbg, int fast_cap) {
+    rot_ring_body(cloud, curv, meta, ds_rate, label, lessflat, seg_edge, seg_cnt, dbg, fast_cap, (int)blockIdx.x);
+}
+
+// The rings of several sweeps in one launch (liliom_extract_resident_batch): session s owns blocks [off[s], off[s + 1]), one per
+// ring, and each block runs the body its solo k_rot_ring launch would, on the session's own buffers.  No debug stamps.
+struct RotRingEntry {
+    const Pt32* cloud; const float* curv; int* meta; int* label; int* lessflat; int* seg_edge; int* seg_cnt;
+    int ds_rate, fast_cap;
+};
+struct RotRingBatch {
+    int n;                              // sessions in this launch
+    int off[kBatchMax + 1];
+    RotRingEntry s[kBatchMax];
+};
+static_assert(sizeof(RotRingBatch) <= 32764, "k_rot_ring_batch's session table must fit in the kernel parameter space");
+
+__global__ void __launch_bounds__(512) k_rot_ring_batch(const __grid_constant__ RotRingBatch tab) {
+    int s = 0;
+    while (s + 1 < tab.n && (int)blockIdx.x >= tab.off[s + 1]) ++s;
+    const RotRingEntry e = tab.s[s];    // a by-value copy, as k_rot_ring's parameters
+    rot_ring_body(e.cloud, e.curv, e.meta, e.ds_rate, e.label, e.lessflat, e.seg_edge, e.seg_cnt, nullptr, e.fast_cap, (int)blockIdx.x - tab.off[s]);
+}
+
 // ---- per-ring VoxelGrid(0.6) of the less-flat points, batched over rings
 // ringmm: [ring][8] a box (vg_box.h) per ring, word 7 unused
-__global__ void k_rot_lf_init(int* ringmm) {
-    int t = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void rot_lf_init_body(int* ringmm, const int bx) {
+    int t = bx * blockDim.x + threadIdx.x;
     if (t >= ROT_MAX_RINGS * 8) return;
     ringmm[t] = vg_box_empty(t & 7);
 }
+__global__ void k_rot_lf_init(int* ringmm) {
+    rot_lf_init_body(ringmm, (int)blockIdx.x);
+}
 
-__global__ void k_rot_lf_gather(const Pt32* __restrict__ cloud, const uint32_t* __restrict__ skeys, const int* __restrict__ lessflat,
+__device__ __forceinline__ void rot_lf_gather_body(const Pt32* __restrict__ cloud, const uint32_t* __restrict__ skeys, const int* __restrict__ lessflat,
                                 const int* __restrict__ lfpos, int n, int n_rings, int* __restrict__ lf_src, int* __restrict__ ringmm,
-                                int* __restrict__ meta) {
+                                int* __restrict__ meta, const int bx) {
     // per-ring boxes: block-local in shared memory first (the cloud is ring-major, so a block meets one to three rings), then one
     // set of global atomics per ring the block saw — per-point global atomics on 64 x 7 words cost this kernel 38 us
     __shared__ int s_mm[ROT_MAX_RINGS * 8];
     for (int t = threadIdx.x; t < n_rings * 8; t += blockDim.x) s_mm[t] = vg_box_empty(t & 7);
     __syncthreads();
-    int k = blockIdx.x * blockDim.x + threadIdx.x;
+    int k = bx * blockDim.x + threadIdx.x;
     if (k == 0) meta[M_NLF] = lfpos[n];
     if (k < n && lessflat[k]) {
         lf_src[lfpos[k]] = k;
@@ -543,17 +597,25 @@ __global__ void k_rot_lf_gather(const Pt32* __restrict__ cloud, const uint32_t* 
         vg_box_atomic(&ringmm[t], f, s_mm[t]);
     }
 }
+__global__ void k_rot_lf_gather(const Pt32* __restrict__ cloud, const uint32_t* __restrict__ skeys, const int* __restrict__ lessflat,
+                                const int* __restrict__ lfpos, int n, int n_rings, int* __restrict__ lf_src, int* __restrict__ ringmm,
+                                int* __restrict__ meta) {
+    rot_lf_gather_body(cloud, skeys, lessflat, lfpos, n, n_rings, lf_src, ringmm, meta, (int)blockIdx.x);
+}
 
-__global__ void k_rot_lf_params(const int* __restrict__ ringmm, float leaf, VgParams* __restrict__ prm) {
+__device__ __forceinline__ void rot_lf_params_body(const int* __restrict__ ringmm, float leaf, VgParams* __restrict__ prm, const int bx) {
     int ring = threadIdx.x;
     if (ring >= ROT_MAX_RINGS) return;
     prm[ring] = vg_params(ringmm + ring * 8, leaf);
 }
+__global__ void k_rot_lf_params(const int* __restrict__ ringmm, float leaf, VgParams* __restrict__ prm) {
+    rot_lf_params_body(ringmm, leaf, prm, (int)blockIdx.x);
+}
 
-__global__ void k_rot_lf_keys(const Pt32* __restrict__ cloud, const uint32_t* __restrict__ skeys, const int* __restrict__ lf_src,
+__device__ __forceinline__ void rot_lf_keys_body(const Pt32* __restrict__ cloud, const uint32_t* __restrict__ skeys, const int* __restrict__ lf_src,
                               const int* __restrict__ meta, const VgParams* __restrict__ prm, unsigned long long* __restrict__ keys,
-                              int* __restrict__ vals, int cap) {
-    int t = blockIdx.x * blockDim.x + threadIdx.x;
+                              int* __restrict__ vals, int cap, const int bx) {
+    int t = bx * blockDim.x + threadIdx.x;
     if (t >= cap) return;
     unsigned long long key = ~0ull;
     if (t < meta[M_NLF]) {
@@ -569,23 +631,33 @@ __global__ void k_rot_lf_keys(const Pt32* __restrict__ cloud, const uint32_t* __
     keys[t] = key;
     vals[t] = t;
 }
+__global__ void k_rot_lf_keys(const Pt32* __restrict__ cloud, const uint32_t* __restrict__ skeys, const int* __restrict__ lf_src,
+                              const int* __restrict__ meta, const VgParams* __restrict__ prm, unsigned long long* __restrict__ keys,
+                              int* __restrict__ vals, int cap) {
+    rot_lf_keys_body(cloud, skeys, lf_src, meta, prm, keys, vals, cap, (int)blockIdx.x);
+}
 
-__global__ void k_rot_lf_centroid(const Pt32* __restrict__ cloud, const int* __restrict__ lf_src, const unsigned long long* __restrict__ keys,
+__device__ __forceinline__ void rot_lf_centroid_body(const Pt32* __restrict__ cloud, const int* __restrict__ lf_src, const unsigned long long* __restrict__ keys,
                                   const int* __restrict__ vals, const int* __restrict__ flags, const int* __restrict__ rank,
-                                  const int* __restrict__ meta, int cap, Pt32* __restrict__ out, int* __restrict__ n_out) {
-    int t = blockIdx.x * blockDim.x + threadIdx.x;
+                                  const int* __restrict__ meta, int cap, Pt32* __restrict__ out, int* __restrict__ n_out, const int bx) {
+    int t = bx * blockDim.x + threadIdx.x;
     if (t == 0) *n_out = rank[cap];
     if (t >= cap || !flags[t]) return;
     const VgAcc<32> a = vg_walk<32>(keys, t, meta[M_NLF], [&](int j) { return lf_src[vals[j]]; },
                                     [&](int m) { return reinterpret_cast<const unsigned char*>(cloud + m); });
     vg_write<32>(a.s, a.n, reinterpret_cast<unsigned char*>(out + rank[t]));
 }
+__global__ void k_rot_lf_centroid(const Pt32* __restrict__ cloud, const int* __restrict__ lf_src, const unsigned long long* __restrict__ keys,
+                                  const int* __restrict__ vals, const int* __restrict__ flags, const int* __restrict__ rank,
+                                  const int* __restrict__ meta, int cap, Pt32* __restrict__ out, int* __restrict__ n_out) {
+    rot_lf_centroid_body(cloud, lf_src, keys, vals, flags, rank, meta, cap, out, n_out, (int)blockIdx.x);
+}
 
 // edge output: segment-major, pick order inside the segment (one block, one thread per possible segment: 128*6 = 768)
 constexpr int ROT_EMIT_THREADS = ROT_MAX_RINGS * 6;
-__global__ void __launch_bounds__(ROT_EMIT_THREADS) k_rot_edge_emit(const Pt32* __restrict__ cloud, const int* __restrict__ seg_edge,
+__device__ __forceinline__ void rot_edge_emit_body(const Pt32* __restrict__ cloud, const int* __restrict__ seg_edge,
                                                                     const int* __restrict__ seg_cnt, int nseg, Pt32* __restrict__ edge,
-                                                                    int* __restrict__ meta) {
+                                                                    int* __restrict__ meta, const int bx) {
     constexpr int nwarps = ROT_EMIT_THREADS / 32;
     __shared__ int wsum[nwarps];
     const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
@@ -600,15 +672,47 @@ __global__ void __launch_bounds__(ROT_EMIT_THREADS) k_rot_edge_emit(const Pt32* 
     const int off = inc - v + wsum[warp];
     for (int e = 0; e < v; ++e) edge[off + e] = cloud[seg_edge[t * 10 + e]];
 }
+__global__ void __launch_bounds__(ROT_EMIT_THREADS) k_rot_edge_emit(const Pt32* __restrict__ cloud, const int* __restrict__ seg_edge,
+                                                                    const int* __restrict__ seg_cnt, int nseg, Pt32* __restrict__ edge,
+                                                                    int* __restrict__ meta) {
+    rot_edge_emit_body(cloud, seg_edge, seg_cnt, nseg, edge, meta, (int)blockIdx.x);
+}
 
-int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut,
-                    const uint16_t* rings, const double* times) {
+// rot_extract_dev in parts, shared by the solo call and the batch (rot_batch_queue): rot_begin checks the parameters and sizes the
+// buffers, rot_front queues the stages before k_rot_ring and rot_back those after it (on the context's stream), rot_finish takes
+// the read-back words (meta[0..8) and the surf count).
+struct RotJob {
+    liliom_ctx* c = nullptr;
+    int n = 0;                          // 0: nothing to queue (an empty sweep, or a refusal)
+    Q4 qI{}, qL{};
+    const Pt32* raw = nullptr;
+    const uint16_t* rings = nullptr;
+    const double* times = nullptr;
+};
+
+// The context's ROT scratch, carved as every stage expects it
+struct RotBufs {
+    int* meta; int* ringmm; VgParams* rprm;
+    uint32_t* keys; uint32_t* keys2; int* vals; int* vals2; float* ori; Pt32* cloud; int* seg_edge; int* seg_cnt;
+    explicit RotBufs(liliom_ctx* c)
+        : meta(c->rot_meta.as<int>()), ringmm(meta + M_SIZE), rprm(reinterpret_cast<VgParams*>(ringmm + ROT_MAX_RINGS * 8)),
+          keys(c->rot_keys.as<uint32_t>()), keys2(c->rot_keys2.as<uint32_t>()), vals(c->rot_vals.as<int>()), vals2(c->rot_vals2.as<int>()),
+          ori(c->rot_ring.as<float>()), cloud(c->rot_cloud.as<Pt32>()), seg_edge(c->rot_seg_edge.as<int>()),
+          seg_cnt(seg_edge + ROT_MAX_RINGS * 6 * 10) {}
+};
+
+static int rot_begin(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut,
+                     const uint16_t* rings, const double* times, RotJob& j) {
+    j = RotJob{};
+    j.c = c;
+    c->feat_ready = false;
     const int n_scans = c->prm.line_num;
     if (!rot_lines_ok(n_scans, rings != nullptr)) return LILIOM_E_LINES;
     if (c->prm.ds_rate < 1) return LILIOM_E_ARG;
     *n_surf = *n_edge = *n_cut = 0;
     c->n_surf_dev = 0; c->n_rot_cloud = 0;
-    if (n <= 0) return LILIOM_OK;
+    c->feat_counts[0] = c->feat_counts[1] = c->feat_counts[2] = 0;
+    if (n <= 0) { c->feat_ready = true; return LILIOM_OK; }
     const size_t N = (size_t)n;
     LILI_CUDA(c, c->rot_keys.ensure(N * 8)); LILI_CUDA(c, c->rot_keys2.ensure(N * 8));
     LILI_CUDA(c, c->rot_vals.ensure(N * 4)); LILI_CUDA(c, c->rot_vals2.ensure(N * 4));
@@ -624,45 +728,106 @@ int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_
     LILI_CUDA(c, c->edge.ensure((size_t)ROT_MAX_RINGS * 6 * 10 * sizeof(Pt32)));
     LILI_CUDA(c, c->vg_flags.ensure((N + 2) * 4)); LILI_CUDA(c, c->vg_rank.ensure((N + 2) * 4));
     LILI_CUDA(c, c->vg_count.ensure(16));
+    LILI_CUDA(c, c->idx_b.ensure(N * 4));
 
-    Q4 qI{q_imu[0], q_imu[1], q_imu[2], q_imu[3]};
-    if (std::isnan(qI.w) || std::isnan(qI.x) || std::isnan(qI.y) || std::isnan(qI.z)) qI = Q4{1, 0, 0, 0};   // :299-301
-    Q4 qL{q_lb[0], q_lb[1], q_lb[2], q_lb[3]};
-    const Pt32* raw = c->raw_src ? reinterpret_cast<const Pt32*>(c->raw_src) : c->raw.as<Pt32>();   // read-only input
-    int* meta = c->rot_meta.as<int>();
-    int* ringmm = meta + M_SIZE;
-    VgParams* rprm = reinterpret_cast<VgParams*>(ringmm + ROT_MAX_RINGS * 8);
-    uint32_t* keys = c->rot_keys.as<uint32_t>(); uint32_t* keys2 = c->rot_keys2.as<uint32_t>();
-    int* vals = c->rot_vals.as<int>(); int* vals2 = c->rot_vals2.as<int>();
-    float* ori = c->rot_ring.as<float>();
-    Pt32* cloud = c->rot_cloud.as<Pt32>();
-    int* seg_edge = c->rot_seg_edge.as<int>();
-    int* seg_cnt = seg_edge + ROT_MAX_RINGS * 6 * 10;
+    j.qI = Q4{q_imu[0], q_imu[1], q_imu[2], q_imu[3]};
+    if (std::isnan(j.qI.w) || std::isnan(j.qI.x) || std::isnan(j.qI.y) || std::isnan(j.qI.z)) j.qI = Q4{1, 0, 0, 0};   // :299-301
+    j.qL = Q4{q_lb[0], q_lb[1], q_lb[2], q_lb[3]};
+    j.raw = c->raw_src ? reinterpret_cast<const Pt32*>(c->raw_src) : c->raw.as<Pt32>();   // read-only input
+    j.rings = rings;
+    j.times = times;
+    j.n = n;
+    return LILIOM_OK;
+}
 
-    k_rot_meta_init<<<1, 256, 0, c->stream>>>(meta);
+// k_rot_meta_init .. k_rot_curv
+static int rot_front(const RotJob& j) {
+    liliom_ctx* c = j.c;
+    const int n = j.n, n_scans = c->prm.line_num;
+    const RotBufs b(c);
+    k_rot_meta_init<<<1, 256, 0, c->stream>>>(b.meta);
     LILI_TRY(launch_check(c, "k_rot_meta_init"));
-    if (times) {
-        k_rot_pre<true><<<cdiv(n, ROT_PRE_THREADS), ROT_PRE_THREADS, 0, c->stream>>>(raw, rings, times, n, n_scans, keys, vals, ori, meta);
+    if (j.times) {
+        k_rot_pre<true><<<cdiv(n, ROT_PRE_THREADS), ROT_PRE_THREADS, 0, c->stream>>>(j.raw, j.rings, j.times, n, n_scans, b.keys, b.vals, b.ori, b.meta);
         LILI_TRY(launch_check(c, "k_rot_pre"));
     } else {
-        k_rot_pre<false><<<cdiv(n, ROT_PRE_THREADS), ROT_PRE_THREADS, 0, c->stream>>>(raw, rings, nullptr, n, n_scans, keys, vals, ori, meta);
+        k_rot_pre<false><<<cdiv(n, ROT_PRE_THREADS), ROT_PRE_THREADS, 0, c->stream>>>(j.raw, j.rings, nullptr, n, n_scans, b.keys, b.vals, b.ori, b.meta);
         LILI_TRY(launch_check(c, "k_rot_pre"));
-        k_rot_hp<<<cdiv(n, 256), 256, 0, c->stream>>>(raw, n, keys, ori, meta);     // the halfPassed latch: azimuth rule only
+        k_rot_hp<<<cdiv(n, 256), 256, 0, c->stream>>>(j.raw, n, b.keys, b.ori, b.meta);     // the halfPassed latch: azimuth rule only
         LILI_TRY(launch_check(c, "k_rot_hp"));
     }
-    LILI_TRY(sort_pairs_u32(c, keys, keys2, vals, vals2, n, 8));
-    if (times) k_rot_build<true><<<cdiv(n, 128), 128, 0, c->stream>>>(raw, n, keys2, vals2, ori, times, qI, qL, cloud, meta);
-    else k_rot_build<false><<<cdiv(n, 128), 128, 0, c->stream>>>(raw, n, keys2, vals2, ori, nullptr, qI, qL, cloud, meta);
+    LILI_TRY(sort_pairs_u32(c, b.keys, b.keys2, b.vals, b.vals2, n, 8));
+    if (j.times) k_rot_build<true><<<cdiv(n, 128), 128, 0, c->stream>>>(j.raw, n, b.keys2, b.vals2, b.ori, j.times, j.qI, j.qL, b.cloud, b.meta);
+    else k_rot_build<false><<<cdiv(n, 128), 128, 0, c->stream>>>(j.raw, n, b.keys2, b.vals2, b.ori, nullptr, j.qI, j.qL, b.cloud, b.meta);
     LILI_TRY(launch_check(c, "k_rot_build"));
-    k_rot_curv<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(cloud, meta, c->rot_curv.as<float>(), c->rot_label.as<int>(),
+    k_rot_curv<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(b.cloud, b.meta, c->rot_curv.as<float>(), c->rot_label.as<int>(),
                                                         c->rot_lessflat.as<int>(), n);
     LILI_TRY(launch_check(c, "k_rot_curv"));
+    return LILIOM_OK;
+}
+
+// k_rot_edge_emit .. k_rot_lf_centroid
+static int rot_back(const RotJob& j) {
+    liliom_ctx* c = j.c;
+    const int n = j.n, n_scans = c->prm.line_num;
+    const RotBufs b(c);
+    k_rot_edge_emit<<<1, ROT_EMIT_THREADS, 0, c->stream>>>(b.cloud, b.seg_edge, b.seg_cnt, n_scans * 6, c->edge.as<Pt32>(), b.meta);
+    LILI_TRY(launch_check(c, "k_rot_edge_emit"));
+    // less-flat -> per-ring VoxelGrid
+    int* lfpos = c->rot_sort.as<int>();
+    int* lf_src = c->rot_picked.as<int>();
+    LILI_TRY(exclusive_scan_i32(c, c->rot_lessflat.as<int>(), lfpos, n));
+    k_rot_lf_init<<<cdiv(ROT_MAX_RINGS * 8, 256), 256, 0, c->stream>>>(b.ringmm);
+    LILI_TRY(launch_check(c, "k_rot_lf_init"));
+    k_rot_lf_gather<<<cdiv(n, 256), 256, 0, c->stream>>>(b.cloud, b.keys2, c->rot_lessflat.as<int>(), lfpos, n, n_scans, lf_src, b.ringmm, b.meta);
+    LILI_TRY(launch_check(c, "k_rot_lf_gather"));
+    k_rot_lf_params<<<1, ROT_MAX_RINGS, 0, c->stream>>>(b.ringmm, c->prm.rot_ds_leaf, b.rprm);
+    LILI_TRY(launch_check(c, "k_rot_lf_params"));
+    unsigned long long* k64 = c->rot_keys.as<unsigned long long>();
+    unsigned long long* k64b = c->rot_keys2.as<unsigned long long>();
+    // keys2 (ring ids, sorted) is still needed by k_rot_lf_keys: stash it before reusing the buffers
+    LILI_CUDA(c, cudaMemcpyAsync(c->idx_b.p, b.keys2, (size_t)n * 4, cudaMemcpyDeviceToDevice, c->stream));
+    const uint32_t* ring_of = c->idx_b.as<uint32_t>();
+    k_rot_lf_keys<<<cdiv(n, 256), 256, 0, c->stream>>>(b.cloud, ring_of, lf_src, b.meta, b.rprm, k64, b.vals, n);
+    LILI_TRY(launch_check(c, "k_rot_lf_keys"));
+    LILI_TRY(sort_pairs_u64(c, k64, k64b, b.vals, b.vals2, n, 40));
+    k_vg_heads<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(k64b, n, b.meta + M_NLF, c->vg_flags.as<int>());
+    LILI_TRY(launch_check(c, "k_vg_heads"));
+    LILI_TRY(exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), n));
+    k_rot_lf_centroid<<<cdiv(n, 128), 128, 0, c->stream>>>(b.cloud, lf_src, k64b, b.vals2, c->vg_flags.as<int>(), c->vg_rank.as<int>(), b.meta, n,
+                                                           c->surf.as<Pt32>(), c->vg_count.as<int>());
+    LILI_TRY(launch_check(c, "k_rot_lf_centroid"));
+    return LILIOM_OK;
+}
+
+// hp: meta[0..8) and the surf count, read back after the chain
+static int rot_finish(const RotJob& j, const int hp[9], int* n_surf, int* n_edge, int* n_cut) {
+    liliom_ctx* c = j.c;
+    if (hp[M_ERR]) { c->last_error = "ring/segment larger than the shared-memory capacity (16384 / 4096 points)"; return LILIOM_E_CAPACITY; }
+    *n_cut = hp[M_NVALID]; *n_edge = hp[M_NEDGE]; *n_surf = hp[8];
+    c->n_surf_dev = hp[8];
+    c->d_nsurf = c->vg_count.as<int>();
+    c->n_surf_max = j.n;
+    c->n_rot_cloud = hp[M_NVALID];
+    c->feat_counts[0] = hp[8]; c->feat_counts[1] = hp[M_NEDGE]; c->feat_counts[2] = hp[M_NVALID];
+    c->feat_ready = true;
+    return LILIOM_OK;
+}
+
+int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4], int* n_surf, int* n_edge, int* n_cut,
+                    const uint16_t* rings, const double* times) {
+    RotJob j;
+    LILI_TRY(rot_begin(c, n, q_imu, q_lb, n_surf, n_edge, n_cut, rings, times, j));
+    if (j.n <= 0) return LILIOM_OK;
+    LILI_TRY(rot_front(j));
+    const int n_scans = c->prm.line_num;
+    const RotBufs b(c);
     // per-device function attribute (cheap; a process may hold contexts on several GPUs)
     LILI_CUDA(c, cudaFuncSetAttribute(k_rot_ring, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RingSmem)));
-    long long* ring_dbg = c->dbg_timing ? reinterpret_cast<long long*>(reinterpret_cast<unsigned char*>(rprm + ROT_MAX_RINGS) + 8) : nullptr;
+    long long* ring_dbg = c->dbg_timing ? reinterpret_cast<long long*>(reinterpret_cast<unsigned char*>(b.rprm + ROT_MAX_RINGS) + 8) : nullptr;
     if (ring_dbg) ring_dbg = reinterpret_cast<long long*>((reinterpret_cast<uintptr_t>(ring_dbg) + 7) & ~(uintptr_t)7);
-    k_rot_ring<<<n_scans, 512, sizeof(RingSmem), c->stream>>>(cloud, c->rot_curv.as<float>(), meta, c->prm.ds_rate, c->rot_label.as<int>(),
-                                                              c->rot_lessflat.as<int>(), seg_edge, seg_cnt, ring_dbg, c->rot_slow_walk ? 0 : ROT_FAST_CAP);
+    k_rot_ring<<<n_scans, 512, sizeof(RingSmem), c->stream>>>(b.cloud, c->rot_curv.as<float>(), b.meta, c->prm.ds_rate, c->rot_label.as<int>(),
+                                                              c->rot_lessflat.as<int>(), b.seg_edge, b.seg_cnt, ring_dbg, c->rot_slow_walk ? 0 : ROT_FAST_CAP);
     LILI_TRY(launch_check(c, "k_rot_ring"));
     if (ring_dbg) {       // LILIOM_DEBUG_TIMING: per-ring stage cycles of this launch
         long long h[ROT_MAX_RINGS * 8];
@@ -684,42 +849,197 @@ int rot_extract_dev(liliom_ctx* c, int n, const double q_imu[4], const double q_
             }
         }
     }
-    k_rot_edge_emit<<<1, ROT_EMIT_THREADS, 0, c->stream>>>(cloud, seg_edge, seg_cnt, n_scans * 6, c->edge.as<Pt32>(), meta);
-    LILI_TRY(launch_check(c, "k_rot_edge_emit"));
-    // less-flat -> per-ring VoxelGrid
-    int* lfpos = c->rot_sort.as<int>();
-    int* lf_src = c->rot_picked.as<int>();
-    LILI_TRY(exclusive_scan_i32(c, c->rot_lessflat.as<int>(), lfpos, n));
-    k_rot_lf_init<<<cdiv(ROT_MAX_RINGS * 8, 256), 256, 0, c->stream>>>(ringmm);
-    LILI_TRY(launch_check(c, "k_rot_lf_init"));
-    k_rot_lf_gather<<<cdiv(n, 256), 256, 0, c->stream>>>(cloud, keys2, c->rot_lessflat.as<int>(), lfpos, n, n_scans, lf_src, ringmm, meta);
-    LILI_TRY(launch_check(c, "k_rot_lf_gather"));
-    k_rot_lf_params<<<1, ROT_MAX_RINGS, 0, c->stream>>>(ringmm, c->prm.rot_ds_leaf, rprm);
-    LILI_TRY(launch_check(c, "k_rot_lf_params"));
-    unsigned long long* k64 = c->rot_keys.as<unsigned long long>();
-    unsigned long long* k64b = c->rot_keys2.as<unsigned long long>();
-    // keys2 (ring ids, sorted) is still needed by k_rot_lf_keys: stash it before reusing the buffers
-    LILI_CUDA(c, c->idx_b.ensure(N * 4));
-    LILI_CUDA(c, cudaMemcpyAsync(c->idx_b.p, keys2, N * 4, cudaMemcpyDeviceToDevice, c->stream));
-    const uint32_t* ring_of = c->idx_b.as<uint32_t>();
-    k_rot_lf_keys<<<cdiv(n, 256), 256, 0, c->stream>>>(cloud, ring_of, lf_src, meta, rprm, k64, vals, n);
-    LILI_TRY(launch_check(c, "k_rot_lf_keys"));
-    LILI_TRY(sort_pairs_u64(c, k64, k64b, vals, vals2, n, 40));
-    k_vg_heads<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(k64b, n, meta + M_NLF, c->vg_flags.as<int>());
-    LILI_TRY(launch_check(c, "k_vg_heads"));
-    LILI_TRY(exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), n));
-    k_rot_lf_centroid<<<cdiv(n, 128), 128, 0, c->stream>>>(cloud, lf_src, k64b, vals2, c->vg_flags.as<int>(), c->vg_rank.as<int>(), meta, n,
-                                                           c->surf.as<Pt32>(), c->vg_count.as<int>());
-    LILI_TRY(launch_check(c, "k_rot_lf_centroid"));
+    LILI_TRY(rot_back(j));
     int hp[9];
-    LILI_TRY(read_back(c, {{hp, meta, 8 * sizeof(int)}, {hp + 8, c->vg_count.p, sizeof(int)}}));
-    if (hp[M_ERR]) { c->last_error = "ring/segment larger than the shared-memory capacity (16384 / 4096 points)"; return LILIOM_E_CAPACITY; }
-    *n_cut = hp[M_NVALID]; *n_edge = hp[M_NEDGE]; *n_surf = hp[8];
-    c->n_surf_dev = hp[8];
-    c->d_nsurf = c->vg_count.as<int>();
-    c->n_surf_max = n;
-    c->n_rot_cloud = hp[M_NVALID];
+    LILI_TRY(read_back(c, {{hp, b.meta, 8 * sizeof(int)}, {hp + 8, c->vg_count.p, sizeof(int)}}));
+    return rot_finish(j, hp, n_surf, n_edge, n_cut);
+}
+
+// ---- the ROT chain of several sessions (liliom_extract_resident_batch): one launch per stage for up to kBatchMax sessions
+// Everything one session's stages read or write, on its own buffers.
+struct RotEntry {
+    const Pt32* raw; const uint16_t* rings; const double* times; Q4 qI, qL;
+    int n, n_scans; float leaf;
+    int* meta; int* ringmm; VgParams* rprm; uint32_t* keys; uint32_t* keys2; int* vals; int* vals2; float* ori; Pt32* cloud;
+    float* curv; int* label; int* lessflat; int* seg_edge; int* seg_cnt; Pt32* edge; int* lfpos; int* lf_src; const uint32_t* ring_of;
+    unsigned long long* k64; unsigned long long* k64b; int* vg_flags; int* vg_rank; Pt32* surf; int* vg_count;
+};
+struct RotTab {
+    int n;                              // sessions in this launch
+    RotEntry s[kBatchMax];
+};
+static_assert(sizeof(RotTab) <= 32764, "k_rot_stage_batch's session table must fit in the kernel parameter space");
+
+static RotEntry rot_entry(const RotJob& j) {
+    liliom_ctx* c = j.c;
+    const RotBufs b(c);
+    return RotEntry{j.raw, j.rings, j.times, j.qI, j.qL, j.n, c->prm.line_num, c->prm.rot_ds_leaf,
+                    b.meta, b.ringmm, b.rprm, b.keys, b.keys2, b.vals, b.vals2, b.ori, b.cloud,
+                    c->rot_curv.as<float>(), c->rot_label.as<int>(), c->rot_lessflat.as<int>(), b.seg_edge, b.seg_cnt, c->edge.as<Pt32>(),
+                    c->rot_sort.as<int>(), c->rot_picked.as<int>(), c->idx_b.as<uint32_t>(),
+                    c->rot_keys.as<unsigned long long>(), c->rot_keys2.as<unsigned long long>(), c->vg_flags.as<int>(), c->vg_rank.as<int>(),
+                    c->surf.as<Pt32>(), c->vg_count.as<int>()};
+}
+
+// One stage of the chain: its block size, its blocks for a sweep of n points and its body, each as the solo launch has them
+// (rot_front / rot_back).  Session s owns the blocks after those of sessions 0 .. s-1.
+#define LILI_ROT_STAGE(NAME, THREADS, BLOCKS, CALL)                                                   \
+    struct NAME {                                                                                     \
+        static constexpr int kThreads = THREADS;                                                      \
+        __host__ __device__ static int blocks(int n) { return BLOCKS; }                               \
+        __device__ static void run(const RotEntry& e, int bx) { CALL; }                               \
+    };
+#define LILI_CDIV(a, b) (((a) + (b) - 1) / (b))
+LILI_ROT_STAGE(RotStMetaInit, 256, 1, rot_meta_init_body(e.meta, bx))
+LILI_ROT_STAGE(RotStPreT, ROT_PRE_THREADS, LILI_CDIV(n, ROT_PRE_THREADS),
+               rot_pre_body<true>(e.raw, e.rings, e.times, e.n, e.n_scans, e.keys, e.vals, e.ori, e.meta, bx))
+LILI_ROT_STAGE(RotStPreA, ROT_PRE_THREADS, LILI_CDIV(n, ROT_PRE_THREADS),
+               rot_pre_body<false>(e.raw, e.rings, nullptr, e.n, e.n_scans, e.keys, e.vals, e.ori, e.meta, bx))
+LILI_ROT_STAGE(RotStHp, 256, LILI_CDIV(n, 256), rot_hp_body(e.raw, e.n, e.keys, e.ori, e.meta, bx))
+LILI_ROT_STAGE(RotStBuildT, 128, LILI_CDIV(n, 128),
+               rot_build_body<true>(e.raw, e.n, e.keys2, e.vals2, e.ori, e.times, e.qI, e.qL, e.cloud, e.meta, bx))
+LILI_ROT_STAGE(RotStBuildA, 128, LILI_CDIV(n, 128),
+               rot_build_body<false>(e.raw, e.n, e.keys2, e.vals2, e.ori, nullptr, e.qI, e.qL, e.cloud, e.meta, bx))
+LILI_ROT_STAGE(RotStCurv, 256, LILI_CDIV(n + 1, 256), rot_curv_body(e.cloud, e.meta, e.curv, e.label, e.lessflat, e.n, bx))
+LILI_ROT_STAGE(RotStEdgeEmit, ROT_EMIT_THREADS, 1, rot_edge_emit_body(e.cloud, e.seg_edge, e.seg_cnt, e.n_scans * 6, e.edge, e.meta, bx))
+LILI_ROT_STAGE(RotStLfInit, 256, LILI_CDIV(ROT_MAX_RINGS * 8, 256), rot_lf_init_body(e.ringmm, bx))
+LILI_ROT_STAGE(RotStLfGather, 256, LILI_CDIV(n, 256),
+               rot_lf_gather_body(e.cloud, e.keys2, e.lessflat, e.lfpos, e.n, e.n_scans, e.lf_src, e.ringmm, e.meta, bx))
+LILI_ROT_STAGE(RotStLfParams, ROT_MAX_RINGS, 1, rot_lf_params_body(e.ringmm, e.leaf, e.rprm, bx))
+LILI_ROT_STAGE(RotStLfKeys, 256, LILI_CDIV(n, 256), rot_lf_keys_body(e.cloud, e.ring_of, e.lf_src, e.meta, e.rprm, e.k64, e.vals, e.n, bx))
+LILI_ROT_STAGE(RotStVgHeads, 256, LILI_CDIV(n + 1, 256), vg_heads_at(e.k64b, e.n, e.meta + M_NLF, e.vg_flags, bx * blockDim.x + threadIdx.x))
+LILI_ROT_STAGE(RotStLfCentroid, 128, LILI_CDIV(n, 128),
+               rot_lf_centroid_body(e.cloud, e.lf_src, e.k64b, e.vals2, e.vg_flags, e.vg_rank, e.meta, e.n, e.surf, e.vg_count, bx))
+#undef LILI_ROT_STAGE
+#undef LILI_CDIV
+
+template <class St>
+__global__ void __launch_bounds__(St::kThreads) k_rot_stage_batch(const __grid_constant__ RotTab tab) {
+    int s = 0, b = (int)blockIdx.x;
+    while (s + 1 < tab.n && b >= St::blocks(tab.s[s].n)) { b -= St::blocks(tab.s[s].n); ++s; }
+    const RotEntry e = tab.s[s];        // a by-value copy, as the solo kernels' parameters
+    St::run(e, b);
+}
+
+// One stage for the sessions `which` (indices into E / cs): launches of up to kBatchMax sessions on c0's stream; each session's
+// launch count advances as its solo call's does.
+template <class St>
+static int rot_stage(liliom_ctx* c0, const std::vector<RotEntry>& E, const std::vector<liliom_ctx*>& cs, const std::vector<int>& which) {
+    for (size_t first = 0; first < which.size(); first += kBatchMax) {
+        RotTab tab{};
+        tab.n = (int)std::min(which.size() - first, (size_t)kBatchMax);
+        int grid = 0;
+        for (int m = 0; m < tab.n; ++m) {
+            tab.s[m] = E[which[first + m]];
+            grid += St::blocks(tab.s[m].n);
+            cs[which[first + m]]->cnt.launches++;
+        }
+        k_rot_stage_batch<St><<<grid, St::kThreads, 0, c0->stream>>>(tab);
+        LILI_CUDA(c0, cudaGetLastError());
+    }
     return LILIOM_OK;
+}
+
+// The rings of the sessions `which`: k_rot_ring_batch launches of up to kBatchMax sessions, one block per ring.
+static int rot_ring_stage(liliom_ctx* c0, const std::vector<liliom_ctx*>& cs, const std::vector<int>& which) {
+    LILI_CUDA(c0, cudaFuncSetAttribute(k_rot_ring_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RingSmem)));
+    for (size_t first = 0; first < which.size(); first += kBatchMax) {
+        RotRingBatch tab{};
+        tab.n = (int)std::min(which.size() - first, (size_t)kBatchMax);
+        for (int m = 0; m < tab.n; ++m) {
+            liliom_ctx* c = cs[which[first + m]];
+            const RotBufs b(c);
+            tab.off[m + 1] = tab.off[m] + c->prm.line_num;
+            tab.s[m] = RotRingEntry{b.cloud, c->rot_curv.as<float>(), b.meta, c->rot_label.as<int>(), c->rot_lessflat.as<int>(), b.seg_edge,
+                                    b.seg_cnt, c->prm.ds_rate, c->rot_slow_walk ? 0 : ROT_FAST_CAP};
+            c->cnt.launches++;
+        }
+        k_rot_ring_batch<<<tab.off[tab.n], 512, sizeof(RingSmem), c0->stream>>>(tab);
+        LILI_CUDA(c0, cudaGetLastError());
+    }
+    return LILIOM_OK;
+}
+
+// Points each session's work at c0's stream while the batch queues it (the CUB sorts and scans take the context's stream), and
+// gives every session its own stream back when it ends.
+struct RotStreams {
+    std::vector<std::pair<liliom_ctx*, cudaStream_t>> saved;
+    RotStreams(const std::vector<liliom_ctx*>& cs, cudaStream_t s) {
+        for (liliom_ctx* c : cs) { saved.emplace_back(c, c->stream); c->stream = s; }
+    }
+    ~RotStreams() { for (auto& p : saved) p.first->stream = p.second; }
+};
+
+// The ROT sessions of liliom_extract_resident_batch.  Every stage of the chain is one launch for all sessions with a sweep
+// (k_rot_stage_batch, k_rot_ring_batch), on c0's stream; the library sorts and scans and the copy of the sorted ring ids stay
+// per session, in order on the same stream.  The stage list is the solo one (rot_front, k_rot_ring, rot_back), so every
+// session's counters advance as in its solo call.  Other sessions' streams are joined before and after with events.  Each
+// session's read-back words are copied into its pinned block at the end; the caller synchronises once for all of them before
+// rot_batch_finish.
+int rot_batch_queue(liliom_ctx* c0, std::vector<RotBatchSession>& ss) {
+    std::vector<RotJob> jobs(ss.size());
+    std::vector<liliom_ctx*> cs;            // sessions with a sweep, in call order
+    std::vector<RotEntry> E;
+    std::vector<int> all, timed, az;        // indices into cs / E: every session, LILIOM_TIME_FIELD, azimuth rule
+    std::vector<int> at;                    // index into ss of each
+    for (size_t k = 0; k < ss.size(); ++k) {
+        RotBatchSession& s = ss[k];
+        s.pending = false;
+        s.status = rot_begin(s.c, s.n, s.q_imu, s.q_lb, s.n_surf, s.n_edge, s.n_cut, s.rings, s.times, jobs[k]);
+        if (s.status != LILIOM_OK || jobs[k].n <= 0) continue;
+        const int i = (int)cs.size();
+        cs.push_back(s.c);
+        E.push_back(rot_entry(jobs[k]));
+        all.push_back(i);
+        (jobs[k].times ? timed : az).push_back(i);
+        at.push_back((int)k);
+    }
+    if (cs.empty()) return LILIOM_OK;
+    for (liliom_ctx* c : cs) LILI_TRY(batch_join_in(c0, c));
+    {
+        const RotStreams on_c0(cs, c0->stream);
+        LILI_TRY(rot_stage<RotStMetaInit>(c0, E, cs, all));
+        LILI_TRY(rot_stage<RotStPreT>(c0, E, cs, timed));
+        LILI_TRY(rot_stage<RotStPreA>(c0, E, cs, az));
+        LILI_TRY(rot_stage<RotStHp>(c0, E, cs, az));             // the halfPassed latch: azimuth rule only
+        for (int i : all) LILI_TRY(sort_pairs_u32(cs[i], E[i].keys, E[i].keys2, E[i].vals, E[i].vals2, E[i].n, 8));
+        LILI_TRY(rot_stage<RotStBuildT>(c0, E, cs, timed));
+        LILI_TRY(rot_stage<RotStBuildA>(c0, E, cs, az));
+        LILI_TRY(rot_stage<RotStCurv>(c0, E, cs, all));
+        LILI_TRY(rot_ring_stage(c0, cs, all));
+        LILI_TRY(rot_stage<RotStEdgeEmit>(c0, E, cs, all));
+        for (int i : all) LILI_TRY(exclusive_scan_i32(cs[i], E[i].lessflat, E[i].lfpos, E[i].n));
+        LILI_TRY(rot_stage<RotStLfInit>(c0, E, cs, all));
+        LILI_TRY(rot_stage<RotStLfGather>(c0, E, cs, all));
+        LILI_TRY(rot_stage<RotStLfParams>(c0, E, cs, all));
+        // keys2 (ring ids, sorted) is still needed by the key stage: stashed before the 64-bit sort reuses the buffers
+        for (int i : all)
+            LILI_CUDA(cs[i], cudaMemcpyAsync(cs[i]->idx_b.p, E[i].keys2, (size_t)E[i].n * 4, cudaMemcpyDeviceToDevice, c0->stream));
+        LILI_TRY(rot_stage<RotStLfKeys>(c0, E, cs, all));
+        for (int i : all) LILI_TRY(sort_pairs_u64(cs[i], E[i].k64, E[i].k64b, E[i].vals, E[i].vals2, E[i].n, 40));
+        LILI_TRY(rot_stage<RotStVgHeads>(c0, E, cs, all));
+        for (int i : all) LILI_TRY(exclusive_scan_i32(cs[i], E[i].vg_flags, E[i].vg_rank, E[i].n));
+        LILI_TRY(rot_stage<RotStLfCentroid>(c0, E, cs, all));
+        for (int i : all) {
+            unsigned char* dst = cs[i]->h_pin->scratch;
+            LILI_CUDA(cs[i], cudaMemcpyAsync(dst, E[i].meta, 8 * sizeof(int), cudaMemcpyDeviceToHost, c0->stream));
+            LILI_CUDA(cs[i], cudaMemcpyAsync(dst + 8 * sizeof(int), E[i].vg_count, sizeof(int), cudaMemcpyDeviceToHost, c0->stream));
+            ss[at[i]].pending = true;
+        }
+    }
+    LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, c0->stream));
+    for (liliom_ctx* c : cs) LILI_TRY(batch_join_out(c0, c));
+    return LILIOM_OK;
+}
+
+int rot_batch_finish(RotBatchSession& s) {
+    int hp[9];
+    memcpy(hp, s.c->h_pin->scratch, sizeof(hp));
+    RotJob j;
+    j.c = s.c;
+    j.n = s.n;
+    s.pending = false;
+    return s.status = rot_finish(j, hp, s.n_surf, s.n_edge, s.n_cut);
 }
 
 }  // namespace lili

@@ -197,18 +197,6 @@ struct PassArgs {
 // Small scans (8 or 16 lanes per query) deal tasks to warps block-cyclically: queries arrive in voxel order (spatially sorted),
 // and dealing neighbouring tasks to different blocks evens out the per-block work (dense vs sparse regions) at the grid barrier;
 // large scans keep neighbours together for L1 reuse.
-// Where a block sits in its session: blk.bi() of blk.G() blocks.  A solo launch reads blockIdx.x / gridDim.x at each use
-// (the kernels keep the code and registers they had before the batched launch existed); a batched launch (k_gn_batch) passes
-// the block's place inside its session's range.
-struct SoloBlock {
-    __device__ __forceinline__ int bi() const { return (int)blockIdx.x; }
-    __device__ __forceinline__ unsigned int G() const { return gridDim.x; }
-};
-struct SessionBlock {
-    int b; unsigned int g;
-    __device__ __forceinline__ int bi() const { return b; }
-    __device__ __forceinline__ unsigned int G() const { return g; }
-};
 
 template <int LANES> __device__ __forceinline__ int first_task(int warp, int bi, int G) {
     return LANES >= 8 ? warp * G + bi : bi * kWarps + warp; }
@@ -1289,19 +1277,6 @@ static const void* gn_batch_kernel(int kind) {
 static const void* knn_batch_kernel(int lanes) {
     return lanes == 16 ? (const void*)k_knn_plane_batch<16> : lanes == 1 ? (const void*)k_knn_plane_batch<1> : lanes == 2 ? (const void*)k_knn_plane_batch<2>
          : lanes == 4 ? (const void*)k_knn_plane_batch<4> : (const void*)k_knn_plane_batch<8>;
-}
-
-// Every other session's stream (its set-up so far) is ordered before the shared launches on ctxs[0]'s stream ...
-static int batch_join_in(liliom_ctx* c0, liliom_ctx* c) {
-    if (c->stream == c0->stream) return LILIOM_OK;
-    LILI_CUDA(c, cudaEventRecord(c->ev_batch, c->stream));
-    LILI_CUDA(c0, cudaStreamWaitEvent(c0->stream, c->ev_batch, 0));
-    return LILIOM_OK;
-}
-// ... and after them (c0->ev_batch recorded behind the last shared launch)
-static int batch_join_out(liliom_ctx* c0, liliom_ctx* c) {
-    if (c->stream != c0->stream) LILI_CUDA(c, cudaStreamWaitEvent(c->stream, c0->ev_batch, 0));
-    return LILIOM_OK;
 }
 
 // Ceres mode: per pass, the sessions' searches in k_knn_plane_batch launches, then their LM solves in k_lm_solve_batch launches,

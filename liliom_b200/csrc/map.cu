@@ -170,6 +170,7 @@ __global__ void k_inc_centroid(const __grid_constant__ FrameTab tab, const u64* 
 static int shard_filter(liliom_ctx* c, const void* in, int n, int stride, float halo, void* out, bool repack, int* kept,
                         int* box = nullptr) {
     LILI_CUDA(c, c->flags.ensure(((size_t)n + 2) * 4));
+    LILI_TRY(feat_keep_cut(c));
     LILI_CUDA(c, c->idx_a.ensure(((size_t)n + 2) * 4));
     const unsigned char* p = (const unsigned char*)in;
     int* flags = c->flags.as<int>();

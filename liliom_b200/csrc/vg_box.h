@@ -285,10 +285,14 @@ VGB_HD VgXyz vg_write(const float* s, int n, unsigned char* dst) {
 // flags[i] = 1 at the first entry of every voxel of a sorted key array; 0 at entries past the valid count (*d_valid, or n
 // when d_valid is null) and at flags[n] (the sentinel of the exclusive scan that numbers the voxels)
 template <typename K>
-__global__ void k_vg_heads(const K* __restrict__ keys, int n, const int* __restrict__ d_valid, int* __restrict__ flags) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void vg_heads_at(const K* __restrict__ keys, int n, const int* __restrict__ d_valid, int* __restrict__ flags,
+                                            const int i) {
     if (i > n) return;
     flags[i] = i < n && vg_is_head(keys, i, d_valid ? *d_valid : n);
+}
+template <typename K>
+__global__ void k_vg_heads(const K* __restrict__ keys, int n, const int* __restrict__ d_valid, int* __restrict__ flags) {
+    vg_heads_at(keys, n, d_valid, flags, blockIdx.x * blockDim.x + threadIdx.x);
 }
 #endif
 
