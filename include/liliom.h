@@ -132,6 +132,15 @@ int liliom_map_rebuild(liliom_ctx* c, int* n_map_out);
  * whose voxel coordinates do not fit 21 bits take the two-step path internally.  _device: d_surf_ds_body is a DEVICE pointer. */
 int liliom_map_update(liliom_ctx* c, const void* surf_ds_body, int n, const double pose7[7], int* n_map_out);
 int liliom_map_update_device(liliom_ctx* c, const void* d_surf_ds_body, int n, const double pose7[7], int* n_map_out);
+/* liliom_map_update with the frame taken from the context itself: surf_last_ds of the context's last liliom_odometry /
+ * liliom_odometry_resident (or its batch forms), as left on the device.  pose7: the pose to save the frame with.  Bit for bit
+ * liliom_map_update(c, <that cloud downloaded through ds_out>, n_ds, pose7, n_map_out), without the cloud crossing PCIe.
+ * The scan is resident from the end of an odometry call (one that returned LILIOM_E_NOMAP / LILIOM_E_FEWMAP included) until
+ * another call rewrites the buffer it lies in: liliom_voxelgrid, liliom_kf_add, liliom_kf_cloud, liliom_loop_align,
+ * liliom_global_map, or an odometry call that fails.  Calls that only search (liliom_scan_to_map and its resident and
+ * batch forms, liliom_find_surf_corr) leave it alone, whatever their feature count: the scan keeps its own count.  With no scan resident: LILIOM_E_ARG (see liliom_last_error), nothing
+ * changed.  The map update itself only reads the scan, so it stays resident across this call (and may be pushed again). */
+int liliom_map_update_resident(liliom_ctx* c, const double pose7[7], int* n_map_out);
 /* surf_from_map_ds with all its fields (point_stride bytes per point), in liliom_map_download order (single GPU): the
  * filtered cloud of the last liliom_map_rebuild or liliom_map_update (empty after liliom_map_clear).  A map installed with
  * liliom_map_set_points, liliom_map_set_cloud or liliom_icp_align has no filtered cloud behind it: LILIOM_E_NOMAP (see
@@ -565,6 +574,24 @@ int liliom_odometry_resident_batch_ex(liliom_ctx* const* ctxs, int B, double* po
  * faster (no event joins). */
 int liliom_extract_resident_batch(liliom_ctx* const* ctxs, int B, const double* q_imu, const double* q_lb,
                                   int* n_surf, int* n_edge, int* n_cut, int* status);
+/* liliom_map_update_resident of B independent sessions in one call.  poses7: 7*B doubles.  n_map: B ints (may be NULL).
+ * status: B ints.  Session i gets exactly what liliom_map_update_resident(ctxs[i], poses7 + 7*i, &n_map[i]) would give it,
+ * bit for bit: status, count, FIFO, filtered cloud (liliom_map_download_cloud), search index (liliom_map_download and every
+ * later scan-to-map), incremental entry array, and launch counters.  A session that needs no update this step is simply left
+ * out of ctxs.  Horizon (48-byte) and ROT (32-byte) contexts may be mixed.
+ * Every kernel of the steady-state update runs once for up to 32 sessions, on ctxs[0]'s stream (other sessions' streams are
+ * joined with events), and the call waits four times for all sessions together (the new frames' boxes, their key flags, the
+ * voxel counts, the cell grids' escape flags) where B solo calls wait five times each.  It returns, like the solo call,
+ * with every session's map complete (one more wait when a session re-built its cell grid or left the steady-state path).  The library sorts and scans stay per
+ * session, in order on the same stream.  Sessions off the steady-state path finish on their solo path inside the call: a
+ * first update or one after liliom_map_push_frame / liliom_map_clear, voxel keys that do not fit 21 bits, max_map_frames
+ * above 64, a cell grid whose box a centroid left.
+ * A session's own error (LILIOM_E_ARG: no scan resident; LILIOM_E_GRID: a map extent over 2^29 cells; a CUDA error) is its
+ * status; the others run.
+ * LILIOM_E_ARG for the whole call, nothing changed: B < 1, a NULL array (ctxs, poses7, status), a NULL or repeated context,
+ * contexts on different devices, a context with a communicator.
+ * For a single session the solo call is faster (no event joins). */
+int liliom_map_update_batch(liliom_ctx* const* ctxs, int B, const double* poses7, int* n_map, int* status);
 
 #ifdef __cplusplus
 }

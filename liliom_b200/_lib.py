@@ -80,6 +80,7 @@ EXPORTS = [
     "liliom_scan_to_map_resident_batch", "liliom_odometry_resident_batch",
     "liliom_scan_to_map_resident_batch_ex", "liliom_odometry_resident_batch_ex",
     "liliom_extract_resident_batch", "liliom_features_download",
+    "liliom_map_update_resident", "liliom_map_update_batch",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -206,6 +207,8 @@ def lib() -> C.CDLL:
     L.liliom_undistort.argtypes = [vp, vp, C.c_int, dp, dp]
     L.liliom_map_update.argtypes = [vp, vp, C.c_int, dp, ip]
     L.liliom_map_update_device.argtypes = [vp, vp, C.c_int, dp, ip]
+    L.liliom_map_update_resident.argtypes = [vp, dp, ip]
+    L.liliom_map_update_batch.argtypes = [C.POINTER(vp), C.c_int, dp, ip, ip]
     L.liliom_map_download_cloud.argtypes = [vp, vp, C.c_int, ip]
     L.liliom_icp_align.argtypes = [vp, vp, C.c_int, vp, C.c_int, C.c_int, C.c_double, C.c_int, C.c_double, C.c_double, dp, dp, ip, ip]
     L.liliom_knn_block_stats.argtypes = [vp, dp, C.POINTER(C.c_ulonglong)]
@@ -372,6 +375,13 @@ class Context:
         p = np.asarray(pose7, dtype=np.float64)
         m = C.c_int()
         self._check(lib().liliom_map_update(self._h, _ptr(pts), len(pts), _dptr(p), C.byref(m)))
+        return m.value
+
+    def map_update_resident(self, pose7) -> int:
+        """map_update with the down-sampled scan the last odometry call left on the device (liliom_map_update_resident)."""
+        p = np.ascontiguousarray(pose7, dtype=np.float64)
+        m = C.c_int(0)
+        self._check(lib().liliom_map_update_resident(self._h, _dptr(p), C.byref(m)))
         return m.value
 
     def map_update_device(self, dev_ptr: int, n: int, pose7) -> int:
@@ -886,6 +896,23 @@ def extract_resident_batch(ctxs, q_imu, q_lb=None):
     if rc != OK:
         raise LiliomError(rc)
     return np.stack([ns, ne, nc], axis=1)[:B], status[:B]
+
+
+def map_update_batch(ctxs, poses7):
+    """map_update_resident of every context in `ctxs` in one call (liliom_map_update_batch): session i gets what
+    ctxs[i].map_update_resident(poses7[i]) would give it.  Returns (map sizes (B,), status (B,)); a session's own error is its
+    status, a whole-call error raises LiliomError."""
+    B = len(ctxs)
+    handles = (C.c_void_p * max(B, 1))(*[c._h if c is not None else None for c in ctxs])
+    poses = np.ascontiguousarray(poses7, dtype=np.float64).reshape(-1) if poses7 is not None else None
+    if poses is not None and len(poses) != 7 * B:
+        raise ValueError(f"poses7: expected {7 * B} doubles (B x 7), got {len(poses)}")
+    n_map = np.zeros(max(B, 1), np.int32)
+    status = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_map_update_batch(handles, B, _dptr(poses) if poses is not None else None, _ip(n_map), _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    return n_map[:B], status[:B]
 
 
 def comm_get_unique_id() -> bytes:

@@ -370,6 +370,7 @@ extern "C" int liliom_voxelgrid(liliom_ctx* c, const void* pts, int n, int strid
     *n_out = 0;
     if (n == 0) return LILIOM_OK;
     LILI_CUDA(c, c->raw.ensure((size_t)n * stride));
+    c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
     LILI_CUDA(c, c->vg_out.ensure((size_t)n * stride));
     LILI_CUDA(c, c->vg_count.ensure(16));
     LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, pts, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
@@ -527,7 +528,7 @@ extern "C" int liliom_extract_resident(liliom_ctx* c, const double q_imu[4], con
 }
 
 // The contexts of a batched call: distinct, single-GPU, on one device.
-static bool batch_ctxs_ok(liliom_ctx* const* ctxs, int B) {
+bool lili::batch_ctxs_ok(liliom_ctx* const* ctxs, int B) {
     if (B < 1 || !ctxs) return false;
     for (int i = 0; i < B; ++i) {
         const liliom_ctx* c = ctxs[i];
@@ -604,6 +605,7 @@ static int odo_filter(liliom_ctx* c, bool spec_failed, int* step) {
     // surf count: exact on the host (n_surf_dev >= 0) or only on the device (resident pipeline, no round trip)
     const int n_max = c->n_surf_dev >= 0 ? c->n_surf_dev : c->n_surf_max;
     const int* d_n = c->n_surf_dev >= 0 ? nullptr : c->d_nsurf;
+    c->n_ds_resident = -1;      // until odo_finish: a call that fails before it leaves no scan for liliom_map_update_resident
     LILI_CUDA(c, c->vg_out.ensure((size_t)(n_max > 0 ? n_max : 1) * stride));
     LILI_CUDA(c, c->vg_count.ensure(16));
     LILI_CUDA(c, c->feats.ensure((size_t)(n_max > 0 ? n_max : 1) * sizeof(float4)));
@@ -653,6 +655,7 @@ static int odo_finish(liliom_ctx* c, bool ran, int rc, void* ds_out, int ds_cap,
     }
     c->d_nfeats = nullptr;
     const int m = c->n_feats_actual;
+    c->n_ds_resident = (!ran || rc == LILIOM_OK) ? m : -1;      // vg_out holds surf_last_ds, m points (liliom_map_update_resident)
     if (n_ds) *n_ds = m;
     if (ds_out) {
         if (m > ds_cap) return LILIOM_E_CAPACITY;

@@ -7,6 +7,7 @@
 #include <cstring>
 #include <initializer_list>
 #include <string>
+#include <utility>
 #include <vector>
 #include "../../include/liliom.h"
 #include "vg_box.h"
@@ -138,6 +139,73 @@ struct SessionBlock {
     __device__ __forceinline__ unsigned int G() const { return g; }
 };
 
+// Bodies of the box and cell-grid kernels (voxelgrid.cu, grid_knn.cu), `i` = the thread's place in its session's launch: the solo
+// kernels pass blockIdx.x * blockDim.x + threadIdx.x, the batched map update (k_map_stage_batch, map.cu) the same place counted
+// from its session's first block.
+__device__ __forceinline__ void vg_box_init(int* __restrict__ mm) {
+    if (threadIdx.x < kBoxInts) mm[threadIdx.x] = vg_box_empty(threadIdx.x);
+}
+template <class Blk>
+__device__ __forceinline__ void vg_minmax_body(const unsigned char* __restrict__ pts, int n_max, const int* __restrict__ d_n, int stride,
+                                               int* __restrict__ mm, const Blk blk) {
+    const int n = d_n ? min(*d_n, n_max) : n_max;
+    int box[kBoxInts];
+#pragma unroll
+    for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_empty(k);
+    for (int i = blk.bi() * blockDim.x + threadIdx.x; i < n; i += blk.G() * blockDim.x) {
+        float4 v = *reinterpret_cast<const float4*>(pts + (size_t)i * stride);
+        if (!(isfinite(v.x) && isfinite(v.y) && isfinite(v.z))) continue;
+        vg_box_add(box, v.x, v.y, v.z);
+    }
+    vg_box_commit(box, mm);
+}
+
+__device__ __forceinline__ void repack_f4_at(const unsigned char* __restrict__ in, int n_max, const int* __restrict__ d_n, int stride,
+                                             float4* __restrict__ out, const int i) {
+    const int n = d_n ? min(*d_n, n_max) : n_max;
+    if (i >= n) return;
+    float4 v = *reinterpret_cast<const float4*>(in + (size_t)i * stride);
+    v.w = __int_as_float(i);
+    out[i] = v;
+}
+
+__device__ __forceinline__ int cell_coord(float v, float inv_cell) { return (int)floorf(v * inv_cell); }
+
+// `escaped` (optional): set when a point lies outside the grid's box — only possible when the box was handed in by the caller
+// (grid_build's host_box); the key is then clamped into range for memory safety and the caller rebuilds with the exact box.
+__device__ __forceinline__ void cell_keys_at(const float4* __restrict__ p, int n, const GridDesc& g, uint32_t* __restrict__ keys,
+                                             int* __restrict__ vals, int* __restrict__ escaped, const int i) {
+    if (i >= n) return;
+    float4 v = p[i];
+    int cx = cell_coord(v.x, g.inv_cell) - g.org[0];
+    int cy = cell_coord(v.y, g.inv_cell) - g.org[1];
+    int cz = cell_coord(v.z, g.inv_cell) - g.org[2];
+    if (escaped && ((unsigned)cx >= (unsigned)g.dim[0] || (unsigned)cy >= (unsigned)g.dim[1] || (unsigned)cz >= (unsigned)g.dim[2])) {
+        *escaped = 1;
+        cx = min(max(cx, 0), g.dim[0] - 1); cy = min(max(cy, 0), g.dim[1] - 1); cz = min(max(cz, 0), g.dim[2] - 1);
+    }
+    keys[i] = (uint32_t)((cz * g.dim[1] + cy) * g.dim[0] + cx);
+    vals[i] = i;
+}
+
+__device__ __forceinline__ void gather_sorted_at(const float4* __restrict__ p, const int* __restrict__ vals, int n, float4* __restrict__ out,
+                                                 const int i) {
+    if (i >= n) return;
+    int src = vals[i];
+    float4 v = p[src];
+    out[i] = make_float4(v.x, v.y, v.z, __int_as_float(src));   // w = index into the un-sorted map array
+}
+
+// cell_start[c] = first sorted position whose key >= c = number of points with key < c = upper bound of cell c-1.
+// Run ENDS are scattered (cell_start[key+1] = position after the run) into a zeroed table and a running maximum fills the
+// empty cells: two streaming passes over the table.  (Filling every gap with one warp per sorted position is an order of
+// magnitude slower on a 10 M-point map.)
+__device__ __forceinline__ void cell_run_ends_at(const uint32_t* __restrict__ keys, int n, int* __restrict__ cell_start, const int w) {
+    if (w >= n) return;
+    const uint32_t k = keys[w];
+    if (w == n - 1 || keys[w + 1] != k) cell_start[(size_t)k + 1] = w + 1;
+}
+
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -216,6 +284,9 @@ struct liliom_ctx {
     const int* d_nfeats = nullptr; // device-side query count for scan-to-map (nullptr: n_feats is exact)
     int last_n_feats = 0;        // query count of the previous scan (kernel-shape predictor)
     int n_feats_actual = 0;      // query count read back with the pose
+    int n_ds_resident = -1;      // >= 0: vg_out holds surf_last_ds of the last odometry call, that many points
+                                 // (liliom_map_update_resident): set by odo_finish, -1 from every other writer of vg_out.  A count
+                                 // of its own: n_feats_actual moves with every scan-to-map call, which leaves vg_out alone
     bool vg_check = false;       // s2m_run also reads vg_params back (speculative key width of the scan VoxelGrid)
     bool vg_used24 = false;      // ... the sort chain ran with 24-bit keys
     bool vg_bail = false;        // ... the cooperative filter declined (valid after the sync)
@@ -414,6 +485,25 @@ inline int grid_build(liliom_ctx* c, int m, const int* host_box = nullptr) {    
     return grid_build(c, c->map, gate_cell(c->prm.knn_max_sqdist), m, host_box);
 }
 
+// grid_build in parts, for callers that share its launches between several indexes (the batched map update, map.cu):
+// grid_begin (host: the grid's box and dimensions, the buffers; done = an empty index, already complete), then k_cell_keys,
+// grid_sort, k_gather_sorted, grid_clear, k_cell_run_ends, grid_scan, and grid_finish with the escape flag read back from
+// `escaped` (0 when escaped is null), which re-builds from the exact box when a point escaped.
+struct GridJob {
+    liliom_ctx* c = nullptr;
+    MapIndex* mi = nullptr;
+    float cell = 0.0f;
+    int m = 0;
+    bool done = false;
+    int bits = 0;                        // key width of the cell sort
+    int* escaped = nullptr;              // device flag of k_cell_keys (a host_box was given)
+};
+int grid_begin(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_box, GridJob& j);
+int grid_sort(const GridJob& j);
+int grid_clear(const GridJob& j);
+int grid_scan(const GridJob& j);
+int grid_finish(const GridJob& j, int esc);
+
 const long long* vg_coop_stamps(liliom_ctx* c);   // voxelgrid.cu
 
 int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int mode, liliom_iter_stats* stats,
@@ -437,6 +527,18 @@ inline int batch_join_out(liliom_ctx* c0, liliom_ctx* c) {
     if (c->stream != c0->stream) LILI_CUDA(c, cudaStreamWaitEvent(c->stream, c0->ev_batch, 0));
     return LILIOM_OK;
 }
+
+// Points each session's work at one stream while a batch queues it (the library sorts and scans, the clears and the read-backs
+// take the context's stream), and gives every session its own stream back when it ends.
+struct BatchStreams {
+    std::vector<std::pair<liliom_ctx*, cudaStream_t>> saved;
+    BatchStreams(const std::vector<liliom_ctx*>& cs, cudaStream_t s) {
+        for (liliom_ctx* c : cs) { saved.emplace_back(c, c->stream); c->stream = s; }
+    }
+    BatchStreams(const BatchStreams&) = delete;
+    BatchStreams& operator=(const BatchStreams&) = delete;
+    ~BatchStreams() { for (auto& p : saved) p.first->stream = p.second; }
+};
 
 int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf, int* n_edge, int* n_cut, bool sync_counts = true);
 // One Horizon session of liliom_extract_resident_batch (n points of the resident sweep): horizon_batch_queue queues every session
@@ -474,6 +576,10 @@ int rot_batch_finish(RotBatchSession& s);
 int icp_align(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,
               double fit_eps, double T16[16], double* fitness, int* converged, int* iters);     // icp.cu
 int map_install_host(liliom_ctx* c, const void* pts, int m, int stride, bool keep_refl);     // map.cu
+// liliom_map_update_resident of B distinct single-GPU contexts on one device (map.cu): status[i] = session i's result, n_map
+// (optional) its voxel count.  Returns a whole-call CUDA error.
+int map_update_batch(liliom_ctx* const* cs, int B, const double* poses7, int* n_map, int* status);
+bool batch_ctxs_ok(liliom_ctx* const* ctxs, int B);      // api.cu: the contexts of a batched call are distinct, single-GPU, on one device
 
 int block27_stats(liliom_ctx* c, const double pose7[7], unsigned long long out[2]);   // grid_knn.cu
 

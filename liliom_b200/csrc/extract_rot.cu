@@ -960,16 +960,6 @@ static int rot_ring_stage(liliom_ctx* c0, const std::vector<liliom_ctx*>& cs, co
     return LILIOM_OK;
 }
 
-// Points each session's work at c0's stream while the batch queues it (the CUB sorts and scans take the context's stream), and
-// gives every session its own stream back when it ends.
-struct RotStreams {
-    std::vector<std::pair<liliom_ctx*, cudaStream_t>> saved;
-    RotStreams(const std::vector<liliom_ctx*>& cs, cudaStream_t s) {
-        for (liliom_ctx* c : cs) { saved.emplace_back(c, c->stream); c->stream = s; }
-    }
-    ~RotStreams() { for (auto& p : saved) p.first->stream = p.second; }
-};
-
 // The ROT sessions of liliom_extract_resident_batch.  Every stage of the chain is one launch for all sessions with a sweep
 // (k_rot_stage_batch, k_rot_ring_batch), on c0's stream; the library sorts and scans and the copy of the sorted ring ids stay
 // per session, in order on the same stream.  The stage list is the solo one (rot_front, k_rot_ring, rot_back), so every
@@ -997,7 +987,7 @@ int rot_batch_queue(liliom_ctx* c0, std::vector<RotBatchSession>& ss) {
     if (cs.empty()) return LILIOM_OK;
     for (liliom_ctx* c : cs) LILI_TRY(batch_join_in(c0, c));
     {
-        const RotStreams on_c0(cs, c0->stream);
+        const BatchStreams on_c0(cs, c0->stream);
         LILI_TRY(rot_stage<RotStMetaInit>(c0, E, cs, all));
         LILI_TRY(rot_stage<RotStPreT>(c0, E, cs, timed));
         LILI_TRY(rot_stage<RotStPreA>(c0, E, cs, az));

@@ -26,12 +26,7 @@ namespace lili {
 
 // ------------------------------------------------------------------ small utilities
 __global__ void k_repack_f4(const unsigned char* __restrict__ in, int n_max, const int* __restrict__ d_n, int stride, float4* __restrict__ out) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const int n = d_n ? min(*d_n, n_max) : n_max;
-    if (i >= n) return;
-    float4 v = *reinterpret_cast<const float4*>(in + (size_t)i * stride);
-    v.w = __int_as_float(i);
-    out[i] = v;
+    repack_f4_at(in, n_max, d_n, stride, out, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
 int repack_to_f4(liliom_ctx* c, const void* d_in, int n, int stride, float4* d_out, const int* d_n) {
@@ -40,44 +35,25 @@ int repack_to_f4(liliom_ctx* c, const void* d_in, int n, int stride, float4* d_o
     return launch_check(c, "k_repack_f4");
 }
 
-// `escaped` (optional): set when a point lies outside the grid's box — only possible when the box was handed in by the caller
-// (grid_build's host_box); the key is then clamped into range for memory safety and the caller rebuilds with the exact box.
+// the cell-grid kernels: bodies in ctx.cuh (the batched map update runs them too)
 __global__ void k_cell_keys(const float4* __restrict__ p, int n, GridDesc g, uint32_t* __restrict__ keys, int* __restrict__ vals,
                             int* __restrict__ escaped) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    float4 v = p[i];
-    int cx = cell_coord(v.x, g.inv_cell) - g.org[0];
-    int cy = cell_coord(v.y, g.inv_cell) - g.org[1];
-    int cz = cell_coord(v.z, g.inv_cell) - g.org[2];
-    if (escaped && ((unsigned)cx >= (unsigned)g.dim[0] || (unsigned)cy >= (unsigned)g.dim[1] || (unsigned)cz >= (unsigned)g.dim[2])) {
-        *escaped = 1;
-        cx = min(max(cx, 0), g.dim[0] - 1); cy = min(max(cy, 0), g.dim[1] - 1); cz = min(max(cz, 0), g.dim[2] - 1);
-    }
-    keys[i] = (uint32_t)((cz * g.dim[1] + cy) * g.dim[0] + cx);
-    vals[i] = i;
+    cell_keys_at(p, n, g, keys, vals, escaped, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
 __global__ void k_gather_sorted(const float4* __restrict__ p, const int* __restrict__ vals, int n, float4* __restrict__ out) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    int src = vals[i];
-    float4 v = p[src];
-    out[i] = make_float4(v.x, v.y, v.z, __int_as_float(src));   // w = index into the un-sorted map array
+    gather_sorted_at(p, vals, n, out, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
-// cell_start[c] = first sorted position whose key >= c = number of points with key < c = upper bound of cell c-1.
-// Run ENDS are scattered (cell_start[key+1] = position after the run) into a zeroed table and a running maximum fills the
-// empty cells: two streaming passes over the table.  (Filling every gap with one warp per sorted position is an order of
-// magnitude slower on a 10 M-point map.)
 __global__ void k_cell_run_ends(const uint32_t* __restrict__ keys, int n, int* __restrict__ cell_start) {
-    const int w = blockIdx.x * blockDim.x + threadIdx.x;
-    if (w >= n) return;
-    const uint32_t k = keys[w];
-    if (w == n - 1 || keys[w + 1] != k) cell_start[(size_t)k + 1] = w + 1;
+    cell_run_ends_at(keys, n, cell_start, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
-int grid_build(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_box) {
+// grid_build in parts (ctx.cuh: GridJob), shared with the batched map update: grid_begin decides the grid and sizes the buffers,
+// grid_sort / grid_clear / grid_scan are the library calls and the clear between the kernels, grid_finish takes the escape flag.
+int grid_begin(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_box, GridJob& j) {
+    j = GridJob{};
+    j.c = c; j.mi = &mi; j.cell = cell; j.m = m;
     mi.ready = false;
     mi.n = m;
     if (m <= 0) {   // empty (shard of the) map: a 1-cell grid with no points, so that collective callers still run every launch
@@ -90,6 +66,7 @@ int grid_build(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_b
         LILI_CUDA(c, mi.xyzw.ensure(sizeof(float4)));
         mi.n = 0;
         mi.ready = true;
+        j.done = true;
         return LILIOM_OK;
     }
     float4* pts = mi.xyzw.as<float4>();
@@ -98,13 +75,12 @@ int grid_build(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_b
     // it by rounding, in which case its cell may not exist: k_cell_keys reports that, and the grid is rebuilt from the exact
     // min/max below.  (One cell of padding instead would be free of the re-run but can push the cell count over a power of
     // 256 and cost every rebuild a whole extra radix pass: 2^24 -> 17.7 M cells on the 10 M-point bench map, +90 us.)
-    int* escaped = nullptr;
     if (host_box) {
         for (int k = 0; k < 6; ++k) h[k] = host_box[k];
         if (c->test_shrink_box) h[3] = h[0];      // test hook: a box that is too small in x -> the escape path below must run
         LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
-        escaped = c->vg_minmax.as<int>() + 7;
-        LILI_CUDA(c, cudaMemsetAsync(escaped, 0, sizeof(int), c->stream));
+        j.escaped = c->vg_minmax.as<int>() + 7;
+        LILI_CUDA(c, cudaMemsetAsync(j.escaped, 0, sizeof(int), c->stream));
     } else {
         LILI_TRY(vg_minmax_dev(c, pts, m, nullptr, sizeof(float4)));
         int hb[kBoxInts];
@@ -131,25 +107,46 @@ int grid_build(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_b
     LILI_CUDA(c, c->grid_vals2.ensure((size_t)m * 4));
     LILI_CUDA(c, mi.sorted.ensure((size_t)m * sizeof(float4)));
     LILI_CUDA(c, mi.cell_start.ensure(((size_t)g.ncells + 2) * 4));
-    k_cell_keys<<<cdiv(m, 256), 256, 0, c->stream>>>(pts, m, g, c->grid_keys.as<uint32_t>(), c->grid_vals.as<int>(), escaped);
+    j.bits = 1;
+    while ((1LL << j.bits) < nc) ++j.bits;
+    return LILIOM_OK;
+}
+
+int grid_sort(const GridJob& j) {
+    liliom_ctx* c = j.c;
+    return sort_pairs_u32(c, c->grid_keys.as<uint32_t>(), c->grid_keys2.as<uint32_t>(), c->grid_vals.as<int>(), c->grid_vals2.as<int>(), j.m, j.bits);
+}
+
+int grid_clear(const GridJob& j) {
+    LILI_CUDA(j.c, cudaMemsetAsync(j.mi->cell_start.p, 0, ((size_t)j.mi->grid.ncells + 2) * 4, j.c->stream));
+    return LILIOM_OK;
+}
+
+int grid_scan(const GridJob& j) { return inclusive_max_scan_i32(j.c, j.mi->cell_start.as<int>(), j.mi->grid.ncells + 1); }
+
+int grid_finish(const GridJob& j, int esc) {
+    if (esc) return grid_build(j.c, *j.mi, j.cell, j.m, nullptr);
+    j.mi->ready = true;
+    return LILIOM_OK;
+}
+
+int grid_build(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_box) {
+    GridJob j;
+    LILI_TRY(grid_begin(c, mi, cell, m, host_box, j));
+    if (j.done) return LILIOM_OK;
+    float4* pts = mi.xyzw.as<float4>();
+    k_cell_keys<<<cdiv(m, 256), 256, 0, c->stream>>>(pts, m, mi.grid, c->grid_keys.as<uint32_t>(), c->grid_vals.as<int>(), j.escaped);
     LILI_TRY(launch_check(c, "k_cell_keys"));
-    int bits = 1;
-    while ((1LL << bits) < nc) ++bits;
-    LILI_TRY(sort_pairs_u32(c, c->grid_keys.as<uint32_t>(), c->grid_keys2.as<uint32_t>(), c->grid_vals.as<int>(),
-                            c->grid_vals2.as<int>(), m, bits));
+    LILI_TRY(grid_sort(j));
     k_gather_sorted<<<cdiv(m, 256), 256, 0, c->stream>>>(pts, c->grid_vals2.as<int>(), m, mi.sorted.as<float4>());
     LILI_TRY(launch_check(c, "k_gather_sorted"));
-    LILI_CUDA(c, cudaMemsetAsync(mi.cell_start.p, 0, ((size_t)g.ncells + 2) * 4, c->stream));
+    LILI_TRY(grid_clear(j));
     k_cell_run_ends<<<cdiv(m, 256), 256, 0, c->stream>>>(c->grid_keys2.as<uint32_t>(), m, mi.cell_start.as<int>());
     LILI_TRY(launch_check(c, "k_cell_run_ends"));
-    LILI_TRY(inclusive_max_scan_i32(c, mi.cell_start.as<int>(), g.ncells + 1));
-    if (escaped) {
-        int esc = 0;
-        LILI_TRY(read_back(c, {{&esc, escaped, sizeof(int)}}));
-        if (esc) return grid_build(c, mi, cell, m, nullptr);
-    }
-    mi.ready = true;
-    return LILIOM_OK;
+    LILI_TRY(grid_scan(j));
+    int esc = 0;
+    if (j.escaped) LILI_TRY(read_back(c, {{&esc, j.escaped, sizeof(int)}}));
+    return grid_finish(j, esc);
 }
 
 // ------------------------------------------------------------------ the hot kernel

@@ -156,6 +156,7 @@ static int kf_cloud_dev(liliom_ctx* c, const int* kf_ids, const double* poses7, 
     *n_in = off;
     if (off == 0) return LILIOM_OK;
     LILI_CUDA(c, c->bmap_raw.ensure((size_t)off * stride));      // scratch: the local map's layers live in bmap_ds / bmap
+    c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
     LILI_CUDA(c, c->vg_out.ensure((size_t)off * stride));
     LILI_TRY(kf_gather(c, c->kf_arena.p, tab, largest, c->bmap_raw.p));
     return voxelgrid_dev(c, c->bmap_raw.p, (int)off, nullptr, stride, leaf, c->vg_out.p, d_count);
@@ -202,6 +203,7 @@ extern "C" int liliom_kf_add(liliom_ctx* c, const liliom_backend_params* bp, con
     const long long n = (long long)n_edge + n_surf;
     LILI_TRY(kf_reserve(c, c->kf_arena, c->kf_used, c->kf_used + n));          // VoxelGrid never outputs more points than it reads
     LILI_CUDA(c, c->raw.ensure((size_t)(n > 0 ? n : 1) * stride));
+    c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
     LILI_CUDA(c, c->vg_out.ensure((size_t)(n_surf > 0 ? n_surf : 1) * stride));
     LILI_CUDA(c, c->vg_count.ensure(16));
     unsigned char* raw = (unsigned char*)c->raw.p;
@@ -426,6 +428,7 @@ extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, con
     const VgParams p = vg_params(box, leaf);
     if (p.overflow)                                               // PCL declines the filter and publishes its input
         return download_sized(c, c->vg_out, (int)N, stride, out, cap, n, [&]() -> int {
+            c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
             LILI_CUDA(c, c->vg_out.ensure((size_t)N * stride));
             return kf_gather(c, arena, tab, largest, c->vg_out.p);
         });
@@ -449,6 +452,7 @@ extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, con
     int m = 0;
     LILI_TRY(read_back(c, {{&m, c->vg_rank.as<int>() + n_fin, sizeof(int)}}));
     return download_sized(c, c->vg_out, m, stride, out, cap, n, [&]() -> int {
+        c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
         LILI_CUDA(c, c->vg_out.ensure((size_t)m * stride));
         if (stride == 48)
             k_kf_centroid<48><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(),

@@ -27,8 +27,6 @@
 
 namespace lili {
 
-__device__ __forceinline__ int cell_coord(float v, float inv_cell) { return (int)floorf(v * inv_cell); }
-
 // Ownership of a point for the sharded map: space is cut into cubes of 1/inv_block metres (a power of two, default 16 m)
 // and the cube's hash picks the rank (SURVEY.md §8 e).  The hash is linear, h = bx + 3 by + 5 bz (mod nranks): over any
 // rectangular stretch of cubes every rank gets the same share (a multiplicative hash left one of 8 ranks 20 % and another

@@ -25,8 +25,10 @@
 #include "ctx.cuh"
 #include "dev_math.cuh"
 #include "knn_core.cuh"
+#include "map_stage.h"
 #include <algorithm>
 #include <climits>
+#include <vector>
 #include <ctime>
 
 namespace lili {
@@ -63,11 +65,16 @@ __global__ void k_compact_repack(const unsigned char* __restrict__ in, const int
     out[pos[i]] = v;
 }
 
-// transformCloud (L/src/LidarOdometry.cpp:246-278; R/src/LidarOdometry.cpp:239-264)
-__global__ void k_transform_cloud(const unsigned char* __restrict__ in, int n, int stride, Q4 q, D3 t, unsigned char* __restrict__ out) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
+// transformCloud (L/src/LidarOdometry.cpp:246-278; R/src/LidarOdometry.cpp:239-264).  Every kernel of the map update has its body in
+// a function of `i`, the thread's place in its session's launch: the solo kernel passes blockIdx.x * blockDim.x + threadIdx.x,
+// the batched update (k_map_stage_batch below) the same place counted from its session's first block.
+__device__ __forceinline__ void transform_cloud_at(const unsigned char* __restrict__ in, int n, int stride, const Q4& q, const D3& t,
+                                                   unsigned char* __restrict__ out, const int i) {
     if (i >= n) return;
     pcl_transform_point(in + (size_t)i * stride, stride, q, t, out + (size_t)i * stride);
+}
+__global__ void k_transform_cloud(const unsigned char* __restrict__ in, int n, int stride, Q4 q, D3 t, unsigned char* __restrict__ out) {
+    transform_cloud_at(in, n, stride, q, t, out, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
 // Concatenation of the FIFO frames (L/src/LidarOdometry.cpp:301-302), up to kConcatMax frames per launch: blockIdx.y = frame,
@@ -90,9 +97,8 @@ struct FrameTab { const unsigned char* base[kIncSlots]; };
 
 // keys of one frame's points (world frame, already transformed), refs = slot << 24 | index; *bad |= 1 when a voxel coordinate
 // does not fit 21 bits (the frame's box and finite count were measured at its push: Frame::mm)
-__global__ void k_inc_keys(const unsigned char* __restrict__ pts, int n, int stride, float inv_leaf, unsigned slot, u64* __restrict__ keys,
-                           unsigned* __restrict__ refs, int* __restrict__ bad) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void inc_keys_at(const unsigned char* __restrict__ pts, int n, int stride, float inv_leaf, unsigned slot,
+                                            u64* __restrict__ keys, unsigned* __restrict__ refs, int* __restrict__ bad, const int i) {
     bool miss = false;
     if (i < n) {
         const float4 v = *reinterpret_cast<const float4*>(pts + (size_t)i * stride);
@@ -102,6 +108,10 @@ __global__ void k_inc_keys(const unsigned char* __restrict__ pts, int n, int str
         refs[i] = (slot << 24) | (unsigned)i;
     }
     if (__any_sync(0xffffffffu, miss) && (threadIdx.x & 31) == 0) atomicOr(bad, 1);
+}
+__global__ void k_inc_keys(const unsigned char* __restrict__ pts, int n, int stride, float inv_leaf, unsigned slot, u64* __restrict__ keys,
+                           unsigned* __restrict__ refs, int* __restrict__ bad) {
+    inc_keys_at(pts, n, stride, inv_leaf, slot, keys, refs, bad, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
 __device__ __forceinline__ int lower_bound_u64(const u64* __restrict__ a, int n, u64 k) {      // first i with a[i] >= k
@@ -116,18 +126,19 @@ __device__ __forceinline__ int upper_bound_u64(const u64* __restrict__ a, int n,
 }
 
 // removed[i] = 1 for the entries of the frame slot that leaves the FIFO; removed[E] = 0 (scan sentinel)
-__global__ void k_inc_mark(const unsigned* __restrict__ refs, int E, int popped, int* __restrict__ removed) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void inc_mark_at(const unsigned* __restrict__ refs, int E, int popped, int* __restrict__ removed, const int i) {
     if (i > E) return;
     removed[i] = (i < E && popped >= 0 && (int)(refs[i] >> 24) == popped) ? 1 : 0;
+}
+__global__ void k_inc_mark(const unsigned* __restrict__ refs, int E, int popped, int* __restrict__ removed) {
+    inc_mark_at(refs, E, popped, removed, blockIdx.x * blockDim.x + threadIdx.x);
 }
 // surviving old entries: down by the removed entries before them, up by the new entries with a smaller key.  The entries of a
 // warp are consecutive in a sorted array, so their lower bounds in the new keys are nested between those of lanes 0 and 31:
 // two full binary searches per warp, then every lane searches only the (short) range between them.
-__global__ void k_inc_merge_old(const u64* __restrict__ keys, const unsigned* __restrict__ refs, const int* __restrict__ removed,
-                                const int* __restrict__ rpos, int E, const u64* __restrict__ newkeys, int nnew, u64* __restrict__ keys2,
-                                unsigned* __restrict__ refs2) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void inc_merge_old_at(const u64* __restrict__ keys, const unsigned* __restrict__ refs, const int* __restrict__ removed,
+                                                 const int* __restrict__ rpos, int E, const u64* __restrict__ newkeys, int nnew,
+                                                 u64* __restrict__ keys2, unsigned* __restrict__ refs2, const int i) {
     const int lane = threadIdx.x & 31;
     const int ic = min(i, E - 1);
     const u64 k = keys[ic];
@@ -139,27 +150,120 @@ __global__ void k_inc_merge_old(const u64* __restrict__ keys, const unsigned* __
     const int pos = i - rpos[i] + lb;
     keys2[pos] = k; refs2[pos] = refs[i];
 }
+__global__ void k_inc_merge_old(const u64* __restrict__ keys, const unsigned* __restrict__ refs, const int* __restrict__ removed,
+                                const int* __restrict__ rpos, int E, const u64* __restrict__ newkeys, int nnew, u64* __restrict__ keys2,
+                                unsigned* __restrict__ refs2) {
+    inc_merge_old_at(keys, refs, removed, rpos, E, newkeys, nnew, keys2, refs2, blockIdx.x * blockDim.x + threadIdx.x);
+}
 // new entries (sorted by key, then index): behind every surviving old entry with key <= their own
-__global__ void k_inc_merge_new(const u64* __restrict__ newkeys, const unsigned* __restrict__ newrefs, int nnew, const u64* __restrict__ keys,
-                                const int* __restrict__ rpos, int E, u64* __restrict__ keys2, unsigned* __restrict__ refs2) {
-    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void inc_merge_new_at(const u64* __restrict__ newkeys, const unsigned* __restrict__ newrefs, int nnew,
+                                                 const u64* __restrict__ keys, const int* __restrict__ rpos, int E, u64* __restrict__ keys2,
+                                                 unsigned* __restrict__ refs2, const int j) {
     if (j >= nnew) return;
     const u64 k = newkeys[j];
     const int ub = upper_bound_u64(keys, E, k);
     const int pos = j + (ub - rpos[ub]);
     keys2[pos] = k; refs2[pos] = newrefs[j];
 }
+__global__ void k_inc_merge_new(const u64* __restrict__ newkeys, const unsigned* __restrict__ newrefs, int nnew, const u64* __restrict__ keys,
+                                const int* __restrict__ rpos, int E, u64* __restrict__ keys2, unsigned* __restrict__ refs2) {
+    inc_merge_new_at(newkeys, newrefs, nnew, keys, rpos, E, keys2, refs2, blockIdx.x * blockDim.x + threadIdx.x);
+}
 // centroid of every voxel, members in entry order (vg_box.h), the points fetched through the frame table
 template <int STRIDE>
-__global__ void k_inc_centroid(const __grid_constant__ FrameTab tab, const u64* __restrict__ keys, const unsigned* __restrict__ refs,
-                               const int* __restrict__ flags, const int* __restrict__ rank, int E, unsigned char* __restrict__ out,
-                               int* __restrict__ count_out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+__device__ __forceinline__ void inc_centroid_at(const FrameTab& tab, const u64* __restrict__ keys, const unsigned* __restrict__ refs,
+                                                const int* __restrict__ flags, const int* __restrict__ rank, int E,
+                                                unsigned char* __restrict__ out, int* __restrict__ count_out, const int i) {
     if (i == 0) *count_out = rank[E];
     if (i >= E || !flags[i]) return;
     const VgAcc<STRIDE> a = vg_walk<STRIDE>(keys, i, E, [&](int j) { return (int)refs[j]; },       // (slot < 64: a ref is below 2^30)
                                             [&](int r) { return tab.base[r >> 24] + (size_t)(r & kIncIdxMask) * STRIDE; });
     vg_write<STRIDE>(a.s, a.n, out + (size_t)rank[i] * STRIDE);
+}
+template <int STRIDE>
+__global__ void k_inc_centroid(const __grid_constant__ FrameTab tab, const u64* __restrict__ keys, const unsigned* __restrict__ refs,
+                               const int* __restrict__ flags, const int* __restrict__ rank, int E, unsigned char* __restrict__ out,
+                               int* __restrict__ count_out) {
+    inc_centroid_at<STRIDE>(tab, keys, refs, flags, rank, E, out, count_out, blockIdx.x * blockDim.x + threadIdx.x);
+}
+
+// ---- the map update of several sessions (liliom_map_update_batch): one launch per stage for up to kBatchMax sessions.
+// Everything one session's stages read or write, on its own buffers; the host parts of the update fill it as they go (MapJob).
+struct MapEntry {
+    // the new frame: transform, box, keys
+    const unsigned char* src; unsigned char* fbuf; int n, stride; Q4 q; D3 t; int* mm; int mm_blocks;
+    float inv_leaf; unsigned slot; u64* newkey; unsigned* newref; int* bad;
+    // merge into the entry array
+    const u64* keys; const unsigned* refs; int E, popped; int* removed; int* rpos; const u64* snewkey; const unsigned* snewref; int nnew;
+    u64* keys2; unsigned* refs2;
+    // voxel heads and centroids of the entry array (ekeys / erefs, E2 entries)
+    const u64* ekeys; const unsigned* erefs; int E2; int* flags; int* rank; unsigned char* ds; int* count;
+    // search index of the m filtered points
+    int m; float4* xyzw; GridDesc g; uint32_t* gkeys; int* gvals; int* escaped; const uint32_t* gkeys2; const int* gvals2; float4* sorted;
+    int* cell_start;
+};
+struct MapTab {
+    int n;                              // sessions in this launch
+    MapEntry s[kBatchMax];
+};
+static_assert(sizeof(MapTab) <= 32764, "k_map_stage_batch's session table must fit in the kernel parameter space");
+// The centroid stage also needs each session's frame pointers
+struct MapCentroidEntry {
+    FrameTab tab;
+    const u64* ekeys; const unsigned* erefs; int E2, stride; const int* flags; const int* rank; unsigned char* ds; int* count;
+};
+struct MapCentroidTab {
+    int n;
+    MapCentroidEntry s[kBatchMax];
+};
+static_assert(sizeof(MapCentroidTab) <= 32764, "the centroid stage's session table must fit in the kernel parameter space");
+
+// One stage of the update: its block size, its blocks for a session and its body, each as the solo launch has them.  Session s
+// owns the blocks after those of sessions 0 .. s-1.  The entry is copied by value, as the solo kernels' parameters are.
+#define LILI_MAP_STAGE(NAME, THREADS, BLOCKS, CALL)                                                   \
+    struct NAME {                                                                                     \
+        typedef MapTab Tab;                                                                           \
+        static constexpr int kThreads = THREADS;                                                      \
+        __host__ __device__ static int blocks(const MapEntry& e) { return BLOCKS; }                   \
+        __device__ static void run(const MapEntry& te, int bx) {                                      \
+            const MapEntry e = te;                                                                    \
+            const int i = bx * THREADS + (int)threadIdx.x;                                            \
+            (void)i;                                                                                  \
+            CALL;                                                                                     \
+        }                                                                                             \
+    };
+LILI_MAP_STAGE(MapStTransform, 256, stage_blocks(e.n, 256), transform_cloud_at(e.src, e.n, e.stride, e.q, e.t, e.fbuf, i))
+LILI_MAP_STAGE(MapStBoxInit, 32, 1, vg_box_init(e.mm))
+LILI_MAP_STAGE(MapStBox, 256, e.mm_blocks, vg_minmax_body(e.fbuf, e.n, nullptr, e.stride, e.mm, SessionBlock{bx, (unsigned)e.mm_blocks}))
+LILI_MAP_STAGE(MapStKeys, 256, stage_blocks(e.n, 256), inc_keys_at(e.fbuf, e.n, e.stride, e.inv_leaf, e.slot, e.newkey, e.newref, e.bad, i))
+LILI_MAP_STAGE(MapStMark, 256, stage_blocks(e.E + 1, 256), inc_mark_at(e.refs, e.E, e.popped, e.removed, i))
+LILI_MAP_STAGE(MapStMergeOld, 256, stage_blocks(e.E, 256),
+               inc_merge_old_at(e.keys, e.refs, e.removed, e.rpos, e.E, e.snewkey, e.nnew, e.keys2, e.refs2, i))
+LILI_MAP_STAGE(MapStMergeNew, 256, stage_blocks(e.nnew, 256),
+               inc_merge_new_at(e.snewkey, e.snewref, e.nnew, e.keys, e.rpos, e.E, e.keys2, e.refs2, i))
+LILI_MAP_STAGE(MapStHeads, 256, stage_blocks(e.E2 + 1, 256), vg_heads_at(e.ekeys, e.E2, (const int*)nullptr, e.flags, i))
+LILI_MAP_STAGE(MapStRepack, 256, stage_blocks(e.m, 256), repack_f4_at(e.ds, e.m, nullptr, e.stride, e.xyzw, i))
+LILI_MAP_STAGE(MapStCellKeys, 256, stage_blocks(e.m, 256), cell_keys_at(e.xyzw, e.m, e.g, e.gkeys, e.gvals, e.escaped, i))
+LILI_MAP_STAGE(MapStGather, 256, stage_blocks(e.m, 256), gather_sorted_at(e.xyzw, e.gvals2, e.m, e.sorted, i))
+LILI_MAP_STAGE(MapStRunEnds, 256, stage_blocks(e.m, 256), cell_run_ends_at(e.gkeys2, e.m, e.cell_start, i))
+#undef LILI_MAP_STAGE
+// The centroids: the scalars by value, the 512-byte frame table read in place from the parameter space (as k_inc_centroid reads its own)
+template <int STRIDE>
+struct MapStCentroid {
+    typedef MapCentroidTab Tab;
+    static constexpr int kThreads = 128;
+    __host__ __device__ static int blocks(const MapCentroidEntry& e) { return stage_blocks(e.E2, 128); }
+    __device__ static void run(const MapCentroidEntry& te, int bx) {
+        const u64* ekeys = te.ekeys; const unsigned* erefs = te.erefs; const int* flags = te.flags; const int* rank = te.rank;
+        inc_centroid_at<STRIDE>(te.tab, ekeys, erefs, flags, rank, te.E2, te.ds, te.count, bx * 128 + (int)threadIdx.x);
+    }
+};
+
+template <class St>
+__global__ void __launch_bounds__(St::kThreads) k_map_stage_batch(const __grid_constant__ typename St::Tab tab) {
+    int b = (int)blockIdx.x;
+    const int s = batch_session_of(tab.n, b, [&](int k) { return St::blocks(tab.s[k]); });
+    St::run(tab.s[s], b);
 }
 
 // ---- host side
@@ -226,42 +330,79 @@ int map_install_host(liliom_ctx* c, const void* pts, int m, int stride, bool kee
 // The frame that left the FIFO in a push: its slot and finite count (slot -1, count 0: none left).
 struct Popped { int slot = -1, nfin = 0; };
 
-// Shared body of the push entry points: d_src = n body-frame points of point_stride bytes ON THE DEVICE.
-static int push_frame_from_device(liliom_ctx* c, const void* d_src, int n, const double pose7[7], bool keep_inc = false,
-                                  Popped* popped = nullptr) {
+// One map update in flight.  The update is written in parts so that the solo call and the batched one (map_update_batch) run
+// the same host code: each *_begin part takes the host's decisions (FIFO, buffer sizes, fall-backs) from the words read back so
+// far and fills the kernel arguments in `e`; the launches between the parts are the solo kernels here and the shared stage
+// launches there.
+struct MapJob {
+    liliom_ctx* c = nullptr;
+    Frame f;                            // the frame being pushed, until push_end moves it into the FIFO
+    Popped popped;
+    MapEntry e{};
+    FrameTab ft{};
+    GridJob g;
+    int m = 0;                          // voxels of the filtered cloud
+};
+
+// Push, part 1: the FIFO makes room (L/src/LidarOdometry.cpp:293-296 pop_front) and the new frame gets its buffer.
+static int push_begin(liliom_ctx* c, const void* d_src, int n, const double pose7[7], bool keep_inc, MapJob& j) {
     const int stride = c->prm.point_stride;
+    j.c = c;
     if (!keep_inc) c->inc_valid = false;        // the entry array of liliom_map_update no longer describes the FIFO
-    Frame f;
+    Frame& f = j.f;
     f.slot = (int)c->frames.size();
-    if ((int)c->frames.size() >= c->prm.max_map_frames && !c->frames.empty()) {      // L/src/LidarOdometry.cpp:293-296 pop_front
+    if ((int)c->frames.size() >= c->prm.max_map_frames && !c->frames.empty()) {
         Frame& old = c->frames.front();
-        if (popped) *popped = Popped{old.slot, old.mm[6]};
+        j.popped = Popped{old.slot, old.mm[6]};
         f.buf = std::move(old.buf);             // the popped frame's allocation is recycled: cudaFree + cudaMalloc per scan cost
         f.slot = old.slot;                      // more than the whole map maintenance of a 10 M-point map (cudaFree synchronises)
         c->frames.erase(c->frames.begin());
     }
     f.n = n;
     if (n > 0) {
-        const Q4 q{pose7[0], pose7[1], pose7[2], pose7[3]};
-        const D3 t{pose7[4], pose7[5], pose7[6]};
         LILI_CUDA(c, f.buf.ensure((size_t)n * stride));
+        LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
+    }
+    MapEntry& e = j.e;
+    e.src = (const unsigned char*)d_src; e.fbuf = (unsigned char*)f.buf.p; e.n = n; e.stride = stride;
+    e.q = Q4{pose7[0], pose7[1], pose7[2], pose7[3]};
+    e.t = D3{pose7[4], pose7[5], pose7[6]};
+    e.mm = c->vg_minmax.as<int>();
+    e.mm_blocks = box_blocks(n, c->sm_count);     // vg_minmax_dev's grid
+    return LILIOM_OK;
+}
+// Push, part 2: the frame's box as read back (nullptr: an empty frame keeps the empty box) and its place in the FIFO.
+static void push_end(MapJob& j, const int* mm) {
+    if (mm) memcpy(j.f.mm, mm, kBoxInts * sizeof(int));
+    j.c->frames.push_back(std::move(j.f));
+}
+
+// Shared body of the push entry points: d_src = n body-frame points of point_stride bytes ON THE DEVICE.
+static int push_frame_from_device(liliom_ctx* c, const void* d_src, int n, const double pose7[7], bool keep_inc = false,
+                                  Popped* popped = nullptr) {
+    MapJob j;
+    LILI_TRY(push_begin(c, d_src, n, pose7, keep_inc, j));
+    if (popped) *popped = j.popped;
+    const MapEntry& e = j.e;
+    Frame& f = j.f;
+    if (n > 0) {
         if (c->nranks == 1) {
-            k_transform_cloud<<<cdiv(n, 256), 256, 0, c->stream>>>((const unsigned char*)d_src, n, stride, q, t, (unsigned char*)f.buf.p);
+            k_transform_cloud<<<cdiv(n, 256), 256, 0, c->stream>>>(e.src, n, e.stride, e.q, e.t, e.fbuf);
             LILI_TRY(launch_check(c, "k_transform_cloud"));
-            LILI_TRY(vg_minmax_dev(c, f.buf.p, n, nullptr, stride));                 // the frame's box, for the rebuilds it takes part in
+            LILI_TRY(vg_minmax_dev(c, f.buf.p, n, nullptr, e.stride));                 // the frame's box, for the rebuilds it takes part in
             LILI_TRY(read_back(c, {{f.mm, c->vg_minmax.p, kBoxInts * sizeof(int)}}));
         } else {
             // sharded map maintenance: every rank receives the frame, keeps the points within (search radius + one voxel
             // diagonal) of a block it owns — every voxel that can reach an owned query's 1 m ball is then complete locally —
             // and voxel-filters / indexes only its shard.  No inter-rank traffic.
-            LILI_CUDA(c, c->map_ds.ensure((size_t)n * stride));
-            k_transform_cloud<<<cdiv(n, 256), 256, 0, c->stream>>>((const unsigned char*)d_src, n, stride, q, t, (unsigned char*)c->map_ds.p);
+            LILI_CUDA(c, c->map_ds.ensure((size_t)n * e.stride));
+            k_transform_cloud<<<cdiv(n, 256), 256, 0, c->stream>>>(e.src, n, e.stride, e.q, e.t, (unsigned char*)c->map_ds.p);
             LILI_TRY(launch_check(c, "k_transform_cloud"));
             const float halo = gate_cell(c->prm.knn_max_sqdist) + 1.7320508f * c->prm.leaf_map + 0.05f;
-            LILI_TRY(shard_filter(c, c->map_ds.p, n, stride, halo, f.buf.p, false, &f.n, f.mm));      // box of the points this rank keeps
+            LILI_TRY(shard_filter(c, c->map_ds.p, n, e.stride, halo, f.buf.p, false, &f.n, f.mm));      // box of the points this rank keeps
         }
     }
-    c->frames.push_back(std::move(f));
+    push_end(j, nullptr);
     return LILIOM_OK;
 }
 
@@ -271,13 +412,19 @@ static void frames_box(const liliom_ctx* c, int mm[kBoxInts]) {
     for (const auto& f : c->frames) vg_box_merge(mm, f.mm);
 }
 
-// tail of the incremental update (single GPU): c->map_ds holds m filtered points
-static int map_finish_from_ds(liliom_ctx* c, int m) {
-    const int stride = c->prm.point_stride;
+// Tail of the incremental update (single GPU), part 1: c->map_ds holds m filtered points; sizes the float4 map for the repack.
+static int finish_begin(liliom_ctx* c, int m, MapEntry& e) {
     LILI_CUDA(c, c->map.xyzw.ensure((size_t)(m > 0 ? m : 1) * sizeof(float4)));
     c->map_n_global = m;
     c->map_ds_n = m;
-    LILI_TRY(repack_to_f4(c, c->map_ds.p, m, stride, c->map.xyzw.as<float4>()));
+    e.ds = (unsigned char*)c->map_ds.p; e.m = m; e.stride = c->prm.point_stride; e.xyzw = c->map.xyzw.as<float4>();
+    return LILIOM_OK;
+}
+
+static int map_finish_from_ds(liliom_ctx* c, int m) {
+    MapEntry e{};
+    LILI_TRY(finish_begin(c, m, e));
+    LILI_TRY(repack_to_f4(c, e.ds, m, e.stride, e.xyzw));
     int mm[kBoxInts];
     frames_box(c, mm);
     LILI_TRY(grid_build(c, m, mm[6] > 0 ? mm : nullptr));
@@ -285,18 +432,26 @@ static int map_finish_from_ds(liliom_ctx* c, int m) {
     return LILIOM_OK;
 }
 
-// keys + refs of frame `f` (points already in f.buf), written at keys/refs, and its key flag; one sync
-static int inc_frame_keys(liliom_ctx* c, Frame& f, u64* keys, unsigned* refs) {
-    const int stride = c->prm.point_stride;
+// keys + refs of frame `f` (points already in f.buf) go to keys / refs and its key flag to c->inc_bad: the flag cleared, the
+// arguments of k_inc_keys in `e`
+static int inc_keys_begin(liliom_ctx* c, const Frame& f, u64* keys, unsigned* refs, MapEntry& e) {
     LILI_CUDA(c, c->inc_bad.ensure(sizeof(int)));
-    int* bad = c->inc_bad.as<int>();
-    LILI_CUDA(c, cudaMemsetAsync(bad, 0, sizeof(int), c->stream));
+    e.fbuf = (unsigned char*)f.buf.p; e.n = f.n; e.stride = c->prm.point_stride;
+    e.inv_leaf = 1.0f / c->prm.leaf_map; e.slot = (unsigned)f.slot; e.newkey = keys; e.newref = refs; e.bad = c->inc_bad.as<int>();
+    LILI_CUDA(c, cudaMemsetAsync(e.bad, 0, sizeof(int), c->stream));
+    return LILIOM_OK;
+}
+
+// keys + refs of frame `f`, written at keys/refs, and its key flag; one sync
+static int inc_frame_keys(liliom_ctx* c, Frame& f, u64* keys, unsigned* refs) {
+    MapEntry e{};
+    LILI_TRY(inc_keys_begin(c, f, keys, refs, e));
     if (f.n > 0) {
-        k_inc_keys<<<cdiv(f.n, 256), 256, 0, c->stream>>>((const unsigned char*)f.buf.p, f.n, stride, 1.0f / c->prm.leaf_map, (unsigned)f.slot, keys, refs, bad);
+        k_inc_keys<<<cdiv(f.n, 256), 256, 0, c->stream>>>(e.fbuf, e.n, e.stride, e.inv_leaf, e.slot, e.newkey, e.newref, e.bad);
         LILI_TRY(launch_check(c, "k_inc_keys"));
     }
     int flag = 0;
-    LILI_TRY(read_back(c, {{&flag, bad, sizeof(int)}}));
+    LILI_TRY(read_back(c, {{&flag, e.bad, sizeof(int)}}));
     f.bad = flag != 0;
     return LILIOM_OK;
 }
@@ -332,29 +487,75 @@ static int inc_build_all(liliom_ctx* c) {
     return LILIOM_OK;
 }
 
-// heads -> ranks -> centroids of the current entry array into c->map_ds; m = number of voxels
-static int inc_emit(liliom_ctx* c, int* m_out) {
+// Emit, part 1: heads -> ranks -> centroids of the current entry array go into c->map_ds.  e.E2 = 0: nothing to launch.
+static int inc_emit_begin(liliom_ctx* c, MapEntry& e, FrameTab& ft) {
     const int stride = c->prm.point_stride;
     const int E = c->inc_E;
-    *m_out = 0;
+    e.E2 = 0;
     LILI_CUDA(c, c->map_ds.ensure((size_t)(E > 0 ? E : 1) * stride));
     LILI_CUDA(c, c->vg_count.ensure(16));
     if (E == 0) return LILIOM_OK;
     LILI_CUDA(c, c->inc_flags.ensure(((size_t)E + 2) * 4));
     LILI_CUDA(c, c->inc_rank.ensure(((size_t)E + 2) * 4));
-    const u64* keys = c->inc_key[c->inc_cur].as<u64>();
-    const unsigned* refs = c->inc_ref[c->inc_cur].as<unsigned>();
-    k_vg_heads<<<cdiv(E + 1, 256), 256, 0, c->stream>>>(keys, E, nullptr, c->inc_flags.as<int>());
+    e.ekeys = c->inc_key[c->inc_cur].as<u64>(); e.erefs = c->inc_ref[c->inc_cur].as<unsigned>(); e.E2 = E; e.stride = stride;
+    e.flags = c->inc_flags.as<int>(); e.rank = c->inc_rank.as<int>(); e.ds = (unsigned char*)c->map_ds.p; e.count = c->vg_count.as<int>();
+    ft = FrameTab{};
+    for (auto& f : c->frames) ft.base[f.slot] = (const unsigned char*)f.buf.p;
+    return LILIOM_OK;
+}
+
+// heads -> ranks -> centroids of the current entry array into c->map_ds; m = number of voxels
+static int inc_emit(liliom_ctx* c, int* m_out) {
+    MapEntry e{};
+    FrameTab tab;
+    *m_out = 0;
+    LILI_TRY(inc_emit_begin(c, e, tab));
+    const int E = e.E2;
+    if (E == 0) return LILIOM_OK;
+    k_vg_heads<<<cdiv(E + 1, 256), 256, 0, c->stream>>>(e.ekeys, E, nullptr, e.flags);
     LILI_TRY(launch_check(c, "k_vg_heads"));
-    LILI_TRY(exclusive_scan_i32(c, c->inc_flags.as<int>(), c->inc_rank.as<int>(), E));
-    FrameTab tab{};
-    for (auto& f : c->frames) tab.base[f.slot] = (const unsigned char*)f.buf.p;
-    if (stride == 48)
-        k_inc_centroid<48><<<cdiv(E, 128), 128, 0, c->stream>>>(tab, keys, refs, c->inc_flags.as<int>(), c->inc_rank.as<int>(), E, (unsigned char*)c->map_ds.p, c->vg_count.as<int>());
+    LILI_TRY(exclusive_scan_i32(c, e.flags, e.rank, E));
+    if (e.stride == 48)
+        k_inc_centroid<48><<<cdiv(E, 128), 128, 0, c->stream>>>(tab, e.ekeys, e.erefs, e.flags, e.rank, E, e.ds, e.count);
     else
-        k_inc_centroid<32><<<cdiv(E, 128), 128, 0, c->stream>>>(tab, keys, refs, c->inc_flags.as<int>(), c->inc_rank.as<int>(), E, (unsigned char*)c->map_ds.p, c->vg_count.as<int>());
+        k_inc_centroid<32><<<cdiv(E, 128), 128, 0, c->stream>>>(tab, e.ekeys, e.erefs, e.flags, e.rank, E, e.ds, e.count);
     LILI_TRY(launch_check(c, "k_inc_centroid"));
-    return read_back(c, {{m_out, c->vg_count.p, sizeof(int)}});
+    return read_back(c, {{m_out, e.count, sizeof(int)}});
+}
+
+// New frame (at the back of c->frames), part 1: where its keys and refs go, unsorted
+static int inc_new_begin(liliom_ctx* c, MapEntry& e) {
+    Frame& fn = c->frames.back();
+    const size_t ncap = (size_t)(fn.n > 0 ? fn.n : 1);
+    for (int b = 0; b < 2; ++b) {
+        LILI_CUDA(c, c->inc_newkey[b].ensure(ncap * sizeof(u64) + 64));
+        LILI_CUDA(c, c->inc_newref[b].ensure(ncap * sizeof(unsigned) + 64));
+    }
+    return inc_keys_begin(c, fn, c->inc_newkey[0].as<u64>(), c->inc_newref[0].as<unsigned>(), e);
+}
+
+// Merge, part 1 (the keys are representable): the new frame's entries sorted on their own, the next entry array sized
+static int inc_merge_begin(liliom_ctx* c, const Popped& popped, MapEntry& e) {
+    Frame& fn = c->frames.back();
+    const int E = c->inc_E, nnew = fn.mm[6];
+    if (fn.n > 0)
+        LILI_TRY(sort_pairs_u64(c, c->inc_newkey[0].as<u64>(), c->inc_newkey[1].as<u64>(), c->inc_newref[0].as<int>(), c->inc_newref[1].as<int>(), fn.n, 64));
+    const int E2 = E - popped.nfin + nnew;
+    const int cur = c->inc_cur, nxt = cur ^ 1;
+    LILI_CUDA(c, c->inc_key[nxt].ensure((size_t)(E2 > 0 ? E2 : 1) * sizeof(u64) + 64));
+    LILI_CUDA(c, c->inc_ref[nxt].ensure((size_t)(E2 > 0 ? E2 : 1) * sizeof(unsigned) + 64));
+    LILI_CUDA(c, c->inc_removed.ensure(((size_t)E + 2) * 4));
+    LILI_CUDA(c, c->inc_rpos.ensure(((size_t)E + 2) * 4));
+    e.keys = c->inc_key[cur].as<u64>(); e.refs = c->inc_ref[cur].as<unsigned>(); e.E = E; e.popped = popped.slot;
+    e.removed = c->inc_removed.as<int>(); e.rpos = c->inc_rpos.as<int>();
+    e.snewkey = c->inc_newkey[1].as<u64>(); e.snewref = c->inc_newref[1].as<unsigned>(); e.nnew = nnew;
+    e.keys2 = c->inc_key[nxt].as<u64>(); e.refs2 = c->inc_ref[nxt].as<unsigned>(); e.E2 = E2;
+    return LILIOM_OK;
+}
+// Merge, part 2 (the merge kernels are queued): the merged array is the current one
+static void inc_merge_end(liliom_ctx* c, const MapEntry& e) {
+    c->inc_cur ^= 1;
+    c->inc_E = e.E2;
 }
 
 // The frame at the back of c->frames has just been pushed (points in its buffer, slot assigned); `popped` is the frame that
@@ -367,39 +568,32 @@ static int map_inc_update(liliom_ctx* c, const Popped& popped, int* m_out) {
         c->inc_valid = true;
         return inc_emit(c, m_out);
     }
+    MapEntry e{};
     {   // new frame: keys, refs, key flag; sorted on its own below
-        const size_t ncap = (size_t)(fn.n > 0 ? fn.n : 1);
-        for (int b = 0; b < 2; ++b) {
-            LILI_CUDA(c, c->inc_newkey[b].ensure(ncap * sizeof(u64) + 64));
-            LILI_CUDA(c, c->inc_newref[b].ensure(ncap * sizeof(unsigned) + 64));
+        LILI_TRY(inc_new_begin(c, e));
+        if (fn.n > 0) {
+            k_inc_keys<<<cdiv(fn.n, 256), 256, 0, c->stream>>>(e.fbuf, e.n, e.stride, e.inv_leaf, e.slot, e.newkey, e.newref, e.bad);
+            LILI_TRY(launch_check(c, "k_inc_keys"));
         }
-        LILI_TRY(inc_frame_keys(c, fn, c->inc_newkey[0].as<u64>(), c->inc_newref[0].as<unsigned>()));
+        int flag = 0;
+        LILI_TRY(read_back(c, {{&flag, e.bad, sizeof(int)}}));
+        fn.bad = flag != 0;
     }
     if (!inc_representable(c)) { c->inc_valid = false; return LILIOM_E_GRID; }
-    const int E = c->inc_E, nnew = fn.mm[6];
-    if (fn.n > 0)
-        LILI_TRY(sort_pairs_u64(c, c->inc_newkey[0].as<u64>(), c->inc_newkey[1].as<u64>(), c->inc_newref[0].as<int>(), c->inc_newref[1].as<int>(), fn.n, 64));
-    const int E2 = E - popped.nfin + nnew;
-    const int cur = c->inc_cur, nxt = cur ^ 1;
-    LILI_CUDA(c, c->inc_key[nxt].ensure((size_t)(E2 > 0 ? E2 : 1) * sizeof(u64) + 64));
-    LILI_CUDA(c, c->inc_ref[nxt].ensure((size_t)(E2 > 0 ? E2 : 1) * sizeof(unsigned) + 64));
-    LILI_CUDA(c, c->inc_removed.ensure(((size_t)E + 2) * 4));
-    LILI_CUDA(c, c->inc_rpos.ensure(((size_t)E + 2) * 4));
-    k_inc_mark<<<cdiv(E + 1, 256), 256, 0, c->stream>>>(c->inc_ref[cur].as<unsigned>(), E, popped.slot, c->inc_removed.as<int>());
+    LILI_TRY(inc_merge_begin(c, popped, e));
+    const int E = e.E, nnew = e.nnew;
+    k_inc_mark<<<cdiv(E + 1, 256), 256, 0, c->stream>>>(e.refs, E, e.popped, e.removed);
     LILI_TRY(launch_check(c, "k_inc_mark"));
-    LILI_TRY(exclusive_scan_i32(c, c->inc_removed.as<int>(), c->inc_rpos.as<int>(), E));
+    LILI_TRY(exclusive_scan_i32(c, e.removed, e.rpos, E));
     if (E > 0) {
-        k_inc_merge_old<<<cdiv(E, 256), 256, 0, c->stream>>>(c->inc_key[cur].as<u64>(), c->inc_ref[cur].as<unsigned>(), c->inc_removed.as<int>(), c->inc_rpos.as<int>(), E,
-                                                            c->inc_newkey[1].as<u64>(), nnew, c->inc_key[nxt].as<u64>(), c->inc_ref[nxt].as<unsigned>());
+        k_inc_merge_old<<<cdiv(E, 256), 256, 0, c->stream>>>(e.keys, e.refs, e.removed, e.rpos, E, e.snewkey, nnew, e.keys2, e.refs2);
         LILI_TRY(launch_check(c, "k_inc_merge_old"));
     }
     if (nnew > 0) {
-        k_inc_merge_new<<<cdiv(nnew, 256), 256, 0, c->stream>>>(c->inc_newkey[1].as<u64>(), c->inc_newref[1].as<unsigned>(), nnew, c->inc_key[cur].as<u64>(),
-                                                               c->inc_rpos.as<int>(), E, c->inc_key[nxt].as<u64>(), c->inc_ref[nxt].as<unsigned>());
+        k_inc_merge_new<<<cdiv(nnew, 256), 256, 0, c->stream>>>(e.snewkey, e.snewref, nnew, e.keys, e.rpos, E, e.keys2, e.refs2);
         LILI_TRY(launch_check(c, "k_inc_merge_new"));
     }
-    c->inc_cur = nxt;
-    c->inc_E = E2;
+    inc_merge_end(c, e);
     return inc_emit(c, m_out);
 }
 
@@ -523,24 +717,32 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
     return LILIOM_OK;
 }
 
+// Whether an update of n points takes the incremental path (otherwise: push + the sort chain)
+static bool map_incremental(const liliom_ctx* c, int n) { return c->nranks == 1 && c->prm.max_map_frames <= kIncSlots && n < (1 << 24); }
+
+// The incremental update behind its push (`popped` left the FIFO in it); falls back to the sort chain where the entry array cannot
+// describe the FIFO
+static int map_update_tail(liliom_ctx* c, const Popped& popped, int* n_map_out) {
+    map_reset(c);
+    int m = 0;
+    const int rc = map_inc_update(c, popped, &m);
+    if (rc == LILIOM_OK) {
+        LILI_TRY(map_finish_from_ds(c, m));
+        if (n_map_out) *n_map_out = m;
+        return LILIOM_OK;
+    }
+    c->inc_valid = false;
+    if (rc != LILIOM_E_GRID) return rc;       // E_GRID: keys not representable / PCL's overflow case -> the sort chain decides
+    return liliom_map_rebuild(c, n_map_out);
+}
+
 // SURVEY §8 (f2): push + incremental refresh; same result as liliom_map_push_frame + liliom_map_rebuild
 static int map_update_from_device(liliom_ctx* c, const void* d_src, int n, const double pose7[7], int* n_map_out) {
     if (n_map_out) *n_map_out = 0;
-    const bool incremental = c->nranks == 1 && c->prm.max_map_frames <= kIncSlots && n < (1 << 24);
+    const bool incremental = map_incremental(c, n);
     Popped popped;
     LILI_TRY(push_frame_from_device(c, d_src, n, pose7, incremental, &popped));
-    if (incremental) {
-        map_reset(c);
-        int m = 0;
-        const int rc = map_inc_update(c, popped, &m);
-        if (rc == LILIOM_OK) {
-            LILI_TRY(map_finish_from_ds(c, m));
-            if (n_map_out) *n_map_out = m;
-            return LILIOM_OK;
-        }
-        c->inc_valid = false;
-        if (rc != LILIOM_E_GRID) return rc;       // E_GRID: keys not representable / PCL's overflow case -> the sort chain decides
-    }
+    if (incremental) return map_update_tail(c, popped, n_map_out);
     return liliom_map_rebuild(c, n_map_out);
 }
 
@@ -559,6 +761,219 @@ extern "C" int liliom_map_update_device(liliom_ctx* c, const void* d_surf_ds_bod
     if (!c || n < 0 || (n > 0 && !d_surf_ds_body) || !pose7) return LILIOM_E_ARG;
     LILI_CUDA(c, cudaSetDevice(c->device));
     return map_update_from_device(c, d_surf_ds_body, n, pose7, n_map_out);
+}
+
+// The frame of liliom_map_update_resident: surf_last_ds of the context's last odometry call, still in vg_out
+static bool resident_frame_ok(liliom_ctx* c) {
+    if (c->n_ds_resident >= 0) return true;
+    c->last_error = "liliom_map_update_resident: no down-sampled scan is resident (an odometry call leaves one; liliom_voxelgrid, "
+                    "liliom_kf_add, liliom_kf_cloud, liliom_loop_align and liliom_global_map overwrite it)";
+    return false;
+}
+
+// The update reads vg_out and never writes it (its VoxelGrid output is map_ds), so the frame stays resident across the call.
+extern "C" int liliom_map_update_resident(liliom_ctx* c, const double pose7[7], int* n_map_out) {
+    if (!c || !pose7) return LILIOM_E_ARG;
+    if (!resident_frame_ok(c)) return LILIOM_E_ARG;
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    return map_update_from_device(c, c->vg_out.p, c->n_ds_resident, pose7, n_map_out);
+}
+
+namespace lili {
+namespace {
+
+// One stage for the sessions `which` (indices into J): launches of up to kBatchMax sessions on c0's stream, fill(entry, job) giving
+// each session's table entry; each session's launch count advances as its solo call's does.
+template <class St, class Fill>
+int map_stage(liliom_ctx* c0, std::vector<MapJob>& J, const std::vector<int>& which, Fill fill) {
+    for (size_t first = 0; first < which.size(); first += kBatchMax) {
+        typename St::Tab tab{};
+        tab.n = (int)std::min(which.size() - first, (size_t)kBatchMax);
+        int grid = 0;
+        for (int m = 0; m < tab.n; ++m) {
+            MapJob& j = J[which[first + m]];
+            fill(tab.s[m], j);
+            grid += St::blocks(tab.s[m]);
+            j.c->cnt.launches++;
+        }
+        k_map_stage_batch<St><<<grid, St::kThreads, 0, c0->stream>>>(tab);
+        LILI_CUDA(c0, cudaGetLastError());
+    }
+    return LILIOM_OK;
+}
+template <class St>
+int map_stage(liliom_ctx* c0, std::vector<MapJob>& J, const std::vector<int>& which) {
+    return map_stage<St>(c0, J, which, [](MapEntry& e, const MapJob& j) { e = j.e; });
+}
+template <int STRIDE>
+int map_centroid_stage(liliom_ctx* c0, std::vector<MapJob>& J, const std::vector<int>& which) {
+    return map_stage<MapStCentroid<STRIDE>>(c0, J, which, [](MapCentroidEntry& t, const MapJob& j) {
+        const MapEntry& e = j.e;
+        t = MapCentroidEntry{j.ft, e.ekeys, e.erefs, e.E2, e.stride, e.flags, e.rank, e.ds, e.count};
+    });
+}
+
+// Where a session of the batch stands: on the shared path, finished (its status set), or off the shared path, to be finished
+// by the solo code it would have run: the whole update, the update behind the push, or the sort chain.
+enum MapWhere { kMapLive, kMapDone, kMapSoloAll, kMapSoloTail, kMapSoloRebuild };
+
+// The shared phases of map_update_batch, every session's stream pointing at c0's.  Each phase: the solo call's host part per
+// session, the stage launches for all of them, every session's read-back words into its own pinned block, ONE synchronise.
+int map_batch_run(liliom_ctx* c0, std::vector<MapJob>& J, std::vector<MapWhere>& where, const double* poses7, int* nm, int* status) {
+    const int B = (int)J.size();
+    auto fail = [&](int i, int rc, bool inc) {
+        status[i] = rc; where[i] = kMapDone;
+        if (inc) J[i].c->inc_valid = false;
+    };
+    auto live = [&](auto pred) {
+        std::vector<int> v;
+        for (int i = 0; i < B; ++i) if (where[i] == kMapLive && pred(J[i])) v.push_back(i);
+        return v;
+    };
+    auto any = [](const MapJob&) { return true; };
+    // `bytes` at src(job) of every session in `which` into its pinned scratch, then the phase's one wait
+    auto wait_words = [&](const std::vector<int>& which, auto src, size_t bytes) -> int {
+        for (int i : which)
+            if (cudaError_t err = cudaMemcpyAsync(J[i].c->h_pin->scratch, src(J[i]), bytes, cudaMemcpyDeviceToHost, c0->stream); err != cudaSuccess)
+                fail(i, fail_cuda(J[i].c, err, "map update batch: read-back"), true);
+        LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+        return LILIOM_OK;
+    };
+    auto word = [&](int i) { int w; memcpy(&w, J[i].c->h_pin->scratch, sizeof(int)); return w; };
+
+    // 1. transform + box of the new frame -> every session's Frame::mm
+    for (int i : live(any)) {
+        liliom_ctx* c = J[i].c;
+        const int n = c->n_ds_resident;
+        if (!map_incremental(c, n)) { where[i] = kMapSoloAll; continue; }
+        if (const int rc = push_begin(c, c->vg_out.p, n, poses7 + 7 * i, true, J[i]); rc != LILIOM_OK) fail(i, rc, false);
+    }
+    {
+        const std::vector<int> w = live([](const MapJob& j) { return j.e.n > 0; });
+        LILI_TRY(map_stage<MapStTransform>(c0, J, w));
+        LILI_TRY(map_stage<MapStBoxInit>(c0, J, w));
+        LILI_TRY(map_stage<MapStBox>(c0, J, w));
+        LILI_TRY(wait_words(w, [](const MapJob& j) { return j.e.mm; }, kBoxInts * sizeof(int)));
+    }
+    for (int i : live(any)) {
+        push_end(J[i], J[i].e.n > 0 ? reinterpret_cast<const int*>(J[i].c->h_pin->scratch) : nullptr);
+        map_reset(J[i].c);
+    }
+    // 2. keys of the new frame + key flag -> inc_representable per session
+    for (int i : live(any)) {
+        liliom_ctx* c = J[i].c;
+        if (!c->inc_valid) { where[i] = kMapSoloTail; continue; }       // first update, or the FIFO was touched: inc_build_all
+        if (const int rc = inc_new_begin(c, J[i].e); rc != LILIOM_OK) fail(i, rc, true);
+    }
+    LILI_TRY(map_stage<MapStKeys>(c0, J, live([](const MapJob& j) { return j.e.n > 0; })));
+    LILI_TRY(wait_words(live(any), [](const MapJob& j) { return j.e.bad; }, sizeof(int)));
+    for (int i : live(any)) J[i].c->frames.back().bad = word(i) != 0;
+    // 3. merge into the entry array, heads, centroids -> every session's voxel count
+    for (int i : live(any)) {
+        liliom_ctx* c = J[i].c;
+        if (!inc_representable(c)) { c->inc_valid = false; where[i] = kMapSoloRebuild; continue; }
+        if (const int rc = inc_merge_begin(c, J[i].popped, J[i].e); rc != LILIOM_OK) fail(i, rc, true);
+    }
+    LILI_TRY(map_stage<MapStMark>(c0, J, live(any)));
+    for (int i : live(any))
+        if (const int rc = exclusive_scan_i32(J[i].c, J[i].e.removed, J[i].e.rpos, J[i].e.E); rc != LILIOM_OK) fail(i, rc, true);
+    LILI_TRY(map_stage<MapStMergeOld>(c0, J, live([](const MapJob& j) { return j.e.E > 0; })));
+    LILI_TRY(map_stage<MapStMergeNew>(c0, J, live([](const MapJob& j) { return j.e.nnew > 0; })));
+    for (int i : live(any)) {
+        inc_merge_end(J[i].c, J[i].e);
+        if (const int rc = inc_emit_begin(J[i].c, J[i].e, J[i].ft); rc != LILIOM_OK) fail(i, rc, true);
+    }
+    {
+        const std::vector<int> w = live([](const MapJob& j) { return j.e.E2 > 0; });
+        LILI_TRY(map_stage<MapStHeads>(c0, J, w));
+        for (int i : w)
+            if (const int rc = exclusive_scan_i32(J[i].c, J[i].e.flags, J[i].e.rank, J[i].e.E2); rc != LILIOM_OK) fail(i, rc, true);
+        LILI_TRY(map_centroid_stage<48>(c0, J, live([](const MapJob& j) { return j.e.E2 > 0 && j.e.stride == 48; })));
+        LILI_TRY(map_centroid_stage<32>(c0, J, live([](const MapJob& j) { return j.e.E2 > 0 && j.e.stride != 48; })));
+        const std::vector<int> counted = live([](const MapJob& j) { return j.e.E2 > 0; });
+        LILI_TRY(wait_words(counted, [](const MapJob& j) { return j.e.count; }, sizeof(int)));
+        for (int i : counted) if (where[i] == kMapLive) J[i].m = word(i);
+    }
+    // 4. repack, cell grid -> escape flags
+    for (int i : live(any))
+        if (const int rc = finish_begin(J[i].c, J[i].m, J[i].e); rc != LILIOM_OK) fail(i, rc, false);
+    LILI_TRY(map_stage<MapStRepack>(c0, J, live([](const MapJob& j) { return j.m > 0; })));
+    for (int i : live(any)) {
+        MapJob& j = J[i];
+        liliom_ctx* c = j.c;
+        int mm[kBoxInts];
+        frames_box(c, mm);
+        if (const int rc = grid_begin(c, c->map, gate_cell(c->prm.knn_max_sqdist), j.m, mm[6] > 0 ? mm : nullptr, j.g); rc != LILIOM_OK) {
+            fail(i, rc, false);
+            continue;
+        }
+        if (j.g.done) { nm[i] = j.m; where[i] = kMapDone; continue; }        // an empty map: nothing to index
+        MapEntry& e = j.e;
+        e.g = c->map.grid; e.gkeys = c->grid_keys.as<uint32_t>(); e.gvals = c->grid_vals.as<int>(); e.escaped = j.g.escaped;
+        e.gkeys2 = c->grid_keys2.as<uint32_t>(); e.gvals2 = c->grid_vals2.as<int>(); e.sorted = c->map.sorted.as<float4>();
+        e.cell_start = c->map.cell_start.as<int>();
+    }
+    LILI_TRY(map_stage<MapStCellKeys>(c0, J, live(any)));
+    for (int i : live(any)) if (const int rc = grid_sort(J[i].g); rc != LILIOM_OK) fail(i, rc, false);
+    LILI_TRY(map_stage<MapStGather>(c0, J, live(any)));
+    for (int i : live(any)) if (const int rc = grid_clear(J[i].g); rc != LILIOM_OK) fail(i, rc, false);
+    LILI_TRY(map_stage<MapStRunEnds>(c0, J, live(any)));
+    for (int i : live(any)) if (const int rc = grid_scan(J[i].g); rc != LILIOM_OK) fail(i, rc, false);
+    LILI_TRY(wait_words(live([](const MapJob& j) { return j.g.escaped != nullptr; }), [](const MapJob& j) { return j.g.escaped; }, sizeof(int)));
+    bool rebuilt = false;
+    for (int i : live(any)) {
+        const int esc = J[i].g.escaped ? word(i) : 0;
+        status[i] = grid_finish(J[i].g, esc);      // an escaped box: the exact re-build, as in the solo call
+        rebuilt = rebuilt || esc != 0;
+        if (status[i] == LILIOM_OK) nm[i] = J[i].m;
+        where[i] = kMapDone;
+    }
+    // the re-build's kernels are still queued: the call returns with every index complete, as the solo call does
+    if (rebuilt) LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+    // 5. sessions that left the shared path finish on their solo path
+    for (int i = 0; i < B; ++i) {
+        liliom_ctx* c = J[i].c;
+        if (where[i] == kMapSoloAll) status[i] = map_update_from_device(c, c->vg_out.p, c->n_ds_resident, poses7 + 7 * i, &nm[i]);
+        else if (where[i] == kMapSoloTail) status[i] = map_update_tail(c, J[i].popped, &nm[i]);
+        else if (where[i] == kMapSoloRebuild) status[i] = liliom_map_rebuild(c, &nm[i]);
+    }
+    return LILIOM_OK;
+}
+
+}  // namespace
+
+// liliom_map_update_resident of several sessions.  Shared launches and waits on cs[0]'s stream (the other sessions' streams
+// joined before and after with events); every buffer, library sort and scan, FIFO and host decision stays the session's own,
+// made by the solo call's code from the session's own read-back words.
+int map_update_batch(liliom_ctx* const* cs, int B, const double* poses7, int* n_map, int* status) {
+    liliom_ctx* c0 = cs[0];
+    std::vector<MapJob> J(B);
+    std::vector<MapWhere> where(B, kMapLive);
+    std::vector<int> nm(B, 0);
+    const std::vector<liliom_ctx*> all(cs, cs + B);
+    for (int i = 0; i < B; ++i) {
+        J[i].c = cs[i];
+        status[i] = LILIOM_OK;
+        if (!resident_frame_ok(cs[i])) { status[i] = LILIOM_E_ARG; where[i] = kMapDone; }
+    }
+    for (liliom_ctx* c : all) LILI_TRY(batch_join_in(c0, c));
+    int rc;
+    {
+        const BatchStreams on_c0(all, c0->stream);
+        rc = map_batch_run(c0, J, where, poses7, nm.data(), status);
+    }
+    LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, c0->stream));
+    for (liliom_ctx* c : all) LILI_TRY(batch_join_out(c0, c));
+    for (int i = 0; n_map && i < B; ++i) n_map[i] = nm[i];
+    return rc;
+}
+
+}  // namespace lili
+
+extern "C" int liliom_map_update_batch(liliom_ctx* const* ctxs, int B, const double* poses7, int* n_map, int* status) {
+    if (!batch_ctxs_ok(ctxs, B) || !poses7 || !status) return LILIOM_E_ARG;
+    LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
+    return map_update_batch(ctxs, B, poses7, n_map, status);
 }
 
 // surf_from_map_ds as a point cloud (all fields), in liliom_map_download order

@@ -6,6 +6,7 @@
 // reproducible and equal to the oracle's.  Compiled with --fmad=false.
 // The box / divisions are computed on the device (VgParams): no host round trip inside the call.
 #include "ctx.cuh"
+#include "map_stage.h"
 #include <climits>
 #include <cmath>
 #include <cstring>
@@ -13,22 +14,11 @@
 
 namespace lili {
 
-__global__ void k_vg_init(int* mm) {
-    if (threadIdx.x < kBoxInts) mm[threadIdx.x] = vg_box_empty(threadIdx.x);
-}
+__global__ void k_vg_init(int* mm) { vg_box_init(mm); }
 
-// box of the finite points (vg_box.h)
+// box of the finite points (vg_box.h; the body in ctx.cuh)
 __global__ void k_vg_minmax(const unsigned char* __restrict__ pts, int n_max, const int* __restrict__ d_n, int stride, int* __restrict__ mm) {
-    const int n = d_n ? min(*d_n, n_max) : n_max;
-    int box[kBoxInts];
-#pragma unroll
-    for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_empty(k);
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        float4 v = *reinterpret_cast<const float4*>(pts + (size_t)i * stride);
-        if (!(isfinite(v.x) && isfinite(v.y) && isfinite(v.z))) continue;
-        vg_box_add(box, v.x, v.y, v.z);
-    }
-    vg_box_commit(box, mm);
+    vg_minmax_body(pts, n_max, d_n, stride, mm, SoloBlock{});
 }
 
 struct VgBox { int mm[kBoxInts]; };      // a box (vg_box.h) by value
@@ -388,7 +378,7 @@ int vg_minmax_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, in
     k_vg_init<<<1, 32, 0, c->stream>>>(mm);
     LILI_TRY(launch_check(c, "k_vg_init"));
     if (n_max > 0) {
-        k_vg_minmax<<<min(cdiv(n_max, 256), c->sm_count * 8), 256, 0, c->stream>>>((const unsigned char*)d_in, n_max, d_n, stride, mm);
+        k_vg_minmax<<<box_blocks(n_max, c->sm_count), 256, 0, c->stream>>>((const unsigned char*)d_in, n_max, d_n, stride, mm);
         LILI_TRY(launch_check(c, "k_vg_minmax"));
     }
     return LILIOM_OK;
