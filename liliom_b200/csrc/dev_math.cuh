@@ -220,7 +220,12 @@ __device__ inline void eigen_sym3(double a00, double a10, double a20, double a11
 // from the origin with sub-metre spread, so normal equations (condition squared) would cost
 // ~1e-4 m in the plane offset — QR keeps it at ~1e-9 m.
 // Everything is register-resident (fully unrolled, column permutation via swaps).
+// kEigenOrder: apply each reflector to the trailing columns as Eigen's applyHouseholderOnTheLeft does (essential^T * bottom
+// first, then the head row), the order of the oracle's copy, so that without contraction the bits are the oracle's
+// (backend_corr.cu).  false keeps the head-row-first order the scan-to-map kernel (grid_knn.cu, compiled with contraction)
+// has always used; moving it is a change of that kernel's results and belongs with its own bit-stability work.
 // ---------------------------------------------------------------------------------------
+template <bool kEigenOrder = true>
 __device__ inline void colpiv_qr_solve_5x3(double A[5][3], double b[5], double x[3]) {
     double nu[3], ndir[3], tau[3];
     int perm[3] = {0, 1, 2};
@@ -277,9 +282,10 @@ __device__ inline void colpiv_qr_solve_5x3(double A[5][3], double b[5], double x
         if (tk != 0) {
 #pragma unroll
             for (int j = k + 1; j < 3; ++j) {
-                double tmp = A[k][j];
+                double tmp = kEigenOrder ? 0.0 : A[k][j];
 #pragma unroll
                 for (int i = k + 1; i < 5; ++i) tmp += A[i][k] * A[i][j];
+                if (kEigenOrder) tmp += A[k][j];
                 A[k][j] -= tk * tmp;
 #pragma unroll
                 for (int i = k + 1; i < 5; ++i) A[i][j] -= tk * A[i][k] * tmp;
@@ -390,7 +396,7 @@ static __device__ __noinline__ void plane_fit5_qr(const float4 m[5], double nv[3
     double A[5][3], B[5];
 #pragma unroll
     for (int j = 0; j < 5; ++j) { A[j][0] = m[j].x; A[j][1] = m[j].y; A[j][2] = m[j].z; B[j] = -1.0; }
-    colpiv_qr_solve_5x3(A, B, nv);
+    colpiv_qr_solve_5x3<false>(A, B, nv);
 }
 
 // 6x6 SPD solve (LDL^T), H given as the 21-scalar upper triangle (row-major), rhs b.

@@ -61,30 +61,82 @@ def test_plane_fit_fast_path_and_qr_fallback(dm, oracle):
     np.testing.assert_allclose(nv, oracle.colpiv_qr_solve(m[:, :3].astype(np.float64), -np.ones(5)), rtol=1e-9, atol=1e-12)
 
 
+def _adversarial_neighbour_sets(oracle):
+    """the 5-NN sets of every adversarial backend query (tests/bk_adversarial.py), as the backend kernels see them: the edge
+    sets' scatter matrices (k_backend_edge's operation order) and the surf sets' QR systems, plain and reflectivity-weighted"""
+    import bk_adversarial as BK
+    scat, qr = [], []
+    for world in BK.WORLDS:
+        W = BK.backend_world(world)
+        for m4, q, edge in ((W["edge_map"], W["edge_q"], True), (BK.f4(W["surf_map"]), W["surf_q"], False)):
+            w = oracle.transform_cloud(q, W["pose"])
+            sel = np.stack([w["x"], w["y"], w["z"], np.ones(len(w), np.float32)], 1)
+            idx, sqd = oracle.KdTree(m4).knn5(sel)
+            for i in range(len(q)):
+                if idx[i, 4] < 0:
+                    continue
+                P = m4[idx[i], :3].astype(np.float64)
+                if edge:
+                    c = [0.0, 0.0, 0.0]
+                    for j in range(5):
+                        c = [c[k] + P[j, k] for k in range(3)]
+                    c = [v / 5.0 for v in c]
+                    a = [0.0] * 6                     # a00 a10 a20 a11 a21 a22
+                    for j in range(5):
+                        z = [P[j, k] - c[k] for k in range(3)]
+                        for t, (r, s) in enumerate(((0, 0), (1, 0), (2, 0), (1, 1), (2, 1), (2, 2))):
+                            a[t] = a[t] + z[r] * z[s]
+                    scat.append(np.array(a))
+                else:
+                    qr.append((P, -np.ones(5)))
+                    fr = q["curvature"][i]
+                    tw = np.abs(fr - W["surf_map"]["curvature"][idx[i]]).astype(np.float64)
+                    sw = 0.0
+                    for v in tw:
+                        sw = sw + v
+                    with np.errstate(divide="ignore", invalid="ignore"):
+                        wv = (1.0 / tw) / sw
+                        if np.isfinite(wv).all():
+                            qr.append((wv[:, None] * P, -wv))
+    return scat, qr
+
+
+def _full3(a):
+    return np.array([[a[0], a[1], a[2]], [a[1], a[3], a[4]], [a[2], a[4], a[5]]])
+
+
 def test_colpiv_qr_device_copy_equals_oracle_copy(dm, oracle):
+    """the device's ColPivHouseholderQR (k_backend_surf's plane fit) and the oracle's copy: the same algorithm in the same order,
+    both without contraction, so the same bits, on random systems, far-from-origin ones and every adversarial neighbour set"""
     rng = np.random.default_rng(1)
-    for _ in range(200):
-        A = rng.uniform(-50, 50, (5, 3)); b = -np.ones(5)
+    cases = [(rng.uniform(-50, 50, (5, 3)), -np.ones(5)) for _ in range(200)]
+    cases += [(rng.uniform(-0.5, 0.5, (5, 3)) + rng.uniform(-700, 700, 3), -np.ones(5)) for _ in range(200)]
+    _, adv = _adversarial_neighbour_sets(oracle)
+    assert len(adv) > 100
+    for A, b in cases + adv:
         x = np.zeros(3)
-        dm.dm_colpiv_qr(_d(np.ascontiguousarray(A.reshape(-1))), _d(b), _d(x))
-        np.testing.assert_allclose(x, oracle.colpiv_qr_solve(A, b), rtol=1e-12, atol=1e-14)
+        dm.dm_colpiv_qr(_d(np.ascontiguousarray(A.reshape(-1))), _d(b.copy()), _d(x))
+        assert x.tobytes() == oracle.colpiv_qr_solve(A, b).tobytes(), (A, b)
 
 
 def test_eigen_sym3_device_copy_equals_oracle_copy(dm, oracle):
+    """the device's 3x3 symmetric eigensolver (k_backend_edge's line fit, the Horizon extractor's patches) and the oracle's copy:
+    the same bits, eigenvector signs included, on random matrices and on every adversarial edge scatter"""
     rng = np.random.default_rng(2)
+    mats = []
     for k in range(300):
         B = rng.normal(size=(3, 3)) * 10.0 ** rng.integers(-3, 3)
         A = B @ B.T
-        a = np.array([A[0, 0], A[1, 0], A[2, 0], A[1, 1], A[2, 1], A[2, 2]])
+        mats.append(np.array([A[0, 0], A[1, 0], A[2, 0], A[1, 1], A[2, 1], A[2, 2]]))
+    adv, _ = _adversarial_neighbour_sets(oracle)
+    assert len(adv) > 100
+    for k, a in enumerate(mats + adv):
         ev = np.zeros(3); vec = np.zeros(9)
         dm.dm_eigen_sym3(_d(a), _d(ev), _d(vec))
-        ev_o, vec_o = oracle.eigen_sym3(A)
-        # two copies of the same algorithm (Eigen's tridiagonal QL): identical eigenvalues, eigenvectors up to sign
-        np.testing.assert_allclose(ev, ev_o, rtol=1e-13, atol=1e-300)
-        V = vec.reshape(3, 3)
-        for c in range(3):
-            assert min(np.abs(V[:, c] - vec_o[:, c]).max(), np.abs(V[:, c] + vec_o[:, c]).max()) < 1e-9
-        np.testing.assert_allclose(ev, np.linalg.eigvalsh(A), rtol=1e-10, atol=1e-12 * np.abs(A).max())
+        ev_o, vec_o = oracle.eigen_sym3(_full3(a))
+        assert ev.tobytes() == ev_o.tobytes() and vec.tobytes() == np.ascontiguousarray(vec_o).reshape(-1).tobytes(), a
+        if k < len(mats):
+            np.testing.assert_allclose(ev, np.linalg.eigvalsh(_full3(a)), rtol=1e-10, atol=1e-12 * np.abs(a).max())
 
 
 def test_solve6_and_pose_plus(dm):

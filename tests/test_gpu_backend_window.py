@@ -91,21 +91,19 @@ def _check_window(c, O, bp, kfs, win_ids, poses_l, layers, bodies):
         v_o, pa_o, pb_o = O.correspond_edge(te, eds, pl, bp.variant)
         v, pa, pb = c.backend_window_corr(slot, 0)
         assert np.array_equal(v, v_o) and int(v.sum()) == ne[slot]
-        both = v == 1
-        # line ends as an unordered pair: a = c + 0.1 u, b = c - 0.1 u (:1579-1580) with u an eigenvector, whose sign is not fixed
-        # when the 5-NN set is nearly symmetric; LidarEdgeFactor is symmetric in a and b
-        swap = np.abs(pa - pa_o).max(1) > np.abs(pa - pb_o).max(1)
-        assert swap[both].sum() <= max(3, both.sum() // 50)
-        pa_m, pb_m = np.where(swap[:, None], pb_o, pa_o), np.where(swap[:, None], pa_o, pb_o)
-        np.testing.assert_allclose(pa[both], pa_m[both], rtol=5e-6, atol=1e-6)
-        np.testing.assert_allclose(pb[both], pb_m[both], rtol=5e-6, atol=1e-6)
+        # line ends a = c + 0.1 u, b = c - 0.1 u (:1579-1580): the same bits, so the same eigenvector sign
+        assert _bytes(pa) == _bytes(pa_o) and _bytes(pb) == _bytes(pb_o), slot
         refl = dict(map_refl=surf_map["curvature"], feat_refl=sds["curvature"], reflect_thres=bp.reflect_thres) if bp.variant == 0 else {}
         vs_o, pl_o, sc_o = O.correspond_surf_backend(ts, sds, pl, bp.kd_max_radius, bp.surf_dist_thres, bp.w_gate, bp.lidar_const, **refl)
         vs, pls, scs = c.backend_window_corr(slot, 1)
         assert np.array_equal(vs, vs_o) and int(vs.sum()) == ns[slot]
-        both = vs == 1
-        np.testing.assert_allclose(pls[both], pl_o[both], rtol=5e-6, atol=1e-6)
-        np.testing.assert_allclose(scs[both], sc_o[both], rtol=1e-6, atol=1e-9)
+        assert _bytes(pls) == _bytes(pl_o), slot
+        if bp.variant == 0:
+            # lidar_const * (weight + exp(-sum_w)): CUDA's exp is within 1 ulp and glibc may round the other way; times lidar_const
+            # that is at most two ulps of the score (tests/test_gpu_backend_adversarial.py)
+            assert np.all(np.abs(scs - sc_o) <= 2 * np.spacing(np.abs(sc_o))), slot
+        else:
+            assert _bytes(scs) == _bytes(sc_o), slot
     q_lb, t_lb = np.array(bp.q_lb[:]), np.array(bp.t_lb[:])
     for body in bodies:
         got = c.backend_window_blocks(body)
