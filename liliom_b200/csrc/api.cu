@@ -571,7 +571,7 @@ extern "C" int liliom_extract_resident_batch(liliom_ctx* const* ctxs, int B, con
     LILI_TRY(rc);
     for (size_t k = 0; k < hz.size(); ++k) status[hz_at[k]] = hz[k].status;
     // one synchronise for the whole call: every session's stream joins ctxs[0]'s
-    for (int i = 0; i < B; ++i) LILI_TRY(batch_join_in(c0, ctxs[i]));
+    LILI_TRY(batch_join_in(c0, std::vector<liliom_ctx*>(ctxs, ctxs + B)));
     LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
     for (size_t k = 0; k < rot.size(); ++k) status[rot_at[k]] = rot[k].pending ? rot_batch_finish(rot[k]) : rot[k].status;
     return LILIOM_OK;

@@ -10,6 +10,7 @@
 #include <utility>
 #include <vector>
 #include "../../include/liliom.h"
+#include "batch.h"
 #include "vg_box.h"
 
 namespace lili {
@@ -139,8 +140,41 @@ struct SessionBlock {
     __device__ __forceinline__ unsigned int G() const { return g; }
 };
 
+// The session of this block in a batched launch (batch.h) and the block's place in that session's range.
+struct BatchSlot {
+    int s;
+    SessionBlock blk;
+};
+template <class Entry>
+__device__ __forceinline__ BatchSlot batch_slot(const BatchTab<Entry>& tab) {
+    const int s = batch_session_of(tab.n, tab.off, (int)blockIdx.x);
+    return BatchSlot{s, SessionBlock{(int)blockIdx.x - tab.off[s], (unsigned int)(tab.off[s + 1] - tab.off[s])}};
+}
+
+// One stage of a batched chain (the ROT extraction in extract_rot.cu, the map update in map.cu): its Entry, its block size, its
+// blocks for a session (host side: the table's off[] carries them to the device) and its body run(entry, bx) for block bx of the
+// session, each as the solo launch has them.  The macro's run copies the entry by value, as the solo kernels' parameters are, and
+// gives CALL `e`, `bx` and the thread's place `i` in its session's launch.
+#define LILI_STAGE(NAME, ENTRY, THREADS, BLOCKS, CALL)                                                \
+    struct NAME {                                                                                     \
+        typedef ENTRY Entry;                                                                          \
+        static constexpr int kThreads = THREADS;                                                      \
+        static int blocks(const Entry& e) { return BLOCKS; }                                          \
+        __device__ static void run(const Entry& te, int bx) {                                         \
+            const Entry e = te;                                                                       \
+            const int i = bx * THREADS + (int)threadIdx.x;                                            \
+            (void)i;                                                                                  \
+            CALL;                                                                                     \
+        }                                                                                             \
+    };
+template <class St>
+__global__ void __launch_bounds__(St::kThreads) k_stage_batch(const __grid_constant__ BatchTab<typename St::Entry> tab) {
+    const BatchSlot at = batch_slot(tab);
+    St::run(tab.s[at.s], at.blk.bi());
+}
+
 // Bodies of the box and cell-grid kernels (voxelgrid.cu, grid_knn.cu), `i` = the thread's place in its session's launch: the solo
-// kernels pass blockIdx.x * blockDim.x + threadIdx.x, the batched map update (k_map_stage_batch, map.cu) the same place counted
+// kernels pass blockIdx.x * blockDim.x + threadIdx.x, the batched map update (k_stage_batch, map.cu) the same place counted
 // from its session's first block.
 __device__ __forceinline__ void vg_box_init(int* __restrict__ mm) {
     if (threadIdx.x < kBoxInts) mm[threadIdx.x] = vg_box_empty(threadIdx.x);
@@ -514,19 +548,61 @@ int s2m_run(liliom_ctx* c, double pose7[7], int match_cnt, int max_num_iter, int
 int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, const int* match_cnt, const int* max_num_iter, int mode,
               liliom_iter_stats* const* stats, int* status);
 
-// A batched call's shared launches run on ctxs[0]'s stream (c0): every other session's stream (its work so far) is ordered
-// before them ...
-inline int batch_join_in(liliom_ctx* c0, liliom_ctx* c) {
-    if (c->stream == c0->stream) return LILIOM_OK;
-    LILI_CUDA(c, cudaEventRecord(c->ev_batch, c->stream));
-    LILI_CUDA(c0, cudaStreamWaitEvent(c0->stream, c->ev_batch, 0));
+// A batched call's shared launches run on ctxs[0]'s stream (c0): the stream of every other session in cs (its work so far) is
+// ordered before them ...
+inline int batch_join_in(liliom_ctx* c0, const std::vector<liliom_ctx*>& cs) {
+    for (liliom_ctx* c : cs) {
+        if (c->stream == c0->stream) continue;
+        LILI_CUDA(c, cudaEventRecord(c->ev_batch, c->stream));
+        LILI_CUDA(c0, cudaStreamWaitEvent(c0->stream, c->ev_batch, 0));
+    }
     return LILIOM_OK;
 }
-// ... and after them (c0->ev_batch recorded behind the last shared launch)
-inline int batch_join_out(liliom_ctx* c0, liliom_ctx* c) {
-    if (c->stream != c0->stream) LILI_CUDA(c, cudaStreamWaitEvent(c->stream, c0->ev_batch, 0));
+// ... and after them: c0->ev_batch is recorded behind the last shared launch, and the others' streams wait for it
+inline int batch_join_out(liliom_ctx* c0, const std::vector<liliom_ctx*>& cs) {
+    LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, c0->stream));
+    for (liliom_ctx* c : cs)
+        if (c->stream != c0->stream) LILI_CUDA(c, cudaStreamWaitEvent(c->stream, c0->ev_batch, 0));
     return LILIOM_OK;
 }
+
+// One session's part of a batched launch: the context whose launch count the launch advances, and the session's blocks.
+struct BatchPart {
+    liliom_ctx* c;
+    int blocks;
+};
+// The launches of type Tab (a BatchTab, batch.h) over the sessions `ids`, in order, at most kBatchMax sessions each (one launch
+// for a packer's launch, which holds no more): part = fill(tab.s[m], ids[m]) writes session m's entry and gives its context and
+// blocks, off[] follows the blocks, every session's launch count advances by one, then launch(tab, grid) queues the launch.
+template <class Tab, class Fill, class Launch>
+int batch_tables(const std::vector<int>& ids, Fill fill, Launch launch) {
+    static_assert(sizeof(Tab) <= 32764, "a batched launch's session table must fit in the kernel parameter space");
+    for (size_t first = 0; first < ids.size(); first += kBatchMax) {
+        Tab tab{};
+        tab.n = (int)(ids.size() - first < (size_t)kBatchMax ? ids.size() - first : (size_t)kBatchMax);
+        for (int m = 0; m < tab.n; ++m) {
+            const BatchPart p = fill(tab.s[m], ids[first + m]);
+            tab.off[m + 1] = tab.off[m] + p.blocks;
+            p.c->cnt.launches++;
+        }
+        LILI_TRY(launch(tab, tab.off[tab.n]));
+    }
+    return LILIOM_OK;
+}
+
+#ifdef __CUDACC__
+// One stage (LILI_STAGE) for the sessions `which` on c0's stream: fill(entry, id) writes session id's entry and returns its context.
+template <class St, class Fill>
+int stage_batch(liliom_ctx* c0, const std::vector<int>& which, Fill fill) {
+    typedef BatchTab<typename St::Entry> Tab;
+    return batch_tables<Tab>(which, [&](typename St::Entry& e, int id) { liliom_ctx* c = fill(e, id); return BatchPart{c, St::blocks(e)}; },
+                             [&](const Tab& tab, int grid) -> int {
+                                 k_stage_batch<St><<<grid, St::kThreads, 0, c0->stream>>>(tab);
+                                 LILI_CUDA(c0, cudaGetLastError());
+                                 return LILIOM_OK;
+                             });
+}
+#endif
 
 // Points each session's work at one stream while a batch queues it (the library sorts and scans, the clears and the read-backs
 // take the context's stream), and gives every session its own stream back when it ends.

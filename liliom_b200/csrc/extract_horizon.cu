@@ -13,7 +13,6 @@
 // non-FMA x86-64 build, so labels and feature indices are bit-exact against the oracle.
 #include "ctx.cuh"
 #include "dev_math.cuh"
-#include "s2m_plan.h"
 #include <algorithm>
 #include <climits>
 
@@ -485,19 +484,13 @@ struct HzBatchEntry {
     Pt48* cut; int* mat; int* blockcnt; int* counts; int* totals; int* ncut_out; Pt48* surf; Pt48* edge; unsigned int* ctl;
     unsigned int call;
 };
-struct HzBatch {
-    int n;                              // sessions in this launch
-    int off[kBatchMax + 1];
-    HzBatchEntry s[kBatchMax];
-};
-static_assert(sizeof(HzBatch) <= 32764, "k_hz_batch's session table must fit in the kernel parameter space");
+typedef BatchTab<HzBatchEntry> HzBatch;
 
 __global__ void __launch_bounds__(HZC_THREADS, 3) k_hz_batch(const __grid_constant__ HzBatch tab) {
-    int s = 0;
-    while (s + 1 < tab.n && (int)blockIdx.x >= tab.off[s + 1]) ++s;
-    const HzBatchEntry e = tab.s[s];    // a by-value copy, as k_hz_coop's parameters
+    const BatchSlot at = batch_slot(tab);
+    const HzBatchEntry e = tab.s[at.s]; // a by-value copy, as k_hz_coop's parameters
     hz_coop_body(e.pts, e.n, e.q_imu, e.surf_thres, e.edge_thres, e.cut, e.mat, e.blockcnt, e.counts, e.totals, e.ncut_out, e.surf,
-                 e.edge, e.ctl, e.call, SessionBlock{(int)blockIdx.x - tab.off[s], (unsigned int)(tab.off[s + 1] - tab.off[s])});
+                 e.edge, e.ctl, e.call, at.blk);
 }
 
 // horizon_extract_dev in parts, shared with the batch (horizon_batch_queue): hz_begin sizes the buffers and decides whether the
@@ -632,24 +625,22 @@ int horizon_extract_dev(liliom_ctx* c, int n, const double q_imu[4], int* n_surf
 }
 
 // The Horizon sessions of liliom_extract_resident_batch.  Sessions whose solo call takes k_hz_coop share cooperative k_hz_batch
-// launches on c0's stream, kHzBatchGrid blocks each, packed by s2m_batch_pack (first-fit, in call order) into launches whose
-// summed grid is co-resident; each keeps its own barrier word and call sequence.  The others (LILIOM_HZ_CHAIN, empty sweeps),
-// and every session when no shared launch fits, take their solo path on their own stream.  The counts stay on the device, as in
-// the solo resident call.
+// launches on c0's stream, kHzBatchGrid blocks each, packed by batch_pack (first-fit, in call order) into launches whose summed
+// grid is co-resident; each keeps its own barrier word and call sequence.  The others (LILIOM_HZ_CHAIN, empty sweeps), and every
+// session when no shared launch fits, take their solo path on their own stream.  The counts stay on the device, as in the solo
+// resident call.
 constexpr int kHzBatchGrid = (HZ_PATCHES + HZC_WARPS - 1) / HZC_WARPS;     // stage C: one warp per patch
 
 int horizon_batch_queue(liliom_ctx* c0, std::vector<HzBatchSession>& ss) {
     std::vector<HzJob> jobs(ss.size());
     std::vector<int> coop;                  // sessions that take k_hz_coop alone
-    std::vector<S2mPlan> plans;
+    std::vector<BatchItem> items;
     for (size_t k = 0; k < ss.size(); ++k) {
         HzBatchSession& s = ss[k];
         s.status = hz_begin(s.c, s.n, s.q_imu, jobs[k]);
         if (s.status != LILIOM_OK) continue;
         if (jobs[k].coop) {
-            S2mPlan p{};
-            p.persistent = true; p.lanes = 1; p.grid = kHzBatchGrid;
-            plans.push_back(p);
+            items.push_back(BatchItem{kHzBatchGrid, 0, true});
             coop.push_back((int)k);
             continue;
         }
@@ -659,38 +650,33 @@ int horizon_batch_queue(liliom_ctx* c0, std::vector<HzBatchSession>& ss) {
     if (coop.empty()) return LILIOM_OK;
     int occ = 0;
     LILI_CUDA(c0, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_hz_batch, HZC_THREADS, 0));
-    int occs[kGnKinds];
-    std::fill(occs, occs + kGnKinds, occ);
-    const S2mPack pack = s2m_batch_pack(plans, occs, c0->sm_count);
+    const BatchPack pack = batch_pack(items, &occ, c0->sm_count);
     for (int j : pack.solo) {
         HzBatchSession& s = ss[coop[j]];
         s.status = hz_coop_solo(jobs[coop[j]]);
         if (s.status == LILIOM_OK) s.status = hz_end(jobs[coop[j]], false, s.n_surf, s.n_edge, s.n_cut);
     }
     if (pack.launches.empty()) return LILIOM_OK;
-    for (const S2mLaunch& l : pack.launches)
-        for (int j : l.sessions) LILI_TRY(batch_join_in(c0, ss[coop[j]].c));
-    for (const S2mLaunch& l : pack.launches) {
-        HzBatch tab{};
-        tab.n = (int)l.sessions.size();
-        for (int m = 0; m < tab.n; ++m) {
-            tab.off[m + 1] = tab.off[m] + kHzBatchGrid;
-            tab.s[m] = hz_coop_entry(jobs[coop[l.sessions[m]]], false);
-        }
-        void* kargs[] = {&tab};
-        LILI_CUDA(c0, cudaLaunchCooperativeKernel((const void*)k_hz_batch, dim3(l.grid), dim3(HZC_THREADS), kargs, 0, c0->stream));
-        LILI_CUDA(c0, cudaGetLastError());
-        for (int j : l.sessions) {
-            HzBatchSession& s = ss[coop[j]];
-            s.c->cnt.launches++;
-            s.c->hz_coop_calls++;
-            s.status = hz_end(jobs[coop[j]], false, s.n_surf, s.n_edge, s.n_cut);
-        }
-    }
-    LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, c0->stream));
-    for (const S2mLaunch& l : pack.launches)
-        for (int j : l.sessions) LILI_TRY(batch_join_out(c0, ss[coop[j]].c));
-    return LILIOM_OK;
+    std::vector<liliom_ctx*> joined;
+    for (const BatchLaunch& l : pack.launches)
+        for (int j : l.sessions) joined.push_back(ss[coop[j]].c);
+    LILI_TRY(batch_join_in(c0, joined));
+    for (const BatchLaunch& l : pack.launches)
+        LILI_TRY(batch_tables<HzBatch>(l.sessions, [&](HzBatchEntry& e, int j) {
+            e = hz_coop_entry(jobs[coop[j]], false);
+            return BatchPart{ss[coop[j]].c, kHzBatchGrid};
+        }, [&](HzBatch& tab, int grid) -> int {
+            void* kargs[] = {&tab};
+            LILI_CUDA(c0, cudaLaunchCooperativeKernel((const void*)k_hz_batch, dim3(grid), dim3(HZC_THREADS), kargs, 0, c0->stream));
+            LILI_CUDA(c0, cudaGetLastError());
+            for (int j : l.sessions) {
+                HzBatchSession& s = ss[coop[j]];
+                s.c->hz_coop_calls++;
+                s.status = hz_end(jobs[coop[j]], false, s.n_surf, s.n_edge, s.n_cut);
+            }
+            return LILIOM_OK;
+        }));
+    return batch_join_out(c0, joined);
 }
 
 }  // namespace lili

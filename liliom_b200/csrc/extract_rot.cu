@@ -25,7 +25,6 @@
 #include "dev_math.cuh"
 #include "detmath.h"
 #include "pc2_fields.h"
-#include "s2m_plan.h"
 #include <climits>
 #include <cstdlib>
 #include <cstdint>
@@ -546,18 +545,12 @@ struct RotRingEntry {
     const Pt32* cloud; const float* curv; int* meta; int* label; int* lessflat; int* seg_edge; int* seg_cnt;
     int ds_rate, fast_cap;
 };
-struct RotRingBatch {
-    int n;                              // sessions in this launch
-    int off[kBatchMax + 1];
-    RotRingEntry s[kBatchMax];
-};
-static_assert(sizeof(RotRingBatch) <= 32764, "k_rot_ring_batch's session table must fit in the kernel parameter space");
+typedef BatchTab<RotRingEntry> RotRingBatch;
 
 __global__ void __launch_bounds__(512) k_rot_ring_batch(const __grid_constant__ RotRingBatch tab) {
-    int s = 0;
-    while (s + 1 < tab.n && (int)blockIdx.x >= tab.off[s + 1]) ++s;
-    const RotRingEntry e = tab.s[s];    // a by-value copy, as k_rot_ring's parameters
-    rot_ring_body(e.cloud, e.curv, e.meta, e.ds_rate, e.label, e.lessflat, e.seg_edge, e.seg_cnt, nullptr, e.fast_cap, (int)blockIdx.x - tab.off[s]);
+    const BatchSlot at = batch_slot(tab);
+    const RotRingEntry e = tab.s[at.s]; // a by-value copy, as k_rot_ring's parameters
+    rot_ring_body(e.cloud, e.curv, e.meta, e.ds_rate, e.label, e.lessflat, e.seg_edge, e.seg_cnt, nullptr, e.fast_cap, at.blk.bi());
 }
 
 // ---- per-ring VoxelGrid(0.6) of the less-flat points, batched over rings
@@ -864,11 +857,6 @@ struct RotEntry {
     float* curv; int* label; int* lessflat; int* seg_edge; int* seg_cnt; Pt32* edge; int* lfpos; int* lf_src; const uint32_t* ring_of;
     unsigned long long* k64; unsigned long long* k64b; int* vg_flags; int* vg_rank; Pt32* surf; int* vg_count;
 };
-struct RotTab {
-    int n;                              // sessions in this launch
-    RotEntry s[kBatchMax];
-};
-static_assert(sizeof(RotTab) <= 32764, "k_rot_stage_batch's session table must fit in the kernel parameter space");
 
 static RotEntry rot_entry(const RotJob& j) {
     liliom_ctx* c = j.c;
@@ -881,87 +869,53 @@ static RotEntry rot_entry(const RotJob& j) {
                     c->surf.as<Pt32>(), c->vg_count.as<int>()};
 }
 
-// One stage of the chain: its block size, its blocks for a sweep of n points and its body, each as the solo launch has them
-// (rot_front / rot_back).  Session s owns the blocks after those of sessions 0 .. s-1.
-#define LILI_ROT_STAGE(NAME, THREADS, BLOCKS, CALL)                                                   \
-    struct NAME {                                                                                     \
-        static constexpr int kThreads = THREADS;                                                      \
-        __host__ __device__ static int blocks(int n) { return BLOCKS; }                               \
-        __device__ static void run(const RotEntry& e, int bx) { CALL; }                               \
-    };
-#define LILI_CDIV(a, b) (((a) + (b) - 1) / (b))
-LILI_ROT_STAGE(RotStMetaInit, 256, 1, rot_meta_init_body(e.meta, bx))
-LILI_ROT_STAGE(RotStPreT, ROT_PRE_THREADS, LILI_CDIV(n, ROT_PRE_THREADS),
-               rot_pre_body<true>(e.raw, e.rings, e.times, e.n, e.n_scans, e.keys, e.vals, e.ori, e.meta, bx))
-LILI_ROT_STAGE(RotStPreA, ROT_PRE_THREADS, LILI_CDIV(n, ROT_PRE_THREADS),
-               rot_pre_body<false>(e.raw, e.rings, nullptr, e.n, e.n_scans, e.keys, e.vals, e.ori, e.meta, bx))
-LILI_ROT_STAGE(RotStHp, 256, LILI_CDIV(n, 256), rot_hp_body(e.raw, e.n, e.keys, e.ori, e.meta, bx))
-LILI_ROT_STAGE(RotStBuildT, 128, LILI_CDIV(n, 128),
-               rot_build_body<true>(e.raw, e.n, e.keys2, e.vals2, e.ori, e.times, e.qI, e.qL, e.cloud, e.meta, bx))
-LILI_ROT_STAGE(RotStBuildA, 128, LILI_CDIV(n, 128),
-               rot_build_body<false>(e.raw, e.n, e.keys2, e.vals2, e.ori, nullptr, e.qI, e.qL, e.cloud, e.meta, bx))
-LILI_ROT_STAGE(RotStCurv, 256, LILI_CDIV(n + 1, 256), rot_curv_body(e.cloud, e.meta, e.curv, e.label, e.lessflat, e.n, bx))
-LILI_ROT_STAGE(RotStEdgeEmit, ROT_EMIT_THREADS, 1, rot_edge_emit_body(e.cloud, e.seg_edge, e.seg_cnt, e.n_scans * 6, e.edge, e.meta, bx))
-LILI_ROT_STAGE(RotStLfInit, 256, LILI_CDIV(ROT_MAX_RINGS * 8, 256), rot_lf_init_body(e.ringmm, bx))
-LILI_ROT_STAGE(RotStLfGather, 256, LILI_CDIV(n, 256),
-               rot_lf_gather_body(e.cloud, e.keys2, e.lessflat, e.lfpos, e.n, e.n_scans, e.lf_src, e.ringmm, e.meta, bx))
-LILI_ROT_STAGE(RotStLfParams, ROT_MAX_RINGS, 1, rot_lf_params_body(e.ringmm, e.leaf, e.rprm, bx))
-LILI_ROT_STAGE(RotStLfKeys, 256, LILI_CDIV(n, 256), rot_lf_keys_body(e.cloud, e.ring_of, e.lf_src, e.meta, e.rprm, e.k64, e.vals, e.n, bx))
-LILI_ROT_STAGE(RotStVgHeads, 256, LILI_CDIV(n + 1, 256), vg_heads_at(e.k64b, e.n, e.meta + M_NLF, e.vg_flags, bx * blockDim.x + threadIdx.x))
-LILI_ROT_STAGE(RotStLfCentroid, 128, LILI_CDIV(n, 128),
-               rot_lf_centroid_body(e.cloud, e.lf_src, e.k64b, e.vals2, e.vg_flags, e.vg_rank, e.meta, e.n, e.surf, e.vg_count, bx))
-#undef LILI_ROT_STAGE
-#undef LILI_CDIV
+// The stages of the chain (k_stage_batch, ctx.cuh), each with the block size, the blocks for a sweep of e.n points and the body
+// of its solo launch (rot_front / rot_back)
+LILI_STAGE(RotStMetaInit, RotEntry, 256, 1, rot_meta_init_body(e.meta, bx))
+LILI_STAGE(RotStPreT, RotEntry, ROT_PRE_THREADS, stage_blocks(e.n, ROT_PRE_THREADS),
+           rot_pre_body<true>(e.raw, e.rings, e.times, e.n, e.n_scans, e.keys, e.vals, e.ori, e.meta, bx))
+LILI_STAGE(RotStPreA, RotEntry, ROT_PRE_THREADS, stage_blocks(e.n, ROT_PRE_THREADS),
+           rot_pre_body<false>(e.raw, e.rings, nullptr, e.n, e.n_scans, e.keys, e.vals, e.ori, e.meta, bx))
+LILI_STAGE(RotStHp, RotEntry, 256, stage_blocks(e.n, 256), rot_hp_body(e.raw, e.n, e.keys, e.ori, e.meta, bx))
+LILI_STAGE(RotStBuildT, RotEntry, 128, stage_blocks(e.n, 128),
+           rot_build_body<true>(e.raw, e.n, e.keys2, e.vals2, e.ori, e.times, e.qI, e.qL, e.cloud, e.meta, bx))
+LILI_STAGE(RotStBuildA, RotEntry, 128, stage_blocks(e.n, 128),
+           rot_build_body<false>(e.raw, e.n, e.keys2, e.vals2, e.ori, nullptr, e.qI, e.qL, e.cloud, e.meta, bx))
+LILI_STAGE(RotStCurv, RotEntry, 256, stage_blocks(e.n + 1, 256), rot_curv_body(e.cloud, e.meta, e.curv, e.label, e.lessflat, e.n, bx))
+LILI_STAGE(RotStEdgeEmit, RotEntry, ROT_EMIT_THREADS, 1, rot_edge_emit_body(e.cloud, e.seg_edge, e.seg_cnt, e.n_scans * 6, e.edge, e.meta, bx))
+LILI_STAGE(RotStLfInit, RotEntry, 256, stage_blocks(ROT_MAX_RINGS * 8, 256), rot_lf_init_body(e.ringmm, bx))
+LILI_STAGE(RotStLfGather, RotEntry, 256, stage_blocks(e.n, 256),
+           rot_lf_gather_body(e.cloud, e.keys2, e.lessflat, e.lfpos, e.n, e.n_scans, e.lf_src, e.ringmm, e.meta, bx))
+LILI_STAGE(RotStLfParams, RotEntry, ROT_MAX_RINGS, 1, rot_lf_params_body(e.ringmm, e.leaf, e.rprm, bx))
+LILI_STAGE(RotStLfKeys, RotEntry, 256, stage_blocks(e.n, 256), rot_lf_keys_body(e.cloud, e.ring_of, e.lf_src, e.meta, e.rprm, e.k64, e.vals, e.n, bx))
+LILI_STAGE(RotStVgHeads, RotEntry, 256, stage_blocks(e.n + 1, 256), vg_heads_at(e.k64b, e.n, e.meta + M_NLF, e.vg_flags, bx * blockDim.x + threadIdx.x))
+LILI_STAGE(RotStLfCentroid, RotEntry, 128, stage_blocks(e.n, 128),
+           rot_lf_centroid_body(e.cloud, e.lf_src, e.k64b, e.vals2, e.vg_flags, e.vg_rank, e.meta, e.n, e.surf, e.vg_count, bx))
 
-template <class St>
-__global__ void __launch_bounds__(St::kThreads) k_rot_stage_batch(const __grid_constant__ RotTab tab) {
-    int s = 0, b = (int)blockIdx.x;
-    while (s + 1 < tab.n && b >= St::blocks(tab.s[s].n)) { b -= St::blocks(tab.s[s].n); ++s; }
-    const RotEntry e = tab.s[s];        // a by-value copy, as the solo kernels' parameters
-    St::run(e, b);
-}
-
-// One stage for the sessions `which` (indices into E / cs): launches of up to kBatchMax sessions on c0's stream; each session's
-// launch count advances as its solo call's does.
+// One stage for the sessions `which` (indices into E / cs); each session's launch count advances as its solo call's does.
 template <class St>
 static int rot_stage(liliom_ctx* c0, const std::vector<RotEntry>& E, const std::vector<liliom_ctx*>& cs, const std::vector<int>& which) {
-    for (size_t first = 0; first < which.size(); first += kBatchMax) {
-        RotTab tab{};
-        tab.n = (int)std::min(which.size() - first, (size_t)kBatchMax);
-        int grid = 0;
-        for (int m = 0; m < tab.n; ++m) {
-            tab.s[m] = E[which[first + m]];
-            grid += St::blocks(tab.s[m].n);
-            cs[which[first + m]]->cnt.launches++;
-        }
-        k_rot_stage_batch<St><<<grid, St::kThreads, 0, c0->stream>>>(tab);
-        LILI_CUDA(c0, cudaGetLastError());
-    }
-    return LILIOM_OK;
+    return stage_batch<St>(c0, which, [&](RotEntry& e, int i) { e = E[i]; return cs[i]; });
 }
 
-// The rings of the sessions `which`: k_rot_ring_batch launches of up to kBatchMax sessions, one block per ring.
+// The rings of the sessions `which`: k_rot_ring_batch launches, one block per ring.
 static int rot_ring_stage(liliom_ctx* c0, const std::vector<liliom_ctx*>& cs, const std::vector<int>& which) {
     LILI_CUDA(c0, cudaFuncSetAttribute(k_rot_ring_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RingSmem)));
-    for (size_t first = 0; first < which.size(); first += kBatchMax) {
-        RotRingBatch tab{};
-        tab.n = (int)std::min(which.size() - first, (size_t)kBatchMax);
-        for (int m = 0; m < tab.n; ++m) {
-            liliom_ctx* c = cs[which[first + m]];
-            const RotBufs b(c);
-            tab.off[m + 1] = tab.off[m] + c->prm.line_num;
-            tab.s[m] = RotRingEntry{b.cloud, c->rot_curv.as<float>(), b.meta, c->rot_label.as<int>(), c->rot_lessflat.as<int>(), b.seg_edge,
-                                    b.seg_cnt, c->prm.ds_rate, c->rot_slow_walk ? 0 : ROT_FAST_CAP};
-            c->cnt.launches++;
-        }
-        k_rot_ring_batch<<<tab.off[tab.n], 512, sizeof(RingSmem), c0->stream>>>(tab);
+    return batch_tables<RotRingBatch>(which, [&](RotRingEntry& e, int i) {
+        liliom_ctx* c = cs[i];
+        const RotBufs b(c);
+        e = RotRingEntry{b.cloud, c->rot_curv.as<float>(), b.meta, c->rot_label.as<int>(), c->rot_lessflat.as<int>(), b.seg_edge,
+                         b.seg_cnt, c->prm.ds_rate, c->rot_slow_walk ? 0 : ROT_FAST_CAP};
+        return BatchPart{c, c->prm.line_num};
+    }, [&](const RotRingBatch& tab, int grid) -> int {
+        k_rot_ring_batch<<<grid, 512, sizeof(RingSmem), c0->stream>>>(tab);
         LILI_CUDA(c0, cudaGetLastError());
-    }
-    return LILIOM_OK;
+        return LILIOM_OK;
+    });
 }
 
 // The ROT sessions of liliom_extract_resident_batch.  Every stage of the chain is one launch for all sessions with a sweep
-// (k_rot_stage_batch, k_rot_ring_batch), on c0's stream; the library sorts and scans and the copy of the sorted ring ids stay
+// (k_stage_batch, k_rot_ring_batch), on c0's stream; the library sorts and scans and the copy of the sorted ring ids stay
 // per session, in order on the same stream.  The stage list is the solo one (rot_front, k_rot_ring, rot_back), so every
 // session's counters advance as in its solo call.  Other sessions' streams are joined before and after with events.  Each
 // session's read-back words are copied into its pinned block at the end; the caller synchronises once for all of them before
@@ -985,7 +939,7 @@ int rot_batch_queue(liliom_ctx* c0, std::vector<RotBatchSession>& ss) {
         at.push_back((int)k);
     }
     if (cs.empty()) return LILIOM_OK;
-    for (liliom_ctx* c : cs) LILI_TRY(batch_join_in(c0, c));
+    LILI_TRY(batch_join_in(c0, cs));
     {
         const BatchStreams on_c0(cs, c0->stream);
         LILI_TRY(rot_stage<RotStMetaInit>(c0, E, cs, all));
@@ -1017,9 +971,7 @@ int rot_batch_queue(liliom_ctx* c0, std::vector<RotBatchSession>& ss) {
             ss[at[i]].pending = true;
         }
     }
-    LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, c0->stream));
-    for (liliom_ctx* c : cs) LILI_TRY(batch_join_out(c0, c));
-    return LILIOM_OK;
+    return batch_join_out(c0, cs);
 }
 
 int rot_batch_finish(RotBatchSession& s) {

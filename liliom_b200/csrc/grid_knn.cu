@@ -176,12 +176,9 @@ struct GnBatchEntry {
     unsigned int bar_base;              // arrivals of the session's earlier launches
     GnIo io;
 };
-struct GnBatch {
-    int n, iters, sync_mode;            // sessions in this launch; GN iterations and LILIOM_GN_SYNC shared by all of them
-    int off[kBatchMax + 1];             // session s owns blocks [off[s], off[s + 1])
-    GnBatchEntry s[kBatchMax];
+struct GnBatch : BatchTab<GnBatchEntry> {
+    int iters, sync_mode;               // GN iterations and LILIOM_GN_SYNC shared by all sessions of the launch
 };
-static_assert(sizeof(GnBatch) <= 32764, "k_gn_batch's session table must fit in the kernel parameter space");
 
 // What only the per-pass kernel (k_knn_plane) reads.
 struct PassArgs {
@@ -592,21 +589,15 @@ struct KnnBatchEntry {
     KnnArgs a;
     PassArgs p;
 };
-struct KnnBatch {
-    int n;                              // sessions in this launch
-    int off[kBatchMax + 1];             // session s owns blocks [off[s], off[s + 1])
-    KnnBatchEntry s[kBatchMax];
-};
-static_assert(sizeof(KnnBatch) <= 32764, "k_knn_plane_batch's session table must fit in the kernel parameter space");
+typedef BatchTab<KnnBatchEntry> KnnBatch;
 
 template <int LANES>
 __global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) k_knn_plane_batch(const __grid_constant__ KnnBatch tab) {
-    int s = 0;
-    while (s + 1 < tab.n && (int)blockIdx.x >= tab.off[s + 1]) ++s;
+    const BatchSlot at = batch_slot(tab);
     const PeerArgs pa{};
-    const KnnArgs a = tab.s[s].a;       // register copies, as k_knn_plane's by-value parameters: the body compiles to the same arithmetic
-    const PassArgs p = tab.s[s].p;
-    knn_plane_body<LANES>(a, p, pa, SessionBlock{(int)blockIdx.x - tab.off[s], (unsigned int)(tab.off[s + 1] - tab.off[s])});
+    const KnnArgs a = tab.s[at.s].a;    // register copies, as k_knn_plane's by-value parameters: the body compiles to the same arithmetic
+    const PassArgs p = tab.s[at.s].p;
+    knn_plane_body<LANES>(a, p, pa, at.blk);
 }
 
 // All GN iterations in ONE cooperative launch (single GPU, GN mode): per iteration the blocks meet at one
@@ -737,12 +728,10 @@ __global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned in
 // (lanes, staging) and the same iteration count; the fused exchange is never attached (communicator contexts are refused).
 template <int LANES, bool TMA = false>
 __global__ void LILI_GN_BOUNDS k_gn_batch(const __grid_constant__ GnBatch tab) {
-    int s = 0;
-    while (s + 1 < tab.n && (int)blockIdx.x >= tab.off[s + 1]) ++s;
-    const GnBatchEntry& e = tab.s[s];
+    const BatchSlot at = batch_slot(tab);
+    const GnBatchEntry& e = tab.s[at.s];
     const PeerArgs pa{};
-    gn_persistent_body<LANES, TMA>(e.a, tab.iters, e.bar, e.stats_base, e.bar_base, tab.sync_mode, pa, e.io,
-                                   SessionBlock{(int)blockIdx.x - tab.off[s], (unsigned int)(tab.off[s + 1] - tab.off[s])});
+    gn_persistent_body<LANES, TMA>(e.a, tab.iters, e.bar, e.stats_base, e.bar_base, tab.sync_mode, pa, e.io, at.blk);
 }
 
 // GN step for the multi-GPU path: runs after the all-reduce of neq[29], identically on every rank.
@@ -930,11 +919,7 @@ __global__ void __launch_bounds__(kLmBlock) k_lm_solve(LmArgs a) { lm_solve_body
 
 // Several sessions' LM solves of one pass, one block each (Ceres-mode liliom_scan_to_map_resident_batch_ex): block s runs
 // session s's solo k_lm_solve, with the same block size and so the same reduction order.
-struct LmBatch {
-    int n;
-    LmArgs s[kBatchMax];
-};
-static_assert(sizeof(LmBatch) <= 32764, "k_lm_solve_batch's session table must fit in the kernel parameter space");
+typedef BatchTab<LmArgs> LmBatch;
 __global__ void __launch_bounds__(kLmBlock) k_lm_solve_batch(const __grid_constant__ LmBatch tab) {
     const LmArgs a = tab.s[blockIdx.x];     // a register copy, as k_lm_solve's by-value parameter: the body compiles to the same arithmetic
     lm_solve_body(a);
@@ -1293,42 +1278,39 @@ static int s2m_batch_ceres(liliom_ctx* const* cs, std::vector<S2mCall>& k, const
     for (int j : live) { lp.push_back(plans[j]); li.push_back(iters[j]); }
     const std::vector<S2mPass> passes = s2m_pass_pack(lp, li);
     if (passes.empty()) return LILIOM_OK;
-    for (int j : live) LILI_TRY(batch_join_in(c0, cs[run[j]]));
+    std::vector<liliom_ctx*> joined;
+    for (int j : live) joined.push_back(cs[run[j]]);
+    LILI_TRY(batch_join_in(c0, joined));
     for (int it = 0; it < (int)passes.size(); ++it) {
         for (const S2mKnnLaunch& l : passes[it].knn) {
-            KnnBatch tab{};
-            tab.n = (int)l.sessions.size();
-            for (int m = 0; m < tab.n; ++m) {
-                const int j = live[l.sessions[m]];
-                liliom_ctx* c = cs[run[j]];
-                tab.off[m + 1] = tab.off[m] + plans[j].grid;
-                tab.s[m] = KnnBatchEntry{k[run[j]].a, pass_args(c, it, 0)};
-                c->cnt.launches++;
-            }
             const size_t dyn = plans[live[l.sessions[0]]].dyn_smem;
-            if (l.lanes == 1) LILI_CUDA(c0, cudaFuncSetAttribute(knn_batch_kernel(1), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
-            void* kargs[] = {&tab};
-            LILI_TRY(timed_launch(c0, timed0, 1, [&]() -> int {
-                LILI_CUDA(c0, cudaLaunchKernel(knn_batch_kernel(l.lanes), dim3(tab.off[tab.n]), dim3(kBlock), kargs, dyn, s0));
+            LILI_TRY(batch_tables<KnnBatch>(l.sessions, [&](KnnBatchEntry& e, int m) {
+                const int j = live[m];
+                liliom_ctx* c = cs[run[j]];
+                e = KnnBatchEntry{k[run[j]].a, pass_args(c, it, 0)};
+                return BatchPart{c, plans[j].grid};
+            }, [&](KnnBatch& tab, int grid) -> int {
+                if (l.lanes == 1) LILI_CUDA(c0, cudaFuncSetAttribute(knn_batch_kernel(1), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn));
+                void* kargs[] = {&tab};
+                return timed_launch(c0, timed0, 1, [&]() -> int {
+                    LILI_CUDA(c0, cudaLaunchKernel(knn_batch_kernel(l.lanes), dim3(grid), dim3(kBlock), kargs, dyn, s0));
+                    LILI_CUDA(c0, cudaGetLastError());
+                    return LILIOM_OK;
+                });
+            }));
+        }
+        for (const std::vector<int>& l : passes[it].lm)
+            LILI_TRY(batch_tables<LmBatch>(l, [&](LmArgs& e, int m) {
+                const int i = run[live[m]];
+                e = lm_args(cs[i], k[i].a, it, max_num_iter[i]);
+                return BatchPart{cs[i], 1};
+            }, [&](const LmBatch& tab, int grid) -> int {
+                k_lm_solve_batch<<<grid, kLmBlock, 0, s0>>>(tab);
                 LILI_CUDA(c0, cudaGetLastError());
                 return LILIOM_OK;
             }));
-        }
-        for (const std::vector<int>& l : passes[it].lm) {
-            LmBatch tab{};
-            tab.n = (int)l.size();
-            for (int m = 0; m < tab.n; ++m) {
-                const int i = run[live[l[m]]];
-                tab.s[m] = lm_args(cs[i], k[i].a, it, max_num_iter[i]);
-                cs[i]->cnt.launches++;
-            }
-            k_lm_solve_batch<<<tab.n, kLmBlock, 0, s0>>>(tab);
-            LILI_CUDA(c0, cudaGetLastError());
-        }
     }
-    LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, s0));
-    for (int j : live) LILI_TRY(batch_join_out(c0, cs[run[j]]));
-    return LILIOM_OK;
+    return batch_join_out(c0, joined);
 }
 
 int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, const int* match_cnt, const int* max_num_iter, int mode,
@@ -1365,37 +1347,31 @@ int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, const int* match_cnt
         LILI_CUDA(c0, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ[kind], gn_batch_kernel(kind), kBlock, dyn));
     }
     const std::vector<S2mGnGroup> groups = s2m_gn_groups(plans, iters, occ, c0->sm_count);
-    bool any = false;
+    std::vector<liliom_ctx*> joined;
     for (const S2mGnGroup& g : groups)
-        for (const S2mLaunch& l : g.pack.launches)
-            for (int j : l.sessions) { LILI_TRY(batch_join_in(c0, cs[run[j]])); any = true; }
+        for (const BatchLaunch& l : g.pack.launches)
+            for (int j : l.sessions) joined.push_back(cs[run[j]]);
+    LILI_TRY(batch_join_in(c0, joined));
     const bool timed0 = !run.empty() && run[0] == 0 && k[0].timed && k[0].p.persistent;     // knn_ms / knn_launches: ctxs[0] only
     for (const S2mGnGroup& g : groups)
-        for (const S2mLaunch& l : g.pack.launches) {
-            GnBatch tab{};
-            tab.n = (int)l.sessions.size(); tab.iters = g.iters; tab.sync_mode = c0->gn_sync;
-            for (int m = 0; m < tab.n; ++m) {
-                const S2mCall& ki = k[run[l.sessions[m]]];
-                tab.off[m + 1] = tab.off[m] + ki.p.grid;
-                tab.s[m] = GnBatchEntry{ki.a, ki.bar, ki.stats_base, ki.bar_base, ki.io};
-            }
-            const S2mPlan& p = plans[l.sessions[0]];
-            void* kargs[] = {&tab};
-            LILI_TRY(timed_launch(c0, timed0, g.iters, [&]() -> int {
-                LILI_CUDA(c0, cudaLaunchCooperativeKernel(gn_batch_kernel(l.kind), dim3(l.grid), dim3(kBlock), kargs, p.dyn_smem, s0));
-                LILI_CUDA(c0, cudaGetLastError());
+        for (const BatchLaunch& l : g.pack.launches)
+            LILI_TRY(batch_tables<GnBatch>(l.sessions, [&](GnBatchEntry& e, int j) {
+                const S2mCall& ki = k[run[j]];
+                e = GnBatchEntry{ki.a, ki.bar, ki.stats_base, ki.bar_base, ki.io};
+                return BatchPart{cs[run[j]], ki.p.grid};
+            }, [&](GnBatch& tab, int grid) -> int {
+                tab.iters = g.iters; tab.sync_mode = c0->gn_sync;
+                const S2mPlan& p = plans[l.sessions[0]];
+                void* kargs[] = {&tab};
+                LILI_TRY(timed_launch(c0, timed0, g.iters, [&]() -> int {
+                    LILI_CUDA(c0, cudaLaunchCooperativeKernel(gn_batch_kernel(l.kind), dim3(grid), dim3(kBlock), kargs, p.dyn_smem, s0));
+                    LILI_CUDA(c0, cudaGetLastError());
+                    return LILIOM_OK;
+                }));
+                for (int j : l.sessions) cs[run[j]]->bar_arrivals += (unsigned int)g.iters * (unsigned int)plans[j].grid;
                 return LILIOM_OK;
             }));
-            for (int j : l.sessions) {
-                liliom_ctx* c = cs[run[j]];
-                c->cnt.launches++;
-                c->bar_arrivals += (unsigned int)g.iters * (unsigned int)plans[j].grid;
-            }
-        }
-    if (any) LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, s0));
-    for (const S2mGnGroup& g : groups)
-        for (const S2mLaunch& l : g.pack.launches)
-            for (int j : l.sessions) LILI_TRY(batch_join_out(c0, cs[run[j]]));
+    if (!joined.empty()) LILI_TRY(batch_join_out(c0, joined));
     // sessions whose plan is not persistent: their solo launches, on their own streams, while the batch runs
     for (const S2mGnGroup& g : groups)
         for (int j : g.pack.solo) {
@@ -1404,7 +1380,7 @@ int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, const int* match_cnt
             if (status[i] == LILIOM_OK) status[i] = s2m_finish(cs[i], k[i], poses7 + 7 * i, stats ? stats[i] : nullptr, nullptr);
         }
     for (const S2mGnGroup& g : groups)
-        for (const S2mLaunch& l : g.pack.launches)
+        for (const BatchLaunch& l : g.pack.launches)
             for (int j : l.sessions) {
                 const int i = run[j];
                 status[i] = s2m_finish(cs[i], k[i], poses7 + 7 * i, stats ? stats[i] : nullptr, nullptr);

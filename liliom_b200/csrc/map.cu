@@ -25,7 +25,6 @@
 #include "ctx.cuh"
 #include "dev_math.cuh"
 #include "knn_core.cuh"
-#include "map_stage.h"
 #include <algorithm>
 #include <climits>
 #include <vector>
@@ -67,7 +66,7 @@ __global__ void k_compact_repack(const unsigned char* __restrict__ in, const int
 
 // transformCloud (L/src/LidarOdometry.cpp:246-278; R/src/LidarOdometry.cpp:239-264).  Every kernel of the map update has its body in
 // a function of `i`, the thread's place in its session's launch: the solo kernel passes blockIdx.x * blockDim.x + threadIdx.x,
-// the batched update (k_map_stage_batch below) the same place counted from its session's first block.
+// the batched update (k_stage_batch, ctx.cuh) the same place counted from its session's first block.
 __device__ __forceinline__ void transform_cloud_at(const unsigned char* __restrict__ in, int n, int stride, const Q4& q, const D3& t,
                                                    unsigned char* __restrict__ out, const int i) {
     if (i >= n) return;
@@ -202,69 +201,38 @@ struct MapEntry {
     int m; float4* xyzw; GridDesc g; uint32_t* gkeys; int* gvals; int* escaped; const uint32_t* gkeys2; const int* gvals2; float4* sorted;
     int* cell_start;
 };
-struct MapTab {
-    int n;                              // sessions in this launch
-    MapEntry s[kBatchMax];
-};
-static_assert(sizeof(MapTab) <= 32764, "k_map_stage_batch's session table must fit in the kernel parameter space");
 // The centroid stage also needs each session's frame pointers
 struct MapCentroidEntry {
     FrameTab tab;
     const u64* ekeys; const unsigned* erefs; int E2, stride; const int* flags; const int* rank; unsigned char* ds; int* count;
 };
-struct MapCentroidTab {
-    int n;
-    MapCentroidEntry s[kBatchMax];
-};
-static_assert(sizeof(MapCentroidTab) <= 32764, "the centroid stage's session table must fit in the kernel parameter space");
 
-// One stage of the update: its block size, its blocks for a session and its body, each as the solo launch has them.  Session s
-// owns the blocks after those of sessions 0 .. s-1.  The entry is copied by value, as the solo kernels' parameters are.
-#define LILI_MAP_STAGE(NAME, THREADS, BLOCKS, CALL)                                                   \
-    struct NAME {                                                                                     \
-        typedef MapTab Tab;                                                                           \
-        static constexpr int kThreads = THREADS;                                                      \
-        __host__ __device__ static int blocks(const MapEntry& e) { return BLOCKS; }                   \
-        __device__ static void run(const MapEntry& te, int bx) {                                      \
-            const MapEntry e = te;                                                                    \
-            const int i = bx * THREADS + (int)threadIdx.x;                                            \
-            (void)i;                                                                                  \
-            CALL;                                                                                     \
-        }                                                                                             \
-    };
-LILI_MAP_STAGE(MapStTransform, 256, stage_blocks(e.n, 256), transform_cloud_at(e.src, e.n, e.stride, e.q, e.t, e.fbuf, i))
-LILI_MAP_STAGE(MapStBoxInit, 32, 1, vg_box_init(e.mm))
-LILI_MAP_STAGE(MapStBox, 256, e.mm_blocks, vg_minmax_body(e.fbuf, e.n, nullptr, e.stride, e.mm, SessionBlock{bx, (unsigned)e.mm_blocks}))
-LILI_MAP_STAGE(MapStKeys, 256, stage_blocks(e.n, 256), inc_keys_at(e.fbuf, e.n, e.stride, e.inv_leaf, e.slot, e.newkey, e.newref, e.bad, i))
-LILI_MAP_STAGE(MapStMark, 256, stage_blocks(e.E + 1, 256), inc_mark_at(e.refs, e.E, e.popped, e.removed, i))
-LILI_MAP_STAGE(MapStMergeOld, 256, stage_blocks(e.E, 256),
-               inc_merge_old_at(e.keys, e.refs, e.removed, e.rpos, e.E, e.snewkey, e.nnew, e.keys2, e.refs2, i))
-LILI_MAP_STAGE(MapStMergeNew, 256, stage_blocks(e.nnew, 256),
-               inc_merge_new_at(e.snewkey, e.snewref, e.nnew, e.keys, e.rpos, e.E, e.keys2, e.refs2, i))
-LILI_MAP_STAGE(MapStHeads, 256, stage_blocks(e.E2 + 1, 256), vg_heads_at(e.ekeys, e.E2, (const int*)nullptr, e.flags, i))
-LILI_MAP_STAGE(MapStRepack, 256, stage_blocks(e.m, 256), repack_f4_at(e.ds, e.m, nullptr, e.stride, e.xyzw, i))
-LILI_MAP_STAGE(MapStCellKeys, 256, stage_blocks(e.m, 256), cell_keys_at(e.xyzw, e.m, e.g, e.gkeys, e.gvals, e.escaped, i))
-LILI_MAP_STAGE(MapStGather, 256, stage_blocks(e.m, 256), gather_sorted_at(e.xyzw, e.gvals2, e.m, e.sorted, i))
-LILI_MAP_STAGE(MapStRunEnds, 256, stage_blocks(e.m, 256), cell_run_ends_at(e.gkeys2, e.m, e.cell_start, i))
-#undef LILI_MAP_STAGE
+// The stages of the update (k_stage_batch, ctx.cuh), each with the block size, the blocks and the body of its solo launch
+LILI_STAGE(MapStTransform, MapEntry, 256, stage_blocks(e.n, 256), transform_cloud_at(e.src, e.n, e.stride, e.q, e.t, e.fbuf, i))
+LILI_STAGE(MapStBoxInit, MapEntry, 32, 1, vg_box_init(e.mm))
+LILI_STAGE(MapStBox, MapEntry, 256, e.mm_blocks, vg_minmax_body(e.fbuf, e.n, nullptr, e.stride, e.mm, SessionBlock{bx, (unsigned)e.mm_blocks}))
+LILI_STAGE(MapStKeys, MapEntry, 256, stage_blocks(e.n, 256), inc_keys_at(e.fbuf, e.n, e.stride, e.inv_leaf, e.slot, e.newkey, e.newref, e.bad, i))
+LILI_STAGE(MapStMark, MapEntry, 256, stage_blocks(e.E + 1, 256), inc_mark_at(e.refs, e.E, e.popped, e.removed, i))
+LILI_STAGE(MapStMergeOld, MapEntry, 256, stage_blocks(e.E, 256),
+           inc_merge_old_at(e.keys, e.refs, e.removed, e.rpos, e.E, e.snewkey, e.nnew, e.keys2, e.refs2, i))
+LILI_STAGE(MapStMergeNew, MapEntry, 256, stage_blocks(e.nnew, 256),
+           inc_merge_new_at(e.snewkey, e.snewref, e.nnew, e.keys, e.rpos, e.E, e.keys2, e.refs2, i))
+LILI_STAGE(MapStHeads, MapEntry, 256, stage_blocks(e.E2 + 1, 256), vg_heads_at(e.ekeys, e.E2, (const int*)nullptr, e.flags, i))
+LILI_STAGE(MapStRepack, MapEntry, 256, stage_blocks(e.m, 256), repack_f4_at(e.ds, e.m, nullptr, e.stride, e.xyzw, i))
+LILI_STAGE(MapStCellKeys, MapEntry, 256, stage_blocks(e.m, 256), cell_keys_at(e.xyzw, e.m, e.g, e.gkeys, e.gvals, e.escaped, i))
+LILI_STAGE(MapStGather, MapEntry, 256, stage_blocks(e.m, 256), gather_sorted_at(e.xyzw, e.gvals2, e.m, e.sorted, i))
+LILI_STAGE(MapStRunEnds, MapEntry, 256, stage_blocks(e.m, 256), cell_run_ends_at(e.gkeys2, e.m, e.cell_start, i))
 // The centroids: the scalars by value, the 512-byte frame table read in place from the parameter space (as k_inc_centroid reads its own)
 template <int STRIDE>
 struct MapStCentroid {
-    typedef MapCentroidTab Tab;
+    typedef MapCentroidEntry Entry;
     static constexpr int kThreads = 128;
-    __host__ __device__ static int blocks(const MapCentroidEntry& e) { return stage_blocks(e.E2, 128); }
+    static int blocks(const MapCentroidEntry& e) { return stage_blocks(e.E2, 128); }
     __device__ static void run(const MapCentroidEntry& te, int bx) {
         const u64* ekeys = te.ekeys; const unsigned* erefs = te.erefs; const int* flags = te.flags; const int* rank = te.rank;
         inc_centroid_at<STRIDE>(te.tab, ekeys, erefs, flags, rank, te.E2, te.ds, te.count, bx * 128 + (int)threadIdx.x);
     }
 };
-
-template <class St>
-__global__ void __launch_bounds__(St::kThreads) k_map_stage_batch(const __grid_constant__ typename St::Tab tab) {
-    int b = (int)blockIdx.x;
-    const int s = batch_session_of(tab.n, b, [&](int k) { return St::blocks(tab.s[k]); });
-    St::run(tab.s[s], b);
-}
 
 // ---- host side
 
@@ -782,34 +750,18 @@ extern "C" int liliom_map_update_resident(liliom_ctx* c, const double pose7[7], 
 namespace lili {
 namespace {
 
-// One stage for the sessions `which` (indices into J): launches of up to kBatchMax sessions on c0's stream, fill(entry, job) giving
-// each session's table entry; each session's launch count advances as its solo call's does.
-template <class St, class Fill>
-int map_stage(liliom_ctx* c0, std::vector<MapJob>& J, const std::vector<int>& which, Fill fill) {
-    for (size_t first = 0; first < which.size(); first += kBatchMax) {
-        typename St::Tab tab{};
-        tab.n = (int)std::min(which.size() - first, (size_t)kBatchMax);
-        int grid = 0;
-        for (int m = 0; m < tab.n; ++m) {
-            MapJob& j = J[which[first + m]];
-            fill(tab.s[m], j);
-            grid += St::blocks(tab.s[m]);
-            j.c->cnt.launches++;
-        }
-        k_map_stage_batch<St><<<grid, St::kThreads, 0, c0->stream>>>(tab);
-        LILI_CUDA(c0, cudaGetLastError());
-    }
-    return LILIOM_OK;
-}
+// One stage for the sessions `which` (indices into J); each session's launch count advances as its solo call's does.
 template <class St>
 int map_stage(liliom_ctx* c0, std::vector<MapJob>& J, const std::vector<int>& which) {
-    return map_stage<St>(c0, J, which, [](MapEntry& e, const MapJob& j) { e = j.e; });
+    return stage_batch<St>(c0, which, [&](MapEntry& e, int i) { e = J[i].e; return J[i].c; });
 }
 template <int STRIDE>
 int map_centroid_stage(liliom_ctx* c0, std::vector<MapJob>& J, const std::vector<int>& which) {
-    return map_stage<MapStCentroid<STRIDE>>(c0, J, which, [](MapCentroidEntry& t, const MapJob& j) {
+    return stage_batch<MapStCentroid<STRIDE>>(c0, which, [&](MapCentroidEntry& t, int i) {
+        const MapJob& j = J[i];
         const MapEntry& e = j.e;
         t = MapCentroidEntry{j.ft, e.ekeys, e.erefs, e.E2, e.stride, e.flags, e.rank, e.ds, e.count};
+        return j.c;
     });
 }
 
@@ -956,14 +908,13 @@ int map_update_batch(liliom_ctx* const* cs, int B, const double* poses7, int* n_
         status[i] = LILIOM_OK;
         if (!resident_frame_ok(cs[i])) { status[i] = LILIOM_E_ARG; where[i] = kMapDone; }
     }
-    for (liliom_ctx* c : all) LILI_TRY(batch_join_in(c0, c));
+    LILI_TRY(batch_join_in(c0, all));
     int rc;
     {
         const BatchStreams on_c0(all, c0->stream);
         rc = map_batch_run(c0, J, where, poses7, nm.data(), status);
     }
-    LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, c0->stream));
-    for (liliom_ctx* c : all) LILI_TRY(batch_join_out(c0, c));
+    LILI_TRY(batch_join_out(c0, all));
     for (int i = 0; n_map && i < B; ++i) n_map[i] = nm[i];
     return rc;
 }

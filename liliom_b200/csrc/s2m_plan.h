@@ -5,6 +5,7 @@
 #include <cstddef>
 #include <vector>
 #include "../../include/liliom.h"
+#include "batch.h"
 
 namespace lili {
 
@@ -12,7 +13,6 @@ constexpr int kBlock = 256;
 constexpr int kWarps = kBlock / 32;
 constexpr int kRunCap = 8;                    // runs per thread of the one-thread-per-query search (thread_knn5, knn_core.cuh)
 constexpr size_t kStageTileBytes = 3616;      // sizeof(StageTile), knn_core.cuh (checked there)
-constexpr int kBatchMax = 32;                 // sessions per batched launch (the tables of k_gn_batch, k_knn_plane_batch, k_lm_solve_batch)
 
 struct S2mPlanIn {
     int n, n_last;                  // query upper bound (the exact count unless dev_count); count of the previous scan (0: none)
@@ -70,33 +70,13 @@ inline int s2m_kind(const S2mPlan& p) {
     return p.tma ? 5 : p.lanes == 1 ? 0 : p.lanes == 2 ? 1 : p.lanes == 4 ? 2 : p.lanes == 8 ? 3 : 4;
 }
 
-// The launches of a batched scan-to-map step (s2m_batch, grid_knn.cu).  Each session keeps the plan its solo call would make.
-// Persistent sessions are grouped by instantiation and packed first-fit, in call order, into cooperative launches whose summed
-// grid is co-resident (occ[kind] blocks per SM of k_gn_batch<kind> times sm_count) and that hold at most max_per_launch
-// sessions; a session whose plan is not persistent (or whose kernel cannot be resident at all) goes to `solo`.
-struct S2mLaunch {
-    int kind, grid;                 // instantiation (s2m_kind), summed grid
-    std::vector<int> sessions;      // indices into the plans, in call order; blocks follow in this order
-};
-struct S2mPack {
-    std::vector<S2mLaunch> launches;
-    std::vector<int> solo;          // sessions that take s2m_run's own path
-};
-inline S2mPack s2m_batch_pack(const std::vector<S2mPlan>& plans, const int occ[kGnKinds], int sm_count, int max_per_launch = kBatchMax) {
-    S2mPack out;
-    for (int i = 0; i < (int)plans.size(); ++i) {
-        const S2mPlan& p = plans[i];
-        const int kind = s2m_kind(p);
-        const long long cap = (long long)occ[kind] * sm_count;
-        if (!p.persistent || p.grid > cap) { out.solo.push_back(i); continue; }
-        S2mLaunch* fit = nullptr;
-        for (S2mLaunch& l : out.launches)
-            if (l.kind == kind && (int)l.sessions.size() < max_per_launch && l.grid + p.grid <= cap) { fit = &l; break; }
-        if (!fit) { out.launches.push_back(S2mLaunch{kind, 0, {}}); fit = &out.launches.back(); }
-        fit->grid += p.grid;
-        fit->sessions.push_back(i);
-    }
-    return out;
+// The launches of a batched scan-to-map step (s2m_batch, grid_knn.cu).  Each session keeps the plan its solo call would make:
+// its grid and instantiation are packed by batch_pack against the occupancy occ[kind] of k_gn_batch<kind>; a session whose plan
+// is not persistent (or whose kernel cannot be resident at all) takes s2m_run's own path.
+inline BatchPack s2m_batch_pack(const std::vector<S2mPlan>& plans, const int occ[kGnKinds], int sm_count, int max_per_launch = kBatchMax) {
+    std::vector<BatchItem> items;
+    for (const S2mPlan& p : plans) items.push_back(BatchItem{p.grid, s2m_kind(p), p.persistent});
+    return batch_pack(items, occ, sm_count, max_per_launch);
 }
 
 // A GN-mode batched step whose sessions run different iteration counts (liliom_scan_to_map_resident_batch_ex): k_gn_batch
@@ -104,7 +84,7 @@ inline S2mPack s2m_batch_pack(const std::vector<S2mPlan>& plans, const int occ[k
 // group is packed by s2m_batch_pack.  The pack's indices are into `plans`, as for one s2m_batch_pack call over all of them.
 struct S2mGnGroup {
     int iters;
-    S2mPack pack;
+    BatchPack pack;
 };
 inline std::vector<S2mGnGroup> s2m_gn_groups(const std::vector<S2mPlan>& plans, const std::vector<int>& iters, const int occ[kGnKinds],
                                              int sm_count, int max_per_launch = kBatchMax) {
@@ -117,7 +97,7 @@ inline std::vector<S2mGnGroup> s2m_gn_groups(const std::vector<S2mPlan>& plans, 
         for (size_t j = i; j < plans.size(); ++j)
             if (!done[j] && iters[j] == iters[i]) { done[j] = 1; members.push_back((int)j); sub.push_back(plans[j]); }
         S2mGnGroup g{iters[i], s2m_batch_pack(sub, occ, sm_count, max_per_launch)};
-        for (S2mLaunch& l : g.pack.launches)
+        for (BatchLaunch& l : g.pack.launches)
             for (int& s : l.sessions) s = members[s];
         for (int& s : g.pack.solo) s = members[s];
         out.push_back(std::move(g));

@@ -6,7 +6,6 @@
 // reproducible and equal to the oracle's.  Compiled with --fmad=false.
 // The box / divisions are computed on the device (VgParams): no host round trip inside the call.
 #include "ctx.cuh"
-#include "map_stage.h"
 #include <climits>
 #include <cmath>
 #include <cstring>

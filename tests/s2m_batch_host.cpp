@@ -11,7 +11,7 @@ extern "C" int sb_pack(int B, const int* plans, const int* occ, int sm_count, in
         ps[i] = lili::S2mPlan{};
         ps[i].lanes = plans[4 * i]; ps[i].tma = plans[4 * i + 1] != 0; ps[i].grid = plans[4 * i + 2]; ps[i].persistent = plans[4 * i + 3] != 0;
     }
-    const lili::S2mPack p = lili::s2m_batch_pack(ps, occ, sm_count, max_per_launch);
+    const lili::BatchPack p = lili::s2m_batch_pack(ps, occ, sm_count, max_per_launch);
     int k = 0;
     for (size_t l = 0; l < p.launches.size(); ++l) {
         out_kind[l] = p.launches[l].kind; out_grid[l] = p.launches[l].grid; out_count[l] = (int)p.launches[l].sessions.size();

@@ -44,7 +44,7 @@ extern "C" int sp_gn_groups(int B, const int* plans, const int* iters, const int
     for (const lili::S2mGnGroup& g : gs) {
         o.put(g.iters);
         o.put((int)g.pack.launches.size());
-        for (const lili::S2mLaunch& l : g.pack.launches) { o.put(l.kind); o.put(l.grid); o.list(l.sessions); }
+        for (const lili::BatchLaunch& l : g.pack.launches) { o.put(l.kind); o.put(l.grid); o.list(l.sessions); }
         o.list(g.pack.solo);
     }
     return o.done();

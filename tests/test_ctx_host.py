@@ -18,7 +18,7 @@ def ctxh():
     if not os.path.exists(os.path.join(CUDA, "include", "cuda_runtime.h")):
         pytest.skip("CUDA headers not found")
     L = host_build.load("ctx_host", ["tests/ctx_host.cpp"], ["-O2", "-std=c++17", "-fPIC", "-Wall", "-Wno-self-move", "-I", os.path.join(CUDA, "include")],
-                        deps=["liliom_b200/csrc/ctx.cuh", "liliom_b200/csrc/vg_box.h", "include/liliom.h"],
+                        deps=["liliom_b200/csrc/ctx.cuh", "liliom_b200/csrc/batch.h", "liliom_b200/csrc/vg_box.h", "include/liliom.h"],
                         link=["-L", lib64, "-Wl,-rpath," + lib64, "-lcudart"])
     L.ctx_host_run.restype = C.c_int
     return L

@@ -25,7 +25,7 @@ def kc():
     L = host_build.load("knncore_host", ["tests/knncore_host.cpp"],
                         ["-O2", "-std=c++20", "-pthread", "-fPIC", "-ffp-contract=off", "-frounding-math", "-D_GNU_SOURCE", "-Wno-attributes",
                          "-Wno-unknown-pragmas", "-I", cuda_inc],
-                        deps=[f"liliom_b200/csrc/{h}" for h in ("knn_core.cuh", "dev_math.cuh", "ctx.cuh", "s2m_plan.h", "pcl_xform.h", "vg_box.h")]
+                        deps=[f"liliom_b200/csrc/{h}" for h in ("knn_core.cuh", "dev_math.cuh", "ctx.cuh", "s2m_plan.h", "batch.h", "pcl_xform.h", "vg_box.h")]
                         + ["include/liliom.h"])
     L.kc_gate_tau.argtypes = [C.c_double]; L.kc_gate_tau.restype = C.c_float
     L.kc_thread_knn5.argtypes = [C.c_float, C.c_float, C.c_float, C.POINTER(C.c_float), C.POINTER(C.c_int), C.c_float,

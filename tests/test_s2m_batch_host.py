@@ -15,13 +15,13 @@ KIND = {(1, 0): 0, (2, 0): 1, (4, 0): 2, (8, 0): 3, (16, 0): 4, (16, 1): 5}
 @pytest.fixture(scope="module")
 def sb():
     L = host_build.load("s2m_batch_host", ["tests/s2m_batch_host.cpp"], ["-O2", "-std=c++17", "-fPIC", "-Wall"],
-                        deps=["liliom_b200/csrc/s2m_plan.h", "include/liliom.h"])
+                        deps=["liliom_b200/csrc/s2m_plan.h", "liliom_b200/csrc/batch.h", "include/liliom.h"])
     ip = C.POINTER(C.c_int)
     L.sb_pack.argtypes = [C.c_int, ip, ip, C.c_int, C.c_int, ip, ip, ip, ip, ip, ip]
     L.sb_pack.restype = C.c_int
     L.sb_batch_max.restype = C.c_int
     sp = host_build.load("s2m_plan_host", ["tests/s2m_plan_host.cpp"], ["-O2", "-std=c++17", "-fPIC", "-Wall"],
-                         deps=["liliom_b200/csrc/s2m_plan.h", "include/liliom.h"])
+                         deps=["liliom_b200/csrc/s2m_plan.h", "liliom_b200/csrc/batch.h", "include/liliom.h"])
     sp.sp_plan.argtypes = [C.c_int] * 12 + [C.POINTER(C.c_longlong)]
     sp.sp_plan.restype = None
     return L, sp

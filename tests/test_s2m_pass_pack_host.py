@@ -15,7 +15,7 @@ LANES = (1, 2, 4, 8, 16)
 @pytest.fixture(scope="module")
 def libs():
     flags = ["-O2", "-std=c++17", "-fPIC", "-Wall"]
-    deps = ["liliom_b200/csrc/s2m_plan.h", "include/liliom.h"]
+    deps = ["liliom_b200/csrc/s2m_plan.h", "liliom_b200/csrc/batch.h", "include/liliom.h"]
     sp = host_build.load("s2m_pass_host", ["tests/s2m_pass_host.cpp"], flags, deps=deps)
     ip = C.POINTER(C.c_int)
     sp.sp_pass_pack.argtypes = [C.c_int, ip, ip, C.c_int, ip, C.c_int]

@@ -36,7 +36,7 @@ TABLE = [
 @pytest.fixture(scope="module")
 def sp():
     L = host_build.load("s2m_plan_host", ["tests/s2m_plan_host.cpp"], ["-O2", "-std=c++17", "-fPIC", "-Wall"],
-                        deps=["liliom_b200/csrc/s2m_plan.h", "include/liliom.h"])
+                        deps=["liliom_b200/csrc/s2m_plan.h", "liliom_b200/csrc/batch.h", "include/liliom.h"])
     L.sp_plan.argtypes = [C.c_int] * 12 + [C.POINTER(C.c_longlong)]
     L.sp_plan.restype = None
     return L
