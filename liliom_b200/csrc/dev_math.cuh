@@ -220,12 +220,12 @@ __device__ inline void eigen_sym3(double a00, double a10, double a20, double a11
 // from the origin with sub-metre spread, so normal equations (condition squared) would cost
 // ~1e-4 m in the plane offset — QR keeps it at ~1e-9 m.
 // Everything is register-resident (fully unrolled, column permutation via swaps).
-// kEigenOrder: apply each reflector to the trailing columns as Eigen's applyHouseholderOnTheLeft does (essential^T * bottom
-// first, then the head row), the order of the oracle's copy, so that without contraction the bits are the oracle's
-// (backend_corr.cu).  false keeps the head-row-first order the scan-to-map kernel (grid_knn.cu, compiled with contraction)
-// has always used; moving it is a change of that kernel's results and belongs with its own bit-stability work.
+// Each reflector is applied to the trailing columns as Eigen's applyHouseholderOnTheLeft does (essential^T * bottom first,
+// then the head row), the order of the oracle's copy, and every product that meets a sum is spelled with mulx / addx / subx,
+// so FMA contraction in the including unit cannot change a bit: the result is the oracle's in backend_corr.cu (built without
+// contraction) and in grid_knn.cu (built with it) alike.  On a rank-deficient system the basic solution depends on the rank
+// decision and the pivot order, so a contracted rounding could give a different plane altogether, not a last-bit difference.
 // ---------------------------------------------------------------------------------------
-template <bool kEigenOrder = true>
 __device__ inline void colpiv_qr_solve_5x3(double A[5][3], double b[5], double x[3]) {
     double nu[3], ndir[3], tau[3];
     int perm[3] = {0, 1, 2};
@@ -233,7 +233,7 @@ __device__ inline void colpiv_qr_solve_5x3(double A[5][3], double b[5], double x
     for (int k = 0; k < 3; ++k) {
         double s = 0;
 #pragma unroll
-        for (int i = 0; i < 5; ++i) s += A[i][k] * A[i][k];
+        for (int i = 0; i < 5; ++i) s = addx(s, mulx(A[i][k], A[i][k]));
         nu[k] = ndir[k] = sqrt(s);
     }
     double maxn = fmax(nu[0], fmax(nu[1], nu[2]));
@@ -263,14 +263,14 @@ __device__ inline void colpiv_qr_solve_5x3(double A[5][3], double b[5], double x
         }
         double tail = 0;
 #pragma unroll
-        for (int i = k + 1; i < 5; ++i) tail += A[i][k] * A[i][k];
+        for (int i = k + 1; i < 5; ++i) tail = addx(tail, mulx(A[i][k], A[i][k]));
         double c0 = A[k][k], beta, tk;
         if (tail <= DBL_MIN) {
             tk = 0; beta = c0;
 #pragma unroll
             for (int i = k + 1; i < 5; ++i) A[i][k] = 0;
         } else {
-            beta = sqrt(c0 * c0 + tail);
+            beta = sqrt(addx(mulx(c0, c0), tail));
             if (c0 >= 0) beta = -beta;
             double inv = c0 - beta;
 #pragma unroll
@@ -282,31 +282,31 @@ __device__ inline void colpiv_qr_solve_5x3(double A[5][3], double b[5], double x
         if (tk != 0) {
 #pragma unroll
             for (int j = k + 1; j < 3; ++j) {
-                double tmp = kEigenOrder ? 0.0 : A[k][j];
+                double tmp = 0.0;
 #pragma unroll
-                for (int i = k + 1; i < 5; ++i) tmp += A[i][k] * A[i][j];
-                if (kEigenOrder) tmp += A[k][j];
-                A[k][j] -= tk * tmp;
+                for (int i = k + 1; i < 5; ++i) tmp = addx(tmp, mulx(A[i][k], A[i][j]));
+                tmp = addx(tmp, A[k][j]);
+                A[k][j] = subx(A[k][j], mulx(tk, tmp));
 #pragma unroll
-                for (int i = k + 1; i < 5; ++i) A[i][j] -= tk * A[i][k] * tmp;
+                for (int i = k + 1; i < 5; ++i) A[i][j] = subx(A[i][j], mulx(mulx(tk, A[i][k]), tmp));
             }
         }
 #pragma unroll
         for (int j = k + 1; j < 3; ++j) {
             if (nu[j] != 0) {
                 double temp = fabs(A[k][j]) / nu[j];
-                temp = (1.0 + temp) * (1.0 - temp);
+                temp = mulx(1.0 + temp, 1.0 - temp);
                 temp = temp < 0 ? 0 : temp;
                 double r = nu[j] / ndir[j];
-                double temp2 = temp * r * r;
+                double temp2 = mulx(mulx(temp, r), r);
                 if (temp2 <= downdate_thr) {
                     double s = 0;
 #pragma unroll
-                    for (int i = k + 1; i < 5; ++i) s += A[i][j] * A[i][j];
+                    for (int i = k + 1; i < 5; ++i) s = addx(s, mulx(A[i][j], A[i][j]));
                     ndir[j] = sqrt(s);
                     nu[j] = ndir[j];
                 } else {
-                    nu[j] *= sqrt(temp);
+                    nu[j] = mulx(nu[j], sqrt(temp));
                 }
             }
         }
@@ -318,10 +318,10 @@ __device__ inline void colpiv_qr_solve_5x3(double A[5][3], double b[5], double x
         if (k < nonzero && tau[k] != 0) {
             double tmp = b[k];
 #pragma unroll
-            for (int i = k + 1; i < 5; ++i) tmp += A[i][k] * b[i];
-            b[k] -= tau[k] * tmp;
+            for (int i = k + 1; i < 5; ++i) tmp = addx(tmp, mulx(A[i][k], b[i]));
+            b[k] = subx(b[k], mulx(tau[k], tmp));
 #pragma unroll
-            for (int i = k + 1; i < 5; ++i) b[i] -= tau[k] * A[i][k] * tmp;
+            for (int i = k + 1; i < 5; ++i) b[i] = subx(b[i], mulx(mulx(tau[k], A[i][k]), tmp));
         }
     }
     double c[3] = {b[0], b[1], b[2]};
@@ -330,7 +330,7 @@ __device__ inline void colpiv_qr_solve_5x3(double A[5][3], double b[5], double x
         if (i < nonzero) {
             double s = c[i];
 #pragma unroll
-            for (int j = i + 1; j < 3; ++j) if (j < nonzero) s -= A[i][j] * c[j];
+            for (int j = i + 1; j < 3; ++j) if (j < nonzero) s = subx(s, mulx(A[i][j], c[j]));
             c[i] = s / A[i][i];
         }
     }
@@ -349,15 +349,22 @@ __device__ inline void colpiv_qr_solve_5x3(double A[5][3], double b[5], double x
 // Fast path of the same least-squares plane  min || A n + 1 ||  (A = the 5 neighbours):
 // with c = centroid, q_j = p_j - c and S = sum q_j q_j^T,   A^T A = S + 5 c c^T,  A^T 1 = 5 c,
 // so by Sherman-Morrison   n = -5 u / (1 + 5 c.u),   u = S^-1 c.
-// S is built from CENTRED coordinates (differences of fp32 values are exact in fp64), so its
-// conditioning is the patch's own spread ratio (~1e3..1e6) instead of (|p|/spread)^2 of the
-// raw normal equations; a 3x3 LDL^T (stable for SPD without pivoting) then gives the same
-// minimiser as the Householder QR to ~1e-12 relative, in ~1/8 of the fp64 instructions.
+// S is built from CENTRED coordinates, so its conditioning is the patch's own spread ratio
+// instead of (|p|/spread)^2 of the raw normal equations; a 3x3 LDL^T (stable for SPD without
+// pivoting) then solves it in ~1/8 of the fp64 instructions of the Householder QR.
+// It does NOT give the QR's bits: the two normals differ by up to ~1e-6 relative on far, thin or
+// nearly collinear patches (mostly the QR's own error on the ill-conditioned raw A), always within
+// the bound rho of plane_fit_gate (tests/test_devmath_host.py measures both).  So it never decides
+// a gate alone: plane_fit_gate refits on the exact path every query whose gate
+// quantities lie within that bound of a threshold, and only then is the accept count exactly the
+// oracle's.  Out, for that bound: kS = tr^3 / (d0 d1 d2) >= cond(S) (lambda_min(S) >= det / tr^2
+// = d0 d1 d2 / tr^2), kA2 = (tr + 5 |c|^2) tr^2 / (d0 d1 d2) >= cond(A)^2 (A^T A = S + 5 c c^T:
+// lambda_max <= tr + 5 |c|^2, lambda_min >= lambda_min(S)) and cn = sqrt(3) max_i |c_i| >= |c|.
 // Returns false when S is numerically singular (collinear / coincident / exactly coplanar
-// neighbours): the caller then takes the rank-revealing QR path, which reproduces Eigen's
-// behaviour for those cases.
+// neighbours): the caller then takes the exact QR path, which reproduces Eigen's behaviour
+// for those cases.
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ bool plane_fit5_fast(const float4 m[5], double nv[3]) {
+__device__ __forceinline__ bool plane_fit5_fast(const float4 m[5], double nv[3], double& kS, double& kA2, double& cn) {
     const double cx = ((double)m[0].x + (double)m[1].x + (double)m[2].x + (double)m[3].x + (double)m[4].x) * 0.2;
     const double cy = ((double)m[0].y + (double)m[1].y + (double)m[2].y + (double)m[3].y + (double)m[4].y) * 0.2;
     const double cz = ((double)m[0].z + (double)m[1].z + (double)m[2].z + (double)m[3].z + (double)m[4].z) * 0.2;
@@ -383,20 +390,26 @@ __device__ __forceinline__ bool plane_fit5_fast(const float4 m[5], double nv[3])
     if (!(d2 > tiny)) return false;
     // u = S^-1 c
     const double y0 = cx, y1 = cy - l10 * y0, y2 = cz - l20 * y0 - l21 * y1;
-    const double z2 = y2 / d2;
+    const double i2 = 1.0 / d2;
+    const double z2 = y2 * i2;
     const double z1 = y1 * i1 - l21 * z2;
     const double z0 = y0 * i0 - l10 * z1 - l20 * z2;
     const double den = 1.0 + 5.0 * (cx * z0 + cy * z1 + cz * z2);
     const double sc = -5.0 / den;
     nv[0] = sc * z0; nv[1] = sc * z1; nv[2] = sc * z2;
+    const double tr2_det = tr * tr * (i0 * i1 * i2);
+    kS = tr * tr2_det;
+    kA2 = kS + 5.0 * (cx * cx + cy * cy + cz * cz) * tr2_det;
+    cn = 1.7320508075688774 * fmax(fmax(fabs(cx), fabs(cy)), fabs(cz));
     return isfinite(nv[0]) && isfinite(nv[1]) && isfinite(nv[2]);
 }
 
+// The exact path: the oracle's column-pivoted QR on the raw neighbours (L/src/LidarOdometry.cpp:375), bit for bit.
 static __device__ __noinline__ void plane_fit5_qr(const float4 m[5], double nv[3]) {
     double A[5][3], B[5];
 #pragma unroll
     for (int j = 0; j < 5; ++j) { A[j][0] = m[j].x; A[j][1] = m[j].y; A[j][2] = m[j].z; B[j] = -1.0; }
-    colpiv_qr_solve_5x3<false>(A, B, nv);
+    colpiv_qr_solve_5x3(A, B, nv);
 }
 
 // 6x6 SPD solve (LDL^T), H given as the 21-scalar upper triangle (row-major), rhs b.
@@ -520,31 +533,122 @@ __device__ inline void pose_plus(const double x[7], const double d[6], double ou
 // 1486-1504) in the reference's mixed fp32/fp64 widths: normalise nv, every neighbour within plane_thres, then the fp32 weight of the
 // transformed query (sx, sy, sz) above w_gate.  `refuse` rejects the plane after the distance test (the backend's reflectivity gate).
 // On acceptance pl = weight * [n, 1/|nv|] and `weight` are set; otherwise neither is touched.
-__device__ __forceinline__ bool plane_gate(double nv[3], const float4 m[5], float sx, float sy, float sz, double plane_thres,
-                                           double w_gate, bool refuse, float4& pl, float& weight) {
-    const double n2 = nv[0] * nv[0] + nv[1] * nv[1] + nv[2] * nv[2];
-    const double nn = sqrt(n2);
+// Every operation is exact (mulx / addx): from the same nv the gate gives the oracle's bits in a contracted unit as well.
+__device__ __forceinline__ double gate_normalise(double nv[3], double& nn) {       // returns normInverse (nn = |nv|), nv normalised
+    const double n2 = addx(addx(mulx(nv[0], nv[0]), mulx(nv[1], nv[1])), mulx(nv[2], nv[2]));
+    nn = sqrt(n2);
     const double normInverse = 1.0 / nn;                                                                      // :376
     if (n2 > 0) { nv[0] /= nn; nv[1] /= nn; nv[2] /= nn; }                                                    // :377
+    return normInverse;
+}
+__device__ __forceinline__ double gate_dist(const double n[3], double normInverse, double x, double y, double z) {   // :386-393
+    return fabs(addx(addx(addx(mulx(n[0], x), mulx(n[1], y)), mulx(n[2], z)), normInverse));
+}
+__device__ __forceinline__ float gate_weight(const double n[3], double normInverse, float sx, float sy, float sz, float& rng) {
+    // :397-398 in the reference's widths
+    const float pd = (float)addx(addx(addx(mulx(n[0], (double)sx), mulx(n[1], (double)sy)), mulx(n[2], (double)sz)), normInverse);
+    rng = __fsqrt_rn(__fsqrt_rn(faddx(faddx(fmulx(sx, sx), fmulx(sy, sy)), fmulx(sz, sz))));
+    return (float)subx(1.0, mulx(0.9, (double)fabsf(pd)) / (double)rng);
+}
+__device__ __forceinline__ void gate_plane(const double n[3], double normInverse, float w, float4& pl) {               // :402-405
+    pl = make_float4((float)mulx((double)w, n[0]), (float)mulx((double)w, n[1]), (float)mulx((double)w, n[2]),
+                     (float)mulx((double)w, normInverse));
+}
+__device__ __forceinline__ bool plane_gate(double nv[3], const float4 m[5], float sx, float sy, float sz, double plane_thres,
+                                           double w_gate, bool refuse, float4& pl, float& weight) {
+    double nn;
+    const double normInverse = gate_normalise(nv, nn);
     bool planeValid = true;
 #pragma unroll
-    for (int j = 0; j < 5; ++j)                                                                                // :386-393
-        if (fabs(nv[0] * m[j].x + nv[1] * m[j].y + nv[2] * m[j].z + normInverse) > plane_thres) planeValid = false;
+    for (int j = 0; j < 5; ++j)
+        if (gate_dist(nv, normInverse, m[j].x, m[j].y, m[j].z) > plane_thres) planeValid = false;
     if (refuse) planeValid = false;
     bool ok = false;
     if (planeValid) {
-        // :397-398; exact ops keep the fp32 roundings stable
-        const float pd = (float)addx(addx(addx(mulx(nv[0], (double)sx), mulx(nv[1], (double)sy)), mulx(nv[2], (double)sz)), normInverse);
-        const float rng = __fsqrt_rn(__fsqrt_rn(faddx(faddx(fmulx(sx, sx), fmulx(sy, sy)), fmulx(sz, sz))));
-        const float w = (float)subx(1.0, mulx(0.9, (double)fabsf(pd)) / (double)rng);
+        float rng;
+        const float w = gate_weight(nv, normInverse, sx, sy, sz, rng);
         if ((double)w > w_gate) {                                                                              // :400
-            pl = make_float4((float)mulx((double)w, nv[0]), (float)mulx((double)w, nv[1]),                     // :402-405
-                             (float)mulx((double)w, nv[2]), (float)mulx((double)w, normInverse));
+            gate_plane(nv, normInverse, w, pl);
             weight = w;
             ok = true;
         }
     }
     return ok;
+}
+
+// Phase B of the scan-to-map pass for one query (grid_knn.cu): plane fit and gates, with the accept decision exactly the oracle's.
+// The fast fit's nv decides only when every gate quantity lies farther from its threshold than the two fits can disagree;
+// otherwise the query is refitted on the exact path (the oracle's QR, bit for bit) and gated again.  path (out): 0 the fast fit
+// decided, 1 the fast fit declined (a singular scatter), 2 the guard band sent the query to the exact path.
+//
+// The guard band, derived (u = 2^-53; first order in u, every constant rounded up):
+//  * Fit error.  Both fits are backward stable solvers of  min |A nv + 1|,  so each lies within rho_k |nv| of the exact minimiser:
+//      fast (LDL^T of the centred scatter S, then Sherman-Morrison):  rho_f <= c u kS (1 + |c| |nv|).  S and its LDL^T carry a
+//        backward error of a few u tr(S), so u = S^-1 c moves by c u cond(S) relative; nv = -5 u / (1 + 5 c.u) amplifies a
+//        relative error of u by at most 1 + 2 |c| |u| / |c.u| <= 1 + 2 |c| |nv| (c.nv ~ -1 for a fitted plane).  The rounding of
+//        the centroid cancels to first order (it moves nv along itself by ~u |c| |nv|).
+//      QR (Householder least squares on the raw 5x3 A, Higham, ASNA 2nd ed., Thm 20.3 and 20.1): backward error gamma_{c m n}
+//        with m n = 15, forward error  rho_q <= c u (cond(A) + cond(A)^2 eta),  eta = |r| / (|A| |nv|) <= t / (1 - t) with
+//        t = max_j |nv . m_j + 1| = dmax |nv| the residual of the fitted plane (|A nv| >= |1| - |r|, all norms sup-norms over
+//        the five rows).
+//    kS >= cond(S) and kA2 >= cond(A)^2 come from the LDL^T pivots (plane_fit5_fast).  rho = 16 eps (kS (1 + cn |nv|) +
+//    sqrt(kA2) + 2 kA2 t) covers rho_f + rho_q with c = 32 for each (the QR's gamma_{15 c'} with c' = 2); cn >= |c| and
+//    2 t >= t / (1 - t) for t < 1/2 keep it free of divisions and of a second square root.
+//  * Distances.  dist_j(nv) = |nv . m_j + 1| / |nv| has gradient norm <= (|m_j| + dist_j) / |nv|, so two fits rho apart (rho < 1/4)
+//    give distances 4 rho (|m_j|_1 + normInverse) apart; each evaluation (exact ops, normalisation included) rounds by less than
+//    16 u (|m_j|_1 + normInverse).  Hence  band_d = 4 (rho + 8 u) M,  M = max_j |m_j|_1 + normInverse, on the largest distance
+//    (the gate is  dmax > plane_thres, and max is 1-Lipschitz).
+//  * Weight.  pd moves by 4 (rho + 8 u) P, P = |s|_1 + normInverse, before its fp32 rounding; two fp32 roundings of values a and b
+//    differ by at most |a - b| + 2^-24 (|a| + |b|); w = 1 - 0.9 |pd| / rng in fp64, then fp32 once more.  Hence
+//    band_w = (4 (rho + 8 u) P + 2^-22 P) / rng + 2^-22 (1 + |w|).
+// A NaN or infinite band (a zero range, a plane through the origin) sends the query to the exact path.  The CPU tier checks the
+// largest fast-vs-QR deviation it meets against rho (tests/test_devmath_host.py).
+constexpr double kGuardRhoC = 16.0 * DBL_EPSILON;
+__device__ __forceinline__ double fit_err_bound(double kS, double kA2, double cn, double nn, double dmax) {      // rho
+    const double t = dmax * nn;                         // t / (1 - t) <= 2 t for t < 1/2
+    return t < 0.5 ? kGuardRhoC * (kS * (1.0 + cn * nn) + sqrt(kA2) + 2.0 * kA2 * t) : (double)INFINITY;
+}
+// the exact path, out of line: it is the cold path of the GN pass
+static __device__ __noinline__ bool plane_fit_gate_exact(const float4 m[5], float sx, float sy, float sz, double plane_thres,
+                                                         double w_gate, float4& pl, float& weight) {
+    double nv[3];
+    plane_fit5_qr(m, nv);
+    return plane_gate(nv, m, sx, sy, sz, plane_thres, w_gate, false, pl, weight);
+}
+__device__ __forceinline__ bool plane_fit_gate(const float4 m[5], float sx, float sy, float sz, double plane_thres, double w_gate,
+                                               float4& pl, float& weight, int& path) {
+    double nv[3], kS, kA2, cn;
+    if (plane_fit5_fast(m, nv, kS, kA2, cn)) {
+        double nn;
+        const double ninv = gate_normalise(nv, nn);
+        double dmax = 0.0, m1 = 0.0;
+#pragma unroll
+        for (int j = 0; j < 5; ++j) {
+            dmax = fmax(dmax, gate_dist(nv, ninv, m[j].x, m[j].y, m[j].z));
+            m1 = fmax(m1, fabs((double)m[j].x) + fabs((double)m[j].y) + fabs((double)m[j].z));
+        }
+        const double rho = fit_err_bound(kS, kA2, cn, nn, dmax);
+        const double eps8 = 4.0 * DBL_EPSILON;
+        const double band_d = 4.0 * (rho + eps8) * (m1 + ninv);
+        if (rho < 0.25 && fabs(dmax - plane_thres) > band_d) {
+            path = 0;
+            if (dmax > plane_thres) return false;
+            float rng;
+            const float w = gate_weight(nv, ninv, sx, sy, sz, rng);
+            const double P = fabs((double)sx) + fabs((double)sy) + fabs((double)sz) + ninv;
+            const double band_w = (4.0 * (rho + eps8) * P + 0x1p-22 * P) / (double)rng + 0x1p-22 * (1.0 + fabs((double)w));
+            if (fabs((double)w - w_gate) > band_w) {
+                if (!((double)w > w_gate)) return false;
+                gate_plane(nv, ninv, w, pl);
+                weight = w;
+                return true;
+            }
+        }
+        path = 2;
+    } else {
+        path = 1;
+    }
+    return plane_fit_gate_exact(m, sx, sy, sz, plane_thres, w_gate, pl, weight);
 }
 
 struct Row { double J[6]; double r; double half_rho; };     // Jacobian row, residual and (after a corrector) rho / 2

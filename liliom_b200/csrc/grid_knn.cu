@@ -317,10 +317,9 @@ __device__ __forceinline__ void knn_phases(const KnnArgs& a, const Q4& q, const 
                 float4 m[5];
 #pragma unroll
                 for (int j = 0; j < 5; ++j) m[j] = __ldg(a.map_orig + s.idx[j]);                                     // :369-371
-                double nv[3];
-                if (!plane_fit5_fast(m, nv)) plane_fit5_qr(m, nv);                                                    // :375 (see dev_math.cuh)
                 float weight;
-                ok = plane_gate(nv, m, s.sx, s.sy, s.sz, a.plane_thres, a.w_gate, false, pl, weight);
+                int path;
+                ok = plane_fit_gate(m, s.sx, s.sy, s.sz, a.plane_thres, a.w_gate, pl, weight, path);                // :375-405 (see dev_math.cuh)
             }
             if (qi < n_q) {
                 if (a.valid) a.valid[qi] = ok ? 1 : 0;

@@ -24,26 +24,25 @@ static inline void transform_point(const double pose7[7], const float p[3], floa
     out[0] = (float)o.x; out[1] = (float)o.y; out[2] = (float)o.z;
 }
 
-// LidarOdometry.cpp:362-410 for one feature, given its 5-NN.  Returns 1 when a
-// correspondence is emitted and fills plane[4] = {w*nx, w*ny, w*nz, w*d}.
-static inline int surf_corr_one(const float* map_xyzw, const float sel[3], const int idx[5], const float sqd[5],
-                                double max_sqd, double plane_thres, double w_gate, float plane[4], float* weight_out) {
-    if (!((double)sqd[4] < max_sqd)) return 0;                       // :365
+// LidarOdometry.cpp:369-405 on the five neighbours mp[j].  Returns 1 when a correspondence is
+// emitted and fills plane[4] = {w*nx, w*ny, w*nz, w*d}; nv_out (optional) gets the QR's
+// un-normalised normal.
+static inline int fit_gate_one(const float* const mp[5], const float sel[3], double plane_thres, double w_gate, float plane[4],
+                               float* weight_out, double* nv_out) {
     double A[15], B[5];
     for (int j = 0; j < 5; ++j) {
-        const float* mp = map_xyzw + 4 * (size_t)idx[j];
-        A[3 * j + 0] = mp[0]; A[3 * j + 1] = mp[1]; A[3 * j + 2] = mp[2];   // :369-371
+        A[3 * j + 0] = mp[j][0]; A[3 * j + 1] = mp[j][1]; A[3 * j + 2] = mp[j][2];   // :369-371
         B[j] = -1.0;                                                  // :363
     }
     double nv[3];
     colpiv_qr_solve_nx3(5, A, B, nv);                                 // :375
+    if (nv_out) for (int k = 0; k < 3; ++k) nv_out[k] = nv[k];
     double nn = std::sqrt(nv[0] * nv[0] + nv[1] * nv[1] + nv[2] * nv[2]);
     double normInverse = 1 / nn;                                      // :376
     double n2 = nv[0] * nv[0] + nv[1] * nv[1] + nv[2] * nv[2];
     if (n2 > 0) { double s = std::sqrt(n2); nv[0] /= s; nv[1] /= s; nv[2] /= s; }   // :377 normalize()
     for (int j = 0; j < 5; ++j) {                                     // :386-393
-        const float* mp = map_xyzw + 4 * (size_t)idx[j];
-        if (std::fabs(nv[0] * mp[0] + nv[1] * mp[1] + nv[2] * mp[2] + normInverse) > plane_thres) return 0;
+        if (std::fabs(nv[0] * mp[j][0] + nv[1] * mp[j][1] + nv[2] * mp[j][2] + normInverse) > plane_thres) return 0;
     }
     // :397-398 — mixed widths exactly as written (fabs/sqrt resolve to the float overloads)
     float pd = nv[0] * sel[0] + nv[1] * sel[1] + nv[2] * sel[2] + normInverse;
@@ -55,6 +54,30 @@ static inline int surf_corr_one(const float* map_xyzw, const float sel[3], const
     plane[3] = weight * normInverse;
     if (weight_out) *weight_out = weight;
     return 1;
+}
+
+// LidarOdometry.cpp:362-410 for one feature, given its 5-NN.
+static inline int surf_corr_one(const float* map_xyzw, const float sel[3], const int idx[5], const float sqd[5],
+                                double max_sqd, double plane_thres, double w_gate, float plane[4], float* weight_out) {
+    if (!((double)sqd[4] < max_sqd)) return 0;                       // :365
+    const float* mp[5];
+    for (int j = 0; j < 5; ++j) mp[j] = map_xyzw + 4 * (size_t)idx[j];
+    return fit_gate_one(mp, sel, plane_thres, w_gate, plane, weight_out, nullptr);
+}
+
+// :369-405 for n neighbourhoods m20 (n x 5 x 4 floats) and transformed queries s3 (n x 3), at the thresholds plane_thres[i], w_gate[i]:
+// ok[i], plane (zero when refused), weight and the QR's un-normalised normal nv3 (n x 3).
+extern "C" void orc_fit_gate_batch(const float* m20, const float* s3, int n, const double* plane_thres, const double* w_gate, unsigned char* ok,
+                                   float* plane4, float* weight, double* nv3) {
+    for (int i = 0; i < n; ++i) {
+        const float* mp[5];
+        for (int j = 0; j < 5; ++j) mp[j] = m20 + 20 * (size_t)i + 4 * j;
+        float pl[4] = {0, 0, 0, 0};
+        float w = 0.0f;
+        ok[i] = (unsigned char)fit_gate_one(mp, s3 + 3 * (size_t)i, plane_thres[i], w_gate[i], pl, &w, nv3 + 3 * (size_t)i);
+        for (int k = 0; k < 4; ++k) plane4[4 * (size_t)i + k] = pl[k];
+        weight[i] = w;
+    }
 }
 
 extern "C" int orc_find_surf_corr(const void* tree, const float* map_xyzw, int m, const float* feats_xyzw, int n,

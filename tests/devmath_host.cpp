@@ -26,9 +26,42 @@ extern "C" {
 int dm_plane_fit5(const float* m20, double nv[3]) {          // returns 1 when the fast path produced the answer, 0 for the QR fallback
     float4 m[5];
     for (int j = 0; j < 5; ++j) m[j] = make_float4(m20[4 * j], m20[4 * j + 1], m20[4 * j + 2], m20[4 * j + 3]);
-    if (plane_fit5_fast(m, nv)) return 1;
+    double kS, kA2, cn;
+    if (plane_fit5_fast(m, nv, kS, kA2, cn)) return 1;
     plane_fit5_qr(m, nv);
     return 0;
+}
+// n neighbourhoods (m20: n x 5 x 4 floats, s3: n x 3 transformed queries) through plane_fit_gate, as phase B of the GN pass runs
+// it, at the thresholds plane_thres[i] and w_gate[i]: ok[i], path[i] (0 fast, 1 declined, 2 guard band), pl4 / weight (left as passed in when refused).  When fit is given, also
+// the fast path's own normal (fit[4 i .. 4 i + 2], un-normalised; fit[4 i + 3] = 1 when the fast path took the set) and its
+// fit-error bound rho (plane_fit_gate's, NaN when the fast path declined) in rho[i].
+void dm_fit_gate_batch(const float* m20, const float* s3, int n, const double* plane_thres, const double* w_gate, unsigned char* ok, int* path,
+                       float* pl4, float* weight, double* fit, double* rho) {
+    for (int i = 0; i < n; ++i) {
+        float4 m[5];
+        const float* p = m20 + 20 * (size_t)i;
+        for (int j = 0; j < 5; ++j) m[j] = make_float4(p[4 * j], p[4 * j + 1], p[4 * j + 2], p[4 * j + 3]);
+        const float* s = s3 + 3 * (size_t)i;
+        float4 pl = make_float4(pl4[4 * i], pl4[4 * i + 1], pl4[4 * i + 2], pl4[4 * i + 3]);
+        ok[i] = plane_fit_gate(m, s[0], s[1], s[2], plane_thres[i], w_gate[i], pl, weight[i], path[i]) ? 1 : 0;
+        pl4[4 * i] = pl.x; pl4[4 * i + 1] = pl.y; pl4[4 * i + 2] = pl.z; pl4[4 * i + 3] = pl.w;
+        if (fit) {
+            double nv[3], kS, kA2, cn;
+            const bool fast = plane_fit5_fast(m, nv, kS, kA2, cn);
+            for (int k = 0; k < 3; ++k) fit[4 * (size_t)i + k] = fast ? nv[k] : 0.0;
+            fit[4 * (size_t)i + 3] = fast ? 1.0 : 0.0;
+            if (fast) {       // plane_fit_gate's rho from the same quantities
+                double n[3] = {nv[0], nv[1], nv[2]};
+                double nn;
+                const double ninv = gate_normalise(n, nn);
+                double dmax = 0.0;
+                for (int j = 0; j < 5; ++j) dmax = fmax(dmax, gate_dist(n, ninv, m[j].x, m[j].y, m[j].z));
+                rho[i] = fit_err_bound(kS, kA2, cn, nn, dmax);
+            } else {
+                rho[i] = NAN;
+            }
+        }
+    }
 }
 int dm_solve6(const double s21[21], const double rhs[6], double x[6]) { return solve6_ldlt(s21, rhs, x) ? 1 : 0; }
 int dm_gn_safe_step(const double s21[21], const double rhs[6], double d[6]) { return gn_safe_step(s21, rhs, d) ? 1 : 0; }

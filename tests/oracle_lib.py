@@ -62,6 +62,7 @@ def lib():
         L.orc_eigen_sym3.argtypes = [dp, dp, dp]; L.orc_eigen_sym3.restype = None
         L.orc_colpiv_qr_solve.argtypes = [C.c_int, dp, dp, dp]; L.orc_colpiv_qr_solve.restype = None
         L.orc_slerp_identity.argtypes = [dp, C.c_double, dp]; L.orc_slerp_identity.restype = None
+        L.orc_fit_gate_batch.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, vp, vp]; L.orc_fit_gate_batch.restype = None
         _lib = L
     return _lib
 
@@ -210,6 +211,19 @@ def colpiv_qr_solve(A, b):
     x = np.zeros(3)
     lib().orc_colpiv_qr_solve(len(A), _d(A.reshape(-1)), _d(b), _d(x))
     return x
+
+
+def fit_gate(m, s, plane_thres=0.06, w_gate=0.4):
+    """L/src/LidarOdometry.cpp:369-405 on n neighbourhoods m (n x 5 x 4 fp32) and transformed queries s (n x 3 fp32): the QR
+    plane fit and both gates at the thresholds (scalars or one per neighbourhood).  Returns (ok, plane, weight, the QR's un-normalised normal)."""
+    m = np.ascontiguousarray(m, np.float32).reshape(-1, 5, 4); s = np.ascontiguousarray(s, np.float32).reshape(-1, 3)
+    n = len(m)
+    ok = np.zeros(max(n, 1), np.uint8); plane = np.zeros((max(n, 1), 4), np.float32)
+    w = np.zeros(max(n, 1), np.float32); nv = np.zeros((max(n, 1), 3))
+    thr = np.ascontiguousarray(np.broadcast_to(np.asarray(plane_thres, np.float64), (n,)))
+    wg = np.ascontiguousarray(np.broadcast_to(np.asarray(w_gate, np.float64), (n,)))
+    lib().orc_fit_gate_batch(_p(m), _p(s), n, _p(thr), _p(wg), _p(ok), _p(plane), _p(w), _p(nv))
+    return ok[:n], plane[:n], w[:n], nv[:n]
 
 
 def slerp_identity(q, t):

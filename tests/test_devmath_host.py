@@ -29,6 +29,7 @@ def dm():
     L.dm_plane_gate.argtypes = [dp, fp, fp, C.c_double, C.c_double, C.c_int, fp, fp]
     L.dm_plane_neq.argtypes = [vp, C.c_int, vp, vp, dp, C.c_double, dp]; L.dm_plane_neq.restype = None
     L.dm_cauchy_fold.argtypes = [dp, dp, C.c_int, C.c_double, dp]; L.dm_cauchy_fold.restype = None
+    L.dm_fit_gate_batch.argtypes = [vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]; L.dm_fit_gate_batch.restype = None
     return L
 
 
@@ -288,6 +289,124 @@ def test_plane_gate_bit_for_bit_against_numpy(dm):
                     else:
                         assert (pl == -7.0).all() and w[0] == -7.0                  # a refused plane leaves the outputs alone
     assert n_ok > 500 and n_edge > 100
+
+
+def fit_gate_device(dm, m, s, plane_thres, w_gate):
+    """dev_math.cuh::plane_fit_gate (phase B of the GN pass) on n neighbourhoods m (n x 5 x 4) and queries s (n x 3), thresholds
+    scalar or per neighbourhood.  Returns (ok, path, plane, weight, the fast fit's normal (n x 3) or zeros, fast flag, rho)."""
+    m = np.ascontiguousarray(m, np.float32).reshape(-1, 5, 4); s = np.ascontiguousarray(s, np.float32).reshape(-1, 3)
+    n = len(m)
+    thr = np.ascontiguousarray(np.broadcast_to(np.asarray(plane_thres, np.float64), (n,)))
+    wg = np.ascontiguousarray(np.broadcast_to(np.asarray(w_gate, np.float64), (n,)))
+    ok = np.zeros(n, np.uint8); path = np.zeros(n, np.int32); pl = np.zeros((n, 4), np.float32); w = np.zeros(n, np.float32)
+    fit = np.zeros((n, 4)); rho = np.zeros(n)
+    dm.dm_fit_gate_batch(m.ctypes.data, s.ctypes.data, n, thr.ctypes.data, wg.ctypes.data, ok.ctypes.data, path.ctypes.data,
+                         pl.ctypes.data, w.ctypes.data, fit.ctypes.data, rho.ctypes.data)
+    return ok, path, pl, w, fit[:, :3], fit[:, 3] == 1.0, rho
+
+
+def oracle_gate_max_dist(nv, m):
+    """the oracle's largest neighbour distance |n . m_j + 1/|nv|| (L:376-393) from its un-normalised normals nv (n x 3), in its
+    operation order, vectorised (NumPy's elementwise fp64 operations round like the oracle's uncontracted build)"""
+    n0, n1, n2 = nv[:, 0], nv[:, 1], nv[:, 2]
+    nn = np.sqrt(n0 * n0 + n1 * n1 + n2 * n2)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        inv = 1.0 / nn
+        nz = (n0 * n0 + n1 * n1 + n2 * n2) > 0
+        s = np.where(nz, nn, 1.0)
+        n0, n1, n2 = np.where(nz, n0 / s, n0), np.where(nz, n1 / s, n1), np.where(nz, n2 / s, n2)
+        p = m[:, :, :3].astype(np.float64)
+        d = np.abs(n0[:, None] * p[:, :, 0] + n1[:, None] * p[:, :, 1] + n2[:, None] * p[:, :, 2] + inv[:, None])
+    return d.max(1)
+
+
+def random_patches(rng, n):
+    """n seeded neighbourhoods with their queries, in families where the fast fit and the QR part most: the recipe of
+    test_plane_gate_bit_for_bit_against_numpy (centres up to 300 m out, 0.6 m spread, nearly planar), far patches (up to
+    2 km), thin sub-millimetre patches hundreds of metres out (scatter pivots near the fast path's 1e-9 tr decline
+    threshold), near-collinear sets, and noisy planes near the origin.  Returns (m: n x 5 x 4 fp32, s: n x 3 fp32)."""
+    fam = rng.integers(0, 5, n)
+    reach = np.choose(fam, [300.0, 2000.0, 500.0, 300.0, 3.0])
+    spread = np.choose(fam, [0.6, 0.6, 5e-4, 0.6, 0.5])
+    c = rng.uniform(-1, 1, (n, 3)) * reach[:, None]
+    nrm = rng.normal(size=(n, 3)); nrm /= np.linalg.norm(nrm, axis=1, keepdims=True)
+    P = c[:, None, :] + rng.uniform(-1, 1, (n, 5, 3)) * spread[:, None, None]
+    flat = 1.0 - 10.0 ** rng.uniform(-6, -0.5, n)                         # out-of-plane share removed
+    P -= ((P - c[:, None, :]) * nrm[:, None, :]).sum(2, keepdims=True) * nrm[:, None, :] * flat[:, None, None]
+    line = fam == 3                                                       # near-collinear: squeeze onto a line through the centre
+    u = rng.normal(size=(n, 3)); u /= np.linalg.norm(u, axis=1, keepdims=True)
+    D = P - c[:, None, :]
+    along = (D * u[:, None, :]).sum(2, keepdims=True) * u[:, None, :]
+    squeeze = 10.0 ** rng.uniform(-7, -2, n)
+    P = np.where(line[:, None, None], c[:, None, :] + along + (D - along) * squeeze[:, None, None], P)
+    m = np.ones((n, 5, 4), np.float32); m[:, :, :3] = P
+    s = (c + nrm * rng.uniform(-0.3, 0.3, (n, 1)) + rng.uniform(-0.3, 0.3, (n, 3)) * spread[:, None]).astype(np.float32)
+    return m, s
+
+
+def test_plane_fit_gate_decisions_equal_oracle(dm, oracle):
+    """dev_math.cuh::plane_fit_gate (fast fit, guard band, exact QR path, gates: what phase B of every GN pass runs) against the
+    oracle's QR fit and gates (L:369-405), decisions bit for bit: on 10^6 seeded neighbourhoods at the defaults (0.06, 0.4) and
+    at 0.2 / 0.1, and on 2x10^5 of them put exactly on a threshold, each at its own: plane_thres at the oracle's own largest
+    distance (kept), one ulp below (refused) and one above (kept); w_gate at the oracle's own weight (refused: the test is >)
+    and one ulp below (kept).  Wherever the exact path decided, the plane and the weight are the oracle's bits.  And the largest
+    fast-vs-QR deviation of the normal stays well inside the fit-error bound rho the guard band is built on."""
+    rng = np.random.default_rng(11)
+    n = 1_000_000
+    m, s = random_patches(rng, n)
+    ok_o, pl_o, w_o, nv_o = oracle.fit_gate(m, s, 1e30, -np.inf)          # every gate open: the oracle's own normal and weight
+    dmax = oracle_gate_max_dist(nv_o, m)
+    paths = np.zeros(3, np.int64)
+    worst = 0.0
+
+    def check(sel, thr, wg, what):
+        nonlocal worst
+        mm, ss = m[sel], s[sel]
+        ok_q, pl_q, w_q, _ = oracle.fit_gate(mm, ss, thr, wg)
+        ok_d, path, pl_d, w_d, nv_f, fast, rho = fit_gate_device(dm, mm, ss, thr, wg)
+        bad = np.nonzero(ok_d != ok_q)[0]
+        assert len(bad) == 0, (what, len(bad), bad[:5], path[bad[:5]])
+        ex = (path != 0) & (ok_d == 1)
+        assert pl_d[ex].tobytes() == pl_q[ex].tobytes() and w_d[ex].tobytes() == w_q[ex].tobytes(), what
+        np.add.at(paths, path, 1)
+        if fast.any():
+            dev = np.linalg.norm(nv_f[fast] - nv_o[sel][fast], axis=1) / np.linalg.norm(nv_o[sel][fast], axis=1)
+            worst = max(worst, float(np.max(dev / rho[fast])))
+        return ok_d
+
+    all_ = np.arange(n)
+    ok_def = check(all_, 0.06, 0.4, "defaults")
+    check(all_, 0.2, 0.1, "0.2 / 0.1")
+    assert 0.05 * n < ok_def.sum() < 0.99 * n
+    k = 200_000
+    sub = all_[:k]
+    sub = sub[np.isfinite(dmax[sub]) & (dmax[sub] > 0)]                  # (a distance of 0 has no float below it)
+    d = dmax[sub]
+    for thr, want in ((d, 1), (np.nextafter(d, 0.0), 0), (np.nextafter(d, np.inf), 1)):
+        got = check(sub, thr, -np.inf, "plane_thres on the oracle's distance")
+        assert (got == want).all()
+    wsub = sub[np.isfinite(w_o[sub])]
+    wq = w_o[wsub].astype(np.float64)
+    assert check(wsub, 1e30, wq, "w_gate == w").sum() == 0
+    assert (check(wsub, 1e30, np.nextafter(wq, -np.inf), "w_gate one ulp below w") == 1).all()
+    # every path ran; the guard band sent the on-threshold cases to the exact path, and the measured deviation is well inside rho
+    assert paths[0] > n // 2 and paths[1] > 1000 and paths[2] > k, paths
+    assert worst < 0.05, worst
+
+
+def test_fast_normal_alone_misdecides_on_threshold_sets(dm, oracle):
+    """Why the guard band exists (not a test of it): the fast fit's normal, gated without a margin, decides a large share of
+    neighbourhoods put exactly on the plane threshold differently from the oracle's QR normal.  The test above shows that
+    plane_fit_gate, which refits such sets on the exact path, decides every one of them as the oracle does."""
+    rng = np.random.default_rng(12)
+    m, s = random_patches(rng, 4000)
+    _, _, _, nv_o = oracle.fit_gate(m, s, 1e30, -np.inf)
+    d = oracle_gate_max_dist(nv_o, m)
+    _, _, _, _, nv_f, fast, _ = fit_gate_device(dm, m, s, 1e30, -np.inf)
+    d_f = oracle_gate_max_dist(nv_f, m)
+    keep = fast & np.isfinite(d)
+    flips = int(np.sum(d_f[keep] > d[keep])) + int(np.sum(d_f[keep] <= np.nextafter(d[keep], 0.0)))
+    assert flips > 100, flips
 
 
 def _qrot_np(q, v):
