@@ -592,6 +592,31 @@ int liliom_extract_resident_batch(liliom_ctx* const* ctxs, int B, const double* 
  * contexts on different devices, a context with a communicator.
  * For a single session the solo call is faster (no event joins). */
 int liliom_map_update_batch(liliom_ctx* const* ctxs, int B, const double* poses7, int* n_map, int* status);
+/* liliom_backend_window_correspond of B independent sessions in one call.  bps: B structs.  kf_ids, poses7_lidar, n_edge_corr,
+ * n_surf_corr: B per-session pointers; k, status: B ints.  Session i gets exactly what
+ * liliom_backend_window_correspond(ctxs[i], &bps[i], kf_ids[i], poses7_lidar[i], k[i], n_edge_corr[i], n_surf_corr[i]) would give
+ * it, bit for bit: status, counts (zeroed up to an unknown id, as the solo call writes them), liliom_last_error, launches, and the
+ * window left resident in ctxs[i], so that solo and batched window calls mix freely (liliom_backend_window_blocks,
+ * liliom_backend_window_corr, liliom_backend_window_blocks_batch).  A session that has no new keyframe is simply left out of ctxs.
+ * Horizon (48-byte, variant 0) and ROT (32-byte, variant 1) sessions may be mixed, with their own k (1..16) and parameters.
+ * A session's own error (every error its solo call returns, a NULL per-session pointer included) is its status; the others run.
+ * The edge searches of every session run in one launch per 32 sessions (k_backend_edge_batch), the surf searches likewise
+ * (k_backend_surf_batch), the counts in one more (k_win_count_batch), all on ctxs[0]'s stream (other sessions' streams are
+ * joined with events); a session without edge (surf) queries takes part in no edge (surf) launch, as in its solo call.  The call
+ * waits once for all sessions, where B solo calls wait B times.
+ * LILIOM_E_ARG for the whole call, nothing changed: B < 1, a NULL array (ctxs, bps, kf_ids, poses7_lidar, k, n_edge_corr,
+ * n_surf_corr, status), a NULL or repeated context, contexts on different devices, a context with a communicator. */
+int liliom_backend_window_correspond_batch(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps,
+                                           const int* const* kf_ids, const double* const* poses7_lidar, const int* k,
+                                           int* const* n_edge_corr, int* const* n_surf_corr, int* status);
+/* liliom_backend_window_blocks of B independent sessions in one call.  poses7_body, out29: B per-session pointers (7 k[i] and
+ * 2 k[i] 29 doubles); k, status: B ints.  Session i gets exactly what liliom_backend_window_blocks(ctxs[i], poses7_body[i], k[i],
+ * out29[i]) would give it, bit for bit (same partition, same fixed-order sums), with status, liliom_last_error and launches as
+ * that call's.  A session whose LM has stopped is simply left out of ctxs.  The segments of up to 32 sessions share one
+ * k_backend_block_batch launch and one k_backend_block_sum launch on ctxs[0]'s stream, and the call reads the blocks of every
+ * session back with one wait.  Per-session errors and whole-call refusals as liliom_backend_window_correspond_batch. */
+int liliom_backend_window_blocks_batch(liliom_ctx* const* ctxs, int B, const double* const* poses7_body, const int* k,
+                                       double* const* out29, int* status);
 
 #ifdef __cplusplus
 }

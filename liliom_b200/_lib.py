@@ -81,6 +81,7 @@ EXPORTS = [
     "liliom_scan_to_map_resident_batch_ex", "liliom_odometry_resident_batch_ex",
     "liliom_extract_resident_batch", "liliom_features_download",
     "liliom_map_update_resident", "liliom_map_update_batch",
+    "liliom_backend_window_correspond_batch", "liliom_backend_window_blocks_batch",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -222,6 +223,9 @@ def lib() -> C.CDLL:
     L.liliom_backend_window_correspond.argtypes = [vp, bpp, ip, dp, C.c_int, ip, ip]
     L.liliom_backend_window_blocks.argtypes = [vp, dp, C.c_int, dp]
     L.liliom_backend_window_corr.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, ip]
+    L.liliom_backend_window_correspond_batch.argtypes = [C.POINTER(vp), C.c_int, bpp, C.POINTER(ip), C.POINTER(dp), ip, C.POINTER(ip),
+                                                         C.POINTER(ip), ip]
+    L.liliom_backend_window_blocks_batch.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(dp), ip, C.POINTER(dp), ip]
     L.liliom_kf_cloud.argtypes = [vp, ip, dp, C.c_int, C.c_float, vp, C.c_int, ip]
     L.liliom_kf_add_full.argtypes = [vp, bpp, C.c_int, vp, C.c_int, ip]
     L.liliom_global_map.argtypes = [vp, C.c_int, ip, dp, C.c_int, dp, C.c_float, vp, C.c_int, ip]
@@ -913,6 +917,56 @@ def map_update_batch(ctxs, poses7):
     if rc != OK:
         raise LiliomError(rc)
     return n_map[:B], status[:B]
+
+
+def _handles(ctxs):
+    return (C.c_void_p * max(len(ctxs), 1))(*[c._h if c is not None else None for c in ctxs])
+
+
+def _ptrs(arrays, ctype):
+    """A C array of per-session pointers; a None entry is a NULL pointer."""
+    P = C.POINTER(ctype)
+    return (P * max(len(arrays), 1))(*[a.ctypes.data_as(P) if a is not None else P() for a in arrays])
+
+
+def backend_window_correspond_batch(ctxs, bps, kf_ids, poses7_lidar):
+    """backend_window_correspond of every context in `ctxs` in one call (liliom_backend_window_correspond_batch): session i gets
+    what ctxs[i].backend_window_correspond(bps[i], kf_ids[i], poses7_lidar[i]) would give it, and keeps its window resident.
+    bps: B BackendParams; kf_ids, poses7_lidar: B sequences (a None entry passes a NULL pointer).  Returns (per-session
+    (n_edge_corr, n_surf_corr) arrays, status (B,)); a session's own error is its status, a whole-call error raises LiliomError."""
+    B = len(ctxs)
+    if len(bps) != B or len(kf_ids) != B or len(poses7_lidar) != B:
+        raise ValueError(f"expected {B} per-session parameters, id lists and pose lists")
+    bparr = (BackendParams * max(B, 1))(*bps)
+    ids = [_ids(x) if x is not None else None for x in kf_ids]
+    k = np.array([len(x) if x is not None else 1 for x in ids] + [0], np.int32)
+    poses = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1) if p is not None else None for p in poses7_lidar]
+    ne = [np.zeros(max(int(k[i]), 1), np.int32) for i in range(B)]
+    ns = [np.zeros(max(int(k[i]), 1), np.int32) for i in range(B)]
+    status = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_backend_window_correspond_batch(_handles(ctxs), B, bparr, _ptrs(ids, C.c_int), _ptrs(poses, C.c_double), _ip(k),
+                                                      _ptrs(ne, C.c_int), _ptrs(ns, C.c_int), _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    return [(ne[i][:k[i]], ns[i][:k[i]]) for i in range(B)], status[:B]
+
+
+def backend_window_blocks_batch(ctxs, poses7_body):
+    """backend_window_blocks of every context in `ctxs` in one call (liliom_backend_window_blocks_batch): session i gets what
+    ctxs[i].backend_window_blocks(poses7_body[i]) would give it.  poses7_body: B sequences of k_i poses.  Returns (per-session
+    (k_i, 2, 29) arrays, status (B,)); a session's own error is its status, a whole-call error raises LiliomError."""
+    B = len(ctxs)
+    if len(poses7_body) != B:
+        raise ValueError(f"expected {B} per-session pose lists")
+    poses = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1, 7) if p is not None else None for p in poses7_body]
+    k = np.array([len(p) if p is not None else 1 for p in poses] + [0], np.int32)
+    out = [np.zeros((max(int(k[i]), 1), 2, 29)) for i in range(B)]
+    status = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_backend_window_blocks_batch(_handles(ctxs), B, _ptrs(poses, C.c_double), _ip(k), _ptrs(out, C.c_double),
+                                                  _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    return [out[i][:k[i]] for i in range(B)], status[:B]
 
 
 def comm_get_unique_id() -> bytes:

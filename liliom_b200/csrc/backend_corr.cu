@@ -10,6 +10,7 @@
 #include "dev_math.cuh"
 #include "knn_core.cuh"
 #include "bk_window.h"
+#include "bk_batch.h"
 
 namespace lili {
 
@@ -26,21 +27,37 @@ struct BkArgs {
     const float* map_refl; double reflect_thres;   // Horizon backend variant (L:1617-1638; query reflectivity = 48-byte field 9), nullptr = ROT variant
 };
 
-// the query's body-frame point and its keyframe's pose
-__device__ __forceinline__ const unsigned char* bk_query(const BkArgs& a, long long qi, Q4& q, D3& t) {
+// The keyframe table of one session's search in a batched call (liliom_backend_window_correspond_batch): the members of its solo
+// BkArgs that describe the queries.  Every session's tables sit in one device buffer; the session's BkSess entry points at its own.
+struct BkTable {
+    const unsigned char* qpts; int qstride;
+    int k; long long start[kWinMax + 1]; long long qoff[kWinMax]; Q4 q[kWinMax]; D3 t[kWinMax];
+};
+// A session's entry in a batched search launch: the rest of its solo BkArgs, n = its query count, kt = its keyframe table.
+struct BkSess {
+    const BkTable* kt; long long n;
+    const float4* map; const float4* map_orig; const int* cell_start; GridDesc g;
+    int variant;
+    double max_sqd, plane_thres, w_gate, lidar_const;
+    float tau0;
+    unsigned char* valid; float* pa; float* pb; float4* plane; double* score;
+    const float* map_refl; double reflect_thres;
+};
+
+// the query's body-frame point and its keyframe's pose (T: a BkArgs or a BkTable)
+template <class T>
+__device__ __forceinline__ const unsigned char* bk_query(const T& a, long long qi, Q4& q, D3& t) {
     const int j = bkw_find(a.start, a.k, qi);
     q = a.q[j]; t = a.t[j];
     return a.qpts + (size_t)(a.qoff[j] + (qi - a.start[j])) * a.qstride;
 }
 
-__global__ void __launch_bounds__(kBlock) k_backend_edge(const __grid_constant__ BkArgs a) {
-    const int lane = threadIdx.x & 31;
-    const int sub = lane & (kLanes - 1), oct = lane / kLanes;
-    const unsigned omask = ((1u << kLanes) - 1u) << (oct * kLanes);
-    const long long qi = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / kLanes;
-    if (qi >= a.start[a.k]) return;   // uniform per octet
-    Q4 q; D3 t;
-    const float4 f = *reinterpret_cast<const float4*>(bk_query(a, qi, q, t));
+// The octet's search and line fit of edge query qi at its body-frame point qp and keyframe pose (q, t), the solo and the batched
+// kernel's one body (Args: a BkArgs or a BkSess, whose members carry the same names).
+template <class Args>
+__device__ __forceinline__ void bk_edge_query(const Args& a, long long qi, const unsigned char* qp, const Q4& q, const D3& t, int sub,
+                                              unsigned omask) {
+    const float4 f = *reinterpret_cast<const float4*>(qp);
     const VgXyz pw = pcl_transform_xyz(q, t, f.x, f.y, f.z);
     const float sx = pw.x, sy = pw.y, sz = pw.z;
     Top5 top;
@@ -90,14 +107,10 @@ __global__ void __launch_bounds__(kBlock) k_backend_edge(const __grid_constant__
     for (int k = 0; k < 3; ++k) { a.pa[3 * (size_t)qi + k] = A3[k]; a.pb[3 * (size_t)qi + k] = B3[k]; }
 }
 
-__global__ void __launch_bounds__(kBlock) k_backend_surf(const __grid_constant__ BkArgs a) {
-    const int lane = threadIdx.x & 31;
-    const int sub = lane & (kLanes - 1), oct = lane / kLanes;
-    const unsigned omask = ((1u << kLanes) - 1u) << (oct * kLanes);
-    const long long qi = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / kLanes;
-    if (qi >= a.start[a.k]) return;
-    Q4 q; D3 t;
-    const unsigned char* qp = bk_query(a, qi, q, t);
+// The octet's search and plane fit of surf query qi (as bk_edge_query).
+template <class Args>
+__device__ __forceinline__ void bk_surf_query(const Args& a, long long qi, const unsigned char* qp, const Q4& q, const D3& t, int sub,
+                                              unsigned omask) {
     const float4 f = *reinterpret_cast<const float4*>(qp);
     const VgXyz pw = pcl_transform_xyz(q, t, f.x, f.y, f.z);
     const float sx = pw.x, sy = pw.y, sz = pw.z;
@@ -145,10 +158,60 @@ __global__ void __launch_bounds__(kBlock) k_backend_surf(const __grid_constant__
     a.score[qi] = sc;
 }
 
+// One octet (kLanes threads) per query of the concatenated table.
+__global__ void __launch_bounds__(kBlock) k_backend_edge(const __grid_constant__ BkArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int sub = lane & (kLanes - 1), oct = lane / kLanes;
+    const unsigned omask = ((1u << kLanes) - 1u) << (oct * kLanes);
+    const long long qi = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / kLanes;
+    if (qi >= a.start[a.k]) return;   // uniform per octet
+    Q4 q; D3 t;
+    const unsigned char* qp = bk_query(a, qi, q, t);
+    bk_edge_query(a, qi, qp, q, t, sub, omask);
+}
+
+__global__ void __launch_bounds__(kBlock) k_backend_surf(const __grid_constant__ BkArgs a) {
+    const int lane = threadIdx.x & 31;
+    const int sub = lane & (kLanes - 1), oct = lane / kLanes;
+    const unsigned omask = ((1u << kLanes) - 1u) << (oct * kLanes);
+    const long long qi = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / kLanes;
+    if (qi >= a.start[a.k]) return;
+    Q4 q; D3 t;
+    const unsigned char* qp = bk_query(a, qi, q, t);
+    bk_surf_query(a, qi, qp, q, t, sub, omask);
+}
+
+// The batched searches: session s owns blocks [off[s], off[s + 1]) and maps its queries onto them as its solo launch does.
+__global__ void __launch_bounds__(kBlock) k_backend_edge_batch(const __grid_constant__ BatchTab<BkSess> tab) {
+    const BatchSlot at = batch_slot(tab);
+    const BkSess& a = tab.s[at.s];
+    const int lane = threadIdx.x & 31;
+    const int sub = lane & (kLanes - 1), oct = lane / kLanes;
+    const unsigned omask = ((1u << kLanes) - 1u) << (oct * kLanes);
+    const long long qi = ((long long)at.blk.bi() * blockDim.x + threadIdx.x) / kLanes;
+    if (qi >= a.n) return;            // uniform per octet
+    Q4 q; D3 t;
+    const unsigned char* qp = bk_query(*a.kt, qi, q, t);
+    bk_edge_query(a, qi, qp, q, t, sub, omask);
+}
+
+__global__ void __launch_bounds__(kBlock) k_backend_surf_batch(const __grid_constant__ BatchTab<BkSess> tab) {
+    const BatchSlot at = batch_slot(tab);
+    const BkSess& a = tab.s[at.s];
+    const int lane = threadIdx.x & 31;
+    const int sub = lane & (kLanes - 1), oct = lane / kLanes;
+    const unsigned omask = ((1u << kLanes) - 1u) << (oct * kLanes);
+    const long long qi = ((long long)at.blk.bi() * blockDim.x + threadIdx.x) / kLanes;
+    if (qi >= a.n) return;
+    Q4 q; D3 t;
+    const unsigned char* qp = bk_query(*a.kt, qi, q, t);
+    bk_surf_query(a, qi, qp, q, t, sub, omask);
+}
+
 // correspondences found per keyframe (vec_edge_res_cnt / vec_surf_res_cnt): blockIdx.x = keyframe, blockIdx.y = kind
 struct CntArgs { const unsigned char* valid[2]; long long start[2][kWinMax + 1]; int* cnt; };   // cnt[kind * kWinMax + keyframe]
-__global__ void k_win_count(const __grid_constant__ CntArgs a) {
-    const int j = blockIdx.x, kind = blockIdx.y;
+// keyframe j, kind `kind`: the count into a.cnt and, when `copy` is set, into copy (the batched call's read-back)
+__device__ __forceinline__ void win_count_body(const CntArgs& a, int j, int kind, int* copy) {
     int s = 0;
     for (long long i = a.start[kind][j] + threadIdx.x; i < a.start[kind][j + 1]; i += blockDim.x) s += a.valid[kind][i];
 #pragma unroll
@@ -160,7 +223,17 @@ __global__ void k_win_count(const __grid_constant__ CntArgs a) {
         int v = 0;
         for (int w = 0; w < (int)(blockDim.x >> 5); ++w) v += red[w];
         a.cnt[kind * kWinMax + j] = v;
+        if (copy) copy[kind * kWinMax + j] = v;
     }
+}
+__global__ void k_win_count(const __grid_constant__ CntArgs a) {
+    win_count_body(a, blockIdx.x, blockIdx.y, nullptr);
+}
+// The batched count: session s owns blocks [off[s], off[s + 1]) of blockIdx.x, one per keyframe; its counts also go to `copy`.
+struct CntSess { CntArgs a; int* copy; };
+__global__ void k_win_count_batch(const __grid_constant__ BatchTab<CntSess> tab) {
+    const BatchSlot at = batch_slot(tab);
+    win_count_body(tab.s[at.s].a, at.blk.bi(), blockIdx.y, tab.s[at.s].copy);
 }
 
 static int search_launch(liliom_ctx* c, bool edge, const BkArgs& a) {
@@ -220,9 +293,10 @@ struct BlkCommon { Q4 qlb_inv; D3 tlb; double cauchy_b; double* partials; };   /
 constexpr int kBlkThreads = 256;
 constexpr int kMaxBlk = 64;
 
-__global__ void __launch_bounds__(kBlkThreads) k_backend_block(const BlkSeg* __restrict__ segs, BlkCommon a) {
+// Block blockIdx.x of segment blockIdx.y: its share of the segment's rows into its partial.  a.partials is not read: the partials
+// go to `partials` (the solo and the batched kernel's one body).
+__device__ __forceinline__ void block_body(const BlkSeg& s, const BlkCommon& a, double* __restrict__ partials) {
     __shared__ double red[kBlkThreads / 32][kNormEq];
-    const BlkSeg& s = segs[blockIdx.y];
     const int nblocks = s.nblocks;
     if ((int)blockIdx.x >= nblocks) return;        // uniform per block
     double acc[kNormEq];
@@ -277,7 +351,17 @@ __global__ void __launch_bounds__(kBlkThreads) k_backend_block(const BlkSeg* __r
         add_row29(acc, R);
     }
     const double v = block_sum29(acc, red, kBlkThreads / 32);
-    if (threadIdx.x < kNormEq) a.partials[((size_t)blockIdx.y * kMaxBlk + blockIdx.x) * kNormEq + threadIdx.x] = v;
+    if (threadIdx.x < kNormEq) partials[((size_t)blockIdx.y * kMaxBlk + blockIdx.x) * kNormEq + threadIdx.x] = v;
+}
+
+__global__ void __launch_bounds__(kBlkThreads) k_backend_block(const BlkSeg* __restrict__ segs, BlkCommon a) {
+    block_body(segs[blockIdx.y], a, a.partials);
+}
+
+// The batched blocks: the segments of several sessions, each with its session's extrinsics and loss in com[segment].
+__global__ void __launch_bounds__(kBlkThreads) k_backend_block_batch(const BlkSeg* __restrict__ segs, const BlkCommon* __restrict__ com,
+                                                                     double* __restrict__ partials) {
+    block_body(segs[blockIdx.y], com[blockIdx.y], partials);
 }
 
 // fixed-order sum over each segment's block partials (run-to-run deterministic): blockIdx.x = segment
@@ -437,8 +521,24 @@ extern "C" int liliom_backend_surf_block(liliom_ctx* c, const double pose7_body[
 }
 
 // ===================== SURVEY §8 (f5): the window's LiDAR rows against the device-resident local map =====================
-extern "C" int liliom_backend_window_correspond(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7_lidar,
-                                                int k, int* n_edge_corr, int* n_surf_corr) {
+namespace lili {
+
+// One session's liliom_backend_window_correspond: its arguments, and the search and count tables win_begin fills.
+struct WinJob {
+    liliom_ctx* c;
+    const liliom_backend_params* bp;
+    const int* ids;
+    int k;
+    int* ne; int* ns;
+    BkArgs ae, as;
+    CntArgs ca;
+};
+
+// The call up to its launches, shared by the solo and the batched call so that their checks, their order and their partial writes
+// are one: the arguments, the counts zeroed up to an unknown id, the resident window dropped (c->win_k = 0), the map gates, the
+// buffers, and both search tables and the count table in j.  An error before c->win_k = 0 leaves the previous window resident.
+static int win_begin(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7_lidar, int k,
+                     int* n_edge_corr, int* n_surf_corr, WinJob& j) {
     if (!c || !bp || !kf_ids || !poses7_lidar || !n_edge_corr || !n_surf_corr || k < 1 || k > kWinMax) return LILIOM_E_ARG;
     if (c->nranks > 1 || (bp->variant != 0 && bp->variant != 1) || !(bp->kd_max_radius > 0) || !(bp->cauchy_b > 0)) return LILIOM_E_ARG;
     for (int i = 0; i < k; ++i) {
@@ -460,8 +560,11 @@ extern "C" int liliom_backend_window_correspond(liliom_ctx* c, const liliom_back
         }
     }
     if (!(c->bmap_n[1] > 50 && c->bmap_n[0] > 0)) return LILIOM_E_FEWMAP;        // L:933
+    j.c = c; j.bp = bp; j.ids = kf_ids; j.k = k; j.ne = n_edge_corr; j.ns = n_surf_corr;
     const int stride = c->prm.point_stride;
-    BkArgs ae{}, as{};
+    BkArgs& ae = j.ae;
+    BkArgs& as = j.as;
+    ae = BkArgs{}; as = BkArgs{};
     for (BkArgs* a : {&ae, &as}) {
         a->qpts = (const unsigned char*)c->kf_arena.p; a->qstride = stride; a->k = k; a->start[0] = 0;
     }
@@ -484,7 +587,6 @@ extern "C" int liliom_backend_window_correspond(liliom_ctx* c, const liliom_back
     ae.variant = bp->variant;
     ae.tau0 = knn_gate_tau(1.0);
     ae.valid = c->win_valid[0].as<unsigned char>(); ae.pa = c->win_line.as<float>(); ae.pb = ae.pa + 3 * (size_t)Qe;
-    LILI_TRY(search_launch(c, true, ae));
     // surf: L:1601-1681 / R:1464-1520 against surf_local_map_ds
     bk_set_map(as, c->bmap[1]);
     as.variant = bp->variant;
@@ -492,24 +594,48 @@ extern "C" int liliom_backend_window_correspond(liliom_ctx* c, const liliom_back
     as.max_sqd = bp->kd_max_radius; as.plane_thres = bp->surf_dist_thres; as.w_gate = bp->w_gate; as.lidar_const = bp->lidar_const;
     if (bp->variant == 0) { as.map_refl = c->bmap[1].refl.as<float>(); as.reflect_thres = bp->reflect_thres; }
     as.valid = c->win_valid[1].as<unsigned char>(); as.plane = c->win_plane.as<float4>(); as.score = c->win_score.as<double>();
-    LILI_TRY(search_launch(c, false, as));
-    CntArgs ca{};
+    CntArgs& ca = j.ca;
+    ca = CntArgs{};
     ca.valid[0] = ae.valid; ca.valid[1] = as.valid; ca.cnt = c->win_cnt.as<int>();
     for (int i = 0; i <= k; ++i) { ca.start[0][i] = ae.start[i]; ca.start[1][i] = as.start[i]; }
-    k_win_count<<<dim3(k, 2), 256, 0, c->stream>>>(ca);
-    LILI_TRY(launch_check(c, "k_win_count"));
-    int cnt[2 * kWinMax];
-    LILI_TRY(read_back(c, {{cnt, c->win_cnt.p, sizeof(cnt)}}));
-    for (int i = 0; i < k; ++i) { n_edge_corr[i] = cnt[i]; n_surf_corr[i] = cnt[kWinMax + i]; }
-    c->win_ids.assign(kf_ids, kf_ids + k);
-    c->win_qoff[0].assign(ae.start, ae.start + k + 1);
-    c->win_qoff[1].assign(as.start, as.start + k + 1);
-    c->win_bp = *bp;
-    c->win_k = k;
     return LILIOM_OK;
 }
 
-extern "C" int liliom_backend_window_blocks(liliom_ctx* c, const double* poses7_body, int k, double* out29) {
+// The call after its read-back: cnt[kind * kWinMax + i] out to the caller, the window resident.
+static void win_end(const WinJob& j, const int* cnt) {
+    liliom_ctx* c = j.c;
+    for (int i = 0; i < j.k; ++i) { j.ne[i] = cnt[i]; j.ns[i] = cnt[kWinMax + i]; }
+    c->win_ids.assign(j.ids, j.ids + j.k);
+    c->win_qoff[0].assign(j.ae.start, j.ae.start + j.k + 1);
+    c->win_qoff[1].assign(j.as.start, j.as.start + j.k + 1);
+    c->win_bp = *j.bp;
+    c->win_k = j.k;
+}
+
+// A session's entry in a batched search: its solo table a, whose keyframe part sits at kt on the device.
+static BkSess bk_sess(const BkArgs& a, const BkTable* kt) {
+    BkSess e{};
+    e.kt = kt; e.n = a.start[a.k];
+    e.map = a.map; e.map_orig = a.map_orig; e.cell_start = a.cell_start; e.g = a.g;
+    e.variant = a.variant;
+    e.max_sqd = a.max_sqd; e.plane_thres = a.plane_thres; e.w_gate = a.w_gate; e.lidar_const = a.lidar_const;
+    e.tau0 = a.tau0;
+    e.valid = a.valid; e.pa = a.pa; e.pb = a.pb; e.plane = a.plane; e.score = a.score;
+    e.map_refl = a.map_refl; e.reflect_thres = a.reflect_thres;
+    return e;
+}
+
+static BkTable bk_table(const BkArgs& a) {
+    BkTable t{};
+    t.qpts = a.qpts; t.qstride = a.qstride; t.k = a.k;
+    for (int i = 0; i <= a.k; ++i) t.start[i] = a.start[i];
+    for (int i = 0; i < a.k; ++i) { t.qoff[i] = a.qoff[i]; t.q[i] = a.q[i]; t.t[i] = a.t[i]; }
+    return t;
+}
+
+// One session's liliom_backend_window_blocks up to its launches (shared by the solo and the batched call): the arguments, then its
+// 2 k segments (bkb_segment's order) and its extrinsics and loss.
+static int blocks_begin(liliom_ctx* c, const double* poses7_body, int k, double* out29, std::vector<BlkSeg>& segs, BlkCommon& a) {
     if (!c || !poses7_body || !out29 || k < 1) return LILIOM_E_ARG;
     if (k != c->win_k) {
         c->last_error = "liliom_backend_window_blocks needs the k of the window left resident by liliom_backend_window_correspond";
@@ -519,7 +645,7 @@ extern "C" int liliom_backend_window_blocks(liliom_ctx* c, const double* poses7_
     const liliom_backend_params& bp = c->win_bp;
     const int stride = c->prm.point_stride;
     const long long Qe = c->win_qoff[0][k];
-    std::vector<BlkSeg> segs((size_t)2 * k);
+    segs.assign((size_t)2 * k, BlkSeg{});
     for (int i = 0; i < k; ++i) {
         const KfEntry& f = c->kfs[c->win_ids[i]];
         const double* p = poses7_body + 7 * (size_t)i;
@@ -540,11 +666,166 @@ extern "C" int liliom_backend_window_blocks(liliom_ctx* c, const double* poses7_
             s.lidar_const = bp.lidar_const;
         }
     }
-    BlkCommon a{};
+    a = BlkCommon{};
     a.qlb_inv = q_inverse(bp.q_lb);
     a.tlb = D3{bp.t_lb[0], bp.t_lb[1], bp.t_lb[2]};
     a.cauchy_b = bp.cauchy_b;
+    return LILIOM_OK;
+}
+
+// c0's batch buffers, grown to a call's device bytes and pinned staging bytes
+static int bk_batch_buffers(liliom_ctx* c0, size_t dev_bytes, size_t pin_bytes) {
+    LILI_CUDA(c0, c0->bk_batch_dev.ensure(dev_bytes));
+    LILI_CUDA(c0, c0->bk_batch_pin.ensure(pin_bytes));
+    return LILIOM_OK;
+}
+
+}  // namespace lili
+
+extern "C" int liliom_backend_window_correspond(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7_lidar,
+                                                int k, int* n_edge_corr, int* n_surf_corr) {
+    WinJob j;
+    LILI_TRY(win_begin(c, bp, kf_ids, poses7_lidar, k, n_edge_corr, n_surf_corr, j));
+    LILI_TRY(search_launch(c, true, j.ae));
+    LILI_TRY(search_launch(c, false, j.as));
+    k_win_count<<<dim3(k, 2), 256, 0, c->stream>>>(j.ca);
+    LILI_TRY(launch_check(c, "k_win_count"));
+    int cnt[2 * kWinMax];
+    LILI_TRY(read_back(c, {{cnt, c->win_cnt.p, sizeof(cnt)}}));
+    win_end(j, cnt);
+    return LILIOM_OK;
+}
+
+extern "C" int liliom_backend_window_blocks(liliom_ctx* c, const double* poses7_body, int k, double* out29) {
+    std::vector<BlkSeg> segs;
+    BlkCommon a;
+    LILI_TRY(blocks_begin(c, poses7_body, k, out29, segs, a));
     return backend_block_run(c, segs, a, out29);
+}
+
+// ---- several sessions in one call: the solo calls' host parts per session, every launch shared on ctxs[0]'s stream, one wait
+extern "C" int liliom_backend_window_correspond_batch(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps,
+                                                      const int* const* kf_ids, const double* const* poses7_lidar, const int* k,
+                                                      int* const* n_edge_corr, int* const* n_surf_corr, int* status) {
+    if (!batch_ctxs_ok(ctxs, B) || !bps || !kf_ids || !poses7_lidar || !k || !n_edge_corr || !n_surf_corr || !status) return LILIOM_E_ARG;
+    liliom_ctx* c0 = ctxs[0];
+    LILI_CUDA(c0, cudaSetDevice(c0->device));
+    std::vector<WinJob> J;
+    for (int i = 0; i < B; ++i) {
+        WinJob j;
+        status[i] = win_begin(ctxs[i], &bps[i], kf_ids[i], poses7_lidar[i], k[i], n_edge_corr[i], n_surf_corr[i], j);
+        if (status[i] == LILIOM_OK) J.push_back(j);
+    }
+    if (J.empty()) return LILIOM_OK;
+    const int n = (int)J.size();
+    // pinned: every session's edge and surf keyframe tables (uploaded), then its counts (read back); the device mirrors them
+    const size_t tab_bytes = bkb_region((size_t)2 * n, sizeof(BkTable)), cnt_bytes = bkb_region((size_t)n * kBkbCntInts, sizeof(int));
+    LILI_TRY(bk_batch_buffers(c0, tab_bytes + cnt_bytes, tab_bytes + cnt_bytes));
+    BkTable* h_tab = c0->bk_batch_pin.as<BkTable>();
+    const BkTable* d_tab = c0->bk_batch_dev.as<BkTable>();
+    int* d_cnt = reinterpret_cast<int*>(c0->bk_batch_dev.as<unsigned char>() + tab_bytes);
+    std::vector<liliom_ctx*> live;
+    for (int m = 0; m < n; ++m) {
+        h_tab[2 * m] = bk_table(J[m].ae);
+        h_tab[2 * m + 1] = bk_table(J[m].as);
+        live.push_back(J[m].c);
+    }
+    LILI_TRY(batch_join_in(c0, live));
+    LILI_CUDA(c0, cudaMemcpyAsync(c0->bk_batch_dev.p, h_tab, (size_t)2 * n * sizeof(BkTable), cudaMemcpyHostToDevice, c0->stream));
+    // the searches: a session without queries of a kind takes part in no launch of that kind, as in its solo call
+    for (int kind = 0; kind < 2; ++kind) {
+        std::vector<int> which;
+        for (int m = 0; m < n; ++m) if ((kind == 0 ? J[m].ae : J[m].as).start[J[m].k] > 0) which.push_back(m);
+        LILI_TRY(batch_tables<BatchTab<BkSess>>(
+            which,
+            [&](BkSess& e, int m) {
+                e = bk_sess(kind == 0 ? J[m].ae : J[m].as, d_tab + 2 * m + kind);
+                return BatchPart{J[m].c, cdiv(e.n * kLanes, kBlock)};
+            },
+            [&](const BatchTab<BkSess>& tab, int grid) -> int {
+                if (kind == 0) k_backend_edge_batch<<<grid, kBlock, 0, c0->stream>>>(tab);
+                else k_backend_surf_batch<<<grid, kBlock, 0, c0->stream>>>(tab);
+                LILI_CUDA(c0, cudaGetLastError());
+                return LILIOM_OK;
+            }));
+    }
+    std::vector<int> all(n);
+    for (int m = 0; m < n; ++m) all[m] = m;
+    LILI_TRY(batch_tables<BatchTab<CntSess>>(
+        all,
+        [&](CntSess& e, int m) {
+            e = CntSess{J[m].ca, d_cnt + (size_t)m * kBkbCntInts};
+            return BatchPart{J[m].c, J[m].k};
+        },
+        [&](const BatchTab<CntSess>& tab, int grid) -> int {
+            k_win_count_batch<<<dim3(grid, 2), 256, 0, c0->stream>>>(tab);
+            LILI_CUDA(c0, cudaGetLastError());
+            return LILIOM_OK;
+        }));
+    int* h_cnt = c0->bk_batch_pin.as<int>(tab_bytes);
+    LILI_CUDA(c0, cudaMemcpyAsync(h_cnt, d_cnt, (size_t)n * kBkbCntInts * sizeof(int), cudaMemcpyDeviceToHost, c0->stream));
+    LILI_TRY(batch_join_out(c0, live));
+    LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+    for (int m = 0; m < n; ++m) win_end(J[m], h_cnt + (size_t)m * kBkbCntInts);
+    return LILIOM_OK;
+}
+
+extern "C" int liliom_backend_window_blocks_batch(liliom_ctx* const* ctxs, int B, const double* const* poses7_body, const int* k,
+                                                  double* const* out29, int* status) {
+    if (!batch_ctxs_ok(ctxs, B) || !poses7_body || !k || !out29 || !status) return LILIOM_E_ARG;
+    liliom_ctx* c0 = ctxs[0];
+    LILI_CUDA(c0, cudaSetDevice(c0->device));
+    std::vector<liliom_ctx*> live;
+    std::vector<double*> outs;
+    std::vector<std::vector<BlkSeg>> segs;
+    std::vector<BlkCommon> coms;
+    std::vector<int> nseg;
+    for (int i = 0; i < B; ++i) {
+        std::vector<BlkSeg> s;
+        BlkCommon a;
+        status[i] = blocks_begin(ctxs[i], poses7_body[i], k[i], out29[i], s, a);
+        if (status[i] != LILIOM_OK) continue;
+        live.push_back(ctxs[i]); outs.push_back(out29[i]); nseg.push_back((int)s.size());
+        segs.push_back(std::move(s)); coms.push_back(a);
+    }
+    if (live.empty()) return LILIOM_OK;
+    const int n = (int)live.size();
+    const std::vector<int> off = bkb_offsets(nseg);
+    const int S = off[n];
+    // pinned: the segments and their sessions' extrinsics and loss (uploaded), then the 29 sums of every segment (read back);
+    // device: the same, and the block partials
+    const size_t seg_bytes = bkb_region(S, sizeof(BlkSeg)), com_bytes = bkb_region(S, sizeof(BlkCommon));
+    const size_t out_bytes = bkb_region((size_t)S * kNormEq, sizeof(double));
+    const size_t part_bytes = bkb_region((size_t)S * kMaxBlk * kNormEq, sizeof(double));
+    LILI_TRY(bk_batch_buffers(c0, seg_bytes + com_bytes + out_bytes + part_bytes, seg_bytes + com_bytes + out_bytes));
+    unsigned char* h = c0->bk_batch_pin.as<unsigned char>();
+    unsigned char* d = c0->bk_batch_dev.as<unsigned char>();
+    BlkSeg* h_seg = reinterpret_cast<BlkSeg*>(h);
+    BlkCommon* h_com = reinterpret_cast<BlkCommon*>(h + seg_bytes);
+    for (int m = 0; m < n; ++m)
+        for (int j = 0; j < nseg[m]; ++j) { h_seg[off[m] + j] = segs[m][j]; h_com[off[m] + j] = coms[m]; }
+    const BlkSeg* d_seg = reinterpret_cast<const BlkSeg*>(d);
+    const BlkCommon* d_com = reinterpret_cast<const BlkCommon*>(d + seg_bytes);
+    double* d_out = reinterpret_cast<double*>(d + seg_bytes + com_bytes);
+    double* d_part = reinterpret_cast<double*>(d + seg_bytes + com_bytes + out_bytes);
+    LILI_TRY(batch_join_in(c0, live));
+    LILI_CUDA(c0, cudaMemcpyAsync(d, h, seg_bytes + com_bytes, cudaMemcpyHostToDevice, c0->stream));
+    for (const BkbLaunch& L : bkb_launches(off)) {
+        int gx = 1;
+        for (int j = L.item0; j < L.item0 + L.items; ++j) gx = max(gx, h_seg[j].nblocks);
+        double* part = d_part + (size_t)L.item0 * kMaxBlk * kNormEq;
+        k_backend_block_batch<<<dim3(gx, L.items), kBlkThreads, 0, c0->stream>>>(d_seg + L.item0, d_com + L.item0, part);
+        LILI_CUDA(c0, cudaGetLastError());
+        k_backend_block_sum<<<L.items, 32, 0, c0->stream>>>(d_seg + L.item0, part, d_out + (size_t)L.item0 * kNormEq);
+        LILI_CUDA(c0, cudaGetLastError());
+        for (int m = L.first; m < L.first + L.n; ++m) live[m]->cnt.launches += 2;
+    }
+    double* h_out = reinterpret_cast<double*>(h + seg_bytes + com_bytes);
+    LILI_CUDA(c0, cudaMemcpyAsync(h_out, d_out, (size_t)S * kNormEq * sizeof(double), cudaMemcpyDeviceToHost, c0->stream));
+    LILI_TRY(batch_join_out(c0, live));
+    LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+    for (int m = 0; m < n; ++m) memcpy(outs[m], h_out + (size_t)off[m] * kNormEq, (size_t)nseg[m] * kNormEq * sizeof(double));
+    return LILIOM_OK;
 }
 
 extern "C" int liliom_backend_window_corr(liliom_ctx* c, int slot, int kind, unsigned char* valid, void* a, void* b, int cap, int* n_out) {

@@ -43,6 +43,26 @@ struct DevBuf {
     template <class T> T* as() const { return reinterpret_cast<T*>(p); }
 };
 
+// One growable pinned host allocation, owned, growing as DevBuf does: the staging of a batched call's tables and results.
+struct PinBuf {
+    void*  p = nullptr;
+    size_t cap = 0;
+    PinBuf() = default;
+    PinBuf(const PinBuf&) = delete;
+    PinBuf& operator=(const PinBuf&) = delete;
+    ~PinBuf() { release(); }
+    cudaError_t ensure(size_t bytes) {
+        if (bytes <= cap) return cudaSuccess;
+        release();
+        size_t want = bytes + bytes / 4 + 256;
+        cudaError_t e = cudaHostAlloc(&p, want, cudaHostAllocDefault);
+        if (e == cudaSuccess) cap = want; else p = nullptr;
+        return e;
+    }
+    void release() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
+    template <class T> T* as(size_t byte_off = 0) const { return reinterpret_cast<T*>(static_cast<unsigned char*>(p) + byte_off); }
+};
+
 // Dense cell grid over the down-sampled map (the kd-tree's stand-in).
 struct GridDesc {
     float inv_cell;        // 1 / cell size (power of two => exact)
@@ -378,6 +398,11 @@ struct liliom_ctx {
     std::vector<int> win_ids;
     std::vector<long long> win_qoff[2];  // per kind: query prefix offsets (k + 1)
     lili::DevBuf win_valid[2], win_line, win_plane, win_score, win_cnt, win_tab;
+    // a batched backend window call whose shared launches run on this context (ctxs[0]): every session's keyframe tables or
+    // block segments, the block partials and the results on the device, and the pinned staging of the one upload and the one
+    // read-back (backend_corr.cu)
+    lili::DevBuf bk_batch_dev;
+    lili::PinBuf bk_batch_pin;
     lili::MapIndex loop;                 // loop-closure target (liliom_loop_align): its own index, so the odometry map stays
     lili::DevBuf loop_src;               // ... and its float4 source
 

@@ -1,0 +1,174 @@
+#!/usr/bin/env python
+"""The backend's sliding-window LiDAR calls of several sessions on one GPU.  Each session has its own seeded keyframe stream
+(synth.make_keyframe_sequence) stored in its own context, and a 40-keyframe local map (solo liliom_bmap_build, built once, not
+timed).  A fleet window step is, for every session, one search of a 3-keyframe window and 16 evaluations of its blocks (15 LM
+iterations and the marginalisation, as tools/backend_bench.py models them):
+  (a) B solo loops: liliom_backend_window_correspond, then 16 liliom_backend_window_blocks, per session;
+  (b) one liliom_backend_window_correspond_batch, then 16 liliom_backend_window_blocks_batch.
+Both legs call the C ABI with argument arrays built once, so that the time is the library's, not the Python wrappers'.
+The legs alternate over --rounds rounds of --steps timed steps each (after --warmup untimed ones).  Per B: the median, smallest
+and largest of the rounds' median ms per fleet window step, the waits per step (each call ends in one stream synchronise),
+and whether (a) and (b) gave byte-identical counts and blocks.  Prints the card, its power limit and maximum SM clock first.
+Reads device state only.
+usage: backend_batch_bench.py [--sessions 1 2 4 8 16 32] [--steps 20] [--warmup 3] [--rounds 5]"""
+import argparse
+import ctypes as C
+import json
+import os
+import subprocess
+import sys
+import time
+from concurrent.futures import ProcessPoolExecutor
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+NKF = 40           # keyframes in the local map
+WIN = 3            # window keyframes
+EVALS = 16         # blocks evaluations per window
+
+
+def card():
+    out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                         capture_output=True, text=True, check=True).stdout.strip().splitlines()[0]
+    name, power, clock = [x.strip() for x in out.split(",")]
+    return dict(gpu=name, power_limit=power, max_sm_clock=clock)
+
+
+def spread(v):
+    return [round(float(np.median(v)), 4), round(float(min(v)), 4), round(float(max(v)), 4)]
+
+
+def stream(seed):
+    from liliom_b200 import synth
+    return synth.make_keyframe_sequence(NKF, stride=48, seed=seed)
+
+
+def nudge(pose, k):
+    from liliom_b200 import synth
+    dq = synth.q_from_axis_angle([1, -1, 2], np.deg2rad(0.1 * k))
+    return np.concatenate([synth.qmul(pose[:4], dq), pose[4:] + 0.005 * k * np.array([1.0, -0.5, 0.25])])
+
+
+class Session:
+    def __init__(self, seq):
+        import liliom_b200 as L
+        self.bp = L.backend_default_params(0)
+        self.c = L.Context(variant=0)
+        for e, s, _ in seq:
+            self.c.kf_add(self.bp, e, s, download=False)
+        self.c.bmap_build(self.bp, list(range(NKF)), [p for _, _, p in seq])
+        self.ids = np.arange(NKF - WIN, NKF, dtype=np.int32)
+        self.poses_l = np.array([nudge(seq[i][2], 1) for i in self.ids])
+        self.bodies = [np.array([nudge(p, 2 + j) for p in self.poses_l]) for j in range(EVALS)]
+        # each leg's own results: counts, then the 16 blocks
+        self.res = {leg: (np.zeros(WIN, np.int32), np.zeros(WIN, np.int32), [np.zeros((WIN, 2, 29)) for _ in range(EVALS)]) for leg in "ab"}
+
+
+def ptr(a, t):
+    return a.ctypes.data_as(C.POINTER(t))
+
+
+class Fleet:
+    """B sessions and the C arguments of both legs, built once: the timed window holds the library's calls only."""
+
+    def __init__(self, S):
+        import liliom_b200 as L
+        self.S, self.lib, B = S, L._binding.lib(), len(S)
+        P, D = C.POINTER(C.c_int), C.POINTER(C.c_double)
+        self.handles = (C.c_void_p * B)(*[s.c._h for s in S])
+        self.bps = (L.BackendParams * B)(*[s.bp for s in S])
+        self.ids = (P * B)(*[ptr(s.ids, C.c_int) for s in S])
+        self.poses = (D * B)(*[ptr(s.poses_l, C.c_double) for s in S])
+        self.k = np.full(B, WIN, np.int32)
+        self.ne = (P * B)(*[ptr(s.res["b"][0], C.c_int) for s in S])
+        self.ns = (P * B)(*[ptr(s.res["b"][1], C.c_int) for s in S])
+        self.bodies = [(D * B)(*[ptr(s.bodies[j], C.c_double) for s in S]) for j in range(EVALS)]
+        self.outs = [(D * B)(*[ptr(s.res["b"][2][j], C.c_double) for s in S]) for j in range(EVALS)]
+        self.status = np.zeros(B, np.int32)
+
+    def leg_a(self):
+        for s in self.S:
+            ne, ns, out = s.res["a"]
+            rc = self.lib.liliom_backend_window_correspond(s.c._h, C.byref(s.bp), ptr(s.ids, C.c_int), ptr(s.poses_l, C.c_double), WIN,
+                                                           ptr(ne, C.c_int), ptr(ns, C.c_int))
+            assert rc == 0, rc
+            for j in range(EVALS):
+                rc = self.lib.liliom_backend_window_blocks(s.c._h, ptr(s.bodies[j], C.c_double), WIN, ptr(out[j], C.c_double))
+                assert rc == 0, rc
+
+    def leg_b(self):
+        B, st = len(self.S), ptr(self.status, C.c_int)
+        rc = self.lib.liliom_backend_window_correspond_batch(self.handles, B, self.bps, self.ids, self.poses, ptr(self.k, C.c_int),
+                                                             self.ne, self.ns, st)
+        assert rc == 0 and not self.status.any(), (rc, self.status)
+        for j in range(EVALS):
+            rc = self.lib.liliom_backend_window_blocks_batch(self.handles, B, self.bodies[j], ptr(self.k, C.c_int), self.outs[j], st)
+            assert rc == 0 and not self.status.any(), (rc, self.status)
+
+    def outputs(self, leg):
+        """leg's results of every session as bytes; cleared for the next step"""
+        out = b""
+        for s in self.S:
+            ne, ns, blocks = s.res[leg]
+            out += ne.tobytes() + ns.tobytes() + b"".join(o.tobytes() for o in blocks)
+            for a in [ne, ns] + blocks:
+                a.fill(0)
+        return out
+
+
+def timed(f, leg, steps):
+    """median ms of `steps` window steps of leg "a" or "b", and the outputs of the last (every call returns with its sessions'
+    work complete)"""
+    import torch
+    run = f.leg_a if leg == "a" else f.leg_b
+    lat = []
+    for _ in range(steps):
+        f.outputs(leg)
+        torch.cuda.synchronize()
+        t = time.perf_counter()
+        run()
+        lat.append((time.perf_counter() - t) * 1e3)
+    return float(np.median(lat)), f.outputs(leg)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--sessions", type=int, nargs="*", default=[1, 2, 4, 8, 16, 32])
+    ap.add_argument("--steps", type=int, default=20)
+    ap.add_argument("--warmup", type=int, default=3)
+    ap.add_argument("--rounds", type=int, default=5)
+    args = ap.parse_args()
+    Bmax = max(args.sessions)
+    with ProcessPoolExecutor(max_workers=min(Bmax, os.cpu_count() or 1)) as ex:     # the streams, before CUDA starts here
+        seqs = list(ex.map(stream, [100 + s for s in range(Bmax)]))
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("backend_batch_bench.py measures on a CUDA device; none is visible")
+    print(json.dumps(dict(card(), keyframes=NKF, window=WIN, evals=EVALS, steps=args.steps, rounds=args.rounds,
+                          figures="[median of rounds, min round, max round], ms per fleet window step")), flush=True)
+    sessions = [Session(seq) for seq in seqs]
+    for B in args.sessions:
+        S = sessions[:B]
+        f = Fleet(S)
+        for leg in "ab":
+            timed(f, leg, args.warmup)
+        ra, rb, same = [], [], True
+        for _ in range(args.rounds):
+            ta, oa = timed(f, "a", args.steps)
+            tb, ob = timed(f, "b", args.steps)
+            ra.append(ta); rb.append(tb)
+            same = same and oa == ob
+        row = dict(sessions=B, edge_map=int(np.median([s.c.bmap_download(0).size for s in S])),
+                   surf_map=int(np.median([s.c.bmap_download(1).size for s in S])),
+                   a_solo_ms=spread(ra), b_batch_ms=spread(rb), a_waits=B * (1 + EVALS), b_waits=1 + EVALS,
+                   speedup=round(float(np.median(ra) / np.median(rb)), 3), identical=bool(same))
+        print(json.dumps(row), flush=True)
+    for s in sessions:
+        s.c.close()
+
+
+if __name__ == "__main__":
+    main()
