@@ -376,16 +376,14 @@ extern "C" int liliom_voxelgrid(liliom_ctx* c, const void* pts, int n, int strid
     LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, pts, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
     bool coop = false;
     LILI_TRY(voxelgrid_coop(c, c->raw.p, n, nullptr, stride, leaf, c->vg_out.p, c->vg_count.as<int>(), nullptr, &coop));
-    int m = 0;
-    if (coop) {      // the cooperative filter may decline the input: its verdict comes back with the count
+    int m = 0, key_bits = 32;
+    if (coop) {      // the cooperative filter may decline the input: its verdict comes back with the count and the box's parameters
         VgParams vp;
         LILI_TRY(read_back(c, {{&m, c->vg_count.p, sizeof(int)}, {&vp, c->vg_params.p, sizeof(VgParams)}}));
         if (vp.bail) coop = false;
+        if (vg_wide_keys(vp)) key_bits = kVgWideKeyBits;
     }
-    if (!coop) {
-        LILI_TRY(voxelgrid_dev(c, c->raw.p, n, nullptr, stride, leaf, c->vg_out.p, c->vg_count.as<int>()));
-        LILI_TRY(read_back(c, {{&m, c->vg_count.p, sizeof(int)}}));
-    }
+    if (!coop) LILI_TRY(voxelgrid_dev_sync(c, c->raw.p, n, stride, leaf, c->vg_out.p, c->vg_count.as<int>(), nullptr, &m, key_bits));
     if (out && m > cap) return LILIOM_E_CAPACITY;
     if (out && m) {
         LILI_CUDA(c, cudaMemcpyAsync(out, c->vg_out.p, (size_t)m * stride, cudaMemcpyDeviceToHost, c->stream));
@@ -612,8 +610,9 @@ static int odo_filter(liliom_ctx* c, bool spec_failed, int* step) {
     if (c->prm.leaf_scan > 0.0f) {
         // L/src/LidarOdometry.cpp:321-322; the centroid kernel also emits the float4 queries
         // speculate that the scan's voxel box has < 2^24 cells (a 200 m sweep at 0.4 m: ~2^21-2^23): one radix pass
-        // less.  The box is read back with the pose; on a miss the step is redone with full-width keys.
-        const int key_bits = (n_max > 24576 || spec_failed) ? 32 : 24;
+        // less.  The box is read back with the pose; on a miss the step is redone with full-width keys, which are the wide ones
+        // when the box's index wraps (vg_wide_keys).
+        const int key_bits = spec_failed ? (c->vg_wide ? kVgWideKeyBits : 32) : n_max > 24576 ? 32 : 24;
         // scan-sized clouds take the single-launch cooperative filter; it may decline (VgParams::bail, read back with the pose)
         bool coop = false;
         if (!spec_failed)
@@ -622,8 +621,9 @@ static int odo_filter(liliom_ctx* c, bool spec_failed, int* step) {
             LILI_TRY(voxelgrid_dev(c, c->surf.p, n_max, d_n, stride, c->prm.leaf_scan, c->vg_out.p, c->vg_count.as<int>(), c->feats.as<float4>(), key_bits));
         c->d_nfeats = c->vg_count.as<int>();
         c->vg_used24 = !coop && key_bits < 32;
-        c->vg_check = coop || key_bits < 32;
+        c->vg_check = coop || key_bits <= 32;
         c->vg_bail = false;
+        c->vg_wide = false;
     } else {   // leaf_scan == 0: benchmark mode, every surf feature is a query
         if (n_max > 0) LILI_CUDA(c, cudaMemcpyAsync(c->vg_out.p, c->surf.p, (size_t)n_max * stride, cudaMemcpyDeviceToDevice, c->stream));
         LILI_TRY(repack_to_f4(c, c->surf.p, n_max, stride, c->feats.as<float4>(), d_n));
@@ -635,10 +635,11 @@ static int odo_filter(liliom_ctx* c, bool spec_failed, int* step) {
 }
 
 // 2. After a step that ran and returned rc: true when the VoxelGrid's speculation missed, and the call must be redone from its
-//    start pose with the sort chain and 32-bit keys (spec_failed).  Clears the check either way.
+//    start pose with the sort chain and full-width keys (spec_failed): 32-bit ones, or the wide ones when the box's index wraps.
+//    Clears the check either way.
 static bool odo_spec_missed(liliom_ctx* c, int rc, bool spec_failed) {
-    const bool miss = rc == LILIOM_OK && c->vg_check && !spec_failed &&
-                      (c->vg_bail || (c->vg_used24 && c->vg_ncells >= (1LL << 24) - 1));
+    const bool miss = rc == LILIOM_OK && c->vg_check &&
+                      ((!spec_failed && (c->vg_bail || (c->vg_used24 && c->vg_ncells >= (1LL << 24) - 1))) || c->vg_wide);
     c->vg_check = false;
     if (miss) c->d_nfeats = nullptr;
     return miss;

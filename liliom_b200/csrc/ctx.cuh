@@ -344,6 +344,7 @@ struct liliom_ctx {
     bool vg_check = false;       // s2m_run also reads vg_params back (speculative key width of the scan VoxelGrid)
     bool vg_used24 = false;      // ... the sort chain ran with 24-bit keys
     bool vg_bail = false;        // ... the cooperative filter declined (valid after the sync)
+    bool vg_wide = false;        // ... ran on keys of <= 32 bits where the index wraps: redo with wide keys (valid after the sync)
     unsigned int vg_coop_calls = 0;   // launches of k_vg_coop so far (selects the rotating control slot)
     lili::DevBuf vg_coop;        // hash table + scratch of the cooperative filter
     lili::DevBuf hz_ctl;         // barrier words + per-block counts of the cooperative Horizon extractor
@@ -531,6 +532,8 @@ int inclusive_max_scan_i32(liliom_ctx* c, int* data, int n);            // in-pl
 // device-side count (<= n_max); d_feats (optional) also receives float4{x,y,z,index}.  key_bits, host_mm: see voxelgrid.cu.
 int voxelgrid_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride, float leaf, void* d_out, int* d_count,
                   float4* d_feats = nullptr, int key_bits = 32, const int* host_mm = nullptr);
+int voxelgrid_dev_sync(liliom_ctx* c, const void* d_in, int n, int stride, float leaf, void* d_out, int* d_count, float4* d_feats, int* m,
+                       int key_bits = 32);
 int vg_minmax_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride);
 int voxelgrid_coop(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride, float leaf, void* d_out, int* d_count, float4* d_feats,
                    bool* used);

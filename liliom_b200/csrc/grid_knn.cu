@@ -1144,6 +1144,7 @@ static int s2m_finish(liliom_ctx* c, const S2mCall& k, double pose7[7], liliom_i
     if (c->vg_check) {
         c->vg_ncells = r.vgp.overflow ? 0 : (long long)r.vgp.div_b[0] * r.vgp.div_b[1] * r.vgp.div_b[2];
         c->vg_bail = r.vgp.bail != 0;
+        c->vg_wide = vg_wide_keys(r.vgp);
     }
     if (iters > 0 && k.peer && r.pose[7] != 0.0) {
         c->last_error = "fused exchange: a peer rank did not publish its sums within the wait bound (collective call not entered on every rank?)";

@@ -13,6 +13,7 @@
 #include "ctx.cuh"
 #include "dev_math.cuh"
 #include "kf_table.h"
+#include <type_traits>
 
 namespace lili {
 
@@ -47,23 +48,26 @@ __global__ void k_kf_box(const unsigned char* __restrict__ arena, const KfRow* _
     vg_box_commit(box, mm);
 }
 
-// PCL's relative voxel index of every transformed point (all-ones: not finite), value = its index in the concatenation
+// PCL's relative voxel index of every transformed point (not finite: all-ones, or bit 32 of a wide key), value = its index in
+// the concatenation
+template <typename K>
 __global__ void k_kf_keys(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride, const VgParams p,
-                          uint32_t* __restrict__ keys, int* __restrict__ vals) {
+                          K* __restrict__ keys, int* __restrict__ vals) {
+    const K sentinel = sizeof(K) == 4 ? (K)0xffffffffu : (K)(1ull << 32);
     for (int y = blockIdx.y; y < rows; y += gridDim.y) {
         const KfRow& r = tab[y];
         for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < r.n; i += gridDim.x * blockDim.x) {
             const VgXyz x = kf_row_xyz(r, arena + (size_t)(r.src_off + i) * stride);
             const long long d = r.dst_off + i;
-            keys[d] = (isfinite(x.x) && isfinite(x.y) && isfinite(x.z)) ? vg_rel_index(p, x.x, x.y, x.z) : 0xffffffffu;
+            keys[d] = (isfinite(x.x) && isfinite(x.y) && isfinite(x.z)) ? (K)vg_rel_index(p, x.x, x.y, x.z) : sentinel;
             vals[d] = (int)d;
         }
     }
 }
 
 // centroid of every voxel of the sorted keys (the first n_fin entries are the finite points), members transformed on load
-template <int STRIDE>
-__global__ void k_kf_centroid(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, const uint32_t* __restrict__ keys,
+template <int STRIDE, typename K>
+__global__ void k_kf_centroid(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, const K* __restrict__ keys,
                               const int* __restrict__ vals, const int* __restrict__ flags, const int* __restrict__ rank, int n_fin,
                               unsigned char* __restrict__ out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -139,9 +143,9 @@ static KfRow kf_row(long long src, long long dst, int n, const double* pose7, co
 }
 
 // detectLoopClosure's cloud of the listed keyframes (:2476-2497, :2502-2547): edge then surf of each, transformed by its pose,
-// concatenated into bmap_raw (one launch), VoxelGrid(leaf) into vg_out with its count at d_count (device).  *n_in: the points
-// read (0: nothing was launched and d_count is not written).
-static int kf_cloud_dev(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, float leaf, int* d_count, long long* n_in) {
+// concatenated into bmap_raw (one launch), VoxelGrid(leaf) into vg_out with its count at d_count (device) and *m (host).
+// *n_in: the points read (0: nothing was launched, d_count is not written and *m = 0).
+static int kf_cloud_dev(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, float leaf, int* d_count, long long* n_in, int* m) {
     const int stride = c->prm.point_stride;
     std::vector<KfRow> tab;
     long long off = 0, largest = 0;
@@ -154,12 +158,13 @@ static int kf_cloud_dev(liliom_ctx* c, const int* kf_ids, const double* poses7, 
         largest = std::max(largest, (long long)std::max(f.n_edge, f.n_surf));
     }
     *n_in = off;
+    *m = 0;
     if (off == 0) return LILIOM_OK;
     LILI_CUDA(c, c->bmap_raw.ensure((size_t)off * stride));      // scratch: the local map's layers live in bmap_ds / bmap
     c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
     LILI_CUDA(c, c->vg_out.ensure((size_t)off * stride));
     LILI_TRY(kf_gather(c, c->kf_arena.p, tab, largest, c->bmap_raw.p));
-    return voxelgrid_dev(c, c->bmap_raw.p, (int)off, nullptr, stride, leaf, c->vg_out.p, d_count);
+    return voxelgrid_dev_sync(c, c->bmap_raw.p, (int)off, stride, leaf, c->vg_out.p, d_count, nullptr, m);
 }
 
 static int backend_check(liliom_ctx* c, const liliom_backend_params* bp) {
@@ -211,11 +216,9 @@ extern "C" int liliom_kf_add(liliom_ctx* c, const liliom_backend_params* bp, con
     if (n_surf) LILI_CUDA(c, cudaMemcpyAsync(raw + (size_t)n_edge * stride, surf_last, (size_t)n_surf * stride, cudaMemcpyHostToDevice, c->stream));
     unsigned char* tail = (unsigned char*)c->kf_arena.p + (size_t)c->kf_used * stride;
     int* cnt = c->vg_count.as<int>();
-    LILI_TRY(voxelgrid_dev(c, raw, n_edge, nullptr, stride, bp->edge_leaf, tail, cnt));                                           // :1502-1507
-    LILI_TRY(voxelgrid_dev(c, raw + (size_t)n_edge * stride, n_surf, nullptr, stride, bp->surf_leaf, c->vg_out.p, cnt + 1));     // :1509-1514
-    int m[2];
-    LILI_TRY(read_back(c, {{m, cnt, sizeof(m)}}));
-    const int me = m[0], ms = m[1];
+    int me = 0, ms = 0;
+    LILI_TRY(voxelgrid_dev_sync(c, raw, n_edge, stride, bp->edge_leaf, tail, cnt, nullptr, &me));                                   // :1502-1507
+    LILI_TRY(voxelgrid_dev_sync(c, raw + (size_t)n_edge * stride, n_surf, stride, bp->surf_leaf, c->vg_out.p, cnt + 1, nullptr, &ms));   // :1509-1514
     if (n_edge_ds) *n_edge_ds = me;
     if (n_surf_ds) *n_surf_ds = ms;
     if ((edge_ds_out && me > edge_cap) || (surf_ds_out && ms > surf_cap)) return LILIOM_E_CAPACITY;   // nothing stored
@@ -268,13 +271,12 @@ extern "C" int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp,
     const unsigned char* src[2] = {(const unsigned char*)c->bmap_raw.p, (const unsigned char*)c->bmap_raw.p + (size_t)E * stride};
     LILI_CUDA(c, c->vg_count.ensure(16));
     int* cnt = c->vg_count.as<int>();
+    int m[2];
     for (int l = 0; l < 2; ++l) {                                 // :1486-1492; the centroid kernel also writes the float4 points
         LILI_CUDA(c, c->bmap_ds[l].ensure((size_t)std::max(nl[l], 1LL) * stride));
         LILI_CUDA(c, c->bmap[l].xyzw.ensure((size_t)std::max(nl[l], 1LL) * sizeof(float4)));
-        LILI_TRY(voxelgrid_dev(c, src[l], (int)nl[l], nullptr, stride, leaf[l], c->bmap_ds[l].p, cnt + l, c->bmap[l].xyzw.as<float4>()));
+        LILI_TRY(voxelgrid_dev_sync(c, src[l], (int)nl[l], stride, leaf[l], c->bmap_ds[l].p, cnt + l, c->bmap[l].xyzw.as<float4>(), m + l));
     }
-    int m[2];
-    LILI_TRY(read_back(c, {{m, cnt, sizeof(m)}}));
     LILI_TRY(grid_build(c, c->bmap[0], gate_cell(1.0), m[0]));                 // :1543 sqdist[4] < 1.0
     LILI_TRY(grid_build(c, c->bmap[1], gate_cell(bp->kd_max_radius), m[1]));   // :1615 sqdist[4] < kd_max_radius
     if (stride == 48) {                                                         // reflectivity of the surf layer (:1617-1638)
@@ -308,10 +310,9 @@ extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* p
     *n_out = 0;
     LILI_CUDA(c, c->vg_count.ensure(16));
     long long off = 0;
-    LILI_TRY(kf_cloud_dev(c, kf_ids, poses7, k, leaf, c->vg_count.as<int>(), &off));
-    if (off == 0) return LILIOM_OK;
     int m = 0;
-    LILI_TRY(read_back(c, {{&m, c->vg_count.p, sizeof(int)}}));
+    LILI_TRY(kf_cloud_dev(c, kf_ids, poses7, k, leaf, c->vg_count.as<int>(), &off, &m));
+    if (off == 0) return LILIOM_OK;
     return download_sized(c, c->vg_out, m, stride, out, cap, n_out);
 }
 
@@ -332,17 +333,15 @@ extern "C" int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double
     LILI_CUDA(c, c->vg_count.ensure(16));
     int* cnt = c->vg_count.as<int>();
     long long off_t = 0, off_s = 0;
+    int m_t = 0, m_s = 0;
     // :2502-2547 his_key_frames_ds -> the loop index's points (float4, w = index), as liliom_icp_align installs a target
-    LILI_TRY(kf_cloud_dev(c, tgt_ids, tgt_poses7, k_tgt, leaf, cnt, &off_t));
+    LILI_TRY(kf_cloud_dev(c, tgt_ids, tgt_poses7, k_tgt, leaf, cnt, &off_t, &m_t));
     LILI_CUDA(c, c->loop.xyzw.ensure((size_t)std::max(off_t, 1LL) * sizeof(float4)));
     LILI_TRY(repack_to_f4(c, c->vg_out.p, (int)off_t, stride, c->loop.xyzw.as<float4>(), cnt));
     // :2476-2497 latest_key_frames_ds -> the source
-    LILI_TRY(kf_cloud_dev(c, src_ids, src_poses7, k_src, leaf, cnt + 1, &off_s));
+    LILI_TRY(kf_cloud_dev(c, src_ids, src_poses7, k_src, leaf, cnt + 1, &off_s, &m_s));
     LILI_CUDA(c, c->loop_src.ensure((size_t)std::max(off_s, 1LL) * sizeof(float4)));
     LILI_TRY(repack_to_f4(c, c->vg_out.p, (int)off_s, stride, c->loop_src.as<float4>(), cnt + 1));
-    int m[2];
-    LILI_TRY(read_back(c, {{m, cnt, sizeof(m)}}));
-    const int m_t = off_t ? m[0] : 0, m_s = off_s ? m[1] : 0;
     if (n_src) *n_src = m_s;
     if (n_tgt) *n_tgt = m_t;
     LILI_TRY(grid_build(c, c->loop, gate_cell(c->prm.knn_max_sqdist), m_t));      // the cell of liliom_icp_align's target
@@ -369,8 +368,7 @@ extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp
         LILI_CUDA(c, c->raw.ensure((size_t)n * stride));
         LILI_CUDA(c, c->vg_count.ensure(16));
         LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, full, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
-        LILI_TRY(voxelgrid_dev(c, c->raw.p, n, nullptr, stride, bp->surf_leaf, tail, c->vg_count.as<int>()));
-        LILI_TRY(read_back(c, {{&m, c->vg_count.p, sizeof(int)}}));
+        LILI_TRY(voxelgrid_dev_sync(c, c->raw.p, n, stride, bp->surf_leaf, tail, c->vg_count.as<int>(), nullptr, &m));
     }
     c->kfs[kf_id].full_off = c->kf_full_used;
     c->kfs[kf_id].n_full = m;
@@ -380,8 +378,9 @@ extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp
 }
 
 // The global map without a concatenation buffer: box, voxel keys and centroids read the stored clouds through the keyframe table
-// and transform every point on load (kf_table.h); the sort chain in between is voxelgrid_dev's (sort_pairs_u32 at the key width of
-// the box, k_vg_heads, the scan).  Device memory: the table, 16 bytes per listed point for keys and values (sort included), and
+// and transform every point on load (kf_table.h); the sort chain in between is voxelgrid_dev's (the sort at the key width of the
+// box, k_vg_heads, the scan).  Device memory: the table, 16 bytes per listed point for keys and values (sort included; 24 with
+// the wide keys), and
 // the output; only PCL's declined case writes the transformed concatenation, which is then the output.
 extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, const double* poses7, int k, const double pre7[7],
                                  float leaf, void* out, int cap, int* n) {
@@ -434,32 +433,38 @@ extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, con
         });
     const int n_fin = p.n_finite;
     if (n_fin == 0) { *n = 0; return LILIOM_OK; }
-    LILI_CUDA(c, c->vg_keys.ensure((size_t)N * 4));
+    const int key_bits = vg_chain_key_bits(box, leaf);            // the wide keys (64-bit) when the index wraps
+    const size_t kb = key_bits > 32 ? 8 : 4;
+    LILI_CUDA(c, c->vg_keys.ensure((size_t)N * kb));
     LILI_CUDA(c, c->vg_vals.ensure((size_t)N * 4));
-    LILI_CUDA(c, c->vg_keys2.ensure((size_t)N * 4));
+    LILI_CUDA(c, c->vg_keys2.ensure((size_t)N * kb));
     LILI_CUDA(c, c->vg_vals2.ensure((size_t)N * 4));
     LILI_CUDA(c, c->vg_flags.ensure(((size_t)n_fin + 2) * 4));
     LILI_CUDA(c, c->vg_rank.ensure(((size_t)n_fin + 2) * 4));
-    k_kf_keys<<<kf_row_grid(tab.size(), largest, 8), 256, 0, c->stream>>>(arena, d_tab, rows, stride, p, c->vg_keys.as<uint32_t>(),
-                                                                             c->vg_vals.as<int>());
-    LILI_TRY(launch_check(c, "k_kf_keys"));
-    // non-finite points carry the all-ones key and sort last: the first n_fin sorted entries are the finite points
-    LILI_TRY(sort_pairs_u32(c, c->vg_keys.as<uint32_t>(), c->vg_keys2.as<uint32_t>(), c->vg_vals.as<int>(), c->vg_vals2.as<int>(), (int)N,
-                            vg_key_bits(box, leaf)));
-    k_vg_heads<<<cdiv(n_fin + 1LL, 256), 256, 0, c->stream>>>(c->vg_keys2.as<uint32_t>(), n_fin, nullptr, c->vg_flags.as<int>());
-    LILI_TRY(launch_check(c, "k_vg_heads"));
-    LILI_TRY(exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin));
-    int m = 0;
-    LILI_TRY(read_back(c, {{&m, c->vg_rank.as<int>() + n_fin, sizeof(int)}}));
-    return download_sized(c, c->vg_out, m, stride, out, cap, n, [&]() -> int {
-        c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
-        LILI_CUDA(c, c->vg_out.ensure((size_t)m * stride));
-        if (stride == 48)
-            k_kf_centroid<48><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(),
-                                                                       c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
-        else
-            k_kf_centroid<32><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(),
-                                                                       c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
-        return launch_check(c, "k_kf_centroid");
-    });
+    auto chain = [&](auto* keys, auto* keys2) -> int {
+        using K = std::remove_pointer_t<decltype(keys)>;
+        k_kf_keys<K><<<kf_row_grid(tab.size(), largest, 8), 256, 0, c->stream>>>(arena, d_tab, rows, stride, p, keys, c->vg_vals.as<int>());
+        LILI_TRY(launch_check(c, "k_kf_keys"));
+        // non-finite points carry the sentinel key and sort last: the first n_fin sorted entries are the finite points
+        if constexpr (sizeof(K) == 4) LILI_TRY(sort_pairs_u32(c, keys, keys2, c->vg_vals.as<int>(), c->vg_vals2.as<int>(), (int)N, key_bits));
+        else LILI_TRY(sort_pairs_u64(c, keys, keys2, c->vg_vals.as<int>(), c->vg_vals2.as<int>(), (int)N, key_bits));
+        k_vg_heads<<<cdiv(n_fin + 1LL, 256), 256, 0, c->stream>>>(keys2, n_fin, nullptr, c->vg_flags.as<int>());
+        LILI_TRY(launch_check(c, "k_vg_heads"));
+        LILI_TRY(exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), n_fin));
+        int m = 0;
+        LILI_TRY(read_back(c, {{&m, c->vg_rank.as<int>() + n_fin, sizeof(int)}}));
+        return download_sized(c, c->vg_out, m, stride, out, cap, n, [&]() -> int {
+            c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
+            LILI_CUDA(c, c->vg_out.ensure((size_t)m * stride));
+            if (stride == 48)
+                k_kf_centroid<48, K><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, keys2, c->vg_vals2.as<int>(), c->vg_flags.as<int>(),
+                                                                              c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
+            else
+                k_kf_centroid<32, K><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, keys2, c->vg_vals2.as<int>(), c->vg_flags.as<int>(),
+                                                                              c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
+            return launch_check(c, "k_kf_centroid");
+        });
+    };
+    if (key_bits > 32) return chain(c->vg_keys.as<unsigned long long>(), c->vg_keys2.as<unsigned long long>());
+    return chain(c->vg_keys.as<uint32_t>(), c->vg_keys2.as<uint32_t>());
 }

@@ -424,13 +424,15 @@ static int inc_frame_keys(liliom_ctx* c, Frame& f, u64* keys, unsigned* refs) {
     return LILIOM_OK;
 }
 
-// the representability of the absolute keys, and PCL's "leaf size too small" test on the union box of the live frames
+// the representability of the absolute keys, PCL's "leaf size too small" test on the union box of the live frames, and that
+// box's index not wrapping (absolute-key order is PCL's index order only then)
 static bool inc_representable(liliom_ctx* c) {
     for (auto& f : c->frames)
         if (f.bad) return false;
     int box[kBoxInts];
     frames_box(c, box);
-    return !vg_params(box, c->prm.leaf_map).overflow;
+    const VgParams p = vg_params(box, c->prm.leaf_map);
+    return !p.overflow && !p.wraps;
 }
 
 // entry array from scratch (first call, or after liliom_map_push_frame / liliom_map_clear touched the FIFO)

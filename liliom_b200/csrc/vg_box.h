@@ -40,6 +40,8 @@ struct VgParams {
     int   n_finite;
     int   bail;        // cooperative single-launch filter declined this input (see k_vg_coop), or a box bound's cell lies outside
                        // int range (vg_params: x86 then sends indices to INT_MIN, outside the box): redo with full-width sort keys
+    int   wraps;       // div_b[0]*div_b[1]*div_b[2] >= 2^32 (vg_wraps): PCL's int index wraps, so two cells can share an index, the
+                       // index order is not the cells' (z, y, x) order, and a finite point can take the all-ones 32-bit index
 };
 
 // float <-> ordered int: integer order = float order (-0 below +0; NaNs of either sign outside every finite value)
@@ -109,6 +111,20 @@ __device__ __forceinline__ void vg_box_commit(int* box, int* mm) {
 
 VGB_HD long long vgb_mul64(long long a, long long b) { return (long long)((unsigned long long)a * (unsigned long long)b); }
 
+// Whether div_b[0]*div_b[1]*div_b[2] >= 2^32, each division read as the unsigned count max_b - min_b + 1 (0: 2^32 cells).  The
+// overflow test multiplies d = trunc((max - min) / leaf) + 1, which can be one smaller per axis than div_b, so this can hold
+// while PCL filters: its int index then wraps modulo 2^32.
+VGB_HD bool vg_wraps(const int* div_b) {
+    unsigned long long c = 1;
+    for (int k = 0; k < 3; ++k) {
+        const unsigned long long d = div_b[k] == 0 ? (1ull << 32) : (unsigned long long)(unsigned)div_b[k];
+        if (d >= (1ull << 32)) return true;
+        c *= d;                                     // < 2^32 * 2^32: no wrap
+        if (c >= (1ull << 32)) return true;
+    }
+    return false;
+}
+
 // float -> int and float -> int64 as PCL's x86-64 build converts them (cvttss2si): truncation toward zero, and INT_MIN /
 // INT64_MIN for NaN, +-inf and every value outside the target's range.  The device's own conversion saturates instead, and in
 // C++ an out-of-range conversion is undefined, so the rule is written out: a far or huge box gives PCL's indices, not clamped ones.
@@ -125,6 +141,7 @@ VGB_HD VgParams vg_params(const int* box, float leaf) {
     p.n_finite = box[6];
     p.overflow = 0;
     p.bail = 0;
+    p.wraps = 0;
     if (p.n_finite == 0) {
         for (int k = 0; k < 3; ++k) { p.min_b[k] = 0; p.div_b[k] = 1; }
     } else {
@@ -139,6 +156,7 @@ VGB_HD VgParams vg_params(const int* box, float leaf) {
             p.div_b[k] = (int)((unsigned)max_b - (unsigned)p.min_b[k] + 1u);
         }
         if (vgb_mul64(vgb_mul64(d[0], d[1]), d[2]) > (long long)INT_MAX) p.overflow = 1;
+        p.wraps = vg_wraps(p.div_b) ? 1 : 0;
     }
     p.mul[0] = 1; p.mul[1] = p.div_b[0]; p.mul[2] = (int)((unsigned)p.div_b[0] * (unsigned)p.div_b[1]);
     return p;
@@ -153,10 +171,10 @@ VGB_HD unsigned vg_rel_index(const VgParams& p, float x, float y, float z) {
     return (unsigned)i0 * (unsigned)p.mul[0] + (unsigned)i1 * (unsigned)p.mul[1] + (unsigned)i2 * (unsigned)p.mul[2];
 }
 
-// Width of the VoxelGrid sort chain's keys for a cloud with this box: the fewest bits (at least 8) that hold every voxel
-// index with the all-ones key of that width left free for the non-finite points' sentinel; 32 when the box is empty, in
-// PCL's overflow case, when the voxel count does not fit, or when a box bound's cell leaves int range (x86 then sends the
-// indices to INT_MIN, outside the box).
+// Width of the VoxelGrid sort chain's keys for a cloud with this box, when they are 32-bit ones: the fewest bits (at least 8)
+// that hold every voxel index with the all-ones key of that width left free for the non-finite points' sentinel; 32 when the
+// box is empty, in PCL's overflow case, when the voxel count does not fit, or when a box bound's cell leaves int range (x86
+// then sends the indices to INT_MIN, outside the box).  Where the index wraps, 32-bit keys do not suffice (vg_chain_key_bits).
 VGB_HD int vg_key_bits(const int* box, float leaf) {
     const VgParams p = vg_params(box, leaf);
     if (p.n_finite <= 0 || p.overflow || p.bail) return 32;
@@ -167,8 +185,21 @@ VGB_HD int vg_key_bits(const int* box, float leaf) {
     return bits;
 }
 
-// Absolute voxel key of a finite point: 21 bits per coordinate floor(p / leaf) + 2^20, packed (z, y, x) from the top, so
-// that key order is PCL's index order for any box.  False (key untouched) when a coordinate is outside (-2^20, 2^20).
+// Sort keys wider than 32 bits: 64-bit keys, the voxel index in the low 32 bits and the non-finite points' flag at bit 32,
+// sorted on 33 bits.  Needed when PCL filters a box whose index wraps (VgParams::wraps): any 32-bit value is then a finite
+// point's index, and an all-ones sentinel would share a key with it.
+constexpr int kVgWideKeyBits = 33;
+VGB_HD bool vg_wide_keys(const VgParams& p) { return p.n_finite > 0 && !p.overflow && p.wraps; }
+
+// The sort chain's key width for a box known in advance: kVgWideKeyBits where the index wraps, vg_key_bits otherwise.
+VGB_HD int vg_chain_key_bits(const int* box, float leaf) {
+    return vg_wide_keys(vg_params(box, leaf)) ? kVgWideKeyBits : vg_key_bits(box, leaf);
+}
+
+// Absolute voxel key of a finite point: 21 bits per coordinate floor(p / leaf) + 2^20, packed (z, y, x) from the top.  Key
+// order is the cells' (z, y, x) order, which is PCL's index order, and distinct cells have distinct PCL indices, only while
+// the index does not wrap (VgParams::wraps): the paths built on these keys decline such boxes.  False (key untouched) when a
+// coordinate is outside (-2^20, 2^20).
 VGB_HD bool vg_abs_key(float x, float y, float z, float inv_leaf, unsigned long long* key) {
     const float fx = floorf(x * inv_leaf), fy = floorf(y * inv_leaf), fz = floorf(z * inv_leaf);
     const float lim = 1048576.0f;

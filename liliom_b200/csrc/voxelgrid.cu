@@ -10,6 +10,7 @@
 #include <cmath>
 #include <cstring>
 #include <cstdlib>
+#include <type_traits>
 
 namespace lili {
 
@@ -30,22 +31,24 @@ __global__ void k_vg_params_box(const VgBox b, float leaf, VgParams* __restrict_
     if (threadIdx.x == 0) *out = vg_params(b.mm, leaf);
 }
 
+// K = uint32_t: non-finite points take the all-ones key; K = unsigned long long (wide keys, vg_wide_keys): the flag at bit 32
+template <typename K>
 __global__ void k_vg_keys(const unsigned char* __restrict__ pts, int n_max, const int* __restrict__ d_n, int stride, const VgParams* __restrict__ pp,
-                          uint32_t* __restrict__ keys, int* __restrict__ vals) {
+                          K* __restrict__ keys, int* __restrict__ vals) {
     int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_max) return;
     const int n = d_n ? min(*d_n, n_max) : n_max;
     const VgParams p = *pp;
     float4 v = make_float4(NAN, 0.f, 0.f, 0.f);
     if (i < n) v = *reinterpret_cast<const float4*>(pts + (size_t)i * stride);
-    uint32_t key = 0xffffffffu;
+    K key = sizeof(K) == 4 ? (K)0xffffffffu : (K)(1ull << 32);
     if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) key = vg_rel_index(p, v.x, v.y, v.z);
     keys[i] = key;
     vals[i] = i;
 }
 
-template <int STRIDE>
-__global__ void k_vg_centroid(const unsigned char* __restrict__ pts, const uint32_t* __restrict__ keys, const int* __restrict__ vals,
+template <int STRIDE, typename K>
+__global__ void k_vg_centroid(const unsigned char* __restrict__ pts, const K* __restrict__ keys, const int* __restrict__ vals,
                               const int* __restrict__ flags, const int* __restrict__ rank, int n_max, const int* __restrict__ d_n,
                               const VgParams* __restrict__ pp, unsigned char* __restrict__ out, int* __restrict__ count_out,
                               float4* __restrict__ feats_out) {
@@ -88,12 +91,13 @@ __global__ void k_vg_centroid(const unsigned char* __restrict__ pts, const uint3
 //   phase 3  one warp per voxel: output rank = number of listed keys below its key (all pairs); members read
 //            from the slot's bucket and ordered by original index (rank by counting in shared memory), fp32
 //            sums in that order — the order of the sort chain and of the oracle — centroid written at the rank
-// Inputs it declines (|cell coordinate| >= 2^20, PCL's index overflow, a voxel with more than VGC_VCAP members)
-// set VgParams::bail and an output count of 0; the caller re-runs the sort chain.  Semantics otherwise
-// identical to k_vg_* above.
+// Inputs it declines (|cell coordinate| >= 2^20, PCL's index overflow, a voxel with more than VGC_VCAP members, a box
+// whose PCL index wraps: VgParams::wraps, where absolute-key order is not PCL's order and distinct cells can share an
+// index) set VgParams::bail and an output count of 0; the box's own parameters are left with the bail mark, so the caller
+// knows which key width the sort chain needs.  Semantics otherwise identical to k_vg_* above.
 // One barrier is enough because every bail condition is final when it is passed: bits 0 (unrepresentable
 // key) and 1 (arrival number VGC_VCAP, i.e. a voxel over VGC_VCAP members) are only set in phase 1, and the
-// overflow test reads the box partials, which phase 1 completes.  So every block takes the same decision, and
+// overflow and wrap tests (bits 2 and 3) read the box partials, which phase 1 completes.  So every block takes the same decision, and
 // no block decides to bail on a bit that another block can still set (a block that bailed on a late bit would
 // never reach a later barrier, and the blocks waiting there would spin forever).  After the barrier a warp
 // touches only its own voxel's slot (count, bucket, and handing the slot back) plus data no block writes any
@@ -250,9 +254,14 @@ __global__ void __launch_bounds__(VGC_THREADS, 1) k_vg_coop(const unsigned char*
             for (int k = 0; k < kBoxInts; ++k) mm[k] = vg_box_join(k, mm[k], __shfl_xor_sync(0xffffffffu, mm[k], o));
         }
         if (lane == 0) {
-            const VgParams p = vg_params(mm, leaf);
+            VgParams p = vg_params(mm, leaf);
             if (p.overflow) bail |= 4u;                                  // PCL copies the input: sort chain
-            if (blockIdx.x == 0 && !bail) { *pp = p; *count_out = U; }
+            if (p.wraps) bail |= 8u;                                     // PCL's index wraps: not the absolute keys' order
+            if (blockIdx.x == 0) {
+                if (bail) p.bail = 1;
+                *pp = p;
+                *count_out = bail ? 0 : U;
+            }
             S.bail = bail;
         }
     } else if (!bail && in_smem) {
@@ -262,16 +271,8 @@ __global__ void __launch_bounds__(VGC_THREADS, 1) k_vg_coop(const unsigned char*
     bail = S.bail;
     if (stamp) stamp[2] = clock64();
     if (bail) {
-        // declined: leave the table clean for the next launch and report an empty result with the bail mark
+        // declined (the bail mark and an empty result are written above): leave the table clean for the next launch
         for (int s = gtid; s < VGC_T; s += gthreads) { B.hkey[s] = VGC_EMPTY; B.hcnt[s] = 0; }
-        if (blockIdx.x == 0 && tid == 0) {
-            VgParams p;
-            p.inv_leaf = inv_leaf;
-            for (int k = 0; k < 3; ++k) { p.min_b[k] = 0; p.div_b[k] = 1; p.mul[k] = 1; }
-            p.overflow = 0; p.n_finite = 0; p.bail = 1;
-            *pp = p;
-            *count_out = 0;
-        }
         return;
     }
 
@@ -384,12 +385,14 @@ int vg_minmax_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, in
 }
 
 // key_bits < 32: the caller speculates that the voxel index fits that width (one onesweep pass less per 8 bits) and must check
-// `ncells <= 2^key_bits - 1` afterwards (vg_params stays on the device).  host_mm (optional): the cloud's box and finite count
-// already known on the host -> no pass over the input for it, and the key width follows from the box (vg_key_bits).
+// `ncells <= 2^key_bits - 1` afterwards (vg_params stays on the device).  key_bits = 32 assumes the index does not wrap: the
+// caller checks vg_wide_keys on the VgParams it reads back and redoes the call with key_bits = kVgWideKeyBits (64-bit keys) on
+// a hit (voxelgrid_dev_sync).  host_mm (optional): the cloud's box and finite count already known on the host -> no pass over
+// the input for it, and the key width follows from the box (vg_chain_key_bits).
 int voxelgrid_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride, float leaf, void* d_out, int* d_count,
                   float4* d_feats, int key_bits, const int* host_mm) {
     if (stride != 48 && stride != 32) return LILIOM_E_ARG;
-    if (host_mm) key_bits = vg_key_bits(host_mm, leaf);
+    if (host_mm) key_bits = vg_chain_key_bits(host_mm, leaf);
     if (n_max <= 0) {
         LILI_CUDA(c, cudaMemsetAsync(d_count, 0, sizeof(int), c->stream));
         return LILIOM_OK;
@@ -398,9 +401,11 @@ int voxelgrid_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, in
     const int n = n_max;
     LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
     LILI_CUDA(c, c->vg_params.ensure(sizeof(VgParams)));
-    LILI_CUDA(c, c->vg_keys.ensure((size_t)n * 4));
+    const bool wide = key_bits > 32;
+    const size_t kb = wide ? 8 : 4;
+    LILI_CUDA(c, c->vg_keys.ensure((size_t)n * kb));
     LILI_CUDA(c, c->vg_vals.ensure((size_t)n * 4));
-    LILI_CUDA(c, c->vg_keys2.ensure((size_t)n * 4));
+    LILI_CUDA(c, c->vg_keys2.ensure((size_t)n * kb));
     LILI_CUDA(c, c->vg_vals2.ensure((size_t)n * 4));
     LILI_CUDA(c, c->vg_flags.ensure(((size_t)n + 2) * 4));
     LILI_CUDA(c, c->vg_rank.ensure(((size_t)n + 2) * 4));
@@ -419,21 +424,42 @@ int voxelgrid_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, in
         k_vg_params<<<1, 32, 0, c->stream>>>(mm, leaf, pp);
         LILI_TRY(launch_check(c, "k_vg_params"));
     }
-    k_vg_keys<<<cdiv(n, 256), 256, 0, c->stream>>>(in, n, d_n, stride, pp, c->vg_keys.as<uint32_t>(), c->vg_vals.as<int>());
-    LILI_TRY(launch_check(c, "k_vg_keys"));
-    // non-finite points carry the all-ones key (folded to the sort's width) and sort last; VgParams::n_finite excludes them
-    LILI_TRY(sort_pairs_u32(c, c->vg_keys.as<uint32_t>(), c->vg_keys2.as<uint32_t>(), c->vg_vals.as<int>(), c->vg_vals2.as<int>(), n, key_bits));
-    k_vg_heads<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(c->vg_keys2.as<uint32_t>(), n, &pp->n_finite, c->vg_flags.as<int>());
-    LILI_TRY(launch_check(c, "k_vg_heads"));
-    LILI_TRY(exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), n));
-    if (stride == 48)
-        k_vg_centroid<48><<<cdiv(n, 128), 128, 0, c->stream>>>(in, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(), c->vg_flags.as<int>(),
-                                                               c->vg_rank.as<int>(), n, d_n, pp, (unsigned char*)d_out, d_count, d_feats);
-    else
-        k_vg_centroid<32><<<cdiv(n, 128), 128, 0, c->stream>>>(in, c->vg_keys2.as<uint32_t>(), c->vg_vals2.as<int>(), c->vg_flags.as<int>(),
-                                                               c->vg_rank.as<int>(), n, d_n, pp, (unsigned char*)d_out, d_count, d_feats);
-    LILI_TRY(launch_check(c, "k_vg_centroid"));
-    return LILIOM_OK;
+    // keys -> sort -> heads -> ranks -> centroids at key type K; non-finite points carry the sentinel key (the all-ones 32-bit key,
+    // folded to the sort's width, or bit 32 of a wide key) and sort last; VgParams::n_finite excludes them
+    auto chain = [&](auto* keys, auto* keys2, int end_bit) -> int {
+        using K = std::remove_pointer_t<decltype(keys)>;
+        k_vg_keys<K><<<cdiv(n, 256), 256, 0, c->stream>>>(in, n, d_n, stride, pp, keys, c->vg_vals.as<int>());
+        LILI_TRY(launch_check(c, "k_vg_keys"));
+        if constexpr (sizeof(K) == 4) LILI_TRY(sort_pairs_u32(c, keys, keys2, c->vg_vals.as<int>(), c->vg_vals2.as<int>(), n, end_bit));
+        else LILI_TRY(sort_pairs_u64(c, keys, keys2, c->vg_vals.as<int>(), c->vg_vals2.as<int>(), n, end_bit));
+        k_vg_heads<<<cdiv(n + 1, 256), 256, 0, c->stream>>>(keys2, n, &pp->n_finite, c->vg_flags.as<int>());
+        LILI_TRY(launch_check(c, "k_vg_heads"));
+        LILI_TRY(exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), n));
+        if (stride == 48)
+            k_vg_centroid<48, K><<<cdiv(n, 128), 128, 0, c->stream>>>(in, keys2, c->vg_vals2.as<int>(), c->vg_flags.as<int>(), c->vg_rank.as<int>(), n,
+                                                                      d_n, pp, (unsigned char*)d_out, d_count, d_feats);
+        else
+            k_vg_centroid<32, K><<<cdiv(n, 128), 128, 0, c->stream>>>(in, keys2, c->vg_vals2.as<int>(), c->vg_flags.as<int>(), c->vg_rank.as<int>(), n,
+                                                                      d_n, pp, (unsigned char*)d_out, d_count, d_feats);
+        return launch_check(c, "k_vg_centroid");
+    };
+    if (wide) return chain(c->vg_keys.as<unsigned long long>(), c->vg_keys2.as<unsigned long long>(), kVgWideKeyBits);
+    return chain(c->vg_keys.as<uint32_t>(), c->vg_keys2.as<uint32_t>(), key_bits);
+}
+
+// voxelgrid_dev of n points (n known on the host) with its output count read back at once: the count and VgParams come back in
+// one sync, and the filter is redone with wide keys when the index wraps.  key_bits: 32, or kVgWideKeyBits when the caller
+// already knows the index wraps.  *m: the output count.
+int voxelgrid_dev_sync(liliom_ctx* c, const void* d_in, int n, int stride, float leaf, void* d_out, int* d_count, float4* d_feats, int* m,
+                       int key_bits) {
+    *m = 0;
+    LILI_TRY(voxelgrid_dev(c, d_in, n, nullptr, stride, leaf, d_out, d_count, d_feats, key_bits));
+    if (n <= 0) return LILIOM_OK;
+    VgParams vp;
+    LILI_TRY(read_back(c, {{m, d_count, sizeof(int)}, {&vp, c->vg_params.p, sizeof(VgParams)}}));
+    if (key_bits > 32 || !vg_wide_keys(vp)) return LILIOM_OK;
+    LILI_TRY(voxelgrid_dev(c, d_in, n, nullptr, stride, leaf, d_out, d_count, d_feats, kVgWideKeyBits));
+    return read_back(c, {{m, d_count, sizeof(int)}});
 }
 
 }  // namespace lili

@@ -30,6 +30,8 @@ extern "C" void vb_params(const int* box, float leaf, int* out, float* inv_leaf)
 }
 
 extern "C" int vb_key_bits(const int* box, float leaf) { return lili::vg_key_bits(box, leaf); }
+extern "C" int vb_chain_key_bits(const int* box, float leaf) { return lili::vg_chain_key_bits(box, leaf); }
+extern "C" int vb_wraps(const int* box, float leaf) { return lili::vg_params(box, leaf).wraps; }
 
 extern "C" int vb_abs_key(float x, float y, float z, float inv_leaf, unsigned long long* key) {
     return lili::vg_abs_key(x, y, z, inv_leaf, key) ? 1 : 0;
@@ -68,8 +70,25 @@ static void vb_stable_sort(std::vector<K>& keys, std::vector<int>& vals) {
 
 static bool vb_finite(const lili::VgF4& v) { return std::isfinite(v.x) && std::isfinite(v.y) && std::isfinite(v.z); }
 
-// The VoxelGrid sort chain (voxelgrid_dev): box -> vg_params -> vg_rel_index keys (all-ones for non-finite points) -> stable
-// sort -> heads over the finite entries -> walk -> writer.  PCL's overflow case copies the input.  Returns the output count.
+// keys of the sort chain: the voxel index of a finite point, the non-finite sentinel otherwise (all-ones for 32-bit keys, the
+// flag at bit 32 for wide ones)
+template <int STRIDE, typename K>
+static int vb_keyed_chain(const unsigned char* pts, int n, const lili::VgParams& p, unsigned char* out, float* xyz) {
+    const K sentinel = sizeof(K) == 4 ? (K)0xffffffffu : (K)(1ull << 32);
+    std::vector<K> keys(n);
+    std::vector<int> vals(n);
+    for (int i = 0; i < n; ++i) {
+        const lili::VgF4 v = lili::vg_ld4(pts + (size_t)i * STRIDE);
+        keys[i] = vb_finite(v) ? (K)lili::vg_rel_index(p, v.x, v.y, v.z) : sentinel;
+        vals[i] = i;
+    }
+    vb_stable_sort(keys, vals);
+    return vb_emit<STRIDE>(pts, keys, vals, p.n_finite, out, xyz);
+}
+
+// The VoxelGrid sort chain (voxelgrid_dev): box -> vg_params -> vg_rel_index keys (sentinel for non-finite points; 64-bit keys
+// when vg_wide_keys) -> stable sort -> heads over the finite entries -> walk -> writer.  PCL's overflow case copies the input.
+// Returns the output count.
 template <int STRIDE>
 static int vb_sort_chain(const unsigned char* pts, int n, float leaf, unsigned char* out, float* xyz) {
     int box[lili::kBoxInts];
@@ -80,15 +99,8 @@ static int vb_sort_chain(const unsigned char* pts, int n, float leaf, unsigned c
     }
     const lili::VgParams p = lili::vg_params(box, leaf);
     if (p.overflow) { memcpy(out, pts, (size_t)n * STRIDE); return n; }
-    std::vector<uint32_t> keys(n);
-    std::vector<int> vals(n);
-    for (int i = 0; i < n; ++i) {
-        const lili::VgF4 v = lili::vg_ld4(pts + (size_t)i * STRIDE);
-        keys[i] = vb_finite(v) ? lili::vg_rel_index(p, v.x, v.y, v.z) : 0xffffffffu;
-        vals[i] = i;
-    }
-    vb_stable_sort(keys, vals);
-    return vb_emit<STRIDE>(pts, keys, vals, p.n_finite, out, xyz);
+    if (lili::vg_wide_keys(p)) return vb_keyed_chain<STRIDE, unsigned long long>(pts, n, p, out, xyz);
+    return vb_keyed_chain<STRIDE, uint32_t>(pts, n, p, out, xyz);
 }
 
 extern "C" int vb_voxelgrid(const void* pts, int n, int stride, float leaf, void* out, float* xyz) {
