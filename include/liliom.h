@@ -618,6 +618,34 @@ int liliom_backend_window_correspond_batch(liliom_ctx* const* ctxs, int B, const
 int liliom_backend_window_blocks_batch(liliom_ctx* const* ctxs, int B, const double* const* poses7_body, const int* k,
                                        double* const* out29, int* status);
 
+/* The settings and the results of one session of liliom_loop_align_batch: liliom_loop_align's arguments and outputs. */
+typedef struct { float leaf; double max_corr_dist; int max_iter; double trans_eps, fit_eps; } liliom_loop_params;
+typedef struct { double T16[16]; double fitness; int converged, iters, n_src, n_tgt; } liliom_loop_result;
+/* liliom_loop_align of B independent sessions in one call.  src_ids, src_poses7, tgt_ids, tgt_poses7: B per-session pointers;
+ * k_src, k_tgt, status: B ints; prm, res: B structs.  Session i gets exactly what
+ *   liliom_loop_align(ctxs[i], src_ids[i], src_poses7[i], k_src[i], tgt_ids[i], tgt_poses7[i], k_tgt[i], prm[i].leaf,
+ *                     prm[i].max_corr_dist, prm[i].max_iter, prm[i].trans_eps, prm[i].fit_eps, res[i].T16, &res[i].fitness,
+ *                     &res[i].converged, &res[i].iters, &res[i].n_src, &res[i].n_tgt)
+ * would give it, bit for bit: status, results, liliom_last_error, launches and lib_launches, and the state left in ctxs[i] (the
+ * loop index and source, no resident scan for liliom_map_update_resident; the odometry map, the local map, the window and the
+ * keyframe store untouched), so that solo and batched calls mix freely.  A session without a loop candidate this tick is simply
+ * left out of ctxs.  Horizon (48-byte) and ROT (32-byte) sessions may be mixed, each with its own lists and settings.
+ * Every kernel of both clouds' composition (gather, VoxelGrid chain, repack) and of the targets' cell grids runs once for up to 32
+ * sessions on ctxs[0]'s stream (other sessions' streams are joined with events); the library sorts and scans stay per session, in
+ * order on the same stream.  The ICPs share cooperative k_icp_batch launches: each session keeps its solo grid, its own barrier
+ * word, partials and pinned results, so its bits do not depend on its neighbours; a session whose solo grid is not co-resident
+ * beside nothing else in k_icp_batch runs k_icp_persistent inside the call.  The call waits three times for all sessions together
+ * (both clouds' counts, the targets' boxes, the results) where B solo calls wait four times each; a session whose voxel index
+ * wraps (wide keys) finishes on its solo path inside the call.  Sessions with an empty source or target get identity,
+ * converged = 0 and iters = 0 without an ICP launch, as in the solo call.  The barrier flavour (LILIOM_GN_SYNC) is ctxs[0]'s.
+ * A session's own error (every error its solo call returns: an unknown id, leaf <= 0, max_corr_dist <= 0, max_iter < 1, a negative
+ * k, a NULL list with k > 0; LILIOM_E_GRID) is its status; the others run.
+ * LILIOM_E_ARG for the whole call, nothing changed: B < 1, a NULL array (ctxs, src_ids, src_poses7, k_src, tgt_ids, tgt_poses7,
+ * k_tgt, prm, res, status), a NULL or repeated context, contexts on different devices, a context with a communicator. */
+int liliom_loop_align_batch(liliom_ctx* const* ctxs, int B, const int* const* src_ids, const double* const* src_poses7, const int* k_src,
+                            const int* const* tgt_ids, const double* const* tgt_poses7, const int* k_tgt,
+                            const liliom_loop_params* prm, liliom_loop_result* res, int* status);
+
 #ifdef __cplusplus
 }
 #endif

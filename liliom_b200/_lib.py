@@ -54,6 +54,18 @@ class BackendParams(C.Structure):
                 ("reflect_thres", C.c_double), ("cauchy_b", C.c_double), ("q_lb", C.c_double * 4), ("t_lb", C.c_double * 3)]
 
 
+class LoopParams(C.Structure):
+    """liliom_loop_params (include/liliom.h): liliom_loop_align's settings of one session of liliom_loop_align_batch."""
+    _fields_ = [("leaf", C.c_float), ("max_corr_dist", C.c_double), ("max_iter", C.c_int), ("trans_eps", C.c_double),
+                ("fit_eps", C.c_double)]
+
+
+class LoopResult(C.Structure):
+    """liliom_loop_result (include/liliom.h): liliom_loop_align's outputs of one session of liliom_loop_align_batch."""
+    _fields_ = [("T16", C.c_double * 16), ("fitness", C.c_double), ("converged", C.c_int), ("iters", C.c_int), ("n_src", C.c_int),
+                ("n_tgt", C.c_int)]
+
+
 class Counters(C.Structure):
     _fields_ = [("launches", C.c_ulonglong), ("lib_launches", C.c_ulonglong), ("knn_ms", C.c_double),
                 ("knn_launches", C.c_ulonglong), ("knn_queries", C.c_ulonglong), ("knn_candidates", C.c_ulonglong)]
@@ -82,6 +94,7 @@ EXPORTS = [
     "liliom_extract_resident_batch", "liliom_features_download",
     "liliom_map_update_resident", "liliom_map_update_batch",
     "liliom_backend_window_correspond_batch", "liliom_backend_window_blocks_batch",
+    "liliom_loop_align_batch",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -231,6 +244,8 @@ def lib() -> C.CDLL:
     L.liliom_global_map.argtypes = [vp, C.c_int, ip, dp, C.c_int, dp, C.c_float, vp, C.c_int, ip]
     L.liliom_loop_align.argtypes = [vp, ip, dp, C.c_int, ip, dp, C.c_int, C.c_float, C.c_double, C.c_int, C.c_double, C.c_double,
                                     dp, dp, ip, ip, ip, ip]
+    L.liliom_loop_align_batch.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(ip), C.POINTER(dp), ip, C.POINTER(ip), C.POINTER(dp), ip,
+                                          C.POINTER(LoopParams), C.POINTER(LoopResult), ip]
     L.liliom_pre_create.argtypes = [vp, C.c_int, dp]; L.liliom_pre_create.restype = vp
     L.liliom_pre_destroy.argtypes = [vp]; L.liliom_pre_destroy.restype = None
     L.liliom_pre_imu.argtypes = [vp, C.c_double, dp]; L.liliom_pre_imu.restype = None
@@ -917,6 +932,34 @@ def map_update_batch(ctxs, poses7):
     if rc != OK:
         raise LiliomError(rc)
     return n_map[:B], status[:B]
+
+
+def loop_align_batch(ctxs, src_ids, src_poses, tgt_ids, tgt_poses, params):
+    """loop_align of every context in `ctxs` in one call (liliom_loop_align_batch): session i gets what
+    ctxs[i].loop_align(src_ids[i], src_poses[i], tgt_ids[i], tgt_poses[i], **params[i]) would give it.  src_ids, src_poses,
+    tgt_ids, tgt_poses: B sequences (a None entry passes a NULL list); params: B dicts of loop_align's settings (leaf, and
+    optionally max_corr_dist, max_iter, trans_eps, fit_eps, with loop_align's defaults).  Returns (B tuples
+    (T 4x4, fitness, converged, iterations, n_src, n_tgt), status (B,)); a session's own error is its status, a whole-call
+    error raises LiliomError."""
+    B = len(ctxs)
+    if len(src_ids) != B or len(src_poses) != B or len(tgt_ids) != B or len(tgt_poses) != B or len(params) != B:
+        raise ValueError(f"expected {B} per-session id lists, pose lists and settings")
+    si = [_ids(x) if x is not None else None for x in src_ids]
+    ti = [_ids(x) if x is not None else None for x in tgt_ids]
+    sp = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1) if p is not None else None for p in src_poses]
+    tp = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1) if p is not None else None for p in tgt_poses]
+    ks = np.array([len(x) if x is not None else 0 for x in si] + [0], np.int32)
+    kt = np.array([len(x) if x is not None else 0 for x in ti] + [0], np.int32)
+    defaults = dict(max_corr_dist=30.0, max_iter=100, trans_eps=1e-6, fit_eps=1e-6)
+    prm = (LoopParams * max(B, 1))(*[LoopParams(**{**defaults, **p}) for p in params])
+    res = (LoopResult * max(B, 1))()
+    status = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_loop_align_batch(_handles(ctxs), B, _ptrs(si, C.c_int), _ptrs(sp, C.c_double), _ip(ks), _ptrs(ti, C.c_int),
+                                       _ptrs(tp, C.c_double), _ip(kt), prm, res, _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    out = [(np.array(r.T16[:], np.float64).reshape(4, 4), r.fitness, bool(r.converged), r.iters, r.n_src, r.n_tgt) for r in res[:B]]
+    return out, status[:B]
 
 
 def _handles(ctxs):

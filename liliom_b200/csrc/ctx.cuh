@@ -149,7 +149,7 @@ struct GnIo {
 #ifdef __CUDACC__
 // Where a block sits in its session: blk.bi() of blk.G() blocks.  A solo launch reads blockIdx.x / gridDim.x at each use
 // (the kernels keep the code and registers they had before the batched launch existed); a batched launch (k_gn_batch,
-// k_hz_batch) passes the block's place inside its session's range.
+// k_hz_batch, k_icp_batch) passes the block's place inside its session's range.
 struct SoloBlock {
     __device__ __forceinline__ int bi() const { return (int)blockIdx.x; }
     __device__ __forceinline__ unsigned int G() const { return gridDim.x; }
@@ -212,6 +212,53 @@ __device__ __forceinline__ void vg_minmax_body(const unsigned char* __restrict__
         vg_box_add(box, v.x, v.y, v.z);
     }
     vg_box_commit(box, mm);
+}
+
+// Bodies of the VoxelGrid chain's parameter, key and centroid kernels (voxelgrid.cu), `i` as above; the batched loop closure
+// (keyframes.cu) runs them too.
+__device__ __forceinline__ void vg_params_at(const int* __restrict__ mm, float leaf, VgParams* __restrict__ out) {
+    if (threadIdx.x == 0) *out = vg_params(mm, leaf);
+}
+
+// K = uint32_t: non-finite points take the all-ones key; K = unsigned long long (wide keys, vg_wide_keys): the flag at bit 32
+template <typename K>
+__device__ __forceinline__ void vg_keys_at(const unsigned char* __restrict__ pts, int n_max, const int* __restrict__ d_n, int stride,
+                                           const VgParams* __restrict__ pp, K* __restrict__ keys, int* __restrict__ vals, const int i) {
+    if (i >= n_max) return;
+    const int n = d_n ? min(*d_n, n_max) : n_max;
+    const VgParams p = *pp;
+    float4 v = make_float4(NAN, 0.f, 0.f, 0.f);
+    if (i < n) v = *reinterpret_cast<const float4*>(pts + (size_t)i * stride);
+    K key = sizeof(K) == 4 ? (K)0xffffffffu : (K)(1ull << 32);
+    if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) key = vg_rel_index(p, v.x, v.y, v.z);
+    keys[i] = key;
+    vals[i] = i;
+}
+
+template <int STRIDE, typename K>
+__device__ __forceinline__ void vg_centroid_at(const unsigned char* __restrict__ pts, const K* __restrict__ keys, const int* __restrict__ vals,
+                                               const int* __restrict__ flags, const int* __restrict__ rank, int n_max, const int* __restrict__ d_n,
+                                               const VgParams* __restrict__ pp, unsigned char* __restrict__ out, int* __restrict__ count_out,
+                                               float4* __restrict__ feats_out, const int i) {
+    const VgParams p = *pp;
+    const int n = d_n ? min(*d_n, n_max) : n_max;
+    if (i == 0) *count_out = p.overflow ? n : rank[n_max];
+    if (p.overflow) {   // PCL: output = *input_ (not the centroids of one-point voxels: the normal and the padding would differ)
+        if (i < n) {
+            const float4* src = reinterpret_cast<const float4*>(pts + (size_t)i * STRIDE);
+            float4* dst = reinterpret_cast<float4*>(out + (size_t)i * STRIDE);
+#pragma unroll
+            for (int k = 0; k < STRIDE / 16; ++k) dst[k] = src[k];
+            if (feats_out) feats_out[i] = make_float4(src[0].x, src[0].y, src[0].z, __int_as_float(i));
+        }
+        return;
+    }
+    if (i >= n || !flags[i]) return;
+    const int o = rank[i];
+    const VgAcc<STRIDE> a = vg_walk<STRIDE>(keys, i, p.n_finite, [&](int j) { return vals[j]; },
+                                            [&](int m) { return pts + (size_t)m * STRIDE; });
+    const VgXyz c = vg_write<STRIDE>(a.s, a.n, out + (size_t)o * STRIDE);
+    if (feats_out) feats_out[o] = make_float4(c.x, c.y, c.z, __int_as_float(o));
 }
 
 __device__ __forceinline__ void repack_f4_at(const unsigned char* __restrict__ in, int n_max, const int* __restrict__ d_n, int stride,
@@ -445,6 +492,8 @@ struct liliom_ctx {
     bool rot_slow_walk = false;          // LILIOM_ROT_SLOW_WALK (test hook): the general walk of k_rot_ring for every segment
     bool hz_chain = false;               // LILIOM_HZ_CHAIN=1 (test hook): the Horizon extractor's multi-launch chain, not k_hz_coop
     bool test_shrink_box = false;        // LILIOM_TEST_SHRINK_BOX (test hook): grid_build takes a box too small in x
+    int test_icp_blocks = 0;             // LILIOM_TEST_ICP_BLOCKS=N (test hook): the batched ICP gives this context's session at most
+                                         // N blocks instead of its solo grid (the bits must not move)
     bool knn_tma = false, knn_tma_smem_set = false;   // LILIOM_KNN_TMA=1: bulk-copy (cp.async.bulk + mbarrier) staging of the runs in the 16-lane search
     bool knn1_smem_set = false;          // dynamic shared memory limit raised for the one-thread-per-query kernels on this device
     std::vector<cudaEvent_t> ev_pool;
@@ -561,6 +610,9 @@ struct GridJob {
     int* escaped = nullptr;              // device flag of k_cell_keys (a host_box was given)
 };
 int grid_begin(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_box, GridJob& j);
+// grid_begin of m > 0 points without a host_box, its box pass (k_vg_init, k_vg_minmax over mi.xyzw) already run and its box
+// (kBoxInts ints) read back by the caller (the batched loop closure reads every session's with one wait)
+int grid_begin_exact(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* hb, GridJob& j);
 int grid_sort(const GridJob& j);
 int grid_clear(const GridJob& j);
 int grid_scan(const GridJob& j);
@@ -679,6 +731,37 @@ int rot_batch_finish(RotBatchSession& s);
 
 int icp_align(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,
               double fit_eps, double T16[16], double* fitness, int* converged, int* iters);     // icp.cu
+
+// icp_align in parts (icp.cu), for the batched loop closure (keyframes.cu), which shares the launches of several sessions:
+// icp_begin (host: the launch's arguments and grid, the buffers, the zeroed barrier word; done = an empty source or target,
+// nothing to launch), icp_launch (the solo cooperative launch), icp_fetch (the results to the pinned block when it is not
+// mapped), and, after a synchronise of the stream, icp_finish (the results out of the pinned block; identity when done).
+struct IcpArgs {
+    const float4* src; int n, nvb;                   // source points (float4 xyz*), virtual blocks cdiv(n, 256)
+    const float4* map; const float4* map_orig; const int* cell_start; GridDesc g;
+    float max_d2;                                    // squared correspondence cut-off
+    int rmax, rmax_fit;                              // shells to visit at most: correspondence passes, the fitness pass
+    int max_iter; double trans_eps, fit_eps;
+    double* partials;                                // [2 parities][kIcpSums][nvb]
+    unsigned int* bar; int sync_mode;                // grid barrier word (zeroed before the launch), LILIOM_GN_SYNC
+    PinIcp* out;                                     // results (the pinned block, or device memory)
+};
+struct IcpJob {
+    liliom_ctx* c = nullptr;
+    IcpArgs a{};
+    int grid = 0;                        // the solo launch's blocks: min(nvb, co-resident k_icp_persistent blocks)
+    bool done = false;
+    PinIcp* dev_out = nullptr;           // the results in device memory when the pinned block is not mapped
+};
+int icp_begin(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,
+              double fit_eps, IcpJob& j);
+int icp_launch(const IcpJob& j);
+int icp_fetch(const IcpJob& j);
+void icp_finish(const IcpJob& j, double T16[16], double* fitness, int* converged, int* iters);
+// The ICP launches of the jobs `jobs` (none done) on c0's stream, every session's stream pointing at it (BatchStreams): sessions
+// share cooperative k_icp_batch launches, each with its solo grid; a session whose grid is not co-resident in k_icp_batch takes
+// icp_launch.  Then icp_fetch of every job.  Returns a whole-call CUDA error.
+int icp_batch_launch(liliom_ctx* c0, const std::vector<IcpJob*>& jobs);
 int map_install_host(liliom_ctx* c, const void* pts, int m, int stride, bool keep_refl);     // map.cu
 // liliom_map_update_resident of B distinct single-GPU contexts on one device (map.cu): status[i] = session i's result, n_map
 // (optional) its voxel count.  Returns a whole-call CUDA error.

@@ -49,13 +49,19 @@ __global__ void k_cell_run_ends(const uint32_t* __restrict__ keys, int n, int* _
     cell_run_ends_at(keys, n, cell_start, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
-// grid_build in parts (ctx.cuh: GridJob), shared with the batched map update: grid_begin decides the grid and sizes the buffers,
-// grid_sort / grid_clear / grid_scan are the library calls and the clear between the kernels, grid_finish takes the escape flag.
-int grid_begin(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_box, GridJob& j) {
+// grid_build in parts (ctx.cuh: GridJob), shared with the batched map update and loop closure: grid_begin decides the grid and
+// sizes the buffers (grid_begin_exact: from a box read back by the caller), grid_sort / grid_clear / grid_scan are the library
+// calls and the clear between the kernels, grid_finish takes the escape flag.
+static void grid_job_init(liliom_ctx* c, MapIndex& mi, float cell, int m, GridJob& j) {
     j = GridJob{};
     j.c = c; j.mi = &mi; j.cell = cell; j.m = m;
     mi.ready = false;
     mi.n = m;
+}
+static int grid_dims(liliom_ctx* c, MapIndex& mi, const int* h, GridJob& j);
+
+int grid_begin(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_box, GridJob& j) {
+    grid_job_init(c, mi, cell, m, j);
     if (m <= 0) {   // empty (shard of the) map: a 1-cell grid with no points, so that collective callers still run every launch
         GridDesc g{};
         g.inv_cell = 1.0f; g.dim[0] = g.dim[1] = g.dim[2] = 1; g.ncells = 1;
@@ -69,27 +75,36 @@ int grid_begin(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* host_b
         j.done = true;
         return LILIOM_OK;
     }
-    float4* pts = mi.xyzw.as<float4>();
-    int h[6];
     // A box handed in by the caller contains the raw points.  A voxel centroid (a sequential fp32 mean of such points) can leave
     // it by rounding, in which case its cell may not exist: k_cell_keys reports that, and the grid is rebuilt from the exact
     // min/max below.  (One cell of padding instead would be free of the re-run but can push the cell count over a power of
     // 256 and cost every rebuild a whole extra radix pass: 2^24 -> 17.7 M cells on the 10 M-point bench map, +90 us.)
     if (host_box) {
+        int h[6];
         for (int k = 0; k < 6; ++k) h[k] = host_box[k];
         if (c->test_shrink_box) h[3] = h[0];      // test hook: a box that is too small in x -> the escape path below must run
         LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
         j.escaped = c->vg_minmax.as<int>() + 7;
         LILI_CUDA(c, cudaMemsetAsync(j.escaped, 0, sizeof(int), c->stream));
-    } else {
-        LILI_TRY(vg_minmax_dev(c, pts, m, nullptr, sizeof(float4)));
-        int hb[kBoxInts];
-        LILI_TRY(read_back(c, {{hb, c->vg_minmax.p, sizeof(hb)}}));
-        if (hb[6] < m) { c->last_error = "non-finite map point"; return LILIOM_E_ARG; }      // the box counts finite points only
-        for (int k = 0; k < 6; ++k) h[k] = hb[k];
+        return grid_dims(c, mi, h, j);
     }
+    LILI_TRY(vg_minmax_dev(c, mi.xyzw.as<float4>(), m, nullptr, sizeof(float4)));
+    int hb[kBoxInts];
+    LILI_TRY(read_back(c, {{hb, c->vg_minmax.p, sizeof(hb)}}));
+    return grid_begin_exact(c, mi, cell, m, hb, j);
+}
+
+int grid_begin_exact(liliom_ctx* c, MapIndex& mi, float cell, int m, const int* hb, GridJob& j) {
+    grid_job_init(c, mi, cell, m, j);
+    if (hb[6] < m) { c->last_error = "non-finite map point"; return LILIOM_E_ARG; }      // the box counts finite points only
+    return grid_dims(c, mi, hb, j);
+}
+
+// the grid over the box h (6 ordered ints) and the buffers of the build
+static int grid_dims(liliom_ctx* c, MapIndex& mi, const int* h, GridJob& j) {
+    const int m = j.m;
     GridDesc g;
-    g.inv_cell = 1.0f / cell;
+    g.inv_cell = 1.0f / j.cell;
     long long nc = 1;
     for (int k = 0; k < 3; ++k) {
         float lo = vg_ord2f(h[k]), hi = vg_ord2f(h[3 + k]);

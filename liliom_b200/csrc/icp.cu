@@ -41,17 +41,6 @@ namespace lili {
 
 constexpr int kIcpBlock = 256;    // points per virtual block = threads per block
 
-struct IcpArgs {
-    const float4* src; int n, nvb;                   // source points (float4 xyz*), virtual blocks cdiv(n, 256)
-    const float4* map; const float4* map_orig; const int* cell_start; GridDesc g;
-    float max_d2;                                    // squared correspondence cut-off
-    int rmax, rmax_fit;                              // shells to visit at most: correspondence passes, the fitness pass
-    int max_iter; double trans_eps, fit_eps;
-    double* partials;                                // [2 parities][kIcpSums][nvb]
-    unsigned int* bar; int sync_mode;                // grid barrier word (zeroed before the launch), LILIOM_GN_SYNC
-    PinIcp* out;                                     // results (the pinned block, or device memory)
-};
-
 __device__ __forceinline__ void icp_run(const float4* __restrict__ map, int b, int e, float sx, float sy, float sz, u64& best) {
     for (int p = b; p < e; ++p) {
         const float4 m = __ldg(map + p);
@@ -142,14 +131,15 @@ __device__ __forceinline__ void icp_vblock(const IcpArgs& a, int vb, const doubl
 }
 
 // One pass over every virtual block under T, the grid barrier `phase`, and the fold of the partials in virtual-block order
-// 0..nvb-1 into sums[] (every block).
+// 0..nvb-1 into sums[] (every block).  blk: the block's place among its session's blocks (ctx.cuh).
+template <class Blk>
 __device__ __forceinline__ void icp_pass(const IcpArgs& a, const double* T, float max_d2, int rmax, int phase, double (*red)[kIcpSums],
-                                         double* sums) {
+                                         double* sums, const Blk blk) {
     double* part = a.partials + (size_t)(phase & 1) * kIcpSums * a.nvb;
-    for (int vb = blockIdx.x; vb < a.nvb; vb += gridDim.x) icp_vblock(a, vb, T, max_d2, rmax, part, red);
+    for (int vb = blk.bi(); vb < a.nvb; vb += blk.G()) icp_vblock(a, vb, T, max_d2, rmax, part, red);
     if (a.sync_mode == 0) __threadfence();
     __syncthreads();
-    if (threadIdx.x == 0) grid_barrier(a.bar, (unsigned int)(phase + 1) * gridDim.x, a.sync_mode, true);
+    if (threadIdx.x == 0) grid_barrier(a.bar, (unsigned int)(phase + 1) * blk.G(), a.sync_mode, true);
     __syncthreads();
     if (threadIdx.x < kIcpSums) {
         const double* p = part + (size_t)threadIdx.x * a.nvb;
@@ -161,7 +151,9 @@ __device__ __forceinline__ void icp_pass(const IcpArgs& a, const double* T, floa
     __syncthreads();
 }
 
-// The step of thread 0 out of line: its fp64 SVD and local arrays stay off the register budget of the search
+// The step of thread 0 out of line: its fp64 SVD and local arrays stay off the register budget of the search.  One copy per
+// kernel (Blk): ptxas allocates the registers of a function with a single caller around that caller.
+template <class Blk>
 __device__ __noinline__ int icp_step_dev(IcpState& st, const double* sums, int max_iter, double trans_eps, double fit_eps) {
     return icp_step(st, sums, max_iter, trans_eps, fit_eps);
 }
@@ -169,11 +161,10 @@ __device__ __noinline__ int icp_step_dev(IcpState& st, const double* sums, int m
 // The whole alignment in one cooperative launch (grid <= co-resident blocks; any grid gives the same bits).  The partials
 // alternate between two buffers by barrier parity: a block can only write phase p + 2's partials after every block has
 // arrived at barrier p + 1, i.e. after every block has folded phase p's.
-__global__ void __launch_bounds__(kIcpBlock) k_icp_persistent(const __grid_constant__ IcpArgs a) {
-    __shared__ double red[8][kIcpSums];
-    __shared__ double sums[kIcpSums];
-    __shared__ double T[12];                // rows 0..2 of F, the transform of the next pass
-    __shared__ int verdict;
+// The kernels declare the shared arrays (k_icp_persistent keeps its shared-memory layout): red[8][kIcpSums], sums[kIcpSums],
+// T[12] (rows 0..2 of F, the transform of the next pass), verdict.
+template <class Blk>
+__device__ __forceinline__ void icp_body(const IcpArgs& a, const Blk blk, double (*red)[kIcpSums], double* sums, double* T, int& verdict) {
     IcpState st;                            // thread 0's copy (the step is redundant across blocks)
     icp_init(st);
     if (threadIdx.x < 12) T[threadIdx.x] = st.F[threadIdx.x / 4][threadIdx.x % 4];
@@ -181,23 +172,43 @@ __global__ void __launch_bounds__(kIcpBlock) k_icp_persistent(const __grid_const
     int phase = 0;
 #pragma unroll 1
     while (true) {
-        icp_pass(a, T, a.max_d2, a.rmax, phase++, red, sums);
+        icp_pass(a, T, a.max_d2, a.rmax, phase++, red, sums, blk);
         if (threadIdx.x == 0) {
-            verdict = icp_step_dev(st, sums, a.max_iter, a.trans_eps, a.fit_eps);
+            verdict = icp_step_dev<Blk>(st, sums, a.max_iter, a.trans_eps, a.fit_eps);
             for (int k = 0; k < 12; ++k) T[k] = st.F[k / 4][k % 4];
         }
         __syncthreads();
         if (verdict != kIcpGo) break;
     }
     // getFitnessScore(): mean squared NN distance of every point of the aligned source, no cut-off
-    icp_pass(a, T, -1.0f, a.rmax_fit, phase, red, sums);
-    if (blockIdx.x == 0 && threadIdx.x == 0) {
+    icp_pass(a, T, -1.0f, a.rmax_fit, phase, red, sums, blk);
+    if (blk.bi() == 0 && threadIdx.x == 0) {
         for (int k = 0; k < 16; ++k) a.out->T[k] = st.F[k / 4][k % 4];
         a.out->fitness = icp_fitness(sums);
         a.out->converged = verdict == kIcpConverged ? 1 : 0;
         a.out->iters = st.it;
         __threadfence_system();
     }
+}
+
+__global__ void __launch_bounds__(kIcpBlock) k_icp_persistent(const __grid_constant__ IcpArgs a) {
+    __shared__ double red[8][kIcpSums];
+    __shared__ double sums[kIcpSums];
+    __shared__ double T[12];
+    __shared__ int verdict;
+    icp_body(a, SoloBlock{}, red, sums, T, verdict);
+}
+
+// Several sessions' alignments in one cooperative launch (liliom_loop_align_batch).  Session s owns blocks [off[s], off[s+1])
+// and runs exactly the body of its solo launch, with its own barrier word, partials and results; the cooperative launch only
+// guarantees that all blocks are resident.  The sessions meet no common barrier, so each ends after its own iterations.
+__global__ void __launch_bounds__(kIcpBlock, 1) k_icp_batch(const __grid_constant__ BatchTab<IcpArgs> tab) {
+    __shared__ double red[8][kIcpSums];
+    __shared__ double sums[kIcpSums];
+    __shared__ double T[12];
+    __shared__ int verdict;
+    const BatchSlot at = batch_slot(tab);
+    icp_body(tab.s[at.s], at.blk, red, sums, T, verdict);
 }
 
 // Largest float t with (double)t <= max_sqd: "d <= t" is then PCL's correspondence test, which rejects (double)d > max_dist_sqr
@@ -208,13 +219,12 @@ static float icp_cut_tau(double max_sqd) {
     return f;
 }
 
-// src (device float4, n points) against the index `tgt`; T16 row-major 4x4 out
-int icp_align(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,
-              double fit_eps, double T16[16], double* fitness, int* converged, int* iters) {
-    for (int k = 0; k < 16; ++k) T16[k] = (k % 5 == 0) ? 1.0 : 0.0;
-    *fitness = 0.0; *converged = 0; *iters = 0;
-    if (n <= 0 || tgt.n <= 0) return LILIOM_OK;
-    IcpArgs a{};
+int icp_begin(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,
+              double fit_eps, IcpJob& j) {
+    j = IcpJob{};
+    j.c = c;
+    if (n <= 0 || tgt.n <= 0) { j.done = true; return LILIOM_OK; }
+    IcpArgs& a = j.a;
     a.src = d_src; a.n = n; a.nvb = cdiv(n, kIcpBlock);
     a.map = tgt.sorted.as<float4>(); a.map_orig = tgt.xyzw.as<float4>(); a.cell_start = tgt.cell_start.as<int>(); a.g = tgt.grid;
     const float cell = 1.0f / tgt.grid.inv_cell;
@@ -225,24 +235,81 @@ int icp_align(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, do
     a.sync_mode = c->gn_sync;
     int per_sm = 0;
     LILI_CUDA(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_icp_persistent, kIcpBlock, 0));
-    const int grid = std::max(1, std::min(a.nvb, per_sm * c->sm_count));
+    j.grid = std::max(1, std::min(a.nvb, per_sm * c->sm_count));
     LILI_CUDA(c, c->partials.ensure((size_t)2 * kIcpSums * a.nvb * sizeof(double)));
     LILI_CUDA(c, c->icp_ctl.ensure(64 + sizeof(PinIcp)));
     LILI_CUDA(c, cudaMemsetAsync(c->icp_ctl.p, 0, sizeof(unsigned int), c->stream));
     a.partials = c->partials.as<double>();
     a.bar = c->icp_ctl.as<unsigned int>();
-    PinIcp* dev_out = reinterpret_cast<PinIcp*>(c->icp_ctl.as<unsigned char>() + 64);
-    a.out = c->h_pin_dev ? &c->h_pin_dev->icp : dev_out;
+    j.dev_out = reinterpret_cast<PinIcp*>(c->icp_ctl.as<unsigned char>() + 64);
+    a.out = c->h_pin_dev ? &c->h_pin_dev->icp : j.dev_out;
+    return LILIOM_OK;
+}
+
+int icp_launch(const IcpJob& j) {
+    liliom_ctx* c = j.c;
+    IcpArgs a = j.a;
     void* kargs[] = {&a};
-    LILI_CUDA(c, cudaLaunchCooperativeKernel((const void*)k_icp_persistent, dim3(grid), dim3(kIcpBlock), kargs, 0, c->stream));
-    LILI_TRY(launch_check(c, "k_icp_persistent"));
-    if (!c->h_pin_dev) LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->icp, dev_out, sizeof(PinIcp), cudaMemcpyDeviceToHost, c->stream));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    const PinIcp& r = c->h_pin->icp;
+    LILI_CUDA(c, cudaLaunchCooperativeKernel((const void*)k_icp_persistent, dim3(j.grid), dim3(kIcpBlock), kargs, 0, c->stream));
+    return launch_check(c, "k_icp_persistent");
+}
+
+int icp_fetch(const IcpJob& j) {
+    liliom_ctx* c = j.c;
+    if (!c->h_pin_dev) LILI_CUDA(c, cudaMemcpyAsync(&c->h_pin->icp, j.dev_out, sizeof(PinIcp), cudaMemcpyDeviceToHost, c->stream));
+    return LILIOM_OK;
+}
+
+void icp_finish(const IcpJob& j, double T16[16], double* fitness, int* converged, int* iters) {
+    for (int k = 0; k < 16; ++k) T16[k] = (k % 5 == 0) ? 1.0 : 0.0;
+    *fitness = 0.0; *converged = 0; *iters = 0;
+    if (j.done) return;
+    const PinIcp& r = j.c->h_pin->icp;
     for (int k = 0; k < 16; ++k) T16[k] = r.T[k];
     *fitness = r.fitness;
     *converged = r.converged;
     *iters = r.iters;
+}
+
+// src (device float4, n points) against the index `tgt`; T16 row-major 4x4 out
+int icp_align(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, double max_corr_dist, int max_iter, double trans_eps,
+              double fit_eps, double T16[16], double* fitness, int* converged, int* iters) {
+    IcpJob j;
+    j.done = true;
+    icp_finish(j, T16, fitness, converged, iters);      // identity until the results are in
+    LILI_TRY(icp_begin(c, tgt, d_src, n, max_corr_dist, max_iter, trans_eps, fit_eps, j));
+    if (!j.done) {
+        LILI_TRY(icp_launch(j));
+        LILI_TRY(icp_fetch(j));
+        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    }
+    icp_finish(j, T16, fitness, converged, iters);
+    return LILIOM_OK;
+}
+
+int icp_batch_launch(liliom_ctx* c0, const std::vector<IcpJob*>& jobs) {
+    if (jobs.empty()) return LILIOM_OK;
+    int occ = 0;
+    LILI_CUDA(c0, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_icp_batch, kIcpBlock, 0));
+    std::vector<BatchItem> items;
+    for (const IcpJob* j : jobs) {
+        const int cap = j->c->test_icp_blocks;
+        items.push_back(BatchItem{cap > 0 ? std::min(cap, j->grid) : j->grid, 0, true});
+    }
+    const BatchPack pack = batch_pack(items, &occ, c0->sm_count);
+    for (const BatchLaunch& l : pack.launches)
+        LILI_TRY(batch_tables<BatchTab<IcpArgs>>(l.sessions, [&](IcpArgs& e, int s) {
+            e = jobs[s]->a;
+            e.sync_mode = c0->gn_sync;          // launch-wide, as the batched GN step's
+            return BatchPart{jobs[s]->c, items[s].grid};
+        }, [&](BatchTab<IcpArgs>& tab, int grid) -> int {
+            void* kargs[] = {&tab};
+            LILI_CUDA(c0, cudaLaunchCooperativeKernel((const void*)k_icp_batch, dim3(grid), dim3(kIcpBlock), kargs, 0, c0->stream));
+            LILI_CUDA(c0, cudaGetLastError());
+            return LILIOM_OK;
+        }));
+    for (int s : pack.solo) LILI_TRY(icp_launch(*jobs[s]));
+    for (const IcpJob* j : jobs) LILI_TRY(icp_fetch(*j));
     return LILIOM_OK;
 }
 

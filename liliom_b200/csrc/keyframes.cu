@@ -4,7 +4,8 @@
 //   local map        buildLocalMapWithLandMark (:1387-1484) + downSampleCloud, map half (:1486-1492): transform + concatenate
 //                    the listed keyframes in ONE launch, VoxelGrid per layer, a cell grid per layer (MapIndex)
 //   loop closure     detectLoopClosure's clouds (:2473-2547): edge then surf per keyframe, transformed, VoxelGrid; with
-//                    performLoopClosure's ICP (:2552-2582) on them in the same call (liliom_loop_align)
+//                    performLoopClosure's ICP (:2552-2582) on them in the same call (liliom_loop_align); several sessions' in one call
+//                    (liliom_loop_align_batch)
 //   full clouds      downSampleCloud, full-cloud half (:1494-1500; R:1373-1376): the /full_point_cloud of a keyframe, stored
 //   global map       publishCompleteMap (:2644-2685) and save_pcd's map (:2703-2718): listed keyframes transformed, concatenated,
 //                    VoxelGrid, in a VoxelGrid that reads the store through the keyframe table (kf_table.h): no concatenation
@@ -23,14 +24,33 @@ static dim3 kf_row_grid(size_t rows, long long largest, int bx_max, int by_max =
     return dim3(std::max(1, std::min(cdiv(largest, 256), bx_max)), (unsigned)std::min<size_t>(rows, by_max));
 }
 
-// the transformed concatenation of the rows
-__global__ void k_kf_gather(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride,
-                            unsigned char* __restrict__ out) {
-    for (int y = blockIdx.y; y < rows; y += gridDim.y) {
+// the transformed concatenation of the rows, block `blk` of its grid: the solo launch's own 2-D grid (KfGridSolo), or the flattened
+// one of a session in the batched loop closure (KfGridAt)
+struct KfGridSolo {
+    __device__ __forceinline__ unsigned int bx() const { return blockIdx.x; }
+    __device__ __forceinline__ unsigned int by() const { return blockIdx.y; }
+    __device__ __forceinline__ unsigned int gx() const { return gridDim.x; }
+    __device__ __forceinline__ unsigned int gy() const { return gridDim.y; }
+};
+struct KfGridAt {
+    unsigned int x, y, w, h;
+    __device__ __forceinline__ unsigned int bx() const { return x; }
+    __device__ __forceinline__ unsigned int by() const { return y; }
+    __device__ __forceinline__ unsigned int gx() const { return w; }
+    __device__ __forceinline__ unsigned int gy() const { return h; }
+};
+template <class Grid>
+__device__ __forceinline__ void kf_gather_at(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride,
+                                             unsigned char* __restrict__ out, const Grid blk) {
+    for (int y = blk.by(); y < rows; y += blk.gy()) {
         const KfRow& r = tab[y];
-        for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < r.n; i += gridDim.x * blockDim.x)
+        for (int i = blk.bx() * blockDim.x + threadIdx.x; i < r.n; i += blk.gx() * blockDim.x)
             kf_row_point(r, arena + (size_t)(r.src_off + i) * stride, stride, out + (size_t)(r.dst_off + i) * stride);
     }
+}
+__global__ void k_kf_gather(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride,
+                            unsigned char* __restrict__ out) {
+    kf_gather_at(arena, tab, rows, stride, out, KfGridSolo{});
 }
 
 // box (vg_box.h) of the finite transformed points of the rows, joined into mm
@@ -145,18 +165,26 @@ static KfRow kf_row(long long src, long long dst, int n, const double* pose7, co
 // detectLoopClosure's cloud of the listed keyframes (:2476-2497, :2502-2547): edge then surf of each, transformed by its pose,
 // concatenated into bmap_raw (one launch), VoxelGrid(leaf) into vg_out with its count at d_count (device) and *m (host).
 // *n_in: the points read (0: nothing was launched, d_count is not written and *m = 0).
-static int kf_cloud_dev(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, float leaf, int* d_count, long long* n_in, int* m) {
-    const int stride = c->prm.point_stride;
-    std::vector<KfRow> tab;
-    long long off = 0, largest = 0;
+// The rows of such a cloud appended to tab (destinations from 0); returns its points, *largest = the largest keyframe cloud.
+static long long kf_cloud_rows(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, std::vector<KfRow>& tab, long long* largest) {
+    long long off = 0;
+    *largest = 0;
     for (int i = 0; i < k; ++i) {                                 // :2492-2493 / :2519-2520: *edge_frames[i] then *surf_frames[i]
         const KfEntry& f = c->kfs[kf_ids[i]];
         if (f.n_edge) tab.push_back(kf_row(f.edge_off, off, f.n_edge, poses7 + 7 * (size_t)i));
         off += f.n_edge;
         if (f.n_surf) tab.push_back(kf_row(f.surf_off, off, f.n_surf, poses7 + 7 * (size_t)i));
         off += f.n_surf;
-        largest = std::max(largest, (long long)std::max(f.n_edge, f.n_surf));
+        *largest = std::max(*largest, (long long)std::max(f.n_edge, f.n_surf));
     }
+    return off;
+}
+
+static int kf_cloud_dev(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, float leaf, int* d_count, long long* n_in, int* m) {
+    const int stride = c->prm.point_stride;
+    std::vector<KfRow> tab;
+    long long largest = 0;
+    const long long off = kf_cloud_rows(c, kf_ids, poses7, k, tab, &largest);
     *n_in = off;
     *m = 0;
     if (off == 0) return LILIOM_OK;
@@ -319,33 +347,310 @@ extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* p
 // detectLoopClosure + performLoopClosure's alignment (:2473-2582) without leaving the device: the history cloud goes into the
 // loop index (its own cell grid: the odometry map, the local map and every resident correspondence stay), the latest cloud into
 // loop_src, and the ICP runs on them (icp.cu).  Scratch shared with the other calls: bmap_raw, vg_out, the sort chain, grid_keys*,
-// partials.  Two stream synchronises: the cloud sizes (the grid build needs the target's on the host), and the grid's box.
-extern "C" int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids,
-                                 const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps,
-                                 double fit_eps, double T16[16], double* fitness, int* converged, int* iters, int* n_src, int* n_tgt) {
-    if (!c || k_src < 0 || k_tgt < 0 || (k_src > 0 && (!src_ids || !src_poses7)) || (k_tgt > 0 && (!tgt_ids || !tgt_poses7)) ||
-        !(leaf > 0) || !(max_corr_dist > 0) || max_iter < 1 || !T16 || !fitness || !converged || !iters)
+// partials.  The call is written in parts so that the solo call and the batched one (liliom_loop_align_batch) run the same
+// code: loop_begin, then per cloud the gather, the VoxelGrid chain and the repack, then grid_begin .. grid_finish of the
+// target's cell grid, then icp_begin .. icp_finish.
+namespace lili {
+
+struct LoopJob {
+    liliom_ctx* c = nullptr;
+    int rows[2] = {0, 0};                // keyframe table rows of the target [0] and the source [1]; the source's follow the target's
+    long long off[2] = {0, 0};           // points of each concatenation
+    long long largest[2] = {0, 0};       // the largest keyframe cloud of each (the gather's grid)
+    float leaf = 0.0f;
+    double max_corr_dist = 0.0, trans_eps = 0.0, fit_eps = 0.0;
+    int max_iter = 0;
+    int m[2] = {0, 0};                   // VoxelGrid output counts
+    GridJob g;
+    IcpJob icp;
+};
+
+static float loop_cell(const liliom_ctx* c) { return gate_cell(c->prm.knn_max_sqdist); }   // the cell of liliom_icp_align's target
+static float4* loop_dst(liliom_ctx* c, int k) { return k == 0 ? c->loop.xyzw.as<float4>() : c->loop_src.as<float4>(); }
+
+// Validation (nothing changes on an error), the keyframe tables of both clouds in one upload (so that both stay valid until
+// their gathers have run) and every buffer of the clouds' chains.
+static int loop_begin(liliom_ctx* c, const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids, const double* tgt_poses7,
+                      int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps, double fit_eps, LoopJob& j) {
+    if (k_src < 0 || k_tgt < 0 || (k_src > 0 && (!src_ids || !src_poses7)) || (k_tgt > 0 && (!tgt_ids || !tgt_poses7)) ||
+        !(leaf > 0) || !(max_corr_dist > 0) || max_iter < 1)
         return LILIOM_E_ARG;
     LILI_TRY(backend_check(c, nullptr));
     if (!kf_ids_ok(c, src_ids, k_src) || !kf_ids_ok(c, tgt_ids, k_tgt)) return LILIOM_E_ARG;     // before anything changes
     LILI_CUDA(c, cudaSetDevice(c->device));
+    j = LoopJob{};
+    j.c = c; j.leaf = leaf; j.max_corr_dist = max_corr_dist; j.max_iter = max_iter; j.trans_eps = trans_eps; j.fit_eps = fit_eps;
+    std::vector<KfRow> tab;
+    // :2502-2547 his_key_frames_ds (the target), :2476-2497 latest_key_frames_ds (the source)
+    j.off[0] = kf_cloud_rows(c, tgt_ids, tgt_poses7, k_tgt, tab, &j.largest[0]);
+    j.rows[0] = (int)tab.size();
+    j.off[1] = kf_cloud_rows(c, src_ids, src_poses7, k_src, tab, &j.largest[1]);
+    j.rows[1] = (int)tab.size() - j.rows[0];
+    const long long n = std::max(j.off[0], j.off[1]);
     const int stride = c->prm.point_stride;
     LILI_CUDA(c, c->vg_count.ensure(16));
-    int* cnt = c->vg_count.as<int>();
-    long long off_t = 0, off_s = 0;
-    int m_t = 0, m_s = 0;
-    // :2502-2547 his_key_frames_ds -> the loop index's points (float4, w = index), as liliom_icp_align installs a target
-    LILI_TRY(kf_cloud_dev(c, tgt_ids, tgt_poses7, k_tgt, leaf, cnt, &off_t, &m_t));
-    LILI_CUDA(c, c->loop.xyzw.ensure((size_t)std::max(off_t, 1LL) * sizeof(float4)));
-    LILI_TRY(repack_to_f4(c, c->vg_out.p, (int)off_t, stride, c->loop.xyzw.as<float4>(), cnt));
-    // :2476-2497 latest_key_frames_ds -> the source
-    LILI_TRY(kf_cloud_dev(c, src_ids, src_poses7, k_src, leaf, cnt + 1, &off_s, &m_s));
-    LILI_CUDA(c, c->loop_src.ensure((size_t)std::max(off_s, 1LL) * sizeof(float4)));
-    LILI_TRY(repack_to_f4(c, c->vg_out.p, (int)off_s, stride, c->loop_src.as<float4>(), cnt + 1));
-    if (n_src) *n_src = m_s;
-    if (n_tgt) *n_tgt = m_t;
-    LILI_TRY(grid_build(c, c->loop, gate_cell(c->prm.knn_max_sqdist), m_t));      // the cell of liliom_icp_align's target
-    return icp_align(c, c->loop, c->loop_src.as<float4>(), m_s, max_corr_dist, max_iter, trans_eps, fit_eps, T16, fitness, converged, iters);
+    if (n > 0) {
+        LILI_TRY(kf_upload_table(c, tab));
+        LILI_CUDA(c, c->bmap_raw.ensure((size_t)n * stride));   // scratch: the local map's layers live in bmap_ds / bmap
+        c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
+        LILI_CUDA(c, c->vg_out.ensure((size_t)n * stride));
+        LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));       // voxelgrid_dev's buffers at 32-bit keys
+        LILI_CUDA(c, c->vg_params.ensure(sizeof(VgParams)));
+        LILI_CUDA(c, c->vg_keys.ensure((size_t)n * 4));
+        LILI_CUDA(c, c->vg_vals.ensure((size_t)n * 4));
+        LILI_CUDA(c, c->vg_keys2.ensure((size_t)n * 4));
+        LILI_CUDA(c, c->vg_vals2.ensure((size_t)n * 4));
+        LILI_CUDA(c, c->vg_flags.ensure(((size_t)n + 2) * 4));
+        LILI_CUDA(c, c->vg_rank.ensure(((size_t)n + 2) * 4));
+    }
+    LILI_CUDA(c, c->loop.xyzw.ensure((size_t)std::max(j.off[0], 1LL) * sizeof(float4)));
+    LILI_CUDA(c, c->loop_src.ensure((size_t)std::max(j.off[1], 1LL) * sizeof(float4)));
+    return LILIOM_OK;
+}
+
+// the gather's grid for cloud k (kf_row_grid)
+static dim3 loop_gather_grid(const LoopJob& j, int k) { return kf_row_grid(j.rows[k], j.largest[k], j.c->sm_count * 4); }
+static const KfRow* loop_rows(const LoopJob& j, int k) { return j.c->kf_tab.as<KfRow>() + (k == 0 ? 0 : j.rows[0]); }
+
+// Cloud k (0 target, 1 source) on the solo path: gather, VoxelGrid with its count read back (voxelgrid_dev_sync: wide keys where
+// the index wraps), repack into the loop index's points or loop_src (the count read on the device).
+static int loop_cloud(LoopJob& j, int k) {
+    liliom_ctx* c = j.c;
+    const int stride = c->prm.point_stride;
+    int* cnt = c->vg_count.as<int>() + k;
+    if (j.off[k] > 0) {
+        k_kf_gather<<<loop_gather_grid(j, k), 256, 0, c->stream>>>((const unsigned char*)c->kf_arena.p, loop_rows(j, k), j.rows[k], stride,
+                                                                   (unsigned char*)c->bmap_raw.p);
+        LILI_TRY(launch_check(c, "k_kf_gather"));
+        LILI_TRY(voxelgrid_dev_sync(c, c->bmap_raw.p, (int)j.off[k], stride, j.leaf, c->vg_out.p, cnt, nullptr, &j.m[k]));
+    }
+    return repack_to_f4(c, c->vg_out.p, (int)j.off[k], stride, loop_dst(c, k), cnt);
+}
+
+static int loop_icp_begin(LoopJob& j) {
+    liliom_ctx* c = j.c;
+    return icp_begin(c, c->loop, c->loop_src.as<float4>(), j.m[1], j.max_corr_dist, j.max_iter, j.trans_eps, j.fit_eps, j.icp);
+}
+
+// ---- the loop closure of several sessions (liliom_loop_align_batch): one launch per stage for up to kBatchMax sessions.
+// Everything one session's stages read or write, on its own buffers.
+struct LoopEntry {
+    // a cloud: the gather of its table rows into bmap_raw, the VoxelGrid chain of its n points into vg_out, the repack into xyzw
+    const unsigned char* arena; const KfRow* tab; int rows, gx, gy;
+    const unsigned char* raw; unsigned char* raw_out; int n, stride; float leaf; int* mm; int mm_blocks; VgParams* pp;
+    uint32_t* keys; int* vals; const uint32_t* keys2; const int* vals2; int* flags; int* rank; unsigned char* ds; int* count;
+    float4* xyzw;
+    // the target's cell grid over its m points
+    int m; GridDesc g; uint32_t* gkeys; int* gvals; float4* sorted; int* cell_start;
+};
+
+// The stages (k_stage_batch, ctx.cuh), each with the block size, the blocks and the body of its solo launch
+LILI_STAGE(LoopStGather, LoopEntry, 256, e.gx * e.gy, kf_gather_at(e.arena, e.tab, e.rows, e.stride, e.raw_out, KfGridAt{(unsigned)(bx % e.gx), (unsigned)(bx / e.gx), (unsigned)e.gx, (unsigned)e.gy}))
+LILI_STAGE(LoopStBoxInit, LoopEntry, 32, 1, vg_box_init(e.mm))
+LILI_STAGE(LoopStBox, LoopEntry, 256, e.mm_blocks, vg_minmax_body(e.raw, e.n, nullptr, e.stride, e.mm, SessionBlock{bx, (unsigned)e.mm_blocks}))
+LILI_STAGE(LoopStParams, LoopEntry, 32, 1, vg_params_at(e.mm, e.leaf, e.pp))
+LILI_STAGE(LoopStKeys, LoopEntry, 256, stage_blocks(e.n, 256), vg_keys_at<uint32_t>(e.raw, e.n, nullptr, e.stride, e.pp, e.keys, e.vals, i))
+LILI_STAGE(LoopStHeads, LoopEntry, 256, stage_blocks(e.n + 1, 256), vg_heads_at(e.keys2, e.n, &e.pp->n_finite, e.flags, i))
+LILI_STAGE(LoopStCentroid48, LoopEntry, 128, stage_blocks(e.n, 128),
+           (vg_centroid_at<48, uint32_t>)(e.raw, e.keys2, e.vals2, e.flags, e.rank, e.n, nullptr, e.pp, e.ds, e.count, nullptr, i))
+LILI_STAGE(LoopStCentroid32, LoopEntry, 128, stage_blocks(e.n, 128),
+           (vg_centroid_at<32, uint32_t>)(e.raw, e.keys2, e.vals2, e.flags, e.rank, e.n, nullptr, e.pp, e.ds, e.count, nullptr, i))
+LILI_STAGE(LoopStRepack, LoopEntry, 256, stage_blocks(e.n, 256), repack_f4_at(e.ds, e.n, e.count, e.stride, e.xyzw, i))
+LILI_STAGE(LoopStGridBox, LoopEntry, 256, e.mm_blocks,
+           vg_minmax_body((const unsigned char*)e.xyzw, e.m, nullptr, (int)sizeof(float4), e.mm, SessionBlock{bx, (unsigned)e.mm_blocks}))
+LILI_STAGE(LoopStCellKeys, LoopEntry, 256, stage_blocks(e.m, 256), cell_keys_at(e.xyzw, e.m, e.g, e.gkeys, e.gvals, nullptr, i))
+LILI_STAGE(LoopStGatherSorted, LoopEntry, 256, stage_blocks(e.m, 256), gather_sorted_at(e.xyzw, e.vals2, e.m, e.sorted, i))
+LILI_STAGE(LoopStRunEnds, LoopEntry, 256, stage_blocks(e.m, 256), cell_run_ends_at(e.keys2, e.m, e.cell_start, i))
+
+// Session j's entry for cloud k (0 target, 1 source), as loop_cloud's launches take their arguments
+static LoopEntry loop_cloud_entry(const LoopJob& j, int k) {
+    liliom_ctx* c = j.c;
+    LoopEntry e{};
+    const dim3 gg = loop_gather_grid(j, k);
+    e.arena = (const unsigned char*)c->kf_arena.p; e.tab = loop_rows(j, k); e.rows = j.rows[k]; e.gx = (int)gg.x; e.gy = (int)gg.y;
+    e.raw = e.raw_out = (unsigned char*)c->bmap_raw.p; e.n = (int)j.off[k]; e.stride = c->prm.point_stride; e.leaf = j.leaf;
+    e.mm = c->vg_minmax.as<int>(); e.mm_blocks = box_blocks(e.n, c->sm_count); e.pp = c->vg_params.as<VgParams>();
+    e.keys = c->vg_keys.as<uint32_t>(); e.vals = c->vg_vals.as<int>(); e.keys2 = c->vg_keys2.as<uint32_t>(); e.vals2 = c->vg_vals2.as<int>();
+    e.flags = c->vg_flags.as<int>(); e.rank = c->vg_rank.as<int>(); e.ds = (unsigned char*)c->vg_out.p; e.count = c->vg_count.as<int>() + k;
+    e.xyzw = loop_dst(c, k);
+    return e;
+}
+// ... and for the target's cell grid (grid_build's launches; grid_begin has sized it)
+static LoopEntry loop_grid_entry(const LoopJob& j) {
+    liliom_ctx* c = j.c;
+    LoopEntry e{};
+    e.xyzw = c->loop.xyzw.as<float4>(); e.m = j.m[0]; e.mm = c->vg_minmax.as<int>(); e.mm_blocks = box_blocks(e.m, c->sm_count);
+    e.g = c->loop.grid; e.gkeys = c->grid_keys.as<uint32_t>(); e.gvals = c->grid_vals.as<int>();
+    e.keys2 = c->grid_keys2.as<uint32_t>(); e.vals2 = c->grid_vals2.as<int>(); e.sorted = c->loop.sorted.as<float4>();
+    e.cell_start = c->loop.cell_start.as<int>();
+    return e;
+}
+
+namespace {
+
+template <class St, class Make>
+int loop_stage(liliom_ctx* c0, std::vector<LoopJob>& J, const std::vector<int>& which, Make make) {
+    return stage_batch<St>(c0, which, [&](LoopEntry& e, int i) { e = make(J[i]); return J[i].c; });
+}
+
+// The shared phases of loop_align_batch, every session's stream pointing at c0's.  Each phase: the solo call's host part per
+// session, the stage launches for all of them, every session's read-back words into its own pinned block, ONE synchronise.
+// wide[i]: session i's index wrapped in one of its clouds (vg_wide_keys); it leaves the shared path after phase 1.
+int loop_batch_run(liliom_ctx* c0, std::vector<LoopJob>& J, std::vector<char>& live, std::vector<char>& wide, liliom_loop_result* res,
+                   int* status) {
+    const int B = (int)J.size();
+    auto fail = [&](int i, int rc) { status[i] = rc; live[i] = 0; };
+    auto sel = [&](auto pred) {
+        std::vector<int> v;
+        for (int i = 0; i < B; ++i) if (live[i] && pred(J[i])) v.push_back(i);
+        return v;
+    };
+    auto copy_back = [&](int i, size_t at, const void* src, size_t bytes) {
+        if (cudaError_t err = cudaMemcpyAsync(J[i].c->h_pin->scratch + at, src, bytes, cudaMemcpyDeviceToHost, c0->stream); err != cudaSuccess)
+            fail(i, fail_cuda(J[i].c, err, "loop closure batch: read-back"));
+    };
+    // 1. both clouds of every session (target, then source: they share bmap_raw, vg_out and the sort chain) -> counts, VgParams
+    for (int k = 0; k < 2; ++k) {
+        auto has = [k](const LoopJob& j) { return j.off[k] > 0; };
+        auto cloud = [k](const LoopJob& j) { return loop_cloud_entry(j, k); };
+        LILI_TRY(loop_stage<LoopStGather>(c0, J, sel(has), cloud));
+        LILI_TRY(loop_stage<LoopStBoxInit>(c0, J, sel(has), cloud));
+        LILI_TRY(loop_stage<LoopStBox>(c0, J, sel(has), cloud));
+        LILI_TRY(loop_stage<LoopStParams>(c0, J, sel(has), cloud));
+        LILI_TRY(loop_stage<LoopStKeys>(c0, J, sel(has), cloud));
+        for (int i : sel(has)) {
+            liliom_ctx* c = J[i].c;
+            if (const int rc = sort_pairs_u32(c, c->vg_keys.as<uint32_t>(), c->vg_keys2.as<uint32_t>(), c->vg_vals.as<int>(), c->vg_vals2.as<int>(),
+                                              (int)J[i].off[k], 32); rc != LILIOM_OK)
+                fail(i, rc);
+        }
+        LILI_TRY(loop_stage<LoopStHeads>(c0, J, sel(has), cloud));
+        for (int i : sel(has))
+            if (const int rc = exclusive_scan_i32(J[i].c, J[i].c->vg_flags.as<int>(), J[i].c->vg_rank.as<int>(), (int)J[i].off[k]); rc != LILIOM_OK)
+                fail(i, rc);
+        LILI_TRY(loop_stage<LoopStCentroid48>(c0, J, sel([k](const LoopJob& j) { return j.off[k] > 0 && j.c->prm.point_stride == 48; }), cloud));
+        LILI_TRY(loop_stage<LoopStCentroid32>(c0, J, sel([k](const LoopJob& j) { return j.off[k] > 0 && j.c->prm.point_stride != 48; }), cloud));
+        LILI_TRY(loop_stage<LoopStRepack>(c0, J, sel(has), cloud));
+        for (int i : sel(has)) copy_back(i, k * sizeof(VgParams), J[i].c->vg_params.p, sizeof(VgParams));
+    }
+    for (int i : sel([](const LoopJob& j) { return j.off[0] > 0 || j.off[1] > 0; }))
+        copy_back(i, 2 * sizeof(VgParams), J[i].c->vg_count.p, 2 * sizeof(int));
+    LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+    for (int i : sel([](const LoopJob&) { return true; })) {
+        const unsigned char* s = J[i].c->h_pin->scratch;
+        for (int k = 0; k < 2; ++k) {
+            if (J[i].off[k] <= 0) continue;
+            VgParams vp;
+            memcpy(&vp, s + k * sizeof(VgParams), sizeof(VgParams));
+            memcpy(&J[i].m[k], s + 2 * sizeof(VgParams) + k * sizeof(int), sizeof(int));
+            if (vg_wide_keys(vp)) { wide[i] = 1; live[i] = 0; }      // the solo path redoes this cloud with wide keys
+        }
+        if (live[i]) { res[i].n_src = J[i].m[1]; res[i].n_tgt = J[i].m[0]; }
+    }
+    // 2. the targets' boxes -> every session's cell grid (grid_begin)
+    {
+        auto has = [](const LoopJob& j) { return j.m[0] > 0; };
+        LILI_TRY(loop_stage<LoopStBoxInit>(c0, J, sel(has), loop_grid_entry));
+        LILI_TRY(loop_stage<LoopStGridBox>(c0, J, sel(has), loop_grid_entry));
+        for (int i : sel(has)) copy_back(i, 0, J[i].c->vg_minmax.p, kBoxInts * sizeof(int));
+        LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+        for (int i : sel([](const LoopJob&) { return true; })) {
+            LoopJob& j = J[i];
+            liliom_ctx* c = j.c;
+            int hb[kBoxInts];
+            memcpy(hb, c->h_pin->scratch, sizeof(hb));
+            const int rc = j.m[0] > 0 ? grid_begin_exact(c, c->loop, loop_cell(c), j.m[0], hb, j.g) : grid_begin(c, c->loop, loop_cell(c), 0, nullptr, j.g);
+            if (rc != LILIOM_OK) { fail(i, rc); continue; }
+            if (const int rc2 = loop_icp_begin(j); rc2 != LILIOM_OK) fail(i, rc2);
+        }
+    }
+    // 3. the targets' cell grids, the ICP launches -> every session's results
+    {
+        auto grid = [](const LoopJob& j) { return !j.g.done; };
+        LILI_TRY(loop_stage<LoopStCellKeys>(c0, J, sel(grid), loop_grid_entry));
+        for (int i : sel(grid)) if (const int rc = grid_sort(J[i].g); rc != LILIOM_OK) fail(i, rc);
+        LILI_TRY(loop_stage<LoopStGatherSorted>(c0, J, sel(grid), loop_grid_entry));
+        for (int i : sel(grid)) if (const int rc = grid_clear(J[i].g); rc != LILIOM_OK) fail(i, rc);
+        LILI_TRY(loop_stage<LoopStRunEnds>(c0, J, sel(grid), loop_grid_entry));
+        for (int i : sel(grid)) if (const int rc = grid_scan(J[i].g); rc != LILIOM_OK) fail(i, rc);
+        for (int i : sel(grid)) if (const int rc = grid_finish(J[i].g, 0); rc != LILIOM_OK) fail(i, rc);
+        std::vector<IcpJob*> jobs;
+        for (int i : sel([](const LoopJob& j) { return !j.icp.done; })) jobs.push_back(&J[i].icp);
+        LILI_TRY(icp_batch_launch(c0, jobs));
+        LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+        for (int i : sel([](const LoopJob&) { return true; })) {
+            liliom_loop_result& r = res[i];
+            icp_finish(J[i].icp, r.T16, &r.fitness, &r.converged, &r.iters);
+            status[i] = LILIOM_OK;
+        }
+    }
+    return LILIOM_OK;
+}
+
+}  // namespace
+
+// liliom_loop_align of several sessions.  Shared launches and waits on cs[0]'s stream (the other sessions' streams joined before
+// and after with events); every buffer, library sort and scan and host decision stays the session's own, made by the solo
+// call's parts from the session's own read-back words.
+int loop_align_batch(liliom_ctx* const* cs, int B, const int* const* src_ids, const double* const* src_poses7, const int* k_src,
+                     const int* const* tgt_ids, const double* const* tgt_poses7, const int* k_tgt, const liliom_loop_params* prm,
+                     liliom_loop_result* res, int* status) {
+    liliom_ctx* c0 = cs[0];
+    std::vector<LoopJob> J(B);
+    std::vector<char> live(B, 0), wide(B, 0);
+    std::vector<std::pair<unsigned long long, unsigned long long>> launches0(B);
+    const std::vector<liliom_ctx*> all(cs, cs + B);
+    LILI_TRY(batch_join_in(c0, all));
+    int rc;
+    {
+        const BatchStreams on_c0(all, c0->stream);
+        for (int i = 0; i < B; ++i) {
+            const liliom_loop_params& p = prm[i];
+            launches0[i] = {cs[i]->cnt.launches, cs[i]->cnt.lib_launches};
+            status[i] = loop_begin(cs[i], src_ids[i], src_poses7[i], k_src[i], tgt_ids[i], tgt_poses7[i], k_tgt[i], p.leaf, p.max_corr_dist,
+                                   p.max_iter, p.trans_eps, p.fit_eps, J[i]);
+            live[i] = status[i] == LILIOM_OK;
+        }
+        rc = loop_batch_run(c0, J, live, wide, res, status);
+        // sessions whose index wrapped finish on their solo path, which takes the wide keys: the whole solo call, its counters
+        // counted from where the batch found them (what this call launched for the session is redone there)
+        for (int i = 0; rc == LILIOM_OK && i < B; ++i) {
+            if (!wide[i]) continue;
+            liliom_ctx* c = cs[i];
+            c->cnt.launches = launches0[i].first; c->cnt.lib_launches = launches0[i].second;
+            const liliom_loop_params& p = prm[i];
+            liliom_loop_result& r = res[i];
+            status[i] = liliom_loop_align(c, src_ids[i], src_poses7[i], k_src[i], tgt_ids[i], tgt_poses7[i], k_tgt[i], p.leaf, p.max_corr_dist,
+                                          p.max_iter, p.trans_eps, p.fit_eps, r.T16, &r.fitness, &r.converged, &r.iters, &r.n_src, &r.n_tgt);
+        }
+    }
+    LILI_TRY(batch_join_out(c0, all));
+    return rc;
+}
+
+}  // namespace lili
+
+extern "C" int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids,
+                                 const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps,
+                                 double fit_eps, double T16[16], double* fitness, int* converged, int* iters, int* n_src, int* n_tgt) {
+    if (!c || !T16 || !fitness || !converged || !iters) return LILIOM_E_ARG;
+    LoopJob j;
+    LILI_TRY(loop_begin(c, src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter, trans_eps, fit_eps, j));
+    LILI_TRY(loop_cloud(j, 0));      // :2502-2547 his_key_frames_ds -> the loop index's points (float4, w = index)
+    LILI_TRY(loop_cloud(j, 1));      // :2476-2497 latest_key_frames_ds -> the source
+    if (n_src) *n_src = j.m[1];
+    if (n_tgt) *n_tgt = j.m[0];
+    LILI_TRY(grid_build(c, c->loop, loop_cell(c), j.m[0]));
+    return icp_align(c, c->loop, c->loop_src.as<float4>(), j.m[1], max_corr_dist, max_iter, trans_eps, fit_eps, T16, fitness, converged, iters);
+}
+
+extern "C" int liliom_loop_align_batch(liliom_ctx* const* ctxs, int B, const int* const* src_ids, const double* const* src_poses7,
+                                       const int* k_src, const int* const* tgt_ids, const double* const* tgt_poses7, const int* k_tgt,
+                                       const liliom_loop_params* prm, liliom_loop_result* res, int* status) {
+    if (!batch_ctxs_ok(ctxs, B) || !src_ids || !src_poses7 || !k_src || !tgt_ids || !tgt_poses7 || !k_tgt || !prm || !res || !status)
+        return LILIOM_E_ARG;
+    LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
+    return loop_align_batch(ctxs, B, src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, prm, res, status);
 }
 
 extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp, int kf_id, const void* full, int n, int* n_stored) {

@@ -24,27 +24,18 @@ __global__ void k_vg_minmax(const unsigned char* __restrict__ pts, int n_max, co
 struct VgBox { int mm[kBoxInts]; };      // a box (vg_box.h) by value
 
 __global__ void k_vg_params(const int* __restrict__ mm, float leaf, VgParams* __restrict__ out) {
-    if (threadIdx.x == 0) *out = vg_params(mm, leaf);
+    vg_params_at(mm, leaf, out);
 }
 // the bounding box is already known on the host (map rebuild: the union of the frames' boxes, kept since their push)
 __global__ void k_vg_params_box(const VgBox b, float leaf, VgParams* __restrict__ out) {
     if (threadIdx.x == 0) *out = vg_params(b.mm, leaf);
 }
 
-// K = uint32_t: non-finite points take the all-ones key; K = unsigned long long (wide keys, vg_wide_keys): the flag at bit 32
+// the key and centroid kernels: bodies in ctx.cuh (the batched loop closure runs them too)
 template <typename K>
 __global__ void k_vg_keys(const unsigned char* __restrict__ pts, int n_max, const int* __restrict__ d_n, int stride, const VgParams* __restrict__ pp,
                           K* __restrict__ keys, int* __restrict__ vals) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_max) return;
-    const int n = d_n ? min(*d_n, n_max) : n_max;
-    const VgParams p = *pp;
-    float4 v = make_float4(NAN, 0.f, 0.f, 0.f);
-    if (i < n) v = *reinterpret_cast<const float4*>(pts + (size_t)i * stride);
-    K key = sizeof(K) == 4 ? (K)0xffffffffu : (K)(1ull << 32);
-    if (isfinite(v.x) && isfinite(v.y) && isfinite(v.z)) key = vg_rel_index(p, v.x, v.y, v.z);
-    keys[i] = key;
-    vals[i] = i;
+    vg_keys_at<K>(pts, n_max, d_n, stride, pp, keys, vals, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
 template <int STRIDE, typename K>
@@ -52,26 +43,7 @@ __global__ void k_vg_centroid(const unsigned char* __restrict__ pts, const K* __
                               const int* __restrict__ flags, const int* __restrict__ rank, int n_max, const int* __restrict__ d_n,
                               const VgParams* __restrict__ pp, unsigned char* __restrict__ out, int* __restrict__ count_out,
                               float4* __restrict__ feats_out) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    const VgParams p = *pp;
-    const int n = d_n ? min(*d_n, n_max) : n_max;
-    if (i == 0) *count_out = p.overflow ? n : rank[n_max];
-    if (p.overflow) {   // PCL: output = *input_ (not the centroids of one-point voxels: the normal and the padding would differ)
-        if (i < n) {
-            const float4* src = reinterpret_cast<const float4*>(pts + (size_t)i * STRIDE);
-            float4* dst = reinterpret_cast<float4*>(out + (size_t)i * STRIDE);
-#pragma unroll
-            for (int k = 0; k < STRIDE / 16; ++k) dst[k] = src[k];
-            if (feats_out) feats_out[i] = make_float4(src[0].x, src[0].y, src[0].z, __int_as_float(i));
-        }
-        return;
-    }
-    if (i >= n || !flags[i]) return;
-    const int o = rank[i];
-    const VgAcc<STRIDE> a = vg_walk<STRIDE>(keys, i, p.n_finite, [&](int j) { return vals[j]; },
-                                            [&](int m) { return pts + (size_t)m * STRIDE; });
-    const VgXyz c = vg_write<STRIDE>(a.s, a.n, out + (size_t)o * STRIDE);
-    if (feats_out) feats_out[o] = make_float4(c.x, c.y, c.z, __int_as_float(o));
+    vg_centroid_at<STRIDE, K>(pts, keys, vals, flags, rank, n_max, d_n, pp, out, count_out, feats_out, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
 // ---------------------------------------------------------------------------------------

@@ -9,8 +9,13 @@ Both legs call the C ABI with argument arrays built once, so that the time is th
 The legs alternate over --rounds rounds of --steps timed steps each (after --warmup untimed ones).  Per B: the median, smallest
 and largest of the rounds' median ms per fleet window step, the waits per step (each call ends in one stream synchronise),
 and whether (a) and (b) gave byte-identical counts and blocks.  Prints the card, its power limit and maximum SM clock first.
+--loop measures a fleet loop-closure tick instead (DESIGN.md §5's loop-closure row per session): each session's store holds
+synth.make_keyframe_sequence(41, revisit=1) (its own seed); the source is the revisit keyframe listed 2 deg / 0.5 m off, the target
+the 41 history keyframes, at the reference's ICP settings (leaf 0.4, 30 m, 100 iterations, 1e-6, 1e-6):
+  (a) B solo liliom_loop_align calls;
+  (b) one liliom_loop_align_batch.
 Reads device state only.
-usage: backend_batch_bench.py [--sessions 1 2 4 8 16 32] [--steps 20] [--warmup 3] [--rounds 5]"""
+usage: backend_batch_bench.py [--loop] [--sessions 1 2 4 8 16 32] [--steps 20] [--warmup 3] [--rounds 5]"""
 import argparse
 import ctypes as C
 import json
@@ -119,6 +124,76 @@ class Fleet:
         return out
 
 
+LC_HIST = 41       # his_key_frames_ds at lc_map_width = 20
+LC_LEAF = 0.4
+
+
+def loop_stream(seed):
+    from liliom_b200 import synth
+    return synth.make_keyframe_sequence(LC_HIST, stride=48, seed=seed, revisit=1)
+
+
+class LoopSession:
+    def __init__(self, seq):
+        import liliom_b200 as L
+        from liliom_b200 import synth
+        bp = L.backend_default_params(0)
+        self.c = L.Context(variant=0)
+        for e, s, _ in seq:
+            self.c.kf_add(bp, e, s, download=False)
+        p = seq[LC_HIST][2]
+        qd = synth.q_from_axis_angle([0.1, -0.1, 1.0], np.deg2rad(2.0))
+        self.src_ids = np.array([LC_HIST], np.int32)
+        self.src_poses = np.concatenate([synth.qmul(qd, p[:4]), p[4:] + np.array([0.4, -0.25, 0.15])])
+        self.tgt_ids = np.arange(LC_HIST, dtype=np.int32)
+        self.tgt_poses = np.ascontiguousarray([q for _, _, q in seq[:LC_HIST]], np.float64).reshape(-1)
+        self.res = {leg: L.LoopResult() for leg in "ab"}
+
+
+class LoopFleet:
+    """B sessions and the C arguments of both legs, built once."""
+
+    def __init__(self, S):
+        import liliom_b200 as L
+        self.S, self.lib, B = S, L._binding.lib(), len(S)
+        P, D = C.POINTER(C.c_int), C.POINTER(C.c_double)
+        self.handles = (C.c_void_p * B)(*[s.c._h for s in S])
+        self.si = (P * B)(*[ptr(s.src_ids, C.c_int) for s in S])
+        self.sp = (D * B)(*[ptr(s.src_poses, C.c_double) for s in S])
+        self.ti = (P * B)(*[ptr(s.tgt_ids, C.c_int) for s in S])
+        self.tp = (D * B)(*[ptr(s.tgt_poses, C.c_double) for s in S])
+        self.ks = np.ones(B, np.int32)
+        self.kt = np.full(B, LC_HIST, np.int32)
+        self.prm = (L.LoopParams * B)(*[L.LoopParams(LC_LEAF, 30.0, 100, 1e-6, 1e-6) for _ in S])
+        self.out = (L.LoopResult * B)()
+        self.status = np.zeros(B, np.int32)
+        # leg (a)'s output pointers: the fields of each session's own LoopResult
+        at = lambda r, name, t: C.cast(C.c_void_p(C.addressof(r) + getattr(L.LoopResult, name).offset), C.POINTER(t))   # noqa: E731
+        self.solo_out = [(at(r, "T16", C.c_double), at(r, "fitness", C.c_double), at(r, "converged", C.c_int), at(r, "iters", C.c_int),
+                          at(r, "n_src", C.c_int), at(r, "n_tgt", C.c_int)) for r in (s.res["a"] for s in S)]
+
+    def leg_a(self):
+        for s, (T, fit, conv, it, ns, nt) in zip(self.S, self.solo_out):
+            rc = self.lib.liliom_loop_align(s.c._h, ptr(s.src_ids, C.c_int), ptr(s.src_poses, C.c_double), 1, ptr(s.tgt_ids, C.c_int),
+                                            ptr(s.tgt_poses, C.c_double), LC_HIST, LC_LEAF, 30.0, 100, 1e-6, 1e-6, T, fit, conv, it, ns, nt)
+            assert rc == 0, rc
+
+    def leg_b(self):
+        B = len(self.S)
+        rc = self.lib.liliom_loop_align_batch(self.handles, B, self.si, self.sp, ptr(self.ks, C.c_int), self.ti, self.tp, ptr(self.kt, C.c_int),
+                                              self.prm, self.out, ptr(self.status, C.c_int))
+        assert rc == 0 and not self.status.any(), (rc, self.status)
+        for s, r in zip(self.S, self.out):
+            C.memmove(C.addressof(s.res["b"]), C.addressof(r), C.sizeof(r))
+
+    def outputs(self, leg):
+        out = b""
+        for s in self.S:
+            out += bytes(s.res[leg])
+            C.memset(C.addressof(s.res[leg]), 0, C.sizeof(s.res[leg]))
+        return out
+
+
 def timed(f, leg, steps):
     """median ms of `steps` window steps of leg "a" or "b", and the outputs of the last (every call returns with its sessions'
     work complete)"""
@@ -140,7 +215,10 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=5)
+    ap.add_argument("--loop", action="store_true", help="the fleet loop-closure tick instead of the window step")
     args = ap.parse_args()
+    if args.loop:
+        return main_loop(args)
     Bmax = max(args.sessions)
     with ProcessPoolExecutor(max_workers=min(Bmax, os.cpu_count() or 1)) as ex:     # the streams, before CUDA starts here
         seqs = list(ex.map(stream, [100 + s for s in range(Bmax)]))
@@ -165,6 +243,39 @@ def main():
                    surf_map=int(np.median([s.c.bmap_download(1).size for s in S])),
                    a_solo_ms=spread(ra), b_batch_ms=spread(rb), a_waits=B * (1 + EVALS), b_waits=1 + EVALS,
                    speedup=round(float(np.median(ra) / np.median(rb)), 3), identical=bool(same))
+        print(json.dumps(row), flush=True)
+    for s in sessions:
+        s.c.close()
+
+
+def main_loop(args):
+    Bmax = max(args.sessions)
+    with ProcessPoolExecutor(max_workers=min(Bmax, os.cpu_count() or 1)) as ex:
+        seqs = list(ex.map(loop_stream, [200 + s for s in range(Bmax)]))
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("backend_batch_bench.py measures on a CUDA device; none is visible")
+    print(json.dumps(dict(card(), leg="loop", history=LC_HIST, leaf=LC_LEAF, steps=args.steps, rounds=args.rounds,
+                          figures="[median of rounds, min round, max round], ms per fleet loop-closure tick")), flush=True)
+    sessions = [LoopSession(seq) for seq in seqs]
+    for B in args.sessions:
+        S = sessions[:B]
+        f = LoopFleet(S)
+        for leg in "ab":
+            timed(f, leg, args.warmup)
+        ra, rb, same = [], [], True
+        for _ in range(args.rounds):
+            ta, oa = timed(f, "a", args.steps)
+            tb, ob = timed(f, "b", args.steps)
+            ra.append(ta); rb.append(tb)
+            same = same and oa == ob
+        f.leg_a()
+        rs = [s.res["a"] for s in S]
+        row = dict(sessions=B, n_src=[min(r.n_src for r in rs), max(r.n_src for r in rs)], n_tgt=[min(r.n_tgt for r in rs), max(r.n_tgt for r in rs)],
+                   iters=[min(r.iters for r in rs), max(r.iters for r in rs)],
+                   a_solo_ms=spread(ra), b_batch_ms=spread(rb), a_waits=4 * B, b_waits=3,
+                   speedup=round(float(np.median(ra) / np.median(rb)), 3), identical=bool(same))
+        f.outputs("a")
         print(json.dumps(row), flush=True)
     for s in sessions:
         s.c.close()
