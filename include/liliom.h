@@ -554,6 +554,37 @@ int liliom_scan_to_map_resident_batch_ex(liliom_ctx* const* ctxs, int B, double*
 int liliom_odometry_resident_batch_ex(liliom_ctx* const* ctxs, int B, double* poses7_inout, const int* match_cnt,
                                       const int* max_num_iter, int mode, liliom_iter_stats* const* stats, void* const* ds_out,
                                       const int* ds_cap, int* n_ds, int* status);
+/* One driver message of a session of liliom_convert_batch: kind LILIOM_WIRE_LIVOX with liliom_convert_livox's custom_pts, n
+ * and stride (19 or 20), or LILIOM_WIRE_PC2 with liliom_convert_pc2's msg.  The fields of the other kind are not read. */
+enum { LILIOM_WIRE_LIVOX = 0, LILIOM_WIRE_PC2 = 1 };
+typedef struct {
+    int kind;
+    const void* custom_pts; int n; int stride;
+    const liliom_pc2_msg* pc2;
+} liliom_wire_msg;
+/* liliom_convert_livox / liliom_convert_pc2 of B independent sessions in one call: the fleet's front door, in front of
+ * liliom_extract_resident_batch.  msgs: B messages; out, cap: NULL, or B entries (a NULL out[i]: no download for session i);
+ * n, status: B ints.  Session i gets exactly what its solo call would give it, bit for bit:
+ *   LIVOX: liliom_convert_livox(ctxs[i], m.custom_pts, m.n, m.stride, out ? out[i] : NULL, cap ? cap[i] : 0), and n[i] = m.n
+ *          on success;
+ *   PC2:   liliom_convert_pc2(ctxs[i], m.pc2, out ? out[i] : NULL, cap ? cap[i] : 0, &n[i]).
+ * That covers the status, n[i] (written where the solo call writes it), the downloaded bytes, the resident sweep and its ring /
+ * time side channels (decoded under the session's own liliom_set_ring_source / liliom_set_time_source), liliom_last_error and
+ * the launch counters, so a later liliom_extract_resident or liliom_extract_resident_batch behaves as after the solo call.
+ * A session's own refusal is its status and leaves that session unchanged; the others run.  The refusals are those of the solo
+ * call (a bad stride, a NULL payload, a malformed PointCloud2, a missing ring or time field under the field sources,
+ * LILIOM_E_CAPACITY), and LILIOM_E_ARG for a kind that does not fit the context: LIVOX on a 32-byte context, PC2 on a 48-byte
+ * one, or an unknown kind.  Horizon (48-byte) and ROT (32-byte) sessions may be mixed.
+ * Each accepted session's payload is copied into its own staging buffer, the copies queued back to back on ctxs[0]'s stream;
+ * then one decode launch per kind for up to 32 sessions (each session's points start on a block boundary), the downloads and
+ * one stream synchronise for the whole call, where B solo calls wait B times.  Sessions with 0 points take part in no launch.
+ * The library does not pin the payloads: page-locked payloads are copied by asynchronous DMA, pageable ones as the solo call
+ * copies them.  Other sessions' streams are joined to ctxs[0]'s with events.
+ * LILIOM_E_ARG for the whole call, nothing changed: B < 1, a NULL array (ctxs, msgs, n, status), a NULL or repeated context,
+ * contexts on different devices, a context with a communicator.
+ * For a single session the solo call is faster (no event joins, no session table). */
+int liliom_convert_batch(liliom_ctx* const* ctxs, int B, const liliom_wire_msg* msgs, void* const* out, const int* cap, int* n,
+                         int* status);
 /* liliom_extract_resident of B independent sessions in one call.  q_imu: 4*B doubles; q_lb: 4*B doubles or NULL (identity,
  * as the solo call's NULL).  n_surf / n_edge / n_cut / status: B ints each.  Horizon (48-byte) and ROT (32-byte) contexts
  * may be mixed.  Session i gets exactly what liliom_extract_resident(ctxs[i], q_imu + 4*i, q_lb ? q_lb + 4*i : NULL, ...)

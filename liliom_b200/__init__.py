@@ -10,11 +10,13 @@ from ._lib import (Context, Params, IterStats, Counters, LiliomError, default_pa
                    BackendParams, backend_default_params, KF_FULL, KF_SURF, RING_ELEVATION, RING_FIELD,
                    TIME_AZIMUTH, TIME_FIELD, scan_to_map_resident_batch, odometry_resident_batch,
                    scan_to_map_resident_batch_ex, odometry_resident_batch_ex, extract_resident_batch, map_update_batch,
-                   backend_window_correspond_batch, backend_window_blocks_batch, loop_align_batch, LoopParams, LoopResult)
+                   backend_window_correspond_batch, backend_window_blocks_batch, loop_align_batch, LoopParams, LoopResult,
+                   convert_batch, WireMsg, WIRE_LIVOX, WIRE_PC2)
 
 __all__ = ["Context", "Params", "IterStats", "Counters", "LiliomError", "default_params", "comm_get_unique_id",
            "PT48", "PT32", "MODE_CERES", "MODE_GN", "LIB_PATH", "EXPORTS",
            "BackendParams", "backend_default_params", "KF_FULL", "KF_SURF", "PC2", "RING_ELEVATION", "RING_FIELD",
            "TIME_AZIMUTH", "TIME_FIELD", "scan_to_map_resident_batch", "odometry_resident_batch",
            "scan_to_map_resident_batch_ex", "odometry_resident_batch_ex", "extract_resident_batch", "map_update_batch",
-           "backend_window_correspond_batch", "backend_window_blocks_batch", "loop_align_batch", "LoopParams", "LoopResult"]
+           "backend_window_correspond_batch", "backend_window_blocks_batch", "loop_align_batch", "LoopParams", "LoopResult",
+           "convert_batch", "WireMsg", "WIRE_LIVOX", "WIRE_PC2"]

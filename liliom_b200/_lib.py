@@ -94,7 +94,7 @@ EXPORTS = [
     "liliom_extract_resident_batch", "liliom_features_download",
     "liliom_map_update_resident", "liliom_map_update_batch",
     "liliom_backend_window_correspond_batch", "liliom_backend_window_blocks_batch",
-    "liliom_loop_align_batch",
+    "liliom_loop_align_batch", "liliom_convert_batch",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -138,6 +138,14 @@ class PC2:
         m = Pc2Msg(self.data.ctypes.data_as(C.c_void_p) if self.data.size else None, self.height, self.width, self.point_step,
                    self.row_step, f, len(self.fields), 1 if self.is_bigendian else 0)
         return m, f
+
+
+WIRE_LIVOX, WIRE_PC2 = 0, 1
+
+
+class WireMsg(C.Structure):
+    """liliom_wire_msg (include/liliom.h): one session's driver message of liliom_convert_batch."""
+    _fields_ = [("kind", C.c_int), ("custom_pts", C.c_void_p), ("n", C.c_int), ("stride", C.c_int), ("pc2", C.POINTER(Pc2Msg))]
 
 
 class LoOutput(C.Structure):
@@ -246,6 +254,7 @@ def lib() -> C.CDLL:
                                     dp, dp, ip, ip, ip, ip]
     L.liliom_loop_align_batch.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(ip), C.POINTER(dp), ip, C.POINTER(ip), C.POINTER(dp), ip,
                                           C.POINTER(LoopParams), C.POINTER(LoopResult), ip]
+    L.liliom_convert_batch.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(WireMsg), C.POINTER(vp), ip, ip, ip]
     L.liliom_pre_create.argtypes = [vp, C.c_int, dp]; L.liliom_pre_create.restype = vp
     L.liliom_pre_destroy.argtypes = [vp]; L.liliom_pre_destroy.restype = None
     L.liliom_pre_imu.argtypes = [vp, C.c_double, dp]; L.liliom_pre_imu.restype = None
@@ -960,6 +969,49 @@ def loop_align_batch(ctxs, src_ids, src_poses, tgt_ids, tgt_poses, params):
         raise LiliomError(rc)
     out = [(np.array(r.T16[:], np.float64).reshape(4, 4), r.fitness, bool(r.converged), r.iters, r.n_src, r.n_tgt) for r in res[:B]]
     return out, status[:B]
+
+
+def wire_msgs(msgs):
+    """(WireMsg array, keep-alive list) of B driver messages: a PC2 is a PointCloud2 (WIRE_PC2); a Livox CustomPoint record
+    array (LIVOX20) or an (array, stride) pair of raw records is a Livox message (WIRE_LIVOX), as Context.convert_livox takes
+    them."""
+    arr = (WireMsg * max(len(msgs), 1))()
+    keep = []
+    for i, m in enumerate(msgs):
+        if isinstance(m, PC2):
+            cm, f = m.c_msg()
+            keep += [m, cm, f]
+            arr[i].kind, arr[i].pc2 = WIRE_PC2, C.pointer(cm)
+        else:
+            a, n, stride = Context._livox(*(m if isinstance(m, tuple) else (m, None)))
+            keep.append(a)
+            arr[i].kind, arr[i].custom_pts, arr[i].n, arr[i].stride = WIRE_LIVOX, _ptr(a) if a.size else None, n, stride
+    return arr, keep
+
+
+def convert_batch(ctxs, msgs, download: bool = False, caps=None):
+    """convert_livox / convert_pc2 of every context in `ctxs` in one call (liliom_convert_batch): session i gets what its solo
+    call on msgs[i] would give it, and keeps the sweep resident.  msgs: B messages as wire_msgs takes them.  download: also
+    return each session's decoded cloud (caps: per-session capacity in points, default the message's size).  Returns (per-session
+    clouds (download; None for a refused session) or the counts n (B,), status (B,)); a session's own error is its status, a
+    whole-call error raises LiliomError."""
+    B = len(ctxs)
+    if len(msgs) != B:
+        raise ValueError(f"expected {B} messages, got {len(msgs)}")
+    arr, _keep = wire_msgs(msgs)
+    sizes = [arr[i].n if arr[i].kind == WIRE_LIVOX else msgs[i].width * msgs[i].height for i in range(B)]
+    caps = [int(x) for x in caps] if caps is not None else sizes
+    bufs = [np.zeros(max(caps[i], 1), ctxs[i].dtype) for i in range(B)] if download else None
+    outs = (C.c_void_p * max(B, 1))(*[b.ctypes.data for b in bufs]) if download else None
+    cap_arr = np.array(caps + [0], np.int32)
+    n = np.zeros(max(B, 1), np.int32)
+    status = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_convert_batch(_handles(ctxs), B, arr, outs, _ip(cap_arr), _ip(n), _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    if download:
+        return [bufs[i][:n[i]] if status[i] == OK else None for i in range(B)], status[:B]
+    return n[:B].copy(), status[:B]
 
 
 def _handles(ctxs):

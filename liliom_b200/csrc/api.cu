@@ -2,6 +2,7 @@
 #include "ctx.cuh"
 #include "dev_math.cuh"
 #include "pc2_fields.h"
+#include "wire_decode.h"
 #include <new>
 #include <cstdlib>
 
@@ -182,46 +183,55 @@ extern "C" int liliom_extract_horizon(liliom_ctx* c, const liliom_pt48* pts, int
     return extract_horizon_from_raw(c, n, q_imu, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut);
 }
 
-// ---- (f3) FormatConvert on the device: livox_ros_driver::CustomPoint[] -> pcl::PointXYZINormal[] (L/src/FormatConvert.cpp:11-24)
+// ---- (f3) FormatConvert on the device: livox_ros_driver::CustomPoint[] -> pcl::PointXYZINormal[] (L/src/FormatConvert.cpp:11-24;
+// the per-point body: wire_decode.h)
 namespace lili {
-// little-endian 32-bit word assembled from bytes: sensor payloads carry fields at any byte offset, never read them wider
-__device__ __forceinline__ unsigned rd32(const unsigned char* p) {
-    return (unsigned)p[0] | ((unsigned)p[1] << 8) | ((unsigned)p[2] << 16) | ((unsigned)p[3] << 24);
-}
 __global__ void k_livox_to_pt48(const unsigned char* __restrict__ in, int n, int stride, float4* __restrict__ out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const unsigned time_end = rd32(in + (size_t)(n - 1) * stride);                       // :13 points.back().offset_time
-    const unsigned char* p = in + (size_t)i * stride;
-    const unsigned off = rd32(p);
-    const float x = __uint_as_float(rd32(p + 4)), y = __uint_as_float(rd32(p + 8)), z = __uint_as_float(rd32(p + 12));
-    const unsigned refl = p[16], line = p[18];
-    const float s = __fdiv_rn(__uint2float_rn(off), __uint2float_rn(time_end));          // :19 float(offset_time / (float)time_end)
-    const float intensity = (float)addx((double)line, mulx((double)s, 0.1));            // :20
-    const float curvature = (float)mulx(0.1, (double)refl);                             // :21
-    out[3 * (size_t)i] = make_float4(x, y, z, 1.0f);                                    // pcl::PointXYZINormal default ctor: data[3] = 1
-    out[3 * (size_t)i + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
-    out[3 * (size_t)i + 2] = make_float4(intensity, curvature, 0.f, 0.f);
+    livox_point_at(in, n, stride, reinterpret_cast<unsigned char*>(out), blockIdx.x * blockDim.x + threadIdx.x);
 }
-static int livox_to_dev(liliom_ctx* c, const void* custom_pts, int n, int stride, void* d_out48) {
+
+// The Livox ingest in parts, shared by the solo calls and liliom_convert_batch: livox_args_ok (the solo calls' refusals),
+// livox_begin (the buffers: dst for the n decoded points, wire_in for the payload), livox_copy (the payload to wire_in on the
+// context's stream) and livox_launch (the decode into dst).
+static bool livox_args_ok(const liliom_ctx* c, const void* custom_pts, int n, int stride) {
+    return c && n >= 0 && (n == 0 || custom_pts) && (stride == 19 || stride == 20) && c->prm.point_stride == 48;
+}
+static int livox_begin(liliom_ctx* c, int n, int stride, DevBuf& dst) {
+    LILI_CUDA(c, dst.ensure((size_t)(n > 0 ? n : 1) * 48));
+    if (n > 0) LILI_CUDA(c, c->wire_in.ensure((size_t)n * stride));
+    return LILIOM_OK;
+}
+static int livox_copy(liliom_ctx* c, const void* custom_pts, int n, int stride) {
+    if (n > 0) LILI_CUDA(c, cudaMemcpyAsync(c->wire_in.p, custom_pts, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
+    return LILIOM_OK;
+}
+static int livox_launch(liliom_ctx* c, int n, int stride, void* d_out48) {
     if (n <= 0) return LILIOM_OK;
-    LILI_CUDA(c, c->wire_in.ensure((size_t)n * stride));
-    LILI_CUDA(c, cudaMemcpyAsync(c->wire_in.p, custom_pts, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
     k_livox_to_pt48<<<cdiv(n, 256), 256, 0, c->stream>>>((const unsigned char*)c->wire_in.p, n, stride, (float4*)d_out48);
     return launch_check(c, "k_livox_to_pt48");
+}
+static int livox_to_dev(liliom_ctx* c, const void* custom_pts, int n, int stride, DevBuf& dst) {
+    LILI_TRY(livox_begin(c, n, stride, dst));
+    LILI_TRY(livox_copy(c, custom_pts, n, stride));
+    return livox_launch(c, n, stride, dst.p);
+}
+
+// The end of a convert call that leaves n points of `stride` bytes resident: the resident count, and the download to out
+// (NULL: none) on the context's stream.
+static int resident_finish(liliom_ctx* c, int n, int stride, void* out) {
+    c->n_raw_scan = n;
+    if (out && n) LILI_CUDA(c, cudaMemcpyAsync(out, c->raw_scan.p, (size_t)n * stride, cudaMemcpyDeviceToHost, c->stream));
+    return LILIOM_OK;
 }
 }  // namespace lili
 
 extern "C" int liliom_convert_livox(liliom_ctx* c, const void* custom_pts, int n, int stride, liliom_pt48* out, int cap) {
-    if (!c || n < 0 || (n > 0 && !custom_pts) || (stride != 19 && stride != 20)) return LILIOM_E_ARG;
-    if (c->prm.point_stride != 48) return LILIOM_E_ARG;
+    if (!livox_args_ok(c, custom_pts, n, stride)) return LILIOM_E_ARG;
     if (out && n > cap) return LILIOM_E_CAPACITY;
     LILI_CUDA(c, cudaSetDevice(c->device));
-    LILI_CUDA(c, c->raw_scan.ensure((size_t)(n > 0 ? n : 1) * 48));
-    LILI_TRY(livox_to_dev(c, custom_pts, n, stride, c->raw_scan.p));
-    c->n_raw_scan = n;
     c->raw_scan_side.clear();
-    if (out && n) LILI_CUDA(c, cudaMemcpyAsync(out, c->raw_scan.p, (size_t)n * 48, cudaMemcpyDeviceToHost, c->stream));
+    LILI_TRY(livox_to_dev(c, custom_pts, n, stride, c->raw_scan));
+    LILI_TRY(resident_finish(c, n, 48, out));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     return LILIOM_OK;
 }
@@ -229,11 +239,9 @@ extern "C" int liliom_convert_livox(liliom_ctx* c, const void* custom_pts, int n
 extern "C" int liliom_extract_horizon_livox(liliom_ctx* c, const void* custom_pts, int n, int stride, const double q_imu[4],
                                             liliom_pt48* surf_out, int surf_cap, int* n_surf, liliom_pt48* edge_out, int edge_cap, int* n_edge,
                                             liliom_pt48* cut_out, int cut_cap, int* n_cut) {
-    if (!c || n < 0 || (n > 0 && !custom_pts) || (stride != 19 && stride != 20) || !q_imu || !n_surf || !n_edge || !n_cut) return LILIOM_E_ARG;
-    if (c->prm.point_stride != 48) return LILIOM_E_ARG;
+    if (!livox_args_ok(c, custom_pts, n, stride) || !q_imu || !n_surf || !n_edge || !n_cut) return LILIOM_E_ARG;
     LILI_CUDA(c, cudaSetDevice(c->device));
-    LILI_CUDA(c, c->raw.ensure((size_t)(n > 0 ? n : 1) * 48));
-    LILI_TRY(livox_to_dev(c, custom_pts, n, stride, c->raw.p));
+    LILI_TRY(livox_to_dev(c, custom_pts, n, stride, c->raw));
     return extract_horizon_from_raw(c, n, q_imu, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut);
 }
 
@@ -255,7 +263,8 @@ extern "C" int liliom_extract_rot(liliom_ctx* c, const liliom_pt32* pts, int n, 
     return extract_rot_from_raw(c, n, q_imu, q_lb, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut);
 }
 
-// ---- (f3) pcl::fromROSMsg(PointCloud2 -> pcl::PointXYZI) on the device (R/src/Preprocessing.cpp:277); field matching: pc2_fields.h
+// ---- (f3) pcl::fromROSMsg(PointCloud2 -> pcl::PointXYZI) on the device (R/src/Preprocessing.cpp:277); field matching: pc2_fields.h,
+// the per-point body: wire_decode.h
 namespace lili {
 // One thread per point, row-major over (row, column).  src = Pc2Map::src of x, y, z, intensity (-1: unmapped -> 0).
 // Kept a pass of its own rather than fused into k_rot_pre: k_rot_hp and k_rot_build read the decoded sweep again.
@@ -264,29 +273,8 @@ namespace lili {
 // time_type).
 __global__ void k_pc2_to_pt32(const unsigned char* __restrict__ in, int n, unsigned width, unsigned point_step, unsigned row_step, int4 src,
                               float4* __restrict__ out, int2 ring, uint16_t* __restrict__ ring_out, int2 tm, double* __restrict__ time_out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const unsigned r = (unsigned)i / width, col = (unsigned)i - r * width;
-    const unsigned char* p = in + (size_t)r * row_step + (size_t)col * point_step;
-    auto fld = [p](int off) { return off < 0 ? 0.0f : __uint_as_float(rd32(p + off)); };
-    out[2 * (size_t)i] = make_float4(fld(src.x), fld(src.y), fld(src.z), 1.0f);          // pcl::PointXYZI default ctor: data[3] = 1
-    out[2 * (size_t)i + 1] = make_float4(fld(src.w), 0.f, 0.f, 0.f);
-    if (ring_out) ring_out[i] = (uint16_t)pc2_ring_value(p, ring.x, ring.y);
-    if (time_out) time_out[i] = pc2_time_value(p, tm.x, tm.y);
-}
-// msg already accepted by pc2_match (m): stage the payload, decode into d_out32 (m.n points of 32 bytes) and, when d_ring is
-// given (m matched with want_ring), the ring ids into d_ring (m.n u16), when d_time is given (m matched with a time name), the
-// times into d_time (m.n double)
-static int pc2_to_dev(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, void* d_out32, uint16_t* d_ring, double* d_time) {
-    if (m.n <= 0) return LILIOM_OK;
-    const size_t bytes = (size_t)msg->height * msg->row_step;
-    LILI_CUDA(c, c->wire_in.ensure(bytes));
-    LILI_CUDA(c, cudaMemcpyAsync(c->wire_in.p, msg->data, bytes, cudaMemcpyHostToDevice, c->stream));
-    k_pc2_to_pt32<<<cdiv(m.n, 256), 256, 0, c->stream>>>((const unsigned char*)c->wire_in.p, m.n, msg->width, msg->point_step, msg->row_step,
-                                                          make_int4(m.src[0], m.src[1], m.src[2], m.src[3]), (float4*)d_out32,
-                                                          make_int2(m.ring_src, m.ring_bytes), d_ring, make_int2(m.time_src, m.time_type),
-                                                          d_time);
-    return launch_check(c, "k_pc2_to_pt32");
+    const Pc2Wire w{width, point_step, row_step, {src.x, src.y, src.z, src.w}, ring.x, ring.y, tm.x, tm.y};
+    pc2_point_at(in, n, w, reinterpret_cast<unsigned char*>(out), ring_out, time_out, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
 // pc2_match under the context's sources: the `ring` field under LILIOM_RING_FIELD, the named time field under LILIOM_TIME_FIELD
@@ -294,18 +282,47 @@ static int pc2_match_ctx(const liliom_ctx* c, const liliom_pc2_msg* msg, Pc2Map*
     return pc2_match(msg, m, c->ring_source == LILIOM_RING_FIELD, c->time_source == LILIOM_TIME_FIELD ? c->time_name : nullptr);
 }
 
-// msg accepted by pc2_match_ctx (m): size out32 and the side buffers of the channels m matched, decode into them and record in
-// side which channels it now holds (none when the decode fails)
-static int pc2_decode(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, DevBuf& out32, Pc2Side& side) {
+// The PointCloud2 ingest of a message accepted by pc2_match_ctx (m) in parts, shared by the solo calls and liliom_convert_batch:
+// pc2_begin (out32 sized for the m.n decoded points, side cleared and its buffers sized for the channels m matched, wire_in for
+// the payload), pc2_copy (the payload to wire_in on the context's stream), pc2_launch (the decode into out32 and the side
+// buffers) and pc2_finish (side records the channels it now holds).
+static size_t pc2_bytes(const liliom_pc2_msg* msg) { return (size_t)msg->height * msg->row_step; }
+static int pc2_begin(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, DevBuf& out32, Pc2Side& side) {
     const size_t n = (size_t)(m.n > 0 ? m.n : 1);
-    const bool ring = m.ring_src >= 0, time = m.time_src >= 0;
     LILI_CUDA(c, out32.ensure(n * 32));
     side.clear();
-    if (ring) LILI_CUDA(c, side.ring.ensure(n * sizeof(uint16_t)));
-    if (time) LILI_CUDA(c, side.time.ensure(n * sizeof(double)));
-    LILI_TRY(pc2_to_dev(c, msg, m, out32.p, ring ? side.ring.as<uint16_t>() : nullptr, time ? side.time.as<double>() : nullptr));
-    side.has_ring = ring;
-    side.has_time = time;
+    if (m.ring_src >= 0) LILI_CUDA(c, side.ring.ensure(n * sizeof(uint16_t)));
+    if (m.time_src >= 0) LILI_CUDA(c, side.time.ensure(n * sizeof(double)));
+    if (m.n > 0) LILI_CUDA(c, c->wire_in.ensure(pc2_bytes(msg)));
+    return LILIOM_OK;
+}
+static int pc2_copy(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m) {
+    if (m.n > 0) LILI_CUDA(c, cudaMemcpyAsync(c->wire_in.p, msg->data, pc2_bytes(msg), cudaMemcpyHostToDevice, c->stream));
+    return LILIOM_OK;
+}
+// the side buffers the decode writes: those of the channels m matched (nullptr for the others)
+static uint16_t* pc2_ring_out(const Pc2Map& m, Pc2Side& side) { return m.ring_src >= 0 ? side.ring.as<uint16_t>() : nullptr; }
+static double* pc2_time_out(const Pc2Map& m, Pc2Side& side) { return m.time_src >= 0 ? side.time.as<double>() : nullptr; }
+static int pc2_launch(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, DevBuf& out32, Pc2Side& side) {
+    if (m.n <= 0) return LILIOM_OK;
+    k_pc2_to_pt32<<<cdiv(m.n, 256), 256, 0, c->stream>>>((const unsigned char*)c->wire_in.p, m.n, msg->width, msg->point_step, msg->row_step,
+                                                          make_int4(m.src[0], m.src[1], m.src[2], m.src[3]), out32.as<float4>(),
+                                                          make_int2(m.ring_src, m.ring_bytes), pc2_ring_out(m, side),
+                                                          make_int2(m.time_src, m.time_type), pc2_time_out(m, side));
+    return launch_check(c, "k_pc2_to_pt32");
+}
+static void pc2_finish(const Pc2Map& m, Pc2Side& side) {
+    side.has_ring = m.ring_src >= 0;
+    side.has_time = m.time_src >= 0;
+}
+
+// msg accepted by pc2_match_ctx (m): decode into out32 and the side channels m matched, and record in side which channels it
+// now holds (none when the decode fails)
+static int pc2_decode(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, DevBuf& out32, Pc2Side& side) {
+    LILI_TRY(pc2_begin(c, msg, m, out32, side));
+    LILI_TRY(pc2_copy(c, msg, m));
+    LILI_TRY(pc2_launch(c, msg, m, out32, side));
+    pc2_finish(m, side);
     return LILIOM_OK;
 }
 }  // namespace lili
@@ -317,8 +334,7 @@ extern "C" int liliom_convert_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, lili
     if (out && m.n > cap) { *n = m.n; return LILIOM_E_CAPACITY; }
     LILI_CUDA(c, cudaSetDevice(c->device));
     LILI_TRY(pc2_decode(c, msg, m, c->raw_scan, c->raw_scan_side));
-    c->n_raw_scan = m.n;
-    if (out && m.n) LILI_CUDA(c, cudaMemcpyAsync(out, c->raw_scan.p, (size_t)m.n * 32, cudaMemcpyDeviceToHost, c->stream));
+    LILI_TRY(resident_finish(c, m.n, 32, out));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     *n = m.n;
     return LILIOM_OK;
@@ -335,6 +351,113 @@ extern "C" int liliom_extract_rot_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, 
     LILI_TRY(pc2_decode(c, msg, m, c->raw, c->raw_side));
     return extract_rot_from_raw(c, m.n, q_imu, q_lb, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut,
                                 c->raw_side.rings(), c->raw_side.times());
+}
+
+// ---- liliom_convert_batch: the solo converts' host parts per session, their decodes in shared launches (k_stage_batch)
+namespace lili {
+// one session's decode, as its solo kernel has it (a block belongs to one session, so the ring / time branches stay uniform)
+struct LivoxEntry {
+    const unsigned char* in;
+    int n, stride;
+    unsigned char* out;
+};
+struct Pc2Entry {
+    const unsigned char* in;
+    int n;
+    Pc2Wire w;
+    unsigned char* out;
+    uint16_t* ring_out;
+    double* time_out;
+};
+LILI_STAGE(WireStLivox, LivoxEntry, 256, stage_blocks(e.n, 256), livox_point_at(e.in, e.n, e.stride, e.out, i))
+LILI_STAGE(WireStPc2, Pc2Entry, 256, stage_blocks(e.n, 256), pc2_point_at(e.in, e.n, e.w, e.out, e.ring_out, e.time_out, i))
+
+// One accepted session of liliom_convert_batch: its message, what pc2_match_ctx made of it (PC2), its points and its download.
+struct WireJob {
+    liliom_ctx* c;
+    const liliom_wire_msg* msg;
+    Pc2Map m;
+    int n;
+    void* out;
+};
+
+// The solo call's refusals of session c's message, in the solo call's order; on LILIOM_OK, j describes the session.  A PC2
+// message refused for capacity reports its size in *n, as liliom_convert_pc2 does.
+static int wire_accept(liliom_ctx* c, const liliom_wire_msg& w, void* out, int cap, int* n, WireJob& j) {
+    j = WireJob{c, &w, Pc2Map{}, 0, out};
+    if (w.kind == LILIOM_WIRE_LIVOX) {
+        if (!livox_args_ok(c, w.custom_pts, w.n, w.stride)) return LILIOM_E_ARG;
+        if (out && w.n > cap) return LILIOM_E_CAPACITY;
+        j.n = w.n;
+        return LILIOM_OK;
+    }
+    if (w.kind != LILIOM_WIRE_PC2 || pc2_match_ctx(c, w.pc2, &j.m) != LILIOM_OK) return LILIOM_E_ARG;
+    if (c->prm.point_stride != 32) return LILIOM_E_ARG;
+    if (out && j.m.n > cap) { *n = j.m.n; return LILIOM_E_CAPACITY; }
+    j.n = j.m.n;
+    return LILIOM_OK;
+}
+static bool wire_is_livox(const WireJob& j) { return j.msg->kind == LILIOM_WIRE_LIVOX; }
+}  // namespace lili
+
+extern "C" int liliom_convert_batch(liliom_ctx* const* ctxs, int B, const liliom_wire_msg* msgs, void* const* out, const int* cap, int* n,
+                                    int* status) {
+    if (!batch_ctxs_ok(ctxs, B) || !msgs || !n || !status) return LILIOM_E_ARG;
+    liliom_ctx* c0 = ctxs[0];
+    LILI_CUDA(c0, cudaSetDevice(c0->device));
+    const std::vector<liliom_ctx*> all(ctxs, ctxs + B);
+    std::vector<WireJob> jobs;
+    std::vector<int> at;                    // index of each job's session in ctxs
+    for (int i = 0; i < B; ++i) {
+        liliom_ctx* c = ctxs[i];
+        void* o = out ? out[i] : nullptr;
+        WireJob j;
+        status[i] = wire_accept(c, msgs[i], o, cap ? cap[i] : 0, n + i, j);
+        if (status[i] != LILIOM_OK) continue;
+        if (wire_is_livox(j)) {
+            c->raw_scan_side.clear();
+            status[i] = livox_begin(c, j.n, j.msg->stride, c->raw_scan);
+        } else {
+            status[i] = pc2_begin(c, j.msg->pc2, j.m, c->raw_scan, c->raw_scan_side);
+        }
+        if (status[i] != LILIOM_OK) continue;
+        jobs.push_back(j);
+        at.push_back(i);
+    }
+    // every session's work so far is ordered before the copies into its buffers; they, the decodes and the downloads then
+    // queue back to back on ctxs[0]'s stream
+    LILI_TRY(batch_join_in(c0, all));
+    {
+        const BatchStreams on_c0(all, c0->stream);
+        std::vector<int> livox, pc2;        // jobs with points, by kind
+        for (size_t k = 0; k < jobs.size(); ++k) {
+            const WireJob& j = jobs[k];
+            if (wire_is_livox(j)) LILI_TRY(livox_copy(j.c, j.msg->custom_pts, j.n, j.msg->stride));
+            else LILI_TRY(pc2_copy(j.c, j.msg->pc2, j.m));
+            if (j.n > 0) (wire_is_livox(j) ? livox : pc2).push_back((int)k);
+        }
+        LILI_TRY(stage_batch<WireStLivox>(c0, livox, [&](LivoxEntry& e, int k) {
+            const WireJob& j = jobs[k];
+            e = LivoxEntry{j.c->wire_in.as<const unsigned char>(), j.n, j.msg->stride, j.c->raw_scan.as<unsigned char>()};
+            return j.c;
+        }));
+        LILI_TRY(stage_batch<WireStPc2>(c0, pc2, [&](Pc2Entry& e, int k) {
+            WireJob& j = jobs[k];
+            Pc2Side& side = j.c->raw_scan_side;
+            e = Pc2Entry{j.c->wire_in.as<const unsigned char>(), j.n, pc2_wire(j.msg->pc2, j.m), j.c->raw_scan.as<unsigned char>(),
+                         pc2_ring_out(j.m, side), pc2_time_out(j.m, side)};
+            return j.c;
+        }));
+        for (WireJob& j : jobs) {
+            if (!wire_is_livox(j)) pc2_finish(j.m, j.c->raw_scan_side);
+            LILI_TRY(resident_finish(j.c, j.n, wire_is_livox(j) ? 48 : 32, j.out));
+        }
+    }
+    // one synchronise for the whole call
+    LILI_TRY(batch_join_out(c0, all));
+    LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+    for (size_t k = 0; k < jobs.size(); ++k) n[at[k]] = jobs[k].n;
+    return LILIOM_OK;
 }
 
 // Shared tail of the ROT entry points: c->raw holds n 32-byte points (upload / decode already queued on the stream); rings: their
