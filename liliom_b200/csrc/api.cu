@@ -127,6 +127,15 @@ extern "C" int liliom_create(liliom_ctx** out, const liliom_params* p, int devic
         if (v >= 8 && v <= 256 && (v & (v - 1)) == 0) c->shard_inv_block = 1.0f / (float)v;
     }
     if (const char* e2 = getenv("LILIOM_KNN_ROUNDS")) { int v = atoi(e2); if (v >= 1 && v <= 32) c->force_rounds = v; }
+    if (const char* e11 = getenv("LILIOM_TEST_LOOPBACK")) {      // <group>:<rank>/<nranks>; a malformed value refuses the context
+        const char* colon = strrchr(e11, ':');
+        int r = -1, nr = 0, used = 0;
+        if (!colon || colon == e11 || sscanf(colon + 1, "%d/%d%n", &r, &nr, &used) != 2 || colon[1 + used] != '\0' || nr < 2 ||
+            nr > kMaxPeers || r < 0 || r >= nr) { liliom_destroy(c); return LILIOM_E_ARG; }
+        c->loopback_group.assign(e11, colon - e11);
+        c->nranks = nr; c->rank = r;
+        if (const char* e12 = getenv("LILIOM_TEST_LOOPBACK_MS")) c->loopback_ms = std::max(1, atoi(e12));
+    }
     *out = c;
     return LILIOM_OK;
 }

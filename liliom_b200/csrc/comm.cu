@@ -3,7 +3,12 @@
 // The only collective on the path is the per-iteration all-reduce of the 29 fp64 scalars
 // (21 J^T J + 6 J^T r + cost + count): 232 bytes, latency-bound over NVLink 5 / NVSwitch.
 #include "ctx.cuh"
+#include <chrono>
+#include <condition_variable>
 #include <dlfcn.h>
+#include <map>
+#include <memory>
+#include <mutex>
 
 namespace lili {
 
@@ -40,7 +45,67 @@ static bool load_nccl(std::string* err) {
     return true;
 }
 
+// ---- loopback all-reduce (LILIOM_TEST_LOOPBACK, a test hook): the ranks are contexts of one process, each called from its own
+// host thread.  A rank copies its vector to the host, meets the other ranks of its group here, and every rank takes the sum of
+// all vectors added in rank order, 0 first, in fp64, so that all ranks hold the same bits.  Only host threads wait; no kernel
+// waits on another context.  One generation per round: a rank that has taken its result cannot enter the next round before
+// every rank has arrived for it, so the result of a round is never overwritten while a rank still reads it.
+struct LoopbackGroup {
+    std::mutex m;
+    std::condition_variable cv;
+    int nranks = 0, arrived = 0, count = 0;
+    unsigned long long gen = 0;
+    std::vector<std::vector<double>> in;
+    std::vector<double> sum;
+};
+
+static int loopback_allreduce(liliom_ctx* c, double* buf, int count) {
+    static std::mutex reg_m;
+    static std::map<std::string, std::unique_ptr<LoopbackGroup>> reg;
+    std::vector<double> h((size_t)count);
+    LILI_CUDA(c, cudaMemcpyAsync(h.data(), buf, (size_t)count * sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    LoopbackGroup* g;
+    {
+        std::lock_guard<std::mutex> lk(reg_m);
+        std::unique_ptr<LoopbackGroup>& slot = reg[c->loopback_group];
+        if (!slot) slot.reset(new LoopbackGroup());
+        g = slot.get();
+    }
+    std::unique_lock<std::mutex> lk(g->m);
+    if (g->arrived == 0) { g->nranks = c->nranks; g->count = count; g->in.assign((size_t)c->nranks, {}); }
+    if (g->nranks != c->nranks || g->count != count || !g->in[c->rank].empty()) {
+        c->last_error = "loopback all-reduce: the ranks of group '" + c->loopback_group + "' disagree on nranks or count, or rank " +
+                        std::to_string(c->rank) + " entered twice";
+        return LILIOM_E_NCCL;
+    }
+    g->in[c->rank] = std::move(h);
+    const unsigned long long my_gen = g->gen;
+    if (++g->arrived == g->nranks) {
+        g->sum = g->in[0];
+        for (int r = 1; r < g->nranks; ++r)
+            for (int k = 0; k < count; ++k) g->sum[k] += g->in[r][k];
+        for (auto& v : g->in) v.clear();
+        g->arrived = 0;
+        ++g->gen;
+        g->cv.notify_all();
+    } else if (!g->cv.wait_for(lk, std::chrono::milliseconds(c->loopback_ms), [&] { return g->gen != my_gen; })) {
+        g->in[c->rank].clear();                 // withdraw: the round stays open for the others
+        --g->arrived;
+        c->last_error = "loopback all-reduce: group '" + c->loopback_group + "' did not gather all " + std::to_string(g->nranks) +
+                        " ranks within " + std::to_string(c->loopback_ms) + " ms (a rank was not called?)";
+        return LILIOM_E_NCCL;
+    }
+    h = g->sum;
+    lk.unlock();
+    LILI_CUDA(c, cudaMemcpyAsync(buf, h.data(), (size_t)count * sizeof(double), cudaMemcpyHostToDevice, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));         // h is released on return
+    c->cnt.lib_launches++;
+    return LILIOM_OK;
+}
+
 int nccl_allreduce_sum_f64(liliom_ctx* c, double* buf, int count) {
+    if (!c->loopback_group.empty()) return loopback_allreduce(c, buf, count);
     if (!c->nccl_comm) return LILIOM_E_NCCL;
     // ncclFloat64 = 8, ncclSum = 0
     int r = g_nccl.AllReduce(buf, buf, (size_t)count, 8, 0, c->nccl_comm, c->stream);
@@ -124,6 +189,11 @@ extern "C" int liliom_comm_peer_export(liliom_ctx* c, void* handle64) {
 
 extern "C" int liliom_comm_peer_attach(liliom_ctx* c, const void* handles, int nranks, int rank) {
     if (!c || !handles || nranks < 1 || nranks > lili::kMaxPeers || rank < 0 || rank >= nranks) return LILIOM_E_ARG;
+    if (!c->loopback_group.empty()) {
+        // loopback ranks share one GPU: two cooperative kernels there, each waiting on the other's sums, can deadlock
+        c->last_error = "liliom_comm_peer_attach: a loopback context (LILIOM_TEST_LOOPBACK) has no fused exchange";
+        return LILIOM_E_ARG;
+    }
     LILI_CUDA(c, cudaSetDevice(c->device));
     if (!c->peer_buf.p) { c->last_error = "liliom_comm_peer_attach: call liliom_comm_peer_export first"; return LILIOM_E_ARG; }
     if (c->nranks != nranks || c->rank != rank) {

@@ -478,6 +478,11 @@ struct liliom_ctx {
     void* peer_ptrs[lili::kMaxPeers] = {};   // every rank's buffer as mapped into this process (cudaIpcOpenMemHandle)
     bool peer_ready = false;
     unsigned int peer_epoch = 0;         // last epoch issued
+    // LILIOM_TEST_LOOPBACK=<group>:<rank>/<nranks> (test hook): this context is rank `rank` of `nranks` contexts in one process,
+    // and its all-reduce meets the group's other ranks on the host (comm.cu) instead of in NCCL.  LILIOM_TEST_LOOPBACK_MS bounds
+    // the wait.  Empty group: not a loopback member.
+    std::string loopback_group;
+    int loopback_ms = 30000;
 
     // ---- instrumentation ----
     liliom_counters cnt{};

@@ -1118,6 +1118,10 @@ static int s2m_begin(liliom_ctx* c, const double pose7[7], int match_cnt, int mo
     if (c->map_n_global < 10) return LILIOM_E_FEWMAP;          // L/src/LidarOdometry.cpp:485-488
     const int n = c->n_feats, iters = match_cnt;
     if (iters < 0) return LILIOM_E_ARG;
+    if (mode != LILIOM_MODE_GN && c->nranks > 1) {      // refused before anything is enqueued: no rank enters a collective
+        c->last_error = "CERES mode is single-GPU (the LM solve is one block); use GN mode with a communicator";
+        return LILIOM_E_ARG;
+    }
     // the per-iteration stats come back through the pinned block: check its capacity before anything is enqueued
     if (want_stats && iters > 0 && offsetof(PinBlock, stats) + (size_t)iters * kStatsDoubles * sizeof(double) > c->h_pin_bytes) return LILIOM_E_CAPACITY;
     k.iters = iters;
@@ -1244,7 +1248,6 @@ static int s2m_launch(liliom_ctx* c, S2mCall& k, const double pose7[7], int max_
             k_gn_update<<<1, 32, 0, c->stream>>>(c->neq.as<double>(), c->pose_dev.as<double>(), pass.stats);
             LILI_TRY(launch_check(c, "k_gn_update"));
         } else if (mode != LILIOM_MODE_GN) {
-            if (multi) { c->last_error = "CERES mode is single-GPU (the LM solve is one block); use GN mode with a communicator"; return LILIOM_E_ARG; }
             k_lm_solve<<<1, kLmBlock, 0, c->stream>>>(lm_args(c, a, it, max_num_iter));
             LILI_TRY(launch_check(c, "k_lm_solve"));
         }

@@ -64,6 +64,15 @@ __global__ void k_compact_repack(const unsigned char* __restrict__ in, const int
     out[pos[i]] = v;
 }
 
+// *count += the points of p[0..n) that this rank owns (owner_of): over all ranks, every voxel of a sharded map counted once
+__global__ void k_count_owned(const float4* __restrict__ p, int n, float inv_block, int nranks, int rank, int* __restrict__ count) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    bool own = false;
+    if (i < n) { const float4 v = p[i]; own = owner_of(v.x, v.y, v.z, nranks, inv_block) == rank; }
+    const unsigned b = __ballot_sync(0xffffffffu, own);
+    if ((threadIdx.x & 31) == 0 && b) atomicAdd(count, __popc(b));
+}
+
 // transformCloud (L/src/LidarOdometry.cpp:246-278; R/src/LidarOdometry.cpp:239-264).  Every kernel of the map update has its body in
 // a function of `i`, the thread's place in its session's launch: the solo kernel passes blockIdx.x * blockDim.x + threadIdx.x,
 // the batched update (k_stage_batch, ctx.cuh) the same place counted from its session's first block.
@@ -366,8 +375,15 @@ static int push_frame_from_device(liliom_ctx* c, const void* d_src, int n, const
             LILI_CUDA(c, c->map_ds.ensure((size_t)n * e.stride));
             k_transform_cloud<<<cdiv(n, 256), 256, 0, c->stream>>>(e.src, n, e.stride, e.q, e.t, (unsigned char*)c->map_ds.p);
             LILI_TRY(launch_check(c, "k_transform_cloud"));
+            // The frame's extent is that of the WHOLE transformed frame, as one GPU measures it: PCL's declined case and its
+            // wrapping index depend on the box, and every rank must decide them as one GPU does.  The finite count is that of the
+            // points this rank keeps, the points its VoxelGrid filters.
+            int whole[kBoxInts];
+            LILI_TRY(vg_minmax_dev(c, c->map_ds.p, n, nullptr, e.stride));
+            LILI_TRY(read_back(c, {{whole, c->vg_minmax.p, kBoxInts * sizeof(int)}}));
             const float halo = gate_cell(c->prm.knn_max_sqdist) + 1.7320508f * c->prm.leaf_map + 0.05f;
-            LILI_TRY(shard_filter(c, c->map_ds.p, n, e.stride, halo, f.buf.p, false, &f.n, f.mm));      // box of the points this rank keeps
+            LILI_TRY(shard_filter(c, c->map_ds.p, n, e.stride, halo, f.buf.p, false, &f.n, f.mm));
+            for (int k = 0; k < 6; ++k) f.mm[k] = whole[k];
         }
     }
     push_end(j, nullptr);
@@ -653,17 +669,26 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
         // Every rank ENTERS the all-reduce whatever happened locally (a rank that returned early would leave its peers waiting
         // in the collective): the local status travels as a second scalar and all ranks fail together.
         // Shard filter: drops the (possibly incomplete) voxels beyond the 1-cell halo, fused with the repack to float4.
+        // owned: the voxels whose centroid this rank owns.  The rank holds each of them complete, and every voxel has one owner.
+        int owned = 0;
         auto shard_and_index = [&]() -> int {
             int local = 0;
             if (m > 0) LILI_TRY(shard_filter(c, c->map_ds.p, m, stride, gate_cell(c->prm.knn_max_sqdist), c->map.xyzw.p, true, &local));
-            return grid_build(c, local, box[6] > 0 ? box : nullptr);
+            LILI_TRY(grid_build(c, local, box[6] > 0 ? box : nullptr));
+            int* d_owned = c->vg_count.as<int>() + 1;
+            LILI_CUDA(c, cudaMemsetAsync(d_owned, 0, sizeof(int), c->stream));
+            if (local > 0) {
+                k_count_owned<<<cdiv(local, 256), 256, 0, c->stream>>>(c->map.xyzw.as<float4>(), local, c->shard_inv_block, c->nranks, c->rank, d_owned);
+                LILI_TRY(launch_check(c, "k_count_owned"));
+            }
+            return read_back(c, {{&owned, d_owned, sizeof(int)}});
         };
         const int rc_local = shard_and_index();
         mark();  // [3] shard filter + cell grid
         // the "< 10 map points" guard (L/src/LidarOdometry.cpp:485-488) is about the whole map: sum the owned-voxel counts
         LILI_CUDA(c, c->neq.ensure(32 * sizeof(double)));
         double* pin = c->h_pin->map_status;
-        pin[0] = rc_local == LILIOM_OK ? (double)c->map.n : 0.0;
+        pin[0] = rc_local == LILIOM_OK ? (double)owned : 0.0;
         pin[1] = rc_local == LILIOM_OK ? 0.0 : 1.0;
         LILI_CUDA(c, cudaMemcpyAsync(c->neq.p, pin, 2 * sizeof(double), cudaMemcpyHostToDevice, c->stream));
         LILI_TRY(nccl_allreduce_sum_f64(c, c->neq.as<double>(), 2));
@@ -671,7 +696,7 @@ extern "C" int liliom_map_rebuild(liliom_ctx* c, int* n_map_out) {
         LILI_CUDA(c, cudaStreamSynchronize(c->stream));
         if (rc_local != LILIOM_OK) return rc_local;
         if (pin[3] != 0.0) { c->map.ready = false; c->last_error = "liliom_map_rebuild failed on another rank"; return LILIOM_E_NCCL; }
-        c->map_n_global = (int)pin[2];                  // halo voxels are counted on several ranks: an upper bound >= the true size
+        c->map_n_global = (int)pin[2];                  // each voxel counted on its owner only: the size one GPU's map has
     } else {
         LILI_TRY(grid_build(c, m, box[6] > 0 ? box : nullptr));     // map_xyzw was written by the VoxelGrid's centroid kernel
     }
