@@ -193,36 +193,11 @@ extern "C" int liliom_extract_horizon(liliom_ctx* c, const liliom_pt48* pts, int
 }
 
 // ---- (f3) FormatConvert on the device: livox_ros_driver::CustomPoint[] -> pcl::PointXYZINormal[] (L/src/FormatConvert.cpp:11-24;
-// the per-point body: wire_decode.h)
+// the per-point body: wire_decode.h; the decode: wire_decode below)
 namespace lili {
-__global__ void k_livox_to_pt48(const unsigned char* __restrict__ in, int n, int stride, float4* __restrict__ out) {
-    livox_point_at(in, n, stride, reinterpret_cast<unsigned char*>(out), blockIdx.x * blockDim.x + threadIdx.x);
-}
-
-// The Livox ingest in parts, shared by the solo calls and liliom_convert_batch: livox_args_ok (the solo calls' refusals),
-// livox_begin (the buffers: dst for the n decoded points, wire_in for the payload), livox_copy (the payload to wire_in on the
-// context's stream) and livox_launch (the decode into dst).
+// the Livox calls' refusals
 static bool livox_args_ok(const liliom_ctx* c, const void* custom_pts, int n, int stride) {
     return c && n >= 0 && (n == 0 || custom_pts) && (stride == 19 || stride == 20) && c->prm.point_stride == 48;
-}
-static int livox_begin(liliom_ctx* c, int n, int stride, DevBuf& dst) {
-    LILI_CUDA(c, dst.ensure((size_t)(n > 0 ? n : 1) * 48));
-    if (n > 0) LILI_CUDA(c, c->wire_in.ensure((size_t)n * stride));
-    return LILIOM_OK;
-}
-static int livox_copy(liliom_ctx* c, const void* custom_pts, int n, int stride) {
-    if (n > 0) LILI_CUDA(c, cudaMemcpyAsync(c->wire_in.p, custom_pts, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
-    return LILIOM_OK;
-}
-static int livox_launch(liliom_ctx* c, int n, int stride, void* d_out48) {
-    if (n <= 0) return LILIOM_OK;
-    k_livox_to_pt48<<<cdiv(n, 256), 256, 0, c->stream>>>((const unsigned char*)c->wire_in.p, n, stride, (float4*)d_out48);
-    return launch_check(c, "k_livox_to_pt48");
-}
-static int livox_to_dev(liliom_ctx* c, const void* custom_pts, int n, int stride, DevBuf& dst) {
-    LILI_TRY(livox_begin(c, n, stride, dst));
-    LILI_TRY(livox_copy(c, custom_pts, n, stride));
-    return livox_launch(c, n, stride, dst.p);
 }
 
 // The end of a convert call that leaves n points of `stride` bytes resident: the resident count, and the download to out
@@ -233,26 +208,6 @@ static int resident_finish(liliom_ctx* c, int n, int stride, void* out) {
     return LILIOM_OK;
 }
 }  // namespace lili
-
-extern "C" int liliom_convert_livox(liliom_ctx* c, const void* custom_pts, int n, int stride, liliom_pt48* out, int cap) {
-    if (!livox_args_ok(c, custom_pts, n, stride)) return LILIOM_E_ARG;
-    if (out && n > cap) return LILIOM_E_CAPACITY;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    c->raw_scan_side.clear();
-    LILI_TRY(livox_to_dev(c, custom_pts, n, stride, c->raw_scan));
-    LILI_TRY(resident_finish(c, n, 48, out));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    return LILIOM_OK;
-}
-
-extern "C" int liliom_extract_horizon_livox(liliom_ctx* c, const void* custom_pts, int n, int stride, const double q_imu[4],
-                                            liliom_pt48* surf_out, int surf_cap, int* n_surf, liliom_pt48* edge_out, int edge_cap, int* n_edge,
-                                            liliom_pt48* cut_out, int cut_cap, int* n_cut) {
-    if (!livox_args_ok(c, custom_pts, n, stride) || !q_imu || !n_surf || !n_edge || !n_cut) return LILIOM_E_ARG;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    LILI_TRY(livox_to_dev(c, custom_pts, n, stride, c->raw));
-    return extract_horizon_from_raw(c, n, q_imu, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut);
-}
 
 static int extract_rot_from_raw(liliom_ctx* c, int n, const double q_imu[4], const double q_lb[4],
                                 liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
@@ -275,96 +230,19 @@ extern "C" int liliom_extract_rot(liliom_ctx* c, const liliom_pt32* pts, int n, 
 // ---- (f3) pcl::fromROSMsg(PointCloud2 -> pcl::PointXYZI) on the device (R/src/Preprocessing.cpp:277); field matching: pc2_fields.h,
 // the per-point body: wire_decode.h
 namespace lili {
-// One thread per point, row-major over (row, column).  src = Pc2Map::src of x, y, z, intensity (-1: unmapped -> 0).
-// Kept a pass of its own rather than fused into k_rot_pre: k_rot_hp and k_rot_build read the decoded sweep again.
-// ring_out (LILIOM_RING_FIELD only; nullptr otherwise, a uniform branch): the point's `ring` field (Pc2Map::ring_src / ring_bytes).
-// time_out (LILIOM_TIME_FIELD only; nullptr otherwise, a uniform branch): the point's time field as double (Pc2Map::time_src /
-// time_type).
-__global__ void k_pc2_to_pt32(const unsigned char* __restrict__ in, int n, unsigned width, unsigned point_step, unsigned row_step, int4 src,
-                              float4* __restrict__ out, int2 ring, uint16_t* __restrict__ ring_out, int2 tm, double* __restrict__ time_out) {
-    const Pc2Wire w{width, point_step, row_step, {src.x, src.y, src.z, src.w}, ring.x, ring.y, tm.x, tm.y};
-    pc2_point_at(in, n, w, reinterpret_cast<unsigned char*>(out), ring_out, time_out, blockIdx.x * blockDim.x + threadIdx.x);
-}
-
 // pc2_match under the context's sources: the `ring` field under LILIOM_RING_FIELD, the named time field under LILIOM_TIME_FIELD
 static int pc2_match_ctx(const liliom_ctx* c, const liliom_pc2_msg* msg, Pc2Map* m) {
     return pc2_match(msg, m, c->ring_source == LILIOM_RING_FIELD, c->time_source == LILIOM_TIME_FIELD ? c->time_name : nullptr);
 }
-
-// The PointCloud2 ingest of a message accepted by pc2_match_ctx (m) in parts, shared by the solo calls and liliom_convert_batch:
-// pc2_begin (out32 sized for the m.n decoded points, side cleared and its buffers sized for the channels m matched, wire_in for
-// the payload), pc2_copy (the payload to wire_in on the context's stream), pc2_launch (the decode into out32 and the side
-// buffers) and pc2_finish (side records the channels it now holds).
 static size_t pc2_bytes(const liliom_pc2_msg* msg) { return (size_t)msg->height * msg->row_step; }
-static int pc2_begin(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, DevBuf& out32, Pc2Side& side) {
-    const size_t n = (size_t)(m.n > 0 ? m.n : 1);
-    LILI_CUDA(c, out32.ensure(n * 32));
-    side.clear();
-    if (m.ring_src >= 0) LILI_CUDA(c, side.ring.ensure(n * sizeof(uint16_t)));
-    if (m.time_src >= 0) LILI_CUDA(c, side.time.ensure(n * sizeof(double)));
-    if (m.n > 0) LILI_CUDA(c, c->wire_in.ensure(pc2_bytes(msg)));
-    return LILIOM_OK;
-}
-static int pc2_copy(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m) {
-    if (m.n > 0) LILI_CUDA(c, cudaMemcpyAsync(c->wire_in.p, msg->data, pc2_bytes(msg), cudaMemcpyHostToDevice, c->stream));
-    return LILIOM_OK;
-}
 // the side buffers the decode writes: those of the channels m matched (nullptr for the others)
 static uint16_t* pc2_ring_out(const Pc2Map& m, Pc2Side& side) { return m.ring_src >= 0 ? side.ring.as<uint16_t>() : nullptr; }
 static double* pc2_time_out(const Pc2Map& m, Pc2Side& side) { return m.time_src >= 0 ? side.time.as<double>() : nullptr; }
-static int pc2_launch(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, DevBuf& out32, Pc2Side& side) {
-    if (m.n <= 0) return LILIOM_OK;
-    k_pc2_to_pt32<<<cdiv(m.n, 256), 256, 0, c->stream>>>((const unsigned char*)c->wire_in.p, m.n, msg->width, msg->point_step, msg->row_step,
-                                                          make_int4(m.src[0], m.src[1], m.src[2], m.src[3]), out32.as<float4>(),
-                                                          make_int2(m.ring_src, m.ring_bytes), pc2_ring_out(m, side),
-                                                          make_int2(m.time_src, m.time_type), pc2_time_out(m, side));
-    return launch_check(c, "k_pc2_to_pt32");
-}
-static void pc2_finish(const Pc2Map& m, Pc2Side& side) {
-    side.has_ring = m.ring_src >= 0;
-    side.has_time = m.time_src >= 0;
-}
 
-// msg accepted by pc2_match_ctx (m): decode into out32 and the side channels m matched, and record in side which channels it
-// now holds (none when the decode fails)
-static int pc2_decode(liliom_ctx* c, const liliom_pc2_msg* msg, const Pc2Map& m, DevBuf& out32, Pc2Side& side) {
-    LILI_TRY(pc2_begin(c, msg, m, out32, side));
-    LILI_TRY(pc2_copy(c, msg, m));
-    LILI_TRY(pc2_launch(c, msg, m, out32, side));
-    pc2_finish(m, side);
-    return LILIOM_OK;
-}
-}  // namespace lili
-
-extern "C" int liliom_convert_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, liliom_pt32* out, int cap, int* n) {
-    Pc2Map m;
-    if (!c || !n || pc2_match_ctx(c, msg, &m) != LILIOM_OK) return LILIOM_E_ARG;
-    if (c->prm.point_stride != 32) return LILIOM_E_ARG;
-    if (out && m.n > cap) { *n = m.n; return LILIOM_E_CAPACITY; }
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    LILI_TRY(pc2_decode(c, msg, m, c->raw_scan, c->raw_scan_side));
-    LILI_TRY(resident_finish(c, m.n, 32, out));
-    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    *n = m.n;
-    return LILIOM_OK;
-}
-
-extern "C" int liliom_extract_rot_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, const double q_imu[4], const double q_lb[4],
-                                      liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
-                                      liliom_pt32* cut_out, int cut_cap, int* n_cut) {
-    Pc2Map m;
-    if (!c || !q_imu || !q_lb || !n_surf || !n_edge || !n_cut || pc2_match_ctx(c, msg, &m) != LILIOM_OK) return LILIOM_E_ARG;
-    if (c->prm.point_stride != 32) return LILIOM_E_ARG;
-    if (c->ring_source == LILIOM_RING_FIELD && !rot_lines_ok(c->prm.line_num, true)) return LILIOM_E_LINES;
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    LILI_TRY(pc2_decode(c, msg, m, c->raw, c->raw_side));
-    return extract_rot_from_raw(c, m.n, q_imu, q_lb, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut,
-                                c->raw_side.rings(), c->raw_side.times());
-}
-
-// ---- liliom_convert_batch: the solo converts' host parts per session, their decodes in shared launches (k_stage_batch)
-namespace lili {
-// one session's decode, as its solo kernel has it (a block belongs to one session, so the ring / time branches stay uniform)
+// ---- the decode of driver messages, one session (the solo calls) or many (liliom_convert_batch): the stages (k_stage_batch),
+// each session's decode as one thread per point; a block belongs to one session, so the ring / time branches stay uniform.
+// The PointCloud2 decode is kept a pass of its own rather than fused into the ROT chain's first stage: the chain reads the
+// decoded sweep again.
 struct LivoxEntry {
     const unsigned char* in;
     int n, stride;
@@ -381,33 +259,145 @@ struct Pc2Entry {
 LILI_STAGE(WireStLivox, LivoxEntry, 256, stage_blocks(e.n, 256), livox_point_at(e.in, e.n, e.stride, e.out, i))
 LILI_STAGE(WireStPc2, Pc2Entry, 256, stage_blocks(e.n, 256), pc2_point_at(e.in, e.n, e.w, e.out, e.ring_out, e.time_out, i))
 
-// One accepted session of liliom_convert_batch: its message, what pc2_match_ctx made of it (PC2), its points and its download.
+// One accepted message of a session: what pc2_match_ctx made of it (PC2), its points, where they go and their download.
 struct WireJob {
     liliom_ctx* c;
     const liliom_wire_msg* msg;
     Pc2Map m;
     int n;
-    void* out;
+    void* out;                  // the convert calls' download (NULL: none)
+    DevBuf* dst;                // the decoded points: the resident sweep (the convert calls) or the extractor's input
+    Pc2Side* side;              // their side channels (NULL: left as they are, liliom_extract_horizon_livox)
 };
 
-// The solo call's refusals of session c's message, in the solo call's order; on LILIOM_OK, j describes the session.  A PC2
-// message refused for capacity reports its size in *n, as liliom_convert_pc2 does.
+// The solo convert call's refusals of session c's message, in its order; on LILIOM_OK, j describes the session, decoded into
+// the resident sweep.  A PC2 message refused for capacity reports its size in *n, as liliom_convert_pc2 does.
 static int wire_accept(liliom_ctx* c, const liliom_wire_msg& w, void* out, int cap, int* n, WireJob& j) {
-    j = WireJob{c, &w, Pc2Map{}, 0, out};
+    j = WireJob{c, &w, Pc2Map{}, 0, out, nullptr, nullptr};
     if (w.kind == LILIOM_WIRE_LIVOX) {
         if (!livox_args_ok(c, w.custom_pts, w.n, w.stride)) return LILIOM_E_ARG;
         if (out && w.n > cap) return LILIOM_E_CAPACITY;
         j.n = w.n;
-        return LILIOM_OK;
+    } else {
+        if (w.kind != LILIOM_WIRE_PC2 || pc2_match_ctx(c, w.pc2, &j.m) != LILIOM_OK) return LILIOM_E_ARG;
+        if (c->prm.point_stride != 32) return LILIOM_E_ARG;
+        if (out && j.m.n > cap) { *n = j.m.n; return LILIOM_E_CAPACITY; }
+        j.n = j.m.n;
     }
-    if (w.kind != LILIOM_WIRE_PC2 || pc2_match_ctx(c, w.pc2, &j.m) != LILIOM_OK) return LILIOM_E_ARG;
-    if (c->prm.point_stride != 32) return LILIOM_E_ARG;
-    if (out && j.m.n > cap) { *n = j.m.n; return LILIOM_E_CAPACITY; }
-    j.n = j.m.n;
+    j.dst = &c->raw_scan;
+    j.side = &c->raw_scan_side;
     return LILIOM_OK;
 }
 static bool wire_is_livox(const WireJob& j) { return j.msg->kind == LILIOM_WIRE_LIVOX; }
+
+// The buffers of an accepted job: dst for its points, side cleared and sized for the channels it matched, wire_in for the payload
+static int wire_begin(const WireJob& j) {
+    liliom_ctx* c = j.c;
+    const size_t n = (size_t)(j.n > 0 ? j.n : 1);
+    if (wire_is_livox(j)) {
+        if (j.side) j.side->clear();
+        LILI_CUDA(c, j.dst->ensure(n * 48));
+        if (j.n > 0) LILI_CUDA(c, c->wire_in.ensure((size_t)j.n * j.msg->stride));
+        return LILIOM_OK;
+    }
+    LILI_CUDA(c, j.dst->ensure(n * 32));
+    j.side->clear();
+    if (j.m.ring_src >= 0) LILI_CUDA(c, j.side->ring.ensure(n * sizeof(uint16_t)));
+    if (j.m.time_src >= 0) LILI_CUDA(c, j.side->time.ensure(n * sizeof(double)));
+    if (j.n > 0) LILI_CUDA(c, c->wire_in.ensure(pc2_bytes(j.msg->pc2)));
+    return LILIOM_OK;
+}
+
+// The decode of jobs past wire_begin, on c0's stream (every job's context stream is c0's): each payload into its context's
+// wire_in, the stages, then each PointCloud2 job's side records the channels it now holds (none when the decode fails).
+static int wire_decode(liliom_ctx* c0, const std::vector<WireJob>& jobs) {
+    std::vector<int> livox, pc2;        // jobs with points, by kind
+    for (size_t k = 0; k < jobs.size(); ++k) {
+        const WireJob& j = jobs[k];
+        if (j.n <= 0) continue;
+        const void* src = wire_is_livox(j) ? j.msg->custom_pts : j.msg->pc2->data;
+        const size_t bytes = wire_is_livox(j) ? (size_t)j.n * j.msg->stride : pc2_bytes(j.msg->pc2);
+        LILI_CUDA(j.c, cudaMemcpyAsync(j.c->wire_in.p, src, bytes, cudaMemcpyHostToDevice, c0->stream));
+        (wire_is_livox(j) ? livox : pc2).push_back((int)k);
+    }
+    LILI_TRY(stage_batch<WireStLivox>(c0, livox, [&](LivoxEntry& e, int k) {
+        const WireJob& j = jobs[k];
+        e = LivoxEntry{j.c->wire_in.as<const unsigned char>(), j.n, j.msg->stride, j.dst->as<unsigned char>()};
+        return j.c;
+    }));
+    LILI_TRY(stage_batch<WireStPc2>(c0, pc2, [&](Pc2Entry& e, int k) {
+        const WireJob& j = jobs[k];
+        e = Pc2Entry{j.c->wire_in.as<const unsigned char>(), j.n, pc2_wire(j.msg->pc2, j.m), j.dst->as<unsigned char>(),
+                     pc2_ring_out(j.m, *j.side), pc2_time_out(j.m, *j.side)};
+        return j.c;
+    }));
+    for (const WireJob& j : jobs) {
+        if (wire_is_livox(j)) continue;
+        j.side->has_ring = j.m.ring_src >= 0;
+        j.side->has_time = j.m.time_src >= 0;
+    }
+    return LILIOM_OK;
+}
+
+// One session's decode on its own stream (the solo calls)
+static int wire_decode_one(const WireJob& j) {
+    LILI_TRY(wire_begin(j));
+    return wire_decode(j.c, {j});
+}
+
+// A solo convert call: the decode into the resident sweep, its download, one synchronise; *n (PC2): the point count
+static int wire_convert(liliom_ctx* c, const liliom_wire_msg& w, void* out, int cap, int* n) {
+    WireJob j;
+    LILI_TRY(wire_accept(c, w, out, cap, n, j));
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    LILI_TRY(wire_decode_one(j));
+    LILI_TRY(resident_finish(c, j.n, wire_is_livox(j) ? 48 : 32, out));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    if (n) *n = j.n;
+    return LILIOM_OK;
+}
 }  // namespace lili
+
+extern "C" int liliom_convert_livox(liliom_ctx* c, const void* custom_pts, int n, int stride, liliom_pt48* out, int cap) {
+    const liliom_wire_msg w{LILIOM_WIRE_LIVOX, custom_pts, n, stride, nullptr};
+    return wire_convert(c, w, out, cap, nullptr);
+}
+
+extern "C" int liliom_convert_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, liliom_pt32* out, int cap, int* n) {
+    if (!c || !n) return LILIOM_E_ARG;
+    const liliom_wire_msg w{LILIOM_WIRE_PC2, nullptr, 0, 0, msg};
+    return wire_convert(c, w, out, cap, n);
+}
+
+extern "C" int liliom_extract_horizon_livox(liliom_ctx* c, const void* custom_pts, int n, int stride, const double q_imu[4],
+                                            liliom_pt48* surf_out, int surf_cap, int* n_surf, liliom_pt48* edge_out, int edge_cap, int* n_edge,
+                                            liliom_pt48* cut_out, int cut_cap, int* n_cut) {
+    if (!q_imu || !n_surf || !n_edge || !n_cut) return LILIOM_E_ARG;
+    const liliom_wire_msg w{LILIOM_WIRE_LIVOX, custom_pts, n, stride, nullptr};
+    WireJob j;
+    LILI_TRY(wire_accept(c, w, nullptr, 0, nullptr, j));
+    j.dst = &c->raw;
+    j.side = nullptr;
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    LILI_TRY(wire_decode_one(j));
+    return extract_horizon_from_raw(c, n, q_imu, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut);
+}
+
+extern "C" int liliom_extract_rot_pc2(liliom_ctx* c, const liliom_pc2_msg* msg, const double q_imu[4], const double q_lb[4],
+                                      liliom_pt32* surf_out, int surf_cap, int* n_surf, liliom_pt32* edge_out, int edge_cap, int* n_edge,
+                                      liliom_pt32* cut_out, int cut_cap, int* n_cut) {
+    if (!c || !q_imu || !q_lb || !n_surf || !n_edge || !n_cut) return LILIOM_E_ARG;
+    const liliom_wire_msg w{LILIOM_WIRE_PC2, nullptr, 0, 0, msg};
+    WireJob j;
+    LILI_TRY(wire_accept(c, w, nullptr, 0, nullptr, j));
+    if (c->ring_source == LILIOM_RING_FIELD && !rot_lines_ok(c->prm.line_num, true)) return LILIOM_E_LINES;
+    j.dst = &c->raw;
+    j.side = &c->raw_side;
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    LILI_TRY(wire_decode_one(j));
+    return extract_rot_from_raw(c, j.n, q_imu, q_lb, surf_out, surf_cap, n_surf, edge_out, edge_cap, n_edge, cut_out, cut_cap, n_cut,
+                                c->raw_side.rings(), c->raw_side.times());
+}
 
 extern "C" int liliom_convert_batch(liliom_ctx* const* ctxs, int B, const liliom_wire_msg* msgs, void* const* out, const int* cap, int* n,
                                     int* status) {
@@ -418,17 +408,9 @@ extern "C" int liliom_convert_batch(liliom_ctx* const* ctxs, int B, const liliom
     std::vector<WireJob> jobs;
     std::vector<int> at;                    // index of each job's session in ctxs
     for (int i = 0; i < B; ++i) {
-        liliom_ctx* c = ctxs[i];
-        void* o = out ? out[i] : nullptr;
         WireJob j;
-        status[i] = wire_accept(c, msgs[i], o, cap ? cap[i] : 0, n + i, j);
-        if (status[i] != LILIOM_OK) continue;
-        if (wire_is_livox(j)) {
-            c->raw_scan_side.clear();
-            status[i] = livox_begin(c, j.n, j.msg->stride, c->raw_scan);
-        } else {
-            status[i] = pc2_begin(c, j.msg->pc2, j.m, c->raw_scan, c->raw_scan_side);
-        }
+        status[i] = wire_accept(ctxs[i], msgs[i], out ? out[i] : nullptr, cap ? cap[i] : 0, n + i, j);
+        if (status[i] == LILIOM_OK) status[i] = wire_begin(j);
         if (status[i] != LILIOM_OK) continue;
         jobs.push_back(j);
         at.push_back(i);
@@ -438,29 +420,8 @@ extern "C" int liliom_convert_batch(liliom_ctx* const* ctxs, int B, const liliom
     LILI_TRY(batch_join_in(c0, all));
     {
         const BatchStreams on_c0(all, c0->stream);
-        std::vector<int> livox, pc2;        // jobs with points, by kind
-        for (size_t k = 0; k < jobs.size(); ++k) {
-            const WireJob& j = jobs[k];
-            if (wire_is_livox(j)) LILI_TRY(livox_copy(j.c, j.msg->custom_pts, j.n, j.msg->stride));
-            else LILI_TRY(pc2_copy(j.c, j.msg->pc2, j.m));
-            if (j.n > 0) (wire_is_livox(j) ? livox : pc2).push_back((int)k);
-        }
-        LILI_TRY(stage_batch<WireStLivox>(c0, livox, [&](LivoxEntry& e, int k) {
-            const WireJob& j = jobs[k];
-            e = LivoxEntry{j.c->wire_in.as<const unsigned char>(), j.n, j.msg->stride, j.c->raw_scan.as<unsigned char>()};
-            return j.c;
-        }));
-        LILI_TRY(stage_batch<WireStPc2>(c0, pc2, [&](Pc2Entry& e, int k) {
-            WireJob& j = jobs[k];
-            Pc2Side& side = j.c->raw_scan_side;
-            e = Pc2Entry{j.c->wire_in.as<const unsigned char>(), j.n, pc2_wire(j.msg->pc2, j.m), j.c->raw_scan.as<unsigned char>(),
-                         pc2_ring_out(j.m, side), pc2_time_out(j.m, side)};
-            return j.c;
-        }));
-        for (WireJob& j : jobs) {
-            if (!wire_is_livox(j)) pc2_finish(j.m, j.c->raw_scan_side);
-            LILI_TRY(resident_finish(j.c, j.n, wire_is_livox(j) ? 48 : 32, j.out));
-        }
+        LILI_TRY(wire_decode(c0, jobs));
+        for (const WireJob& j : jobs) LILI_TRY(resident_finish(j.c, j.n, wire_is_livox(j) ? 48 : 32, j.out));
     }
     // one synchronise for the whole call
     LILI_TRY(batch_join_out(c0, all));

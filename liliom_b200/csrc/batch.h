@@ -15,13 +15,14 @@ namespace lili {
 
 constexpr int kBatchMax = 32;                 // sessions per batched launch
 
-// The session table of a batched launch.  A launch that needs launch-wide scalars declares them beside it in a derived struct.
-// Every table must fit the 32 764-byte kernel parameter space: batch_tables (ctx.cuh), which fills them all, checks it.
-template <class Entry>
+// The session table of a batched launch, for up to N sessions.  A launch that needs launch-wide scalars declares them beside it
+// in a derived struct.  Every table must fit the 32 764-byte kernel parameter space: batch_tables (ctx.cuh), which fills them
+// all, checks it.  The stage chains launch a one-session launch with N = 1, so that it carries one entry rather than kBatchMax.
+template <class Entry, int N = kBatchMax>
 struct BatchTab {
     int n;                              // sessions in this launch
-    int off[kBatchMax + 1];             // session s owns blocks [off[s], off[s + 1])
-    Entry s[kBatchMax];
+    int off[N + 1];                     // session s owns blocks [off[s], off[s + 1])
+    Entry s[N];
 };
 
 // The session that block b of a shared grid belongs to: the last s with off[s] <= b.  A session without blocks owns none; the last

@@ -165,8 +165,8 @@ struct BatchSlot {
     int s;
     SessionBlock blk;
 };
-template <class Entry>
-__device__ __forceinline__ BatchSlot batch_slot(const BatchTab<Entry>& tab) {
+template <class Entry, int N>
+__device__ __forceinline__ BatchSlot batch_slot(const BatchTab<Entry, N>& tab) {
     const int s = batch_session_of(tab.n, tab.off, (int)blockIdx.x);
     return BatchSlot{s, SessionBlock{(int)blockIdx.x - tab.off[s], (unsigned int)(tab.off[s + 1] - tab.off[s])}};
 }
@@ -187,8 +187,8 @@ __device__ __forceinline__ BatchSlot batch_slot(const BatchTab<Entry>& tab) {
             CALL;                                                                                     \
         }                                                                                             \
     };
-template <class St>
-__global__ void __launch_bounds__(St::kThreads) k_stage_batch(const __grid_constant__ BatchTab<typename St::Entry> tab) {
+template <class St, int N>
+__global__ void __launch_bounds__(St::kThreads) k_stage_batch(const __grid_constant__ BatchTab<typename St::Entry, N> tab) {
     const BatchSlot at = batch_slot(tab);
     St::run(tab.s[at.s], at.blk.bi());
 }
@@ -643,11 +643,16 @@ inline int batch_join_in(liliom_ctx* c0, const std::vector<liliom_ctx*>& cs) {
     }
     return LILIOM_OK;
 }
-// ... and after them: c0->ev_batch is recorded behind the last shared launch, and the others' streams wait for it
+// ... and after them: c0->ev_batch is recorded behind the last shared launch, and the others' streams wait for it (no event when
+// every session is on c0's stream)
 inline int batch_join_out(liliom_ctx* c0, const std::vector<liliom_ctx*>& cs) {
-    LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, c0->stream));
-    for (liliom_ctx* c : cs)
-        if (c->stream != c0->stream) LILI_CUDA(c, cudaStreamWaitEvent(c->stream, c0->ev_batch, 0));
+    bool recorded = false;
+    for (liliom_ctx* c : cs) {
+        if (c->stream == c0->stream) continue;
+        if (!recorded) LILI_CUDA(c0, cudaEventRecord(c0->ev_batch, c0->stream));
+        recorded = true;
+        LILI_CUDA(c, cudaStreamWaitEvent(c->stream, c0->ev_batch, 0));
+    }
     return LILIOM_OK;
 }
 
@@ -657,20 +662,25 @@ struct BatchPart {
     int blocks;
 };
 // The launches of type Tab (a BatchTab, batch.h) over the sessions `ids`, in order, at most kBatchMax sessions each (one launch
-// for a packer's launch, which holds no more): part = fill(tab.s[m], ids[m]) writes session m's entry and gives its context and
-// blocks, off[] follows the blocks, every session's launch count advances by one, then launch(tab, grid) queues the launch.
-template <class Tab, class Fill, class Launch>
+// for a packer's launch, which holds no more); a launch of one session fills a Tab1 instead (the one-entry table of the stage
+// chains).  part = fill(tab.s[m], ids[m]) writes session m's entry and gives its context and blocks, off[] follows the blocks,
+// every session's launch count advances by one, then launch(tab, grid) queues the launch.
+template <class Tab, class Tab1 = Tab, class Fill, class Launch>
 int batch_tables(const std::vector<int>& ids, Fill fill, Launch launch) {
-    static_assert(sizeof(Tab) <= 32764, "a batched launch's session table must fit in the kernel parameter space");
-    for (size_t first = 0; first < ids.size(); first += kBatchMax) {
-        Tab tab{};
-        tab.n = (int)(ids.size() - first < (size_t)kBatchMax ? ids.size() - first : (size_t)kBatchMax);
-        for (int m = 0; m < tab.n; ++m) {
+    static_assert(sizeof(Tab) <= 32764 && sizeof(Tab1) <= 32764, "a batched launch's session table must fit in the kernel parameter space");
+    auto queue = [&](auto& tab, size_t first, int n) -> int {
+        tab.n = n;
+        for (int m = 0; m < n; ++m) {
             const BatchPart p = fill(tab.s[m], ids[first + m]);
             tab.off[m + 1] = tab.off[m] + p.blocks;
             p.c->cnt.launches++;
         }
-        LILI_TRY(launch(tab, tab.off[tab.n]));
+        return launch(tab, tab.off[n]);
+    };
+    for (size_t first = 0; first < ids.size(); first += kBatchMax) {
+        const int n = (int)(ids.size() - first < (size_t)kBatchMax ? ids.size() - first : (size_t)kBatchMax);
+        if (n == 1) { Tab1 tab{}; LILI_TRY(queue(tab, first, n)); }
+        else { Tab tab{}; LILI_TRY(queue(tab, first, n)); }
     }
     return LILIOM_OK;
 }
@@ -679,13 +689,14 @@ int batch_tables(const std::vector<int>& ids, Fill fill, Launch launch) {
 // One stage (LILI_STAGE) for the sessions `which` on c0's stream: fill(entry, id) writes session id's entry and returns its context.
 template <class St, class Fill>
 int stage_batch(liliom_ctx* c0, const std::vector<int>& which, Fill fill) {
-    typedef BatchTab<typename St::Entry> Tab;
-    return batch_tables<Tab>(which, [&](typename St::Entry& e, int id) { liliom_ctx* c = fill(e, id); return BatchPart{c, St::blocks(e)}; },
-                             [&](const Tab& tab, int grid) -> int {
-                                 k_stage_batch<St><<<grid, St::kThreads, 0, c0->stream>>>(tab);
-                                 LILI_CUDA(c0, cudaGetLastError());
-                                 return LILIOM_OK;
-                             });
+    typedef typename St::Entry Entry;
+    return batch_tables<BatchTab<Entry>, BatchTab<Entry, 1>>(
+        which, [&](Entry& e, int id) { liliom_ctx* c = fill(e, id); return BatchPart{c, St::blocks(e)}; },
+        [&](const auto& tab, int grid) -> int {
+            k_stage_batch<St><<<grid, St::kThreads, 0, c0->stream>>>(tab);
+            LILI_CUDA(c0, cudaGetLastError());
+            return LILIOM_OK;
+        });
 }
 #endif
 

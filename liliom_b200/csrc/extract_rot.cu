@@ -545,9 +545,8 @@ struct RotRingEntry {
     const Pt32* cloud; const float* curv; int* meta; int* label; int* lessflat; int* seg_edge; int* seg_cnt;
     int ds_rate, fast_cap;
 };
-typedef BatchTab<RotRingEntry> RotRingBatch;
-
-__global__ void __launch_bounds__(512) k_rot_ring_batch(const __grid_constant__ RotRingBatch tab) {
+template <int N>
+__global__ void __launch_bounds__(512) k_rot_ring_batch(const __grid_constant__ BatchTab<RotRingEntry, N> tab) {
     const BatchSlot at = batch_slot(tab);
     const RotRingEntry e = tab.s[at.s]; // a by-value copy, as k_rot_ring's parameters
     rot_ring_body(e.cloud, e.curv, e.meta, e.ds_rate, e.label, e.lessflat, e.seg_edge, e.seg_cnt, nullptr, e.fast_cap, at.blk.bi());
@@ -900,14 +899,15 @@ static int rot_stage(liliom_ctx* c0, const std::vector<RotEntry>& E, const std::
 
 // The rings of the sessions `which`: k_rot_ring_batch launches, one block per ring.
 static int rot_ring_stage(liliom_ctx* c0, const std::vector<liliom_ctx*>& cs, const std::vector<int>& which) {
-    LILI_CUDA(c0, cudaFuncSetAttribute(k_rot_ring_batch, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RingSmem)));
-    return batch_tables<RotRingBatch>(which, [&](RotRingEntry& e, int i) {
+    LILI_CUDA(c0, cudaFuncSetAttribute(k_rot_ring_batch<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RingSmem)));
+    LILI_CUDA(c0, cudaFuncSetAttribute(k_rot_ring_batch<kBatchMax>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(RingSmem)));
+    return batch_tables<BatchTab<RotRingEntry>, BatchTab<RotRingEntry, 1>>(which, [&](RotRingEntry& e, int i) {
         liliom_ctx* c = cs[i];
         const RotBufs b(c);
         e = RotRingEntry{b.cloud, c->rot_curv.as<float>(), b.meta, c->rot_label.as<int>(), c->rot_lessflat.as<int>(), b.seg_edge,
                          b.seg_cnt, c->prm.ds_rate, c->rot_slow_walk ? 0 : ROT_FAST_CAP};
         return BatchPart{c, c->prm.line_num};
-    }, [&](const RotRingBatch& tab, int grid) -> int {
+    }, [&](const auto& tab, int grid) -> int {
         k_rot_ring_batch<<<grid, 512, sizeof(RingSmem), c0->stream>>>(tab);
         LILI_CUDA(c0, cudaGetLastError());
         return LILIOM_OK;

@@ -1,6 +1,5 @@
-// The per-point decode of the two driver formats the library takes, shared by the solo kernels (k_livox_to_pt48,
-// k_pc2_to_pt32), the batched stages of liliom_convert_batch (api.cu) and the CPU tests (tests/wire_host.cpp compiles this
-// same file):
+// The per-point decode of the two driver formats the library takes, shared by the decode stages (WireStLivox, WireStPc2 in
+// api.cu) and the CPU tests (tests/wire_host.cpp compiles this same file):
 //   * livox_ros_driver::CustomPoint -> pcl::PointXYZINormal (FormatConvert, L/src/FormatConvert.cpp:11-24);
 //   * one point of a sensor_msgs/PointCloud2 -> pcl::PointXYZI (pcl::fromROSMsg, R/src/Preprocessing.cpp:277), with the ring
 //     and time side channels of LILIOM_RING_FIELD / LILIOM_TIME_FIELD (field matching: pc2_fields.h).
@@ -69,7 +68,7 @@ VGB_HD void pc2_point_at(const unsigned char* __restrict__ in, int n, const Pc2W
     const unsigned r = (unsigned)i / w.width, col = (unsigned)i - r * w.width;
     const unsigned char* p = in + (size_t)r * w.row_step + (size_t)col * w.point_step;
     auto fld = [p](int off) { return off < 0 ? 0.0f : wire_bits_f32(rd32(p + off)); };
-    // the fields are read before each output address is formed, the order that keeps k_pc2_to_pt32's SASS (and 32 registers)
+    // the fields are read before each output address is formed, the order that keeps the decode at 32 registers
     const float x = fld(w.src[0]), y = fld(w.src[1]), z = fld(w.src[2]);
     vg_st4(out + (size_t)i * 32, x, y, z, 1.0f);                                        // pcl::PointXYZI default ctor: data[3] = 1
     const float intensity = fld(w.src[3]);

@@ -6,12 +6,21 @@ extern "C" int bh_stage_blocks(int items, int threads) { return lili::stage_bloc
 extern "C" int bh_box_blocks(int n, int sm_count) { return lili::box_blocks(n, sm_count); }
 // session of block b among n <= kBatchMax sessions with blocks[s] blocks each, looked up in the prefix offsets of a launch's
 // table; *place: the block's place inside its session
-extern "C" int bh_session_of(int n, const int* blocks, int b, int* place) {
-    int off[lili::kBatchMax + 1] = {0};
-    for (int s = 0; s < n; ++s) off[s + 1] = off[s] + blocks[s];
-    const int s = lili::batch_session_of(n, off, b);
-    *place = b - off[s];
+template <class Tab>
+static int session_of(int n, const int* blocks, int b, int* place) {
+    Tab tab{};
+    tab.n = n;
+    for (int s = 0; s < n; ++s) tab.off[s + 1] = tab.off[s] + blocks[s];
+    const int s = lili::batch_session_of(tab.n, tab.off, b);
+    *place = b - tab.off[s];
     return s;
+}
+extern "C" int bh_session_of(int n, const int* blocks, int b, int* place) {
+    return session_of<lili::BatchTab<int>>(n, blocks, b, place);
+}
+// the same in the one-entry table of a one-session launch (n == 1)
+extern "C" int bh_session_of1(int n, const int* blocks, int b, int* place) {
+    return session_of<lili::BatchTab<int, 1>>(n, blocks, b, place);
 }
 // batch_pack of B sessions {grid, kind, coop}: out_kind / out_grid / out_count per launch, out_sess the launches' sessions in
 // order, solo the sessions on their solo path.  Returns the launch count; *n_solo the solo count.

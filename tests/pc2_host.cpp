@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE: host build of liliom_b200/csrc/pc2_fields.h, the PointCloud2 field matching and validation of
 // liliom_convert_pc2 / liliom_extract_rot_pc2 / liliom_pre_cloud_pc2 (with the `ring` field of LILIOM_RING_FIELD and the time
-// field of LILIOM_TIME_FIELD), the per-point reads k_pc2_to_pt32 shares with the host (pc2_ring_value, pc2_time_value) and the
+// field of LILIOM_TIME_FIELD), the per-point reads the PointCloud2 decode stage shares with the host (pc2_ring_value, pc2_time_value) and the
 // relTime expression k_rot_build uses (pc2_rel_time), so that the CPU test tier checks the SAME SOURCE they use.
 #include "../liliom_b200/csrc/pc2_fields.h"
 

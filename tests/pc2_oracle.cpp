@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE: an independent CPU restatement of pcl::fromROSMsg(sensor_msgs::PointCloud2 -> pcl::PointXYZI)
-// (R/src/Preprocessing.cpp:277), the reference the device decode (k_pc2_to_pt32) is compared against.  It deliberately does not
+// (R/src/Preprocessing.cpp:277), the reference the device decode (WireStPc2) is compared against.  It deliberately does not
 // include the library's pc2_fields.h: field matching and the copy are written out again here.
 // from-knowledge (PCL 1.8-1.10, conversions.h / point_cloud.h): createMapping maps each field of the point type to the FIRST
 // message field with the same name, the same datatype (FLOAT32 = 7) and count 1 (or 0); fromPCLPointCloud2 then copies each

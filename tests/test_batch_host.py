@@ -15,16 +15,18 @@ def ms():
                         deps=["liliom_b200/csrc/batch.h"])
     ip = C.POINTER(C.c_int)
     L.bh_session_of.argtypes = [C.c_int, ip, C.c_int, ip]
+    L.bh_session_of1.argtypes = [C.c_int, ip, C.c_int, ip]
     L.bh_pack.argtypes = [C.c_int, ip, ip, C.c_int, C.c_int, ip, ip, ip, ip, ip, ip]
     L.bh_pack.restype = C.c_int
     L.bh_batch_max.restype = C.c_int
     return L
 
 
-def _walk(ms, blocks, b):
+def _walk(ms, blocks, b, one_entry=False):
     arr = (C.c_int * len(blocks))(*blocks)
     place = C.c_int()
-    return ms.bh_session_of(len(blocks), arr, b, C.byref(place)), place.value
+    lookup = ms.bh_session_of1 if one_entry else ms.bh_session_of
+    return lookup(len(blocks), arr, b, C.byref(place)), place.value
 
 
 def _pack(ms, items, occ, sm, maxper):
@@ -66,13 +68,15 @@ def test_every_block_finds_its_session_and_place(ms):
         if sum(blocks) == 0:
             continue
         want = [(s, p) for s, n in enumerate(blocks) for p in range(n)]
-        got = [_walk(ms, blocks, b) for b in range(sum(blocks))]
-        assert got == want, blocks
+        for one_entry in ((False, True) if len(blocks) == 1 else (False,)):    # a one-session launch carries a one-entry table
+            got = [_walk(ms, blocks, b, one_entry) for b in range(sum(blocks))]
+            assert got == want, (blocks, one_entry)
 
 
 def test_one_session_owns_the_whole_grid(ms):
-    for b in range(9):
-        assert _walk(ms, [9], b) == (0, b)
+    for one_entry in (False, True):
+        for b in range(9):
+            assert _walk(ms, [9], b, one_entry) == (0, b)
 
 
 def test_horizon_sessions_four_per_launch(ms):

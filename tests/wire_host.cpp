@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE: host build of liliom_b200/csrc/wire_decode.h, the per-point decode of the Livox CustomPoint records and
-// of PointCloud2 messages that the solo kernels (k_livox_to_pt48, k_pc2_to_pt32) and the batched stages of liliom_convert_batch
-// share, so that the CPU test tier checks the SAME SOURCE they run.
+// of PointCloud2 messages that the decode stages of the convert calls (WireStLivox, WireStPc2 in api.cu) run, so that the
+// CPU test tier checks the SAME SOURCE they run.
 #include "../liliom_b200/csrc/wire_decode.h"
 
 // n records of `stride` bytes -> n PointXYZINormal (48 bytes each) at out
