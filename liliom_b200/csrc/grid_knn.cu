@@ -766,6 +766,10 @@ __global__ void k_gn_update(const double* __restrict__ neq, double* __restrict__
 // TrustRegionMinimizer + LevenbergMarquardtStrategy on thread 0 (Jacobi scaling fixed at
 // iteration 0, D = sqrt(clamp(diag)/radius), rho-based radius update), with the dense QR on
 // [J; D] replaced by its normal equations (J^T J + D^2) y = J^T r in fp64 (6x6 LDL^T).
+// Three Ceres rules, as tests/lm_reference.py settles them: the start counts as a successful step, so the gradient test
+// also runs before iteration 1 (TrustRegionMinimizer::IterationZero); the gradient's size is |x - Plus(x, -g)|_inf in the
+// ambient coordinates (TrustRegionMinimizer::EvaluateGradientAndJacobian); an invalid step is a rejected one, radius divided
+// by decrease_factor, which doubles, diagonal kept (LevenbergMarquardtStrategy::StepIsInvalid -> StepRejected(0)).
 struct LmArgs {
     const float4* feats; const unsigned char* valid; const float4* plane; int n; const int* n_dev;
     double* pose;         // in/out
@@ -808,7 +812,7 @@ __device__ __forceinline__ void lm_solve_body(const LmArgs& a) {
     lm_eval(a, x, S, red);          // iteration 0: cost, gradient, J^T J at x
     // --- thread-0 state (replicated arithmetic is avoided: only thread 0 decides) ---
     double radius = 1e4, decrease_factor = 2.0;
-    bool reuse_diagonal = false, last_successful = false;
+    bool reuse_diagonal = false, last_successful = true;      // IterationZero: the start is a successful step
     double diagonal[6], scaling[6];
     double x_cost = S[27];
     int iteration = 0, invalid = 0;
@@ -826,10 +830,18 @@ __device__ __forceinline__ void lm_solve_body(const LmArgs& a) {
             for (;;) {   // loop over invalid steps without evaluation
                 if (count0 <= 0.0) { cmd = 0; break; }
                 if (iteration >= a.max_num_iter) { cmd = 0; break; }
-                if (last_successful) {
-                    double gmax = 0;
-                    for (int k = 0; k < 6; ++k) gmax = fmax(gmax, fabs(S[21 + k]));
-                    if (gmax <= 1e-10) { cmd = 0; break; }
+                if (last_successful) {      // |x - Plus(x, -g)|_inf
+                    // the translation part first, as Plus forms it: when it alone exceeds the tolerance the decision is
+                    // made, and the quaternion part (sincos on this single thread for a large g) is only formed near a stop
+                    double tmax = 0;
+                    for (int k = 0; k < 3; ++k) tmax = fmax(tmax, fabs(x[4 + k] - (x[4 + k] + -S[24 + k])));
+                    if (tmax <= 1e-10) {
+                        double ng[6], xg[7], gmax = 0;
+                        for (int k = 0; k < 6; ++k) ng[k] = -S[21 + k];
+                        pose_plus(x, ng, xg);
+                        for (int k = 0; k < 7; ++k) gmax = fmax(gmax, fabs(x[k] - xg[k]));
+                        if (gmax <= 1e-10) { cmd = 0; break; }
+                    }
                 }
                 if (radius < 1e-32) { cmd = 0; break; }
                 ++iteration;
@@ -868,7 +880,8 @@ __device__ __forceinline__ void lm_solve_body(const LmArgs& a) {
                 }
                 if (!ok || !(model_cost_change > 0.0)) {
                     if (++invalid >= 5) { cmd = 0; break; }
-                    radius *= 0.5; reuse_diagonal = false;
+                    radius = radius / decrease_factor;      // StepIsInvalid = StepRejected(0)
+                    decrease_factor *= 2.0;
                     continue;
                 }
                 invalid = 0;

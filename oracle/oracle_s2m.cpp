@@ -271,6 +271,10 @@ extern "C" int orc_scan_to_map_gn(const void* tree, const float* map_xyzw, int m
 //   jacobi scaling 1/(1+||col||) fixed at iteration 0; D = sqrt(clamp(diag(J^T J),1e-6,1e32)/radius);
 //   radius0 = 1e4, max 1e16, min 1e-32; min_relative_decrease 1e-3; function_tolerance 1e-6;
 //   parameter_tolerance 1e-8; gradient_tolerance 1e-10; monotonic steps.
+//   The start counts as a successful step (TrustRegionMinimizer::IterationZero), so the gradient test runs before
+//   iteration 1 too; the gradient's size is |x - Plus(x, -g)|_inf (EvaluateGradientAndJacobian); an invalid step is
+//   LevenbergMarquardtStrategy::StepIsInvalid = StepRejected(0): radius / decrease_factor, decrease_factor doubled,
+//   diagonal kept.  tests/lm_reference.py restates the same rules with their sources.
 // ---------------------------------------------------------------------------------------
 namespace {
 struct Corr { float p[4]; float pl[4]; };
@@ -365,12 +369,15 @@ static int ceres_lm(const std::vector<Corr>& c, double x[7], int max_num_iter, d
     scale_jac();
     double x_norm = 0; for (int k = 0; k < 7; ++k) x_norm += x[k] * x[k]; x_norm = std::sqrt(x_norm);
     int iteration = 0, invalid = 0;
-    bool last_successful = false;
+    bool last_successful = true;        // IterationZero marks the start a successful step
     for (;;) {
         // FinalizeIterationAndCheckIfMinimizerCanContinue
         if (iteration >= max_num_iter) break;
-        if (last_successful) {
-            double gmax = 0; for (int k = 0; k < 6; ++k) gmax = std::max(gmax, std::fabs(L.g[k]));
+        if (last_successful) {           // GradientToleranceReached on |x - Plus(x, -g)|_inf
+            double ng[6], xg[7], gmax = 0;
+            for (int k = 0; k < 6; ++k) ng[k] = -L.g[k];
+            pose_plus(x, ng, xg);
+            for (int k = 0; k < 7; ++k) gmax = std::max(gmax, std::fabs(x[k] - xg[k]));
             if (gmax <= gradient_tolerance) break;
         }
         if (radius < min_radius) break;
@@ -399,9 +406,10 @@ static int ceres_lm(const std::vector<Corr>& c, double x[7], int max_num_iter, d
             }
         }
         if (!ok || !(model_cost_change > 0.0)) {
-            // HandleInvalidStep
+            // HandleInvalidStep -> StepIsInvalid = StepRejected(0)
             if (++invalid >= 5) break;
-            radius *= 0.5; reuse_diagonal = false;
+            radius = radius / decrease_factor;
+            decrease_factor *= 2.0;
             continue;
         }
         invalid = 0;

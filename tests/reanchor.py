@@ -21,6 +21,14 @@ Ceres-faithful mode (check_ceres), every outer iteration k from start_k: the ora
 at rtol 1e-9; the device's planes when probed, as in (b)), then oracle.ceres_solve on them from start_k must take exactly
 st[k].lm_iters iterations and land within ceres_tolerance of st[k].pose7.
 
+Per LM iteration (check_ceres with `truncated`): a match_cnt = 1 call stops as soon as its iteration count reaches
+max_num_iter and freezes its correspondences at its start, so the calls truncated(start_k, j) for j = 0 .. lm_iters + 1
+return the device's iterate after each iteration, bit for bit the computation of the full pass.  lm_reference.follow carries
+Ceres' trust-region state along those iterates: every decision (moved = accepted; unmoved = rejected, invalid or stopped)
+must match an admissible reference trace, the stop iteration exactly, and every accepted step must land within the one-step
+bound of the reference's candidate (the block reduction's gamma_d sum(|terms|) per scalar, the damped system's conditioning
+and LDL^T's backward error, and the radius carried).  The distance from the QR step is reported next to it.
+
 Both raise ReanchorError (an AssertionError) naming the pass and the check that failed, and return a report of the largest
 deviations seen, each next to its bound.
 """
@@ -256,9 +264,48 @@ def ceres_tolerance(start, pose_o, s29, lm_iters, e):
         PLUS_ULPS * U * max(lm_iters, 1) * max(1.0, float(np.linalg.norm(np.asarray(start)[4:])) + move)
 
 
-def check_ceres(oracle, tree, feats, guess, st, max_num_iter, nthreads=1, what="CERES", probe=None):
+def trace_pass(feats, valid, plane, start, lm_iters, truncated, max_num_iter, k, what, rep):
+    """The per-iteration check of one outer pass (see the module docstring): truncated(start, j) -> (pose after j LM
+    iterations, the call's iteration count)."""
+    import lm_reference as LR
+    iterates = [np.asarray(start, np.float64)]
+    for j in range(1, lm_iters + 2):
+        if j > max_num_iter:
+            break
+        pose, it = truncated(start, j)
+        if it != min(j, lm_iters):
+            _fail(f"{what} pass {k}: the call capped at {j} LM iterations reports {it}, the uncapped one {lm_iters}")
+        iterates.append(np.asarray(pose, np.float64))
+    try:
+        tr = LR.follow(feats, valid, plane, start, iterates, lm_iters, max_num_iter)
+    except LR.TraceError as e:
+        _fail(f"{what} pass {k}: trace: {e}")
+    rep["trace_ratio"] = max(rep.get("trace_ratio", 0.0), tr["ratio"])
+    if tr["ratio"] >= rep.get("trace_ratio", 0.0):
+        rep["trace_dev"], rep["trace_bound"] = tr["dev"], tr["bound"]
+    rep.setdefault("branches", []).extend(tr["branches"])
+    rep.setdefault("stops", []).append(tr["stop"])
+    qr = [r["dev_qr"] for r in tr["records"] if "dev_qr" in r]
+    if qr:
+        rep["qr_dev"] = max(rep.get("qr_dev", 0.0), max(qr))
+        # what a QR solve itself meets on the augmented system: u (kappa + kappa^2 |res| / (|A| |y|)) |y|, first order
+        rep["qr_bound"] = max(rep.get("qr_bound", 0.0), max(U * (r["cond_aug"] + r["cond_aug"] ** 2) * float(np.linalg.norm(r["y_qr"]))
+                                                              for r in tr["records"] if "dev_qr" in r))
+    acc = [r for r in tr["records"] if r["branch"] == "accepted" and "candidate" in r]
+    rep["bound_over_step"] = max([rep.get("bound_over_step", 0.0)] +
+                                 [r["step_bound"] / max(float(np.linalg.norm(r["candidate"] - r["x_before"])), 1e-300) for r in acc])
+    rep["mcc_gap"] = max([rep.get("mcc_gap", 0.0)] + [abs(r["mcc_normal"] - r["mcc_qr"]) / abs(r["mcc_normal"])
+                                                      for r in tr["records"] if "mcc_qr" in r and r["mcc_normal"] != 0])
+    rep["open_decisions"] = rep.get("open_decisions", 0) + sum(len(r["open"]) for r in tr["records"])
+    rep["step_bound_sum"] = max(rep.get("step_bound_sum", 0.0), sum(r.get("step_bound", 0.0) for r in tr["records"] if r["branch"] == "accepted"))
+    return tr
+
+
+def check_ceres(oracle, tree, feats, guess, st, max_num_iter, nthreads=1, what="CERES", probe=None, truncated=None,
+                trace_passes=None):
     """Check every outer iteration of one Ceres-faithful call.  Returns the largest sum deviation as a share of its bound and the
-    largest pose deviation with the bound it was held to."""
+    largest pose deviation with the bound it was held to.  With truncated(start, j) (the device's match_cnt = 1 call capped at
+    j LM iterations from `start`), the passes in trace_passes (all by default) are also checked iteration by iteration."""
     rep = dict(sum_ratio=0.0, pose_dev=0.0, pose_bound=0.0, pose_ratio=0.0, lm_iters=[s.lm_iters for s in st])
     for k, (start, s) in enumerate(zip(start_poses(guess, st), st)):
         valid, plane, e = _oracle_pass(oracle, tree, feats, start, s, k, nthreads, what, probe, rep)
@@ -275,4 +322,6 @@ def check_ceres(oracle, tree, feats, guess, st, max_num_iter, nthreads=1, what="
         if dev > rep["pose_dev"]:
             rep["pose_dev"], rep["pose_bound"] = dev, tol
         rep["pose_ratio"] = max(rep["pose_ratio"], dev / tol)
+        if truncated is not None and (trace_passes is None or k in trace_passes):
+            trace_pass(feats, valid, plane, start, s.lm_iters, truncated, max_num_iter, k, what, rep)
     return rep

@@ -12,7 +12,9 @@ Covered: world_small's down-sampled scan, every surf feature, 3000 of them, 40 a
 upload_feats + scan_to_map_resident; every forced search shape of test_gpu_knn_exact.py, on the persistent launch and on per-pass
 launches, and the 16-lane persistent launch with bulk-copy staging (LILIOM_KNN_TMA=1, one round and three); odometry_resident after extract_resident (Horizon and ROT), whose want_stats=False pose must carry the same bits; the
 single plane (plain step), the exactly flat plane (damped step), and a guess rolled 0.8 rad over both (trust-region clip); and
-BASELINE configs 1 and 2 at size (1 M and 2 M maps).  Each check prints one `reanchor` line with its largest deviations and bounds."""
+BASELINE configs 1 and 2 at size (1 M and 2 M maps).  In the Ceres-faithful mode the scan_to_map calls are also checked LM
+iteration by LM iteration (reanchor.trace_pass; configs 1 and 2 on their first outer pass).  Each check prints one `reanchor`
+line with its largest deviations and bounds."""
 import json
 
 import numpy as np
@@ -38,7 +40,10 @@ def _same_points(a, b):
 
 
 def _say(what, rep):
-    keep = {k: (round(float(v), 4) if k.endswith("ratio") else float(v)) for k, v in rep.items() if k not in ("branches", "n_corr", "lm_iters")}
+    keep = {k: (round(float(v), 4) if k.endswith("ratio") else float(v)) for k, v in rep.items()
+            if k not in ("branches", "n_corr", "lm_iters", "stops")}
+    if "stops" in rep:
+        keep["stops"] = sorted(set(rep["stops"]))
     if "branches" in rep:
         keep["branches"] = sorted(set(rep["branches"]))
     print(f"reanchor {what} {json.dumps(keep)}")
@@ -56,8 +61,20 @@ def _gn(oracle, dm, tree, feats, guess, st, what, probe, nthreads=8):  # noqa: F
     return rep
 
 
-def _ceres(oracle, tree, feats, guess, st, what, probe, nthreads=8):
-    rep = RA.check_ceres(oracle, tree, feats, guess, st, CERES_LM, nthreads, what, probe)
+def truncated_of(ctx, feats):
+    """The device's match_cnt = 1 Ceres-faithful call from `start` capped at j LM iterations: (pose, its iteration count).
+    From a context like probe_of's, so the call under test is not disturbed."""
+    import liliom_b200 as L
+
+    def run(start, j):
+        pose, st = ctx.scan_to_map(feats, start, 1, max_num_iter=j, mode=L.MODE_CERES)
+        return pose, st[0].lm_iters
+    return run
+
+
+def _ceres(oracle, tree, feats, guess, st, what, probe, nthreads=8, truncated=None, trace_passes=None):
+    """The end-of-pass check and, given truncated (truncated_of), every LM iteration of the passes in trace_passes."""
+    rep = RA.check_ceres(oracle, tree, feats, guess, st, CERES_LM, nthreads, what, probe, truncated, trace_passes)
     _say(what, rep)
     return rep
 
@@ -95,7 +112,7 @@ def test_world_small_every_pass(oracle, dm, ws, fs):  # noqa: F811
         pose_n, none = c.scan_to_map_resident(guess, ITERS, mode=L.MODE_GN, want_stats=False)
         assert none is None and pose_n.tobytes() == pose_r.tobytes()
         pose, st = c.scan_to_map(feats, guess, CERES_OUTER, max_num_iter=CERES_LM, mode=L.MODE_CERES)
-        _ceres(oracle, tree, feats, guess, st, f"world_small/{fs}/scan_to_map", pr)
+        _ceres(oracle, tree, feats, guess, st, f"world_small/{fs}/scan_to_map", pr, truncated=truncated_of(pc, feats))
         pose_r, st_r = c.scan_to_map_resident(guess, CERES_OUTER, max_num_iter=CERES_LM, mode=L.MODE_CERES, want_stats=True)
         _ceres(oracle, tree, feats, guess, st_r, f"world_small/{fs}/resident", pr)
     finally:
@@ -122,7 +139,7 @@ def test_forced_search_shapes_every_pass(oracle, dm, ws, shape):  # noqa: F811
         _, st = c.scan_to_map(big, guess, 4, mode=L.MODE_GN)
         _gn(oracle, dm, tree, big, guess, st, f"shape {_ids(shape)}/per_pass", probe_of(pc, big))
         _, st = c.scan_to_map(f4, guess, CERES_OUTER, max_num_iter=CERES_LM, mode=L.MODE_CERES)
-        _ceres(oracle, tree, f4, guess, st, f"shape {_ids(shape)}/ceres", probe_of(pc, f4))
+        _ceres(oracle, tree, f4, guess, st, f"shape {_ids(shape)}/ceres", probe_of(pc, f4), truncated=truncated_of(pc, f4))
     finally:
         c.close(); pc.close()
 
@@ -212,7 +229,7 @@ def test_degenerate_geometry_branches(oracle, dm, name):  # noqa: F811
             assert set(rep["branches"]) == {"damped"}
         assert np.all(np.isfinite(pose))
         _, st = c.scan_to_map(feats, guess, CERES_OUTER, max_num_iter=CERES_LM, mode=L.MODE_CERES)
-        _ceres(oracle, tree, feats, guess, st, f"plane/{name}/ceres", pr)
+        _ceres(oracle, tree, feats, guess, st, f"plane/{name}/ceres", pr, truncated=truncated_of(pc, feats))
     finally:
         c.close(); pc.close()
 
@@ -244,6 +261,6 @@ def test_configs_at_size_every_pass(oracle, dm, config):  # noqa: F811
         _same_points(ds, ds_o)
         _gn(oracle, dm, tree, ds_o, guess, st, f"config{config}/odometry", pr)
         _, st = c.scan_to_map(ds_o, guess, 2, max_num_iter=CERES_LM, mode=L.MODE_CERES)
-        _ceres(oracle, tree, ds_o, guess, st, f"config{config}/ceres", pr)
+        _ceres(oracle, tree, ds_o, guess, st, f"config{config}/ceres", pr, truncated=truncated_of(pc, ds_o), trace_passes=(0,))
     finally:
         c.close(); pc.close()

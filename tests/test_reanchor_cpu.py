@@ -6,6 +6,7 @@ pass by the check that covers it."""
 import numpy as np
 import pytest
 
+import lm_reference as LR
 import reanchor as RA
 from test_devmath_host import dm  # noqa: F401  (the host build of dev_math.cuh, a fixture)
 
@@ -235,56 +236,10 @@ def test_rejects_damping_skipped(oracle, dm, worlds, gn_runs):  # noqa: F811
 
 
 def lm_restated(oracle, feats, valid, plane, start, max_num_iter, grow=None):
-    """grid_knn.cu::k_lm_solve (the device's Ceres-faithful LM on frozen correspondences) restated in NumPy: Jacobi-scaled normal
-    equations, Levenberg damping diag / radius, the model cost change, and Ceres' accept / reject and radius rules.  grow(radius,
-    relative_decrease) replaces the radius update after a successful step, to plant a fault.  Returns (iterations, pose)."""
-    x = np.array(start, np.float64)
-    S = oracle.normal_equations(feats, valid, plane, x)
-    if not S[28] > 0:
-        return 0, RA.unify(x)
-    H, g = RA.unpack(S)
-    scaling = 1.0 / (1.0 + np.sqrt(np.diag(H)))
-    radius, decrease_factor, reuse, last_ok = 1e4, 2.0, False, False
-    x_cost, it, invalid = S[27], 0, 0
-    diag = None
-    while True:
-        if it >= max_num_iter: break
-        if last_ok and np.max(np.abs(g)) <= 1e-10: break
-        if radius < 1e-32: break
-        it += 1; last_ok = False
-        Hs = H * np.outer(scaling, scaling); gs = g * scaling
-        if not reuse:
-            diag = np.clip(np.diag(Hs), 1e-6, 1e32)
-        reuse = True
-        try:
-            step = -np.linalg.solve(Hs + np.diag(diag / radius), gs)
-            ok = np.all(np.isfinite(step))
-        except np.linalg.LinAlgError:
-            ok = False
-        mcc = -(step @ gs + 0.5 * step @ Hs @ step) if ok else 0.0
-        if not ok or not mcc > 0:
-            invalid += 1
-            if invalid >= 5: break
-            radius *= 0.5; reuse = False
-            continue
-        invalid = 0
-        xc = RA.ceres_plus(x, step * scaling)
-        Sc = oracle.normal_equations(feats, valid, plane, xc)
-        if np.linalg.norm(x - xc) <= 1e-8 * (np.linalg.norm(x) + 1e-8): break
-        cc = x_cost - Sc[27]
-        if abs(cc) <= 1e-6 * x_cost: break
-        rd = cc / mcc
-        if rd > 1e-3:
-            x, S, x_cost, last_ok = xc, Sc, Sc[27], True
-            H, g = RA.unpack(S)
-            if grow is None:
-                radius = min(1e16, radius / max(1/3, 1 - (2 * rd - 1) ** 3))
-            else:
-                radius = min(1e16, grow(radius, rd))
-            decrease_factor, reuse = 2.0, False
-        else:
-            radius /= decrease_factor; decrease_factor *= 2.0; reuse = True
-    return it, RA.unify(x)
+    """The Ceres-faithful LM restated in NumPy (tests/lm_reference.py); grow(radius, relative_decrease) replaces the radius
+    update after a successful step, to plant a fault.  Returns (iterations, pose)."""
+    t = LR.run(feats, valid, plane, start, max_num_iter, rules=dict(grow=grow))
+    return t["iters"], t["x"]
 
 
 def test_lm_restatement_matches_oracle_lm(oracle, worlds):
