@@ -668,7 +668,7 @@ typedef struct { double T16[16]; double fitness; int converged, iters, n_src, n_
  * beside nothing else in k_icp_batch runs k_icp_persistent inside the call.  The call waits three times for all sessions together
  * (both clouds' counts, the targets' boxes, the results) where B solo calls wait four times each; a session whose voxel index
  * wraps (wide keys) finishes on its solo path inside the call.  Sessions with an empty source or target get identity,
- * converged = 0 and iters = 0 without an ICP launch, as in the solo call.  The barrier flavour (LILIOM_GN_SYNC) is ctxs[0]'s.
+ * converged = 0 and iters = 0 without an ICP launch, as in the solo call.
  * A session's own error (every error its solo call returns: an unknown id, leaf <= 0, max_corr_dist <= 0, max_iter < 1, a negative
  * k, a NULL list with k > 0; LILIOM_E_GRID) is its status; the others run.
  * LILIOM_E_ARG for the whole call, nothing changed: B < 1, a NULL array (ctxs, src_ids, src_poses7, k_src, tgt_ids, tgt_poses7,

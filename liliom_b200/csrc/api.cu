@@ -121,7 +121,6 @@ extern "C" int liliom_create(liliom_ctx** out, const liliom_params* p, int devic
     c->test_shrink_box = getenv("LILIOM_TEST_SHRINK_BOX") != nullptr;
     if (const char* e10 = getenv("LILIOM_TEST_ICP_BLOCKS")) c->test_icp_blocks = std::max(0, atoi(e10));
     if (const char* e8 = getenv("LILIOM_KNN_TMA")) c->knn_tma = atoi(e8) != 0;
-    if (const char* e5 = getenv("LILIOM_GN_SYNC")) { int v = atoi(e5); if (v == 0 || v == 1 || v == 3) c->gn_sync = v; }
     if (const char* e4 = getenv("LILIOM_SHARD_BLOCK")) {      // shard block edge in metres (power of two, 8..256): larger blocks = thinner halos
         int v = atoi(e4);
         if (v >= 8 && v <= 256 && (v & (v - 1)) == 0) c->shard_inv_block = 1.0f / (float)v;

@@ -313,21 +313,37 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
     return t;
 }
 
-// Grid barrier of the persistent kernels (k_gn_persistent, k_icp_persistent), run by thread 0 of each block after the block's
-// __syncthreads: one arrival on `bar`, then, when `wait`, a poll until the arrivals reach `target`.  sync_mode (LILIOM_GN_SYNC,
-// see liliom_ctx::gn_sync): 3 = release-only arrival and a relaxed poll, 1 = acquire poll, 0 = full fences on both sides.
-__device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int target, int sync_mode, bool wait) {
-    unsigned int v;
-    if (sync_mode == 0) {
+// The grid barrier of every cooperative kernel.  grid_barrier is called by all threads of a block: the block's writes are
+// ordered before one arrival of thread 0 on `bar`, thread 0 polls until the arrivals reach `target`, and the block meets again.
+// grid_arrive is thread 0's part, for a caller that places the block barriers itself: the GN step, whose multi-GPU followers
+// arrive without waiting (wait = false), and the ICP pass.  The flavour is fixed per kernel:
+//   kReleaseOnly (GN, ICP): one release by thread 0 after the block barrier (cumulative over bar.sync, as in cooperative
+//     groups' grid.sync; SASS: MEMBAR.ALL.GPU + RED, no L1 invalidate) and NO acquire fence after the relaxed poll.  An acquire
+//     would only add an L1 invalidation: everything these kernels read through L1 (map, cell table, features, source points) is
+//     immutable for the launch, and the partials are read with L2-scope loads (__ldcg) issued after the poll's control
+//     dependency and a bar.sync.  (The PTX model formally asks for the acquire; an acquire poll and the fenced flavour give the
+//     same bits and are slower per pass: 12.70 us fenced against 11.99 us release-only for the headline GN pass.)
+//   kFenced (Horizon extractor, cooperative VoxelGrid): __threadfence on both sides of an atomicAdd arrival and a volatile poll.
+//     The release-only flavour is legal there too (every cross-block read is an L2-scope load) and was measured to change
+//     nothing: 4586/4629 vs 4653/4563 scans/s.  Those kernels spend their time in the stages, not in the three fences.
+enum GridBarrierFlavour { kReleaseOnly, kFenced };
+template <GridBarrierFlavour F>
+__device__ __forceinline__ void grid_arrive(unsigned int* bar, unsigned int target, bool wait) {
+    if constexpr (F == kFenced) {
         atomicAdd(bar, 1u);
         if (wait) { while ((int)(*reinterpret_cast<volatile unsigned int*>(bar) - target) < 0) { } __threadfence(); }
     } else {
         asm volatile("red.release.gpu.global.add.u32 [%0], %1;" ::"l"(bar), "r"(1u) : "memory");
-        if (wait) {
-            if (sync_mode == 1) { do { asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory"); } while ((int)(v - target) < 0); }
-            else { do { asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory"); } while ((int)(v - target) < 0); }
-        }
+        unsigned int v;
+        if (wait) { do { asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory"); } while ((int)(v - target) < 0); }
     }
+}
+template <GridBarrierFlavour F>
+__device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int target) {
+    if constexpr (F == kFenced) __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) grid_arrive<F>(bar, target, true);
+    __syncthreads();
 }
 #endif
 
@@ -491,8 +507,6 @@ struct liliom_ctx {
     unsigned time_calls = 0;
     // run-time switches: read by liliom_create and nowhere else (DESIGN.md §6)
     int force_lanes = 0, force_rounds = 0;   // tuning override (LILIOM_KNN_LANES / LILIOM_KNN_ROUNDS)
-    int gn_sync = 3;                     // persistent kernels' grid barrier (LILIOM_GN_SYNC): 3 = release-only arrival, no acquire fence (default),
-                                         // 1 = acquire poll, 0 = full fences on both sides
     bool dbg_timing = false;             // LILIOM_DEBUG_TIMING: stage clocks of the cooperative kernels, printed by s2m_run
     bool rot_slow_walk = false;          // LILIOM_ROT_SLOW_WALK (test hook): the general walk of k_rot_ring for every segment
     bool hz_chain = false;               // LILIOM_HZ_CHAIN=1 (test hook): the Horizon extractor's multi-launch chain, not k_hz_coop
@@ -759,7 +773,7 @@ struct IcpArgs {
     int rmax, rmax_fit;                              // shells to visit at most: correspondence passes, the fitness pass
     int max_iter; double trans_eps, fit_eps;
     double* partials;                                // [2 parities][kIcpSums][nvb]
-    unsigned int* bar; int sync_mode;                // grid barrier word (zeroed before the launch), LILIOM_GN_SYNC
+    unsigned int* bar;                               // grid barrier word (zeroed before the launch)
     PinIcp* out;                                     // results (the pinned block, or device memory)
 };
 struct IcpJob {

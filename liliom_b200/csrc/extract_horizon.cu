@@ -374,20 +374,6 @@ __global__ void k_hz_emit(const Pt48* __restrict__ stage_surf, const Pt48* __res
 constexpr int HZC_THREADS = 256;
 constexpr int HZC_WARPS = HZC_THREADS / 32;
 
-// (A release-only variant of this barrier — one cumulative red.release by thread 0, no acquire fence; legal here because
-// every cross-block read is an L2-scope load — was measured in round 1 and changed nothing: 4586/4629 vs 4653/4563 scans/s.
-// These kernels spend their time in the stages, not in the three fences.)
-__device__ __forceinline__ void hz_grid_barrier(unsigned int* bar, unsigned int target) {
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        atomicAdd(bar, 1u);
-        while ((int)(*reinterpret_cast<volatile unsigned int*>(bar) - target) < 0) { }
-        __threadfence();
-    }
-    __syncthreads();
-}
-
 // The body of k_hz_coop for the block at blk: blk.bi() of the blk.G() blocks of its session (SoloBlock: the whole grid).
 // A session's output does not depend on G: a kept point's place in the cutted cloud is the count of kept points before it
 // (the preceding blocks' counts plus the in-block prefix), and stage C gives each patch its own warp for any G with
@@ -427,7 +413,7 @@ __device__ __forceinline__ void hz_coop_body(const Pt48* __restrict__ pts, int n
     int tpre = inc - mine;
     for (int w = 0; w < warp; ++w) tpre += wsum[w];
     if (tid == HZC_THREADS - 1) blockcnt[b] = tpre + mine;
-    hz_grid_barrier(bar, (unsigned int)G);
+    grid_barrier<kFenced>(bar, (unsigned int)G);
     if (stamp) stamp[1] = clock64();
     // ---- B
     if (warp == 0) {
@@ -445,7 +431,7 @@ __device__ __forceinline__ void hz_coop_body(const Pt48* __restrict__ pts, int n
             if (i < n && hz_keep(pts, i)) { hz_deskew_bin_point(pts, i, ci, q_imu, cut, mat); ++ci; }
         }
     }
-    hz_grid_barrier(bar, 2u * (unsigned int)G);
+    grid_barrier<kFenced>(bar, 2u * (unsigned int)G);
     if (stamp) stamp[2] = clock64();
     // ---- C  (host guarantees G * HZC_WARPS >= HZ_PATCHES: one patch per warp)
     const int patch = b * HZC_WARPS + warp;
@@ -454,7 +440,7 @@ __device__ __forceinline__ void hz_coop_body(const Pt48* __restrict__ pts, int n
         hz_patch_eval<true>(P, cut, mat, patch, lane, surf_thres, edge_thres, (stamp && warp == 0) ? stamp + 5 : nullptr);
         if (lane == 0) { counts[patch] = P.ns; counts[HZ_PATCHES + 1 + patch] = P.ne; }
     }
-    hz_grid_barrier(bar, 3u * (unsigned int)G);
+    grid_barrier<kFenced>(bar, 3u * (unsigned int)G);
     if (stamp) stamp[3] = clock64();
     // ---- D
     if (patch < HZ_PATCHES) {

@@ -192,7 +192,7 @@ struct GnBatchEntry {
     GnIo io;
 };
 struct GnBatch : BatchTab<GnBatchEntry> {
-    int iters, sync_mode;               // GN iterations and LILIOM_GN_SYNC shared by all sessions of the launch
+    int iters;                          // GN iterations shared by all sessions of the launch
 };
 
 // What only the per-pass kernel (k_knn_plane) reads.
@@ -631,7 +631,7 @@ __global__ void __launch_bounds__(kBlock, LANES == 1 ? LILI_KNN1_MINBLOCKS : 2) 
 // buffers, `bar` and io, so sessions of one batched launch never wait for one another.
 template <int LANES, bool TMA, class Blk>
 __device__ __forceinline__ void gn_persistent_body(KnnArgs a, int iters, unsigned int* bar, double* stats_base, unsigned int bar_base,
-                                                   int sync_mode, const PeerArgs& pa, const GnIo& io, const Blk blk) {
+                                                   const PeerArgs& pa, const GnIo& io, const Blk blk) {
     __shared__ __align__(16) KnnSmem S;
     unsigned stage_phase = 0;
     if constexpr (TMA) {       // one mbarrier per lane group, 16 arrivals (every lane of the group, with or without a run to stage)
@@ -672,21 +672,13 @@ __device__ __forceinline__ void gn_persistent_body(KnnArgs a, int iters, unsigne
         if (stamp) a.dbg[16] = clock64();
         knn_phases<LANES, TMA>(a, q, t, n_q, S, acc, cand, it > 0, blk, keep ? &f_keep : nullptr, &stage_phase);
         if (stamp) a.dbg[17] = clock64();
-        // ---- grid barrier + cross-block sum.  Mode 3 (default; measured 12.70 -> 11.99 us per pass against mode 0): one release by
-        // thread 0 after the block barrier (cumulative over bar.sync, as in cooperative groups' grid.sync; SASS: MEMBAR.ALL.GPU +
-        // RED, no L1 invalidate) and NO acquire fence after the relaxed poll.  An acquire would only add an L1 invalidation:
-        // everything this kernel reads through L1 (map, cell table, features) is immutable for the launch, and the partials are
-        // read with L2-scope loads (__ldcg) issued after the poll's control dependency and a bar.sync.  The PTX model formally
-        // asks for the acquire: mode 1 polls with ld.acquire (slower per pass: tools/ab_variants.py), mode 0 fences both
-        // sides; tests pin all three to the same bits (test_gpu_variants.py, test_persistent_barrier_stress_all_sync_modes).
-        // Multi-GPU (fused exchange): the other blocks of this GPU arrive but do not wait here — they wait for block 0's
-        // republished sums over all ranks.
+        // ---- grid barrier (release-only, see grid_barrier) + cross-block sum.  Multi-GPU (fused exchange): the other blocks of
+        // this GPU arrive but do not wait here — they wait for block 0's republished sums over all ranks.
         const bool follower = pa.enabled && blk.bi() != 0;
         write_block_partials(a, S, acc, cand, blk);
-        if (sync_mode == 0) __threadfence();
         __syncthreads();
         if (stamp) a.dbg[18] = clock64();
-        if (threadIdx.x == 0) grid_barrier(bar, bar_base + (unsigned int)(it + 1) * blk.G(), sync_mode, !follower);
+        if (threadIdx.x == 0) grid_arrive<kReleaseOnly>(bar, bar_base + (unsigned int)(it + 1) * blk.G(), !follower);
         if (!follower) {
             __syncthreads();
             if (stamp) a.dbg[19] = clock64();
@@ -732,8 +724,8 @@ __device__ __forceinline__ void gn_persistent_body(KnnArgs a, int iters, unsigne
 
 template <int LANES, bool TMA = false>
 __global__ void LILI_GN_BOUNDS k_gn_persistent(KnnArgs a, int iters, unsigned int* bar, double* stats_base, unsigned int bar_base,
-                                                             int sync_mode, const __grid_constant__ PeerArgs pa, const __grid_constant__ GnIo io) {
-    gn_persistent_body<LANES, TMA>(a, iters, bar, stats_base, bar_base, sync_mode, pa, io, SoloBlock{});
+                                                             const __grid_constant__ PeerArgs pa, const __grid_constant__ GnIo io) {
+    gn_persistent_body<LANES, TMA>(a, iters, bar, stats_base, bar_base, pa, io, SoloBlock{});
 }
 
 // Several sessions' persistent GN steps in one cooperative launch (liliom_scan_to_map_resident_batch).  Session s owns blocks
@@ -745,7 +737,7 @@ __global__ void LILI_GN_BOUNDS k_gn_batch(const __grid_constant__ GnBatch tab) {
     const BatchSlot at = batch_slot(tab);
     const GnBatchEntry& e = tab.s[at.s];
     const PeerArgs pa{};
-    gn_persistent_body<LANES, TMA>(e.a, tab.iters, e.bar, e.stats_base, e.bar_base, tab.sync_mode, pa, e.io, at.blk);
+    gn_persistent_body<LANES, TMA>(e.a, tab.iters, e.bar, e.stats_base, e.bar_base, pa, e.io, at.blk);
 }
 
 // GN step for the multi-GPU path: runs after the all-reduce of neq[29], identically on every rank.
@@ -1230,8 +1222,8 @@ static int s2m_launch(liliom_ctx* c, S2mCall& k, const double pose7[7], int max_
     KnnArgs& a = k.a;
     const int iters = k.iters;
     if (p.persistent) {
-        int iters_arg = iters, sync_mode = c->gn_sync;
-        void* kargs[] = {&a, &iters_arg, &k.bar, &k.stats_base, &k.bar_base, &sync_mode, &k.pa, &k.io};
+        int iters_arg = iters;
+        void* kargs[] = {&a, &iters_arg, &k.bar, &k.stats_base, &k.bar_base, &k.pa, &k.io};
         LILI_TRY(timed_launch(c, k.timed, iters, [&] {
             LILI_CUDA(c, cudaLaunchCooperativeKernel(gn_kernel(p.lanes, p.tma), dim3(p.grid), dim3(kBlock), kargs, p.dyn_smem, c->stream));
             return launch_check(c, "k_gn_persistent");
@@ -1391,7 +1383,7 @@ int s2m_batch(liliom_ctx* const* cs, int B, double* poses7, const int* match_cnt
                 e = GnBatchEntry{ki.a, ki.bar, ki.stats_base, ki.bar_base, ki.io};
                 return BatchPart{cs[run[j]], ki.p.grid};
             }, [&](GnBatch& tab, int grid) -> int {
-                tab.iters = g.iters; tab.sync_mode = c0->gn_sync;
+                tab.iters = g.iters;
                 const S2mPlan& p = plans[l.sessions[0]];
                 void* kargs[] = {&tab};
                 LILI_TRY(timed_launch(c0, timed0, g.iters, [&]() -> int {

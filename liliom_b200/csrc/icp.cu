@@ -137,9 +137,10 @@ __device__ __forceinline__ void icp_pass(const IcpArgs& a, const double* T, floa
                                          double* sums, const Blk blk) {
     double* part = a.partials + (size_t)(phase & 1) * kIcpSums * a.nvb;
     for (int vb = blk.bi(); vb < a.nvb; vb += blk.G()) icp_vblock(a, vb, T, max_d2, rmax, part, red);
-    if (a.sync_mode == 0) __threadfence();
+    // grid_barrier spelled out: thread 0 computes the target after the first block barrier (as an argument of grid_barrier it
+    // would be computed before it, and the kernel would take one register more)
     __syncthreads();
-    if (threadIdx.x == 0) grid_barrier(a.bar, (unsigned int)(phase + 1) * blk.G(), a.sync_mode, true);
+    if (threadIdx.x == 0) grid_arrive<kReleaseOnly>(a.bar, (unsigned int)(phase + 1) * blk.G(), true);
     __syncthreads();
     if (threadIdx.x < kIcpSums) {
         const double* p = part + (size_t)threadIdx.x * a.nvb;
@@ -232,7 +233,6 @@ int icp_begin(liliom_ctx* c, const MapIndex& tgt, const float4* d_src, int n, do
     a.rmax_fit = std::max(tgt.grid.dim[0], std::max(tgt.grid.dim[1], tgt.grid.dim[2])) + 1;
     a.rmax = (int)std::min(std::ceil(max_corr_dist / cell) + 1.0, (double)a.rmax_fit);
     a.max_iter = max_iter; a.trans_eps = trans_eps; a.fit_eps = fit_eps;
-    a.sync_mode = c->gn_sync;
     int per_sm = 0;
     LILI_CUDA(c, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_icp_persistent, kIcpBlock, 0));
     j.grid = std::max(1, std::min(a.nvb, per_sm * c->sm_count));
@@ -300,7 +300,6 @@ int icp_batch_launch(liliom_ctx* c0, const std::vector<IcpJob*>& jobs) {
     for (const BatchLaunch& l : pack.launches)
         LILI_TRY(batch_tables<BatchTab<IcpArgs>>(l.sessions, [&](IcpArgs& e, int s) {
             e = jobs[s]->a;
-            e.sync_mode = c0->gn_sync;          // launch-wide, as the batched GN step's
             return BatchPart{jobs[s]->c, items[s].grid};
         }, [&](BatchTab<IcpArgs>& tab, int grid) -> int {
             void* kargs[] = {&tab};

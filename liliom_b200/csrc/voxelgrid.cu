@@ -105,17 +105,6 @@ static size_t vgc_layout(VgCoopBufs& B, unsigned char* base, int grid) {
     return off;
 }
 
-__device__ __forceinline__ void vgc_barrier(unsigned int* bar, unsigned int target) {
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        atomicAdd(bar, 1u);
-        while ((int)(*reinterpret_cast<volatile unsigned int*>(bar) - target) < 0) { }
-        __threadfence();
-    }
-    __syncthreads();
-}
-
 constexpr int VGC_UKEYS = 8192;    // occupied-voxel keys a block holds in shared memory for the ranks (more: read through L2)
 struct VgCoopSmem {
     int   red[7][VGC_WARPS];
@@ -204,7 +193,7 @@ __global__ void __launch_bounds__(VGC_THREADS, 1) k_vg_coop(const unsigned char*
         for (int w = 1; w < VGC_WARPS; ++w) v = vg_box_join(tid, v, S.red[tid][w]);
         B.mmpart[tid * G + blockIdx.x] = v;
     }
-    vgc_barrier(&ctl[0], G);
+    grid_barrier<kFenced>(&ctl[0], G);
     if (stamp) stamp[1] = clock64();
 
     // ---- phase 2: box parameters (every block, warp 0) and the key list in shared memory (the other warps)

@@ -8,6 +8,9 @@ Tolerance (BASELINE.json): pose within 1e-4 m / 1e-4 rad at equal iteration coun
 import numpy as np
 import pytest
 
+from test_devmath_host import dm  # noqa: F401  (the host build of dev_math.cuh, a fixture)
+from test_gpu_reanchored import _gn, probe_of
+
 pytestmark = pytest.mark.gpu
 
 F48 = ["x", "y", "z", "nx", "ny", "nz", "intensity", "curvature"]
@@ -184,35 +187,30 @@ def test_gn_step_stays_bounded_on_a_single_plane(oracle):
     c.close()
 
 
-def test_persistent_barrier_stress_all_sync_modes(oracle, world_small):
+def test_persistent_barrier_stress(oracle, dm, world_small):  # noqa: F811
     """VERDICT r1 'What's weak' #7: the persistent GN kernel's grid barrier.  Many launches with varying grid sizes and
-    iteration counts, in the three barrier modes (3 release-only arrival + relaxed poll, 1 release + ACQUIRE poll — the
-    formally complete pairing —, 0 full fences): every pose and every per-iteration sum must be bit-identical.  A stale
-    partial read past the barrier would show up as a differing sum."""
-    import os
+    iteration counts, six times over: every repetition's poses and per-iteration sums must equal the first's bit for bit, and
+    every pass of the first is re-anchored against the oracle (tests/reanchor.py) with the device's own correspondences from a
+    second context's find_surf_corr, the per-pass kernel, which has no grid barrier.  A stale or missing block partial read past
+    the barrier would show up as a differing sum: it cannot meet the sums' rtol of 1e-9."""
     import liliom_b200 as L
     surf, _, _ = oracle.extract_horizon(world_small["hz"], world_small["q_hz"])
     ds = oracle.voxelgrid(surf, 0.4)
+    tree, guess = oracle.KdTree(world_small["map"]), world_small["guess"]
     rng = np.random.default_rng(17)
     scans = [ds[rng.permutation(len(ds))[: int(n)]] for n in rng.integers(40, len(ds), 24)]
-    ref = None
-    for mode in ("3", "1", "0"):
-        old = os.environ.get("LILIOM_GN_SYNC")
-        os.environ["LILIOM_GN_SYNC"] = mode
-        try:
-            c = L.Context(variant=0)
-        finally:
-            if old is None:
-                os.environ.pop("LILIOM_GN_SYNC", None)
-            else:
-                os.environ["LILIOM_GN_SYNC"] = old
-        c.map_set_points(world_small["map"])
-        out = []
+    c, pc = L.Context(variant=0), L.Context(variant=0)
+    try:
+        c.map_set_points(world_small["map"]); pc.map_set_points(world_small["map"])
+        ref = []
         for rep in range(6):
             for k, f in enumerate(scans):
-                pose, st = c.scan_to_map(f, world_small["guess"], 3 + (k % 9), mode=L.MODE_GN)
-                out.append(pose.tobytes() + b"".join(np.array(s.jtj_jtr).tobytes() for s in st))
-        c.close()
-        if ref is None:
-            ref = out
-        assert out == ref, mode
+                pose, st = c.scan_to_map(f, guess, 3 + (k % 9), mode=L.MODE_GN)
+                out = pose.tobytes() + b"".join(np.array(s.jtj_jtr).tobytes() for s in st)
+                if rep == 0:
+                    ref.append(out)
+                    _gn(oracle, dm, tree, f, guess, st, f"barrier stress/scan {k} ({len(f)} queries)", probe_of(pc, f))
+                else:
+                    assert out == ref[k], (rep, k)
+    finally:
+        c.close(); pc.close()

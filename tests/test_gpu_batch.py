@@ -3,8 +3,6 @@
 Twin context sets get the same maps and inputs; set A steps with solo calls, set B with one batch call per step.  Per session
 and step the pose, status, every liliom_iter_stats entry, the DS cloud and the device-side query / candidate counts must be
 equal as bytes; after the batched steps one more solo call on both sets checks the state the batch left in every context."""
-import os
-
 import numpy as np
 import pytest
 
@@ -28,18 +26,9 @@ def world():
     return dict(big=big, small=small, sweeps=sweeps, hdl=hdl, q_hdl=q_hdl, guess=synth.perturbed_pose(T0))
 
 
-def _ctx(variant=0, sync=None):
+def _ctx(variant=0):
     import liliom_b200 as L
-    old = os.environ.get("LILIOM_GN_SYNC")
-    if sync is not None:
-        os.environ["LILIOM_GN_SYNC"] = str(sync)          # read at liliom_create
-    try:
-        c = L.Context(variant=variant)
-    finally:
-        if old is None:
-            os.environ.pop("LILIOM_GN_SYNC", None)
-        else:
-            os.environ["LILIOM_GN_SYNC"] = old
+    c = L.Context(variant=variant)
     c.set_kernel_timing(1)                                 # device-side query / candidate counts
     return c
 
@@ -53,9 +42,9 @@ def _counts(c):
     return (k.knn_queries, k.knn_candidates, k.launches)
 
 
-def _twins(n, variant=0, sync=None):
-    return [_ctx(variant if np.isscalar(variant) else variant[i], sync) for i in range(n)], \
-           [_ctx(variant if np.isscalar(variant) else variant[i], sync) for i in range(n)]
+def _twins(n, variant=0):
+    return [_ctx(variant if np.isscalar(variant) else variant[i]) for i in range(n)], \
+           [_ctx(variant if np.isscalar(variant) else variant[i]) for i in range(n)]
 
 
 def _odo_solo(ctxs, poses):
@@ -268,21 +257,6 @@ def test_more_sessions_than_one_launch(world):
     assert all(r[1] == 0 for r in rb)
     _same(_s2m_solo(A, poses), _s2m_solo(Bs, poses), "solo after batch")
     _close(A, Bs)
-
-
-def test_barrier_modes_same_bits(world):
-    feats, poses = _small_sessions(world, 12)
-    ref = None
-    for sync in (3, 1, 0):
-        A, Bs = _twins(12, sync=sync)
-        for c in A + Bs:
-            c.map_set_points(world["small"])
-        rb = _run_s2m(A, Bs, feats, poses)
-        got = [r[0].tobytes() + b"".join(_stats_bytes(r[2])) for r in rb]
-        if ref is None:
-            ref = got
-        assert got == ref, sync
-        _close(A, Bs)
 
 
 def test_caller_streams(world):

@@ -3,9 +3,7 @@ icp_trace bit for bit: the final T (16 doubles), the fitness over every source p
 by pass, since PCL's loop under a cap of k iterations is the first k passes of the uncapped loop.  The adversarial world at 1 m and
 2 m cells and four cut-offs (cell corners and faces, ties, a clump, source points far outside the target's grid on every face,
 pairs on the correspondence cut), the default loop-closure world at every source size that changes the launch and in all three
-point layouts, the grid barrier's three modes, and one loop-closure call from the keyframe store."""
-import os
-
+point layouts, and one loop-closure call from the keyframe store."""
 import numpy as np
 import pytest
 
@@ -134,26 +132,6 @@ def test_far_source_has_a_finite_fitness():
         c.close()
     assert not got[2] and got[3] == 0 and np.array_equal(got[0], np.eye(4))
     _check(got, tr, "far source")
-
-
-def test_barrier_modes_give_the_same_bits(world_small):
-    import liliom_b200 as L
-    src, tgt = default_world(world_small, 12000)
-    tr = R.icp_trace(src, tgt)
-    old = os.environ.get("LILIOM_GN_SYNC")
-    try:
-        for mode in ("0", "1", "3"):
-            os.environ["LILIOM_GN_SYNC"] = mode               # read when the context is created
-            c = L.Context(variant=0)
-            try:
-                _check(c.icp_align(src, tgt), tr, f"LILIOM_GN_SYNC={mode}")
-            finally:
-                c.close()
-    finally:
-        if old is None:
-            os.environ.pop("LILIOM_GN_SYNC", None)
-        else:
-            os.environ["LILIOM_GN_SYNC"] = old
 
 
 @pytest.mark.parametrize("stride", [48, 32])

@@ -3,7 +3,7 @@ sessions' solo liliom_loop_align calls, bit for bit.  Twin context sets hold the
 batched, and every result, status, counter and later solo call is compared on bytes.  Covered: B = 1, 2, 8, 32 and 34 (two
 table launches) with 48- and 32-byte sessions mixed and per-session settings; sessions of 1 iteration beside sessions that run
 to max_iter; a 300k-point source that fills a co-resident grid by itself; a session whose voxel index wraps (wide keys); empty
-and out-of-reach sessions; per-session errors; whole-call refusals; caller streams; every barrier mode; and the context's
+and out-of-reach sessions; per-session errors; whole-call refusals; caller streams; and the context's
 resident state."""
 import ctypes as C
 import os
@@ -185,11 +185,11 @@ def _wide_store(stride):
 IDENT = np.array([1.0, 0, 0, 0, 0, 0, 0])
 
 
-def _special_sessions(stride_of, env=None):
+def _special_sessions(stride_of):
     """ordinary, 300k-point source, wide keys, empty source, empty target, out of reach, four erroring sessions, ordinary"""
     rng = np.random.default_rng(5)
     cs, specs = [], []
-    c, poses = _store(stride_of(0), 11, env)
+    c, poses = _store(stride_of(0), 11)
     hist, hp = list(range(N_HIST)), [poses[k] for k in range(N_HIST)]
     cs.append(c); specs.append(dict(si=[REVISIT], sp=[poses[REVISIT]], ti=hist, tp=hp, prm=dict(leaf=0.4)))
     cs.append(_big_store(stride_of(1), rng))
@@ -206,7 +206,7 @@ def _special_sessions(stride_of, env=None):
                            dict(si=[REVISIT], sp=[poses[0]], ti=hist, tp=hp, prm=dict(leaf=0.0)),
                            dict(si=[REVISIT], sp=[poses[0]], ti=hist, tp=hp, prm=dict(leaf=0.4, max_iter=0)),
                            dict(si=[1, 2], sp=[poses[1], poses[2]], ti=hist, tp=hp, prm=dict(leaf=0.6, max_corr_dist=2.0, max_iter=3))]):
-        c, _ = _store(stride_of(3 + k), 11 + k % 2, env)
+        c, _ = _store(stride_of(3 + k), 11 + k % 2)
         cs.append(c); specs.append(s)
     return cs, specs
 
@@ -230,11 +230,9 @@ def test_large_wide_empty_and_erroring_sessions_beside_ordinary_ones():
             c.close()
 
 
-def test_caller_streams_and_barrier_modes():
-    """two sessions on caller streams (ctxs[0] among them); then whole batches created under each LILIOM_GN_SYNC mode against
-    solo calls in the default mode"""
+def test_caller_streams():
+    """two sessions on caller streams (ctxs[0] among them)"""
     import torch
-    stride_of = lambda i: _stride(i)                                      # noqa: E731
     A, Bc, poses = [], [], []
     for i in range(5):
         a, p = _store(_stride(i), 7 + i % 3)
@@ -249,14 +247,6 @@ def test_caller_streams_and_barrier_modes():
     finally:
         for c in A + Bc:
             c.close()
-    for mode in ("0", "1", "3"):
-        A, specs = _special_sessions(stride_of)
-        Bc, _ = _special_sessions(stride_of, env={"LILIOM_GN_SYNC": mode})
-        try:
-            _compare(A, Bc, specs, f"LILIOM_GN_SYNC={mode}")
-        finally:
-            for c in A + Bc:
-                c.close()
 
 
 def test_whole_call_refusals_change_nothing(pool):

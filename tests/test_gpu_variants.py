@@ -1,6 +1,4 @@
-"""The switches of the small-scan GN kernel must not change a single bit:
-  LILIOM_GN_SYNC  = 3 counter grid barrier with a release-only arrival and a relaxed poll (default) | 1 release arrival +
-                    acquire poll | 0 full fences on both sides
+"""The variants of the small-scan GN kernel must not change a single bit:
   fused peer exchange of one rank with itself (the whole NVLink protocol on a single GPU)
   LILIOM_KNN_TMA  = 1 the 16-lane search stages every run with one cp.async.bulk into shared memory (mbarrier) instead of
                     batches of 16-byte loads through registers
@@ -12,27 +10,24 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 
-# mode % 10 = LILIOM_GN_SYNC; +20: fused peer exchange with itself; +30: bulk-copy staging
-VARIANTS = [3, 1, 0, 23, 33]
+# the default kernel; the fused peer exchange with itself; bulk-copy staging
+VARIANTS = ["default", "peer", "tma"]
 
 
 def _ctx(ll):
     import liliom_b200 as L
-    keys = ("LILIOM_GN_SYNC", "LILIOM_KNN_TMA")
-    old = {k: os.environ.get(k) for k in keys}
-    os.environ["LILIOM_GN_SYNC"] = str(ll % 10)
-    os.environ["LILIOM_KNN_TMA"] = "1" if 30 <= ll < 40 else "0"
+    old = os.environ.get("LILIOM_KNN_TMA")
+    os.environ["LILIOM_KNN_TMA"] = "1" if ll == "tma" else "0"
     try:
-        c = L.Context(variant=0)             # the switches are read at liliom_create
-        if 20 <= ll < 30:                    # one rank exchanging with itself: the whole protocol on a single GPU
+        c = L.Context(variant=0)             # the switch is read at liliom_create
+        if ll == "peer":                     # one rank exchanging with itself: the whole protocol on a single GPU
             c.comm_peer_attach([c.comm_peer_export()], 0)
         return c
     finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
+        if old is None:
+            os.environ.pop("LILIOM_KNN_TMA", None)
+        else:
+            os.environ["LILIOM_KNN_TMA"] = old
 
 
 def test_gn_variants_bit_identical(oracle, world_small):
@@ -95,7 +90,7 @@ def test_peer_epoch_resync(oracle, world_small):
     import liliom_b200 as L
     surf, _, _ = oracle.extract_horizon(world_small["hz"], world_small["q_hz"])
     ds = oracle.voxelgrid(surf, 0.4)
-    c = _ctx(23)                                   # one rank exchanging with itself
+    c = _ctx("peer")                                   # one rank exchanging with itself
     c.map_set_points(world_small["map"])
     e0 = c.comm_peer_epoch()
     p1, _ = c.scan_to_map(ds, world_small["guess"], 10, mode=L.MODE_GN)
