@@ -174,7 +174,11 @@ typedef struct {
  * mode CERES: match_cnt outer iterations of [findCorrespondingSurfFeatures (:352-413) + a
  *   Ceres-2.0-default LM of <= max_num_iter iterations, Huber(0.1), 15 ms cap disabled];
  * mode GN   : match_cnt iterations of [re-associate + one Gauss-Newton step] (max_num_iter ignored).
- * stats: NULL or match_cnt entries. */
+ * stats: NULL or match_cnt entries.
+ * On a context with a communicator mode CERES is refused with LILIOM_E_ARG unless liliom_comm_set_ceres(c, 1): then every
+ * LM evaluation of an outer iteration is one all-reduce of the 29 sums over the ranks' own correspondences, and every rank
+ * takes the same trust-region decisions and returns the same pose bits.  That pose is not bit-identical to one GPU's (the
+ * sums are added in another order); it agrees with it within the LM's rounding bounds. */
 int liliom_scan_to_map(liliom_ctx* c, const void* feats_body, int n, int stride, double pose7_inout[7],
                        int match_cnt, int max_num_iter, int mode, liliom_iter_stats* stats);
 
@@ -447,13 +451,22 @@ int liliom_set_time_source(liliom_ctx* c, int source, const char* field_name);
 /* 128-byte NCCL unique id: rank 0 calls get, the launcher broadcasts it, every rank calls init.
  * After init, liliom_map_set_points shards the map by 16 m block hash (+halo) and every
  * liliom_scan_to_map / liliom_odometry_resident is COLLECTIVE: per iteration one all-reduce of
- * the 27 J^T J|J^T r scalars (+cost,count) then an identical 6x6 solve on every rank. */
+ * the 27 J^T J|J^T r scalars (+cost,count) then an identical 6x6 solve on every rank.
+ * In mode CERES (after liliom_comm_set_ceres(c, 1)) each outer iteration all-reduces the linearisation sums once and then
+ * runs the LM in exactly 1 + max(0, max_num_iter) rounds of [the 29 sums over this rank's correspondences, their all-reduce,
+ * the same trust-region step on every rank]; rounds after the LM stopped still all-reduce (zeros), so every rank issues the
+ * same collectives.  Its pose bits depend on nranks and the shard block.  An all-reduce failure returns LILIOM_E_NCCL with
+ * the pose untouched.  The batch calls (liliom_*_batch*) still refuse communicator contexts. */
 int liliom_comm_get_unique_id(void* id128);
 int liliom_comm_init(liliom_ctx* c, const void* id128, int nranks, int rank);
 /* Edge of the cubes the map is sharded by (metres, a power of two in [8, 256]; default 16).  Larger cubes replicate less
  * halo (a 64 m cube with its 1 m + voxel-diagonal rim holds ~1.1x its own points, a 16 m cube ~1.45x) at a coarser load
  * balance.  Must be the same on every rank and set before the map is installed / the first frame is pushed. */
 int liliom_comm_set_shard_block(liliom_ctx* c, int metres);
+/* Ceres mode on a context with a communicator.  0 (the default): LILIOM_E_ARG, as without this call.  1: the collective LM
+ * above.  Any other value: LILIOM_E_ARG.  Accepted on any context, at any time (before or after liliom_comm_init); only calls
+ * on a context with a communicator read it.  Must be the same on every rank, like liliom_comm_set_shard_block. */
+int liliom_comm_set_ceres(liliom_ctx* c, int on);
 
 /* Fused exchange over peer memory (single node, NVLink / NVSwitch; optional, after liliom_comm_init): every rank exports the
  * 64-byte cudaIpcMemHandle of its exchange buffer, the launcher all-gathers them, every rank attaches all of them in rank

@@ -84,7 +84,7 @@ EXPORTS = [
     "liliom_pc2_layout", "liliom_comm_peer_export", "liliom_comm_peer_attach",
     "liliom_map_push_frame_device", "liliom_knn_block_stats", "liliom_comm_set_shard_block", "liliom_undistort",
     "liliom_map_update", "liliom_map_update_device", "liliom_map_download_cloud", "liliom_icp_align",
-    "liliom_comm_peer_epoch", "liliom_comm_peer_set_epoch",
+    "liliom_comm_peer_epoch", "liliom_comm_peer_set_epoch", "liliom_comm_set_ceres",
     "liliom_backend_default_params", "liliom_kf_add", "liliom_kf_count", "liliom_kf_clear", "liliom_bmap_build",
     "liliom_bmap_download", "liliom_backend_window_correspond", "liliom_backend_window_blocks", "liliom_backend_window_corr",
     "liliom_kf_cloud", "liliom_kf_add_full", "liliom_global_map", "liliom_loop_align",
@@ -226,6 +226,7 @@ def lib() -> C.CDLL:
     L.liliom_comm_peer_set_epoch.argtypes = [vp, C.c_uint]
     L.liliom_map_push_frame_device.argtypes = [vp, vp, C.c_int, dp]
     L.liliom_comm_set_shard_block.argtypes = [vp, C.c_int]
+    L.liliom_comm_set_ceres.argtypes = [vp, C.c_int]
     L.liliom_undistort.argtypes = [vp, vp, C.c_int, dp, dp]
     L.liliom_map_update.argtypes = [vp, vp, C.c_int, dp, ip]
     L.liliom_map_update_device.argtypes = [vp, vp, C.c_int, dp, ip]
@@ -761,6 +762,11 @@ class Context:
 
     def comm_set_shard_block(self, metres: int):
         self._check(lib().liliom_comm_set_shard_block(self._h, metres))
+
+    def comm_set_ceres(self, on: int):
+        """1: MODE_CERES on a context with a communicator runs the collective LM (every LM evaluation one all-reduce of the 29
+        sums); 0 (the default): such a call is refused.  The same on every rank (include/liliom.h)."""
+        self._check(lib().liliom_comm_set_ceres(self._h, int(on)))
 
     def comm_peer_export(self) -> bytes:
         """64-byte IPC handle of this rank's exchange buffer (fused multi-GPU exchange, include/liliom.h)."""

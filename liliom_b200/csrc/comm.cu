@@ -1,7 +1,8 @@
 // Multi-GPU plumbing: NCCL is resolved at run time with dlopen so that single-GPU users need no
 // NCCL at all, and so that inside a PyTorch process the already-loaded libnccl.so.2 is reused.
 // The only collective on the path is the per-iteration all-reduce of the 29 fp64 scalars
-// (21 J^T J + 6 J^T r + cost + count): 232 bytes, latency-bound over NVLink 5 / NVSwitch.
+// (21 J^T J + 6 J^T r + cost + count): 232 bytes, latency-bound over NVLink 5 / NVSwitch.  The collective
+// LM (Ceres mode, liliom_comm_set_ceres) issues the same all-reduce once per LM evaluation round.
 #include "ctx.cuh"
 #include <chrono>
 #include <condition_variable>
@@ -160,6 +161,12 @@ extern "C" int liliom_comm_init(liliom_ctx* c, const void* id128, int nranks, in
 extern "C" int liliom_comm_set_shard_block(liliom_ctx* c, int metres) {
     if (!c || metres < 8 || metres > 256 || (metres & (metres - 1)) != 0) return LILIOM_E_ARG;
     c->shard_inv_block = 1.0f / (float)metres;
+    return LILIOM_OK;
+}
+
+extern "C" int liliom_comm_set_ceres(liliom_ctx* c, int on) {
+    if (!c || (on != 0 && on != 1)) return LILIOM_E_ARG;
+    c->comm_ceres = on == 1;
     return LILIOM_OK;
 }
 

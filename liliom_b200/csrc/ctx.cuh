@@ -481,6 +481,7 @@ struct liliom_ctx {
     lili::DevBuf stats_dev;              // iterations x kStatsDoubles
     lili::DevBuf counter;                // last-block ticket + scratch ints
     lili::DevBuf lm_state;
+    lili::DevBuf lm_coll;                // the collective LM's state and round sums (grid_knn.cu: LmColl)
     lili::DevBuf icp_ctl;                // ICP kernel: barrier word, and its results when the pinned block is not mappable
     int bk_kind = 0, bk_n = 0;           // backend correspondences resident from the last liliom_correspond_* call (1 edge, 2 surf)
     unsigned int bar_arrivals = 0;       // total grid-barrier arrivals issued so far (persistent GN kernel)
@@ -489,6 +490,7 @@ struct liliom_ctx {
     void* nccl_comm = nullptr;
     int nranks = 1, rank = 0;
     float shard_inv_block = 0.0625f;     // 1 / shard block edge (LILIOM_SHARD_BLOCK, metres, power of two; must agree on all ranks)
+    bool comm_ceres = false;             // liliom_comm_set_ceres: Ceres mode with a communicator runs the collective LM
     lili::DevBuf peer_local;             // block 0 -> other blocks of this GPU: [2][32] doubles + 2 epoch words (fused exchange)
     lili::DevBuf peer_buf;               // this rank's exchange buffer: [2 parities][kMaxPeers][32] {epoch|lo32, epoch|hi32}
     void* peer_ptrs[lili::kMaxPeers] = {};   // every rank's buffer as mapped into this process (cudaIpcOpenMemHandle)

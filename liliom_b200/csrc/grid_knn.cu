@@ -21,6 +21,7 @@
 #include "ctx.cuh"
 #include "dev_math.cuh"
 #include "knn_core.cuh"
+#include "lm_tr.cuh"
 
 namespace lili {
 
@@ -518,18 +519,6 @@ __device__ __forceinline__ void gn_step(const double* sums, bool peer_lost, cons
     }
 }
 
-// Part k of one row of the per-iteration stats (kStatsDoubles doubles: n_corr, lm_iters, cost, the 27 sums, pose7, pad).
-// Part k < kNormEq is scalar k of the sums s; part kNormEq is the LM iteration count and the pose xn after the step.  The block
-// kernels store one part per thread, the one-thread kernels every part.
-__device__ __forceinline__ void write_stats(double* st, int k, const double* s, double lm_iters, const double* xn) {
-    if (k < kNormEq) st[k < 27 ? 3 + k : k == 27 ? 2 : 0] = s[k];
-    else {
-        st[1] = lm_iters;
-#pragma unroll
-        for (int j = 0; j < 7; ++j) st[30 + j] = xn[j];
-    }
-}
-
 __device__ __forceinline__ void write_neq_stats(const KnnArgs& a, const KnnSmem& S, double* stats) {
     if (threadIdx.x < kNormEq) {
         a.neq[threadIdx.x] = S.red[0][threadIdx.x];
@@ -793,97 +782,22 @@ __device__ void lm_eval(const LmArgs& a, const double x[7], double out[kNormEq],
     __syncthreads();
 }
 
-// The LM solve of one session, by one block of kLmBlock threads.
+// The LM solve of one session, by one block of kLmBlock threads: every evaluation block-wide, every decision on thread 0
+// (lm_tr.cuh).
 __device__ __forceinline__ void lm_solve_body(const LmArgs& a) {
     __shared__ double red[kLmBlock / 32][kNormEq];
     __shared__ double sh_x[7];
     __shared__ int sh_cmd;   // 0 = stop, 1 = evaluate candidate in sh_x
-    double x[7];
-    for (int k = 0; k < 7; ++k) x[k] = a.pose[k];
-    double S[kNormEq];
-    lm_eval(a, x, S, red);          // iteration 0: cost, gradient, J^T J at x
-    // --- thread-0 state (replicated arithmetic is avoided: only thread 0 decides) ---
-    double radius = 1e4, decrease_factor = 2.0;
-    bool reuse_diagonal = false, last_successful = true;      // IterationZero: the start is a successful step
-    double diagonal[6], scaling[6];
-    double x_cost = S[27];
-    int iteration = 0, invalid = 0;
-    if (threadIdx.x == 0) {
-        int kk = 0;
-        for (int i = 0; i < 6; ++i) for (int j = i; j < 6; ++j) { if (i == j) scaling[i] = 1.0 / (1.0 + sqrt(S[kk])); ++kk; }
-    }
-    const double count0 = S[28];
-    double step_keep[6];
-    double model_cost_change = 0;
+    LmState st;              // thread 0's
+    for (int k = 0; k < 7; ++k) st.x[k] = a.pose[k];
+    lm_eval(a, st.x, st.S, red);       // iteration 0: cost, gradient, J^T J at x
+    st.max_num_iter = a.max_num_iter;
+    if (threadIdx.x == 0) lm_begin(st, st.S);
     for (;;) {
         if (threadIdx.x == 0) {
-            int cmd = 1;
-            double xc[7];
-            for (;;) {   // loop over invalid steps without evaluation
-                if (count0 <= 0.0) { cmd = 0; break; }
-                if (iteration >= a.max_num_iter) { cmd = 0; break; }
-                if (last_successful) {      // |x - Plus(x, -g)|_inf
-                    // the translation part first, as Plus forms it: when it alone exceeds the tolerance the decision is
-                    // made, and the quaternion part (sincos on this single thread for a large g) is only formed near a stop
-                    double tmax = 0;
-                    for (int k = 0; k < 3; ++k) tmax = fmax(tmax, fabs(x[4 + k] - (x[4 + k] + -S[24 + k])));
-                    if (tmax <= 1e-10) {
-                        double ng[6], xg[7], gmax = 0;
-                        for (int k = 0; k < 6; ++k) ng[k] = -S[21 + k];
-                        pose_plus(x, ng, xg);
-                        for (int k = 0; k < 7; ++k) gmax = fmax(gmax, fabs(x[k] - xg[k]));
-                        if (gmax <= 1e-10) { cmd = 0; break; }
-                    }
-                }
-                if (radius < 1e-32) { cmd = 0; break; }
-                ++iteration;
-                last_successful = false;
-                // scaled normal equations  Hs = S H S, gs = S g
-                double Hs[21], gs[6];
-                int kk = 0;
-                for (int i = 0; i < 6; ++i) for (int j = i; j < 6; ++j) { Hs[kk] = S[kk] * scaling[i] * scaling[j]; ++kk; }
-                for (int i = 0; i < 6; ++i) gs[i] = S[21 + i] * scaling[i];
-                if (!reuse_diagonal) {
-                    kk = 0;
-                    for (int i = 0; i < 6; ++i) for (int j = i; j < 6; ++j) { if (i == j) diagonal[i] = fmin(fmax(Hs[kk], 1e-6), 1e32); ++kk; }
-                }
-                double Ha[21];
-                kk = 0;
-                for (int i = 0; i < 6; ++i) for (int j = i; j < 6; ++j) { Ha[kk] = Hs[kk] + (i == j ? diagonal[i] / radius : 0.0); ++kk; }
-                double y[6];
-                bool ok = solve6_ldlt(Ha, gs, y);
-                reuse_diagonal = true;
-                double step[6];
-                model_cost_change = 0;
-                if (ok) {
-                    for (int k = 0; k < 6; ++k) step[k] = -y[k];
-                    // -(step.gs + 1/2 step^T Hs step)
-                    double Hfull[6][6];
-                    kk = 0;
-                    for (int i = 0; i < 6; ++i) for (int j = i; j < 6; ++j) { Hfull[i][j] = Hs[kk]; Hfull[j][i] = Hs[kk]; ++kk; }
-                    double sg = 0, shs = 0;
-                    for (int i = 0; i < 6; ++i) {
-                        sg += step[i] * gs[i];
-                        double hv = 0;
-                        for (int j = 0; j < 6; ++j) hv += Hfull[i][j] * step[j];
-                        shs += step[i] * hv;
-                    }
-                    model_cost_change = -(sg + 0.5 * shs);
-                }
-                if (!ok || !(model_cost_change > 0.0)) {
-                    if (++invalid >= 5) { cmd = 0; break; }
-                    radius = radius / decrease_factor;      // StepIsInvalid = StepRejected(0)
-                    decrease_factor *= 2.0;
-                    continue;
-                }
-                invalid = 0;
-                for (int k = 0; k < 6; ++k) step_keep[k] = step[k] * scaling[k];
-                pose_plus(x, step_keep, xc);
-                for (int k = 0; k < 7; ++k) sh_x[k] = xc[k];
-                cmd = 1;
-                break;
-            }
-            sh_cmd = cmd;
+            const bool cmd = lm_propose(st);
+            if (cmd) for (int k = 0; k < 7; ++k) sh_x[k] = st.xc[k];
+            sh_cmd = cmd ? 1 : 0;
         }
         __syncthreads();
         if (sh_cmd == 0) break;
@@ -891,47 +805,12 @@ __device__ __forceinline__ void lm_solve_body(const LmArgs& a) {
         for (int k = 0; k < 7; ++k) xc[k] = sh_x[k];
         double Sc[kNormEq];
         lm_eval(a, xc, Sc, red);
-        int stop = 0;
-        if (threadIdx.x == 0) {
-            double candidate_cost = Sc[27];
-            double xn = 0, sn = 0;
-            for (int k = 0; k < 7; ++k) { xn += x[k] * x[k]; sn += (x[k] - xc[k]) * (x[k] - xc[k]); }
-            xn = sqrt(xn); sn = sqrt(sn);
-            double cost_change = x_cost - candidate_cost;
-            if (sn <= 1e-8 * (xn + 1e-8)) stop = 1;                                   // parameter tolerance
-            else if (fabs(cost_change) <= 1e-6 * x_cost) stop = 1;                    // function tolerance
-            else {
-                double relative_decrease = cost_change / model_cost_change;
-                if (relative_decrease > 1e-3) {
-                    for (int k = 0; k < 7; ++k) x[k] = xc[k];
-                    for (int k = 0; k < kNormEq; ++k) S[k] = Sc[k];
-                    x_cost = candidate_cost;
-                    last_successful = true;
-                    double qd = 2.0 * relative_decrease - 1.0;
-                    radius = radius / fmax(1.0 / 3.0, 1.0 - qd * qd * qd);
-                    radius = fmin(1e16, radius);
-                    decrease_factor = 2.0;
-                    reuse_diagonal = false;
-                } else {
-                    radius = radius / decrease_factor;
-                    decrease_factor *= 2.0;
-                    reuse_diagonal = true;
-                }
-            }
-            sh_cmd = stop ? 0 : 1;
-        }
+        if (threadIdx.x == 0) sh_cmd = lm_judge(st, Sc) ? 1 : 0;
         __syncthreads();
         if (sh_cmd == 0) break;
         __syncthreads();
     }
-    if (threadIdx.x == 0) {
-        if (x[0] < 0) { x[0] = -x[0]; x[1] = -x[1]; x[2] = -x[2]; x[3] = -x[3]; }     // :539-549
-        for (int k = 0; k < 7; ++k) a.pose[k] = x[k];
-        if (a.stats) {
-#pragma unroll
-            for (int k = 0; k <= kNormEq; ++k) write_stats(a.stats, k, a.neq0, (double)iteration, x);
-        }
-    }
+    if (threadIdx.x == 0) lm_end(st, a.pose, a.stats, a.neq0);
 }
 
 __global__ void __launch_bounds__(kLmBlock) k_lm_solve(LmArgs a) { lm_solve_body(a); }
@@ -942,6 +821,63 @@ typedef BatchTab<LmArgs> LmBatch;
 __global__ void __launch_bounds__(kLmBlock) k_lm_solve_batch(const __grid_constant__ LmBatch tab) {
     const LmArgs a = tab.s[blockIdx.x];     // a register copy, as k_lm_solve's by-value parameter: the body compiles to the same arithmetic
     lm_solve_body(a);
+}
+
+// ------------------------------------------------------------------ the collective LM (Ceres mode on a sharded context)
+// lm_solve_body's loop cut at its evaluations (liliom_comm_set_ceres): in every round each rank sums the rows of the
+// correspondences it owns (k_lm_eval_part), the ranks all-reduce the 29 sums (added in rank order), and every rank takes the
+// same decision from the same sums (k_lm_advance).  The host runs exactly 1 + max(0, max_num_iter) rounds, which is enough for
+// any solve (lm_tr.cuh); the rounds after a stop are no-ops whose all-reduces still run, so every rank issues the same
+// collectives whatever its state.
+struct LmColl {
+    LmState st;             // re-initialised by the first round of every outer iteration
+    double sums[32];        // the round's 29 sums: this rank's, then (after the all-reduce) all ranks'
+};
+
+// Round 0 evaluates at the pose (the start of the outer iteration) and starts the state there; a later round evaluates at the
+// candidate, or writes zeros once the solve is done.  A rank that owns no correspondence writes zeros as well.
+__global__ void __launch_bounds__(kLmBlock) k_lm_eval_part(LmArgs a, LmColl* lc, int round) {
+    __shared__ double red[kLmBlock / 32][kNormEq];
+    double x[7];
+    if (round == 0) {
+        for (int k = 0; k < 7; ++k) x[k] = a.pose[k];
+    } else {
+        if (lc->st.done != kLmRunning) {
+            if (threadIdx.x < kNormEq) lc->sums[threadIdx.x] = 0.0;
+            return;
+        }
+        for (int k = 0; k < 7; ++k) x[k] = lc->st.xc[k];
+    }
+    double S[kNormEq];
+    lm_eval(a, x, S, red);
+    if (threadIdx.x == 0) {
+        for (int k = 0; k < kNormEq; ++k) lc->sums[k] = S[k];
+        if (round == 0) {
+            for (int k = 0; k < 7; ++k) lc->st.x[k] = x[k];
+            lc->st.done = kLmRunning;
+        }
+    }
+}
+
+// After the round's all-reduce: round 0 begins the solve from the sums at the start, every later round judges the candidate;
+// then the next candidate is proposed, unless the solve stopped.
+__global__ void k_lm_advance(LmColl* lc, int max_num_iter, int round) {
+    LmState st = lc->st;
+    if (round == 0) {
+        st.max_num_iter = max_num_iter;
+        lm_begin(st, lc->sums);
+        lm_propose(st);
+    } else {
+        if (st.done != kLmRunning) return;
+        if (lm_judge(st, lc->sums)) lm_propose(st);
+    }
+    lc->st = st;
+}
+
+// The outer iteration's pose and stats row (from the all-reduced linearisation sums neq0).
+__global__ void k_lm_end(LmColl* lc, double* pose, double* stats, const double* neq0) {
+    LmState st = lc->st;
+    lm_end(st, pose, stats, neq0);
 }
 
 // ------------------------------------------------------------------ instrumentation: the C-bar of SURVEY.md §8(d)
@@ -1123,8 +1059,8 @@ static int s2m_begin(liliom_ctx* c, const double pose7[7], int match_cnt, int mo
     if (c->map_n_global < 10) return LILIOM_E_FEWMAP;          // L/src/LidarOdometry.cpp:485-488
     const int n = c->n_feats, iters = match_cnt;
     if (iters < 0) return LILIOM_E_ARG;
-    if (mode != LILIOM_MODE_GN && c->nranks > 1) {      // refused before anything is enqueued: no rank enters a collective
-        c->last_error = "CERES mode is single-GPU (the LM solve is one block); use GN mode with a communicator";
+    if (mode != LILIOM_MODE_GN && c->nranks > 1 && !c->comm_ceres) {      // refused before anything is enqueued: no rank enters a collective
+        c->last_error = "CERES mode with a communicator needs liliom_comm_set_ceres(c, 1) on every rank (or GN mode)";
         return LILIOM_E_ARG;
     }
     // the per-iteration stats come back through the pinned block: check its capacity before anything is enqueued
@@ -1216,6 +1152,23 @@ static LmArgs lm_args(liliom_ctx* c, const KnnArgs& a, int it, int max_num_iter)
     return l;
 }
 
+// The LM of outer iteration `it` on a sharded context: the rounds of the collective LM, then its result.
+static int lm_collective(liliom_ctx* c, const KnnArgs& a, int it, int max_num_iter) {
+    LILI_CUDA(c, c->lm_coll.ensure(sizeof(LmColl)));
+    LmColl* lc = c->lm_coll.as<LmColl>();
+    const LmArgs l = lm_args(c, a, it, max_num_iter);
+    const int rounds = 1 + max(0, max_num_iter);
+    for (int r = 0; r < rounds; ++r) {
+        k_lm_eval_part<<<1, kLmBlock, 0, c->stream>>>(l, lc, r);
+        LILI_TRY(launch_check(c, "k_lm_eval_part"));
+        LILI_TRY(nccl_allreduce_sum_f64(c, lc->sums, kNormEq));
+        k_lm_advance<<<1, 1, 0, c->stream>>>(lc, max_num_iter, r);
+        LILI_TRY(launch_check(c, "k_lm_advance"));
+    }
+    k_lm_end<<<1, 1, 0, c->stream>>>(lc, l.pose, l.stats, l.neq0);
+    return launch_check(c, "k_lm_end");
+}
+
 // The launches of a call that s2m_begin planned, on the context's own stream.
 static int s2m_launch(liliom_ctx* c, S2mCall& k, const double pose7[7], int max_num_iter, int mode, bool want_corr) {
     const S2mPlan& p = k.p;
@@ -1252,6 +1205,8 @@ static int s2m_launch(liliom_ctx* c, S2mCall& k, const double pose7[7], int max_
         if (mode == LILIOM_MODE_GN && multi && !peer_iter) {
             k_gn_update<<<1, 32, 0, c->stream>>>(c->neq.as<double>(), c->pose_dev.as<double>(), pass.stats);
             LILI_TRY(launch_check(c, "k_gn_update"));
+        } else if (mode != LILIOM_MODE_GN && multi) {
+            LILI_TRY(lm_collective(c, a, it, max_num_iter));
         } else if (mode != LILIOM_MODE_GN) {
             k_lm_solve<<<1, kLmBlock, 0, c->stream>>>(lm_args(c, a, it, max_num_iter));
             LILI_TRY(launch_check(c, "k_lm_solve"));

@@ -1,7 +1,9 @@
 #!/usr/bin/env python
 """torchrun --nproc-per-node N tools/multi_check.py : sharded scan-to-map (map split by 8 m block hash,
-29-scalar NCCL all-reduce per iteration) must give the single-GPU pose."""
-import os, sys
+29-scalar NCCL all-reduce per iteration) must give the single-GPU pose.
+LILIOM_MODE=ceres adds the Ceres-faithful leg (liliom_comm_set_ceres): every rank must hold the same pose bits, within
+1e-4 m / 1e-4 rad of the single-GPU Ceres pose; each scan's time is printed next to the single-GPU Ceres scan's."""
+import os, sys, time
 import numpy as np
 import torch, torch.distributed as dist
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -43,6 +45,28 @@ if rank == 0:
     print(f"world={world} shard sizes={sizes} (global {n_map}); pose delta vs single GPU: {dt:.3e} m, 1-|q.q'|={dq:.2e}; "
           f"n_corr {st[0].n_corr} vs {st_ref[0].n_corr}; identical across ranks: {same}")
     assert dt < 1e-6 and dq < 1e-12 and same and st[0].n_corr == st_ref[0].n_corr
+# ---- Ceres-faithful leg: the collective LM (every LM evaluation one NCCL all-reduce of the 29 sums)
+if os.environ.get("LILIOM_MODE") == "ceres":
+    def timed(c, n=5):
+        out, ms = None, []
+        for _ in range(n):
+            dist.barrier(); torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            out = c.scan_to_map(ds, guess, 2, max_num_iter=15, mode=L.MODE_CERES)
+            ms.append(1e3 * (time.perf_counter() - t0))
+        return out, float(np.median(ms))
+    (pc_ref, sc_ref), ms_ref = timed(ref)
+    ctx.comm_set_ceres(1)
+    (pc, sc), ms = timed(ctx)
+    cposes = [None] * world
+    dist.all_gather_object(cposes, pc.tobytes())
+    if rank == 0:
+        same = all(p == cposes[0] for p in cposes)
+        dt = np.linalg.norm(pc[4:] - pc_ref[4:]); da = 2 * np.arccos(min(1.0, abs(float(np.dot(pc[:4], pc_ref[:4])))))
+        print(f"ceres: pose delta vs single GPU {dt:.3e} m, {da:.3e} rad; LM iterations {[s.lm_iters for s in sc]} vs "
+              f"{[s.lm_iters for s in sc_ref]}; identical across ranks: {same}; scan {ms:.3f} ms on {world} ranks vs {ms_ref:.3f} ms "
+              f"on one GPU (median of 5, map {n_map})")
+        assert same and dt < 1e-4 and da < 1e-4
 # ---- streamed lifecycle with SHARDED map maintenance: every rank runs the same LidarOdometry node on its shard
 def run_sequence(c):
     node = L.LidarOdometryNode(c, max_num_iter=15, scan_match_cnt=2, if_to_deskew=False, mode=L.MODE_GN)
