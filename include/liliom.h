@@ -136,7 +136,7 @@ int liliom_map_update_device(liliom_ctx* c, const void* d_surf_ds_body, int n, c
  * liliom_odometry_resident (or its batch forms), as left on the device.  pose7: the pose to save the frame with.  Bit for bit
  * liliom_map_update(c, <that cloud downloaded through ds_out>, n_ds, pose7, n_map_out), without the cloud crossing PCIe.
  * The scan is resident from the end of an odometry call (one that returned LILIOM_E_NOMAP / LILIOM_E_FEWMAP included) until
- * another call rewrites the buffer it lies in: liliom_voxelgrid, liliom_kf_add, liliom_kf_cloud, liliom_loop_align,
+ * another call rewrites the buffer it lies in: liliom_voxelgrid, liliom_kf_add, liliom_kf_add_resident, liliom_kf_cloud, liliom_loop_align,
  * liliom_global_map, or an odometry call that fails.  Calls that only search (liliom_scan_to_map and its resident and
  * batch forms, liliom_find_surf_corr) leave it alone, whatever their feature count: the scan keeps its own count.  With no scan resident: LILIOM_E_ARG (see liliom_last_error), nothing
  * changed.  The map update itself only reads the scan, so it stays resident across this call (and may be pushed again). */
@@ -315,6 +315,20 @@ int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double* src_poses
  * VoxelGrid(surf_leaf) of it (full_clouds_ds).  Once per keyframe (a second call: LILIOM_E_ARG, nothing changes).
  * *n_stored (optional) = points stored.  The full clouds have a device arena of their own (geometric growth, copying). */
 int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp, int kf_id, const void* full, int n, int* n_stored);
+/* The backend's keyframe from the clouds an extraction left resident on src (BackendFusion's edge_last / surf_last / full_cloud):
+ * bit for bit what
+ *   liliom_features_download(src, S, .., &ns, E, .., &ne, F, .., &nf);
+ *   liliom_kf_add(c, bp, E, ne, S, ns, kf_id, NULL, 0, n_edge_ds, NULL, 0, n_surf_ds);
+ *   liliom_kf_add_full(c, bp, *kf_id, F, nf, n_full_stored);
+ * does to c: the same id, counts, stored clouds (edge/surf arena and full arena) and state (vg_out rewritten: no scan for
+ * liliom_map_update_resident on c).  src is not changed.  src == c is allowed.  All or nothing: on any error nothing is stored and
+ * liliom_kf_count(c) is unchanged.  n_edge_ds / n_surf_ds / n_full_stored are optional.
+ * Streams: c's work is ordered after src's work so far (an event when their streams differ); the call is synchronous, so src
+ * may be reused as soon as it returns.
+ * LILIOM_E_ARG, nothing changed: NULL c / bp / src / kf_id, an invalid bp (as liliom_kf_add), no clouds resident on src,
+ * different point strides or devices, a communicator on either context. */
+int liliom_kf_add_resident(liliom_ctx* c, const liliom_backend_params* bp, liliom_ctx* src,
+                           int* kf_id, int* n_edge_ds, int* n_surf_ds, int* n_full_stored);
 
 enum { LILIOM_KF_FULL = 0, LILIOM_KF_SURF = 1 };
 /* publishCompleteMap (L:2644-2685, R:2409-2447) / the save_pcd map of mapVisualizationThread (L:2703-2718, R:2463-2477).
@@ -360,6 +374,13 @@ int liliom_icp_align(liliom_ctx* c, const void* src, int n_src, const void* tgt,
  * p' = slerp(I, quat; ratio) * p + ratio * trans, ratio = min(frac(intensity) / 0.1, 1).  publishCloudLast (:624-632) calls it
  * on the three keyframe clouds with quat = identity and trans = the relative translation of the scan. */
 int liliom_undistort(liliom_ctx* c, void* pts_inout, int n, const double trans[3], const double quat_wxyz[4]);
+/* publishCloudLast's undistortion (L/src/LidarOdometry.cpp:178-199, :624-632) on the three clouds the last extraction on c left
+ * resident (surf, edge, cut / laserCloud), in place, in one launch, with no host traffic.  Afterwards liliom_features_download(c)
+ * returns, bit for bit, what liliom_undistort(c, cloud, n, trans, quat) returns on each cloud it returned before the call (the
+ * payload publishCloudLast publishes).  Counts, the odometry's down-sampled scan (liliom_map_update_resident), the queries, the map
+ * and everything else on c are left alone.  Calling it twice de-skews twice, as calling undistortion twice does.
+ * LILIOM_E_ARG, nothing changed: no clouds resident (as liliom_features_download), NULL trans / quat. */
+int liliom_undistort_resident(liliom_ctx* c, const double trans[3], const double quat_wxyz[4]);
 
 /* ---- SURVEY §8 (f3), publishing side: the PointCloud2 layout pcl::toROSMsg gives these clouds ----
  * L/src/Preprocessing.cpp:385-401, L/src/LidarOdometry.cpp:634-649: pcl::toROSMsg copies the point array verbatim into

@@ -94,7 +94,7 @@ EXPORTS = [
     "liliom_extract_resident_batch", "liliom_features_download",
     "liliom_map_update_resident", "liliom_map_update_batch",
     "liliom_backend_window_correspond_batch", "liliom_backend_window_blocks_batch",
-    "liliom_loop_align_batch", "liliom_convert_batch",
+    "liliom_loop_align_batch", "liliom_convert_batch", "liliom_undistort_resident", "liliom_kf_add_resident",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -228,6 +228,7 @@ def lib() -> C.CDLL:
     L.liliom_comm_set_shard_block.argtypes = [vp, C.c_int]
     L.liliom_comm_set_ceres.argtypes = [vp, C.c_int]
     L.liliom_undistort.argtypes = [vp, vp, C.c_int, dp, dp]
+    L.liliom_undistort_resident.argtypes = [vp, dp, dp]
     L.liliom_map_update.argtypes = [vp, vp, C.c_int, dp, ip]
     L.liliom_map_update_device.argtypes = [vp, vp, C.c_int, dp, ip]
     L.liliom_map_update_resident.argtypes = [vp, dp, ip]
@@ -250,6 +251,7 @@ def lib() -> C.CDLL:
     L.liliom_backend_window_blocks_batch.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(dp), ip, C.POINTER(dp), ip]
     L.liliom_kf_cloud.argtypes = [vp, ip, dp, C.c_int, C.c_float, vp, C.c_int, ip]
     L.liliom_kf_add_full.argtypes = [vp, bpp, C.c_int, vp, C.c_int, ip]
+    L.liliom_kf_add_resident.argtypes = [vp, bpp, vp, ip, ip, ip, ip]
     L.liliom_global_map.argtypes = [vp, C.c_int, ip, dp, C.c_int, dp, C.c_float, vp, C.c_int, ip]
     L.liliom_loop_align.argtypes = [vp, ip, dp, C.c_int, ip, dp, C.c_int, C.c_float, C.c_double, C.c_int, C.c_double, C.c_double,
                                     dp, dp, ip, ip, ip, ip]
@@ -397,6 +399,12 @@ class Context:
         t = np.asarray(trans, dtype=np.float64); q = np.asarray(quat, dtype=np.float64)
         self._check(lib().liliom_undistort(self._h, _ptr(out), len(out), _dptr(t), _dptr(q)))
         return out
+
+    def undistort_resident(self, trans, quat=(1.0, 0.0, 0.0, 0.0)):
+        """undistort, in place, of the three clouds the last extraction left resident (liliom_undistort_resident): what
+        features_download returns afterwards is the de-skewed payload publishCloudLast publishes."""
+        t = np.ascontiguousarray(trans, dtype=np.float64); q = np.ascontiguousarray(quat, dtype=np.float64)
+        self._check(lib().liliom_undistort_resident(self._h, _dptr(t), _dptr(q)))
 
     def map_update(self, pts: np.ndarray, pose7) -> int:
         """push_frame + incremental refresh of the filtered map (SURVEY §8 f2); returns the map size."""
@@ -677,6 +685,13 @@ class Context:
         m = C.c_int()
         self._check(lib().liliom_kf_add_full(self._h, C.byref(bp), int(kf_id), _ptr(f), len(f), C.byref(m)))
         return m.value
+
+    def kf_add_resident(self, bp: BackendParams, src: "Context"):
+        """kf_add + kf_add_full of the clouds the last extraction on `src` left resident (liliom_kf_add_resident), without
+        the clouds leaving the device.  Returns (kf_id, n_edge_ds, n_surf_ds, n_full_stored)."""
+        kid, ne, ns, nf = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+        self._check(lib().liliom_kf_add_resident(self._h, C.byref(bp), src._h, C.byref(kid), C.byref(ne), C.byref(ns), C.byref(nf)))
+        return kid.value, ne.value, ns.value, nf.value
 
     def global_map(self, kind: int, kf_ids, poses7, leaf: float, pre7=None) -> np.ndarray:
         """publishCompleteMap / save_pcd's map: the stored cloud of `kind` (KF_FULL or KF_SURF) of every listed keyframe,

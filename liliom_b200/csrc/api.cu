@@ -9,10 +9,22 @@
 namespace lili {
 void nccl_destroy(liliom_ctx* c);
 
-// LidarOdometry::undistortion (L/src/LidarOdometry.cpp:178-199), in place on device points
-__global__ void k_undistort(unsigned char* __restrict__ pts, int n, int stride, D3 trans, Q4 quat) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+// LidarOdometry::undistortion (L/src/LidarOdometry.cpp:178-199), in place on device clouds: one segment per cloud, segment s owns
+// blocks [off[s], off[s + 1]) of the grid (batch.h).  A segment's size is n, or min(*d_n, n) when it is only on the device (n:
+// a host upper bound).  liliom_undistort launches one segment, liliom_undistort_resident the three resident clouds.
+struct UndistortSeg {
+    unsigned char* pts;
+    int n;
+    const int* d_n;
+};
+typedef BatchTab<UndistortSeg, 3> UndistortTab;
+
+__global__ void k_undistort(const __grid_constant__ UndistortTab tab, int stride, D3 trans, Q4 quat) {
+    const BatchSlot at = batch_slot(tab);
+    const UndistortSeg& s = tab.s[at.s];
+    const int i = at.blk.bi() * blockDim.x + threadIdx.x;
+    if (i >= (s.d_n ? min(*s.d_n, s.n) : s.n)) return;
+    unsigned char* pts = s.pts;
     float4* p0 = reinterpret_cast<float4*>(pts + (size_t)i * stride);
     float4 a = p0[0];
     const float intensity = *reinterpret_cast<const float*>(pts + (size_t)i * stride + (stride == 48 ? 32 : 16));
@@ -26,6 +38,20 @@ __global__ void k_undistort(unsigned char* __restrict__ pts, int n, int stride, 
     a.y = (float)addx(r.y, mulx(ratio_i, trans.y));
     a.z = (float)addx(r.z, mulx(ratio_i, trans.z));
     p0[0] = a;
+}
+
+// k_undistort over k <= 3 segments on the context's stream (segments without points get no blocks; none at all: no launch)
+static int undistort_launch(liliom_ctx* c, const UndistortSeg* segs, int k, const double trans[3], const double quat_wxyz[4]) {
+    UndistortTab tab{};
+    tab.n = k;
+    for (int s = 0; s < k; ++s) {
+        tab.s[s] = segs[s];
+        tab.off[s + 1] = tab.off[s] + stage_blocks(segs[s].n, 256);
+    }
+    if (tab.off[k] == 0) return LILIOM_OK;
+    k_undistort<<<tab.off[k], 256, 0, c->stream>>>(tab, c->prm.point_stride, D3{trans[0], trans[1], trans[2]},
+                                                   Q4{quat_wxyz[0], quat_wxyz[1], quat_wxyz[2], quat_wxyz[3]});
+    return launch_check(c, "k_undistort");
 }
 
 static int upload_feats(liliom_ctx* c, const void* feats, int n, int stride) {
@@ -494,10 +520,23 @@ extern "C" int liliom_undistort(liliom_ctx* c, void* pts_inout, int n, const dou
     const int stride = c->prm.point_stride;
     LILI_CUDA(c, c->raw.ensure((size_t)n * stride));
     LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, pts_inout, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
-    k_undistort<<<cdiv(n, 256), 256, 0, c->stream>>>((unsigned char*)c->raw.p, n, stride, D3{trans[0], trans[1], trans[2]},
-                                                    Q4{quat_wxyz[0], quat_wxyz[1], quat_wxyz[2], quat_wxyz[3]});
-    LILI_TRY(launch_check(c, "k_undistort"));
+    const UndistortSeg seg{c->raw.as<unsigned char>(), n, nullptr};
+    LILI_TRY(undistort_launch(c, &seg, 1, trans, quat_wxyz));
     LILI_CUDA(c, cudaMemcpyAsync(pts_inout, c->raw.p, (size_t)n * stride, cudaMemcpyDeviceToHost, c->stream));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    return LILIOM_OK;
+}
+
+// publishCloudLast's undistortion (:624-632) of the three clouds the last extraction left resident, in place, in one launch;
+// a resident Horizon extraction's sizes are read on the device
+extern "C" int liliom_undistort_resident(liliom_ctx* c, const double trans[3], const double quat_wxyz[4]) {
+    if (!c || !trans || !quat_wxyz) return LILIOM_E_ARG;
+    FeatCloud f[3];
+    LILI_TRY(feat_clouds(c, f));
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    UndistortSeg segs[3];
+    for (int k = 0; k < 3; ++k) segs[k] = UndistortSeg{f[k].buf->as<unsigned char>(), f[k].n_max, f[k].d_n};
+    LILI_TRY(undistort_launch(c, segs, 3, trans, quat_wxyz));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     return LILIOM_OK;
 }
@@ -671,19 +710,18 @@ extern "C" int liliom_extract_resident_batch(liliom_ctx* const* ctxs, int B, con
 extern "C" int liliom_features_download(liliom_ctx* c, void* surf, int surf_cap, int* n_surf, void* edge, int edge_cap, int* n_edge,
                                         void* cut, int cut_cap, int* n_cut) {
     if (!c || !n_surf || !n_edge || !n_cut) return LILIOM_E_ARG;
-    if (!c->feat_ready) return LILIOM_E_ARG;
+    FeatCloud f[3];
+    LILI_TRY(feat_clouds(c, f));
     LILI_CUDA(c, cudaSetDevice(c->device));
     const int stride = c->prm.point_stride;
-    int m[3] = {c->feat_counts[0], c->feat_counts[1], c->feat_counts[2]};
-    if (m[0] < 0)        // resident Horizon extraction: the counts are on the device
-        LILI_TRY(read_back(c, {{m, c->feat_dcounts, 2 * sizeof(int)}, {m + 2, c->feat_dcut, sizeof(int)}}));
+    int m[3];
+    LILI_TRY(feat_sizes(c, f, m));
     *n_surf = m[0]; *n_edge = m[1]; *n_cut = m[2];
-    const DevBuf* src[3] = {&c->surf, &c->edge, stride == 48 ? &c->cut : &c->rot_cloud};
     void* out[3] = {surf, edge, cut};
     const int cap[3] = {surf_cap, edge_cap, cut_cap};
     for (int k = 0; k < 3; ++k) if (out[k] && m[k] > cap[k]) return LILIOM_E_CAPACITY;
     for (int k = 0; k < 3; ++k)
-        if (out[k] && m[k] > 0) LILI_CUDA(c, cudaMemcpyAsync(out[k], src[k]->p, (size_t)m[k] * stride, cudaMemcpyDeviceToHost, c->stream));
+        if (out[k] && m[k] > 0) LILI_CUDA(c, cudaMemcpyAsync(out[k], f[k].buf->p, (size_t)m[k] * stride, cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     return LILIOM_OK;
 }

@@ -426,6 +426,7 @@ struct liliom_ctx {
     // the clouds the last extraction left resident (surf, edge and cut / laserCloud; liliom_features_download)
     bool feat_ready = false;
     int feat_counts[3] = {0, 0, 0};      // their sizes; -1: only on the device (resident Horizon extraction)
+    int feat_max[3] = {0, 0, 0};         // Horizon: host upper bounds of those sizes (the extractor sizes the buffers from them)
     int* feat_dcounts = nullptr;         // Horizon: the surf and edge counts on the device, a spare word behind them
     const int* feat_dcut = nullptr;      // Horizon: the cut count on the device (idx_a[n], or feat_dcounts[2] once idx_a is reused)
 
@@ -589,6 +590,31 @@ inline int feat_keep_cut(liliom_ctx* c) {
     if (!c->feat_ready || c->feat_counts[2] >= 0 || c->feat_dcut == c->feat_dcounts + 2) return LILIOM_OK;
     LILI_CUDA(c, cudaMemcpyAsync(c->feat_dcounts + 2, c->feat_dcut, sizeof(int), cudaMemcpyDeviceToDevice, c->stream));
     c->feat_dcut = c->feat_dcounts + 2;
+    return LILIOM_OK;
+}
+
+// The clouds the last extraction left resident, in the order surf, edge, cut (ROT: laserCloud): the buffer each lies in and its
+// size, known on the host (n >= 0, n_max = n, d_n = nullptr) or only on the device after a resident Horizon extraction (n = -1,
+// n_max a host upper bound, d_n the size on the device).  LILIOM_E_ARG when nothing is resident.
+struct FeatCloud {
+    DevBuf* buf;
+    int n, n_max;
+    const int* d_n;
+};
+inline int feat_clouds(liliom_ctx* c, FeatCloud f[3]) {
+    if (!c->feat_ready) return LILIOM_E_ARG;
+    DevBuf* buf[3] = {&c->surf, &c->edge, c->prm.point_stride == 48 ? &c->cut : &c->rot_cloud};
+    const int* d_n[3] = {c->feat_dcounts, c->feat_dcounts + 1, c->feat_dcut};
+    for (int k = 0; k < 3; ++k) {
+        const int n = c->feat_counts[k];
+        f[k] = n >= 0 ? FeatCloud{buf[k], n, n, nullptr} : FeatCloud{buf[k], n, c->feat_max[k], d_n[k]};
+    }
+    return LILIOM_OK;
+}
+// Their sizes on the host: one read-back of all three when they are only on the device.
+inline int feat_sizes(liliom_ctx* c, const FeatCloud f[3], int m[3]) {
+    for (int k = 0; k < 3; ++k) m[k] = f[k].n;
+    if (f[0].d_n) LILI_TRY(read_back(c, {{m, f[0].d_n, sizeof(int)}, {m + 1, f[1].d_n, sizeof(int)}, {m + 2, f[2].d_n, sizeof(int)}}));
     return LILIOM_OK;
 }
 

@@ -585,6 +585,9 @@ static int hz_end(const HzJob& j, bool sync_counts, int* n_surf, int* n_edge, in
     c->n_surf_max = min(n, HZ_PATCHES * 36);
     c->feat_dcounts = totals;
     c->feat_dcut = c->idx_a.as<int>() + n;
+    c->feat_max[0] = c->n_surf_max;
+    c->feat_max[1] = min(n, HZ_PATCHES * 6);
+    c->feat_max[2] = n;
     if (!sync_counts) {          // resident pipeline: the counts stay on the device, no host round trip
         c->n_surf_dev = -1;
         *n_surf = *n_edge = *n_cut = -1;

@@ -202,6 +202,53 @@ static int backend_check(liliom_ctx* c, const liliom_backend_params* bp) {
     return LILIOM_OK;
 }
 
+// The keyframe store's writes, from clouds already on the device (the host calls upload them first; liliom_kf_add_resident
+// reads them where an extraction left them).  The caller has reserved room behind the stored points (kf_reserve) and records
+// the keyframe (KfEntry) once everything it stores is written.
+// The scan half (:1502-1514): VoxelGrid(edge_leaf) of edge and VoxelGrid(surf_leaf) of surf behind the stored points of
+// kf_arena, edge first; the surf output also stays in vg_out.
+static int kf_scan_dev(liliom_ctx* c, const liliom_backend_params* bp, const void* edge, int n_edge, const void* surf, int n_surf,
+                       int* me, int* ms) {
+    const int stride = c->prm.point_stride;
+    c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
+    LILI_CUDA(c, c->vg_out.ensure((size_t)(n_surf > 0 ? n_surf : 1) * stride));
+    LILI_CUDA(c, c->vg_count.ensure(16));
+    unsigned char* tail = (unsigned char*)c->kf_arena.p + (size_t)c->kf_used * stride;
+    int* cnt = c->vg_count.as<int>();
+    LILI_TRY(voxelgrid_dev_sync(c, edge, n_edge, stride, bp->edge_leaf, tail, cnt, nullptr, me));                 // :1502-1507
+    LILI_TRY(voxelgrid_dev_sync(c, surf, n_surf, stride, bp->surf_leaf, c->vg_out.p, cnt + 1, nullptr, ms));      // :1509-1514
+    if (*ms) LILI_CUDA(c, cudaMemcpyAsync(tail + (size_t)*me * stride, c->vg_out.p, (size_t)*ms * stride, cudaMemcpyDeviceToDevice, c->stream));
+    return LILIOM_OK;
+}
+
+// The full-cloud half (L:1494-1500 / R:1373-1376) behind the stored points of kf_full: variant 0 the n points as received (one
+// copy from wherever they lie, host or device), variant 1 VoxelGrid(surf_leaf) of them (on the device).  *m: the points written.
+static int kf_full_dev(liliom_ctx* c, const liliom_backend_params* bp, const void* full, int n, int* m) {
+    const int stride = c->prm.point_stride;
+    unsigned char* tail = (unsigned char*)c->kf_full.p + (size_t)c->kf_full_used * stride;
+    *m = n;
+    if (n > 0 && bp->variant == 0) {                              // L:1498-1500 full_clouds: the cloud as received
+        LILI_CUDA(c, cudaMemcpyAsync(tail, full, (size_t)n * stride, cudaMemcpyDefault, c->stream));
+    } else if (n > 0) {                                           // R:1373-1376 full_clouds_ds: VoxelGrid(surf_leaf) of it
+        LILI_CUDA(c, c->vg_count.ensure(16));
+        LILI_TRY(voxelgrid_dev_sync(c, full, n, stride, bp->surf_leaf, tail, c->vg_count.as<int>(), nullptr, m));
+    }
+    return LILIOM_OK;
+}
+
+// Records a keyframe whose scan half (me edge + ms surf points) kf_scan_dev has written; returns its id
+static int kf_push(liliom_ctx* c, int me, int ms) {
+    c->kfs.push_back(KfEntry{c->kf_used, c->kf_used + me, me, ms});
+    c->kf_used += (long long)me + ms;
+    return (int)c->kfs.size() - 1;
+}
+// ... and its full cloud (m points) that kf_full_dev has written
+static void kf_push_full(liliom_ctx* c, int kf_id, int m) {
+    c->kfs[kf_id].full_off = c->kf_full_used;
+    c->kfs[kf_id].n_full = m;
+    c->kf_full_used += m;
+}
+
 }  // namespace lili
 
 using namespace lili;
@@ -236,27 +283,47 @@ extern "C" int liliom_kf_add(liliom_ctx* c, const liliom_backend_params* bp, con
     const long long n = (long long)n_edge + n_surf;
     LILI_TRY(kf_reserve(c, c->kf_arena, c->kf_used, c->kf_used + n));          // VoxelGrid never outputs more points than it reads
     LILI_CUDA(c, c->raw.ensure((size_t)(n > 0 ? n : 1) * stride));
-    c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
-    LILI_CUDA(c, c->vg_out.ensure((size_t)(n_surf > 0 ? n_surf : 1) * stride));
-    LILI_CUDA(c, c->vg_count.ensure(16));
     unsigned char* raw = (unsigned char*)c->raw.p;
     if (n_edge) LILI_CUDA(c, cudaMemcpyAsync(raw, edge_last, (size_t)n_edge * stride, cudaMemcpyHostToDevice, c->stream));
     if (n_surf) LILI_CUDA(c, cudaMemcpyAsync(raw + (size_t)n_edge * stride, surf_last, (size_t)n_surf * stride, cudaMemcpyHostToDevice, c->stream));
-    unsigned char* tail = (unsigned char*)c->kf_arena.p + (size_t)c->kf_used * stride;
-    int* cnt = c->vg_count.as<int>();
     int me = 0, ms = 0;
-    LILI_TRY(voxelgrid_dev_sync(c, raw, n_edge, stride, bp->edge_leaf, tail, cnt, nullptr, &me));                                   // :1502-1507
-    LILI_TRY(voxelgrid_dev_sync(c, raw + (size_t)n_edge * stride, n_surf, stride, bp->surf_leaf, c->vg_out.p, cnt + 1, nullptr, &ms));   // :1509-1514
+    LILI_TRY(kf_scan_dev(c, bp, raw, n_edge, raw + (size_t)n_edge * stride, n_surf, &me, &ms));
     if (n_edge_ds) *n_edge_ds = me;
     if (n_surf_ds) *n_surf_ds = ms;
     if ((edge_ds_out && me > edge_cap) || (surf_ds_out && ms > surf_cap)) return LILIOM_E_CAPACITY;   // nothing stored
-    if (ms) LILI_CUDA(c, cudaMemcpyAsync(tail + (size_t)me * stride, c->vg_out.p, (size_t)ms * stride, cudaMemcpyDeviceToDevice, c->stream));
+    const unsigned char* tail = (const unsigned char*)c->kf_arena.p + (size_t)c->kf_used * stride;
     if (edge_ds_out && me) LILI_CUDA(c, cudaMemcpyAsync(edge_ds_out, tail, (size_t)me * stride, cudaMemcpyDeviceToHost, c->stream));
     if (surf_ds_out && ms) LILI_CUDA(c, cudaMemcpyAsync(surf_ds_out, c->vg_out.p, (size_t)ms * stride, cudaMemcpyDeviceToHost, c->stream));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    c->kfs.push_back(KfEntry{c->kf_used, c->kf_used + me, me, ms});
-    c->kf_used += (long long)me + ms;
-    *kf_id = (int)c->kfs.size() - 1;
+    *kf_id = kf_push(c, me, ms);
+    return LILIOM_OK;
+}
+
+// publishCloudLast -> BackendFusion's keyframe without the host: the scan half and the full cloud from the clouds an extraction
+// left resident on src (surf_last, edge_last, full_cloud), on c's stream ordered after src's, in one all-or-nothing call.
+extern "C" int liliom_kf_add_resident(liliom_ctx* c, const liliom_backend_params* bp, liliom_ctx* src, int* kf_id, int* n_edge_ds,
+                                      int* n_surf_ds, int* n_full_stored) {
+    if (!c || !bp || !src || !kf_id) return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, bp));
+    if (src->nranks > 1) { c->last_error = "the source context has a communicator: the backend keyframe store is single-GPU"; return LILIOM_E_ARG; }
+    if (src->prm.point_stride != c->prm.point_stride || src->device != c->device) return LILIOM_E_ARG;
+    FeatCloud f[3];                                               // surf, edge, cut (ROT: laserCloud)
+    LILI_TRY(feat_clouds(src, f));
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    int m[3];
+    LILI_TRY(feat_sizes(src, f, m));                              // they size the arenas and the filters
+    LILI_TRY(batch_join_in(c, {src}));                            // src's work so far before c's reads of its clouds
+    LILI_TRY(kf_reserve(c, c->kf_arena, c->kf_used, c->kf_used + (long long)m[1] + m[0]));   // both arenas before any write
+    LILI_TRY(kf_reserve(c, c->kf_full, c->kf_full_used, c->kf_full_used + m[2]));
+    int me = 0, ms = 0, mf = 0;
+    LILI_TRY(kf_scan_dev(c, bp, f[1].buf->p, m[1], f[0].buf->p, m[0], &me, &ms));
+    LILI_TRY(kf_full_dev(c, bp, f[2].buf->p, m[2], &mf));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    *kf_id = kf_push(c, me, ms);
+    kf_push_full(c, *kf_id, mf);
+    if (n_edge_ds) *n_edge_ds = me;
+    if (n_surf_ds) *n_surf_ds = ms;
+    if (n_full_stored) *n_full_stored = mf;
     return LILIOM_OK;
 }
 
@@ -664,20 +731,16 @@ extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp
     LILI_CUDA(c, cudaSetDevice(c->device));
     const int stride = c->prm.point_stride;
     LILI_TRY(kf_reserve(c, c->kf_full, c->kf_full_used, c->kf_full_used + n));     // VoxelGrid never outputs more points than it reads
-    unsigned char* tail = (unsigned char*)c->kf_full.p + (size_t)c->kf_full_used * stride;
-    int m = n;
-    if (n > 0 && bp->variant == 0) {                              // L:1498-1500 full_clouds: the cloud as received
-        LILI_CUDA(c, cudaMemcpyAsync(tail, full, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
-        LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    } else if (n > 0) {                                           // R:1373-1376 full_clouds_ds: VoxelGrid(surf_leaf) of it
+    const void* in = full;                                        // variant 0 copies the host cloud straight into the arena
+    if (n > 0 && bp->variant == 1) {                              // variant 1 filters it on the device
         LILI_CUDA(c, c->raw.ensure((size_t)n * stride));
-        LILI_CUDA(c, c->vg_count.ensure(16));
         LILI_CUDA(c, cudaMemcpyAsync(c->raw.p, full, (size_t)n * stride, cudaMemcpyHostToDevice, c->stream));
-        LILI_TRY(voxelgrid_dev_sync(c, c->raw.p, n, stride, bp->surf_leaf, tail, c->vg_count.as<int>(), nullptr, &m));
+        in = c->raw.p;
     }
-    c->kfs[kf_id].full_off = c->kf_full_used;
-    c->kfs[kf_id].n_full = m;
-    c->kf_full_used += m;
+    int m = 0;
+    LILI_TRY(kf_full_dev(c, bp, in, n, &m));
+    LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    kf_push_full(c, kf_id, m);
     if (n_stored) *n_stored = m;
     return LILIOM_OK;
 }
