@@ -752,7 +752,7 @@ static int odo_filter(liliom_ctx* c, bool spec_failed, int* step) {
             LILI_TRY(voxelgrid_dev(c, c->surf.p, n_max, d_n, stride, c->prm.leaf_scan, c->vg_out.p, c->vg_count.as<int>(), c->feats.as<float4>(), key_bits));
         c->d_nfeats = c->vg_count.as<int>();
         c->vg_used24 = !coop && key_bits < 32;
-        c->vg_check = coop || key_bits <= 32;
+        c->vg_check = n_max > 0 && (coop || key_bits <= 32);   // an empty scan writes no vg_params: nothing of this call to read back
         c->vg_bail = false;
         c->vg_wide = false;
     } else {   // leaf_scan == 0: benchmark mode, every surf feature is a query
