@@ -329,6 +329,31 @@ int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp, int kf_id
  * different point strides or devices, a communicator on either context. */
 int liliom_kf_add_resident(liliom_ctx* c, const liliom_backend_params* bp, liliom_ctx* src,
                            int* kf_id, int* n_edge_ds, int* n_surf_ds, int* n_full_stored);
+/* liliom_kf_add_resident of B independent sessions in one call: session i stores into ctxs[i] the clouds left resident on srcs[i].
+ * bps: B structs; srcs: B contexts; kf_id, status: B ints; n_edge_ds, n_surf_ds, n_full_stored: B ints each, or NULL.  Session i
+ * gets exactly what liliom_kf_add_resident(ctxs[i], &bps[i], srcs[i], &kf_id[i], &n_edge_ds[i], &n_surf_ds[i], &n_full_stored[i])
+ * would give it, bit for bit: status, liliom_last_error, id and counts, the stored edge/surf and full clouds and their places in
+ * both arenas, launches and lib_launches, and the state left in both contexts (no resident scan for liliom_map_update_resident on
+ * ctxs[i]; srcs[i] unchanged), so that solo and batched calls mix freely.  A session with no keyframe this tick is simply left
+ * out.  Horizon (48-byte, usually variant 0) and ROT (32-byte, usually variant 1) sessions may be mixed, each with its own
+ * parameters.
+ * Sources: srcs[i] may be ctxs[i] itself, another session's backend, or the source of several sessions.  The store never writes a
+ * source's resident clouds, and every source's sizes are read before any session writes, so the result is that of the solo calls
+ * run in any order.
+ * Every kernel of the VoxelGrid chains runs once for up to 32 sessions on ctxs[0]'s stream (the edge chains of every session, then
+ * the surf chains, then variant 1's full chains); the library sorts and scans stay per session, in order on the same stream, and
+ * variant 0's full clouds are device-to-device copies.  The streams of every backend and of every running session's source are
+ * joined in before the shared launches with events, and every backend's stream is joined out after them.  The call waits three
+ * times for all sessions together (the sizes of the sources whose sizes are only on the device, every cloud's count, the stored
+ * clouds) where B solo calls wait four times each (Horizon with variant 0, ROT with variant 1); a batch without device-only sizes
+ * waits twice.  A session whose voxel index wraps (wide keys) finishes on its solo path inside the call.  An arena's growth copy
+ * is queued on ctxs[0]'s stream and waits once more.  The call is synchronous: a source may be reused as soon as it returns.
+ * A session's own error (every error its solo call returns: no clouds resident on the source, an invalid bp, different strides
+ * or devices, a source with a communicator, a NULL srcs[i]) is its status, and that session is left unchanged; the others run.
+ * LILIOM_E_ARG for the whole call, nothing changed: B < 1, a NULL array (ctxs, bps, srcs, kf_id, status), a NULL or repeated
+ * backend context, backend contexts on different devices, a backend context with a communicator. */
+int liliom_kf_add_resident_batch(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps, liliom_ctx* const* srcs,
+                                 int* kf_id, int* n_edge_ds, int* n_surf_ds, int* n_full_stored, int* status);
 
 enum { LILIOM_KF_FULL = 0, LILIOM_KF_SURF = 1 };
 /* publishCompleteMap (L:2644-2685, R:2409-2447) / the save_pcd map of mapVisualizationThread (L:2703-2718, R:2463-2477).
@@ -381,6 +406,18 @@ int liliom_undistort(liliom_ctx* c, void* pts_inout, int n, const double trans[3
  * and everything else on c are left alone.  Calling it twice de-skews twice, as calling undistortion twice does.
  * LILIOM_E_ARG, nothing changed: no clouds resident (as liliom_features_download), NULL trans / quat. */
 int liliom_undistort_resident(liliom_ctx* c, const double trans[3], const double quat_wxyz[4]);
+/* liliom_undistort_resident of B independent sessions in one call.  trans: 3*B doubles, quat_wxyz: 4*B doubles, status: B ints.
+ * Session i gets exactly what liliom_undistort_resident(ctxs[i], trans + 3*i, quat_wxyz + 4*i) would give it, bit for bit: status,
+ * liliom_last_error, the de-skewed clouds (liliom_features_download), launches, and everything else on ctxs[i] left alone, so that
+ * solo and batched calls mix freely.  A session without a keyframe this tick is simply left out of ctxs.  Horizon (48-byte) and
+ * ROT (32-byte) sessions may be mixed, each with its own motion.
+ * The three clouds of up to 32 sessions share one k_undistort_batch launch on ctxs[0]'s stream (other sessions' streams are
+ * joined with events), each cloud with its solo launch's blocks; a resident Horizon extraction's sizes are read on the device; a
+ * session whose clouds have no points takes part in no launch, as in its solo call.  The call waits once for all sessions.
+ * A session's own error (LILIOM_E_ARG: no clouds resident) is its status; the others run.
+ * LILIOM_E_ARG for the whole call, nothing changed: B < 1, a NULL array (ctxs, trans, quat_wxyz, status), a NULL or repeated
+ * context, contexts on different devices, a context with a communicator. */
+int liliom_undistort_resident_batch(liliom_ctx* const* ctxs, int B, const double* trans, const double* quat_wxyz, int* status);
 
 /* ---- SURVEY §8 (f3), publishing side: the PointCloud2 layout pcl::toROSMsg gives these clouds ----
  * L/src/Preprocessing.cpp:385-401, L/src/LidarOdometry.cpp:634-649: pcl::toROSMsg copies the point array verbatim into

@@ -95,6 +95,7 @@ EXPORTS = [
     "liliom_map_update_resident", "liliom_map_update_batch",
     "liliom_backend_window_correspond_batch", "liliom_backend_window_blocks_batch",
     "liliom_loop_align_batch", "liliom_convert_batch", "liliom_undistort_resident", "liliom_kf_add_resident",
+    "liliom_undistort_resident_batch", "liliom_kf_add_resident_batch",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -229,6 +230,7 @@ def lib() -> C.CDLL:
     L.liliom_comm_set_ceres.argtypes = [vp, C.c_int]
     L.liliom_undistort.argtypes = [vp, vp, C.c_int, dp, dp]
     L.liliom_undistort_resident.argtypes = [vp, dp, dp]
+    L.liliom_undistort_resident_batch.argtypes = [C.POINTER(vp), C.c_int, dp, dp, ip]
     L.liliom_map_update.argtypes = [vp, vp, C.c_int, dp, ip]
     L.liliom_map_update_device.argtypes = [vp, vp, C.c_int, dp, ip]
     L.liliom_map_update_resident.argtypes = [vp, dp, ip]
@@ -252,6 +254,7 @@ def lib() -> C.CDLL:
     L.liliom_kf_cloud.argtypes = [vp, ip, dp, C.c_int, C.c_float, vp, C.c_int, ip]
     L.liliom_kf_add_full.argtypes = [vp, bpp, C.c_int, vp, C.c_int, ip]
     L.liliom_kf_add_resident.argtypes = [vp, bpp, vp, ip, ip, ip, ip]
+    L.liliom_kf_add_resident_batch.argtypes = [C.POINTER(vp), C.c_int, bpp, C.POINTER(vp), ip, ip, ip, ip, ip]
     L.liliom_global_map.argtypes = [vp, C.c_int, ip, dp, C.c_int, dp, C.c_float, vp, C.c_int, ip]
     L.liliom_loop_align.argtypes = [vp, ip, dp, C.c_int, ip, dp, C.c_int, C.c_float, C.c_double, C.c_int, C.c_double, C.c_double,
                                     dp, dp, ip, ip, ip, ip]
@@ -990,6 +993,43 @@ def loop_align_batch(ctxs, src_ids, src_poses, tgt_ids, tgt_poses, params):
         raise LiliomError(rc)
     out = [(np.array(r.T16[:], np.float64).reshape(4, 4), r.fitness, bool(r.converged), r.iters, r.n_src, r.n_tgt) for r in res[:B]]
     return out, status[:B]
+
+
+def undistort_resident_batch(ctxs, trans, quats):
+    """undistort_resident of every context in `ctxs` in one call (liliom_undistort_resident_batch): session i gets what
+    ctxs[i].undistort_resident(trans[i], quats[i]) would give it.  trans: (B, 3); quats: (B, 4) wxyz.  Returns status (B,); a
+    session's own error is its status, a whole-call error raises LiliomError."""
+    B = len(ctxs)
+    t = np.ascontiguousarray(trans, dtype=np.float64).reshape(-1) if trans is not None else None
+    q = np.ascontiguousarray(quats, dtype=np.float64).reshape(-1) if quats is not None else None
+    for name, a, w in (("trans", t, 3), ("quats", q, 4)):
+        if a is not None and len(a) != w * B:
+            raise ValueError(f"{name}: expected {w * B} doubles (B x {w}), got {len(a)}")
+    status = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_undistort_resident_batch(_handles(ctxs), B, _dptr(t) if t is not None else None,
+                                               _dptr(q) if q is not None else None, _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    return status[:B]
+
+
+def kf_add_resident_batch(ctxs, bps, srcs):
+    """kf_add_resident of every context in `ctxs` in one call (liliom_kf_add_resident_batch): session i gets what
+    ctxs[i].kf_add_resident(bps[i], srcs[i]) would give it.  bps: B BackendParams; srcs: B contexts (None: a NULL source, that
+    session's error).  Returns (ids (B,), counts (B, 3) as (n_edge_ds, n_surf_ds, n_full_stored), status (B,)); a session's
+    own error is its status, a whole-call error raises LiliomError."""
+    B = len(ctxs)
+    if len(bps) != B or len(srcs) != B:
+        raise ValueError(f"expected {B} backend parameter sets and sources")
+    prm = (BackendParams * max(B, 1))(*bps)
+    ids = np.full(max(B, 1), -1, np.int32)
+    counts = np.zeros((max(B, 1), 3), np.int32)
+    ne, ns, nf = (np.ascontiguousarray(counts[:, k]) for k in range(3))
+    status = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_kf_add_resident_batch(_handles(ctxs), B, prm, _handles(srcs), _ip(ids), _ip(ne), _ip(ns), _ip(nf), _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    return ids[:B], np.stack([ne, ns, nf], axis=1)[:B], status[:B]
 
 
 def wire_msgs(msgs):

@@ -11,7 +11,8 @@ void nccl_destroy(liliom_ctx* c);
 
 // LidarOdometry::undistortion (L/src/LidarOdometry.cpp:178-199), in place on device clouds: one segment per cloud, segment s owns
 // blocks [off[s], off[s + 1]) of the grid (batch.h).  A segment's size is n, or min(*d_n, n) when it is only on the device (n:
-// a host upper bound).  liliom_undistort launches one segment, liliom_undistort_resident the three resident clouds.
+// a host upper bound).  liliom_undistort launches one segment, liliom_undistort_resident the three resident clouds,
+// liliom_undistort_resident_batch the three of each of up to kBatchMax sessions (k_undistort_batch).
 struct UndistortSeg {
     unsigned char* pts;
     int n;
@@ -19,10 +20,8 @@ struct UndistortSeg {
 };
 typedef BatchTab<UndistortSeg, 3> UndistortTab;
 
-__global__ void k_undistort(const __grid_constant__ UndistortTab tab, int stride, D3 trans, Q4 quat) {
-    const BatchSlot at = batch_slot(tab);
-    const UndistortSeg& s = tab.s[at.s];
-    const int i = at.blk.bi() * blockDim.x + threadIdx.x;
+// point i of segment s (:181-197)
+__device__ __forceinline__ void undistort_at(const UndistortSeg& s, int i, int stride, const D3& trans, const Q4& quat) {
     if (i >= (s.d_n ? min(*s.d_n, s.n) : s.n)) return;
     unsigned char* pts = s.pts;
     float4* p0 = reinterpret_cast<float4*>(pts + (size_t)i * stride);
@@ -40,6 +39,28 @@ __global__ void k_undistort(const __grid_constant__ UndistortTab tab, int stride
     p0[0] = a;
 }
 
+__global__ void k_undistort(const __grid_constant__ UndistortTab tab, int stride, D3 trans, Q4 quat) {
+    const BatchSlot at = batch_slot(tab);
+    undistort_at(tab.s[at.s], at.blk.bi() * blockDim.x + threadIdx.x, stride, trans, quat);
+}
+
+// a segment of the batched launch: the session's stride and motion travel with each of its clouds, so that Horizon and ROT
+// sessions share a launch
+struct UndistortBatchSeg {
+    UndistortSeg seg;
+    int stride;
+    D3 trans;
+    Q4 quat;
+};
+typedef BatchTab<UndistortBatchSeg, 3 * kBatchMax> UndistortBatchTab;
+static_assert(sizeof(UndistortBatchTab) <= 32764, "a batched launch's session table must fit in the kernel parameter space");
+
+__global__ void k_undistort_batch(const __grid_constant__ UndistortBatchTab tab) {
+    const BatchSlot at = batch_slot(tab);
+    const UndistortBatchSeg& s = tab.s[at.s];
+    undistort_at(s.seg, at.blk.bi() * blockDim.x + threadIdx.x, s.stride, s.trans, s.quat);
+}
+
 // k_undistort over k <= 3 segments on the context's stream (segments without points get no blocks; none at all: no launch)
 static int undistort_launch(liliom_ctx* c, const UndistortSeg* segs, int k, const double trans[3], const double quat_wxyz[4]) {
     UndistortTab tab{};
@@ -52,6 +73,14 @@ static int undistort_launch(liliom_ctx* c, const UndistortSeg* segs, int k, cons
     k_undistort<<<tab.off[k], 256, 0, c->stream>>>(tab, c->prm.point_stride, D3{trans[0], trans[1], trans[2]},
                                                    Q4{quat_wxyz[0], quat_wxyz[1], quat_wxyz[2], quat_wxyz[3]});
     return launch_check(c, "k_undistort");
+}
+
+// the three resident clouds of c as undistort segments (feat_clouds: LILIOM_E_ARG when nothing is resident)
+static int undistort_resident_segs(liliom_ctx* c, UndistortSeg segs[3]) {
+    FeatCloud f[3];
+    LILI_TRY(feat_clouds(c, f));
+    for (int k = 0; k < 3; ++k) segs[k] = UndistortSeg{f[k].buf->as<unsigned char>(), f[k].n_max, f[k].d_n};
+    return LILIOM_OK;
 }
 
 static int upload_feats(liliom_ctx* c, const void* feats, int n, int stride) {
@@ -531,13 +560,48 @@ extern "C" int liliom_undistort(liliom_ctx* c, void* pts_inout, int n, const dou
 // a resident Horizon extraction's sizes are read on the device
 extern "C" int liliom_undistort_resident(liliom_ctx* c, const double trans[3], const double quat_wxyz[4]) {
     if (!c || !trans || !quat_wxyz) return LILIOM_E_ARG;
-    FeatCloud f[3];
-    LILI_TRY(feat_clouds(c, f));
-    LILI_CUDA(c, cudaSetDevice(c->device));
     UndistortSeg segs[3];
-    for (int k = 0; k < 3; ++k) segs[k] = UndistortSeg{f[k].buf->as<unsigned char>(), f[k].n_max, f[k].d_n};
+    LILI_TRY(undistort_resident_segs(c, segs));
+    LILI_CUDA(c, cudaSetDevice(c->device));
     LILI_TRY(undistort_launch(c, segs, 3, trans, quat_wxyz));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
+    return LILIOM_OK;
+}
+
+// liliom_undistort_resident of several sessions: the three clouds of up to kBatchMax sessions per k_undistort_batch launch, each
+// segment with its solo launch's blocks; a session whose clouds have no points takes part in no launch, as in its solo call
+extern "C" int liliom_undistort_resident_batch(liliom_ctx* const* ctxs, int B, const double* trans, const double* quat_wxyz, int* status) {
+    if (!batch_ctxs_ok(ctxs, B) || !trans || !quat_wxyz || !status) return LILIOM_E_ARG;
+    liliom_ctx* c0 = ctxs[0];
+    LILI_CUDA(c0, cudaSetDevice(c0->device));
+    std::vector<UndistortBatchSeg> segs;    // three per session that launches
+    std::vector<liliom_ctx*> who;
+    for (int i = 0; i < B; ++i) {
+        liliom_ctx* c = ctxs[i];
+        UndistortSeg s[3];
+        status[i] = undistort_resident_segs(c, s);
+        if (status[i] != LILIOM_OK || stage_blocks(s[0].n, 256) + stage_blocks(s[1].n, 256) + stage_blocks(s[2].n, 256) == 0) continue;
+        const double* t = trans + 3 * (size_t)i;
+        const double* q = quat_wxyz + 4 * (size_t)i;
+        for (int k = 0; k < 3; ++k) segs.push_back(UndistortBatchSeg{s[k], c->prm.point_stride, D3{t[0], t[1], t[2]}, Q4{q[0], q[1], q[2], q[3]}});
+        who.push_back(c);
+    }
+    const std::vector<liliom_ctx*> all(ctxs, ctxs + B);
+    LILI_TRY(batch_join_in(c0, all));
+    for (size_t first = 0; first < who.size(); first += kBatchMax) {
+        const int n = (int)std::min(who.size() - first, (size_t)kBatchMax);
+        UndistortBatchTab tab{};
+        tab.n = 3 * n;
+        for (int m = 0; m < 3 * n; ++m) {
+            tab.s[m] = segs[3 * first + m];
+            tab.off[m + 1] = tab.off[m] + stage_blocks(tab.s[m].seg.n, 256);
+        }
+        k_undistort_batch<<<tab.off[3 * n], 256, 0, c0->stream>>>(tab);
+        LILI_CUDA(c0, cudaGetLastError());
+        for (int m = 0; m < n; ++m) who[first + m]->cnt.launches++;
+    }
+    LILI_TRY(batch_join_out(c0, all));
+    LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
     return LILIOM_OK;
 }
 

@@ -631,6 +631,7 @@ int voxelgrid_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, in
 int voxelgrid_dev_sync(liliom_ctx* c, const void* d_in, int n, int stride, float leaf, void* d_out, int* d_count, float4* d_feats, int* m,
                        int key_bits = 32);
 int vg_minmax_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride);
+int vg_chain_ensure(liliom_ctx* c, long long n, size_t kb);     // the buffers of voxelgrid_dev's chain over n points, kb-byte keys
 int voxelgrid_coop(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, int stride, float leaf, void* d_out, int* d_count, float4* d_feats,
                    bool* used);
 __global__ void k_kf_refl(const unsigned char* __restrict__ pts, int n, float* __restrict__ out);      // keyframes.cu: reflectivity of 48-byte points

@@ -14,6 +14,7 @@
 #include "ctx.cuh"
 #include "dev_math.cuh"
 #include "kf_table.h"
+#include <algorithm>
 #include <type_traits>
 
 namespace lili {
@@ -202,6 +203,14 @@ static int backend_check(liliom_ctx* c, const liliom_backend_params* bp) {
     return LILIOM_OK;
 }
 
+// the scan half's surf output (ms points in vg_out) behind its me edge points, at the tail of kf_arena
+static int kf_surf_behind(liliom_ctx* c, int me, int ms) {
+    const size_t stride = (size_t)c->prm.point_stride;
+    unsigned char* tail = (unsigned char*)c->kf_arena.p + (size_t)c->kf_used * stride;
+    if (ms) LILI_CUDA(c, cudaMemcpyAsync(tail + (size_t)me * stride, c->vg_out.p, (size_t)ms * stride, cudaMemcpyDeviceToDevice, c->stream));
+    return LILIOM_OK;
+}
+
 // The keyframe store's writes, from clouds already on the device (the host calls upload them first; liliom_kf_add_resident
 // reads them where an extraction left them).  The caller has reserved room behind the stored points (kf_reserve) and records
 // the keyframe (KfEntry) once everything it stores is written.
@@ -217,8 +226,7 @@ static int kf_scan_dev(liliom_ctx* c, const liliom_backend_params* bp, const voi
     int* cnt = c->vg_count.as<int>();
     LILI_TRY(voxelgrid_dev_sync(c, edge, n_edge, stride, bp->edge_leaf, tail, cnt, nullptr, me));                 // :1502-1507
     LILI_TRY(voxelgrid_dev_sync(c, surf, n_surf, stride, bp->surf_leaf, c->vg_out.p, cnt + 1, nullptr, ms));      // :1509-1514
-    if (*ms) LILI_CUDA(c, cudaMemcpyAsync(tail + (size_t)*me * stride, c->vg_out.p, (size_t)*ms * stride, cudaMemcpyDeviceToDevice, c->stream));
-    return LILIOM_OK;
+    return kf_surf_behind(c, *me, *ms);
 }
 
 // The full-cloud half (L:1494-1500 / R:1373-1376) behind the stored points of kf_full: variant 0 the n points as received (one
@@ -247,6 +255,41 @@ static void kf_push_full(liliom_ctx* c, int kf_id, int m) {
     c->kfs[kf_id].full_off = c->kf_full_used;
     c->kfs[kf_id].n_full = m;
     c->kf_full_used += m;
+}
+
+// liliom_kf_add_resident in parts, run by the solo call and by the batch (liliom_kf_add_resident_batch): kf_res_begin (validation,
+// nothing changes on an error; the source's clouds), their sizes (feat_sizes), kf_res_reserve (both arenas before any write), the
+// VoxelGrid chain of each cloud (kf_scan_dev and kf_full_dev on the solo path), kf_res_finish (the keyframe's records).
+struct KfResJob {
+    liliom_ctx* c = nullptr;                 // the backend
+    const liliom_backend_params* bp = nullptr;
+    FeatCloud f[3];                          // the source's surf, edge and cut (ROT: laserCloud)
+    int m[3] = {0, 0, 0};                    // their sizes
+    int me = 0, ms = 0, mf = 0;              // points stored: edge, surf, full
+};
+
+static int kf_res_begin(liliom_ctx* c, const liliom_backend_params* bp, liliom_ctx* src, KfResJob& j) {
+    if (!src) return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, bp));
+    if (src->nranks > 1) { c->last_error = "the source context has a communicator: the backend keyframe store is single-GPU"; return LILIOM_E_ARG; }
+    if (src->prm.point_stride != c->prm.point_stride || src->device != c->device) return LILIOM_E_ARG;
+    j = KfResJob{};
+    j.c = c; j.bp = bp;
+    return feat_clouds(src, j.f);
+}
+
+static int kf_res_reserve(const KfResJob& j) {
+    liliom_ctx* c = j.c;
+    LILI_TRY(kf_reserve(c, c->kf_arena, c->kf_used, c->kf_used + (long long)j.m[1] + j.m[0]));
+    return kf_reserve(c, c->kf_full, c->kf_full_used, c->kf_full_used + j.m[2]);
+}
+
+static void kf_res_finish(const KfResJob& j, int* kf_id, int* n_edge_ds, int* n_surf_ds, int* n_full_stored) {
+    *kf_id = kf_push(j.c, j.me, j.ms);
+    kf_push_full(j.c, *kf_id, j.mf);
+    if (n_edge_ds) *n_edge_ds = j.me;
+    if (n_surf_ds) *n_surf_ds = j.ms;
+    if (n_full_stored) *n_full_stored = j.mf;
 }
 
 }  // namespace lili
@@ -304,26 +347,16 @@ extern "C" int liliom_kf_add(liliom_ctx* c, const liliom_backend_params* bp, con
 extern "C" int liliom_kf_add_resident(liliom_ctx* c, const liliom_backend_params* bp, liliom_ctx* src, int* kf_id, int* n_edge_ds,
                                       int* n_surf_ds, int* n_full_stored) {
     if (!c || !bp || !src || !kf_id) return LILIOM_E_ARG;
-    LILI_TRY(backend_check(c, bp));
-    if (src->nranks > 1) { c->last_error = "the source context has a communicator: the backend keyframe store is single-GPU"; return LILIOM_E_ARG; }
-    if (src->prm.point_stride != c->prm.point_stride || src->device != c->device) return LILIOM_E_ARG;
-    FeatCloud f[3];                                               // surf, edge, cut (ROT: laserCloud)
-    LILI_TRY(feat_clouds(src, f));
+    KfResJob j;
+    LILI_TRY(kf_res_begin(c, bp, src, j));
     LILI_CUDA(c, cudaSetDevice(c->device));
-    int m[3];
-    LILI_TRY(feat_sizes(src, f, m));                              // they size the arenas and the filters
+    LILI_TRY(feat_sizes(src, j.f, j.m));                          // they size the arenas and the filters
     LILI_TRY(batch_join_in(c, {src}));                            // src's work so far before c's reads of its clouds
-    LILI_TRY(kf_reserve(c, c->kf_arena, c->kf_used, c->kf_used + (long long)m[1] + m[0]));   // both arenas before any write
-    LILI_TRY(kf_reserve(c, c->kf_full, c->kf_full_used, c->kf_full_used + m[2]));
-    int me = 0, ms = 0, mf = 0;
-    LILI_TRY(kf_scan_dev(c, bp, f[1].buf->p, m[1], f[0].buf->p, m[0], &me, &ms));
-    LILI_TRY(kf_full_dev(c, bp, f[2].buf->p, m[2], &mf));
+    LILI_TRY(kf_res_reserve(j));
+    LILI_TRY(kf_scan_dev(c, bp, j.f[1].buf->p, j.m[1], j.f[0].buf->p, j.m[0], &j.me, &j.ms));
+    LILI_TRY(kf_full_dev(c, bp, j.f[2].buf->p, j.m[2], &j.mf));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    *kf_id = kf_push(c, me, ms);
-    kf_push_full(c, *kf_id, mf);
-    if (n_edge_ds) *n_edge_ds = me;
-    if (n_surf_ds) *n_surf_ds = ms;
-    if (n_full_stored) *n_full_stored = mf;
+    kf_res_finish(j, kf_id, n_edge_ds, n_surf_ds, n_full_stored);
     return LILIOM_OK;
 }
 
@@ -461,14 +494,7 @@ static int loop_begin(liliom_ctx* c, const int* src_ids, const double* src_poses
         LILI_CUDA(c, c->bmap_raw.ensure((size_t)n * stride));   // scratch: the local map's layers live in bmap_ds / bmap
         c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
         LILI_CUDA(c, c->vg_out.ensure((size_t)n * stride));
-        LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));       // voxelgrid_dev's buffers at 32-bit keys
-        LILI_CUDA(c, c->vg_params.ensure(sizeof(VgParams)));
-        LILI_CUDA(c, c->vg_keys.ensure((size_t)n * 4));
-        LILI_CUDA(c, c->vg_vals.ensure((size_t)n * 4));
-        LILI_CUDA(c, c->vg_keys2.ensure((size_t)n * 4));
-        LILI_CUDA(c, c->vg_vals2.ensure((size_t)n * 4));
-        LILI_CUDA(c, c->vg_flags.ensure(((size_t)n + 2) * 4));
-        LILI_CUDA(c, c->vg_rank.ensure(((size_t)n + 2) * 4));
+        LILI_TRY(vg_chain_ensure(c, n, 4));                       // voxelgrid_dev's buffers at 32-bit keys
     }
     LILI_CUDA(c, c->loop.xyzw.ensure((size_t)std::max(j.off[0], 1LL) * sizeof(float4)));
     LILI_CUDA(c, c->loop_src.ensure((size_t)std::max(j.off[1], 1LL) * sizeof(float4)));
@@ -529,16 +555,24 @@ LILI_STAGE(LoopStCellKeys, LoopEntry, 256, stage_blocks(e.m, 256), cell_keys_at(
 LILI_STAGE(LoopStGatherSorted, LoopEntry, 256, stage_blocks(e.m, 256), gather_sorted_at(e.xyzw, e.vals2, e.m, e.sorted, i))
 LILI_STAGE(LoopStRunEnds, LoopEntry, 256, stage_blocks(e.m, 256), cell_run_ends_at(e.keys2, e.m, e.cell_start, i))
 
+// The entry of voxelgrid_dev's chain at 32-bit keys on c's buffers: n points at `in` -> `out`, the count at `count` (the stages
+// LoopStBoxInit .. LoopStCentroid32; the keyframe store's batch runs them too)
+static LoopEntry vg_chain_entry(liliom_ctx* c, const void* in, int n, float leaf, void* out, int* count) {
+    LoopEntry e{};
+    e.raw = (const unsigned char*)in; e.n = n; e.stride = c->prm.point_stride; e.leaf = leaf;
+    e.mm = c->vg_minmax.as<int>(); e.mm_blocks = box_blocks(e.n, c->sm_count); e.pp = c->vg_params.as<VgParams>();
+    e.keys = c->vg_keys.as<uint32_t>(); e.vals = c->vg_vals.as<int>(); e.keys2 = c->vg_keys2.as<uint32_t>(); e.vals2 = c->vg_vals2.as<int>();
+    e.flags = c->vg_flags.as<int>(); e.rank = c->vg_rank.as<int>(); e.ds = (unsigned char*)out; e.count = count;
+    return e;
+}
+
 // Session j's entry for cloud k (0 target, 1 source), as loop_cloud's launches take their arguments
 static LoopEntry loop_cloud_entry(const LoopJob& j, int k) {
     liliom_ctx* c = j.c;
-    LoopEntry e{};
+    LoopEntry e = vg_chain_entry(c, c->bmap_raw.p, (int)j.off[k], j.leaf, c->vg_out.p, c->vg_count.as<int>() + k);
     const dim3 gg = loop_gather_grid(j, k);
     e.arena = (const unsigned char*)c->kf_arena.p; e.tab = loop_rows(j, k); e.rows = j.rows[k]; e.gx = (int)gg.x; e.gy = (int)gg.y;
-    e.raw = e.raw_out = (unsigned char*)c->bmap_raw.p; e.n = (int)j.off[k]; e.stride = c->prm.point_stride; e.leaf = j.leaf;
-    e.mm = c->vg_minmax.as<int>(); e.mm_blocks = box_blocks(e.n, c->sm_count); e.pp = c->vg_params.as<VgParams>();
-    e.keys = c->vg_keys.as<uint32_t>(); e.vals = c->vg_vals.as<int>(); e.keys2 = c->vg_keys2.as<uint32_t>(); e.vals2 = c->vg_vals2.as<int>();
-    e.flags = c->vg_flags.as<int>(); e.rank = c->vg_rank.as<int>(); e.ds = (unsigned char*)c->vg_out.p; e.count = c->vg_count.as<int>() + k;
+    e.raw_out = (unsigned char*)c->bmap_raw.p;
     e.xyzw = loop_dst(c, k);
     return e;
 }
@@ -558,6 +592,39 @@ namespace {
 template <class St, class Make>
 int loop_stage(liliom_ctx* c0, std::vector<LoopJob>& J, const std::vector<int>& which, Make make) {
     return stage_batch<St>(c0, which, [&](LoopEntry& e, int i) { e = make(J[i]); return J[i].c; });
+}
+
+// voxelgrid_dev's chain at 32-bit keys (box, parameters, keys, sort, heads, scan, centroids) of the sessions sel() on c0's stream:
+// session i's cloud is entry(i) (vg_chain_entry) on ctx(i)'s buffers.  One k_stage_batch launch per stage for up to kBatchMax
+// sessions; the library sort and scan per session, in order.  fail(i, rc): session i's sort or scan was not queued (sel() leaves it
+// out from then on).
+template <class Sel, class Make, class Ctx, class Fail>
+int vg_chain_batch(liliom_ctx* c0, Sel sel, Make entry, Ctx ctx, Fail fail) {
+    auto stage = [&](auto st, const std::vector<int>& which) -> int {
+        return stage_batch<decltype(st)>(c0, which, [&](LoopEntry& e, int i) { e = entry(i); return ctx(i); });
+    };
+    auto of_stride = [&](bool s48) {
+        std::vector<int> v;
+        for (int i : sel()) if ((ctx(i)->prm.point_stride == 48) == s48) v.push_back(i);
+        return v;
+    };
+    LILI_TRY(stage(LoopStBoxInit{}, sel()));
+    LILI_TRY(stage(LoopStBox{}, sel()));
+    LILI_TRY(stage(LoopStParams{}, sel()));
+    LILI_TRY(stage(LoopStKeys{}, sel()));
+    for (int i : sel()) {
+        liliom_ctx* c = ctx(i);
+        if (const int rc = sort_pairs_u32(c, c->vg_keys.as<uint32_t>(), c->vg_keys2.as<uint32_t>(), c->vg_vals.as<int>(), c->vg_vals2.as<int>(),
+                                          entry(i).n, 32); rc != LILIOM_OK)
+            fail(i, rc);
+    }
+    LILI_TRY(stage(LoopStHeads{}, sel()));
+    for (int i : sel()) {
+        liliom_ctx* c = ctx(i);
+        if (const int rc = exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), entry(i).n); rc != LILIOM_OK) fail(i, rc);
+    }
+    LILI_TRY(stage(LoopStCentroid48{}, of_stride(true)));
+    return stage(LoopStCentroid32{}, of_stride(false));
 }
 
 // The shared phases of loop_align_batch, every session's stream pointing at c0's.  Each phase: the solo call's host part per
@@ -581,22 +648,7 @@ int loop_batch_run(liliom_ctx* c0, std::vector<LoopJob>& J, std::vector<char>& l
         auto has = [k](const LoopJob& j) { return j.off[k] > 0; };
         auto cloud = [k](const LoopJob& j) { return loop_cloud_entry(j, k); };
         LILI_TRY(loop_stage<LoopStGather>(c0, J, sel(has), cloud));
-        LILI_TRY(loop_stage<LoopStBoxInit>(c0, J, sel(has), cloud));
-        LILI_TRY(loop_stage<LoopStBox>(c0, J, sel(has), cloud));
-        LILI_TRY(loop_stage<LoopStParams>(c0, J, sel(has), cloud));
-        LILI_TRY(loop_stage<LoopStKeys>(c0, J, sel(has), cloud));
-        for (int i : sel(has)) {
-            liliom_ctx* c = J[i].c;
-            if (const int rc = sort_pairs_u32(c, c->vg_keys.as<uint32_t>(), c->vg_keys2.as<uint32_t>(), c->vg_vals.as<int>(), c->vg_vals2.as<int>(),
-                                              (int)J[i].off[k], 32); rc != LILIOM_OK)
-                fail(i, rc);
-        }
-        LILI_TRY(loop_stage<LoopStHeads>(c0, J, sel(has), cloud));
-        for (int i : sel(has))
-            if (const int rc = exclusive_scan_i32(J[i].c, J[i].c->vg_flags.as<int>(), J[i].c->vg_rank.as<int>(), (int)J[i].off[k]); rc != LILIOM_OK)
-                fail(i, rc);
-        LILI_TRY(loop_stage<LoopStCentroid48>(c0, J, sel([k](const LoopJob& j) { return j.off[k] > 0 && j.c->prm.point_stride == 48; }), cloud));
-        LILI_TRY(loop_stage<LoopStCentroid32>(c0, J, sel([k](const LoopJob& j) { return j.off[k] > 0 && j.c->prm.point_stride != 48; }), cloud));
+        LILI_TRY(vg_chain_batch(c0, [&] { return sel(has); }, [&](int i) { return cloud(J[i]); }, [&](int i) { return J[i].c; }, fail));
         LILI_TRY(loop_stage<LoopStRepack>(c0, J, sel(has), cloud));
         for (int i : sel(has)) copy_back(i, k * sizeof(VgParams), J[i].c->vg_params.p, sizeof(VgParams));
     }
@@ -695,6 +747,149 @@ int loop_align_batch(liliom_ctx* const* cs, int B, const int* const* src_ids, co
     return rc;
 }
 
+// ---- the keyframe hand-off of several sessions (liliom_kf_add_resident_batch): the solo call's parts per session, the VoxelGrid
+// chains of every session in shared launches (vg_chain_batch), three waits for all of them.
+namespace {
+
+// Cloud k of session j's source (0 surf, 1 edge, 2 cut / laserCloud) is filtered: the scan half's two, variant 1's full cloud
+bool kf_filtered(const KfResJob& j, int k) { return k != 2 || j.bp->variant == 1; }
+
+// ... and its chain's entry, writing where kf_scan_dev / kf_full_dev write: the edge cloud behind the stored points of kf_arena (its
+// count in vg_count[0]), the surf cloud into vg_out (vg_count[1]), the full cloud behind those of kf_full (vg_count[0])
+LoopEntry kf_cloud_entry(const KfResJob& j, int k) {
+    liliom_ctx* c = j.c;
+    const size_t stride = (size_t)c->prm.point_stride;
+    int* cnt = c->vg_count.as<int>();
+    if (k == 1) return vg_chain_entry(c, j.f[1].buf->p, j.m[1], j.bp->edge_leaf, (unsigned char*)c->kf_arena.p + (size_t)c->kf_used * stride, cnt);
+    if (k == 0) return vg_chain_entry(c, j.f[0].buf->p, j.m[0], j.bp->surf_leaf, c->vg_out.p, cnt + 1);
+    return vg_chain_entry(c, j.f[2].buf->p, j.m[2], j.bp->surf_leaf, (unsigned char*)c->kf_full.p + (size_t)c->kf_full_used * stride, cnt);
+}
+
+// The buffers the solo call's filters size, in its order (kf_scan_dev, then voxelgrid_dev per cloud, kf_full_dev)
+int kf_res_buffers(const KfResJob& j) {
+    liliom_ctx* c = j.c;
+    c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
+    LILI_CUDA(c, c->vg_out.ensure((size_t)(j.m[0] > 0 ? j.m[0] : 1) * c->prm.point_stride));
+    LILI_CUDA(c, c->vg_count.ensure(16));
+    for (int k : {1, 0, 2})
+        if (kf_filtered(j, k) && j.m[k] > 0) LILI_TRY(vg_chain_ensure(c, j.m[k], 4));
+    return LILIOM_OK;
+}
+
+// The shared phases, every backend's stream pointing at c0's.  Session i's read-back words land in its backend's pinned scratch:
+// the sizes, then per filtered cloud k its VgParams and count at k * kSlot.  wide[i]: session i's index wrapped in one of its
+// clouds (vg_wide_keys); it leaves the shared path after the counts.
+int kf_batch_run(liliom_ctx* c0, std::vector<KfResJob>& J, std::vector<char>& live, std::vector<char>& wide, int* status) {
+    constexpr size_t kSlot = sizeof(VgParams) + sizeof(int);
+    static_assert(3 * kSlot <= sizeof(PinBlock::scratch), "the three clouds' words fit the pinned scratch");
+    const int B = (int)J.size();
+    auto fail = [&](int i, int rc) { status[i] = rc; live[i] = 0; };
+    auto sel = [&](auto pred) {
+        std::vector<int> v;
+        for (int i = 0; i < B; ++i) if (live[i] && pred(J[i])) v.push_back(i);
+        return v;
+    };
+    auto any = [](const KfResJob&) { return true; };
+    auto copy_back = [&](int i, size_t at, const void* src, size_t bytes) {
+        if (cudaError_t err = cudaMemcpyAsync(J[i].c->h_pin->scratch + at, src, bytes, cudaMemcpyDeviceToHost, c0->stream); err != cudaSuccess)
+            fail(i, fail_cuda(J[i].c, err, "keyframe batch: read-back"));
+    };
+    // 1. the sizes only on the device (a resident Horizon extraction's): every such source's, one wait; then both arenas
+    auto on_device = [](const KfResJob& j) { return j.f[0].d_n != nullptr; };
+    for (int i : sel(any))
+        for (int k = 0; k < 3; ++k) J[i].m[k] = J[i].f[k].n;
+    if (!sel(on_device).empty()) {
+        for (int i : sel(on_device))
+            for (int k = 0; k < 3; ++k) copy_back(i, k * sizeof(int), J[i].f[k].d_n, sizeof(int));
+        LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+        for (int i : sel(on_device)) memcpy(J[i].m, J[i].c->h_pin->scratch, 3 * sizeof(int));
+    }
+    for (int i : sel(any)) {
+        int rc = kf_res_reserve(J[i]);
+        if (rc == LILIOM_OK) rc = kf_res_buffers(J[i]);
+        if (rc != LILIOM_OK) fail(i, rc);
+    }
+    // 2. the edge chains, the surf chains, the full chains (variant 1; variant 0 copies the cloud) -> counts, VgParams; one wait
+    for (int k : {1, 0, 2}) {
+        for (int i : sel([k](const KfResJob& j) { return k != 2 && j.m[k] == 0; }))      // voxelgrid_dev's count of an empty cloud
+            if (cudaError_t err = cudaMemsetAsync(kf_cloud_entry(J[i], k).count, 0, sizeof(int), c0->stream); err != cudaSuccess)
+                fail(i, fail_cuda(J[i].c, err, "keyframe batch: empty count"));
+        auto has = [k](const KfResJob& j) { return kf_filtered(j, k) && j.m[k] > 0; };
+        LILI_TRY(vg_chain_batch(c0, [&] { return sel(has); }, [&](int i) { return kf_cloud_entry(J[i], k); }, [&](int i) { return J[i].c; }, fail));
+        for (int i : sel(has)) {
+            copy_back(i, k * kSlot, J[i].c->vg_params.p, sizeof(VgParams));
+            copy_back(i, k * kSlot + sizeof(VgParams), kf_cloud_entry(J[i], k).count, sizeof(int));
+        }
+    }
+    for (int i : sel([](const KfResJob& j) { return !kf_filtered(j, 2) && j.m[2] > 0; })) {      // L:1498-1500 as received
+        liliom_ctx* c = J[i].c;
+        const size_t stride = (size_t)c->prm.point_stride;
+        if (cudaError_t err = cudaMemcpyAsync((unsigned char*)c->kf_full.p + (size_t)c->kf_full_used * stride, J[i].f[2].buf->p,
+                                              (size_t)J[i].m[2] * stride, cudaMemcpyDeviceToDevice, c0->stream); err != cudaSuccess)
+            fail(i, fail_cuda(c, err, "keyframe batch: full cloud"));
+    }
+    LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+    for (int i : sel(any)) {
+        KfResJob& j = J[i];
+        int cnt[3] = {0, 0, j.m[2]};
+        for (int k = 0; k < 3; ++k) {
+            if (!kf_filtered(j, k) || j.m[k] == 0) continue;
+            const unsigned char* s = j.c->h_pin->scratch + k * kSlot;
+            VgParams vp;
+            memcpy(&vp, s, sizeof(VgParams));
+            memcpy(&cnt[k], s + sizeof(VgParams), sizeof(int));
+            if (vg_wide_keys(vp)) { wide[i] = 1; live[i] = 0; }       // the solo path redoes the session with wide keys
+        }
+        j.ms = cnt[0]; j.me = cnt[1]; j.mf = cnt[2];
+    }
+    // 3. the surf points behind the edge points; one wait
+    for (int i : sel(any))
+        if (const int rc = kf_surf_behind(J[i].c, J[i].me, J[i].ms); rc != LILIOM_OK) fail(i, rc);
+    LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+    return LILIOM_OK;
+}
+
+}  // namespace
+
+// liliom_kf_add_resident of several sessions.  Shared launches and waits on cs[0]'s stream (every backend's and source's stream
+// joined before, every backend's after, with events); every buffer, library sort and scan and host decision stays the backend's
+// own, made by the solo call's parts from the session's own read-back words.  The sources are only read, and every size is read
+// before any session writes: the result is that of the solo calls in any order.
+int kf_add_resident_batch(liliom_ctx* const* cs, int B, const liliom_backend_params* bps, liliom_ctx* const* srcs, int* kf_id, int* n_edge_ds,
+                          int* n_surf_ds, int* n_full_stored, int* status) {
+    liliom_ctx* c0 = cs[0];
+    std::vector<KfResJob> J(B);
+    std::vector<char> live(B, 0), wide(B, 0);
+    std::vector<std::pair<unsigned long long, unsigned long long>> launches0(B);
+    const std::vector<liliom_ctx*> all(cs, cs + B);
+    std::vector<liliom_ctx*> joined(all);
+    for (int i = 0; i < B; ++i) {
+        launches0[i] = {cs[i]->cnt.launches, cs[i]->cnt.lib_launches};
+        status[i] = kf_res_begin(cs[i], bps + i, srcs[i], J[i]);
+        live[i] = status[i] == LILIOM_OK;
+        if (live[i] && std::find(joined.begin(), joined.end(), srcs[i]) == joined.end()) joined.push_back(srcs[i]);
+    }
+    LILI_TRY(batch_join_in(c0, joined));
+    int rc;
+    {
+        const BatchStreams on_c0(all, c0->stream);
+        rc = kf_batch_run(c0, J, live, wide, status);
+        for (int i = 0; rc == LILIOM_OK && i < B; ++i) {
+            auto at = [i](int* p) { return p ? p + i : nullptr; };
+            if (live[i]) {
+                kf_res_finish(J[i], kf_id + i, at(n_edge_ds), at(n_surf_ds), at(n_full_stored));
+            } else if (wide[i]) {
+                // the whole solo call, which takes the wide keys, its counters counted from where the batch found them
+                liliom_ctx* c = cs[i];
+                c->cnt.launches = launches0[i].first; c->cnt.lib_launches = launches0[i].second;
+                status[i] = liliom_kf_add_resident(c, bps + i, srcs[i], kf_id + i, at(n_edge_ds), at(n_surf_ds), at(n_full_stored));
+            }
+        }
+    }
+    LILI_TRY(batch_join_out(c0, all));
+    return rc;
+}
+
 }  // namespace lili
 
 extern "C" int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids,
@@ -718,6 +913,13 @@ extern "C" int liliom_loop_align_batch(liliom_ctx* const* ctxs, int B, const int
         return LILIOM_E_ARG;
     LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
     return loop_align_batch(ctxs, B, src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, prm, res, status);
+}
+
+extern "C" int liliom_kf_add_resident_batch(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps, liliom_ctx* const* srcs,
+                                            int* kf_id, int* n_edge_ds, int* n_surf_ds, int* n_full_stored, int* status) {
+    if (!batch_ctxs_ok(ctxs, B) || !bps || !srcs || !kf_id || !status) return LILIOM_E_ARG;
+    LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
+    return kf_add_resident_batch(ctxs, B, bps, srcs, kf_id, n_edge_ds, n_surf_ds, n_full_stored, status);
 }
 
 extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp, int kf_id, const void* full, int n, int* n_stored) {

@@ -345,6 +345,19 @@ int vg_minmax_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, in
     return LILIOM_OK;
 }
 
+// the buffers of voxelgrid_dev's chain over n points at kb-byte keys
+int vg_chain_ensure(liliom_ctx* c, long long n, size_t kb) {
+    LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
+    LILI_CUDA(c, c->vg_params.ensure(sizeof(VgParams)));
+    LILI_CUDA(c, c->vg_keys.ensure((size_t)n * kb));
+    LILI_CUDA(c, c->vg_vals.ensure((size_t)n * 4));
+    LILI_CUDA(c, c->vg_keys2.ensure((size_t)n * kb));
+    LILI_CUDA(c, c->vg_vals2.ensure((size_t)n * 4));
+    LILI_CUDA(c, c->vg_flags.ensure(((size_t)n + 2) * 4));
+    LILI_CUDA(c, c->vg_rank.ensure(((size_t)n + 2) * 4));
+    return LILIOM_OK;
+}
+
 // key_bits < 32: the caller speculates that the voxel index fits that width (one onesweep pass less per 8 bits) and must check
 // `ncells <= 2^key_bits - 1` afterwards (vg_params stays on the device).  key_bits = 32 assumes the index does not wrap: the
 // caller checks vg_wide_keys on the VgParams it reads back and redoes the call with key_bits = kVgWideKeyBits (64-bit keys) on
@@ -360,16 +373,8 @@ int voxelgrid_dev(liliom_ctx* c, const void* d_in, int n_max, const int* d_n, in
     }
     const unsigned char* in = (const unsigned char*)d_in;
     const int n = n_max;
-    LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
-    LILI_CUDA(c, c->vg_params.ensure(sizeof(VgParams)));
     const bool wide = key_bits > 32;
-    const size_t kb = wide ? 8 : 4;
-    LILI_CUDA(c, c->vg_keys.ensure((size_t)n * kb));
-    LILI_CUDA(c, c->vg_vals.ensure((size_t)n * 4));
-    LILI_CUDA(c, c->vg_keys2.ensure((size_t)n * kb));
-    LILI_CUDA(c, c->vg_vals2.ensure((size_t)n * 4));
-    LILI_CUDA(c, c->vg_flags.ensure(((size_t)n + 2) * 4));
-    LILI_CUDA(c, c->vg_rank.ensure(((size_t)n + 2) * 4));
+    LILI_TRY(vg_chain_ensure(c, n, wide ? 8 : 4));
     int* mm = c->vg_minmax.as<int>();
     VgParams* pp = c->vg_params.as<VgParams>();
     if (host_mm) {

@@ -15,7 +15,17 @@ the 41 history keyframes, at the reference's ICP settings (leaf 0.4, 30 m, 100 i
   (a) B solo liliom_loop_align calls;
   (b) one liliom_loop_align_batch.
 Reads device state only.
-usage: backend_batch_bench.py [--loop] [--sessions 1 2 4 8 16 32] [--steps 20] [--warmup 3] [--rounds 5]"""
+--handoff measures a fleet keyframe hand-off tick instead, the worst tick, when every session's keyframe falls due together: each
+session extracts its own seeded sweep (Horizon: synth.make_horizon_sweep with backend variant 0; HDL-64E: synth.make_hdl64_sweep
+with variant 1) before every tick, untimed, and hands its three resident clouds to its backend with publishCloudLast's
+translation:
+  (a) B x (liliom_undistort_resident + liliom_kf_add_resident);
+  (b) one liliom_undistort_resident_batch + one liliom_kf_add_resident_batch.
+Each leg stores into backends of its own, whose arenas are grown before the timed window (the whole run's keyframes stored once,
+then liliom_kf_clear), so that no timed call reallocates.  Fleets: all Horizon, all HDL-64E, and mixed (alternating).  The legs'
+ids and counts of every tick and every session's last stored clouds are checked byte-identical in the same run.  The waits per
+tick (waits_by_design) are derived from the calls' structure, not counted in the run.
+usage: backend_batch_bench.py [--loop | --handoff] [--sessions 1 2 4 8 16 32] [--steps 20] [--warmup 3] [--rounds 5]"""
 import argparse
 import ctypes as C
 import json
@@ -123,6 +133,9 @@ class Fleet:
                 a.fill(0)
         return out
 
+    def prepare(self):
+        pass
+
 
 LC_HIST = 41       # his_key_frames_ds at lc_map_width = 20
 LC_LEAF = 0.4
@@ -193,6 +206,105 @@ class LoopFleet:
             C.memset(C.addressof(s.res[leg]), 0, C.sizeof(s.res[leg]))
         return out
 
+    def prepare(self):
+        pass
+
+
+HO_TRANS = (0.31, -0.12, 0.05)           # publishCloudLast's relative translation; the reference passes the identity rotation
+HO_FLEETS = {"horizon": lambda i: 0, "hdl64": lambda i: 1, "mixed": lambda i: i % 2}
+
+
+def handoff_sweep(args):
+    from liliom_b200 import synth
+    variant, seed = args
+    T = synth.default_true_pose()
+    if variant == 0:
+        return synth.make_horizon_sweep(T, seed=seed)
+    return synth.make_hdl64_sweep(T, seed=seed)
+
+
+class HandoffSession:
+    def __init__(self, variant, sweep):
+        import liliom_b200 as L
+        self.variant, (self.pts, q) = variant, sweep
+        self.q = np.asarray(q, np.float64)
+        self.bp = L.backend_default_params(variant)
+        self.odo = L.Context(variant=variant)
+        self.bk = {leg: L.Context(variant=variant) for leg in "ab"}
+        self.odo.upload_scan(self.pts)           # the resident sweep; every tick re-extracts it
+        self.res = {leg: np.zeros(5, np.int32) for leg in "ab"}     # kf_id, 3 counts, status of the leg's last tick
+
+    def grow(self, keyframes):
+        """both legs' arenas grown to `keyframes` hand-offs, then emptied: no timed call reallocates"""
+        for bk in self.bk.values():
+            for _ in range(keyframes):
+                self.odo.extract_resident(self.q)
+                self.odo.undistort_resident(HO_TRANS)
+                bk.kf_add_resident(self.bp, self.odo)
+            bk.kf_clear()
+
+    def close(self):
+        for c in (self.odo, *self.bk.values()):
+            c.close()
+
+
+class HandoffFleet:
+    """B sessions and the C arguments of both legs, built once."""
+
+    def __init__(self, S):
+        import liliom_b200 as L
+        self.S, self.lib, B = S, L._binding.lib(), len(S)
+        for s in S:
+            for bk in s.bk.values():
+                bk.kf_clear()
+        self.odos = (C.c_void_p * B)(*[s.odo._h for s in S])
+        self.bks = {leg: (C.c_void_p * B)(*[s.bk[leg]._h for s in S]) for leg in "ab"}
+        self.trans = np.tile(np.array(HO_TRANS), B)
+        self.quat = np.tile(np.array([1.0, 0, 0, 0]), B)
+        self.bps = (L.BackendParams * B)(*[s.bp for s in S])
+        self.out = np.zeros((5, B), np.int32)     # kf_id, n_edge_ds, n_surf_ds, n_full_stored, status
+        self.t, self.q = ptr(np.array(HO_TRANS), C.c_double), ptr(np.array([1.0, 0, 0, 0]), C.c_double)
+        self.solo_out = [[ptr(s.res["a"][k:], C.c_int) for k in range(4)] for s in S]
+
+    def prepare(self):
+        for s in self.S:
+            s.odo.extract_resident(s.q)
+
+    def leg_a(self):
+        for s, (kid, ne, ns, nf) in zip(self.S, self.solo_out):
+            rc = self.lib.liliom_undistort_resident(s.odo._h, self.t, self.q)
+            rc = rc or self.lib.liliom_kf_add_resident(s.bk["a"]._h, C.byref(s.bp), s.odo._h, kid, ne, ns, nf)
+            assert rc == 0, rc
+
+    def leg_b(self):
+        B = len(self.S)
+        st = self.out[4]
+        rc = self.lib.liliom_undistort_resident_batch(self.odos, B, ptr(self.trans, C.c_double), ptr(self.quat, C.c_double), ptr(st, C.c_int))
+        assert rc == 0 and not st.any(), (rc, st)
+        o = [np.ascontiguousarray(self.out[k]) for k in range(4)]
+        rc = self.lib.liliom_kf_add_resident_batch(self.bks["b"], B, self.bps, self.odos, *[ptr(x, C.c_int) for x in o], ptr(st, C.c_int))
+        assert rc == 0 and not st.any(), (rc, st)
+        for i, s in enumerate(self.S):
+            s.res["b"][:4] = [x[i] for x in o]
+
+    def outputs(self, leg):
+        out = b"".join(s.res[leg].tobytes() for s in self.S)
+        for s in self.S:
+            s.res[leg][:] = 0
+        return out
+
+    def stores(self, leg):
+        """every session's last stored keyframe: its surf and full clouds as stored, and the store's size"""
+        import liliom_b200 as L
+        out = b""
+        for s in self.S:
+            bk = s.bk[leg]
+            n = bk.kf_count()
+            out += np.int32(n).tobytes()
+            for kind in (L.KF_SURF, L.KF_FULL):
+                out += bk.global_map(kind, [n - 1], [[1.0, 0, 0, 0, 0, 0, 0]], 1e-4).tobytes()
+        return out
+
 
 def timed(f, leg, steps):
     """median ms of `steps` window steps of leg "a" or "b", and the outputs of the last (every call returns with its sessions'
@@ -202,6 +314,7 @@ def timed(f, leg, steps):
     lat = []
     for _ in range(steps):
         f.outputs(leg)
+        f.prepare()
         torch.cuda.synchronize()
         t = time.perf_counter()
         run()
@@ -216,9 +329,12 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--loop", action="store_true", help="the fleet loop-closure tick instead of the window step")
+    ap.add_argument("--handoff", action="store_true", help="the fleet keyframe hand-off tick instead of the window step")
     args = ap.parse_args()
     if args.loop:
         return main_loop(args)
+    if args.handoff:
+        return main_handoff(args)
     Bmax = max(args.sessions)
     with ProcessPoolExecutor(max_workers=min(Bmax, os.cpu_count() or 1)) as ex:     # the streams, before CUDA starts here
         seqs = list(ex.map(stream, [100 + s for s in range(Bmax)]))
@@ -279,6 +395,43 @@ def main_loop(args):
         print(json.dumps(row), flush=True)
     for s in sessions:
         s.c.close()
+
+
+def main_handoff(args):
+    Bmax = max(args.sessions)
+    jobs = [(v, 300 + 2 * s + v) for s in range(Bmax) for v in (0, 1)]
+    with ProcessPoolExecutor(max_workers=min(len(jobs), os.cpu_count() or 1)) as ex:
+        sw = dict(zip(jobs, ex.map(handoff_sweep, jobs)))
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("backend_batch_bench.py measures on a CUDA device; none is visible")
+    print(json.dumps(dict(card(), leg="handoff", steps=args.steps, warmup=args.warmup, rounds=args.rounds,
+                          figures="[median of rounds, min round, max round], ms per fleet hand-off tick")), flush=True)
+    ticks = args.warmup + args.rounds * args.steps + 1
+    for fleet, variant_of in HO_FLEETS.items():
+        sessions = [HandoffSession(variant_of(s), sw[variant_of(s), 300 + 2 * s + variant_of(s)]) for s in range(Bmax)]
+        for s in sessions:
+            s.grow(ticks)
+        for B in args.sessions:
+            S = sessions[:B]
+            f = HandoffFleet(S)
+            for leg in "ab":
+                timed(f, leg, args.warmup)
+            ra, rb, same = [], [], True
+            for _ in range(args.rounds):
+                ta, oa = timed(f, "a", args.steps)
+                tb, ob = timed(f, "b", args.steps)
+                ra.append(ta); rb.append(tb)
+                same = same and oa == ob
+            same = same and f.stores("a") == f.stores("b")
+            n_hz = sum(1 for s in S if s.variant == 0)
+            # the waits follow from the calls' structure (include/liliom.h); the run does not count them
+            row = dict(fleet=fleet, sessions=B, a_solo_ms=spread(ra), b_batch_ms=spread(rb),
+                       waits_by_design=[5 * B, 1 + (3 if n_hz else 2)],
+                       speedup=round(float(np.median(ra) / np.median(rb)), 3), identical=bool(same))
+            print(json.dumps(row), flush=True)
+        for s in sessions:
+            s.close()
 
 
 if __name__ == "__main__":
