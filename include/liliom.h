@@ -272,6 +272,24 @@ int liliom_kf_clear(liliom_ctx* c);      /* drops every keyframe, the local map 
  * the previous layers stay.  k = 0 builds empty layers. */
 int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7, int k,
                       int* n_edge_map, int* n_surf_map);
+/* liliom_bmap_build of B independent sessions in one call.  bps, k, status: B entries; kf_ids, poses7: B per-session pointers;
+ * n_edge_map, n_surf_map: B ints each, or NULL.  Session i gets exactly what
+ * liliom_bmap_build(ctxs[i], &bps[i], kf_ids[i], poses7[i], k[i], &n_edge_map[i], &n_surf_map[i]) would give it, bit for bit:
+ * status, liliom_last_error, both counts, both layers (liliom_bmap_download), both cell grids and the surf layer's reflectivity as
+ * every later window search sees them, launches and lib_launches, and everything else on ctxs[i] left alone (the keyframe store,
+ * the resident window, the odometry map and a resident scan for liliom_map_update_resident), so that solo and batched calls mix
+ * freely.  Horizon (48-byte, variant 0) and ROT (32-byte, variant 1) sessions may be mixed, each with its own list and parameters.
+ * Every kernel of the keyframe gather, both layers' VoxelGrid chains (edge, then surf), both layers' box passes and cell grids and
+ * the reflectivity runs once for up to 32 sessions on ctxs[0]'s stream (other sessions' streams are joined with events); the
+ * library sorts and scans stay per session, in order on the same stream.  The call waits three times for all sessions together
+ * (the layers' counts, the cell grids' boxes, the end) where a solo call waits five times when both layers hold points.  A
+ * session whose voxel index wraps (wide keys) finishes on its solo path inside the call.
+ * A session's own error (every error its solo call returns: an unknown id, the previous layers staying downloadable; k < 0; a
+ * NULL list with k > 0; an invalid bp; LILIOM_E_GRID; a non-finite layer point) is its status; the others run.
+ * LILIOM_E_ARG for the whole call, nothing changed: B < 1, a NULL array (ctxs, bps, kf_ids, poses7, k, status), a NULL or
+ * repeated context, contexts on different devices, a context with a communicator. */
+int liliom_bmap_build_batch(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps, const int* const* kf_ids,
+                            const double* const* poses7, const int* k, int* n_edge_map, int* n_surf_map, int* status);
 /* edge_local_map_ds (layer 0) / surf_local_map_ds (layer 1) with all fields (published on every run, :1516-1526).
  * out = NULL: *m = size only. */
 int liliom_bmap_download(liliom_ctx* c, int layer, void* out, int cap, int* m);

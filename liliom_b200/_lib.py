@@ -95,7 +95,7 @@ EXPORTS = [
     "liliom_map_update_resident", "liliom_map_update_batch",
     "liliom_backend_window_correspond_batch", "liliom_backend_window_blocks_batch",
     "liliom_loop_align_batch", "liliom_convert_batch", "liliom_undistort_resident", "liliom_kf_add_resident",
-    "liliom_undistort_resident_batch", "liliom_kf_add_resident_batch",
+    "liliom_undistort_resident_batch", "liliom_kf_add_resident_batch", "liliom_bmap_build_batch",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -244,6 +244,7 @@ def lib() -> C.CDLL:
     L.liliom_kf_count.argtypes = [vp]
     L.liliom_kf_clear.argtypes = [vp]
     L.liliom_bmap_build.argtypes = [vp, bpp, ip, dp, C.c_int, ip, ip]
+    L.liliom_bmap_build_batch.argtypes = [C.POINTER(vp), C.c_int, bpp, C.POINTER(ip), C.POINTER(dp), ip, ip, ip, ip]
     L.liliom_bmap_download.argtypes = [vp, C.c_int, vp, C.c_int, ip]
     L.liliom_backend_window_correspond.argtypes = [vp, bpp, ip, dp, C.c_int, ip, ip]
     L.liliom_backend_window_blocks.argtypes = [vp, dp, C.c_int, dp]
@@ -1083,6 +1084,28 @@ def _ptrs(arrays, ctype):
     """A C array of per-session pointers; a None entry is a NULL pointer."""
     P = C.POINTER(ctype)
     return (P * max(len(arrays), 1))(*[a.ctypes.data_as(P) if a is not None else P() for a in arrays])
+
+
+def bmap_build_batch(ctxs, bps, kf_ids, poses7):
+    """bmap_build of every context in `ctxs` in one call (liliom_bmap_build_batch): session i gets what
+    ctxs[i].bmap_build(bps[i], kf_ids[i], poses7[i]) would give it.  bps: B BackendParams; kf_ids, poses7: B sequences (a None
+    entry passes a NULL pointer with k = 1).  Returns (counts (B, 2) as (n_edge_map, n_surf_map), status (B,)); a session's own
+    error is its status, a whole-call error raises LiliomError."""
+    B = len(ctxs)
+    if len(bps) != B or len(kf_ids) != B or len(poses7) != B:
+        raise ValueError(f"expected {B} per-session parameters, id lists and pose lists")
+    bparr = (BackendParams * max(B, 1))(*bps)
+    ids = [_ids(x) if x is not None else None for x in kf_ids]
+    k = np.array([len(x) if x is not None else 1 for x in ids] + [0], np.int32)
+    poses = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1) if p is not None else None for p in poses7]
+    ne = np.zeros(max(B, 1), np.int32)
+    ns = np.zeros(max(B, 1), np.int32)
+    status = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_bmap_build_batch(_handles(ctxs), B, bparr, _ptrs(ids, C.c_int), _ptrs(poses, C.c_double), _ip(k), _ip(ne),
+                                       _ip(ns), _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    return np.stack([ne, ns], axis=1)[:B], status[:B]
 
 
 def backend_window_correspond_batch(ctxs, bps, kf_ids, poses7_lidar):

@@ -97,10 +97,12 @@ __global__ void k_kf_centroid(const unsigned char* __restrict__ arena, const KfR
     vg_write<STRIDE>(a.s, a.n, out + (size_t)rank[i] * STRIDE);
 }
 
-// reflectivity (curvature = 0.1 * reflectivity, L/src/FormatConvert.cpp:21) of 48-byte points
-__global__ void k_kf_refl(const unsigned char* __restrict__ pts, int n, float* __restrict__ out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+// reflectivity (curvature = 0.1 * reflectivity, L/src/FormatConvert.cpp:21) of 48-byte points; `i` as in the other bodies
+__device__ __forceinline__ void kf_refl_at(const unsigned char* __restrict__ pts, int n, float* __restrict__ out, const int i) {
     if (i < n) out[i] = reinterpret_cast<const float*>(pts + (size_t)i * 48)[9];
+}
+__global__ void k_kf_refl(const unsigned char* __restrict__ pts, int n, float* __restrict__ out) {
+    kf_refl_at(pts, n, out, blockIdx.x * blockDim.x + threadIdx.x);
 }
 
 // Room for `pts` points in `arena`, of which the first `used` are stored.  Grows geometrically and COPIES the stored points
@@ -292,6 +294,71 @@ static void kf_res_finish(const KfResJob& j, int* kf_id, int* n_edge_ds, int* n_
     if (n_full_stored) *n_full_stored = j.mf;
 }
 
+// liliom_bmap_build in parts, run by the solo call and by the batch (liliom_bmap_build_batch): bmap_begin (validation, nothing
+// changes on an error; the keyframe table, uploaded, and the buffers of both layers), the gather of the table into bmap_raw, per
+// layer voxelgrid_dev's chain into bmap_ds[l] and bmap[l].xyzw, each layer's cell grid, the surf layer's reflectivity (48-byte
+// points), bmap_finish (the counts).
+struct BmapJob {
+    liliom_ctx* c = nullptr;
+    const liliom_backend_params* bp = nullptr;
+    int rows = 0;                        // keyframe table rows: edge rows (destinations from 0) and surf rows (from E), list order
+    long long largest = 0;               // the largest keyframe cloud (the gather's grid)
+    long long n[2] = {0, 0};             // points of each layer's concatenation: E (edge), S (surf, behind the edge points)
+    int m[2] = {0, 0};                   // the layers' points (VoxelGrid output counts)
+    GridJob g[2];                        // the layers' cell grids (the batch's grid_begin .. grid_finish)
+    bool grid[2] = {false, false};       // the batch: layer l's cell grid is begun and its launches are still to run
+    unsigned long long launches_surf_box = 0;      // the batch: launches before the surf layer's box pass
+};
+
+static float bmap_leaf(const BmapJob& j, int l) { return l == 0 ? j.bp->edge_leaf : j.bp->surf_leaf; }
+// :1543 sqdist[4] < 1.0 (edge), :1615 sqdist[4] < kd_max_radius (surf)
+static float bmap_cell(const BmapJob& j, int l) { return l == 0 ? gate_cell(1.0) : gate_cell(j.bp->kd_max_radius); }
+static const unsigned char* bmap_in(const BmapJob& j, int l) {
+    return (const unsigned char*)j.c->bmap_raw.p + (l == 0 ? 0 : (size_t)j.n[0] * j.c->prm.point_stride);
+}
+static dim3 bmap_gather_grid(const BmapJob& j) { return kf_row_grid(j.rows, j.largest, j.c->sm_count * 4); }
+
+static int bmap_begin(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7, int k, BmapJob& j) {
+    if (k < 0 || (k > 0 && (!kf_ids || !poses7))) return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, bp));
+    if (!kf_ids_ok(c, kf_ids, k)) return LILIOM_E_ARG;           // before anything changes: the previous layers stay
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    const int stride = c->prm.point_stride;
+    c->bmap_built = false;
+    j = BmapJob{};
+    j.c = c; j.bp = bp;
+    long long E = 0, S = 0;
+    for (int i = 0; i < k; ++i) { const KfEntry& f = c->kfs[kf_ids[i]]; E += f.n_edge; S += f.n_surf; j.largest = std::max(j.largest, (long long)std::max(f.n_edge, f.n_surf)); }
+    std::vector<KfRow> tab;
+    tab.reserve(2 * (size_t)k);
+    long long de = 0, ds = E;
+    for (int i = 0; i < k; ++i) {                                 // :1479-1483 edge and surf layers, list order
+        const KfEntry& f = c->kfs[kf_ids[i]];
+        if (f.n_edge) tab.push_back(kf_row(f.edge_off, de, f.n_edge, poses7 + 7 * (size_t)i));
+        if (f.n_surf) tab.push_back(kf_row(f.surf_off, ds, f.n_surf, poses7 + 7 * (size_t)i));
+        de += f.n_edge; ds += f.n_surf;
+    }
+    j.rows = (int)tab.size();
+    j.n[0] = E; j.n[1] = S;
+    LILI_CUDA(c, c->bmap_raw.ensure((size_t)std::max(E + S, 1LL) * stride));
+    if (j.rows > 0) LILI_TRY(kf_upload_table(c, tab));
+    LILI_CUDA(c, c->vg_count.ensure(16));
+    for (int l = 0; l < 2; ++l) {                                 // the centroid kernel also writes the float4 points
+        LILI_CUDA(c, c->bmap_ds[l].ensure((size_t)std::max(j.n[l], 1LL) * stride));
+        LILI_CUDA(c, c->bmap[l].xyzw.ensure((size_t)std::max(j.n[l], 1LL) * sizeof(float4)));
+        if (j.n[l] > 0) LILI_TRY(vg_chain_ensure(c, j.n[l], 4));   // voxelgrid_dev's buffers at 32-bit keys
+    }
+    return LILIOM_OK;
+}
+
+static void bmap_finish(const BmapJob& j, int* n_edge_map, int* n_surf_map) {
+    liliom_ctx* c = j.c;
+    c->bmap_n[0] = j.m[0]; c->bmap_n[1] = j.m[1];
+    c->bmap_built = true;
+    if (n_edge_map) *n_edge_map = j.m[0];
+    if (n_surf_map) *n_surf_map = j.m[1];
+}
+
 }  // namespace lili
 
 using namespace lili;
@@ -375,50 +442,28 @@ extern "C" int liliom_kf_clear(liliom_ctx* c) {
 
 extern "C" int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7, int k,
                                  int* n_edge_map, int* n_surf_map) {
-    if (!c || !bp || k < 0 || (k > 0 && (!kf_ids || !poses7))) return LILIOM_E_ARG;
-    LILI_TRY(backend_check(c, bp));
-    if (!kf_ids_ok(c, kf_ids, k)) return LILIOM_E_ARG;           // before anything changes: the previous layers stay
-    LILI_CUDA(c, cudaSetDevice(c->device));
+    if (!c || !bp) return LILIOM_E_ARG;
+    BmapJob j;
+    LILI_TRY(bmap_begin(c, bp, kf_ids, poses7, k, j));
     const int stride = c->prm.point_stride;
-    c->bmap_built = false;
-    long long E = 0, S = 0, largest = 0;
-    for (int i = 0; i < k; ++i) { const KfEntry& f = c->kfs[kf_ids[i]]; E += f.n_edge; S += f.n_surf; largest = std::max(largest, (long long)std::max(f.n_edge, f.n_surf)); }
-    std::vector<KfRow> tab;
-    tab.reserve(2 * (size_t)k);
-    long long de = 0, ds = E;
-    for (int i = 0; i < k; ++i) {                                 // :1479-1483 edge and surf layers, list order
-        const KfEntry& f = c->kfs[kf_ids[i]];
-        if (f.n_edge) tab.push_back(kf_row(f.edge_off, de, f.n_edge, poses7 + 7 * (size_t)i));
-        if (f.n_surf) tab.push_back(kf_row(f.surf_off, ds, f.n_surf, poses7 + 7 * (size_t)i));
-        de += f.n_edge; ds += f.n_surf;
+    if (j.rows > 0) {
+        k_kf_gather<<<bmap_gather_grid(j), 256, 0, c->stream>>>((const unsigned char*)c->kf_arena.p, c->kf_tab.as<KfRow>(), j.rows, stride,
+                                                                (unsigned char*)c->bmap_raw.p);
+        LILI_TRY(launch_check(c, "k_kf_gather"));
     }
-    LILI_CUDA(c, c->bmap_raw.ensure((size_t)std::max(E + S, 1LL) * stride));
-    LILI_TRY(kf_gather(c, c->kf_arena.p, tab, largest, c->bmap_raw.p));
-    const long long nl[2] = {E, S};
-    const float leaf[2] = {bp->edge_leaf, bp->surf_leaf};
-    const unsigned char* src[2] = {(const unsigned char*)c->bmap_raw.p, (const unsigned char*)c->bmap_raw.p + (size_t)E * stride};
-    LILI_CUDA(c, c->vg_count.ensure(16));
-    int* cnt = c->vg_count.as<int>();
-    int m[2];
-    for (int l = 0; l < 2; ++l) {                                 // :1486-1492; the centroid kernel also writes the float4 points
-        LILI_CUDA(c, c->bmap_ds[l].ensure((size_t)std::max(nl[l], 1LL) * stride));
-        LILI_CUDA(c, c->bmap[l].xyzw.ensure((size_t)std::max(nl[l], 1LL) * sizeof(float4)));
-        LILI_TRY(voxelgrid_dev_sync(c, src[l], (int)nl[l], stride, leaf[l], c->bmap_ds[l].p, cnt + l, c->bmap[l].xyzw.as<float4>(), m + l));
-    }
-    LILI_TRY(grid_build(c, c->bmap[0], gate_cell(1.0), m[0]));                 // :1543 sqdist[4] < 1.0
-    LILI_TRY(grid_build(c, c->bmap[1], gate_cell(bp->kd_max_radius), m[1]));   // :1615 sqdist[4] < kd_max_radius
+    for (int l = 0; l < 2; ++l)                                   // :1486-1492
+        LILI_TRY(voxelgrid_dev_sync(c, bmap_in(j, l), (int)j.n[l], stride, bmap_leaf(j, l), c->bmap_ds[l].p, c->vg_count.as<int>() + l,
+                                    c->bmap[l].xyzw.as<float4>(), &j.m[l]));
+    for (int l = 0; l < 2; ++l) LILI_TRY(grid_build(c, c->bmap[l], bmap_cell(j, l), j.m[l]));
     if (stride == 48) {                                                         // reflectivity of the surf layer (:1617-1638)
-        LILI_CUDA(c, c->bmap[1].refl.ensure((size_t)std::max(m[1], 1) * sizeof(float)));
-        if (m[1] > 0) {
-            k_kf_refl<<<cdiv(m[1], 256), 256, 0, c->stream>>>((const unsigned char*)c->bmap_ds[1].p, m[1], c->bmap[1].refl.as<float>());
+        LILI_CUDA(c, c->bmap[1].refl.ensure((size_t)std::max(j.m[1], 1) * sizeof(float)));
+        if (j.m[1] > 0) {
+            k_kf_refl<<<cdiv(j.m[1], 256), 256, 0, c->stream>>>((const unsigned char*)c->bmap_ds[1].p, j.m[1], c->bmap[1].refl.as<float>());
             LILI_TRY(launch_check(c, "k_kf_refl"));
         }
     }
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
-    c->bmap_n[0] = m[0]; c->bmap_n[1] = m[1];
-    c->bmap_built = true;
-    if (n_edge_map) *n_edge_map = m[0];
-    if (n_surf_map) *n_surf_map = m[1];
+    bmap_finish(j, n_edge_map, n_surf_map);
     return LILIOM_OK;
 }
 
@@ -529,6 +574,8 @@ static int loop_icp_begin(LoopJob& j) {
 // Everything one session's stages read or write, on its own buffers.
 struct LoopEntry {
     // a cloud: the gather of its table rows into bmap_raw, the VoxelGrid chain of its n points into vg_out, the repack into xyzw
+    // (the local map's chain has no repack: its centroid stage writes the float4 points into xyzw, as voxelgrid_dev's d_feats;
+    // every other chain runs with xyzw null)
     const unsigned char* arena; const KfRow* tab; int rows, gx, gy;
     const unsigned char* raw; unsigned char* raw_out; int n, stride; float leaf; int* mm; int mm_blocks; VgParams* pp;
     uint32_t* keys; int* vals; const uint32_t* keys2; const int* vals2; int* flags; int* rank; unsigned char* ds; int* count;
@@ -548,6 +595,11 @@ LILI_STAGE(LoopStCentroid48, LoopEntry, 128, stage_blocks(e.n, 128),
            (vg_centroid_at<48, uint32_t>)(e.raw, e.keys2, e.vals2, e.flags, e.rank, e.n, nullptr, e.pp, e.ds, e.count, nullptr, i))
 LILI_STAGE(LoopStCentroid32, LoopEntry, 128, stage_blocks(e.n, 128),
            (vg_centroid_at<32, uint32_t>)(e.raw, e.keys2, e.vals2, e.flags, e.rank, e.n, nullptr, e.pp, e.ds, e.count, nullptr, i))
+// ... and those that also write the float4 points into xyzw (the local map's chain; the others keep the stages without the store)
+LILI_STAGE(LoopStCentroidXyzw48, LoopEntry, 128, stage_blocks(e.n, 128),
+           (vg_centroid_at<48, uint32_t>)(e.raw, e.keys2, e.vals2, e.flags, e.rank, e.n, nullptr, e.pp, e.ds, e.count, e.xyzw, i))
+LILI_STAGE(LoopStCentroidXyzw32, LoopEntry, 128, stage_blocks(e.n, 128),
+           (vg_centroid_at<32, uint32_t>)(e.raw, e.keys2, e.vals2, e.flags, e.rank, e.n, nullptr, e.pp, e.ds, e.count, e.xyzw, i))
 LILI_STAGE(LoopStRepack, LoopEntry, 256, stage_blocks(e.n, 256), repack_f4_at(e.ds, e.n, e.count, e.stride, e.xyzw, i))
 LILI_STAGE(LoopStGridBox, LoopEntry, 256, e.mm_blocks,
            vg_minmax_body((const unsigned char*)e.xyzw, e.m, nullptr, (int)sizeof(float4), e.mm, SessionBlock{bx, (unsigned)e.mm_blocks}))
@@ -556,7 +608,7 @@ LILI_STAGE(LoopStGatherSorted, LoopEntry, 256, stage_blocks(e.m, 256), gather_so
 LILI_STAGE(LoopStRunEnds, LoopEntry, 256, stage_blocks(e.m, 256), cell_run_ends_at(e.keys2, e.m, e.cell_start, i))
 
 // The entry of voxelgrid_dev's chain at 32-bit keys on c's buffers: n points at `in` -> `out`, the count at `count` (the stages
-// LoopStBoxInit .. LoopStCentroid32; the keyframe store's batch runs them too)
+// LoopStBoxInit .. LoopStCentroidXyzw32; the keyframe store's and the local map's batches run them too)
 static LoopEntry vg_chain_entry(liliom_ctx* c, const void* in, int n, float leaf, void* out, int* count) {
     LoopEntry e{};
     e.raw = (const unsigned char*)in; e.n = n; e.stride = c->prm.point_stride; e.leaf = leaf;
@@ -566,26 +618,32 @@ static LoopEntry vg_chain_entry(liliom_ctx* c, const void* in, int n, float leaf
     return e;
 }
 
-// Session j's entry for cloud k (0 target, 1 source), as loop_cloud's launches take their arguments
+// Session j's entry for cloud k (0 target, 1 source), as loop_cloud's launches take their arguments (the repack's output aside:
+// loop_repack_entry)
 static LoopEntry loop_cloud_entry(const LoopJob& j, int k) {
     liliom_ctx* c = j.c;
     LoopEntry e = vg_chain_entry(c, c->bmap_raw.p, (int)j.off[k], j.leaf, c->vg_out.p, c->vg_count.as<int>() + k);
     const dim3 gg = loop_gather_grid(j, k);
     e.arena = (const unsigned char*)c->kf_arena.p; e.tab = loop_rows(j, k); e.rows = j.rows[k]; e.gx = (int)gg.x; e.gy = (int)gg.y;
     e.raw_out = (unsigned char*)c->bmap_raw.p;
-    e.xyzw = loop_dst(c, k);
     return e;
 }
-// ... and for the target's cell grid (grid_build's launches; grid_begin has sized it)
-static LoopEntry loop_grid_entry(const LoopJob& j) {
-    liliom_ctx* c = j.c;
+static LoopEntry loop_repack_entry(const LoopJob& j, int k) {
+    LoopEntry e = loop_cloud_entry(j, k);
+    e.xyzw = loop_dst(j.c, k);
+    return e;
+}
+// The launches of grid_build over index mi's m points (grid_begin has sized it)
+static LoopEntry grid_entry(liliom_ctx* c, MapIndex& mi, int m) {
     LoopEntry e{};
-    e.xyzw = c->loop.xyzw.as<float4>(); e.m = j.m[0]; e.mm = c->vg_minmax.as<int>(); e.mm_blocks = box_blocks(e.m, c->sm_count);
-    e.g = c->loop.grid; e.gkeys = c->grid_keys.as<uint32_t>(); e.gvals = c->grid_vals.as<int>();
-    e.keys2 = c->grid_keys2.as<uint32_t>(); e.vals2 = c->grid_vals2.as<int>(); e.sorted = c->loop.sorted.as<float4>();
-    e.cell_start = c->loop.cell_start.as<int>();
+    e.xyzw = mi.xyzw.as<float4>(); e.m = m; e.mm = c->vg_minmax.as<int>(); e.mm_blocks = box_blocks(e.m, c->sm_count);
+    e.g = mi.grid; e.gkeys = c->grid_keys.as<uint32_t>(); e.gvals = c->grid_vals.as<int>();
+    e.keys2 = c->grid_keys2.as<uint32_t>(); e.vals2 = c->grid_vals2.as<int>(); e.sorted = mi.sorted.as<float4>();
+    e.cell_start = mi.cell_start.as<int>();
     return e;
 }
+// ... the target's cell grid
+static LoopEntry loop_grid_entry(const LoopJob& j) { return grid_entry(j.c, j.c->loop, j.m[0]); }
 
 namespace {
 
@@ -603,9 +661,9 @@ int vg_chain_batch(liliom_ctx* c0, Sel sel, Make entry, Ctx ctx, Fail fail) {
     auto stage = [&](auto st, const std::vector<int>& which) -> int {
         return stage_batch<decltype(st)>(c0, which, [&](LoopEntry& e, int i) { e = entry(i); return ctx(i); });
     };
-    auto of_stride = [&](bool s48) {
+    auto of_kind = [&](bool s48, bool xyzw) {
         std::vector<int> v;
-        for (int i : sel()) if ((ctx(i)->prm.point_stride == 48) == s48) v.push_back(i);
+        for (int i : sel()) if ((ctx(i)->prm.point_stride == 48) == s48 && (entry(i).xyzw != nullptr) == xyzw) v.push_back(i);
         return v;
     };
     LILI_TRY(stage(LoopStBoxInit{}, sel()));
@@ -623,8 +681,10 @@ int vg_chain_batch(liliom_ctx* c0, Sel sel, Make entry, Ctx ctx, Fail fail) {
         liliom_ctx* c = ctx(i);
         if (const int rc = exclusive_scan_i32(c, c->vg_flags.as<int>(), c->vg_rank.as<int>(), entry(i).n); rc != LILIOM_OK) fail(i, rc);
     }
-    LILI_TRY(stage(LoopStCentroid48{}, of_stride(true)));
-    return stage(LoopStCentroid32{}, of_stride(false));
+    LILI_TRY(stage(LoopStCentroid48{}, of_kind(true, false)));
+    LILI_TRY(stage(LoopStCentroid32{}, of_kind(false, false)));
+    LILI_TRY(stage(LoopStCentroidXyzw48{}, of_kind(true, true)));
+    return stage(LoopStCentroidXyzw32{}, of_kind(false, true));
 }
 
 // The shared phases of loop_align_batch, every session's stream pointing at c0's.  Each phase: the solo call's host part per
@@ -649,7 +709,7 @@ int loop_batch_run(liliom_ctx* c0, std::vector<LoopJob>& J, std::vector<char>& l
         auto cloud = [k](const LoopJob& j) { return loop_cloud_entry(j, k); };
         LILI_TRY(loop_stage<LoopStGather>(c0, J, sel(has), cloud));
         LILI_TRY(vg_chain_batch(c0, [&] { return sel(has); }, [&](int i) { return cloud(J[i]); }, [&](int i) { return J[i].c; }, fail));
-        LILI_TRY(loop_stage<LoopStRepack>(c0, J, sel(has), cloud));
+        LILI_TRY(loop_stage<LoopStRepack>(c0, J, sel(has), [k](const LoopJob& j) { return loop_repack_entry(j, k); }));
         for (int i : sel(has)) copy_back(i, k * sizeof(VgParams), J[i].c->vg_params.p, sizeof(VgParams));
     }
     for (int i : sel([](const LoopJob& j) { return j.off[0] > 0 || j.off[1] > 0; }))
@@ -890,6 +950,170 @@ int kf_add_resident_batch(liliom_ctx* const* cs, int B, const liliom_backend_par
     return rc;
 }
 
+// ---- the backend local map of several sessions (liliom_bmap_build_batch): the solo call's parts per session, the gather, the
+// VoxelGrid chains, the box passes and the cell grids of every session in shared launches, three waits for all of them.
+struct BmapReflEntry {
+    const unsigned char* pts; int n; float* out;
+};
+LILI_STAGE(BmapStRefl, BmapReflEntry, 256, stage_blocks(e.n, 256), kf_refl_at(e.pts, e.n, e.out, i))
+
+namespace {
+
+// Session j's entries, as the solo call's launches take their arguments: the gather of its table, layer l's chain (the float4 points
+// into bmap[l].xyzw, as voxelgrid_dev's d_feats) and its cell grid
+LoopEntry bmap_gather_entry(const BmapJob& j) {
+    liliom_ctx* c = j.c;
+    LoopEntry e{};
+    const dim3 gg = bmap_gather_grid(j);
+    e.arena = (const unsigned char*)c->kf_arena.p; e.tab = c->kf_tab.as<KfRow>(); e.rows = j.rows; e.gx = (int)gg.x; e.gy = (int)gg.y;
+    e.stride = c->prm.point_stride; e.raw_out = (unsigned char*)c->bmap_raw.p;
+    return e;
+}
+LoopEntry bmap_layer_entry(const BmapJob& j, int l) {
+    liliom_ctx* c = j.c;
+    LoopEntry e = vg_chain_entry(c, bmap_in(j, l), (int)j.n[l], bmap_leaf(j, l), c->bmap_ds[l].p, c->vg_count.as<int>() + l);
+    e.xyzw = c->bmap[l].xyzw.as<float4>();
+    return e;
+}
+LoopEntry bmap_grid_entry(const BmapJob& j, int l) { return grid_entry(j.c, j.c->bmap[l], j.m[l]); }
+
+// The shared phases, every session's stream pointing at c0's.  Session i's read-back words land in its pinned scratch: per layer l
+// its VgParams and count at l * kSlot (phase 1), its grid box at l * kBox (phase 2).  wide[i]: session i's index wrapped in one of
+// its layers (vg_wide_keys); it leaves the shared path after phase 1.
+int bmap_batch_run(liliom_ctx* c0, std::vector<BmapJob>& J, std::vector<char>& live, std::vector<char>& wide, int* status) {
+    constexpr size_t kSlot = sizeof(VgParams) + sizeof(int), kBox = kBoxInts * sizeof(int);
+    static_assert(2 * kSlot <= sizeof(PinBlock::scratch) && 2 * kBox <= sizeof(PinBlock::scratch), "both layers' words fit the pinned scratch");
+    const int B = (int)J.size();
+    auto fail = [&](int i, int rc) { status[i] = rc; live[i] = 0; J[i].grid[0] = J[i].grid[1] = false; };
+    auto sel = [&](auto pred) {
+        std::vector<int> v;
+        for (int i = 0; i < B; ++i) if (live[i] && pred(J[i])) v.push_back(i);
+        return v;
+    };
+    auto any = [](const BmapJob&) { return true; };
+    auto copy_back = [&](int i, size_t at, const void* src, size_t bytes) {
+        if (cudaError_t err = cudaMemcpyAsync(J[i].c->h_pin->scratch + at, src, bytes, cudaMemcpyDeviceToHost, c0->stream); err != cudaSuccess)
+            fail(i, fail_cuda(J[i].c, err, "local map batch: read-back"));
+    };
+    // 1. every table's gather, the edge chains, then the surf chains (they share each session's sort chain) -> counts, VgParams
+    LILI_TRY(stage_batch<LoopStGather>(c0, sel([](const BmapJob& j) { return j.rows > 0; }),
+                                       [&](LoopEntry& e, int i) { e = bmap_gather_entry(J[i]); return J[i].c; }));
+    for (int l = 0; l < 2; ++l) {
+        for (int i : sel([l](const BmapJob& j) { return j.n[l] == 0; }))      // voxelgrid_dev's count of an empty layer
+            if (cudaError_t err = cudaMemsetAsync(J[i].c->vg_count.as<int>() + l, 0, sizeof(int), c0->stream); err != cudaSuccess)
+                fail(i, fail_cuda(J[i].c, err, "local map batch: empty count"));
+        auto has = [l](const BmapJob& j) { return j.n[l] > 0; };
+        LILI_TRY(vg_chain_batch(c0, [&] { return sel(has); }, [&](int i) { return bmap_layer_entry(J[i], l); }, [&](int i) { return J[i].c; }, fail));
+        for (int i : sel(has)) {
+            copy_back(i, l * kSlot, J[i].c->vg_params.p, sizeof(VgParams));
+            copy_back(i, l * kSlot + sizeof(VgParams), J[i].c->vg_count.as<int>() + l, sizeof(int));
+        }
+    }
+    LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+    for (int i : sel(any)) {
+        for (int l = 0; l < 2; ++l) {
+            if (J[i].n[l] <= 0) continue;
+            const unsigned char* s = J[i].c->h_pin->scratch + l * kSlot;
+            VgParams vp;
+            memcpy(&vp, s, sizeof(VgParams));
+            memcpy(&J[i].m[l], s + sizeof(VgParams), sizeof(int));
+            if (vg_wide_keys(vp)) { wide[i] = 1; live[i] = 0; }      // the solo path redoes the session with wide keys
+        }
+    }
+    // 2. each layer's box (vg_minmax in stream order) -> both cell grids of every session (grid_begin)
+    for (int l = 0; l < 2; ++l) {
+        auto has = [l](const BmapJob& j) { return j.m[l] > 0; };
+        if (l == 1) for (int i : sel(any)) J[i].launches_surf_box = J[i].c->cnt.launches;
+        LILI_TRY(stage_batch<LoopStBoxInit>(c0, sel(has), [&](LoopEntry& e, int i) { e = bmap_grid_entry(J[i], l); return J[i].c; }));
+        LILI_TRY(stage_batch<LoopStGridBox>(c0, sel(has), [&](LoopEntry& e, int i) { e = bmap_grid_entry(J[i], l); return J[i].c; }));
+        for (int i : sel(has)) copy_back(i, l * kBox, J[i].c->vg_minmax.p, kBox);
+    }
+    LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+    for (int i : sel(any)) {
+        BmapJob& j = J[i];
+        liliom_ctx* c = j.c;
+        for (int l = 0; l < 2; ++l) {
+            int hb[kBoxInts];
+            memcpy(hb, c->h_pin->scratch + l * kBox, sizeof(hb));
+            const int rc = j.m[l] > 0 ? grid_begin_exact(c, c->bmap[l], bmap_cell(j, l), j.m[l], hb, j.g[l])
+                                      : grid_begin(c, c->bmap[l], bmap_cell(j, l), 0, nullptr, j.g[l]);
+            if (rc != LILIOM_OK) {
+                const bool edge_built = l == 1 && j.grid[0];
+                fail(i, rc);
+                j.grid[0] = edge_built;           // the solo call builds the edge grid before it meets the surf layer's error
+                if (l == 0) c->cnt.launches = j.launches_surf_box;     // ... and never reaches the surf layer's box
+                break;
+            }
+            j.grid[l] = !j.g[l].done;
+        }
+    }
+    // 3. every begun cell grid, edge then surf, then the reflectivity of the 48-byte surf layers; one wait
+    for (int l = 0; l < 2; ++l) {
+        auto grid = [&]() {
+            std::vector<int> v;
+            for (int i = 0; i < B; ++i) if (J[i].grid[l]) v.push_back(i);
+            return v;
+        };
+        auto entry = [&](LoopEntry& e, int i) { e = bmap_grid_entry(J[i], l); return J[i].c; };
+        LILI_TRY(stage_batch<LoopStCellKeys>(c0, grid(), entry));
+        for (int i : grid()) if (const int rc = grid_sort(J[i].g[l]); rc != LILIOM_OK) fail(i, rc);
+        LILI_TRY(stage_batch<LoopStGatherSorted>(c0, grid(), entry));
+        for (int i : grid()) if (const int rc = grid_clear(J[i].g[l]); rc != LILIOM_OK) fail(i, rc);
+        LILI_TRY(stage_batch<LoopStRunEnds>(c0, grid(), entry));
+        for (int i : grid()) if (const int rc = grid_scan(J[i].g[l]); rc != LILIOM_OK) fail(i, rc);
+        for (int i : grid()) if (const int rc = grid_finish(J[i].g[l], 0); rc != LILIOM_OK) fail(i, rc);
+    }
+    auto s48 = [](const BmapJob& j) { return j.c->prm.point_stride == 48; };
+    for (int i : sel(s48))
+        if (cudaError_t err = J[i].c->bmap[1].refl.ensure((size_t)std::max(J[i].m[1], 1) * sizeof(float)); err != cudaSuccess)
+            fail(i, fail_cuda(J[i].c, err, "local map batch: reflectivity"));
+    LILI_TRY(stage_batch<BmapStRefl>(c0, sel([&](const BmapJob& j) { return s48(j) && j.m[1] > 0; }), [&](BmapReflEntry& e, int i) {
+        liliom_ctx* c = J[i].c;
+        e = BmapReflEntry{(const unsigned char*)c->bmap_ds[1].p, J[i].m[1], c->bmap[1].refl.as<float>()};
+        return c;
+    }));
+    LILI_CUDA(c0, cudaStreamSynchronize(c0->stream));
+    return LILIOM_OK;
+}
+
+}  // namespace
+
+// liliom_bmap_build of several sessions.  Shared launches and waits on cs[0]'s stream (the other sessions' streams joined before and
+// after with events); every buffer, library sort and scan and host decision stays the session's own, made by the solo call's parts
+// from the session's own read-back words.
+int bmap_build_batch(liliom_ctx* const* cs, int B, const liliom_backend_params* bps, const int* const* kf_ids, const double* const* poses7,
+                     const int* k, int* n_edge_map, int* n_surf_map, int* status) {
+    liliom_ctx* c0 = cs[0];
+    std::vector<BmapJob> J(B);
+    std::vector<char> live(B, 0), wide(B, 0);
+    std::vector<std::pair<unsigned long long, unsigned long long>> launches0(B);
+    const std::vector<liliom_ctx*> all(cs, cs + B);
+    LILI_TRY(batch_join_in(c0, all));
+    int rc;
+    {
+        const BatchStreams on_c0(all, c0->stream);
+        for (int i = 0; i < B; ++i) {
+            launches0[i] = {cs[i]->cnt.launches, cs[i]->cnt.lib_launches};
+            status[i] = bmap_begin(cs[i], bps + i, kf_ids[i], poses7[i], k[i], J[i]);
+            live[i] = status[i] == LILIOM_OK;
+        }
+        rc = bmap_batch_run(c0, J, live, wide, status);
+        for (int i = 0; rc == LILIOM_OK && i < B; ++i) {
+            auto at = [i](int* p) { return p ? p + i : nullptr; };
+            if (live[i]) {
+                bmap_finish(J[i], at(n_edge_map), at(n_surf_map));
+            } else if (wide[i]) {
+                // the whole solo call, which takes the wide keys, its counters counted from where the batch found them
+                liliom_ctx* c = cs[i];
+                c->cnt.launches = launches0[i].first; c->cnt.lib_launches = launches0[i].second;
+                status[i] = liliom_bmap_build(c, bps + i, kf_ids[i], poses7[i], k[i], at(n_edge_map), at(n_surf_map));
+            }
+        }
+    }
+    LILI_TRY(batch_join_out(c0, all));
+    return rc;
+}
+
 }  // namespace lili
 
 extern "C" int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids,
@@ -920,6 +1144,13 @@ extern "C" int liliom_kf_add_resident_batch(liliom_ctx* const* ctxs, int B, cons
     if (!batch_ctxs_ok(ctxs, B) || !bps || !srcs || !kf_id || !status) return LILIOM_E_ARG;
     LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
     return kf_add_resident_batch(ctxs, B, bps, srcs, kf_id, n_edge_ds, n_surf_ds, n_full_stored, status);
+}
+
+extern "C" int liliom_bmap_build_batch(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps, const int* const* kf_ids,
+                                       const double* const* poses7, const int* k, int* n_edge_map, int* n_surf_map, int* status) {
+    if (!batch_ctxs_ok(ctxs, B) || !bps || !kf_ids || !poses7 || !k || !status) return LILIOM_E_ARG;
+    LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
+    return bmap_build_batch(ctxs, B, bps, kf_ids, poses7, k, n_edge_map, n_surf_map, status);
 }
 
 extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp, int kf_id, const void* full, int n, int* n_stored) {

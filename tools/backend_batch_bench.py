@@ -25,7 +25,17 @@ Each leg stores into backends of its own, whose arenas are grown before the time
 then liliom_kf_clear), so that no timed call reallocates.  Fleets: all Horizon, all HDL-64E, and mixed (alternating).  The legs'
 ids and counts of every tick and every session's last stored clouds are checked byte-identical in the same run.  The waits per
 tick (waits_by_design) are derived from the calls' structure, not counted in the run.
-usage: backend_batch_bench.py [--loop | --handoff] [--sessions 1 2 4 8 16 32] [--steps 20] [--warmup 3] [--rounds 5]"""
+--localmap measures a fleet's backend local map instead: each session stores its own seeded 40-keyframe stream
+(synth.make_keyframe_sequence: stride 48 with backend variant 0, stride 32 with variant 1), and every tick lists the 40 keyframes
+with their poses nudged per tick:
+  (a) B solo liliom_bmap_build calls;
+  (b) one liliom_bmap_build_batch.
+A second row per B times the whole backend keyframe step: (a) per session the solo local map, window search and 16 block
+evaluations; (b) the three batched calls (liliom_bmap_build_batch, liliom_backend_window_correspond_batch, 16
+liliom_backend_window_blocks_batch).  Fleets: all Horizon, all ROT, and mixed (alternating).  Each leg has contexts of its own;
+the legs' counts, windows and blocks of the last tick of every round, and both layers of every session at the end, are checked
+byte-identical in the same run.
+usage: backend_batch_bench.py [--loop | --handoff | --localmap] [--sessions 1 2 4 8 16 32] [--steps 20] [--warmup 3] [--rounds 5]"""
 import argparse
 import ctypes as C
 import json
@@ -133,7 +143,7 @@ class Fleet:
                 a.fill(0)
         return out
 
-    def prepare(self):
+    def prepare(self, leg):
         pass
 
 
@@ -206,7 +216,7 @@ class LoopFleet:
             C.memset(C.addressof(s.res[leg]), 0, C.sizeof(s.res[leg]))
         return out
 
-    def prepare(self):
+    def prepare(self, leg):
         pass
 
 
@@ -266,7 +276,7 @@ class HandoffFleet:
         self.t, self.q = ptr(np.array(HO_TRANS), C.c_double), ptr(np.array([1.0, 0, 0, 0]), C.c_double)
         self.solo_out = [[ptr(s.res["a"][k:], C.c_int) for k in range(4)] for s in S]
 
-    def prepare(self):
+    def prepare(self, leg):
         for s in self.S:
             s.odo.extract_resident(s.q)
 
@@ -306,6 +316,114 @@ class HandoffFleet:
         return out
 
 
+LM_FLEETS = {"horizon": lambda i: 0, "rot": lambda i: 1, "mixed": lambda i: i % 2}
+
+
+def lm_stream(args):
+    from liliom_b200 import synth
+    variant, seed = args
+    return synth.make_keyframe_sequence(NKF, stride=48 if variant == 0 else 32, seed=seed)
+
+
+class LocalMapSession:
+    """one session's store on a context per leg, the 40-keyframe list, and the window step's arguments (as Session's)"""
+
+    def __init__(self, variant, seq):
+        import liliom_b200 as L
+        self.variant, self.bp = variant, L.backend_default_params(variant)
+        self.c = {leg: L.Context(variant=variant) for leg in "ab"}
+        for c in self.c.values():
+            for e, s, _ in seq:
+                c.kf_add(self.bp, e, s, download=False)
+        self.base = [p for _, _, p in seq]
+        self.ids = np.arange(NKF, dtype=np.int32)
+        self.poses = {leg: np.zeros((NKF, 7)) for leg in "ab"}       # the tick's list poses, written in place by prepare
+        self.tick = {leg: 0 for leg in "ab"}
+        self.counts = {leg: np.zeros(2, np.int32) for leg in "ab"}
+        self.win_ids = np.arange(NKF - WIN, NKF, dtype=np.int32)
+        self.poses_l = np.array([nudge(seq[i][2], 1) for i in self.win_ids])
+        self.bodies = [np.array([nudge(p, 2 + j) for p in self.poses_l]) for j in range(EVALS)]
+        self.res = {leg: (np.zeros(WIN, np.int32), np.zeros(WIN, np.int32), [np.zeros((WIN, 2, 29)) for _ in range(EVALS)]) for leg in "ab"}
+
+    def close(self):
+        for c in self.c.values():
+            c.close()
+
+
+class LocalMapFleet:
+    """B sessions and the C arguments of both legs, built once; step=True adds the window search and the 16 block evaluations"""
+
+    def __init__(self, S, step):
+        import liliom_b200 as L
+        self.S, self.lib, self.step, B = S, L._binding.lib(), step, len(S)
+        P, D = C.POINTER(C.c_int), C.POINTER(C.c_double)
+        self.handles = {leg: (C.c_void_p * B)(*[s.c[leg]._h for s in S]) for leg in "ab"}
+        self.bps = (L.BackendParams * B)(*[s.bp for s in S])
+        self.ids = (P * B)(*[ptr(s.ids, C.c_int) for s in S])
+        self.poses = (D * B)(*[ptr(s.poses["b"], C.c_double) for s in S])
+        self.k = np.full(B, NKF, np.int32)
+        self.ne_map, self.ns_map = np.zeros(B, np.int32), np.zeros(B, np.int32)
+        self.win_ids = (P * B)(*[ptr(s.win_ids, C.c_int) for s in S])
+        self.win_poses = (D * B)(*[ptr(s.poses_l, C.c_double) for s in S])
+        self.kw = np.full(B, WIN, np.int32)
+        self.ne = (P * B)(*[ptr(s.res["b"][0], C.c_int) for s in S])
+        self.ns = (P * B)(*[ptr(s.res["b"][1], C.c_int) for s in S])
+        self.bodies = [(D * B)(*[ptr(s.bodies[j], C.c_double) for s in S]) for j in range(EVALS)]
+        self.outs = [(D * B)(*[ptr(s.res["b"][2][j], C.c_double) for s in S]) for j in range(EVALS)]
+        self.status = np.zeros(B, np.int32)
+
+    def prepare(self, leg):
+        for s in self.S:
+            t = s.tick[leg]
+            s.poses[leg][:] = [nudge(p, t % 5) for p in s.base]
+            s.tick[leg] = t + 1
+
+    def leg_a(self):
+        for s in self.S:
+            h, cnt = s.c["a"]._h, s.counts["a"]
+            rc = self.lib.liliom_bmap_build(h, C.byref(s.bp), ptr(s.ids, C.c_int), ptr(s.poses["a"], C.c_double), NKF, ptr(cnt, C.c_int),
+                                            ptr(cnt[1:], C.c_int))
+            assert rc == 0, rc
+            if not self.step:
+                continue
+            ne, ns, out = s.res["a"]
+            rc = self.lib.liliom_backend_window_correspond(h, C.byref(s.bp), ptr(s.win_ids, C.c_int), ptr(s.poses_l, C.c_double), WIN,
+                                                           ptr(ne, C.c_int), ptr(ns, C.c_int))
+            assert rc == 0, rc
+            for j in range(EVALS):
+                rc = self.lib.liliom_backend_window_blocks(h, ptr(s.bodies[j], C.c_double), WIN, ptr(out[j], C.c_double))
+                assert rc == 0, rc
+
+    def leg_b(self):
+        B, st, h = len(self.S), ptr(self.status, C.c_int), self.handles["b"]
+        rc = self.lib.liliom_bmap_build_batch(h, B, self.bps, self.ids, self.poses, ptr(self.k, C.c_int), ptr(self.ne_map, C.c_int),
+                                              ptr(self.ns_map, C.c_int), st)
+        assert rc == 0 and not self.status.any(), (rc, self.status)
+        for i, s in enumerate(self.S):
+            s.counts["b"][:] = (self.ne_map[i], self.ns_map[i])
+        if not self.step:
+            return
+        rc = self.lib.liliom_backend_window_correspond_batch(h, B, self.bps, self.win_ids, self.win_poses, ptr(self.kw, C.c_int), self.ne,
+                                                             self.ns, st)
+        assert rc == 0 and not self.status.any(), (rc, self.status)
+        for j in range(EVALS):
+            rc = self.lib.liliom_backend_window_blocks_batch(h, B, self.bodies[j], ptr(self.kw, C.c_int), self.outs[j], st)
+            assert rc == 0 and not self.status.any(), (rc, self.status)
+
+    def outputs(self, leg):
+        """leg's counts (and window results) of every session as bytes; cleared for the next step"""
+        out = b""
+        for s in self.S:
+            ne, ns, blocks = s.res[leg]
+            out += s.counts[leg].tobytes() + ne.tobytes() + ns.tobytes() + b"".join(o.tobytes() for o in blocks)
+            for a in [s.counts[leg], ne, ns] + blocks:
+                a.fill(0)
+        return out
+
+    def layers(self, leg):
+        return b"".join(s.c[leg].bmap_download(layer).tobytes() for s in self.S for layer in (0, 1))
+
+
 def timed(f, leg, steps):
     """median ms of `steps` window steps of leg "a" or "b", and the outputs of the last (every call returns with its sessions'
     work complete)"""
@@ -314,7 +432,7 @@ def timed(f, leg, steps):
     lat = []
     for _ in range(steps):
         f.outputs(leg)
-        f.prepare()
+        f.prepare(leg)
         torch.cuda.synchronize()
         t = time.perf_counter()
         run()
@@ -330,11 +448,14 @@ def main():
     ap.add_argument("--rounds", type=int, default=5)
     ap.add_argument("--loop", action="store_true", help="the fleet loop-closure tick instead of the window step")
     ap.add_argument("--handoff", action="store_true", help="the fleet keyframe hand-off tick instead of the window step")
+    ap.add_argument("--localmap", action="store_true", help="the fleet backend local map (and keyframe step) instead of the window step")
     args = ap.parse_args()
     if args.loop:
         return main_loop(args)
     if args.handoff:
         return main_handoff(args)
+    if args.localmap:
+        return main_localmap(args)
     Bmax = max(args.sessions)
     with ProcessPoolExecutor(max_workers=min(Bmax, os.cpu_count() or 1)) as ex:     # the streams, before CUDA starts here
         seqs = list(ex.map(stream, [100 + s for s in range(Bmax)]))
@@ -430,6 +551,44 @@ def main_handoff(args):
                        waits_by_design=[5 * B, 1 + (3 if n_hz else 2)],
                        speedup=round(float(np.median(ra) / np.median(rb)), 3), identical=bool(same))
             print(json.dumps(row), flush=True)
+        for s in sessions:
+            s.close()
+
+
+def main_localmap(args):
+    Bmax = max(args.sessions)
+    jobs = [(v, 400 + 2 * s + v) for s in range(Bmax) for v in (0, 1)]
+    with ProcessPoolExecutor(max_workers=min(len(jobs), os.cpu_count() or 1)) as ex:
+        seqs = dict(zip(jobs, ex.map(lm_stream, jobs)))
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("backend_batch_bench.py measures on a CUDA device; none is visible")
+    print(json.dumps(dict(card(), leg="localmap", keyframes=NKF, window=WIN, evals=EVALS, steps=args.steps, warmup=args.warmup,
+                          rounds=args.rounds, figures="[median of rounds, min round, max round], ms per fleet tick")), flush=True)
+    for fleet, variant_of in LM_FLEETS.items():
+        sessions = [LocalMapSession(variant_of(s), seqs[variant_of(s), 400 + 2 * s + variant_of(s)]) for s in range(Bmax)]
+        for B in args.sessions:
+            S = sessions[:B]
+            for step in (False, True):
+                f = LocalMapFleet(S, step)
+                for leg in "ab":
+                    timed(f, leg, args.warmup)
+                ra, rb, same = [], [], True
+                for _ in range(args.rounds):
+                    ta, oa = timed(f, "a", args.steps)
+                    tb, ob = timed(f, "b", args.steps)
+                    ra.append(ta); rb.append(tb)
+                    same = same and oa == ob
+                same = same and f.layers("a") == f.layers("b")
+                # the waits follow from the calls' structure (include/liliom.h); the run does not count them: a solo local map with
+                # both layers non-empty waits five times, the batch three; a window search and a blocks call wait once each
+                per = 1 + EVALS if step else 0
+                row = dict(fleet=fleet, sessions=B, call="keyframe_step" if step else "local_map",
+                           edge_map=int(np.median([s.c["a"].bmap_download(0).size for s in S])),
+                           surf_map=int(np.median([s.c["a"].bmap_download(1).size for s in S])),
+                           a_solo_ms=spread(ra), b_batch_ms=spread(rb), waits_by_design=[B * (5 + per), 3 + per],
+                           speedup=round(float(np.median(ra) / np.median(rb)), 3), identical=bool(same))
+                print(json.dumps(row), flush=True)
         for s in sessions:
             s.close()
 
