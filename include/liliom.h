@@ -385,6 +385,28 @@ enum { LILIOM_KF_FULL = 0, LILIOM_KF_SURF = 1 };
 int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, const double* poses7, int k, const double pre7[7],
                       float leaf, void* out, int cap, int* n);
 
+/* ---- the keyframes of several stores (a fleet's sessions, or a restarted session and its previous run's context) ----
+ * A store is any backend context (liliom_kf_add*); the calls below read the listed keyframes where they lie in each store's
+ * arenas and run everything else on c, into c's buffers, exactly as the single-store call on c: the result is bit for bit that
+ * of liliom_global_map / liliom_loop_align on a context D whose store holds the same clouds (e.g. the same kf_add / kf_add_full
+ * calls replayed), called with the mapped list; with every entry naming c, that of the single-store call on c.
+ * They write what that call writes on c (the keyframe table, VoxelGrid scratch, vg_out: no resident scan for
+ * liliom_map_update_resident afterwards; liliom_loop_align_multi also the loop index and source) and never write a store.
+ * Each distinct store stream is joined into c's stream with an event before the first read; the call returns with every read
+ * done.  No other host thread may call into a store during the call (growing an arena frees the old one).
+ * LILIOM_E_ARG, nothing changed: a NULL array or store, a store on another device, of another point_stride or with a
+ * communicator, an id unknown to its store, KF_FULL on a keyframe without a full cloud, and whatever the single-store call
+ * refuses.  LILIOM_E_CAPACITY, nothing changed: 2^31 listed points or more (per cloud for the loop closure). */
+/* publishCompleteMap / save_pcd over keyframes of several stores.  Entry i = keyframe kf_ids[i] of stores[i], placed by
+ * poses7[7i..] (after pre7s[7i..] when pre7s is not NULL: each robot's own Tbl).  The result runs on c, into c's buffers. */
+int liliom_global_map_multi(liliom_ctx* c, int kind, liliom_ctx* const* stores, const int* kf_ids, const double* poses7, int k,
+                            const double* pre7s, float leaf, void* out, int cap, int* n);
+/* liliom_loop_align with each cloud's keyframes drawn from any stores; the ICP and its index on c. */
+int liliom_loop_align_multi(liliom_ctx* c, liliom_ctx* const* src_stores, const int* src_ids, const double* src_poses7, int k_src,
+                            liliom_ctx* const* tgt_stores, const int* tgt_ids, const double* tgt_poses7, int k_tgt, float leaf,
+                            double max_corr_dist, int max_iter, double trans_eps, double fit_eps,
+                            double T16[16], double* fitness, int* converged, int* iters, int* n_src, int* n_tgt);
+
 /* ---- SURVEY §8 (f3): wire format on the sensor side — FormatConvert's livoxLidarHandler on the device ----
  * L/src/FormatConvert.cpp:11-24: livox_ros_driver::CustomPoint {uint32 offset_time; float x,y,z; uint8 reflectivity,
  * tag, line} -> pcl::PointXYZINormal with intensity = line + 0.1*float(offset_time/(float)time_end) (:19-20),

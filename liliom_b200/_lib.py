@@ -96,6 +96,7 @@ EXPORTS = [
     "liliom_backend_window_correspond_batch", "liliom_backend_window_blocks_batch",
     "liliom_loop_align_batch", "liliom_convert_batch", "liliom_undistort_resident", "liliom_kf_add_resident",
     "liliom_undistort_resident_batch", "liliom_kf_add_resident_batch", "liliom_bmap_build_batch",
+    "liliom_global_map_multi", "liliom_loop_align_multi",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -259,6 +260,9 @@ def lib() -> C.CDLL:
     L.liliom_global_map.argtypes = [vp, C.c_int, ip, dp, C.c_int, dp, C.c_float, vp, C.c_int, ip]
     L.liliom_loop_align.argtypes = [vp, ip, dp, C.c_int, ip, dp, C.c_int, C.c_float, C.c_double, C.c_int, C.c_double, C.c_double,
                                     dp, dp, ip, ip, ip, ip]
+    L.liliom_global_map_multi.argtypes = [vp, C.c_int, C.POINTER(vp), ip, dp, C.c_int, dp, C.c_float, vp, C.c_int, ip]
+    L.liliom_loop_align_multi.argtypes = [vp, C.POINTER(vp), ip, dp, C.c_int, C.POINTER(vp), ip, dp, C.c_int, C.c_float, C.c_double,
+                                          C.c_int, C.c_double, C.c_double, dp, dp, ip, ip, ip, ip]
     L.liliom_loop_align_batch.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(ip), C.POINTER(dp), ip, C.POINTER(ip), C.POINTER(dp), ip,
                                           C.POINTER(LoopParams), C.POINTER(LoopResult), ip]
     L.liliom_convert_batch.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(WireMsg), C.POINTER(vp), ip, ip, ip]
@@ -710,6 +714,40 @@ class Context:
         out = np.zeros(max(n.value, 1), self.dtype)
         self._check(lib().liliom_global_map(*args, _ptr(out), len(out), C.byref(n)))
         return out[:n.value]
+
+    def global_map_multi(self, kind: int, stores, kf_ids, poses7, leaf: float, pre7s=None) -> np.ndarray:
+        """global_map over keyframes of several stores (liliom_global_map_multi): entry i is keyframe kf_ids[i] of the Context
+        stores[i], placed by poses7[i] after pre7s[i] (pre7s: None, one 7-vector for every entry, or one per entry).  The filter
+        runs on this context; the stores are only read."""
+        ids = _ids(kf_ids); k = len(ids); p = _poses(poses7, k)
+        assert len(stores) == k
+        st = _handles(stores)
+        pre = None
+        if pre7s is not None:
+            pre = np.ascontiguousarray(pre7s, dtype=np.float64)
+            pre = np.ascontiguousarray(np.tile(pre.reshape(1, 7), (max(k, 1), 1)) if pre.size == 7 else pre.reshape(-1, 7))
+        ipp = C.POINTER(C.c_int)
+        args = (self._h, int(kind), st, ids.ctypes.data_as(ipp), _dptr(p), k, None if pre is None else _dptr(pre), leaf)
+        n = C.c_int()
+        self._check(lib().liliom_global_map_multi(*args, None, 0, C.byref(n)))
+        out = np.zeros(max(n.value, 1), self.dtype)
+        self._check(lib().liliom_global_map_multi(*args, _ptr(out), len(out), C.byref(n)))
+        return out[:n.value]
+
+    def loop_align_multi(self, src_stores, src_ids, src_poses, tgt_stores, tgt_ids, tgt_poses, leaf: float, max_corr_dist=30.0,
+                         max_iter=100, trans_eps=1e-6, fit_eps=1e-6):
+        """loop_align with each cloud's keyframes drawn from any stores (liliom_loop_align_multi): src_ids[i] of the Context
+        src_stores[i], likewise the target; the ICP and its index on this context.  Returns loop_align's tuple."""
+        si = _ids(src_ids); sp = _poses(src_poses, len(si))
+        ti = _ids(tgt_ids); tp = _poses(tgt_poses, len(ti))
+        assert len(src_stores) == len(si) and len(tgt_stores) == len(ti)
+        ss = _handles(src_stores); ts = _handles(tgt_stores)
+        ipp = C.POINTER(C.c_int)
+        T = np.zeros(16, np.float64); fit = C.c_double(); conv = C.c_int(); it = C.c_int(); ns = C.c_int(); nt = C.c_int()
+        self._check(lib().liliom_loop_align_multi(self._h, ss, si.ctypes.data_as(ipp), _dptr(sp), len(si), ts, ti.ctypes.data_as(ipp), _dptr(tp),
+                                                  len(ti), leaf, max_corr_dist, max_iter, trans_eps, fit_eps, _dptr(T), C.byref(fit),
+                                                  C.byref(conv), C.byref(it), C.byref(ns), C.byref(nt)))
+        return T.reshape(4, 4), fit.value, bool(conv.value), it.value, ns.value, nt.value
 
     # ---- wire formats (f3) ----
     @staticmethod

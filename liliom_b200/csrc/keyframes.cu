@@ -15,6 +15,7 @@
 #include "dev_math.cuh"
 #include "kf_table.h"
 #include <algorithm>
+#include <tuple>
 #include <type_traits>
 
 namespace lili {
@@ -40,29 +41,27 @@ struct KfGridAt {
     __device__ __forceinline__ unsigned int gx() const { return w; }
     __device__ __forceinline__ unsigned int gy() const { return h; }
 };
-template <class Grid>
-__device__ __forceinline__ void kf_gather_at(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride,
+template <class Row, class Grid>
+__device__ __forceinline__ void kf_gather_at(const unsigned char* __restrict__ arena, const Row* __restrict__ tab, int rows, int stride,
                                              unsigned char* __restrict__ out, const Grid blk) {
     for (int y = blk.by(); y < rows; y += blk.gy()) {
-        const KfRow& r = tab[y];
+        const Row& r = tab[y];
         for (int i = blk.bx() * blockDim.x + threadIdx.x; i < r.n; i += blk.gx() * blockDim.x)
-            kf_row_point(r, arena + (size_t)(r.src_off + i) * stride, stride, out + (size_t)(r.dst_off + i) * stride);
+            kf_row_point(r, kf_row_src(r, arena, stride, r.src_off + i), stride, out + (size_t)(r.dst_off + i) * stride);
     }
-}
-__global__ void k_kf_gather(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride,
-                            unsigned char* __restrict__ out) {
-    kf_gather_at(arena, tab, rows, stride, out, KfGridSolo{});
 }
 
 // box (vg_box.h) of the finite transformed points of the rows, joined into mm
-__global__ void k_kf_box(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride, int* __restrict__ mm) {
+template <class Row>
+__device__ __forceinline__ void kf_box_at(const unsigned char* __restrict__ arena, const Row* __restrict__ tab, int rows, int stride,
+                                          int* __restrict__ mm) {
     int box[kBoxInts];
 #pragma unroll
     for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_empty(k);
     for (int y = blockIdx.y; y < rows; y += gridDim.y) {
-        const KfRow& r = tab[y];
+        const Row& r = tab[y];
         for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < r.n; i += gridDim.x * blockDim.x) {
-            const VgXyz p = kf_row_xyz(r, arena + (size_t)(r.src_off + i) * stride);
+            const VgXyz p = kf_row_xyz(r, kf_row_src(r, arena, stride, r.src_off + i));
             if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) vg_box_add(box, p.x, p.y, p.z);
         }
     }
@@ -71,14 +70,14 @@ __global__ void k_kf_box(const unsigned char* __restrict__ arena, const KfRow* _
 
 // PCL's relative voxel index of every transformed point (not finite: all-ones, or bit 32 of a wide key), value = its index in
 // the concatenation
-template <typename K>
-__global__ void k_kf_keys(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride, const VgParams p,
-                          K* __restrict__ keys, int* __restrict__ vals) {
+template <typename K, class Row>
+__device__ __forceinline__ void kf_keys_at(const unsigned char* __restrict__ arena, const Row* __restrict__ tab, int rows, int stride,
+                                           const VgParams p, K* __restrict__ keys, int* __restrict__ vals) {
     const K sentinel = sizeof(K) == 4 ? (K)0xffffffffu : (K)(1ull << 32);
     for (int y = blockIdx.y; y < rows; y += gridDim.y) {
-        const KfRow& r = tab[y];
+        const Row& r = tab[y];
         for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < r.n; i += gridDim.x * blockDim.x) {
-            const VgXyz x = kf_row_xyz(r, arena + (size_t)(r.src_off + i) * stride);
+            const VgXyz x = kf_row_xyz(r, kf_row_src(r, arena, stride, r.src_off + i));
             const long long d = r.dst_off + i;
             keys[d] = (isfinite(x.x) && isfinite(x.y) && isfinite(x.z)) ? (K)vg_rel_index(p, x.x, x.y, x.z) : sentinel;
             vals[d] = (int)d;
@@ -87,15 +86,69 @@ __global__ void k_kf_keys(const unsigned char* __restrict__ arena, const KfRow* 
 }
 
 // centroid of every voxel of the sorted keys (the first n_fin entries are the finite points), members transformed on load
+template <int STRIDE, typename K, class Row>
+__device__ __forceinline__ void kf_centroid_at(const unsigned char* arena, const Row* tab, int rows,
+                                               const K* keys, const int* vals, const int* flags,
+                                               const int* rank, int n_fin, unsigned char* out) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_fin || !flags[i]) return;
+    const VgAcc<STRIDE> a = vg_walk<STRIDE>(keys, i, n_fin, [&](int j) { return vals[j]; }, KfRowLoader<STRIDE, Row>{arena, tab, rows});
+    vg_write<STRIDE>(a.s, a.n, out + (size_t)rank[i] * STRIDE);
+}
+
+// The table kernels over one store's arena (KfRow) ...
+__global__ void k_kf_gather(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride,
+                            unsigned char* __restrict__ out) {
+    kf_gather_at(arena, tab, rows, stride, out, KfGridSolo{});
+}
+__global__ void k_kf_box(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride, int* __restrict__ mm) {
+    kf_box_at(arena, tab, rows, stride, mm);
+}
+template <typename K>
+__global__ void k_kf_keys(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride, const VgParams p,
+                          K* __restrict__ keys, int* __restrict__ vals) {
+    kf_keys_at(arena, tab, rows, stride, p, keys, vals);
+}
 template <int STRIDE, typename K>
 __global__ void k_kf_centroid(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, const K* __restrict__ keys,
                               const int* __restrict__ vals, const int* __restrict__ flags, const int* __restrict__ rank, int n_fin,
                               unsigned char* __restrict__ out) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_fin || !flags[i]) return;
-    const VgAcc<STRIDE> a = vg_walk<STRIDE>(keys, i, n_fin, [&](int j) { return vals[j]; }, KfRowLoader<STRIDE>{arena, tab, rows});
-    vg_write<STRIDE>(a.s, a.n, out + (size_t)rank[i] * STRIDE);
+    kf_centroid_at<STRIDE>(arena, tab, rows, keys, vals, flags, rank, n_fin, out);
 }
+// ... and over rows of several stores (KfRowM: each row names its arena; `arena` is not read)
+__global__ void k_kf_gather_m(const unsigned char* __restrict__ arena, const KfRowM* __restrict__ tab, int rows, int stride,
+                              unsigned char* __restrict__ out) {
+    kf_gather_at(arena, tab, rows, stride, out, KfGridSolo{});
+}
+__global__ void k_kf_box_m(const unsigned char* __restrict__ arena, const KfRowM* __restrict__ tab, int rows, int stride, int* __restrict__ mm) {
+    kf_box_at(arena, tab, rows, stride, mm);
+}
+template <typename K>
+__global__ void k_kf_keys_m(const unsigned char* __restrict__ arena, const KfRowM* __restrict__ tab, int rows, int stride, const VgParams p,
+                            K* __restrict__ keys, int* __restrict__ vals) {
+    kf_keys_at(arena, tab, rows, stride, p, keys, vals);
+}
+template <int STRIDE, typename K>
+__global__ void k_kf_centroid_m(const unsigned char* __restrict__ arena, const KfRowM* __restrict__ tab, int rows, const K* __restrict__ keys,
+                                const int* __restrict__ vals, const int* __restrict__ flags, const int* __restrict__ rank, int n_fin,
+                                unsigned char* __restrict__ out) {
+    kf_centroid_at<STRIDE>(arena, tab, rows, keys, vals, flags, rank, n_fin, out);
+}
+
+// Each row type's kernels, for the host code written once over both (kf_gather, gmap_run, loop_cloud)
+template <class Row> struct KfKern;
+template <> struct KfKern<KfRow> {
+    static constexpr auto gather = k_kf_gather;
+    static constexpr auto box = k_kf_box;
+    template <typename K> static constexpr auto keys = k_kf_keys<K>;
+    template <int S, typename K> static constexpr auto centroid = k_kf_centroid<S, K>;
+};
+template <> struct KfKern<KfRowM> {
+    static constexpr auto gather = k_kf_gather_m;
+    static constexpr auto box = k_kf_box_m;
+    template <typename K> static constexpr auto keys = k_kf_keys_m<K>;
+    template <int S, typename K> static constexpr auto centroid = k_kf_centroid_m<S, K>;
+};
 
 // reflectivity (curvature = 0.1 * reflectivity, L/src/FormatConvert.cpp:21) of 48-byte points; `i` as in the other bodies
 __device__ __forceinline__ void kf_refl_at(const unsigned char* __restrict__ pts, int n, float* __restrict__ out, const int i) {
@@ -136,18 +189,20 @@ static bool kf_ids_ok(liliom_ctx* c, const int* ids, int k) {
     return true;
 }
 
-static int kf_upload_table(liliom_ctx* c, const std::vector<KfRow>& tab) {
-    LILI_CUDA(c, c->kf_tab.ensure(tab.size() * sizeof(KfRow)));
-    LILI_CUDA(c, cudaMemcpyAsync(c->kf_tab.p, tab.data(), tab.size() * sizeof(KfRow), cudaMemcpyHostToDevice, c->stream));
+template <class Row>
+static int kf_upload_table(liliom_ctx* c, const std::vector<Row>& tab) {
+    LILI_CUDA(c, c->kf_tab.ensure(tab.size() * sizeof(Row)));
+    LILI_CUDA(c, cudaMemcpyAsync(c->kf_tab.p, tab.data(), tab.size() * sizeof(Row), cudaMemcpyHostToDevice, c->stream));
     return LILIOM_OK;
 }
 
-// Transform + concatenate rows of `arena` into `out` (one launch).
-static int kf_gather(liliom_ctx* c, const void* arena, const std::vector<KfRow>& tab, long long largest, void* out) {
+// Transform + concatenate rows (of `arena`, or each of its own: KfRowM) into `out` (one launch).
+template <class Row>
+static int kf_gather(liliom_ctx* c, const void* arena, const std::vector<Row>& tab, long long largest, void* out) {
     if (tab.empty() || largest <= 0) return LILIOM_OK;
     LILI_TRY(kf_upload_table(c, tab));
-    k_kf_gather<<<kf_row_grid(tab.size(), largest, c->sm_count * 4), 256, 0, c->stream>>>(
-        (const unsigned char*)arena, c->kf_tab.as<KfRow>(), (int)tab.size(), c->prm.point_stride, (unsigned char*)out);
+    KfKern<Row>::gather<<<kf_row_grid(tab.size(), largest, c->sm_count * 4), 256, 0, c->stream>>>(
+        (const unsigned char*)arena, c->kf_tab.as<Row>(), (int)tab.size(), c->prm.point_stride, (unsigned char*)out);
     return launch_check(c, "k_kf_gather");
 }
 
@@ -164,19 +219,39 @@ static KfRow kf_row(long long src, long long dst, int n, const double* pose7, co
     }
     return e;
 }
+// ... of the table's row type: a KfRowM also names the arena its points lie in
+template <class Row> Row kf_row_in(const DevBuf& arena, long long src, long long dst, int n, const double* pose7, const double* pre7 = nullptr);
+template <> KfRow kf_row_in<KfRow>(const DevBuf&, long long src, long long dst, int n, const double* pose7, const double* pre7) {
+    return kf_row(src, dst, n, pose7, pre7);
+}
+template <> KfRowM kf_row_in<KfRowM>(const DevBuf& arena, long long src, long long dst, int n, const double* pose7, const double* pre7) {
+    KfRowM e{};
+    static_cast<KfRow&>(e) = kf_row(src, dst, n, pose7, pre7);
+    e.base = (const unsigned char*)arena.p;
+    return e;
+}
+
+// The store of each list entry: c for every entry (the single-store calls) or stores[i] (liliom_*_multi)
+struct KfStores {
+    liliom_ctx* c;
+    liliom_ctx* const* per = nullptr;
+    liliom_ctx* operator[](int i) const { return per ? per[i] : c; }
+};
 
 // detectLoopClosure's cloud of the listed keyframes (:2476-2497, :2502-2547): edge then surf of each, transformed by its pose,
 // concatenated into bmap_raw (one launch), VoxelGrid(leaf) into vg_out with its count at d_count (device) and *m (host).
 // *n_in: the points read (0: nothing was launched, d_count is not written and *m = 0).
 // The rows of such a cloud appended to tab (destinations from 0); returns its points, *largest = the largest keyframe cloud.
-static long long kf_cloud_rows(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, std::vector<KfRow>& tab, long long* largest) {
+template <class Row>
+static long long kf_cloud_rows(KfStores s, const int* kf_ids, const double* poses7, int k, std::vector<Row>& tab, long long* largest) {
     long long off = 0;
     *largest = 0;
     for (int i = 0; i < k; ++i) {                                 // :2492-2493 / :2519-2520: *edge_frames[i] then *surf_frames[i]
-        const KfEntry& f = c->kfs[kf_ids[i]];
-        if (f.n_edge) tab.push_back(kf_row(f.edge_off, off, f.n_edge, poses7 + 7 * (size_t)i));
+        const KfEntry& f = s[i]->kfs[kf_ids[i]];
+        const DevBuf& arena = s[i]->kf_arena;
+        if (f.n_edge) tab.push_back(kf_row_in<Row>(arena, f.edge_off, off, f.n_edge, poses7 + 7 * (size_t)i));
         off += f.n_edge;
-        if (f.n_surf) tab.push_back(kf_row(f.surf_off, off, f.n_surf, poses7 + 7 * (size_t)i));
+        if (f.n_surf) tab.push_back(kf_row_in<Row>(arena, f.surf_off, off, f.n_surf, poses7 + 7 * (size_t)i));
         off += f.n_surf;
         *largest = std::max(*largest, (long long)std::max(f.n_edge, f.n_surf));
     }
@@ -187,7 +262,7 @@ static int kf_cloud_dev(liliom_ctx* c, const int* kf_ids, const double* poses7, 
     const int stride = c->prm.point_stride;
     std::vector<KfRow> tab;
     long long largest = 0;
-    const long long off = kf_cloud_rows(c, kf_ids, poses7, k, tab, &largest);
+    const long long off = kf_cloud_rows(KfStores{c}, kf_ids, poses7, k, tab, &largest);
     *n_in = off;
     *m = 0;
     if (off == 0) return LILIOM_OK;
@@ -513,23 +588,27 @@ struct LoopJob {
 static float loop_cell(const liliom_ctx* c) { return gate_cell(c->prm.knn_max_sqdist); }   // the cell of liliom_icp_align's target
 static float4* loop_dst(liliom_ctx* c, int k) { return k == 0 ? c->loop.xyzw.as<float4>() : c->loop_src.as<float4>(); }
 
-// Validation (nothing changes on an error), the keyframe tables of both clouds in one upload (so that both stay valid until
-// their gathers have run) and every buffer of the clouds' chains.
-static int loop_begin(liliom_ctx* c, const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids, const double* tgt_poses7,
-                      int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps, double fit_eps, LoopJob& j) {
-    if (k_src < 0 || k_tgt < 0 || (k_src > 0 && (!src_ids || !src_poses7)) || (k_tgt > 0 && (!tgt_ids || !tgt_poses7)) ||
-        !(leaf > 0) || !(max_corr_dist > 0) || max_iter < 1)
-        return LILIOM_E_ARG;
-    LILI_TRY(backend_check(c, nullptr));
-    if (!kf_ids_ok(c, src_ids, k_src) || !kf_ids_ok(c, tgt_ids, k_tgt)) return LILIOM_E_ARG;     // before anything changes
+// liliom_loop_align's arguments, the keyframe lists aside
+static bool loop_args_ok(const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids, const double* tgt_poses7, int k_tgt,
+                         float leaf, double max_corr_dist, int max_iter) {
+    return k_src >= 0 && k_tgt >= 0 && (k_src == 0 || (src_ids && src_poses7)) && (k_tgt == 0 || (tgt_ids && tgt_poses7)) && leaf > 0 &&
+           max_corr_dist > 0 && max_iter >= 1;
+}
+
+// After validation: the keyframe tables of both clouds in one upload (so that both stay valid until their gathers have run), rows
+// of the table's type read from each entry's store, and every buffer of the clouds' chains.
+template <class Row>
+static int loop_tables(liliom_ctx* c, KfStores src, const int* src_ids, const double* src_poses7, int k_src, KfStores tgt, const int* tgt_ids,
+                       const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps, double fit_eps,
+                       LoopJob& j) {
     LILI_CUDA(c, cudaSetDevice(c->device));
     j = LoopJob{};
     j.c = c; j.leaf = leaf; j.max_corr_dist = max_corr_dist; j.max_iter = max_iter; j.trans_eps = trans_eps; j.fit_eps = fit_eps;
-    std::vector<KfRow> tab;
+    std::vector<Row> tab;
     // :2502-2547 his_key_frames_ds (the target), :2476-2497 latest_key_frames_ds (the source)
-    j.off[0] = kf_cloud_rows(c, tgt_ids, tgt_poses7, k_tgt, tab, &j.largest[0]);
+    j.off[0] = kf_cloud_rows(tgt, tgt_ids, tgt_poses7, k_tgt, tab, &j.largest[0]);
     j.rows[0] = (int)tab.size();
-    j.off[1] = kf_cloud_rows(c, src_ids, src_poses7, k_src, tab, &j.largest[1]);
+    j.off[1] = kf_cloud_rows(src, src_ids, src_poses7, k_src, tab, &j.largest[1]);
     j.rows[1] = (int)tab.size() - j.rows[0];
     const long long n = std::max(j.off[0], j.off[1]);
     const int stride = c->prm.point_stride;
@@ -546,23 +625,48 @@ static int loop_begin(liliom_ctx* c, const int* src_ids, const double* src_poses
     return LILIOM_OK;
 }
 
+// Validation (nothing changes on an error), then loop_tables over c's own store.
+static int loop_begin(liliom_ctx* c, const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids, const double* tgt_poses7,
+                      int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps, double fit_eps, LoopJob& j) {
+    if (!loop_args_ok(src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter)) return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, nullptr));
+    if (!kf_ids_ok(c, src_ids, k_src) || !kf_ids_ok(c, tgt_ids, k_tgt)) return LILIOM_E_ARG;     // before anything changes
+    return loop_tables<KfRow>(c, KfStores{c}, src_ids, src_poses7, k_src, KfStores{c}, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist,
+                              max_iter, trans_eps, fit_eps, j);
+}
+
 // the gather's grid for cloud k (kf_row_grid)
 static dim3 loop_gather_grid(const LoopJob& j, int k) { return kf_row_grid(j.rows[k], j.largest[k], j.c->sm_count * 4); }
-static const KfRow* loop_rows(const LoopJob& j, int k) { return j.c->kf_tab.as<KfRow>() + (k == 0 ? 0 : j.rows[0]); }
+template <class Row = KfRow>
+static const Row* loop_rows(const LoopJob& j, int k) { return j.c->kf_tab.as<Row>() + (k == 0 ? 0 : j.rows[0]); }
 
 // Cloud k (0 target, 1 source) on the solo path: gather, VoxelGrid with its count read back (voxelgrid_dev_sync: wide keys where
 // the index wraps), repack into the loop index's points or loop_src (the count read on the device).
+template <class Row>
 static int loop_cloud(LoopJob& j, int k) {
     liliom_ctx* c = j.c;
     const int stride = c->prm.point_stride;
     int* cnt = c->vg_count.as<int>() + k;
     if (j.off[k] > 0) {
-        k_kf_gather<<<loop_gather_grid(j, k), 256, 0, c->stream>>>((const unsigned char*)c->kf_arena.p, loop_rows(j, k), j.rows[k], stride,
-                                                                   (unsigned char*)c->bmap_raw.p);
+        KfKern<Row>::gather<<<loop_gather_grid(j, k), 256, 0, c->stream>>>((const unsigned char*)c->kf_arena.p, loop_rows<Row>(j, k), j.rows[k],
+                                                                           stride, (unsigned char*)c->bmap_raw.p);
         LILI_TRY(launch_check(c, "k_kf_gather"));
         LILI_TRY(voxelgrid_dev_sync(c, c->bmap_raw.p, (int)j.off[k], stride, j.leaf, c->vg_out.p, cnt, nullptr, &j.m[k]));
     }
     return repack_to_f4(c, c->vg_out.p, (int)j.off[k], stride, loop_dst(c, k), cnt);
+}
+
+// The solo call after loop_begin / its multi-store form's validation: both clouds, the target's cell grid, the ICP
+template <class Row>
+static int loop_run(LoopJob& j, double T16[16], double* fitness, int* converged, int* iters, int* n_src, int* n_tgt) {
+    liliom_ctx* c = j.c;
+    LILI_TRY(loop_cloud<Row>(j, 0));      // :2502-2547 his_key_frames_ds -> the loop index's points (float4, w = index)
+    LILI_TRY(loop_cloud<Row>(j, 1));      // :2476-2497 latest_key_frames_ds -> the source
+    if (n_src) *n_src = j.m[1];
+    if (n_tgt) *n_tgt = j.m[0];
+    LILI_TRY(grid_build(c, c->loop, loop_cell(c), j.m[0]));
+    return icp_align(c, c->loop, c->loop_src.as<float4>(), j.m[1], j.max_corr_dist, j.max_iter, j.trans_eps, j.fit_eps, T16, fitness,
+                     converged, iters);
 }
 
 static int loop_icp_begin(LoopJob& j) {
@@ -1122,12 +1226,7 @@ extern "C" int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double
     if (!c || !T16 || !fitness || !converged || !iters) return LILIOM_E_ARG;
     LoopJob j;
     LILI_TRY(loop_begin(c, src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter, trans_eps, fit_eps, j));
-    LILI_TRY(loop_cloud(j, 0));      // :2502-2547 his_key_frames_ds -> the loop index's points (float4, w = index)
-    LILI_TRY(loop_cloud(j, 1));      // :2476-2497 latest_key_frames_ds -> the source
-    if (n_src) *n_src = j.m[1];
-    if (n_tgt) *n_tgt = j.m[0];
-    LILI_TRY(grid_build(c, c->loop, loop_cell(c), j.m[0]));
-    return icp_align(c, c->loop, c->loop_src.as<float4>(), j.m[1], max_corr_dist, max_iter, trans_eps, fit_eps, T16, fitness, converged, iters);
+    return loop_run<KfRow>(j, T16, fitness, converged, iters, n_src, n_tgt);
 }
 
 extern "C" int liliom_loop_align_batch(liliom_ctx* const* ctxs, int B, const int* const* src_ids, const double* const* src_poses7,
@@ -1178,50 +1277,95 @@ extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp
     return LILIOM_OK;
 }
 
+namespace lili {
+
+// Every listed keyframe of kind LILIOM_KF_FULL has its full cloud (ids known to their stores)
+static bool kf_full_ok(liliom_ctx* c, KfStores s, int kind, const int* kf_ids, int k) {
+    for (int i = 0; i < k && kind == LILIOM_KF_FULL; ++i)
+        if (s[i]->kfs[kf_ids[i]].n_full < 0) {
+            c->last_error = "keyframe " + std::to_string(kf_ids[i]) + " has no full cloud (liliom_kf_add_full)";
+            if (s.per) c->last_error += " in store " + std::to_string(i);
+            return false;
+        }
+    return true;
+}
+
+// The multi-store calls' lists: every store there, on c's device, of c's point layout and without a communicator, every id known
+// to its store.  Nothing changes on an error.
+static bool kf_stores_ok(liliom_ctx* c, liliom_ctx* const* stores, const int* kf_ids, int k) {
+    for (int i = 0; i < k; ++i) {
+        const liliom_ctx* st = stores[i];
+        const char* why = !st ? "is NULL"
+                        : st->device != c->device ? "is on another device"
+                        : st->prm.point_stride != c->prm.point_stride ? "has another point_stride"
+                        : st->nranks > 1 ? "has a communicator: the backend keyframe store is single-GPU" : nullptr;
+        if (why) { c->last_error = "store of entry " + std::to_string(i) + " " + why; return false; }
+        if (kf_ids[i] < 0 || kf_ids[i] >= (int)st->kfs.size()) {
+            c->last_error = "unknown keyframe id " + std::to_string(kf_ids[i]) + " in the store of entry " + std::to_string(i) + " (" +
+                            std::to_string(st->kfs.size()) + " stored)";
+            return false;
+        }
+    }
+    return true;
+}
+
+// The stores' work so far before c's reads of their arenas (as liliom_kf_add_resident joins its source): each distinct stream once
+static int kf_join_stores(liliom_ctx* c, std::initializer_list<std::pair<liliom_ctx* const*, int>> lists) {
+    std::vector<liliom_ctx*> v;
+    for (const auto& l : lists)
+        for (int i = 0; i < l.second; ++i)
+            if (std::find(v.begin(), v.end(), l.first[i]) == v.end()) v.push_back(l.first[i]);
+    return batch_join_in(c, v);
+}
+
+// The sort chain's values and PCL's indices are ints
+static int kf_points_ok(liliom_ctx* c, long long N) {
+    if (N < (1LL << 31)) return LILIOM_OK;
+    c->last_error = "the listed keyframes hold " + std::to_string(N) + " points (at most 2^31 - 1)";
+    return LILIOM_E_CAPACITY;
+}
+
+// The global map's table (:2652-2662 list order, one cloud per keyframe): the stored cloud of `kind` of every entry, transformed by
+// pre7s + pre_step * i (none when pre7s is null; pre_step 0: one for every entry) and then by its pose.  Returns the points.
+template <class Row>
+static long long gmap_rows(KfStores s, int kind, const int* kf_ids, const double* poses7, int k, const double* pre7s, size_t pre_step,
+                           std::vector<Row>& tab, long long* largest) {
+    long long N = 0;
+    *largest = 0;
+    for (int i = 0; i < k; ++i) {
+        const KfEntry& f = s[i]->kfs[kf_ids[i]];
+        const DevBuf& arena = kind == LILIOM_KF_FULL ? s[i]->kf_full : s[i]->kf_arena;
+        const long long off = kind == LILIOM_KF_FULL ? f.full_off : f.surf_off;
+        const int m = kind == LILIOM_KF_FULL ? f.n_full : f.n_surf;
+        if (m) tab.push_back(kf_row_in<Row>(arena, off, N, m, poses7 + 7 * (size_t)i, pre7s ? pre7s + pre_step * i : nullptr));
+        N += m;
+        *largest = std::max(*largest, (long long)m);
+    }
+    return N;
+}
+
 // The global map without a concatenation buffer: box, voxel keys and centroids read the stored clouds through the keyframe table
 // and transform every point on load (kf_table.h); the sort chain in between is voxelgrid_dev's (the sort at the key width of the
 // box, k_vg_heads, the scan).  Device memory: the table, 16 bytes per listed point for keys and values (sort included; 24 with
 // the wide keys), and
 // the output; only PCL's declined case writes the transformed concatenation, which is then the output.
-extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, const double* poses7, int k, const double pre7[7],
-                                 float leaf, void* out, int cap, int* n) {
-    if (!c || !n || k < 0 || (k > 0 && (!kf_ids || !poses7)) || (kind != LILIOM_KF_FULL && kind != LILIOM_KF_SURF) || !(leaf > 0))
-        return LILIOM_E_ARG;
-    LILI_TRY(backend_check(c, nullptr));
-    if (!kf_ids_ok(c, kf_ids, k)) return LILIOM_E_ARG;
-    for (int i = 0; i < k && kind == LILIOM_KF_FULL; ++i)
-        if (c->kfs[kf_ids[i]].n_full < 0) {
-            c->last_error = "keyframe " + std::to_string(kf_ids[i]) + " has no full cloud (liliom_kf_add_full)";
-            return LILIOM_E_ARG;
-        }
-    const int stride = c->prm.point_stride;
-    std::vector<KfRow> tab;
-    long long N = 0, largest = 0;
-    for (int i = 0; i < k; ++i) {                                 // :2652-2662 list order, one cloud per keyframe
-        const KfEntry& f = c->kfs[kf_ids[i]];
-        const long long off = kind == LILIOM_KF_FULL ? f.full_off : f.surf_off;
-        const int m = kind == LILIOM_KF_FULL ? f.n_full : f.n_surf;
-        if (m) tab.push_back(kf_row(off, N, m, poses7 + 7 * (size_t)i, pre7));
-        N += m;
-        largest = std::max(largest, (long long)m);
-    }
-    if (N >= (1LL << 31)) {                                       // the sort chain's values and PCL's indices are ints
-        c->last_error = "the listed keyframes hold " + std::to_string(N) + " points (at most 2^31 - 1)";
-        return LILIOM_E_CAPACITY;
-    }
+// arena: the store KfRow rows read (KfRowM rows name their own); N <= 2^31 - 1 points (kf_points_ok).
+template <class Row>
+static int gmap_run(liliom_ctx* c, const unsigned char* arena, const std::vector<Row>& tab, long long N, long long largest, float leaf,
+                    void* out, int cap, int* n) {
     if (N == 0) { *n = 0; return LILIOM_OK; }
     LILI_CUDA(c, cudaSetDevice(c->device));
-    const unsigned char* arena = (const unsigned char*)(kind == LILIOM_KF_FULL ? c->kf_full.p : c->kf_arena.p);
+    const int stride = c->prm.point_stride;
     const int rows = (int)tab.size();
     LILI_TRY(kf_upload_table(c, tab));
-    const KfRow* d_tab = c->kf_tab.as<KfRow>();
+    const Row* d_tab = c->kf_tab.as<Row>();
     // box of the transformed concatenation (pcl::getMinMax3D), read back: the overflow test and the key width are decided here
     LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
     int* mm = c->vg_minmax.as<int>();
     int* empty = reinterpret_cast<int*>(c->h_pin->scratch);       // pinned staging of the empty box; the stream orders the read-back after it
     for (int w = 0; w < kBoxInts; ++w) empty[w] = vg_box_empty(w);
     LILI_CUDA(c, cudaMemcpyAsync(mm, empty, kBoxInts * sizeof(int), cudaMemcpyHostToDevice, c->stream));
-    k_kf_box<<<kf_row_grid(tab.size(), largest, 8, 1024), 256, 0, c->stream>>>(arena, d_tab, rows, stride, mm);
+    KfKern<Row>::box<<<kf_row_grid(tab.size(), largest, 8, 1024), 256, 0, c->stream>>>(arena, d_tab, rows, stride, mm);
     LILI_TRY(launch_check(c, "k_kf_box"));
     int box[kBoxInts];
     LILI_TRY(read_back(c, {{box, mm, sizeof(box)}}));
@@ -1244,7 +1388,8 @@ extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, con
     LILI_CUDA(c, c->vg_rank.ensure(((size_t)n_fin + 2) * 4));
     auto chain = [&](auto* keys, auto* keys2) -> int {
         using K = std::remove_pointer_t<decltype(keys)>;
-        k_kf_keys<K><<<kf_row_grid(tab.size(), largest, 8), 256, 0, c->stream>>>(arena, d_tab, rows, stride, p, keys, c->vg_vals.as<int>());
+        const auto k_keys = KfKern<Row>::template keys<K>;
+        k_keys<<<kf_row_grid(tab.size(), largest, 8), 256, 0, c->stream>>>(arena, d_tab, rows, stride, p, keys, c->vg_vals.as<int>());
         LILI_TRY(launch_check(c, "k_kf_keys"));
         // non-finite points carry the sentinel key and sort last: the first n_fin sorted entries are the finite points
         if constexpr (sizeof(K) == 4) LILI_TRY(sort_pairs_u32(c, keys, keys2, c->vg_vals.as<int>(), c->vg_vals2.as<int>(), (int)N, key_bits));
@@ -1257,15 +1402,68 @@ extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, con
         return download_sized(c, c->vg_out, m, stride, out, cap, n, [&]() -> int {
             c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
             LILI_CUDA(c, c->vg_out.ensure((size_t)m * stride));
-            if (stride == 48)
-                k_kf_centroid<48, K><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, keys2, c->vg_vals2.as<int>(), c->vg_flags.as<int>(),
-                                                                              c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
-            else
-                k_kf_centroid<32, K><<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, keys2, c->vg_vals2.as<int>(), c->vg_flags.as<int>(),
-                                                                              c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
+            const auto k_centroid = stride == 48 ? KfKern<Row>::template centroid<48, K> : KfKern<Row>::template centroid<32, K>;
+            k_centroid<<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, keys2, c->vg_vals2.as<int>(), c->vg_flags.as<int>(),
+                                                                c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
             return launch_check(c, "k_kf_centroid");
         });
     };
     if (key_bits > 32) return chain(c->vg_keys.as<unsigned long long>(), c->vg_keys2.as<unsigned long long>());
     return chain(c->vg_keys.as<uint32_t>(), c->vg_keys2.as<uint32_t>());
+}
+
+}  // namespace lili
+
+extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, const double* poses7, int k, const double pre7[7],
+                                 float leaf, void* out, int cap, int* n) {
+    if (!c || !n || k < 0 || (k > 0 && (!kf_ids || !poses7)) || (kind != LILIOM_KF_FULL && kind != LILIOM_KF_SURF) || !(leaf > 0))
+        return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, nullptr));
+    if (!kf_ids_ok(c, kf_ids, k) || !kf_full_ok(c, KfStores{c}, kind, kf_ids, k)) return LILIOM_E_ARG;
+    std::vector<KfRow> tab;
+    long long largest = 0;
+    const long long N = gmap_rows(KfStores{c}, kind, kf_ids, poses7, k, pre7, 0, tab, &largest);
+    LILI_TRY(kf_points_ok(c, N));
+    const unsigned char* arena = (const unsigned char*)(kind == LILIOM_KF_FULL ? c->kf_full.p : c->kf_arena.p);
+    return gmap_run(c, arena, tab, N, largest, leaf, out, cap, n);
+}
+
+// liliom_global_map over keyframes of several stores: rows that name their store's arena, the rest unchanged on c
+extern "C" int liliom_global_map_multi(liliom_ctx* c, int kind, liliom_ctx* const* stores, const int* kf_ids, const double* poses7, int k,
+                                       const double* pre7s, float leaf, void* out, int cap, int* n) {
+    if (!c || !n || k < 0 || (k > 0 && (!stores || !kf_ids || !poses7)) || (kind != LILIOM_KF_FULL && kind != LILIOM_KF_SURF) || !(leaf > 0))
+        return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, nullptr));
+    if (!kf_stores_ok(c, stores, kf_ids, k) || !kf_full_ok(c, KfStores{c, stores}, kind, kf_ids, k)) return LILIOM_E_ARG;
+    std::vector<KfRowM> tab;
+    long long largest = 0;
+    const long long N = gmap_rows(KfStores{c, stores}, kind, kf_ids, poses7, k, pre7s, 7, tab, &largest);
+    LILI_TRY(kf_points_ok(c, N));
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    LILI_TRY(kf_join_stores(c, {{stores, k}}));
+    return gmap_run(c, (const unsigned char*)c->kf_arena.p, tab, N, largest, leaf, out, cap, n);
+}
+
+// liliom_loop_align over keyframes of several stores: both clouds' rows name their store's arena, the rest unchanged on c
+extern "C" int liliom_loop_align_multi(liliom_ctx* c, liliom_ctx* const* src_stores, const int* src_ids, const double* src_poses7, int k_src,
+                                       liliom_ctx* const* tgt_stores, const int* tgt_ids, const double* tgt_poses7, int k_tgt, float leaf,
+                                       double max_corr_dist, int max_iter, double trans_eps, double fit_eps, double T16[16], double* fitness,
+                                       int* converged, int* iters, int* n_src, int* n_tgt) {
+    if (!c || !T16 || !fitness || !converged || !iters) return LILIOM_E_ARG;
+    if (!loop_args_ok(src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter) || (k_src > 0 && !src_stores) ||
+        (k_tgt > 0 && !tgt_stores))
+        return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, nullptr));
+    if (!kf_stores_ok(c, src_stores, src_ids, k_src) || !kf_stores_ok(c, tgt_stores, tgt_ids, k_tgt)) return LILIOM_E_ARG;
+    for (const auto& [st, ids, k] : {std::make_tuple(src_stores, src_ids, k_src), std::make_tuple(tgt_stores, tgt_ids, k_tgt)}) {
+        long long N = 0;
+        for (int i = 0; i < k; ++i) N += (long long)st[i]->kfs[ids[i]].n_edge + st[i]->kfs[ids[i]].n_surf;
+        LILI_TRY(kf_points_ok(c, N));
+    }
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    LILI_TRY(kf_join_stores(c, {{src_stores, k_src}, {tgt_stores, k_tgt}}));
+    LoopJob j;
+    LILI_TRY(loop_tables<KfRowM>(c, KfStores{c, src_stores}, src_ids, src_poses7, k_src, KfStores{c, tgt_stores}, tgt_ids, tgt_poses7, k_tgt,
+                                 leaf, max_corr_dist, max_iter, trans_eps, fit_eps, j));
+    return loop_run<KfRowM>(j, T16, fitness, converged, iters, n_src, n_tgt);
 }

@@ -5,14 +5,23 @@
 //   * the global map's VoxelGrid (liliom_global_map) measures its box and its voxel keys from kf_row_xyz and sums its centroids
 //     through KfRowLoader, which finds a member's row by binary search over dst_off.
 // The three transforms of a point (box, key, centroid) are the same code, so they give the same bits.
+// Two row types: KfRow reads the one arena its kernel is given (one context's store), KfRowM carries its own arena (the calls
+// over keyframes of several stores, liliom_global_map_multi / liliom_loop_align_multi).  kf_row_src gives either's stored point.
 #pragma once
 #include "pcl_xform.h"
+#include <type_traits>
 
 namespace lili {
 
 // n points of the arena from src_off (in points) -> dst_off of the concatenation: transformed by (pq, pt) when `pre` is set (the
 // intermediate point stored in fp32, as the pcl::PointCloud in between holds it), then by (q, t).
 struct KfRow { long long src_off, dst_off; Q4 q; D3 t; Q4 pq; D3 pt; int n, pre; };
+// ... whose points lie in `base` (its store's arena) instead of the kernel's arena
+struct KfRowM : KfRow { const unsigned char* base; };
+
+// point j (an index into its arena: r.src_off + the point's index in the row) of the arena row r reads, stride bytes each
+VGB_HD const unsigned char* kf_row_src(const KfRow&, const unsigned char* arena, int stride, long long j) { return arena + (size_t)j * stride; }
+VGB_HD const unsigned char* kf_row_src(const KfRowM& r, const unsigned char*, int stride, long long j) { return r.base + (size_t)j * stride; }
 
 // the transformed xyz of a stored point of row r
 VGB_HD VgXyz kf_row_xyz(const KfRow& r, const unsigned char* src) {
@@ -34,7 +43,8 @@ VGB_HD void kf_row_point(const KfRow& r, const unsigned char* src, int stride, u
 }
 
 // the row holding concatenation index i: the last row with dst_off <= i (rows in ascending dst_off, none empty)
-VGB_HD int kf_row_of(const KfRow* tab, int rows, long long i) {
+template <class Row>
+VGB_HD int kf_row_of(const Row* tab, int rows, long long i) {
     int lo = 0, hi = rows - 1;
     while (lo < hi) {
         const int mid = (lo + hi + 1) >> 1;
@@ -44,16 +54,18 @@ VGB_HD int kf_row_of(const KfRow* tab, int rows, long long i) {
     return lo;
 }
 
-// vg_walk's loader over the table: the fields of concatenation index m, transformed on load
-template <int STRIDE>
+// vg_walk's loader over the table: the fields of concatenation index m, transformed on load (arena: KfRow's, unused by KfRowM)
+template <int STRIDE, class Row = KfRow>
 struct KfRowLoader {
     const unsigned char* arena;
-    const KfRow* tab;
+    const Row* tab;
     int rows;
     VGB_HD void operator()(int m, float* f) const {
-        const KfRow& r = tab[kf_row_of(tab, rows, m)];
+        const Row& r = tab[kf_row_of(tab, rows, m)];
         alignas(16) unsigned char p[STRIDE];
-        kf_row_point(r, arena + (size_t)(r.src_off + (m - r.dst_off)) * STRIDE, STRIDE, p);
+        // KfRow's address spelled out: through kf_row_src ptxas allocates the 32-byte kernels' registers differently
+        if constexpr (std::is_same<Row, KfRow>::value) kf_row_point(r, arena + (size_t)(r.src_off + (m - r.dst_off)) * STRIDE, STRIDE, p);
+        else kf_row_point(r, kf_row_src(r, arena, STRIDE, r.src_off + (m - r.dst_off)), STRIDE, p);
         vg_load<STRIDE>(p, f);
     }
 };
