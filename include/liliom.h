@@ -290,6 +290,23 @@ int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp, const int*
  * repeated context, contexts on different devices, a context with a communicator. */
 int liliom_bmap_build_batch(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps, const int* const* kf_ids,
                             const double* const* poses7, const int* k, int* n_edge_map, int* n_surf_map, int* status);
+/* liliom_bmap_build_multi of B independent sessions in one call (a fleet tracking in a shared prior map).  stores: B per-session
+ * arrays, stores[i][e] the store of session i's entry e (liliom_bmap_build_multi's stores); the other arguments as
+ * liliom_bmap_build_batch.  Session i gets exactly what liliom_bmap_build_multi(ctxs[i], &bps[i], stores[i], kf_ids[i], poses7[i],
+ * k[i], &n_edge_map[i], &n_surf_map[i]) would give it, bit for bit, with everything liliom_bmap_build_batch promises (status,
+ * liliom_last_error, counts, layers, cell grids, reflectivity, launches and lib_launches, everything else on ctxs[i] left alone),
+ * so that solo and batched calls mix freely.  Launches and waits as liliom_bmap_build_batch; the gather of every session reads the
+ * stores' arenas where they lie.  A session whose voxel index wraps finishes on its solo multi-store path inside the call.
+ * Stores: a store may be any backend context on the device: a session's own caller, another session's caller in the same batch, or
+ * one store shared by every session.  They are only read.  The streams of every caller and of every distinct store of a running
+ * session are joined into ctxs[0]'s stream with events before the first read; the call returns with every read done.  No other
+ * host thread may call into a store during the call.
+ * A session's own error (every error its solo call returns: a NULL stores[i] or store, a store on another device, of another
+ * point_stride or with a communicator, an id unknown to its store, and every liliom_bmap_build_batch session error) is its status;
+ * the others run.  LILIOM_E_ARG for the whole call, nothing changed: as liliom_bmap_build_batch, and a NULL stores. */
+int liliom_bmap_build_batch_multi(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps, liliom_ctx* const* const* stores,
+                                  const int* const* kf_ids, const double* const* poses7, const int* k, int* n_edge_map, int* n_surf_map,
+                                  int* status);
 /* edge_local_map_ds (layer 0) / surf_local_map_ds (layer 1) with all fields (published on every run, :1516-1526).
  * out = NULL: *m = size only. */
 int liliom_bmap_download(liliom_ctx* c, int layer, void* out, int cap, int* m);
@@ -406,6 +423,17 @@ int liliom_loop_align_multi(liliom_ctx* c, liliom_ctx* const* src_stores, const 
                             liliom_ctx* const* tgt_stores, const int* tgt_ids, const double* tgt_poses7, int k_tgt, float leaf,
                             double max_corr_dist, int max_iter, double trans_eps, double fit_eps,
                             double T16[16], double* fitness, int* converged, int* iters, int* n_src, int* n_tgt);
+/* liliom_bmap_build over keyframes of several stores: entry i = keyframe kf_ids[i] of stores[i], placed by poses7[7i..].  The
+ * result is bit for bit liliom_bmap_build on a context D whose store holds the same clouds, called with the mapped list: status,
+ * both counts, both layers (liliom_bmap_download), both cell grids and the Horizon layer's reflectivity as every later
+ * liliom_backend_window_correspond / _blocks on c sees them; with every entry naming c, liliom_bmap_build on c.  A store may be any
+ * backend context on c's device: c itself, another session's, or a prior run's store that several sessions share (a fleet tracking
+ * in a prior map).  The stores are only read; each distinct store stream is joined into c's stream with an event before the first
+ * read, and the call returns with every read done.  No other host thread may call into a store during the call.
+ * LILIOM_E_ARG, nothing changed (the previous layers stay downloadable): a NULL array or store (k > 0), a store on another device,
+ * of another point_stride or with a communicator, an id unknown to its store, and whatever liliom_bmap_build refuses. */
+int liliom_bmap_build_multi(liliom_ctx* c, const liliom_backend_params* bp, liliom_ctx* const* stores, const int* kf_ids,
+                            const double* poses7, int k, int* n_edge_map, int* n_surf_map);
 
 /* ---- SURVEY §8 (f3): wire format on the sensor side — FormatConvert's livoxLidarHandler on the device ----
  * L/src/FormatConvert.cpp:11-24: livox_ros_driver::CustomPoint {uint32 offset_time; float x,y,z; uint8 reflectivity,
@@ -787,6 +815,20 @@ typedef struct { double T16[16]; double fitness; int converged, iters, n_src, n_
 int liliom_loop_align_batch(liliom_ctx* const* ctxs, int B, const int* const* src_ids, const double* const* src_poses7, const int* k_src,
                             const int* const* tgt_ids, const double* const* tgt_poses7, const int* k_tgt,
                             const liliom_loop_params* prm, liliom_loop_result* res, int* status);
+/* liliom_loop_align_multi of B independent sessions in one call (many inter-robot or prior-map loop candidates at once).
+ * src_stores, tgt_stores: B per-session arrays (liliom_loop_align_multi's stores); the other arguments as liliom_loop_align_batch.
+ * Session i gets exactly what liliom_loop_align_multi(ctxs[i], src_stores[i], src_ids[i], src_poses7[i], k_src[i], tgt_stores[i],
+ * tgt_ids[i], tgt_poses7[i], k_tgt[i], prm[i]..., res[i]...) would give it, bit for bit, with everything liliom_loop_align_batch
+ * promises (status, results, liliom_last_error, launches and lib_launches, the state left in ctxs[i]); launches and waits as
+ * liliom_loop_align_batch.  Stores as liliom_bmap_build_batch_multi: any backend context on the device, only read, every distinct
+ * store stream joined into ctxs[0]'s stream before the first read, every read done when the call returns, no other host thread
+ * calling into a store meanwhile.  A session's own error (every error its solo call returns, the stores' included) is its status;
+ * the others run.  LILIOM_E_ARG for the whole call, nothing changed: as liliom_loop_align_batch, and a NULL src_stores or
+ * tgt_stores. */
+int liliom_loop_align_batch_multi(liliom_ctx* const* ctxs, int B, liliom_ctx* const* const* src_stores, const int* const* src_ids,
+                                  const double* const* src_poses7, const int* k_src, liliom_ctx* const* const* tgt_stores,
+                                  const int* const* tgt_ids, const double* const* tgt_poses7, const int* k_tgt,
+                                  const liliom_loop_params* prm, liliom_loop_result* res, int* status);
 
 #ifdef __cplusplus
 }

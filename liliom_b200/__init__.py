@@ -12,7 +12,7 @@ from ._lib import (Context, Params, IterStats, Counters, LiliomError, default_pa
                    scan_to_map_resident_batch_ex, odometry_resident_batch_ex, extract_resident_batch, map_update_batch,
                    backend_window_correspond_batch, backend_window_blocks_batch, loop_align_batch, LoopParams, LoopResult,
                    convert_batch, WireMsg, WIRE_LIVOX, WIRE_PC2, undistort_resident_batch, kf_add_resident_batch,
-                   bmap_build_batch)
+                   bmap_build_batch, bmap_build_batch_multi, loop_align_batch_multi)
 
 __all__ = ["Context", "Params", "IterStats", "Counters", "LiliomError", "default_params", "comm_get_unique_id",
            "PT48", "PT32", "MODE_CERES", "MODE_GN", "LIB_PATH", "EXPORTS",
@@ -21,4 +21,4 @@ __all__ = ["Context", "Params", "IterStats", "Counters", "LiliomError", "default
            "scan_to_map_resident_batch_ex", "odometry_resident_batch_ex", "extract_resident_batch", "map_update_batch",
            "backend_window_correspond_batch", "backend_window_blocks_batch", "loop_align_batch", "LoopParams", "LoopResult",
            "convert_batch", "WireMsg", "WIRE_LIVOX", "WIRE_PC2", "undistort_resident_batch", "kf_add_resident_batch",
-           "bmap_build_batch"]
+           "bmap_build_batch", "bmap_build_batch_multi", "loop_align_batch_multi"]

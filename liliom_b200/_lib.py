@@ -97,6 +97,7 @@ EXPORTS = [
     "liliom_loop_align_batch", "liliom_convert_batch", "liliom_undistort_resident", "liliom_kf_add_resident",
     "liliom_undistort_resident_batch", "liliom_kf_add_resident_batch", "liliom_bmap_build_batch",
     "liliom_global_map_multi", "liliom_loop_align_multi",
+    "liliom_bmap_build_multi", "liliom_bmap_build_batch_multi", "liliom_loop_align_batch_multi",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -265,6 +266,12 @@ def lib() -> C.CDLL:
                                           C.c_int, C.c_double, C.c_double, dp, dp, ip, ip, ip, ip]
     L.liliom_loop_align_batch.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(ip), C.POINTER(dp), ip, C.POINTER(ip), C.POINTER(dp), ip,
                                           C.POINTER(LoopParams), C.POINTER(LoopResult), ip]
+    L.liliom_bmap_build_multi.argtypes = [vp, bpp, C.POINTER(vp), ip, dp, C.c_int, ip, ip]
+    L.liliom_bmap_build_batch_multi.argtypes = [C.POINTER(vp), C.c_int, bpp, C.POINTER(C.POINTER(vp)), C.POINTER(ip), C.POINTER(dp), ip, ip,
+                                                ip, ip]
+    L.liliom_loop_align_batch_multi.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(C.POINTER(vp)), C.POINTER(ip), C.POINTER(dp), ip,
+                                                C.POINTER(C.POINTER(vp)), C.POINTER(ip), C.POINTER(dp), ip, C.POINTER(LoopParams),
+                                                C.POINTER(LoopResult), ip]
     L.liliom_convert_batch.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(WireMsg), C.POINTER(vp), ip, ip, ip]
     L.liliom_pre_create.argtypes = [vp, C.c_int, dp]; L.liliom_pre_create.restype = vp
     L.liliom_pre_destroy.argtypes = [vp]; L.liliom_pre_destroy.restype = None
@@ -624,6 +631,17 @@ class Context:
         ne, ns = C.c_int(), C.c_int()
         self._check(lib().liliom_bmap_build(self._h, C.byref(bp), ids.ctypes.data_as(C.POINTER(C.c_int)), _dptr(p), len(ids),
                                             C.byref(ne), C.byref(ns)))
+        return ne.value, ns.value
+
+    def bmap_build_multi(self, bp: BackendParams, stores, kf_ids, poses7):
+        """bmap_build over keyframes of several stores (liliom_bmap_build_multi): entry i is keyframe kf_ids[i] of the Context
+        stores[i], placed by poses7[i]; the layers and their cell grids on this context, the stores only read.  Returns
+        (edge layer size, surf layer size)."""
+        ids = _ids(kf_ids); k = len(ids); p = _poses(poses7, k)
+        assert len(stores) == k
+        ne, ns = C.c_int(), C.c_int()
+        self._check(lib().liliom_bmap_build_multi(self._h, C.byref(bp), _handles(stores), ids.ctypes.data_as(C.POINTER(C.c_int)), _dptr(p),
+                                                  k, C.byref(ne), C.byref(ns)))
         return ne.value, ns.value
 
     def bmap_download(self, layer: int) -> np.ndarray:
@@ -1144,6 +1162,66 @@ def bmap_build_batch(ctxs, bps, kf_ids, poses7):
     if rc != OK:
         raise LiliomError(rc)
     return np.stack([ne, ns], axis=1)[:B], status[:B]
+
+
+def _store_lists(lists):
+    """A C array of B per-session store arrays (a None entry is a NULL array, a None store a NULL store) and the arrays to keep
+    alive while it is used."""
+    arrs = [_handles(x) if x is not None else None for x in lists]
+    P = C.POINTER(C.c_void_p)
+    return (P * max(len(arrs), 1))(*[C.cast(a, P) if a is not None else P() for a in arrs]), arrs
+
+
+def bmap_build_batch_multi(ctxs, bps, stores, kf_ids, poses7):
+    """bmap_build_multi of every context in `ctxs` in one call (liliom_bmap_build_batch_multi): session i gets what
+    ctxs[i].bmap_build_multi(bps[i], stores[i], kf_ids[i], poses7[i]) would give it.  stores: B sequences of Contexts (one per
+    entry; a store may be any session's caller or one store shared by all); the rest as bmap_build_batch.  Returns (counts (B, 2),
+    status (B,)); a session's own error is its status, a whole-call error raises LiliomError."""
+    B = len(ctxs)
+    if len(bps) != B or len(stores) != B or len(kf_ids) != B or len(poses7) != B:
+        raise ValueError(f"expected {B} per-session parameters, store lists, id lists and pose lists")
+    bparr = (BackendParams * max(B, 1))(*bps)
+    st, _keep = _store_lists(stores)
+    ids = [_ids(x) if x is not None else None for x in kf_ids]
+    k = np.array([len(x) if x is not None else 1 for x in ids] + [0], np.int32)
+    poses = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1) if p is not None else None for p in poses7]
+    ne = np.zeros(max(B, 1), np.int32)
+    ns = np.zeros(max(B, 1), np.int32)
+    status = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_bmap_build_batch_multi(_handles(ctxs), B, bparr, st, _ptrs(ids, C.c_int), _ptrs(poses, C.c_double), _ip(k), _ip(ne),
+                                             _ip(ns), _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    return np.stack([ne, ns], axis=1)[:B], status[:B]
+
+
+def loop_align_batch_multi(ctxs, src_stores, src_ids, src_poses, tgt_stores, tgt_ids, tgt_poses, params):
+    """loop_align_multi of every context in `ctxs` in one call (liliom_loop_align_batch_multi): session i gets what
+    ctxs[i].loop_align_multi(src_stores[i], src_ids[i], src_poses[i], tgt_stores[i], tgt_ids[i], tgt_poses[i], **params[i])
+    would give it.  src_stores, tgt_stores: B sequences of Contexts, one per entry; the rest as loop_align_batch.  Returns
+    loop_align_batch's (results, status)."""
+    B = len(ctxs)
+    if (len(src_stores) != B or len(src_ids) != B or len(src_poses) != B or len(tgt_stores) != B or len(tgt_ids) != B or
+            len(tgt_poses) != B or len(params) != B):
+        raise ValueError(f"expected {B} per-session store lists, id lists, pose lists and settings")
+    ss, _keep_s = _store_lists(src_stores)
+    ts, _keep_t = _store_lists(tgt_stores)
+    si = [_ids(x) if x is not None else None for x in src_ids]
+    ti = [_ids(x) if x is not None else None for x in tgt_ids]
+    sp = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1) if p is not None else None for p in src_poses]
+    tp = [np.ascontiguousarray(p, dtype=np.float64).reshape(-1) if p is not None else None for p in tgt_poses]
+    ks = np.array([len(x) if x is not None else 0 for x in si] + [0], np.int32)
+    kt = np.array([len(x) if x is not None else 0 for x in ti] + [0], np.int32)
+    defaults = dict(max_corr_dist=30.0, max_iter=100, trans_eps=1e-6, fit_eps=1e-6)
+    prm = (LoopParams * max(B, 1))(*[LoopParams(**{**defaults, **p}) for p in params])
+    res = (LoopResult * max(B, 1))()
+    status = np.zeros(max(B, 1), np.int32)
+    rc = lib().liliom_loop_align_batch_multi(_handles(ctxs), B, ss, _ptrs(si, C.c_int), _ptrs(sp, C.c_double), _ip(ks), ts,
+                                             _ptrs(ti, C.c_int), _ptrs(tp, C.c_double), _ip(kt), prm, res, _ip(status))
+    if rc != OK:
+        raise LiliomError(rc)
+    out = [(np.array(r.T16[:], np.float64).reshape(4, 4), r.fitness, bool(r.converged), r.iters, r.n_src, r.n_tgt) for r in res[:B]]
+    return out, status[:B]
 
 
 def backend_window_correspond_batch(ctxs, bps, kf_ids, poses7_lidar):

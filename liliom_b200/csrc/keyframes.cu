@@ -206,37 +206,58 @@ static int kf_gather(liliom_ctx* c, const void* arena, const std::vector<Row>& t
     return launch_check(c, "k_kf_gather");
 }
 
-// a table row: n points from src -> dst, transformed by pre7 (optional) and then by pose7
-static KfRow kf_row(long long src, long long dst, int n, const double* pose7, const double* pre7 = nullptr) {
-    KfRow e{};
-    e.src_off = src; e.dst_off = dst; e.n = n;
-    e.q = Q4{pose7[0], pose7[1], pose7[2], pose7[3]};
-    e.t = D3{pose7[4], pose7[5], pose7[6]};
-    if (pre7) {
-        e.pre = 1;
-        e.pq = Q4{pre7[0], pre7[1], pre7[2], pre7[3]};
-        e.pt = D3{pre7[4], pre7[5], pre7[6]};
-    }
-    return e;
-}
-// ... of the table's row type: a KfRowM also names the arena its points lie in
-template <class Row> Row kf_row_in(const DevBuf& arena, long long src, long long dst, int n, const double* pose7, const double* pre7 = nullptr);
-template <> KfRow kf_row_in<KfRow>(const DevBuf&, long long src, long long dst, int n, const double* pose7, const double* pre7) {
-    return kf_row(src, dst, n, pose7, pre7);
-}
-template <> KfRowM kf_row_in<KfRowM>(const DevBuf& arena, long long src, long long dst, int n, const double* pose7, const double* pre7) {
-    KfRowM e{};
-    static_cast<KfRow&>(e) = kf_row(src, dst, n, pose7, pre7);
-    e.base = (const unsigned char*)arena.p;
-    return e;
-}
-
 // The store of each list entry: c for every entry (the single-store calls) or stores[i] (liliom_*_multi)
 struct KfStores {
     liliom_ctx* c;
     liliom_ctx* const* per = nullptr;
     liliom_ctx* operator[](int i) const { return per ? per[i] : c; }
 };
+
+// The multi-store calls' lists: every store there, on c's device, of c's point layout and without a communicator, every id known
+// to its store.  Nothing changes on an error.
+static bool kf_stores_ok(liliom_ctx* c, liliom_ctx* const* stores, const int* kf_ids, int k) {
+    for (int i = 0; i < k; ++i) {
+        const liliom_ctx* st = stores[i];
+        const char* why = !st ? "is NULL"
+                        : st->device != c->device ? "is on another device"
+                        : st->prm.point_stride != c->prm.point_stride ? "has another point_stride"
+                        : st->nranks > 1 ? "has a communicator: the backend keyframe store is single-GPU" : nullptr;
+        if (why) { c->last_error = "store of entry " + std::to_string(i) + " " + why; return false; }
+        if (kf_ids[i] < 0 || kf_ids[i] >= (int)st->kfs.size()) {
+            c->last_error = "unknown keyframe id " + std::to_string(kf_ids[i]) + " in the store of entry " + std::to_string(i) + " (" +
+                            std::to_string(st->kfs.size()) + " stored)";
+            return false;
+        }
+    }
+    return true;
+}
+
+// The ids of a list: known to c's own store (KfRow) or each to its entry's store (KfRowM, kf_stores_ok).  Nothing changes on an error.
+template <class Row>
+static bool kf_list_ok(liliom_ctx* c, liliom_ctx* const* stores, const int* kf_ids, int k) {
+    if constexpr (std::is_same<Row, KfRowM>::value) return kf_stores_ok(c, stores, kf_ids, k);
+    else return kf_ids_ok(c, kf_ids, k);
+}
+
+// The distinct stores of the lists, in order of first appearance, appended to v (each once)
+static void kf_add_stores(std::vector<liliom_ctx*>& v, liliom_ctx* const* stores, int k) {
+    for (int i = 0; i < k; ++i)
+        if (std::find(v.begin(), v.end(), stores[i]) == v.end()) v.push_back(stores[i]);
+}
+
+// The stores' work so far before c's reads of their arenas (as liliom_kf_add_resident joins its source): each distinct stream once
+static int kf_join_stores(liliom_ctx* c, std::initializer_list<std::pair<liliom_ctx* const*, int>> lists) {
+    std::vector<liliom_ctx*> v;
+    for (const auto& l : lists) kf_add_stores(v, l.first, l.second);
+    return batch_join_in(c, v);
+}
+
+// The sort chain's values and PCL's indices are ints
+static int kf_points_ok(liliom_ctx* c, long long N) {
+    if (N < (1LL << 31)) return LILIOM_OK;
+    c->last_error = "the listed keyframes hold " + std::to_string(N) + " points (at most 2^31 - 1)";
+    return LILIOM_E_CAPACITY;
+}
 
 // detectLoopClosure's cloud of the listed keyframes (:2476-2497, :2502-2547): edge then surf of each, transformed by its pose,
 // concatenated into bmap_raw (one launch), VoxelGrid(leaf) into vg_out with its count at d_count (device) and *m (host).
@@ -248,7 +269,7 @@ static long long kf_cloud_rows(KfStores s, const int* kf_ids, const double* pose
     *largest = 0;
     for (int i = 0; i < k; ++i) {                                 // :2492-2493 / :2519-2520: *edge_frames[i] then *surf_frames[i]
         const KfEntry& f = s[i]->kfs[kf_ids[i]];
-        const DevBuf& arena = s[i]->kf_arena;
+        const void* arena = s[i]->kf_arena.p;
         if (f.n_edge) tab.push_back(kf_row_in<Row>(arena, f.edge_off, off, f.n_edge, poses7 + 7 * (size_t)i));
         off += f.n_edge;
         if (f.n_surf) tab.push_back(kf_row_in<Row>(arena, f.surf_off, off, f.n_surf, poses7 + 7 * (size_t)i));
@@ -369,8 +390,9 @@ static void kf_res_finish(const KfResJob& j, int* kf_id, int* n_edge_ds, int* n_
     if (n_full_stored) *n_full_stored = j.mf;
 }
 
-// liliom_bmap_build in parts, run by the solo call and by the batch (liliom_bmap_build_batch): bmap_begin (validation, nothing
-// changes on an error; the keyframe table, uploaded, and the buffers of both layers), the gather of the table into bmap_raw, per
+// liliom_bmap_build in parts, run by the solo calls and by the batches (liliom_bmap_build(_batch)(_multi)): bmap_check (validation,
+// nothing changes on an error), bmap_tables (the keyframe table, uploaded, and the buffers of both layers), the gather of the table
+// into bmap_raw, per
 // layer voxelgrid_dev's chain into bmap_ds[l] and bmap[l].xyzw, each layer's cell grid, the surf layer's reflectivity (48-byte
 // points), bmap_finish (the counts).
 struct BmapJob {
@@ -393,29 +415,36 @@ static const unsigned char* bmap_in(const BmapJob& j, int l) {
 }
 static dim3 bmap_gather_grid(const BmapJob& j) { return kf_row_grid(j.rows, j.largest, j.c->sm_count * 4); }
 
-static int bmap_begin(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7, int k, BmapJob& j) {
-    if (k < 0 || (k > 0 && (!kf_ids || !poses7))) return LILIOM_E_ARG;
+// Validation, nothing changes on an error (the previous layers stay): the entries' keyframes are c's own (KfRow, stores unused)
+// or each of its entry's store (KfRowM, liliom_bmap_build_multi)
+template <class Row>
+static int bmap_check(liliom_ctx* c, const liliom_backend_params* bp, liliom_ctx* const* stores, const int* kf_ids, const double* poses7,
+                      int k) {
+    constexpr bool multi = std::is_same<Row, KfRowM>::value;
+    if (k < 0 || (k > 0 && (!kf_ids || !poses7 || (multi && !stores)))) return LILIOM_E_ARG;
     LILI_TRY(backend_check(c, bp));
-    if (!kf_ids_ok(c, kf_ids, k)) return LILIOM_E_ARG;           // before anything changes: the previous layers stay
+    return kf_list_ok<Row>(c, stores, kf_ids, k) ? LILIOM_OK : LILIOM_E_ARG;
+}
+
+// After bmap_check: the keyframe table (rows of the table's type, read from each entry's store), uploaded, and the buffers of both
+// layers.  Every call over either row type runs this one builder (kf_bmap_rows), largest-cloud rule and sizing.
+template <class Row>
+static int bmap_tables(liliom_ctx* c, const liliom_backend_params* bp, KfStores s, const int* kf_ids, const double* poses7, int k,
+                       BmapJob& j) {
     LILI_CUDA(c, cudaSetDevice(c->device));
     const int stride = c->prm.point_stride;
     c->bmap_built = false;
     j = BmapJob{};
     j.c = c; j.bp = bp;
-    long long E = 0, S = 0;
-    for (int i = 0; i < k; ++i) { const KfEntry& f = c->kfs[kf_ids[i]]; E += f.n_edge; S += f.n_surf; j.largest = std::max(j.largest, (long long)std::max(f.n_edge, f.n_surf)); }
-    std::vector<KfRow> tab;
-    tab.reserve(2 * (size_t)k);
-    long long de = 0, ds = E;
-    for (int i = 0; i < k; ++i) {                                 // :1479-1483 edge and surf layers, list order
-        const KfEntry& f = c->kfs[kf_ids[i]];
-        if (f.n_edge) tab.push_back(kf_row(f.edge_off, de, f.n_edge, poses7 + 7 * (size_t)i));
-        if (f.n_surf) tab.push_back(kf_row(f.surf_off, ds, f.n_surf, poses7 + 7 * (size_t)i));
-        de += f.n_edge; ds += f.n_surf;
-    }
+    std::vector<Row> tab;
+    kf_bmap_rows(
+        [&](int i) {
+            const KfEntry& f = s[i]->kfs[kf_ids[i]];
+            return KfClouds{s[i]->kf_arena.p, f.edge_off, f.surf_off, f.n_edge, f.n_surf};
+        },
+        poses7, k, tab, j.n, &j.largest);
     j.rows = (int)tab.size();
-    j.n[0] = E; j.n[1] = S;
-    LILI_CUDA(c, c->bmap_raw.ensure((size_t)std::max(E + S, 1LL) * stride));
+    LILI_CUDA(c, c->bmap_raw.ensure((size_t)std::max(j.n[0] + j.n[1], 1LL) * stride));
     if (j.rows > 0) LILI_TRY(kf_upload_table(c, tab));
     LILI_CUDA(c, c->vg_count.ensure(16));
     for (int l = 0; l < 2; ++l) {                                 // the centroid kernel also writes the float4 points
@@ -515,15 +544,17 @@ extern "C" int liliom_kf_clear(liliom_ctx* c) {
     return LILIOM_OK;
 }
 
-extern "C" int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7, int k,
-                                 int* n_edge_map, int* n_surf_map) {
-    if (!c || !bp) return LILIOM_E_ARG;
-    BmapJob j;
-    LILI_TRY(bmap_begin(c, bp, kf_ids, poses7, k, j));
+namespace lili {
+
+// The solo call after bmap_tables: the gather (of c's own arena, or of the arena each KfRowM row names), both layers' VoxelGrid
+// chains and cell grids, the reflectivity, one wait at the end
+template <class Row>
+static int bmap_run(BmapJob& j, int* n_edge_map, int* n_surf_map) {
+    liliom_ctx* c = j.c;
     const int stride = c->prm.point_stride;
     if (j.rows > 0) {
-        k_kf_gather<<<bmap_gather_grid(j), 256, 0, c->stream>>>((const unsigned char*)c->kf_arena.p, c->kf_tab.as<KfRow>(), j.rows, stride,
-                                                                (unsigned char*)c->bmap_raw.p);
+        KfKern<Row>::gather<<<bmap_gather_grid(j), 256, 0, c->stream>>>((const unsigned char*)c->kf_arena.p, c->kf_tab.as<Row>(), j.rows,
+                                                                        stride, (unsigned char*)c->bmap_raw.p);
         LILI_TRY(launch_check(c, "k_kf_gather"));
     }
     for (int l = 0; l < 2; ++l)                                   // :1486-1492
@@ -540,6 +571,29 @@ extern "C" int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp,
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     bmap_finish(j, n_edge_map, n_surf_map);
     return LILIOM_OK;
+}
+
+}  // namespace lili
+
+extern "C" int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7, int k,
+                                 int* n_edge_map, int* n_surf_map) {
+    if (!c || !bp) return LILIOM_E_ARG;
+    LILI_TRY(bmap_check<KfRow>(c, bp, nullptr, kf_ids, poses7, k));
+    BmapJob j;
+    LILI_TRY(bmap_tables<KfRow>(c, bp, KfStores{c}, kf_ids, poses7, k, j));
+    return bmap_run<KfRow>(j, n_edge_map, n_surf_map);
+}
+
+// liliom_bmap_build over keyframes of several stores: rows that name their store's arena, the rest unchanged on c
+extern "C" int liliom_bmap_build_multi(liliom_ctx* c, const liliom_backend_params* bp, liliom_ctx* const* stores, const int* kf_ids,
+                                       const double* poses7, int k, int* n_edge_map, int* n_surf_map) {
+    if (!c || !bp) return LILIOM_E_ARG;
+    LILI_TRY(bmap_check<KfRowM>(c, bp, stores, kf_ids, poses7, k));
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    LILI_TRY(kf_join_stores(c, {{stores, k}}));
+    BmapJob j;
+    LILI_TRY(bmap_tables<KfRowM>(c, bp, KfStores{c, stores}, kf_ids, poses7, k, j));
+    return bmap_run<KfRowM>(j, n_edge_map, n_surf_map);
 }
 
 extern "C" int liliom_bmap_download(liliom_ctx* c, int layer, void* out, int cap, int* m_out) {
@@ -567,9 +621,9 @@ extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* p
 // detectLoopClosure + performLoopClosure's alignment (:2473-2582) without leaving the device: the history cloud goes into the
 // loop index (its own cell grid: the odometry map, the local map and every resident correspondence stay), the latest cloud into
 // loop_src, and the ICP runs on them (icp.cu).  Scratch shared with the other calls: bmap_raw, vg_out, the sort chain, grid_keys*,
-// partials.  The call is written in parts so that the solo call and the batched one (liliom_loop_align_batch) run the same
-// code: loop_begin, then per cloud the gather, the VoxelGrid chain and the repack, then grid_begin .. grid_finish of the
-// target's cell grid, then icp_begin .. icp_finish.
+// partials.  The call is written in parts so that the solo calls and the batched ones (liliom_loop_align(_batch)(_multi)) run the
+// same code: loop_check and loop_tables, then per cloud the gather, the VoxelGrid chain and the repack, then grid_begin ..
+// grid_finish of the target's cell grid, then icp_begin .. icp_finish.
 namespace lili {
 
 struct LoopJob {
@@ -625,14 +679,25 @@ static int loop_tables(liliom_ctx* c, KfStores src, const int* src_ids, const do
     return LILIOM_OK;
 }
 
-// Validation (nothing changes on an error), then loop_tables over c's own store.
-static int loop_begin(liliom_ctx* c, const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids, const double* tgt_poses7,
-                      int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps, double fit_eps, LoopJob& j) {
-    if (!loop_args_ok(src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter)) return LILIOM_E_ARG;
+// Validation before loop_tables, nothing changes on an error: both lists' keyframes are c's own (KfRow, the stores unused) or each
+// of its entry's store (KfRowM, liliom_loop_align_multi: also fewer than 2^31 points per cloud)
+template <class Row>
+static int loop_check(liliom_ctx* c, liliom_ctx* const* src_stores, const int* src_ids, const double* src_poses7, int k_src,
+                      liliom_ctx* const* tgt_stores, const int* tgt_ids, const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist,
+                      int max_iter) {
+    constexpr bool multi = std::is_same<Row, KfRowM>::value;
+    if (!loop_args_ok(src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter) ||
+        (multi && ((k_src > 0 && !src_stores) || (k_tgt > 0 && !tgt_stores))))
+        return LILIOM_E_ARG;
     LILI_TRY(backend_check(c, nullptr));
-    if (!kf_ids_ok(c, src_ids, k_src) || !kf_ids_ok(c, tgt_ids, k_tgt)) return LILIOM_E_ARG;     // before anything changes
-    return loop_tables<KfRow>(c, KfStores{c}, src_ids, src_poses7, k_src, KfStores{c}, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist,
-                              max_iter, trans_eps, fit_eps, j);
+    if (!kf_list_ok<Row>(c, src_stores, src_ids, k_src) || !kf_list_ok<Row>(c, tgt_stores, tgt_ids, k_tgt)) return LILIOM_E_ARG;
+    if constexpr (multi)
+        for (const auto& [st, ids, k] : {std::make_tuple(src_stores, src_ids, k_src), std::make_tuple(tgt_stores, tgt_ids, k_tgt)}) {
+            long long N = 0;
+            for (int i = 0; i < k; ++i) N += (long long)st[i]->kfs[ids[i]].n_edge + st[i]->kfs[ids[i]].n_surf;
+            LILI_TRY(kf_points_ok(c, N));
+        }
+    return LILIOM_OK;
 }
 
 // the gather's grid for cloud k (kf_row_grid)
@@ -656,7 +721,7 @@ static int loop_cloud(LoopJob& j, int k) {
     return repack_to_f4(c, c->vg_out.p, (int)j.off[k], stride, loop_dst(c, k), cnt);
 }
 
-// The solo call after loop_begin / its multi-store form's validation: both clouds, the target's cell grid, the ICP
+// The solo call after loop_check and loop_tables: both clouds, the target's cell grid, the ICP
 template <class Row>
 static int loop_run(LoopJob& j, double T16[16], double* fitness, int* converged, int* iters, int* n_src, int* n_tgt) {
     liliom_ctx* c = j.c;
@@ -711,6 +776,38 @@ LILI_STAGE(LoopStCellKeys, LoopEntry, 256, stage_blocks(e.m, 256), cell_keys_at(
 LILI_STAGE(LoopStGatherSorted, LoopEntry, 256, stage_blocks(e.m, 256), gather_sorted_at(e.xyzw, e.vals2, e.m, e.sorted, i))
 LILI_STAGE(LoopStRunEnds, LoopEntry, 256, stage_blocks(e.m, 256), cell_run_ends_at(e.keys2, e.m, e.cell_start, i))
 
+// LoopStGather's body over a table of rows that each name their store's arena (KfRowM: the batched multi-store calls).  An entry
+// of its own, so that LoopEntry and every LoopSt* stage keep their parameters.
+struct KfGatherMEntry {
+    const KfRowM* tab; int rows, gx, gy, stride; unsigned char* out;
+};
+LILI_STAGE(KfStGatherM, KfGatherMEntry, 256, e.gx * e.gy, kf_gather_at((const unsigned char*)nullptr, e.tab, e.rows, e.stride, e.out, KfGridAt{(unsigned)(bx % e.gx), (unsigned)(bx / e.gx), (unsigned)e.gx, (unsigned)e.gy}))
+
+// One session's gather in a batched launch, as its solo launch takes it: rows of c's keyframe table, its grid, the output
+template <class Row>
+struct KfGatherAt {
+    liliom_ctx* c; const Row* tab; int rows; dim3 grid; void* out;
+};
+// The gathers of the sessions `which` (at(i): session i's KfGatherAt) on c0's stream: LoopStGather over c's own arena (KfRow),
+// KfStGatherM over the arenas the rows name (KfRowM)
+template <class Row, class At>
+static int kf_gather_batch(liliom_ctx* c0, const std::vector<int>& which, At at) {
+    if constexpr (std::is_same<Row, KfRow>::value)
+        return stage_batch<LoopStGather>(c0, which, [&](LoopEntry& e, int i) {
+            const KfGatherAt<KfRow> a = at(i);
+            e = LoopEntry{};
+            e.arena = (const unsigned char*)a.c->kf_arena.p; e.tab = a.tab; e.rows = a.rows; e.gx = (int)a.grid.x; e.gy = (int)a.grid.y;
+            e.stride = a.c->prm.point_stride; e.raw_out = (unsigned char*)a.out;
+            return a.c;
+        });
+    else
+        return stage_batch<KfStGatherM>(c0, which, [&](KfGatherMEntry& e, int i) {
+            const KfGatherAt<KfRowM> a = at(i);
+            e = KfGatherMEntry{a.tab, a.rows, (int)a.grid.x, (int)a.grid.y, a.c->prm.point_stride, (unsigned char*)a.out};
+            return a.c;
+        });
+}
+
 // The entry of voxelgrid_dev's chain at 32-bit keys on c's buffers: n points at `in` -> `out`, the count at `count` (the stages
 // LoopStBoxInit .. LoopStCentroidXyzw32; the keyframe store's and the local map's batches run them too)
 static LoopEntry vg_chain_entry(liliom_ctx* c, const void* in, int n, float leaf, void* out, int* count) {
@@ -722,15 +819,15 @@ static LoopEntry vg_chain_entry(liliom_ctx* c, const void* in, int n, float leaf
     return e;
 }
 
-// Session j's entry for cloud k (0 target, 1 source), as loop_cloud's launches take their arguments (the repack's output aside:
-// loop_repack_entry)
+// Session j's gather of cloud k (0 target, 1 source) and its chain's entry, as loop_cloud's launches take their arguments (the
+// repack's output aside: loop_repack_entry)
+template <class Row>
+static KfGatherAt<Row> loop_gather_at(const LoopJob& j, int k) {
+    return KfGatherAt<Row>{j.c, loop_rows<Row>(j, k), j.rows[k], loop_gather_grid(j, k), j.c->bmap_raw.p};
+}
 static LoopEntry loop_cloud_entry(const LoopJob& j, int k) {
     liliom_ctx* c = j.c;
-    LoopEntry e = vg_chain_entry(c, c->bmap_raw.p, (int)j.off[k], j.leaf, c->vg_out.p, c->vg_count.as<int>() + k);
-    const dim3 gg = loop_gather_grid(j, k);
-    e.arena = (const unsigned char*)c->kf_arena.p; e.tab = loop_rows(j, k); e.rows = j.rows[k]; e.gx = (int)gg.x; e.gy = (int)gg.y;
-    e.raw_out = (unsigned char*)c->bmap_raw.p;
-    return e;
+    return vg_chain_entry(c, c->bmap_raw.p, (int)j.off[k], j.leaf, c->vg_out.p, c->vg_count.as<int>() + k);
 }
 static LoopEntry loop_repack_entry(const LoopJob& j, int k) {
     LoopEntry e = loop_cloud_entry(j, k);
@@ -793,7 +890,9 @@ int vg_chain_batch(liliom_ctx* c0, Sel sel, Make entry, Ctx ctx, Fail fail) {
 
 // The shared phases of loop_align_batch, every session's stream pointing at c0's.  Each phase: the solo call's host part per
 // session, the stage launches for all of them, every session's read-back words into its own pinned block, ONE synchronise.
-// wide[i]: session i's index wrapped in one of its clouds (vg_wide_keys); it leaves the shared path after phase 1.
+// wide[i]: session i's index wrapped in one of its clouds (vg_wide_keys); it leaves the shared path after phase 1.  Row: the
+// keyframe tables' row type (KfRow: each session's own store; KfRowM: rows naming their stores).
+template <class Row>
 int loop_batch_run(liliom_ctx* c0, std::vector<LoopJob>& J, std::vector<char>& live, std::vector<char>& wide, liliom_loop_result* res,
                    int* status) {
     const int B = (int)J.size();
@@ -811,7 +910,7 @@ int loop_batch_run(liliom_ctx* c0, std::vector<LoopJob>& J, std::vector<char>& l
     for (int k = 0; k < 2; ++k) {
         auto has = [k](const LoopJob& j) { return j.off[k] > 0; };
         auto cloud = [k](const LoopJob& j) { return loop_cloud_entry(j, k); };
-        LILI_TRY(loop_stage<LoopStGather>(c0, J, sel(has), cloud));
+        LILI_TRY(kf_gather_batch<Row>(c0, sel(has), [&](int i) { return loop_gather_at<Row>(J[i], k); }));
         LILI_TRY(vg_chain_batch(c0, [&] { return sel(has); }, [&](int i) { return cloud(J[i]); }, [&](int i) { return J[i].c; }, fail));
         LILI_TRY(loop_stage<LoopStRepack>(c0, J, sel(has), [k](const LoopJob& j) { return loop_repack_entry(j, k); }));
         for (int i : sel(has)) copy_back(i, k * sizeof(VgParams), J[i].c->vg_params.p, sizeof(VgParams));
@@ -874,27 +973,44 @@ int loop_batch_run(liliom_ctx* c0, std::vector<LoopJob>& J, std::vector<char>& l
 
 // liliom_loop_align of several sessions.  Shared launches and waits on cs[0]'s stream (the other sessions' streams joined before
 // and after with events); every buffer, library sort and scan and host decision stays the session's own, made by the solo
-// call's parts from the session's own read-back words.
-int loop_align_batch(liliom_ctx* const* cs, int B, const int* const* src_ids, const double* const* src_poses7, const int* k_src,
-                     const int* const* tgt_ids, const double* const* tgt_poses7, const int* k_tgt, const liliom_loop_params* prm,
-                     liliom_loop_result* res, int* status) {
+// call's parts from the session's own read-back words.  Row: KfRow, each session's keyframes from its own store (src_stores and
+// tgt_stores NULL), or KfRowM, session i's from the stores src_stores[i] / tgt_stores[i] list, whose streams are joined in too.
+template <class Row>
+int loop_align_batch(liliom_ctx* const* cs, int B, liliom_ctx* const* const* src_stores, const int* const* src_ids,
+                     const double* const* src_poses7, const int* k_src, liliom_ctx* const* const* tgt_stores, const int* const* tgt_ids,
+                     const double* const* tgt_poses7, const int* k_tgt, const liliom_loop_params* prm, liliom_loop_result* res, int* status) {
+    constexpr bool multi = std::is_same<Row, KfRowM>::value;
+    auto stores = [](liliom_ctx* const* const* s, int i) { return multi ? s[i] : nullptr; };
     liliom_ctx* c0 = cs[0];
     std::vector<LoopJob> J(B);
     std::vector<char> live(B, 0), wide(B, 0);
     std::vector<std::pair<unsigned long long, unsigned long long>> launches0(B);
     const std::vector<liliom_ctx*> all(cs, cs + B);
-    LILI_TRY(batch_join_in(c0, all));
+    std::vector<liliom_ctx*> joined(all);
+    for (int i = 0; i < B; ++i) {
+        const liliom_loop_params& p = prm[i];
+        launches0[i] = {cs[i]->cnt.launches, cs[i]->cnt.lib_launches};
+        status[i] = loop_check<Row>(cs[i], stores(src_stores, i), src_ids[i], src_poses7[i], k_src[i], stores(tgt_stores, i), tgt_ids[i],
+                                    tgt_poses7[i], k_tgt[i], p.leaf, p.max_corr_dist, p.max_iter);
+        live[i] = status[i] == LILIOM_OK;
+        if (multi && live[i]) {
+            kf_add_stores(joined, stores(src_stores, i), k_src[i]);
+            kf_add_stores(joined, stores(tgt_stores, i), k_tgt[i]);
+        }
+    }
+    LILI_TRY(batch_join_in(c0, joined));
     int rc;
     {
         const BatchStreams on_c0(all, c0->stream);
         for (int i = 0; i < B; ++i) {
+            if (!live[i]) continue;
             const liliom_loop_params& p = prm[i];
-            launches0[i] = {cs[i]->cnt.launches, cs[i]->cnt.lib_launches};
-            status[i] = loop_begin(cs[i], src_ids[i], src_poses7[i], k_src[i], tgt_ids[i], tgt_poses7[i], k_tgt[i], p.leaf, p.max_corr_dist,
-                                   p.max_iter, p.trans_eps, p.fit_eps, J[i]);
+            status[i] = loop_tables<Row>(cs[i], KfStores{cs[i], stores(src_stores, i)}, src_ids[i], src_poses7[i], k_src[i],
+                                         KfStores{cs[i], stores(tgt_stores, i)}, tgt_ids[i], tgt_poses7[i], k_tgt[i], p.leaf, p.max_corr_dist,
+                                         p.max_iter, p.trans_eps, p.fit_eps, J[i]);
             live[i] = status[i] == LILIOM_OK;
         }
-        rc = loop_batch_run(c0, J, live, wide, res, status);
+        rc = loop_batch_run<Row>(c0, J, live, wide, res, status);
         // sessions whose index wrapped finish on their solo path, which takes the wide keys: the whole solo call, its counters
         // counted from where the batch found them (what this call launched for the session is redone there)
         for (int i = 0; rc == LILIOM_OK && i < B; ++i) {
@@ -903,8 +1019,14 @@ int loop_align_batch(liliom_ctx* const* cs, int B, const int* const* src_ids, co
             c->cnt.launches = launches0[i].first; c->cnt.lib_launches = launches0[i].second;
             const liliom_loop_params& p = prm[i];
             liliom_loop_result& r = res[i];
-            status[i] = liliom_loop_align(c, src_ids[i], src_poses7[i], k_src[i], tgt_ids[i], tgt_poses7[i], k_tgt[i], p.leaf, p.max_corr_dist,
-                                          p.max_iter, p.trans_eps, p.fit_eps, r.T16, &r.fitness, &r.converged, &r.iters, &r.n_src, &r.n_tgt);
+            if constexpr (multi)
+                status[i] = liliom_loop_align_multi(c, src_stores[i], src_ids[i], src_poses7[i], k_src[i], tgt_stores[i], tgt_ids[i], tgt_poses7[i],
+                                                    k_tgt[i], p.leaf, p.max_corr_dist, p.max_iter, p.trans_eps, p.fit_eps, r.T16, &r.fitness,
+                                                    &r.converged, &r.iters, &r.n_src, &r.n_tgt);
+            else
+                status[i] = liliom_loop_align(c, src_ids[i], src_poses7[i], k_src[i], tgt_ids[i], tgt_poses7[i], k_tgt[i], p.leaf,
+                                              p.max_corr_dist, p.max_iter, p.trans_eps, p.fit_eps, r.T16, &r.fitness, &r.converged, &r.iters,
+                                              &r.n_src, &r.n_tgt);
         }
     }
     LILI_TRY(batch_join_out(c0, all));
@@ -1065,13 +1187,9 @@ namespace {
 
 // Session j's entries, as the solo call's launches take their arguments: the gather of its table, layer l's chain (the float4 points
 // into bmap[l].xyzw, as voxelgrid_dev's d_feats) and its cell grid
-LoopEntry bmap_gather_entry(const BmapJob& j) {
-    liliom_ctx* c = j.c;
-    LoopEntry e{};
-    const dim3 gg = bmap_gather_grid(j);
-    e.arena = (const unsigned char*)c->kf_arena.p; e.tab = c->kf_tab.as<KfRow>(); e.rows = j.rows; e.gx = (int)gg.x; e.gy = (int)gg.y;
-    e.stride = c->prm.point_stride; e.raw_out = (unsigned char*)c->bmap_raw.p;
-    return e;
+template <class Row>
+KfGatherAt<Row> bmap_gather_at(const BmapJob& j) {
+    return KfGatherAt<Row>{j.c, j.c->kf_tab.as<Row>(), j.rows, bmap_gather_grid(j), j.c->bmap_raw.p};
 }
 LoopEntry bmap_layer_entry(const BmapJob& j, int l) {
     liliom_ctx* c = j.c;
@@ -1083,7 +1201,8 @@ LoopEntry bmap_grid_entry(const BmapJob& j, int l) { return grid_entry(j.c, j.c-
 
 // The shared phases, every session's stream pointing at c0's.  Session i's read-back words land in its pinned scratch: per layer l
 // its VgParams and count at l * kSlot (phase 1), its grid box at l * kBox (phase 2).  wide[i]: session i's index wrapped in one of
-// its layers (vg_wide_keys); it leaves the shared path after phase 1.
+// its layers (vg_wide_keys); it leaves the shared path after phase 1.  Row: the keyframe tables' row type, as in loop_batch_run.
+template <class Row>
 int bmap_batch_run(liliom_ctx* c0, std::vector<BmapJob>& J, std::vector<char>& live, std::vector<char>& wide, int* status) {
     constexpr size_t kSlot = sizeof(VgParams) + sizeof(int), kBox = kBoxInts * sizeof(int);
     static_assert(2 * kSlot <= sizeof(PinBlock::scratch) && 2 * kBox <= sizeof(PinBlock::scratch), "both layers' words fit the pinned scratch");
@@ -1100,8 +1219,7 @@ int bmap_batch_run(liliom_ctx* c0, std::vector<BmapJob>& J, std::vector<char>& l
             fail(i, fail_cuda(J[i].c, err, "local map batch: read-back"));
     };
     // 1. every table's gather, the edge chains, then the surf chains (they share each session's sort chain) -> counts, VgParams
-    LILI_TRY(stage_batch<LoopStGather>(c0, sel([](const BmapJob& j) { return j.rows > 0; }),
-                                       [&](LoopEntry& e, int i) { e = bmap_gather_entry(J[i]); return J[i].c; }));
+    LILI_TRY(kf_gather_batch<Row>(c0, sel([](const BmapJob& j) { return j.rows > 0; }), [&](int i) { return bmap_gather_at<Row>(J[i]); }));
     for (int l = 0; l < 2; ++l) {
         for (int i : sel([l](const BmapJob& j) { return j.n[l] == 0; }))      // voxelgrid_dev's count of an empty layer
             if (cudaError_t err = cudaMemsetAsync(J[i].c->vg_count.as<int>() + l, 0, sizeof(int), c0->stream); err != cudaSuccess)
@@ -1184,24 +1302,35 @@ int bmap_batch_run(liliom_ctx* c0, std::vector<BmapJob>& J, std::vector<char>& l
 
 // liliom_bmap_build of several sessions.  Shared launches and waits on cs[0]'s stream (the other sessions' streams joined before and
 // after with events); every buffer, library sort and scan and host decision stays the session's own, made by the solo call's parts
-// from the session's own read-back words.
-int bmap_build_batch(liliom_ctx* const* cs, int B, const liliom_backend_params* bps, const int* const* kf_ids, const double* const* poses7,
-                     const int* k, int* n_edge_map, int* n_surf_map, int* status) {
+// from the session's own read-back words.  Row: KfRow, each session's keyframes from its own store (stores NULL), or KfRowM,
+// session i's from the stores stores[i] lists, whose streams are joined in too.
+template <class Row>
+int bmap_build_batch(liliom_ctx* const* cs, int B, const liliom_backend_params* bps, liliom_ctx* const* const* stores, const int* const* kf_ids,
+                     const double* const* poses7, const int* k, int* n_edge_map, int* n_surf_map, int* status) {
+    constexpr bool multi = std::is_same<Row, KfRowM>::value;
+    auto stores_of = [stores](int i) { return multi ? stores[i] : nullptr; };
     liliom_ctx* c0 = cs[0];
     std::vector<BmapJob> J(B);
     std::vector<char> live(B, 0), wide(B, 0);
     std::vector<std::pair<unsigned long long, unsigned long long>> launches0(B);
     const std::vector<liliom_ctx*> all(cs, cs + B);
-    LILI_TRY(batch_join_in(c0, all));
+    std::vector<liliom_ctx*> joined(all);
+    for (int i = 0; i < B; ++i) {
+        launches0[i] = {cs[i]->cnt.launches, cs[i]->cnt.lib_launches};
+        status[i] = bmap_check<Row>(cs[i], bps + i, stores_of(i), kf_ids[i], poses7[i], k[i]);
+        live[i] = status[i] == LILIOM_OK;
+        if (multi && live[i]) kf_add_stores(joined, stores_of(i), k[i]);
+    }
+    LILI_TRY(batch_join_in(c0, joined));
     int rc;
     {
         const BatchStreams on_c0(all, c0->stream);
         for (int i = 0; i < B; ++i) {
-            launches0[i] = {cs[i]->cnt.launches, cs[i]->cnt.lib_launches};
-            status[i] = bmap_begin(cs[i], bps + i, kf_ids[i], poses7[i], k[i], J[i]);
+            if (!live[i]) continue;
+            status[i] = bmap_tables<Row>(cs[i], bps + i, KfStores{cs[i], stores_of(i)}, kf_ids[i], poses7[i], k[i], J[i]);
             live[i] = status[i] == LILIOM_OK;
         }
-        rc = bmap_batch_run(c0, J, live, wide, status);
+        rc = bmap_batch_run<Row>(c0, J, live, wide, status);
         for (int i = 0; rc == LILIOM_OK && i < B; ++i) {
             auto at = [i](int* p) { return p ? p + i : nullptr; };
             if (live[i]) {
@@ -1210,7 +1339,10 @@ int bmap_build_batch(liliom_ctx* const* cs, int B, const liliom_backend_params* 
                 // the whole solo call, which takes the wide keys, its counters counted from where the batch found them
                 liliom_ctx* c = cs[i];
                 c->cnt.launches = launches0[i].first; c->cnt.lib_launches = launches0[i].second;
-                status[i] = liliom_bmap_build(c, bps + i, kf_ids[i], poses7[i], k[i], at(n_edge_map), at(n_surf_map));
+                if constexpr (multi)
+                    status[i] = liliom_bmap_build_multi(c, bps + i, stores[i], kf_ids[i], poses7[i], k[i], at(n_edge_map), at(n_surf_map));
+                else
+                    status[i] = liliom_bmap_build(c, bps + i, kf_ids[i], poses7[i], k[i], at(n_edge_map), at(n_surf_map));
             }
         }
     }
@@ -1224,8 +1356,10 @@ extern "C" int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double
                                  const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps,
                                  double fit_eps, double T16[16], double* fitness, int* converged, int* iters, int* n_src, int* n_tgt) {
     if (!c || !T16 || !fitness || !converged || !iters) return LILIOM_E_ARG;
+    LILI_TRY(loop_check<KfRow>(c, nullptr, src_ids, src_poses7, k_src, nullptr, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter));
     LoopJob j;
-    LILI_TRY(loop_begin(c, src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter, trans_eps, fit_eps, j));
+    LILI_TRY(loop_tables<KfRow>(c, KfStores{c}, src_ids, src_poses7, k_src, KfStores{c}, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist,
+                                max_iter, trans_eps, fit_eps, j));
     return loop_run<KfRow>(j, T16, fitness, converged, iters, n_src, n_tgt);
 }
 
@@ -1235,7 +1369,18 @@ extern "C" int liliom_loop_align_batch(liliom_ctx* const* ctxs, int B, const int
     if (!batch_ctxs_ok(ctxs, B) || !src_ids || !src_poses7 || !k_src || !tgt_ids || !tgt_poses7 || !k_tgt || !prm || !res || !status)
         return LILIOM_E_ARG;
     LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
-    return loop_align_batch(ctxs, B, src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, prm, res, status);
+    return loop_align_batch<KfRow>(ctxs, B, nullptr, src_ids, src_poses7, k_src, nullptr, tgt_ids, tgt_poses7, k_tgt, prm, res, status);
+}
+
+extern "C" int liliom_loop_align_batch_multi(liliom_ctx* const* ctxs, int B, liliom_ctx* const* const* src_stores, const int* const* src_ids,
+                                             const double* const* src_poses7, const int* k_src, liliom_ctx* const* const* tgt_stores,
+                                             const int* const* tgt_ids, const double* const* tgt_poses7, const int* k_tgt,
+                                             const liliom_loop_params* prm, liliom_loop_result* res, int* status) {
+    if (!batch_ctxs_ok(ctxs, B) || !src_stores || !src_ids || !src_poses7 || !k_src || !tgt_stores || !tgt_ids || !tgt_poses7 || !k_tgt ||
+        !prm || !res || !status)
+        return LILIOM_E_ARG;
+    LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
+    return loop_align_batch<KfRowM>(ctxs, B, src_stores, src_ids, src_poses7, k_src, tgt_stores, tgt_ids, tgt_poses7, k_tgt, prm, res, status);
 }
 
 extern "C" int liliom_kf_add_resident_batch(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps, liliom_ctx* const* srcs,
@@ -1249,7 +1394,15 @@ extern "C" int liliom_bmap_build_batch(liliom_ctx* const* ctxs, int B, const lil
                                        const double* const* poses7, const int* k, int* n_edge_map, int* n_surf_map, int* status) {
     if (!batch_ctxs_ok(ctxs, B) || !bps || !kf_ids || !poses7 || !k || !status) return LILIOM_E_ARG;
     LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
-    return bmap_build_batch(ctxs, B, bps, kf_ids, poses7, k, n_edge_map, n_surf_map, status);
+    return bmap_build_batch<KfRow>(ctxs, B, bps, nullptr, kf_ids, poses7, k, n_edge_map, n_surf_map, status);
+}
+
+extern "C" int liliom_bmap_build_batch_multi(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps, liliom_ctx* const* const* stores,
+                                             const int* const* kf_ids, const double* const* poses7, const int* k, int* n_edge_map,
+                                             int* n_surf_map, int* status) {
+    if (!batch_ctxs_ok(ctxs, B) || !bps || !stores || !kf_ids || !poses7 || !k || !status) return LILIOM_E_ARG;
+    LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
+    return bmap_build_batch<KfRowM>(ctxs, B, bps, stores, kf_ids, poses7, k, n_edge_map, n_surf_map, status);
 }
 
 extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp, int kf_id, const void* full, int n, int* n_stored) {
@@ -1290,41 +1443,6 @@ static bool kf_full_ok(liliom_ctx* c, KfStores s, int kind, const int* kf_ids, i
     return true;
 }
 
-// The multi-store calls' lists: every store there, on c's device, of c's point layout and without a communicator, every id known
-// to its store.  Nothing changes on an error.
-static bool kf_stores_ok(liliom_ctx* c, liliom_ctx* const* stores, const int* kf_ids, int k) {
-    for (int i = 0; i < k; ++i) {
-        const liliom_ctx* st = stores[i];
-        const char* why = !st ? "is NULL"
-                        : st->device != c->device ? "is on another device"
-                        : st->prm.point_stride != c->prm.point_stride ? "has another point_stride"
-                        : st->nranks > 1 ? "has a communicator: the backend keyframe store is single-GPU" : nullptr;
-        if (why) { c->last_error = "store of entry " + std::to_string(i) + " " + why; return false; }
-        if (kf_ids[i] < 0 || kf_ids[i] >= (int)st->kfs.size()) {
-            c->last_error = "unknown keyframe id " + std::to_string(kf_ids[i]) + " in the store of entry " + std::to_string(i) + " (" +
-                            std::to_string(st->kfs.size()) + " stored)";
-            return false;
-        }
-    }
-    return true;
-}
-
-// The stores' work so far before c's reads of their arenas (as liliom_kf_add_resident joins its source): each distinct stream once
-static int kf_join_stores(liliom_ctx* c, std::initializer_list<std::pair<liliom_ctx* const*, int>> lists) {
-    std::vector<liliom_ctx*> v;
-    for (const auto& l : lists)
-        for (int i = 0; i < l.second; ++i)
-            if (std::find(v.begin(), v.end(), l.first[i]) == v.end()) v.push_back(l.first[i]);
-    return batch_join_in(c, v);
-}
-
-// The sort chain's values and PCL's indices are ints
-static int kf_points_ok(liliom_ctx* c, long long N) {
-    if (N < (1LL << 31)) return LILIOM_OK;
-    c->last_error = "the listed keyframes hold " + std::to_string(N) + " points (at most 2^31 - 1)";
-    return LILIOM_E_CAPACITY;
-}
-
 // The global map's table (:2652-2662 list order, one cloud per keyframe): the stored cloud of `kind` of every entry, transformed by
 // pre7s + pre_step * i (none when pre7s is null; pre_step 0: one for every entry) and then by its pose.  Returns the points.
 template <class Row>
@@ -1337,7 +1455,7 @@ static long long gmap_rows(KfStores s, int kind, const int* kf_ids, const double
         const DevBuf& arena = kind == LILIOM_KF_FULL ? s[i]->kf_full : s[i]->kf_arena;
         const long long off = kind == LILIOM_KF_FULL ? f.full_off : f.surf_off;
         const int m = kind == LILIOM_KF_FULL ? f.n_full : f.n_surf;
-        if (m) tab.push_back(kf_row_in<Row>(arena, off, N, m, poses7 + 7 * (size_t)i, pre7s ? pre7s + pre_step * i : nullptr));
+        if (m) tab.push_back(kf_row_in<Row>(arena.p, off, N, m, poses7 + 7 * (size_t)i, pre7s ? pre7s + pre_step * i : nullptr));
         N += m;
         *largest = std::max(*largest, (long long)m);
     }
@@ -1450,16 +1568,8 @@ extern "C" int liliom_loop_align_multi(liliom_ctx* c, liliom_ctx* const* src_sto
                                        double max_corr_dist, int max_iter, double trans_eps, double fit_eps, double T16[16], double* fitness,
                                        int* converged, int* iters, int* n_src, int* n_tgt) {
     if (!c || !T16 || !fitness || !converged || !iters) return LILIOM_E_ARG;
-    if (!loop_args_ok(src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter) || (k_src > 0 && !src_stores) ||
-        (k_tgt > 0 && !tgt_stores))
-        return LILIOM_E_ARG;
-    LILI_TRY(backend_check(c, nullptr));
-    if (!kf_stores_ok(c, src_stores, src_ids, k_src) || !kf_stores_ok(c, tgt_stores, tgt_ids, k_tgt)) return LILIOM_E_ARG;
-    for (const auto& [st, ids, k] : {std::make_tuple(src_stores, src_ids, k_src), std::make_tuple(tgt_stores, tgt_ids, k_tgt)}) {
-        long long N = 0;
-        for (int i = 0; i < k; ++i) N += (long long)st[i]->kfs[ids[i]].n_edge + st[i]->kfs[ids[i]].n_surf;
-        LILI_TRY(kf_points_ok(c, N));
-    }
+    LILI_TRY(loop_check<KfRowM>(c, src_stores, src_ids, src_poses7, k_src, tgt_stores, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist,
+                                max_iter));
     LILI_CUDA(c, cudaSetDevice(c->device));
     LILI_TRY(kf_join_stores(c, {{src_stores, k_src}, {tgt_stores, k_tgt}}));
     LoopJob j;
