@@ -1,4 +1,4 @@
-/* ORACLE — TEST INFRASTRUCTURE ONLY (see oracle_math.h header).  PARITY UNPINNED.
+/* ORACLE — TEST INFRASTRUCTURE ONLY (see oracle_math.h header); what is pinned: DESIGN.md §6.
  *
  * C interface of the CPU restatement of LiLi-OM's per-scan hot path.  Loaded through
  * ctypes by tests/, __graft_entry__.smoke() and bench.py's CPU-baseline legs — never by

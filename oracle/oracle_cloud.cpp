@@ -1,4 +1,4 @@
-// ORACLE — TEST INFRASTRUCTURE ONLY (see oracle_math.h).  PARITY UNPINNED.
+// ORACLE — TEST INFRASTRUCTURE ONLY (see oracle_math.h).  Pinned to the reference's own code: DESIGN.md §6.
 // pcl::VoxelGrid, exact 5-NN (pcl::KdTreeFLANN semantics) and transformCloud restated.
 #include "oracle_api.h"
 #include "oracle_math.h"

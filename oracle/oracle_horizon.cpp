@@ -1,4 +1,4 @@
-// ORACLE — TEST INFRASTRUCTURE ONLY (see oracle_math.h).  PARITY UNPINNED.
+// ORACLE — TEST INFRASTRUCTURE ONLY (see oracle_math.h).  Pinned to the reference's own code: DESIGN.md §6.
 // Livox-Horizon feature extractor restated: the body of Preprocessing::cloudHandler between
 // fromROSMsg and toROSMsg, LiLi-OM/src/Preprocessing.cpp:219-383, plus getDepth (:99-102),
 // undistortion (:104-127) and removeClosedPointCloud (:72-97).  The gyro integration that

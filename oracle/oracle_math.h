@@ -2,12 +2,12 @@
 // Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference
 // legs may build, load or call anything under oracle/.
 //
-// PARITY UNPINNED: the reference (KIT-ISAS/lili-om) ships no tests, golden vectors or
-// fixtures for this path, and cannot be built here (needs ROS, PCL, Eigen, Ceres, glog —
-// none present, no network).  This file restates, from knowledge, the third-party
-// numerical routines the reference calls on the hot path (marked "from-knowledge"),
-// so that the rest of the oracle can follow the reference source expression by
-// expression.  Citations are relative to the reference repository's root.
+// The reference (KIT-ISAS/lili-om) ships no tests, golden vectors or fixtures for this path, and its libraries (ROS, PCL,
+// Eigen, Ceres, glog) are not installed.  This file restates, from knowledge, the third-party numerical routines the
+// reference calls on the hot path (marked "from-knowledge"), so that the rest of the oracle can follow the reference source
+// expression by expression.  The front end and the odometry are pinned to the reference's own translation units, compiled
+// against oracle/ref/'s shims, which forward to the routines here (`make ref`, DESIGN.md §6); these routines themselves,
+// the Ceres step and the backend are not.  Citations are relative to the reference repository's root.
 //
 // Compile with -O3 -ffp-contract=off (the reference builds with -O3 for generic x86-64:
 // no FMA contraction, LiLi-OM/CMakeLists.txt:5).

@@ -1,4 +1,4 @@
-// ORACLE — TEST INFRASTRUCTURE ONLY (see oracle_math.h).  PARITY UNPINNED.
+// ORACLE — TEST INFRASTRUCTURE ONLY (see oracle_math.h).  Pinned to the reference's own code: DESIGN.md §6.
 // Spinning-LiDAR (LOAM-style) feature extractor restated: the body of
 // Preprocessing::cloudHandler in LiLi-OM-ROT/src/Preprocessing.cpp:276-509, with
 // undistortion (:153-177) and removeClosedPointCloud (:120-145).  qIMU is an input (the
@@ -133,8 +133,9 @@ extern "C" int orc_extract_rot(const orc_pt32* pts, int n, const double q_imu_in
         if (scanEndInd[i] - scanStartInd[i] < 6 || i % ds_rate != 0) continue;
         std::vector<orc_pt32> lessFlatScan;
         for (int j = 0; j < 6; j++) {
-            int sp = scanStartInd[i] + (scanEndInd[i] - scanStartInd[i]) * j / 6;
-            int ep = scanStartInd[i] + (scanEndInd[i] - scanStartInd[i]) * (j + 1) / 6 - 1;
+            const int span = scanEndInd[i] - scanStartInd[i];
+            int sp = scanStartInd[i] + span * j / 6;
+            int ep = scanStartInd[i] + span * (j + 1) / 6 - 1;
             std::stable_sort(sortInd.begin() + sp, sortInd.begin() + ep + 1, [&](int a, int b) { return rot_curv_less(curv[a], curv[b]); });  // :410
 
             int largestPickedNum = 0;

@@ -1,4 +1,4 @@
-// ORACLE — TEST INFRASTRUCTURE ONLY (see oracle_math.h).  PARITY UNPINNED.
+// ORACLE — TEST INFRASTRUCTURE ONLY (see oracle_math.h).  Pinned to the reference's own code: DESIGN.md §6.
 // Scan-to-map step of LidarOdometry restated: LiLi-OM/src/LidarOdometry.cpp:221-244
 // (transformPoint), :352-413 (findCorrespondingSurfFeatures), :483-561
 // (updateTransformationWithCeres), LiLi-OM/include/factors/LidarKeyframeFactor.h:111-139

@@ -161,8 +161,9 @@ int extract_rot(const orc_pt32* pts, const int* rings, const double* times, int 
         if (scanEndInd[i] - scanStartInd[i] < 6 || i % ds_rate != 0) continue;
         std::vector<orc_pt32> lessFlatScan;
         for (int j = 0; j < 6; j++) {
-            int sp = scanStartInd[i] + (scanEndInd[i] - scanStartInd[i]) * j / 6;
-            int ep = scanStartInd[i] + (scanEndInd[i] - scanStartInd[i]) * (j + 1) / 6 - 1;
+            const int span = scanEndInd[i] - scanStartInd[i];
+            int sp = scanStartInd[i] + span * j / 6;
+            int ep = scanStartInd[i] + span * (j + 1) / 6 - 1;
             std::stable_sort(sortInd.begin() + sp, sortInd.begin() + ep + 1, [&](int a, int b) { return rot_curv_less(curv[a], curv[b]); });  // :410
 
             int largestPickedNum = 0;
