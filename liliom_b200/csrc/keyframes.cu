@@ -15,7 +15,6 @@
 #include "dev_math.cuh"
 #include "kf_table.h"
 #include <algorithm>
-#include <tuple>
 #include <type_traits>
 
 namespace lili {
@@ -41,43 +40,44 @@ struct KfGridAt {
     __device__ __forceinline__ unsigned int gx() const { return w; }
     __device__ __forceinline__ unsigned int gy() const { return h; }
 };
-template <class Row, class Grid>
-__device__ __forceinline__ void kf_gather_at(const unsigned char* __restrict__ arena, const Row* __restrict__ tab, int rows, int stride,
-                                             unsigned char* __restrict__ out, const Grid blk) {
+template <class Grid>
+__device__ __forceinline__ void kf_gather_at(const KfRow* __restrict__ tab, int rows, int stride, unsigned char* __restrict__ out, const Grid blk) {
     for (int y = blk.by(); y < rows; y += blk.gy()) {
-        const Row& r = tab[y];
+        const KfRow& r = tab[y];
         for (int i = blk.bx() * blockDim.x + threadIdx.x; i < r.n; i += blk.gx() * blockDim.x)
-            kf_row_point(r, kf_row_src(r, arena, stride, r.src_off + i), stride, out + (size_t)(r.dst_off + i) * stride);
+            kf_row_point(r, kf_row_src(r, stride, r.src_off + i), stride, out + (size_t)(r.dst_off + i) * stride);
     }
 }
 
-// box (vg_box.h) of the finite transformed points of the rows, joined into mm
-template <class Row>
-__device__ __forceinline__ void kf_box_at(const unsigned char* __restrict__ arena, const Row* __restrict__ tab, int rows, int stride,
-                                          int* __restrict__ mm) {
+// The table kernels, one set for every table: the gather (its body above, also the batched stage LoopStGather) ...
+__global__ void k_kf_gather(const KfRow* __restrict__ tab, int rows, int stride, unsigned char* __restrict__ out) {
+    kf_gather_at(tab, rows, stride, out, KfGridSolo{});
+}
+
+// ... the box (vg_box.h) of the finite transformed points of the rows, joined into mm
+__global__ void k_kf_box(const KfRow* __restrict__ tab, int rows, int stride, int* __restrict__ mm) {
     int box[kBoxInts];
 #pragma unroll
     for (int k = 0; k < kBoxInts; ++k) box[k] = vg_box_empty(k);
     for (int y = blockIdx.y; y < rows; y += gridDim.y) {
-        const Row& r = tab[y];
+        const KfRow& r = tab[y];
         for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < r.n; i += gridDim.x * blockDim.x) {
-            const VgXyz p = kf_row_xyz(r, kf_row_src(r, arena, stride, r.src_off + i));
+            const VgXyz p = kf_row_xyz(r, kf_row_src(r, stride, r.src_off + i));
             if (isfinite(p.x) && isfinite(p.y) && isfinite(p.z)) vg_box_add(box, p.x, p.y, p.z);
         }
     }
     vg_box_commit(box, mm);
 }
 
-// PCL's relative voxel index of every transformed point (not finite: all-ones, or bit 32 of a wide key), value = its index in
+// ... PCL's relative voxel index of every transformed point (not finite: all-ones, or bit 32 of a wide key), value = its index in
 // the concatenation
-template <typename K, class Row>
-__device__ __forceinline__ void kf_keys_at(const unsigned char* __restrict__ arena, const Row* __restrict__ tab, int rows, int stride,
-                                           const VgParams p, K* __restrict__ keys, int* __restrict__ vals) {
+template <typename K>
+__global__ void k_kf_keys(const KfRow* __restrict__ tab, int rows, int stride, const VgParams p, K* __restrict__ keys, int* __restrict__ vals) {
     const K sentinel = sizeof(K) == 4 ? (K)0xffffffffu : (K)(1ull << 32);
     for (int y = blockIdx.y; y < rows; y += gridDim.y) {
-        const Row& r = tab[y];
+        const KfRow& r = tab[y];
         for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < r.n; i += gridDim.x * blockDim.x) {
-            const VgXyz x = kf_row_xyz(r, kf_row_src(r, arena, stride, r.src_off + i));
+            const VgXyz x = kf_row_xyz(r, kf_row_src(r, stride, r.src_off + i));
             const long long d = r.dst_off + i;
             keys[d] = (isfinite(x.x) && isfinite(x.y) && isfinite(x.z)) ? (K)vg_rel_index(p, x.x, x.y, x.z) : sentinel;
             vals[d] = (int)d;
@@ -85,70 +85,15 @@ __device__ __forceinline__ void kf_keys_at(const unsigned char* __restrict__ are
     }
 }
 
-// centroid of every voxel of the sorted keys (the first n_fin entries are the finite points), members transformed on load
-template <int STRIDE, typename K, class Row>
-__device__ __forceinline__ void kf_centroid_at(const unsigned char* arena, const Row* tab, int rows,
-                                               const K* keys, const int* vals, const int* flags,
-                                               const int* rank, int n_fin, unsigned char* out) {
+// ... and the centroid of every voxel of the sorted keys (the first n_fin entries are the finite points), members transformed on load
+template <int STRIDE, typename K>
+__global__ void k_kf_centroid(const KfRow* __restrict__ tab, int rows, const K* __restrict__ keys, const int* __restrict__ vals,
+                              const int* __restrict__ flags, const int* __restrict__ rank, int n_fin, unsigned char* __restrict__ out) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n_fin || !flags[i]) return;
-    const VgAcc<STRIDE> a = vg_walk<STRIDE>(keys, i, n_fin, [&](int j) { return vals[j]; }, KfRowLoader<STRIDE, Row>{arena, tab, rows});
+    const VgAcc<STRIDE> a = vg_walk<STRIDE>(keys, i, n_fin, [&](int j) { return vals[j]; }, KfRowLoader<STRIDE>{tab, rows});
     vg_write<STRIDE>(a.s, a.n, out + (size_t)rank[i] * STRIDE);
 }
-
-// The table kernels over one store's arena (KfRow) ...
-__global__ void k_kf_gather(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride,
-                            unsigned char* __restrict__ out) {
-    kf_gather_at(arena, tab, rows, stride, out, KfGridSolo{});
-}
-__global__ void k_kf_box(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride, int* __restrict__ mm) {
-    kf_box_at(arena, tab, rows, stride, mm);
-}
-template <typename K>
-__global__ void k_kf_keys(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, int stride, const VgParams p,
-                          K* __restrict__ keys, int* __restrict__ vals) {
-    kf_keys_at(arena, tab, rows, stride, p, keys, vals);
-}
-template <int STRIDE, typename K>
-__global__ void k_kf_centroid(const unsigned char* __restrict__ arena, const KfRow* __restrict__ tab, int rows, const K* __restrict__ keys,
-                              const int* __restrict__ vals, const int* __restrict__ flags, const int* __restrict__ rank, int n_fin,
-                              unsigned char* __restrict__ out) {
-    kf_centroid_at<STRIDE>(arena, tab, rows, keys, vals, flags, rank, n_fin, out);
-}
-// ... and over rows of several stores (KfRowM: each row names its arena; `arena` is not read)
-__global__ void k_kf_gather_m(const unsigned char* __restrict__ arena, const KfRowM* __restrict__ tab, int rows, int stride,
-                              unsigned char* __restrict__ out) {
-    kf_gather_at(arena, tab, rows, stride, out, KfGridSolo{});
-}
-__global__ void k_kf_box_m(const unsigned char* __restrict__ arena, const KfRowM* __restrict__ tab, int rows, int stride, int* __restrict__ mm) {
-    kf_box_at(arena, tab, rows, stride, mm);
-}
-template <typename K>
-__global__ void k_kf_keys_m(const unsigned char* __restrict__ arena, const KfRowM* __restrict__ tab, int rows, int stride, const VgParams p,
-                            K* __restrict__ keys, int* __restrict__ vals) {
-    kf_keys_at(arena, tab, rows, stride, p, keys, vals);
-}
-template <int STRIDE, typename K>
-__global__ void k_kf_centroid_m(const unsigned char* __restrict__ arena, const KfRowM* __restrict__ tab, int rows, const K* __restrict__ keys,
-                                const int* __restrict__ vals, const int* __restrict__ flags, const int* __restrict__ rank, int n_fin,
-                                unsigned char* __restrict__ out) {
-    kf_centroid_at<STRIDE>(arena, tab, rows, keys, vals, flags, rank, n_fin, out);
-}
-
-// Each row type's kernels, for the host code written once over both (kf_gather, gmap_run, loop_cloud)
-template <class Row> struct KfKern;
-template <> struct KfKern<KfRow> {
-    static constexpr auto gather = k_kf_gather;
-    static constexpr auto box = k_kf_box;
-    template <typename K> static constexpr auto keys = k_kf_keys<K>;
-    template <int S, typename K> static constexpr auto centroid = k_kf_centroid<S, K>;
-};
-template <> struct KfKern<KfRowM> {
-    static constexpr auto gather = k_kf_gather_m;
-    static constexpr auto box = k_kf_box_m;
-    template <typename K> static constexpr auto keys = k_kf_keys_m<K>;
-    template <int S, typename K> static constexpr auto centroid = k_kf_centroid_m<S, K>;
-};
 
 // reflectivity (curvature = 0.1 * reflectivity, L/src/FormatConvert.cpp:21) of 48-byte points; `i` as in the other bodies
 __device__ __forceinline__ void kf_refl_at(const unsigned char* __restrict__ pts, int n, float* __restrict__ out, const int i) {
@@ -178,31 +123,18 @@ static int kf_reserve(liliom_ctx* c, DevBuf& arena, long long used, long long pt
     return LILIOM_OK;
 }
 
-static bool kf_ids_ok(liliom_ctx* c, const int* ids, int k) {
-    for (int i = 0; i < k; ++i)
-        if (ids[i] < 0 || ids[i] >= (int)c->kfs.size()) {
-            char buf[96];
-            snprintf(buf, sizeof(buf), "unknown keyframe id %d (%d stored)", ids[i], (int)c->kfs.size());
-            c->last_error = buf;
-            return false;
-        }
-    return true;
-}
-
-template <class Row>
-static int kf_upload_table(liliom_ctx* c, const std::vector<Row>& tab) {
-    LILI_CUDA(c, c->kf_tab.ensure(tab.size() * sizeof(Row)));
-    LILI_CUDA(c, cudaMemcpyAsync(c->kf_tab.p, tab.data(), tab.size() * sizeof(Row), cudaMemcpyHostToDevice, c->stream));
+static int kf_upload_table(liliom_ctx* c, const std::vector<KfRow>& tab) {
+    LILI_CUDA(c, c->kf_tab.ensure(tab.size() * sizeof(KfRow)));
+    LILI_CUDA(c, cudaMemcpyAsync(c->kf_tab.p, tab.data(), tab.size() * sizeof(KfRow), cudaMemcpyHostToDevice, c->stream));
     return LILIOM_OK;
 }
 
-// Transform + concatenate rows (of `arena`, or each of its own: KfRowM) into `out` (one launch).
-template <class Row>
-static int kf_gather(liliom_ctx* c, const void* arena, const std::vector<Row>& tab, long long largest, void* out) {
+// Transform + concatenate rows into `out` (one launch).
+static int kf_gather(liliom_ctx* c, const std::vector<KfRow>& tab, long long largest, void* out) {
     if (tab.empty() || largest <= 0) return LILIOM_OK;
     LILI_TRY(kf_upload_table(c, tab));
-    KfKern<Row>::gather<<<kf_row_grid(tab.size(), largest, c->sm_count * 4), 256, 0, c->stream>>>(
-        (const unsigned char*)arena, c->kf_tab.as<Row>(), (int)tab.size(), c->prm.point_stride, (unsigned char*)out);
+    k_kf_gather<<<kf_row_grid(tab.size(), largest, c->sm_count * 4), 256, 0, c->stream>>>(c->kf_tab.as<KfRow>(), (int)tab.size(),
+                                                                                          c->prm.point_stride, (unsigned char*)out);
     return launch_check(c, "k_kf_gather");
 }
 
@@ -213,66 +145,69 @@ struct KfStores {
     liliom_ctx* operator[](int i) const { return per ? per[i] : c; }
 };
 
-// The multi-store calls' lists: every store there, on c's device, of c's point layout and without a communicator, every id known
-// to its store.  Nothing changes on an error.
-static bool kf_stores_ok(liliom_ctx* c, liliom_ctx* const* stores, const int* kf_ids, int k) {
+// The clouds of a listed keyframe that a call reads: its full cloud (LILIOM_KF_FULL), its surf cloud (LILIOM_KF_SURF), or its edge
+// and surf clouds (kKfScan: the local map, the loop-closure clouds)
+enum { kKfScan = -1 };
+
+// A list of k keyframes: every entry's store there, on c's device, of c's point layout and without a communicator, every id known
+// to its store, every keyframe with the clouds of `kind` (LILIOM_KF_FULL: a full cloud), and fewer than 2^31 listed points (the sort
+// chain's values and PCL's indices are ints).  Nothing changes on an error.
+static int kf_list_ok(liliom_ctx* c, KfStores s, const int* kf_ids, int k, int kind) {
     for (int i = 0; i < k; ++i) {
-        const liliom_ctx* st = stores[i];
+        const liliom_ctx* st = s[i];
         const char* why = !st ? "is NULL"
                         : st->device != c->device ? "is on another device"
                         : st->prm.point_stride != c->prm.point_stride ? "has another point_stride"
                         : st->nranks > 1 ? "has a communicator: the backend keyframe store is single-GPU" : nullptr;
-        if (why) { c->last_error = "store of entry " + std::to_string(i) + " " + why; return false; }
+        if (why) { c->last_error = "store of entry " + std::to_string(i) + " " + why; return LILIOM_E_ARG; }
         if (kf_ids[i] < 0 || kf_ids[i] >= (int)st->kfs.size()) {
-            c->last_error = "unknown keyframe id " + std::to_string(kf_ids[i]) + " in the store of entry " + std::to_string(i) + " (" +
-                            std::to_string(st->kfs.size()) + " stored)";
-            return false;
+            c->last_error = "unknown keyframe id " + std::to_string(kf_ids[i]) + (s.per ? " in the store of entry " + std::to_string(i) : "") +
+                            " (" + std::to_string(st->kfs.size()) + " stored)";
+            return LILIOM_E_ARG;
         }
     }
-    return true;
-}
-
-// The ids of a list: known to c's own store (KfRow) or each to its entry's store (KfRowM, kf_stores_ok).  Nothing changes on an error.
-template <class Row>
-static bool kf_list_ok(liliom_ctx* c, liliom_ctx* const* stores, const int* kf_ids, int k) {
-    if constexpr (std::is_same<Row, KfRowM>::value) return kf_stores_ok(c, stores, kf_ids, k);
-    else return kf_ids_ok(c, kf_ids, k);
-}
-
-// The distinct stores of the lists, in order of first appearance, appended to v (each once)
-static void kf_add_stores(std::vector<liliom_ctx*>& v, liliom_ctx* const* stores, int k) {
-    for (int i = 0; i < k; ++i)
-        if (std::find(v.begin(), v.end(), stores[i]) == v.end()) v.push_back(stores[i]);
-}
-
-// The stores' work so far before c's reads of their arenas (as liliom_kf_add_resident joins its source): each distinct stream once
-static int kf_join_stores(liliom_ctx* c, std::initializer_list<std::pair<liliom_ctx* const*, int>> lists) {
-    std::vector<liliom_ctx*> v;
-    for (const auto& l : lists) kf_add_stores(v, l.first, l.second);
-    return batch_join_in(c, v);
-}
-
-// The sort chain's values and PCL's indices are ints
-static int kf_points_ok(liliom_ctx* c, long long N) {
+    long long N = 0;
+    for (int i = 0; i < k; ++i) {
+        const KfEntry& f = s[i]->kfs[kf_ids[i]];
+        if (kind == LILIOM_KF_FULL && f.n_full < 0) {
+            c->last_error = "keyframe " + std::to_string(kf_ids[i]) + " has no full cloud (liliom_kf_add_full)";
+            if (s.per) c->last_error += " in store " + std::to_string(i);
+            return LILIOM_E_ARG;
+        }
+        N += kind == LILIOM_KF_FULL ? f.n_full : kind == LILIOM_KF_SURF ? f.n_surf : (long long)f.n_edge + f.n_surf;
+    }
     if (N < (1LL << 31)) return LILIOM_OK;
     c->last_error = "the listed keyframes hold " + std::to_string(N) + " points (at most 2^31 - 1)";
     return LILIOM_E_CAPACITY;
+}
+
+// The distinct stores of a list, in order of first appearance, appended to v (each once)
+static void kf_add_stores(std::vector<liliom_ctx*>& v, KfStores s, int k) {
+    for (int i = 0; i < k; ++i)
+        if (std::find(v.begin(), v.end(), s[i]) == v.end()) v.push_back(s[i]);
+}
+
+// The stores' work so far before c's reads of their arenas (as liliom_kf_add_resident joins its source): each distinct stream once
+// (none for c's own store)
+static int kf_join_stores(liliom_ctx* c, std::initializer_list<std::pair<KfStores, int>> lists) {
+    std::vector<liliom_ctx*> v;
+    for (const auto& l : lists) kf_add_stores(v, l.first, l.second);
+    return batch_join_in(c, v);
 }
 
 // detectLoopClosure's cloud of the listed keyframes (:2476-2497, :2502-2547): edge then surf of each, transformed by its pose,
 // concatenated into bmap_raw (one launch), VoxelGrid(leaf) into vg_out with its count at d_count (device) and *m (host).
 // *n_in: the points read (0: nothing was launched, d_count is not written and *m = 0).
 // The rows of such a cloud appended to tab (destinations from 0); returns its points, *largest = the largest keyframe cloud.
-template <class Row>
-static long long kf_cloud_rows(KfStores s, const int* kf_ids, const double* poses7, int k, std::vector<Row>& tab, long long* largest) {
+static long long kf_cloud_rows(KfStores s, const int* kf_ids, const double* poses7, int k, std::vector<KfRow>& tab, long long* largest) {
     long long off = 0;
     *largest = 0;
     for (int i = 0; i < k; ++i) {                                 // :2492-2493 / :2519-2520: *edge_frames[i] then *surf_frames[i]
         const KfEntry& f = s[i]->kfs[kf_ids[i]];
         const void* arena = s[i]->kf_arena.p;
-        if (f.n_edge) tab.push_back(kf_row_in<Row>(arena, f.edge_off, off, f.n_edge, poses7 + 7 * (size_t)i));
+        if (f.n_edge) tab.push_back(kf_row_in(arena, f.edge_off, off, f.n_edge, poses7 + 7 * (size_t)i));
         off += f.n_edge;
-        if (f.n_surf) tab.push_back(kf_row_in<Row>(arena, f.surf_off, off, f.n_surf, poses7 + 7 * (size_t)i));
+        if (f.n_surf) tab.push_back(kf_row_in(arena, f.surf_off, off, f.n_surf, poses7 + 7 * (size_t)i));
         off += f.n_surf;
         *largest = std::max(*largest, (long long)std::max(f.n_edge, f.n_surf));
     }
@@ -290,7 +225,7 @@ static int kf_cloud_dev(liliom_ctx* c, const int* kf_ids, const double* poses7, 
     LILI_CUDA(c, c->bmap_raw.ensure((size_t)off * stride));      // scratch: the local map's layers live in bmap_ds / bmap
     c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
     LILI_CUDA(c, c->vg_out.ensure((size_t)off * stride));
-    LILI_TRY(kf_gather(c, c->kf_arena.p, tab, largest, c->bmap_raw.p));
+    LILI_TRY(kf_gather(c, tab, largest, c->bmap_raw.p));
     return voxelgrid_dev_sync(c, c->bmap_raw.p, (int)off, stride, leaf, c->vg_out.p, d_count, nullptr, m);
 }
 
@@ -415,20 +350,14 @@ static const unsigned char* bmap_in(const BmapJob& j, int l) {
 }
 static dim3 bmap_gather_grid(const BmapJob& j) { return kf_row_grid(j.rows, j.largest, j.c->sm_count * 4); }
 
-// Validation, nothing changes on an error (the previous layers stay): the entries' keyframes are c's own (KfRow, stores unused)
-// or each of its entry's store (KfRowM, liliom_bmap_build_multi)
-template <class Row>
-static int bmap_check(liliom_ctx* c, const liliom_backend_params* bp, liliom_ctx* const* stores, const int* kf_ids, const double* poses7,
-                      int k) {
-    constexpr bool multi = std::is_same<Row, KfRowM>::value;
-    if (k < 0 || (k > 0 && (!kf_ids || !poses7 || (multi && !stores)))) return LILIOM_E_ARG;
+// Validation, nothing changes on an error (the previous layers stay): the entries' keyframes, each of its entry's store
+static int bmap_check(liliom_ctx* c, const liliom_backend_params* bp, KfStores s, const int* kf_ids, const double* poses7, int k) {
+    if (k < 0 || (k > 0 && (!kf_ids || !poses7))) return LILIOM_E_ARG;
     LILI_TRY(backend_check(c, bp));
-    return kf_list_ok<Row>(c, stores, kf_ids, k) ? LILIOM_OK : LILIOM_E_ARG;
+    return kf_list_ok(c, s, kf_ids, k, kKfScan);
 }
 
-// After bmap_check: the keyframe table (rows of the table's type, read from each entry's store), uploaded, and the buffers of both
-// layers.  Every call over either row type runs this one builder (kf_bmap_rows), largest-cloud rule and sizing.
-template <class Row>
+// After bmap_check: the keyframe table (read from each entry's store), uploaded, and the buffers of both layers
 static int bmap_tables(liliom_ctx* c, const liliom_backend_params* bp, KfStores s, const int* kf_ids, const double* poses7, int k,
                        BmapJob& j) {
     LILI_CUDA(c, cudaSetDevice(c->device));
@@ -436,7 +365,7 @@ static int bmap_tables(liliom_ctx* c, const liliom_backend_params* bp, KfStores 
     c->bmap_built = false;
     j = BmapJob{};
     j.c = c; j.bp = bp;
-    std::vector<Row> tab;
+    std::vector<KfRow> tab;
     kf_bmap_rows(
         [&](int i) {
             const KfEntry& f = s[i]->kfs[kf_ids[i]];
@@ -546,15 +475,12 @@ extern "C" int liliom_kf_clear(liliom_ctx* c) {
 
 namespace lili {
 
-// The solo call after bmap_tables: the gather (of c's own arena, or of the arena each KfRowM row names), both layers' VoxelGrid
-// chains and cell grids, the reflectivity, one wait at the end
-template <class Row>
+// The solo call after bmap_tables: the gather, both layers' VoxelGrid chains and cell grids, the reflectivity, one wait at the end
 static int bmap_run(BmapJob& j, int* n_edge_map, int* n_surf_map) {
     liliom_ctx* c = j.c;
     const int stride = c->prm.point_stride;
     if (j.rows > 0) {
-        KfKern<Row>::gather<<<bmap_gather_grid(j), 256, 0, c->stream>>>((const unsigned char*)c->kf_arena.p, c->kf_tab.as<Row>(), j.rows,
-                                                                        stride, (unsigned char*)c->bmap_raw.p);
+        k_kf_gather<<<bmap_gather_grid(j), 256, 0, c->stream>>>(c->kf_tab.as<KfRow>(), j.rows, stride, (unsigned char*)c->bmap_raw.p);
         LILI_TRY(launch_check(c, "k_kf_gather"));
     }
     for (int l = 0; l < 2; ++l)                                   // :1486-1492
@@ -573,27 +499,30 @@ static int bmap_run(BmapJob& j, int* n_edge_map, int* n_surf_map) {
     return LILIOM_OK;
 }
 
+// liliom_bmap_build over the keyframes of c's own store (stores NULL) or entry i's of stores[i]; the layers on c
+static int bmap_build(liliom_ctx* c, const liliom_backend_params* bp, liliom_ctx* const* stores, const int* kf_ids, const double* poses7, int k,
+                      int* n_edge_map, int* n_surf_map) {
+    if (!c || !bp) return LILIOM_E_ARG;
+    const KfStores s{c, stores};
+    LILI_TRY(bmap_check(c, bp, s, kf_ids, poses7, k));
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    LILI_TRY(kf_join_stores(c, {{s, k}}));
+    BmapJob j;
+    LILI_TRY(bmap_tables(c, bp, s, kf_ids, poses7, k, j));
+    return bmap_run(j, n_edge_map, n_surf_map);
+}
+
 }  // namespace lili
 
 extern "C" int liliom_bmap_build(liliom_ctx* c, const liliom_backend_params* bp, const int* kf_ids, const double* poses7, int k,
                                  int* n_edge_map, int* n_surf_map) {
-    if (!c || !bp) return LILIOM_E_ARG;
-    LILI_TRY(bmap_check<KfRow>(c, bp, nullptr, kf_ids, poses7, k));
-    BmapJob j;
-    LILI_TRY(bmap_tables<KfRow>(c, bp, KfStores{c}, kf_ids, poses7, k, j));
-    return bmap_run<KfRow>(j, n_edge_map, n_surf_map);
+    return bmap_build(c, bp, nullptr, kf_ids, poses7, k, n_edge_map, n_surf_map);
 }
 
-// liliom_bmap_build over keyframes of several stores: rows that name their store's arena, the rest unchanged on c
 extern "C" int liliom_bmap_build_multi(liliom_ctx* c, const liliom_backend_params* bp, liliom_ctx* const* stores, const int* kf_ids,
                                        const double* poses7, int k, int* n_edge_map, int* n_surf_map) {
-    if (!c || !bp) return LILIOM_E_ARG;
-    LILI_TRY(bmap_check<KfRowM>(c, bp, stores, kf_ids, poses7, k));
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    LILI_TRY(kf_join_stores(c, {{stores, k}}));
-    BmapJob j;
-    LILI_TRY(bmap_tables<KfRowM>(c, bp, KfStores{c, stores}, kf_ids, poses7, k, j));
-    return bmap_run<KfRowM>(j, n_edge_map, n_surf_map);
+    if (k > 0 && !stores) return LILIOM_E_ARG;
+    return bmap_build(c, bp, stores, kf_ids, poses7, k, n_edge_map, n_surf_map);
 }
 
 extern "C" int liliom_bmap_download(liliom_ctx* c, int layer, void* out, int cap, int* m_out) {
@@ -606,7 +535,7 @@ extern "C" int liliom_bmap_download(liliom_ctx* c, int layer, void* out, int cap
 extern "C" int liliom_kf_cloud(liliom_ctx* c, const int* kf_ids, const double* poses7, int k, float leaf, void* out, int cap, int* n_out) {
     if (!c || !n_out || k < 0 || (k > 0 && (!kf_ids || !poses7)) || !(leaf > 0)) return LILIOM_E_ARG;
     LILI_TRY(backend_check(c, nullptr));
-    if (!kf_ids_ok(c, kf_ids, k)) return LILIOM_E_ARG;
+    LILI_TRY(kf_list_ok(c, KfStores{c}, kf_ids, k, kKfScan));
     LILI_CUDA(c, cudaSetDevice(c->device));
     const int stride = c->prm.point_stride;
     *n_out = 0;
@@ -650,15 +579,14 @@ static bool loop_args_ok(const int* src_ids, const double* src_poses7, int k_src
 }
 
 // After validation: the keyframe tables of both clouds in one upload (so that both stay valid until their gathers have run), rows
-// of the table's type read from each entry's store, and every buffer of the clouds' chains.
-template <class Row>
+// read from each entry's store, and every buffer of the clouds' chains.
 static int loop_tables(liliom_ctx* c, KfStores src, const int* src_ids, const double* src_poses7, int k_src, KfStores tgt, const int* tgt_ids,
                        const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps, double fit_eps,
                        LoopJob& j) {
     LILI_CUDA(c, cudaSetDevice(c->device));
     j = LoopJob{};
     j.c = c; j.leaf = leaf; j.max_corr_dist = max_corr_dist; j.max_iter = max_iter; j.trans_eps = trans_eps; j.fit_eps = fit_eps;
-    std::vector<Row> tab;
+    std::vector<KfRow> tab;
     // :2502-2547 his_key_frames_ds (the target), :2476-2497 latest_key_frames_ds (the source)
     j.off[0] = kf_cloud_rows(tgt, tgt_ids, tgt_poses7, k_tgt, tab, &j.largest[0]);
     j.rows[0] = (int)tab.size();
@@ -679,42 +607,27 @@ static int loop_tables(liliom_ctx* c, KfStores src, const int* src_ids, const do
     return LILIOM_OK;
 }
 
-// Validation before loop_tables, nothing changes on an error: both lists' keyframes are c's own (KfRow, the stores unused) or each
-// of its entry's store (KfRowM, liliom_loop_align_multi: also fewer than 2^31 points per cloud)
-template <class Row>
-static int loop_check(liliom_ctx* c, liliom_ctx* const* src_stores, const int* src_ids, const double* src_poses7, int k_src,
-                      liliom_ctx* const* tgt_stores, const int* tgt_ids, const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist,
-                      int max_iter) {
-    constexpr bool multi = std::is_same<Row, KfRowM>::value;
-    if (!loop_args_ok(src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter) ||
-        (multi && ((k_src > 0 && !src_stores) || (k_tgt > 0 && !tgt_stores))))
-        return LILIOM_E_ARG;
+// Validation before loop_tables, nothing changes on an error: both lists' keyframes, each of its entry's store
+static int loop_check(liliom_ctx* c, KfStores src, const int* src_ids, const double* src_poses7, int k_src, KfStores tgt, const int* tgt_ids,
+                      const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist, int max_iter) {
+    if (!loop_args_ok(src_ids, src_poses7, k_src, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter)) return LILIOM_E_ARG;
     LILI_TRY(backend_check(c, nullptr));
-    if (!kf_list_ok<Row>(c, src_stores, src_ids, k_src) || !kf_list_ok<Row>(c, tgt_stores, tgt_ids, k_tgt)) return LILIOM_E_ARG;
-    if constexpr (multi)
-        for (const auto& [st, ids, k] : {std::make_tuple(src_stores, src_ids, k_src), std::make_tuple(tgt_stores, tgt_ids, k_tgt)}) {
-            long long N = 0;
-            for (int i = 0; i < k; ++i) N += (long long)st[i]->kfs[ids[i]].n_edge + st[i]->kfs[ids[i]].n_surf;
-            LILI_TRY(kf_points_ok(c, N));
-        }
-    return LILIOM_OK;
+    LILI_TRY(kf_list_ok(c, src, src_ids, k_src, kKfScan));
+    return kf_list_ok(c, tgt, tgt_ids, k_tgt, kKfScan);
 }
 
 // the gather's grid for cloud k (kf_row_grid)
 static dim3 loop_gather_grid(const LoopJob& j, int k) { return kf_row_grid(j.rows[k], j.largest[k], j.c->sm_count * 4); }
-template <class Row = KfRow>
-static const Row* loop_rows(const LoopJob& j, int k) { return j.c->kf_tab.as<Row>() + (k == 0 ? 0 : j.rows[0]); }
+static const KfRow* loop_rows(const LoopJob& j, int k) { return j.c->kf_tab.as<KfRow>() + (k == 0 ? 0 : j.rows[0]); }
 
 // Cloud k (0 target, 1 source) on the solo path: gather, VoxelGrid with its count read back (voxelgrid_dev_sync: wide keys where
 // the index wraps), repack into the loop index's points or loop_src (the count read on the device).
-template <class Row>
 static int loop_cloud(LoopJob& j, int k) {
     liliom_ctx* c = j.c;
     const int stride = c->prm.point_stride;
     int* cnt = c->vg_count.as<int>() + k;
     if (j.off[k] > 0) {
-        KfKern<Row>::gather<<<loop_gather_grid(j, k), 256, 0, c->stream>>>((const unsigned char*)c->kf_arena.p, loop_rows<Row>(j, k), j.rows[k],
-                                                                           stride, (unsigned char*)c->bmap_raw.p);
+        k_kf_gather<<<loop_gather_grid(j, k), 256, 0, c->stream>>>(loop_rows(j, k), j.rows[k], stride, (unsigned char*)c->bmap_raw.p);
         LILI_TRY(launch_check(c, "k_kf_gather"));
         LILI_TRY(voxelgrid_dev_sync(c, c->bmap_raw.p, (int)j.off[k], stride, j.leaf, c->vg_out.p, cnt, nullptr, &j.m[k]));
     }
@@ -722,16 +635,30 @@ static int loop_cloud(LoopJob& j, int k) {
 }
 
 // The solo call after loop_check and loop_tables: both clouds, the target's cell grid, the ICP
-template <class Row>
 static int loop_run(LoopJob& j, double T16[16], double* fitness, int* converged, int* iters, int* n_src, int* n_tgt) {
     liliom_ctx* c = j.c;
-    LILI_TRY(loop_cloud<Row>(j, 0));      // :2502-2547 his_key_frames_ds -> the loop index's points (float4, w = index)
-    LILI_TRY(loop_cloud<Row>(j, 1));      // :2476-2497 latest_key_frames_ds -> the source
+    LILI_TRY(loop_cloud(j, 0));      // :2502-2547 his_key_frames_ds -> the loop index's points (float4, w = index)
+    LILI_TRY(loop_cloud(j, 1));      // :2476-2497 latest_key_frames_ds -> the source
     if (n_src) *n_src = j.m[1];
     if (n_tgt) *n_tgt = j.m[0];
     LILI_TRY(grid_build(c, c->loop, loop_cell(c), j.m[0]));
     return icp_align(c, c->loop, c->loop_src.as<float4>(), j.m[1], j.max_corr_dist, j.max_iter, j.trans_eps, j.fit_eps, T16, fitness,
                      converged, iters);
+}
+
+// liliom_loop_align over the keyframes of c's own store (src_stores / tgt_stores NULL) or entry i's of src_stores[i] / tgt_stores[i]
+static int loop_align(liliom_ctx* c, liliom_ctx* const* src_stores, const int* src_ids, const double* src_poses7, int k_src,
+                      liliom_ctx* const* tgt_stores, const int* tgt_ids, const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist,
+                      int max_iter, double trans_eps, double fit_eps, double T16[16], double* fitness, int* converged, int* iters, int* n_src,
+                      int* n_tgt) {
+    if (!c || !T16 || !fitness || !converged || !iters) return LILIOM_E_ARG;
+    const KfStores src{c, src_stores}, tgt{c, tgt_stores};
+    LILI_TRY(loop_check(c, src, src_ids, src_poses7, k_src, tgt, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter));
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    LILI_TRY(kf_join_stores(c, {{src, k_src}, {tgt, k_tgt}}));
+    LoopJob j;
+    LILI_TRY(loop_tables(c, src, src_ids, src_poses7, k_src, tgt, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter, trans_eps, fit_eps, j));
+    return loop_run(j, T16, fitness, converged, iters, n_src, n_tgt);
 }
 
 static int loop_icp_begin(LoopJob& j) {
@@ -745,7 +672,7 @@ struct LoopEntry {
     // a cloud: the gather of its table rows into bmap_raw, the VoxelGrid chain of its n points into vg_out, the repack into xyzw
     // (the local map's chain has no repack: its centroid stage writes the float4 points into xyzw, as voxelgrid_dev's d_feats;
     // every other chain runs with xyzw null)
-    const unsigned char* arena; const KfRow* tab; int rows, gx, gy;
+    const KfRow* tab; int rows, gx, gy;
     const unsigned char* raw; unsigned char* raw_out; int n, stride; float leaf; int* mm; int mm_blocks; VgParams* pp;
     uint32_t* keys; int* vals; const uint32_t* keys2; const int* vals2; int* flags; int* rank; unsigned char* ds; int* count;
     float4* xyzw;
@@ -754,7 +681,7 @@ struct LoopEntry {
 };
 
 // The stages (k_stage_batch, ctx.cuh), each with the block size, the blocks and the body of its solo launch
-LILI_STAGE(LoopStGather, LoopEntry, 256, e.gx * e.gy, kf_gather_at(e.arena, e.tab, e.rows, e.stride, e.raw_out, KfGridAt{(unsigned)(bx % e.gx), (unsigned)(bx / e.gx), (unsigned)e.gx, (unsigned)e.gy}))
+LILI_STAGE(LoopStGather, LoopEntry, 256, e.gx * e.gy, kf_gather_at(e.tab, e.rows, e.stride, e.raw_out, KfGridAt{(unsigned)(bx % e.gx), (unsigned)(bx / e.gx), (unsigned)e.gx, (unsigned)e.gy}))
 LILI_STAGE(LoopStBoxInit, LoopEntry, 32, 1, vg_box_init(e.mm))
 LILI_STAGE(LoopStBox, LoopEntry, 256, e.mm_blocks, vg_minmax_body(e.raw, e.n, nullptr, e.stride, e.mm, SessionBlock{bx, (unsigned)e.mm_blocks}))
 LILI_STAGE(LoopStParams, LoopEntry, 32, 1, vg_params_at(e.mm, e.leaf, e.pp))
@@ -776,36 +703,11 @@ LILI_STAGE(LoopStCellKeys, LoopEntry, 256, stage_blocks(e.m, 256), cell_keys_at(
 LILI_STAGE(LoopStGatherSorted, LoopEntry, 256, stage_blocks(e.m, 256), gather_sorted_at(e.xyzw, e.vals2, e.m, e.sorted, i))
 LILI_STAGE(LoopStRunEnds, LoopEntry, 256, stage_blocks(e.m, 256), cell_run_ends_at(e.keys2, e.m, e.cell_start, i))
 
-// LoopStGather's body over a table of rows that each name their store's arena (KfRowM: the batched multi-store calls).  An entry
-// of its own, so that LoopEntry and every LoopSt* stage keep their parameters.
-struct KfGatherMEntry {
-    const KfRowM* tab; int rows, gx, gy, stride; unsigned char* out;
-};
-LILI_STAGE(KfStGatherM, KfGatherMEntry, 256, e.gx * e.gy, kf_gather_at((const unsigned char*)nullptr, e.tab, e.rows, e.stride, e.out, KfGridAt{(unsigned)(bx % e.gx), (unsigned)(bx / e.gx), (unsigned)e.gx, (unsigned)e.gy}))
-
-// One session's gather in a batched launch, as its solo launch takes it: rows of c's keyframe table, its grid, the output
-template <class Row>
-struct KfGatherAt {
-    liliom_ctx* c; const Row* tab; int rows; dim3 grid; void* out;
-};
-// The gathers of the sessions `which` (at(i): session i's KfGatherAt) on c0's stream: LoopStGather over c's own arena (KfRow),
-// KfStGatherM over the arenas the rows name (KfRowM)
-template <class Row, class At>
-static int kf_gather_batch(liliom_ctx* c0, const std::vector<int>& which, At at) {
-    if constexpr (std::is_same<Row, KfRow>::value)
-        return stage_batch<LoopStGather>(c0, which, [&](LoopEntry& e, int i) {
-            const KfGatherAt<KfRow> a = at(i);
-            e = LoopEntry{};
-            e.arena = (const unsigned char*)a.c->kf_arena.p; e.tab = a.tab; e.rows = a.rows; e.gx = (int)a.grid.x; e.gy = (int)a.grid.y;
-            e.stride = a.c->prm.point_stride; e.raw_out = (unsigned char*)a.out;
-            return a.c;
-        });
-    else
-        return stage_batch<KfStGatherM>(c0, which, [&](KfGatherMEntry& e, int i) {
-            const KfGatherAt<KfRowM> a = at(i);
-            e = KfGatherMEntry{a.tab, a.rows, (int)a.grid.x, (int)a.grid.y, a.c->prm.point_stride, (unsigned char*)a.out};
-            return a.c;
-        });
+// One session's gather (LoopStGather), as its solo launch takes it: rows of c's keyframe table, its grid, the output
+static LoopEntry kf_gather_entry(liliom_ctx* c, const KfRow* tab, int rows, dim3 grid, void* out) {
+    LoopEntry e{};
+    e.tab = tab; e.rows = rows; e.gx = (int)grid.x; e.gy = (int)grid.y; e.stride = c->prm.point_stride; e.raw_out = (unsigned char*)out;
+    return e;
 }
 
 // The entry of voxelgrid_dev's chain at 32-bit keys on c's buffers: n points at `in` -> `out`, the count at `count` (the stages
@@ -821,9 +723,8 @@ static LoopEntry vg_chain_entry(liliom_ctx* c, const void* in, int n, float leaf
 
 // Session j's gather of cloud k (0 target, 1 source) and its chain's entry, as loop_cloud's launches take their arguments (the
 // repack's output aside: loop_repack_entry)
-template <class Row>
-static KfGatherAt<Row> loop_gather_at(const LoopJob& j, int k) {
-    return KfGatherAt<Row>{j.c, loop_rows<Row>(j, k), j.rows[k], loop_gather_grid(j, k), j.c->bmap_raw.p};
+static LoopEntry loop_gather_entry(const LoopJob& j, int k) {
+    return kf_gather_entry(j.c, loop_rows(j, k), j.rows[k], loop_gather_grid(j, k), j.c->bmap_raw.p);
 }
 static LoopEntry loop_cloud_entry(const LoopJob& j, int k) {
     liliom_ctx* c = j.c;
@@ -890,9 +791,7 @@ int vg_chain_batch(liliom_ctx* c0, Sel sel, Make entry, Ctx ctx, Fail fail) {
 
 // The shared phases of loop_align_batch, every session's stream pointing at c0's.  Each phase: the solo call's host part per
 // session, the stage launches for all of them, every session's read-back words into its own pinned block, ONE synchronise.
-// wide[i]: session i's index wrapped in one of its clouds (vg_wide_keys); it leaves the shared path after phase 1.  Row: the
-// keyframe tables' row type (KfRow: each session's own store; KfRowM: rows naming their stores).
-template <class Row>
+// wide[i]: session i's index wrapped in one of its clouds (vg_wide_keys); it leaves the shared path after phase 1.
 int loop_batch_run(liliom_ctx* c0, std::vector<LoopJob>& J, std::vector<char>& live, std::vector<char>& wide, liliom_loop_result* res,
                    int* status) {
     const int B = (int)J.size();
@@ -910,7 +809,7 @@ int loop_batch_run(liliom_ctx* c0, std::vector<LoopJob>& J, std::vector<char>& l
     for (int k = 0; k < 2; ++k) {
         auto has = [k](const LoopJob& j) { return j.off[k] > 0; };
         auto cloud = [k](const LoopJob& j) { return loop_cloud_entry(j, k); };
-        LILI_TRY(kf_gather_batch<Row>(c0, sel(has), [&](int i) { return loop_gather_at<Row>(J[i], k); }));
+        LILI_TRY(loop_stage<LoopStGather>(c0, J, sel(has), [k](const LoopJob& j) { return loop_gather_entry(j, k); }));
         LILI_TRY(vg_chain_batch(c0, [&] { return sel(has); }, [&](int i) { return cloud(J[i]); }, [&](int i) { return J[i].c; }, fail));
         LILI_TRY(loop_stage<LoopStRepack>(c0, J, sel(has), [k](const LoopJob& j) { return loop_repack_entry(j, k); }));
         for (int i : sel(has)) copy_back(i, k * sizeof(VgParams), J[i].c->vg_params.p, sizeof(VgParams));
@@ -973,14 +872,12 @@ int loop_batch_run(liliom_ctx* c0, std::vector<LoopJob>& J, std::vector<char>& l
 
 // liliom_loop_align of several sessions.  Shared launches and waits on cs[0]'s stream (the other sessions' streams joined before
 // and after with events); every buffer, library sort and scan and host decision stays the session's own, made by the solo
-// call's parts from the session's own read-back words.  Row: KfRow, each session's keyframes from its own store (src_stores and
-// tgt_stores NULL), or KfRowM, session i's from the stores src_stores[i] / tgt_stores[i] list, whose streams are joined in too.
-template <class Row>
+// call's parts from the session's own read-back words.  Each session's keyframes come from its own store (src_stores and tgt_stores
+// NULL), or session i's from the stores src_stores[i] / tgt_stores[i] list, whose streams are joined in too.
 int loop_align_batch(liliom_ctx* const* cs, int B, liliom_ctx* const* const* src_stores, const int* const* src_ids,
                      const double* const* src_poses7, const int* k_src, liliom_ctx* const* const* tgt_stores, const int* const* tgt_ids,
                      const double* const* tgt_poses7, const int* k_tgt, const liliom_loop_params* prm, liliom_loop_result* res, int* status) {
-    constexpr bool multi = std::is_same<Row, KfRowM>::value;
-    auto stores = [](liliom_ctx* const* const* s, int i) { return multi ? s[i] : nullptr; };
+    auto stores = [](liliom_ctx* const* const* s, int i) { return s ? s[i] : nullptr; };
     liliom_ctx* c0 = cs[0];
     std::vector<LoopJob> J(B);
     std::vector<char> live(B, 0), wide(B, 0);
@@ -990,12 +887,15 @@ int loop_align_batch(liliom_ctx* const* cs, int B, liliom_ctx* const* const* src
     for (int i = 0; i < B; ++i) {
         const liliom_loop_params& p = prm[i];
         launches0[i] = {cs[i]->cnt.launches, cs[i]->cnt.lib_launches};
-        status[i] = loop_check<Row>(cs[i], stores(src_stores, i), src_ids[i], src_poses7[i], k_src[i], stores(tgt_stores, i), tgt_ids[i],
-                                    tgt_poses7[i], k_tgt[i], p.leaf, p.max_corr_dist, p.max_iter);
+        const KfStores src{cs[i], stores(src_stores, i)}, tgt{cs[i], stores(tgt_stores, i)};
+        status[i] = (src_stores && k_src[i] > 0 && !src.per) || (tgt_stores && k_tgt[i] > 0 && !tgt.per)
+                        ? LILIOM_E_ARG
+                        : loop_check(cs[i], src, src_ids[i], src_poses7[i], k_src[i], tgt, tgt_ids[i], tgt_poses7[i], k_tgt[i], p.leaf,
+                                     p.max_corr_dist, p.max_iter);
         live[i] = status[i] == LILIOM_OK;
-        if (multi && live[i]) {
-            kf_add_stores(joined, stores(src_stores, i), k_src[i]);
-            kf_add_stores(joined, stores(tgt_stores, i), k_tgt[i]);
+        if (live[i]) {
+            kf_add_stores(joined, src, k_src[i]);
+            kf_add_stores(joined, tgt, k_tgt[i]);
         }
     }
     LILI_TRY(batch_join_in(c0, joined));
@@ -1005,12 +905,12 @@ int loop_align_batch(liliom_ctx* const* cs, int B, liliom_ctx* const* const* src
         for (int i = 0; i < B; ++i) {
             if (!live[i]) continue;
             const liliom_loop_params& p = prm[i];
-            status[i] = loop_tables<Row>(cs[i], KfStores{cs[i], stores(src_stores, i)}, src_ids[i], src_poses7[i], k_src[i],
-                                         KfStores{cs[i], stores(tgt_stores, i)}, tgt_ids[i], tgt_poses7[i], k_tgt[i], p.leaf, p.max_corr_dist,
-                                         p.max_iter, p.trans_eps, p.fit_eps, J[i]);
+            status[i] = loop_tables(cs[i], KfStores{cs[i], stores(src_stores, i)}, src_ids[i], src_poses7[i], k_src[i],
+                                    KfStores{cs[i], stores(tgt_stores, i)}, tgt_ids[i], tgt_poses7[i], k_tgt[i], p.leaf, p.max_corr_dist,
+                                    p.max_iter, p.trans_eps, p.fit_eps, J[i]);
             live[i] = status[i] == LILIOM_OK;
         }
-        rc = loop_batch_run<Row>(c0, J, live, wide, res, status);
+        rc = loop_batch_run(c0, J, live, wide, res, status);
         // sessions whose index wrapped finish on their solo path, which takes the wide keys: the whole solo call, its counters
         // counted from where the batch found them (what this call launched for the session is redone there)
         for (int i = 0; rc == LILIOM_OK && i < B; ++i) {
@@ -1019,14 +919,9 @@ int loop_align_batch(liliom_ctx* const* cs, int B, liliom_ctx* const* const* src
             c->cnt.launches = launches0[i].first; c->cnt.lib_launches = launches0[i].second;
             const liliom_loop_params& p = prm[i];
             liliom_loop_result& r = res[i];
-            if constexpr (multi)
-                status[i] = liliom_loop_align_multi(c, src_stores[i], src_ids[i], src_poses7[i], k_src[i], tgt_stores[i], tgt_ids[i], tgt_poses7[i],
-                                                    k_tgt[i], p.leaf, p.max_corr_dist, p.max_iter, p.trans_eps, p.fit_eps, r.T16, &r.fitness,
-                                                    &r.converged, &r.iters, &r.n_src, &r.n_tgt);
-            else
-                status[i] = liliom_loop_align(c, src_ids[i], src_poses7[i], k_src[i], tgt_ids[i], tgt_poses7[i], k_tgt[i], p.leaf,
-                                              p.max_corr_dist, p.max_iter, p.trans_eps, p.fit_eps, r.T16, &r.fitness, &r.converged, &r.iters,
-                                              &r.n_src, &r.n_tgt);
+            status[i] = loop_align(c, stores(src_stores, i), src_ids[i], src_poses7[i], k_src[i], stores(tgt_stores, i), tgt_ids[i], tgt_poses7[i],
+                                   k_tgt[i], p.leaf, p.max_corr_dist, p.max_iter, p.trans_eps, p.fit_eps, r.T16, &r.fitness, &r.converged,
+                                   &r.iters, &r.n_src, &r.n_tgt);
         }
     }
     LILI_TRY(batch_join_out(c0, all));
@@ -1187,9 +1082,8 @@ namespace {
 
 // Session j's entries, as the solo call's launches take their arguments: the gather of its table, layer l's chain (the float4 points
 // into bmap[l].xyzw, as voxelgrid_dev's d_feats) and its cell grid
-template <class Row>
-KfGatherAt<Row> bmap_gather_at(const BmapJob& j) {
-    return KfGatherAt<Row>{j.c, j.c->kf_tab.as<Row>(), j.rows, bmap_gather_grid(j), j.c->bmap_raw.p};
+LoopEntry bmap_gather_entry(const BmapJob& j) {
+    return kf_gather_entry(j.c, j.c->kf_tab.as<KfRow>(), j.rows, bmap_gather_grid(j), j.c->bmap_raw.p);
 }
 LoopEntry bmap_layer_entry(const BmapJob& j, int l) {
     liliom_ctx* c = j.c;
@@ -1201,8 +1095,7 @@ LoopEntry bmap_grid_entry(const BmapJob& j, int l) { return grid_entry(j.c, j.c-
 
 // The shared phases, every session's stream pointing at c0's.  Session i's read-back words land in its pinned scratch: per layer l
 // its VgParams and count at l * kSlot (phase 1), its grid box at l * kBox (phase 2).  wide[i]: session i's index wrapped in one of
-// its layers (vg_wide_keys); it leaves the shared path after phase 1.  Row: the keyframe tables' row type, as in loop_batch_run.
-template <class Row>
+// its layers (vg_wide_keys); it leaves the shared path after phase 1.
 int bmap_batch_run(liliom_ctx* c0, std::vector<BmapJob>& J, std::vector<char>& live, std::vector<char>& wide, int* status) {
     constexpr size_t kSlot = sizeof(VgParams) + sizeof(int), kBox = kBoxInts * sizeof(int);
     static_assert(2 * kSlot <= sizeof(PinBlock::scratch) && 2 * kBox <= sizeof(PinBlock::scratch), "both layers' words fit the pinned scratch");
@@ -1219,7 +1112,10 @@ int bmap_batch_run(liliom_ctx* c0, std::vector<BmapJob>& J, std::vector<char>& l
             fail(i, fail_cuda(J[i].c, err, "local map batch: read-back"));
     };
     // 1. every table's gather, the edge chains, then the surf chains (they share each session's sort chain) -> counts, VgParams
-    LILI_TRY(kf_gather_batch<Row>(c0, sel([](const BmapJob& j) { return j.rows > 0; }), [&](int i) { return bmap_gather_at<Row>(J[i]); }));
+    LILI_TRY(stage_batch<LoopStGather>(c0, sel([](const BmapJob& j) { return j.rows > 0; }), [&](LoopEntry& e, int i) {
+        e = bmap_gather_entry(J[i]);
+        return J[i].c;
+    }));
     for (int l = 0; l < 2; ++l) {
         for (int i : sel([l](const BmapJob& j) { return j.n[l] == 0; }))      // voxelgrid_dev's count of an empty layer
             if (cudaError_t err = cudaMemsetAsync(J[i].c->vg_count.as<int>() + l, 0, sizeof(int), c0->stream); err != cudaSuccess)
@@ -1302,13 +1198,11 @@ int bmap_batch_run(liliom_ctx* c0, std::vector<BmapJob>& J, std::vector<char>& l
 
 // liliom_bmap_build of several sessions.  Shared launches and waits on cs[0]'s stream (the other sessions' streams joined before and
 // after with events); every buffer, library sort and scan and host decision stays the session's own, made by the solo call's parts
-// from the session's own read-back words.  Row: KfRow, each session's keyframes from its own store (stores NULL), or KfRowM,
-// session i's from the stores stores[i] lists, whose streams are joined in too.
-template <class Row>
+// from the session's own read-back words.  Each session's keyframes come from its own store (stores NULL), or session i's from the
+// stores stores[i] lists, whose streams are joined in too.
 int bmap_build_batch(liliom_ctx* const* cs, int B, const liliom_backend_params* bps, liliom_ctx* const* const* stores, const int* const* kf_ids,
                      const double* const* poses7, const int* k, int* n_edge_map, int* n_surf_map, int* status) {
-    constexpr bool multi = std::is_same<Row, KfRowM>::value;
-    auto stores_of = [stores](int i) { return multi ? stores[i] : nullptr; };
+    auto stores_of = [stores](int i) { return stores ? stores[i] : nullptr; };
     liliom_ctx* c0 = cs[0];
     std::vector<BmapJob> J(B);
     std::vector<char> live(B, 0), wide(B, 0);
@@ -1317,9 +1211,10 @@ int bmap_build_batch(liliom_ctx* const* cs, int B, const liliom_backend_params* 
     std::vector<liliom_ctx*> joined(all);
     for (int i = 0; i < B; ++i) {
         launches0[i] = {cs[i]->cnt.launches, cs[i]->cnt.lib_launches};
-        status[i] = bmap_check<Row>(cs[i], bps + i, stores_of(i), kf_ids[i], poses7[i], k[i]);
+        const KfStores s{cs[i], stores_of(i)};
+        status[i] = stores && k[i] > 0 && !s.per ? LILIOM_E_ARG : bmap_check(cs[i], bps + i, s, kf_ids[i], poses7[i], k[i]);
         live[i] = status[i] == LILIOM_OK;
-        if (multi && live[i]) kf_add_stores(joined, stores_of(i), k[i]);
+        if (live[i]) kf_add_stores(joined, s, k[i]);
     }
     LILI_TRY(batch_join_in(c0, joined));
     int rc;
@@ -1327,10 +1222,10 @@ int bmap_build_batch(liliom_ctx* const* cs, int B, const liliom_backend_params* 
         const BatchStreams on_c0(all, c0->stream);
         for (int i = 0; i < B; ++i) {
             if (!live[i]) continue;
-            status[i] = bmap_tables<Row>(cs[i], bps + i, KfStores{cs[i], stores_of(i)}, kf_ids[i], poses7[i], k[i], J[i]);
+            status[i] = bmap_tables(cs[i], bps + i, KfStores{cs[i], stores_of(i)}, kf_ids[i], poses7[i], k[i], J[i]);
             live[i] = status[i] == LILIOM_OK;
         }
-        rc = bmap_batch_run<Row>(c0, J, live, wide, status);
+        rc = bmap_batch_run(c0, J, live, wide, status);
         for (int i = 0; rc == LILIOM_OK && i < B; ++i) {
             auto at = [i](int* p) { return p ? p + i : nullptr; };
             if (live[i]) {
@@ -1339,10 +1234,7 @@ int bmap_build_batch(liliom_ctx* const* cs, int B, const liliom_backend_params* 
                 // the whole solo call, which takes the wide keys, its counters counted from where the batch found them
                 liliom_ctx* c = cs[i];
                 c->cnt.launches = launches0[i].first; c->cnt.lib_launches = launches0[i].second;
-                if constexpr (multi)
-                    status[i] = liliom_bmap_build_multi(c, bps + i, stores[i], kf_ids[i], poses7[i], k[i], at(n_edge_map), at(n_surf_map));
-                else
-                    status[i] = liliom_bmap_build(c, bps + i, kf_ids[i], poses7[i], k[i], at(n_edge_map), at(n_surf_map));
+                status[i] = bmap_build(c, bps + i, stores_of(i), kf_ids[i], poses7[i], k[i], at(n_edge_map), at(n_surf_map));
             }
         }
     }
@@ -1355,12 +1247,8 @@ int bmap_build_batch(liliom_ctx* const* cs, int B, const liliom_backend_params* 
 extern "C" int liliom_loop_align(liliom_ctx* c, const int* src_ids, const double* src_poses7, int k_src, const int* tgt_ids,
                                  const double* tgt_poses7, int k_tgt, float leaf, double max_corr_dist, int max_iter, double trans_eps,
                                  double fit_eps, double T16[16], double* fitness, int* converged, int* iters, int* n_src, int* n_tgt) {
-    if (!c || !T16 || !fitness || !converged || !iters) return LILIOM_E_ARG;
-    LILI_TRY(loop_check<KfRow>(c, nullptr, src_ids, src_poses7, k_src, nullptr, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter));
-    LoopJob j;
-    LILI_TRY(loop_tables<KfRow>(c, KfStores{c}, src_ids, src_poses7, k_src, KfStores{c}, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist,
-                                max_iter, trans_eps, fit_eps, j));
-    return loop_run<KfRow>(j, T16, fitness, converged, iters, n_src, n_tgt);
+    return loop_align(c, nullptr, src_ids, src_poses7, k_src, nullptr, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter, trans_eps,
+                      fit_eps, T16, fitness, converged, iters, n_src, n_tgt);
 }
 
 extern "C" int liliom_loop_align_batch(liliom_ctx* const* ctxs, int B, const int* const* src_ids, const double* const* src_poses7,
@@ -1369,7 +1257,7 @@ extern "C" int liliom_loop_align_batch(liliom_ctx* const* ctxs, int B, const int
     if (!batch_ctxs_ok(ctxs, B) || !src_ids || !src_poses7 || !k_src || !tgt_ids || !tgt_poses7 || !k_tgt || !prm || !res || !status)
         return LILIOM_E_ARG;
     LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
-    return loop_align_batch<KfRow>(ctxs, B, nullptr, src_ids, src_poses7, k_src, nullptr, tgt_ids, tgt_poses7, k_tgt, prm, res, status);
+    return loop_align_batch(ctxs, B, nullptr, src_ids, src_poses7, k_src, nullptr, tgt_ids, tgt_poses7, k_tgt, prm, res, status);
 }
 
 extern "C" int liliom_loop_align_batch_multi(liliom_ctx* const* ctxs, int B, liliom_ctx* const* const* src_stores, const int* const* src_ids,
@@ -1380,7 +1268,7 @@ extern "C" int liliom_loop_align_batch_multi(liliom_ctx* const* ctxs, int B, lil
         !prm || !res || !status)
         return LILIOM_E_ARG;
     LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
-    return loop_align_batch<KfRowM>(ctxs, B, src_stores, src_ids, src_poses7, k_src, tgt_stores, tgt_ids, tgt_poses7, k_tgt, prm, res, status);
+    return loop_align_batch(ctxs, B, src_stores, src_ids, src_poses7, k_src, tgt_stores, tgt_ids, tgt_poses7, k_tgt, prm, res, status);
 }
 
 extern "C" int liliom_kf_add_resident_batch(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps, liliom_ctx* const* srcs,
@@ -1394,7 +1282,7 @@ extern "C" int liliom_bmap_build_batch(liliom_ctx* const* ctxs, int B, const lil
                                        const double* const* poses7, const int* k, int* n_edge_map, int* n_surf_map, int* status) {
     if (!batch_ctxs_ok(ctxs, B) || !bps || !kf_ids || !poses7 || !k || !status) return LILIOM_E_ARG;
     LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
-    return bmap_build_batch<KfRow>(ctxs, B, bps, nullptr, kf_ids, poses7, k, n_edge_map, n_surf_map, status);
+    return bmap_build_batch(ctxs, B, bps, nullptr, kf_ids, poses7, k, n_edge_map, n_surf_map, status);
 }
 
 extern "C" int liliom_bmap_build_batch_multi(liliom_ctx* const* ctxs, int B, const liliom_backend_params* bps, liliom_ctx* const* const* stores,
@@ -1402,13 +1290,13 @@ extern "C" int liliom_bmap_build_batch_multi(liliom_ctx* const* ctxs, int B, con
                                              int* n_surf_map, int* status) {
     if (!batch_ctxs_ok(ctxs, B) || !bps || !stores || !kf_ids || !poses7 || !k || !status) return LILIOM_E_ARG;
     LILI_CUDA(ctxs[0], cudaSetDevice(ctxs[0]->device));
-    return bmap_build_batch<KfRowM>(ctxs, B, bps, stores, kf_ids, poses7, k, n_edge_map, n_surf_map, status);
+    return bmap_build_batch(ctxs, B, bps, stores, kf_ids, poses7, k, n_edge_map, n_surf_map, status);
 }
 
 extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp, int kf_id, const void* full, int n, int* n_stored) {
     if (!c || !bp || n < 0 || (n > 0 && !full)) return LILIOM_E_ARG;
     LILI_TRY(backend_check(c, bp));
-    if (!kf_ids_ok(c, &kf_id, 1)) return LILIOM_E_ARG;
+    LILI_TRY(kf_list_ok(c, KfStores{c}, &kf_id, 1, kKfScan));
     if (c->kfs[kf_id].n_full >= 0) {
         c->last_error = "keyframe " + std::to_string(kf_id) + " already has its full cloud";
         return LILIOM_E_ARG;
@@ -1432,22 +1320,10 @@ extern "C" int liliom_kf_add_full(liliom_ctx* c, const liliom_backend_params* bp
 
 namespace lili {
 
-// Every listed keyframe of kind LILIOM_KF_FULL has its full cloud (ids known to their stores)
-static bool kf_full_ok(liliom_ctx* c, KfStores s, int kind, const int* kf_ids, int k) {
-    for (int i = 0; i < k && kind == LILIOM_KF_FULL; ++i)
-        if (s[i]->kfs[kf_ids[i]].n_full < 0) {
-            c->last_error = "keyframe " + std::to_string(kf_ids[i]) + " has no full cloud (liliom_kf_add_full)";
-            if (s.per) c->last_error += " in store " + std::to_string(i);
-            return false;
-        }
-    return true;
-}
-
 // The global map's table (:2652-2662 list order, one cloud per keyframe): the stored cloud of `kind` of every entry, transformed by
 // pre7s + pre_step * i (none when pre7s is null; pre_step 0: one for every entry) and then by its pose.  Returns the points.
-template <class Row>
 static long long gmap_rows(KfStores s, int kind, const int* kf_ids, const double* poses7, int k, const double* pre7s, size_t pre_step,
-                           std::vector<Row>& tab, long long* largest) {
+                           std::vector<KfRow>& tab, long long* largest) {
     long long N = 0;
     *largest = 0;
     for (int i = 0; i < k; ++i) {
@@ -1455,7 +1331,7 @@ static long long gmap_rows(KfStores s, int kind, const int* kf_ids, const double
         const DevBuf& arena = kind == LILIOM_KF_FULL ? s[i]->kf_full : s[i]->kf_arena;
         const long long off = kind == LILIOM_KF_FULL ? f.full_off : f.surf_off;
         const int m = kind == LILIOM_KF_FULL ? f.n_full : f.n_surf;
-        if (m) tab.push_back(kf_row_in<Row>(arena.p, off, N, m, poses7 + 7 * (size_t)i, pre7s ? pre7s + pre_step * i : nullptr));
+        if (m) tab.push_back(kf_row_in(arena.p, off, N, m, poses7 + 7 * (size_t)i, pre7s ? pre7s + pre_step * i : nullptr));
         N += m;
         *largest = std::max(*largest, (long long)m);
     }
@@ -1466,24 +1342,22 @@ static long long gmap_rows(KfStores s, int kind, const int* kf_ids, const double
 // and transform every point on load (kf_table.h); the sort chain in between is voxelgrid_dev's (the sort at the key width of the
 // box, k_vg_heads, the scan).  Device memory: the table, 16 bytes per listed point for keys and values (sort included; 24 with
 // the wide keys), and
-// the output; only PCL's declined case writes the transformed concatenation, which is then the output.
-// arena: the store KfRow rows read (KfRowM rows name their own); N <= 2^31 - 1 points (kf_points_ok).
-template <class Row>
-static int gmap_run(liliom_ctx* c, const unsigned char* arena, const std::vector<Row>& tab, long long N, long long largest, float leaf,
-                    void* out, int cap, int* n) {
+// the output; only PCL's declined case writes the transformed concatenation, which is then the output.  N <= 2^31 - 1 points
+// (kf_list_ok).
+static int gmap_run(liliom_ctx* c, const std::vector<KfRow>& tab, long long N, long long largest, float leaf, void* out, int cap, int* n) {
     if (N == 0) { *n = 0; return LILIOM_OK; }
     LILI_CUDA(c, cudaSetDevice(c->device));
     const int stride = c->prm.point_stride;
     const int rows = (int)tab.size();
     LILI_TRY(kf_upload_table(c, tab));
-    const Row* d_tab = c->kf_tab.as<Row>();
+    const KfRow* d_tab = c->kf_tab.as<KfRow>();
     // box of the transformed concatenation (pcl::getMinMax3D), read back: the overflow test and the key width are decided here
     LILI_CUDA(c, c->vg_minmax.ensure(8 * sizeof(int)));
     int* mm = c->vg_minmax.as<int>();
     int* empty = reinterpret_cast<int*>(c->h_pin->scratch);       // pinned staging of the empty box; the stream orders the read-back after it
     for (int w = 0; w < kBoxInts; ++w) empty[w] = vg_box_empty(w);
     LILI_CUDA(c, cudaMemcpyAsync(mm, empty, kBoxInts * sizeof(int), cudaMemcpyHostToDevice, c->stream));
-    KfKern<Row>::box<<<kf_row_grid(tab.size(), largest, 8, 1024), 256, 0, c->stream>>>(arena, d_tab, rows, stride, mm);
+    k_kf_box<<<kf_row_grid(tab.size(), largest, 8, 1024), 256, 0, c->stream>>>(d_tab, rows, stride, mm);
     LILI_TRY(launch_check(c, "k_kf_box"));
     int box[kBoxInts];
     LILI_TRY(read_back(c, {{box, mm, sizeof(box)}}));
@@ -1492,7 +1366,7 @@ static int gmap_run(liliom_ctx* c, const unsigned char* arena, const std::vector
         return download_sized(c, c->vg_out, (int)N, stride, out, cap, n, [&]() -> int {
             c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
             LILI_CUDA(c, c->vg_out.ensure((size_t)N * stride));
-            return kf_gather(c, arena, tab, largest, c->vg_out.p);
+            return kf_gather(c, tab, largest, c->vg_out.p);
         });
     const int n_fin = p.n_finite;
     if (n_fin == 0) { *n = 0; return LILIOM_OK; }
@@ -1506,8 +1380,7 @@ static int gmap_run(liliom_ctx* c, const unsigned char* arena, const std::vector
     LILI_CUDA(c, c->vg_rank.ensure(((size_t)n_fin + 2) * 4));
     auto chain = [&](auto* keys, auto* keys2) -> int {
         using K = std::remove_pointer_t<decltype(keys)>;
-        const auto k_keys = KfKern<Row>::template keys<K>;
-        k_keys<<<kf_row_grid(tab.size(), largest, 8), 256, 0, c->stream>>>(arena, d_tab, rows, stride, p, keys, c->vg_vals.as<int>());
+        k_kf_keys<K><<<kf_row_grid(tab.size(), largest, 8), 256, 0, c->stream>>>(d_tab, rows, stride, p, keys, c->vg_vals.as<int>());
         LILI_TRY(launch_check(c, "k_kf_keys"));
         // non-finite points carry the sentinel key and sort last: the first n_fin sorted entries are the finite points
         if constexpr (sizeof(K) == 4) LILI_TRY(sort_pairs_u32(c, keys, keys2, c->vg_vals.as<int>(), c->vg_vals2.as<int>(), (int)N, key_bits));
@@ -1520,8 +1393,8 @@ static int gmap_run(liliom_ctx* c, const unsigned char* arena, const std::vector
         return download_sized(c, c->vg_out, m, stride, out, cap, n, [&]() -> int {
             c->n_ds_resident = -1;      // vg_out is rewritten: no scan for liliom_map_update_resident
             LILI_CUDA(c, c->vg_out.ensure((size_t)m * stride));
-            const auto k_centroid = stride == 48 ? KfKern<Row>::template centroid<48, K> : KfKern<Row>::template centroid<32, K>;
-            k_centroid<<<cdiv(n_fin, 128), 128, 0, c->stream>>>(arena, d_tab, rows, keys2, c->vg_vals2.as<int>(), c->vg_flags.as<int>(),
+            const auto k_centroid = stride == 48 ? k_kf_centroid<48, K> : k_kf_centroid<32, K>;
+            k_centroid<<<cdiv(n_fin, 128), 128, 0, c->stream>>>(d_tab, rows, keys2, c->vg_vals2.as<int>(), c->vg_flags.as<int>(),
                                                                 c->vg_rank.as<int>(), n_fin, (unsigned char*)c->vg_out.p);
             return launch_check(c, "k_kf_centroid");
         });
@@ -1530,50 +1403,41 @@ static int gmap_run(liliom_ctx* c, const unsigned char* arena, const std::vector
     return chain(c->vg_keys.as<uint32_t>(), c->vg_keys2.as<uint32_t>());
 }
 
+// liliom_global_map over the keyframes of c's own store (stores NULL) or entry i's of stores[i]; entry i's pre-transform at
+// pre7s + pre_step * i (pre_step 0: one for every entry)
+static int global_map(liliom_ctx* c, int kind, liliom_ctx* const* stores, const int* kf_ids, const double* poses7, int k, const double* pre7s,
+                      size_t pre_step, float leaf, void* out, int cap, int* n) {
+    if (!c || !n || k < 0 || (k > 0 && (!kf_ids || !poses7)) || (kind != LILIOM_KF_FULL && kind != LILIOM_KF_SURF) || !(leaf > 0))
+        return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, nullptr));
+    const KfStores s{c, stores};
+    LILI_TRY(kf_list_ok(c, s, kf_ids, k, kind));
+    std::vector<KfRow> tab;
+    long long largest = 0;
+    const long long N = gmap_rows(s, kind, kf_ids, poses7, k, pre7s, pre_step, tab, &largest);
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    LILI_TRY(kf_join_stores(c, {{s, k}}));
+    return gmap_run(c, tab, N, largest, leaf, out, cap, n);
+}
+
 }  // namespace lili
 
 extern "C" int liliom_global_map(liliom_ctx* c, int kind, const int* kf_ids, const double* poses7, int k, const double pre7[7],
                                  float leaf, void* out, int cap, int* n) {
-    if (!c || !n || k < 0 || (k > 0 && (!kf_ids || !poses7)) || (kind != LILIOM_KF_FULL && kind != LILIOM_KF_SURF) || !(leaf > 0))
-        return LILIOM_E_ARG;
-    LILI_TRY(backend_check(c, nullptr));
-    if (!kf_ids_ok(c, kf_ids, k) || !kf_full_ok(c, KfStores{c}, kind, kf_ids, k)) return LILIOM_E_ARG;
-    std::vector<KfRow> tab;
-    long long largest = 0;
-    const long long N = gmap_rows(KfStores{c}, kind, kf_ids, poses7, k, pre7, 0, tab, &largest);
-    LILI_TRY(kf_points_ok(c, N));
-    const unsigned char* arena = (const unsigned char*)(kind == LILIOM_KF_FULL ? c->kf_full.p : c->kf_arena.p);
-    return gmap_run(c, arena, tab, N, largest, leaf, out, cap, n);
+    return global_map(c, kind, nullptr, kf_ids, poses7, k, pre7, 0, leaf, out, cap, n);
 }
 
-// liliom_global_map over keyframes of several stores: rows that name their store's arena, the rest unchanged on c
 extern "C" int liliom_global_map_multi(liliom_ctx* c, int kind, liliom_ctx* const* stores, const int* kf_ids, const double* poses7, int k,
                                        const double* pre7s, float leaf, void* out, int cap, int* n) {
-    if (!c || !n || k < 0 || (k > 0 && (!stores || !kf_ids || !poses7)) || (kind != LILIOM_KF_FULL && kind != LILIOM_KF_SURF) || !(leaf > 0))
-        return LILIOM_E_ARG;
-    LILI_TRY(backend_check(c, nullptr));
-    if (!kf_stores_ok(c, stores, kf_ids, k) || !kf_full_ok(c, KfStores{c, stores}, kind, kf_ids, k)) return LILIOM_E_ARG;
-    std::vector<KfRowM> tab;
-    long long largest = 0;
-    const long long N = gmap_rows(KfStores{c, stores}, kind, kf_ids, poses7, k, pre7s, 7, tab, &largest);
-    LILI_TRY(kf_points_ok(c, N));
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    LILI_TRY(kf_join_stores(c, {{stores, k}}));
-    return gmap_run(c, (const unsigned char*)c->kf_arena.p, tab, N, largest, leaf, out, cap, n);
+    if (k > 0 && !stores) return LILIOM_E_ARG;
+    return global_map(c, kind, stores, kf_ids, poses7, k, pre7s, 7, leaf, out, cap, n);
 }
 
-// liliom_loop_align over keyframes of several stores: both clouds' rows name their store's arena, the rest unchanged on c
 extern "C" int liliom_loop_align_multi(liliom_ctx* c, liliom_ctx* const* src_stores, const int* src_ids, const double* src_poses7, int k_src,
                                        liliom_ctx* const* tgt_stores, const int* tgt_ids, const double* tgt_poses7, int k_tgt, float leaf,
                                        double max_corr_dist, int max_iter, double trans_eps, double fit_eps, double T16[16], double* fitness,
                                        int* converged, int* iters, int* n_src, int* n_tgt) {
-    if (!c || !T16 || !fitness || !converged || !iters) return LILIOM_E_ARG;
-    LILI_TRY(loop_check<KfRowM>(c, src_stores, src_ids, src_poses7, k_src, tgt_stores, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist,
-                                max_iter));
-    LILI_CUDA(c, cudaSetDevice(c->device));
-    LILI_TRY(kf_join_stores(c, {{src_stores, k_src}, {tgt_stores, k_tgt}}));
-    LoopJob j;
-    LILI_TRY(loop_tables<KfRowM>(c, KfStores{c, src_stores}, src_ids, src_poses7, k_src, KfStores{c, tgt_stores}, tgt_ids, tgt_poses7, k_tgt,
-                                 leaf, max_corr_dist, max_iter, trans_eps, fit_eps, j));
-    return loop_run<KfRowM>(j, T16, fitness, converged, iters, n_src, n_tgt);
+    if ((k_src > 0 && !src_stores) || (k_tgt > 0 && !tgt_stores)) return LILIOM_E_ARG;
+    return loop_align(c, src_stores, src_ids, src_poses7, k_src, tgt_stores, tgt_ids, tgt_poses7, k_tgt, leaf, max_corr_dist, max_iter,
+                      trans_eps, fit_eps, T16, fitness, converged, iters, n_src, n_tgt);
 }

@@ -1,8 +1,8 @@
-// TEST INFRASTRUCTURE: host build of the backend local map's table (liliom_b200/csrc/kf_table.h's kf_bmap_rows) for both row
-// types, composed the way liliom_bmap_build and liliom_bmap_build_multi compose it on the device: the gather (k_kf_gather's body:
-// kf_row_point of every row's points at their destinations) into the edge-then-surf concatenation, then each layer's VoxelGrid
-// (box -> vg_params -> keys -> stable sort -> heads -> walk -> writer; PCL's declined case passes the layer through).  KfRow rows
-// read one arena (the merged store), KfRowM rows each the arena of their entry's store.  Compiled with -ffp-contract=off.
+// TEST INFRASTRUCTURE: host build of the backend local map's table (liliom_b200/csrc/kf_table.h's kf_bmap_rows), composed the way
+// liliom_bmap_build and liliom_bmap_build_multi compose it on the device: the gather (k_kf_gather's body: kf_row_point of every
+// row's points at their destinations) into the edge-then-surf concatenation, then each layer's VoxelGrid (box -> vg_params -> keys
+// -> stable sort -> heads -> walk -> writer; PCL's declined case passes the layer through).  Rows over one arena (the merged store)
+// against rows that each name the arena of their entry's store.  Compiled with -ffp-contract=off.
 #include "../liliom_b200/csrc/kf_table.h"
 #include <algorithm>
 #include <cstdint>
@@ -14,21 +14,19 @@ using namespace lili;
 
 static bool bm_finite(const VgXyz& p) { return std::isfinite(p.x) && std::isfinite(p.y) && std::isfinite(p.z); }
 
-// The table of k entries (entry i: n_edge[i] edge points from edge_off[i] and n_surf[i] surf points from surf_off[i] of arenas[i]
-// for KfRowM, of arenas[0] for KfRow), gathered into out (E + S points).  rows_out: dst_off, n, src_off of every row (3 per row).
-// n[0] = E, n[1] = S, *largest as the device's gather grid takes it.  Returns the rows.
-template <class Row>
-static int bm_gather(const void* const* arenas, int stride, const long long* edge_off, const long long* surf_off, const int* n_edge,
-                     const int* n_surf, int k, const double* poses7, unsigned char* out, long long* n, long long* largest, long long* rows_out) {
-    constexpr bool multi = std::is_same<Row, KfRowM>::value;
-    std::vector<Row> tab;
-    kf_bmap_rows([&](int i) { return KfClouds{multi ? arenas[i] : nullptr, edge_off[i], surf_off[i], n_edge[i], n_surf[i]}; }, poses7, k, tab,
-                 n, largest);
-    const unsigned char* arena = multi ? nullptr : (const unsigned char*)arenas[0];
+// The table of k entries (entry i: n_edge[i] edge points from edge_off[i] and n_surf[i] surf points from surf_off[i] of
+// arenas[arena_step * i]), gathered into out (E + S points).  rows_out: dst_off, n, src_off of every row (3 per row).  n[0] = E,
+// n[1] = S, *largest as the device's gather grid takes it.  Returns the rows.
+static int bm_gather(const void* const* arenas, size_t arena_step, int stride, const long long* edge_off, const long long* surf_off,
+                     const int* n_edge, const int* n_surf, int k, const double* poses7, unsigned char* out, long long* n, long long* largest,
+                     long long* rows_out) {
+    std::vector<KfRow> tab;
+    kf_bmap_rows([&](int i) { return KfClouds{arenas[arena_step * i], edge_off[i], surf_off[i], n_edge[i], n_surf[i]}; }, poses7, k, tab, n,
+                 largest);
     for (size_t y = 0; y < tab.size(); ++y) {
-        const Row& r = tab[y];
+        const KfRow& r = tab[y];
         for (int i = 0; i < r.n; ++i)
-            kf_row_point(r, kf_row_src(r, arena, stride, r.src_off + i), stride, out + (size_t)(r.dst_off + i) * stride);
+            kf_row_point(r, kf_row_src(r, stride, r.src_off + i), stride, out + (size_t)(r.dst_off + i) * stride);
         rows_out[3 * y] = r.dst_off; rows_out[3 * y + 1] = r.n; rows_out[3 * y + 2] = r.src_off;
     }
     return (int)tab.size();
@@ -38,14 +36,14 @@ static int bm_gather(const void* const* arenas, int stride, const long long* edg
 extern "C" int bm_gather_single(const void* const* arenas, int stride, const long long* edge_off, const long long* surf_off, const int* n_edge,
                                 const int* n_surf, int k, const double* poses7, unsigned char* out, long long* n, long long* largest,
                                 long long* rows_out) {
-    return bm_gather<KfRow>(arenas, stride, edge_off, surf_off, n_edge, n_surf, k, poses7, out, n, largest, rows_out);
+    return bm_gather(arenas, 0, stride, edge_off, surf_off, n_edge, n_surf, k, poses7, out, n, largest, rows_out);
 }
 
 // several stores: entry i's clouds in arenas[i]
 extern "C" int bm_gather_multi(const void* const* arenas, int stride, const long long* edge_off, const long long* surf_off, const int* n_edge,
                                const int* n_surf, int k, const double* poses7, unsigned char* out, long long* n, long long* largest,
                                long long* rows_out) {
-    return bm_gather<KfRowM>(arenas, stride, edge_off, surf_off, n_edge, n_surf, k, poses7, out, n, largest, rows_out);
+    return bm_gather(arenas, 1, stride, edge_off, surf_off, n_edge, n_surf, k, poses7, out, n, largest, rows_out);
 }
 
 // A layer's VoxelGrid (voxelgrid_dev's chain on the concatenation): N points at pts -> out; returns the points written

@@ -1,9 +1,9 @@
 """CPU tier for the multi-store backend local map (liliom_bmap_build_multi and its batch): the local map's table builder
-(kf_table.h's kf_bmap_rows) compiled for the host for both row types (tests/bmap_multi_host.cpp) and composed as the device
-composes it.  Rows that each name the arena of their entry's store (KfRowM) must give, byte for byte, the rows and the
-edge-then-surf concatenation that KfRow rows over one merged arena holding the same clouds give; each layer's VoxelGrid must be
-the oracle's voxelgrid(concat(transform_cloud(...))).  Both point layouts, interleaved and repeated lists, stores of different
-sizes, and keyframes whose edge or surf cloud is empty."""
+(kf_table.h's kf_bmap_rows) compiled for the host (tests/bmap_multi_host.cpp) and composed as the device composes it.  Rows that
+each name the arena of their entry's store must give, byte for byte, the rows and the edge-then-surf concatenation that rows
+over one merged arena holding the same clouds give; each layer's VoxelGrid must be the oracle's
+voxelgrid(concat(transform_cloud(...))).  Both point layouts, interleaved and repeated lists, stores of different sizes, and
+keyframes whose edge or surf cloud is empty."""
 import ctypes as C
 
 import numpy as np

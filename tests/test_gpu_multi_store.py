@@ -288,6 +288,7 @@ def test_stores_untouched_and_refusals_change_nothing():
         for i, st in enumerate(f.stores + [c]):
             _resident(st, i)
         kid, _, _ = f.stores[2].kf_add(f.bp, f.seqs[2][0][0], f.seqs[2][0][1], download=False)     # no full cloud
+        n_scan = len(f.stores[0].kf_cloud([0], [IDENT], TINY_LEAF))       # keyframe 0's edge and surf points
         snaps = [_snapshot(st) for st in f.stores]
         e = [(0, 1), (1, 0), (2, 3), (0, 1), (1, 4), (2, 3)]              # interleaved, repeated; ids of 5-keyframe stores
         ids, poses = [i for _, i in e], [f.pose(s, i) for s, i in e]
@@ -325,6 +326,23 @@ def test_stores_untouched_and_refusals_change_nothing():
             ("loop unknown id", lambda: loop_rc([s0], [0], [s1], [50]), L._binding.E_ARG),
             ("loop leaf", lambda: loop_rc([s0], [0], [s1], [1], leaf=0.0), L._binding.E_ARG),
             ("loop max_iter", lambda: loop_rc([s0], [0], [s1], [1], max_iter=0), L._binding.E_ARG),
+        ]
+
+        def rc_of(call):
+            try:
+                call()
+            except L.LiliomError as err:
+                return err.code
+            return L._binding.OK
+        # 2^31 listed edge and surf points, in the single-store calls and the multi-store local map: one keyframe listed over and over
+        reps = (1 << 31) // n_scan + 1
+        big_ids, big_poses = np.zeros(reps, np.int32), np.tile(IDENT, (reps, 1))
+        refused += [
+            ("loop 2^31 points", lambda: rc_of(lambda: s0.loop_align([0], [IDENT], big_ids, big_poses, 0.4)), L._binding.E_CAPACITY),
+            ("local map 2^31 points", lambda: rc_of(lambda: s0.bmap_build(f.bp, big_ids, big_poses)), L._binding.E_CAPACITY),
+            ("local map multi 2^31 points", lambda: rc_of(lambda: c.bmap_build_multi(f.bp, [s0] * reps, big_ids, big_poses)),
+             L._binding.E_CAPACITY),
+            ("kf_cloud 2^31 points", lambda: rc_of(lambda: s0.kf_cloud(big_ids, big_poses, 0.4)), L._binding.E_CAPACITY),
         ]
         for what, call, rc in refused:
             assert call() == rc, what
