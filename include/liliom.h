@@ -264,6 +264,29 @@ int liliom_kf_add(liliom_ctx* c, const liliom_backend_params* bp, const void* ed
 int liliom_kf_count(const liliom_ctx* c);
 int liliom_kf_clear(liliom_ctx* c);      /* drops every keyframe, the local map and the window correspondences */
 
+/* A keyframe store across restarts: the stored clouds of listed keyframes as one checked byte image, and that image appended to
+ * any context's store, bit for bit.  Layout (liliom_b200/csrc/kf_image.h), little-endian: a 64-byte header (magic "LILIKF01",
+ * version 1, point_stride, k, flags, edge+surf points, full points, table checksum, points checksum), k 16-byte records
+ * (n_edge, n_surf, n_full with -1 = no full cloud, a reserved zero), section A (each keyframe's edge then surf points, in table
+ * order), section F (the full clouds); size = 64 + 16 k + point_stride * (points).  Only the point layout is recorded: the
+ * backend parameters stay per call, the poses stay the caller's.  Importing an image of store C's keyframes L into D gives every
+ * call that reads keyframes (bmap_build and the window calls, kf_cloud, loop_align, global_map, every _multi and _batch_multi
+ * form with D as a store) on D with the mapped ids the bytes it gives on C with L, and liliom_kf_export(D) gives the image back. */
+enum { LILIOM_KF_IMAGE_FULL = 1 };   /* export flag: include the full clouds */
+/* The listed keyframes of c's store as one byte image, in list order.  kf_ids == NULL: every keyframe, in id order (k ignored).
+ * Repeated ids give repeated keyframes.  Without LILIOM_KF_IMAGE_FULL every record has n_full = -1 and F is empty.
+ * image == NULL: *bytes = the image size only.  cap < size: LILIOM_E_CAPACITY, *bytes = the size, nothing written.
+ * LILIOM_E_ARG: unknown id, k < 0, unknown flag bits, a sharded context.
+ * Writes no state that another call reads: the store, the local map layers, the resident window, the odometry map and a resident
+ * scan (liliom_map_update_resident) stay as they were.  One launch gathers and checksums the points on the device. */
+int liliom_kf_export(liliom_ctx* c, const int* kf_ids, int k, int flags, void* image, long long cap, long long* bytes);
+/* Appends the image's keyframes to c's store: their ids are *first_id .. *first_id + *k - 1, in image order.  All or nothing.
+ * A malformed image gives LILIOM_E_ARG with liliom_last_error naming the first failed check (in order: magic and version,
+ * point_stride equal to c's, flags, counts, totals, exact length, table checksum, points checksum; the last on the device after
+ * the upload), and then liliom_kf_count and every stored byte are unchanged (an arena may have grown).  A sharded context:
+ * LILIOM_E_ARG.  Leaves the same state alone as liliom_kf_export. */
+int liliom_kf_import(liliom_ctx* c, const void* image, long long bytes, int* first_id, int* k);
+
 /* Backend local map: buildLocalMapWithLandMark (L:1387-1484) + downSampleCloud, map half (:1486-1492).  For each listed keyframe,
  * in list order, its stored clouds transformed by poses7[i] (transformCloud, :730-767; the caller composes q_po*q_bl,
  * q_po*t_bl + t_po as at :1425-1426), edge and surf concatenated separately (:1479-1483), VoxelGrid(edge_leaf) /

@@ -28,6 +28,7 @@ assert PT48.itemsize == 48 and PT32.itemsize == 32 and LIVOX20.itemsize == 20
 OK, E_ARG, E_CUDA, E_FEWMAP, E_CAPACITY, E_GRID, E_LINES, E_NCCL, E_NOMAP = 0, -1, -2, -3, -4, -5, -6, -7, -8
 MODE_CERES, MODE_GN = 0, 1
 KF_FULL, KF_SURF = 0, 1      # liliom_global_map: which stored cloud of each keyframe
+KF_IMAGE_FULL = 1             # liliom_kf_export: include the full clouds
 RING_ELEVATION, RING_FIELD = 0, 1   # liliom_set_ring_source: ROT scanID from the elevation tables / the PointCloud2 `ring` field
 TIME_AZIMUTH, TIME_FIELD = 0, 1     # liliom_set_time_source: ROT relTime from the azimuth rule / a PointCloud2 per-point time field
 
@@ -98,6 +99,7 @@ EXPORTS = [
     "liliom_undistort_resident_batch", "liliom_kf_add_resident_batch", "liliom_bmap_build_batch",
     "liliom_global_map_multi", "liliom_loop_align_multi",
     "liliom_bmap_build_multi", "liliom_bmap_build_batch_multi", "liliom_loop_align_batch_multi",
+    "liliom_kf_export", "liliom_kf_import",
 ]
 NODE_EXPORTS = ["liliom_pre_create", "liliom_pre_destroy", "liliom_pre_imu", "liliom_pre_cloud", "liliom_pre_cloud_pc2",
                 "liliom_lo_create", "liliom_lo_destroy", "liliom_lo_edge", "liliom_lo_surf", "liliom_lo_full", "liliom_lo_run"]
@@ -266,6 +268,8 @@ def lib() -> C.CDLL:
                                           C.c_int, C.c_double, C.c_double, dp, dp, ip, ip, ip, ip]
     L.liliom_loop_align_batch.argtypes = [C.POINTER(vp), C.c_int, C.POINTER(ip), C.POINTER(dp), ip, C.POINTER(ip), C.POINTER(dp), ip,
                                           C.POINTER(LoopParams), C.POINTER(LoopResult), ip]
+    L.liliom_kf_export.argtypes = [vp, ip, C.c_int, C.c_int, vp, C.c_longlong, C.POINTER(C.c_longlong)]
+    L.liliom_kf_import.argtypes = [vp, vp, C.c_longlong, ip, ip]
     L.liliom_bmap_build_multi.argtypes = [vp, bpp, C.POINTER(vp), ip, dp, C.c_int, ip, ip]
     L.liliom_bmap_build_batch_multi.argtypes = [C.POINTER(vp), C.c_int, bpp, C.POINTER(C.POINTER(vp)), C.POINTER(ip), C.POINTER(dp), ip, ip,
                                                 ip, ip]
@@ -624,6 +628,28 @@ class Context:
 
     def kf_clear(self):
         self._check(lib().liliom_kf_clear(self._h))
+
+    def kf_export(self, kf_ids=None, full: bool = True) -> bytes:
+        """The listed keyframes' stored clouds as one checked byte image (liliom_kf_export): every keyframe in id order when
+        kf_ids is None; the full clouds too when `full`.  The poses stay the caller's: save them beside the image."""
+        ids = None if kf_ids is None else _ids(kf_ids)
+        k = 0 if ids is None else len(ids)
+        ip = None if ids is None else ids.ctypes.data_as(C.POINTER(C.c_int))
+        flags = KF_IMAGE_FULL if full else 0
+        n = C.c_longlong()
+        self._check(lib().liliom_kf_export(self._h, ip, k, flags, None, 0, C.byref(n)))
+        out = bytearray(n.value)
+        buf = (C.c_char * len(out)).from_buffer(out)
+        self._check(lib().liliom_kf_export(self._h, ip, k, flags, buf, len(out), C.byref(n)))
+        return bytes(out)
+
+    def kf_import(self, image) -> tuple[int, int]:
+        """Appends an image of liliom_kf_export (any bytes-like object) to this context's store, all or nothing.  Returns
+        (first_id, k): the image's keyframes are ids first_id .. first_id + k - 1, in image order."""
+        a = np.frombuffer(image, np.uint8)
+        first, k = C.c_int(), C.c_int()
+        self._check(lib().liliom_kf_import(self._h, a.ctypes.data_as(C.c_void_p) if a.size else None, a.size, C.byref(first), C.byref(k)))
+        return first.value, k.value
 
     def bmap_build(self, bp: BackendParams, kf_ids, poses7):
         """buildLocalMapWithLandMark + downSampleCloud (map half) on the device: returns (edge layer size, surf layer size)."""

@@ -454,6 +454,7 @@ struct liliom_ctx {
     long long kf_full_used = 0;          // points in use
     std::vector<lili::KfEntry> kfs;      // per keyframe: offsets and counts (host)
     lili::DevBuf kf_tab;                 // per-call keyframe table (kf_table.h: k_kf_gather, the global map's kernels)
+    lili::DevBuf kf_img, kf_img_seg, kf_img_sum;   // liliom_kf_export's staged points, the image calls' segments and checksum word
     lili::MapIndex bmap[2];              // backend local map: [0] edge layer, [1] surf layer
     lili::DevBuf bmap_raw, bmap_ds[2];   // concatenation of the transformed keyframes; the filtered layers (all fields)
     int bmap_n[2] = {0, 0};

@@ -14,6 +14,7 @@
 #include "ctx.cuh"
 #include "dev_math.cuh"
 #include "kf_table.h"
+#include "kf_image.h"
 #include <algorithm>
 #include <type_traits>
 
@@ -457,6 +458,173 @@ extern "C" int liliom_kf_add_resident(liliom_ctx* c, const liliom_backend_params
     LILI_TRY(kf_full_dev(c, bp, j.f[2].buf->p, j.m[2], &j.mf));
     LILI_CUDA(c, cudaStreamSynchronize(c->stream));
     kf_res_finish(j, kf_id, n_edge_ds, n_surf_ds, n_full_stored);
+    return LILIOM_OK;
+}
+
+// ---- the keyframe image (kf_image.h): liliom_kf_export / liliom_kf_import ----
+namespace lili {
+
+// nv 16-byte vectors at src, which are vectors v0 .. v0 + nv - 1 of the image's points (sections A and F).  A call's segments are
+// in ascending v0, back to back, none empty.
+struct KfiSeg { const uint4* src; long long v0, nv; };
+constexpr int kKfiChunk = 2048;          // vectors per block and pass (32 KB)
+
+// The points checksum of the segments (kfi_term of each word at its position in the image's points), added into *sum, and when
+// dst is set a plain byte copy of every vector to dst[v].  Each block takes chunks of kKfiChunk vectors of the concatenation,
+// finds the segment of its first vector by binary search and walks on; its 64-bit partial is folded into *sum by one atomicAdd
+// (integer sums: the order of the blocks does not change a bit).
+__global__ void __launch_bounds__(256) k_kf_image(const KfiSeg* __restrict__ segs, int nseg, long long total, uint4* __restrict__ dst,
+                                                  unsigned long long* __restrict__ sum) {
+    uint64_t h = 0;
+    for (long long c0 = (long long)blockIdx.x * kKfiChunk; c0 < total; c0 += (long long)gridDim.x * kKfiChunk) {
+        int lo = 0, hi = nseg - 1;                               // the last segment with v0 <= c0
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (segs[mid].v0 <= c0) lo = mid;
+            else hi = mid - 1;
+        }
+        const long long c1 = min(c0 + kKfiChunk, total);
+        int s = lo;
+        KfiSeg g = segs[s];
+        for (long long v = c0 + threadIdx.x; v < c1; v += blockDim.x) {
+            while (v >= g.v0 + g.nv) g = segs[++s];
+            const uint4 x = g.src[v - g.v0];
+            const uint64_t j = 2 * (uint64_t)v;
+            h += kfi_term((uint64_t)x.y << 32 | x.x, j) + kfi_term((uint64_t)x.w << 32 | x.z, j + 1);
+            if (dst) dst[v] = x;
+        }
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) h += __shfl_xor_sync(0xffffffffu, h, o);
+    __shared__ uint64_t warp[8];
+    if ((threadIdx.x & 31) == 0) warp[threadIdx.x >> 5] = h;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < (int)(blockDim.x >> 5); ++w) h += warp[w];
+        atomicAdd(sum, (unsigned long long)h);
+    }
+}
+
+// Pushes the segment of n points of `arena` from point `off` (none when n == 0); *v: the image vector it starts at
+static void kfi_push(std::vector<KfiSeg>& segs, const DevBuf& arena, long long off, long long n, int stride, long long* v) {
+    if (n <= 0) return;
+    const long long nv = n * stride / 16;
+    segs.push_back(KfiSeg{(const uint4*)((const unsigned char*)arena.p + (size_t)off * stride), *v, nv});
+    *v += nv;
+}
+
+// One k_kf_image launch over the segments, its checksum read back into *h.  out (export): the segments are also gathered into
+// kf_img and copied from there to the host at `out` before the read-back's wait.
+static int kfi_run(liliom_ctx* c, const std::vector<KfiSeg>& segs, void* out, uint64_t* h) {
+    *h = 0;
+    if (segs.empty()) return LILIOM_OK;
+    const long long total = segs.back().v0 + segs.back().nv;
+    if (out) LILI_CUDA(c, c->kf_img.ensure((size_t)total * 16));
+    LILI_CUDA(c, c->kf_img_seg.ensure(segs.size() * sizeof(KfiSeg)));
+    LILI_CUDA(c, c->kf_img_sum.ensure(sizeof(unsigned long long)));
+    LILI_CUDA(c, cudaMemcpyAsync(c->kf_img_seg.p, segs.data(), segs.size() * sizeof(KfiSeg), cudaMemcpyHostToDevice, c->stream));
+    LILI_CUDA(c, cudaMemsetAsync(c->kf_img_sum.p, 0, sizeof(unsigned long long), c->stream));
+    const int grid = std::max(1, std::min(cdiv(total, kKfiChunk), c->sm_count * 8));
+    k_kf_image<<<grid, 256, 0, c->stream>>>(c->kf_img_seg.as<KfiSeg>(), (int)segs.size(), total, out ? c->kf_img.as<uint4>() : nullptr,
+                                            c->kf_img_sum.as<unsigned long long>());
+    LILI_TRY(launch_check(c, "k_kf_image"));
+    if (out) LILI_CUDA(c, cudaMemcpyAsync(out, c->kf_img.p, (size_t)total * 16, cudaMemcpyDeviceToHost, c->stream));
+    return read_back(c, {{h, c->kf_img_sum.p, sizeof(uint64_t)}});
+}
+
+}  // namespace lili
+
+extern "C" int liliom_kf_export(liliom_ctx* c, const int* kf_ids, int k, int flags, void* image, long long cap, long long* bytes) {
+    if (!c || !bytes || (kf_ids && k < 0)) return LILIOM_E_ARG;
+    if (flags & ~LILIOM_KF_IMAGE_FULL) { c->last_error = "unknown keyframe image flags"; return LILIOM_E_ARG; }
+    LILI_TRY(backend_check(c, nullptr));
+    const int n_kf = (int)c->kfs.size();
+    if (!kf_ids) k = n_kf;
+    std::vector<int> ids(k);
+    for (int i = 0; i < k; ++i) {
+        ids[i] = kf_ids ? kf_ids[i] : i;
+        if (ids[i] < 0 || ids[i] >= n_kf) {
+            c->last_error = "unknown keyframe id " + std::to_string(ids[i]) + " (" + std::to_string(n_kf) + " stored)";
+            return LILIOM_E_ARG;
+        }
+    }
+    const bool full = flags & LILIOM_KF_IMAGE_FULL;
+    const int stride = c->prm.point_stride;
+    std::vector<KfiRecord> tab(k);
+    long long ns = 0, nf = 0;
+    for (int i = 0; i < k; ++i) {
+        const KfEntry& f = c->kfs[ids[i]];
+        tab[i] = KfiRecord{f.n_edge, f.n_surf, full ? f.n_full : -1, 0};
+        ns += (long long)f.n_edge + f.n_surf;
+        nf += full && f.n_full > 0 ? f.n_full : 0;
+    }
+    const long long size = kfi_size(stride, k, ns, nf);
+    *bytes = size;
+    if (!image) return LILIOM_OK;
+    if (cap < size) return LILIOM_E_CAPACITY;
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    // section A (edge then surf of each entry), then section F, gathered into kf_img by one launch that also sums them
+    std::vector<KfiSeg> segs;
+    long long v = 0;
+    for (int i = 0; i < k; ++i) {
+        const KfEntry& f = c->kfs[ids[i]];
+        kfi_push(segs, c->kf_arena, f.edge_off, f.n_edge, stride, &v);
+        kfi_push(segs, c->kf_arena, f.surf_off, f.n_surf, stride, &v);
+    }
+    for (int i = 0; full && i < k; ++i) {
+        const KfEntry& f = c->kfs[ids[i]];
+        kfi_push(segs, c->kf_full, f.full_off, f.n_full, stride, &v);
+    }
+    unsigned char* out = (unsigned char*)image;
+    KfiHeader hd = kfi_header(stride, k, full ? kKfiFlagFull : 0, ns, nf);
+    LILI_TRY(kfi_run(c, segs, out + kKfiHeader + kKfiRecord * k, &hd.points_sum));
+    kfi_write_head(out, hd, tab.data(), k);
+    return LILIOM_OK;
+}
+
+// The host checks (kfi_check), both arenas reserved once, sections A and F uploaded behind the stored points, one k_kf_image launch
+// over what was written; only a matching points checksum records the keyframes and advances both counts.
+extern "C" int liliom_kf_import(liliom_ctx* c, const void* image, long long bytes, int* first_id, int* k) {
+    if (!c || !first_id || !k || bytes < 0 || (bytes > 0 && !image)) return LILIOM_E_ARG;
+    LILI_TRY(backend_check(c, nullptr));
+    const int stride = c->prm.point_stride;
+    const unsigned char* img = (const unsigned char*)image;
+    KfiHeader h;
+    if (const int e = kfi_check(img, bytes, stride, &h); e != kKfiOk) {
+        c->last_error = std::string("keyframe image: ") + kfi_check_name(e);
+        return LILIOM_E_ARG;
+    }
+    if ((long long)c->kfs.size() + h.k > INT_MAX) { c->last_error = "keyframe image: the store would exceed 2^31 - 1 keyframes"; return LILIOM_E_ARG; }
+    LILI_CUDA(c, cudaSetDevice(c->device));
+    const long long ns = (long long)h.n_scan, nf = (long long)h.n_full;
+    LILI_TRY(kf_reserve(c, c->kf_arena, c->kf_used, c->kf_used + ns));
+    LILI_TRY(kf_reserve(c, c->kf_full, c->kf_full_used, c->kf_full_used + nf));
+    const unsigned char* pts = img + kKfiHeader + kKfiRecord * h.k;
+    if (ns) LILI_CUDA(c, cudaMemcpyAsync((unsigned char*)c->kf_arena.p + (size_t)c->kf_used * stride, pts, (size_t)ns * stride,
+                                         cudaMemcpyHostToDevice, c->stream));
+    if (nf) LILI_CUDA(c, cudaMemcpyAsync((unsigned char*)c->kf_full.p + (size_t)c->kf_full_used * stride, pts + (size_t)ns * stride,
+                                         (size_t)nf * stride, cudaMemcpyHostToDevice, c->stream));
+    std::vector<KfiSeg> segs;
+    long long v = 0;
+    kfi_push(segs, c->kf_arena, c->kf_used, ns, stride, &v);
+    kfi_push(segs, c->kf_full, c->kf_full_used, nf, stride, &v);
+    uint64_t sum = 0;
+    LILI_TRY(kfi_run(c, segs, nullptr, &sum));
+    if (sum != h.points_sum) { c->last_error = std::string("keyframe image: ") + kfi_check_name(kKfiBadPointsSum); return LILIOM_E_ARG; }
+    *first_id = (int)c->kfs.size();
+    *k = h.k;
+    for (int i = 0; i < h.k; ++i) {
+        KfiRecord r;
+        memcpy(&r, img + kKfiHeader + kKfiRecord * i, sizeof(r));
+        KfEntry f{c->kf_used, c->kf_used + r.n_edge, r.n_edge, r.n_surf};
+        c->kf_used += (long long)r.n_edge + r.n_surf;
+        if (r.n_full >= 0) {
+            f.full_off = c->kf_full_used;
+            f.n_full = r.n_full;
+            c->kf_full_used += r.n_full;
+        }
+        c->kfs.push_back(f);
+    }
     return LILIOM_OK;
 }
 
